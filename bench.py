@@ -2,6 +2,7 @@
 """bench.py -- rays/s of the NeRF per-ray hot path on synthetic lego-shaped input.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--arch A1|A0|A2] [--config 2|3|4]
+                    [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]; SURVEY.md section 8d): config/lego.yml as written -- 8x128
 FlexibleNeRFModel with skip every 3 (coarse + fine), L_xyz 10, L_dir 4 -- 400x400 lego-like camera
@@ -16,6 +17,10 @@ HOST buffers (H2D of origins/directions/targets and D2H of the loss inside the t
 
 --config selects the BASELINE.json workload: 2 (default) = lego 400x400, 4096 rays; 3 = lego 800x800, 8192 rays;
 4 = LLFF-like fern (378x504, NDC rays, L_xyz 6, noise std 1.0), 4096 rays.  (Config 5 = config 3's shape at --gpus 8.)
+
+--dump-outputs DIR writes what the last timed training step computed, as float32 .npy files: the six render outputs
+of run_one_iter_of_nerf, the loss, and per network the flat gradient and the parameters after the Adam update.  All
+inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 --impl reference times the reference's CPU implementation of the same step (the oracle port: the same
 ATen ops in the same order as the unmodified reference, all host threads) on the SAME batch size (falls back to a
@@ -92,7 +97,7 @@ def make_options():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -139,8 +144,9 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        return d, "measured bf16 cuBLAS burst (MEASURED_PEAKS.json)"
+    # NVIDIA's H100 SXM data sheet (700 W card): HBM3 bandwidth and dense BF16 / FP16 tensor rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet, dense BF16/FP16 (not measured)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -240,7 +246,7 @@ def workload_config(args, world):
                     "train step = fwd + mse(coarse)+mse(fine) + bwd + grad all-reduce + Adam",
         "rays_per_gpu": RAYS_PER_GPU, "global_rays": RAYS_PER_GPU * world, "n_coarse": NC, "n_fine": NF,
         "parallelism": f"ray-sharded dp{world}, one flat-gradient all-reduce per step",
-        "cache": "no L2 flush: every step streams its activation stash (GBs, >> 126 MB L2) through HBM; "
+        "cache": "no L2 flush: every step streams its activation stash (GBs, >> 50 MB L2) through HBM; "
                  "weights/rays are L2-resident as in real training",
     }
 
@@ -261,7 +267,7 @@ def run_ours(args):
     dev = torch.device("cuda", local)
     impl = {"simt": ops.IMPL_SIMT, "tc": ops.IMPL_TC}[args.kernels]
     if args.arch == "A2":
-        # hidden 256: training on the fp32 CUDA-core kernels, inference (`fwd_only`) on the tcgen05 forward -- the library's
+        # hidden 256: training on the fp32 CUDA-core kernels, inference (`fwd_only`) on the wgmma forward -- the library's
         # automatic choice; the per-kernel roofline below probes the fp32 kernels
         impl, args.kernels = ops.IMPL_SIMT, "simt (training), tc (inference forward)"
         nb.set_default_impl(None)
@@ -299,9 +305,12 @@ def run_ours(args):
         optim.step()          # fused Adam over the flat parameter buffers
         return loss
 
+    last = {}
+
     def step(ro_, rd_, tgt_):
         out = nb.run_one_iter_of_nerf(H, W, FOCAL, mc, mf, ro_, rd_, options, mode="train",
                                       encode_position_fn=epf, encode_direction_fn=edf)
+        last["out"] = out
         return finish(out, tgt_)
 
     loss_host = torch.empty((), dtype=torch.float32).pin_memory()
@@ -350,6 +359,8 @@ def run_ours(args):
     l0 = ops.launch_count()
     total_ms = timed(lambda: losses.append(step(ro, rd, tgt).detach()), args.steps)
     launches = (ops.launch_count() - l0) // args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["out"], losses[-1], optim)
     ms_per_step = total_ms / args.steps
     value = RAYS_PER_GPU * world / (ms_per_step / 1e3)
 
@@ -379,36 +390,24 @@ def run_ours(args):
             return timed(fn, n) / n if world == 1 else None
 
         if world == 1:
-            # DRAM traffic per launch is not measurable from inside the run: it is read from the committed ncu
-            # summary of the same kernels at the same size (profiles/r2_ncu_summary.json, `ncu --set full`), and says so
-            traffic = traffic_b = None
-            summ = os.path.join(ROOT, "profiles", "r2_ncu_summary.json")
-            if os.path.exists(summ) and args.config == 2:
-                js = json.load(open(summ))
-                traffic = js.get(f"mlp_fwd_{args.kernels.split()[0]}_{args.arch}_dram_bytes")
-                traffic_b = js.get(f"mlp_bwd_{args.kernels.split()[0]}_{args.arch}_dram_bytes")
             t = t_alone(lambda: ops.mlp_fwd(arch, blob, rays, z, impl=impl))
             ach = flops_fwd / (t * 1e-3) / 1e12
             roof = {"kernel": f"mlp_fwd_{args.kernels.split()[0]} (fine pass, {RAYS_PER_GPU}x{NC + NF} points)", "bound": "tensor",
-                    "achieved": ach, "peak": peaks["bf16_tflops"], "peak_source": f"{peak_kind} bf16 cuBLAS burst",
-                    "unit": "TFLOP/s", "frac": ach / peaks["bf16_tflops"], "traffic": traffic,
-                    "traffic_source": "profiles/r2_ncu_summary.json (ncu --set full of this kernel, same size)", "ms": t,
-                    "algorithmic_flops": flops_fwd}
+                    "achieved": ach, "peak": peaks["bf16_tflops"], "peak_source": peak_kind,
+                    "unit": "TFLOP/s", "frac": ach / peaks["bf16_tflops"], "ms": t, "algorithmic_flops": flops_fwd}
             raw, stash = ops.mlp_fwd(arch, blob, rays, z, impl=impl, want_stash=True)
             roof["ms_training_forward"] = t_alone(lambda: ops.mlp_fwd(arch, blob, rays, z, impl=impl, want_stash=True), n=5)
             G = torch.randn_like(raw)
             tb = t_alone(lambda: ops.mlp_bwd(arch, blob, rays, z, G, stash, impl=impl))
             achb = 2 * flops_fwd / (tb * 1e-3) / 1e12
             roof_bwd = {"kernel": "mlp_bwd (dgrad + wgrad kernels, fine pass)", "bound": "tensor", "achieved": achb,
-                        "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": achb / peaks["bf16_tflops"], "ms": tb,
-                        "traffic": traffic_b,
-                        "traffic_source": "profiles/r2_ncu_summary.json (ncu --set full of this kernel, same size)"}
+                        "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": achb / peaks["bf16_tflops"], "ms": tb}
             if impl == ops.IMPL_TC:
                 # one fused kernel (data-gradient chain + all weight gradients): tensor-bound; its HBM side is the
                 # activation tiles it streams back (algorithmic bytes from the library)
                 bbytes = float(ops.bwd_bytes_per_point(arch)) * RAYS_PER_GPU * (NC + NF)
                 roof_bwd["kernel"] = "mlp_bwd_tc (fused dgrad + wgrad, fine pass)"
-                roof_bwd["peak_source"] = f"{peak_kind} bf16 cuBLAS burst"
+                roof_bwd["peak_source"] = peak_kind
                 roof_bwd["algorithmic_flops"] = 2 * flops_fwd
                 roof_bwd["hbm"] = {"algorithmic_bytes": bbytes, "achieved": bbytes / (tb * 1e-3) / 1e9,
                                    "peak": peaks["hbm_gbs"], "unit": "GB/s",
@@ -473,6 +472,21 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(path, out, loss, optim):
+    """The last timed step's results as float32 .npy files (a few MB for the default workloads)."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    names = ("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine")
+    arrays = {n: t for n, t in zip(names, out) if t is not None}
+    arrays["loss"] = loss.reshape(1)
+    for net, it in zip(("coarse", "fine"), optim.items):
+        arrays[f"grad_{net}"] = torch.cat([p.grad.reshape(-1) for p in it["params"]])
+        arrays[f"params_{net}"] = it["flat"]
+    for n, t in arrays.items():
+        np.save(os.path.join(path, n + ".npy"), t.detach().float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -483,6 +497,8 @@ def main():
     ap.add_argument("--kernels", default=os.environ.get("NERFB200_KERNELS", "tc"), choices=["simt", "tc"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--config", type=int, default=2, choices=sorted(CONFIGS))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs, gradients and updated parameters as .npy files to DIR")
     args = ap.parse_args()
     global CFG, RAYS_PER_GPU
     CFG = CONFIGS[args.config]

@@ -1,5 +1,5 @@
 /*
- * nerfb200.h -- C ABI of the B200-native NeRF per-ray hot path.
+ * nerfb200.h -- C ABI of the H100-native NeRF per-ray hot path.
  *
  * Drop-in boundary (SURVEY.md section 8b): the reference (krrish94/nerf-pytorch @ a14357d) has no
  * FFI; its hot path is plain Python behind two functions,
@@ -65,12 +65,12 @@ int32_t nerfb200_version(void);
 const char* nerfb200_last_error(void);
 /* number of CUDA kernels this library has launched in this process (all threads) */
 int64_t nerfb200_launch_count(void);
-/* HBM bytes the tcgen05 backward reads per point: one activation-tile row (4 bytes per feature: fp16 hi + lo) per
+/* HBM bytes the wgmma backward reads per point: one activation-tile row (4 bytes per feature: fp16 hi + lo) per
  * weight-gradient job, the ReLU bit masks and d_raw -- the algorithmic traffic of its roofline */
 int64_t nerfb200_bwd_bytes_per_point(const nerfb200_arch_t* arch);
-/* NERFB200_OK if `impl` (0 fp32 CUDA cores, 1 tcgen05) can run this architecture forward AND backward with
+/* NERFB200_OK if `impl` (0 fp32 CUDA cores, 1 wgmma) can run this architecture forward AND backward with
  * n_samples samples per ray, else NERFB200_ERR_UNSUPPORTED (reason in nerfb200_last_error()).  impl = 2 asks for the
- * tcgen05 FORWARD alone (inference: training = 0 in render_fwd / stash = NULL in mlp_fwd with impl = 1), which also
+ * wgmma FORWARD alone (inference: training = 0 in render_fwd / stash = NULL in mlp_fwd with impl = 1), which also
  * covers hidden_size 256 */
 int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, int32_t impl);
 
@@ -124,7 +124,7 @@ int32_t nerfb200_encode(const nerfb200_arch_t* arch, int32_t which, const float*
  * stash: NULL (inference) or fp32[nerfb200_stash_floats(arch, n_rays*n_samples)] receiving the
  * post-activation output of every hidden linear (needed by the backward entry points; private layout of the
  * implementation that wrote it: the backward must run with the same impl).
- * impl: 0 = fp32 CUDA cores (bit-faithful fp32 FMA), 1 = tcgen05 tensor cores: every product as a three-term
+ * impl: 0 = fp32 CUDA cores (bit-faithful fp32 FMA), 1 = wgmma tensor cores: every product as a three-term
  * split (fp16 x 2 operands with a 2^11-scaled residual, fp32 accumulation; ~22 significant bits per operand).
  * The split carries 22 bits for magnitudes in 6.1e-5 .. 65504 and resolves 1.5e-11 absolutely below; larger
  * activations / weights saturate (a NeRF's stay far inside; use impl 0 for networks that do not). */
@@ -170,7 +170,7 @@ int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const f
 /* The two halves of nerfb200_mlp_bwd as separate calls (autograd's accumulation of nn.Linear backward,
  * nerf/models.py:233-256 replayed in reverse): dgrad walks the chain backwards and fills `gstash` with the
  * pre-activation gradients; wgrad reduces dW = dY^T X over all points into `flat_grad` (+=).  impl 0 only: the
- * tcgen05 backward is one fused kernel that never writes the gradients out (NERFB200_ERR_UNSUPPORTED). */
+ * wgmma backward is one fused kernel that never writes the gradients out (NERFB200_ERR_UNSUPPORTED). */
 int32_t nerfb200_mlp_dgrad(const nerfb200_arch_t* arch, const float* blob, const float* d_raw, const float* stash,
                            float* gstash, int64_t n_points, int32_t impl, void* stream);
 int32_t nerfb200_mlp_wgrad(const nerfb200_arch_t* arch, const float* rays, int32_t ray_stride, const float* z,

@@ -1,4 +1,4 @@
-"""nerf_pytorch_b200 -- a Blackwell-native (sm_100a) per-ray render/train path that drops in behind
+"""nerf_pytorch_b200 -- an H100-native (sm_90a) per-ray render/train path that drops in behind
 krrish94/nerf-pytorch's ``run_one_iter_of_nerf`` / ``predict_and_render_radiance``.
 
 Host side: Python/PyTorch (device memory, streams, torch.distributed).  Everything per ray runs in

@@ -86,7 +86,7 @@ _lib = None
 
 
 def build_library(verbose: bool = False) -> str:
-    """Compile csrc/*.cu into libnerfb200.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/*.cu into libnerfb200.so for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:

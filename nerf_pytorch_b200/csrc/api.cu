@@ -21,6 +21,13 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int device_sms() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  return sms;
+}
+
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
 int check_cuda(cudaError_t e, const char* what) {
@@ -210,7 +217,7 @@ static void carve(const Plan& pc, const Plan* pf, const nerfb200_render_opts_t& 
     const int64_t sf = fine ? pad128(n * ns) * pf->sum_n : 0;
     w->stash_c = take(sc);
     w->stash_f = take(sf);
-    // backward scratch: the gradient stash of the CUDA-core path / the gradient blob of the tcgen05 path
+    // backward scratch: the gradient stash of the CUDA-core path / the gradient blob of the wgmma path
     int64_t gs = sc > sf ? sc : sf;
     const int64_t bc = pc.hidden == 128 ? bwd_tc_scratch_floats(pc) : 0;
     const int64_t bf = (fine && pf->hidden == 128) ? bwd_tc_scratch_floats(*pf) : 0;
@@ -275,7 +282,7 @@ int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, 
   NB_TRY(build_plan(arch, &p));
   if (impl == 0) return NERFB200_OK;
   if (impl == 1) return bwd_tc_supported(p, n_samples, "impl_supported");
-  if (impl == 2) return tc_supported(p, n_samples, "impl_supported", /*training=*/false);  // tcgen05 forward only (inference)
+  if (impl == 2) return tc_supported(p, n_samples, "impl_supported", /*training=*/false);  // wgmma forward only (inference)
   set_error("unknown impl %d", impl);
   return NERFB200_ERR_INVALID;
 }
@@ -305,7 +312,7 @@ int64_t nerfb200_blob_floats(const nerfb200_arch_t* arch) {
 int64_t nerfb200_stash_floats(const nerfb200_arch_t* arch, int64_t n_points) {
   Plan p;
   if (build_plan(arch, &p) != NERFB200_OK || n_points < 0) return -1;
-  return ((n_points + 127) & ~int64_t(127)) * p.sum_n;  // whole 128-point tiles (the tcgen05 path stores tiles)
+  return ((n_points + 127) & ~int64_t(127)) * p.sum_n;  // whole 128-point tiles (the wgmma path stores tiles)
 }
 
 int32_t nerfb200_flat_layout(const nerfb200_arch_t* arch, int32_t slot, int64_t* w_off, int64_t* b_off,

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations for the nerfb200 CUDA library (sm_100a).
+// common.cuh -- shared declarations for the nerfb200 CUDA library (sm_90a).
 //
 // The "plan" is the host-built description of one FlexibleNeRFModel (nerf/models.py:185-256 of the
 // reference) as a chain of GEMM layers (outputs of 64*NJ columns, evaluated tile-by-tile) and up
@@ -30,9 +30,9 @@ struct GemmLayer {
   int flat_w;    // offset of weight[n][k_h + enc_real] in the flat (torch-layout) vector
   int flat_b;    // offset of bias[n] in the flat vector
   int src;       // gemm index whose output is this layer's h-input (-1 for layer1)
-  // tcgen05 operand copy (mlp_tc.cu): k_tc = K the tensor-core path contracts over (the direction
+  // wgmma operand copy (mlp_tc.cu): k_tc = K the tensor-core path contracts over (the direction
   // encoding of layers_dir[0] is hoisted out per ray, so k_tc = k_h there); per k-step of 16 the blob
-  // holds [hi slab0 | hi slab1 | lo slab0 | lo slab1], slab = [n][8 fp16] (UMMA canonical K-major,
+  // holds [hi slab0 | hi slab1 | lo slab0 | lo slab1], slab = [n][8 fp16] (the wgmma canonical K-major,
   // no swizzle: 8-row core matrices 128 B apart, the two K halves one slab apart); fp16 x 2 split with a
   // 2^11-scaled residual (tc_common.cuh split_f16x2).
   int k_tc;
@@ -61,7 +61,7 @@ struct Plan {
   int enc_cum[2];  // stash slice of the xyz / direction encoding: base + n_points * enc_cum[sel], width enc_tile_w / dim_dir_pad
   int mask_base;   // stash slice of the ReLU bit masks: base + n_points * (mask_base + g.mask_cum), n/32 words per point
   int dim_xyz, dim_xyz_pad, dim_dir, dim_dir_pad;
-  int enc_tile_w;  // dim_xyz padded to 16: width of the xyz-encoding operand tile of the tcgen05 path (tc_common.cuh)
+  int enc_tile_w;  // dim_xyz padded to 16: width of the xyz-encoding operand tile of the wgmma path (tc_common.cuh)
   int n_freq_xyz, n_freq_dir, inc_xyz, inc_dir;
   int blob_floats, flat_floats;
   int use_viewdirs;
@@ -76,6 +76,7 @@ int build_plan(const nerfb200_arch_t* arch, Plan* plan);  // 0 or NERFB200_ERR_*
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 void count_launch();  // one call per kernel launched (nerfb200_launch_count)
+int device_sms();     // SM count of the current device (grid sizes of persistent / grid-stride kernels)
 
 // launchers (one per .cu), all return NERFB200_OK or an error code
 int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s);
@@ -97,8 +98,8 @@ int launch_mlp_dgrad(const Plan& p, const float* blob, const float* d_raw, const
 int launch_mlp_wgrad(const Plan& p, const float* rays, int ray_stride, const float* z, int64_t n_rays, int n_samples,
                      const float* d_raw, const float* stash, const float* gstash, float* flat_grad, int impl,
                      cudaStream_t s);
-// tcgen05 backward (mlp_tc_bwd.cu): data-gradient chain + every weight gradient in one kernel; `scratch` holds the
-// L2-resident gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into
+// wgmma backward (mlp_tc_bwd.cu): data-gradient chain + every weight gradient in one kernel; `scratch` holds the
+// L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into
 int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
                       const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
 int64_t bwd_tc_scratch_floats(const Plan& p);
@@ -115,7 +116,7 @@ int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, 
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s);
 int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2,
                 float eps, float grad_scale, cudaStream_t s);
-// tcgen05 path (mlp_tc.cu, mlp_tc_bwd.cu)
+// wgmma path (mlp_tc.cu, mlp_tc_bwd.cu)
 int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
                       int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s);
 

@@ -260,7 +260,7 @@ mlp_fwd_simt_kernel(const __grid_constant__ Plan p, const FwdSmem sm, const floa
       }
       __syncthreads();
       if (stash && tid < kTileRows && p0 + tid < P) {
-        // ReLU bit mask of this row (read by the tcgen05 dgrad kernel): bit c = output c > 0
+        // ReLU bit mask of this row (read by the wgmma dgrad kernel): bit c = output c > 0
         uint32_t* mk = reinterpret_cast<uint32_t*>(stash) + (size_t)P * (p.mask_base + g.mask_cum) +
                        (size_t)(p0 + tid) * (g.n / 32);
         for (int w = 0; w < g.n / 32; ++w) {
@@ -639,8 +639,9 @@ int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const fl
       "mlp_bwd_wgrad smem attribute");
   if (rc) return rc;
   const int64_t stages = (P + kWgPts - 1) / kWgPts;
-  int split = (int)((148 * 2 * 4 + n_items - 1) / n_items);
-  if (split > 1184) split = 1184;
+  const int sms = device_sms();
+  int split = (int)((sms * 8 + n_items - 1) / n_items);
+  if (split > sms * 8) split = sms * 8;
   if (split > stages) split = (int)stages;
   if (split < 1) split = 1;
   dim3 grid(split, n_items);
@@ -650,12 +651,12 @@ int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const fl
   return check_cuda(cudaGetLastError(), "mlp_bwd_wgrad launch");
 }
 
-// The two halves of the CUDA-core backward as stage-level entry points.  The tcgen05 backward is one fused kernel
+// The two halves of the CUDA-core backward as stage-level entry points.  The wgmma backward is one fused kernel
 // (mlp_tc_bwd.cu) that never materialises the gradient stash, so impl 1 has no halves.
 int launch_mlp_dgrad(const Plan& p, const float* blob, const float* d_raw, const float* stash, float* gstash, int64_t P,
                      int impl, cudaStream_t s) {
   if (impl == 1) {
-    set_error("mlp_dgrad: impl=1 (tcgen05) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
+    set_error("mlp_dgrad: impl=1 (wgmma) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
     return NERFB200_ERR_UNSUPPORTED;
   }
   return launch_dgrad_simt(p, blob, d_raw, stash, gstash, P, s);
@@ -665,7 +666,7 @@ int launch_mlp_wgrad(const Plan& p, const float* rays, int ray_stride, const flo
                      const float* d_raw, const float* stash, const float* gstash, float* flat_grad, int impl,
                      cudaStream_t s) {
   if (impl == 1) {
-    set_error("mlp_wgrad: impl=1 (tcgen05) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
+    set_error("mlp_wgrad: impl=1 (wgmma) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
     return NERFB200_ERR_UNSUPPORTED;
   }
   return launch_wgrad_simt(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, n_rays * n_samples, flat_grad, 0,

@@ -1,74 +1,56 @@
-// mlp_tc.cu -- tcgen05 (5th-generation tensor core) implementation of the layer-chained forward kernel
+// mlp_tc.cu -- Hopper tensor-core (wgmma) implementation of the layer-chained forward kernel
 //   points -> positional encoding -> FlexibleNeRFModel   (nerf/train_utils.py:67, :8-25; nerf/models.py:233-256)
 // (the backward lives in mlp_tc_bwd.cu) for hidden_size 128 (and 256 in inference), fp32-faithful through a 3-term split of every product
 //     a * w  ~=  a_hi*w_hi + a_lo*w_hi + a_hi*w_lo          (SURVEY.md section 7.3 item 1)
-// on tcgen05.mma.kind::f16 (K = 16 per instruction): both operands are fp16 pairs (hi = fp16(x), lo = fp16((x - hi) 2^11),
-// 22 significant bits, tc_common.cuh split_f16x2); the weights come in three pre-scaled copies (hs | h | l, split_w3) so
-// that the three products of a k-step land at the SAME scale 2^11 in ONE fp32 accumulator in tensor memory.
-// The A operand holds activation / 16 (fp16 range 65504 -> 1.05e6: the shipped lego checkpoints reach 6e4);
-// conversions do not saturate, an out-of-range value turns the output into inf / NaN instead of clamping.
+// on wgmma.mma_async (fp16 operands, K = 16 per instruction, fp32 accumulator): both operands are fp16 pairs
+// (hi = fp16(x), lo = fp16((x - hi) 2^11), 22 significant bits, tc_common.cuh split_f16x2); the weights come in three
+// pre-scaled copies (hs | h | l, split_w3) so that the three products of a k-step land at the SAME scale 2^11 in ONE
+// fp32 accumulator.  The A operand holds activation / 16 (fp16 range 65504 -> 1.05e6: the shipped lego checkpoints
+// reach 6e4); conversions do not saturate, an out-of-range value turns the output into inf / NaN instead of clamping.
 //
-// Persistent kernel, one CTA per SM, 576 threads, TWO 128-point tiles in flight per CTA ("slots") for hidden 128, each
-// with its OWN eight epilogue warps: the two slots' epilogues overlap on the four schedulers and each slot's MMAs run
-// under the other slot's epilogue.  (Hidden 256, inference only: ONE slot takes all of tensor memory; kH template.)
-//   warps 0-7 / 8-15  prologue/epilogue of slot 0 / 1: thread (row = gtid % 128, half = gtid / 128) owns half of the
-//              columns of row `row` of a tile (= TMEM lane row).  Per layer and 32-column chunk: tcgen05.ld the fp32
-//              accumulator, add the bias at the accumulator's 2^11 scale, NaN-propagating max (ReLU), narrow heads as
-//              register dot products, split into fp16 hi + lo (mixed-precision FMA, tc_common.cuh split_f16x2_y) and
-//              tcgen05.st back into tensor memory as the NEXT layer's A operand: 5 instructions per element.
-//              Training: the SAME hi / lo registers are also stored to the activation stash as an operand tile
-//              (tc_common.cuh "Operand tiles": eight lanes write one full 128-byte line), plus one ReLU bit per
-//              activation; no staging buffer, no extra barrier.  ONE instance of this code per kernel (55 KB of
-//              SASS; an earlier version with the chunk code inlined eight times spent 10 % of its issue slots on
-//              instruction fetch).
-//   warp 16    MMA issuer: one elected lane, tcgen05.mma.kind::f16 M=128, N=256|128|64, K=16, three per k-step, two
-//              ring stages (twelve MMAs) per batch; A from tensor memory (hidden activations) or shared memory
-//              (encodings), B = the three weight copies from the shared-memory ring (24 KB per stage).
-//   warp 17    weight producer: one cp.async.bulk per stage from the L2-resident blob, mbarrier complete_tx
-//              (measured: 113-123 B/cycle/SM of L2 -> shared bulk copies with all SMs streaming, profiles/r2_microbench*).
-// The MMA issuer and the producer walk a fixed interleaving of the two slots' layers (Seq / Cursor below); slot 1 lags
-// slot 0 by half a tile so that one slot's prologue / last layer falls under the other slot's mid-chain layers.
-// Tensor memory (512 columns), per slot s at 2 H s: [0,H) accumulator, [H,3H/2) A_hi, [3H/2,2H) A_lo (two fp16 per
-// column).  The direction encoding enters layers_dir[0] through a per-ray fp32 bias computed on the CUDA cores
-// (it is constant along a ray: SURVEY.md section 7.3 item 5), so that layer contracts over K = H only.
-// Measured (A1, 4096 x 192 points): 0.76 ms inference / 1.17 ms training, tensor pipe 46 % / 30 % (profiles/r2_final_*).
+// Persistent kernel, one CTA per SM.  A tile is 64 points per consumer warpgroup: two warpgroups (128 points) for
+// hidden 128, one (64 points) for hidden 256, whose 64 x 256 fp32 accumulator takes half of a thread's registers.
+//   consumer warpgroups  per tile: positional encodings of its 64 rows -> fp16 operand tile (shared memory); per layer:
+//              wgmma over the ring's weight stages (A = the warpgroup's rows of the activation or encoding tile, B =
+//              the weight copies), then the epilogue on the accumulator registers: bias at the accumulator's 2^11
+//              scale, NaN-propagating max (ReLU), narrow heads as register dot products reduced over the quad, split
+//              into fp16 hi + lo (mixed-precision FMA, tc_common.cuh split_f16x2_y) -> the activation tile in shared
+//              memory, the next layer's A operand.  Training: the same hi / lo registers also go to the activation
+//              stash as an operand tile (tc_common.cuh "Operand tiles"), plus one ReLU bit per activation.
+//              The two warpgroups run independently; each one's epilogue overlaps the other's MMAs.
+//   last warp  weight producer: one cp.async.bulk per ring stage (24 KB) from the L2-resident blob, mbarrier
+//              complete_tx; a stage is free again once every consumer warp has seen its MMAs complete.
+// The direction encoding enters layers_dir[0] through a per-ray fp32 bias computed on the CUDA cores (it is constant
+// along a ray: SURVEY.md section 7.3 item 5), so that layer contracts over K = H only.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 
 namespace nerfb200 {
 
 namespace tc {
-constexpr int kEpiThreads = 256;                     // per slot: two dedicated warpgroups
-constexpr int kThreadsTc = 576;                      // 16 epilogue warps + MMA issuer + weight producer: 65536 / 576 -> 112
-                                                     // registers per thread for everyone (no setmaxnreg: a CTA's register
-                                                     // pool is threads x launch registers, NOT the whole file -- a first
-                                                     // version with 640 threads x 96 could not raise 512 threads to 112 and
-                                                     // hung in setmaxnreg.inc)
-constexpr int kMmaWarp = 16, kProdWarp = 17;
-constexpr int kStepsPerStage = 2;                    // k-steps per ring stage
+constexpr int kStepsPerStage = 2;                       // k-steps per ring stage at N <= 128
 constexpr int kStageBytes = kStepsPerStage * 96 * 128;  // 24 KB: 3 copies x 2 slabs x 128 rows x 16 B per k-step
 constexpr int kMaxStages = 6;
-constexpr int kEncBytes = 32768;                     // per slot: encoding operand tile, hi block then lo block (<= 64 wide)
 constexpr int kMaxRaysPerTile = 10;
-constexpr uint32_t kTmemCols = 512;
-// Tensor-memory columns of one slot: [0, H) accumulator, [H, 3H/2) A_hi, [3H/2, 2H) A_lo (two fp16 per column).
-// hidden 128: two slots of 256 columns; hidden 256 (inference only): ONE slot fills all 512 columns.
-__host__ __device__ inline int n_slots(const Plan& p) { return p.hidden == 128 ? 2 : 1; }
-constexpr int kSmemLimit = 232448 - 1024;            // 227 KB minus the alignment slack
+constexpr int kSmemLimit = 232448 - 1024;               // 227 KB minus the alignment slack
+
+__host__ __device__ inline int n_wg(int hidden) { return hidden == 128 ? 2 : 1; }  // consumer warpgroups = tile / 64
 
 // Shared memory map (bytes from the 1 KB-aligned base), computed identically on host and device.
 struct SmemMap {
-  int enc, ring, bias, headw, viewb, encd, hpart, wv, bars, total, n_stages;
+  int act, enc, ring, bias, headw, viewb, encd, wv, bars, total, n_stages;
 };
 __host__ __device__ inline SmemMap smem_map(const Plan& p) {
   SmemMap m;
-  m.enc = 0;                                        // 2 slots x 32 KB: encodings as fp16 operand tiles (hi | lo)
-  int off = m.enc + 2 * kEncBytes;
+  const int rows = 64 * n_wg(p.hidden);
+  m.act = 0;                                        // activation operand tile, hi | lo, up to hidden wide
+  int off = rows * p.hidden * 4;
+  m.enc = off;       off += rows * 64 * 4;          // encoding operand tile, hi | lo (<= 64 wide)
   m.bias = off;      off += p.enc_cum[0] * 4;       // sum of n over the gemm layers (bias * 2048 / 16)
   m.headw = off;     off += (4 * p.hidden + 3 * (p.hidden / 2) + 16) * 4;
-  m.viewb = off;     off += 2 * kMaxRaysPerTile * (p.hidden / 2) * 4;
-  m.encd = off;      off += 2 * kMaxRaysPerTile * 32 * 4;
-  m.hpart = off;     off += 2 * 2 * 128 * 4 * 4;    // [slot][head][row][4]
+  m.viewb = off;     off += n_wg(p.hidden) * kMaxRaysPerTile * (p.hidden / 2) * 4;
+  m.encd = off;      off += n_wg(p.hidden) * kMaxRaysPerTile * 32 * 4;
   m.wv = off;        off += 32 * (p.hidden / 2) * 4;  // direction-encoding rows of layers_dir[0]'s weight: Wt[k_h + k][n]
   m.bars = off;      off += 256;
   off = (off + 1023) & ~1023;
@@ -80,179 +62,207 @@ __host__ __device__ inline SmemMap smem_map(const Plan& p) {
   return m;
 }
 
-// The fixed interleaving of the two slots' events.  A tile is E = n_gemm + 1 events: event 0 = prologue (encodings),
-// event e = epilogue of layer e - 1; it is followed by MMA #e = layer e (e < n_gemm) whose A operand it wrote.
-// Every role walks the same sequence of half-ticks h = 0, 1, 2, ...: slot h & 1 at tick h >> 1; slot 1 starts E / 2
-// ticks after slot 0.  A Cursor is one slot's position; the roles keep the two cursors in registers and swap them
-// after every half-tick (no division, no dynamically indexed state).
-struct Cursor {
-  int idx, j, e, n;  // idx: ticks since the slot's start (negative: not started); tile counter; event; tiles of the slot
-  __device__ __forceinline__ bool active() const { return idx >= 0 && j < n; }
-  __device__ __forceinline__ void next(int E) {
-    if (idx >= 0 && ++e == E) { e = 0; ++j; }
-    ++idx;
-  }
-};
-struct Seq {
-  int E, half_ticks;
-  Cursor c0, c1;
-  __device__ __forceinline__ Seq(int events, int my_tiles, int slots) {
-    E = events;
-    const int off1 = events >> 1;
-    const int n0 = slots == 2 ? (my_tiles + 1) >> 1 : my_tiles, n1 = slots == 2 ? my_tiles >> 1 : 0;
-    const int t0 = n0 * E, t1 = n1 > 0 ? off1 + n1 * E : 0;
-    half_ticks = 2 * (t0 > t1 ? t0 : t1);
-    c0.idx = 0; c0.j = 0; c0.e = 0; c0.n = n0;
-    c1.idx = -off1; c1.j = 0; c1.e = 0; c1.n = n1;
-  }
-};
-template <typename T>
-__device__ __forceinline__ void swap2(T& a, T& b) { const T t = a; a = b; b = t; }
-
-// what MMA #e (= layer e) contracts: weights, shapes
+// what the MMAs of layer e contract: weights, shapes
 struct MmaInfo {
   const uint8_t* src;   // blob copy of the layer's weights (three fp16 copies, k-step major)
   uint32_t kbytes;      // bytes of one k-step
-  int ksteps, ksteps_h; // k-steps, of which the first ksteps_h read A from tensor memory (the rest: encodings)
-  int n_mma;            // N of the instruction
+  int ksteps, ksteps_h; // k-steps, of which the first ksteps_h read the activation tile (the rest: encodings)
   int sps;              // k-steps per ring stage (a stage holds 24 KB: two k-steps at N <= 128, one at N = 256)
 };
 __device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, int e) {
   MmaInfo mi;
   const GemmLayer& g = p.g[e];
   mi.src = reinterpret_cast<const uint8_t*>(blob + g.tc_off);
-  mi.n_mma = g.n;
   mi.ksteps = (g.k_tc + 15) >> 4;
   mi.ksteps_h = g.k_h >> 4;
-  mi.kbytes = 96u * (uint32_t)mi.n_mma;
-  mi.sps = mi.n_mma > 128 ? 1 : kStepsPerStage;   // (always kStepsPerStage in the hidden-128 instantiations)
+  mi.kbytes = 96u * (uint32_t)g.n;
+  mi.sps = g.n > 128 ? 1 : kStepsPerStage;
   return mi;
 }
 
-// per-slot state an epilogue thread carries across the events of one tile
-struct TileState {
-  int64_t p0 = 0, pt = 0, tile = 0;
-  bool valid = false;
-  int ray_slot = 0;
-  uint32_t acc_phase = 0;
+struct Pipe2 {  // ring position + the stage whose MMAs are still in flight
+  Pipe pp;
+  uint32_t prev = 0;
+  bool has_prev = false;
 };
 
 }  // namespace tc
 
 using namespace tc;
 
-// Development build only (make EXTRA=-DNERFB200_PROF): lane 0 of warp 0 (slot 0's epilogue), of the MMA warp and of the
-// producer warp of CTA 0 add up the cycles they spend in each phase (shared-memory counters, flushed at the end).
-#ifdef NERFB200_PROF
-__device__ unsigned long long g_prof_fwd[32];
-#define FPROF_ON (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (threadIdx.x < 32 || threadIdx.x >= 512))
-#define FPROF_SCOPE(i, stmt) do { const long long _ps = clock64(); stmt; if (FPROF_ON) s_prof[i] += (uint32_t)(clock64() - _ps); } while (0)
-#define FPROF_MARK(name) const long long name = clock64()
-#define FPROF_SINCE(i, name) do { if (FPROF_ON) s_prof[i] += (uint32_t)(clock64() - name); } while (0)
-#define FPROF_COUNT(i) do { if (FPROF_ON) s_prof[i] += 1u; } while (0)
-extern "C" void nerfb200_prof_read_fwd(unsigned long long* out32, int reset) {
-  cudaDeviceSynchronize();
-  cudaMemcpyFromSymbol(out32, g_prof_fwd, sizeof(g_prof_fwd));
-  if (reset) {
-    unsigned long long z[32] = {0};
-    cudaMemcpyToSymbol(g_prof_fwd, z, sizeof(z));
-  }
-}
-#else
-#define FPROF_SCOPE(i, stmt) do { stmt; } while (0)
-#define FPROF_MARK(name)
-#define FPROF_SINCE(i, name)
-#define FPROF_COUNT(i)
-#endif
-
-// One 32-column chunk of one row in the epilogue (the hot loop; ONE instance per kernel: the code must stay inside the
-// instruction cache -- the four head-count specialisations of the previous version, each inlined at two call sites of
-// two slot copies, made the kernel 160 KB and 10 % of the issue slots were instruction-fetch stalls):
-//   Y = max(acc + 2048 bias/16, lb), ys = Y / 2048 = activation / 16   (lb = 0 with ReLU, -inf without; the bias already
-//   holds the per-ray direction term for layers_dir[0]); head rows accumulate ys * (16 w) in a separate short pass;
-// then -> fp16 hi / lo -> tensor memory (next layer's A operand) and, in training, the stash tile.
-struct ChunkArgs {
-  const float* bias;      // this layer's bias * 2048 / 16 (or the per-ray bias of layers_dir[0])
-  float lb;               // ReLU lower bound
-  const float* hw;        // head weights [hn][hk] in smem (pre-multiplied by 16)
-  int hk, hn;
-  uint32_t* mword_out;    // train: where to store the ReLU mask word (or nullptr when the row is out of range)
-  uint8_t* stash_hi;      // train: this row's first 16-byte piece of the layer's stash tile (hi block), feature block 0
-  int stash_lo_off;       // train: byte offset of the lo block
-  uint32_t tmem_hi, tmem_lo;  // destination addresses (already offset to column c0)
-  bool has_next;
+// per-tile state a consumer thread carries over the layers: its two accumulator rows
+struct RowState {
+  int64_t pt[2];
+  bool valid[2];
+  int ray_slot[2];
 };
 
-template <bool kTrain>
-__device__ __forceinline__ void epilogue_chunk(const uint32_t (&v)[32], int c0, const ChunkArgs& a, float (&hacc)[4]) {
-  // Y = max(acc + 2048 bias/16, lb) = 2048 ys (the accumulator's own scale: the biases are stored pre-multiplied),
-  // x = ys = Y / 2048 exactly
-  float Y[32], x[32];
+// One layer of one warpgroup: MMAs over the ring, then the epilogue on the accumulator fragment.
+// Fragment of wgmma m64nN (per warp 16 rows): thread (warp wi, lane) holds rows r = 16 wi + lane / 4 (+ 8) and columns
+// 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row r + 8 i, column 8 j + 2 (lane % 4) + c).
+template <bool kTrain, int N>
+__device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, float* __restrict__ raw, float* __restrict__ stash,
+                                          uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t tile,
+                                          int64_t P_pad, const RowState& rs, Pipe2& pl, uint32_t bar_full,
+                                          uint32_t bar_empty, uint32_t n_stages, const float* s_bias, const float* s_headw,
+                                          const float* s_headb, const float* viewb, int hw1) {
+  const int wt = threadIdx.x & 127, wi = wt >> 5, lane = wt & 31, q = lane & 3;
+  const GemmLayer& g = p.g[e];
+  const MmaInfo mi = mma_info(p, blob, e);
+  const int enc_w = p.enc_tile_w;
+  const uint32_t act_a = smem_u32(sm + mp.act), enc_a = smem_u32(sm + mp.enc), ring_a = smem_u32(sm + mp.ring);
+  const int fin = g.k_h > 0 ? g.k_h : 16;
+  // this warpgroup's 64 rows of the K-major operand tiles (SBO = next 8 points, LBO = next 8 features)
+  const uint64_t a_hi0 = make_desc(act_a + (uint32_t)(wg * 64 * fin * 2), 128, (uint32_t)fin * 16);
+  const uint32_t a_lo_off = (uint32_t)(rows * fin * 2);
+  const uint64_t e_hi0 = make_desc(enc_a + (uint32_t)(wg * 64 * enc_w * 2), 128, (uint32_t)enc_w * 16);
+  const uint32_t e_lo_off = (uint32_t)(rows * enc_w * 2);
+  const uint32_t slab_b = 16u * (uint32_t)N;
+  const uint64_t b_ring = make_desc(ring_a, slab_b, 128);
+
+  float acc[N / 2];
 #pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 b = *reinterpret_cast<const float4*>(a.bias + c0 + j);
-    // NaN-propagating ReLU: an activation or weight beyond the fp16 x 2 range must surface as a non-finite output,
-    // never as a silently wrong finite one
-    Y[j] = fmax_nan(__uint_as_float(v[j]) + b.x, a.lb);
-    Y[j + 1] = fmax_nan(__uint_as_float(v[j + 1]) + b.y, a.lb);
-    Y[j + 2] = fmax_nan(__uint_as_float(v[j + 2]) + b.z, a.lb);
-    Y[j + 3] = fmax_nan(__uint_as_float(v[j + 3]) + b.w, a.lb);
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  wgmma_fence();
+  for (int ks0 = 0; ks0 < mi.ksteps; ks0 += mi.sps) {
+    const uint32_t st = pl.pp.stage;
+    mbar_wait(bar_full + 8 * st, pl.pp.phase);
+    const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStageBytes);
 #pragma unroll
-    for (int q = 0; q < 4; ++q) x[j + q] = Y[j + q] * kLoInv;
-  }
-  if (a.hn > 0) {  // narrow heads reading this layer (2 of the 9 layers): register dot products
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      if (c < a.hn) {
-        const float4* w4 = reinterpret_cast<const float4*>(a.hw + c * a.hk + c0);
-        float acc = hacc[c];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 w = w4[j];
-          acc = fmaf(x[4 * j], w.x, fmaf(x[4 * j + 1], w.y, fmaf(x[4 * j + 2], w.z, fmaf(x[4 * j + 3], w.w, acc))));
+    for (int hh = 0; hh < kStepsPerStage; ++hh) {
+      const int ks = ks0 + hh;
+      if (hh < mi.sps && ks < mi.ksteps) {
+        const uint64_t b_hs = desc_adv(b_st, hh * 6 * slab_b);
+        const uint64_t b_h = desc_adv(b_hs, 2 * slab_b), b_l = desc_adv(b_hs, 4 * slab_b);
+        uint64_t ah, al;
+        if (ks < mi.ksteps_h) {
+          ah = desc_adv(a_hi0, (uint32_t)ks * 256u);
+          al = desc_adv(ah, a_lo_off);
+        } else {
+          ah = desc_adv(e_hi0, (uint32_t)(ks - mi.ksteps_h) * 256u);
+          al = desc_adv(ah, e_lo_off);
         }
-        hacc[c] = acc;
+        wgmma_f16<N>(acc, ah, b_hs, ks > 0 ? 1 : 0);
+        wgmma_f16<N>(acc, al, b_h, 1);
+        wgmma_f16<N>(acc, ah, b_l, 1);
+      }
+    }
+    wgmma_commit();
+    if (pl.has_prev) {  // the previous stage's MMAs are complete: hand it back to the producer
+      wgmma_wait<1>();
+      reg_fence(acc);
+      if (lane == 0) mbar_arrive(bar_empty + 8 * pl.prev);
+    }
+    pl.prev = st;
+    pl.has_prev = true;
+    pl.pp.advance(n_stages);
+  }
+  wgmma_wait<0>();
+  reg_fence(acc);
+  if (lane == 0) mbar_arrive(bar_empty + 8 * pl.prev);
+  pl.has_prev = false;
+
+  // ---------------- epilogue ----------------
+  const int wg_bar_id = 1 + wg;
+  asm volatile("bar.sync %0, 128;" ::"r"(wg_bar_id) : "memory");  // every warp's MMAs have read the activation tile
+  const bool has_next = e + 1 < p.n_gemm;
+  int hsel = -1;
+  if (p.h[0].src == e) hsel = 0;
+  if (p.n_head > 1 && p.h[1].src == e) hsel = 1;
+  const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
+  const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
+  const bool is_dir = p.use_viewdirs && e == p.n_gemm - 1;
+  const float lb = g.relu ? 0.f : -3.4e38f;
+  const int vbs = p.hidden / 2;
+  const float* brow[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) brow[i] = is_dir ? viewb + rs.ray_slot[i] * vbs : s_bias + g.cum_n;
+  float hacc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+  uint32_t mbits[2][N / 32];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int m = 0; m < N / 32; ++m) mbits[i][m] = 0u;
+  uint8_t* act = sm + mp.act;
+  const int act_lo = rows * N * 2;
+  uint8_t* st_hi = nullptr;
+  if (kTrain) st_hi = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * g.cum_n) + (size_t)tile * tile_bytes(N);
+  const int r0 = 64 * wg + 16 * wi + (lane >> 2);  // tile row of acc row 0 (row 1: + 8)
+
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = 8 * j + 2 * q;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float2 b = *reinterpret_cast<const float2*>(brow[i] + col);
+      const float Y0 = fmax_nan(acc[4 * j + 2 * i] + b.x, lb), Y1 = fmax_nan(acc[4 * j + 2 * i + 1] + b.y, lb);
+      const float x0 = Y0 * kLoInv, x1 = Y1 * kLoInv;
+      if (hn > 0) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < hn) {
+            const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
+            hacc[i][c] = fmaf(x0, w.x, fmaf(x1, w.y, hacc[i][c]));
+          }
+      }
+      if (kTrain)  // ReLU bits (Y >= 0 here: Y > 0 <=> a nonzero bit pattern)
+        mbits[i][j >> 2] |= (min(__float_as_uint(Y0), 1u) | (min(__float_as_uint(Y1), 1u) << 1)) << (8 * (j & 3) + 2 * q);
+      if (has_next || kTrain) {
+        uint32_t hi, lo;
+        split_f16x2_y(Y0, Y1, x0, x1, hi, lo);
+        const int off = tile_piece(r0 + 8 * i, j, N) + q * 4;
+        if (has_next) {
+          *reinterpret_cast<uint32_t*>(act + off) = hi;
+          *reinterpret_cast<uint32_t*>(act + act_lo + off) = lo;
+        }
+        if (kTrain) {
+          __stcs(reinterpret_cast<unsigned int*>(st_hi + off), hi);
+          __stcs(reinterpret_cast<unsigned int*>(st_hi + tile_half_bytes(N) + off), lo);
+        }
       }
     }
   }
-  if (kTrain && a.mword_out) {
-    // ReLU bit mask: Y >= 0 here, so Y > 0 <=> its bit pattern is a positive integer; min(bits, 1) is the mask bit and
-    // bits = 2 bits + m shifts it in (2 instructions per element), element 31 first so that element j ends at bit j
-    uint32_t bits = 0;
-#pragma unroll
-    for (int j = 31; j >= 0; --j) bits = bits * 2u + min(__float_as_uint(Y[j]), 1u);
-    *a.mword_out = bits;
+  if (has_next) {
+    fence_proxy_async();  // generic-proxy stores -> the next layer's wgmma reads them through the async proxy
+    asm volatile("bar.sync %0, 128;" ::"r"(wg_bar_id) : "memory");
   }
-  if (a.has_next || kTrain) {
-    // fp16 x 2: two K-adjacent values per tensor-memory column / per 32-bit word of a stash piece
-    uint32_t hi[16], lo[16];
+  if (kTrain) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) split_f16x2_y(Y[2 * j], Y[2 * j + 1], x[2 * j], x[2 * j + 1], hi[j], lo[j]);
-    if (a.has_next) {
-      tmem_st16(a.tmem_hi, hi);
-      tmem_st16(a.tmem_lo, lo);
-    }
-    if (kTrain) {
-      // four 16-byte pieces (8 features each) per block; lanes p & 7 = 0..7 of a quarter warp fill one 128-byte line
-      uint8_t* dh = a.stash_hi + (c0 >> 3) * 128;
+    for (int i = 0; i < 2; ++i) {
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        __stcs(reinterpret_cast<uint4*>(dh + q * 128), make_uint4(hi[4 * q], hi[4 * q + 1], hi[4 * q + 2], hi[4 * q + 3]));
-        __stcs(reinterpret_cast<uint4*>(dh + a.stash_lo_off + q * 128),
-               make_uint4(lo[4 * q], lo[4 * q + 1], lo[4 * q + 2], lo[4 * q + 3]));
+      for (int m = 0; m < N / 32; ++m) {
+        uint32_t w = mbits[i][m];
+        w |= __shfl_xor_sync(0xffffffffu, w, 1);
+        w |= __shfl_xor_sync(0xffffffffu, w, 2);
+        if ((m & 3) == q && rs.valid[i])
+          reinterpret_cast<uint32_t*>(stash)[(size_t)P_pad * (p.mask_base + g.mask_cum) + (size_t)rs.pt[i] * (N >> 5) + m] = w;
       }
+    }
+  }
+  if (hsel >= 0) {
+    const int hcol = p.h[hsel].out_col;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 1);
+        hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 2);
+      }
+      if (q == 0 && rs.valid[i])
+        for (int c = 0; c < hn; ++c) raw[rs.pt[i] * 4 + hcol + c] = hacc[i][c] + s_headb[hsel * 4 + c];
     }
   }
 }
 
 // kTrain: the forward also writes the activation stash (operand tiles + ReLU bit masks + the encoding tile).
-// kH = hidden size (compile-time: the tensor-memory column map and the slot count fold into constants)
+// kH = hidden size (compile-time: the accumulator width and the warpgroup count fold into constants)
 template <bool kTrain, int kH>
-__global__ void __launch_bounds__(kThreadsTc, 1)
+__global__ void __launch_bounds__(128 * (kH == 128 ? 2 : 1) + 32, 1)
 mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ z, int64_t P, int S, int64_t n_tiles,
                   float* __restrict__ raw,          // out [P][4]
                   float* __restrict__ stash) {      // out (kTrain)
+  constexpr int kWG = kH == 128 ? 2 : 1, kRows = 64 * kWG, kThreads = 128 * kWG + 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1 KB aligned base
   const SmemMap mp = smem_map(p);
@@ -260,391 +270,179 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
   float* s_viewb = reinterpret_cast<float*>(sm + mp.viewb);
   float* s_encd = reinterpret_cast<float*>(sm + mp.encd);
-  float* s_hpart = reinterpret_cast<float*>(sm + mp.hpart);
   float* s_wv = reinterpret_cast<float*>(sm + mp.wv);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + mp.bars);
-  // barrier addresses are kept as 32-bit shared-memory addresses (8 bytes per barrier)
   const uint32_t bar_full = smem_u32(bars);                // [kMaxStages]  weights landed
-  const uint32_t bar_empty = bar_full + 8 * kMaxStages;    // [kMaxStages]  stage consumed by the MMAs
-  // per slot: bar_a = the next MMA's A operand is in tensor memory and the accumulator is drained (all 256 threads of
-  // the slot's epilogue group); bar_acc = accumulator complete
-  const uint32_t bar_a = bar_empty + 8 * kMaxStages;       // [2]
-  const uint32_t bar_acc = bar_a + 32;                     // [2]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 6);
+  const uint32_t bar_empty = bar_full + 8 * kMaxStages;    // [kMaxStages]  stage consumed by every consumer warp
   const uint32_t n_stages = (uint32_t)mp.n_stages;
-#ifdef NERFB200_PROF
-  uint32_t* s_prof = reinterpret_cast<uint32_t*>(bars) + 40;  // 24 counters in the spare part of the barrier block
-  if (threadIdx.x < 24) s_prof[threadIdx.x] = 0u;
-#endif
 
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int64_t P_pad = n_tiles * kTileRows;       // the stash sections are sized in whole tiles
+  const int64_t P_pad = n_tiles * kTileRows;       // the stash sections are sized in 128-point tiles
   const int enc_w = p.enc_tile_w;                  // encoding operand tile width (dim_xyz padded to 16)
-  const int enc_half = tile_half_bytes(enc_w);
 
   if (tid == 0) {
     for (int i = 0; i < kMaxStages; ++i) {
       mbar_init(&bars[i], 1);
-      mbar_init(&bars[kMaxStages + i], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars[2 * kMaxStages + s], kEpiThreads);      // bar_a
-      mbar_init(&bars[2 * kMaxStages + 4 + s], 1);            // bar_acc
+      mbar_init(&bars[kMaxStages + i], 4 * kWG);
     }
     fence_barrier_init();
   }
-  if (warp == kMmaWarp) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
   // biases (/16) + head weights (x16, they multiply activation / 16): once per CTA
   for (int gi = 0; gi < p.n_gemm; ++gi)
-    for (int i = tid; i < p.g[gi].n; i += kThreadsTc) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
+    for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
   const int hw1 = p.h[0].n_out * p.h[0].k;
   const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
-  for (int i = tid; i < hw1; i += kThreadsTc) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
-  for (int i = tid; i < hw2; i += kThreadsTc) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
+  for (int i = tid; i < hw1; i += kThreads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
+  for (int i = tid; i < hw2; i += kThreads) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
   float* s_headb = s_headw + ((hw1 + hw2 + 3) & ~3);
   if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
   if (tid >= 4 && tid < 8) s_headb[tid] = p.n_head > 1 ? blob[p.h[1].b_off + tid - 4] : 0.f;
-  for (int i = tid; i < 2 * kMaxRaysPerTile * 32; i += kThreadsTc) s_encd[i] = 0.f;  // padding channels stay zero
+  for (int i = tid; i < kWG * kMaxRaysPerTile * 32; i += kThreads) s_encd[i] = 0.f;  // padding channels stay zero
   if (p.use_viewdirs) {
-    // the per-ray direction term reads these 27 x 64 weights for every tile: from shared memory, not from L2 (the
-    // dependent global loads made the prologue 10.6 k cycles per tile)
     const GemmLayer& gd = p.g[p.n_gemm - 1];
     const float* wv_g = blob + gd.wt_off + (size_t)gd.k_h * gd.n;  // rows k_h.. of Wt[k][n]
-    for (int i = tid; i < p.dim_dir * gd.n; i += kThreadsTc) s_wv[i] = wv_g[i];
+    for (int i = tid; i < p.dim_dir * gd.n; i += kThreads) s_wv[i] = wv_g[i];
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *s_tmem;
 
   const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
-  const int E = p.n_gemm + 1;
-  const int nM = E - 1;
-  constexpr int slots = kH == 128 ? 2 : 1;
-  const Seq seq(E, my_tiles, slots);
-  constexpr uint32_t kSlotCols = 2u * kH, kColAcc = 0u, kColAhi = kH, kColAlo = kH + kH / 2;
-  constexpr int vbs = kH / 2;   // row stride of the per-ray bias table (= width of layers_dir[0])
-  const uint32_t ring_a = smem_u32(sm + mp.ring);
 
-  if (warp == kProdWarp) {
+  if (warp == 4 * kWG) {
     // ===================== weight producer =====================
     if ((tid & 31) == 0) {
       Pipe pp;
       const uint64_t pol = l2_policy_evict_last();
-      Cursor cur = seq.c0, oth = seq.c1;
-      for (int h = 0; h < seq.half_ticks; ++h) {
-        if (cur.active() && cur.e < nM) {
-          const MmaInfo mi = mma_info(p, blob, cur.e);
-          const int sps = kH == 128 ? kStepsPerStage : mi.sps;
-          for (int ks = 0; ks < mi.ksteps; ks += sps) {
-            const uint32_t bytes = (uint32_t)min(sps, mi.ksteps - ks) * mi.kbytes;
-            FPROF_SCOPE(11, mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1));
+      const uint32_t ring_a = smem_u32(sm + mp.ring);
+      for (int j = 0; j < my_tiles; ++j)
+        for (int e = 0; e < p.n_gemm; ++e) {
+          const MmaInfo mi = mma_info(p, blob, e);
+          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
+            const uint32_t bytes = (uint32_t)min(mi.sps, mi.ksteps - ks) * mi.kbytes;
+            mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1);
             mbar_arrive_expect_tx(bar_full + 8 * pp.stage, bytes);
-            bulk_g2s_hint(ring_a + pp.stage * kStageBytes, mi.src + (size_t)ks * mi.kbytes, bytes,
-                          bar_full + 8 * pp.stage, pol);
+            bulk_g2s_hint(ring_a + pp.stage * kStageBytes, mi.src + (size_t)ks * mi.kbytes, bytes, bar_full + 8 * pp.stage,
+                          pol);
             pp.advance(n_stages);
           }
         }
-        cur.next(E);
-        swap2(cur, oth);
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    Pipe pp;
-    uint32_t a_ph = 0, a_ph_oth = 0;  // phase of this slot's bar_a1 / bar_a2 (swapped with the cursors)
-    Cursor cur = seq.c0, oth = seq.c1;
-    for (int h = 0; h < seq.half_ticks; ++h) {
-      if (cur.active() && cur.e < nM) {
-        const uint32_t s = (uint32_t)(h & 1);
-        const MmaInfo mi = mma_info(p, blob, cur.e);
-        const int sps = kH == 128 ? kStepsPerStage : mi.sps;
-        const uint32_t idesc = make_idesc_f16(mi.n_mma);
-        const uint32_t slab_b = 16u * (uint32_t)mi.n_mma;  // bytes of one weight slab
-        const uint32_t t_acc = tmem + s * kSlotCols + kColAcc;
-        const uint32_t t_ahi = tmem + s * kSlotCols + kColAhi, t_alo = tmem + s * kSlotCols + kColAlo;
-        // descriptors are built once per layer; the loops below only advance their start-address fields
-        const uint64_t b_ring = make_desc(ring_a, slab_b, 128);
-        const uint64_t e_hi_d0 = make_desc(smem_u32(sm + mp.enc) + s * kEncBytes, 128, (uint32_t)(enc_w >> 3) * 128u);
-        const uint64_t e_lo_d0 = desc_adv(e_hi_d0, (uint32_t)enc_half);
-        FPROF_MARK(_tm);
-        FPROF_SCOPE(8, mbar_wait(bar_a + 8 * s, a_ph));
-        tc_fence_after();
-        // Two ring stages (four k-steps, twelve MMAs) per batch: the hand-over between stages (commit, barrier wait,
-        // fence, election, descriptor arithmetic: ~100 cycles during which the tensor pipe runs dry -- measured 82
-        // cycles per MMA against 64 nominal with one stage per batch) is paid half as often.
-        for (int ks0 = 0; ks0 < mi.ksteps;) {
-          const uint32_t st0 = pp.stage;
-          FPROF_SCOPE(9, mbar_wait(bar_full + 8 * st0, pp.phase));
-          pp.advance(n_stages);
-          const bool two = ks0 + sps < mi.ksteps;
-          const uint32_t st1 = pp.stage;
-          if (two) {
-            FPROF_SCOPE(9, mbar_wait(bar_full + 8 * st1, pp.phase));
-            pp.advance(n_stages);
-          }
-          tc_fence_after();
-#if defined(NERFB200_EXP) && NERFB200_EXP == 2   // timing experiment: no MMAs (results are garbage)
-          if (elect_one()) {
-            mma_commit(bar_empty + 8 * st0);
-            if (two) mma_commit(bar_empty + 8 * st1);
-          }
-          if (false) {
-#else
-          if (elect_one()) {
-#endif
-#pragma unroll
-            for (int half_b = 0; half_b < 2; ++half_b) {
-              if (half_b == 0 || two) {
-                const uint32_t st = half_b ? st1 : st0;
-                const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStageBytes);
-#pragma unroll
-                for (int hh = 0; hh < kStepsPerStage; ++hh) {
-                  const int ks = ks0 + half_b * sps + hh;
-                  if (hh < sps && ks < mi.ksteps) {
-                    const uint64_t b_hs = desc_adv(b_st, hh * 6 * slab_b);
-                    const uint64_t b_h = desc_adv(b_hs, 2 * slab_b);
-                    const uint64_t b_l = desc_adv(b_hs, 4 * slab_b);
-                    const uint32_t acc0 = ks > 0 ? 1u : 0u;
-                    if (ks < mi.ksteps_h) {
-                      mma_ts_f16(t_acc, t_ahi + 8 * ks, b_hs, idesc, acc0);
-                      mma_ts_f16(t_acc, t_alo + 8 * ks, b_h, idesc, 1u);
-                      mma_ts_f16(t_acc, t_ahi + 8 * ks, b_l, idesc, 1u);
-                    } else {  // encodings: K-major view of the operand tile (SBO = next 8 points, LBO = next 8 features)
-                      const uint32_t off = (uint32_t)(ks - mi.ksteps_h) * 256u;
-                      const uint64_t e_hi_d = desc_adv(e_hi_d0, off), e_lo_d = desc_adv(e_lo_d0, off);
-                      mma_ss_f16(t_acc, e_hi_d, b_hs, idesc, acc0);
-                      mma_ss_f16(t_acc, e_lo_d, b_h, idesc, 1u);
-                      mma_ss_f16(t_acc, e_hi_d, b_l, idesc, 1u);
-                    }
-                  }
-                }
-                mma_commit(bar_empty + 8 * st);  // frees the ring stage once these MMAs have read it
-              }
-            }
-          }
-          __syncwarp();
-          ks0 += (two ? 2 : 1) * sps;
-        }
-        a_ph ^= 1;
-        if (elect_one()) mma_commit(bar_acc + 8 * s);  // accumulator of this MMA complete
-        __syncwarp();
-        FPROF_SINCE(10, _tm);
-        FPROF_COUNT(12);
-      }
-      cur.next(E);
-      swap2(cur, oth);
-      swap2(a_ph, a_ph_oth);
     }
   } else {
-    // ===================== prologue / epilogue warps: warps 0-7 serve slot 0, warps 8-15 slot 1 =====================
-    // Each slot's tile chain runs on its own eight warps, so the two slots' epilogues overlap on the four schedulers
-    // (four epilogue warps each instead of two taking turns) and each slot's MMAs run under the other slot's epilogue.
-    const int s = warp >> 3;               // the slot this warp serves
-    const int gtid = tid & 255;            // thread index inside the slot's group
-    const int row = gtid & 127, half = gtid >> 7;
-    const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
-    TileState ts;
-    auto epi_bar = [&]() { asm volatile("bar.sync %0, 256;" ::"r"(1 + s) : "memory"); };
-
-    auto run_event = [&](const int j, const int e) {
-      const uint32_t t_acc = tmem + lane_base + s * kSlotCols + kColAcc;
-      const uint32_t t_ahi = tmem + lane_base + s * kSlotCols + kColAhi;
-      const uint32_t t_alo = tmem + lane_base + s * kSlotCols + kColAlo;
-      uint8_t* e_hi = sm + mp.enc + s * kEncBytes;
-      float* viewb = s_viewb + s * kMaxRaysPerTile * vbs;
-      float* encd = s_encd + s * kMaxRaysPerTile * 32;
-      float* hpart = s_hpart + s * 2 * 128 * 4;
-
-      FPROF_MARK(_te0);
-      if (e == 0) {
-        // ================= new tile: encodings of this row -> operand tile (value / 16), the two halves split the
-        // frequencies
-        ts.tile = blockIdx.x + (int64_t)(slots * j + s) * gridDim.x;
-        ts.p0 = ts.tile * kTileRows;
-        ts.pt = ts.p0 + row;
-        ts.valid = ts.pt < P;
-        if (!ts.valid) ts.pt = P - 1;
-        const int64_t p0 = ts.p0, pt = ts.pt;
-        // fewer than 2^31 points per call (checked on the host): 32-bit divisions instead of emulated 64-bit ones
-        const int64_t ray = (int64_t)((uint32_t)pt / (uint32_t)S);
-        const int64_t first_ray = (int64_t)((uint32_t)p0 / (uint32_t)S);
-        const int64_t last_pt = (p0 + kTileRows - 1 < P) ? p0 + kTileRows - 1 : P - 1;
-        const int n_rays_tile = (int)((uint32_t)last_pt / (uint32_t)S) - (int)first_ray + 1;
-        ts.ray_slot = (int)(ray - first_ray);
-        if (kTrain) {  // the previous tile's encoding store must have finished reading this buffer
-          if (gtid == 0) bulk_wait_read();
-          epi_bar();
-        }
-        {
-          const float* rr = rays + ray * ray_stride;
-          const float zz = z[pt];
-          const int nf = p.n_freq_xyz, mid = nf >> 1;
-          const int f0 = half ? mid : 0, f1 = half ? nf : mid;
-          const int base = p.inc_xyz ? 3 : 0;
-          auto put = [&](int k, float v) {
-            uint32_t hi, lo;
-            split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
-            const int off = tile_piece(row, k >> 3, enc_w) + (k & 7) * 2;
-            *reinterpret_cast<uint16_t*>(e_hi + off) = (uint16_t)hi;
-            *reinterpret_cast<uint16_t*>(e_hi + enc_half + off) = (uint16_t)lo;
-          };
-          for (int c = 0; c < 3; ++c) {
-            const float x = __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));  // pts = ro + rd * z (train_utils.py:67)
-            if (p.inc_xyz && half == 0) put(c, x);
-            for (int f = f0; f < f1; ++f) {
-              float sn, cs;
-              sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
-              put(base + 6 * f + c, sn);
-              put(base + 6 * f + 3 + c, cs);
-            }
-          }
-          if (half == 1)  // zero padding up to the operand width (one fp16 k-step = 16 granular)
-            for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
-        }
-        // ---- per-ray direction term of layers_dir[0]: vb[ray][n] = (sum_k enc_dir(ray)[k] * W[n][H + k] + b[n]) / 16
-        if (p.use_viewdirs) {
-          if (gtid < n_rays_tile * 3) {
-            const int jr = gtid / 3, c = gtid - 3 * jr;
-            const float v = rays[(first_ray + jr) * ray_stride + 8 + c];
-            encode_coord(v, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + jr * 32);
-          }
-          epi_bar();
-          const GemmLayer& gd = p.g[p.n_gemm - 1];
-          for (int i = gtid; i < n_rays_tile * gd.n; i += kEpiThreads) {
-            const int jr = i / gd.n, n = i - jr * gd.n;
-            float a = 0.f;
-            for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[jr * 32 + k], s_wv[k * gd.n + n], a);
-            viewb[jr * vbs + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);  // per-ray bias of layers_dir[0] (x 2048 / 16)
-          }
-        }
-        tc_fence_before();
-        fence_proxy_async();  // E was written through the generic proxy; the MMAs / the bulk store read it via the async proxy
-        epi_bar();         // also publishes viewb
-        if (kTrain && gtid == 0)  // the encoding tile goes to the stash as it is: one bulk store
-          bulk_s2g(reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * p.enc_cum[0]) + (size_t)ts.tile * tile_bytes(enc_w),
-                   e_hi, (uint32_t)tile_bytes(enc_w));
-        mbar_arrive(bar_a + 8 * s);
-        FPROF_SINCE(4, _te0);
-        FPROF_COUNT(6);
-        return;
-      }
-
-      // ================= one layer =================
-      const int64_t pt = ts.pt;
-      const bool valid = ts.valid;
-      const int t = e - 1;
-      const GemmLayer& g = p.g[t];
-      const bool has_next = e < nM;
-      int hsel = -1;
-      if (p.h[0].src == t) hsel = 0;
-      if (p.n_head > 1 && p.h[1].src == t) hsel = 1;
-      const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
-      const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
-      const int hcol = hsel >= 0 ? p.h[hsel].out_col : 0;
-      float hacc[4] = {0.f, 0.f, 0.f, 0.f};
-      const bool is_dir = p.use_viewdirs && t == p.n_gemm - 1;
-      uint32_t* mask_row = nullptr;
-      if (kTrain && valid)
-        mask_row = reinterpret_cast<uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) + (size_t)pt * (g.n >> 5);
-
-      FPROF_SCOPE(0, mbar_wait(bar_acc + 8 * s, ts.acc_phase));
-      ts.acc_phase ^= 1;
-      tc_fence_after();
-
-      {
-        ChunkArgs ca;
-        ca.bias = is_dir ? viewb + ts.ray_slot * vbs : s_bias + g.cum_n;
-        ca.lb = g.relu ? 0.f : -3.4e38f;
-        ca.hw = hw; ca.hk = hk; ca.hn = hn;
-        ca.has_next = has_next;
-        ca.stash_hi = nullptr;
-        ca.stash_lo_off = tile_half_bytes(g.n);
-        if (kTrain)
-          ca.stash_hi = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * g.cum_n) + (size_t)ts.tile * tile_bytes(g.n) +
-                        tile_piece(row, 0, g.n);
-        // column chunks of this thread: [32*half, +32) and, for 128-wide layers, [64 + 32*half, +32), one after the
-        // other (112 registers per thread: one 32-column chunk at a time)
-        const int nch = g.n >> 6;  // 64-column pairs of chunks: 4 / 2 / 1 for 256 / 128 / 64-wide layers
+    // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
+    const int wg = warp >> 2, wt = tid & 127, lane = tid & 31;
+    const int row = wt & 63, half = wt >> 6;       // prologue: two threads per row split the frequencies
+    const int vbs = kH / 2;
+    float* viewb = s_viewb + wg * kMaxRaysPerTile * vbs;
+    float* encd = s_encd + wg * kMaxRaysPerTile * 32;
+    uint8_t* enc = sm + mp.enc;
+    const int enc_hb = kRows * enc_w * 2;          // bytes of the hi (or lo) block of the encoding tile
+    Pipe2 pl;
+    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
 #pragma unroll 1
-        for (int ch = 0; ch < nch; ++ch) {
-          const int c0 = 64 * ch + 32 * half;
-          uint32_t v[32];
-#if defined(NERFB200_EXP) && NERFB200_EXP == 1   // timing experiment: epilogue without its arithmetic (results are garbage)
-          continue;
-#endif
-          FPROF_SCOPE(1, { tmem_ld32(t_acc + c0, v); tmem_wait_ld(); });
-          ca.mword_out = mask_row ? mask_row + (c0 >> 5) : nullptr;
-          ca.tmem_hi = t_ahi + c0 / 2;  // two fp16 per tensor-memory column
-          ca.tmem_lo = t_alo + c0 / 2;
-          FPROF_SCOPE(2, epilogue_chunk<kTrain>(v, c0, ca, hacc));
-        }
-      }
-      FPROF_MARK(_te1);
-
-      if (hsel >= 0 && half == 1)
-        *reinterpret_cast<float4*>(hpart + (hsel * 128 + row) * 4) = make_float4(hacc[0], hacc[1], hacc[2], hacc[3]);
-      if (has_next) {  // A operand of the next layer stored, accumulator drained: the slot's next MMA may start
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(bar_a + 8 * s);
-      } else {
-        tc_fence_before();
-      }
-      FPROF_SINCE(3, _te1);
-      if (hsel >= 0) {
-        epi_bar();  // head partials in hpart
-        if (half == 0 && valid) {
-          const float4 o = *reinterpret_cast<const float4*>(hpart + (hsel * 128 + row) * 4);
-          const float tot[4] = {hacc[0] + o.x + s_headb[hsel * 4 + 0], hacc[1] + o.y + s_headb[hsel * 4 + 1],
-                                hacc[2] + o.z + s_headb[hsel * 4 + 2], hacc[3] + o.w + s_headb[hsel * 4 + 3]};
+    for (int j = 0; j < my_tiles; ++j) {
+      const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
+      const int64_t p0 = tile * kRows + 64 * wg;   // first point of this warpgroup
+      // fewer than 2^31 points per call (checked on the host): 32-bit divisions instead of emulated 64-bit ones
+      const int64_t first_ray = (int64_t)((uint32_t)(p0 < P ? p0 : P - 1) / (uint32_t)S);
+      const int64_t last_pt = (p0 + 63 < P) ? p0 + 63 : P - 1;
+      const int n_rays_wg = (int)((uint32_t)last_pt / (uint32_t)S) - (int)first_ray + 1;
+      RowState rs;
 #pragma unroll
-          for (int c = 0; c < 4; ++c)
-            if (c < hn) raw[pt * 4 + hcol + c] = tot[c];
+      for (int i = 0; i < 2; ++i) {
+        const int64_t pt = p0 + 16 * (wt >> 5) + (lane >> 2) + 8 * i;
+        rs.valid[i] = pt < P;
+        rs.pt[i] = pt < P ? pt : P - 1;
+        rs.ray_slot[i] = (int)((uint32_t)rs.pt[i] / (uint32_t)S - first_ray);
+      }
+      // ================= encodings of this row -> operand tile (value / 16), the two halves split the frequencies
+      if (kTrain) {  // the previous tile's encoding store must have finished reading the tile
+        if (wt == 0) bulk_wait_read();
+        wg_bar();
+      }
+      {
+        const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
+        const int64_t ray = (int64_t)((uint32_t)pt / (uint32_t)S);
+        const float* rr = rays + ray * ray_stride;
+        const float zz = z[pt];
+        const int nf = p.n_freq_xyz, mid = nf >> 1;
+        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
+        const int base = p.inc_xyz ? 3 : 0;
+        const int trow = 64 * wg + row;
+        auto put = [&](int k, float v) {
+          uint32_t hi, lo;
+          split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
+          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
+          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
+          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
+        };
+        for (int c = 0; c < 3; ++c) {
+          const float x = __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));  // pts = ro + rd * z (train_utils.py:67)
+          if (p.inc_xyz && half == 0) put(c, x);
+          for (int f = f0; f < f1; ++f) {
+            float sn, cs;
+            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
+            put(base + 6 * f + c, sn);
+            put(base + 6 * f + 3 + c, cs);
+          }
+        }
+        if (half == 1)  // zero padding up to the operand width (one fp16 k-step = 16 granular)
+          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+      }
+      // ---- per-ray direction term of layers_dir[0]: vb[ray][n] = (sum_k enc_dir(ray)[k] * W[n][H + k] + b[n]) / 16
+      if (p.use_viewdirs) {
+        if (wt < n_rays_wg * 3) {
+          const int jr = wt / 3, c = wt - 3 * jr;
+          const float v = rays[(first_ray + jr) * ray_stride + 8 + c];
+          encode_coord(v, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + jr * 32);
+        }
+        wg_bar();
+        const GemmLayer& gd = p.g[p.n_gemm - 1];
+        for (int i = wt; i < n_rays_wg * gd.n; i += 128) {
+          const int jr = i / gd.n, n = i - jr * gd.n;
+          float a = 0.f;
+          for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[jr * 32 + k], s_wv[k * gd.n + n], a);
+          viewb[jr * vbs + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);  // per-ray bias of layers_dir[0] (x 2048 / 16)
         }
       }
-      FPROF_SINCE(5, _te0);
-      FPROF_COUNT(7);
-    };
-
-    const int n_mine = s ? seq.c1.n : seq.c0.n;
+      fence_proxy_async();  // the tile was written through the generic proxy; wgmma / the bulk store read it via the async proxy
+      wg_bar();             // also publishes viewb
+      if (kTrain && wt == 0) {  // this warpgroup's half of the encoding tile goes to the stash as it is: two bulk stores
+        uint8_t* dst = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * p.enc_cum[0]) + (size_t)tile * tile_bytes(enc_w);
+        const int part = enc_hb / kWG;
+        bulk_s2g(dst + wg * part, enc + wg * part, (uint32_t)part);
+        bulk_s2g(dst + tile_half_bytes(enc_w) + wg * part, enc + enc_hb + wg * part, (uint32_t)part);
+      }
 #pragma unroll 1
-    for (int j = 0; j < n_mine; ++j)
-#pragma unroll 1
-      for (int e = 0; e < E; ++e) run_event(j, e);
-    if (gtid == 0) bulk_wait_all();  // this group's encoding-tile stores
+      for (int e = 0; e < p.n_gemm; ++e) {
+        if (p.g[e].n == kH)
+          fwd_layer<kTrain, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full, bar_empty,
+                                n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+        else
+          fwd_layer<kTrain, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full, bar_empty,
+                                    n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+      }
+    }
+    if (kTrain && wt == 0) bulk_wait_all();  // this warpgroup's encoding-tile stores
   }
-
-  tc_fence_before();
-  __syncthreads();
-#ifdef NERFB200_PROF
-  if (blockIdx.x == 0 && threadIdx.x < 24) g_prof_fwd[threadIdx.x] += s_prof[threadIdx.x];
-#endif
-  if (warp == kMmaWarp) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemCols));
 }
 
 // training = the forward must also write the activation stash for the fused backward (hidden 128 only); the
-// inference forward also runs hidden 256 (one tile in flight per CTA, N = 256 MMAs)
+// inference forward also runs hidden 256 (one warpgroup, 64-point tiles, N = 256 MMAs)
 int tc_supported(const Plan& p, int n_samples, const char* what, bool training) {
   if (p.hidden != 128 && (training || p.hidden != 256)) {
-    set_error("%s impl=1 (tcgen05): hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
+    set_error("%s impl=1 (wgmma): hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
               p.hidden);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (p.dim_xyz_pad > 64 || p.dim_dir > 32) {
-    set_error("%s impl=1 (tcgen05): encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what);
+    set_error("%s impl=1 (wgmma): encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (n_samples > 0 && (kTileRows + n_samples - 1) / n_samples + 1 > kMaxRaysPerTile) {
-    set_error("%s impl=1 (tcgen05): fewer than 16 samples per ray not supported; use impl=0", what);
+    set_error("%s impl=1 (wgmma): fewer than 16 samples per ray not supported; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map(p).n_stages < 2) {
-    set_error("%s impl=1 (tcgen05): network too deep for the shared-memory budget (%d layers); use impl=0", what,
+    set_error("%s impl=1 (wgmma): network too deep for the shared-memory budget (%d layers); use impl=0", what,
               p.n_gemm);
     return NERFB200_ERR_UNSUPPORTED;
   }
@@ -654,18 +452,16 @@ int tc_supported(const Plan& p, int n_samples, const char* what, bool training) 
 template <bool kTrain, int kH>
 static int launch_fwd(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z, int64_t P,
                       int n_samples, float* raw, float* stash, cudaStream_t s, const char* what) {
-  const int64_t tiles = (P + kTileRows - 1) / kTileRows;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  // two tiles in flight per CTA (hidden 128): do not spread fewer than 2 tiles per CTA over more CTAs than needed
-  int64_t want = n_slots(p) == 2 ? (tiles + 1) / 2 : tiles;
-  const int grid = (int)(want < sms ? (want < 1 ? 1 : want) : sms);
+  constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
+  const int64_t tiles = (P + kRows - 1) / kRows;
+  const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // = tiles whenever the stash is written (hidden 128)
+  const int sms = device_sms();
+  const int grid = (int)(tiles < sms ? tiles : sms);
   const size_t bytes = (size_t)smem_map(p).total + 1024;
   auto kern = mlp_fwd_tc_kernel<kTrain, kH>;
   int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes), what);
   if (rc) return rc;
-  kern<<<grid, kThreadsTc, bytes, s>>>(p, blob, rays, ray_stride, z, P, n_samples, tiles, raw, stash);
+  kern<<<grid, kThreads, bytes, s>>>(p, blob, rays, ray_stride, z, P, n_samples, kTrain ? stash_tiles : tiles, raw, stash);
   count_launch();
   return check_cuda(cudaGetLastError(), what);
 }

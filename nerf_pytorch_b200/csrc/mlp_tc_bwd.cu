@@ -1,81 +1,64 @@
-// mlp_tc_bwd.cu -- tcgen05 backward of FlexibleNeRFModel (nerf/models.py:233-256, autograd of train_nerf.py:259) for
-// hidden_size 128: the data-gradient chain AND every weight gradient of a 128-point tile in ONE kernel, so that the
-// per-layer pre-activation gradients G_t never leave the SM (no gradient stash in HBM).
+// mlp_tc_bwd.cu -- Hopper tensor-core (wgmma) backward of FlexibleNeRFModel (nerf/models.py:233-256, autograd of
+// train_nerf.py:259) for hidden_size 128: the data-gradient chain AND every weight gradient of a 128-point tile in ONE
+// kernel, so that the per-layer pre-activation gradients G_t never leave the SM (no gradient stash in HBM).
 //
 //   chain  : G_t = (G_{t+1} W_{t+1}[:, :hidden] + d_raw W_head) (.) relu'(layer t)          (M = points, K = features)
 //   wgrad  : dW_t[n][k] += sum_p G_t[p][n] X_{t-1}[p][k]                                    (M = features n, K = points)
-// Both are 3-term split-precision products on tcgen05.mma.kind::f16 (tc_common.cuh split_f16x2).  The trick that
-// makes the fusion cheap is the operand tile (tc_common.cuh "Operand tiles"): G_t is split into fp16 hi / lo ONCE in
-// the epilogue registers; the registers go to tensor memory (A operand of the chain MMA) and ONCE to a shared-memory
-// tile whose MN-major view is the A operand of the weight-gradient MMAs; the forward stashed every
-// layer's activation X_t as the same kind of tile, so the B operand of the weight-gradient MMAs is a plain bulk copy
-// from HBM.  Nothing is transposed on the CUDA cores.
+// Both are 3-term split-precision products on wgmma with fp16 operands (tc_common.cuh split_f16x2).  G_t is split into
+// fp16 hi / lo ONCE in the epilogue registers and stored ONCE to a shared-memory operand tile (tc_common.cuh "Operand
+// tiles"): its K-major view is the A operand of the chain, its MN-major view the A operand of the weight-gradient MMAs;
+// the forward stashed every layer's activation X_t as the same kind of tile, so the B operand of the weight-gradient
+// MMAs is a plain bulk copy from HBM.  Nothing is transposed on the CUDA cores.
 //
 // Precision: the whole tile runs in ONE power-of-two scale (max |d_raw| of the tile -> [4, 8)): the reduction of a
 // weight gradient runs over points, so rows must share a scale, and rows that are tiny next to the tile's largest
 // contribute below fp32 resolution to dW anyway.  The residual products carry a factor 2^11 (lo = (x - hi) 2^11 on
-// both sides); they are accumulated first and folded in by the scale-input-d form of the first hi*hi MMA
-// (D = A*B + D * 2^-11), so a weight gradient needs ONE accumulator and no pre-scaled operand copies.
+// both sides); they are accumulated first, the accumulator registers are multiplied by 2^-11, then the hi*hi products
+// are added: ONE accumulator per weight gradient and no pre-scaled operand copies.
 //
-// Persistent kernel, one CTA per SM, 512 threads (register file rebalanced between the roles with setmaxnreg):
-//   warps 0-7  epilogue (thread = (point row, column half)): per layer  part A: chain accumulator -> + head term, ReLU
-//              mask, split into hi / lo registers (mixed-precision FMA split at the accumulator's 2^11 scale) ->
-//              TENSOR memory as the chain's A operand (the chain MMA may start);  part B (once the previous layer's
-//              jobs have finished reading the G tile): the same registers -> shared-memory G tile (the jobs may start).
-//   warp 8     MMA issuer: chain MMA of the layer (A = this layer's G from tensor memory, B = weights from the ring:
-//              an SS MMA at N = 128 reads 8 KB of shared memory per 64 cycles, the whole port, so the chain must not
-//              take both operands from there), then the layer's weight-gradient jobs (A = G tile, B = activation tile,
-//              both MN-major from shared memory), the 16-column ray-indicator job that yields the bias gradients and
-//              the per-ray sums of layers_dir[0], and the two narrow heads' jobs with the roles swapped (A = activation
-//              tile, B = d_raw = feature rows 64..79 of the first layer's G tile).
-//   warp 9     weight producer (cp.async.bulk ring, one k-step per stage, two stages per MMA batch)
-//   warp 10    activation-tile producer (hi block / lo block of one job at a time)
-//   warps 12-15 drain (thread = accumulator row): the finished weight-gradient accumulators of the layer (single-
-//              buffered: the next layer's jobs wait for acc_free): tcgen05.ld 32 columns -> unscale -> swizzled 16 KB
-//              staging chunk (two, alternating) -> cp.reduce.async.bulk .add.f32 into the L2-resident gradient blob;
-//              indicator sums -> bias accumulators (shared memory) and the direction-encoding part of
-//              dW(layers_dir[0]) (registers); heads' rows -> atomics.
-// Tensor memory: [0,128) chain accumulator; [128,192) / [192,256) chain A operand hi / lo; [256,400) main job 128 +
-// indicator sums 16; [400,464) the second job of a layer (encoding part of a skip layer / of layer1's neighbour, at
-// most 64 wide); [464,480) / [480,496) the heads' jobs.
-// Measured (A1, 4096 x 192 points): 2.2 ms, tensor pipe 33 %, 4.35 GB of DRAM traffic (profiles/r2_final_*); the MMA warp
-// is occupied for the whole layer (cycle counters: tools/bwd_prof.py on a -DNERFB200_PROF build).
+// Persistent kernel, one CTA per SM, two consumer warpgroups (warpgroup w owns points [64 w, 64 w + 64) of the chain
+// and features [64 w, 64 w + 64) of every weight gradient) and one producer warp streaming the chain's weight copies
+// through a cp.async.bulk ring.  Per layer: epilogue (chain accumulator + head term, ReLU mask, split -> G tile), chain
+// MMA of the warpgroup's rows, then the layer's weight-gradient jobs: A = the G tile (MN-major), B = the activation
+// tile (bulk-copied from the stash one job ahead), the 16-column ray-indicator job that yields the bias gradients and
+// the per-ray sums of layers_dir[0], and the two narrow heads' jobs with the roles swapped (A = activation tile, B =
+// d_raw = feature rows 64..79 of the first layer's G tile).  Finished weight-gradient accumulators are unscaled into
+// a swizzled staging chunk as 64-bit fixed point and added into the L2-resident gradient blob with cp.reduce.async.bulk
+// .add.u64; integer sums do not depend on the order of the adds, so the gradients are reproducible bit for bit.
 #include "common.cuh"
 #include "tc_common.cuh"
+#include "wgmma.cuh"
 
 namespace nerfb200 {
 
 namespace tcb {
-constexpr int kThreadsB = 512;
-constexpr int kDrainWarp0 = 12, kDrainThreads = 128;
-constexpr int kEpi = 256;
+constexpr int kWG = 2;                            // consumer warpgroups
+constexpr int kThreadsB = 128 * kWG + 32;         // + the weight producer warp
 constexpr int kWStage = 96 * 128;                 // one k-step of a 128-wide layer: 3 copies x 2 slabs x 128 x 16 B
 constexpr int kMaxWStages = 6;
 constexpr int kGBytes = 65536;                    // G tile: hi block 32 KB, lo block 32 KB (128 features)
 constexpr int kXBytes = 65536;                    // activation tile of the running job
-constexpr int kStgBytes = 16384;                  // staging chunk: 128 rows x 32 fp32; two alternate
+constexpr int kStgBytes = 8192;                   // staging chunk: 64 rows x 16 fixed-point int64; two alternate per warpgroup
 constexpr int kIndBytes = 4096;                   // ray-indicator tile: 128 points x 16 "features" (hi only)
 constexpr int kMaxRays = 10;
-constexpr uint32_t kTmemColsB = 512;
-// tensor memory: [0,128) chain accumulator, [128,192) / [192,256) the chain's A operand (G tile, hi / lo, two fp16 per
-// column), [256,400) main job (128) + indicator sums (16), [400,464) second job, [464,496) the heads' jobs
-constexpr uint32_t kColAcc = 0, kColAhi = 128, kColAlo = 192, kColMain = 256, kIndOff = 128, kColSecond = 400, kColHead0 = 464;
 constexpr int kSmemLimitB = 232448 - 1024;
 
 struct SmemMapB {
-  int g, x, stg, ind, headw, bgrad, encd, misc, bars, ring, total, n_stages;
+  int g, x, stg, ind, headw, bgrad, encd, sums, dacc, misc, bars, ring, total, n_stages;
 };
 __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   SmemMapB m;
   int off = 0;
   m.g = off;      off += kGBytes;
   m.x = off;      off += kXBytes;
-  m.stg = off;    off += 2 * kStgBytes;
+  m.stg = off;    off += 2 * kWG * kStgBytes;
   m.ind = off;    off += kIndBytes;
   m.headw = off;  off += (4 * 128 + 3 * 64 + 16) * 4;
   m.bgrad = off;  off += (p.enc_cum[0] + 8) * 4;   // bias gradients of every gemm layer + the heads' (8)
   m.encd = off;   off += kMaxRays * 32 * 4;
-  m.misc = off;   off += 256;              // tile maxima / unscale factors (+ the development build's cycle counters)
+  m.sums = off;   off += 64 * 16 * 4;             // per-ray sums of layers_dir[0]'s G (one tile)
+  m.dacc = off;   off += 64 * 28 * 4;             // direction-encoding part of dW(layers_dir[0]), whole kernel
+  m.misc = off;   off += 256;                     // tile maxima
   m.bars = off;   off += 256;
   off = (off + 1023) & ~1023;
   m.ring = off;
@@ -86,15 +69,13 @@ __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   return m;
 }
 
-// One weight-gradient job: accumulator[n][k] = sum_p G[p][n] * B[p][k] over the tile's 128 points.
+// One weight-gradient job: accumulator[n][k] = sum_p A[p][n] * B[p][k] over the tile's 128 points.
 struct BwdJob {
   int src_enc;   // B tile: 1 = the xyz-encoding tile, 0 = the stashed output of gemm layer `src`
   int src;
   int n_b;       // columns = width of the B tile (multiple of 16)
-  int col;       // tensor-memory column of the accumulator (main jobs: of buffer 0; + kMainStride for odd layers)
-  int dbuf;      // unused (the accumulators are single-buffered since the chain's A operand took their columns)
   int row0, nrows;  // accumulator rows that carry gradients
-  int gb_off;    // float offset of this job's block in the gradient blob: [n_b / 32 chunks][128 rows][32] (16 wide: one chunk of 16)
+  int gb_off;    // offset (int64 words) of this job's block in the gradient blob: [n_b / 16 chunks][128 rows][16]
   int dst_head;  // -1: rows are output features of gemm layer `dst`; else head index, rows row0.. are its outputs
   int dst;       // gemm index
   int dst_col0;  // first input column of the destination weight this block covers
@@ -111,21 +92,19 @@ __host__ __device__ inline int bwd_jobs(const Plan& p, int e, BwdJob* out, int* 
     const GemmLayer& g = p.g[t];
     int n = 0;
     BwdJob jb[kMaxJobs];
-    auto add = [&](int src_enc, int src, int n_b, int col, int row0, int nrows, int dst_head, int dst, int dst_col0,
-                   int ncols, int kind) {
+    auto add = [&](int src_enc, int src, int n_b, int row0, int nrows, int dst_head, int dst, int dst_col0, int ncols,
+                   int kind) {
       BwdJob& j = jb[n++];
-      j.src_enc = src_enc; j.src = src; j.n_b = n_b; j.col = col; j.row0 = row0; j.nrows = nrows;
+      j.src_enc = src_enc; j.src = src; j.n_b = n_b; j.row0 = row0; j.nrows = nrows;
       j.gb_off = gb; j.dst_head = dst_head; j.dst = dst; j.dst_col0 = dst_col0; j.ncols = ncols; j.kind = kind;
-      j.dbuf = (col == (int)kColMain) ? 1 : 0;
-      if (kind == 0) gb += ((n_b + 31) / 32) * 128 * 32;
+      if (kind == 0) gb += ((n_b + 15) / 16) * 128 * 16;
     };
-    if (g.k_h > 0) add(0, g.src, g.k_h, (int)kColMain, 0, g.n, -1, t, 0, g.k_h, 0);
-    if (g.k_enc > 0 && g.enc_sel == 0)
-      add(1, 0, p.enc_tile_w, g.k_h > 0 ? (int)kColSecond : (int)kColMain, 0, g.n, -1, t, g.k_h, g.enc_real, 0);
+    if (g.k_h > 0) add(0, g.src, g.k_h, 0, g.n, -1, t, 0, g.k_h, 0);
+    if (g.k_enc > 0 && g.enc_sel == 0) add(1, 0, p.enc_tile_w, 0, g.n, -1, t, g.k_h, g.enc_real, 0);
     if (p.use_viewdirs && t == p.n_gemm - 1) {
       // the narrow heads: dW_head[c][k] = sum_p d_raw[p][c] X[p][k] with the activation tile on the M side
-      add(0, t, g.n, (int)kColHead0, 0, p.h[1].k, 1, t, 0, 16, 1);                               // fc_rgb reads this layer's output
-      add(0, p.h[0].src, p.g[p.h[0].src].n, (int)kColHead0 + 16, 0, p.h[0].k, 0, t, 0, 16, 1);   // fc_alpha reads the trunk output
+      add(0, t, g.n, 0, p.h[1].k, 1, t, 0, 16, 1);                               // fc_rgb reads this layer's output
+      add(0, p.h[0].src, p.g[p.h[0].src].n, 0, p.h[0].k, 0, t, 0, 16, 1);        // fc_alpha reads the trunk output
     }
     if (ev == e && out)
       for (int i = 0; i < n; ++i) out[i] = jb[i];
@@ -141,6 +120,28 @@ struct BwdPlan {
   BwdJob jobs[kMaxGemm][kMaxJobs];
   int gb_total;
 };
+// The gradient blob: ONE L2-resident buffer of 64-bit fixed-point sums (value * 2^32, two's complement) that every CTA
+// adds into.  Integer addition is associative, so the sums -- and the gradients -- are the same bits whatever order the
+// CTAs' reduce-adds and atomics arrive in.  Resolution 2^-32 (2.3e-10) per added term; every partial sum must stay
+// below 2^31 in magnitude.
+//   [0, gb_total)  weight-gradient blocks of the jobs (bulk reduce-add .u64 from the staging chunks)
+//   xb: bias gradients of the gemm layers (cum_n order) + the heads' 4 biases (+ 4 spare)
+//   xd: direction-encoding part of dW(layers_dir[0]) [64][28]
+//   xh: the heads' weight gradients [head][4 outputs][128 inputs]
+constexpr float kFix = 4294967296.f;   // 2^32
+struct BlobMap {
+  int xb, xd, xh, words;
+};
+__host__ __device__ inline BlobMap blob_map(const Plan& p, int gb_total) {
+  BlobMap m;
+  m.xb = gb_total;
+  m.xd = m.xb + p.enc_cum[0] + 8;
+  m.xh = m.xd + 64 * 28;
+  m.words = (m.xh + 2 * 4 * 128 + 15) & ~15;
+  return m;
+}
+__device__ __forceinline__ unsigned long long to_fix(float v) { return (unsigned long long)__float2ll_rn(v * kFix); }
+
 inline BwdPlan make_bwd_plan(const Plan& p) {
   BwdPlan bp;
   for (int e = 0; e < p.n_gemm; ++e) bp.n_jobs[e] = bwd_jobs(p, e, bp.jobs[e]);
@@ -153,58 +154,96 @@ inline BwdPlan make_bwd_plan(const Plan& p) {
 using namespace tc;
 using namespace tcb;
 
-// Development build only (make EXTRA=-DNERFB200_PROF): CTA 0 adds up the cycles its roles spend in each phase.
-#ifdef NERFB200_PROF
-__device__ unsigned long long g_prof[32];
-// counters live in shared memory (lane 0 of warps 0, 8, 9, 10, 12 of CTA 0 record), flushed to g_prof when the kernel ends
-#define PROF_DECL uint32_t* s_prof = reinterpret_cast<uint32_t*>(sm + mp.misc + 64); if (threadIdx.x < 32) s_prof[threadIdx.x] = 0u;
-#define PROF_ON (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (threadIdx.x < 32 || (threadIdx.x >= 256 && threadIdx.x < 352) || (threadIdx.x >= 384 && threadIdx.x < 416)))
-#define PROF_SCOPE(i, stmt) do { const long long _ps = clock64(); stmt; if (PROF_ON) s_prof[i] += (uint32_t)(clock64() - _ps); } while (0)
-#define PROF_MARK(name) const long long name = clock64()
-#define PROF_SINCE(i, name) do { if (PROF_ON) s_prof[i] += (uint32_t)(clock64() - name); } while (0)
-#define PROF_FLUSH do { __syncthreads(); if (blockIdx.x == 0 && threadIdx.x < 32) g_prof[threadIdx.x] += s_prof[threadIdx.x]; } while (0)
-#else
-#define PROF_DECL
-#define PROF_SCOPE(i, stmt) do { stmt; } while (0)
-#define PROF_MARK(name)
-#define PROF_SINCE(i, name)
-#define PROF_FLUSH
-#endif
+__device__ __forceinline__ void cta_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // both warpgroups
 
-__device__ __forceinline__ void bar_half(int half) {  // the 128 threads of one column half
-  asm volatile("bar.sync %0, 128;" ::"r"(2 + half) : "memory");
+// weight-gradient job of width N (columns of the B tile) for this warpgroup's 64 accumulator rows:
+//   acc = 2^-11 sum_ks (A_lo^T B_hi + A_hi^T B_lo) + sum_ks A_hi^T B_hi     (A, B MN-major; K = the tile's 128 points)
+// plus, when `ind`, the 16-column indicator product into acc_i (B = the exact 0 / 1 indicator tile, no lo part)
+template <int N>
+__device__ __forceinline__ void job_mma(float (&acc)[N / 2], float (&acc_i)[8], bool ind, uint64_t a_hi, uint32_t a_lo_off,
+                                        uint32_t a_ks, uint64_t b_hi, uint32_t b_lo_off, uint32_t b_ks, uint64_t i_d) {
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) {
+    const uint64_t ah = desc_adv(a_hi, ks * a_ks), bh = desc_adv(b_hi, ks * b_ks);
+    wgmma_f16<N, 1, 1>(acc, desc_adv(ah, a_lo_off), bh, ks > 0 ? 1 : 0);
+    wgmma_f16<N, 1, 1>(acc, ah, desc_adv(bh, b_lo_off), 1);
+    if (ind) wgmma_f16<16, 1, 1>(acc_i, desc_adv(ah, a_lo_off), desc_adv(i_d, ks * 512u), ks > 0 ? 1 : 0);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(acc);
+  reg_fence(acc_i);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] *= kLoInv;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc_i[i] *= kLoInv;
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) {
+    const uint64_t ah = desc_adv(a_hi, ks * a_ks);
+    wgmma_f16<N, 1, 1>(acc, ah, desc_adv(b_hi, ks * b_ks), 1);
+    if (ind) wgmma_f16<16, 1, 1>(acc_i, ah, desc_adv(i_d, ks * 512u), 1);
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(acc);
+  reg_fence(acc_i);
+}
+
+// the finished accumulator (64 rows of this warpgroup x N columns) -> unscale -> fixed point -> swizzled staging chunks
+// -> bulk reduce-add into the job's block of the gradient blob ([chunk][128 rows][16 words], the eight 16-byte pieces
+// of a row XOR-swizzled by row & 7)
+template <int N>
+__device__ __forceinline__ void job_drain(const float (&acc)[N / 2], float us, unsigned long long* gdst,
+                                          unsigned long long* stg, uint32_t& stg_n, int wg) {
+  const int wt = threadIdx.x & 127, lane = wt & 31, q = lane & 3;
+  const int r0 = 16 * (wt >> 5) + (lane >> 2);
+#pragma unroll
+  for (int c = 0; c < (N + 15) / 16; ++c) {
+    unsigned long long* sb = stg + (stg_n & 1u) * (kStgBytes / 8);
+    if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      const int j = 2 * c + jj;
+      if (j < N / 8) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int r = r0 + 8 * i, piece = 4 * jj + q;  // columns 8 jj + 2 q, + 1 of the chunk
+          *reinterpret_cast<ulonglong2*>(sb + r * 16 + 2 * (piece ^ (r & 7))) =
+              make_ulonglong2(to_fix(acc[4 * j + 2 * i] * us), to_fix(acc[4 * j + 2 * i + 1] * us));
+        }
+      }
+    }
+    fence_proxy_async();
+    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+    if (wt == 0) bulk_reduce_add_u64(gdst + (size_t)c * 2048 + 64 * wg * 16, sb, 64u * 128u);
+    ++stg_n;
+  }
 }
 
 __global__ void __launch_bounds__(kThreadsB, 1)
 mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P, int S,
-                  int64_t n_tiles, float* __restrict__ gblob, float* __restrict__ flat_grad,
+                  int64_t n_tiles, float* __restrict__ gblob,
                   const __grid_constant__ BwdPlan bp) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const SmemMapB mp = smem_map_b(p);
-  PROF_DECL
   uint8_t* sG = sm + mp.g;
   uint8_t* sX = sm + mp.x;
   uint8_t* sInd = sm + mp.ind;
   float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
   float* s_bgrad = reinterpret_cast<float*>(sm + mp.bgrad);
   float* s_encd = reinterpret_cast<float*>(sm + mp.encd);
+  float* s_sums = reinterpret_cast<float*>(sm + mp.sums);
+  float* s_dacc = reinterpret_cast<float*>(sm + mp.dacc);
   uint32_t* s_max = reinterpret_cast<uint32_t*>(sm + mp.misc);      // [2]: tile max of |d_raw| (alternating tiles)
-  float* s_us = reinterpret_cast<float*>(sm + mp.misc) + 2;         // [2]: the tile's unscale factor, for the drain
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + mp.bars);
   uint64_t* w_full = bars;                      // [kMaxWStages]
   uint64_t* w_empty = bars + kMaxWStages;       // [kMaxWStages]
-  uint64_t* bar_acc = bars + 2 * kMaxWStages;   // chain MMA complete
-  uint64_t* bar_g = bar_acc + 1;                // G tile (+ indicator tile) written to shared memory (the jobs' A operand)
-  uint64_t* xh_full = bar_g + 1;
-  uint64_t* xl_full = xh_full + 1;
-  uint64_t* xh_free = xl_full + 1;
-  uint64_t* xl_free = xh_free + 1;
-  uint64_t* job_done = xl_free + 1;             // [2][kMaxJobs]: job i of a layer of that parity complete
-  uint64_t* acc_free = job_done + 2 * kMaxJobs; // [0]: the drain is done with the layer's accumulators
-  uint64_t* bar_a = acc_free + 2;               // the chain's A operand (this layer's G, hi / lo) is in tensor memory
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bar_a + 1);
+  uint64_t* x_full = bars + 2 * kMaxWStages;    // the running job's activation tile landed
   const uint32_t n_stages = (uint32_t)mp.n_stages;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -212,50 +251,32 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   const int E = p.n_gemm;
   const int hw1 = p.h[0].n_out * p.h[0].k;
   const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
+  const BlobMap bm = blob_map(p, bp.gb_total);
+  unsigned long long* gb = reinterpret_cast<unsigned long long*>(gblob);
 
   if (tid == 0) {
     for (int i = 0; i < kMaxWStages; ++i) {
       mbar_init(&w_full[i], 1);
-      mbar_init(&w_empty[i], 1);
+      mbar_init(&w_empty[i], 4 * kWG);
     }
-    mbar_init(bar_acc, 1);
-    mbar_init(bar_g, kEpi);
-    mbar_init(bar_a, kEpi);
-    mbar_init(xh_full, 1);
-    mbar_init(xl_full, 1);
-    mbar_init(xh_free, 1);
-    mbar_init(xl_free, 1);
-    for (int i = 0; i < 2 * kMaxJobs; ++i) mbar_init(&job_done[i], 1);
-    mbar_init(&acc_free[0], kDrainThreads);
-    mbar_init(&acc_free[1], kDrainThreads);
+    mbar_init(x_full, 1);
     fence_barrier_init();
     s_max[0] = s_max[1] = 0u;
-  }
-  if (warp == 8) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "r"(kTmemColsB));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
   }
   // head weights at the chain accumulator's 2^11 scale (the epilogue works on Y = 2048 y, tc_common.cuh split_f16x2_y)
   for (int i = tid; i < hw1; i += kThreadsB) s_headw[i] = blob[p.h[0].w_off + i] * kLoScale;
   for (int i = tid; i < hw2; i += kThreadsB) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kLoScale;
   for (int i = tid; i < p.enc_cum[0] + 8; i += kThreadsB) s_bgrad[i] = 0.f;
   for (int i = tid; i < kMaxRays * 32; i += kThreadsB) s_encd[i] = 0.f;
+  for (int i = tid; i < 64 * 28; i += kThreadsB) s_dacc[i] = 0.f;
   for (int i = tid; i < kGBytes / 16; i += kThreadsB) reinterpret_cast<uint4*>(sG)[i] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *s_tmem;
 
   const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
 
-  // 512 threads start with 128 registers each; the epilogue warpgroups take what the others give back
-  // (setmaxnreg sits at the top of each role's branch so that the register allocator sees the role's budget)
-  if (warp >= 8 && warp < kDrainWarp0) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-  if (warp == 9) {
-    // ===================== weight producer: the chain MMA of event e streams layer t's transposed copies ============
+  if (warp == 4 * kWG) {
+    // ===================== weight producer: the chain of event e streams layer t's transposed copies ============
     if (lane == 0) {
       Pipe pp;
       const uint64_t pol = l2_policy_evict_last();
@@ -265,571 +286,362 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
           const uint8_t* src = reinterpret_cast<const uint8_t*>(blob + g.tcd_off);
           const uint32_t kbytes = 96u * (uint32_t)g.k_h;
           for (int ks = 0; ks < (g.n >> 4); ++ks) {
-            PROF_SCOPE(18, mbar_wait(&w_empty[pp.stage], pp.phase ^ 1));
+            mbar_wait(&w_empty[pp.stage], pp.phase ^ 1);
             mbar_arrive_expect_tx(&w_full[pp.stage], kbytes);
             bulk_g2s_hint(sm + mp.ring + pp.stage * kWStage, src + (size_t)ks * kbytes, kbytes, &w_full[pp.stage], pol);
             pp.advance(n_stages);
           }
         }
     }
-  } else if (warp == 10) {
-    // ===================== activation-tile producer: lo block, then hi block of every job, in job order ============
-    if (lane == 0) {
-      uint32_t ph = 0;  // phase of the free barriers this job waits on (flips once per job)
-      for (int it = 0; it < my_tiles; ++it) {
-        const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-        for (int e = 0; e < E; ++e) {
-          const int nj = bp.n_jobs[e];
-          for (int i = 0; i < nj; ++i) {
-            const BwdJob& jq = bp.jobs[e][i];
-            const int w = jq.n_b;
-            const uint8_t* src = reinterpret_cast<const uint8_t*>(
-                                     stash + (size_t)P_pad * (jq.src_enc ? p.enc_cum[0] : p.g[jq.src].cum_n)) +
-                                 (size_t)tile * tile_bytes(w);
-            const uint32_t hb = (uint32_t)tile_half_bytes(w);
-            PROF_SCOPE(16, mbar_wait(xl_free, ph ^ 1));
-            mbar_arrive_expect_tx(xl_full, hb);
-            bulk_g2s(sX + 32768, src + hb, hb, xl_full);
-            PROF_SCOPE(17, mbar_wait(xh_free, ph ^ 1));
-            mbar_arrive_expect_tx(xh_full, hb);
-            bulk_g2s(sX, src, hb, xh_full);
-            ph ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 8) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    Pipe pp;
-    uint32_t g_ph = 0, a_ph = 0, x_ph = 0, gev = 0;  // gev: layers processed so far
-    uint32_t free_ph = 0;
-    const uint32_t t_acc = tmem + kColAcc, t_ahi = tmem + kColAhi, t_alo = tmem + kColAlo;
-    // every descriptor is built ONCE; the loops only advance start-address fields (tc_common.cuh desc_adv)
-    const uint64_t g_hi_m = make_desc(smem_u32(sG), 2048, 128), g_lo_m = desc_adv(g_hi_m, 32768);    // MN-major view (job A)
-    const uint64_t ind_d = make_desc(smem_u32(sInd), 256, 128);
-    // d_raw as a 16-column operand (heads' jobs, first layer of a tile): feature rows 64..79 of that layer's G tile
-    // (rows 64..67 carry d_raw, the rest is zero): MN-major view, 8-point blocks 2048 B apart
-    const uint64_t d_hi_d = make_desc(smem_u32(sG) + 1024, 2048, 128), d_lo_d = desc_adv(d_hi_d, 32768);
-    const uint32_t x_hi_a = smem_u32(sX), x_lo_a = x_hi_a + 32768;
-    for (int it = 0; it < my_tiles; ++it)
-      for (int e = 0; e < E; ++e, ++gev) {
-        const GemmLayer& g = p.g[E - 1 - e];
-        PROF_MARK(_tm0);
-        PROF_SCOPE(8, mbar_wait(bar_a, a_ph));
-        a_ph ^= 1;
-        tc_fence_after();
-        if (e + 1 < E) {
-          // ---- chain: accumulator[p][k] = 2^11 sum_n G_t[p][n] W_t[n][k], N = k_h, K = n; A = this layer's G from
-          // TENSOR memory (the epilogue stores the hi / lo registers there first: the chain neither waits for the
-          // shared-memory tile nor reads it -- an SS MMA at N = 128 alone saturates the shared-memory port)
-          const uint32_t idesc = make_idesc_f16(g.k_h);
-          const uint32_t slab_b = 16u * (uint32_t)g.k_h;
-          const uint64_t b_ring = make_desc(smem_u32(sm + mp.ring), slab_b, 128);
-          // two ring stages (k-steps) per batch: six MMAs back to back, the stage hand-over is paid half as often
-          for (int ks = 0; ks < (g.n >> 4); ks += 2) {
-            const uint32_t st0 = pp.stage;
-            PROF_SCOPE(9, mbar_wait(&w_full[st0], pp.phase));
-            pp.advance(n_stages);
-            const uint32_t st1 = pp.stage;
-            PROF_SCOPE(9, mbar_wait(&w_full[st1], pp.phase));   // g.n is a multiple of 32: k-steps come in pairs
-            pp.advance(n_stages);
-            tc_fence_after();
-            if (elect_one()) {
-#pragma unroll
-              for (int hb = 0; hb < 2; ++hb) {
-                const uint32_t st = hb ? st1 : st0;
-                const uint64_t b_hs = desc_adv(b_ring, st * (uint32_t)kWStage);
-                const uint64_t b_h = desc_adv(b_hs, 2 * slab_b);
-                const uint64_t b_l = desc_adv(b_hs, 4 * slab_b);
-                mma_ts_f16(t_acc, t_ahi + 8 * (ks + hb), b_hs, idesc, (ks + hb) > 0 ? 1u : 0u);
-                mma_ts_f16(t_acc, t_alo + 8 * (ks + hb), b_h, idesc, 1u);
-                mma_ts_f16(t_acc, t_ahi + 8 * (ks + hb), b_l, idesc, 1u);
-                mma_commit(&w_empty[st]);
-              }
-            }
-            __syncwarp();
-          }
-          if (elect_one()) mma_commit(bar_acc);
-          __syncwarp();
-        }
-        // ---- weight-gradient jobs of this event: A = the G tile in shared memory (MN-major view); the accumulators
-        // are single-buffered: the drain must be done with the previous layer's
-        PROF_SINCE(14, _tm0);
-        PROF_MARK(_tm1);
-        PROF_SCOPE(10, mbar_wait(bar_g, g_ph));
-        g_ph ^= 1;
-        tc_fence_after();
-        if (gev >= 1) {
-          PROF_SCOPE(13, mbar_wait(&acc_free[0], free_ph));
-          free_ph ^= 1;
-          tc_fence_after();
-        }
-        const int nj = bp.n_jobs[e];
-        for (int i = 0; i < nj; ++i) {
-          const BwdJob& jq = bp.jobs[e][i];
-          const int w = jq.n_b;
-          const uint32_t fstr = (uint32_t)(w >> 3) * 128u;  // bytes between 8-point blocks of the activation tile
-          const uint32_t d = tmem + (uint32_t)jq.col;
-          const uint64_t x_hi_d = make_desc(x_hi_a, fstr, 128), x_lo_d = make_desc(x_lo_a, fstr, 128);  // MN-major views
-          if (jq.kind == 1) {
-            // head job: A = activation tile (rows = its features: SBO 128, K = points: LBO fstr), B = d_raw tile (N = 16)
-            const uint32_t id16 = make_idesc_f16_mn(16, 1, 1);
-            PROF_SCOPE(11, mbar_wait(xl_full, x_ph));
-            tc_fence_after();
-            if (elect_one()) {
-#pragma unroll
-              for (int ks = 0; ks < 8; ++ks)
-                mma_ss_f16(d, desc_adv(x_lo_d, ks * 2 * fstr), desc_adv(d_hi_d, ks * 4096), id16, ks > 0 ? 1u : 0u);
-              mma_commit(xl_free);
-            }
-            __syncwarp();
-            PROF_SCOPE(12, mbar_wait(xh_full, x_ph));
-            tc_fence_after();
-            x_ph ^= 1;
-            if (elect_one()) {
-#pragma unroll
-              for (int ks = 0; ks < 8; ++ks)
-                mma_ss_f16(d, desc_adv(x_hi_d, ks * 2 * fstr), desc_adv(d_lo_d, ks * 4096), id16, 1u);
-              mma_ss_f16_scale11(d, x_hi_d, d_hi_d, id16);
-#pragma unroll
-              for (int ks = 1; ks < 8; ++ks)
-                mma_ss_f16(d, desc_adv(x_hi_d, ks * 2 * fstr), desc_adv(d_hi_d, ks * 4096), id16, 1u);
-              mma_commit(xh_free);
-              mma_commit(&job_done[i]);
-            }
-            __syncwarp();
-            continue;
-          }
-          const uint32_t id_mn = make_idesc_f16_mn(w, 1, 1);
-          // A = G^T: rows = features (SBO 128), K = points (LBO 16 * 128); one k-step = 16 points = 2 point blocks
-          PROF_SCOPE(11, mbar_wait(xl_full, x_ph));
-          tc_fence_after();
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-              mma_ss_f16(d, desc_adv(g_hi_m, ks * 4096), desc_adv(x_lo_d, ks * 2 * fstr), id_mn, ks > 0 ? 1u : 0u);
-            mma_commit(xl_free);
-          }
-          __syncwarp();
-          PROF_SCOPE(12, mbar_wait(xh_full, x_ph));
-          tc_fence_after();
-          x_ph ^= 1;
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < 8; ++ks)
-              mma_ss_f16(d, desc_adv(g_lo_m, ks * 4096), desc_adv(x_hi_d, ks * 2 * fstr), id_mn, 1u);
-            mma_ss_f16_scale11(d, g_hi_m, x_hi_d, id_mn);
-#pragma unroll
-            for (int ks = 1; ks < 8; ++ks)
-              mma_ss_f16(d, desc_adv(g_hi_m, ks * 4096), desc_adv(x_hi_d, ks * 2 * fstr), id_mn, 1u);
-            mma_commit(xh_free);
-#if defined(NERFB200_EXPB) && (NERFB200_EXPB & 2)   // timing experiment: no indicator MMAs
-            if (false) {
-#else
-            if (i == 0) {
-#endif
-              // indicator job: sums[n][j] = sum over the points of ray j of the tile of G[p][n] (16 columns)
-              const uint32_t id16 = make_idesc_f16_mn(16, 1, 1);
-              const uint32_t di = d + kIndOff;
-#pragma unroll
-              for (int ks = 0; ks < 8; ++ks)
-                mma_ss_f16(di, desc_adv(g_lo_m, ks * 4096), desc_adv(ind_d, ks * 512), id16, ks > 0 ? 1u : 0u);
-              mma_ss_f16_scale11(di, g_hi_m, ind_d, id16);
-#pragma unroll
-              for (int ks = 1; ks < 8; ++ks)
-                mma_ss_f16(di, desc_adv(g_hi_m, ks * 4096), desc_adv(ind_d, ks * 512), id16, 1u);
-            }
-            mma_commit(&job_done[i]);
-          }
-          __syncwarp();
-        }
-        PROF_SINCE(15, _tm1);
-      }
-  }
-  } else if (warp >= kDrainWarp0) {
-    // ===================== drain warps: thread = accumulator row (tensor-memory lane) =====================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-    const int row = tid - kDrainWarp0 * 32;
-    const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
-    float* stg = reinterpret_cast<float*>(sm + mp.stg);
-    float dacc[28];  // direction-encoding part of dW(layers_dir[0]) for output feature `row` (< 64), whole kernel
-#pragma unroll
-    for (int k = 0; k < 28; ++k) dacc[k] = 0.f;
-    uint32_t stg_n = 0, gev = 0;  // chunks staged so far (selects one of the two staging buffers); layers drained
-    uint32_t job_ph[kMaxJobs] = {0u, 0u, 0u};
-    for (int it = 0; it < my_tiles; ++it) {
-      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
-      const int64_t p0 = tile * kTileRows;
-      const int64_t last_pt = (p0 + kTileRows - 1 < P) ? p0 + kTileRows - 1 : P - 1;
-      const int n_rays_tile = (int)(last_pt / S - p0 / S) + 1;
-      for (int de = 0; de < E; ++de, ++gev) {
-        const int nj = bp.n_jobs[de];
-        const GemmLayer& g = p.g[E - 1 - de];
-        for (int i = 0; i < nj; ++i) {
-          PROF_SCOPE(3, mbar_wait(&job_done[i], job_ph[i]));
-          job_ph[i] ^= 1;
-          tc_fence_after();
-          const float us = s_us[it & 1];  // written by the epilogue before this tile's first job could be issued
-          const BwdJob& j = bp.jobs[de][i];
-          const uint32_t jcol = (uint32_t)j.col;
-          if (j.kind == 1) {
-            // head job: lane = input feature k of the head, columns = d_raw channels: dW_head[c][k], a handful of atomics
-            uint32_t v16[16];
-            tmem_ld16(tmem + lane_base + jcol, v16);
-            tmem_wait_ld();
-            const HeadLayer& h = p.h[j.dst_head];
-            if (row < h.k)
-              for (int c = 0; c < h.n_out; ++c)
-                atomicAdd(flat_grad + h.flat_w + (size_t)c * h.k + row, __uint_as_float(v16[(h.out_col + c) & 15]) * us);
-            continue;
-          }
-          // 32-column chunks through two alternating 16 KB staging buffers: a buffer is rewritten only after the bulk
-          // reduction issued two chunks ago has finished reading it.  Rows are 128 bytes; the eight 16-byte pieces of a
-          // row are XOR-swizzled by (row & 7) so that a warp's stores spread over all banks.  (Tried and rejected:
-          // red.global.add.v4.f32 straight from the registers -- 1.3 cycles per lane on the SM side and every CTA hits
-          // the same L2 lines: 2.37 -> 2.76 ms.)  A 48-wide job's second chunk carries 16 columns of padding.
-          const int nchunk = (j.n_b + 31) >> 5;
-          PROF_MARK(_td0);
-          for (int c = 0; c < nchunk; ++c) {
-            uint32_t v[32];
-            tmem_ld32(tmem + lane_base + jcol + 32 * c, v);
-#if defined(NERFB200_EXPB) && (NERFB200_EXPB & 1)   // timing experiment: drain without staging / reduction
-            tmem_wait_ld();
-            continue;
-#endif
-            float* sb = stg + (stg_n & 1u) * (kStgBytes / 4);
-            if (row == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-            bar_half(0);
-            tmem_wait_ld();
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              *reinterpret_cast<float4*>(sb + row * 32 + ((q ^ (row & 7)) << 2)) =
-                  make_float4(__uint_as_float(v[4 * q]) * us, __uint_as_float(v[4 * q + 1]) * us,
-                              __uint_as_float(v[4 * q + 2]) * us, __uint_as_float(v[4 * q + 3]) * us);
-            fence_proxy_async();
-            bar_half(0);
-            if (row == 0)
-              bulk_reduce_add_f32(gblob + j.gb_off + (size_t)c * 4096 + j.row0 * 32, sb + j.row0 * 32, (uint32_t)j.nrows * 128u);
-            ++stg_n;
-          }
-          PROF_SINCE(6, _td0);
-          if (i == 0) {
-            // indicator sums of this layer: bias gradient (all rays) and, for layers_dir[0], the direction-encoding part
-            uint32_t v16[16];
-            tmem_ld16(tmem + lane_base + jcol + kIndOff, v16);
-            tmem_wait_ld();
-            float tot = 0.f;
-#pragma unroll
-            for (int q = 0; q < 16; ++q) tot += __uint_as_float(v16[q]);
-            const float su = us * kActScale;  // the indicator is an exact 1, not an activation / 16
-            if (row < g.n) s_bgrad[g.cum_n + row] += tot * su;
-            if (de == 0 && p.use_viewdirs) {
-              if (row >= 64 && row < 68) s_bgrad[p.enc_cum[0] + row - 64] += tot * su;  // d_rgb, d_sigma sums
-#pragma unroll
-              for (int k = 0; k < 28; ++k) {
-                if (k < p.dim_dir) {
-                  float a = 0.f;
-#pragma unroll
-                  for (int q = 0; q < kMaxRays; ++q)
-                    if (q < n_rays_tile) a = fmaf(__uint_as_float(v16[q]), s_encd[q * 32 + k], a);
-                  dacc[k] = fmaf(a, su, dacc[k]);
-                }
-              }
-            }
-          }
-        }
-        tc_fence_before();
-        mbar_arrive(&acc_free[0]);
-      }
-    }
-    if (row == 0) bulk_wait_all();
-    bar_half(0);
-    // ---- flush the bias / direction-encoding accumulators of this CTA
-    for (int gi = 0; gi < p.n_gemm; ++gi)
-      for (int i = row; i < p.g[gi].n; i += kDrainThreads) atomicAdd(flat_grad + p.g[gi].flat_b + i, s_bgrad[p.g[gi].cum_n + i]);
-    if (p.use_viewdirs) {
-      const GemmLayer& gd = p.g[p.n_gemm - 1];
-      const int in_real = gd.k_h + gd.enc_real;
-      if (row < gd.n) {
-#pragma unroll
-        for (int k = 0; k < 28; ++k)
-          if (k < p.dim_dir) atomicAdd(flat_grad + gd.flat_w + (size_t)row * in_real + gd.k_h + k, dacc[k]);
-      }
-      if (row < 3) atomicAdd(flat_grad + p.h[1].flat_b + row, s_bgrad[p.enc_cum[0] + row]);
-      if (row == 3) atomicAdd(flat_grad + p.h[0].flat_b, s_bgrad[p.enc_cum[0] + 3]);
-    }
   } else {
-    // ===================== epilogue warps =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-    const int row = tid & 127, half = tid >> 7;
-    const uint32_t lane_base = ((uint32_t)((warp & 3) * 32)) << 16;
-    const uint32_t t_acc = tmem + lane_base + kColAcc;
-    uint32_t acc_ph = 0, gev = 0;  // gev: layers processed so far (parity of the job barriers)
-    uint32_t job_ph[kMaxJobs] = {0u, 0u, 0u};
-    int prev_e = -1;  // the previous layer: its jobs must have finished reading the G tile before this layer's is written
-
-    auto wait_jobs = [&](const int de) {  // every job of that layer complete
-      const int nj = bp.n_jobs[de];
-      for (int i = 0; i < nj; ++i) {
-        PROF_SCOPE(2, mbar_wait(&job_done[i], job_ph[i]));
-        job_ph[i] ^= 1;
-      }
-      tc_fence_after();
+    // ===================== consumer warpgroups =====================
+    const int wg = warp >> 2, wt = tid & 127, q = lane & 3;
+    const int r0 = 16 * (wt >> 5) + (lane >> 2);   // warpgroup-local row of accumulator row 0 (row 1: + 8)
+    unsigned long long* stg = reinterpret_cast<unsigned long long*>(sm + mp.stg) + wg * 2 * (kStgBytes / 8);
+    uint32_t stg_n = 0, x_ph = 0;
+    Pipe pp;
+    // activation tile of job (it, e, i): hi block, lo block (issued by thread 0 one job ahead)
+    auto issue_x = [&](int it, int e, int i) {
+      const BwdJob& jq = bp.jobs[e][i];
+      const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
+      const uint8_t* src = reinterpret_cast<const uint8_t*>(stash + (size_t)P_pad * (jq.src_enc ? p.enc_cum[0] : p.g[jq.src].cum_n)) +
+                           (size_t)tile * tile_bytes(jq.n_b);
+      const uint32_t hb = (uint32_t)tile_half_bytes(jq.n_b);
+      mbar_arrive_expect_tx(x_full, 2 * hb);
+      bulk_g2s(sX, src, hb, x_full);
+      bulk_g2s(sX + 32768, src + hb, hb, x_full);
     };
+    if (tid == 0 && my_tiles > 0) issue_x(0, 0, 0);
 
     for (int it = 0; it < my_tiles; ++it) {
       const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
       const int64_t p0 = tile * kTileRows;
-      int64_t pt = p0 + row;
-      const bool valid = pt < P;
-      if (!valid) pt = P - 1;
       const int64_t first_ray = p0 / S;
       const int64_t last_pt = (p0 + kTileRows - 1 < P) ? p0 + kTileRows - 1 : P - 1;
       const int n_rays_tile = (int)(last_pt / S - first_ray) + 1;
-      const int ray_slot = (int)(pt / S - first_ray);
+      int64_t pt[2];
+      bool valid[2];
+      int ray_slot[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        pt[i] = p0 + 64 * wg + r0 + 8 * i;
+        valid[i] = pt[i] < P;
+        if (!valid[i]) pt[i] = P - 1;
+        ray_slot[i] = (int)(pt[i] / S - first_ray);
+      }
       // ---- tile scale: max |d_raw| -> [4, 8)
-      const float4 d4 = valid ? reinterpret_cast<const float4*>(d_raw)[pt] : make_float4(0.f, 0.f, 0.f, 0.f);
       {
+        const int rowm = tid & 127;
+        const float4 d4 = (p0 + rowm < P && tid < 128) ? reinterpret_cast<const float4*>(d_raw)[p0 + rowm]
+                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
         const float m = fmaxf(fmaxf(fabsf(d4.x), fabsf(d4.y)), fmaxf(fabsf(d4.z), fabsf(d4.w)));
         uint32_t mb = __float_as_uint(m);
         mb = __reduce_max_sync(0xffffffffu, mb);
         if (lane == 0) atomicMax(&s_max[it & 1], mb);
-        epi_bar256();
+        cta_bar();
         if (tid == 0) s_max[(it + 1) & 1] = 0u;  // reset the other slot for the next tile
       }
       const uint32_t ex = (s_max[it & 1] >> 23) & 0xFFu;
       const bool scaled = ex >= 3u && ex <= 254u;
       const float sc = scaled ? __uint_as_float((256u - ex) << 23) : 1.f;
-      const float unscale = (scaled ? __uint_as_float((ex - 2u) << 23) : 1.f) * kActInv;  // activations are stored / 16
-      const float dr[4] = {d4.x * sc, d4.y * sc, d4.z * sc, d4.w * sc};
-      if (tid == 0) s_us[it & 1] = unscale;
+      const float us = (scaled ? __uint_as_float((ex - 2u) << 23) : 1.f) * kActInv;  // activations are stored / 16
+      float dr[2][4];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float4 d4 = valid[i] ? reinterpret_cast<const float4*>(d_raw)[pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
+        dr[i][0] = d4.x * sc; dr[i][1] = d4.y * sc; dr[i][2] = d4.z * sc; dr[i][3] = d4.w * sc;
+      }
 
+      float chain[64];  // G_{t+1} W_{t+1}[:, :128] of this warpgroup's rows (the previous event's chain MMA)
+#pragma unroll
+      for (int i = 0; i < 64; ++i) chain[i] = 0.f;
       for (int e = 0; e < E; ++e) {
         const int t = E - 1 - e;
         const GemmLayer& g = p.g[t];
-        const bool has_mma = e >= 1;
         int hsel = -1;
         if (p.h[0].src == t) hsel = 0;
         if (p.n_head > 1 && p.h[1].src == t) hsel = 1;
         const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
         const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
         const int hcol = hsel >= 0 ? p.h[hsel].out_col : 0;
-        // this row's ReLU mask words (fetched before the accumulator wait)
-        uint32_t mw[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
-        if (g.relu) {
-          const uint32_t* mask_row = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) +
-                                     (size_t)pt * (g.n >> 5);
-          mw[0] = valid ? __ldg(mask_row + half) : 0u;
-          mw[1] = (valid && g.n == 128) ? __ldg(mask_row + 2 + half) : 0u;
-        }
-        if (has_mma) {
-          PROF_SCOPE(0, mbar_wait(bar_acc, acc_ph));
-          acc_ph ^= 1;
-          tc_fence_after();
-        }
-        PROF_MARK(_ta);
-        // ---------------- part A: G_t of this row -> hi / lo registers and tensor memory ----------------
-        // (both column chunks are pulled out of the accumulator before any arithmetic; the head term only exists for
-        // the two layers a head reads and stays out of the hot loop)
-        const int nch = g.n >> 6;
-        uint32_t hi[2][16], lo[2][16];
-        {
-          uint32_t v[2][32];
-          if (has_mma) {
-            tmem_ld32(t_acc + 32 * half, v[0]);
-            if (nch == 2) tmem_ld32(t_acc + 64 + 32 * half, v[1]);
-            tmem_wait_ld();
+        // this thread's ReLU mask words (two rows, up to four 32-column words each)
+        uint32_t mw[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int m = 0; m < 4; ++m) {
+            mw[i][m] = 0xFFFFFFFFu;
+            if (g.relu && m < (g.n >> 5)) {
+              const uint32_t* mask_row = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) +
+                                         (size_t)pt[i] * (g.n >> 5);
+              mw[i][m] = valid[i] ? __ldg(mask_row + m) : 0u;
+            }
           }
+        // ---------------- epilogue: G_t of this thread's elements -> hi / lo -> the G tile ----------------
 #pragma unroll
-          for (int ch = 0; ch < 2; ++ch) {
-            if (ch < nch) {
-              const int c0 = 64 * ch + 32 * half;
-              float y[32];  // Y = 2048 x (pre-activation gradient), the accumulator's own scale
+        for (int j = 0; j < 16; ++j) {
+          if (j < (g.n >> 3)) {
+            const int col = 8 * j + 2 * q;
 #pragma unroll
-              for (int q = 0; q < 32; ++q) y[q] = has_mma ? __uint_as_float(v[ch][q]) : 0.f;
-              if (hn > 0) {
-                for (int c = 0; c < hn; ++c) {
-                  const float dd = dr[(hcol + c) & 3];
-                  const float4* w4 = reinterpret_cast<const float4*>(hw + c * hk + c0);
-#pragma unroll
-                  for (int q = 0; q < 8; ++q) {
-                    const float4 w = w4[q];
-                    y[4 * q] = fmaf(dd, w.x, y[4 * q]);
-                    y[4 * q + 1] = fmaf(dd, w.y, y[4 * q + 1]);
-                    y[4 * q + 2] = fmaf(dd, w.z, y[4 * q + 2]);
-                    y[4 * q + 3] = fmaf(dd, w.w, y[4 * q + 3]);
-                  }
-                }
+            for (int i = 0; i < 2; ++i) {
+              float y0 = chain[4 * j + 2 * i], y1 = chain[4 * j + 2 * i + 1];  // Y = 2048 x, the accumulator's own scale
+              for (int c = 0; c < hn; ++c) {
+                const float dd = dr[i][(hcol + c) & 3];
+                const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
+                y0 = fmaf(dd, w.x, y0);
+                y1 = fmaf(dd, w.y, y1);
               }
-              const uint32_t mword = mw[ch];
-#pragma unroll
-              for (int q = 0; q < 32; q += 2) {
-                const float y0 = (mword & (1u << q)) ? y[q] : 0.f;
-                const float y1 = (mword & (2u << q)) ? y[q + 1] : 0.f;
-                split_f16x2_y(y0, y1, y0 * kLoInv, y1 * kLoInv, hi[ch][q >> 1], lo[ch][q >> 1]);
-              }
+              const uint32_t word = mw[i][j >> 2];
+              const int bit = 8 * (j & 3) + 2 * q;
+              y0 = (word & (1u << bit)) ? y0 : 0.f;
+              y1 = (word & (2u << bit)) ? y1 : 0.f;
+              uint32_t hi, lo;
+              split_f16x2_y(y0, y1, y0 * kLoInv, y1 * kLoInv, hi, lo);
+              const int off = tile_piece(64 * wg + r0 + 8 * i, j, 128) + 4 * q;
+              *reinterpret_cast<uint32_t*>(sG + off) = hi;
+              *reinterpret_cast<uint32_t*>(sG + 32768 + off) = lo;
             }
           }
         }
-        tc_fence_before();
-        PROF_SINCE(1, _ta);
-        // ---- the chain's A operand: the same hi / lo registers -> tensor memory (two fp16 per column), then the chain
-        // MMA of this layer may start; it has nothing to do with the shared-memory tile written below
-        PROF_MARK(_tst);
-        {
-          const uint32_t t_ahi = tmem + lane_base + kColAhi, t_alo = tmem + lane_base + kColAlo;
-#pragma unroll
-          for (int ch = 0; ch < 2; ++ch) {
-            if (ch < nch) {
-              const int c0 = 64 * ch + 32 * half;
-              tmem_st16(t_ahi + c0 / 2, hi[ch]);
-              tmem_st16(t_alo + c0 / 2, lo[ch]);
-            }
-          }
-          tmem_wait_st();
-          tc_fence_before();
-          mbar_arrive(bar_a);
-        }
-        PROF_SINCE(4, _tst);
-        // the previous layer's jobs read the G tile: they must be complete before it is overwritten
-        if (prev_e >= 0) wait_jobs(prev_e);
-        PROF_MARK(_tc);
-
-        // ---------------- part B: the held registers -> G tile (MN-major A operand of this event's jobs) ----------------
-#pragma unroll
-        for (int ch = 0; ch < 2; ++ch) {
-          if (ch < nch) {
-            const int fb0 = 8 * ch + 4 * half;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int off = tile_piece(row, fb0 + q, 128);
-              *reinterpret_cast<uint4*>(sG + off) = make_uint4(hi[ch][4 * q], hi[ch][4 * q + 1], hi[ch][4 * q + 2], hi[ch][4 * q + 3]);
-              *reinterpret_cast<uint4*>(sG + 32768 + off) =
-                  make_uint4(lo[ch][4 * q], lo[ch][4 * q + 1], lo[ch][4 * q + 2], lo[ch][4 * q + 3]);
-            }
-          }
-        }
-        if (nch == 1) {
+        if (g.n == 64 && q == 0) {
           // 64-wide layer (layers_dir[0], first event of a tile): feature rows 64..67 carry d_raw for the heads' weight
           // gradients, the rest of the upper half is zero
           const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
-          if (half == 0) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int r = 64 * wg + r0 + 8 * i;
             uint32_t h01, l01, h23, l23;
-            split_f16x2(dr[0], dr[1], h01, l01);
-            split_f16x2(dr[2], dr[3], h23, l23);
-            const int off = tile_piece(row, 8, 128);
-            *reinterpret_cast<uint4*>(sG + off) = make_uint4(h01, h23, 0u, 0u);
-            *reinterpret_cast<uint4*>(sG + 32768 + off) = make_uint4(l01, l23, 0u, 0u);
+            split_f16x2(dr[i][0], dr[i][1], h01, l01);
+            split_f16x2(dr[i][2], dr[i][3], h23, l23);
+            *reinterpret_cast<uint4*>(sG + tile_piece(r, 8, 128)) = make_uint4(h01, h23, 0u, 0u);
+            *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(r, 8, 128)) = make_uint4(l01, l23, 0u, 0u);
 #pragma unroll
-            for (int q = 9; q < 12; ++q) {
-              *reinterpret_cast<uint4*>(sG + tile_piece(row, q, 128)) = z4;
-              *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(row, q, 128)) = z4;
-            }
-          } else {
-#pragma unroll
-            for (int q = 12; q < 16; ++q) {
-              *reinterpret_cast<uint4*>(sG + tile_piece(row, q, 128)) = z4;
-              *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(row, q, 128)) = z4;
+            for (int fb = 9; fb < 16; ++fb) {
+              *reinterpret_cast<uint4*>(sG + tile_piece(r, fb, 128)) = z4;
+              *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(r, fb, 128)) = z4;
             }
           }
         }
         if (e == 0) {
           // ray-indicator tile of this tile: I[p][j] = 1 iff point p belongs to the tile's j-th ray; direction encodings
-          if (half == 0) {
-            uint32_t w[8];
+          if (q == 0) {
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const uint32_t lo16 = (ray_slot == 2 * q && valid) ? 0x3C00u : 0u;
-              const uint32_t hi16 = (ray_slot == 2 * q + 1 && valid) ? 0x3C00u : 0u;
-              w[q] = lo16 | (hi16 << 16);
+            for (int i = 0; i < 2; ++i) {
+              uint32_t w[8];
+#pragma unroll
+              for (int k = 0; k < 8; ++k) {
+                const uint32_t lo16 = (ray_slot[i] == 2 * k && valid[i]) ? 0x3C00u : 0u;
+                const uint32_t hi16 = (ray_slot[i] == 2 * k + 1 && valid[i]) ? 0x3C00u : 0u;
+                w[k] = lo16 | (hi16 << 16);
+              }
+              const int r = 64 * wg + r0 + 8 * i;
+              *reinterpret_cast<uint4*>(sInd + tile_piece(r, 0, 16)) = make_uint4(w[0], w[1], w[2], w[3]);
+              *reinterpret_cast<uint4*>(sInd + tile_piece(r, 1, 16)) = make_uint4(w[4], w[5], w[6], w[7]);
             }
-            *reinterpret_cast<uint4*>(sInd + tile_piece(row, 0, 16)) = make_uint4(w[0], w[1], w[2], w[3]);
-            *reinterpret_cast<uint4*>(sInd + tile_piece(row, 1, 16)) = make_uint4(w[4], w[5], w[6], w[7]);
-          } else {
-            if (p.use_viewdirs && row < n_rays_tile * 3) {
-              const int jr = row / 3, c = row - 3 * jr;
-              const float vv = rays[(first_ray + jr) * ray_stride + 8 + c];
-              encode_coord(vv, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, s_encd + jr * 32);
-            }
+          }
+          if (p.use_viewdirs && tid < n_rays_tile * 3) {
+            const int jr = tid / 3, c = tid - 3 * jr;
+            const float vv = rays[(first_ray + jr) * ray_stride + 8 + c];
+            encode_coord(vv, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, s_encd + jr * 32);
           }
         }
         fence_proxy_async();
-        mbar_arrive(bar_g);
-        PROF_SINCE(5, _tc);
-#ifdef NERFB200_PROF
-        if (PROF_ON) s_prof[7] += 1;
-#endif
-        prev_e = e;
-        ++gev;
+        cta_bar();  // the G tile (and the indicator tile) complete
+
+        if (e + 1 < E) {
+          // ---- chain: chain[p][k] = 2^11 sum_n G_t[p][n] W_t[n][k], N = k_h = 128, K = n: A = this warpgroup's rows of
+          // the G tile (K-major), B = the three weight copies from the ring (one k-step per stage)
+          const uint64_t a_hi = make_desc(smem_u32(sG) + (uint32_t)wg * 16384u, 128, 2048);
+          const uint64_t b_ring = make_desc(smem_u32(sm + mp.ring), 2048, 128);
+          uint32_t prev = 0;
+          wgmma_fence();
+          for (int ks = 0; ks < (g.n >> 4); ++ks) {
+            const uint32_t st = pp.stage;
+            mbar_wait(&w_full[st], pp.phase);
+            const uint64_t b_hs = desc_adv(b_ring, st * (uint32_t)kWStage);
+            const uint64_t ah = desc_adv(a_hi, ks * 256u);
+            wgmma_f16<128>(chain, ah, b_hs, ks > 0 ? 1 : 0);
+            wgmma_f16<128>(chain, desc_adv(ah, 32768u), desc_adv(b_hs, 2 * 2048u), 1);
+            wgmma_f16<128>(chain, ah, desc_adv(b_hs, 4 * 2048u), 1);
+            wgmma_commit();
+            if (ks > 0) {
+              wgmma_wait<1>();
+              reg_fence(chain);
+              if (lane == 0) mbar_arrive(&w_empty[prev]);
+            }
+            prev = st;
+            pp.advance(n_stages);
+          }
+          wgmma_wait<0>();
+          reg_fence(chain);
+          if (lane == 0) mbar_arrive(&w_empty[prev]);
+        }
+
+        // ---- weight-gradient jobs of this event
+        const int nj = bp.n_jobs[e];
+        for (int i = 0; i < nj; ++i) {
+          const BwdJob& jq = bp.jobs[e][i];
+          const int w = jq.n_b;
+          const uint32_t fstr = (uint32_t)(w >> 3) * 128u;  // bytes between 8-point blocks of the activation tile
+          mbar_wait(x_full, x_ph);
+          x_ph ^= 1;
+          if (jq.kind == 1) {
+            // head job: A = activation tile (rows = its features, MN-major), B = d_raw (feature rows 64..79 of the G tile)
+            if (64 * wg < jq.nrows) {
+              float acc[8], dummy[8];
+              const uint64_t xa = make_desc(smem_u32(sX) + (uint32_t)wg * 1024u, fstr, 128);
+              const uint64_t db = make_desc(smem_u32(sG) + 1024u, 2048, 128);
+              // residual products first: A_lo B_hi + A_hi B_lo (job_mma's scheme with B's lo block 32 KB on)
+              job_mma<16>(acc, dummy, false, xa, 32768u, 2 * fstr, db, 32768u, 4096u, 0);
+              const HeadLayer& h = p.h[jq.dst_head];
+#pragma unroll
+              for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+                for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+                  for (int cc = 0; cc < 2; ++cc) {
+                    const int k = 64 * wg + r0 + 8 * ii, c = 8 * jj + 2 * q + cc - h.out_col;
+                    if (k < h.k && c >= 0 && c < h.n_out)
+                      atomicAdd(gb + bm.xh + jq.dst_head * 512 + c * 128 + k, to_fix(acc[4 * jj + 2 * ii + cc] * us));
+                  }
+            }
+          } else if (64 * wg < jq.nrows || (i == 0 && e == 0 && p.use_viewdirs)) {
+            // (warpgroup 1 of layers_dir[0]'s first job only sums the d_raw rows 64..67 of the indicator product)
+            const uint64_t ga = make_desc(smem_u32(sG) + (uint32_t)wg * 1024u, 2048, 128);  // G^T: rows = features
+            const uint64_t xb = make_desc(smem_u32(sX), fstr, 128);
+            const uint64_t id = make_desc(smem_u32(sInd), 256, 128);
+            float acc_i[8];
+            unsigned long long* gdst = gb + jq.gb_off;
+#define NB_JOB(NN)                                                                                   \
+  {                                                                                                  \
+    float acc[NN / 2];                                                                               \
+    job_mma<NN>(acc, acc_i, i == 0, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);                    \
+    if (64 * wg < jq.nrows) job_drain<NN>(acc, us, gdst, stg, stg_n, wg);                            \
+  }
+            if (w == 128) NB_JOB(128) else if (w == 64) NB_JOB(64) else if (w == 48) NB_JOB(48)
+            else if (w == 32) NB_JOB(32) else NB_JOB(16)
+#undef NB_JOB
+            if (i == 0) {
+              // indicator sums of this layer: bias gradient (all rays) and, for layers_dir[0], the direction-encoding
+              // part of its weight gradient (per-ray sums x direction encodings, below)
+              const float su = us * kActScale;  // the indicator is an exact 1, not an activation / 16
+#pragma unroll
+              for (int ii = 0; ii < 2; ++ii) {
+                const int n = 64 * wg + r0 + 8 * ii;
+                float tot = acc_i[2 * ii] + acc_i[2 * ii + 1] + acc_i[4 + 2 * ii] + acc_i[4 + 2 * ii + 1];
+                tot += __shfl_xor_sync(0xffffffffu, tot, 1);
+                tot += __shfl_xor_sync(0xffffffffu, tot, 2);
+                if (q == 0) {
+                  if (n < g.n) s_bgrad[g.cum_n + n] += tot * su;
+                  if (e == 0 && p.use_viewdirs && n >= 64 && n < 68) s_bgrad[p.enc_cum[0] + n - 64] += tot * su;  // d_rgb, d_sigma sums
+                }
+                if (e == 0 && p.use_viewdirs && n < 64) {
+                  s_sums[n * 16 + 2 * q] = acc_i[2 * ii] * su;
+                  s_sums[n * 16 + 2 * q + 1] = acc_i[2 * ii + 1] * su;
+                  s_sums[n * 16 + 8 + 2 * q] = acc_i[4 + 2 * ii] * su;
+                  s_sums[n * 16 + 9 + 2 * q] = acc_i[4 + 2 * ii + 1] * su;
+                }
+              }
+            }
+          }
+          cta_bar();  // both warpgroups are done with the activation tile (and the per-ray sums are in place)
+          if (e == 0 && i == 0 && p.use_viewdirs) {
+            for (int idx = tid; idx < 64 * p.dim_dir; idx += 128 * kWG) {
+              const int n = idx / p.dim_dir, k = idx - n * p.dim_dir;
+              float a = 0.f;
+              for (int jr = 0; jr < n_rays_tile; ++jr) a = fmaf(s_sums[n * 16 + jr], s_encd[jr * 32 + k], a);
+              s_dacc[n * 28 + k] += a;
+            }
+          }
+          if (tid == 0) {  // the next job's activation tile
+            int ni = i + 1, ne = e, nit = it;
+            if (ni == nj) {
+              ni = 0;
+              if (++ne == E) { ne = 0; ++nit; }
+            }
+            if (nit < my_tiles) issue_x(nit, ne, ni);
+          }
+        }
       }
     }
+    if (wt == 0) bulk_wait_all();
   }
-
-  tc_fence_before();
   __syncthreads();
-  PROF_FLUSH;
-  if (warp == 8) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(kTmemColsB));
+  // ---- the bias / direction-encoding accumulators of this CTA go to the blob
+  for (int i = tid; i < p.enc_cum[0] + 8; i += kThreadsB) atomicAdd(gb + bm.xb + i, to_fix(s_bgrad[i]));
+  for (int i = tid; i < 64 * 28; i += kThreadsB) atomicAdd(gb + bm.xd + i, to_fix(s_dacc[i]));
 }
 
-// gradient blob -> flat (torch-layout) gradient vector: every job block is [chunk][row][32 floats] with the eight
-// 16-byte pieces of a row XOR-swizzled by (row & 7) (the staging tile's bank-conflict-free layout)
+// gradient blob (fixed point) -> flat (torch-layout) gradient vector: every blob word is added to the one flat element it
+// belongs to.  Weight-gradient job blocks are [chunk][row][16 words] with the eight 16-byte pieces of a row XOR-swizzled
+// by (row & 7) (the staging tile's bank-conflict-free layout).
 __global__ void unpack_grad_kernel(const __grid_constant__ Plan p, const __grid_constant__ BwdPlan bp,
-                                   const float* __restrict__ gblob, float* __restrict__ flat_grad) {
-  const int gb_total = bp.gb_total;
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < gb_total; idx += gridDim.x * blockDim.x) {
-    for (int e = 0; e < p.n_gemm; ++e) {
-      const int nj = bp.n_jobs[e];
-      bool done = false;
-      for (int i = 0; i < nj && !done; ++i) {
-        const BwdJob& j = bp.jobs[e][i];
-        if (j.kind != 0) continue;
-        const int sz = ((j.n_b + 31) / 32) * 4096;
-        if (idx < j.gb_off || idx >= j.gb_off + sz) continue;
-        done = true;
-        const int r = idx - j.gb_off;
-        const int c = r >> 12, rr = (r >> 5) & 127, w = r & 31;
-        const int col = 32 * c + ((((w >> 2) ^ (rr & 7)) << 2) | (w & 3));
-        if (rr < j.row0 || rr >= j.row0 + j.nrows || col >= j.ncols) break;
-        const float v = gblob[idx];
-        const GemmLayer& g = p.g[j.dst];
-        atomicAdd(flat_grad + g.flat_w + (size_t)rr * (g.k_h + g.enc_real) + j.dst_col0 + col, v);
+                                   const unsigned long long* __restrict__ gb, float* __restrict__ flat_grad) {
+  const BlobMap sl = blob_map(p, bp.gb_total);
+  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < sl.words; idx += gridDim.x * blockDim.x) {
+    int64_t dst = -1;
+    if (idx < bp.gb_total) {
+      for (int e = 0; e < p.n_gemm && dst < 0; ++e) {
+        const int nj = bp.n_jobs[e];
+        for (int i = 0; i < nj; ++i) {
+          const BwdJob& j = bp.jobs[e][i];
+          if (j.kind != 0) continue;
+          const int sz = ((j.n_b + 15) / 16) * 2048;
+          if (idx < j.gb_off || idx >= j.gb_off + sz) continue;
+          const int r = idx - j.gb_off;
+          const int c = r >> 11, rr = (r >> 4) & 127, w = r & 15;
+          const int col = 16 * c + ((((w >> 1) ^ (rr & 7)) << 1) | (w & 1));
+          const GemmLayer& g = p.g[j.dst];
+          if (rr >= j.row0 && rr < j.row0 + j.nrows && col < j.ncols)
+            dst = g.flat_w + (int64_t)rr * (g.k_h + g.enc_real) + j.dst_col0 + col;
+          e = p.n_gemm;  // found the block
+          break;
+        }
       }
-      if (done) break;
+    } else if (idx < sl.xd) {
+      const int i = idx - sl.xb;
+      if (i < p.enc_cum[0]) {
+        for (int gi = 0; gi < p.n_gemm; ++gi)
+          if (i >= p.g[gi].cum_n && i < p.g[gi].cum_n + p.g[gi].n) dst = p.g[gi].flat_b + (i - p.g[gi].cum_n);
+      } else if (p.use_viewdirs) {
+        const int j = i - p.enc_cum[0];
+        if (j < 3) dst = p.h[1].flat_b + j;
+        else if (j == 3) dst = p.h[0].flat_b;
+      }
+    } else if (idx < sl.xh) {
+      const int i = idx - sl.xd, n = i / 28, k = i - 28 * n;
+      const GemmLayer& gd = p.g[p.n_gemm - 1];
+      if (p.use_viewdirs && n < gd.n && k < p.dim_dir) dst = gd.flat_w + (int64_t)n * (gd.k_h + gd.enc_real) + gd.k_h + k;
+    } else if (idx < sl.xh + 1024 && p.use_viewdirs) {
+      const int i = idx - sl.xh, hd = i >> 9, c = (i >> 7) & 3, k = i & 127;
+      const HeadLayer& h = p.h[hd];
+      if (c < h.n_out && k < h.k) dst = h.flat_w + (int64_t)c * h.k + k;
     }
+    if (dst < 0) continue;
+    flat_grad[dst] += (float)((double)(long long)gb[idx] * (1.0 / 4294967296.0));  // the only writer of this element
   }
 }
 
-#ifdef NERFB200_PROF
-extern "C" void nerfb200_prof_read(unsigned long long* out32, int reset) {
-  cudaDeviceSynchronize();
-  cudaMemcpyFromSymbol(out32, g_prof, sizeof(g_prof));
-  if (reset) {
-    unsigned long long z[32] = {0};
-    cudaMemcpyToSymbol(g_prof, z, sizeof(z));
-  }
-}
-#endif
-
-
+// the gradient blob, in floats (two per 64-bit word)
 int64_t bwd_tc_scratch_floats(const Plan& p) {
   int total = 0;
   bwd_jobs(p, 0, nullptr, &total);
-  return total;
+  return 2 * (int64_t)blob_map(p, total).words;
 }
 
 int bwd_tc_supported(const Plan& p, int n_samples, const char* what) {
   int rc = tc_supported(p, n_samples, what, /*training=*/true);
   if (rc) return rc;
   if (!p.use_viewdirs) {
-    set_error("%s impl=1 (tcgen05): the fused backward needs a view-dependent model (fc_rgb / fc_alpha heads); use impl=0", what);
+    set_error("%s impl=1 (wgmma): the fused backward needs a view-dependent model (fc_rgb / fc_alpha heads); use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (p.dim_dir > 28) {
-    set_error("%s impl=1 (tcgen05): direction encodings wider than 28 not supported by the fused backward; use impl=0", what);
+    set_error("%s impl=1 (wgmma): direction encodings wider than 28 not supported by the fused backward; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map_b(p).n_stages < 2) {
-    set_error("%s impl=1 (tcgen05): network too deep for the backward's shared-memory budget; use impl=0", what);
+    set_error("%s impl=1 (wgmma): network too deep for the backward's shared-memory budget; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   return NERFB200_OK;
@@ -841,26 +653,22 @@ int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int r
   if (rc) return rc;
   const int64_t P = n_rays * n_samples;
   const int64_t tiles = (P + kTileRows - 1) / kTileRows;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int sms = device_sms();
   const int grid = (int)(tiles < sms ? tiles : sms);
   const BwdPlan bp = make_bwd_plan(p);
-  const int gb_total = bp.gb_total;
-  rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)gb_total * 4, s), "mlp_bwd_tc blob memset");
+  const BlobMap bm = blob_map(p, bp.gb_total);
+  rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)bm.words * 8, s), "mlp_bwd_tc blob memset");
   if (rc) return rc;
   const size_t bytes = (size_t)smem_map_b(p).total + 1024;
   rc = check_cuda(cudaFuncSetAttribute(mlp_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes),
                   "mlp_bwd_tc smem attribute");
   if (rc) return rc;
-  mlp_bwd_tc_kernel<<<grid, kThreadsB, bytes, s>>>(p, blob, rays, ray_stride, d_raw, stash, P, n_samples, tiles, gblob,
-                                                    flat_grad, bp);
+  mlp_bwd_tc_kernel<<<grid, kThreadsB, bytes, s>>>(p, blob, rays, ray_stride, d_raw, stash, P, n_samples, tiles, gblob, bp);
   count_launch();
   rc = check_cuda(cudaGetLastError(), "mlp_bwd_tc launch");
   if (rc) return rc;
-  int blocks = (gb_total + 255) / 256;
-  if (blocks > 1184) blocks = 1184;
-  unpack_grad_kernel<<<blocks, 256, 0, s>>>(p, bp, gblob, flat_grad);
+  const int blocks = (bm.words + 255) / 256;
+  unpack_grad_kernel<<<blocks, 256, 0, s>>>(p, bp, reinterpret_cast<const unsigned long long*>(gblob), flat_grad);
   count_launch();
   return check_cuda(cudaGetLastError(), "unpack_grad launch");
 }

@@ -100,7 +100,7 @@ int launch_gen_rays(const float* c2w12_host, int height, int width, float focal,
   int rc = fill_args(&a, c2w12_host, height, width, focal, ndc, near, far, use_viewdirs, out_stride);
   if (rc) return rc;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   gen_rays_kernel<<<(unsigned)blocks, 256, 0, s>>>(a, pix, n, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "gen_rays launch");
@@ -112,7 +112,7 @@ int launch_pack_rays(const float* ro, const float* rd, int64_t n, int height, in
   int rc = fill_args(&a, nullptr, height, width, focal, ndc, near, far, use_viewdirs, out_stride);
   if (rc) return rc;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   pack_rays_kernel<<<(unsigned)blocks, 256, 0, s>>>(a, ro, rd, n, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "pack_rays launch");

@@ -277,7 +277,7 @@ __global__ void pack_kernel(Plan p, const float* __restrict__ flat, float* __res
 int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s) {
   const int threads = 256;
   int blocks = (p.blob_floats + threads - 1) / threads;
-  if (blocks > 1184) blocks = 1184;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   pack_kernel<<<blocks, threads, 0, s>>>(p, flat, blob);
   count_launch();
   return check_cuda(cudaGetLastError(), "pack launch");
@@ -306,7 +306,7 @@ int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int ste
   const double bc2 = 1.0 - pow((double)b2, (double)step);
   const int threads = 256;
   int64_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
   adam_kernel<<<(unsigned)blocks, threads, 0, s>>>(p, g, m, v, n, (float)(lr / bc1), (float)(1.0 / sqrt(bc2)), b1, b2,
                                                    eps, grad_scale);
   count_launch();

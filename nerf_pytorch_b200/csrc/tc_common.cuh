@@ -1,5 +1,5 @@
-// tc_common.cuh -- inline-PTX wrappers for the Blackwell tensor-core path: mbarrier, bulk async copy,
-// tcgen05 (alloc / mma / commit / ld / st / fences) and the UMMA shared-memory / instruction descriptors.
+// tc_common.cuh -- inline-PTX helpers of the Hopper tensor-core path: mbarrier, bulk async copy (TMA engine), the wgmma
+// shared-memory matrix descriptor and the fp16 x 2 operand split (the MMAs themselves: wgmma.cuh).
 #pragma once
 #include "common.cuh"
 
@@ -53,8 +53,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // L2 eviction-priority policy for the weight stream: every CTA re-reads the same ~1 MB blob for every tile
 // while GBs of stash stream through L2 in training, so the weights are pinned (evict_last) and the
@@ -87,58 +85,21 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                : "memory");
 }
 
-// UMMA shared-memory descriptor, K-major, no swizzle: 8-row core matrices (8 x 16 B) `sbo` bytes apart
-// along M/N, the two K halves of one instruction `lbo` bytes apart.  Bit layout per the PTX ISA matrix
-// descriptor (cute::UMMA::SmemDescriptor): [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, [46,48) version = 1.
+// wgmma shared-memory matrix descriptor, no swizzle ("interleave" layout type 0): 8-row core matrices (8 x 16 B).
+// K-major operand: LBO = bytes between the two K halves of one instruction, SBO = bytes between 8-row groups along M/N;
+// MN-major operand: LBO = bytes between 8-deep groups along K, SBO = bytes between 8-wide groups along M/N.
+// Bit layout per the PTX ISA (cute::GMMA::GmmaDescriptor): [0,14) addr>>4, [16,30) LBO>>4, [32,46) SBO>>4, base offset
+// and layout type 0.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-         (1ull << 46);
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// Advance a descriptor's 14-bit start-address field by `bytes` with ONE 32-bit add.  The MMA issue loops must stay
-// lean: the issuing thread runs alone, every dependent integer instruction costs it ~5 cycles, and rebuilding 64-bit
-// descriptors per instruction made an MMA cost ~80-115 cycles of issue time against 64 on the tensor pipe
-// (tools/mma_rate.cu; with precomputed descriptors all flavours run at the nominal N / 2 cycles).
+// Advance a descriptor's 14-bit start-address field by `bytes` with one 32-bit add (descriptors are built once per
+// layer; the MMA loops only move their start addresses).
 __device__ __forceinline__ uint64_t desc_adv(uint64_t d, uint32_t bytes) {
   return (d & 0xFFFFFFFF00000000ull) | (uint64_t)((uint32_t)d + (bytes >> 4));
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major, M = 128
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ void mma_ss(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n" ::"r"(d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ts(uint32_t d, uint32_t a_tmem, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d),
-      "r"(a_tmem), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// fp16 operands (forward chain): D = F32, A = B = F16, both K-major, M = 128; K = 16 per instruction
-__device__ __forceinline__ uint32_t make_idesc_f16(int n) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ void mma_ss_f16(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ts_f16(uint32_t d, uint32_t a_tmem, uint64_t b, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n" ::"r"(d),
-      "r"(a_tmem), "l"(b), "r"(idesc), "r"(acc)
-      : "memory");
-}
 // fp16 x 2 split of a pair of fp32 values: hi = fp16(x), lo = fp16((x - hi) * 2^11); both packed with the FIRST
-// value in the low half (= the lower K index of a 16-bit tensor-memory / shared-memory operand).
+// value in the low half (= the lower K index of a 16-bit operand).
 // The residual is scaled by 2^11 so that it is a NORMAL fp16 number whenever hi is (it would be subnormal below
 // |x| = 0.125 otherwise and the split would degrade to 3e-8 absolute resolution): x = hi + lo * 2^-11 carries 22
 // significant bits for 6.1e-5 <= |x| < 65504 and resolves 1.5e-11 absolutely below (tests/test_host_cpu.py).
@@ -155,16 +116,13 @@ __device__ __forceinline__ void split_f16x2(float x0, float x1, uint32_t& hi, ui
   asm("{\n.reg .b16 a, b;\nmov.b32 {a, b}, %2;\ncvt.f32.f16 %0, a;\ncvt.f32.f16 %1, b;\n}\n" : "=f"(h0), "=f"(h1) : "r"(hi));
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"((x1 - h1) * kLoScale), "f"((x0 - h0) * kLoScale));
 }
-// The same split from Y = 2048 x (exact scaling): hi = fp16(x), lo = fp16(Y - 2048 hi) with the mixed-precision FMA
-// (fma.rn.f32.f16: fp16 x fp16 + fp32, one instruction per element, takes the packed halves directly) instead of
-// unpack + subtract + multiply.  Bit-identical to split_f16x2(Y0 / 2048, Y1 / 2048): x - hi is exact in fp32.
+// The same split from Y = 2048 x (exact scaling): hi = fp16(x), lo = fp16(Y - 2048 hi), one FMA per element instead of
+// subtract + multiply.  Bit-identical to split_f16x2(Y0 / 2048, Y1 / 2048): x - hi is exact in fp32.
 __device__ __forceinline__ void split_f16x2_y(float Y0, float Y1, float x0, float x1, uint32_t& hi, uint32_t& lo) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
-  float r0, r1;
-  asm("{\n.reg .b16 a, b, m;\nmov.b32 {a, b}, %2;\nmov.b16 m, 0xE800;\n"   // 0xE800 = -2048 in fp16
-      "fma.rn.f32.f16 %0, a, m, %3;\nfma.rn.f32.f16 %1, b, m, %4;\n}\n"
-      : "=f"(r0), "=f"(r1)
-      : "r"(hi), "f"(Y0), "f"(Y1));
+  float h0, h1;
+  asm("{\n.reg .b16 a, b;\nmov.b32 {a, b}, %2;\ncvt.f32.f16 %0, a;\ncvt.f32.f16 %1, b;\n}\n" : "=f"(h0), "=f"(h1) : "r"(hi));
+  const float r0 = fmaf(h0, -kLoScale, Y0), r1 = fmaf(h1, -kLoScale, Y1);
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
 }
 // the three weight copies of one pair (same packing)
@@ -174,30 +132,6 @@ __device__ __forceinline__ void split_w3(float w0, float w1, uint32_t& hs, uint3
   asm("{\n.reg .b16 a, b;\nmov.b32 {a, b}, %2;\ncvt.f32.f16 %0, a;\ncvt.f32.f16 %1, b;\n}\n" : "=f"(h0), "=f"(h1) : "r"(h));
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hs) : "f"(h1 * kLoScale), "f"(h0 * kLoScale));
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(l) : "f"((w1 - h1) * kLoScale), "f"((w0 - h0) * kLoScale));
-}
-__device__ __forceinline__ float f16_lo_to_f32(uint32_t pair) {
-  float f;
-  asm("{\n.reg .b16 a, b;\nmov.b32 {a, b}, %1;\ncvt.f32.f16 %0, a;\n}\n" : "=f"(f) : "r"(pair));
-  return f;
-}
-__device__ __forceinline__ float f16_hi_to_f32(uint32_t pair) {
-  float f;
-  asm("{\n.reg .b16 a, b;\nmov.b32 {a, b}, %1;\ncvt.f32.f16 %0, b;\n}\n" : "=f"(f) : "r"(pair));
-  return f;
-}
-// one lane of a converged warp (the warp runs the surrounding loop uniformly so that descriptors and addresses
-// live in uniform registers; only the tcgen05 instruction itself is predicated on the elected lane)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n.reg .b32 rx;\n.reg .pred px;\n"
-      "elect.sync rx|px, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, px;\n}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
 }
 __device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
   asm volatile(
@@ -211,62 +145,16 @@ __device__ __forceinline__ float fmax_nan(float a, float b) {
   asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 }
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-#define NB_R32(v, o)                                                                                              \
-  "=r"(v[o + 0]), "=r"(v[o + 1]), "=r"(v[o + 2]), "=r"(v[o + 3]), "=r"(v[o + 4]), "=r"(v[o + 5]), "=r"(v[o + 6]), \
-      "=r"(v[o + 7])
-#define NB_W32(v, o)                                                                                       \
-  "r"(v[o + 0]), "r"(v[o + 1]), "r"(v[o + 2]), "r"(v[o + 3]), "r"(v[o + 4]), "r"(v[o + 5]), "r"(v[o + 6]), \
-      "r"(v[o + 7])
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31}, [%32];\n"
-      : NB_R32(v, 0), NB_R32(v, 8), NB_R32(v, 16), NB_R32(v, 24)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,"
-      "%29,%30,%31};\n" ::NB_W32(v, 0),
-      NB_W32(v, 8), NB_W32(v, 16), NB_W32(v, 24), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : NB_R32(v, 0), NB_R32(v, 8)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15};\n" ::NB_W32(v, 0),
-      NB_W32(v, 8), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // ---------------------------------------------------------------------------------------------------------------
 // Operand tiles.  A 128-point x (8 F)-feature block of fp16 values is kept as 16 x F core matrices of 128 bytes,
 //     T[pb = point / 8][fb = feature / 8][point % 8][feature % 8]            (pb-major, F * 128 bytes per pb)
 // and a value x as two such blocks, hi = fp16(x) then lo = fp16((x - hi) 2^11)  (split_f16x2), 16 F 128 bytes apart.
-// The SAME bytes serve tcgen05.mma as
-//   K-major  operand (rows = points,   K = features): SBO = F * 128 (next 8 points),  LBO = 128 (next 8 features)
-//   MN-major operand (rows = features, K = points)  : SBO = 128 (next 8 features),    LBO = F * 128 (next 8 points)
-// (checked on hardware by tools/mn_test.cu), so the training forward writes every layer's activation tile ONCE --
-// into HBM, straight from the registers that also feed the next layer's tensor-memory operand -- and the fused
-// backward (mlp_tc_bwd.cu) bulk-copies it back and uses it as the B operand of the weight-gradient MMAs unchanged.
+// The SAME bytes serve wgmma as
+//   K-major  operand (rows = points,   K = features): SBO = F * 16 (next 8 points),   LBO = 128 (next 8 features)
+//   MN-major operand (rows = features, K = points)  : SBO = 128 (next 8 features),    LBO = F * 16 (next 8 points)
+// so the training forward writes every layer's activation tile ONCE -- into HBM, straight from the accumulator
+// registers that also fill the next layer's shared-memory operand -- and the fused backward (mlp_tc_bwd.cu) bulk-copies
+// it back and uses it as the MN-major B operand of the weight-gradient MMAs unchanged.
 // ---------------------------------------------------------------------------------------------------------------
 __host__ __device__ inline int tile_half_bytes(int n_feat) { return 16 * (n_feat >> 3) * 128; }   // one of hi / lo
 __host__ __device__ inline int tile_bytes(int n_feat) { return 2 * tile_half_bytes(n_feat); }      // = 128 * n * 4
@@ -274,30 +162,12 @@ __host__ __device__ inline int tile_bytes(int n_feat) { return 2 * tile_half_byt
 __host__ __device__ inline int tile_piece(int row, int fb, int n_feat) {
   return (row >> 3) * (n_feat >> 3) * 128 + fb * 128 + (row & 7) * 16;
 }
-// instruction descriptor for kind::f16 with selectable operand majors (bit 15: A is MN-major, bit 16: B is MN-major)
-__device__ __forceinline__ uint32_t make_idesc_f16_mn(int n, int a_mn, int b_mn) {
-  return (1u << 4) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(n >> 3) << 17) | ((128u >> 4) << 24);
-}
-// D = A * B + D * 2^-11 (scale-input-d): folds the 2^11-scaled residual products into the main sum without a
-// second accumulator: first all lo*hi + hi*lo products, then the first hi*hi product with this variant
-__device__ __forceinline__ void mma_ss_f16_scale11(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p, 11;\n}\n" ::"r"(d),
-      "l"(a), "l"(b), "r"(idesc)
-      : "memory");
-}
-// shared -> global bulk reduction (TMA engine): global[i] += shared[i], fp32
-__device__ __forceinline__ void bulk_reduce_add_f32(float* gdst, const void* ssrc, uint32_t bytes) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(gdst),
+// shared -> global bulk reduction (TMA engine): global[i] += shared[i], 64-bit integers
+__device__ __forceinline__ void bulk_reduce_add_u64(unsigned long long* gdst, const void* ssrc, uint32_t bytes) {
+  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(gdst),
                "r"(smem_u32(ssrc)), "r"(bytes)
                : "memory");
   asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-
-// 16-byte vector reduction into global memory (L2 atomic unit), no return value
-__device__ __forceinline__ void red_add_v4(float* gdst, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(gdst), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
 struct Pipe {  // role-local ring state
@@ -306,8 +176,6 @@ struct Pipe {  // role-local ring state
     if (++stage == n_stages) { stage = 0; phase ^= 1; }
   }
 };
-
-__device__ __forceinline__ void epi_bar256() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 }  // namespace tc
 }  // namespace nerfb200

@@ -1,4 +1,4 @@
-// wgrad_items.cuh -- the weight-gradient work list shared by the SIMT and tcgen05 wgrad kernels:
+// wgrad_items.cuh -- the weight-gradient work list of the SIMT wgrad kernel:
 // one item per (gemm layer, output-row block, input-column block) + one per narrow head.
 #pragma once
 #include "common.cuh"
@@ -57,24 +57,5 @@ __host__ __device__ inline WgItem wg_decode(const Plan& p, int item) {
   it.n0 = 0; it.nblk = p.h[item].n_out; it.k0 = 0; it.kblk = p.h[item].k; it.bias = 1;
   return it;
 }
-
-// floats one point costs an item in the tcgen05 kernel: one dY row + one X row (both read from HBM exactly once)
-__host__ __device__ inline void wg_row_widths(const Plan& p, const WgItem& it, int* wa, int* wb) {
-  if (it.kind == 2) {
-    *wa = 4;
-    *wb = p.g[p.h[it.t].src].n;
-  } else {
-    const GemmLayer& g = p.g[it.t];
-    *wa = g.n;
-    *wb = it.kind == 0 ? p.g[g.src].n : (g.enc_sel ? p.dim_dir_pad : p.dim_xyz_pad);
-  }
-}
-
-constexpr int kWgMaxItems = 32;
-// CTA -> (item, part) map of the tcgen05 kernel: item i owns CTAs [start[i], start[i+1]), sized by its HBM bytes
-struct WgGrid {
-  int n_items;
-  short start[kWgMaxItems + 1];
-};
 
 }  // namespace nerfb200

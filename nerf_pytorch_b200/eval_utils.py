@@ -22,7 +22,7 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
     ``train_utils.COMPAT_MODE_QUIRK`` is switched off (the reference forgets to forward ``mode``, train_utils.py:171-181);
     the chunk size comes from ``options.nerf.<mode>.chunksize`` (``rays_per_chunk`` overrides it: the fused kernels
-    need no small chunks, 180 GB of HBM hold a whole 800 x 800 image's intermediates)."""
+    need no small chunks, an H100's 80 GB of HBM hold a whole 800 x 800 image's intermediates)."""
     if device is None:
         device = next(model_coarse.parameters()).device
     use_viewdirs = bool(options.nerf.use_viewdirs)

@@ -15,8 +15,8 @@ from . import _lib
 from ._lib import Arch, RenderOpts
 
 IMPL_SIMT = 0  # fp32 CUDA cores
-IMPL_TC = 1    # tcgen05 tensor cores (fp16x2 three-term splits, fp32 accumulation)
-IMPL_TC_FWD = 2  # query only (impl_supported): the tcgen05 forward alone (inference), which also runs hidden 256
+IMPL_TC = 1    # wgmma tensor cores (fp16x2 three-term splits, fp32 accumulation)
+IMPL_TC_FWD = 2  # query only (impl_supported): the wgmma forward alone (inference), which also runs hidden 256
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -263,7 +263,7 @@ def mlp_wgrad(arch: ArchSpec, rays, z, d_raw, stash, gstash, impl=IMPL_SIMT, fla
 
 
 def bwd_bytes_per_point(arch: ArchSpec) -> int:
-    """HBM bytes the tcgen05 backward reads per point (activation tiles of its weight-gradient jobs, masks, d_raw)."""
+    """HBM bytes the wgmma backward reads per point (activation tiles of its weight-gradient jobs, masks, d_raw)."""
     return int(_lib.load().nerfb200_bwd_bytes_per_point(C.byref(arch.c_struct())))
 
 

@@ -2,7 +2,7 @@
 
 Rays are independent units: each rank renders its own contiguous shard of the global batch
 (weak scaling: 4096 rays per GPU) with replicated weights, and the ONLY collective of a step is
-one all-reduce (NCCL over NVLink 5 / NVSwitch on GPUs, gloo in the CPU tests) of the flat
+one all-reduce (NCCL over NVLink / NVSwitch on GPUs, gloo in the CPU tests) of the flat
 gradient vector that the backward kernels write for BOTH networks (train_utils._RenderChunk).
 A fused Adam over the flat parameter buffer follows on every rank, so replicas stay identical."""
 from __future__ import annotations

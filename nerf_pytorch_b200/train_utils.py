@@ -26,13 +26,13 @@ from .nerf_helpers import Embedder, get_minibatches
 # so validation renders use options.nerf.train.* for sampling/noise.  True reproduces that.
 COMPAT_MODE_QUIRK = True
 
-# None: tcgen05 tensor cores (three-term split-precision products) wherever the kernels support the configuration (training: hidden
+# None: wgmma tensor cores (three-term split-precision products) wherever the kernels support the configuration (training: hidden
 # 128; inference: hidden 128 or 256; encodings <= 64 wide, >= 16 samples per ray), fp32 CUDA cores otherwise; 0 / 1 force one.
 DEFAULT_IMPL = None
 
 
 def _auto_impl(arch_c, arch_f, n_coarse, n_fine, training=True):
-    # inference only needs the tcgen05 forward (hidden 128 and 256); training needs the fused backward too (hidden 128)
+    # inference only needs the wgmma forward (hidden 128 and 256); training needs the fused backward too (hidden 128)
     what = ops.IMPL_TC if training else ops.IMPL_TC_FWD
     ok = all(a is None or ops.impl_supported(a, n_coarse, what) for a in (arch_c, arch_f))
     return ops.IMPL_TC if ok else ops.IMPL_SIMT

@@ -1,10 +1,10 @@
 """Generate tests/golden/*.npz from the UNMODIFIED reference  --  TEST INFRASTRUCTURE.
 
-Run in the authoring container only (needs /root/reference, which does not exist on the GPU
-box):  ``python oracle/make_golden.py``.
+Needs a checkout of the unmodified krrish94/nerf-pytorch, named by the environment variable NERF_PYTORCH_REFERENCE:
+``NERF_PYTORCH_REFERENCE=/path/to/nerf-pytorch python oracle/make_golden.py``.  The tests only read what it wrote.
 
 What it does, per case:
-  1. imports krrish94/nerf-pytorch from /root/reference with two ``sys.modules`` shims
+  1. imports krrish94/nerf-pytorch from that checkout with two ``sys.modules`` shims
      (``imageio`` is only used by the dataset loaders; ``torchsearchsorted`` -- an unpinned
      third-party wheel, requirements.txt:9 -- is replaced by ``torch.searchsorted`` which has
      the same numpy ``side="right"`` semantics);
@@ -28,7 +28,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 from oracle import nerf_oracle as O  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("NERF_PYTORCH_REFERENCE", "")
 GOLD = os.path.join(REPO, "tests", "golden")
 
 
@@ -37,6 +37,8 @@ def import_reference():
     ts = types.ModuleType("torchsearchsorted")
     ts.searchsorted = lambda a, v, out=None, side="left": torch.searchsorted(a, v, right=(side == "right"))
     sys.modules["torchsearchsorted"] = ts
+    if not os.path.isdir(REF):
+        raise SystemExit("set NERF_PYTORCH_REFERENCE to a checkout of the unmodified krrish94/nerf-pytorch")
     sys.path.insert(0, REF)
     import nerf  # noqa
 

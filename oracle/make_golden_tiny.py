@@ -4,7 +4,7 @@ BASELINE.json configs[0] ("tiny_nerf.py lego 100x100, 1024 rays, 64 coarse sampl
 `run_one_iter_of_tinynerf` (tiny_nerf.py:109-155) on a 32 x 32 image (= 1024 rays) with 64 samples per ray, L = 10,
 pose_spherical(30, -30, 4), seeded `VeryTinyNerfModel`; then the same through oracle/tiny_oracle.py, from the same seed and
 with the recorded random tensor injected, ASSERTING bit equality of the image, the loss and every gradient.
-Run in the authoring container only (needs /root/reference): ``python oracle/make_golden_tiny.py``."""
+Needs NERF_PYTORCH_REFERENCE like oracle/make_golden.py: ``NERF_PYTORCH_REFERENCE=... python oracle/make_golden_tiny.py``."""
 from __future__ import annotations
 
 import os

@@ -8,14 +8,14 @@ product package (``nerf_pytorch_b200``) never does.
 
 Pinning status: the reference ships NO golden vectors or known-answer tests for this path
 (SURVEY.md section 4), so the oracle is pinned against outputs of the reference itself:
-``oracle/make_golden.py`` imports the unmodified reference from ``/root/reference`` (two
+``oracle/make_golden.py`` imports the unmodified reference from a checkout of it (two
 ``sys.modules`` shims, see that script), runs it on seeded inputs with the shipped
 ``pretrained/lego-lowres`` weights, asserts THIS restatement reproduces every output
 bit-for-bit (same ATen ops in the same order, same RNG draw order), and commits the vectors
 under ``tests/golden/``.  ``tests/test_oracle_golden.py`` re-checks the oracle against those
 vectors on every run.
 
-Every function cites the reference file:line (paths relative to /root/reference) it follows.
+Every function cites the reference file:line (paths relative to the reference repository) it follows.
 Differences from the reference are limited to:
   * randoms can be injected (``randoms=dict(t_rand=, noise_c=, u=, noise_f=)``); when absent
     they are drawn from the torch global RNG in the reference's order, so that a shared seed

@@ -1,6 +1,6 @@
 """GPU: BASELINE.json's full-size configurations through size-independent properties (the oracle is too slow at
 these sizes): sortedness / containment of the merged depths, compositing invariants, bit-determinism, ray-chunk
-invariance, agreement of the two kernel families (fp32 CUDA cores vs tcgen05 split precision) forward and backward."""
+invariance, agreement of the two kernel families (fp32 CUDA cores vs wgmma split precision) forward and backward."""
 import math
 
 import pytest
@@ -104,7 +104,7 @@ def test_fern_ndc_full_size_runs_and_kernel_families_agree():            # BASEL
 
 
 def test_kernel_families_agree_on_gradients_at_full_size():
-    """One train step at the bench size (A1 = config/lego.yml as written): tcgen05 vs fp32 kernels."""
+    """One train step at the bench size (A1 = config/lego.yml as written): wgmma vs fp32 kernels."""
     nb, mc, mf, ro, rd, options, epf, edf, (H, W, f) = _setup(
         4096, arch=(8, 128, 3), weights=None, num_coarse=64, num_fine=128, perturb=True, radiance_field_noise_std=0.2)
     rnd = _randoms(4096, 64, 128, seed=9)

@@ -142,7 +142,7 @@ def test_shard_bounds_partition():
 
 
 def test_fp16x2_split_precision_model():
-    """CPU model of the operand split the tcgen05 chain kernels use (csrc/tc_common.cuh split_f16x2):
+    """CPU model of the operand split the wgmma chain kernels use (csrc/tc_common.cuh split_f16x2):
     hi = fp16(x) saturating, lo = fp16((x - hi) * 2^11); x ~= hi + lo * 2^-11.  Pins the documented claims: ~22
     significant bits over 6.1e-5 <= |x| < 65504 (1.5e-11 absolute below), and a three-term product sum (hi*hi + 2^-11 (lo*hi + hi*lo), fp32
     accumulation) that stays far inside the 1e-4 parity bar where a plain fp16 or tf32 product does not."""

@@ -178,7 +178,7 @@ def test_render_image_matches_run_one_iter_validation():
 
 
 def test_tc_out_of_range_activations_are_visible_not_clamped():
-    """The fp16 x 2 operands cover |activation| < 1.05e6 (value / 16 in fp16): beyond that the tcgen05 forward produces
+    """The fp16 x 2 operands cover |activation| < 1.05e6 (value / 16 in fp16): beyond that the wgmma forward produces
     inf / NaN (non-saturating conversions) instead of silently clamping -- and stays exact below."""
     from nerf_pytorch_b200 import ops
     from test_stage_parity_gpu import _arch

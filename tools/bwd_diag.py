@@ -1,4 +1,4 @@
-"""Dev tool: per-tensor error of the tcgen05 fused backward (and the CUDA-core one) against fp64 autograd of the oracle
+"""Dev tool: per-tensor error of the wgmma fused backward (and the CUDA-core one) against fp64 autograd of the oracle
 MLP, on golden cases and on ragged synthetic sizes.    python tools/bwd_diag.py"""
 import os
 import sys

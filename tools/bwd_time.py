@@ -1,4 +1,4 @@
-"""Dev tool: CUDA-event time of the fused tcgen05 backward (fine-pass size) -- used with the timing-experiment builds."""
+"""Dev tool: CUDA-event time of the fused wgmma backward alone (fine-pass size, A1)."""
 import os, sys
 import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,4 +22,4 @@ torch.cuda.synchronize(); e0.record()
 for _ in range(10):
     ops.mlp_bwd(arch, blob, rays, z, G, stash, impl=1)
 e1.record(); torch.cuda.synchronize()
-print(f"mlp_bwd (fused tcgen05, 4096 x 192 points, A1): {e0.elapsed_time(e1) / 10:.3f} ms")
+print(f"mlp_bwd (fused wgmma, 4096 x 192 points, A1): {e0.elapsed_time(e1) / 10:.3f} ms")

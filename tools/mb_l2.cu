@@ -1,7 +1,7 @@
 // mb_l2.cu -- micro-benchmarks that size the chain kernels' weight stream (dev tool, not product):
 //   (1) cp.async.bulk global(L2-resident) -> shared, all SMs, ring of 4 stages: aggregate GB/s vs chunk size
 //   (2) cp.reduce.async.bulk shared -> global .add.f32 into a small L2-resident region: aggregate GB/s
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bin/mb_l2 tools/mb_l2.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/mb_l2 tools/mb_l2.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

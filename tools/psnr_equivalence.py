@@ -5,7 +5,7 @@ lego-lowres fine network rendered through this library's deterministic forward (
 rays of spherical poses (load_blender.py:32-37).  Both students are 4x128 FlexibleNeRFModels (the architecture
 the reference CLI actually trains, SURVEY section 0.1) started from the SAME initial weights and fed the SAME
 ray batches in the same order; each draws its own sampling noise, like two runs of the reference would.
-PSNR is measured on held-out rays with the deterministic sampler.  Writes profiles/r1_psnr.json.
+PSNR is measured on held-out rays with the deterministic sampler.  Writes psnr_out/psnr_equivalence.json.
 """
 import json, math, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -108,6 +108,6 @@ res = {"iters": ITERS, "batch_rays": BATCH, "arch": "A0 4x128 (as the reference 
        "psnr_ours": curve_ours, "psnr_reference_cpu": curve_ref, "seconds_ours": t_ours, "seconds_reference_cpu": t_ref,
        "cpu_threads": THREADS, "psnr_ours_final_all_seeds": finals,
        "final_gap_db_vs_mean": sum(finals) / len(finals) - curve_ref[-1][1]}
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r1_psnr.json"), "w"), indent=1)
+os.makedirs(os.path.join(ROOT, "psnr_out"), exist_ok=True)
+json.dump(res, open(os.path.join(ROOT, "psnr_out", "psnr_equivalence.json"), "w"), indent=1)
 print(json.dumps(res))

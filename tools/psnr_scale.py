@@ -6,7 +6,7 @@ network rendered through this library's deterministic forward (perturb off, nois
 (load_blender.py:32-37).  Students: config/lego.yml as written (A1 = 8 x 128, skip every 3, coarse + fine, 64 + 128 samples,
 perturb on, noise std 0.2, Adam 5e-3 with the reference's exponential decay), started from the SAME initial weights and
 fed the SAME ray batches in the same order; every run draws its own sampling noise, like two runs of the reference would.
-PSNR is measured on 8192 held-out rays with the deterministic sampler.  Writes gpurun_out/r2_psnr_scale.json.
+PSNR is measured on 8192 held-out rays with the deterministic sampler.  Writes psnr_out/psnr_scale.json.
 
     PSNR_ITERS=5000 PSNR_BATCH=1024 PSNR_SEEDS=3 python tools/psnr_scale.py
 """
@@ -139,6 +139,6 @@ res["final_psnr_reference"] = fr
 if fo and fr:
     res["final_gap_db_mean"] = sum(fo) / len(fo) - sum(fr) / len(fr)
     res["speedup_vs_eager_gpu"] = (sum(r["seconds"] for r in res["reference_eager_gpu"]) / len(fr)) / (sum(r["seconds"] for r in res["ours"]) / len(fo))
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-json.dump(res, open(os.path.join(ROOT, "gpurun_out", "r2_psnr_scale.json"), "w"), indent=1)
+os.makedirs(os.path.join(ROOT, "psnr_out"), exist_ok=True)
+json.dump(res, open(os.path.join(ROOT, "psnr_out", "psnr_scale.json"), "w"), indent=1)
 print(json.dumps({k: v for k, v in res.items() if k not in ("ours", "reference_eager_gpu")}))
