@@ -276,7 +276,8 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   const uint32_t bar_empty = bar_full + 8 * kMaxStages;    // [kMaxStages]  stage consumed by every consumer warp
   const uint32_t n_stages = (uint32_t)mp.n_stages;
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
   const int64_t P_pad = n_tiles * kTileRows;       // the stash sections are sized in 128-point tiles
   const int enc_w = p.enc_tile_w;                  // encoding operand tile width (dim_xyz padded to 16)
 

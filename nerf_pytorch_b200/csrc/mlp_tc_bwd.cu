@@ -17,10 +17,13 @@
 // are added: ONE accumulator per weight gradient and no pre-scaled operand copies.
 //
 // Persistent kernel, one CTA per SM, two consumer warpgroups (warpgroup w owns points [64 w, 64 w + 64) of the chain
-// and features [64 w, 64 w + 64) of every weight gradient) and one producer warp streaming the chain's weight copies
-// through a cp.async.bulk ring.  Per layer: epilogue (chain accumulator + head term, ReLU mask, split -> G tile), chain
-// MMA of the warpgroup's rows, then the layer's weight-gradient jobs: A = the G tile (MN-major), B = the activation
-// tile (bulk-copied from the stash one job ahead), the 16-column ray-indicator job that yields the bias gradients and
+// and features [64 w, 64 w + 64) of every weight gradient) and one producer warpgroup, of which one thread streams the
+// chain's weight copies through a cp.async.bulk ring; the producer gives its registers to the consumers (setmaxnreg), which
+// hold the chain accumulator and a job accumulator at once.  Every wgmma is issued in warpgroup-uniform control flow (the
+// warp index is broadcast from lane 0), so ptxas keeps the MMAs of a k-loop asynchronous.  Per layer: epilogue (chain
+// accumulator + head term, ReLU mask, split -> G tile), chain MMA of the warpgroup's rows, then the layer's
+// weight-gradient jobs: A = the G tile (MN-major), B = the activation tile (bulk-copied from the stash one job ahead and
+// requested as soon as both warpgroups' MMAs of the running job are complete), the 16-column ray-indicator job that yields the bias gradients and
 // the per-ray sums of layers_dir[0], and the two narrow heads' jobs with the roles swapped (A = activation tile, B =
 // d_raw = feature rows 64..79 of the first layer's G tile).  Finished weight-gradient accumulators are unscaled into
 // a swizzled staging chunk as 64-bit fixed point and added into the L2-resident gradient blob with cp.reduce.async.bulk
@@ -33,7 +36,8 @@ namespace nerfb200 {
 
 namespace tcb {
 constexpr int kWG = 2;                            // consumer warpgroups
-constexpr int kThreadsB = 128 * kWG + 32;         // + the weight producer warp
+constexpr int kThreadsB = 128 * (kWG + 1);       // + the producer warpgroup (one thread of it streams the weights)
+constexpr int kProdRegs = 24, kConsRegs = 240;   // setmaxnreg split: (24 + 2 x 240) x 128 = 168 x 384 registers
 constexpr int kWStage = 96 * 128;                 // one k-step of a 128-wide layer: 3 copies x 2 slabs x 128 x 16 B
 constexpr int kMaxWStages = 6;
 constexpr int kGBytes = 65536;                    // G tile: hi block 32 KB, lo block 32 KB (128 features)
@@ -158,9 +162,9 @@ __device__ __forceinline__ void cta_bar() { asm volatile("bar.sync 1, 256;" ::: 
 
 // weight-gradient job of width N (columns of the B tile) for this warpgroup's 64 accumulator rows:
 //   acc = 2^-11 sum_ks (A_lo^T B_hi + A_hi^T B_lo) + sum_ks A_hi^T B_hi     (A, B MN-major; K = the tile's 128 points)
-// plus, when `ind`, the 16-column indicator product into acc_i (B = the exact 0 / 1 indicator tile, no lo part)
-template <int N>
-__device__ __forceinline__ void job_mma(float (&acc)[N / 2], float (&acc_i)[8], bool ind, uint64_t a_hi, uint32_t a_lo_off,
+// plus, when kInd, the 16-column indicator product into acc_i (B = the exact 0 / 1 indicator tile, no lo part)
+template <int N, bool kInd>
+__device__ __forceinline__ void job_mma(float (&acc)[N / 2], float (&acc_i)[8], uint64_t a_hi, uint32_t a_lo_off,
                                         uint32_t a_ks, uint64_t b_hi, uint32_t b_lo_off, uint32_t b_ks, uint64_t i_d) {
   wgmma_fence();
 #pragma unroll
@@ -168,27 +172,29 @@ __device__ __forceinline__ void job_mma(float (&acc)[N / 2], float (&acc_i)[8], 
     const uint64_t ah = desc_adv(a_hi, ks * a_ks), bh = desc_adv(b_hi, ks * b_ks);
     wgmma_f16<N, 1, 1>(acc, desc_adv(ah, a_lo_off), bh, ks > 0 ? 1 : 0);
     wgmma_f16<N, 1, 1>(acc, ah, desc_adv(bh, b_lo_off), 1);
-    if (ind) wgmma_f16<16, 1, 1>(acc_i, desc_adv(ah, a_lo_off), desc_adv(i_d, ks * 512u), ks > 0 ? 1 : 0);
+    if (kInd) wgmma_f16<16, 1, 1>(acc_i, desc_adv(ah, a_lo_off), desc_adv(i_d, ks * 512u), ks > 0 ? 1 : 0);
   }
   wgmma_commit();
   wgmma_wait<0>();
   reg_fence(acc);
-  reg_fence(acc_i);
+  if (kInd) reg_fence(acc_i);
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] *= kLoInv;
+  if (kInd) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) acc_i[i] *= kLoInv;
+    for (int i = 0; i < 8; ++i) acc_i[i] *= kLoInv;
+  }
   wgmma_fence();
 #pragma unroll
   for (int ks = 0; ks < 8; ++ks) {
     const uint64_t ah = desc_adv(a_hi, ks * a_ks);
     wgmma_f16<N, 1, 1>(acc, ah, desc_adv(b_hi, ks * b_ks), 1);
-    if (ind) wgmma_f16<16, 1, 1>(acc_i, ah, desc_adv(i_d, ks * 512u), 1);
+    if (kInd) wgmma_f16<16, 1, 1>(acc_i, ah, desc_adv(i_d, ks * 512u), 1);
   }
   wgmma_commit();
   wgmma_wait<0>();
   reg_fence(acc);
-  reg_fence(acc_i);
+  if (kInd) reg_fence(acc_i);
 }
 
 // the finished accumulator (64 rows of this warpgroup x N columns) -> unscale -> fixed point -> swizzled staging chunks
@@ -246,7 +252,8 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   uint64_t* x_full = bars + 2 * kMaxWStages;    // the running job's activation tile landed
   const uint32_t n_stages = (uint32_t)mp.n_stages;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
   const int64_t P_pad = n_tiles * kTileRows;
   const int E = p.n_gemm;
   const int hw1 = p.h[0].n_out * p.h[0].k;
@@ -275,9 +282,10 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 
   const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
 
-  if (warp == 4 * kWG) {
+  if (warp >= 4 * kWG) {
     // ===================== weight producer: the chain of event e streams layer t's transposed copies ============
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProdRegs));
+    if (warp == 4 * kWG && lane == 0) {
       Pipe pp;
       const uint64_t pol = l2_policy_evict_last();
       for (int it = 0; it < my_tiles; ++it)
@@ -295,6 +303,7 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     }
   } else {
     // ===================== consumer warpgroups =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsRegs));
     const int wg = warp >> 2, wt = tid & 127, q = lane & 3;
     const int r0 = 16 * (wt >> 5) + (lane >> 2);   // warpgroup-local row of accumulator row 0 (row 1: + 8)
     unsigned long long* stg = reinterpret_cast<unsigned long long*>(sm + mp.stg) + wg * 2 * (kStgBytes / 8);
@@ -345,12 +354,6 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       const bool scaled = ex >= 3u && ex <= 254u;
       const float sc = scaled ? __uint_as_float((256u - ex) << 23) : 1.f;
       const float us = (scaled ? __uint_as_float((ex - 2u) << 23) : 1.f) * kActInv;  // activations are stored / 16
-      float dr[2][4];
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const float4 d4 = valid[i] ? reinterpret_cast<const float4*>(d_raw)[pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
-        dr[i][0] = d4.x * sc; dr[i][1] = d4.y * sc; dr[i][2] = d4.z * sc; dr[i][3] = d4.w * sc;
-      }
 
       float chain[64];  // G_{t+1} W_{t+1}[:, :128] of this warpgroup's rows (the previous event's chain MMA)
 #pragma unroll
@@ -377,6 +380,21 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
               mw[i][m] = valid[i] ? __ldg(mask_row + m) : 0u;
             }
           }
+        // d_raw of this thread's rows at the tile scale (re-read per event rather than kept live through the MMAs), and
+        // the head outputs' entries of it selected once (a runtime index into dr would put it in local memory)
+        float dr[2][4], hd[2][4];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float4 d4 = valid[i] ? reinterpret_cast<const float4*>(d_raw)[pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
+          dr[i][0] = d4.x * sc; dr[i][1] = d4.y * sc; dr[i][2] = d4.z * sc; dr[i][3] = d4.w * sc;
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            const int k = (hcol + c) & 3;
+            hd[i][c] = k == 0 ? dr[i][0] : k == 1 ? dr[i][1] : k == 2 ? dr[i][2] : dr[i][3];
+          }
         // ---------------- epilogue: G_t of this thread's elements -> hi / lo -> the G tile ----------------
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -385,11 +403,13 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
               float y0 = chain[4 * j + 2 * i], y1 = chain[4 * j + 2 * i + 1];  // Y = 2048 x, the accumulator's own scale
-              for (int c = 0; c < hn; ++c) {
-                const float dd = dr[i][(hcol + c) & 3];
-                const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
-                y0 = fmaf(dd, w.x, y0);
-                y1 = fmaf(dd, w.y, y1);
+#pragma unroll
+              for (int c = 0; c < 4; ++c) {
+                if (c < hn) {
+                  const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
+                  y0 = fmaf(hd[i][c], w.x, y0);
+                  y1 = fmaf(hd[i][c], w.y, y1);
+                }
               }
               const uint32_t word = mw[i][j >> 2];
               const int bit = 8 * (j & 3) + 2 * q;
@@ -485,6 +505,20 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
           const uint32_t fstr = (uint32_t)(w >> 3) * 128u;  // bytes between 8-point blocks of the activation tile
           mbar_wait(x_full, x_ph);
           x_ph ^= 1;
+          // Called once per job by every consumer thread as soon as its warpgroup's MMAs are complete: once both
+          // warpgroups are through, nothing reads the activation tile any more and thread 0 requests the next job's, so
+          // that the load overlaps this job's drain instead of following it.
+          auto release_x = [&]() {
+            cta_bar();
+            if (tid == 0) {
+              int ni = i + 1, ne = e, nit = it;
+              if (ni == nj) {
+                ni = 0;
+                if (++ne == E) { ne = 0; ++nit; }
+              }
+              if (nit < my_tiles) issue_x(nit, ne, ni);
+            }
+          };
           if (jq.kind == 1) {
             // head job: A = activation tile (rows = its features, MN-major), B = d_raw (feature rows 64..79 of the G tile)
             if (64 * wg < jq.nrows) {
@@ -492,7 +526,8 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
               const uint64_t xa = make_desc(smem_u32(sX) + (uint32_t)wg * 1024u, fstr, 128);
               const uint64_t db = make_desc(smem_u32(sG) + 1024u, 2048, 128);
               // residual products first: A_lo B_hi + A_hi B_lo (job_mma's scheme with B's lo block 32 KB on)
-              job_mma<16>(acc, dummy, false, xa, 32768u, 2 * fstr, db, 32768u, 4096u, 0);
+              job_mma<16, false>(acc, dummy, xa, 32768u, 2 * fstr, db, 32768u, 4096u, 0);
+              release_x();
               const HeadLayer& h = p.h[jq.dst_head];
 #pragma unroll
               for (int jj = 0; jj < 2; ++jj)
@@ -504,6 +539,8 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
                     if (k < h.k && c >= 0 && c < h.n_out)
                       atomicAdd(gb + bm.xh + jq.dst_head * 512 + c * 128 + k, to_fix(acc[4 * jj + 2 * ii + cc] * us));
                   }
+            } else {
+              release_x();
             }
           } else if (64 * wg < jq.nrows || (i == 0 && e == 0 && p.use_viewdirs)) {
             // (warpgroup 1 of layers_dir[0]'s first job only sums the d_raw rows 64..67 of the indicator product)
@@ -515,7 +552,9 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #define NB_JOB(NN)                                                                                   \
   {                                                                                                  \
     float acc[NN / 2];                                                                               \
-    job_mma<NN>(acc, acc_i, i == 0, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);                    \
+    if (i == 0) job_mma<NN, true>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);          \
+    else job_mma<NN, false>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);                \
+    release_x();                                                                                     \
     if (64 * wg < jq.nrows) job_drain<NN>(acc, us, gdst, stg, stg_n, wg);                            \
   }
             if (w == 128) NB_JOB(128) else if (w == 64) NB_JOB(64) else if (w == 48) NB_JOB(48)
@@ -543,23 +582,17 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
                 }
               }
             }
+          } else {
+            release_x();
           }
-          cta_bar();  // both warpgroups are done with the activation tile (and the per-ray sums are in place)
           if (e == 0 && i == 0 && p.use_viewdirs) {
+            cta_bar();  // the per-ray sums of both warpgroups are in place
             for (int idx = tid; idx < 64 * p.dim_dir; idx += 128 * kWG) {
               const int n = idx / p.dim_dir, k = idx - n * p.dim_dir;
               float a = 0.f;
               for (int jr = 0; jr < n_rays_tile; ++jr) a = fmaf(s_sums[n * 16 + jr], s_encd[jr * 32 + k], a);
               s_dacc[n * 28 + k] += a;
             }
-          }
-          if (tid == 0) {  // the next job's activation tile
-            int ni = i + 1, ne = e, nit = it;
-            if (ni == nj) {
-              ni = 0;
-              if (++ne == E) { ne = 0; ++nit; }
-            }
-            if (nit < my_tiles) issue_x(nit, ne, ni);
           }
         }
       }

@@ -1,6 +1,7 @@
 // mb_l2.cu -- micro-benchmarks that size the chain kernels' weight stream (dev tool, not product):
 //   (1) cp.async.bulk global(L2-resident) -> shared, all SMs, ring of 4 stages: aggregate GB/s vs chunk size
-//   (2) cp.reduce.async.bulk shared -> global .add.f32 into a small L2-resident region: aggregate GB/s
+//   (2) cp.reduce.async.bulk shared -> global .add.f32 and .add.u64 (the backward's fixed-point gradient blob) into a
+//       small L2-resident region: aggregate GB/s
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/mb_l2 tools/mb_l2.cu
 #include <cstdio>
 #include <cstdint>
@@ -49,20 +50,30 @@ __global__ void __launch_bounds__(64, 1) stream_kernel(const uint8_t* __restrict
   }
 }
 
-__global__ void __launch_bounds__(128, 1) reduce_kernel(float* __restrict__ dst, size_t dst_floats, uint32_t chunk, int iters) {
+template <bool kU64>
+__global__ void __launch_bounds__(128, 1) reduce_kernel(void* __restrict__ dst_v, size_t dst_bytes, uint32_t chunk, int iters) {
   extern __shared__ __align__(1024) uint8_t sm[];
-  float* tile = reinterpret_cast<float*>(sm);
-  for (uint32_t i = threadIdx.x; i < chunk / 4; i += blockDim.x) tile[i] = 1.0f;
+  uint8_t* dst = reinterpret_cast<uint8_t*>(dst_v);
+  if (kU64) {
+    unsigned long long* tile = reinterpret_cast<unsigned long long*>(sm);
+    for (uint32_t i = threadIdx.x; i < chunk / 8; i += blockDim.x) tile[i] = 1ull;
+  } else {
+    float* tile = reinterpret_cast<float*>(sm);
+    for (uint32_t i = threadIdx.x; i < chunk / 4; i += blockDim.x) tile[i] = 1.0f;
+  }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
   if (threadIdx.x == 0) {
-    size_t off = ((size_t)blockIdx.x * 104729u * (chunk / 4)) % (dst_floats - chunk / 4);
-    off &= ~(size_t)31;
+    size_t off = ((size_t)blockIdx.x * 104729u * chunk) % (dst_bytes - chunk);
+    off &= ~(size_t)127;
     for (int it = 0; it < iters; ++it) {
-      asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst + off), "r"(smem_u32(tile)), "r"(chunk) : "memory");
+      if (kU64)
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(dst + off), "r"(smem_u32(sm)), "r"(chunk) : "memory");
+      else
+        asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f32 [%0], [%1], %2;" ::"l"(dst + off), "r"(smem_u32(sm)), "r"(chunk) : "memory");
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       if ((it & 3) == 3) asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory");
-      off += chunk / 4; if (off + chunk / 4 > dst_floats) off = 0;
+      off += chunk; if (off + chunk > dst_bytes) off = 0;
     }
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
@@ -75,7 +86,6 @@ int main() {
   long long* cyc; cudaMalloc(&cyc, sizeof(long long) * 1024);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaFuncSetAttribute(stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-  cudaFuncSetAttribute(reduce_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
   const uint32_t chunks[] = {8192, 12288, 24576, 32768, 49152};
   for (uint32_t chunk : chunks) {
     const int iters = (int)((size_t)256 * 1024 * 1024 / chunk / 4);
@@ -92,16 +102,22 @@ int main() {
              (double)iters * chunk / (double)c0, (double)c0 / ms * 1e-3);
     }
   }
-  float* dst; const size_t dst_floats = 672 * 1024 / 4; cudaMalloc(&dst, dst_floats * 4); cudaMemset(dst, 0, dst_floats * 4);
-  for (uint32_t chunk : {16384u, 65536u}) {
-    const int iters = (int)((size_t)64 * 1024 * 1024 / chunk);
-    reduce_kernel<<<sms, 128, chunk>>>(dst, dst_floats, chunk, 16);
-    cudaEventRecord(e0);
-    reduce_kernel<<<sms, 128, chunk>>>(dst, dst_floats, chunk, iters);
-    cudaEventRecord(e1); cudaEventSynchronize(e1);
-    float ms; cudaEventElapsedTime(&ms, e0, e1);
-    printf("reduce-add chunk %6u: %.3f ms  %.1f GB/s aggregate\n", chunk, ms, (double)sms * iters * chunk / ms * 1e-6);
-  }
+  // the destination is sized like the fine backward's gradient blob (~0.6 MB): L2-resident, every SM adds into it
+  void* dst; const size_t dst_bytes = 672 * 1024; cudaMalloc(&dst, dst_bytes); cudaMemset(dst, 0, dst_bytes);
+  cudaFuncSetAttribute(reduce_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+  cudaFuncSetAttribute(reduce_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
+  for (int u64 = 0; u64 < 2; ++u64)
+    for (uint32_t chunk : {8192u, 16384u, 65536u}) {
+      auto kern = u64 ? reduce_kernel<true> : reduce_kernel<false>;
+      const int iters = (int)((size_t)64 * 1024 * 1024 / chunk);
+      kern<<<sms, 128, chunk>>>(dst, dst_bytes, chunk, 16);
+      cudaEventRecord(e0);
+      kern<<<sms, 128, chunk>>>(dst, dst_bytes, chunk, iters);
+      cudaEventRecord(e1); cudaEventSynchronize(e1);
+      float ms; cudaEventElapsedTime(&ms, e0, e1);
+      printf("reduce-add .%s chunk %6u: %.3f ms  %.1f GB/s aggregate\n", u64 ? "u64" : "f32", chunk, ms,
+             (double)sms * iters * chunk / ms * 1e-6);
+    }
   printf("err: %s\n", cudaGetErrorString(cudaGetLastError()));
   return 0;
 }
