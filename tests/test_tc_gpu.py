@@ -156,6 +156,7 @@ def test_tc_forward_hidden_256_matches_oracle_and_fp32_kernel(viewdirs):
     e_tc = (raw1.cpu().double() - want).abs().max().item()
     e_simt = (raw0.cpu().double() - want).abs().max().item()
     assert e_tc <= 3e-5 * scale + 1e-6, (e_tc, e_simt, scale)
+    assert e_simt <= 3e-5 * scale, (e_tc, e_simt, scale)   # the fp32 kernels measure <= 3.3e-6 (test_simt_hidden256_gpu)
     assert torch.isfinite(raw1).all()
 
 
