@@ -213,6 +213,38 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl,
                             int32_t parts, void* stream);
 
+/* ---- seeded random numbers ----------------------------------------------------------------------
+ * The render path's four random inputs as a pure function of (seed, step, stream, global ray, sample), generated
+ * inside the kernels that use them: Philox4x32-10 keyed by the seed, counter (sample / 4, stream + 4 * step, global
+ * ray low 32 bits, high 32 bits); streams 0 t_rand, 1 noise_c, 2 u, 3 noise_f.  Uniforms are (w >> 8) * 2^-24 in
+ * [0, 1); normals are Box-Muller on word pairs with u1 = ((w >> 8) + 1) * 2^-24 (the exact definition is in
+ * csrc/common.cuh).  A ray's numbers do not depend on how the batch is chunked or sharded. */
+typedef struct nerfb200_rng {
+  uint64_t seed;
+  uint64_t step;      /* training step (< 2^30) */
+  int64_t ray_offset; /* global index of the call's first ray (>= 0) */
+} nerfb200_rng_t;
+
+/* render_fwd / render_bwd with the random tensors generated in-kernel from *rng (stream ids as above).  With perturb
+ * off the fine pass's u is the det=True linspace, as in render_fwd.  render_bwd_seeded regenerates the noise for the
+ * sigma ReLU gate and reads no noise tensor; pass it the same *rng as the render_fwd_seeded call that filled the
+ * workspace. */
+int32_t nerfb200_render_fwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                   const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
+                                   const nerfb200_rng_t* rng, float* out_coarse, float* out_fine, void* workspace,
+                                   int32_t training, int32_t impl, void* stream);
+int32_t nerfb200_render_bwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                   const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                   const float* g_coarse, const float* g_fine, void* workspace, float* flat_grad_c,
+                                   float* flat_grad_f, int32_t impl, int32_t parts, void* stream);
+/* Materialises stream `stream_id` (0..3) for rays ray_offset .. ray_offset + n_rays - 1, samples 0 .. per_ray - 1:
+ * out[n_rays][per_ray], uniforms for streams 0 and 2, unit normals for 1 and 3.  The numbers the render kernels use,
+ * through the same device function: what render_fwd_seeded consumes equals render_fwd fed these tensors. */
+int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64_t n_rays, int32_t per_ray, float* out,
+                             void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

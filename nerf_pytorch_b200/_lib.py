@@ -46,9 +46,19 @@ class RenderOpts(C.Structure):
     ]
 
 
+class Rng(C.Structure):
+    """nerfb200_rng_t"""
+
+    _fields_ = [
+        ("seed", C.c_uint64),
+        ("step", C.c_uint64),
+        ("ray_offset", C.c_int64),
+    ]
+
+
 P = C.c_void_p
 I32, I64, F32 = C.c_int32, C.c_int64, C.c_float
-AP, OP = C.POINTER(Arch), C.POINTER(RenderOpts)
+AP, OP, RP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng)
 
 # name -> (restype, argtypes); mirrors include/nerfb200.h one-to-one
 SIGNATURES = {
@@ -79,6 +89,9 @@ SIGNATURES = {
     "nerfb200_render_workspace_layout": (I32, [AP, AP, OP, I64, I32, C.POINTER(I64)]),
     "nerfb200_render_fwd": (I32, [AP, AP, OP, P, P, P, I32, I64, P, P, P, P, I32, P, P, P, P, I32, I32, P]),
     "nerfb200_render_bwd": (I32, [AP, AP, OP, P, P, P, I32, I64, P, P, P, P, P, P, P, I32, I32, P]),
+    "nerfb200_render_fwd_seeded": (I32, [AP, AP, OP, P, P, P, I32, I64, P, RP, P, P, P, I32, I32, P]),
+    "nerfb200_render_bwd_seeded": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, I32, I32, P]),
+    "nerfb200_random_fill": (I32, [RP, I32, I64, I32, P, P]),
     "nerfb200_adam_step": (I32, [P, P, P, P, I64, I32, F32, F32, F32, F32, F32, P]),
 }
 

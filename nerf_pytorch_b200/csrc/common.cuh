@@ -71,6 +71,47 @@ struct Plan {
   float freq_dir[NERFB200_MAX_FREQS];
 };
 
+// ---------------------------------------------------------------------------------------------
+// Random inputs of the render kernels.  Each one comes either from a tensor the host drew (the reference's
+// torch.rand / torch.randn order) or from the seeded counter-based stream defined below (nerfb200_rng_t).
+//
+// The seeded stream is Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011):
+//   key     = (seed & 0xffffffff, seed >> 32)
+//   counter = (sample >> 2, stream + 4 * step, ray & 0xffffffff, ray >> 32)
+// with ray the GLOBAL ray index (ray_offset + the ray's row in the call) and stream 0 t_rand, 1 noise_c, 2 u, 3 noise_f.
+// One call yields the four 32-bit words w[0..3] of samples 4b .. 4b + 3 of one ray in one stream.
+//   uniform (t_rand, u):     sample j = 4b + i is (w[i] >> 8) * 2^-24, in [0, 1) (torch's 24-bit construction)
+//   normal (noise_c, noise_f): Box-Muller on the pairs (w[0], w[1]) -> samples 4b, 4b + 1 and (w[2], w[3]) -> 4b + 2,
+//                            4b + 3: u1 = ((w[2p] >> 8) + 1) * 2^-24 in (0, 1], u2 = (w[2p + 1] >> 8) * 2^-24,
+//                            r = sqrt(-2 ln u1), sample 4b + 2p = r cos(2 pi u2), sample 4b + 2p + 1 = r sin(2 pi u2),
+//                            evaluated in fp64 and rounded once to fp32.
+// So every random number is a pure function of (seed, step, stream, global ray, sample): a ray gets the same numbers
+// whatever the chunking of the batch or its sharding across GPUs.  step < 2^30 keeps stream + 4 * step in 32 bits.
+// ---------------------------------------------------------------------------------------------
+enum RandStream { kRandTRand = 0, kRandNoiseC = 1, kRandU = 2, kRandNoiseF = 3 };
+
+struct RandSrc {
+  const float* ptr;    // tensor source [ray][stride], or nullptr
+  int64_t stride;      // floats per ray in ptr (0: one row shared by every ray)
+  int seeded;          // ptr == nullptr and seeded: generate from the stream below; neither: no source
+  uint32_t key0, key1; // the seed
+  uint32_t ctr1;       // stream + 4 * step
+  int64_t ray_offset;  // global index of the call's first ray
+
+  __host__ __device__ bool present() const { return ptr != nullptr || seeded; }
+#ifdef __CUDACC__
+  __device__ __forceinline__ float uniform(int64_t ray, int j) const;
+  __device__ __forceinline__ float normal(int64_t ray, int j) const;
+#endif
+};
+
+inline RandSrc rand_none() { return RandSrc{nullptr, 0, 0, 0, 0, 0, 0}; }
+inline RandSrc rand_tensor(const float* p, int64_t stride) { return RandSrc{p, stride, 0, 0, 0, 0, 0}; }
+inline RandSrc rand_seeded(const nerfb200_rng_t& r, int stream) {
+  return RandSrc{nullptr, 0, 1, (uint32_t)r.seed, (uint32_t)(r.seed >> 32), (uint32_t)stream + 4u * (uint32_t)r.step,
+                 r.ray_offset};
+}
+
 // host side (api.cu)
 int build_plan(const nerfb200_arch_t* arch, Plan* plan);  // 0 or NERFB200_ERR_*
 void set_error(const char* fmt, ...);
@@ -81,7 +122,9 @@ int device_sms();     // SM count of the current device (grid sizes of persisten
 // launchers (one per .cu), all return NERFB200_OK or an error code
 int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s);
 int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const float* t_vals,
-                         const float* t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s);
+                         const RandSrc& t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s);
+// materialises n_rays x per_ray numbers of a seeded stream (uniform for t_rand / u, normal for noise_c / noise_f)
+int launch_random_fill(const RandSrc& src, int stream_id, int64_t n_rays, int per_ray, float* out, cudaStream_t s);
 int launch_gen_rays(const float* c2w12_host, int height, int width, float focal, const int64_t* pix, int64_t n, int ndc,
                     float near, float far, int use_viewdirs, int out_stride, float* out, cudaStream_t s);
 int launch_pack_rays(const float* ro, const float* rd, int64_t n, int height, int width, float focal, int ndc, float near,
@@ -105,13 +148,14 @@ int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int r
 int64_t bwd_tc_scratch_floats(const Plan& p);
 int tc_supported(const Plan& p, int n_samples, const char* what, bool training);  // forward (training: + stash)
 int bwd_tc_supported(const Plan& p, int n_samples, const char* what);  // forward + backward
-int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const float* noise,
+int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s);
-int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const float* noise,
+int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          const float* g_out, int64_t n_rays, int n_samples, float noise_std, int white_bkgd,
                          float* d_raw, cudaStream_t s);
-int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const float* u, int u_stride,
+// u: a tensor ([n_rays][n_fine], or one shared row with stride 0), the seeded stream, or none (the det=True linspace)
+int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const RandSrc& u,
                             const float* cdf_in, int64_t n_rays, int n_coarse, int n_fine, float* z_fine,
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s);
 int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2,
@@ -146,6 +190,52 @@ __device__ __forceinline__ void encode_coord(float x, int c, int include, int f_
     row[base + 6 * f + c] = s;
     row[base + 6 * f + 3 + c] = co;
   }
+}
+
+// Philox4x32-10: ten rounds, the key bumped by the Weyl constants between rounds (Random123's philox4x32_R(10, ...)).
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    if (i) {
+      k0 += 0x9E3779B9u;
+      k1 += 0xBB67AE85u;
+    }
+    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+
+__device__ __forceinline__ uint4 rand_block(const RandSrc& s, int64_t ray, int j) {
+  const uint64_t g = (uint64_t)(s.ray_offset + ray);
+  return philox4x32_10(make_uint4((uint32_t)j >> 2, s.ctr1, (uint32_t)g, (uint32_t)(g >> 32)), s.key0, s.key1);
+}
+
+__device__ __forceinline__ float RandSrc::uniform(int64_t ray, int j) const {
+  if (ptr) return ptr[ray * stride + j];
+  const uint4 w = rand_block(*this, ray, j);
+  const uint32_t x = (j & 2) ? ((j & 1) ? w.w : w.z) : ((j & 1) ? w.y : w.x);
+  return (float)(x >> 8) * 0x1p-24f;
+}
+
+__device__ __forceinline__ float RandSrc::normal(int64_t ray, int j) const {
+  if (ptr) return ptr[ray * stride + j];
+  const uint4 w = rand_block(*this, ray, j);
+  const uint32_t a = (j & 2) ? w.z : w.x, b = (j & 2) ? w.w : w.y;
+  const double u1 = (double)((a >> 8) + 1) * 0x1p-24, u2 = (double)(b >> 8) * 0x1p-24;
+  const double r = sqrt(-2.0 * log(u1));
+  double sn, cs;
+  sincospi(2.0 * u2, &sn, &cs);
+  return (float)(r * ((j & 1) ? sn : cs));
+}
+
+// torch.linspace(0, 1, n)[q] as torch's CUDA kernel evaluates it (the det=True u of sample_pdf, nerf_helpers.py:272-276)
+__device__ __forceinline__ float linspace01(int q, int n) {
+  if (n == 1) return 0.f;
+  const float step = __fdiv_rn(1.0f, (float)(n - 1));
+  if (q < n / 2) return __fmul_rn(step, (float)q);
+  return __fmaf_rn(-step, (float)(n - q - 1), 1.0f);
 }
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {

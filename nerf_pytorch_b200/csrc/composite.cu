@@ -3,8 +3,9 @@
 // owns the contiguous chunk of samples [L*C, (L+1)*C), C = ceil(S/32); the exclusive product /
 // suffix sum across chunks is a warp shuffle scan.
 //
-// Algorithmic HBM bytes per ray (fp32): forward reads raw (16 S) + z (4 S) + noise (4 S) + ray (12),
-// writes weights (4 S, coarse only) + 32 B of outputs; SURVEY.md section 8(d).
+// Algorithmic HBM bytes per ray (fp32): forward reads raw (16 S) + z (4 S) + noise (4 S; none when the noise is
+// generated in-kernel from the seeded stream) + ray (12), writes weights (4 S, coarse only) + 32 B of outputs;
+// SURVEY.md section 8(d).
 #include "common.cuh"
 
 namespace nerfb200 {
@@ -67,7 +68,7 @@ __device__ __forceinline__ float warp_excl_suffix_sum(float v, int lane) {
 
 __global__ void __launch_bounds__(kCompWarps * 32)
 composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ rays,
-                     int ray_stride, const float* __restrict__ noise, int64_t n_rays, int S, float noise_std,
+                     int ray_stride, const RandSrc noise, int64_t n_rays, int S, float noise_std,
                      int white_bkgd, float* __restrict__ out, float* __restrict__ weights) {
   extern __shared__ float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -81,15 +82,14 @@ composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
   const float4* raw4 = reinterpret_cast<const float4*>(raw) + r * S;
   const float* zr = z + r * S;
-  const float* nr = noise ? noise + r * S : nullptr;
-  const bool has_noise = (nr != nullptr) && noise_std > 0.f;
+  const bool has_noise = noise.present() && noise_std > 0.f;
 
   float prod = 1.0f;
   for (int j = j0; j < j1; ++j) {
     const float zi = zr[j];
     const bool last = (j == S - 1);
     const float zn = last ? 0.f : zr[j + 1];
-    const SampleTerms t = sample_terms(raw4[j].w, has_noise ? nr[j] : 0.f, noise_std, has_noise, zi, zn, last, dnorm);
+    const SampleTerms t = sample_terms(raw4[j].w, has_noise ? noise.normal(r, j) : 0.f, noise_std, has_noise, zi, zn, last, dnorm);
     s_alpha[j] = t.alpha;
     prod *= t.q;
   }
@@ -125,7 +125,7 @@ composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
 
 __global__ void __launch_bounds__(kCompWarps * 32)
 composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ rays,
-                     int ray_stride, const float* __restrict__ noise, const float* __restrict__ g_out,
+                     int ray_stride, const RandSrc noise, const float* __restrict__ g_out,
                      int64_t n_rays, int S, float noise_std, int white_bkgd, float* __restrict__ d_raw) {
   extern __shared__ float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -141,8 +141,7 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
   const float4* raw4 = reinterpret_cast<const float4*>(raw) + r * S;
   const float* zr = z + r * S;
-  const float* nr = noise ? noise + r * S : nullptr;
-  const bool has_noise = (nr != nullptr) && noise_std > 0.f;
+  const bool has_noise = noise.present() && noise_std > 0.f;
   const float4 g0 = reinterpret_cast<const float4*>(g_out + r * 8)[0];  // d r g b disp
   const float g_acc_in = g_out[r * 8 + 4];
 
@@ -151,7 +150,7 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   for (int j = j0; j < j1; ++j) {
     const bool last = (j == S - 1);
     const SampleTerms t =
-        sample_terms(raw4[j].w, has_noise ? nr[j] : 0.f, noise_std, has_noise, zr[j], last ? 0.f : zr[j + 1], last, dnorm);
+        sample_terms(raw4[j].w, has_noise ? noise.normal(r, j) : 0.f, noise_std, has_noise, zr[j], last ? 0.f : zr[j + 1], last, dnorm);
     s_alpha[j] = t.alpha;
     prod *= t.q;
   }
@@ -199,7 +198,7 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
     suffix += v * a * Tj;
     const bool last = (j == S - 1);
     const SampleTerms t =
-        sample_terms(raw4[j].w, has_noise ? nr[j] : 0.f, noise_std, has_noise, zr[j], last ? 0.f : zr[j + 1], last, dnorm);
+        sample_terms(raw4[j].w, has_noise ? noise.normal(r, j) : 0.f, noise_std, has_noise, zr[j], last ? 0.f : zr[j + 1], last, dnorm);
     const float dsigma = t.gate ? dalpha * t.delta * t.sigma_delta_exp : 0.f;
     const float w = a * Tj;
     const float4 rv = raw4[j];
@@ -208,7 +207,7 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   }
 }
 
-int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const float* noise,
+int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s) {
   const size_t smem = (size_t)kCompWarps * n_samples * sizeof(float);
@@ -219,7 +218,7 @@ int launch_composite_fwd(const float* raw, const float* z, const float* rays, in
   return check_cuda(cudaGetLastError(), "composite_fwd launch");
 }
 
-int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const float* noise,
+int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          const float* g_out, int64_t n_rays, int n_samples, float noise_std, int white_bkgd,
                          float* d_raw, cudaStream_t s) {
   const size_t smem = (size_t)kCompWarps * 3 * n_samples * sizeof(float);

@@ -25,7 +25,7 @@ __device__ __forceinline__ float coarse_depth(float near, float far, float t, in
 }
 
 __global__ void sample_coarse_kernel(const float* __restrict__ rays, int ray_stride, int64_t n_rays,
-                                     const float* __restrict__ t_vals, const float* __restrict__ t_rand,
+                                     const float* __restrict__ t_vals, const RandSrc t_rand,
                                      int nc, int perturb, int lindisp, float* __restrict__ z) {
   const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (idx >= n_rays * nc) return;
@@ -40,11 +40,11 @@ __global__ void sample_coarse_kernel(const float* __restrict__ rays, int ray_str
   float upper = zi, lower = zi;
   if (i + 1 < nc) upper = __fmul_rn(0.5f, __fadd_rn(coarse_depth(near, far, t_vals[i + 1], lindisp), zi));
   if (i > 0) lower = __fmul_rn(0.5f, __fadd_rn(zi, coarse_depth(near, far, t_vals[i - 1], lindisp)));
-  z[idx] = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), t_rand[idx]));
+  z[idx] = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), t_rand.uniform(r, i)));
 }
 
 int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const float* t_vals,
-                         const float* t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s) {
+                         const RandSrc& t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s) {
   const int64_t total = n_rays * n_coarse;
   const int threads = 256;
   const int64_t blocks = (total + threads - 1) / threads;
@@ -52,6 +52,27 @@ int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, cons
                                                             perturb, lindisp, z);
   count_launch();
   return check_cuda(cudaGetLastError(), "sample_coarse launch");
+}
+
+// ---------------------------------------------------------------------------------------------
+// a seeded stream written out (nerfb200_random_fill): the same RandSrc calls the render kernels make
+// ---------------------------------------------------------------------------------------------
+__global__ void random_fill_kernel(const RandSrc src, int normal, int64_t n_rays, int per_ray, float* __restrict__ out) {
+  const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (idx >= n_rays * per_ray) return;
+  const int64_t r = idx / per_ray;
+  const int j = (int)(idx - r * per_ray);
+  out[idx] = normal ? src.normal(r, j) : src.uniform(r, j);
+}
+
+int launch_random_fill(const RandSrc& src, int stream_id, int64_t n_rays, int per_ray, float* out, cudaStream_t s) {
+  const int64_t total = n_rays * per_ray;
+  const int threads = 256;
+  const int64_t blocks = (total + threads - 1) / threads;
+  const int normal = stream_id == kRandNoiseC || stream_id == kRandNoiseF;
+  random_fill_kernel<<<(unsigned)blocks, threads, 0, s>>>(src, normal, n_rays, per_ray, out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "random_fill launch");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -84,7 +105,7 @@ constexpr int kPdfWarps = 4;
 
 __global__ void __launch_bounds__(kPdfWarps * 32)
 sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restrict__ weights,
-                        const float* __restrict__ u, int u_stride, const float* __restrict__ cdf_in,
+                        const RandSrc u, const float* __restrict__ cdf_in,
                         int64_t n_rays, int nc, int nf, int npow2, float* __restrict__ z_fine,
                         float* __restrict__ z_samples, int32_t* __restrict__ inds_out,
                         float* __restrict__ cdf_out) {
@@ -135,7 +156,7 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
 
   // inverse CDF (nerf_helpers.py:286-300): searchsorted(cdf, u, side="right") by binary search
   for (int q = lane; q < nf; q += 32) {
-    const float uq = u[(u_stride ? r * (int64_t)u_stride : 0) + q];
+    const float uq = u.present() ? u.uniform(r, q) : linspace01(q, nf);
     int lo = 0, hi = nb;
     while (lo < hi) {
       const int mid = (lo + hi) >> 1;
@@ -177,8 +198,7 @@ sample_pdf_merge_kernel(const float* __restrict__ z_coarse, const float* __restr
   }
 }
 
-int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const float* u, int u_stride,
-                            const float* cdf_in, int64_t n_rays, int n_coarse, int n_fine, float* z_fine,
+int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const RandSrc& u, const float* cdf_in, int64_t n_rays, int n_coarse, int n_fine, float* z_fine,
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s) {
   int npow2 = 1;
   while (npow2 < n_coarse + n_fine) npow2 <<= 1;
@@ -191,7 +211,7 @@ int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, 
   }
   const int64_t blocks = (n_rays + kPdfWarps - 1) / kPdfWarps;
   sample_pdf_merge_kernel<<<(unsigned)blocks, kPdfWarps * 32, smem, s>>>(
-      z_coarse, weights_coarse, u, u_stride, cdf_in, n_rays, n_coarse, n_fine, npow2, z_fine, z_samples, inds,
+      z_coarse, weights_coarse, u, cdf_in, n_rays, n_coarse, n_fine, npow2, z_fine, z_samples, inds,
       cdf_out);
   count_launch();
   return check_cuda(cudaGetLastError(), "sample_pdf_merge launch");

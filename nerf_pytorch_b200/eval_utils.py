@@ -12,17 +12,23 @@ from typing import Optional
 import torch
 
 from . import ops, train_utils
+from .ops import SeededRandoms
 
 
 def render_image(height, width, focal_length, tform_cam2world, model_coarse, model_fine, options, mode="validation",
                  encode_position_fn=None, encode_direction_fn=None, *, rays_per_chunk: Optional[int] = None,
-                 device=None, impl: Optional[int] = None):
+                 device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None):
     """One pose -> (rgb_coarse (H,W,3), disp_coarse (H,W), acc_coarse (H,W), rgb_fine, disp_fine, acc_fine).
 
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
     ``train_utils.COMPAT_MODE_QUIRK`` is switched off (the reference forgets to forward ``mode``, train_utils.py:171-181);
     the chunk size comes from ``options.nerf.<mode>.chunksize`` (``rays_per_chunk`` overrides it: the fused kernels
-    need no small chunks, an H100's 80 GB of HBM hold a whole 800 x 800 image's intermediates)."""
+    need no small chunks, an H100's 80 GB of HBM hold a whole 800 x 800 image's intermediates).
+
+    ``randoms``: a ``SeededRandoms`` makes a render with ``perturb`` or noise on reproducible: pixel ``j * width + i`` is
+    ray ``ray_offset + j * width + i`` of the seeded stream whatever the chunk size.  Default: torch draws per chunk."""
+    if randoms is not None and not isinstance(randoms, SeededRandoms):
+        raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:
         device = next(model_coarse.parameters()).device
     use_viewdirs = bool(options.nerf.use_viewdirs)
@@ -36,7 +42,8 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
         parts = [train_utils.predict_and_render_radiance(
             rays[i:i + chunk], model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
-            encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl)
+            encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl,
+            randoms=randoms.shifted(i) if randoms is not None else None)
             for i in range(0, n, chunk)]
     cols = [torch.cat(c, 0) if c[0] is not None else None for c in zip(*parts)]
     shapes = [(height, width, 3), (height, width), (height, width)] * 2

@@ -12,7 +12,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import Arch, RenderOpts
+from ._lib import Arch, RenderOpts, Rng
 
 IMPL_SIMT = 0  # fp32 CUDA cores
 IMPL_TC = 1    # wgmma tensor cores (fp16x2 three-term splits, fp32 accumulation)
@@ -123,6 +123,49 @@ class ArchSpec:
         if n < 0:
             _lib.check(_lib.ERR_UNSUPPORTED, "blob_floats")
         return n
+
+
+@dataclass(frozen=True)
+class SeededRandoms:
+    """The render path's random inputs generated in-kernel from a counter-based stream (include/nerfb200.h,
+    ``nerfb200_rng_t``): every number is a pure function of (seed, step, stream, global ray index, sample), so a ray gets
+    the same numbers however the batch is chunked or sharded.  ``ray_offset`` is the global index of the first ray
+    passed; give each optimisation step its own ``step`` (< 2^30)."""
+
+    seed: int
+    step: int = 0
+    ray_offset: int = 0
+
+    def __post_init__(self):
+        if not 0 <= int(self.seed) < 2 ** 64:
+            raise ValueError("SeededRandoms: seed must be in [0, 2^64)")
+        if not 0 <= int(self.step) < 2 ** 30:
+            raise ValueError("SeededRandoms: step must be in [0, 2^30)")
+        if int(self.ray_offset) < 0:
+            raise ValueError("SeededRandoms: ray_offset must be >= 0")
+
+    def shifted(self, n_rays: int) -> "SeededRandoms":
+        """The same stream for the rays that start ``n_rays`` further on (a later chunk or shard)."""
+        return SeededRandoms(self.seed, self.step, self.ray_offset + int(n_rays))
+
+    def c_struct(self) -> Rng:
+        return Rng(int(self.seed), int(self.step), int(self.ray_offset))
+
+
+RAND_STREAMS = {"t_rand": 0, "noise_c": 1, "u": 2, "noise_f": 3}
+
+
+def random_fill(rng: SeededRandoms, stream, n_rays: int, per_ray: int, device=None) -> torch.Tensor:
+    """Stream ``stream`` (a name of RAND_STREAMS or its id) of ``rng`` for ``n_rays`` rays from ``rng.ray_offset`` on:
+    (n_rays, per_ray) fp32, uniforms in [0, 1) for t_rand / u, unit normals for noise_c / noise_f.  These are exactly
+    the numbers the seeded render kernels consume."""
+    lib = _lib.load()
+    sid = RAND_STREAMS[stream] if isinstance(stream, str) else int(stream)
+    out = torch.empty(int(n_rays), int(per_ray), dtype=torch.float32,
+                      device=device if device is not None else torch.cuda.current_device())
+    _lib.check(lib.nerfb200_random_fill(C.byref(rng.c_struct()), sid, int(n_rays), int(per_ray), _ptr(out), _stream()),
+               "random_fill")
+    return out
 
 
 def make_opts(n_coarse, n_fine, perturb, lindisp, white_bkgd, noise_std) -> RenderOpts:
@@ -359,6 +402,42 @@ def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, t_vals, t
                                        _ptr(noise_f) if fine else None, _ptr(out_c), _ptr(out_f), _ptr(workspace),
                                        int(training), impl, _stream()), "render_fwd")
     return out_c, out_f, workspace
+
+
+def render_fwd_seeded(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, t_vals, rng: SeededRandoms,
+                      training: bool, impl: int = IMPL_SIMT, workspace: Optional[torch.Tensor] = None):
+    """``render_fwd`` with the random inputs generated in-kernel from ``rng`` (no random tensors)."""
+    lib = _lib.load()
+    n = rays.shape[0]
+    dev = rays.device
+    fine = opts.n_fine > 0
+    need = render_workspace_bytes(arch_c, arch_f if fine else None, opts, n, training)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
+    ac = arch_c.c_struct()
+    af = arch_f.c_struct() if fine else None
+    _lib.check(lib.nerfb200_render_fwd_seeded(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
+                                              _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
+                                              _ptr(t_vals), C.byref(rng.c_struct()), _ptr(out_c), _ptr(out_f),
+                                              _ptr(workspace), int(training), impl, _stream()), "render_fwd_seeded")
+    return out_c, out_f, workspace
+
+
+def render_bwd_seeded(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, rng: SeededRandoms, g_c, g_f, workspace,
+                      flat_grad_c, flat_grad_f, impl: int = IMPL_SIMT, parts: int = 3):
+    """``render_bwd`` of a ``render_fwd_seeded`` workspace: the noise is regenerated from ``rng``, not read."""
+    lib = _lib.load()
+    fine = opts.n_fine > 0
+    ac = arch_c.c_struct()
+    af = arch_f.c_struct() if fine else None
+    _lib.check(lib.nerfb200_render_bwd_seeded(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
+                                              _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
+                                              rays.shape[0], C.byref(rng.c_struct()), _ptr(g_c),
+                                              _ptr(g_f) if fine else None, _ptr(workspace), _ptr(flat_grad_c),
+                                              _ptr(flat_grad_f) if fine else None, impl, int(parts), _stream()),
+               "render_bwd_seeded")
 
 
 def render_bwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, noise_c, noise_f, g_c, g_f, workspace,

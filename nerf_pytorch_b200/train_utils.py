@@ -8,18 +8,20 @@ same 6-tuple result, differentiable w.r.t. the parameters of both models.  Every
 (stratified sampling, encoding, both MLPs, compositing, hierarchical resampling, their backward)
 runs in libnerfb200.so; this file only moves pointers: it reads the options, draws the random
 tensors in the reference's order (so a shared torch seed gives the reference-on-GPU's random
-stream), flattens the parameters and calls the C ABI through ``ops``.
+stream) or hands the kernels a seed instead (``ops.SeededRandoms``), flattens the parameters and
+calls the C ABI through ``ops``.
 
 There is no PyTorch fallback: an unsupported model / device / dtype raises.
 """
 from __future__ import annotations
 
 import weakref
-from typing import Optional
+from typing import Optional, Union
 
 import torch
 
 from . import ops
+from .ops import SeededRandoms
 from .nerf_helpers import Embedder, get_minibatches
 
 # The reference does not forward ``mode`` to predict_and_render_radiance (train_utils.py:171-181),
@@ -208,13 +210,21 @@ def _packed(model, arch: ops.ArchSpec):
 class _RenderChunk(torch.autograd.Function):
     @staticmethod
     def forward(ctx, cfg, rays, t_vals, t_rand, noise_c, u, noise_f, *params):
-        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks = cfg
-        out_c, out_f, ws = ops.render_fwd(arch_c, arch_f, opts, blob_c, blob_f, rays, t_vals, t_rand, noise_c, u,
-                                          noise_f, training=training, impl=impl)
+        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks, rng = cfg
+        if rng is None:
+            out_c, out_f, ws = ops.render_fwd(arch_c, arch_f, opts, blob_c, blob_f, rays, t_vals, t_rand, noise_c, u,
+                                              noise_f, training=training, impl=impl)
+        else:
+            out_c, out_f, ws = ops.render_fwd_seeded(arch_c, arch_f, opts, blob_c, blob_f, rays, t_vals, rng,
+                                                     training=training, impl=impl)
         if training:
             ctx.cfg = cfg
             ctx.ws = ws
-            ctx.save_for_backward(rays, noise_c, noise_f)
+            # seeded: the backward regenerates the noise in-kernel, so no noise tensor is kept
+            if rng is None:
+                ctx.save_for_backward(rays, noise_c, noise_f)
+            else:
+                ctx.save_for_backward(rays)
         ctx.set_materialize_grads(False)
         if out_f is None:
             return out_c, None
@@ -222,8 +232,8 @@ class _RenderChunk(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_c, g_f):
-        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks = ctx.cfg
-        rays, noise_c, noise_f = ctx.saved_tensors
+        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks, rng = ctx.cfg
+        rays = ctx.saved_tensors[0]
         fine = opts.n_fine > 0
         n = rays.shape[0]
         if g_c is None:
@@ -235,8 +245,12 @@ class _RenderChunk(torch.autograd.Function):
         flat_grad = torch.zeros(nc + nf, dtype=torch.float32, device=rays.device)
         g_c = g_c.contiguous()
         g_f = g_f.contiguous() if fine else None
-        args = (arch_c, arch_f, opts, blob_c, blob_f, rays, noise_c, noise_f, g_c, g_f, ctx.ws, flat_grad[:nc],
-                flat_grad[nc:] if fine else None)
+        grad_out = (g_c, g_f, ctx.ws, flat_grad[:nc], flat_grad[nc:] if fine else None)
+        if rng is None:
+            noise_c, noise_f = ctx.saved_tensors[1:]
+            bwd, args = ops.render_bwd, (arch_c, arch_f, opts, blob_c, blob_f, rays, noise_c, noise_f) + grad_out
+        else:
+            bwd, args = ops.render_bwd_seeded, (arch_c, arch_f, opts, blob_c, blob_f, rays, rng) + grad_out
         sync = _GRAD_SYNC
         if sync is not None and n_chunks != 1:
             # several chunks per step: no collective here (ranks may even differ in their chunk counts); the summed
@@ -245,7 +259,7 @@ class _RenderChunk(torch.autograd.Function):
             _PENDING_SYNC = True
             sync = None
         if sync is None:
-            ops.render_bwd(*args, impl=impl)
+            bwd(*args, impl=impl)
         else:
             # the ONE collective of a data-parallel step, split in two so that the fine network's half (final as soon
             # as its backward is done) crosses NVLink while the coarse network's backward is still running
@@ -254,9 +268,9 @@ class _RenderChunk(torch.autograd.Function):
             group, world = sync
             works = []
             if fine:
-                ops.render_bwd(*args, impl=impl, parts=1)
+                bwd(*args, impl=impl, parts=1)
                 works.append(dist.all_reduce(flat_grad[nc:], op=dist.ReduceOp.SUM, group=group, async_op=True))
-            ops.render_bwd(*args, impl=impl, parts=2 if fine else 3)
+            bwd(*args, impl=impl, parts=2 if fine else 3)
             works.append(dist.all_reduce(flat_grad[:nc], op=dist.ReduceOp.SUM, group=group, async_op=True))
             for w in works:
                 w.wait()
@@ -282,7 +296,7 @@ def predict_and_render_radiance(
     encode_position_fn=None,
     encode_direction_fn=None,
     *,
-    randoms: Optional[dict] = None,
+    randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
     _n_chunks: int = 1,
 ):
@@ -290,7 +304,8 @@ def predict_and_render_radiance(
 
     ``randoms`` (keyword-only, optional) injects the four random tensors the reference would draw
     (t_rand, noise_c, u, noise_f); by default they are drawn here with torch.rand/randn in the
-    reference's order."""
+    reference's order.  A ``SeededRandoms`` instead has the kernels generate them from its seed, step and
+    ``ray_offset`` (the global index of ``ray_batch[0]``): no torch random number is drawn."""
     o = getattr(options.nerf, mode)
     if not ray_batch.is_cuda:
         raise NotImplementedError("nerfb200: rays must be on a CUDA device (there is no CPU path)")
@@ -312,7 +327,8 @@ def predict_and_render_radiance(
     perturb = bool(o.perturb)
     opts = ops.make_opts(nc, nf, perturb, o.lindisp, o.white_background, noise_std)
 
-    rnd = randoms or {}
+    rng = randoms if isinstance(randoms, SeededRandoms) else None
+    rnd = randoms if isinstance(randoms, dict) else {}
 
     def take(name, shape, fn):
         t = rnd.get(name)
@@ -322,15 +338,16 @@ def predict_and_render_radiance(
 
     # reference draw order: rand(N,Nc) -> randn(N,Nc) -> rand(N,Nf) -> randn(N,Nc+Nf)  (SURVEY section 5)
     t_vals = torch.linspace(0.0, 1.0, nc, dtype=torch.float32, device=dev)
-    t_rand = take("t_rand", (n, nc), torch.rand) if perturb else None
-    noise_c = take("noise_c", (n, nc), torch.randn) if noise_std > 0.0 else None
-    u = noise_f = None
-    if fine:
-        if perturb:
-            u = take("u", (n, nf), torch.rand)
-        else:  # det = (perturb == 0.0): shared linspace, nerf_helpers.py:272-276
-            u = torch.linspace(0.0, 1.0, steps=nf, dtype=torch.float32, device=dev)
-        noise_f = take("noise_f", (n, nc + nf), torch.randn) if noise_std > 0.0 else None
+    t_rand = noise_c = u = noise_f = None
+    if rng is None:  # seeded: the kernels generate all four (and the det=True u when perturb is off)
+        t_rand = take("t_rand", (n, nc), torch.rand) if perturb else None
+        noise_c = take("noise_c", (n, nc), torch.randn) if noise_std > 0.0 else None
+        if fine:
+            if perturb:
+                u = take("u", (n, nf), torch.rand)
+            else:  # det = (perturb == 0.0): shared linspace, nerf_helpers.py:272-276
+                u = torch.linspace(0.0, 1.0, steps=nf, dtype=torch.float32, device=dev)
+            noise_f = take("noise_f", (n, nc + nf), torch.randn) if noise_std > 0.0 else None
 
     all_params = list(params_c) + list(params_f)
     training = torch.is_grad_enabled() and any(p.requires_grad for p in all_params)
@@ -338,7 +355,7 @@ def predict_and_render_radiance(
         impl = DEFAULT_IMPL
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, int(impl), int(_n_chunks))
+    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, int(impl), int(_n_chunks), rng)
     out_c, out_f = _RenderChunk.apply(cfg, rays, t_vals, t_rand, noise_c, u, noise_f, *all_params)
     rgb_c, disp_c, acc_c = out_c[:, :3], out_c[:, 3], out_c[:, 4]
     if out_f is None:
@@ -359,7 +376,7 @@ def run_one_iter_of_nerf(
     encode_position_fn=None,
     encode_direction_fn=None,
     *,
-    randoms: Optional[dict] = None,
+    randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
 ):
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
@@ -394,7 +411,7 @@ def run_one_iter_of_nerf_from_pose(
     encode_position_fn=None,
     encode_direction_fn=None,
     *,
-    randoms: Optional[dict] = None,
+    randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
 ):
     """``run_one_iter_of_nerf`` for callers that hold a pose and pixel ids instead of ray tensors (SURVEY.md section 8f-2):
@@ -414,9 +431,12 @@ def run_one_iter_of_nerf_from_pose(
 
 def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn, encode_direction_fn,
                    randoms, impl):
-    """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202."""
-    batches = get_minibatches(rays, chunksize=getattr(options.nerf, mode).chunksize)
-    if randoms is not None and len(batches) != 1:
+    """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202.
+    Seeded randoms follow each ray: chunk i starts at ``ray_offset`` + the index of its first ray."""
+    chunksize = getattr(options.nerf, mode).chunksize
+    batches = get_minibatches(rays, chunksize=chunksize)
+    seeded = isinstance(randoms, SeededRandoms)
+    if randoms is not None and not seeded and len(batches) != 1:
         raise ValueError("injected randoms require a single ray chunk")
     inner_mode = "train" if COMPAT_MODE_QUIRK else mode
     pred = [
@@ -424,9 +444,9 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             batch, model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if options.nerf.use_viewdirs else None,
-            randoms=randoms, impl=impl, _n_chunks=len(batches),
+            randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, _n_chunks=len(batches),
         )
-        for batch in batches
+        for i, batch in enumerate(batches)
     ]
     synthesized_images = list(zip(*pred))
     synthesized_images = [
