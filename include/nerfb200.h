@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define NERFB200_VERSION 100 /* 0.1.0 */
+#define NERFB200_VERSION 101 /* 0.1.1 */
 
 #define NERFB200_OK 0
 #define NERFB200_ERR_INVALID (-1)     /* bad argument (null pointer, size <= 0, ...) */
@@ -93,11 +93,10 @@ int32_t nerfb200_pack_weights(const nerfb200_arch_t* arch, const float* flat, fl
 /* ---- stage-level entry points (each is also a test hook; SURVEY.md section 8b) ------------------ */
 
 /* Stratified depths, train_utils.py:45-65.  rays[n_rays][ray_stride] = [o(3) d(3) near far (viewdir(3))];
- * t_vals[n_coarse] = torch.linspace(0,1,n_coarse); t_rand[n_rays][n_coarse] uniform [0,1) or NULL
- * when !perturb.  Writes z[n_rays][n_coarse]. */
-int32_t nerfb200_sample_coarse(const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                               const float* t_rand, int32_t n_coarse, int32_t perturb, int32_t lindisp,
-                               float* z, void* stream);
+ * t_rand[n_rays][n_coarse] uniform [0,1) or NULL when !perturb.  The grid t = torch.linspace(0,1,n_coarse) is
+ * computed in the kernel, bit for bit as torch's CUDA linspace computes it.  Writes z[n_rays][n_coarse]. */
+int32_t nerfb200_sample_coarse(const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_rand,
+                               int32_t n_coarse, int32_t perturb, int32_t lindisp, float* z, void* stream);
 
 /* Ray generation / packing in one launch (SURVEY.md section 8f-2).  Output rows of `out_stride` floats:
  *   11: [o(3) d(3) near far viewdir(3)]  (train_utils.py:164-168, use_viewdirs)   8: without the view direction
@@ -148,15 +147,14 @@ int32_t nerfb200_composite_bwd(const float* raw, const float* z, const float* ra
 
 /* sample_pdf_2 (nerf_helpers.py:260-302) + detach/cat/sort (train_utils.py:96-105):
  * bins = mid-points of z_coarse, weights_coarse[...,1:-1] + 1e-5 -> pdf -> cdf (63 entries for 64
- * coarse samples) -> inverse-CDF samples at u[n_rays][n_fine] (u_stride = n_fine) or at a shared
- * u[n_fine] (u_stride = 0: the det=True linspace) -> z_fine[n_rays][n_coarse+n_fine] ascending.
+ * coarse samples) -> inverse-CDF samples at u[n_rays][n_fine], or, u = NULL, at the det=True
+ * torch.linspace(0,1,n_fine) computed in the kernel -> z_fine[n_rays][n_coarse+n_fine] ascending.
  * Optional outputs (NULL to skip): z_samples[n_rays][n_fine] (unsorted), inds int32 [n_rays][n_fine]
  * (searchsorted(cdf, u, right) result), cdf_out[n_rays][n_coarse-1].
  * cdf_in (optional): use this cdf instead of computing it ("bit-exact indices given the same cdf"). */
 int32_t nerfb200_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const float* u,
-                                  int32_t u_stride, const float* cdf_in, int64_t n_rays, int32_t n_coarse,
-                                  int32_t n_fine, float* z_fine, float* z_samples, int32_t* inds,
-                                  float* cdf_out, void* stream);
+                                  const float* cdf_in, int64_t n_rays, int32_t n_coarse, int32_t n_fine,
+                                  float* z_fine, float* z_samples, int32_t* inds, float* cdf_out, void* stream);
 
 /* Backward of nerfb200_mlp_fwd w.r.t. the parameters.  d_raw[n_points][4]; stash from the forward (same impl).
  * gstash: scratch fp32[nerfb200_bwd_scratch_floats(arch, n_points, impl)] (impl 0: the per-layer gradient stash;
@@ -189,34 +187,16 @@ int32_t nerfb200_render_workspace_layout(const nerfb200_arch_t* coarse, const ne
                                          const nerfb200_render_opts_t* opts, int64_t n_rays, int32_t training,
                                          int64_t* offsets9);
 
-/* predict_and_render_radiance for one ray chunk (train_utils.py:28-127).
- * Randoms follow the reference's draw order (SURVEY.md section 5): t_rand[n][nc] (perturb),
- * noise_c[n][nc] (noise_std>0), u[n][nf] (perturb; else the host passes linspace with u_stride 0),
- * noise_f[n][nc+nf].  t_vals[nc] = linspace(0,1,nc).
- * out_coarse/out_fine[n][8] = [r g b disp acc depth 0 0] (out_fine NULL when n_fine == 0).
- * workspace: nerfb200_render_workspace_bytes(...) bytes; keeps z/raw/stash for render_bwd. */
-int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                            const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                            const float* t_rand, const float* noise_c, const float* u, int32_t u_stride,
-                            const float* noise_f, float* out_coarse, float* out_fine, void* workspace,
-                            int32_t training, int32_t impl, void* stream);
-
-/* Backward of render_fwd: g_coarse/g_fine[n][8] upstream grads (g_fine NULL when no fine pass);
- * accumulates into flat_grad_c / flat_grad_f (may alias different ranges of one buffer).
- * parts: bit 0 = the fine network's backward, bit 1 = the coarse network's (3 = both, fine first).  Two calls (1, then
- * 2) let the host start the all-reduce of the fine network's gradient while the coarse backward runs. */
-int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                            const float* rays, int32_t ray_stride, int64_t n_rays, const float* noise_c,
-                            const float* noise_f, const float* g_coarse, const float* g_fine,
-                            void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl,
-                            int32_t parts, void* stream);
-
-/* ---- seeded random numbers ----------------------------------------------------------------------
- * The render path's four random inputs as a pure function of (seed, step, stream, global ray, sample), generated
- * inside the kernels that use them: Philox4x32-10 keyed by the seed, counter (sample / 4, stream + 4 * step, global
- * ray low 32 bits, high 32 bits); streams 0 t_rand, 1 noise_c, 2 u, 3 noise_f.  Uniforms are (w >> 8) * 2^-24 in
+/* ---- random numbers of the render path ---------------------------------------------------------
+ * predict_and_render_radiance has four random inputs, in the reference's draw order (SURVEY.md section 5):
+ *   stream 0 t_rand [n][nc]     uniform [0, 1), used when perturb is set
+ *   stream 1 noise_c[n][nc]     unit normal,    used when noise_std > 0
+ *   stream 2 u      [n][nf]     uniform [0, 1), used when perturb is set and n_fine > 0
+ *   stream 3 noise_f[n][nc+nf]  unit normal,    used when noise_std > 0 and n_fine > 0
+ * With perturb off the fine pass resamples at the det=True torch.linspace(0,1,nf), computed in the kernel.
+ * Each input comes from a tensor the caller drew, or from the seeded stream: a pure function of (seed, step, stream,
+ * global ray, sample), generated inside the kernels that use it.  That stream is Philox4x32-10 keyed by the seed,
+ * counter (sample / 4, stream + 4 * step, global ray low 32 bits, high 32 bits).  Uniforms are (w >> 8) * 2^-24 in
  * [0, 1); normals are Box-Muller on word pairs with u1 = ((w >> 8) + 1) * 2^-24 (the exact definition is in
  * csrc/common.cuh).  A ray's numbers do not depend on how the batch is chunked or sharded. */
 typedef struct nerfb200_rng {
@@ -225,25 +205,35 @@ typedef struct nerfb200_rng {
   int64_t ray_offset; /* global index of the call's first ray (>= 0) */
 } nerfb200_rng_t;
 
-/* render_fwd / render_bwd with the random tensors generated in-kernel from *rng (stream ids as above).  With perturb
- * off the fine pass's u is the det=True linspace, as in render_fwd.  render_bwd_seeded regenerates the noise for the
- * sigma ReLU gate and reads no noise tensor; pass it the same *rng as the render_fwd_seeded call that filled the
- * workspace. */
-int32_t nerfb200_render_fwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                                   const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                                   const nerfb200_rng_t* rng, float* out_coarse, float* out_fine, void* workspace,
-                                   int32_t training, int32_t impl, void* stream);
-int32_t nerfb200_render_bwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                                   const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                                   const float* g_coarse, const float* g_fine, void* workspace, float* flat_grad_c,
-                                   float* flat_grad_f, int32_t impl, int32_t parts, void* stream);
 /* Materialises stream `stream_id` (0..3) for rays ray_offset .. ray_offset + n_rays - 1, samples 0 .. per_ray - 1:
  * out[n_rays][per_ray], uniforms for streams 0 and 2, unit normals for 1 and 3.  The numbers the render kernels use,
- * through the same device function: what render_fwd_seeded consumes equals render_fwd fed these tensors. */
+ * through the same device function: a render call given *rng equals one given these tensors. */
 int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64_t n_rays, int32_t per_ray, float* out,
                              void* stream);
+
+/* predict_and_render_radiance for one ray chunk (train_utils.py:28-127), and its backward.
+ * Random inputs (streams above): rng non-NULL generates every one in-kernel, and then every random tensor pointer
+ * must be NULL.  rng NULL reads the tensors t_rand, noise_c, u, noise_f, each only when the options use it: t_rand and
+ * u must then be given, a noise tensor left NULL means no noise.  render_bwd needs the noise again for the sigma ReLU gate: pass it the same *rng,
+ * or the same noise tensors, as the render_fwd call that filled the workspace (seeded, it reads no noise tensor).
+ * render_fwd: out_coarse/out_fine[n][8] = [r g b disp acc depth 0 0] (out_fine NULL when n_fine == 0).
+ *   workspace: nerfb200_render_workspace_bytes(...) bytes; keeps z/raw/stash for render_bwd.
+ * render_bwd: g_coarse/g_fine[n][8] upstream grads (g_fine NULL when no fine pass); accumulates into flat_grad_c /
+ *   flat_grad_f (may alias different ranges of one buffer).  parts: bit 0 = the fine network's backward, bit 1 = the
+ *   coarse network's (3 = both, fine first).  Two calls (1, then 2) let the host start the all-reduce of the fine
+ *   network's gradient while the coarse backward runs. */
+int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                            const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                            float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
+                            void* stream);
+int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                            const float* noise_c, const float* noise_f, const float* g_coarse, const float* g_fine,
+                            void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
+                            void* stream);
 
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale

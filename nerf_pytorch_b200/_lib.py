@@ -72,7 +72,7 @@ SIGNATURES = {
     "nerfb200_blob_floats": (I64, [AP]),
     "nerfb200_flat_layout": (I32, [AP, I32, C.POINTER(I64), C.POINTER(I64), C.POINTER(I32), C.POINTER(I32)]),
     "nerfb200_pack_weights": (I32, [AP, P, P, P]),
-    "nerfb200_sample_coarse": (I32, [P, I32, I64, P, P, I32, I32, I32, P, P]),
+    "nerfb200_sample_coarse": (I32, [P, I32, I64, P, I32, I32, I32, P, P]),
     "nerfb200_gen_rays": (I32, [C.POINTER(F32), I32, I32, F32, P, I64, I32, F32, F32, I32, I32, P, P]),
     "nerfb200_pack_rays": (I32, [P, P, I64, I32, I32, F32, I32, F32, F32, I32, I32, P, P]),
     "nerfb200_encode": (I32, [AP, I32, P, I64, P, P]),
@@ -80,17 +80,15 @@ SIGNATURES = {
     "nerfb200_mlp_fwd": (I32, [AP, P, P, I32, P, I64, I32, P, P, I32, P]),
     "nerfb200_composite_fwd": (I32, [P, P, P, I32, P, I64, I32, F32, I32, P, P, P]),
     "nerfb200_composite_bwd": (I32, [P, P, P, I32, P, P, I64, I32, F32, I32, P, P]),
-    "nerfb200_sample_pdf_merge": (I32, [P, P, P, I32, P, I64, I32, I32, P, P, P, P, P]),
+    "nerfb200_sample_pdf_merge": (I32, [P, P, P, P, I64, I32, I32, P, P, P, P, P]),
     "nerfb200_bwd_scratch_floats": (I64, [AP, I64, I32]),
     "nerfb200_mlp_bwd": (I32, [AP, P, P, I32, P, I64, I32, P, P, P, P, I32, P]),
     "nerfb200_mlp_dgrad": (I32, [AP, P, P, P, P, I64, I32, P]),
     "nerfb200_mlp_wgrad": (I32, [AP, P, I32, P, I64, I32, P, P, P, P, I32, P]),
     "nerfb200_render_workspace_bytes": (I64, [AP, AP, OP, I64, I32]),
     "nerfb200_render_workspace_layout": (I32, [AP, AP, OP, I64, I32, C.POINTER(I64)]),
-    "nerfb200_render_fwd": (I32, [AP, AP, OP, P, P, P, I32, I64, P, P, P, P, I32, P, P, P, P, I32, I32, P]),
-    "nerfb200_render_bwd": (I32, [AP, AP, OP, P, P, P, I32, I64, P, P, P, P, P, P, P, I32, I32, P]),
-    "nerfb200_render_fwd_seeded": (I32, [AP, AP, OP, P, P, P, I32, I64, P, RP, P, P, P, I32, I32, P]),
-    "nerfb200_render_bwd_seeded": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, I32, I32, P]),
+    "nerfb200_render_fwd": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, P, P, I32, I32, P]),
+    "nerfb200_render_bwd": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, P, P, I32, I32, P]),
     "nerfb200_random_fill": (I32, [RP, I32, I64, I32, P, P]),
     "nerfb200_adam_step": (I32, [P, P, P, P, I64, I32, F32, F32, F32, F32, F32, P]),
 }

@@ -349,15 +349,14 @@ int32_t nerfb200_pack_weights(const nerfb200_arch_t* arch, const float* flat, fl
   return launch_pack(p, flat, blob, static_cast<cudaStream_t>(stream));
 }
 
-int32_t nerfb200_sample_coarse(const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                               const float* t_rand, int32_t n_coarse, int32_t perturb, int32_t lindisp,
-                               float* z, void* stream) {
-  if (!rays || !t_vals || !z || n_rays <= 0 || n_coarse < 2 || ray_stride < 8 || (perturb && !t_rand)) {
+int32_t nerfb200_sample_coarse(const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_rand,
+                               int32_t n_coarse, int32_t perturb, int32_t lindisp, float* z, void* stream) {
+  if (!rays || !z || n_rays <= 0 || n_coarse < 2 || ray_stride < 8 || (perturb && !t_rand)) {
     set_error("sample_coarse: invalid argument");
     return NERFB200_ERR_INVALID;
   }
-  return launch_sample_coarse(rays, ray_stride, n_rays, t_vals, perturb ? rand_tensor(t_rand, n_coarse) : rand_none(),
-                              n_coarse, perturb, lindisp, z, static_cast<cudaStream_t>(stream));
+  return launch_sample_coarse(rays, ray_stride, n_rays, perturb ? rand_tensor(t_rand, n_coarse) : rand_none(), n_coarse,
+                              perturb, lindisp, z, static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_gen_rays(const float* c2w12_host, int32_t height, int32_t width, float focal, const int64_t* pixel_ids,
@@ -489,15 +488,15 @@ int32_t nerfb200_composite_bwd(const float* raw, const float* z, const float* ra
 }
 
 int32_t nerfb200_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const float* u,
-                                  int32_t u_stride, const float* cdf_in, int64_t n_rays, int32_t n_coarse,
-                                  int32_t n_fine, float* z_fine, float* z_samples, int32_t* inds,
-                                  float* cdf_out, void* stream) {
-  if (!z_coarse || (!weights_coarse && !cdf_in) || !u || n_rays <= 0 || n_coarse < 4 || n_fine <= 0 ||
-      n_coarse + n_fine > 1024 || (u_stride != 0 && u_stride != n_fine)) {
+                                  const float* cdf_in, int64_t n_rays, int32_t n_coarse, int32_t n_fine,
+                                  float* z_fine, float* z_samples, int32_t* inds, float* cdf_out, void* stream) {
+  if (!z_coarse || (!weights_coarse && !cdf_in) || n_rays <= 0 || n_coarse < 4 || n_fine <= 0 ||
+      n_coarse + n_fine > 1024) {
     set_error("sample_pdf_merge: invalid argument");
     return NERFB200_ERR_INVALID;
   }
-  return launch_sample_pdf_merge(z_coarse, weights_coarse, rand_tensor(u, u_stride), cdf_in, n_rays, n_coarse, n_fine,
+  // u NULL: no source, so the kernel resamples at the det=True linspace
+  return launch_sample_pdf_merge(z_coarse, weights_coarse, rand_tensor(u, n_fine), cdf_in, n_rays, n_coarse, n_fine,
                                  z_fine, z_samples, inds, cdf_out, static_cast<cudaStream_t>(stream));
 }
 
@@ -536,113 +535,6 @@ int32_t nerfb200_render_workspace_layout(const nerfb200_arch_t* coarse, const ne
 
 namespace nerfb200 {
 
-// The four random inputs of one render call: rnd[kRandTRand], rnd[kRandNoiseC], rnd[kRandU], rnd[kRandNoiseF].
-// det_u: the fine pass's u is the det=True linspace, built in the resampling kernel (rnd[kRandU] is then unused).
-static int render_fwd_impl(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                           const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                           const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                           const RandSrc* rnd, bool det_u, float* out_coarse, float* out_fine, void* workspace, int32_t training,
-                           int32_t impl, cudaStream_t s) {
-  Plan pc, pf;
-  NB_TRY(build_plan(arch_c, &pc));
-  NB_TRY(check_opts(opts));
-  const bool fine = opts->n_fine > 0;
-  if (fine) {
-    if (!arch_f || !blob_f || !out_fine || (!det_u && !rnd[kRandU].present())) {
-      set_error("render_fwd: fine pass requested but fine model / output / u missing");
-      return NERFB200_ERR_INVALID;
-    }
-    NB_TRY(build_plan(arch_f, &pf));
-  }
-  if (!rays || !t_vals || !out_coarse || !workspace || !blob_c || n_rays <= 0) {
-    set_error("render_fwd: null pointer or empty batch");
-    return NERFB200_ERR_INVALID;
-  }
-  if (opts->perturb && !rnd[kRandTRand].present()) {
-    set_error("render_fwd: perturb set but t_rand missing");
-    return NERFB200_ERR_INVALID;
-  }
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
-  char* base = static_cast<char*>(workspace);
-  auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  const RandSrc none = rand_none();
-
-  // coarse pass: stratified depths -> MLP -> compositing (train_utils.py:45-94)
-  NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, t_vals, opts->perturb ? rnd[kRandTRand] : none, nc,
-                              opts->perturb, opts->lindisp, F(w.z_c), s));
-  float* stash_c = training ? F(w.stash_c) : nullptr;
-  NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
-  if (impl == 1)
-    NB_TRY(launch_mlp_fwd_tc(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
-  else
-    NB_TRY(launch_mlp_fwd_simt(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
-  NB_TRY(launch_composite_fwd(F(w.raw_c), F(w.z_c), rays, ray_stride, opts->noise_std > 0.f ? rnd[kRandNoiseC] : none,
-                              n_rays, nc, opts->noise_std, opts->white_bkgd, out_coarse, F(w.w_c), s));
-  if (!fine) return NERFB200_OK;
-
-  // hierarchical resampling + merge (train_utils.py:96-105), fine pass (:107-125)
-  NB_TRY(launch_sample_pdf_merge(F(w.z_c), F(w.w_c), det_u ? none : rnd[kRandU], nullptr, n_rays, nc, opts->n_fine, F(w.z_f),
-                                 nullptr, nullptr, nullptr, s));
-  float* stash_f = training ? F(w.stash_f) : nullptr;
-  NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
-  if (impl == 1)
-    NB_TRY(launch_mlp_fwd_tc(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
-  else
-    NB_TRY(launch_mlp_fwd_simt(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
-  NB_TRY(launch_composite_fwd(F(w.raw_f), F(w.z_f), rays, ray_stride, opts->noise_std > 0.f ? rnd[kRandNoiseF] : none,
-                              n_rays, ns, opts->noise_std, opts->white_bkgd, out_fine, nullptr, s));
-  return NERFB200_OK;
-}
-
-static int render_bwd_impl(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                           const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                           const float* rays, int32_t ray_stride, int64_t n_rays, const RandSrc& noise_c,
-                           const RandSrc& noise_f, const float* g_coarse, const float* g_fine, void* workspace,
-                           float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts, cudaStream_t s) {
-  Plan pc, pf;
-  NB_TRY(build_plan(arch_c, &pc));
-  NB_TRY(check_opts(opts));
-  const bool fine = opts->n_fine > 0;
-  if (fine) {
-    if (!arch_f || !blob_f || !g_fine || !flat_grad_f) {
-      set_error("render_bwd: fine pass present but fine model / grads missing");
-      return NERFB200_ERR_INVALID;
-    }
-    NB_TRY(build_plan(arch_f, &pf));
-  }
-  if (!rays || !g_coarse || !workspace || !blob_c || !flat_grad_c || n_rays <= 0) {
-    set_error("render_bwd: null pointer or empty batch");
-    return NERFB200_ERR_INVALID;
-  }
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/1, &w);
-  char* base = static_cast<char*>(workspace);
-  auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  const RandSrc none = rand_none();
-
-  if ((parts & 3) == 0) {
-    set_error("render_bwd: parts must select the fine (1) and / or the coarse (2) backward");
-    return NERFB200_ERR_INVALID;
-  }
-  if (fine && (parts & 1)) {
-    NB_TRY(launch_composite_bwd(F(w.raw_f), F(w.z_f), rays, ray_stride, opts->noise_std > 0.f ? noise_f : none,
-                                g_fine, n_rays, ns, opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
-    NB_TRY(launch_mlp_bwd(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.d_raw), F(w.stash_f), F(w.gstash),
-                          flat_grad_f, impl, s));
-  }
-  if (!(parts & 2)) return NERFB200_OK;
-  // the coarse weights feed the resampler only through a detach (train_utils.py:103), so the
-  // coarse net's gradient comes from rgb/disp/acc_coarse alone.
-  NB_TRY(launch_composite_bwd(F(w.raw_c), F(w.z_c), rays, ray_stride, opts->noise_std > 0.f ? noise_c : none,
-                              g_coarse, n_rays, nc, opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
-  NB_TRY(launch_mlp_bwd(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.d_raw), F(w.stash_c), F(w.gstash),
-                        flat_grad_c, impl, s));
-  return NERFB200_OK;
-}
-
 static int check_rng(const nerfb200_rng_t* rng, const char* what) {
   if (!rng) {
     set_error("%s: null rng", what);
@@ -656,60 +548,141 @@ static int check_rng(const nerfb200_rng_t* rng, const char* what) {
   return NERFB200_OK;
 }
 
+// The four random inputs of one render call, rnd[kRandTRand], rnd[kRandNoiseC], rnd[kRandU], rnd[kRandNoiseF]: the
+// seeded stream when rng is set, else the tensors.  An input the options do not use gets no source, so with perturb off
+// the resampling kernel builds the det=True linspace for u.
+static int render_randoms(const char* what, const nerfb200_render_opts_t& o, const nerfb200_rng_t* rng,
+                          const float* const tensor[4], RandSrc rnd[4]) {
+  if (rng) {
+    NB_TRY(check_rng(rng, what));
+    for (int s = 0; s < 4; ++s)
+      if (tensor[s]) {
+        set_error("%s: both an rng and a random tensor (stream %d) given", what, s);
+        return NERFB200_ERR_INVALID;
+      }
+  }
+  const bool fine = o.n_fine > 0, noise = o.noise_std > 0.f;
+  const bool used[4] = {o.perturb != 0, noise, o.perturb && fine, noise && fine};
+  const int64_t per_ray[4] = {o.n_coarse, o.n_coarse, o.n_fine, o.n_coarse + o.n_fine};
+  for (int s = 0; s < 4; ++s)
+    rnd[s] = !used[s] ? rand_none() : rng ? rand_seeded(*rng, s) : rand_tensor(tensor[s], per_ray[s]);
+  return NERFB200_OK;
+}
+
 }  // namespace nerfb200
 
 extern "C" {
 
 int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
                             const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                            const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                            const float* t_rand, const float* noise_c, const float* u, int32_t u_stride,
-                            const float* noise_f, float* out_coarse, float* out_fine, void* workspace,
-                            int32_t training, int32_t impl, void* stream) {
-  if (!opts) return check_opts(opts);
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  const RandSrc rnd[4] = {t_rand ? rand_tensor(t_rand, nc) : rand_none(), noise_c ? rand_tensor(noise_c, nc) : rand_none(),
-                          u ? rand_tensor(u, u_stride) : rand_none(), noise_f ? rand_tensor(noise_f, ns) : rand_none()};
-  return render_fwd_impl(arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, t_vals, rnd, /*det_u=*/false,
-                         out_coarse, out_fine, workspace, training, impl, static_cast<cudaStream_t>(stream));
-}
-
-int32_t nerfb200_render_fwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                                   const float* rays, int32_t ray_stride, int64_t n_rays, const float* t_vals,
-                                   const nerfb200_rng_t* rng, float* out_coarse, float* out_fine, void* workspace,
-                                   int32_t training, int32_t impl, void* stream) {
-  NB_TRY(check_rng(rng, "render_fwd_seeded"));
+                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                            const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                            float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
+                            void* stream) {
+  Plan pc, pf;
+  NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
-  const RandSrc rnd[4] = {rand_seeded(*rng, kRandTRand), rand_seeded(*rng, kRandNoiseC), rand_seeded(*rng, kRandU),
-                          rand_seeded(*rng, kRandNoiseF)};
-  return render_fwd_impl(arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, t_vals, rnd,
-                         /*det_u=*/!opts->perturb, out_coarse, out_fine, workspace, training, impl,
-                         static_cast<cudaStream_t>(stream));
+  const float* const tensor[4] = {t_rand, noise_c, u, noise_f};
+  RandSrc rnd[4];
+  NB_TRY(render_randoms("render_fwd", *opts, rng, tensor, rnd));
+  const bool fine = opts->n_fine > 0;
+  if (fine) {
+    if (!arch_f || !blob_f || !out_fine) {
+      set_error("render_fwd: fine pass requested but fine model / output missing");
+      return NERFB200_ERR_INVALID;
+    }
+    NB_TRY(build_plan(arch_f, &pf));
+  }
+  if (!rays || !out_coarse || !workspace || !blob_c || n_rays <= 0) {
+    set_error("render_fwd: null pointer or empty batch");
+    return NERFB200_ERR_INVALID;
+  }
+  if (opts->perturb && (!rnd[kRandTRand].present() || (fine && !rnd[kRandU].present()))) {
+    set_error("render_fwd: perturb set but t_rand or u missing");
+    return NERFB200_ERR_INVALID;
+  }
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
+  char* base = static_cast<char*>(workspace);
+  auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
+  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+
+  // coarse pass: stratified depths -> MLP -> compositing (train_utils.py:45-94)
+  NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, F(w.z_c), s));
+  float* stash_c = training ? F(w.stash_c) : nullptr;
+  NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
+  if (impl == 1)
+    NB_TRY(launch_mlp_fwd_tc(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
+  else
+    NB_TRY(launch_mlp_fwd_simt(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
+  NB_TRY(launch_composite_fwd(F(w.raw_c), F(w.z_c), rays, ray_stride, rnd[kRandNoiseC], n_rays, nc, opts->noise_std,
+                              opts->white_bkgd, out_coarse, F(w.w_c), s));
+  if (!fine) return NERFB200_OK;
+
+  // hierarchical resampling + merge (train_utils.py:96-105), fine pass (:107-125)
+  NB_TRY(launch_sample_pdf_merge(F(w.z_c), F(w.w_c), rnd[kRandU], nullptr, n_rays, nc, opts->n_fine, F(w.z_f), nullptr,
+                                 nullptr, nullptr, s));
+  float* stash_f = training ? F(w.stash_f) : nullptr;
+  NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
+  if (impl == 1)
+    NB_TRY(launch_mlp_fwd_tc(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
+  else
+    NB_TRY(launch_mlp_fwd_simt(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
+  NB_TRY(launch_composite_fwd(F(w.raw_f), F(w.z_f), rays, ray_stride, rnd[kRandNoiseF], n_rays, ns, opts->noise_std,
+                              opts->white_bkgd, out_fine, nullptr, s));
+  return NERFB200_OK;
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
                             const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                            const float* rays, int32_t ray_stride, int64_t n_rays, const float* noise_c,
-                            const float* noise_f, const float* g_coarse, const float* g_fine, void* workspace,
-                            float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts, void* stream) {
-  if (!opts) return check_opts(opts);
+                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                            const float* noise_c, const float* noise_f, const float* g_coarse, const float* g_fine,
+                            void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
+                            void* stream) {
+  Plan pc, pf;
+  NB_TRY(build_plan(arch_c, &pc));
+  NB_TRY(check_opts(opts));
+  const float* const tensor[4] = {nullptr, noise_c, nullptr, noise_f};
+  RandSrc rnd[4];
+  NB_TRY(render_randoms("render_bwd", *opts, rng, tensor, rnd));
+  const bool fine = opts->n_fine > 0;
+  if (fine) {
+    if (!arch_f || !blob_f || !g_fine || !flat_grad_f) {
+      set_error("render_bwd: fine pass present but fine model / grads missing");
+      return NERFB200_ERR_INVALID;
+    }
+    NB_TRY(build_plan(arch_f, &pf));
+  }
+  if (!rays || !g_coarse || !workspace || !blob_c || !flat_grad_c || n_rays <= 0) {
+    set_error("render_bwd: null pointer or empty batch");
+    return NERFB200_ERR_INVALID;
+  }
+  if ((parts & 3) == 0) {
+    set_error("render_bwd: parts must select the fine (1) and / or the coarse (2) backward");
+    return NERFB200_ERR_INVALID;
+  }
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/1, &w);
+  char* base = static_cast<char*>(workspace);
+  auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
   const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  return render_bwd_impl(arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays,
-                         noise_c ? rand_tensor(noise_c, nc) : rand_none(), noise_f ? rand_tensor(noise_f, ns) : rand_none(),
-                         g_coarse, g_fine, workspace, flat_grad_c, flat_grad_f, impl, parts,
-                         static_cast<cudaStream_t>(stream));
-}
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
 
-int32_t nerfb200_render_bwd_seeded(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                                   const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                                   const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                                   const float* g_coarse, const float* g_fine, void* workspace, float* flat_grad_c,
-                                   float* flat_grad_f, int32_t impl, int32_t parts, void* stream) {
-  NB_TRY(check_rng(rng, "render_bwd_seeded"));
-  return render_bwd_impl(arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rand_seeded(*rng, kRandNoiseC),
-                         rand_seeded(*rng, kRandNoiseF), g_coarse, g_fine, workspace, flat_grad_c, flat_grad_f, impl,
-                         parts, static_cast<cudaStream_t>(stream));
+  if (fine && (parts & 1)) {
+    NB_TRY(launch_composite_bwd(F(w.raw_f), F(w.z_f), rays, ray_stride, rnd[kRandNoiseF], g_fine, n_rays, ns,
+                                opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
+    NB_TRY(launch_mlp_bwd(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.d_raw), F(w.stash_f), F(w.gstash),
+                          flat_grad_f, impl, s));
+  }
+  if (!(parts & 2)) return NERFB200_OK;
+  // the coarse weights feed the resampler only through a detach (train_utils.py:103), so the
+  // coarse net's gradient comes from rgb/disp/acc_coarse alone.
+  NB_TRY(launch_composite_bwd(F(w.raw_c), F(w.z_c), rays, ray_stride, rnd[kRandNoiseC], g_coarse, n_rays, nc,
+                              opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
+  NB_TRY(launch_mlp_bwd(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.d_raw), F(w.stash_c), F(w.gstash),
+                        flat_grad_c, impl, s));
+  return NERFB200_OK;
 }
 
 int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64_t n_rays, int32_t per_ray, float* out,

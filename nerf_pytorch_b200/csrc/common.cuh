@@ -92,7 +92,7 @@ enum RandStream { kRandTRand = 0, kRandNoiseC = 1, kRandU = 2, kRandNoiseF = 3 }
 
 struct RandSrc {
   const float* ptr;    // tensor source [ray][stride], or nullptr
-  int64_t stride;      // floats per ray in ptr (0: one row shared by every ray)
+  int64_t stride;      // floats per ray in ptr
   int seeded;          // ptr == nullptr and seeded: generate from the stream below; neither: no source
   uint32_t key0, key1; // the seed
   uint32_t ctr1;       // stream + 4 * step
@@ -121,8 +121,8 @@ int device_sms();     // SM count of the current device (grid sizes of persisten
 
 // launchers (one per .cu), all return NERFB200_OK or an error code
 int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s);
-int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const float* t_vals,
-                         const RandSrc& t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s);
+int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const RandSrc& t_rand, int n_coarse,
+                         int perturb, int lindisp, float* z, cudaStream_t s);
 // materialises n_rays x per_ray numbers of a seeded stream (uniform for t_rand / u, normal for noise_c / noise_f)
 int launch_random_fill(const RandSrc& src, int stream_id, int64_t n_rays, int per_ray, float* out, cudaStream_t s);
 int launch_gen_rays(const float* c2w12_host, int height, int width, float focal, const int64_t* pix, int64_t n, int ndc,
@@ -154,7 +154,7 @@ int launch_composite_fwd(const float* raw, const float* z, const float* rays, in
 int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          const float* g_out, int64_t n_rays, int n_samples, float noise_std, int white_bkgd,
                          float* d_raw, cudaStream_t s);
-// u: a tensor ([n_rays][n_fine], or one shared row with stride 0), the seeded stream, or none (the det=True linspace)
+// u: a tensor [n_rays][n_fine], the seeded stream, or none (the det=True linspace)
 int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const RandSrc& u,
                             const float* cdf_in, int64_t n_rays, int n_coarse, int n_fine, float* z_fine,
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s);
@@ -230,7 +230,8 @@ __device__ __forceinline__ float RandSrc::normal(int64_t ray, int j) const {
   return (float)(r * ((j & 1) ? sn : cs));
 }
 
-// torch.linspace(0, 1, n)[q] as torch's CUDA kernel evaluates it (the det=True u of sample_pdf, nerf_helpers.py:272-276)
+// torch.linspace(0, 1, n)[q] as torch's CUDA kernel evaluates it: the stratified sampler's grid (train_utils.py:45)
+// and the det=True u of sample_pdf (nerf_helpers.py:272-276)
 __device__ __forceinline__ float linspace01(int q, int n) {
   if (n == 1) return 0.f;
   const float step = __fdiv_rn(1.0f, (float)(n - 1));

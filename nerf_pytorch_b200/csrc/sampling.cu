@@ -25,31 +25,30 @@ __device__ __forceinline__ float coarse_depth(float near, float far, float t, in
 }
 
 __global__ void sample_coarse_kernel(const float* __restrict__ rays, int ray_stride, int64_t n_rays,
-                                     const float* __restrict__ t_vals, const RandSrc t_rand,
-                                     int nc, int perturb, int lindisp, float* __restrict__ z) {
+                                     const RandSrc t_rand, int nc, int perturb, int lindisp, float* __restrict__ z) {
   const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (idx >= n_rays * nc) return;
   const int64_t r = idx / nc;
   const int i = (int)(idx - r * nc);
   const float near = rays[r * ray_stride + 6], far = rays[r * ray_stride + 7];
-  const float zi = coarse_depth(near, far, t_vals[i], lindisp);
+  const float zi = coarse_depth(near, far, linspace01(i, nc), lindisp);
   if (!perturb) {
     z[idx] = zi;
     return;
   }
   float upper = zi, lower = zi;
-  if (i + 1 < nc) upper = __fmul_rn(0.5f, __fadd_rn(coarse_depth(near, far, t_vals[i + 1], lindisp), zi));
-  if (i > 0) lower = __fmul_rn(0.5f, __fadd_rn(zi, coarse_depth(near, far, t_vals[i - 1], lindisp)));
+  if (i + 1 < nc) upper = __fmul_rn(0.5f, __fadd_rn(coarse_depth(near, far, linspace01(i + 1, nc), lindisp), zi));
+  if (i > 0) lower = __fmul_rn(0.5f, __fadd_rn(zi, coarse_depth(near, far, linspace01(i - 1, nc), lindisp)));
   z[idx] = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), t_rand.uniform(r, i)));
 }
 
-int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const float* t_vals,
-                         const RandSrc& t_rand, int n_coarse, int perturb, int lindisp, float* z, cudaStream_t s) {
+int launch_sample_coarse(const float* rays, int ray_stride, int64_t n_rays, const RandSrc& t_rand, int n_coarse,
+                         int perturb, int lindisp, float* z, cudaStream_t s) {
   const int64_t total = n_rays * n_coarse;
   const int threads = 256;
   const int64_t blocks = (total + threads - 1) / threads;
-  sample_coarse_kernel<<<(unsigned)blocks, threads, 0, s>>>(rays, ray_stride, n_rays, t_vals, t_rand, n_coarse,
-                                                            perturb, lindisp, z);
+  sample_coarse_kernel<<<(unsigned)blocks, threads, 0, s>>>(rays, ray_stride, n_rays, t_rand, n_coarse, perturb,
+                                                            lindisp, z);
   count_launch();
   return check_cuda(cudaGetLastError(), "sample_coarse launch");
 }

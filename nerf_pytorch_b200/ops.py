@@ -203,12 +203,12 @@ def pack_weights(arch: ArchSpec, flat: torch.Tensor, blob: Optional[torch.Tensor
 # ------------------------------------------------------------------------------------------------
 # stage-level ops (test hooks + building blocks)
 # ------------------------------------------------------------------------------------------------
-def sample_coarse(rays, t_vals, t_rand, n_coarse, perturb, lindisp):
+def sample_coarse(rays, t_rand, n_coarse, perturb, lindisp):
     lib = _lib.load()
     n = rays.shape[0]
     z = torch.empty(n, n_coarse, dtype=torch.float32, device=rays.device)
-    _lib.check(lib.nerfb200_sample_coarse(_ptr(rays), rays.shape[1], n, _ptr(t_vals), _ptr(t_rand) if perturb else None,
-                                          n_coarse, int(bool(perturb)), int(bool(lindisp)), _ptr(z), _stream()),
+    _lib.check(lib.nerfb200_sample_coarse(_ptr(rays), rays.shape[1], n, _ptr(t_rand) if perturb else None, n_coarse,
+                                          int(bool(perturb)), int(bool(lindisp)), _ptr(z), _stream()),
                "sample_coarse")
     return z
 
@@ -332,17 +332,18 @@ def composite_bwd(raw, z, rays, noise, g_out, noise_std, white_bkgd):
 
 
 def sample_pdf_merge(z_coarse, weights_coarse, u, n_fine, cdf_in=None, want_aux=False):
-    """u: (n_rays, n_fine) or (n_fine,) shared by all rays (the det=True linspace)."""
+    """u: (n_rays, n_fine), or None for the det=True linspace (built in the kernel)."""
     lib = _lib.load()
     n, nc = z_coarse.shape
+    if u is not None and tuple(u.shape) != (n, n_fine):
+        raise ValueError(f"nerfb200 sample_pdf_merge: u has shape {tuple(u.shape)}, expected {(n, n_fine)}")
     dev = z_coarse.device
     z_fine = torch.empty(n, nc + n_fine, dtype=torch.float32, device=dev)
     zs = torch.empty(n, n_fine, dtype=torch.float32, device=dev) if want_aux else None
     inds = torch.empty(n, n_fine, dtype=torch.int32, device=dev) if want_aux else None
     cdf = torch.empty(n, nc - 1, dtype=torch.float32, device=dev) if want_aux else None
-    u_stride = 0 if u.dim() == 1 else n_fine
-    _lib.check(lib.nerfb200_sample_pdf_merge(_ptr(z_coarse), _ptr(weights_coarse), _ptr(u), u_stride, _ptr(cdf_in), n,
-                                             nc, n_fine, _ptr(z_fine), _ptr(zs), _ptr(inds), _ptr(cdf), _stream()),
+    _lib.check(lib.nerfb200_sample_pdf_merge(_ptr(z_coarse), _ptr(weights_coarse), _ptr(u), _ptr(cdf_in), n, nc, n_fine,
+                                             _ptr(z_fine), _ptr(zs), _ptr(inds), _ptr(cdf), _stream()),
                "sample_pdf_merge")
     return (z_fine, zs, inds, cdf) if want_aux else z_fine
 
@@ -381,8 +382,16 @@ def render_workspace_layout(arch_c, arch_f, opts: RenderOpts, n_rays: int, train
     return dict(zip(WS_SECTIONS, list(offs)))
 
 
-def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, t_vals, t_rand, noise_c, u, noise_f,
-               training: bool, impl: int = IMPL_SIMT, workspace: Optional[torch.Tensor] = None):
+def _random_args(randoms):
+    """The C arguments (rng, t_rand, noise_c, u, noise_f) of a render call.  ``randoms`` is a ``SeededRandoms`` (the
+    kernels generate all four inputs) or a dict of tensors keyed by RAND_STREAMS (a missing key: not supplied)."""
+    if isinstance(randoms, SeededRandoms):
+        return (C.byref(randoms.c_struct()), None, None, None, None)
+    return (None,) + tuple(_ptr(randoms.get(k)) for k in RAND_STREAMS)
+
+
+def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, training: bool, impl: int = IMPL_SIMT,
+               workspace: Optional[torch.Tensor] = None):
     """One ray chunk through the whole path.  Returns (out_coarse[N,8], out_fine[N,8] | None, workspace)."""
     lib = _lib.load()
     n = rays.shape[0]
@@ -395,59 +404,24 @@ def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, t_vals, t
     out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
     ac = arch_c.c_struct()
     af = arch_f.c_struct() if fine else None
-    u_stride = 0 if (u is not None and u.dim() == 1) else opts.n_fine
     _lib.check(lib.nerfb200_render_fwd(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
                                        _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
-                                       _ptr(t_vals), _ptr(t_rand), _ptr(noise_c), _ptr(u) if fine else None, u_stride,
-                                       _ptr(noise_f) if fine else None, _ptr(out_c), _ptr(out_f), _ptr(workspace),
+                                       *_random_args(randoms), _ptr(out_c), _ptr(out_f), _ptr(workspace),
                                        int(training), impl, _stream()), "render_fwd")
     return out_c, out_f, workspace
 
 
-def render_fwd_seeded(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, t_vals, rng: SeededRandoms,
-                      training: bool, impl: int = IMPL_SIMT, workspace: Optional[torch.Tensor] = None):
-    """``render_fwd`` with the random inputs generated in-kernel from ``rng`` (no random tensors)."""
-    lib = _lib.load()
-    n = rays.shape[0]
-    dev = rays.device
-    fine = opts.n_fine > 0
-    need = render_workspace_bytes(arch_c, arch_f if fine else None, opts, n, training)
-    if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
-    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
-    _lib.check(lib.nerfb200_render_fwd_seeded(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                              _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
-                                              _ptr(t_vals), C.byref(rng.c_struct()), _ptr(out_c), _ptr(out_f),
-                                              _ptr(workspace), int(training), impl, _stream()), "render_fwd_seeded")
-    return out_c, out_f, workspace
-
-
-def render_bwd_seeded(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, rng: SeededRandoms, g_c, g_f, workspace,
-                      flat_grad_c, flat_grad_f, impl: int = IMPL_SIMT, parts: int = 3):
-    """``render_bwd`` of a ``render_fwd_seeded`` workspace: the noise is regenerated from ``rng``, not read."""
+def render_bwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, g_c, g_f, workspace, flat_grad_c,
+               flat_grad_f, impl: int = IMPL_SIMT, parts: int = 3):
+    """Backward of a ``render_fwd`` workspace, given the same ``randoms`` (only the noise is needed again: a
+    ``SeededRandoms`` regenerates it in-kernel, a dict supplies the tensors)."""
     lib = _lib.load()
     fine = opts.n_fine > 0
     ac = arch_c.c_struct()
     af = arch_f.c_struct() if fine else None
-    _lib.check(lib.nerfb200_render_bwd_seeded(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                              _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
-                                              rays.shape[0], C.byref(rng.c_struct()), _ptr(g_c),
-                                              _ptr(g_f) if fine else None, _ptr(workspace), _ptr(flat_grad_c),
-                                              _ptr(flat_grad_f) if fine else None, impl, int(parts), _stream()),
-               "render_bwd_seeded")
-
-
-def render_bwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, noise_c, noise_f, g_c, g_f, workspace,
-               flat_grad_c, flat_grad_f, impl: int = IMPL_SIMT, parts: int = 3):
-    lib = _lib.load()
-    fine = opts.n_fine > 0
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
+    rng, _, noise_c, _, noise_f = _random_args(randoms)
     _lib.check(lib.nerfb200_render_bwd(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
                                        _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
-                                       rays.shape[0], _ptr(noise_c), _ptr(noise_f) if fine else None, _ptr(g_c),
-                                       _ptr(g_f) if fine else None, _ptr(workspace), _ptr(flat_grad_c),
-                                       _ptr(flat_grad_f) if fine else None, impl, int(parts), _stream()), "render_bwd")
+                                       rays.shape[0], rng, noise_c, noise_f, _ptr(g_c), _ptr(g_f) if fine else None,
+                                       _ptr(workspace), _ptr(flat_grad_c), _ptr(flat_grad_f) if fine else None, impl,
+                                       int(parts), _stream()), "render_bwd")

@@ -209,22 +209,17 @@ def _packed(model, arch: ops.ArchSpec):
 # --------------------------------------------------------------------------------------------------
 class _RenderChunk(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, cfg, rays, t_vals, t_rand, noise_c, u, noise_f, *params):
-        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks, rng = cfg
-        if rng is None:
-            out_c, out_f, ws = ops.render_fwd(arch_c, arch_f, opts, blob_c, blob_f, rays, t_vals, t_rand, noise_c, u,
-                                              noise_f, training=training, impl=impl)
-        else:
-            out_c, out_f, ws = ops.render_fwd_seeded(arch_c, arch_f, opts, blob_c, blob_f, rays, t_vals, rng,
-                                                     training=training, impl=impl)
+    def forward(ctx, cfg, rays, randoms, *params):
+        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks = cfg
+        out_c, out_f, ws = ops.render_fwd(arch_c, arch_f, opts, blob_c, blob_f, rays, randoms, training=training,
+                                          impl=impl)
         if training:
             ctx.cfg = cfg
             ctx.ws = ws
-            # seeded: the backward regenerates the noise in-kernel, so no noise tensor is kept
-            if rng is None:
-                ctx.save_for_backward(rays, noise_c, noise_f)
-            else:
-                ctx.save_for_backward(rays)
+            # the backward needs the noise again: a SeededRandoms regenerates it in-kernel, drawn tensors are kept
+            ctx.rng = randoms if isinstance(randoms, SeededRandoms) else None
+            noise = (None, None) if ctx.rng is not None else (randoms.get("noise_c"), randoms.get("noise_f"))
+            ctx.save_for_backward(rays, *noise)
         ctx.set_materialize_grads(False)
         if out_f is None:
             return out_c, None
@@ -232,8 +227,8 @@ class _RenderChunk(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_c, g_f):
-        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks, rng = ctx.cfg
-        rays = ctx.saved_tensors[0]
+        arch_c, arch_f, opts, blob_c, blob_f, training, impl, n_chunks = ctx.cfg
+        rays, noise_c, noise_f = ctx.saved_tensors
         fine = opts.n_fine > 0
         n = rays.shape[0]
         if g_c is None:
@@ -245,12 +240,9 @@ class _RenderChunk(torch.autograd.Function):
         flat_grad = torch.zeros(nc + nf, dtype=torch.float32, device=rays.device)
         g_c = g_c.contiguous()
         g_f = g_f.contiguous() if fine else None
-        grad_out = (g_c, g_f, ctx.ws, flat_grad[:nc], flat_grad[nc:] if fine else None)
-        if rng is None:
-            noise_c, noise_f = ctx.saved_tensors[1:]
-            bwd, args = ops.render_bwd, (arch_c, arch_f, opts, blob_c, blob_f, rays, noise_c, noise_f) + grad_out
-        else:
-            bwd, args = ops.render_bwd_seeded, (arch_c, arch_f, opts, blob_c, blob_f, rays, rng) + grad_out
+        randoms = ctx.rng if ctx.rng is not None else dict(noise_c=noise_c, noise_f=noise_f)
+        args = (arch_c, arch_f, opts, blob_c, blob_f, rays, randoms, g_c, g_f, ctx.ws, flat_grad[:nc],
+                flat_grad[nc:] if fine else None)
         sync = _GRAD_SYNC
         if sync is not None and n_chunks != 1:
             # several chunks per step: no collective here (ranks may even differ in their chunk counts); the summed
@@ -259,7 +251,7 @@ class _RenderChunk(torch.autograd.Function):
             _PENDING_SYNC = True
             sync = None
         if sync is None:
-            bwd(*args, impl=impl)
+            ops.render_bwd(*args, impl=impl)
         else:
             # the ONE collective of a data-parallel step, split in two so that the fine network's half (final as soon
             # as its backward is done) crosses NVLink while the coarse network's backward is still running
@@ -268,9 +260,9 @@ class _RenderChunk(torch.autograd.Function):
             group, world = sync
             works = []
             if fine:
-                bwd(*args, impl=impl, parts=1)
+                ops.render_bwd(*args, impl=impl, parts=1)
                 works.append(dist.all_reduce(flat_grad[nc:], op=dist.ReduceOp.SUM, group=group, async_op=True))
-            bwd(*args, impl=impl, parts=2 if fine else 3)
+            ops.render_bwd(*args, impl=impl, parts=2 if fine else 3)
             works.append(dist.all_reduce(flat_grad[:nc], op=dist.ReduceOp.SUM, group=group, async_op=True))
             for w in works:
                 w.wait()
@@ -281,7 +273,7 @@ class _RenderChunk(torch.autograd.Function):
             for _, w_off, b_off, fin, fout in arch.flat_layout():
                 grads.append(flat_grad[base + w_off: base + w_off + fin * fout].view(fout, fin))
                 grads.append(flat_grad[base + b_off: base + b_off + fout])
-        return (None,) * 7 + tuple(grads)
+        return (None,) * 3 + tuple(grads)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -327,27 +319,27 @@ def predict_and_render_radiance(
     perturb = bool(o.perturb)
     opts = ops.make_opts(nc, nf, perturb, o.lindisp, o.white_background, noise_std)
 
-    rng = randoms if isinstance(randoms, SeededRandoms) else None
-    rnd = randoms if isinstance(randoms, dict) else {}
+    rnd = randoms
+    if not isinstance(randoms, SeededRandoms):  # seeded: the kernels generate all four
+        given = randoms or {}
 
-    def take(name, shape, fn):
-        t = rnd.get(name)
-        if t is None:
-            return fn(shape, dtype=torch.float32, device=dev)
-        return t.to(device=dev, dtype=torch.float32).contiguous()
+        def take(name, shape, fn):
+            t = given.get(name)
+            if t is None:
+                return fn(shape, dtype=torch.float32, device=dev)
+            return t.to(device=dev, dtype=torch.float32).contiguous()
 
-    # reference draw order: rand(N,Nc) -> randn(N,Nc) -> rand(N,Nf) -> randn(N,Nc+Nf)  (SURVEY section 5)
-    t_vals = torch.linspace(0.0, 1.0, nc, dtype=torch.float32, device=dev)
-    t_rand = noise_c = u = noise_f = None
-    if rng is None:  # seeded: the kernels generate all four (and the det=True u when perturb is off)
-        t_rand = take("t_rand", (n, nc), torch.rand) if perturb else None
-        noise_c = take("noise_c", (n, nc), torch.randn) if noise_std > 0.0 else None
-        if fine:
-            if perturb:
-                u = take("u", (n, nf), torch.rand)
-            else:  # det = (perturb == 0.0): shared linspace, nerf_helpers.py:272-276
-                u = torch.linspace(0.0, 1.0, steps=nf, dtype=torch.float32, device=dev)
-            noise_f = take("noise_f", (n, nc + nf), torch.randn) if noise_std > 0.0 else None
+        # reference draw order: rand(N,Nc) -> randn(N,Nc) -> rand(N,Nf) -> randn(N,Nc+Nf)  (SURVEY section 5); with
+        # perturb off the fine pass resamples at the det=True linspace, which the kernel builds (nerf_helpers.py:272-276)
+        rnd = {}
+        if perturb:
+            rnd["t_rand"] = take("t_rand", (n, nc), torch.rand)
+        if noise_std > 0.0:
+            rnd["noise_c"] = take("noise_c", (n, nc), torch.randn)
+        if fine and perturb:
+            rnd["u"] = take("u", (n, nf), torch.rand)
+        if fine and noise_std > 0.0:
+            rnd["noise_f"] = take("noise_f", (n, nc + nf), torch.randn)
 
     all_params = list(params_c) + list(params_f)
     training = torch.is_grad_enabled() and any(p.requires_grad for p in all_params)
@@ -355,8 +347,8 @@ def predict_and_render_radiance(
         impl = DEFAULT_IMPL
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, int(impl), int(_n_chunks), rng)
-    out_c, out_f = _RenderChunk.apply(cfg, rays, t_vals, t_rand, noise_c, u, noise_f, *all_params)
+    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, int(impl), int(_n_chunks))
+    out_c, out_f = _RenderChunk.apply(cfg, rays, rnd, *all_params)
     rgb_c, disp_c, acc_c = out_c[:, :3], out_c[:, 3], out_c[:, 4]
     if out_f is None:
         return rgb_c, disp_c, acc_c, None, None, None

@@ -394,8 +394,8 @@ def test_seeded_step_leaves_torch_generators_alone_and_saves_no_noise():
 
 @gpu
 @pytest.mark.parametrize("impl", [0, 1], ids=["simt", "tc"])
-def test_render_bwd_seeded_reads_no_noise_tensor(impl):
-    """The C entry points directly: render_fwd_seeded + render_bwd_seeded against render_fwd + render_bwd fed the
+def test_seeded_render_bwd_reads_no_noise_tensor(impl):
+    """The C entry points directly: render_fwd + render_bwd given a SeededRandoms against the same calls fed the
     random_fill tensors.  The seeded backward regenerates the noise for the sigma ReLU gate."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
@@ -410,22 +410,18 @@ def test_render_bwd_seeded_reads_no_noise_tensor(impl):
                          c.options.dataset.no_ndc is False, c.options.dataset.near, c.options.dataset.far, True)
     n, nc, nf = rays.shape[0], o.num_coarse, o.num_fine
     opts = ops.make_opts(nc, nf, o.perturb, o.lindisp, o.white_background, o.radiance_field_noise_std)
-    t_vals = torch.linspace(0.0, 1.0, nc, device="cuda")
     rng = nb.SeededRandoms(31337, 4, 10 ** 6)
     r = _tensors_of(rng, n, o, True)
     g = torch.Generator().manual_seed(3)
     g_c, g_f = torch.randn(n, 8, generator=g).cuda(), torch.randn(n, 8, generator=g).cuda()
     nfl = arch.flat_param_count()
 
-    out_s = ops.render_fwd_seeded(arch, arch, opts, blob_c, blob_f, rays, t_vals, rng, training=True, impl=impl)
+    out_s = ops.render_fwd(arch, arch, opts, blob_c, blob_f, rays, rng, training=True, impl=impl)
     fg_s = torch.zeros(2 * nfl, device="cuda")
-    ops.render_bwd_seeded(arch, arch, opts, blob_c, blob_f, rays, rng, g_c, g_f, out_s[2], fg_s[:nfl], fg_s[nfl:],
-                          impl=impl)
-    out_d = ops.render_fwd(arch, arch, opts, blob_c, blob_f, rays, t_vals, r["t_rand"], r["noise_c"], r["u"],
-                           r["noise_f"], training=True, impl=impl)
+    ops.render_bwd(arch, arch, opts, blob_c, blob_f, rays, rng, g_c, g_f, out_s[2], fg_s[:nfl], fg_s[nfl:], impl=impl)
+    out_d = ops.render_fwd(arch, arch, opts, blob_c, blob_f, rays, r, training=True, impl=impl)
     fg_d = torch.zeros(2 * nfl, device="cuda")
-    ops.render_bwd(arch, arch, opts, blob_c, blob_f, rays, r["noise_c"], r["noise_f"], g_c, g_f, out_d[2], fg_d[:nfl],
-                   fg_d[nfl:], impl=impl)
+    ops.render_bwd(arch, arch, opts, blob_c, blob_f, rays, r, g_c, g_f, out_d[2], fg_d[:nfl], fg_d[nfl:], impl=impl)
     assert _bits_equal(out_s[0], out_d[0]) and _bits_equal(out_s[1], out_d[1])
     if impl == 1:
         assert _bits_equal(fg_s, fg_d)
@@ -448,6 +444,87 @@ def test_library_refuses_out_of_range_rng():
         _lib.ERR_INVALID
     assert lib.nerfb200_random_fill(C.byref(_lib.Rng(0, 2 ** 30 - 1, 0)), 3, 4, 4, C.c_void_p(out.data_ptr()), stream) == \
         _lib.OK
+
+
+@gpu
+def test_render_entry_points_refuse_rng_with_tensors_and_out_of_range_rng():
+    """render_fwd / render_bwd take the randoms from an rng or from tensors, never both, and check the rng."""
+    import ctypes as C
+
+    from nerf_pytorch_b200 import _lib, ops
+
+    lib = _lib.load()
+    arch = ops.ArchSpec()
+    nc, nf, n = 64, 64, 128
+    opts = ops.make_opts(nc, nf, True, False, False, 1.0)
+    nfl = arch.flat_param_count()
+    blob = ops.pack_weights(arch, torch.zeros(nfl, device="cuda"))
+    rays = torch.rand(n, 11, device="cuda")
+    rays[:, 6], rays[:, 7] = 2.0, 6.0
+    ws = torch.empty(ops.render_workspace_bytes(arch, arch, opts, n, True), dtype=torch.uint8, device="cuda")
+    out = torch.empty(2, n, 8, device="cuda")
+    g = torch.zeros(n, 8, device="cuda")
+    fg = torch.zeros(2 * nfl, device="cuda")
+    rnd = torch.rand(n, nc + nf, device="cuda")  # large enough for any of the four inputs
+    p = lambda t: C.c_void_p(t.data_ptr())
+    a, o = C.byref(arch.c_struct()), C.byref(opts)
+    stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def fwd(rng, tensors):
+        return lib.nerfb200_render_fwd(a, a, o, p(blob), p(blob), p(rays), 11, n, rng, *tensors, p(out[0]), p(out[1]),
+                                       p(ws), 1, ops.IMPL_SIMT, stream)
+
+    def bwd(rng, tensors):
+        return lib.nerfb200_render_bwd(a, a, o, p(blob), p(blob), p(rays), 11, n, rng, *tensors, p(g), p(g), p(ws),
+                                       p(fg[:nfl]), p(fg[nfl:]), ops.IMPL_SIMT, 3, stream)
+
+    def one_tensor(k, count):
+        return [p(rnd) if i == k else None for i in range(count)]
+
+    rng = C.byref(_lib.Rng(5, 6, 7))
+    assert fwd(rng, [None] * 4) == _lib.OK and bwd(rng, [None] * 2) == _lib.OK
+    for k in range(4):
+        assert fwd(rng, one_tensor(k, 4)) == _lib.ERR_INVALID, k
+        assert b"random tensor" in lib.nerfb200_last_error()
+    for k in range(2):
+        assert bwd(rng, one_tensor(k, 2)) == _lib.ERR_INVALID, k
+        assert b"random tensor" in lib.nerfb200_last_error()
+    for bad in (_lib.Rng(0, 2 ** 30, 0), _lib.Rng(0, 0, -1)):
+        assert fwd(C.byref(bad), [None] * 4) == _lib.ERR_INVALID
+        assert bwd(C.byref(bad), [None] * 2) == _lib.ERR_INVALID
+    torch.cuda.synchronize()
+
+
+@gpu
+def test_sample_coarse_grid_is_torch_linspace_at_every_sample_count():
+    """The stratified grid is built in the kernel: with near 0, far 1 and no jitter, z = 0 * (1 - t) + 1 * t = t exactly,
+    so z must be torch's CUDA linspace bit for bit at every n_coarse the library accepts."""
+    from nerf_pytorch_b200 import ops
+
+    rays = torch.zeros(3, 8, device="cuda")
+    rays[:, 7] = 1.0
+    for nc in range(2, 1025):
+        z = ops.sample_coarse(rays, None, nc, False, False)
+        want = torch.linspace(0.0, 1.0, nc, device="cuda").expand(3, nc)
+        assert _bits_equal(z, want), nc
+
+
+@gpu
+def test_sample_pdf_det_u_is_torch_linspace_at_every_fine_count():
+    """u = None resamples at the det=True linspace built in the kernel: the same bits as feeding torch's CUDA linspace
+    to every ray, at every n_fine the library accepts for n_coarse 64."""
+    from nerf_pytorch_b200 import ops
+
+    g = torch.Generator(device="cuda").manual_seed(11)
+    n, nc = 8, 64
+    zc = torch.sort(torch.rand(n, nc, device="cuda", generator=g) * 4 + 2, -1).values.contiguous()
+    w = (torch.rand(n, nc, device="cuda", generator=g) ** 4).contiguous()
+    for nf in range(1, 1024 - nc + 1):
+        got = ops.sample_pdf_merge(zc, w, None, nf, want_aux=True)
+        u = torch.linspace(0.0, 1.0, nf, device="cuda").expand(n, nf).contiguous()
+        want = ops.sample_pdf_merge(zc, w, u, nf, want_aux=True)
+        for a, b in zip(got, want):
+            assert _bits_equal(a, b), nf
 
 
 @gpu

@@ -21,15 +21,14 @@ def _arch(c: Case):
 
 
 @pytest.mark.parametrize("name", CASES)
-def test_sample_coarse_bit_exact(name):
+def test_sample_coarse_in_kernel_grid_bit_exact(name):
     from nerf_pytorch_b200 import ops
 
     c = Case(name)
     rays, _, aux = c.aux()
     o = c.options.nerf.train
-    t_vals = torch.linspace(0.0, 1.0, o.num_coarse, device="cuda")
     t_rand = c.randoms["t_rand"].cuda() if o.perturb else None
-    z = ops.sample_coarse(rays.cuda(), t_vals, t_rand, o.num_coarse, o.perturb, o.lindisp)
+    z = ops.sample_coarse(rays.cuda(), t_rand, o.num_coarse, o.perturb, o.lindisp)
     assert torch.equal(z.cpu(), aux["z_coarse"]), err_stats(z, aux["z_coarse"])
 
 
@@ -135,7 +134,7 @@ def test_sample_pdf_indices_exact_given_cdf_and_values(name):
     assert (z_fine2[:, 1:] >= z_fine2[:, :-1]).all()
 
 
-def test_sample_pdf_deterministic_linspace():
+def test_sample_pdf_in_kernel_det_linspace():
     from nerf_pytorch_b200 import ops
     from oracle import nerf_oracle as O
 
@@ -143,8 +142,8 @@ def test_sample_pdf_deterministic_linspace():
     _, _, aux = c.aux()
     o = c.options.nerf.train
     zc, wc = aux["z_coarse"].cuda().contiguous(), aux["weights_coarse"].cuda().contiguous()
-    u = torch.linspace(0.0, 1.0, steps=o.num_fine, device="cuda")
-    z_fine, zs, inds, cdf = ops.sample_pdf_merge(zc, wc, u, o.num_fine, cdf_in=aux["cdf"].cuda().contiguous(), want_aux=True)
+    z_fine, zs, inds, cdf = ops.sample_pdf_merge(zc, wc, None, o.num_fine, cdf_in=aux["cdf"].cuda().contiguous(),
+                                                 want_aux=True)
     assert torch.equal(inds.cpu().long(), aux["inds"])  # includes u = 1.0 -> index len(cdf)
     assert torch.equal(z_fine.cpu(), aux["z_fine"])
 
