@@ -439,7 +439,7 @@ int tc_supported(const Plan& p, int n_samples, const char* what, bool training) 
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (n_samples > 0 && (kTileRows + n_samples - 1) / n_samples + 1 > kMaxRaysPerTile) {
-    set_error("%s impl=1 (wgmma): fewer than 16 samples per ray not supported; use impl=0", what);
+    set_error("%s impl=1 (wgmma): fewer than 15 samples per ray not supported; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map(p).n_stages < 2) {

@@ -271,13 +271,15 @@ def impl_supported(arch: ArchSpec, n_samples: int, impl: int) -> bool:
     return _lib.load().nerfb200_impl_supported(C.byref(arch.c_struct()), int(n_samples), int(impl)) == _lib.OK
 
 
-def mlp_bwd(arch: ArchSpec, blob, rays, z, d_raw, stash, impl=IMPL_SIMT):
-    """Returns (flat_grad, scratch): scratch is the gradient stash for impl 0, the gradient blob for impl 1."""
+def mlp_bwd(arch: ArchSpec, blob, rays, z, d_raw, stash, impl=IMPL_SIMT, flat_grad=None):
+    """Parameter gradients, accumulated into ``flat_grad`` (a fresh zero vector when None).  Returns (flat_grad,
+    scratch): scratch is the gradient stash for impl 0, the gradient blob for impl 1."""
     lib = _lib.load()
     n, s = z.shape
     gstash = torch.empty(lib.nerfb200_bwd_scratch_floats(C.byref(arch.c_struct()), n * s, impl), dtype=torch.float32,
                          device=z.device)
-    flat_grad = torch.zeros(arch.flat_param_count(), dtype=torch.float32, device=z.device)
+    if flat_grad is None:
+        flat_grad = torch.zeros(arch.flat_param_count(), dtype=torch.float32, device=z.device)
     _lib.check(lib.nerfb200_mlp_bwd(C.byref(arch.c_struct()), _ptr(blob), _ptr(rays), rays.shape[1], _ptr(z), n, s,
                                     _ptr(d_raw), _ptr(stash), _ptr(gstash), _ptr(flat_grad), impl, _stream()),
                "mlp_bwd")

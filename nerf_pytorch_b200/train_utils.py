@@ -29,7 +29,7 @@ from .nerf_helpers import Embedder, get_minibatches
 COMPAT_MODE_QUIRK = True
 
 # None: wgmma tensor cores (three-term split-precision products) wherever the kernels support the configuration (training: hidden
-# 128; inference: hidden 128 or 256; encodings <= 64 wide, >= 16 samples per ray), fp32 CUDA cores otherwise; 0 / 1 force one.
+# 128; inference: hidden 128 or 256; encodings <= 64 wide, >= 15 samples per ray), fp32 CUDA cores otherwise; 0 / 1 force one.
 DEFAULT_IMPL = None
 
 

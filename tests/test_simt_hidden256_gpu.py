@@ -112,14 +112,17 @@ def _scaled(sd, c):
     return {k: v * c if v.shape[0] >= 64 else v for k, v in sd.items()}  # gemm layers only, not the heads
 
 
-@functools.lru_cache(maxsize=None)
 def _weights(name, state):
-    """Seeded reference init; "scaled": every gemm layer's weight and bias times one factor c, found by bisection so
-    that max |raw| over a probe batch is ~3e3."""
+    return arch_weights(_spec(name), state)
+
+
+@functools.lru_cache(maxsize=None)
+def arch_weights(arch, state):
+    """Seeded reference init of `arch` (an ops.ArchSpec); "scaled": every gemm layer's weight and bias times one factor
+    c, found by bisection so that max |raw| over a probe batch is ~3e3."""
     from oracle import nerf_oracle as O
 
-    arch = _spec(name)
-    sd = O.init_flexible_nerf(arch.num_layers, 256, 4, arch.n_freq_xyz, arch.n_freq_dir,
+    sd = O.init_flexible_nerf(arch.num_layers, arch.hidden, arch.skip_every, arch.n_freq_xyz, arch.n_freq_dir,
                               include_input_xyz=arch.include_input_xyz, include_input_dir=arch.include_input_dir,
                               use_viewdirs=arch.use_viewdirs, generator=torch.Generator().manual_seed(2024))
     if state == "init":
