@@ -71,7 +71,7 @@ int64_t nerfb200_bwd_bytes_per_point(const nerfb200_arch_t* arch);
 /* NERFB200_OK if `impl` (0 fp32 CUDA cores, 1 wgmma) can run this architecture forward AND backward with
  * n_samples samples per ray, else NERFB200_ERR_UNSUPPORTED (reason in nerfb200_last_error()).  impl = 2 asks for the
  * wgmma FORWARD alone (inference: training = 0 in render_fwd / stash = NULL in mlp_fwd with impl = 1), which also
- * covers hidden_size 256 */
+ * covers hidden_size 256.  impl = 3 (the single-pass fp16 forward, see nerfb200_mlp_fwd) gives the same answer as 2. */
 int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, int32_t impl);
 
 /* ---- parameters -------------------------------------------------------------------------------
@@ -126,7 +126,12 @@ int32_t nerfb200_encode(const nerfb200_arch_t* arch, int32_t which, const float*
  * impl: 0 = fp32 CUDA cores (bit-faithful fp32 FMA), 1 = wgmma tensor cores: every product as a three-term
  * split (fp16 x 2 operands with a 2^11-scaled residual, fp32 accumulation; ~22 significant bits per operand).
  * The split carries 22 bits for magnitudes in 6.1e-5 .. 65504 and resolves 1.5e-11 absolutely below; larger
- * activations / weights saturate (a NeRF's stay far inside; use impl 0 for networks that do not). */
+ * activations / weights saturate (a NeRF's stay far inside; use impl 0 for networks that do not).
+ * impl 3 = single-pass fp16 wgmma forward, INFERENCE ONLY: one product fp16(w) x fp16(activation / 16) per k-step,
+ * fp32 accumulation (~11 significant bits per operand; the 1- and 3-wide heads and the direction term stay fp32).
+ * Judged by the PSNR of the rendered image, not by parity with impl 0 / 1.  Accepted where impl 2 is; stash must be
+ * NULL (NERFB200_ERR_UNSUPPORTED otherwise), and mlp_bwd, mlp_dgrad, mlp_wgrad, bwd_scratch_floats and render_bwd
+ * refuse it.  |activation| >= 1.05e6 or |weight| >= 32 turns the output into inf / NaN, as with impl 1. */
 int64_t nerfb200_stash_floats(const nerfb200_arch_t* arch, int64_t n_points);
 int32_t nerfb200_mlp_fwd(const nerfb200_arch_t* arch, const float* blob, const float* rays, int32_t ray_stride,
                          const float* z, int64_t n_rays, int32_t n_samples, float* raw, float* stash,
@@ -217,6 +222,8 @@ int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64
  * u must then be given, a noise tensor left NULL means no noise.  render_bwd needs the noise again for the sigma ReLU gate: pass it the same *rng,
  * or the same noise tensors, as the render_fwd call that filled the workspace (seeded, it reads no noise tensor).
  * render_fwd: out_coarse/out_fine[n][8] = [r g b disp acc depth 0 0] (out_fine NULL when n_fine == 0).
+ *   impl: the MLP kernels as in nerfb200_mlp_fwd (1 wgmma, 3 single-pass fp16 wgmma, anything else fp32 CUDA cores);
+ *   impl 3 renders only: training = 1 is refused with NERFB200_ERR_UNSUPPORTED.
  *   workspace: nerfb200_render_workspace_bytes(...) bytes; keeps z/raw/stash for render_bwd.
  * render_bwd: g_coarse/g_fine[n][8] upstream grads (g_fine NULL when no fine pass); accumulates into flat_grad_c /
  *   flat_grad_f (may alias different ranges of one buffer).  parts: bit 0 = the fine network's backward, bit 1 = the

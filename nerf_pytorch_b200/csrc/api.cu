@@ -231,6 +231,12 @@ static void carve(const Plan& pc, const Plan* pf, const nerfb200_render_opts_t& 
   w->total = off;
 }
 
+// impl 3, the single-pass fp16 wgmma forward, renders images; every entry point that trains refuses it
+static int refuse_fast(const char* what) {
+  set_error("%s: impl=3 (single-pass fp16 wgmma forward) is inference only; train with impl=0 or impl=1", what);
+  return NERFB200_ERR_UNSUPPORTED;
+}
+
 static int check_opts(const nerfb200_render_opts_t* o) {
   if (!o) {
     set_error("null render options");
@@ -283,6 +289,7 @@ int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, 
   if (impl == 0) return NERFB200_OK;
   if (impl == 1) return bwd_tc_supported(p, n_samples, "impl_supported");
   if (impl == 2) return tc_supported(p, n_samples, "impl_supported", /*training=*/false);  // wgmma forward only (inference)
+  if (impl == 3) return tc_supported(p, n_samples, "impl_supported", /*training=*/false, /*fast=*/true);
   set_error("unknown impl %d", impl);
   return NERFB200_ERR_INVALID;
 }
@@ -290,6 +297,10 @@ int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, 
 int64_t nerfb200_bwd_scratch_floats(const nerfb200_arch_t* arch, int64_t n_points, int32_t impl) {
   Plan p;
   if (build_plan(arch, &p) != NERFB200_OK || n_points < 0) return -1;
+  if (impl == 3) {
+    refuse_fast("bwd_scratch_floats");
+    return -1;
+  }
   if (impl == 1) return bwd_tc_scratch_floats(p);
   return ((n_points + 127) & ~int64_t(127)) * p.sum_n;
 }
@@ -422,6 +433,10 @@ int32_t nerfb200_mlp_fwd(const nerfb200_arch_t* arch, const float* blob, const f
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (impl == 0) return launch_mlp_fwd_simt(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
   if (impl == 1) return launch_mlp_fwd_tc(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
+  if (impl == 3) {
+    if (stash) return refuse_fast("mlp_fwd with a stash");
+    return launch_mlp_fwd_tc_fast(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, s);
+  }
   set_error("mlp_fwd: unknown impl %d", impl);
   return NERFB200_ERR_INVALID;
 }
@@ -429,6 +444,7 @@ int32_t nerfb200_mlp_fwd(const nerfb200_arch_t* arch, const float* blob, const f
 int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const float* rays, int32_t ray_stride,
                          const float* z, int64_t n_rays, int32_t n_samples, const float* d_raw,
                          const float* stash, float* gstash, float* flat_grad, int32_t impl, void* stream) {
+  if (impl == 3) return refuse_fast("mlp_bwd");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   NB_TRY(check_mlp_args(p, blob, rays, ray_stride, z, n_rays, n_samples));
@@ -442,6 +458,7 @@ int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const f
 
 int32_t nerfb200_mlp_dgrad(const nerfb200_arch_t* arch, const float* blob, const float* d_raw, const float* stash,
                            float* gstash, int64_t n_points, int32_t impl, void* stream) {
+  if (impl == 3) return refuse_fast("mlp_dgrad");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   if (!blob || !d_raw || !stash || !gstash || n_points <= 0) {
@@ -454,6 +471,7 @@ int32_t nerfb200_mlp_dgrad(const nerfb200_arch_t* arch, const float* blob, const
 int32_t nerfb200_mlp_wgrad(const nerfb200_arch_t* arch, const float* rays, int32_t ray_stride, const float* z,
                            int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash,
                            const float* gstash, float* flat_grad, int32_t impl, void* stream) {
+  if (impl == 3) return refuse_fast("mlp_wgrad");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   if (!rays || !z || !d_raw || !stash || !gstash || !flat_grad || n_rays <= 0 || n_samples <= 0) {
@@ -579,6 +597,7 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
                             float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
                             void* stream) {
+  if (impl == 3 && training) return refuse_fast("render_fwd with training = 1");
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
@@ -614,6 +633,8 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
   if (impl == 1)
     NB_TRY(launch_mlp_fwd_tc(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
+  else if (impl == 3)
+    NB_TRY(launch_mlp_fwd_tc_fast(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), s));
   else
     NB_TRY(launch_mlp_fwd_simt(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
   NB_TRY(launch_composite_fwd(F(w.raw_c), F(w.z_c), rays, ray_stride, rnd[kRandNoiseC], n_rays, nc, opts->noise_std,
@@ -627,6 +648,8 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
   if (impl == 1)
     NB_TRY(launch_mlp_fwd_tc(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
+  else if (impl == 3)
+    NB_TRY(launch_mlp_fwd_tc_fast(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), s));
   else
     NB_TRY(launch_mlp_fwd_simt(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
   NB_TRY(launch_composite_fwd(F(w.raw_f), F(w.z_f), rays, ray_stride, rnd[kRandNoiseF], n_rays, ns, opts->noise_std,
@@ -640,6 +663,7 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* noise_c, const float* noise_f, const float* g_coarse, const float* g_fine,
                             void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
                             void* stream) {
+  if (impl == 3) return refuse_fast("render_bwd");
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));

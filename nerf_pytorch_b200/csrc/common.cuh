@@ -146,7 +146,11 @@ int launch_mlp_wgrad(const Plan& p, const float* rays, int ray_stride, const flo
 int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
                       const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
 int64_t bwd_tc_scratch_floats(const Plan& p);
-int tc_supported(const Plan& p, int n_samples, const char* what, bool training);  // forward (training: + stash)
+// forward (training: + stash; fast: the single-pass inference forward, impl 3)
+int tc_supported(const Plan& p, int n_samples, const char* what, bool training, bool fast = false);
+// single-pass fp16 wgmma forward (mlp_tc.cu, kFast): inference only, no stash
+int launch_mlp_fwd_tc_fast(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                           int64_t n_rays, int n_samples, float* raw, cudaStream_t s);
 int bwd_tc_supported(const Plan& p, int n_samples, const char* what);  // forward + backward
 int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,

@@ -22,6 +22,13 @@
 //              complete_tx; a stage is free again once every consumer warp has seen its MMAs complete.
 // The direction encoding enters layers_dir[0] through a per-ray fp32 bias computed on the CUDA cores (it is constant
 // along a ray: SURVEY.md section 7.3 item 5), so that layer contracts over K = H only.
+//
+// Single-pass variant (kFast, inference only, impl 3): one wgmma per k-step, a_hi * hs, against the hs = fp16(w) 2^11
+// copy the blob already holds, so the accumulator sits at the same 2^11 scale and bias, ReLU, heads and the per-ray
+// view bias are unchanged.  Products are fp16(activation / 16) * fp16(w) with fp32 accumulation (~11 significant bits
+// per operand instead of 22); the heads and the direction term stay fp32.  The producer streams only the hs part of
+// each k-step (32 n bytes, contiguous in the blob) and packs kStageBytes / (32 n) k-steps into a ring stage; the
+// prologue and the epilogue write only the hi half of the operand tiles.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "wgmma.cuh"
@@ -67,16 +74,19 @@ struct MmaInfo {
   const uint8_t* src;   // blob copy of the layer's weights (three fp16 copies, k-step major)
   uint32_t kbytes;      // bytes of one k-step
   int ksteps, ksteps_h; // k-steps, of which the first ksteps_h read the activation tile (the rest: encodings)
-  int sps;              // k-steps per ring stage (a stage holds 24 KB: two k-steps at N <= 128, one at N = 256)
+  int sps;              // k-steps per ring stage (a stage holds 24 KB: two k-steps at N <= 128, one at N = 256;
+                        // single-pass: fast_sps(n) hs parts)
 };
-__device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, int e) {
+// single pass: k-steps per ring stage, each the 32 n bytes of its hs copy (12 at N = 64, 6 at 128, 3 at 256)
+__host__ __device__ constexpr int fast_sps(int n) { return kStageBytes / (32 * n); }
+__device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, int e, bool fast) {
   MmaInfo mi;
   const GemmLayer& g = p.g[e];
   mi.src = reinterpret_cast<const uint8_t*>(blob + g.tc_off);
   mi.ksteps = (g.k_tc + 15) >> 4;
   mi.ksteps_h = g.k_h >> 4;
   mi.kbytes = 96u * (uint32_t)g.n;
-  mi.sps = g.n > 128 ? 1 : kStepsPerStage;
+  mi.sps = fast ? fast_sps(g.n) : g.n > 128 ? 1 : kStepsPerStage;
   return mi;
 }
 
@@ -100,15 +110,17 @@ struct RowState {
 // One layer of one warpgroup: MMAs over the ring, then the epilogue on the accumulator fragment.
 // Fragment of wgmma m64nN (per warp 16 rows): thread (warp wi, lane) holds rows r = 16 wi + lane / 4 (+ 8) and columns
 // 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row r + 8 i, column 8 j + 2 (lane % 4) + c).
-template <bool kTrain, int N>
+template <bool kTrain, bool kFast, int N>
 __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, float* __restrict__ raw, float* __restrict__ stash,
                                           uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t tile,
                                           int64_t P_pad, const RowState& rs, Pipe2& pl, uint32_t bar_full,
                                           uint32_t bar_empty, uint32_t n_stages, const float* s_bias, const float* s_headw,
                                           const float* s_headb, const float* viewb, int hw1) {
+  static_assert(!(kTrain && kFast), "the single-pass forward is inference only");
+  constexpr int kSps = kFast ? fast_sps(N) : kStepsPerStage;  // k-steps a ring stage can hold
   const int wt = threadIdx.x & 127, wi = wt >> 5, lane = wt & 31, q = lane & 3;
   const GemmLayer& g = p.g[e];
-  const MmaInfo mi = mma_info(p, blob, e);
+  const MmaInfo mi = mma_info(p, blob, e, kFast);
   const int enc_w = p.enc_tile_w;
   const uint32_t act_a = smem_u32(sm + mp.act), enc_a = smem_u32(sm + mp.enc), ring_a = smem_u32(sm + mp.ring);
   const int fin = g.k_h > 0 ? g.k_h : 16;
@@ -129,11 +141,11 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
     mbar_wait(bar_full + 8 * st, pl.pp.phase);
     const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStageBytes);
 #pragma unroll
-    for (int hh = 0; hh < kStepsPerStage; ++hh) {
+    for (int hh = 0; hh < kSps; ++hh) {
       const int ks = ks0 + hh;
       if (hh < mi.sps && ks < mi.ksteps) {
-        const uint64_t b_hs = desc_adv(b_st, hh * 6 * slab_b);
-        const uint64_t b_h = desc_adv(b_hs, 2 * slab_b), b_l = desc_adv(b_hs, 4 * slab_b);
+        // a stage holds per k-step [hs | h | l][2 slabs], or [hs][2 slabs] alone in the single pass
+        const uint64_t b_hs = desc_adv(b_st, hh * (kFast ? 2 : 6) * slab_b);
         uint64_t ah, al;
         if (ks < mi.ksteps_h) {
           ah = desc_adv(a_hi0, (uint32_t)ks * 256u);
@@ -143,8 +155,11 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
           al = desc_adv(ah, e_lo_off);
         }
         wgmma_f16<N>(acc, ah, b_hs, ks > 0 ? 1 : 0);
-        wgmma_f16<N>(acc, al, b_h, 1);
-        wgmma_f16<N>(acc, ah, b_l, 1);
+        if (!kFast) {
+          const uint64_t b_h = desc_adv(b_hs, 2 * slab_b), b_l = desc_adv(b_hs, 4 * slab_b);
+          wgmma_f16<N>(acc, al, b_h, 1);
+          wgmma_f16<N>(acc, ah, b_l, 1);
+        }
       }
     }
     wgmma_commit();
@@ -207,7 +222,10 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
       }
       if (kTrain)  // ReLU bits (Y >= 0 here: Y > 0 <=> a nonzero bit pattern)
         mbits[i][j >> 2] |= (min(__float_as_uint(Y0), 1u) | (min(__float_as_uint(Y1), 1u) << 1)) << (8 * (j & 3) + 2 * q);
-      if (has_next || kTrain) {
+      if (kFast) {
+        if (has_next)
+          *reinterpret_cast<uint32_t*>(act + tile_piece(r0 + 8 * i, j, N) + q * 4) = f16x2_hi(x0, x1);
+      } else if (has_next || kTrain) {
         uint32_t hi, lo;
         split_f16x2_y(Y0, Y1, x0, x1, hi, lo);
         const int off = tile_piece(r0 + 8 * i, j, N) + q * 4;
@@ -256,7 +274,8 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
 
 // kTrain: the forward also writes the activation stash (operand tiles + ReLU bit masks + the encoding tile).
 // kH = hidden size (compile-time: the accumulator width and the warpgroup count fold into constants)
-template <bool kTrain, int kH>
+// kFast: the single-pass fp16 products (inference only, see the file header)
+template <bool kTrain, int kH, bool kFast>
 __global__ void __launch_bounds__(128 * (kH == 128 ? 2 : 1) + 32, 1)
 mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ z, int64_t P, int S, int64_t n_tiles,
@@ -316,8 +335,19 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       const uint32_t ring_a = smem_u32(sm + mp.ring);
       for (int j = 0; j < my_tiles; ++j)
         for (int e = 0; e < p.n_gemm; ++e) {
-          const MmaInfo mi = mma_info(p, blob, e);
+          const MmaInfo mi = mma_info(p, blob, e, kFast);
           for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
+            if (kFast) {  // the hs part of each k-step: one bulk copy each, their sum on the stage's barrier
+              const int nk = min(mi.sps, mi.ksteps - ks);
+              const uint32_t hs_bytes = mi.kbytes / 3, full = bar_full + 8 * pp.stage;
+              mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1);
+              mbar_arrive_expect_tx(full, (uint32_t)nk * hs_bytes);
+              for (int hh = 0; hh < nk; ++hh)
+                bulk_g2s_hint(ring_a + pp.stage * kStageBytes + hh * hs_bytes, mi.src + (size_t)(ks + hh) * mi.kbytes,
+                              hs_bytes, full, pol);
+              pp.advance(n_stages);
+              continue;
+            }
             const uint32_t bytes = (uint32_t)min(mi.sps, mi.ksteps - ks) * mi.kbytes;
             mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1);
             mbar_arrive_expect_tx(bar_full + 8 * pp.stage, bytes);
@@ -369,11 +399,14 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
         const int base = p.inc_xyz ? 3 : 0;
         const int trow = 64 * wg + row;
         auto put = [&](int k, float v) {
-          uint32_t hi, lo;
-          split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
+          uint32_t hi, lo = 0;
+          if (kFast)
+            hi = f16x2_hi(v * kActScale, 0.f);
+          else
+            split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
           const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
           *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
-          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
+          if (!kFast) *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
         };
         for (int c = 0; c < 3; ++c) {
           const float x = __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));  // pts = ro + rd * z (train_utils.py:67)
@@ -415,11 +448,11 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll 1
       for (int e = 0; e < p.n_gemm; ++e) {
         if (p.g[e].n == kH)
-          fwd_layer<kTrain, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full, bar_empty,
-                                n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+          fwd_layer<kTrain, kFast, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full,
+                                       bar_empty, n_stages, s_bias, s_headw, s_headb, viewb, hw1);
         else
-          fwd_layer<kTrain, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full, bar_empty,
-                                    n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+          fwd_layer<kTrain, kFast, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full,
+                                           bar_empty, n_stages, s_bias, s_headw, s_headb, viewb, hw1);
       }
     }
     if (kTrain && wt == 0) bulk_wait_all();  // this warpgroup's encoding-tile stores
@@ -428,29 +461,31 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 
 // training = the forward must also write the activation stash for the fused backward (hidden 128 only); the
 // inference forward also runs hidden 256 (one warpgroup, 64-point tiles, N = 256 MMAs)
-int tc_supported(const Plan& p, int n_samples, const char* what, bool training) {
+// fast: the single-pass forward (impl 3), accepted exactly where the inference forward is
+int tc_supported(const Plan& p, int n_samples, const char* what, bool training, bool fast) {
+  const char* impl = fast ? "impl=3 (single-pass fp16 wgmma)" : "impl=1 (wgmma)";
   if (p.hidden != 128 && (training || p.hidden != 256)) {
-    set_error("%s impl=1 (wgmma): hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
-              p.hidden);
+    set_error("%s %s: hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
+              impl, p.hidden);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (p.dim_xyz_pad > 64 || p.dim_dir > 32) {
-    set_error("%s impl=1 (wgmma): encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what);
+    set_error("%s %s: encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what, impl);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (n_samples > 0 && (kTileRows + n_samples - 1) / n_samples + 1 > kMaxRaysPerTile) {
-    set_error("%s impl=1 (wgmma): fewer than 15 samples per ray not supported; use impl=0", what);
+    set_error("%s %s: fewer than 15 samples per ray not supported; use impl=0", what, impl);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map(p).n_stages < 2) {
-    set_error("%s impl=1 (wgmma): network too deep for the shared-memory budget (%d layers); use impl=0", what,
-              p.n_gemm);
+    set_error("%s %s: network too deep for the shared-memory budget (%d layers); use impl=0", what,
+              impl, p.n_gemm);
     return NERFB200_ERR_UNSUPPORTED;
   }
   return NERFB200_OK;
 }
 
-template <bool kTrain, int kH>
+template <bool kTrain, int kH, bool kFast>
 static int launch_fwd(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z, int64_t P,
                       int n_samples, float* raw, float* stash, cudaStream_t s, const char* what) {
   constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
@@ -459,7 +494,7 @@ static int launch_fwd(const Plan& p, const float* blob, const float* rays, int r
   const int sms = device_sms();
   const int grid = (int)(tiles < sms ? tiles : sms);
   const size_t bytes = (size_t)smem_map(p).total + 1024;
-  auto kern = mlp_fwd_tc_kernel<kTrain, kH>;
+  auto kern = mlp_fwd_tc_kernel<kTrain, kH, kFast>;
   int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes), what);
   if (rc) return rc;
   kern<<<grid, kThreads, bytes, s>>>(p, blob, rays, ray_stride, z, P, n_samples, kTrain ? stash_tiles : tiles, raw, stash);
@@ -472,13 +507,24 @@ int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int r
   int rc = tc_supported(p, n_samples, "mlp_fwd", stash != nullptr);
   if (rc) return rc;
   if (stash)
-    return launch_fwd<true, 128>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, stash, s,
-                                 "mlp_fwd_tc launch");
+    return launch_fwd<true, 128, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, stash, s,
+                                        "mlp_fwd_tc launch");
   if (p.hidden == 256)
-    return launch_fwd<false, 256>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                  "mlp_fwd_tc launch");
-  return launch_fwd<false, 128>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                "mlp_fwd_tc launch");
+    return launch_fwd<false, 256, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
+                                         "mlp_fwd_tc launch");
+  return launch_fwd<false, 128, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
+                                       "mlp_fwd_tc launch");
+}
+
+int launch_mlp_fwd_tc_fast(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                           int64_t n_rays, int n_samples, float* raw, cudaStream_t s) {
+  int rc = tc_supported(p, n_samples, "mlp_fwd", /*training=*/false, /*fast=*/true);
+  if (rc) return rc;
+  if (p.hidden == 256)
+    return launch_fwd<false, 256, true>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
+                                        "mlp_fwd_tc_fast launch");
+  return launch_fwd<false, 128, true>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
+                                      "mlp_fwd_tc_fast launch");
 }
 
 }  // namespace nerfb200

@@ -125,6 +125,12 @@ __device__ __forceinline__ void split_f16x2_y(float Y0, float Y1, float x0, floa
   const float r0 = fmaf(h0, -kLoScale, Y0), r1 = fmaf(h1, -kLoScale, Y1);
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(r1), "f"(r0));
 }
+// hi = fp16(x) alone (same packing): the operand of the single-pass forward, which drops the lo half
+__device__ __forceinline__ uint32_t f16x2_hi(float x0, float x1) {
+  uint32_t hi;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hi) : "f"(x1), "f"(x0));
+  return hi;
+}
 // the three weight copies of one pair (same packing)
 __device__ __forceinline__ void split_w3(float w0, float w1, uint32_t& hs, uint32_t& h, uint32_t& l) {
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(h) : "f"(w1), "f"(w0));

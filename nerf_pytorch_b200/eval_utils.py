@@ -26,7 +26,10 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
     need no small chunks, an H100's 80 GB of HBM hold a whole 800 x 800 image's intermediates).
 
     ``randoms``: a ``SeededRandoms`` makes a render with ``perturb`` or noise on reproducible: pixel ``j * width + i`` is
-    ray ``ray_offset + j * width + i`` of the seeded stream whatever the chunk size.  Default: torch draws per chunk."""
+    ray ``ray_offset + j * width + i`` of the seeded stream whatever the chunk size.  Default: torch draws per chunk.
+
+    ``impl=ops.IMPL_TC_FAST`` renders with the single-pass fp16 wgmma forward (INTEGRATION.md, "Optional fast paths"):
+    fewer MMAs, fp16 operands, judged by PSNR against the default path rather than by parity with it."""
     if randoms is not None and not isinstance(randoms, SeededRandoms):
         raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:

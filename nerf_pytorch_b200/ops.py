@@ -17,6 +17,10 @@ from ._lib import Arch, RenderOpts, Rng
 IMPL_SIMT = 0  # fp32 CUDA cores
 IMPL_TC = 1    # wgmma tensor cores (fp16x2 three-term splits, fp32 accumulation)
 IMPL_TC_FWD = 2  # query only (impl_supported): the wgmma forward alone (inference), which also runs hidden 256
+# inference only: single-pass fp16 wgmma forward (one fp16(w) x fp16(activation / 16) product per k-step, fp32
+# accumulation); ~3x fewer MMAs than IMPL_TC at ~11 significant bits per operand.  Renders, never trains; never chosen
+# automatically.  Accepted exactly where IMPL_TC_FWD is.
+IMPL_TC_FAST = 3
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -276,8 +280,10 @@ def mlp_bwd(arch: ArchSpec, blob, rays, z, d_raw, stash, impl=IMPL_SIMT, flat_gr
     scratch): scratch is the gradient stash for impl 0, the gradient blob for impl 1."""
     lib = _lib.load()
     n, s = z.shape
-    gstash = torch.empty(lib.nerfb200_bwd_scratch_floats(C.byref(arch.c_struct()), n * s, impl), dtype=torch.float32,
-                         device=z.device)
+    n_scratch = lib.nerfb200_bwd_scratch_floats(C.byref(arch.c_struct()), n * s, impl)
+    if n_scratch < 0 and impl == IMPL_TC_FAST:
+        _lib.check(_lib.ERR_UNSUPPORTED, "mlp_bwd")  # the library's refusal: the single-pass forward does not train
+    gstash = torch.empty(n_scratch, dtype=torch.float32, device=z.device)
     if flat_grad is None:
         flat_grad = torch.zeros(arch.flat_param_count(), dtype=torch.float32, device=z.device)
     _lib.check(lib.nerfb200_mlp_bwd(C.byref(arch.c_struct()), _ptr(blob), _ptr(rays), rays.shape[1], _ptr(z), n, s,

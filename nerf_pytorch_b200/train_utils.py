@@ -30,6 +30,7 @@ COMPAT_MODE_QUIRK = True
 
 # None: wgmma tensor cores (three-term split-precision products) wherever the kernels support the configuration (training: hidden
 # 128; inference: hidden 128 or 256; encodings <= 64 wide, >= 15 samples per ray), fp32 CUDA cores otherwise; 0 / 1 force one.
+# 3 (ops.IMPL_TC_FAST, single-pass fp16 products) is for renders only: a call that would train with it raises.
 DEFAULT_IMPL = None
 
 
@@ -44,6 +45,18 @@ _GRAD_SYNC = None
 # set when a step rendered its rays in several chunks: their gradients are summed by autograd first and
 # all-reduced ONCE afterwards (parallel.sync_gradients / FusedAdam.step), never once per chunk
 _PENDING_SYNC = False
+
+
+def _refuse_fast_training(impl, *models):
+    """ops.IMPL_TC_FAST renders only (no stash, no backward): a call that would train with it (grad enabled and
+    parameters that require grad) raises here, before anything is launched."""
+    if impl is None:
+        impl = DEFAULT_IMPL
+    if impl is None or int(impl) != ops.IMPL_TC_FAST or not torch.is_grad_enabled():
+        return
+    if any(p.requires_grad for m in models if m is not None for p in m.parameters()):
+        raise NotImplementedError("nerfb200: impl=3 (single-pass fp16 wgmma forward) is inference only; train with "
+                                  "impl=0 or impl=1, or render under torch.no_grad()")
 
 
 def set_default_impl(impl):
@@ -297,7 +310,11 @@ def predict_and_render_radiance(
     ``randoms`` (keyword-only, optional) injects the four random tensors the reference would draw
     (t_rand, noise_c, u, noise_f); by default they are drawn here with torch.rand/randn in the
     reference's order.  A ``SeededRandoms`` instead has the kernels generate them from its seed, step and
-    ``ray_offset`` (the global index of ``ray_batch[0]``): no torch random number is drawn."""
+    ``ray_offset`` (the global index of ``ray_batch[0]``): no torch random number is drawn.
+
+    ``impl``: None picks the kernels (``DEFAULT_IMPL``, else the automatic choice); ``ops.IMPL_TC_FAST`` renders with
+    the single-pass fp16 forward and raises ``NotImplementedError`` if the call would train."""
+    _refuse_fast_training(impl, model_coarse, model_fine)
     o = getattr(options.nerf, mode)
     if not ray_batch.is_cuda:
         raise NotImplementedError("nerfb200: rays must be on a CUDA device (there is no CPU path)")
@@ -374,6 +391,7 @@ def run_one_iter_of_nerf(
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
     the reshape back to image shape."""
+    _refuse_fast_training(impl, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     restore_shapes = [ray_directions.shape, ray_directions.shape[:-1], ray_directions.shape[:-1]]
     if model_fine:
@@ -411,6 +429,7 @@ def run_one_iter_of_nerf_from_pose(
     thousand it samples (train_nerf.py:196-226); here the rays of exactly those pixels are generated on the device
     (csrc/raygen.cu) in the packed layout the render kernels read.  ``pixel_ids``: int64, ``j * width + i``, on the
     target device (None = the whole image, returned image-shaped in "validation" mode)."""
+    _refuse_fast_training(impl, model_coarse, model_fine)
     dev = pixel_ids.device if pixel_ids is not None else next(model_coarse.parameters()).device
     use_viewdirs = bool(options.nerf.use_viewdirs)
     rays = ops.gen_rays(tform_cam2world, height, width, focal_length, pixel_ids, dev, ndc=options.dataset.no_ndc is False,
