@@ -69,9 +69,11 @@ int64_t nerfb200_launch_count(void);
  * weight-gradient job, the ReLU bit masks and d_raw -- the algorithmic traffic of its roofline */
 int64_t nerfb200_bwd_bytes_per_point(const nerfb200_arch_t* arch);
 /* NERFB200_OK if `impl` (0 fp32 CUDA cores, 1 wgmma) can run this architecture forward AND backward with
- * n_samples samples per ray, else NERFB200_ERR_UNSUPPORTED (reason in nerfb200_last_error()).  impl = 2 asks for the
- * wgmma FORWARD alone (inference: training = 0 in render_fwd / stash = NULL in mlp_fwd with impl = 1), which also
- * covers hidden_size 256.  impl = 3 (the single-pass fp16 forward, see nerfb200_mlp_fwd) gives the same answer as 2. */
+ * n_samples samples per ray, else NERFB200_ERR_UNSUPPORTED (reason in nerfb200_last_error()); impl 0 refuses only
+ * networks whose forward tiles exceed shared memory.  impl = 2 asks for the wgmma FORWARD alone (inference:
+ * training = 0 in render_fwd / stash = NULL in mlp_fwd with impl = 1), which also covers hidden_size 256.  impl = 3
+ * (the single-pass fp16 forward, see nerfb200_mlp_fwd) gives the same answer as 2.  Any other code:
+ * NERFB200_ERR_INVALID. */
 int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, int32_t impl);
 
 /* ---- parameters -------------------------------------------------------------------------------
@@ -163,7 +165,8 @@ int32_t nerfb200_sample_pdf_merge(const float* z_coarse, const float* weights_co
 
 /* Backward of nerfb200_mlp_fwd w.r.t. the parameters.  d_raw[n_points][4]; stash from the forward (same impl).
  * gstash: scratch fp32[nerfb200_bwd_scratch_floats(arch, n_points, impl)] (impl 0: the per-layer gradient stash;
- * impl 1: the L2-resident gradient blob the fused kernel reduces its weight-gradient tiles into).
+ * impl 1: the L2-resident gradient blob the fused kernel reduces its weight-gradient tiles into; -1 where the
+ * backward refuses the impl, reason in nerfb200_last_error()).
  * flat_grad: fp32[flat_param_count], ACCUMULATED into (zero it first).  Gradients w.r.t. rays / z are not
  * produced (the reference detaches the fine depths, train_utils.py:103, and rays are data). */
 int64_t nerfb200_bwd_scratch_floats(const nerfb200_arch_t* arch, int64_t n_points, int32_t impl);
@@ -222,8 +225,9 @@ int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64
  * u must then be given, a noise tensor left NULL means no noise.  render_bwd needs the noise again for the sigma ReLU gate: pass it the same *rng,
  * or the same noise tensors, as the render_fwd call that filled the workspace (seeded, it reads no noise tensor).
  * render_fwd: out_coarse/out_fine[n][8] = [r g b disp acc depth 0 0] (out_fine NULL when n_fine == 0).
- *   impl: the MLP kernels as in nerfb200_mlp_fwd (1 wgmma, 3 single-pass fp16 wgmma, anything else fp32 CUDA cores);
- *   impl 3 renders only: training = 1 is refused with NERFB200_ERR_UNSUPPORTED.
+ *   impl: the MLP kernels as in nerfb200_mlp_fwd (0 fp32 CUDA cores, 1 wgmma, 3 single-pass fp16 wgmma; any other
+ *   code is NERFB200_ERR_INVALID); impl 3 renders only: training = 1 is refused with NERFB200_ERR_UNSUPPORTED.
+ *   Both calls check every network they will run before their first launch, so a refusal writes nothing.
  *   workspace: nerfb200_render_workspace_bytes(...) bytes; keeps z/raw/stash for render_bwd.
  * render_bwd: g_coarse/g_fine[n][8] upstream grads (g_fine NULL when no fine pass); accumulates into flat_grad_c /
  *   flat_grad_f (may alias different ranges of one buffer).  parts: bit 0 = the fine network's backward, bit 1 = the

@@ -7,7 +7,12 @@
 #include <atomic>
 
 #include "common.cuh"
-#include "wgrad_items.cuh"
+
+#define NB_TRY(expr)                    \
+  do {                                  \
+    int _rc = (expr);                   \
+    if (_rc != NERFB200_OK) return _rc; \
+  } while (0)
 
 namespace nerfb200 {
 
@@ -192,6 +197,9 @@ static bool slot_lookup(const Plan& p, int slot, bool* is_head, int* idx) {
 
 static inline int64_t align256(int64_t bytes) { return (bytes + 255) & ~int64_t(255); }
 
+// activation stash of n points: whole 128-point tiles (the wgmma path stores tiles)
+static inline int64_t stash_floats(const Plan& p, int64_t n) { return ((n + 127) & ~int64_t(127)) * p.sum_n; }
+
 struct Workspace {
   int64_t z_c, raw_c, w_c, z_f, raw_f, stash_c, stash_f, gstash, d_raw, total;
 };
@@ -212,9 +220,8 @@ static void carve(const Plan& pc, const Plan* pf, const nerfb200_render_opts_t& 
   w->z_f = take(fine ? n * ns : 0);
   w->raw_f = take(fine ? n * ns * 4 : 0);
   if (training) {
-    auto pad128 = [](int64_t v) { return (v + 127) & ~int64_t(127); };
-    const int64_t sc = pad128(n * nc) * pc.sum_n;
-    const int64_t sf = fine ? pad128(n * ns) * pf->sum_n : 0;
+    const int64_t sc = stash_floats(pc, n * nc);
+    const int64_t sf = fine ? stash_floats(*pf, n * ns) : 0;
     w->stash_c = take(sc);
     w->stash_f = take(sf);
     // backward scratch: the gradient stash of the CUDA-core path / the gradient blob of the wgmma path
@@ -231,10 +238,60 @@ static void carve(const Plan& pc, const Plan* pf, const nerfb200_render_opts_t& 
   w->total = off;
 }
 
-// impl 3, the single-pass fp16 wgmma forward, renders images; every entry point that trains refuses it
-static int refuse_fast(const char* what) {
-  set_error("%s: impl=3 (single-pass fp16 wgmma forward) is inference only; train with impl=0 or impl=1", what);
-  return NERFB200_ERR_UNSUPPORTED;
+// What a call needs of the MLP kernels it selects with `impl`.
+enum Need {
+  kInference,  // the forward alone: render_fwd(training = 0), mlp_fwd without a stash
+  kStash,      // the forward that writes the activation stash a backward reads
+  kBackward,   // the backward (its forward has run)
+  kHalves,     // the backward as two calls, mlp_dgrad and mlp_wgrad: the fp32 kernels only
+};
+
+// The one place that maps an impl code to the kernel families' predicates: 0 the fp32 CUDA cores, 1 wgmma, 3 the
+// single-pass fp16 wgmma forward, which renders only.  Every other code is refused (2 is a query of impl_supported,
+// not a family).  A refusal reads "<what> impl=N (<label>): <reason>".
+static int check_impl(const Plan& p, int impl, int n_samples, Need need, const char* what) {
+  char who[96];
+  switch (impl) {
+    case 0:
+      snprintf(who, sizeof(who), "%s impl=0 (fp32 CUDA cores)", what);
+      return simt_supported(p, who);
+    case 1:
+      if (need == kHalves) {
+        set_error("%s: impl=1 (wgmma) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd", what);
+        return NERFB200_ERR_UNSUPPORTED;
+      }
+      snprintf(who, sizeof(who), "%s impl=1 (wgmma)", what);
+      NB_TRY(tc_supported(p, n_samples, /*training=*/need != kInference, who));
+      return need == kBackward ? bwd_tc_supported(p, who) : NERFB200_OK;
+    case 3:
+      if (need != kInference) {
+        set_error("%s: impl=3 (single-pass fp16 wgmma forward) is inference only; train with impl=0 or impl=1", what);
+        return NERFB200_ERR_UNSUPPORTED;
+      }
+      snprintf(who, sizeof(who), "%s impl=3 (single-pass fp16 wgmma)", what);
+      return tc_supported(p, n_samples, /*training=*/false, who);
+    default:
+      set_error("%s: unknown impl %d", what, impl);
+      return NERFB200_ERR_INVALID;
+  }
+}
+
+// The MLP forward of one network on the kernels check_impl accepted; a non-null stash is written for the backward.
+static int mlp_forward(const Plan& p, int impl, const float* blob, const float* rays, int ray_stride, const float* z,
+                       int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s) {
+  if (impl == 0) return launch_mlp_fwd_simt(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
+  return launch_mlp_fwd_tc(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, /*fast=*/impl == 3, s);
+}
+
+// Its backward, accumulated into flat_grad.  gstash: impl 0 the gradient stash, impl 1 the gradient blob.
+static int mlp_backward(const Plan& p, int impl, const float* blob, const float* rays, int ray_stride, const float* z,
+                        int64_t n_rays, int n_samples, const float* d_raw, const float* stash, float* gstash,
+                        float* flat_grad, cudaStream_t s) {
+  if (impl == 1)
+    return launch_mlp_bwd_tc(p, blob, rays, ray_stride, n_rays, n_samples, d_raw, stash, gstash, flat_grad, s);
+  const int64_t P = n_rays * n_samples;
+  NB_TRY(launch_dgrad_simt(p, blob, d_raw, stash, gstash, P, s));
+  return launch_wgrad_simt(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, P, flat_grad, s);
 }
 
 static int check_opts(const nerfb200_render_opts_t* o) {
@@ -258,12 +315,6 @@ static int check_opts(const nerfb200_render_opts_t* o) {
 
 using namespace nerfb200;
 
-#define NB_TRY(expr)                    \
-  do {                                  \
-    int _rc = (expr);                   \
-    if (_rc != NERFB200_OK) return _rc; \
-  } while (0)
-
 extern "C" {
 
 int32_t nerfb200_version(void) { return NERFB200_VERSION; }
@@ -286,23 +337,16 @@ int64_t nerfb200_bwd_bytes_per_point(const nerfb200_arch_t* arch) {
 int32_t nerfb200_impl_supported(const nerfb200_arch_t* arch, int32_t n_samples, int32_t impl) {
   Plan p;
   NB_TRY(build_plan(arch, &p));
-  if (impl == 0) return NERFB200_OK;
-  if (impl == 1) return bwd_tc_supported(p, n_samples, "impl_supported");
-  if (impl == 2) return tc_supported(p, n_samples, "impl_supported", /*training=*/false);  // wgmma forward only (inference)
-  if (impl == 3) return tc_supported(p, n_samples, "impl_supported", /*training=*/false, /*fast=*/true);
-  set_error("unknown impl %d", impl);
-  return NERFB200_ERR_INVALID;
+  if (impl == 2) return check_impl(p, 1, n_samples, kInference, "impl_supported");  // the wgmma forward alone
+  return check_impl(p, impl, n_samples, impl == 3 ? kInference : kBackward, "impl_supported");
 }
 
 int64_t nerfb200_bwd_scratch_floats(const nerfb200_arch_t* arch, int64_t n_points, int32_t impl) {
   Plan p;
-  if (build_plan(arch, &p) != NERFB200_OK || n_points < 0) return -1;
-  if (impl == 3) {
-    refuse_fast("bwd_scratch_floats");
+  if (build_plan(arch, &p) != NERFB200_OK || n_points < 0 ||
+      check_impl(p, impl, 0, kBackward, "bwd_scratch_floats") != NERFB200_OK)
     return -1;
-  }
-  if (impl == 1) return bwd_tc_scratch_floats(p);
-  return ((n_points + 127) & ~int64_t(127)) * p.sum_n;
+  return impl == 1 ? bwd_tc_scratch_floats(p) : stash_floats(p, n_points);
 }
 
 int64_t nerfb200_num_linear(const nerfb200_arch_t* arch) {
@@ -323,7 +367,7 @@ int64_t nerfb200_blob_floats(const nerfb200_arch_t* arch) {
 int64_t nerfb200_stash_floats(const nerfb200_arch_t* arch, int64_t n_points) {
   Plan p;
   if (build_plan(arch, &p) != NERFB200_OK || n_points < 0) return -1;
-  return ((n_points + 127) & ~int64_t(127)) * p.sum_n;  // whole 128-point tiles (the wgmma path stores tiles)
+  return stash_floats(p, n_points);
 }
 
 int32_t nerfb200_flat_layout(const nerfb200_arch_t* arch, int32_t slot, int64_t* w_off, int64_t* b_off,
@@ -430,21 +474,14 @@ int32_t nerfb200_mlp_fwd(const nerfb200_arch_t* arch, const float* blob, const f
     set_error("mlp_fwd: null output");
     return NERFB200_ERR_INVALID;
   }
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (impl == 0) return launch_mlp_fwd_simt(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
-  if (impl == 1) return launch_mlp_fwd_tc(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
-  if (impl == 3) {
-    if (stash) return refuse_fast("mlp_fwd with a stash");
-    return launch_mlp_fwd_tc_fast(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, s);
-  }
-  set_error("mlp_fwd: unknown impl %d", impl);
-  return NERFB200_ERR_INVALID;
+  NB_TRY(check_impl(p, impl, n_samples, stash ? kStash : kInference, "mlp_fwd"));
+  return mlp_forward(p, impl, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash,
+                     static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const float* rays, int32_t ray_stride,
                          const float* z, int64_t n_rays, int32_t n_samples, const float* d_raw,
                          const float* stash, float* gstash, float* flat_grad, int32_t impl, void* stream) {
-  if (impl == 3) return refuse_fast("mlp_bwd");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   NB_TRY(check_mlp_args(p, blob, rays, ray_stride, z, n_rays, n_samples));
@@ -452,34 +489,35 @@ int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const f
     set_error("mlp_bwd: null pointer");
     return NERFB200_ERR_INVALID;
   }
-  return launch_mlp_bwd(p, blob, rays, ray_stride, z, n_rays, n_samples, d_raw, stash, gstash, flat_grad, impl,
-                        static_cast<cudaStream_t>(stream));
+  NB_TRY(check_impl(p, impl, n_samples, kBackward, "mlp_bwd"));
+  return mlp_backward(p, impl, blob, rays, ray_stride, z, n_rays, n_samples, d_raw, stash, gstash, flat_grad,
+                      static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_mlp_dgrad(const nerfb200_arch_t* arch, const float* blob, const float* d_raw, const float* stash,
                            float* gstash, int64_t n_points, int32_t impl, void* stream) {
-  if (impl == 3) return refuse_fast("mlp_dgrad");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   if (!blob || !d_raw || !stash || !gstash || n_points <= 0) {
     set_error("mlp_dgrad: null pointer or empty input");
     return NERFB200_ERR_INVALID;
   }
-  return launch_mlp_dgrad(p, blob, d_raw, stash, gstash, n_points, impl, static_cast<cudaStream_t>(stream));
+  NB_TRY(check_impl(p, impl, 0, kHalves, "mlp_dgrad"));
+  return launch_dgrad_simt(p, blob, d_raw, stash, gstash, n_points, static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_mlp_wgrad(const nerfb200_arch_t* arch, const float* rays, int32_t ray_stride, const float* z,
                            int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash,
                            const float* gstash, float* flat_grad, int32_t impl, void* stream) {
-  if (impl == 3) return refuse_fast("mlp_wgrad");
   Plan p;
   NB_TRY(build_plan(arch, &p));
   if (!rays || !z || !d_raw || !stash || !gstash || !flat_grad || n_rays <= 0 || n_samples <= 0) {
     set_error("mlp_wgrad: null pointer or empty input");
     return NERFB200_ERR_INVALID;
   }
-  return launch_mlp_wgrad(p, rays, ray_stride, z, n_rays, n_samples, d_raw, stash, gstash, flat_grad, impl,
-                          static_cast<cudaStream_t>(stream));
+  NB_TRY(check_impl(p, impl, n_samples, kHalves, "mlp_wgrad"));
+  return launch_wgrad_simt(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, n_rays * n_samples, flat_grad,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_composite_fwd(const float* raw, const float* z, const float* rays, int32_t ray_stride,
@@ -597,7 +635,6 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
                             float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
                             void* stream) {
-  if (impl == 3 && training) return refuse_fast("render_fwd with training = 1");
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
@@ -626,35 +663,30 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
   const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-
-  // coarse pass: stratified depths -> MLP -> compositing (train_utils.py:45-94)
-  NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, F(w.z_c), s));
-  float* stash_c = training ? F(w.stash_c) : nullptr;
+  const Need need = training ? kStash : kInference;
   NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
-  if (impl == 1)
-    NB_TRY(launch_mlp_fwd_tc(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
-  else if (impl == 3)
-    NB_TRY(launch_mlp_fwd_tc_fast(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), s));
-  else
-    NB_TRY(launch_mlp_fwd_simt(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.raw_c), stash_c, s));
-  NB_TRY(launch_composite_fwd(F(w.raw_c), F(w.z_c), rays, ray_stride, rnd[kRandNoiseC], n_rays, nc, opts->noise_std,
-                              opts->white_bkgd, out_coarse, F(w.w_c), s));
-  if (!fine) return NERFB200_OK;
+  NB_TRY(check_impl(pc, impl, nc, need, "render_fwd"));
+  if (fine) {
+    NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
+    NB_TRY(check_impl(pf, impl, ns, need, "render_fwd"));
+  }
 
-  // hierarchical resampling + merge (train_utils.py:96-105), fine pass (:107-125)
-  NB_TRY(launch_sample_pdf_merge(F(w.z_c), F(w.w_c), rnd[kRandU], nullptr, n_rays, nc, opts->n_fine, F(w.z_f), nullptr,
-                                 nullptr, nullptr, s));
-  float* stash_f = training ? F(w.stash_f) : nullptr;
-  NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
-  if (impl == 1)
-    NB_TRY(launch_mlp_fwd_tc(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
-  else if (impl == 3)
-    NB_TRY(launch_mlp_fwd_tc_fast(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), s));
-  else
-    NB_TRY(launch_mlp_fwd_simt(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.raw_f), stash_f, s));
-  NB_TRY(launch_composite_fwd(F(w.raw_f), F(w.z_f), rays, ray_stride, rnd[kRandNoiseF], n_rays, ns, opts->noise_std,
-                              opts->white_bkgd, out_fine, nullptr, s));
-  return NERFB200_OK;
+  // one pass: depths -> MLP -> compositing.  The coarse pass (train_utils.py:45-94) takes stratified depths, the fine
+  // pass (:96-125) resamples the coarse weights' pdf and merges the two sets.
+  auto pass = [&](bool is_fine, const Plan& p, const float* blob, int n, float* z, float* raw, float* stash,
+                  float* out, float* weights) {
+    if (is_fine)
+      NB_TRY(launch_sample_pdf_merge(F(w.z_c), F(w.w_c), rnd[kRandU], nullptr, n_rays, nc, opts->n_fine, z, nullptr,
+                                     nullptr, nullptr, s));
+    else
+      NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, z, s));
+    NB_TRY(mlp_forward(p, impl, blob, rays, ray_stride, z, n_rays, n, raw, training ? stash : nullptr, s));
+    return launch_composite_fwd(raw, z, rays, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
+                                opts->noise_std, opts->white_bkgd, out, weights, s);
+  };
+  NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse, F(w.w_c)));
+  if (!fine) return NERFB200_OK;
+  return pass(true, pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), out_fine, nullptr);
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
@@ -663,7 +695,6 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* noise_c, const float* noise_f, const float* g_coarse, const float* g_fine,
                             void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
                             void* stream) {
-  if (impl == 3) return refuse_fast("render_bwd");
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
@@ -686,27 +717,29 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
     set_error("render_bwd: parts must select the fine (1) and / or the coarse (2) backward");
     return NERFB200_ERR_INVALID;
   }
+  const bool run_fine = fine && (parts & 1), run_coarse = parts & 2;
+  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
+  if (run_fine) NB_TRY(check_impl(pf, impl, ns, kBackward, "render_bwd"));
+  if (run_coarse) NB_TRY(check_impl(pc, impl, nc, kBackward, "render_bwd"));
   Workspace w;
   carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/1, &w);
   char* base = static_cast<char*>(workspace);
   auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 
-  if (fine && (parts & 1)) {
-    NB_TRY(launch_composite_bwd(F(w.raw_f), F(w.z_f), rays, ray_stride, rnd[kRandNoiseF], g_fine, n_rays, ns,
-                                opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
-    NB_TRY(launch_mlp_bwd(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns, F(w.d_raw), F(w.stash_f), F(w.gstash),
-                          flat_grad_f, impl, s));
-  }
-  if (!(parts & 2)) return NERFB200_OK;
+  // one network's part: compositing backward into d_raw, then the MLP backward
+  auto part = [&](const Plan& p, const float* blob, int n, const float* z, const float* raw, const float* stash,
+                  const RandSrc& noise, const float* g, float* flat_grad) {
+    NB_TRY(launch_composite_bwd(raw, z, rays, ray_stride, noise, g, n_rays, n, opts->noise_std, opts->white_bkgd,
+                                F(w.d_raw), s));
+    return mlp_backward(p, impl, blob, rays, ray_stride, z, n_rays, n, F(w.d_raw), stash, F(w.gstash), flat_grad, s);
+  };
+  if (run_fine)
+    NB_TRY(part(pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), rnd[kRandNoiseF], g_fine, flat_grad_f));
+  if (!run_coarse) return NERFB200_OK;
   // the coarse weights feed the resampler only through a detach (train_utils.py:103), so the
   // coarse net's gradient comes from rgb/disp/acc_coarse alone.
-  NB_TRY(launch_composite_bwd(F(w.raw_c), F(w.z_c), rays, ray_stride, rnd[kRandNoiseC], g_coarse, n_rays, nc,
-                              opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
-  NB_TRY(launch_mlp_bwd(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc, F(w.d_raw), F(w.stash_c), F(w.gstash),
-                        flat_grad_c, impl, s));
-  return NERFB200_OK;
+  return part(pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), rnd[kRandNoiseC], g_coarse, flat_grad_c);
 }
 
 int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64_t n_rays, int32_t per_ray, float* out,

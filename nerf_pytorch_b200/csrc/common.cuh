@@ -130,28 +130,6 @@ int launch_gen_rays(const float* c2w12_host, int height, int width, float focal,
 int launch_pack_rays(const float* ro, const float* rd, int64_t n, int height, int width, float focal, int ndc, float near,
                      float far, int use_viewdirs, int out_stride, float* out, cudaStream_t s);
 int launch_encode(const Plan& p, int which, const float* x, int64_t n, float* out, cudaStream_t s);
-int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                        int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s);
-int launch_mlp_bwd(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                   int64_t n_rays, int n_samples, const float* d_raw, const float* stash, float* gstash,
-                   float* flat_grad, int impl, cudaStream_t s);
-// the two halves of launch_mlp_bwd (stage-level entry points: tests and per-kernel timing)
-int launch_mlp_dgrad(const Plan& p, const float* blob, const float* d_raw, const float* stash, float* gstash, int64_t P,
-                     int impl, cudaStream_t s);
-int launch_mlp_wgrad(const Plan& p, const float* rays, int ray_stride, const float* z, int64_t n_rays, int n_samples,
-                     const float* d_raw, const float* stash, const float* gstash, float* flat_grad, int impl,
-                     cudaStream_t s);
-// wgmma backward (mlp_tc_bwd.cu): data-gradient chain + every weight gradient in one kernel; `scratch` holds the
-// L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into
-int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
-                      const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
-int64_t bwd_tc_scratch_floats(const Plan& p);
-// forward (training: + stash; fast: the single-pass inference forward, impl 3)
-int tc_supported(const Plan& p, int n_samples, const char* what, bool training, bool fast = false);
-// single-pass fp16 wgmma forward (mlp_tc.cu, kFast): inference only, no stash
-int launch_mlp_fwd_tc_fast(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                           int64_t n_rays, int n_samples, float* raw, cudaStream_t s);
-int bwd_tc_supported(const Plan& p, int n_samples, const char* what);  // forward + backward
 int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s);
@@ -164,9 +142,32 @@ int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, 
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s);
 int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2,
                 float eps, float grad_scale, cudaStream_t s);
-// wgmma path (mlp_tc.cu, mlp_tc_bwd.cu)
+
+// The MLP kernel families.  Each file's predicate says whether its kernels take a plan (NERFB200_OK, else the reason
+// in the last error, prefixed with `what`); api.cu's check_impl maps an impl code to them, and its mlp_forward /
+// mlp_backward pick the launchers, which do not check again.
+// fp32 CUDA cores (mlp_simt.cu), impl 0: the forward, then the backward's two halves (dgrad fills the gradient stash
+// `gstash`, wgrad reduces it into flat_grad)
+int simt_supported(const Plan& p, const char* what);
+int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                        int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s);
+int launch_dgrad_simt(const Plan& p, const float* blob, const float* d_raw, const float* stash, float* gstash,
+                      int64_t P, cudaStream_t s);
+int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const float* z, int n_samples,
+                      const float* d_raw, const float* stash, const float* gstash, int64_t P, float* flat_grad,
+                      cudaStream_t s);
+// wgmma forward (mlp_tc.cu), impl 1 and 3: training writes the stash (hidden 128 only); fast is the single-pass
+// fp16 inference forward (impl 3, no stash)
+int tc_supported(const Plan& p, int n_samples, bool training, const char* what);
 int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                      int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s);
+                      int64_t n_rays, int n_samples, float* raw, float* stash, bool fast, cudaStream_t s);
+// wgmma backward (mlp_tc_bwd.cu), impl 1: data-gradient chain + every weight gradient in one kernel; `scratch` holds
+// the L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into.
+// bwd_tc_supported checks what it needs beyond tc_supported(training = true).
+int bwd_tc_supported(const Plan& p, const char* what);
+int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
+                      const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
+int64_t bwd_tc_scratch_floats(const Plan& p);
 
 // ---------------------------------------------------------------------------------------------
 // device helpers

@@ -260,7 +260,8 @@ mlp_fwd_simt_kernel(const __grid_constant__ Plan p, const FwdSmem sm, const floa
       }
       __syncthreads();
       if (stash && tid < kTileRows && p0 + tid < P) {
-        // ReLU bit mask of this row (read by the wgmma dgrad kernel): bit c = output c > 0
+        // ReLU bit mask of this row, bit c = output c > 0: it fills the stash's mask section, which only the wgmma
+        // backward reads (from its own forward's stash); the fp32 backward does not
         uint32_t* mk = reinterpret_cast<uint32_t*>(stash) + (size_t)P * (p.mask_base + g.mask_cum) +
                        (size_t)(p0 + tid) * (g.n / 32);
         for (int w = 0; w < g.n / 32; ++w) {
@@ -290,14 +291,20 @@ mlp_fwd_simt_kernel(const __grid_constant__ Plan p, const FwdSmem sm, const floa
   }
 }
 
+// the forward's tiles must fit one CTA's shared memory (the backward kernels need less)
+int simt_supported(const Plan& p, const char* what) {
+  const size_t bytes = (size_t)fwd_smem_layout(p).total_floats * sizeof(float);
+  if (bytes > 227 * 1024) {
+    set_error("%s: configuration needs %zu bytes of shared memory (> 227 KB)", what, bytes);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  return NERFB200_OK;
+}
+
 int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
                         int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s) {
   const FwdSmem sm = fwd_smem_layout(p);
   const size_t bytes = (size_t)sm.total_floats * sizeof(float);
-  if (bytes > 227 * 1024) {
-    set_error("mlp_fwd: configuration needs %zu bytes of shared memory (> 227 KB)", bytes);
-    return NERFB200_ERR_UNSUPPORTED;
-  }
   const int64_t P = n_rays * n_samples;
   const int64_t tiles = (P + kTileRows - 1) / kTileRows;
   auto kern = p.hidden == 256 ? mlp_fwd_simt_kernel<4> : mlp_fwd_simt_kernel<2>;
@@ -574,9 +581,9 @@ __global__ void __launch_bounds__(kThreads, 2)
 mlp_bwd_wgrad_kernel(const __grid_constant__ Plan p, const float* __restrict__ rays, int ray_stride,
                      const float* __restrict__ z, int S, const float* __restrict__ d_raw,
                      const float* __restrict__ stash, const float* __restrict__ gstash, int64_t P,
-                     float* __restrict__ flat_grad, int item_base) {
+                     float* __restrict__ flat_grad) {
   extern __shared__ __align__(16) float smem[];
-  const WgItem it = wg_decode(p, blockIdx.y + item_base);
+  const WgItem it = wg_decode(p, blockIdx.y);
   // contiguous point range of this CTA, in units of kWgPts
   const int64_t stages = (P + kWgPts - 1) / kWgPts;
   const int64_t per = (stages + gridDim.x - 1) / gridDim.x;
@@ -628,11 +635,11 @@ int launch_dgrad_simt(const Plan& p, const float* blob, const float* d_raw, cons
   return check_cuda(cudaGetLastError(), "mlp_bwd_dgrad launch");
 }
 
-// weight-gradient items [item_base, item_base + n_items) of wgrad_items.cuh on the CUDA cores
+// every weight-gradient item of wgrad_items.cuh on the CUDA cores
 int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const float* z, int n_samples,
                       const float* d_raw, const float* stash, const float* gstash, int64_t P, float* flat_grad,
-                      int item_base, int n_items, cudaStream_t s) {
-  if (n_items <= 0) return NERFB200_OK;
+                      cudaStream_t s) {
+  const int n_items = wg_item_count(p);
   const size_t bytes = (size_t)2 * kWgPts * (132 + 132) * sizeof(float);
   int rc = check_cuda(
       cudaFuncSetAttribute(mlp_bwd_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes),
@@ -646,41 +653,9 @@ int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const fl
   if (split < 1) split = 1;
   dim3 grid(split, n_items);
   mlp_bwd_wgrad_kernel<<<grid, kThreads, bytes, s>>>(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, P,
-                                                     flat_grad, item_base);
+                                                     flat_grad);
   count_launch();
   return check_cuda(cudaGetLastError(), "mlp_bwd_wgrad launch");
-}
-
-// The two halves of the CUDA-core backward as stage-level entry points.  The wgmma backward is one fused kernel
-// (mlp_tc_bwd.cu) that never materialises the gradient stash, so impl 1 has no halves.
-int launch_mlp_dgrad(const Plan& p, const float* blob, const float* d_raw, const float* stash, float* gstash, int64_t P,
-                     int impl, cudaStream_t s) {
-  if (impl == 1) {
-    set_error("mlp_dgrad: impl=1 (wgmma) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
-    return NERFB200_ERR_UNSUPPORTED;
-  }
-  return launch_dgrad_simt(p, blob, d_raw, stash, gstash, P, s);
-}
-
-int launch_mlp_wgrad(const Plan& p, const float* rays, int ray_stride, const float* z, int64_t n_rays, int n_samples,
-                     const float* d_raw, const float* stash, const float* gstash, float* flat_grad, int impl,
-                     cudaStream_t s) {
-  if (impl == 1) {
-    set_error("mlp_wgrad: impl=1 (wgmma) fuses dgrad and wgrad into one kernel; call nerfb200_mlp_bwd");
-    return NERFB200_ERR_UNSUPPORTED;
-  }
-  return launch_wgrad_simt(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, n_rays * n_samples, flat_grad, 0,
-                           wg_item_count(p), s);
-}
-
-// `gstash`: impl 0: the gradient stash (stash-sized); impl 1: scratch for the gradient blob (bwd_tc_scratch_floats)
-int launch_mlp_bwd(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                   int64_t n_rays, int n_samples, const float* d_raw, const float* stash, float* gstash,
-                   float* flat_grad, int impl, cudaStream_t s) {
-  if (impl == 1) return launch_mlp_bwd_tc(p, blob, rays, ray_stride, n_rays, n_samples, d_raw, stash, gstash, flat_grad, s);
-  int rc = launch_mlp_dgrad(p, blob, d_raw, stash, gstash, n_rays * n_samples, impl, s);
-  if (rc) return rc;
-  return launch_mlp_wgrad(p, rays, ray_stride, z, n_rays, n_samples, d_raw, stash, gstash, flat_grad, impl, s);
 }
 
 }  // namespace nerfb200

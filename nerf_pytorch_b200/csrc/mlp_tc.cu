@@ -460,26 +460,24 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 }
 
 // training = the forward must also write the activation stash for the fused backward (hidden 128 only); the
-// inference forward also runs hidden 256 (one warpgroup, 64-point tiles, N = 256 MMAs)
-// fast: the single-pass forward (impl 3), accepted exactly where the inference forward is
-int tc_supported(const Plan& p, int n_samples, const char* what, bool training, bool fast) {
-  const char* impl = fast ? "impl=3 (single-pass fp16 wgmma)" : "impl=1 (wgmma)";
+// inference forwards also run hidden 256 (one warpgroup, 64-point tiles, N = 256 MMAs).  The single-pass forward
+// (impl 3) is accepted exactly where the inference forward is.  `what` names the call and the impl.
+int tc_supported(const Plan& p, int n_samples, bool training, const char* what) {
   if (p.hidden != 128 && (training || p.hidden != 256)) {
-    set_error("%s %s: hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
-              impl, p.hidden);
+    set_error("%s: hidden_size %d not supported (training: 128 only; inference: 128 or 256); use impl=0", what,
+              p.hidden);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (p.dim_xyz_pad > 64 || p.dim_dir > 32) {
-    set_error("%s %s: encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what, impl);
+    set_error("%s: encodings wider than 64 (xyz) / 32 (dir) not supported; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (n_samples > 0 && (kTileRows + n_samples - 1) / n_samples + 1 > kMaxRaysPerTile) {
-    set_error("%s %s: fewer than 15 samples per ray not supported; use impl=0", what, impl);
+    set_error("%s: fewer than 15 samples per ray not supported; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map(p).n_stages < 2) {
-    set_error("%s %s: network too deep for the shared-memory budget (%d layers); use impl=0", what,
-              impl, p.n_gemm);
+    set_error("%s: network too deep for the shared-memory budget (%d layers); use impl=0", what, p.n_gemm);
     return NERFB200_ERR_UNSUPPORTED;
   }
   return NERFB200_OK;
@@ -502,29 +500,16 @@ static int launch_fwd(const Plan& p, const float* blob, const float* rays, int r
   return check_cuda(cudaGetLastError(), what);
 }
 
+// stash non-null: the training forward; fast: the single-pass forward (never with a stash)
 int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                      int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s) {
-  int rc = tc_supported(p, n_samples, "mlp_fwd", stash != nullptr);
-  if (rc) return rc;
-  if (stash)
-    return launch_fwd<true, 128, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, stash, s,
-                                        "mlp_fwd_tc launch");
-  if (p.hidden == 256)
-    return launch_fwd<false, 256, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                         "mlp_fwd_tc launch");
-  return launch_fwd<false, 128, false>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                       "mlp_fwd_tc launch");
-}
-
-int launch_mlp_fwd_tc_fast(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                           int64_t n_rays, int n_samples, float* raw, cudaStream_t s) {
-  int rc = tc_supported(p, n_samples, "mlp_fwd", /*training=*/false, /*fast=*/true);
-  if (rc) return rc;
-  if (p.hidden == 256)
-    return launch_fwd<false, 256, true>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                        "mlp_fwd_tc_fast launch");
-  return launch_fwd<false, 128, true>(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, nullptr, s,
-                                      "mlp_fwd_tc_fast launch");
+                      int64_t n_rays, int n_samples, float* raw, float* stash, bool fast, cudaStream_t s) {
+  auto go = [&](auto launch, const char* what) {
+    return launch(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, stash, s, what);
+  };
+  if (stash) return go(launch_fwd<true, 128, false>, "mlp_fwd_tc launch");
+  if (fast)
+    return go(p.hidden == 256 ? launch_fwd<false, 256, true> : launch_fwd<false, 128, true>, "mlp_fwd_tc_fast launch");
+  return go(p.hidden == 256 ? launch_fwd<false, 256, false> : launch_fwd<false, 128, false>, "mlp_fwd_tc launch");
 }
 
 }  // namespace nerfb200

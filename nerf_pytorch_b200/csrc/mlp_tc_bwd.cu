@@ -662,19 +662,18 @@ int64_t bwd_tc_scratch_floats(const Plan& p) {
   return 2 * (int64_t)blob_map(p, total).words;
 }
 
-int bwd_tc_supported(const Plan& p, int n_samples, const char* what) {
-  int rc = tc_supported(p, n_samples, what, /*training=*/true);
-  if (rc) return rc;
+// what the fused backward needs beyond the training forward (tc_supported); `what` names the call and the impl
+int bwd_tc_supported(const Plan& p, const char* what) {
   if (!p.use_viewdirs) {
-    set_error("%s impl=1 (wgmma): the fused backward needs a view-dependent model (fc_rgb / fc_alpha heads); use impl=0", what);
+    set_error("%s: the fused backward needs a view-dependent model (fc_rgb / fc_alpha heads); use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (p.dim_dir > 28) {
-    set_error("%s impl=1 (wgmma): direction encodings wider than 28 not supported by the fused backward; use impl=0", what);
+    set_error("%s: direction encodings wider than 28 not supported by the fused backward; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   if (smem_map_b(p).n_stages < 2) {
-    set_error("%s impl=1 (wgmma): network too deep for the backward's shared-memory budget; use impl=0", what);
+    set_error("%s: network too deep for the backward's shared-memory budget; use impl=0", what);
     return NERFB200_ERR_UNSUPPORTED;
   }
   return NERFB200_OK;
@@ -682,15 +681,13 @@ int bwd_tc_supported(const Plan& p, int n_samples, const char* what) {
 
 int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
                       const float* d_raw, const float* stash, float* gblob, float* flat_grad, cudaStream_t s) {
-  int rc = bwd_tc_supported(p, n_samples, "mlp_bwd");
-  if (rc) return rc;
   const int64_t P = n_rays * n_samples;
   const int64_t tiles = (P + kTileRows - 1) / kTileRows;
   const int sms = device_sms();
   const int grid = (int)(tiles < sms ? tiles : sms);
   const BwdPlan bp = make_bwd_plan(p);
   const BlobMap bm = blob_map(p, bp.gb_total);
-  rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)bm.words * 8, s), "mlp_bwd_tc blob memset");
+  int rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)bm.words * 8, s), "mlp_bwd_tc blob memset");
   if (rc) return rc;
   const size_t bytes = (size_t)smem_map_b(p).total + 1024;
   rc = check_cuda(cudaFuncSetAttribute(mlp_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes),

@@ -281,8 +281,8 @@ def mlp_bwd(arch: ArchSpec, blob, rays, z, d_raw, stash, impl=IMPL_SIMT, flat_gr
     lib = _lib.load()
     n, s = z.shape
     n_scratch = lib.nerfb200_bwd_scratch_floats(C.byref(arch.c_struct()), n * s, impl)
-    if n_scratch < 0 and impl == IMPL_TC_FAST:
-        _lib.check(_lib.ERR_UNSUPPORTED, "mlp_bwd")  # the library's refusal: the single-pass forward does not train
+    if n_scratch < 0:
+        _lib.check(_lib.ERR_UNSUPPORTED, "mlp_bwd")  # the library's refusal, e.g. impl 3, which does not train
     gstash = torch.empty(n_scratch, dtype=torch.float32, device=z.device)
     if flat_grad is None:
         flat_grad = torch.zeros(arch.flat_param_count(), dtype=torch.float32, device=z.device)

@@ -47,16 +47,20 @@ _GRAD_SYNC = None
 _PENDING_SYNC = False
 
 
-def _refuse_fast_training(impl, *models):
-    """ops.IMPL_TC_FAST renders only (no stash, no backward): a call that would train with it (grad enabled and
-    parameters that require grad) raises here, before anything is launched."""
-    if impl is None:
-        impl = DEFAULT_IMPL
-    if impl is None or int(impl) != ops.IMPL_TC_FAST or not torch.is_grad_enabled():
-        return
-    if any(p.requires_grad for m in models if m is not None for p in m.parameters()):
+def _trains(params) -> bool:
+    """A call trains when autograd is on and one of its parameters requires grad."""
+    return torch.is_grad_enabled() and any(p.requires_grad for p in params)
+
+
+def _requested_impl(impl, *models):
+    """The kernels a call asks for: ``impl``, else ``DEFAULT_IMPL``; None leaves the choice to ``_auto_impl``.
+    ops.IMPL_TC_FAST renders only (no stash, no backward): a call that would train with it raises here, before
+    anything is launched."""
+    impl = DEFAULT_IMPL if impl is None else int(impl)
+    if impl == ops.IMPL_TC_FAST and _trains(p for m in models if m is not None for p in m.parameters()):
         raise NotImplementedError("nerfb200: impl=3 (single-pass fp16 wgmma forward) is inference only; train with "
                                   "impl=0 or impl=1, or render under torch.no_grad()")
+    return impl
 
 
 def set_default_impl(impl):
@@ -314,7 +318,7 @@ def predict_and_render_radiance(
 
     ``impl``: None picks the kernels (``DEFAULT_IMPL``, else the automatic choice); ``ops.IMPL_TC_FAST`` renders with
     the single-pass fp16 forward and raises ``NotImplementedError`` if the call would train."""
-    _refuse_fast_training(impl, model_coarse, model_fine)
+    impl = _requested_impl(impl, model_coarse, model_fine)
     o = getattr(options.nerf, mode)
     if not ray_batch.is_cuda:
         raise NotImplementedError("nerfb200: rays must be on a CUDA device (there is no CPU path)")
@@ -359,12 +363,10 @@ def predict_and_render_radiance(
             rnd["noise_f"] = take("noise_f", (n, nc + nf), torch.randn)
 
     all_params = list(params_c) + list(params_f)
-    training = torch.is_grad_enabled() and any(p.requires_grad for p in all_params)
-    if impl is None:
-        impl = DEFAULT_IMPL
+    training = _trains(all_params)
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, int(impl), int(_n_chunks))
+    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, impl, int(_n_chunks))
     out_c, out_f = _RenderChunk.apply(cfg, rays, rnd, *all_params)
     rgb_c, disp_c, acc_c = out_c[:, :3], out_c[:, 3], out_c[:, 4]
     if out_f is None:
@@ -391,7 +393,7 @@ def run_one_iter_of_nerf(
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
     the reshape back to image shape."""
-    _refuse_fast_training(impl, model_coarse, model_fine)
+    impl = _requested_impl(impl, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     restore_shapes = [ray_directions.shape, ray_directions.shape[:-1], ray_directions.shape[:-1]]
     if model_fine:
@@ -429,7 +431,7 @@ def run_one_iter_of_nerf_from_pose(
     thousand it samples (train_nerf.py:196-226); here the rays of exactly those pixels are generated on the device
     (csrc/raygen.cu) in the packed layout the render kernels read.  ``pixel_ids``: int64, ``j * width + i``, on the
     target device (None = the whole image, returned image-shaped in "validation" mode)."""
-    _refuse_fast_training(impl, model_coarse, model_fine)
+    impl = _requested_impl(impl, model_coarse, model_fine)
     dev = pixel_ids.device if pixel_ids is not None else next(model_coarse.parameters()).device
     use_viewdirs = bool(options.nerf.use_viewdirs)
     rays = ops.gen_rays(tform_cam2world, height, width, focal_length, pixel_ids, dev, ndc=options.dataset.no_ndc is False,
