@@ -25,9 +25,10 @@
 // weight-gradient jobs: A = the G tile (MN-major), B = the activation tile (bulk-copied from the stash one job ahead and
 // requested as soon as both warpgroups' MMAs of the running job are complete), the 16-column ray-indicator job that yields the bias gradients and
 // the per-ray sums of layers_dir[0], and the two narrow heads' jobs with the roles swapped (A = activation tile, B =
-// d_raw = feature rows 64..79 of the first layer's G tile).  Finished weight-gradient accumulators are unscaled into
-// a swizzled staging chunk as 64-bit fixed point and added into the L2-resident gradient blob with cp.reduce.async.bulk
-// .add.u64; integer sums do not depend on the order of the adds, so the gradients are reproducible bit for bit.
+// d_raw = feature rows 64..79 of the first layer's G tile).  Finished weight-gradient accumulators are unscaled,
+// converted to 64-bit fixed point and added into the L2-resident gradient blob straight from the registers with
+// red.global.add.u64 (the warpgroup goes on to its next MMAs while the adds drain); integer sums do not depend on the
+// order of the adds, so the gradients are reproducible bit for bit.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "wgmma.cuh"
@@ -39,23 +40,21 @@ constexpr int kWG = 2;                            // consumer warpgroups
 constexpr int kThreadsB = 128 * (kWG + 1);       // + the producer warpgroup (one thread of it streams the weights)
 constexpr int kProdRegs = 24, kConsRegs = 240;   // setmaxnreg split: (24 + 2 x 240) x 128 = 168 x 384 registers
 constexpr int kWStage = 96 * 128;                 // one k-step of a 128-wide layer: 3 copies x 2 slabs x 128 x 16 B
-constexpr int kMaxWStages = 6;
+constexpr int kMaxWStages = 6;                    // smem_map_b leaves room for all 6 for A0 and A1 (73 KB for A1)
 constexpr int kGBytes = 65536;                    // G tile: hi block 32 KB, lo block 32 KB (128 features)
 constexpr int kXBytes = 65536;                    // activation tile of the running job
-constexpr int kStgBytes = 8192;                   // staging chunk: 64 rows x 16 fixed-point int64; two alternate per warpgroup
 constexpr int kIndBytes = 4096;                   // ray-indicator tile: 128 points x 16 "features" (hi only)
 constexpr int kMaxRays = 10;
 constexpr int kSmemLimitB = 232448 - 1024;
 
 struct SmemMapB {
-  int g, x, stg, ind, headw, bgrad, encd, sums, dacc, misc, bars, ring, total, n_stages;
+  int g, x, ind, headw, bgrad, encd, sums, dacc, misc, bars, ring, total, n_stages;
 };
 __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   SmemMapB m;
   int off = 0;
   m.g = off;      off += kGBytes;
   m.x = off;      off += kXBytes;
-  m.stg = off;    off += 2 * kWG * kStgBytes;
   m.ind = off;    off += kIndBytes;
   m.headw = off;  off += (4 * 128 + 3 * 64 + 16) * 4;
   m.bgrad = off;  off += (p.enc_cum[0] + 8) * 4;   // bias gradients of every gemm layer + the heads' (8)
@@ -79,7 +78,7 @@ struct BwdJob {
   int src;
   int n_b;       // columns = width of the B tile (multiple of 16)
   int row0, nrows;  // accumulator rows that carry gradients
-  int gb_off;    // offset (int64 words) of this job's block in the gradient blob: [n_b / 16 chunks][128 rows][16]
+  int gb_off;    // offset (int64 words) of this job's block in the gradient blob: 128 rows x n_b words, layout below blob_map
   int dst_head;  // -1: rows are output features of gemm layer `dst`; else head index, rows row0.. are its outputs
   int dst;       // gemm index
   int dst_col0;  // first input column of the destination weight this block covers
@@ -128,7 +127,7 @@ struct BwdPlan {
 // adds into.  Integer addition is associative, so the sums -- and the gradients -- are the same bits whatever order the
 // CTAs' reduce-adds and atomics arrive in.  Resolution 2^-32 (2.3e-10) per added term; every partial sum must stay
 // below 2^31 in magnitude.
-//   [0, gb_total)  weight-gradient blocks of the jobs (bulk reduce-add .u64 from the staging chunks)
+//   [0, gb_total)  weight-gradient blocks of the jobs (red.global.add.u64 from the accumulator registers)
 //   xb: bias gradients of the gemm layers (cum_n order) + the heads' 4 biases (+ 4 spare)
 //   xd: direction-encoding part of dW(layers_dir[0]) [64][28]
 //   xh: the heads' weight gradients [head][4 outputs][128 inputs]
@@ -145,6 +144,13 @@ __host__ __device__ inline BlobMap blob_map(const Plan& p, int gb_total) {
   return m;
 }
 __device__ __forceinline__ unsigned long long to_fix(float v) { return (unsigned long long)__float2ll_rn(v * kFix); }
+// A job's block (128 rows x ncol columns, ncol = n_b rounded up to 16) follows the accumulator fragment: element
+// (row, col) is word  ((row >> 3) (ncol >> 3) + (col >> 3)) 64 + (col & 1) 32 + (row & 7) 4 + ((col & 7) >> 1),
+// i.e. 8 x 8 (row-octet, column-octet) sub-blocks of 64 words, row-octets outer, each ordered [col & 1][row & 7]
+// [(col & 7) / 2].  A wgmma m64nNk16 fragment holds rows 16 warp + lane / 4 (+ 8) and columns 8 j + 2 (lane & 3) (+ 1),
+// so one warp-wide red of one accumulator register covers 256 contiguous bytes (8 whole 32-byte sectors).  With a
+// row-major block the same reds touch 8 rows x 4 strided words each and reach less than half the aggregate rate
+// (tools/mb_l2.cu).
 
 inline BwdPlan make_bwd_plan(const Plan& p) {
   BwdPlan bp;
@@ -197,36 +203,19 @@ __device__ __forceinline__ void job_mma(float (&acc)[N / 2], float (&acc_i)[8], 
   if (kInd) reg_fence(acc_i);
 }
 
-// the finished accumulator (64 rows of this warpgroup x N columns) -> unscale -> fixed point -> swizzled staging chunks
-// -> bulk reduce-add into the job's block of the gradient blob ([chunk][128 rows][16 words], the eight 16-byte pieces
-// of a row XOR-swizzled by row & 7)
+// the finished accumulator (64 rows of this warpgroup x N columns) -> unscale -> fixed point -> red.global.add.u64 into
+// the job's block of the gradient blob (the fragment layout above: one 256-byte span per warp and register)
 template <int N>
-__device__ __forceinline__ void job_drain(const float (&acc)[N / 2], float us, unsigned long long* gdst,
-                                          unsigned long long* stg, uint32_t& stg_n, int wg) {
-  const int wt = threadIdx.x & 127, lane = wt & 31, q = lane & 3;
-  const int r0 = 16 * (wt >> 5) + (lane >> 2);
+__device__ __forceinline__ void job_drain(const float (&acc)[N / 2], float us, unsigned long long* gdst, int wg) {
+  const int wt = threadIdx.x & 127, lane = wt & 31;
+  // row-octets 8 wg + 2 warp (+ 1) of the block; lane = 4 (row & 7) + (col & 7) / 2
+  unsigned long long* d = gdst + (8 * wg + 2 * (wt >> 5)) * (N / 8) * 64 + lane;
 #pragma unroll
-  for (int c = 0; c < (N + 15) / 16; ++c) {
-    unsigned long long* sb = stg + (stg_n & 1u) * (kStgBytes / 8);
-    if (wt == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+  for (int j = 0; j < N / 8; ++j)
 #pragma unroll
-    for (int jj = 0; jj < 2; ++jj) {
-      const int j = 2 * c + jj;
-      if (j < N / 8) {
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int r = r0 + 8 * i, piece = 4 * jj + q;  // columns 8 jj + 2 q, + 1 of the chunk
-          *reinterpret_cast<ulonglong2*>(sb + r * 16 + 2 * (piece ^ (r & 7))) =
-              make_ulonglong2(to_fix(acc[4 * j + 2 * i] * us), to_fix(acc[4 * j + 2 * i + 1] * us));
-        }
-      }
-    }
-    fence_proxy_async();
-    asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
-    if (wt == 0) bulk_reduce_add_u64(gdst + (size_t)c * 2048 + 64 * wg * 16, sb, 64u * 128u);
-    ++stg_n;
-  }
+      for (int c = 0; c < 2; ++c) red_add_u64(d + (i * (N / 8) + j) * 64 + 32 * c, to_fix(acc[4 * j + 2 * i + c] * us));
 }
 
 __global__ void __launch_bounds__(kThreadsB, 1)
@@ -306,8 +295,7 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsRegs));
     const int wg = warp >> 2, wt = tid & 127, q = lane & 3;
     const int r0 = 16 * (wt >> 5) + (lane >> 2);   // warpgroup-local row of accumulator row 0 (row 1: + 8)
-    unsigned long long* stg = reinterpret_cast<unsigned long long*>(sm + mp.stg) + wg * 2 * (kStgBytes / 8);
-    uint32_t stg_n = 0, x_ph = 0;
+    uint32_t x_ph = 0;
     Pipe pp;
     // activation tile of job (it, e, i): hi block, lo block (issued by thread 0 one job ahead)
     auto issue_x = [&](int it, int e, int i) {
@@ -555,7 +543,7 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     if (i == 0) job_mma<NN, true>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);          \
     else job_mma<NN, false>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);                \
     release_x();                                                                                     \
-    if (64 * wg < jq.nrows) job_drain<NN>(acc, us, gdst, stg, stg_n, wg);                            \
+    if (64 * wg < jq.nrows) job_drain<NN>(acc, us, gdst, wg);                                        \
   }
             if (w == 128) NB_JOB(128) else if (w == 64) NB_JOB(64) else if (w == 48) NB_JOB(48)
             else if (w == 32) NB_JOB(32) else NB_JOB(16)
@@ -597,7 +585,6 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
         }
       }
     }
-    if (wt == 0) bulk_wait_all();
   }
   __syncthreads();
   // ---- the bias / direction-encoding accumulators of this CTA go to the blob
@@ -606,8 +593,7 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 }
 
 // gradient blob (fixed point) -> flat (torch-layout) gradient vector: every blob word is added to the one flat element it
-// belongs to.  Weight-gradient job blocks are [chunk][row][16 words] with the eight 16-byte pieces of a row XOR-swizzled
-// by (row & 7) (the staging tile's bank-conflict-free layout).
+// belongs to.  Weight-gradient job blocks follow the accumulator fragment (above make_bwd_plan).
 __global__ void unpack_grad_kernel(const __grid_constant__ Plan p, const __grid_constant__ BwdPlan bp,
                                    const unsigned long long* __restrict__ gb, float* __restrict__ flat_grad) {
   const BlobMap sl = blob_map(p, bp.gb_total);
@@ -619,11 +605,11 @@ __global__ void unpack_grad_kernel(const __grid_constant__ Plan p, const __grid_
         for (int i = 0; i < nj; ++i) {
           const BwdJob& j = bp.jobs[e][i];
           if (j.kind != 0) continue;
-          const int sz = ((j.n_b + 15) / 16) * 2048;
+          const int ncol = ((j.n_b + 15) / 16) * 16, sz = 128 * ncol;
           if (idx < j.gb_off || idx >= j.gb_off + sz) continue;
-          const int r = idx - j.gb_off;
-          const int c = r >> 11, rr = (r >> 4) & 127, w = r & 15;
-          const int col = 16 * c + ((((w >> 1) ^ (rr & 7)) << 1) | (w & 1));
+          const int r = idx - j.gb_off, blk = r >> 6, w = r & 63;
+          const int rr = 8 * (blk / (ncol >> 3)) + ((w >> 2) & 7);
+          const int col = 8 * (blk % (ncol >> 3)) + 2 * (w & 3) + (w >> 5);
           const GemmLayer& g = p.g[j.dst];
           if (rr >= j.row0 && rr < j.row0 + j.nrows && col < j.ncols)
             dst = g.flat_w + (int64_t)rr * (g.k_h + g.enc_real) + j.dst_col0 + col;

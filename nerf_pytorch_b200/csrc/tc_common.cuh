@@ -168,12 +168,9 @@ __host__ __device__ inline int tile_bytes(int n_feat) { return 2 * tile_half_byt
 __host__ __device__ inline int tile_piece(int row, int fb, int n_feat) {
   return (row >> 3) * (n_feat >> 3) * 128 + fb * 128 + (row & 7) * 16;
 }
-// shared -> global bulk reduction (TMA engine): global[i] += shared[i], 64-bit integers
-__device__ __forceinline__ void bulk_reduce_add_u64(unsigned long long* gdst, const void* ssrc, uint32_t bytes) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.u64 [%0], [%1], %2;" ::"l"(gdst),
-               "r"(smem_u32(ssrc)), "r"(bytes)
-               : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+// register -> global reduction without a return value (the thread does not wait for it): *gdst += v, 64-bit integers
+__device__ __forceinline__ void red_add_u64(unsigned long long* gdst, unsigned long long v) {
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(gdst), "l"(v) : "memory");
 }
 
 struct Pipe {  // role-local ring state

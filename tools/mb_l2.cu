@@ -2,6 +2,8 @@
 //   (1) cp.async.bulk global(L2-resident) -> shared, all SMs, ring of 4 stages: aggregate GB/s vs chunk size
 //   (2) cp.reduce.async.bulk shared -> global .add.f32 and .add.u64 (the backward's fixed-point gradient blob) into a
 //       small L2-resident region: aggregate GB/s
+//   (3) red.global.add.u64 from the registers of a wgmma accumulator fragment into a 1.31 MB region (fragment-blocked
+//       and row-major layouts): aggregate GB/s
 // build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/mb_l2 tools/mb_l2.cu
 #include <cstdio>
 #include <cstdint>
@@ -79,9 +81,34 @@ __global__ void __launch_bounds__(128, 1) reduce_kernel(void* __restrict__ dst_v
   }
 }
 
+// (3) red.global.add.u64 straight from registers: two warpgroups per SM, each thread holding the 64 fp32 accumulator
+// registers of a wgmma m64n128 fragment (rows 16 warp + lane / 4 (+ 8), columns 8 j + 2 (lane & 3) (+ 1)); a warpgroup
+// job adds its 64 x 128 block of words into one of kRedJobs such blocks.  kFrag: the blob stores each 8 x 8 (row-octet,
+// column-octet) block contiguously, column parity first, so one warp-wide red covers 256 contiguous bytes; otherwise the
+// block is row-major (a warp-wide red touches 8 rows x 4 strided words).
+constexpr int kRedJobs = 21;   // 21 x 64 KB = 1.31 MB, one tile's weight gradients in the A1 backward
+template <bool kFrag>
+__global__ void __launch_bounds__(256, 1) red_kernel(unsigned long long* __restrict__ dst, int iters) {
+  const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31, q = lane & 3;
+  for (int it = 0; it < iters; ++it) {
+    unsigned long long* job = dst + (size_t)((blockIdx.x * 2 + wg + it * 5) % kRedJobs) * 8192;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const size_t w = kFrag ? (size_t)((2 * warp + i) * 16 + j) * 64 + c * 32 + lane
+                                 : (size_t)(16 * warp + (lane >> 2) + 8 * i) * 128 + 8 * j + 2 * q + c;
+          asm volatile("red.global.add.u64 [%0], %1;" ::"l"(job + w), "l"((unsigned long long)(it + lane + c)) : "memory");
+        }
+  }
+}
+
 int main() {
   int sms = 0; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
-  printf("SMs %d\n", sms);
+  cudaDeviceProp prop; cudaGetDeviceProperties(&prop, 0);
+  printf("%s, SMs %d\n", prop.name, sms);
   uint8_t* src; const size_t src_bytes = 1536 * 1024; cudaMalloc(&src, src_bytes); cudaMemset(src, 1, src_bytes);
   long long* cyc; cudaMalloc(&cyc, sizeof(long long) * 1024);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
@@ -118,6 +145,18 @@ int main() {
       printf("reduce-add .%s chunk %6u: %.3f ms  %.1f GB/s aggregate\n", u64 ? "u64" : "f32", chunk, ms,
              (double)sms * iters * chunk / ms * 1e-6);
     }
+  unsigned long long* rdst; cudaMalloc(&rdst, (size_t)kRedJobs * 8192 * 8); cudaMemset(rdst, 0, (size_t)kRedJobs * 8192 * 8);
+  for (int frag = 1; frag >= 0; --frag) {
+    auto kern = frag ? red_kernel<true> : red_kernel<false>;
+    const int iters = 512;
+    kern<<<sms, 256>>>(rdst, 16);
+    cudaEventRecord(e0);
+    kern<<<sms, 256>>>(rdst, iters);
+    cudaEventRecord(e1); cudaEventSynchronize(e1);
+    float ms; cudaEventElapsedTime(&ms, e0, e1);
+    printf("red.global.add.u64 from registers, %s layout: %.3f ms  %.1f GB/s aggregate\n", frag ? "fragment" : "row-major",
+           ms, (double)sms * iters * 2 * 65536 / ms * 1e-6);
+  }
   printf("err: %s\n", cudaGetErrorString(cudaGetLastError()));
   return 0;
 }
