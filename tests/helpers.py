@@ -111,6 +111,42 @@ def pack_rays(case: Case, dtype=torch.float32):
     return rays.contiguous()
 
 
+def arch_of(case: Case):
+    """The ops.ArchSpec of a golden case's networks."""
+    from nerf_pytorch_b200 import ops
+
+    c = case
+    return ops.ArchSpec(num_layers=c.num_layers, hidden=c.hidden, skip_every=c.skip, use_viewdirs=c.use_viewdirs,
+                        n_freq_xyz=c.enc_xyz[0], n_freq_dir=c.enc_dir[0], include_input_xyz=c.enc_xyz[1],
+                        include_input_dir=c.enc_dir[1], log_sampling_xyz=c.enc_xyz[2], log_sampling_dir=c.enc_dir[2])
+
+
+def build_models(c: Case):
+    """The golden case's coarse and fine FlexibleNeRFModels (fine None if it has none) on the GPU, and its encoders."""
+    import nerf_pytorch_b200 as nb
+
+    def mk(sd):
+        m = nb.FlexibleNeRFModel(num_layers=c.num_layers, hidden_size=c.hidden, skip_connect_every=c.skip,
+                                 num_encoding_fn_xyz=c.enc_xyz[0], num_encoding_fn_dir=c.enc_dir[0],
+                                 include_input_xyz=c.enc_xyz[1], include_input_dir=c.enc_dir[1],
+                                 use_viewdirs=c.use_viewdirs)
+        m.load_state_dict(sd)
+        return m.cuda()
+
+    mc = mk(c.sd_c)
+    mf = mk(c.sd_f) if c.sd_f is not None else None
+    epf = nb.get_embedding_function(*c.enc_xyz)
+    edf = nb.get_embedding_function(*c.enc_dir) if c.use_viewdirs else None
+    return mc, mf, epf, edf
+
+
+def bits_equal(a, b):
+    """Same shape and the same bits (4-byte elements); two Nones are equal."""
+    if a is None or b is None:
+        return a is None and b is None
+    return a.shape == b.shape and torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
+
+
 def err_stats(a: torch.Tensor, b: torch.Tensor):
     a, b = a.detach().double().cpu(), b.detach().double().cpu()
     both_nan = torch.isnan(a) & torch.isnan(b)

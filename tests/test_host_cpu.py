@@ -46,23 +46,23 @@ def test_flat_layout_matches_reference_state_dict_shapes():
 
 
 def test_tc_gradient_blocks_partition_the_flat_gradient():
-    """The blocks the wgmma architecture sweep compares one by one (tests/test_tc_arch_sweep_gpu.py, _tc_blocks) cover
+    """The blocks the wgmma architecture sweep compares one by one (tests/mlp_checks.py, tc_blocks) cover
     every element of every swept architecture's flat gradient exactly once, so no element goes unchecked; the xyz-
     encoding blocks sit on layer1 and the wide layers the skip rule allocates, and the direction-encoding block has the
     width of the direction encoding (at most 28 columns in the fused backward)."""
     import re
 
     from nerf_pytorch_b200 import ops
-    from test_tc_arch_sweep_gpu import ALL_ARCHS, ARCHS, _as_sd, _block, _spec, _tc_blocks
+    from mlp_checks import ALL_ARCHS, TC_ARCHS, as_state_dict, block, spec, tc_blocks
 
     for name in ALL_ARCHS:
-        arch = _spec(name)
-        assert ops.impl_supported(arch, 15, ops.IMPL_TC) == (name in ARCHS), name
+        arch = spec(name)
+        assert ops.impl_supported(arch, 15, ops.IMPL_TC) == (name in TC_ARCHS), name
         hits = torch.zeros(arch.flat_param_count(), dtype=torch.int32)
-        sd = _as_sd(arch, hits)
-        blocks = _tc_blocks(arch)
+        sd = as_state_dict(arch, hits)
+        blocks = tc_blocks(arch)
         for _, key, rows, cols, _ in blocks:
-            _block(sd[key], rows, cols).add_(1)
+            block(sd[key], rows, cols).add_(1)
         assert (hits == 1).all(), (name, int((hits == 0).sum()), int((hits > 1).sum()))
         wide = {f"layers_xyz.{i}" for i in range(arch.num_layers - 1) if i % arch.skip_every == 0 and i > 0}
         enc = {re.sub(r"\.weight.*", "", b[0]) for b in blocks if "xyz enc" in b[0]}
@@ -70,7 +70,7 @@ def test_tc_gradient_blocks_partition_the_flat_gradient():
         dirs = [b for b in blocks if "dir enc" in b[0]]
         if arch.use_viewdirs:
             assert len(dirs) == 1 and sd[dirs[0][1]][dirs[0][2], dirs[0][3]].shape == (64, arch.dim_dir), name
-            assert arch.dim_dir <= 28 or name not in ARCHS, name
+            assert arch.dim_dir <= 28 or name not in TC_ARCHS, name
         else:
             assert not dirs, name
 

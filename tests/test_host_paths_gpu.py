@@ -6,7 +6,7 @@ import math
 import pytest
 import torch
 
-from helpers import CASES, Case, pack_rays
+from helpers import CASES, Case, arch_of, build_models, pack_rays
 from oracle import nerf_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -155,7 +155,6 @@ def test_render_image_matches_run_one_iter_validation():
     """eval_utils.render_image (rays generated on the device from the pose, chunked forward) == run_one_iter_of_nerf in
     validation mode on get_ray_bundle's rays; uint8 conversions of eval_nerf.py:23-36."""
     import nerf_pytorch_b200 as nb
-    from test_render_parity_gpu import build_models
 
     c = Case("lego_a0_det_white_val")        # deterministic sampler, white background
     mc, mf, epf, edf = build_models(c)
@@ -181,11 +180,10 @@ def test_tc_out_of_range_activations_are_visible_not_clamped():
     """The fp16 x 2 operands cover |activation| < 1.05e6 (value / 16 in fp16): beyond that the wgmma forward produces
     inf / NaN (non-saturating conversions) instead of silently clamping -- and stays exact below."""
     from nerf_pytorch_b200 import ops
-    from test_stage_parity_gpu import _arch
 
     c = Case("lego_a0_train")
     rays, _, aux = c.aux()
-    arch = _arch(c)
+    arch = arch_of(c)
     z = aux["z_fine"].cuda().contiguous()
     flat = ops.flatten_state_dict(arch, c.sd_f, "cuda")
     for scale, expect_finite in ((1.0, True), (40.0, False)):

@@ -16,10 +16,9 @@ def _worker(rank, world, port, ret):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
                       LOCAL_RANK=str(rank))
     import torch.distributed as dist
-    from helpers import Case
+    from helpers import Case, build_models
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import parallel
-    from test_render_parity_gpu import build_models
 
     parallel.init_distributed()
     c = Case("a0_noview_coarse_only")

@@ -9,27 +9,9 @@ a fraction-of-elements criterion at rtol 1e-4."""
 import pytest
 import torch
 
-from helpers import CASES, Case, OUT_NAMES, err_stats, frac_close
+from helpers import CASES, Case, OUT_NAMES, build_models, err_stats, frac_close
 
 pytestmark = pytest.mark.gpu
-
-
-def build_models(c: Case, device="cuda"):
-    import nerf_pytorch_b200 as nb
-
-    def mk(sd):
-        m = nb.FlexibleNeRFModel(num_layers=c.num_layers, hidden_size=c.hidden, skip_connect_every=c.skip,
-                                 num_encoding_fn_xyz=c.enc_xyz[0], num_encoding_fn_dir=c.enc_dir[0],
-                                 include_input_xyz=c.enc_xyz[1], include_input_dir=c.enc_dir[1],
-                                 use_viewdirs=c.use_viewdirs)
-        m.load_state_dict(sd)
-        return m.to(device)
-
-    mc = mk(c.sd_c)
-    mf = mk(c.sd_f) if c.sd_f is not None else None
-    epf = nb.get_embedding_function(*c.enc_xyz)
-    edf = nb.get_embedding_function(*c.enc_dir) if c.use_viewdirs else None
-    return mc, mf, epf, edf
 
 
 def run_ours(c: Case, with_grad=False):

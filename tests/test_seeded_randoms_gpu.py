@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import Case, OUT_NAMES
+from helpers import Case, OUT_NAMES, bits_equal, build_models
 
 # ------------------------------------------------------------------------------------------------
 # numpy restatement of the stream (csrc/common.cuh)
@@ -166,24 +166,6 @@ def test_every_key_component_changes_the_words():
 # ------------------------------------------------------------------------------------------------
 # GPU: the render path consumes exactly that stream
 # ------------------------------------------------------------------------------------------------
-def _models(c: Case):
-    import nerf_pytorch_b200 as nb
-
-    def mk(sd):
-        m = nb.FlexibleNeRFModel(num_layers=c.num_layers, hidden_size=c.hidden, skip_connect_every=c.skip,
-                                 num_encoding_fn_xyz=c.enc_xyz[0], num_encoding_fn_dir=c.enc_dir[0],
-                                 include_input_xyz=c.enc_xyz[1], include_input_dir=c.enc_dir[1],
-                                 use_viewdirs=c.use_viewdirs)
-        m.load_state_dict(sd)
-        return m.cuda()
-
-    mc = mk(c.sd_c)
-    mf = mk(c.sd_f) if c.sd_f is not None else None
-    epf = nb.get_embedding_function(*c.enc_xyz)
-    edf = nb.get_embedding_function(*c.enc_dir) if c.use_viewdirs else None
-    return mc, mf, epf, edf
-
-
 def _tensors_of(rng, n, opts_train, fine):
     nc, nf = int(opts_train.num_coarse), int(opts_train.num_fine)
     d = dict(t_rand=_fill(rng, "t_rand", n, nc), noise_c=_fill(rng, "noise_c", n, nc))
@@ -211,12 +193,6 @@ def _step(c, mc, mf, epf, edf, options, randoms, impl, tgt=None, grad=True):
     return [o.detach().clone() if o is not None else None for o in out], loss, grads
 
 
-def _bits_equal(a, b):
-    if a is None or b is None:
-        return a is None and b is None
-    return a.shape == b.shape and torch.equal(a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
-
-
 # (golden case, overrides of options.nerf.train): A0 lego weights, A1 at init, NDC, coarse-only
 EXACT_CASES = {
     "perturb_noise": ("lego_a0_train", {}),
@@ -242,7 +218,7 @@ def test_seeded_step_equals_injected_tensors_bit_for_bit(key, impl):
     options = copy.deepcopy(c.options)
     for k, v in over.items():
         setattr(options.nerf.train, k, v)
-    mc, mf, epf, edf = _models(c)
+    mc, mf, epf, edf = build_models(c)
     if options.nerf.train.num_fine == 0:
         mf = None
     rng = SeededRandoms(0xC0FFEE, 17, 0)
@@ -251,12 +227,12 @@ def test_seeded_step_equals_injected_tensors_bit_for_bit(key, impl):
     tens = _tensors_of(rng, n, options.nerf.train, mf is not None)
     out_d, loss_d, g_d = _step(c, mc, mf, epf, edf, options, tens, impl)
     for nm, a, b in zip(OUT_NAMES, out_s, out_d):
-        assert _bits_equal(a, b), (key, nm)
-    assert _bits_equal(loss_s, loss_d), (loss_s.item(), loss_d.item())
+        assert bits_equal(a, b), (key, nm)
+    assert bits_equal(loss_s, loss_d), (loss_s.item(), loss_d.item())
     if impl == 1:
         # the wgmma backward sums its gradients in fixed point: the same inputs give the same bits
         for i, (a, b) in enumerate(zip(g_s, g_d)):
-            assert _bits_equal(a, b), (key, i)
+            assert bits_equal(a, b), (key, i)
     else:
         # the fp32 CUDA-core weight-gradient kernel flushes its partial sums with float atomics, so two runs on the same
         # inputs already differ in summation order: compare against that run-to-run spread
@@ -292,7 +268,7 @@ def _a1_models(seed=0):
 
 
 def _lego_models():
-    return _models(Case("lego_a0_train"))[:4]
+    return build_models(Case("lego_a0_train"))[:4]
 
 
 @gpu
@@ -323,8 +299,8 @@ def test_chunking_and_sharding_do_not_change_a_ray(impl):
     b, g_b = run(ro[k:], rd[k:], tgt[k:], n, rng.shifted(k))
     shards = [torch.cat([x, y]) for x, y in zip(a, b)]
     for nm, w, t, s in zip(OUT_NAMES, whole, thirds, shards):
-        assert _bits_equal(w, t), ("chunked", nm)
-        assert _bits_equal(w, s), ("sharded", nm)
+        assert bits_equal(w, t), ("chunked", nm)
+        assert bits_equal(w, s), ("sharded", nm)
     # gradients: the chunks' sums are added in fp32 afterwards, so they agree to that rounding (measured on an H100:
     # 5.6e-7 of the tensor's max on the fp32 kernels, 1.6e-7 on the wgmma kernels)
     worst = 0.0
@@ -353,8 +329,8 @@ def test_seeded_full_image_render_is_reproducible_across_chunk_sizes():
     again = render(4096, rng)
     other = render(1500, rng)
     for nm, a, b, c in zip(OUT_NAMES, first, again, other):
-        assert _bits_equal(a, b), ("twice", nm)
-        assert _bits_equal(a, c), ("chunk size", nm)
+        assert bits_equal(a, b), ("twice", nm)
+        assert bits_equal(a, c), ("chunk size", nm)
     # a different step renders different jitter
     assert not torch.equal(render(4096, nb.SeededRandoms(7, 1))[3], first[3])
     with pytest.raises(TypeError):
@@ -366,7 +342,7 @@ def test_seeded_step_leaves_torch_generators_alone_and_saves_no_noise():
     import nerf_pytorch_b200 as nb
 
     c = Case("lego_a0_train")
-    mc, mf, epf, edf = _models(c)
+    mc, mf, epf, edf = build_models(c)
     n = c.ro.shape[0]
     nc, nf = c.options.nerf.train.num_coarse, c.options.nerf.train.num_fine
     saved = []
@@ -401,7 +377,7 @@ def test_seeded_render_bwd_reads_no_noise_tensor(impl):
     from nerf_pytorch_b200 import ops, train_utils
 
     c = Case("fern_a0_ndc")  # noise std 1.0: many gates flip
-    mc, mf, epf, edf = _models(c)
+    mc, mf, epf, edf = build_models(c)
     o = c.options.nerf.train
     arch = train_utils._arch_of(mc, c.enc_xyz, c.enc_dir)
     _, blob_c = train_utils._packed(mc, arch)
@@ -422,9 +398,9 @@ def test_seeded_render_bwd_reads_no_noise_tensor(impl):
     out_d = ops.render_fwd(arch, arch, opts, blob_c, blob_f, rays, r, training=True, impl=impl)
     fg_d = torch.zeros(2 * nfl, device="cuda")
     ops.render_bwd(arch, arch, opts, blob_c, blob_f, rays, r, g_c, g_f, out_d[2], fg_d[:nfl], fg_d[nfl:], impl=impl)
-    assert _bits_equal(out_s[0], out_d[0]) and _bits_equal(out_s[1], out_d[1])
+    assert bits_equal(out_s[0], out_d[0]) and bits_equal(out_s[1], out_d[1])
     if impl == 1:
-        assert _bits_equal(fg_s, fg_d)
+        assert bits_equal(fg_s, fg_d)
     else:  # float atomics in the fp32 weight-gradient flush (see the step test)
         torch.testing.assert_close(fg_s, fg_d, rtol=1e-5, atol=1e-6 * fg_d.abs().max().item())
 
@@ -506,7 +482,7 @@ def test_sample_coarse_grid_is_torch_linspace_at_every_sample_count():
     for nc in range(2, 1025):
         z = ops.sample_coarse(rays, None, nc, False, False)
         want = torch.linspace(0.0, 1.0, nc, device="cuda").expand(3, nc)
-        assert _bits_equal(z, want), nc
+        assert bits_equal(z, want), nc
 
 
 @gpu
@@ -524,7 +500,7 @@ def test_sample_pdf_det_u_is_torch_linspace_at_every_fine_count():
         u = torch.linspace(0.0, 1.0, nf, device="cuda").expand(n, nf).contiguous()
         want = ops.sample_pdf_merge(zc, w, u, nf, want_aux=True)
         for a, b in zip(got, want):
-            assert _bits_equal(a, b), nf
+            assert bits_equal(a, b), nf
 
 
 @gpu
@@ -554,5 +530,5 @@ def test_seeded_fused_adam_training_is_bit_reproducible():
     l1, p1 = train()
     l2, p2 = train()
     print("seeded losses:", [round(x, 6) for x in l1.tolist()])
-    assert _bits_equal(l1, l2) and _bits_equal(p1, p2)
+    assert bits_equal(l1, l2) and bits_equal(p1, p2)
     assert l1[-1].item() < l1[0].item()

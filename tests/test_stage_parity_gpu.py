@@ -7,17 +7,9 @@ floor stated per test."""
 import pytest
 import torch
 
-from helpers import CASES, Case, err_stats, frac_close
+from helpers import CASES, Case, arch_of, err_stats, frac_close
 
 pytestmark = pytest.mark.gpu
-
-
-def _arch(c: Case):
-    from nerf_pytorch_b200 import ops
-
-    return ops.ArchSpec(num_layers=c.num_layers, hidden=c.hidden, skip_every=c.skip, use_viewdirs=c.use_viewdirs,
-                        n_freq_xyz=c.enc_xyz[0], n_freq_dir=c.enc_dir[0], include_input_xyz=c.enc_xyz[1],
-                        include_input_dir=c.enc_dir[1], log_sampling_xyz=c.enc_xyz[2], log_sampling_dir=c.enc_dir[2])
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -57,7 +49,7 @@ def test_mlp_forward(name):
     c = Case(name)
     rays, _, aux = c.aux()
     _, _, aux64 = c.aux(torch.float64)
-    arch = _arch(c)
+    arch = arch_of(c)
     for tag, sd in (("coarse", c.sd_c), ("fine", c.sd_f)):
         if sd is None:
             continue
@@ -180,7 +172,7 @@ def test_mlp_backward_matches_autograd(name):
 
     c = Case(name)
     rays, _, aux = c.aux()
-    arch = _arch(c)
+    arch = arch_of(c)
     sd = c.sd_c
     z = aux["z_coarse"]
     gen = torch.Generator().manual_seed(11)

@@ -1,8 +1,7 @@
 """GPU: the single-pass fp16 wgmma forward (impl 3, ops.IMPL_TC_FAST), the inference-only forward that issues one
 fp16(w) x fp16(activation / 16) product per k-step with fp32 accumulation instead of impl 1's three-term split.
   1. raw outputs against fp64 and against an fp64 oracle that rounds each gemm layer's weights and its input / 16 to
-     fp16 as the kernel does, over the hidden-128 architectures of test_tc_arch_sweep_gpu.py and the hidden-256 ones
-     of test_simt_hidden256_gpu.py;
+     fp16 as the kernel does, over the hidden-128 and hidden-256 architectures of mlp_checks.py;
   2. PSNR of whole renders of the shipped lego and fern checkpoints, fast against impl 1;
   3. bit-identical repeats, chunkings and seeded renders;
   4. the refusals: anything that trains, and every configuration the wgmma inference forward refuses;
@@ -15,10 +14,9 @@ import math
 import pytest
 import torch
 
-from helpers import OUT_NAMES, load_weights
-from test_simt_hidden256_gpu import ARCHS as H256_ARCHS
-from test_simt_hidden256_gpu import _embed, _oracle, _points, _report, arch_weights
-from test_tc_arch_sweep_gpu import ALL_ARCHS, FWD_TOL as PARITY_FWD_TOL, SHAPES, _shape
+from helpers import OUT_NAMES, bits_equal, load_weights
+from mlp_checks import (ALL_ARCHS, H256_ARCHS, SHAPES, STATES, TC_FWD_TOL, arch_weights, encodings, oracle, points,
+                        report, sms_shape, spec)
 
 pytestmark = pytest.mark.gpu
 
@@ -35,17 +33,9 @@ EMU_WORST = 1e-2       # against the fp16-rounding oracle, every point [4.2e-3]
 EMU_TOL = 1e-4
 FLIP_FRAC = {"init": 0.35, "scaled": 0.8}  # fraction of points beyond EMU_TOL [0.20, 0.60 (9 of 15 points)]
 
-# every architecture of those files the wgmma inference forward takes (8x256_ldir6's 39 direction channels are > 32)
-ARCHS = {**{f"h128_{k}": dict(hidden=128, **v) for k, v in ALL_ARCHS.items()},
-         **{f"h256_{k}": dict(hidden=256, skip_every=4, **v) for k, v in H256_ARCHS.items() if k != "8x256_ldir6"}}
-STATES = ["init", "scaled"]
+# every architecture of mlp_checks the wgmma inference forward takes (8x256_ldir6's 39 direction channels are > 32)
+ARCHS = [f"h128_{k}" for k in ALL_ARCHS] + [f"h256_{k}" for k in H256_ARCHS if k != "8x256_ldir6"]
 FWD_SHAPES = SHAPES + [("sms+1", 128)]  # the last: more tiles than SMs, so one CTA runs two
-
-
-def _spec(name):
-    from nerf_pytorch_b200 import ops
-
-    return ops.ArchSpec(**ARCHS[name])
 
 
 def _f16(x):
@@ -57,11 +47,9 @@ def _oracle_fp16(arch, sd, rays, z):
     """fp64 raw [P][4] of the network with every gemm layer computing fp16(input / 16) * 16 @ fp16(W)^T + b: the
     single-pass kernel's operands.  The heads (fc_alpha, fc_rgb, fc_out) and the direction-encoding columns of
     layers_dir.0 take fp64 inputs and weights, as the kernel's fp32 register dot products and per-ray bias do."""
-    n, s = z.shape
     H = arch.hidden
     sd = {k: v.double() for k, v in sd.items()}
-    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).reshape(-1, 3)  # fp32, as the kernel forms them
-    xyz = _embed(pts, arch.n_freq_xyz, arch.include_input_xyz, arch.log_sampling_xyz)
+    xyz, view = encodings(arch, rays, z)  # of the fp32 points, as the kernel forms them
 
     def gemm(x, w):
         return (_f16(x / 16) * 16) @ _f16(w).T
@@ -80,8 +68,6 @@ def _oracle_fp16(arch, sd, rays, z):
         h = torch.relu(layer(h, name))
     if not arch.use_viewdirs:
         return head(h, "fc_out")
-    vd = rays[:, None, 8:11].expand(n, s, 3).reshape(-1, 3)
-    view = _embed(vd, arch.n_freq_dir, arch.include_input_dir, arch.log_sampling_dir)
     feat = torch.relu(layer(h, "fc_feat"))
     w = sd["layers_dir.0.weight"]
     d = torch.relu(gemm(feat, w[:, :H]) + view @ w[:, H:].T + sd["layers_dir.0.bias"])
@@ -93,13 +79,13 @@ def _oracle_fp16(arch, sd, rays, z):
 # ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("state", STATES)
 @pytest.mark.parametrize("shape", FWD_SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")
-@pytest.mark.parametrize("name", list(ARCHS))
+@pytest.mark.parametrize("name", ARCHS)
 def test_fast_forward_matches_fp64_and_fp16_oracle(name, shape, state):
     from nerf_pytorch_b200 import ops
 
-    arch = _spec(name)
+    arch = spec(name.split("_", 1)[1])
     sd = arch_weights(arch, state)
-    rays, z = _points(arch, *_shape(shape), seed=1)
+    rays, z = points(arch, *sms_shape(shape), seed=1)
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, sd, "cuda"))
     ctx = (name, state, tuple(z.shape))
     assert ops.impl_supported(arch, z.shape[1], ops.IMPL_TC_FAST)
@@ -109,10 +95,10 @@ def test_fast_forward_matches_fp64_and_fp16_oracle(name, shape, state):
     got = fast.reshape(-1, 4).double().cpu()
     assert torch.isfinite(got).all(), ctx
 
-    want = _oracle(arch, sd, rays, z)[0]
+    want = oracle(arch, sd, rays, z)[0]
     scale = want.abs().amax(0)
     e64 = ((got - want).abs().amax(0) / scale).max().item()
-    _report("fast vs fp64", ctx, e64)
+    report("fast vs fp64", ctx, e64)
     assert e64 <= FAST_TOL, ctx + (e64,)
 
     emu = _oracle_fp16(arch, sd, rays, z)
@@ -120,17 +106,17 @@ def test_fast_forward_matches_fp64_and_fp16_oracle(name, shape, state):
     flipped = rel > EMU_TOL
     n_flip = int(flipped.sum())
     worst_rest = rel[~flipped].max().item() if n_flip < rel.numel() else 0.0
-    _report("fast vs fp16 oracle: worst unflipped point", ctx, worst_rest)
-    _report("fast vs fp16 oracle: fraction of points beyond EMU_TOL", ctx, n_flip / rel.numel())
-    _report("fast vs fp16 oracle: worst point", ctx, rel.max().item())
+    report("fast vs fp16 oracle: worst unflipped point", ctx, worst_rest)
+    report("fast vs fp16 oracle: fraction of points beyond EMU_TOL", ctx, n_flip / rel.numel())
+    report("fast vs fp16 oracle: worst point", ctx, rel.max().item())
     assert n_flip <= FLIP_FRAC[state] * rel.numel(), ctx + (n_flip, rel.numel())
     assert rel.max().item() <= EMU_WORST, ctx + (rel.max().item(),)
 
     # the single-pass kernel ran: its output is NOT within impl 1's parity bar
     e_tc = ((tc.reshape(-1, 4).double().cpu() - got).abs().amax(0) / scale).max().item()
-    _report("fast vs impl 1", ctx, e_tc)
+    report("fast vs impl 1", ctx, e_tc)
     if state == "scaled":
-        assert e_tc > PARITY_FWD_TOL, ctx + (e_tc,)
+        assert e_tc > TC_FWD_TOL, ctx + (e_tc,)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -198,9 +184,9 @@ def test_fast_render_psnr_against_impl1(view):
         assert torch.isfinite(a).all(), (view, out)
         p = _psnr(a, b)
         d = (a - b).abs()
-        _report(f"PSNR dB fast vs impl 1 {out}", (view,), p)
-        _report(f"max abs fast vs impl 1 {out}", (view,), d.max().item())
-        _report(f"fraction of pixels off by > 1/255 {out}", (view,), (d.amax(-1) > 1 / 255).double().mean().item())
+        report(f"PSNR dB fast vs impl 1 {out}", (view,), p)
+        report(f"max abs fast vs impl 1 {out}", (view,), d.max().item())
+        report(f"fraction of pixels off by > 1/255 {out}", (view,), (d.amax(-1) > 1 / 255).double().mean().item())
         assert p >= PSNR_BARS[(view, out)], (view, out, p)
     assert PSNR_BARS[("lego", "rgb_fine")] >= 45.0
 
@@ -208,12 +194,8 @@ def test_fast_render_psnr_against_impl1(view):
 # ------------------------------------------------------------------------------------------------------------------------
 # 3. determinism and chunking
 # ------------------------------------------------------------------------------------------------------------------------
-def _bits(t):
-    return None if t is None else t.contiguous().view(torch.int32)
-
-
 def _same_bits(x, y):
-    return all((a is None and b is None) or torch.equal(_bits(a), _bits(b)) for a, b in zip(x, y))
+    return all(bits_equal(a, b) for a, b in zip(x, y))
 
 
 def test_fast_render_is_bit_reproducible_and_chunking_invariant():
@@ -271,7 +253,7 @@ def test_library_refuses_the_fast_forward_wherever_it_would_train():
     arch = ops.ArchSpec(num_layers=4, hidden=128, n_freq_xyz=10)
     sd = arch_weights(arch, "init")
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, sd, "cuda"))
-    rays, z = _points(arch, 64, 64, seed=2)
+    rays, z = points(arch, 64, 64, seed=2)
     rays, z = rays.cuda(), z.cuda()
     before = ops.mlp_fwd(arch, blob, rays, z, impl=ops.IMPL_TC)
     _, stash = ops.mlp_fwd(arch, blob, rays, z, impl=ops.IMPL_TC, want_stash=True)
@@ -305,11 +287,11 @@ def test_fast_forward_is_refused_where_the_wgmma_inference_forward_is():
 
     arch = ops.ArchSpec(num_layers=4, hidden=128, n_freq_xyz=6)
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, arch_weights(arch, "init"), "cuda"))
-    rays, z = _points(arch, 9, 14, seed=12)
+    rays, z = points(arch, 9, 14, seed=12)
     rays, z = rays.cuda(), z.cuda()
     wide = ops.ArchSpec(num_layers=4, hidden=128, n_freq_xyz=11, include_input_xyz=False)
     blob_w = ops.pack_weights(wide, torch.zeros(wide.flat_param_count(), device="cuda"))
-    z64 = _points(wide, 9, 64, seed=13)[1].cuda()
+    z64 = points(wide, 9, 64, seed=13)[1].cuda()
     before = ops.mlp_fwd(arch, blob, rays, z, impl=ops.IMPL_SIMT)
     for a, b, zz, reason in ((arch, blob, z, "fewer than 15 samples"), (wide, blob_w, z64, "wider than 64")):
         assert not ops.impl_supported(a, zz.shape[1], ops.IMPL_TC_FWD)
@@ -336,7 +318,7 @@ def test_fast_out_of_range_operands_are_visible_not_clamped(what):
 
     arch = ops.ArchSpec(num_layers=4, hidden=128, n_freq_xyz=10)
     sd = arch_weights(arch, "init")
-    rays, z = _points(arch, 64, 64, seed=5)
+    rays, z = points(arch, 64, 64, seed=5)
     rays, z = rays.cuda(), z.cuda()
     flat = ops.flatten_state_dict(arch, sd, "cuda")
     layout = {name: (w_off, b_off, fin, fout) for name, w_off, b_off, fin, fout in arch.flat_layout()}

@@ -7,94 +7,14 @@ checkpoints; the asserts below are written against that (with headroom for the s
 import pytest
 import torch
 
-from helpers import CASES, Case, frac_close
-from test_stage_parity_gpu import _arch
+from helpers import Case, arch_of, build_models, frac_close
+from mlp_checks import (StashLayout, as_state_dict, check_blocks, mask_words, oracle, read_layer, relu_ties,
+                        tensor_blocks)
 
 pytestmark = pytest.mark.gpu
 
 TC_CASES = ["lego_a0_train", "fern_a0_ndc", "a1_skip_lindisp", "a0_noview_coarse_only"]
 TC_TRAIN_CASES = ["lego_a0_train", "fern_a0_ndc", "a1_skip_lindisp"]  # the fused backward needs the view-dependent heads
-
-
-def gemm_layers(arch):
-    """(name, out_features, cum_n) of the gemm layers in the library's order (heads skipped)."""
-    out, cum = [], 0
-    for name, _, _, _, fout in arch.flat_layout():
-        if fout >= 64:
-            out.append((name, fout, cum))
-            cum += fout
-    return out, cum
-
-
-def decode_tc_stash_layer(stash, n_points, cum_n, n):
-    """Operand tiles of the wgmma forward (csrc/tc_common.cuh "Operand tiles") -> activations [n_points][n] (fp64)."""
-    tiles = (n_points + 127) // 128
-    p_pad = tiles * 128
-    raw = stash.view(torch.int16)[2 * p_pad * cum_n: 2 * p_pad * (cum_n + n)]
-    t = raw.view(tiles, 2, 16, n // 8, 8, 8).view(torch.float16).double()     # [tile][hi|lo][pb][fb][p%8][f%8]
-    val = (t[:, 0] + t[:, 1] / 2048.0) * 16.0
-    return val.permute(0, 1, 3, 2, 4).reshape(p_pad, n)[:n_points]
-
-
-def decode_simt_stash_layer(stash, n_points, cum_n, n):
-    """fp32 rows with 16-byte chunks XOR-swizzled by (point & 7) inside each 128-byte segment (csrc/common.cuh swz_col)."""
-    x = stash[n_points * cum_n: n_points * (cum_n + n)].view(n_points, n // 32, 8, 4)
-    pt = torch.arange(n_points, device=stash.device) & 7
-    q = torch.arange(8, device=stash.device)
-    idx = (q[None, :] ^ pt[:, None])                                   # stored position of logical chunk q
-    return torch.gather(x, 2, idx[:, None, :, None].expand(n_points, n // 32, 8, 4)).reshape(n_points, n).double()
-
-
-def oracle_mlp_grads(c, sd, rays, z, G):
-    """fp64 autograd of the oracle MLP: d(sum(raw * G))/d(params)."""
-    from oracle import nerf_oracle as O
-
-    sd64 = {k: v.double().clone().requires_grad_(True) for k, v in sd.items()}
-    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).double()  # fp32 points, then promoted (train_utils.py:67)
-    raw64 = O.run_network(sd64, pts, rays.double(), 1 << 20, c.enc_xyz, c.enc_dir if c.use_viewdirs else None)
-    (raw64 * G.double()).sum().backward()
-    return {k: v.grad for k, v in sd64.items()}
-
-
-def oracle_mlp_acts(c, sd, rays, z):
-    """fp64 activations of every gemm layer of the oracle MLP, in the library's gemm order: [P][n] each."""
-    from oracle import nerf_oracle as O
-
-    sd64 = {k: v.double() for k, v in sd.items()}
-    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).double().reshape(-1, 3)
-    emb = O.positional_encoding(pts, *c.enc_xyz)
-    dim_xyz = emb.shape[-1]
-    if c.use_viewdirs:
-        vd = rays[:, None, -3:].double().expand(z.shape[0], z.shape[1], 3).reshape(-1, 3)
-        emb = torch.cat((emb, O.positional_encoding(vd, *c.enc_dir)), -1)
-    _, acts = O.flexible_nerf_forward(sd64, emb, dim_xyz, return_acts=True)
-    out, i = [acts["h0"]], 1
-    while f"h{i}" in acts:
-        out.append(acts[f"h{i}"])
-        i += 1
-    if c.use_viewdirs:
-        out += [acts["feat"], acts["d"]]
-    return out
-
-
-def tc_mask_view(arch, stash, n_points, layer_index, layers, cum_total):
-    """The ReLU bit-mask words of gemm layer `layer_index` inside a wgmma forward stash: int32 [P][n/32]."""
-    p_pad = (n_points + 127) // 128 * 128
-    enc_tile_w = (arch.dim_xyz + 15) & ~15
-    dir_pad = (arch.dim_dir + 7) & ~7
-    mask_base = cum_total + enc_tile_w + dir_pad
-    mask_cum = sum(n // 32 for _, n, _ in layers[:layer_index])
-    n = layers[layer_index][1]
-    start = p_pad * (mask_base + mask_cum)
-    return stash.view(torch.int32)[start:start + n_points * (n // 32)].view(n_points, n // 32)
-
-
-def pack_mask(act):
-    """bool [P][n] -> int32 words [P][n/32], bit j of word w = column 32 w + j."""
-    P, n = act.shape
-    b = act.view(P, n // 32, 32).to(torch.int64)
-    w = (b << torch.arange(32, device=act.device, dtype=torch.int64)).sum(-1)
-    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
 
 
 @pytest.mark.parametrize("name", TC_CASES)
@@ -103,8 +23,8 @@ def test_tc_forward_matches_simt_and_oracle(name):
 
     c = Case(name)
     rays, _, aux = c.aux()
-    arch = _arch(c)
-    layers, _ = gemm_layers(arch)
+    arch = arch_of(c)
+    layers = StashLayout(arch).layers
     for tag, sd in (("coarse", c.sd_c), ("fine", c.sd_f)):
         if sd is None:
             continue
@@ -123,8 +43,8 @@ def test_tc_forward_matches_simt_and_oracle(name):
         # the stash the backward consumes: every layer's activation tile decodes to the fp32 kernel's activations
         P = z.numel()
         for lname, n, cum in layers:
-            a0 = decode_simt_stash_layer(st0, P, cum, n)
-            a1 = decode_tc_stash_layer(st1, P, cum, n)
+            a0 = read_layer(st0, P, cum, n, "fp32")
+            a1 = read_layer(st1, P, cum, n, "wgmma")
             s = a0.abs().max().item()
             assert (a1 - a0).abs().max().item() <= 3e-5 * s + 1e-7, (tag, lname, (a1 - a0).abs().max().item(), s)
 
@@ -149,9 +69,7 @@ def test_tc_forward_hidden_256_matches_oracle_and_fp32_kernel(viewdirs):
     raw0 = ops.mlp_fwd(arch, blob, rays.cuda(), z.cuda(), impl=ops.IMPL_SIMT)
     raw1 = ops.mlp_fwd(arch, blob, rays.cuda(), z.cuda(), impl=ops.IMPL_TC)
     torch.cuda.synchronize()
-    sd64 = {k: v.double() for k, v in sd.items()}
-    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).double()
-    want = O.run_network(sd64, pts, rays.double(), 1 << 20, (10, True, True), (4, True, True) if viewdirs else None)
+    want = oracle(arch, sd, rays, z)[0].view(n, s_, 4)
     scale = want.abs().max().item()
     e_tc = (raw1.cpu().double() - want).abs().max().item()
     e_simt = (raw0.cpu().double() - want).abs().max().item()
@@ -209,7 +127,7 @@ def test_tc_ragged_tail_and_sizes():
     from nerf_pytorch_b200 import ops
 
     c = Case("lego_a0_train")
-    arch = _arch(c)
+    arch = arch_of(c)
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, c.sd_f, "cuda"))
     g = torch.Generator().manual_seed(5)
     for n, s in ((1, 64), (3, 192), (7, 50), (33, 17), (129, 100)):
@@ -223,17 +141,6 @@ def test_tc_ragged_tail_and_sizes():
         assert (r1 - r0).abs().max().item() <= 3e-5 * scale + 1e-6, (n, s, (r1 - r0).abs().max().item(), scale)
 
 
-def _check_grads(arch, got_flat, want_sd, tol, ctx):
-    for lname, w_off, b_off, fin, fout in arch.flat_layout():
-        gw = got_flat[w_off:w_off + fin * fout].view(fout, fin).double().cpu()
-        gb = got_flat[b_off:b_off + fout].double().cpu()
-        for got, want, what in ((gw, want_sd[lname + ".weight"], "weight"), (gb, want_sd[lname + ".bias"], "bias")):
-            want = want.double().cpu()
-            scale = want.abs().max().item() + 1e-30
-            e = (got - want).abs().max().item()
-            assert e <= tol * scale, ctx + (lname, what, e, scale)
-
-
 @pytest.mark.parametrize("name", TC_TRAIN_CASES)
 def test_tc_backward_matches_fp64_oracle(name):
     """The fused wgmma backward (data-gradient chain + every weight gradient in one kernel) against fp64 autograd of
@@ -242,7 +149,7 @@ def test_tc_backward_matches_fp64_oracle(name):
 
     c = Case(name)
     rays, _, aux = c.aux()
-    arch = _arch(c)
+    arch = arch_of(c)
     for tag, sd in (("coarse", c.sd_c), ("fine", c.sd_f)):
         if sd is None:
             continue
@@ -251,7 +158,7 @@ def test_tc_backward_matches_fp64_oracle(name):
         G = torch.randn(z.shape[0], z.shape[1], 4, generator=gen)
         # realistic upstream gradients span decades across the samples of a ray (compositing weights): scale the rows
         G = G * torch.exp(torch.randn(z.shape[0], z.shape[1], 1, generator=gen) * 3.0)
-        want = oracle_mlp_grads(c, sd, rays, z, G)
+        _, acts, _, want = oracle(arch, sd, rays, z, G)
         blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, sd, "cuda"))
         zc, Gc = z.cuda().contiguous(), G.cuda().contiguous()
         _, stash = ops.mlp_fwd(arch, blob, rays.cuda(), zc, impl=ops.IMPL_TC, want_stash=True)
@@ -259,37 +166,11 @@ def test_tc_backward_matches_fp64_oracle(name):
         # arithmetic (fp64 oracle / fp32 reference / split-precision forward) -- a genuine discontinuity of the
         # function, not a property of the backward.  Count the forward's disagreements with the fp64 oracle, check
         # each is such a tie, then give the backward the oracle's masks so the comparison below measures the
-        # backward's arithmetic alone.
-        layers, cum_total = gemm_layers(arch)
-        acts = oracle_mlp_acts(c, sd, rays, z)
-        P = z.numel()
-        n_ties = 0
-        for li, (lname, n, _) in enumerate(layers):
-            if li == 0:
-                continue  # layer1 has no ReLU (models.py:238)
-            mv = tc_mask_view(arch, stash, P, li, layers, cum_total)
-            wantm = pack_mask((acts[li] > 0).cuda())
-            diff = (mv ^ wantm).ne(0)
-            if diff.any():
-                a = acts[li].cuda()
-                bits = ((mv ^ wantm).unsqueeze(-1) >> torch.arange(32, device="cuda", dtype=torch.int32)) & 1
-                flipped = bits.view(P, n).bool()
-                n_ties += int(flipped.sum())
-                # every disagreement sits within 2e-5 of the layer's scale of zero
-                assert a[flipped].abs().max().item() <= 2e-5 * a.abs().max().item(), (name, tag, lname)
-            mv.copy_(wantm)
-        assert n_ties <= 1e-5 * P * cum_total + 2, (name, tag, n_ties)
+        # backward's arithmetic alone.  Every disagreement sits within 2e-5 of the layer's scale of zero.
+        n_ties = relu_ties(arch, stash, z.numel(), acts, "wgmma", 2e-5, (name, tag), adopt=True)
         g1, _ = ops.mlp_bwd(arch, blob, rays.cuda(), zc, Gc, stash, impl=ops.IMPL_TC)
         torch.cuda.synchronize()
-        _check_grads(arch, g1, want, 2e-5, (name, tag, f"{n_ties} relu ties patched"))
-
-
-def _as_sd(arch, flat):
-    out = {}
-    for lname, w_off, b_off, fin, fout in arch.flat_layout():
-        out[lname + ".weight"] = flat[w_off:w_off + fin * fout].view(fout, fin)
-        out[lname + ".bias"] = flat[b_off:b_off + fout]
-    return out
+        check_blocks(arch, g1, want, tensor_blocks(arch), 2e-5, (name, tag, f"{n_ties} relu ties patched"), None)
 
 
 def test_tc_backward_ragged_sizes():
@@ -299,7 +180,7 @@ def test_tc_backward_ragged_sizes():
 
     for case in ("lego_a0_train", "a1_skip_lindisp"):
         c = Case(case)
-        arch = _arch(c)
+        arch = arch_of(c)
         blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, c.sd_f, "cuda"))
         g = torch.Generator().manual_seed(7)
         for n, s in ((1, 16), (7, 50), (33, 17), (5, 37), (129, 100)):
@@ -312,17 +193,11 @@ def test_tc_backward_ragged_sizes():
             _, st0 = ops.mlp_fwd(arch, blob, rays, z, impl=ops.IMPL_SIMT, want_stash=True)
             _, st1 = ops.mlp_fwd(arch, blob, rays, z, impl=ops.IMPL_TC, want_stash=True)
             # same ReLU decisions for both (see test_tc_backward_matches_fp64_oracle): copy the fp32 kernel's masks
-            layers, cum_total = gemm_layers(arch)
-            P = n * s
-            for li in range(1, len(layers)):
-                n_l = layers[li][1]
-                mask_cum = sum(m // 32 for _, m, _ in layers[:li])
-                mask_base = cum_total + ((arch.dim_xyz + 15) & ~15) + ((arch.dim_dir + 7) & ~7)
-                simt_words = st0.view(torch.int32)[P * (mask_base + mask_cum):P * (mask_base + mask_cum) + P * (n_l // 32)]
-                tc_mask_view(arch, st1, P, li, layers, cum_total).copy_(simt_words.view(P, n_l // 32))
+            for li in range(1, len(StashLayout(arch).layers)):
+                mask_words(arch, st1, n * s, li, "wgmma").copy_(mask_words(arch, st0, n * s, li, "fp32"))
             g0, _ = ops.mlp_bwd(arch, blob, rays, z, G, st0, impl=ops.IMPL_SIMT)
             g1, _ = ops.mlp_bwd(arch, blob, rays, z, G, st1, impl=ops.IMPL_TC)
-            _check_grads(arch, g1, _as_sd(arch, g0), 3e-5, (case, n, s))
+            check_blocks(arch, g1, as_state_dict(arch, g0), tensor_blocks(arch), 3e-5, (case, n, s), None)
 
 
 def test_tc_backward_accumulates_and_repeats():
@@ -332,7 +207,7 @@ def test_tc_backward_accumulates_and_repeats():
 
     c = Case("a1_skip_lindisp")
     rays, _, aux = c.aux()
-    arch = _arch(c)
+    arch = arch_of(c)
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, c.sd_c, "cuda"))
     z = aux["z_coarse"].cuda().contiguous()
     G = torch.randn(z.shape[0], z.shape[1], 4, generator=torch.Generator().manual_seed(3)).cuda()
@@ -368,7 +243,6 @@ def test_tc_unsupported_configs_are_refused():
 @pytest.mark.parametrize("name", ["lego_a0_train", "a1_skip_lindisp"])
 def test_tc_end_to_end_against_reference_golden(name):
     import nerf_pytorch_b200 as nb
-    from test_render_parity_gpu import build_models
 
     c = Case(name)
     mc, mf, epf, edf = build_models(c)

@@ -8,9 +8,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from helpers import Case  # noqa: E402
-from test_stage_parity_gpu import _arch  # noqa: E402
-from test_tc_gpu import oracle_mlp_grads  # noqa: E402
+from helpers import Case, arch_of  # noqa: E402
+from mlp_checks import oracle  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
 
 
@@ -35,7 +34,7 @@ def report(tag, arch, flat, want):
 
 for case in ("lego_a0_train", "a1_skip_lindisp"):
     c = Case(case)
-    arch = _arch(c)
+    arch = arch_of(c)
     sd = c.sd_f
     blob = ops.pack_weights(arch, ops.flatten_state_dict(arch, sd, "cuda"))
     g = torch.Generator().manual_seed(7)
@@ -45,7 +44,7 @@ for case in ("lego_a0_train", "a1_skip_lindisp"):
                           torch.full((n, 1), 2.0), torch.full((n, 1), 6.0), d / d.norm(dim=-1, keepdim=True)], -1)
         z = torch.sort(torch.rand(n, s, generator=g) * 4 + 2, -1).values
         G = torch.randn(n, s, 4, generator=g)
-        want = oracle_mlp_grads(c, sd, rays, z, G)
+        want = oracle(arch, sd, rays, z, G)[3]
         rc, zc, Gc = rays.cuda().contiguous(), z.cuda().contiguous(), G.cuda().contiguous()
         print(case, n, s)
         for impl, tag in ((ops.IMPL_SIMT, "simt"), (ops.IMPL_TC, "tc  ")):
