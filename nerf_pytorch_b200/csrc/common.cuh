@@ -177,7 +177,8 @@ int64_t bwd_tc_scratch_floats(const Plan& p);
 // Stash row swizzle.  The activation / gradient stashes ([points][n] fp32, workspace private to this library) keep
 // every 16-byte chunk of a row at chunk index (q ^ (point & 7)) inside its 128-byte segment.  Global access
 // patterns are unchanged (a permutation inside each 128 B line), and a 128-row tile of the stash is byte-identical
-// to a bank-conflict-free shared-memory tile, so the tensor-core kernels write it with ONE cp.async.bulk per layer.
+// to a bank-conflict-free shared-memory tile.  The fp32 kernels use it; the tensor-core kernels stash operand tiles
+// instead (tc_common.cuh "Operand tiles"), written from the epilogue registers.
 __device__ __forceinline__ int swz_col(int col, int64_t point) { return (((col >> 2) ^ (int)(point & 7)) << 2) | (col & 3); }
 
 // Positional encoding of one scalar coordinate (nerf_helpers.py:113-157): writes x (if include) and

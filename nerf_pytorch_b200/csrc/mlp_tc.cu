@@ -18,8 +18,9 @@
 //              memory, the next layer's A operand.  Training: the same hi / lo registers also go to the activation
 //              stash as an operand tile (tc_common.cuh "Operand tiles"), plus one ReLU bit per activation.
 //              The two warpgroups run independently; each one's epilogue overlaps the other's MMAs.
-//   last warp  weight producer: one cp.async.bulk per ring stage (24 KB) from the L2-resident blob, mbarrier
-//              complete_tx; a stage is free again once every consumer warp has seen its MMAs complete.
+//   last warp  weight producer: fills the weight ring (tc_common.cuh WeightRing) with one cp.async.bulk per 24 KB
+//              stage from the L2-resident blob, mbarrier complete_tx; a stage is free again once every consumer warp
+//              has seen its MMAs complete.
 // The direction encoding enters layers_dir[0] through a per-ray fp32 bias computed on the CUDA cores (it is constant
 // along a ray: SURVEY.md section 7.3 item 5), so that layer contracts over K = H only.
 //
@@ -31,16 +32,12 @@
 // prologue and the epilogue write only the hi half of the operand tiles.
 #include "common.cuh"
 #include "tc_common.cuh"
-#include "wgmma.cuh"
 
 namespace nerfb200 {
 
 namespace tc {
 constexpr int kStepsPerStage = 2;                       // k-steps per ring stage at N <= 128
 constexpr int kStageBytes = kStepsPerStage * 96 * 128;  // 24 KB: 3 copies x 2 slabs x 128 rows x 16 B per k-step
-constexpr int kMaxStages = 6;
-constexpr int kMaxRaysPerTile = 10;
-constexpr int kSmemLimit = 232448 - 1024;               // 227 KB minus the alignment slack
 
 __host__ __device__ inline int n_wg(int hidden) { return hidden == 128 ? 2 : 1; }  // consumer warpgroups = tile / 64
 
@@ -60,12 +57,9 @@ __host__ __device__ inline SmemMap smem_map(const Plan& p) {
   m.encd = off;      off += n_wg(p.hidden) * kMaxRaysPerTile * 32 * 4;
   m.wv = off;        off += 32 * (p.hidden / 2) * 4;  // direction-encoding rows of layers_dir[0]'s weight: Wt[k_h + k][n]
   m.bars = off;      off += 256;
-  off = (off + 1023) & ~1023;
-  m.ring = off;
-  int ns = (kSmemLimit - off) / kStageBytes;
-  if (ns > kMaxStages) ns = kMaxStages;
-  m.n_stages = ns;
-  m.total = off + (ns > 0 ? ns : 0) * kStageBytes;
+  m.ring = (off + 1023) & ~1023;
+  m.n_stages = ring_depth(m.ring, kStageBytes);
+  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * kStageBytes;
   return m;
 }
 
@@ -90,22 +84,10 @@ __device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, in
   return mi;
 }
 
-struct Pipe2 {  // ring position + the stage whose MMAs are still in flight
-  Pipe pp;
-  uint32_t prev = 0;
-  bool has_prev = false;
-};
-
 }  // namespace tc
 
 using namespace tc;
-
-// per-tile state a consumer thread carries over the layers: its two accumulator rows
-struct RowState {
-  int64_t pt[2];
-  bool valid[2];
-  int ray_slot[2];
-};
+using Ring = WeightRing<kStageBytes>;
 
 // One layer of one warpgroup: MMAs over the ring, then the epilogue on the accumulator fragment.
 // Fragment of wgmma m64nN (per warp 16 rows): thread (warp wi, lane) holds rows r = 16 wi + lane / 4 (+ 8) and columns
@@ -113,16 +95,15 @@ struct RowState {
 template <bool kTrain, bool kFast, int N>
 __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, float* __restrict__ raw, float* __restrict__ stash,
                                           uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t tile,
-                                          int64_t P_pad, const RowState& rs, Pipe2& pl, uint32_t bar_full,
-                                          uint32_t bar_empty, uint32_t n_stages, const float* s_bias, const float* s_headw,
-                                          const float* s_headb, const float* viewb, int hw1) {
+                                          int64_t P_pad, const RowState& rs, Ring& ring, const float* s_bias,
+                                          const float* s_headw, const float* s_headb, const float* viewb, int hw1) {
   static_assert(!(kTrain && kFast), "the single-pass forward is inference only");
   constexpr int kSps = kFast ? fast_sps(N) : kStepsPerStage;  // k-steps a ring stage can hold
   const int wt = threadIdx.x & 127, wi = wt >> 5, lane = wt & 31, q = lane & 3;
   const GemmLayer& g = p.g[e];
   const MmaInfo mi = mma_info(p, blob, e, kFast);
   const int enc_w = p.enc_tile_w;
-  const uint32_t act_a = smem_u32(sm + mp.act), enc_a = smem_u32(sm + mp.enc), ring_a = smem_u32(sm + mp.ring);
+  const uint32_t act_a = smem_u32(sm + mp.act), enc_a = smem_u32(sm + mp.enc);
   const int fin = g.k_h > 0 ? g.k_h : 16;
   // this warpgroup's 64 rows of the K-major operand tiles (SBO = next 8 points, LBO = next 8 features)
   const uint64_t a_hi0 = make_desc(act_a + (uint32_t)(wg * 64 * fin * 2), 128, (uint32_t)fin * 16);
@@ -130,15 +111,14 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
   const uint64_t e_hi0 = make_desc(enc_a + (uint32_t)(wg * 64 * enc_w * 2), 128, (uint32_t)enc_w * 16);
   const uint32_t e_lo_off = (uint32_t)(rows * enc_w * 2);
   const uint32_t slab_b = 16u * (uint32_t)N;
-  const uint64_t b_ring = make_desc(ring_a, slab_b, 128);
+  const uint64_t b_ring = make_desc(ring.base, slab_b, 128);
 
   float acc[N / 2];
 #pragma unroll
   for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
   wgmma_fence();
   for (int ks0 = 0; ks0 < mi.ksteps; ks0 += mi.sps) {
-    const uint32_t st = pl.pp.stage;
-    mbar_wait(bar_full + 8 * st, pl.pp.phase);
+    const uint32_t st = ring.acquire();
     const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStageBytes);
 #pragma unroll
     for (int hh = 0; hh < kSps; ++hh) {
@@ -163,27 +143,15 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
       }
     }
     wgmma_commit();
-    if (pl.has_prev) {  // the previous stage's MMAs are complete: hand it back to the producer
-      wgmma_wait<1>();
-      reg_fence(acc);
-      if (lane == 0) mbar_arrive(bar_empty + 8 * pl.prev);
-    }
-    pl.prev = st;
-    pl.has_prev = true;
-    pl.pp.advance(n_stages);
+    ring.release_behind(acc);
   }
-  wgmma_wait<0>();
-  reg_fence(acc);
-  if (lane == 0) mbar_arrive(bar_empty + 8 * pl.prev);
-  pl.has_prev = false;
+  ring.release_last(acc);
 
   // ---------------- epilogue ----------------
   const int wg_bar_id = 1 + wg;
   asm volatile("bar.sync %0, 128;" ::"r"(wg_bar_id) : "memory");  // every warp's MMAs have read the activation tile
   const bool has_next = e + 1 < p.n_gemm;
-  int hsel = -1;
-  if (p.h[0].src == e) hsel = 0;
-  if (p.n_head > 1 && p.h[1].src == e) hsel = 1;
+  const int hsel = head_of(p, e);
   const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
   const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
   const bool is_dir = p.use_viewdirs && e == p.n_gemm - 1;
@@ -267,7 +235,7 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
         hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 2);
       }
       if (q == 0 && rs.valid[i])
-        for (int c = 0; c < hn; ++c) raw[rs.pt[i] * 4 + hcol + c] = hacc[i][c] + s_headb[hsel * 4 + c];
+        for (int c = 0; c < hn; ++c) raw[(int64_t)rs.pt[i] * 4 + hcol + c] = hacc[i][c] + s_headb[hsel * 4 + c];
     }
   }
 }
@@ -282,18 +250,14 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
                   float* __restrict__ raw,          // out [P][4]
                   float* __restrict__ stash) {      // out (kTrain)
   constexpr int kWG = kH == 128 ? 2 : 1, kRows = 64 * kWG, kThreads = 128 * kWG + 32;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // 1 KB aligned base
+  uint8_t* sm = smem_base();
   const SmemMap mp = smem_map(p);
   float* s_bias = reinterpret_cast<float*>(sm + mp.bias);
   float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
   float* s_viewb = reinterpret_cast<float*>(sm + mp.viewb);
   float* s_encd = reinterpret_cast<float*>(sm + mp.encd);
   float* s_wv = reinterpret_cast<float*>(sm + mp.wv);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + mp.bars);
-  const uint32_t bar_full = smem_u32(bars);                // [kMaxStages]  weights landed
-  const uint32_t bar_empty = bar_full + 8 * kMaxStages;    // [kMaxStages]  stage consumed by every consumer warp
-  const uint32_t n_stages = (uint32_t)mp.n_stages;
+  Ring ring{smem_u32(sm + mp.ring), smem_u32(sm + mp.bars), (uint32_t)mp.n_stages};
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
@@ -301,10 +265,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   const int enc_w = p.enc_tile_w;                  // encoding operand tile width (dim_xyz padded to 16)
 
   if (tid == 0) {
-    for (int i = 0; i < kMaxStages; ++i) {
-      mbar_init(&bars[i], 1);
-      mbar_init(&bars[kMaxStages + i], 4 * kWG);
-    }
+    ring.init(4 * kWG);
     fence_barrier_init();
   }
   // biases (/16) + head weights (x16, they multiply activation / 16): once per CTA
@@ -330,60 +291,38 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   if (warp == 4 * kWG) {
     // ===================== weight producer =====================
     if ((tid & 31) == 0) {
-      Pipe pp;
       const uint64_t pol = l2_policy_evict_last();
-      const uint32_t ring_a = smem_u32(sm + mp.ring);
       for (int j = 0; j < my_tiles; ++j)
         for (int e = 0; e < p.n_gemm; ++e) {
           const MmaInfo mi = mma_info(p, blob, e, kFast);
           for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
-            if (kFast) {  // the hs part of each k-step: one bulk copy each, their sum on the stage's barrier
-              const int nk = min(mi.sps, mi.ksteps - ks);
-              const uint32_t hs_bytes = mi.kbytes / 3, full = bar_full + 8 * pp.stage;
-              mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1);
-              mbar_arrive_expect_tx(full, (uint32_t)nk * hs_bytes);
-              for (int hh = 0; hh < nk; ++hh)
-                bulk_g2s_hint(ring_a + pp.stage * kStageBytes + hh * hs_bytes, mi.src + (size_t)(ks + hh) * mi.kbytes,
-                              hs_bytes, full, pol);
-              pp.advance(n_stages);
-              continue;
-            }
-            const uint32_t bytes = (uint32_t)min(mi.sps, mi.ksteps - ks) * mi.kbytes;
-            mbar_wait(bar_empty + 8 * pp.stage, pp.phase ^ 1);
-            mbar_arrive_expect_tx(bar_full + 8 * pp.stage, bytes);
-            bulk_g2s_hint(ring_a + pp.stage * kStageBytes, mi.src + (size_t)ks * mi.kbytes, bytes, bar_full + 8 * pp.stage,
-                          pol);
-            pp.advance(n_stages);
+            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
+            const uint8_t* src = mi.src + (size_t)ks * mi.kbytes;
+            if (kFast)  // the hs part of each k-step: one bulk copy each
+              ring.fill(src, nk, mi.kbytes / 3, mi.kbytes, pol);
+            else        // the k-steps' three copies are contiguous in the blob: one bulk copy
+              ring.fill(src, 1, nk * mi.kbytes, 0, pol);
           }
         }
     }
   } else {
     // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
-    const int wg = warp >> 2, wt = tid & 127, lane = tid & 31;
+    const int wg = warp >> 2, wt = tid & 127;
     const int row = wt & 63, half = wt >> 6;       // prologue: two threads per row split the frequencies
     const int vbs = kH / 2;
     float* viewb = s_viewb + wg * kMaxRaysPerTile * vbs;
     float* encd = s_encd + wg * kMaxRaysPerTile * 32;
     uint8_t* enc = sm + mp.enc;
     const int enc_hb = kRows * enc_w * 2;          // bytes of the hi (or lo) block of the encoding tile
-    Pipe2 pl;
     auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
 #pragma unroll 1
     for (int j = 0; j < my_tiles; ++j) {
       const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
       const int64_t p0 = tile * kRows + 64 * wg;   // first point of this warpgroup
-      // fewer than 2^31 points per call (checked on the host): 32-bit divisions instead of emulated 64-bit ones
-      const int64_t first_ray = (int64_t)((uint32_t)(p0 < P ? p0 : P - 1) / (uint32_t)S);
-      const int64_t last_pt = (p0 + 63 < P) ? p0 + 63 : P - 1;
-      const int n_rays_wg = (int)((uint32_t)last_pt / (uint32_t)S) - (int)first_ray + 1;
-      RowState rs;
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int64_t pt = p0 + 16 * (wt >> 5) + (lane >> 2) + 8 * i;
-        rs.valid[i] = pt < P;
-        rs.pt[i] = pt < P ? pt : P - 1;
-        rs.ray_slot[i] = (int)((uint32_t)rs.pt[i] / (uint32_t)S - first_ray);
-      }
+      const TileRays tr = tile_rays(p0, 64, P, S);
+      const int64_t first_ray = tr.first;
+      const int n_rays_wg = tr.n;
+      const RowState rs = row_state(p0, 16 * (wt >> 5) + ((tid & 31) >> 2), P, S, first_ray);
       // ================= encodings of this row -> operand tile (value / 16), the two halves split the frequencies
       if (kTrain) {  // the previous tile's encoding store must have finished reading the tile
         if (wt == 0) bulk_wait_read();
@@ -448,11 +387,11 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll 1
       for (int e = 0; e < p.n_gemm; ++e) {
         if (p.g[e].n == kH)
-          fwd_layer<kTrain, kFast, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full,
-                                       bar_empty, n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+          fwd_layer<kTrain, kFast, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, ring, s_bias,
+                                    s_headw, s_headb, viewb, hw1);
         else
-          fwd_layer<kTrain, kFast, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, pl, bar_full,
-                                           bar_empty, n_stages, s_bias, s_headw, s_headb, viewb, hw1);
+          fwd_layer<kTrain, kFast, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, ring, s_bias,
+                                        s_headw, s_headb, viewb, hw1);
       }
     }
     if (kTrain && wt == 0) bulk_wait_all();  // this warpgroup's encoding-tile stores
@@ -489,15 +428,8 @@ static int launch_fwd(const Plan& p, const float* blob, const float* rays, int r
   constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
   const int64_t tiles = (P + kRows - 1) / kRows;
   const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // = tiles whenever the stash is written (hidden 128)
-  const int sms = device_sms();
-  const int grid = (int)(tiles < sms ? tiles : sms);
-  const size_t bytes = (size_t)smem_map(p).total + 1024;
-  auto kern = mlp_fwd_tc_kernel<kTrain, kH, kFast>;
-  int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes), what);
-  if (rc) return rc;
-  kern<<<grid, kThreads, bytes, s>>>(p, blob, rays, ray_stride, z, P, n_samples, kTrain ? stash_tiles : tiles, raw, stash);
-  count_launch();
-  return check_cuda(cudaGetLastError(), what);
+  return launch_persistent(mlp_fwd_tc_kernel<kTrain, kH, kFast>, tiles, kThreads, smem_map(p).total, s, what, p, blob,
+                           rays, ray_stride, z, P, n_samples, kTrain ? stash_tiles : tiles, raw, stash);
 }
 
 // stash non-null: the training forward; fast: the single-pass forward (never with a stash)

@@ -18,34 +18,31 @@
 //
 // Persistent kernel, one CTA per SM, two consumer warpgroups (warpgroup w owns points [64 w, 64 w + 64) of the chain
 // and features [64 w, 64 w + 64) of every weight gradient) and one producer warpgroup, of which one thread streams the
-// chain's weight copies through a cp.async.bulk ring; the producer gives its registers to the consumers (setmaxnreg), which
-// hold the chain accumulator and a job accumulator at once.  Every wgmma is issued in warpgroup-uniform control flow (the
-// warp index is broadcast from lane 0), so ptxas keeps the MMAs of a k-loop asynchronous.  Per layer: epilogue (chain
-// accumulator + head term, ReLU mask, split -> G tile), chain MMA of the warpgroup's rows, then the layer's
-// weight-gradient jobs: A = the G tile (MN-major), B = the activation tile (bulk-copied from the stash one job ahead and
-// requested as soon as both warpgroups' MMAs of the running job are complete), the 16-column ray-indicator job that yields the bias gradients and
-// the per-ray sums of layers_dir[0], and the two narrow heads' jobs with the roles swapped (A = activation tile, B =
-// d_raw = feature rows 64..79 of the first layer's G tile).  Finished weight-gradient accumulators are unscaled,
-// converted to 64-bit fixed point and added into the L2-resident gradient blob straight from the registers with
-// red.global.add.u64 (the warpgroup goes on to its next MMAs while the adds drain); integer sums do not depend on the
-// order of the adds, so the gradients are reproducible bit for bit.
+// chain's weight copies through the weight ring (tc_common.cuh WeightRing); the producer gives its registers to the
+// consumers (setmaxnreg), which hold the chain accumulator and a job accumulator at once.  Every wgmma is issued in
+// warpgroup-uniform control flow (the warp index is broadcast from lane 0), so ptxas keeps the MMAs of a k-loop
+// asynchronous.  The consumers' phases, per tile: tile_scale; per event e (layer t = n_gemm - 1 - e): g_epilogue (chain +
+// head term, ReLU mask, hi / lo split -> G tile), chain_mma, then one job loop whose wgrad_job waits for the job's
+// activation tile (bulk-copied from the stash one job ahead), runs its MMAs, hands the tile back (thread 0 requests the
+// next job's once both warpgroups have) and drains the accumulator into the L2-resident gradient blob as 64-bit fixed
+// point with red.global.add.u64 -- integer sums do not depend on the order of the adds, so the gradients are
+// reproducible bit for bit; indicator_sums and dir_accumulate; at the end flush_cta.
 #include "common.cuh"
 #include "tc_common.cuh"
-#include "wgmma.cuh"
 
 namespace nerfb200 {
+
+using namespace tc;
 
 namespace tcb {
 constexpr int kWG = 2;                            // consumer warpgroups
 constexpr int kThreadsB = 128 * (kWG + 1);       // + the producer warpgroup (one thread of it streams the weights)
 constexpr int kProdRegs = 24, kConsRegs = 240;   // setmaxnreg split: (24 + 2 x 240) x 128 = 168 x 384 registers
 constexpr int kWStage = 96 * 128;                 // one k-step of a 128-wide layer: 3 copies x 2 slabs x 128 x 16 B
-constexpr int kMaxWStages = 6;                    // smem_map_b leaves room for all 6 for A0 and A1 (73 KB for A1)
+                                                  // (all kMaxStages fit for A0 and A1: 73 KB for A1)
 constexpr int kGBytes = 65536;                    // G tile: hi block 32 KB, lo block 32 KB (128 features)
 constexpr int kXBytes = 65536;                    // activation tile of the running job
 constexpr int kIndBytes = 4096;                   // ray-indicator tile: 128 points x 16 "features" (hi only)
-constexpr int kMaxRays = 10;
-constexpr int kSmemLimitB = 232448 - 1024;
 
 struct SmemMapB {
   int g, x, ind, headw, bgrad, encd, sums, dacc, misc, bars, ring, total, n_stages;
@@ -58,17 +55,14 @@ __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   m.ind = off;    off += kIndBytes;
   m.headw = off;  off += (4 * 128 + 3 * 64 + 16) * 4;
   m.bgrad = off;  off += (p.enc_cum[0] + 8) * 4;   // bias gradients of every gemm layer + the heads' (8)
-  m.encd = off;   off += kMaxRays * 32 * 4;
+  m.encd = off;   off += kMaxRaysPerTile * 32 * 4;
   m.sums = off;   off += 64 * 16 * 4;             // per-ray sums of layers_dir[0]'s G (one tile)
   m.dacc = off;   off += 64 * 28 * 4;             // direction-encoding part of dW(layers_dir[0]), whole kernel
   m.misc = off;   off += 256;                     // tile maxima
   m.bars = off;   off += 256;
-  off = (off + 1023) & ~1023;
-  m.ring = off;
-  int ns = (kSmemLimitB - off) / kWStage;
-  if (ns > kMaxWStages) ns = kMaxWStages;
-  m.n_stages = ns;
-  m.total = off + (ns > 0 ? ns : 0) * kWStage;
+  m.ring = (off + 1023) & ~1023;
+  m.n_stages = ring_depth(m.ring, kWStage);
+  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * kWStage;
   return m;
 }
 
@@ -77,51 +71,20 @@ struct BwdJob {
   int src_enc;   // B tile: 1 = the xyz-encoding tile, 0 = the stashed output of gemm layer `src`
   int src;
   int n_b;       // columns = width of the B tile (multiple of 16)
-  int row0, nrows;  // accumulator rows that carry gradients
-  int gb_off;    // offset (int64 words) of this job's block in the gradient blob: 128 rows x n_b words, layout below blob_map
-  int dst_head;  // -1: rows are output features of gemm layer `dst`; else head index, rows row0.. are its outputs
-  int dst;       // gemm index
-  int dst_col0;  // first input column of the destination weight this block covers
-  int ncols;     // real columns
+  int nrows;     // accumulator rows 0.. that carry gradients
+  int gb_off;    // kind 0: offset (int64 words) of this job's block in the gradient blob: 128 rows x n_b words, layout below blob_map
+  int dst;       // kind 0: the gemm layer whose weight gradient this is; kind 1: the head, rows 0.. are its outputs
+  int dst_col0;  // kind 0: first input column of the destination weight this block covers
+  int ncols;     // kind 0: real columns
   int kind;      // 0: A = G tile, B = activation tile;  1: head job, A = activation tile (rows = its features), B = d_raw tile
 };
 constexpr int kMaxJobs = 3;
 
-// jobs of event e (layer t = n_gemm - 1 - e); returns their number.  gb offsets are cumulative over the events.
-__host__ __device__ inline int bwd_jobs(const Plan& p, int e, BwdJob* out, int* gb_total = nullptr) {
-  int gb = 0, n_out = 0;
-  for (int ev = 0; ev <= (gb_total ? p.n_gemm - 1 : e); ++ev) {
-    const int t = p.n_gemm - 1 - ev;
-    const GemmLayer& g = p.g[t];
-    int n = 0;
-    BwdJob jb[kMaxJobs];
-    auto add = [&](int src_enc, int src, int n_b, int row0, int nrows, int dst_head, int dst, int dst_col0, int ncols,
-                   int kind) {
-      BwdJob& j = jb[n++];
-      j.src_enc = src_enc; j.src = src; j.n_b = n_b; j.row0 = row0; j.nrows = nrows;
-      j.gb_off = gb; j.dst_head = dst_head; j.dst = dst; j.dst_col0 = dst_col0; j.ncols = ncols; j.kind = kind;
-      if (kind == 0) gb += ((n_b + 15) / 16) * 128 * 16;
-    };
-    if (g.k_h > 0) add(0, g.src, g.k_h, 0, g.n, -1, t, 0, g.k_h, 0);
-    if (g.k_enc > 0 && g.enc_sel == 0) add(1, 0, p.enc_tile_w, 0, g.n, -1, t, g.k_h, g.enc_real, 0);
-    if (p.use_viewdirs && t == p.n_gemm - 1) {
-      // the narrow heads: dW_head[c][k] = sum_p d_raw[p][c] X[p][k] with the activation tile on the M side
-      add(0, t, g.n, 0, p.h[1].k, 1, t, 0, 16, 1);                               // fc_rgb reads this layer's output
-      add(0, p.h[0].src, p.g[p.h[0].src].n, 0, p.h[0].k, 0, t, 0, 16, 1);        // fc_alpha reads the trunk output
-    }
-    if (ev == e && out)
-      for (int i = 0; i < n; ++i) out[i] = jb[i];
-    if (ev == e) n_out = n;
-  }
-  if (gb_total) *gb_total = gb;
-  return n_out;
-}
-
 // the job table of a network, built on the host once per launch and passed by value (no per-thread enumeration)
 struct BwdPlan {
   int n_jobs[kMaxGemm];
-  BwdJob jobs[kMaxGemm][kMaxJobs];
-  int gb_total;
+  BwdJob jobs[kMaxGemm][kMaxJobs];  // [event e (layer t = n_gemm - 1 - e)][job]
+  int gb_total;                      // words of the jobs' blocks, laid out in event and job order
 };
 // The gradient blob: ONE L2-resident buffer of 64-bit fixed-point sums (value * 2^32, two's complement) that every CTA
 // adds into.  Integer addition is associative, so the sums -- and the gradients -- are the same bits whatever order the
@@ -154,19 +117,204 @@ __device__ __forceinline__ unsigned long long to_fix(float v) { return (unsigned
 
 inline BwdPlan make_bwd_plan(const Plan& p) {
   BwdPlan bp;
-  for (int e = 0; e < p.n_gemm; ++e) bp.n_jobs[e] = bwd_jobs(p, e, bp.jobs[e]);
-  bwd_jobs(p, 0, nullptr, &bp.gb_total);
+  bp.gb_total = 0;
+  for (int e = 0; e < p.n_gemm; ++e) {
+    const int t = p.n_gemm - 1 - e;
+    const GemmLayer& g = p.g[t];
+    int& n = bp.n_jobs[e];
+    n = 0;
+    auto add = [&](int src_enc, int src, int n_b, int nrows, int dst, int dst_col0, int ncols, int kind) {
+      BwdJob& j = bp.jobs[e][n++];
+      j.src_enc = src_enc; j.src = src; j.n_b = n_b; j.nrows = nrows;
+      j.gb_off = bp.gb_total; j.dst = dst; j.dst_col0 = dst_col0; j.ncols = ncols; j.kind = kind;
+      if (kind == 0) bp.gb_total += ((n_b + 15) / 16) * 128 * 16;
+    };
+    if (g.k_h > 0) add(0, g.src, g.k_h, g.n, t, 0, g.k_h, 0);
+    if (g.k_enc > 0 && g.enc_sel == 0) add(1, 0, p.enc_tile_w, g.n, t, g.k_h, g.enc_real, 0);
+    if (p.use_viewdirs && t == p.n_gemm - 1) {
+      // the narrow heads: dW_head[c][k] = sum_p d_raw[p][c] X[p][k] with the activation tile on the M side
+      add(0, t, g.n, p.h[1].k, 1, 0, 16, 1);                               // fc_rgb reads this layer's output
+      add(0, p.h[0].src, p.g[p.h[0].src].n, p.h[0].k, 0, 0, 16, 1);        // fc_alpha reads the trunk output
+    }
+  }
   return bp;
 }
 
 }  // namespace tcb
 
-using namespace tc;
 using namespace tcb;
+using RingB = WeightRing<kWStage>;
 
 __device__ __forceinline__ void cta_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }  // both warpgroups
 
-// weight-gradient job of width N (columns of the B tile) for this warpgroup's 64 accumulator rows:
+// shared-memory regions of the consumers
+struct BwdSmem {
+  uint8_t *g, *x, *ind;  // G tile, activation tile of the running job, ray-indicator tile
+  float *headw, *bgrad, *encd, *sums, *dacc;
+  uint32_t* max;         // [2]: tile max of |d_raw| (alternating tiles)
+};
+
+// per-tile state of a consumer thread
+struct BwdTile {
+  RowState rs;   // its two accumulator rows
+  TileRays tr;   // the tile's rays
+  float sc, us;  // d_raw scale of the tile, and the factor that takes the gradients back (and undoes the stash's / 16)
+};
+
+// Tile scale: max |d_raw| of the tile's points (warpgroup 0, one point per thread) -> a power of two that puts it in
+// [4, 8).  The maxima alternate between two slots, so the one barrier both publishes this tile's and orders the reset
+// of the next tile's slot after every read of the previous one.
+__device__ __forceinline__ void tile_scale(const float* __restrict__ d_raw, int64_t p0, int64_t P, uint32_t* s_max, int it,
+                                           BwdTile& tl) {
+  const int tid = threadIdx.x, rowm = tid & 127;
+  const float4 d4 = (p0 + rowm < P && tid < 128) ? reinterpret_cast<const float4*>(d_raw)[p0 + rowm]
+                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
+  const float m = fmaxf(fmaxf(fabsf(d4.x), fabsf(d4.y)), fmaxf(fabsf(d4.z), fabsf(d4.w)));
+  uint32_t mb = __float_as_uint(m);
+  mb = __reduce_max_sync(0xffffffffu, mb);
+  if ((tid & 31) == 0) atomicMax(&s_max[it & 1], mb);
+  cta_bar();
+  if (tid == 0) s_max[(it + 1) & 1] = 0u;  // reset the other slot for the next tile
+  const uint32_t ex = (s_max[it & 1] >> 23) & 0xFFu;
+  const bool scaled = ex >= 3u && ex <= 254u;
+  tl.sc = scaled ? __uint_as_float((256u - ex) << 23) : 1.f;
+  tl.us = (scaled ? __uint_as_float((ex - 2u) << 23) : 1.f) * kActInv;  // activations are stored / 16
+}
+
+// G-tile epilogue of event e (layer t): G_t of this thread's elements = (chain + d_raw W_head) (.) relu'(layer t) -> hi /
+// lo -> the G tile (r0: warpgroup-local row of accumulator row 0).  The 64-wide layers_dir[0] also puts d_raw into feature
+// rows 64..67 (zeros up to 79) for the heads' jobs; event 0 writes the ray-indicator tile and the direction encodings.
+__device__ __forceinline__ void g_epilogue(const Plan& p, int e, const float (&chain)[64], const BwdTile& tl,
+                                           const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P_pad,
+                                           const float* __restrict__ rays, int ray_stride, const BwdSmem& s, int hw1, int wg,
+                                           int r0) {
+  const int tid = threadIdx.x, q = tid & 3;
+  const int t = p.n_gemm - 1 - e;
+  const GemmLayer& g = p.g[t];
+  const int hsel = head_of(p, t);
+  const float* hw = hsel == 1 ? s.headw + hw1 : s.headw;
+  const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
+  const int hcol = hsel >= 0 ? p.h[hsel].out_col : 0;
+  // this thread's ReLU mask words (two rows, up to four 32-column words each)
+  uint32_t mw[2][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+      mw[i][m] = 0xFFFFFFFFu;
+      if (g.relu && m < (g.n >> 5)) {
+        const uint32_t* mask_row = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) +
+                                   (size_t)tl.rs.pt[i] * (g.n >> 5);
+        mw[i][m] = tl.rs.valid[i] ? __ldg(mask_row + m) : 0u;
+      }
+    }
+  // d_raw of this thread's rows at the tile scale (re-read per event rather than kept live through the MMAs), and
+  // the head outputs' entries of it selected once (a runtime index into dr would put it in local memory)
+  float dr[2][4], hd[2][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float4 d4 = tl.rs.valid[i] ? reinterpret_cast<const float4*>(d_raw)[tl.rs.pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
+    dr[i][0] = d4.x * tl.sc; dr[i][1] = d4.y * tl.sc; dr[i][2] = d4.z * tl.sc; dr[i][3] = d4.w * tl.sc;
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      const int k = (hcol + c) & 3;
+      hd[i][c] = k == 0 ? dr[i][0] : k == 1 ? dr[i][1] : k == 2 ? dr[i][2] : dr[i][3];
+    }
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    if (j < (g.n >> 3)) {
+      const int col = 8 * j + 2 * q;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float y0 = chain[4 * j + 2 * i], y1 = chain[4 * j + 2 * i + 1];  // Y = 2048 x, the accumulator's own scale
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          if (c < hn) {
+            const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
+            y0 = fmaf(hd[i][c], w.x, y0);
+            y1 = fmaf(hd[i][c], w.y, y1);
+          }
+        }
+        const uint32_t word = mw[i][j >> 2];
+        const int bit = 8 * (j & 3) + 2 * q;
+        y0 = (word & (1u << bit)) ? y0 : 0.f;
+        y1 = (word & (2u << bit)) ? y1 : 0.f;
+        uint32_t hi, lo;
+        split_f16x2_y(y0, y1, y0 * kLoInv, y1 * kLoInv, hi, lo);
+        const int off = tile_piece(64 * wg + r0 + 8 * i, j, 128) + 4 * q;
+        *reinterpret_cast<uint32_t*>(s.g + off) = hi;
+        *reinterpret_cast<uint32_t*>(s.g + 32768 + off) = lo;
+      }
+    }
+  }
+  if (g.n == 64 && q == 0) {
+    // 64-wide layer (layers_dir[0], first event of a tile): feature rows 64..67 carry d_raw for the heads' weight
+    // gradients, the rest of the upper half is zero
+    const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 64 * wg + r0 + 8 * i;
+      uint32_t h01, l01, h23, l23;
+      split_f16x2(dr[i][0], dr[i][1], h01, l01);
+      split_f16x2(dr[i][2], dr[i][3], h23, l23);
+      *reinterpret_cast<uint4*>(s.g + tile_piece(r, 8, 128)) = make_uint4(h01, h23, 0u, 0u);
+      *reinterpret_cast<uint4*>(s.g + 32768 + tile_piece(r, 8, 128)) = make_uint4(l01, l23, 0u, 0u);
+#pragma unroll
+      for (int fb = 9; fb < 16; ++fb) {
+        *reinterpret_cast<uint4*>(s.g + tile_piece(r, fb, 128)) = z4;
+        *reinterpret_cast<uint4*>(s.g + 32768 + tile_piece(r, fb, 128)) = z4;
+      }
+    }
+  }
+  if (e == 0) {
+    // ray-indicator tile of this tile: I[p][j] = 1 iff point p belongs to the tile's j-th ray; direction encodings
+    if (q == 0) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        uint32_t w[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+          const uint32_t lo16 = (tl.rs.ray_slot[i] == 2 * k && tl.rs.valid[i]) ? 0x3C00u : 0u;
+          const uint32_t hi16 = (tl.rs.ray_slot[i] == 2 * k + 1 && tl.rs.valid[i]) ? 0x3C00u : 0u;
+          w[k] = lo16 | (hi16 << 16);
+        }
+        const int r = 64 * wg + r0 + 8 * i;
+        *reinterpret_cast<uint4*>(s.ind + tile_piece(r, 0, 16)) = make_uint4(w[0], w[1], w[2], w[3]);
+        *reinterpret_cast<uint4*>(s.ind + tile_piece(r, 1, 16)) = make_uint4(w[4], w[5], w[6], w[7]);
+      }
+    }
+    if (p.use_viewdirs && tid < tl.tr.n * 3) {
+      const int jr = tid / 3, c = tid - 3 * jr;
+      const float vv = rays[(tl.tr.first + jr) * ray_stride + 8 + c];
+      encode_coord(vv, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, s.encd + jr * 32);
+    }
+  }
+}
+
+// chain[p][k] = 2^11 sum_n G_t[p][n] W_t[n][k] of this warpgroup's rows, N = k_h = 128, K = n: A = the warpgroup's rows
+// of the G tile (K-major), B = the three weight copies from the ring (one k-step per stage)
+__device__ __forceinline__ void chain_mma(float (&chain)[64], RingB& ring, const uint8_t* sG, int n, int wg) {
+  const uint64_t a_hi = make_desc(smem_u32(sG) + (uint32_t)wg * 16384u, 128, 2048);
+  const uint64_t b_ring = make_desc(ring.base, 2048, 128);
+  wgmma_fence();
+#pragma unroll 1
+  for (int ks = 0; ks < (n >> 4); ++ks) {
+    const uint32_t st = ring.acquire();
+    const uint64_t b_hs = desc_adv(b_ring, st * (uint32_t)kWStage);
+    const uint64_t ah = desc_adv(a_hi, ks * 256u);
+    wgmma_f16<128>(chain, ah, b_hs, ks > 0 ? 1 : 0);
+    wgmma_f16<128>(chain, desc_adv(ah, 32768u), desc_adv(b_hs, 2 * 2048u), 1);
+    wgmma_f16<128>(chain, ah, desc_adv(b_hs, 4 * 2048u), 1);
+    wgmma_commit();
+    ring.release_behind(chain);
+  }
+  ring.release_last(chain);
+}
+
+// weight-gradient MMAs of width N (columns of the B tile) for this warpgroup's 64 accumulator rows:
 //   acc = 2^-11 sum_ks (A_lo^T B_hi + A_hi^T B_lo) + sum_ks A_hi^T B_hi     (A, B MN-major; K = the tile's 128 points)
 // plus, when kInd, the 16-column indicator product into acc_i (B = the exact 0 / 1 indicator tile, no lo part)
 template <int N, bool kInd>
@@ -218,28 +366,123 @@ __device__ __forceinline__ void job_drain(const float (&acc)[N / 2], float us, u
       for (int c = 0; c < 2; ++c) red_add_u64(d + (i * (N / 8) + j) * 64 + 32 * c, to_fix(acc[4 * j + 2 * i + c] * us));
 }
 
+// a head job's accumulator (rows = the head's inputs k, columns = d_raw channels) -> its outputs' weight gradients
+__device__ __forceinline__ void head_drain(const float (&acc)[8], const HeadLayer& h, int head, float us,
+                                           unsigned long long* gh, int wg, int r0) {
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int jj = 0; jj < 2; ++jj)
+#pragma unroll
+    for (int ii = 0; ii < 2; ++ii)
+#pragma unroll
+      for (int cc = 0; cc < 2; ++cc) {
+        const int k = 64 * wg + r0 + 8 * ii, c = 8 * jj + 2 * q + cc - h.out_col;
+        if (k < h.k && c >= 0 && c < h.n_out) atomicAdd(gh + head * 512 + c * 128 + k, to_fix(acc[4 * jj + 2 * ii + cc] * us));
+      }
+}
+
+// indicator sums of layer t (event e): its bias gradient (all rays) and, for layers_dir[0], the per-ray sums that
+// dir_accumulate turns into the direction-encoding part of its weight gradient
+__device__ __forceinline__ void indicator_sums(const Plan& p, int e, const float (&acc_i)[8], float us, const BwdSmem& s,
+                                               int wg, int r0) {
+  const int q = threadIdx.x & 3;
+  const GemmLayer& g = p.g[p.n_gemm - 1 - e];
+  const float su = us * kActScale;  // the indicator is an exact 1, not an activation / 16
+#pragma unroll
+  for (int ii = 0; ii < 2; ++ii) {
+    const int n = 64 * wg + r0 + 8 * ii;
+    float tot = acc_i[2 * ii] + acc_i[2 * ii + 1] + acc_i[4 + 2 * ii] + acc_i[4 + 2 * ii + 1];
+    tot += __shfl_xor_sync(0xffffffffu, tot, 1);
+    tot += __shfl_xor_sync(0xffffffffu, tot, 2);
+    if (q == 0) {
+      if (n < g.n) s.bgrad[g.cum_n + n] += tot * su;
+      if (e == 0 && p.use_viewdirs && n >= 64 && n < 68) s.bgrad[p.enc_cum[0] + n - 64] += tot * su;  // d_rgb, d_sigma sums
+    }
+    if (e == 0 && p.use_viewdirs && n < 64) {
+      s.sums[n * 16 + 2 * q] = acc_i[2 * ii] * su;
+      s.sums[n * 16 + 2 * q + 1] = acc_i[2 * ii + 1] * su;
+      s.sums[n * 16 + 8 + 2 * q] = acc_i[4 + 2 * ii] * su;
+      s.sums[n * 16 + 9 + 2 * q] = acc_i[4 + 2 * ii + 1] * su;
+    }
+  }
+}
+
+// direction-encoding part of dW(layers_dir[0]) of this tile: the per-ray sums of G x the rays' direction encodings
+__device__ __forceinline__ void dir_accumulate(const Plan& p, const BwdSmem& s, int n_rays) {
+  for (int idx = threadIdx.x; idx < 64 * p.dim_dir; idx += 128 * kWG) {
+    const int n = idx / p.dim_dir, k = idx - n * p.dim_dir;
+    float a = 0.f;
+    for (int jr = 0; jr < n_rays; ++jr) a = fmaf(s.sums[n * 16 + jr], s.encd[jr * 32 + k], a);
+    s.dacc[n * 28 + k] += a;
+  }
+}
+
+// whether this warpgroup runs a job's MMAs (warpgroup-uniform): it has accumulator rows in the job -- or, for warpgroup 1
+// of layers_dir[0]'s first job, only the d_raw rows 64..67 of the indicator product
+__device__ __forceinline__ bool takes_part(const Plan& p, const BwdJob& jq, int e, bool first, int wg) {
+  return 64 * wg < jq.nrows || (jq.kind == 0 && first && e == 0 && p.use_viewdirs);
+}
+
+// One weight-gradient job of width N (kHead: a narrow head's job; N = 0: this warpgroup takes no part) on the landed
+// activation tile: the MMAs, hand_back() once they are complete, then the drain.
+template <int N, bool kHead, class HandBack>
+__device__ __forceinline__ void wgrad_job(const Plan& p, const BwdJob& jq, int e, bool first, const BwdSmem& s,
+                                          const BwdTile& tl, unsigned long long* gb, const BlobMap& bm, int wg, int r0,
+                                          HandBack&& hand_back) {
+  const uint32_t fstr = (uint32_t)(jq.n_b >> 3) * 128u;  // bytes between 8-point blocks of the activation tile
+  const bool ind = !kHead && first;                       // the event's first job also runs the indicator product
+  float acc[N > 0 ? N / 2 : 1], acc_i[8];
+  if constexpr (N > 0) {
+    if constexpr (kHead) {
+      // A = activation tile (rows = its features, MN-major), B = d_raw (feature rows 64..79 of the G tile); the residual
+      // products first as in every job, with B's lo block 32 KB on
+      const uint64_t xa = make_desc(smem_u32(s.x) + (uint32_t)wg * 1024u, fstr, 128);
+      const uint64_t db = make_desc(smem_u32(s.g) + 1024u, 2048, 128);
+      job_mma<16, false>(acc, acc_i, xa, 32768u, 2 * fstr, db, 32768u, 4096u, 0);
+    } else {
+      const uint64_t ga = make_desc(smem_u32(s.g) + (uint32_t)wg * 1024u, 2048, 128);  // G^T: rows = features
+      const uint64_t xb = make_desc(smem_u32(s.x), fstr, 128);
+      const uint64_t id = make_desc(smem_u32(s.ind), 256, 128);
+      if (ind) job_mma<N, true>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);
+      else job_mma<N, false>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);
+    }
+  }
+  hand_back();
+  if constexpr (N == 0) {
+    return;
+  } else if constexpr (kHead) {
+    head_drain(acc, p.h[jq.dst], jq.dst, tl.us, gb + bm.xh, wg, r0);
+  } else {
+    if (64 * wg < jq.nrows) job_drain<N>(acc, tl.us, gb + jq.gb_off, wg);
+    if (ind) indicator_sums(p, e, acc_i, tl.us, s, wg, r0);
+  }
+}
+
+// the CTA's bias and direction-encoding sums -> the gradient blob
+__device__ __forceinline__ void flush_cta(const Plan& p, const BwdSmem& s, unsigned long long* gb, const BlobMap& bm) {
+  for (int i = threadIdx.x; i < p.enc_cum[0] + 8; i += kThreadsB) atomicAdd(gb + bm.xb + i, to_fix(s.bgrad[i]));
+  for (int i = threadIdx.x; i < 64 * 28; i += kThreadsB) atomicAdd(gb + bm.xd + i, to_fix(s.dacc[i]));
+}
+
 __global__ void __launch_bounds__(kThreadsB, 1)
 mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P, int S,
                   int64_t n_tiles, float* __restrict__ gblob,
                   const __grid_constant__ BwdPlan bp) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* sm = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* sm = smem_base();
   const SmemMapB mp = smem_map_b(p);
-  uint8_t* sG = sm + mp.g;
-  uint8_t* sX = sm + mp.x;
-  uint8_t* sInd = sm + mp.ind;
-  float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
-  float* s_bgrad = reinterpret_cast<float*>(sm + mp.bgrad);
-  float* s_encd = reinterpret_cast<float*>(sm + mp.encd);
-  float* s_sums = reinterpret_cast<float*>(sm + mp.sums);
-  float* s_dacc = reinterpret_cast<float*>(sm + mp.dacc);
-  uint32_t* s_max = reinterpret_cast<uint32_t*>(sm + mp.misc);      // [2]: tile max of |d_raw| (alternating tiles)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + mp.bars);
-  uint64_t* w_full = bars;                      // [kMaxWStages]
-  uint64_t* w_empty = bars + kMaxWStages;       // [kMaxWStages]
-  uint64_t* x_full = bars + 2 * kMaxWStages;    // the running job's activation tile landed
-  const uint32_t n_stages = (uint32_t)mp.n_stages;
+  BwdSmem s;
+  s.g = sm + mp.g;
+  s.x = sm + mp.x;
+  s.ind = sm + mp.ind;
+  s.headw = reinterpret_cast<float*>(sm + mp.headw);
+  s.bgrad = reinterpret_cast<float*>(sm + mp.bgrad);
+  s.encd = reinterpret_cast<float*>(sm + mp.encd);
+  s.sums = reinterpret_cast<float*>(sm + mp.sums);
+  s.dacc = reinterpret_cast<float*>(sm + mp.dacc);
+  s.max = reinterpret_cast<uint32_t*>(sm + mp.misc);
+  RingB ring{smem_u32(sm + mp.ring), smem_u32(sm + mp.bars), (uint32_t)mp.n_stages};
+  const uint32_t x_full = ring.bars + 16 * kMaxStages;  // the running job's activation tile landed (after the ring's)
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
@@ -251,21 +494,18 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   unsigned long long* gb = reinterpret_cast<unsigned long long*>(gblob);
 
   if (tid == 0) {
-    for (int i = 0; i < kMaxWStages; ++i) {
-      mbar_init(&w_full[i], 1);
-      mbar_init(&w_empty[i], 4 * kWG);
-    }
+    ring.init(4 * kWG);
     mbar_init(x_full, 1);
     fence_barrier_init();
-    s_max[0] = s_max[1] = 0u;
+    s.max[0] = s.max[1] = 0u;
   }
   // head weights at the chain accumulator's 2^11 scale (the epilogue works on Y = 2048 y, tc_common.cuh split_f16x2_y)
-  for (int i = tid; i < hw1; i += kThreadsB) s_headw[i] = blob[p.h[0].w_off + i] * kLoScale;
-  for (int i = tid; i < hw2; i += kThreadsB) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kLoScale;
-  for (int i = tid; i < p.enc_cum[0] + 8; i += kThreadsB) s_bgrad[i] = 0.f;
-  for (int i = tid; i < kMaxRays * 32; i += kThreadsB) s_encd[i] = 0.f;
-  for (int i = tid; i < 64 * 28; i += kThreadsB) s_dacc[i] = 0.f;
-  for (int i = tid; i < kGBytes / 16; i += kThreadsB) reinterpret_cast<uint4*>(sG)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = tid; i < hw1; i += kThreadsB) s.headw[i] = blob[p.h[0].w_off + i] * kLoScale;
+  for (int i = tid; i < hw2; i += kThreadsB) s.headw[hw1 + i] = blob[p.h[1].w_off + i] * kLoScale;
+  for (int i = tid; i < p.enc_cum[0] + 8; i += kThreadsB) s.bgrad[i] = 0.f;
+  for (int i = tid; i < kMaxRaysPerTile * 32; i += kThreadsB) s.encd[i] = 0.f;
+  for (int i = tid; i < 64 * 28; i += kThreadsB) s.dacc[i] = 0.f;
+  for (int i = tid; i < kGBytes / 16; i += kThreadsB) reinterpret_cast<uint4*>(s.g)[i] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async();
   __syncthreads();
 
@@ -275,28 +515,21 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     // ===================== weight producer: the chain of event e streams layer t's transposed copies ============
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProdRegs));
     if (warp == 4 * kWG && lane == 0) {
-      Pipe pp;
       const uint64_t pol = l2_policy_evict_last();
       for (int it = 0; it < my_tiles; ++it)
         for (int e = 0; e + 1 < E; ++e) {
           const GemmLayer& g = p.g[E - 1 - e];
           const uint8_t* src = reinterpret_cast<const uint8_t*>(blob + g.tcd_off);
           const uint32_t kbytes = 96u * (uint32_t)g.k_h;
-          for (int ks = 0; ks < (g.n >> 4); ++ks) {
-            mbar_wait(&w_empty[pp.stage], pp.phase ^ 1);
-            mbar_arrive_expect_tx(&w_full[pp.stage], kbytes);
-            bulk_g2s_hint(sm + mp.ring + pp.stage * kWStage, src + (size_t)ks * kbytes, kbytes, &w_full[pp.stage], pol);
-            pp.advance(n_stages);
-          }
+          for (int ks = 0; ks < (g.n >> 4); ++ks) ring.fill(src + (size_t)ks * kbytes, 1, kbytes, 0, pol);
         }
     }
   } else {
     // ===================== consumer warpgroups =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsRegs));
-    const int wg = warp >> 2, wt = tid & 127, q = lane & 3;
+    const int wg = warp >> 2, wt = tid & 127;
     const int r0 = 16 * (wt >> 5) + (lane >> 2);   // warpgroup-local row of accumulator row 0 (row 1: + 8)
     uint32_t x_ph = 0;
-    Pipe pp;
     // activation tile of job (it, e, i): hi block, lo block (issued by thread 0 one job ahead)
     auto issue_x = [&](int it, int e, int i) {
       const BwdJob& jq = bp.jobs[e][i];
@@ -305,198 +538,37 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
                            (size_t)tile * tile_bytes(jq.n_b);
       const uint32_t hb = (uint32_t)tile_half_bytes(jq.n_b);
       mbar_arrive_expect_tx(x_full, 2 * hb);
-      bulk_g2s(sX, src, hb, x_full);
-      bulk_g2s(sX + 32768, src + hb, hb, x_full);
+      bulk_g2s(smem_u32(s.x), src, hb, x_full);
+      bulk_g2s(smem_u32(s.x) + 32768u, src + hb, hb, x_full);
     };
     if (tid == 0 && my_tiles > 0) issue_x(0, 0, 0);
 
     for (int it = 0; it < my_tiles; ++it) {
       const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
       const int64_t p0 = tile * kTileRows;
-      const int64_t first_ray = p0 / S;
-      const int64_t last_pt = (p0 + kTileRows - 1 < P) ? p0 + kTileRows - 1 : P - 1;
-      const int n_rays_tile = (int)(last_pt / S - first_ray) + 1;
-      int64_t pt[2];
-      bool valid[2];
-      int ray_slot[2];
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        pt[i] = p0 + 64 * wg + r0 + 8 * i;
-        valid[i] = pt[i] < P;
-        if (!valid[i]) pt[i] = P - 1;
-        ray_slot[i] = (int)(pt[i] / S - first_ray);
-      }
-      // ---- tile scale: max |d_raw| -> [4, 8)
-      {
-        const int rowm = tid & 127;
-        const float4 d4 = (p0 + rowm < P && tid < 128) ? reinterpret_cast<const float4*>(d_raw)[p0 + rowm]
-                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
-        const float m = fmaxf(fmaxf(fabsf(d4.x), fabsf(d4.y)), fmaxf(fabsf(d4.z), fabsf(d4.w)));
-        uint32_t mb = __float_as_uint(m);
-        mb = __reduce_max_sync(0xffffffffu, mb);
-        if (lane == 0) atomicMax(&s_max[it & 1], mb);
-        cta_bar();
-        if (tid == 0) s_max[(it + 1) & 1] = 0u;  // reset the other slot for the next tile
-      }
-      const uint32_t ex = (s_max[it & 1] >> 23) & 0xFFu;
-      const bool scaled = ex >= 3u && ex <= 254u;
-      const float sc = scaled ? __uint_as_float((256u - ex) << 23) : 1.f;
-      const float us = (scaled ? __uint_as_float((ex - 2u) << 23) : 1.f) * kActInv;  // activations are stored / 16
+      BwdTile tl;
+      tl.tr = tile_rays(p0, kTileRows, P, S);
+      tl.rs = row_state(p0 + 64 * wg, r0, P, S, tl.tr.first);
+      tile_scale(d_raw, p0, P, s.max, it, tl);
 
       float chain[64];  // G_{t+1} W_{t+1}[:, :128] of this warpgroup's rows (the previous event's chain MMA)
 #pragma unroll
       for (int i = 0; i < 64; ++i) chain[i] = 0.f;
       for (int e = 0; e < E; ++e) {
-        const int t = E - 1 - e;
-        const GemmLayer& g = p.g[t];
-        int hsel = -1;
-        if (p.h[0].src == t) hsel = 0;
-        if (p.n_head > 1 && p.h[1].src == t) hsel = 1;
-        const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
-        const int hk = hsel >= 0 ? p.h[hsel].k : 0, hn = hsel >= 0 ? p.h[hsel].n_out : 0;
-        const int hcol = hsel >= 0 ? p.h[hsel].out_col : 0;
-        // this thread's ReLU mask words (two rows, up to four 32-column words each)
-        uint32_t mw[2][4];
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-#pragma unroll
-          for (int m = 0; m < 4; ++m) {
-            mw[i][m] = 0xFFFFFFFFu;
-            if (g.relu && m < (g.n >> 5)) {
-              const uint32_t* mask_row = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) +
-                                         (size_t)pt[i] * (g.n >> 5);
-              mw[i][m] = valid[i] ? __ldg(mask_row + m) : 0u;
-            }
-          }
-        // d_raw of this thread's rows at the tile scale (re-read per event rather than kept live through the MMAs), and
-        // the head outputs' entries of it selected once (a runtime index into dr would put it in local memory)
-        float dr[2][4], hd[2][4];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float4 d4 = valid[i] ? reinterpret_cast<const float4*>(d_raw)[pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
-          dr[i][0] = d4.x * sc; dr[i][1] = d4.y * sc; dr[i][2] = d4.z * sc; dr[i][3] = d4.w * sc;
-        }
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            const int k = (hcol + c) & 3;
-            hd[i][c] = k == 0 ? dr[i][0] : k == 1 ? dr[i][1] : k == 2 ? dr[i][2] : dr[i][3];
-          }
-        // ---------------- epilogue: G_t of this thread's elements -> hi / lo -> the G tile ----------------
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (j < (g.n >> 3)) {
-            const int col = 8 * j + 2 * q;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              float y0 = chain[4 * j + 2 * i], y1 = chain[4 * j + 2 * i + 1];  // Y = 2048 x, the accumulator's own scale
-#pragma unroll
-              for (int c = 0; c < 4; ++c) {
-                if (c < hn) {
-                  const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
-                  y0 = fmaf(hd[i][c], w.x, y0);
-                  y1 = fmaf(hd[i][c], w.y, y1);
-                }
-              }
-              const uint32_t word = mw[i][j >> 2];
-              const int bit = 8 * (j & 3) + 2 * q;
-              y0 = (word & (1u << bit)) ? y0 : 0.f;
-              y1 = (word & (2u << bit)) ? y1 : 0.f;
-              uint32_t hi, lo;
-              split_f16x2_y(y0, y1, y0 * kLoInv, y1 * kLoInv, hi, lo);
-              const int off = tile_piece(64 * wg + r0 + 8 * i, j, 128) + 4 * q;
-              *reinterpret_cast<uint32_t*>(sG + off) = hi;
-              *reinterpret_cast<uint32_t*>(sG + 32768 + off) = lo;
-            }
-          }
-        }
-        if (g.n == 64 && q == 0) {
-          // 64-wide layer (layers_dir[0], first event of a tile): feature rows 64..67 carry d_raw for the heads' weight
-          // gradients, the rest of the upper half is zero
-          const uint4 z4 = make_uint4(0u, 0u, 0u, 0u);
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int r = 64 * wg + r0 + 8 * i;
-            uint32_t h01, l01, h23, l23;
-            split_f16x2(dr[i][0], dr[i][1], h01, l01);
-            split_f16x2(dr[i][2], dr[i][3], h23, l23);
-            *reinterpret_cast<uint4*>(sG + tile_piece(r, 8, 128)) = make_uint4(h01, h23, 0u, 0u);
-            *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(r, 8, 128)) = make_uint4(l01, l23, 0u, 0u);
-#pragma unroll
-            for (int fb = 9; fb < 16; ++fb) {
-              *reinterpret_cast<uint4*>(sG + tile_piece(r, fb, 128)) = z4;
-              *reinterpret_cast<uint4*>(sG + 32768 + tile_piece(r, fb, 128)) = z4;
-            }
-          }
-        }
-        if (e == 0) {
-          // ray-indicator tile of this tile: I[p][j] = 1 iff point p belongs to the tile's j-th ray; direction encodings
-          if (q == 0) {
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              uint32_t w[8];
-#pragma unroll
-              for (int k = 0; k < 8; ++k) {
-                const uint32_t lo16 = (ray_slot[i] == 2 * k && valid[i]) ? 0x3C00u : 0u;
-                const uint32_t hi16 = (ray_slot[i] == 2 * k + 1 && valid[i]) ? 0x3C00u : 0u;
-                w[k] = lo16 | (hi16 << 16);
-              }
-              const int r = 64 * wg + r0 + 8 * i;
-              *reinterpret_cast<uint4*>(sInd + tile_piece(r, 0, 16)) = make_uint4(w[0], w[1], w[2], w[3]);
-              *reinterpret_cast<uint4*>(sInd + tile_piece(r, 1, 16)) = make_uint4(w[4], w[5], w[6], w[7]);
-            }
-          }
-          if (p.use_viewdirs && tid < n_rays_tile * 3) {
-            const int jr = tid / 3, c = tid - 3 * jr;
-            const float vv = rays[(first_ray + jr) * ray_stride + 8 + c];
-            encode_coord(vv, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, s_encd + jr * 32);
-          }
-        }
+        g_epilogue(p, e, chain, tl, d_raw, stash, P_pad, rays, ray_stride, s, hw1, wg, r0);
         fence_proxy_async();
         cta_bar();  // the G tile (and the indicator tile) complete
+        if (e + 1 < E) chain_mma(chain, ring, s.g, p.g[E - 1 - e].n, wg);
 
-        if (e + 1 < E) {
-          // ---- chain: chain[p][k] = 2^11 sum_n G_t[p][n] W_t[n][k], N = k_h = 128, K = n: A = this warpgroup's rows of
-          // the G tile (K-major), B = the three weight copies from the ring (one k-step per stage)
-          const uint64_t a_hi = make_desc(smem_u32(sG) + (uint32_t)wg * 16384u, 128, 2048);
-          const uint64_t b_ring = make_desc(smem_u32(sm + mp.ring), 2048, 128);
-          uint32_t prev = 0;
-          wgmma_fence();
-          for (int ks = 0; ks < (g.n >> 4); ++ks) {
-            const uint32_t st = pp.stage;
-            mbar_wait(&w_full[st], pp.phase);
-            const uint64_t b_hs = desc_adv(b_ring, st * (uint32_t)kWStage);
-            const uint64_t ah = desc_adv(a_hi, ks * 256u);
-            wgmma_f16<128>(chain, ah, b_hs, ks > 0 ? 1 : 0);
-            wgmma_f16<128>(chain, desc_adv(ah, 32768u), desc_adv(b_hs, 2 * 2048u), 1);
-            wgmma_f16<128>(chain, ah, desc_adv(b_hs, 4 * 2048u), 1);
-            wgmma_commit();
-            if (ks > 0) {
-              wgmma_wait<1>();
-              reg_fence(chain);
-              if (lane == 0) mbar_arrive(&w_empty[prev]);
-            }
-            prev = st;
-            pp.advance(n_stages);
-          }
-          wgmma_wait<0>();
-          reg_fence(chain);
-          if (lane == 0) mbar_arrive(&w_empty[prev]);
-        }
-
-        // ---- weight-gradient jobs of this event
+        // ---- the job loop: every consumer thread waits for each job's activation tile once and hands it back once
         const int nj = bp.n_jobs[e];
         for (int i = 0; i < nj; ++i) {
           const BwdJob& jq = bp.jobs[e][i];
-          const int w = jq.n_b;
-          const uint32_t fstr = (uint32_t)(w >> 3) * 128u;  // bytes between 8-point blocks of the activation tile
           mbar_wait(x_full, x_ph);
           x_ph ^= 1;
-          // Called once per job by every consumer thread as soon as its warpgroup's MMAs are complete: once both
-          // warpgroups are through, nothing reads the activation tile any more and thread 0 requests the next job's, so
-          // that the load overlaps this job's drain instead of following it.
-          auto release_x = [&]() {
+          // Once both warpgroups are through, nothing reads the activation tile any more and thread 0 requests the
+          // next job's, so that the load overlaps this job's drain instead of following it.
+          auto hand_back_x = [&]() {
             cta_bar();
             if (tid == 0) {
               int ni = i + 1, ne = e, nit = it;
@@ -507,89 +579,28 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
               if (nit < my_tiles) issue_x(nit, ne, ni);
             }
           };
-          if (jq.kind == 1) {
-            // head job: A = activation tile (rows = its features, MN-major), B = d_raw (feature rows 64..79 of the G tile)
-            if (64 * wg < jq.nrows) {
-              float acc[8], dummy[8];
-              const uint64_t xa = make_desc(smem_u32(sX) + (uint32_t)wg * 1024u, fstr, 128);
-              const uint64_t db = make_desc(smem_u32(sG) + 1024u, 2048, 128);
-              // residual products first: A_lo B_hi + A_hi B_lo (job_mma's scheme with B's lo block 32 KB on)
-              job_mma<16, false>(acc, dummy, xa, 32768u, 2 * fstr, db, 32768u, 4096u, 0);
-              release_x();
-              const HeadLayer& h = p.h[jq.dst_head];
-#pragma unroll
-              for (int jj = 0; jj < 2; ++jj)
-#pragma unroll
-                for (int ii = 0; ii < 2; ++ii)
-#pragma unroll
-                  for (int cc = 0; cc < 2; ++cc) {
-                    const int k = 64 * wg + r0 + 8 * ii, c = 8 * jj + 2 * q + cc - h.out_col;
-                    if (k < h.k && c >= 0 && c < h.n_out)
-                      atomicAdd(gb + bm.xh + jq.dst_head * 512 + c * 128 + k, to_fix(acc[4 * jj + 2 * ii + cc] * us));
-                  }
-            } else {
-              release_x();
-            }
-          } else if (64 * wg < jq.nrows || (i == 0 && e == 0 && p.use_viewdirs)) {
-            // (warpgroup 1 of layers_dir[0]'s first job only sums the d_raw rows 64..67 of the indicator product)
-            const uint64_t ga = make_desc(smem_u32(sG) + (uint32_t)wg * 1024u, 2048, 128);  // G^T: rows = features
-            const uint64_t xb = make_desc(smem_u32(sX), fstr, 128);
-            const uint64_t id = make_desc(smem_u32(sInd), 256, 128);
-            float acc_i[8];
-            unsigned long long* gdst = gb + jq.gb_off;
-#define NB_JOB(NN)                                                                                   \
-  {                                                                                                  \
-    float acc[NN / 2];                                                                               \
-    if (i == 0) job_mma<NN, true>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);          \
-    else job_mma<NN, false>(acc, acc_i, ga, 32768u, 4096u, xb, 32768u, 2 * fstr, id);                \
-    release_x();                                                                                     \
-    if (64 * wg < jq.nrows) job_drain<NN>(acc, us, gdst, wg);                                        \
-  }
-            if (w == 128) NB_JOB(128) else if (w == 64) NB_JOB(64) else if (w == 48) NB_JOB(48)
-            else if (w == 32) NB_JOB(32) else NB_JOB(16)
-#undef NB_JOB
-            if (i == 0) {
-              // indicator sums of this layer: bias gradient (all rays) and, for layers_dir[0], the direction-encoding
-              // part of its weight gradient (per-ray sums x direction encodings, below)
-              const float su = us * kActScale;  // the indicator is an exact 1, not an activation / 16
-#pragma unroll
-              for (int ii = 0; ii < 2; ++ii) {
-                const int n = 64 * wg + r0 + 8 * ii;
-                float tot = acc_i[2 * ii] + acc_i[2 * ii + 1] + acc_i[4 + 2 * ii] + acc_i[4 + 2 * ii + 1];
-                tot += __shfl_xor_sync(0xffffffffu, tot, 1);
-                tot += __shfl_xor_sync(0xffffffffu, tot, 2);
-                if (q == 0) {
-                  if (n < g.n) s_bgrad[g.cum_n + n] += tot * su;
-                  if (e == 0 && p.use_viewdirs && n >= 64 && n < 68) s_bgrad[p.enc_cum[0] + n - 64] += tot * su;  // d_rgb, d_sigma sums
-                }
-                if (e == 0 && p.use_viewdirs && n < 64) {
-                  s_sums[n * 16 + 2 * q] = acc_i[2 * ii] * su;
-                  s_sums[n * 16 + 2 * q + 1] = acc_i[2 * ii + 1] * su;
-                  s_sums[n * 16 + 8 + 2 * q] = acc_i[4 + 2 * ii] * su;
-                  s_sums[n * 16 + 9 + 2 * q] = acc_i[4 + 2 * ii + 1] * su;
-                }
-              }
-            }
+          if (!takes_part(p, jq, e, i == 0, wg)) {
+            wgrad_job<0, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
+          } else if (jq.kind == 1) {
+            wgrad_job<16, true>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
           } else {
-            release_x();
+            const int w = jq.n_b;
+            if (w == 128) wgrad_job<128, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
+            else if (w == 64) wgrad_job<64, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
+            else if (w == 48) wgrad_job<48, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
+            else if (w == 32) wgrad_job<32, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
+            else wgrad_job<16, false>(p, jq, e, i == 0, s, tl, gb, bm, wg, r0, hand_back_x);
           }
           if (e == 0 && i == 0 && p.use_viewdirs) {
             cta_bar();  // the per-ray sums of both warpgroups are in place
-            for (int idx = tid; idx < 64 * p.dim_dir; idx += 128 * kWG) {
-              const int n = idx / p.dim_dir, k = idx - n * p.dim_dir;
-              float a = 0.f;
-              for (int jr = 0; jr < n_rays_tile; ++jr) a = fmaf(s_sums[n * 16 + jr], s_encd[jr * 32 + k], a);
-              s_dacc[n * 28 + k] += a;
-            }
+            dir_accumulate(p, s, tl.tr.n);
           }
         }
       }
     }
   }
   __syncthreads();
-  // ---- the bias / direction-encoding accumulators of this CTA go to the blob
-  for (int i = tid; i < p.enc_cum[0] + 8; i += kThreadsB) atomicAdd(gb + bm.xb + i, to_fix(s_bgrad[i]));
-  for (int i = tid; i < 64 * 28; i += kThreadsB) atomicAdd(gb + bm.xd + i, to_fix(s_dacc[i]));
+  flush_cta(p, s, gb, bm);
 }
 
 // gradient blob (fixed point) -> flat (torch-layout) gradient vector: every blob word is added to the one flat element it
@@ -611,7 +622,7 @@ __global__ void unpack_grad_kernel(const __grid_constant__ Plan p, const __grid_
           const int rr = 8 * (blk / (ncol >> 3)) + ((w >> 2) & 7);
           const int col = 8 * (blk % (ncol >> 3)) + 2 * (w & 3) + (w >> 5);
           const GemmLayer& g = p.g[j.dst];
-          if (rr >= j.row0 && rr < j.row0 + j.nrows && col < j.ncols)
+          if (rr < j.nrows && col < j.ncols)
             dst = g.flat_w + (int64_t)rr * (g.k_h + g.enc_real) + j.dst_col0 + col;
           e = p.n_gemm;  // found the block
           break;
@@ -642,11 +653,7 @@ __global__ void unpack_grad_kernel(const __grid_constant__ Plan p, const __grid_
 }
 
 // the gradient blob, in floats (two per 64-bit word)
-int64_t bwd_tc_scratch_floats(const Plan& p) {
-  int total = 0;
-  bwd_jobs(p, 0, nullptr, &total);
-  return 2 * (int64_t)blob_map(p, total).words;
-}
+int64_t bwd_tc_scratch_floats(const Plan& p) { return 2 * (int64_t)blob_map(p, make_bwd_plan(p).gb_total).words; }
 
 // what the fused backward needs beyond the training forward (tc_supported); `what` names the call and the impl
 int bwd_tc_supported(const Plan& p, const char* what) {
@@ -669,19 +676,12 @@ int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int r
                       const float* d_raw, const float* stash, float* gblob, float* flat_grad, cudaStream_t s) {
   const int64_t P = n_rays * n_samples;
   const int64_t tiles = (P + kTileRows - 1) / kTileRows;
-  const int sms = device_sms();
-  const int grid = (int)(tiles < sms ? tiles : sms);
   const BwdPlan bp = make_bwd_plan(p);
   const BlobMap bm = blob_map(p, bp.gb_total);
   int rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)bm.words * 8, s), "mlp_bwd_tc blob memset");
   if (rc) return rc;
-  const size_t bytes = (size_t)smem_map_b(p).total + 1024;
-  rc = check_cuda(cudaFuncSetAttribute(mlp_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes),
-                  "mlp_bwd_tc smem attribute");
-  if (rc) return rc;
-  mlp_bwd_tc_kernel<<<grid, kThreadsB, bytes, s>>>(p, blob, rays, ray_stride, d_raw, stash, P, n_samples, tiles, gblob, bp);
-  count_launch();
-  rc = check_cuda(cudaGetLastError(), "mlp_bwd_tc launch");
+  rc = launch_persistent(mlp_bwd_tc_kernel, tiles, kThreadsB, smem_map_b(p).total, s, "mlp_bwd_tc launch", p, blob, rays,
+                         ray_stride, d_raw, stash, P, n_samples, tiles, gblob, bp);
   if (rc) return rc;
   const int blocks = (bm.words + 255) / 256;
   unpack_grad_kernel<<<blocks, 256, 0, s>>>(p, bp, reinterpret_cast<const unsigned long long*>(gblob), flat_grad);

@@ -2,36 +2,18 @@
 // shared-memory matrix descriptor and the fp16 x 2 operand split (the MMAs themselves: wgmma.cuh).
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace nerfb200 {
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+// mbarriers and bulk copies take 32-bit shared-memory addresses (smem_u32): the hot loops keep them in registers instead
+// of converting a generic pointer on every call
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_LOOP:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra WAIT_DONE;\n"
-      "bra WAIT_LOOP;\n"
-      "WAIT_DONE:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-// the same on precomputed 32-bit shared-memory addresses (the hot loops keep barrier addresses in registers instead of
-// converting a generic pointer on every call)
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
@@ -62,11 +44,10 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
   return pol;
 }
-__device__ __forceinline__ void bulk_g2s_hint(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
   asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-          smem_u32(dst)),
-      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
+      "l"(src), "r"(bytes), "r"(bar), "l"(pol)
       : "memory");
 }
 // shared -> global bulk store (TMA engine, bulk async-group completion)
@@ -78,10 +59,9 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* ssrc, uint32_t 
 // all committed bulk stores have finished READING their shared-memory source
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src),
+               "r"(bytes), "r"(bar)
                : "memory");
 }
 
@@ -139,12 +119,6 @@ __device__ __forceinline__ void split_w3(float w0, float w1, uint32_t& hs, uint3
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hs) : "f"(h1 * kLoScale), "f"(h0 * kLoScale));
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(l) : "f"((w1 - h1) * kLoScale), "f"((w0 - h0) * kLoScale));
 }
-__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "l"(pol)
-      : "memory");
-}
 // NaN-propagating max (fmaxf would turn the NaN of an out-of-range operand into a plausible 0)
 __device__ __forceinline__ float fmax_nan(float a, float b) {
   float r;
@@ -173,12 +147,137 @@ __device__ __forceinline__ void red_add_u64(unsigned long long* gdst, unsigned l
   asm volatile("red.global.add.u64 [%0], %1;" ::"l"(gdst), "l"(v) : "memory");
 }
 
-struct Pipe {  // role-local ring state
+// ---------------------------------------------------------------------------------------------------------------
+// The persistent kernels (mlp_tc.cu forward, mlp_tc_bwd.cu fused backward): one CTA per SM walks tiles blockIdx.x,
+// blockIdx.x + gridDim.x, ...; dynamic shared memory is used from a 1 KB-aligned base, fixed regions first and the weight
+// ring in whatever is left of the budget.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kSmemAlign = 1024;
+constexpr int kSmemBudget = 232448 - kSmemAlign;  // 227 KB of dynamic shared memory per block minus the alignment slack
+constexpr int kMaxStages = 6;                     // weight-ring stages at most (the mbarriers are laid out for this many)
+constexpr int kMaxRaysPerTile = 10;               // rays one tile may touch (tc_supported: at least 15 samples per ray)
+
+// stages of `stage_bytes` that fit from `ring` (the 1 KB-aligned end of the fixed regions) to the end of the budget
+__host__ __device__ inline int ring_depth(int ring, int stage_bytes) {
+  const int ns = (kSmemBudget - ring) / stage_bytes;
+  return ns < kMaxStages ? ns : kMaxStages;
+}
+__device__ __forceinline__ uint8_t* smem_base() {
+  extern __shared__ uint8_t smem_raw[];
+  return smem_raw + ((kSmemAlign - (smem_u32(smem_raw) & (kSmemAlign - 1))) & (kSmemAlign - 1));
+}
+
+// the head that reads gemm layer e's output: 0, 1 or -1
+__host__ __device__ inline int head_of(const Plan& p, int e) {
+  int hsel = -1;
+  if (p.h[0].src == e) hsel = 0;
+  if (p.n_head > 1 && p.h[1].src == e) hsel = 1;
+  return hsel;
+}
+
+// Ray geometry.  Fewer than 2^31 points per call (check_mlp_args), so the divisions are 32-bit instead of emulated
+// 64-bit ones.  The rays of the `rows` points from p0 (the last point stands in for points past the end):
+struct TileRays {
+  int64_t first;
+  int n;
+};
+__device__ __forceinline__ TileRays tile_rays(int64_t p0, int rows, int64_t P, int S) {
+  TileRays tr;
+  tr.first = (int64_t)((uint32_t)(p0 < P ? p0 : P - 1) / (uint32_t)S);
+  const int64_t last_pt = (p0 + rows - 1 < P) ? p0 + rows - 1 : P - 1;
+  tr.n = (int)((uint32_t)last_pt / (uint32_t)S) - (int)tr.first + 1;
+  return tr;
+}
+// per-tile state of a consumer thread: its two accumulator rows p0 + r0 and p0 + r0 + 8 (r0 = 16 warp + lane / 4 in the
+// warpgroup whose first point is p0); rows past the end are invalid and alias the last point
+struct RowState {
+  int pt[2];         // a point index fits in an int: fewer than 2^31 points per call
+  bool valid[2];
+  int ray_slot[2];  // ray - first_ray
+};
+__device__ __forceinline__ RowState row_state(int64_t p0, int r0, int64_t P, int S, int64_t first_ray) {
+  RowState rs;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int64_t pt = p0 + r0 + 8 * i;
+    rs.valid[i] = pt < P;
+    rs.pt[i] = (int)(pt < P ? pt : P - 1);
+    rs.ray_slot[i] = (int)((uint32_t)rs.pt[i] / (uint32_t)S - first_ray);
+  }
+  return rs;
+}
+
+// Weight ring: n_stages stages of kStage bytes from `base`, filled by one producer thread with bulk copies from the
+// L2-resident blob and read by the consumer warpgroups' MMAs.  full[i] (bars + 8 i, one producer arrival + the bytes):
+// stage i has landed; empty[i] (bars + 8 (kMaxStages + i), one arrival per consumer warp): every consumer warp's MMAs
+// on it are complete.  Each role walks the ring with its own copy (stage, phase).
+template <int kStage>
+struct WeightRing {
+  uint32_t base, bars, n_stages;
   uint32_t stage = 0, phase = 0;
-  __device__ __forceinline__ void advance(uint32_t n_stages) {
+  uint32_t prev = 0;      // consumer: the stage whose MMAs may still be in flight ...
+  bool has_prev = false;  // ... if any (false at the start of each pass over the ring)
+  __device__ __forceinline__ uint32_t full(uint32_t s) const { return bars + 8 * s; }
+  __device__ __forceinline__ uint32_t empty(uint32_t s) const { return bars + 8 * (kMaxStages + s); }
+  __device__ __forceinline__ void init(uint32_t consumer_warps) const {
+    for (int i = 0; i < kMaxStages; ++i) {
+      mbar_init(full(i), 1);
+      mbar_init(empty(i), consumer_warps);
+    }
+  }
+  __device__ __forceinline__ void advance() {
     if (++stage == n_stages) { stage = 0; phase ^= 1; }
   }
+  // producer: once every consumer warp has handed the next stage back, fill it with n bulk copies of `bytes`, src_step
+  // apart in the blob and packed in the stage (evict_last policy `pol`)
+  __device__ __forceinline__ void fill(const uint8_t* src, uint32_t n, uint32_t bytes, size_t src_step, uint64_t pol) {
+    const uint32_t f = full(stage), dst = base + stage * kStage;
+    mbar_wait(empty(stage), phase ^ 1);
+    mbar_arrive_expect_tx(f, n * bytes);
+    for (uint32_t i = 0; i < n; ++i) bulk_g2s_hint(dst + i * bytes, src + i * src_step, bytes, f, pol);
+    advance();
+  }
+  // consumer: wait until the next stage has landed; returns its index
+  __device__ __forceinline__ uint32_t acquire() const {
+    mbar_wait(full(stage), phase);
+    return stage;
+  }
+  // consumer, after committing the MMAs on the acquired stage: hand back the stage before it, if the pass has one,
+  // once its MMAs are complete -- wait_group 1 leaves the group just committed in flight
+  template <int R>
+  __device__ __forceinline__ void release_behind(float (&acc)[R]) {
+    if (has_prev) {
+      wgmma_wait<1>();
+      reg_fence(acc);
+      if ((threadIdx.x & 31) == 0) mbar_arrive(empty(prev));
+    }
+    prev = stage;
+    has_prev = true;
+    advance();
+  }
+  // consumer, after the pass's last stage: wait for every MMA and hand back that stage
+  template <int R>
+  __device__ __forceinline__ void release_last(float (&acc)[R]) {
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if ((threadIdx.x & 31) == 0) mbar_arrive(empty(prev));
+    has_prev = false;
+  }
 };
+
+// Launch a persistent kernel: grid = min(tiles, SMs), `smem` bytes of dynamic shared memory past the aligned base.
+template <typename Kernel, typename... Args>
+int launch_persistent(Kernel kern, int64_t tiles, int threads, int smem, cudaStream_t s, const char* what,
+                      const Args&... args) {
+  const int sms = device_sms();
+  const int grid = (int)(tiles < sms ? tiles : sms);
+  const int bytes = smem + kSmemAlign;
+  int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), what);
+  if (rc) return rc;
+  kern<<<grid, threads, bytes, s>>>(args...);
+  count_launch();
+  return check_cuda(cudaGetLastError(), what);
+}
 
 }  // namespace tc
 }  // namespace nerfb200

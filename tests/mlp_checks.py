@@ -294,7 +294,7 @@ def tensor_blocks(arch):
 
 def tc_blocks(arch):
     """(label, key, rows, cols, per_cta) of every block the fused backward produces on its own path, from the rules of
-    bwd_jobs / blob_map (mlp_tc_bwd.cu):
+    make_bwd_plan / blob_map (mlp_tc_bwd.cu):
       * gemm layer with hidden inputs: the kind-0 job on the hidden columns; warpgroup w owns output rows [64 w, +64);
       * layer1 and every wide layer: the xyz-encoding job (B = the encoding tile), per row half;
       * layers_dir.0: its direction-encoding columns come from the per-ray sums x s_encd (s_dacc -> blob region xd);

@@ -2,7 +2,7 @@
 against fp64 autograd of the oracle MLP, block by block.
 
 Every hidden-128 model trains on these kernels by default (train_utils._auto_impl), so every architecture family that
-bwd_tc_supported accepts gets its own job table (bwd_jobs), gradient-blob layout (blob_map) and unpack mapping.  The
+bwd_tc_supported accepts gets its own job table (make_bwd_plan), gradient-blob layout (blob_map) and unpack mapping.  The
 sweep reaches what the golden cases do not:
   * 1 layer (the heads and fc_feat read layer1's output, which has no ReLU), 16 layers (18 gemm layers), up to four wide
     (skip) layers, a wide layer every 1, 2, 3, 4 or 5 layers;
