@@ -183,6 +183,36 @@ int32_t nerfb200_mlp_wgrad(const nerfb200_arch_t* arch, const float* rays, int32
                            int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash,
                            const float* gstash, float* flat_grad, int32_t impl, void* stream);
 
+/* ---- caller-given samples (run_network, nerf/train_utils.py:8-25; volume_render_radiance_field,
+ * nerf/volume_rendering_utils.py:6-53) ----------------------------------------------------------------
+ * The same kernels as the stage entry points above, on points and depths the caller chose instead of the stratified /
+ * hierarchical samples of a ray row.  Ray r's view direction is the 3 floats at dirs + r * dir_stride (dir_stride >= 0,
+ * in floats; 0 broadcasts one direction), so the last three columns of any ray row can be read in place.
+ *
+ * mlp_fwd_pts: nerfb200_mlp_fwd with the points given: pts[n_rays][n_samples][3]; sample s of row r takes row r's view
+ *   direction.  dirs must be NULL iff the architecture has no view directions (NERFB200_ERR_INVALID otherwise).  impl
+ *   codes, stash and refusals exactly as nerfb200_mlp_fwd (with n_samples the samples per row).
+ * mlp_bwd_pts: its backward w.r.t. the parameters (impl 0 or 1), as nerfb200_mlp_bwd: it reads the encodings from the
+ *   stash, so it takes no points; impl 1 reads the view directions again.  No gradient w.r.t. points or directions. */
+int32_t nerfb200_mlp_fwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* pts, const float* dirs,
+                             int32_t dir_stride, int64_t n_rays, int32_t n_samples, float* raw, float* stash,
+                             int32_t impl, void* stream);
+int32_t nerfb200_mlp_bwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* dirs, int32_t dir_stride,
+                             int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash, float* gstash,
+                             float* flat_grad, int32_t impl, void* stream);
+/* volume_render_fwd: nerfb200_composite_fwd with the directions through (dirs, dir_stride): raw[n_rays][n_samples][4],
+ *   z[n_rays][n_samples], 1 <= n_samples <= 1024, noise unit normals [n_rays][n_samples] or NULL.
+ *   out[n_rays][8] = [r g b disp acc depth 0 0]; weights[n_rays][n_samples] may be NULL.
+ * volume_render_bwd: its backward w.r.t. raw, taking every output: g_out[n_rays][8] = dL/d[r g b disp acc depth . .]
+ *   (the depth slot included, unlike nerfb200_composite_bwd) and g_weights[n_rays][n_samples] = dL/dweights or NULL.
+ *   Writes d_raw[n_rays][n_samples][4]. */
+int32_t nerfb200_volume_render_fwd(const float* raw, const float* z, const float* dirs, int32_t dir_stride,
+                                   const float* noise, int64_t n_rays, int32_t n_samples, float noise_std,
+                                   int32_t white_bkgd, float* out, float* weights, void* stream);
+int32_t nerfb200_volume_render_bwd(const float* raw, const float* z, const float* dirs, int32_t dir_stride,
+                                   const float* noise, const float* g_out, const float* g_weights, int64_t n_rays,
+                                   int32_t n_samples, float noise_std, int32_t white_bkgd, float* d_raw, void* stream);
+
 /* ---- whole-path entry points ------------------------------------------------------------------- */
 
 /* Workspace (device bytes) needed by nerfb200_render_fwd for n_rays rays; training adds the stashes. */

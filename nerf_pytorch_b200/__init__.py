@@ -7,8 +7,9 @@ here mirror ``from nerf import ...`` of the reference for the hot path."""
 from .models import FlexibleNeRFModel
 from .nerf_helpers import (Embedder, get_embedding_function, get_minibatches, get_ray_bundle, img2mse,
                            meshgrid_xy, mse2psnr, ndc_rays, positional_encoding, sample_pdf)
-from .train_utils import (invalidate, predict_and_render_radiance, run_one_iter_of_nerf, run_one_iter_of_nerf_from_pose,
-                          set_default_impl)
+from .train_utils import (invalidate, predict_and_render_radiance, run_network, run_one_iter_of_nerf,
+                          run_one_iter_of_nerf_from_pose, set_default_impl)
+from .volume_rendering_utils import volume_render_radiance_field
 from .eval_utils import cast_to_disparity_image, cast_to_image, render_image
 from .cache_pool import CachedRayPool, CachedValidationSet
 from .ops import SeededRandoms
@@ -17,6 +18,7 @@ from . import ops, parallel
 __all__ = [
     "FlexibleNeRFModel", "Embedder", "get_embedding_function", "get_minibatches", "get_ray_bundle", "img2mse",
     "meshgrid_xy", "mse2psnr", "ndc_rays", "positional_encoding", "sample_pdf", "predict_and_render_radiance",
+    "run_network", "volume_render_radiance_field",
     "run_one_iter_of_nerf", "run_one_iter_of_nerf_from_pose", "set_default_impl", "invalidate", "render_image", "cast_to_image", "cast_to_disparity_image", "CachedRayPool", "CachedValidationSet", "SeededRandoms", "ops",
     "parallel",
 ]

@@ -85,6 +85,10 @@ SIGNATURES = {
     "nerfb200_mlp_bwd": (I32, [AP, P, P, I32, P, I64, I32, P, P, P, P, I32, P]),
     "nerfb200_mlp_dgrad": (I32, [AP, P, P, P, P, I64, I32, P]),
     "nerfb200_mlp_wgrad": (I32, [AP, P, I32, P, I64, I32, P, P, P, P, I32, P]),
+    "nerfb200_mlp_fwd_pts": (I32, [AP, P, P, P, I32, I64, I32, P, P, I32, P]),
+    "nerfb200_mlp_bwd_pts": (I32, [AP, P, P, I32, I64, I32, P, P, P, P, I32, P]),
+    "nerfb200_volume_render_fwd": (I32, [P, P, P, I32, P, I64, I32, F32, I32, P, P, P]),
+    "nerfb200_volume_render_bwd": (I32, [P, P, P, I32, P, P, P, I64, I32, F32, I32, P, P]),
     "nerfb200_render_workspace_bytes": (I64, [AP, AP, OP, I64, I32]),
     "nerfb200_render_workspace_layout": (I32, [AP, AP, OP, I64, I32, C.POINTER(I64)]),
     "nerfb200_render_fwd": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, P, P, I32, I32, P]),

@@ -276,22 +276,27 @@ static int check_impl(const Plan& p, int impl, int n_samples, Need need, const c
   }
 }
 
-// The MLP forward of one network on the kernels check_impl accepted; a non-null stash is written for the backward.
-static int mlp_forward(const Plan& p, int impl, const float* blob, const float* rays, int ray_stride, const float* z,
-                       int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s) {
-  if (impl == 0) return launch_mlp_fwd_simt(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, s);
-  return launch_mlp_fwd_tc(p, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash, /*fast=*/impl == 3, s);
+// The points of the render path: o + d z from the ray rows, view directions in columns 8..10.
+static PointSrc ray_points(const float* rays, int ray_stride, const float* z) {
+  return PointSrc{rays, ray_stride, z, nullptr, rays + 8, ray_stride};
 }
 
-// Its backward, accumulated into flat_grad.  gstash: impl 0 the gradient stash, impl 1 the gradient blob.
-static int mlp_backward(const Plan& p, int impl, const float* blob, const float* rays, int ray_stride, const float* z,
-                        int64_t n_rays, int n_samples, const float* d_raw, const float* stash, float* gstash,
-                        float* flat_grad, cudaStream_t s) {
+// The MLP forward of one network on the kernels check_impl accepted; a non-null stash is written for the backward.
+static int mlp_forward(const Plan& p, int impl, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples,
+                       float* raw, float* stash, cudaStream_t s) {
+  if (impl == 0) return launch_mlp_fwd_simt(p, blob, src, n_rays, n_samples, raw, stash, s);
+  return launch_mlp_fwd_tc(p, blob, src, n_rays, n_samples, raw, stash, /*fast=*/impl == 3, s);
+}
+
+// Its backward, accumulated into flat_grad.  gstash: impl 0 the gradient stash, impl 1 the gradient blob.  Both read
+// the encodings from the stash; only the fused backward reads the view directions again.
+static int mlp_backward(const Plan& p, int impl, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples,
+                        const float* d_raw, const float* stash, float* gstash, float* flat_grad, cudaStream_t s) {
   if (impl == 1)
-    return launch_mlp_bwd_tc(p, blob, rays, ray_stride, n_rays, n_samples, d_raw, stash, gstash, flat_grad, s);
+    return launch_mlp_bwd_tc(p, blob, src.dirs, src.dir_stride, n_rays, n_samples, d_raw, stash, gstash, flat_grad, s);
   const int64_t P = n_rays * n_samples;
   NB_TRY(launch_dgrad_simt(p, blob, d_raw, stash, gstash, P, s));
-  return launch_wgrad_simt(p, rays, ray_stride, z, n_samples, d_raw, stash, gstash, P, flat_grad, s);
+  return launch_wgrad_simt(p, src.rays, src.ray_stride, src.z, n_samples, d_raw, stash, gstash, P, flat_grad, s);
 }
 
 static int check_opts(const nerfb200_render_opts_t* o) {
@@ -475,7 +480,7 @@ int32_t nerfb200_mlp_fwd(const nerfb200_arch_t* arch, const float* blob, const f
     return NERFB200_ERR_INVALID;
   }
   NB_TRY(check_impl(p, impl, n_samples, stash ? kStash : kInference, "mlp_fwd"));
-  return mlp_forward(p, impl, blob, rays, ray_stride, z, n_rays, n_samples, raw, stash,
+  return mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n_samples, raw, stash,
                      static_cast<cudaStream_t>(stream));
 }
 
@@ -490,8 +495,8 @@ int32_t nerfb200_mlp_bwd(const nerfb200_arch_t* arch, const float* blob, const f
     return NERFB200_ERR_INVALID;
   }
   NB_TRY(check_impl(p, impl, n_samples, kBackward, "mlp_bwd"));
-  return mlp_backward(p, impl, blob, rays, ray_stride, z, n_rays, n_samples, d_raw, stash, gstash, flat_grad,
-                      static_cast<cudaStream_t>(stream));
+  return mlp_backward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n_samples, d_raw, stash, gstash,
+                      flat_grad, static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_mlp_dgrad(const nerfb200_arch_t* arch, const float* blob, const float* d_raw, const float* stash,
@@ -527,7 +532,7 @@ int32_t nerfb200_composite_fwd(const float* raw, const float* z, const float* ra
     set_error("composite_fwd: invalid argument");
     return NERFB200_ERR_INVALID;
   }
-  return launch_composite_fwd(raw, z, rays, ray_stride, rand_tensor(noise, n_samples), n_rays, n_samples, noise_std,
+  return launch_composite_fwd(raw, z, rays + 3, ray_stride, rand_tensor(noise, n_samples), n_rays, n_samples, noise_std,
                               white_bkgd, out, weights, static_cast<cudaStream_t>(stream));
 }
 
@@ -539,8 +544,91 @@ int32_t nerfb200_composite_bwd(const float* raw, const float* z, const float* ra
     set_error("composite_bwd: invalid argument");
     return NERFB200_ERR_INVALID;
   }
-  return launch_composite_bwd(raw, z, rays, ray_stride, rand_tensor(noise, n_samples), g_out, n_rays, n_samples,
-                              noise_std, white_bkgd, d_raw, static_cast<cudaStream_t>(stream));
+  return launch_composite_bwd(raw, z, rays + 3, ray_stride, rand_tensor(noise, n_samples), g_out, nullptr,
+                              /*sample_grads=*/false, n_rays, n_samples, noise_std, white_bkgd, d_raw,
+                              static_cast<cudaStream_t>(stream));
+}
+
+static int check_pts_args(const Plan& p, const float* dirs, int dir_stride, int64_t n_rays, int n_samples,
+                          const char* what) {
+  if (n_rays <= 0 || n_samples <= 0) {
+    set_error("%s: empty input", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if ((dirs != nullptr) != (p.use_viewdirs != 0) || dir_stride < 0) {
+    set_error("%s: dirs must be given iff the architecture uses view directions (use_viewdirs %d, dirs %s, "
+              "dir_stride %d >= 0)", what, p.use_viewdirs, dirs ? "given" : "NULL", dir_stride);
+    return NERFB200_ERR_INVALID;
+  }
+  if (n_rays * (int64_t)n_samples >= (int64_t(1) << 31)) {
+    set_error("%s: more than 2^31 points in one call; chunk the points", what);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  return NERFB200_OK;
+}
+
+int32_t nerfb200_mlp_fwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* pts, const float* dirs,
+                             int32_t dir_stride, int64_t n_rays, int32_t n_samples, float* raw, float* stash,
+                             int32_t impl, void* stream) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  NB_TRY(check_pts_args(p, dirs, dir_stride, n_rays, n_samples, "mlp_fwd_pts"));
+  if (!blob || !pts || !raw) {
+    set_error("mlp_fwd_pts: null pointer");
+    return NERFB200_ERR_INVALID;
+  }
+  NB_TRY(check_impl(p, impl, n_samples, stash ? kStash : kInference, "mlp_fwd_pts"));
+  return mlp_forward(p, impl, blob, PointSrc{nullptr, 0, nullptr, pts, dirs, dir_stride}, n_rays, n_samples, raw,
+                     stash, static_cast<cudaStream_t>(stream));
+}
+
+int32_t nerfb200_mlp_bwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* dirs, int32_t dir_stride,
+                             int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash, float* gstash,
+                             float* flat_grad, int32_t impl, void* stream) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  NB_TRY(check_pts_args(p, dirs, dir_stride, n_rays, n_samples, "mlp_bwd_pts"));
+  if (!blob || !d_raw || !stash || !gstash || !flat_grad) {
+    set_error("mlp_bwd_pts: null pointer");
+    return NERFB200_ERR_INVALID;
+  }
+  NB_TRY(check_impl(p, impl, n_samples, kBackward, "mlp_bwd_pts"));
+  return mlp_backward(p, impl, blob, PointSrc{nullptr, 0, nullptr, nullptr, dirs, dir_stride}, n_rays, n_samples,
+                      d_raw, stash, gstash, flat_grad, static_cast<cudaStream_t>(stream));
+}
+
+static int check_volume_render_args(const float* raw, const float* z, const float* dirs, int dir_stride,
+                                    int64_t n_rays, int n_samples, const char* what) {
+  if (!raw || !z || !dirs || dir_stride < 0 || n_rays <= 0 || n_samples <= 0 || n_samples > 1024) {
+    set_error("%s: invalid argument (null pointer, dir_stride < 0, or n_samples outside 1..1024)", what);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
+}
+
+int32_t nerfb200_volume_render_fwd(const float* raw, const float* z, const float* dirs, int32_t dir_stride,
+                                   const float* noise, int64_t n_rays, int32_t n_samples, float noise_std,
+                                   int32_t white_bkgd, float* out, float* weights, void* stream) {
+  NB_TRY(check_volume_render_args(raw, z, dirs, dir_stride, n_rays, n_samples, "volume_render_fwd"));
+  if (!out) {
+    set_error("volume_render_fwd: null output");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_composite_fwd(raw, z, dirs, dir_stride, rand_tensor(noise, n_samples), n_rays, n_samples, noise_std,
+                              white_bkgd, out, weights, static_cast<cudaStream_t>(stream));
+}
+
+int32_t nerfb200_volume_render_bwd(const float* raw, const float* z, const float* dirs, int32_t dir_stride,
+                                   const float* noise, const float* g_out, const float* g_weights, int64_t n_rays,
+                                   int32_t n_samples, float noise_std, int32_t white_bkgd, float* d_raw, void* stream) {
+  NB_TRY(check_volume_render_args(raw, z, dirs, dir_stride, n_rays, n_samples, "volume_render_bwd"));
+  if (!g_out || !d_raw) {
+    set_error("volume_render_bwd: null pointer");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_composite_bwd(raw, z, dirs, dir_stride, rand_tensor(noise, n_samples), g_out, g_weights,
+                              /*sample_grads=*/true, n_rays, n_samples, noise_std, white_bkgd, d_raw,
+                              static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const float* u,
@@ -680,8 +768,8 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                                      nullptr, nullptr, s));
     else
       NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, z, s));
-    NB_TRY(mlp_forward(p, impl, blob, rays, ray_stride, z, n_rays, n, raw, training ? stash : nullptr, s));
-    return launch_composite_fwd(raw, z, rays, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
+    NB_TRY(mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, training ? stash : nullptr, s));
+    return launch_composite_fwd(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
                                 opts->noise_std, opts->white_bkgd, out, weights, s);
   };
   NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse, F(w.w_c)));
@@ -730,9 +818,10 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   // one network's part: compositing backward into d_raw, then the MLP backward
   auto part = [&](const Plan& p, const float* blob, int n, const float* z, const float* raw, const float* stash,
                   const RandSrc& noise, const float* g, float* flat_grad) {
-    NB_TRY(launch_composite_bwd(raw, z, rays, ray_stride, noise, g, n_rays, n, opts->noise_std, opts->white_bkgd,
-                                F(w.d_raw), s));
-    return mlp_backward(p, impl, blob, rays, ray_stride, z, n_rays, n, F(w.d_raw), stash, F(w.gstash), flat_grad, s);
+    NB_TRY(launch_composite_bwd(raw, z, rays + 3, ray_stride, noise, g, nullptr, /*sample_grads=*/false, n_rays, n,
+                                opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
+    return mlp_backward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, F(w.d_raw), stash, F(w.gstash),
+                        flat_grad, s);
   };
   if (run_fine)
     NB_TRY(part(pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), rnd[kRandNoiseF], g_fine, flat_grad_f));

@@ -112,6 +112,18 @@ inline RandSrc rand_seeded(const nerfb200_rng_t& r, int stream) {
                  r.ray_offset};
 }
 
+// Where the MLP forwards read a sample's position and its ray's view direction.  The render path forms the point
+// o + d z from the ray row and the depth (train_utils.py:67); a caller that chose its own points gives them as pts.
+// Ray r's view direction is the 3 floats at dirs + r * dir_stride: rays + 8 and ray_stride on the render path.
+struct PointSrc {
+  const float* rays;  // [n_rays][ray_stride] = [o(3) d(3) ...], read when pts is null
+  int ray_stride;
+  const float* z;     // [n_points], read when pts is null
+  const float* pts;   // [n_points][3], or null: the point is o + d z
+  const float* dirs;  // null without view directions
+  int dir_stride;
+};
+
 // host side (api.cu)
 int build_plan(const nerfb200_arch_t* arch, Plan* plan);  // 0 or NERFB200_ERR_*
 void set_error(const char* fmt, ...);
@@ -130,12 +142,15 @@ int launch_gen_rays(const float* c2w12_host, int height, int width, float focal,
 int launch_pack_rays(const float* ro, const float* rd, int64_t n, int height, int width, float focal, int ndc, float near,
                      float far, int use_viewdirs, int out_stride, float* out, cudaStream_t s);
 int launch_encode(const Plan& p, int which, const float* x, int64_t n, float* out, cudaStream_t s);
-int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
+// compositing: ray r's direction (its norm scales the sample spacing) is the 3 floats at dirs + r * dir_stride
+int launch_composite_fwd(const float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s);
-int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
-                         const float* g_out, int64_t n_rays, int n_samples, float noise_std, int white_bkgd,
-                         float* d_raw, cudaStream_t s);
+// sample_grads: also take the upstream gradient of depth (g_out[r][5]) and of the weights (g_w[n_rays][n_samples],
+// may be null); the render path's backward takes neither
+int launch_composite_bwd(const float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
+                         const float* g_out, const float* g_w, bool sample_grads, int64_t n_rays, int n_samples,
+                         float noise_std, int white_bkgd, float* d_raw, cudaStream_t s);
 // u: a tensor [n_rays][n_fine], the seeded stream, or none (the det=True linspace)
 int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, const RandSrc& u,
                             const float* cdf_in, int64_t n_rays, int n_coarse, int n_fine, float* z_fine,
@@ -149,8 +164,8 @@ int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int ste
 // fp32 CUDA cores (mlp_simt.cu), impl 0: the forward, then the backward's two halves (dgrad fills the gradient stash
 // `gstash`, wgrad reduces it into flat_grad)
 int simt_supported(const Plan& p, const char* what);
-int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                        int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s);
+int launch_mlp_fwd_simt(const Plan& p, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples, float* raw,
+                        float* stash, cudaStream_t s);
 int launch_dgrad_simt(const Plan& p, const float* blob, const float* d_raw, const float* stash, float* gstash,
                       int64_t P, cudaStream_t s);
 int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const float* z, int n_samples,
@@ -159,13 +174,13 @@ int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const fl
 // wgmma forward (mlp_tc.cu), impl 1 and 3: training writes the stash (hidden 128 only); fast is the single-pass
 // fp16 inference forward (impl 3, no stash)
 int tc_supported(const Plan& p, int n_samples, bool training, const char* what);
-int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                      int64_t n_rays, int n_samples, float* raw, float* stash, bool fast, cudaStream_t s);
+int launch_mlp_fwd_tc(const Plan& p, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples, float* raw,
+                      float* stash, bool fast, cudaStream_t s);
 // wgmma backward (mlp_tc_bwd.cu), impl 1: data-gradient chain + every weight gradient in one kernel; `scratch` holds
 // the L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into.
 // bwd_tc_supported checks what it needs beyond tc_supported(training = true).
 int bwd_tc_supported(const Plan& p, const char* what);
-int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
+int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* dirs, int dir_stride, int64_t n_rays, int n_samples,
                       const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
 int64_t bwd_tc_scratch_floats(const Plan& p);
 

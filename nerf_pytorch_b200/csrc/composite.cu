@@ -67,8 +67,8 @@ __device__ __forceinline__ float warp_excl_suffix_sum(float v, int lane) {
 }
 
 __global__ void __launch_bounds__(kCompWarps * 32)
-composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ rays,
-                     int ray_stride, const RandSrc noise, int64_t n_rays, int S, float noise_std,
+composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ dirs,
+                     int dir_stride, const RandSrc noise, int64_t n_rays, int S, float noise_std,
                      int white_bkgd, float* __restrict__ out, float* __restrict__ weights) {
   extern __shared__ float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -77,8 +77,8 @@ composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   float* s_alpha = smem + (size_t)warp * S;
   const int C = (S + 31) >> 5;
   const int j0 = lane * C, j1 = min(S, j0 + C);
-  const float* rr = rays + r * ray_stride;
-  const float dx = rr[3], dy = rr[4], dz = rr[5];
+  const float* rd = dirs + r * dir_stride;
+  const float dx = rd[0], dy = rd[1], dz = rd[2];
   const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
   const float4* raw4 = reinterpret_cast<const float4*>(raw) + r * S;
   const float* zr = z + r * S;
@@ -123,10 +123,14 @@ composite_fwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   }
 }
 
+// kSampleGrads: the upstream gradient also has a depth slot g_out[r][5] and, when g_w is not null, per-sample
+// weight terms g_w[r][S]; the render path's instance reads neither
+template <bool kSampleGrads>
 __global__ void __launch_bounds__(kCompWarps * 32)
-composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ rays,
-                     int ray_stride, const RandSrc noise, const float* __restrict__ g_out,
-                     int64_t n_rays, int S, float noise_std, int white_bkgd, float* __restrict__ d_raw) {
+composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ dirs,
+                     int dir_stride, const RandSrc noise, const float* __restrict__ g_out,
+                     const float* __restrict__ g_w, int64_t n_rays, int S, float noise_std, int white_bkgd,
+                     float* __restrict__ d_raw) {
   extern __shared__ float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t r = blockIdx.x * (int64_t)kCompWarps + warp;
@@ -136,8 +140,8 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   float* s_T = s_v + S;
   const int C = (S + 31) >> 5;
   const int j0 = lane * C, j1 = min(S, j0 + C);
-  const float* rr = rays + r * ray_stride;
-  const float dx = rr[3], dy = rr[4], dz = rr[5];
+  const float* rd = dirs + r * dir_stride;
+  const float dx = rd[0], dy = rd[1], dz = rd[2];
   const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
   const float4* raw4 = reinterpret_cast<const float4*>(raw) + r * S;
   const float* zr = z + r * S;
@@ -167,8 +171,8 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   adepth = warp_sum(adepth);
   aacc = warp_sum(aacc);
 
-  // upstream coefficients: L = sum_i w_i * v_i,  v_i = g_rgb . c_i + G_acc + G_depth * z_i
-  float G_acc = g_acc_in, G_depth = 0.f;
+  // upstream coefficients: L = sum_i w_i * v_i,  v_i = g_rgb . c_i + G_acc + G_depth * z_i (+ g_w_i)
+  float G_acc = g_acc_in, G_depth = kSampleGrads ? g_out[r * 8 + 5] : 0.f;
   if (white_bkgd) G_acc -= (g0.x + g0.y + g0.z);  // rgb_map += 1 - acc  (:50-51)
   if (g0.w != 0.f) {                              // disp = 1 / max(1e-10, depth / acc)  (:48)
     const float ratio = adepth / aacc;
@@ -183,7 +187,8 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   float local = 0.f;
   for (int j = j0; j < j1; ++j) {
     const float4 rv = raw4[j];
-    const float v = g0.x * sigmoidf_(rv.x) + g0.y * sigmoidf_(rv.y) + g0.z * sigmoidf_(rv.z) + G_acc + G_depth * zr[j];
+    float v = g0.x * sigmoidf_(rv.x) + g0.y * sigmoidf_(rv.y) + g0.z * sigmoidf_(rv.z) + G_acc + G_depth * zr[j];
+    if (kSampleGrads && g_w) v += g_w[r * S + j];
     s_v[j] = v;
     local += v * s_alpha[j] * s_T[j];
   }
@@ -207,24 +212,25 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   }
 }
 
-int launch_composite_fwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
+int launch_composite_fwd(const float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s) {
   const size_t smem = (size_t)kCompWarps * n_samples * sizeof(float);
   const int64_t blocks = (n_rays + kCompWarps - 1) / kCompWarps;
-  composite_fwd_kernel<<<(unsigned)blocks, kCompWarps * 32, smem, s>>>(raw, z, rays, ray_stride, noise, n_rays,
+  composite_fwd_kernel<<<(unsigned)blocks, kCompWarps * 32, smem, s>>>(raw, z, dirs, dir_stride, noise, n_rays,
                                                                        n_samples, noise_std, white_bkgd, out, weights);
   count_launch();
   return check_cuda(cudaGetLastError(), "composite_fwd launch");
 }
 
-int launch_composite_bwd(const float* raw, const float* z, const float* rays, int ray_stride, const RandSrc& noise,
-                         const float* g_out, int64_t n_rays, int n_samples, float noise_std, int white_bkgd,
-                         float* d_raw, cudaStream_t s) {
+int launch_composite_bwd(const float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
+                         const float* g_out, const float* g_w, bool sample_grads, int64_t n_rays, int n_samples,
+                         float noise_std, int white_bkgd, float* d_raw, cudaStream_t s) {
   const size_t smem = (size_t)kCompWarps * 3 * n_samples * sizeof(float);
   const int64_t blocks = (n_rays + kCompWarps - 1) / kCompWarps;
-  composite_bwd_kernel<<<(unsigned)blocks, kCompWarps * 32, smem, s>>>(raw, z, rays, ray_stride, noise, g_out, n_rays,
-                                                                       n_samples, noise_std, white_bkgd, d_raw);
+  auto kern = sample_grads ? composite_bwd_kernel<true> : composite_bwd_kernel<false>;
+  kern<<<(unsigned)blocks, kCompWarps * 32, smem, s>>>(raw, z, dirs, dir_stride, noise, g_out, g_w, n_rays, n_samples,
+                                                       noise_std, white_bkgd, d_raw);
   count_launch();
   return check_cuda(cudaGetLastError(), "composite_bwd launch");
 }

@@ -101,8 +101,7 @@ __device__ __forceinline__ void gemm_tile(const float* __restrict__ Wt, int w_ld
 }
 
 // encodings of the tile's points into shared memory (rows beyond the last point replicate it)
-__device__ __forceinline__ void encode_tile(const Plan& p, const float* __restrict__ rays, int ray_stride,
-                                            const float* __restrict__ z, int64_t p0, int64_t P, int S, int rows,
+__device__ __forceinline__ void encode_tile(const Plan& p, const PointSrc& src, int64_t p0, int64_t P, int S, int rows,
                                             float* encx, int encx_ld, float* encd, int encd_ld, int tid,
                                             int nthreads) {
   for (int it = tid; it < rows * 6; it += nthreads) {
@@ -110,9 +109,14 @@ __device__ __forceinline__ void encode_tile(const Plan& p, const float* __restri
     const int c = rem % 3, half = rem / 3;
     int64_t pt = p0 + row;
     if (pt >= P) pt = P - 1;
-    const int64_t ray = pt / S;
-    const float o = rays[ray * ray_stride + c], d = rays[ray * ray_stride + 3 + c];
-    const float x = __fadd_rn(o, __fmul_rn(d, z[pt]));  // pts = ro + rd * z  (train_utils.py:67)
+    float x;
+    if (src.pts) {
+      x = src.pts[pt * 3 + c];
+    } else {
+      const int64_t ray = pt / S;
+      const float o = src.rays[ray * src.ray_stride + c], d = src.rays[ray * src.ray_stride + 3 + c];
+      x = __fadd_rn(o, __fmul_rn(d, src.z[pt]));  // pts = ro + rd * z  (train_utils.py:67)
+    }
     const int nf = p.n_freq_xyz, mid = nf >> 1;
     encode_coord(x, c, p.inc_xyz, half ? mid : 0, half ? nf : mid, p.freq_xyz, encx + row * encx_ld);
   }
@@ -127,7 +131,7 @@ __device__ __forceinline__ void encode_tile(const Plan& p, const float* __restri
       int64_t pt = p0 + row;
       if (pt >= P) pt = P - 1;
       const int64_t ray = pt / S;
-      const float v = rays[ray * ray_stride + 8 + c];  // viewdirs = ray_batch[..., -3:]  (train_utils.py:13)
+      const float v = src.dirs[ray * src.dir_stride + c];  // viewdirs = ray_batch[..., -3:]  (train_utils.py:13)
       encode_coord(v, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + row * encd_ld);
     }
     const int padd = p.dim_dir_pad - p.dim_dir;
@@ -189,8 +193,7 @@ __device__ __forceinline__ void head_eval(const HeadLayer& h, const float* act, 
 template <int NJH>  // hidden = 64 * NJH
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_fwd_simt_kernel(const __grid_constant__ Plan p, const FwdSmem sm, const float* __restrict__ blob,
-                    const float* __restrict__ rays, int ray_stride, const float* __restrict__ z, int64_t P, int S,
-                    float* __restrict__ raw, float* __restrict__ stash) {
+                    const PointSrc src, int64_t P, int S, float* __restrict__ raw, float* __restrict__ stash) {
   extern __shared__ __align__(16) float smem[];
   float* act = smem + sm.act_off;
   float* encx = smem + sm.encx_off;
@@ -209,7 +212,7 @@ mlp_fwd_simt_kernel(const __grid_constant__ Plan p, const FwdSmem sm, const floa
   if (tid < 4) hb[tid] = blob[p.h[0].b_off + tid];
   if (tid >= 4 && tid < 8 && p.n_head > 1) hb[tid] = blob[p.h[1].b_off + tid - 4];
 
-  encode_tile(p, rays, ray_stride, z, p0, P, S, kTileRows, encx, sm.encx_ld, encd, sm.encd_ld, tid, kThreads);
+  encode_tile(p, src, p0, P, S, kTileRows, encx, sm.encx_ld, encd, sm.encd_ld, tid, kThreads);
   if (stash) {  // the backward reads the encodings back instead of recomputing 60 sin/cos per point
     __syncthreads();
     float* sx = stash + (size_t)P * p.enc_cum[0];
@@ -301,8 +304,8 @@ int simt_supported(const Plan& p, const char* what) {
   return NERFB200_OK;
 }
 
-int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                        int64_t n_rays, int n_samples, float* raw, float* stash, cudaStream_t s) {
+int launch_mlp_fwd_simt(const Plan& p, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples, float* raw,
+                        float* stash, cudaStream_t s) {
   const FwdSmem sm = fwd_smem_layout(p);
   const size_t bytes = (size_t)sm.total_floats * sizeof(float);
   const int64_t P = n_rays * n_samples;
@@ -311,7 +314,7 @@ int launch_mlp_fwd_simt(const Plan& p, const float* blob, const float* rays, int
   int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes),
                       "mlp_fwd smem attribute");
   if (rc) return rc;
-  kern<<<(unsigned)tiles, kThreads, bytes, s>>>(p, sm, blob, rays, ray_stride, z, P, n_samples, raw, stash);
+  kern<<<(unsigned)tiles, kThreads, bytes, s>>>(p, sm, blob, src, P, n_samples, raw, stash);
   count_launch();
   return check_cuda(cudaGetLastError(), "mlp_fwd_simt launch");
 }

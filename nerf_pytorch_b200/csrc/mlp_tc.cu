@@ -243,12 +243,15 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
 // kTrain: the forward also writes the activation stash (operand tiles + ReLU bit masks + the encoding tile).
 // kH = hidden size (compile-time: the accumulator width and the warpgroup count fold into constants)
 // kFast: the single-pass fp16 products (inference only, see the file header)
-template <bool kTrain, int kH, bool kFast>
+// kPts: the points come from pts[P][3] and the view directions from (dirs, dir_stride) instead of o + d z and the ray
+// rows' columns 8..10 (a template parameter, so that the render path's instances compile as they did without it)
+template <bool kTrain, int kH, bool kFast, bool kPts>
 __global__ void __launch_bounds__(128 * (kH == 128 ? 2 : 1) + 32, 1)
 mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ z, int64_t P, int S, int64_t n_tiles,
                   float* __restrict__ raw,          // out [P][4]
-                  float* __restrict__ stash) {      // out (kTrain)
+                  float* __restrict__ stash,        // out (kTrain)
+                  const float* __restrict__ pts, const float* __restrict__ dirs, int dir_stride) {  // kPts
   constexpr int kWG = kH == 128 ? 2 : 1, kRows = 64 * kWG, kThreads = 128 * kWG + 32;
   uint8_t* sm = smem_base();
   const SmemMap mp = smem_map(p);
@@ -332,7 +335,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
         const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
         const int64_t ray = (int64_t)((uint32_t)pt / (uint32_t)S);
         const float* rr = rays + ray * ray_stride;
-        const float zz = z[pt];
+        const float zz = kPts ? 0.f : z[pt];
         const int nf = p.n_freq_xyz, mid = nf >> 1;
         const int f0 = half ? mid : 0, f1 = half ? nf : mid;
         const int base = p.inc_xyz ? 3 : 0;
@@ -348,7 +351,8 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
           if (!kFast) *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
         };
         for (int c = 0; c < 3; ++c) {
-          const float x = __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));  // pts = ro + rd * z (train_utils.py:67)
+          // pts = ro + rd * z (train_utils.py:67), or the caller's point
+          const float x = kPts ? pts[pt * 3 + c] : __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));
           if (p.inc_xyz && half == 0) put(c, x);
           for (int f = f0; f < f1; ++f) {
             float sn, cs;
@@ -364,7 +368,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       if (p.use_viewdirs) {
         if (wt < n_rays_wg * 3) {
           const int jr = wt / 3, c = wt - 3 * jr;
-          const float v = rays[(first_ray + jr) * ray_stride + 8 + c];
+          const float v = kPts ? dirs[(first_ray + jr) * dir_stride + c] : rays[(first_ray + jr) * ray_stride + 8 + c];
           encode_coord(v, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + jr * 32);
         }
         wg_bar();
@@ -423,20 +427,21 @@ int tc_supported(const Plan& p, int n_samples, bool training, const char* what) 
 }
 
 template <bool kTrain, int kH, bool kFast>
-static int launch_fwd(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z, int64_t P,
-                      int n_samples, float* raw, float* stash, cudaStream_t s, const char* what) {
+static int launch_fwd(const Plan& p, const float* blob, const PointSrc& src, int64_t P, int n_samples, float* raw,
+                      float* stash, cudaStream_t s, const char* what) {
   constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
   const int64_t tiles = (P + kRows - 1) / kRows;
   const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // = tiles whenever the stash is written (hidden 128)
-  return launch_persistent(mlp_fwd_tc_kernel<kTrain, kH, kFast>, tiles, kThreads, smem_map(p).total, s, what, p, blob,
-                           rays, ray_stride, z, P, n_samples, kTrain ? stash_tiles : tiles, raw, stash);
+  auto kern = src.pts ? mlp_fwd_tc_kernel<kTrain, kH, kFast, true> : mlp_fwd_tc_kernel<kTrain, kH, kFast, false>;
+  return launch_persistent(kern, tiles, kThreads, smem_map(p).total, s, what, p, blob, src.rays, src.ray_stride, src.z, P,
+                           n_samples, kTrain ? stash_tiles : tiles, raw, stash, src.pts, src.dirs, src.dir_stride);
 }
 
 // stash non-null: the training forward; fast: the single-pass forward (never with a stash)
-int launch_mlp_fwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
-                      int64_t n_rays, int n_samples, float* raw, float* stash, bool fast, cudaStream_t s) {
+int launch_mlp_fwd_tc(const Plan& p, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples, float* raw,
+                      float* stash, bool fast, cudaStream_t s) {
   auto go = [&](auto launch, const char* what) {
-    return launch(p, blob, rays, ray_stride, z, n_rays * n_samples, n_samples, raw, stash, s, what);
+    return launch(p, blob, src, n_rays * n_samples, n_samples, raw, stash, s, what);
   };
   if (stash) return go(launch_fwd<true, 128, false>, "mlp_fwd_tc launch");
   if (fast)

@@ -186,7 +186,7 @@ __device__ __forceinline__ void tile_scale(const float* __restrict__ d_raw, int6
 // rows 64..67 (zeros up to 79) for the heads' jobs; event 0 writes the ray-indicator tile and the direction encodings.
 __device__ __forceinline__ void g_epilogue(const Plan& p, int e, const float (&chain)[64], const BwdTile& tl,
                                            const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P_pad,
-                                           const float* __restrict__ rays, int ray_stride, const BwdSmem& s, int hw1, int wg,
+                                           const float* __restrict__ dirs, int dir_stride, const BwdSmem& s, int hw1, int wg,
                                            int r0) {
   const int tid = threadIdx.x, q = tid & 3;
   const int t = p.n_gemm - 1 - e;
@@ -288,7 +288,7 @@ __device__ __forceinline__ void g_epilogue(const Plan& p, int e, const float (&c
     }
     if (p.use_viewdirs && tid < tl.tr.n * 3) {
       const int jr = tid / 3, c = tid - 3 * jr;
-      const float vv = rays[(tl.tr.first + jr) * ray_stride + 8 + c];
+      const float vv = dirs[(tl.tr.first + jr) * dir_stride + c];
       encode_coord(vv, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, s.encd + jr * 32);
     }
   }
@@ -465,8 +465,8 @@ __device__ __forceinline__ void flush_cta(const Plan& p, const BwdSmem& s, unsig
 }
 
 __global__ void __launch_bounds__(kThreadsB, 1)
-mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
-                  int ray_stride, const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P, int S,
+mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ dirs,
+                  int dir_stride, const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P, int S,
                   int64_t n_tiles, float* __restrict__ gblob,
                   const __grid_constant__ BwdPlan bp) {
   uint8_t* sm = smem_base();
@@ -555,7 +555,7 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll
       for (int i = 0; i < 64; ++i) chain[i] = 0.f;
       for (int e = 0; e < E; ++e) {
-        g_epilogue(p, e, chain, tl, d_raw, stash, P_pad, rays, ray_stride, s, hw1, wg, r0);
+        g_epilogue(p, e, chain, tl, d_raw, stash, P_pad, dirs, dir_stride, s, hw1, wg, r0);
         fence_proxy_async();
         cta_bar();  // the G tile (and the indicator tile) complete
         if (e + 1 < E) chain_mma(chain, ring, s.g, p.g[E - 1 - e].n, wg);
@@ -672,7 +672,7 @@ int bwd_tc_supported(const Plan& p, const char* what) {
   return NERFB200_OK;
 }
 
-int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int ray_stride, int64_t n_rays, int n_samples,
+int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* dirs, int dir_stride, int64_t n_rays, int n_samples,
                       const float* d_raw, const float* stash, float* gblob, float* flat_grad, cudaStream_t s) {
   const int64_t P = n_rays * n_samples;
   const int64_t tiles = (P + kTileRows - 1) / kTileRows;
@@ -680,8 +680,8 @@ int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* rays, int r
   const BlobMap bm = blob_map(p, bp.gb_total);
   int rc = check_cuda(cudaMemsetAsync(gblob, 0, (size_t)bm.words * 8, s), "mlp_bwd_tc blob memset");
   if (rc) return rc;
-  rc = launch_persistent(mlp_bwd_tc_kernel, tiles, kThreadsB, smem_map_b(p).total, s, "mlp_bwd_tc launch", p, blob, rays,
-                         ray_stride, d_raw, stash, P, n_samples, tiles, gblob, bp);
+  rc = launch_persistent(mlp_bwd_tc_kernel, tiles, kThreadsB, smem_map_b(p).total, s, "mlp_bwd_tc launch", p, blob, dirs,
+                         dir_stride, d_raw, stash, P, n_samples, tiles, gblob, bp);
   if (rc) return rc;
   const int blocks = (bm.words + 255) / 256;
   unpack_grad_kernel<<<blocks, 256, 0, s>>>(p, bp, reinterpret_cast<const unsigned long long*>(gblob), flat_grad);

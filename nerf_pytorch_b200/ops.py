@@ -313,6 +313,75 @@ def mlp_wgrad(arch: ArchSpec, rays, z, d_raw, stash, gstash, impl=IMPL_SIMT, fla
     return flat_grad
 
 
+def _rows_ptr(dirs: Optional[torch.Tensor]):
+    """(pointer, row stride) of an (n, 3) fp32 CUDA tensor whose rows may be any distance apart (a column slice of
+    wider rows, or stride 0 for one shared row), or (None, 0)."""
+    if dirs is None:
+        return None, 0
+    if not dirs.is_cuda or dirs.dtype != torch.float32:
+        raise RuntimeError("nerfb200: view directions must be an fp32 CUDA tensor")
+    if dirs.dim() != 2 or dirs.shape[1] != 3 or dirs.stride(1) != 1 or not 0 <= dirs.stride(0) < 2 ** 31:
+        raise RuntimeError(f"nerfb200: view directions must be (n, 3) rows of unit column stride, got shape "
+                           f"{tuple(dirs.shape)} strides {dirs.stride()}")
+    return C.c_void_p(dirs.data_ptr()), dirs.stride(0)
+
+
+def mlp_fwd_pts(arch: ArchSpec, blob, pts, dirs, impl=IMPL_SIMT, want_stash=False):
+    """The MLP at caller-given points ``pts`` (n_rays, n_samples, 3); ``dirs`` (n_rays, 3) gives each row's view
+    direction (None without view directions) and may be a strided view.  Returns raw (n_rays, n_samples, 4)[, stash]."""
+    lib = _lib.load()
+    n, s, _ = pts.shape
+    raw = torch.empty(n, s, 4, dtype=torch.float32, device=pts.device)
+    stash = torch.empty(stash_floats(arch, n * s), dtype=torch.float32, device=pts.device) if want_stash else None
+    dptr, dstride = _rows_ptr(dirs)
+    _lib.check(lib.nerfb200_mlp_fwd_pts(C.byref(arch.c_struct()), _ptr(blob), _ptr(pts), dptr, dstride, n, s, _ptr(raw),
+                                        _ptr(stash), impl, _stream()), "mlp_fwd_pts")
+    return (raw, stash) if want_stash else raw
+
+
+def mlp_bwd_pts(arch: ArchSpec, blob, dirs, d_raw, stash, impl=IMPL_SIMT, flat_grad=None):
+    """Backward of ``mlp_fwd_pts`` w.r.t. the parameters, accumulated into ``flat_grad`` (a fresh zero vector when
+    None); ``d_raw`` (n_rays, n_samples, 4).  Returns flat_grad."""
+    lib = _lib.load()
+    n, s, _ = d_raw.shape
+    n_scratch = lib.nerfb200_bwd_scratch_floats(C.byref(arch.c_struct()), n * s, impl)
+    if n_scratch < 0:
+        _lib.check(_lib.ERR_UNSUPPORTED, "mlp_bwd_pts")
+    gstash = torch.empty(n_scratch, dtype=torch.float32, device=d_raw.device)
+    if flat_grad is None:
+        flat_grad = torch.zeros(arch.flat_param_count(), dtype=torch.float32, device=d_raw.device)
+    dptr, dstride = _rows_ptr(dirs)
+    _lib.check(lib.nerfb200_mlp_bwd_pts(C.byref(arch.c_struct()), _ptr(blob), dptr, dstride, n, s, _ptr(d_raw),
+                                        _ptr(stash), _ptr(gstash), _ptr(flat_grad), impl, _stream()), "mlp_bwd_pts")
+    return flat_grad
+
+
+def volume_render_fwd(raw, z, dirs, noise, noise_std, white_bkgd):
+    """Compositing of caller-given samples: raw (n, s, 4), z (n, s), dirs (n, 3) rows (strided allowed), noise unit
+    normals (n, s) or None.  Returns (out[n, 8] = [r g b disp acc depth 0 0], weights[n, s])."""
+    lib = _lib.load()
+    n, s = z.shape
+    out = torch.empty(n, 8, dtype=torch.float32, device=z.device)
+    w = torch.empty(n, s, dtype=torch.float32, device=z.device)
+    dptr, dstride = _rows_ptr(dirs)
+    _lib.check(lib.nerfb200_volume_render_fwd(_ptr(raw), _ptr(z), dptr, dstride, _ptr(noise), n, s, float(noise_std),
+                                              int(bool(white_bkgd)), _ptr(out), _ptr(w), _stream()), "volume_render_fwd")
+    return out, w
+
+
+def volume_render_bwd(raw, z, dirs, noise, g_out, g_weights, noise_std, white_bkgd):
+    """d_raw (n, s, 4) from the upstream gradients of every output: g_out (n, 8) incl. the depth slot, g_weights (n, s)
+    or None."""
+    lib = _lib.load()
+    n, s = z.shape
+    d_raw = torch.empty(n, s, 4, dtype=torch.float32, device=z.device)
+    dptr, dstride = _rows_ptr(dirs)
+    _lib.check(lib.nerfb200_volume_render_bwd(_ptr(raw), _ptr(z), dptr, dstride, _ptr(noise), _ptr(g_out),
+                                              _ptr(g_weights), n, s, float(noise_std), int(bool(white_bkgd)),
+                                              _ptr(d_raw), _stream()), "volume_render_bwd")
+    return d_raw
+
+
 def bwd_bytes_per_point(arch: ArchSpec) -> int:
     """HBM bytes the wgmma backward reads per point (activation tiles of its weight-gradient jobs, masks, d_raw)."""
     return int(_lib.load().nerfb200_bwd_bytes_per_point(C.byref(arch.c_struct())))

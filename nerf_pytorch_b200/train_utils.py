@@ -15,6 +15,7 @@ There is no PyTorch fallback: an unsupported model / device / dtype raises.
 """
 from __future__ import annotations
 
+import math
 import weakref
 from typing import Optional, Union
 
@@ -293,9 +294,88 @@ class _RenderChunk(torch.autograd.Function):
         return (None,) * 3 + tuple(grads)
 
 
+class _RunNetwork(torch.autograd.Function):
+    """The MLP at caller-given points (ops.mlp_fwd_pts) and its parameter backward."""
+
+    @staticmethod
+    def forward(ctx, cfg, pts, dirs, *params):
+        arch, blob, training, impl = cfg
+        if not training:
+            return ops.mlp_fwd_pts(arch, blob, pts, dirs, impl=impl)
+        raw, stash = ops.mlp_fwd_pts(arch, blob, pts, dirs, impl=impl, want_stash=True)
+        ctx.cfg, ctx.stash, ctx.dirs = cfg, stash, dirs
+        return raw
+
+    @staticmethod
+    def backward(ctx, g):
+        arch, blob, training, impl = ctx.cfg
+        flat_grad = ops.mlp_bwd_pts(arch, blob, ctx.dirs, g.contiguous(), ctx.stash, impl=impl)
+        ctx.stash = ctx.dirs = None
+        # a step may query the network any number of times: its gradients are summed by autograd and reduced once by
+        # parallel.sync_gradients / FusedAdam.step (which only clear the flag when gradient sync is off)
+        global _PENDING_SYNC
+        _PENDING_SYNC = True
+        grads = []
+        for _, w_off, b_off, fin, fout in arch.flat_layout():
+            grads.append(flat_grad[w_off: w_off + fin * fout].view(fout, fin))
+            grads.append(flat_grad[b_off: b_off + fout])
+        return (None,) * 3 + tuple(grads)
+
+
 # --------------------------------------------------------------------------------------------------
 # public API
 # --------------------------------------------------------------------------------------------------
+def run_network(network_fn, pts, ray_batch, chunksize, embed_fn, embeddirs_fn, *, impl: Optional[int] = None):
+    """nerf/train_utils.py:8-25: ``network_fn`` (a FlexibleNeRFModel) on the positional encodings of caller-chosen
+    points, fused in one kernel.  ``pts`` (*B, S, 3); with ``embeddirs_fn`` every point of row b takes the view
+    direction ``ray_batch[b, -3:]`` (``ray_batch`` (*B, C), C >= 3, read in place).  Without view directions ``pts``
+    may have any leading shape.  Returns ``pts.shape[:-1] + (4,)`` fp32, differentiable w.r.t. the parameters of
+    ``network_fn`` (not w.r.t. ``pts``).  ``chunksize`` is accepted; the result does not depend on it.
+
+    ``impl``: as in ``predict_and_render_radiance``, with S samples per row."""
+    impl = _requested_impl(impl, network_fn)
+    if not pts.is_cuda or (embeddirs_fn is not None and not ray_batch.is_cuda):
+        raise NotImplementedError("nerfb200: points and rays must be on a CUDA device (there is no CPU path)")
+    if torch.is_grad_enabled() and pts.requires_grad:
+        raise NotImplementedError("nerfb200: run_network gives no gradient w.r.t. the points; detach them")
+    if pts.dim() < 1 or pts.shape[-1] != 3:
+        raise ValueError(f"nerfb200: pts must be (..., 3), got shape {tuple(pts.shape)}")
+    enc_xyz = _probe_encoder(embed_fn, None)
+    if enc_xyz is None:
+        raise RuntimeError("nerfb200: embed_fn is required (the reference crashes without it too)")
+    arch = _arch_of(network_fn, enc_xyz, _probe_encoder(embeddirs_fn, None))
+    out_shape = tuple(pts.shape[:-1]) + (4,)
+    dirs = None
+    if embeddirs_fn is not None:
+        # the reference expands ray_batch[..., None, -3:] to pts.shape
+        lead = tuple(pts.shape[:-2])
+        if pts.dim() < 2 or tuple(ray_batch.shape[:-1]) != lead or ray_batch.shape[-1] < 3:
+            raise ValueError(f"nerfb200: ray_batch {tuple(ray_batch.shape)} does not match pts {tuple(pts.shape)}: "
+                             "need pts (*B, S, 3) and ray_batch (*B, C >= 3)")
+        n_rays, n_samples = math.prod(lead), pts.shape[-2]
+        if arch.use_viewdirs:
+            d = ray_batch.detach()[..., -3:].float()
+            try:
+                dirs = d.view(n_rays, 3)
+            except RuntimeError:  # rows not evenly spaced in memory
+                dirs = d.reshape(n_rays, 3)
+            if dirs.stride(1) != 1:
+                dirs = dirs.contiguous()
+    else:
+        # no direction per row: the grouping into rows is free, so one row of all the points
+        n_rays, n_samples = 1, pts.numel() // 3
+    if n_rays * n_samples == 0:
+        raise ValueError("nerfb200: run_network on an empty point set")
+    params, blob = _packed(network_fn, arch)
+    training = _trains(params)
+    if impl is None:
+        impl = _auto_impl(arch, None, n_samples, 0, training)
+    p = pts.detach().float().contiguous().view(n_rays, n_samples, 3)
+    raw = _RunNetwork.apply((arch, blob, training, impl), p, dirs, *params)
+    return raw.view(out_shape)
+
+
+
 def predict_and_render_radiance(
     ray_batch,
     model_coarse,
