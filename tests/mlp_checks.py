@@ -1,11 +1,13 @@
 """Shared machinery of the MLP-kernel tests (not a test module): parameter tables, the fp64 oracle MLP, the forward
-stash's layout, the ReLU-tie rule, per-block gradient comparisons and one training step against the oracle.
+stash's layout, the ReLU-tie rule, per-block gradient comparisons with the wgmma backward's absolute floors, the oracle
+in chunks of whole tiles on the device for training-size batches, and one training step against the oracle.
 
 The oracle is O.flexible_nerf_forward in fp64, fed the encoding run_network builds, with the points formed in fp32 as the
 reference forms them (train_utils.py:67).  Its sin / cos arguments are the fp32 products x * f the reference evaluates
 (nerf_helpers.py:149-151), promoted to fp64: for log-sampled bands that is exactly run_network's fp64 encoding (x * 2^k
 is exact), for linear bands it removes the rounding of x * f that an fp64 run would not do."""
 import functools
+import types
 
 import torch
 
@@ -188,39 +190,45 @@ def _rows(n_points, family):
     return (n_points + 127) // 128 * 128 if family == "wgmma" else n_points
 
 
-def read_layer(stash, n_points, cum, n, family):
-    """Columns [cum, cum + n) of a stash as fp64 [n_points][n].  "wgmma": operand tiles (csrc/tc_common.cuh "Operand
-    tiles"), fp16 hi + lo 2^-11 of value / 16; "fp32": fp32 rows with 16-byte chunks XOR-swizzled by (point & 7) inside
-    each 128-byte segment (csrc/common.cuh swz_col)."""
+def read_layer(stash, n_points, cum, n, family, rows=None):
+    """Columns [cum, cum + n) of a stash as fp64 [n_points][n], or of the points rows = (p0, p1) alone (for "wgmma"
+    p0 a multiple of 128).  "wgmma": operand tiles (csrc/tc_common.cuh "Operand tiles"), fp16 hi + lo 2^-11 of
+    value / 16; "fp32": fp32 rows with 16-byte chunks XOR-swizzled by (point & 7) inside each 128-byte segment
+    (csrc/common.cuh swz_col)."""
+    p0, p1 = rows or (0, n_points)
     if family == "wgmma":
-        tiles = (n_points + 127) // 128
-        p_pad = tiles * 128
-        raw = stash.view(torch.int16)[2 * p_pad * cum: 2 * p_pad * (cum + n)]
-        t = raw.view(tiles, 2, 16, n // 8, 8, 8).view(torch.float16).double()  # [tile][hi|lo][pb][fb][p%8][f%8]
+        assert p0 % 128 == 0, p0
+        t0, t1 = p0 // 128, (p1 + 127) // 128
+        base = 2 * _rows(n_points, family) * cum
+        raw = stash.view(torch.int16)[base + 256 * n * t0: base + 256 * n * t1]  # 2 x 128 x n halves per tile
+        t = raw.view(t1 - t0, 2, 16, n // 8, 8, 8).view(torch.float16).double()  # [tile][hi|lo][pb][fb][p%8][f%8]
         val = (t[:, 0] + t[:, 1] / 2048.0) * 16.0
-        return val.permute(0, 1, 3, 2, 4).reshape(p_pad, n)[:n_points]
-    x = stash[n_points * cum: n_points * (cum + n)].view(n_points, n // 32, 8, 4)
-    pt = torch.arange(n_points, device=stash.device) & 7
+        return val.permute(0, 1, 3, 2, 4).reshape((t1 - t0) * 128, n)[:p1 - p0]
+    x = stash[n_points * cum + p0 * n: n_points * cum + p1 * n].view(p1 - p0, n // 32, 8, 4)
+    pt = torch.arange(p0, p1, device=stash.device) & 7
     q = torch.arange(8, device=stash.device)
     idx = (q[None, :] ^ pt[:, None])                                   # stored position of logical chunk q
-    return torch.gather(x, 2, idx[:, None, :, None].expand(n_points, n // 32, 8, 4)).reshape(n_points, n).double()
+    return torch.gather(x, 2, idx[:, None, :, None].expand(p1 - p0, n // 32, 8, 4)).reshape(p1 - p0, n).double()
 
 
-def write_simt_layer(stash, P, cum, n, val):
-    """Inverse of read_layer(..., "fp32"): store val [P][n] with the stash's row swizzle."""
-    x = stash[P * cum: P * (cum + n)].view(P, n // 32, 8, 4)
-    pt = torch.arange(P, device=stash.device) & 7
+def write_simt_layer(stash, P, cum, n, val, rows=None):
+    """Inverse of read_layer(..., "fp32"): store val [P][n] (or [p1 - p0][n], rows = (p0, p1)) with the stash's row
+    swizzle."""
+    p0, p1 = rows or (0, P)
+    x = stash[P * cum + p0 * n: P * cum + p1 * n].view(p1 - p0, n // 32, 8, 4)
+    pt = torch.arange(p0, p1, device=stash.device) & 7
     idx = torch.arange(8, device=stash.device)[None, :] ^ pt[:, None]
-    x.scatter_(2, idx[:, None, :, None].expand(P, n // 32, 8, 4), val.float().view(P, n // 32, 8, 4))
+    x.scatter_(2, idx[:, None, :, None].expand(p1 - p0, n // 32, 8, 4), val.float().view(p1 - p0, n // 32, 8, 4))
 
 
-def mask_words(arch, stash, n_points, li, family):
-    """The ReLU mask words of gemm layer `li` in a forward stash: an int32 view [P][n/32], bit j of word w = column
-    32 w + j."""
+def mask_words(arch, stash, n_points, li, family, rows=None):
+    """The ReLU mask words of gemm layer `li` in a forward stash: an int32 view [P][n/32] (or of the points
+    rows = (p0, p1) alone), bit j of word w = column 32 w + j."""
     lay = StashLayout(arch)
     n = lay.layers[li][1]
     start = _rows(n_points, family) * (lay.mask_base + lay.mask_cum[li])
-    return stash.view(torch.int32)[start:start + n_points * (n // 32)].view(n_points, n // 32)
+    p0, p1 = rows or (0, n_points)
+    return stash.view(torch.int32)[start:start + n_points * (n // 32)].view(n_points, n // 32)[p0:p1]
 
 
 def pack_mask(act):
@@ -231,39 +239,43 @@ def pack_mask(act):
     return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
 
 
-def relu_ties(arch, stash, P, acts, family, tol, ctx, adopt):
+def relu_ties(arch, stash, P, acts, family, tol, ctx, adopt, rows=None, scales=None):
     """ReLU ties: a unit whose pre-activation is within rounding of zero is on in the kernel and off in fp64 or the
     reverse, a discontinuity of the function, not an error of the kernel.  Counts the forward's disagreements with the
     fp64 activations `acts`, checks that each is such a tie and that their number is bounded, and with `adopt` gives the
     stash the oracle's decisions so that a backward run on it is measured on its own arithmetic.  Returns the count.
       * "fp32": the data-gradient kernel takes its decision from the stashed activation (mlp_simt.cu, finish: a > 0); a
         tie is |a32 - a64| <= tol * scale, and adopting overwrites the activation with a64;
-      * "wgmma": the backward reads the mask words; a tie is |a64| <= tol * scale, and adopting overwrites the words."""
+      * "wgmma": the backward reads the mask words; a tie is |a64| <= tol * scale, and adopting overwrites the words.
+    rows = (p0, p1): `acts` are those points' alone (for "wgmma" p0 a multiple of 128), and the count is bounded for
+    them; scales: every layer's scale (the whole run's max |activation|) instead of that of `acts`."""
     lay = StashLayout(arch)
     shifts = torch.arange(32, device=stash.device, dtype=torch.int32)
+    n_pts = rows[1] - rows[0] if rows else P
     n_ties = 0
     for li, (lname, n, cum) in enumerate(lay.layers):
         if li == 0:
             continue  # layer1 has no ReLU (models.py:238); the backward does not read its decisions
         a64 = acts[li].to(stash.device)
         if family == "wgmma":
-            words = mask_words(arch, stash, P, li, family)
+            words = mask_words(arch, stash, P, li, family, rows)
             want = pack_mask(a64 > 0)
-            flip = (((words ^ want).unsqueeze(-1) >> shifts) & 1).view(P, n).bool()
+            flip = (((words ^ want).unsqueeze(-1) >> shifts) & 1).view(n_pts, n).bool()
             off = a64
         else:
-            a32 = read_layer(stash, P, cum, n, family)
+            a32 = read_layer(stash, P, cum, n, family, rows)
             flip = (a32 > 0) != (a64 > 0)
             off = a32 - a64
         k = int(flip.sum())
         if k:
-            assert off[flip].abs().max().item() <= tol * a64.abs().max().item(), ctx + (lname,)
+            scale = scales[li] if scales else a64.abs().max().item()
+            assert off[flip].abs().max().item() <= tol * scale, ctx + (lname,)
         if adopt and family == "wgmma":
             words.copy_(want)
         elif adopt and k:
-            write_simt_layer(stash, P, cum, n, torch.where(flip, a64, a32))
+            write_simt_layer(stash, P, cum, n, torch.where(flip, a64, a32), rows)
         n_ties += k
-    assert n_ties <= 1e-5 * P * lay.cum_total + 2, ctx + (n_ties,)
+    assert n_ties <= 1e-5 * n_pts * lay.cum_total + 2, ctx + (n_ties,)
     return n_ties
 
 
@@ -351,6 +363,129 @@ def random_previous(arch, g, blocks, seed):
         b = block(prev_sd[key], rows, cols)
         b.copy_(torch.randn(b.shape, generator=gen) * block(g_sd[key], rows, cols).abs().max())
     return prev
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# the wgmma backward's absolute floors
+# ------------------------------------------------------------------------------------------------------------------------
+FIX_LSB = 2.0 ** -33  # rounding of one add into the fixed-point gradient blob (resolution 2^-32)
+# Resolution of the fp16x2 split below fp16's normal range (tc_common.cuh split_f16x2): hi and lo are subnormal there,
+# so x = hi + lo 2^-11 is resolved to 2^-36 absolutely.  The fused backward splits G (and d_raw) at the tile's scale,
+# max |d_raw| of the tile -> [4, 8), so a G element is resolved to 2^-36 / 4 = 2^-38 of the tile's max |d_raw|, however
+# small it is; the stash holds activation / 16, resolved to 2^-36 * 16 = 2^-32 absolutely.
+G_SPLIT_LSB = 2.0 ** -38
+ACT_SPLIT_LSB = 2.0 ** -32
+BLOB_MAX = 2.0 ** 28  # the gradient blob holds sums below 2^31 (mlp_tc_bwd.cu); the checks keep every gradient below this
+
+
+def _floors(arch, n_points, split_floors=None):
+    """label -> the floor of every tc_blocks block: the fixed-point rounding n_adds * 2^-33 plus, for the wgmma kernels,
+    the split's resolution floor of that block (_split_floors)."""
+    n_tiles = -(-n_points // 128)
+    n_ctas = min(n_tiles, sms())
+    return {label: (n_ctas if per_cta else n_tiles) * FIX_LSB + (split_floors or {}).get(label, 0.0)
+            for label, _, _, _, per_cta in tc_blocks(arch)}
+
+
+def blob_range_factor(grads):
+    """The power of two (1 or below) that brings every parameter gradient below BLOB_MAX."""
+    m = max(v.abs().max().item() for v in grads.values())
+    return 2.0 ** -int(torch.tensor(m / BLOB_MAX).log2().ceil().item()) if m > BLOB_MAX else 1.0
+
+
+def _in_blob_range(arch, sd, rays, z, G):
+    """fp64 oracle of sum(raw * G), with G scaled by a power of two (exact on both sides) if needed so that every
+    parameter gradient stays below BLOB_MAX.  Returns (G, acts, dpre, grads)."""
+    _, acts, dpre, want = oracle(arch, sd, rays, z, G)
+    c = blob_range_factor(want)
+    if c != 1.0:
+        G, dpre, want = G * c, [x * c for x in dpre], {k: v * c for k, v in want.items()}
+    return G, acts, dpre, want
+
+
+def _split_floors(arch, G, acts, dpre, rays, z, into=None):
+    """label -> the wgmma backward's resolution floor of that block, from the split's absolute resolution:
+        sum_p G_SPLIT_LSB * D(p) * max |X[p]|  +  ACT_SPLIT_LSB * max |G[p]|
+    over the points p, with D(p) the max |d_raw| of p's tile, X the block's input columns (activations, encodings, or 1
+    for the indicator sums) and G the block's output rows of the pre-activation gradient (d_raw for the heads).  It
+    matters where G is many decades below d_raw: the deep layers of an initialised network, whose gradient vanishes.
+    A sum over points: given `into` (a previous result), the sums of these points, whole 128-point tiles from a tile's
+    first point, are added to it, so that a run can be accumulated chunk by chunk."""
+    P = z.numel()
+    d_raw = G.reshape(-1, 4).double().abs()
+    D = torch.nn.functional.pad(d_raw.amax(1), (0, -P % 128)).view(-1, 128).amax(1).repeat_interleave(128)[:P]
+    xyz, view = encodings(arch, rays, z)
+    x_enc = xyz.abs().amax(1)
+    x_dir = None if view is None else view.abs().amax(1)
+    index = {lname: li for li, (lname, _, _) in enumerate(StashLayout(arch).layers)}
+    heads = {"fc_alpha": (arch.num_layers - 1, [3]), "fc_rgb": (len(acts) - 1, [0, 1, 2]),
+             "fc_out": (arch.num_layers - 1, [0, 1, 2, 3])}
+    out = {}
+    for label, key, rows, cols, _ in tc_blocks(arch):
+        lname, kind = key.rsplit(".", 1)
+        g = 0.0
+        if lname in heads:
+            src, outs = heads[lname]
+            x = 1.0 if kind == "bias" else acts[src][:, cols].abs().amax(1)
+            if kind == "weight":
+                g = d_raw[:, outs].amax(1)
+        elif kind == "bias":
+            x = 1.0
+        elif "dir enc" in label:
+            x = x_dir  # per-ray sums (indicator) x the fp32 direction encoding: no activation split
+        else:
+            x = x_enc if "xyz enc" in label else acts[index[lname] - 1].abs().amax(1)
+            g = dpre[index[lname]][:, rows].abs().amax(1)
+        out[label] = (G_SPLIT_LSB * (D * x).sum() + ACT_SPLIT_LSB * torch.as_tensor(g).sum()).item()
+    if into is not None:
+        out = {label: into[label] + v for label, v in out.items()}
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# the oracle at training size: chunks of whole tiles on the device
+# ------------------------------------------------------------------------------------------------------------------------
+def oracle_tiles(arch, sd, rays, z, G=None, tiles=None, chunk_tiles=128, visit=None):
+    """The oracle over the points of (rays [n][C], z [n][S]), 128-point tile by tile in chunks of chunk_tiles on the
+    device of z, or over tiles = (t0, t1) of them alone: a run at training size decodes to tens of GB in fp64 at once.
+    Returns a namespace with, for the points covered,
+      raw      fp64 [points][4];
+      masks    per gemm layer, the fp64 ReLU decisions as pack_mask words [points][n / 32];
+      act_max  per gemm layer, max |activation|;
+    and given G [n][S][4] (the upstream gradient of every point), the sums over the chunks of
+      grads    every parameter gradient of sum(raw * G) (a state_dict, fp64);
+      split    _split_floors of those points.
+    visit(p0, p1, rays_c, z_c, acts) sees each chunk: points [p0, p1), one row per point of rays and z, and their fp64
+    activations."""
+    dev = z.device
+    n_rays, S = z.shape
+    P = n_rays * S
+    t0, t1 = tiles or (0, (P + 127) // 128)
+    sd_d = {k: v.to(dev) for k, v in sd.items()}
+    lay = StashLayout(arch)
+    first = t0 * 128
+    n_pts = min(t1 * 128, P) - first
+    out = types.SimpleNamespace(raw=torch.empty(n_pts, 4, dtype=torch.float64, device=dev),
+                                masks=[torch.empty(n_pts, n // 32, dtype=torch.int32, device=dev)
+                                       for _, n, _ in lay.layers],
+                                act_max=[0.0] * len(lay.layers), grads=None, split=None)
+    for c0 in range(t0, t1, chunk_tiles):
+        p0, p1 = c0 * 128, min(min(c0 + chunk_tiles, t1) * 128, P)
+        idx = torch.arange(p0, p1, device=dev)
+        rays_c, z_c = rays[idx // S], z.reshape(-1)[p0:p1, None]
+        G_c = None if G is None else G.reshape(-1, 4)[p0:p1]
+        raw, acts, dpre, grads = oracle(arch, sd_d, rays_c, z_c, G_c)
+        out.raw[p0 - first:p1 - first] = raw.detach()
+        for li, a in enumerate(acts):
+            out.masks[li][p0 - first:p1 - first] = pack_mask(a > 0)
+            out.act_max[li] = max(out.act_max[li], a.abs().max().item())
+        if G is not None:
+            out.grads = grads if out.grads is None else {k: out.grads[k] + v for k, v in grads.items()}
+            out.split = _split_floors(arch, G_c, acts, dpre, rays_c, z_c, into=out.split)
+        if visit is not None:
+            visit(p0, p1, rays_c, z_c, acts)
+        del raw, acts, dpre, grads
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------------

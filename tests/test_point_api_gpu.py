@@ -13,16 +13,14 @@ import pytest
 import torch
 
 from helpers import Case, bits_equal, build_models
-from mlp_checks import (ALL_ARCHS, H256_ARCHS, SHAPES, TC_ARCHS, TC_FWD_TOL, StashLayout, arch_weights,
-                        check_blocks, encodings, oracle, report, sms, spec, tc_blocks, upstream)
+from mlp_checks import (ALL_ARCHS, H256_ARCHS, SHAPES, TC_ARCHS, TC_FWD_TOL, _floors, _split_floors, arch_weights,
+                        check_blocks, oracle, report, spec, tc_blocks, upstream)
 
 pytestmark = pytest.mark.gpu
 
 SIMT_FWD_TOL = 3e-5     # the fp32 kernels' raw outputs per column (test_simt_hidden256_gpu.py FWD_TOL)
 FAST_TOL = 2e-2         # the single-pass forward against fp64 (test_tc_fast_gpu.py FAST_TOL)
 BLOCK_TOL = 3e-5        # parameter gradients per block (test_tc_arch_sweep_gpu.py BLOCK_TOL)
-# the wgmma backward's fixed-point add rounding and split resolution (test_tc_arch_sweep_gpu.py)
-FIX_LSB, G_SPLIT_LSB, ACT_SPLIT_LSB = 2.0 ** -33, 2.0 ** -38, 2.0 ** -32
 COMP_TOL = 1e-4         # compositing outputs, per output, relative to its scale
 COMP_GRAD_TOL = 2e-4    # d_raw relative to its scale (test_stage_parity_gpu.py)
 
@@ -121,42 +119,6 @@ def _box_points(arch, lead, s, seed):
     if not arch.use_viewdirs:
         per_point = per_point[:, :8]
     return (pts.reshape(*lead, s, 3), ray_batch.reshape(*lead, 11), per_point.contiguous(), torch.zeros(n * s, 1))
-
-
-def _split_floors(arch, G, acts, dpre, rays, z):
-    """label -> the wgmma backward's resolution floor of each tc_blocks block (the rule of test_tc_arch_sweep_gpu.py):
-    sum over points of G_SPLIT_LSB * (the point's tile max |d_raw|) * max |X[p]| + ACT_SPLIT_LSB * max |G[p]|."""
-    P = z.numel()
-    d_raw = G.reshape(-1, 4).double().abs()
-    D = torch.nn.functional.pad(d_raw.amax(1), (0, -P % 128)).view(-1, 128).amax(1).repeat_interleave(128)[:P]
-    xyz, view = encodings(arch, rays, z)
-    index = {lname: li for li, (lname, _, _) in enumerate(StashLayout(arch).layers)}
-    heads = {"fc_alpha": (arch.num_layers - 1, [3]), "fc_rgb": (len(acts) - 1, [0, 1, 2]),
-             "fc_out": (arch.num_layers - 1, [0, 1, 2, 3])}
-    out = {}
-    for label, key, rows, cols, _ in tc_blocks(arch):
-        lname, kind = key.rsplit(".", 1)
-        g = 0.0
-        if lname in heads:
-            src, outs = heads[lname]
-            x = 1.0 if kind == "bias" else acts[src][:, cols].abs().amax(1)
-            if kind == "weight":
-                g = d_raw[:, outs].amax(1)
-        elif kind == "bias":
-            x = 1.0
-        elif "dir enc" in label:
-            x = view.abs().amax(1)
-        else:
-            x = xyz.abs().amax(1) if "xyz enc" in label else acts[index[lname] - 1].abs().amax(1)
-            g = dpre[index[lname]][:, rows].abs().amax(1)
-        out[label] = (G_SPLIT_LSB * (D * x).sum() + ACT_SPLIT_LSB * torch.as_tensor(g).sum()).item()
-    return out
-
-
-def _floors(arch, n_points, split=None):
-    n_tiles = -(-n_points // 128)
-    return {label: (min(n_tiles, sms()) if per_cta else n_tiles) * FIX_LSB + (split or {}).get(label, 0.0)
-            for label, _, _, _, per_cta in tc_blocks(arch)}
 
 
 FWD_SHAPES = [((n,), s) for n, s in SHAPES] + [((1,), 100000), ((2, 3, 4), 16)]

@@ -36,9 +36,10 @@ Bars: each is below 10x the worst figure measured on an H100 over every paramete
 import pytest
 import torch
 
-from mlp_checks import (ALL_ARCHS, FWD_ONLY_ARCHS, SHAPES, STATES, TC_ARCHS as ARCHS, TC_FWD_TOL as FWD_TOL,
-                        StashLayout, as_state_dict, check_blocks, encodings, oracle, random_previous, read_layer,
-                        relu_ties, report, setup, sms, spec, tc_blocks, training_step_vs_oracle, upstream)
+from mlp_checks import (ALL_ARCHS, FIX_LSB, FWD_ONLY_ARCHS, SHAPES, STATES, TC_ARCHS as ARCHS,
+                        TC_FWD_TOL as FWD_TOL, StashLayout, _floors, _in_blob_range, _split_floors, as_state_dict,
+                        check_blocks, encodings, oracle, random_previous, read_layer, relu_ties, report, setup, spec,
+                        tc_blocks, training_step_vs_oracle, upstream)
 
 pytestmark = pytest.mark.gpu
 
@@ -48,14 +49,6 @@ STASH_TOL = 2e-5     # stashed activation and encoding tiles, per layer; also ho
 BLOCK_TOL = 3e-5     # parameter gradients, per block: wgmma [1.3e-5], fp32 kernels [5.2e-6]
 ACCUM_TOL = 2e-6     # accumulated minus previous contents vs the gradient, per block [2.5e-7]
 FP32_TIE_TOL = 1e-5  # how far from zero an fp32 ReLU tie may sit: test_simt_hidden256_gpu.py's STASH_TOL [1.4e-6]
-FIX_LSB = 2.0 ** -33  # rounding of one add into the fixed-point gradient blob (resolution 2^-32)
-# Resolution of the fp16x2 split below fp16's normal range (tc_common.cuh split_f16x2): hi and lo are subnormal there,
-# so x = hi + lo 2^-11 is resolved to 2^-36 absolutely.  The fused backward splits G (and d_raw) at the tile's scale,
-# max |d_raw| of the tile -> [4, 8), so a G element is resolved to 2^-36 / 4 = 2^-38 of the tile's max |d_raw|, however
-# small it is; the stash holds activation / 16, resolved to 2^-36 * 16 = 2^-32 absolutely.
-G_SPLIT_LSB = 2.0 ** -38
-ACT_SPLIT_LSB = 2.0 ** -32
-BLOB_MAX = 2.0 ** 28  # the gradient blob holds sums below 2^31 (mlp_tc_bwd.cu); the checks keep every gradient below this
 
 # tiles inside one ray; one CTA with two tiles; ~four tiles per CTA ("sms": the device's multiprocessor count)
 MULTI_ARCHS = ["6x128_skip1", "16x128_skip5"]
@@ -70,61 +63,6 @@ def _ids(case):
 FWD_CASES = [(a, s) for a in ALL_ARCHS for s in SHAPES] + [(a, s) for a in MULTI_ARCHS for s in MULTI_SHAPES]
 BWD_CASES = [(a, s) for a in [*ARCHS, "4x128_noview"] for s in SHAPES] + [(a, s) for a in MULTI_ARCHS
                                                                          for s in MULTI_SHAPES]
-
-
-def _floors(arch, n_points, split_floors=None):
-    """label -> the floor of every tc_blocks block: the fixed-point rounding n_adds * 2^-33 plus, for the wgmma kernels,
-    the split's resolution floor of that block (_split_floors)."""
-    n_tiles = -(-n_points // 128)
-    n_ctas = min(n_tiles, sms())
-    return {label: (n_ctas if per_cta else n_tiles) * FIX_LSB + (split_floors or {}).get(label, 0.0)
-            for label, _, _, _, per_cta in tc_blocks(arch)}
-
-
-def _in_blob_range(arch, sd, rays, z, G):
-    """fp64 oracle of sum(raw * G), with G scaled by a power of two (exact on both sides) if needed so that every
-    parameter gradient stays below BLOB_MAX.  Returns (G, acts, dpre, grads)."""
-    _, acts, dpre, want = oracle(arch, sd, rays, z, G)
-    m = max(v.abs().max().item() for v in want.values())
-    if m > BLOB_MAX:
-        c = 2.0 ** -int(torch.tensor(m / BLOB_MAX).log2().ceil().item())
-        G, dpre, want = G * c, [x * c for x in dpre], {k: v * c for k, v in want.items()}
-    return G, acts, dpre, want
-
-
-def _split_floors(arch, G, acts, dpre, rays, z):
-    """label -> the wgmma backward's resolution floor of that block, from the split's absolute resolution:
-        sum_p G_SPLIT_LSB * D(p) * max |X[p]|  +  ACT_SPLIT_LSB * max |G[p]|
-    over the points p, with D(p) the max |d_raw| of p's tile, X the block's input columns (activations, encodings, or 1
-    for the indicator sums) and G the block's output rows of the pre-activation gradient (d_raw for the heads).  It
-    matters where G is many decades below d_raw: the deep layers of an initialised network, whose gradient vanishes."""
-    P = z.numel()
-    d_raw = G.reshape(-1, 4).double().abs()
-    D = torch.nn.functional.pad(d_raw.amax(1), (0, -P % 128)).view(-1, 128).amax(1).repeat_interleave(128)[:P]
-    xyz, view = encodings(arch, rays, z)
-    x_enc = xyz.abs().amax(1)
-    x_dir = None if view is None else view.abs().amax(1)
-    index = {lname: li for li, (lname, _, _) in enumerate(StashLayout(arch).layers)}
-    heads = {"fc_alpha": (arch.num_layers - 1, [3]), "fc_rgb": (len(acts) - 1, [0, 1, 2]),
-             "fc_out": (arch.num_layers - 1, [0, 1, 2, 3])}
-    out = {}
-    for label, key, rows, cols, _ in tc_blocks(arch):
-        lname, kind = key.rsplit(".", 1)
-        g = 0.0
-        if lname in heads:
-            src, outs = heads[lname]
-            x = 1.0 if kind == "bias" else acts[src][:, cols].abs().amax(1)
-            if kind == "weight":
-                g = d_raw[:, outs].amax(1)
-        elif kind == "bias":
-            x = 1.0
-        elif "dir enc" in label:
-            x = x_dir  # per-ray sums (indicator) x the fp32 direction encoding: no activation split
-        else:
-            x = x_enc if "xyz enc" in label else acts[index[lname] - 1].abs().amax(1)
-            g = dpre[index[lname]][:, rows].abs().amax(1)
-        out[label] = (G_SPLIT_LSB * (D * x).sum() + ACT_SPLIT_LSB * torch.as_tensor(g).sum()).item()
-    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------------
