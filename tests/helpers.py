@@ -140,6 +140,42 @@ def build_models(c: Case):
     return mc, mf, epf, edf
 
 
+def composite64(raw, z, dirs, noise_std=0.0, white_background=False, noise=None, raw64=None):
+    """fp64 O.volume_render_radiance_field of the fp32 samples raw [.., S, 4], z [.., S], dirs [.., 3] with unit normals
+    noise [.., S]: (rgb, disp, acc, weights, depth), differentiable with respect to raw64 (default raw.double()).
+
+    The ReLU gate of sigma and the last sample's sigma are taken from the fp32 pre-activation
+    fp32(raw + fp32(noise * std)) that the kernels and the reference round: the gate is the function's one
+    discontinuity, and the last sample's alpha, 1 - exp(-sigma * 1e10 |d|), turns a rounding of a tiny sigma into an
+    O(1) change.  Every other sigma is raw + noise * std in fp64.  disp is NaN where acc is 0, as in the reference, with
+    a gradient that stays finite on the other rays.  Plain tensor ops: it runs on the device of its inputs."""
+    if raw64 is None:
+        raw64 = raw.double()
+    pre32, pre64 = raw[..., 3], raw64[..., 3]
+    if noise_std > 0.0:
+        std32 = torch.tensor(noise_std, dtype=torch.float32, device=raw.device)
+        nz32 = noise.float() * std32
+        pre32 = pre32 + nz32
+        pre64 = pre64 + noise.double() * float(std32)
+    gate = pre32 > 0
+    last = pre32[..., -1:].double() + (pre64[..., -1:] - pre64[..., -1:].detach())
+    sigma = torch.where(gate, torch.cat((pre64[..., :-1], last), -1), 0.0)
+    z64 = z.double()
+    dists = torch.cat((z64[..., 1:] - z64[..., :-1], torch.full_like(z64[..., :1], 1e10)), -1)
+    dists = dists * dirs.double().norm(p=2, dim=-1)[..., None]
+    alpha = 1.0 - torch.exp(-sigma * dists)
+    weights = alpha * O.cumprod_exclusive(1.0 - alpha + 1e-10)
+    rgb = (weights[..., None] * torch.sigmoid(raw64[..., :3])).sum(-2)
+    depth = (weights * z64).sum(-1)
+    acc = weights.sum(-1)
+    some = acc > 0
+    disp = 1.0 / torch.clamp_min(depth / torch.where(some, acc, 1.0), 1e-10)
+    disp = torch.where(some, disp, float("nan"))
+    if white_background:
+        rgb = rgb + (1.0 - acc[..., None])
+    return rgb, disp, acc, weights, depth
+
+
 def bits_equal(a, b):
     """Same shape and the same bits (4-byte elements); two Nones are equal."""
     if a is None or b is None:

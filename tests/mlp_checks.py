@@ -47,6 +47,19 @@ SHAPES = [(1, 15), (37, 15), (33, 17)]
 # Worst raw element per output column as a fraction of the column's scale, wgmma forward (stash-writing and inference)
 # against fp64.  Measured on an H100 80GB HBM3, worst over all parameter sets and both weight states [1.1e-5].
 TC_FWD_TOL = 3e-5
+# The fp32 kernels' raw outputs per column (test_simt_hidden256_gpu.py FWD_TOL) [7.8e-7, test_tc_full_size_gpu.py].
+SIMT_FWD_TOL = 3e-5
+# Parameter gradients per block, relative to the block's scale (test_tc_arch_sweep_gpu.py BLOCK_TOL): at training size
+# wgmma [6.3e-6, a probe], fp32 kernels [4.1e-6, A2] (test_tc_full_size_gpu.py, H100 80GB HBM3, 700 W, 1980 MHz).
+BLOCK_TOL = 3e-5
+# How far from zero a ReLU tie may sit, relative to the layer's scale: the wgmma stash [1.1e-5, A0 fern], and the fp32
+# kernels' (test_tc_arch_sweep_gpu.py FP32_TIE_TOL).
+STASH_TOL = 2e-5
+FP32_TIE_TOL = 1e-5
+# Compositing against fp64 (helpers.composite64): every output relative to its scale, and d_raw relative to its scale
+# (test_stage_parity_gpu.py).
+COMP_TOL = 1e-4
+COMP_GRAD_TOL = 2e-4
 
 
 def spec(name):
@@ -277,6 +290,12 @@ def relu_ties(arch, stash, P, acts, family, tol, ctx, adopt, rows=None, scales=N
         n_ties += k
     assert n_ties <= 1e-5 * n_pts * lay.cum_total + 2, ctx + (n_ties,)
     return n_ties
+
+
+def _adopt_masks(arch, stash, P, masks):
+    """Give a wgmma stash the oracle's ReLU decisions (layer1 has no ReLU; the backward does not read its words)."""
+    for li in range(1, len(StashLayout(arch).layers)):
+        mask_words(arch, stash, P, li, "wgmma").copy_(masks[li])
 
 
 # ------------------------------------------------------------------------------------------------------------------------

@@ -12,17 +12,15 @@ import math
 import pytest
 import torch
 
-from helpers import Case, bits_equal, build_models
-from mlp_checks import (ALL_ARCHS, H256_ARCHS, SHAPES, TC_ARCHS, TC_FWD_TOL, _floors, _split_floors, arch_weights,
-                        check_blocks, oracle, report, spec, tc_blocks, upstream)
+from helpers import Case, bits_equal, build_models, composite64
+from mlp_checks import (ALL_ARCHS, BLOCK_TOL, COMP_GRAD_TOL, COMP_TOL, H256_ARCHS, SHAPES, SIMT_FWD_TOL, TC_ARCHS,
+                        TC_FWD_TOL, _floors, _split_floors, arch_weights, check_blocks, oracle, report, spec,
+                        tc_blocks, upstream)
 
 pytestmark = pytest.mark.gpu
 
-SIMT_FWD_TOL = 3e-5     # the fp32 kernels' raw outputs per column (test_simt_hidden256_gpu.py FWD_TOL)
 FAST_TOL = 2e-2         # the single-pass forward against fp64 (test_tc_fast_gpu.py FAST_TOL)
-BLOCK_TOL = 3e-5        # parameter gradients per block (test_tc_arch_sweep_gpu.py BLOCK_TOL)
-COMP_TOL = 1e-4         # compositing outputs, per output, relative to its scale
-COMP_GRAD_TOL = 2e-4    # d_raw relative to its scale (test_stage_parity_gpu.py)
+REF32_FACTOR = 4.0      # trained compositing regime, each output alone: x the fp32 reference's own error [2.0]
 
 
 def _nb():
@@ -216,20 +214,55 @@ def _comp_inputs(n, s, seed, empty_rays=0):
     return raw, z, dirs, noise
 
 
-@pytest.mark.parametrize("s", [2, 64, 192, 1024])
+def _trained_inputs(n, s, seed):
+    """Samples as a trained network makes them (raw sigma at 1e2 .. 1e4, surfaces, merged depths clustering there):
+    sigma * delta log-uniform over 1e-3 .. 1e3; a run of six samples at sigma * delta = 1e3 where the ray has room
+    (alpha rounds to 1 in fp32 and q to 1e-10, so T passes through the fp32 subnormals to 0); exact duplicate depths
+    (delta = 0); a last sample (delta = 1e10) with a tiny positive sigma, sigma * 1e10 |d| in 1e-2 .. 3, and no noise
+    so that it stays so.  The first sample's sigma is at least 3, so that no ray is empty."""
+    g = torch.Generator().manual_seed(seed)
+    z = torch.sort(torch.rand(n, s, generator=g) * 4 + 2, -1).values
+    if s >= 3:  # z[j + 1] = z[j] for some j >= 1, from the old values: z stays sorted
+        z[:, 2:] = torch.where(torch.rand(n, s - 2, generator=g) < 0.05, z[:, 1:-1], z[:, 2:])
+    if s >= 4:
+        z[:, s // 2] = z[:, s // 2 - 1]
+    dirs = torch.randn(n, 3, generator=g)
+    dnorm = dirs.norm(dim=-1, keepdim=True)
+    x = 10.0 ** (torch.rand(n, s, generator=g) * 6 - 3)
+    if s >= 10:
+        k = torch.randint(1, s - 7, (n, 1), generator=g)
+        j = torch.arange(s)[None]
+        x = torch.where((j >= k) & (j < k + 6), 1e3, x)
+    sigma = x[:, :-1] / ((z[:, 1:] - z[:, :-1]) * dnorm).clamp_min(1e-6)  # delta = 0: alpha is 0 whatever sigma
+    sigma[:, 0] = sigma[:, 0].clamp_min(3.0)
+    last = 10.0 ** (torch.rand(n, 1, generator=g) * 2.5 - 2) / (1e10 * dnorm)
+    raw = torch.randn(n, s, 4, generator=g) * 2
+    raw[..., 3] = torch.cat((sigma, last), -1)
+    noise = torch.randn(n, s, generator=g)
+    noise[:, -1] = 0.0
+    return raw, z, dirs, noise
+
+
+# "random": raw ~ 2 N(0, 1); "trained": the saturated regime of _trained_inputs, also at 199 samples (not a multiple of
+# the warp's 32 lanes).  The random regime keeps its original test ids.
+COMP_REGIMES = [("random", s) for s in (2, 64, 192, 1024)] + [("trained", s) for s in (2, 64, 192, 199, 1024)]
+COMP_IDS = [str(s) if r == "random" else f"{r}-{s}" for r, s in COMP_REGIMES]
+
+
+@pytest.mark.parametrize("regime, s", COMP_REGIMES, ids=COMP_IDS)
 @pytest.mark.parametrize("white", [False, True])
 @pytest.mark.parametrize("noise_std", [0.0, 0.3])
-def test_volume_render_outputs_and_gradients_match_fp64(s, white, noise_std):
+def test_volume_render_outputs_and_gradients_match_fp64(regime, s, white, noise_std):
     from oracle import nerf_oracle as O
 
     nb = _nb()
     n = 37
-    raw, z, dirs, noise = _comp_inputs(n, s, seed=51 + s)
+    raw, z, dirs, noise = (_comp_inputs if regime == "random" else _trained_inputs)(n, s, seed=51 + s)
     raw64 = raw.double().requires_grad_(True)
-    want = O.volume_render_radiance_field(raw64, z.double(), dirs.double(), noise_std, white, noise=noise.double())
+    want = composite64(raw, z, dirs, noise_std, white, noise, raw64=raw64)
     raw_c = raw.cuda().requires_grad_(True)
     got = nb.volume_render_radiance_field(raw_c, z.cuda(), dirs.cuda(), noise_std, white, noise=noise.cuda())
-    ctx = (s, white, noise_std)
+    ctx = (regime, s, white, noise_std)
     names = ("rgb", "disp", "acc", "weights", "depth")
     for name, a, b in zip(names, got, want):
         assert a.shape == b.shape and a.dtype == torch.float32, ctx + (name,)
@@ -244,16 +277,28 @@ def test_volume_render_outputs_and_gradients_match_fp64(s, white, noise_std):
     e = (raw_c.grad.double().cpu() - raw64.grad).abs().max().item()
     report("volume_render d_raw", ctx, e / scale)
     assert e <= COMP_GRAD_TOL * scale, ctx + (e, scale)
-    # each output alone, the two the render backward never took (weights and depth) included
+    # each output alone, the two the render backward never took (weights and depth) included.  In the trained regime the
+    # gradient of acc alone is cancellation: on an opaque ray acc = 1 - T_end is flat in every sigma (d acc / d sigma_i
+    # ~ T_end ~ 0) while the terms that cancel are ~T_i, so no fp32 evaluation resolves it; there the bar adds
+    # REF32_FACTOR x the error of the fp32 reference itself (O.volume_render_radiance_field in fp32 autograd, 1.5e2 ..
+    # 5.5e2 x the gradient's scale; the kernel's is at most 2.0 x the reference's, on an H100 80GB HBM3 at 700 W).
     for i, name in enumerate(names):
         raw64.grad = raw_c.grad = None
-        w64 = O.volume_render_radiance_field(raw64, z.double(), dirs.double(), noise_std, white, noise=noise.double())
+        w64 = composite64(raw, z, dirs, noise_std, white, noise, raw64=raw64)
         wc = nb.volume_render_radiance_field(raw_c, z.cuda(), dirs.cuda(), noise_std, white, noise=noise.cuda())
         (w64[i] * ups[i]).sum().backward()
         (wc[i] * ups[i].float().cuda()).sum().backward()
         scale = raw64.grad.abs().max().item()
         e = (raw_c.grad.double().cpu() - raw64.grad).abs().max().item()
-        assert e <= COMP_GRAD_TOL * scale, ctx + (name, e, scale)
+        e_ref = 0.0
+        if regime == "trained":
+            r32 = raw.clone().requires_grad_(True)
+            w32 = O.volume_render_radiance_field(r32, z, dirs, noise_std, white, noise=noise)
+            (w32[i] * ups[i].float()).sum().backward()
+            e_ref = (r32.grad.double() - raw64.grad).abs().max().item()
+            report(f"volume_render d_raw of {name} alone / (bar + fp32 reference's error)", ctx,
+                   e / (COMP_GRAD_TOL * scale + REF32_FACTOR * e_ref))
+        assert e <= COMP_GRAD_TOL * scale + REF32_FACTOR * e_ref, ctx + (name, e, scale, e_ref)
 
 
 def test_volume_render_empty_rays_give_the_references_nan_disparity():

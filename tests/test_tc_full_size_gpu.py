@@ -30,19 +30,18 @@ import pytest
 import torch
 
 from helpers import load_weights
-from mlp_checks import (TC_FWD_TOL, StashLayout, _floors, _split_floors, arch_weights, blob_range_factor,
-                        check_blocks, encodings, mask_words, oracle, oracle_tiles, pack_mask, points,
-                        random_previous, read_layer, relu_ties, report, sms, tc_blocks, upstream)
+from mlp_checks import (BLOCK_TOL, FP32_TIE_TOL, SIMT_FWD_TOL, STASH_TOL, TC_FWD_TOL, StashLayout, _adopt_masks,
+                        _floors, _split_floors, arch_weights, blob_range_factor, check_blocks, encodings, oracle,
+                        oracle_tiles, pack_mask, points, random_previous, read_layer, relu_ties, report, sms, tc_blocks,
+                        upstream)
 
 pytestmark = pytest.mark.gpu
 
-# Worst element as a fraction of the compared scale: the bars of test_tc_arch_sweep_gpu.py (TC_FWD_TOL, 3e-5, from
-# mlp_checks), the worst figure over this file's cases in brackets, measured on an H100 80GB HBM3 at a 700 W power limit
-# and 1980 MHz SM clock.  wgmma forward raw [2.8e-5, A0 fern]: its pretrained weights far outside their scene.
-STASH_TOL = 2e-5     # stashed activation and encoding tiles; also how far from zero a ReLU tie may sit [1.1e-5, A0 fern]
-BLOCK_TOL = 3e-5     # parameter gradients, per block: wgmma [6.3e-6, a probe], fp32 kernels [4.1e-6, A2]
-FP32_TIE_TOL = 1e-5  # how far from zero an fp32 ReLU tie may sit (test_tc_arch_sweep_gpu.py FP32_TIE_TOL)
-SIMT_FWD_TOL = 3e-5  # the fp32 kernels' raw outputs per column (test_simt_hidden256_gpu.py FWD_TOL) [7.8e-7]
+# Worst element as a fraction of the compared scale: the bars of test_tc_arch_sweep_gpu.py (TC_FWD_TOL, BLOCK_TOL,
+# SIMT_FWD_TOL, all 3e-5, and STASH_TOL, 2e-5, for stashed activation and encoding tiles too, from mlp_checks), the worst
+# figure over this file's cases in brackets, measured on an H100 80GB HBM3 at a 700 W power limit and 1980 MHz SM clock.
+# wgmma forward raw [2.8e-5, A0 fern]: its pretrained weights far outside their scene; stashed tiles [1.1e-5, A0 fern];
+# parameter gradients per block: wgmma [6.3e-6, a probe], fp32 kernels [4.1e-6, A2]; the fp32 kernels' raw [7.8e-7].
 ORACLE_PIN = 1e-12   # the device oracle against the CPU oracle, relative to each tensor's scale [2.4e-15]
 
 NETS = {  # ops.ArchSpec arguments
@@ -121,12 +120,6 @@ def _compositing_upstream(raw, rays, z, seed):
     rgb = nb.volume_render_radiance_field(r, z, rays[:, 3:6], 0.0, False)[0]
     G, = torch.autograd.grad(torch.nn.functional.mse_loss(rgb, target), r)
     return _to_4_8(G).contiguous()
-
-
-def _adopt_masks(arch, stash, P, masks):
-    """Give a wgmma stash the oracle's ReLU decisions (layer1 has no ReLU; the backward does not read its words)."""
-    for li in range(1, len(StashLayout(arch).layers)):
-        mask_words(arch, stash, P, li, "wgmma").copy_(masks[li])
 
 
 # ------------------------------------------------------------------------------------------------------------------------
