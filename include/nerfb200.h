@@ -282,6 +282,49 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
 int32_t nerfb200_adam_step(float* p, const float* g, float* m, float* v, int64_t n, int32_t step, float lr,
                            float beta1, float beta2, float eps, float grad_scale, void* stream);
 
+/* ---- a training step with no host work between its launches (one CUDA graph per step) ------------------
+ * A captured graph freezes kernel arguments, so the one value that changes between replays is a step counter in device
+ * memory: step_dev (int64) holds the number of optimisation steps done before this one, and every entry point below
+ * that depends on the step reads it there when it runs.  nerfb200_step_advance adds 1 after the step's updates.
+ *
+ * random_fill_dev: nerfb200_random_fill with rng->step replaced by *step_dev (rng->step must be 0); the same device
+ *   function, so the render kernels fed these tensors give the bits of a render call given the rng at that step.
+ *   *step_dev >= 2^30 writes NaN (its counters would alias another step's).
+ * draw_pixels: from (seed, *step_dev), *image_out = one image uniformly out of n_images and ids_out[n] = n distinct
+ *   pixel ids out of n_pixels, uniform without replacement (the reference's two np.random.choice calls): each pixel gets a
+ *   64-bit Philox key and the n smallest (key, id) pairs are taken, in ascending key order.  Exact and deterministic;
+ *   its Philox counters never coincide with the render streams' (csrc/common.cuh).  n > n_pixels: NERFB200_ERR_INVALID.
+ *   workspace: nerfb200_draw_workspace_bytes(n_pixels) bytes (-1: n_pixels outside 1 .. 2^31 - 1).
+ * gen_rays_posed: nerfb200_gen_rays with the pose read on the device: the top 3 x 4 block of poses[*image] of a
+ *   [n_images][pose_rows][4] table (pose_rows 3 or 4); the same rows as gen_rays given that pose, bit for bit.
+ * gather_rows: out[k][0..2] = src[*image * rows_per_image + ids[k]][0..2] (targets, or a ray pool's rows).
+ * mse_loss: *loss = mse(out_coarse[:, :3], target) + mse(out_fine[:, :3], target) (the coarse term alone when out_fine is
+ *   NULL), out_* the [n][8] rows of render_fwd, target [n][3]; g_coarse / g_fine [n][8] receive the upstream gradients
+ *   render_bwd takes, bit for bit what autograd of torch's mean mse_loss gives: fp32(fp32(2 / 3n) * fp32(x - t)) in
+ *   columns 0..2, zero elsewhere.  The loss sums the squares in fp64 and rounds each mean once.
+ * lr_schedule: lr_out[i] = the rate parallel.FusedAdam uses for the step after done[i] steps, lr0 * lr_decay_factor **
+ *   (max(done[i] - 1, 0) / (lr_decay * 1000)) in fp64 rounded once to fp32 (lr0 when lr_decay is 0).
+ * adam_step_dev: nerfb200_adam_step for step *step_dev + 1 at rate lr_schedule(*step_dev); same bits as adam_step given
+ *   that step and rate. */
+int32_t nerfb200_random_fill_dev(const nerfb200_rng_t* rng, const int64_t* step_dev, int32_t stream_id, int64_t n_rays,
+                                 int32_t per_ray, float* out, void* stream);
+int64_t nerfb200_draw_workspace_bytes(int64_t n_pixels);
+int32_t nerfb200_draw_pixels(uint64_t seed, const int64_t* step_dev, int32_t n_images, int64_t n_pixels, int64_t n,
+                             int64_t* image_out, int64_t* ids_out, void* workspace, void* stream);
+int32_t nerfb200_gen_rays_posed(const float* poses, int32_t pose_rows, const int64_t* image, int32_t height,
+                                int32_t width, float focal, const int64_t* pixel_ids, int64_t n, int32_t ndc, float near,
+                                float far, int32_t use_viewdirs, int32_t out_stride, float* out, void* stream);
+int32_t nerfb200_gather_rows(const float* src, int64_t rows_per_image, const int64_t* image, const int64_t* ids,
+                             int64_t n, float* out, void* stream);
+int32_t nerfb200_mse_loss(const float* out_coarse, const float* out_fine, const float* target, int64_t n, float* loss,
+                          float* g_coarse, float* g_fine, void* stream);
+int32_t nerfb200_lr_schedule(const int64_t* done, int64_t n, double lr0, double lr_decay, double lr_decay_factor,
+                             float* lr_out, void* stream);
+int32_t nerfb200_adam_step_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* step_dev,
+                               double lr0, double lr_decay, double lr_decay_factor, float beta1, float beta2, float eps,
+                               float grad_scale, void* stream);
+int32_t nerfb200_step_advance(int64_t* step_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -57,7 +57,7 @@ class Rng(C.Structure):
 
 
 P = C.c_void_p
-I32, I64, F32 = C.c_int32, C.c_int64, C.c_float
+I32, I64, F32, F64, U64 = C.c_int32, C.c_int64, C.c_float, C.c_double, C.c_uint64
 AP, OP, RP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng)
 
 # name -> (restype, argtypes); mirrors include/nerfb200.h one-to-one
@@ -95,6 +95,15 @@ SIGNATURES = {
     "nerfb200_render_bwd": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, P, P, P, I32, I32, P]),
     "nerfb200_random_fill": (I32, [RP, I32, I64, I32, P, P]),
     "nerfb200_adam_step": (I32, [P, P, P, P, I64, I32, F32, F32, F32, F32, F32, P]),
+    "nerfb200_random_fill_dev": (I32, [RP, P, I32, I64, I32, P, P]),
+    "nerfb200_draw_workspace_bytes": (I64, [I64]),
+    "nerfb200_draw_pixels": (I32, [U64, P, I32, I64, I64, P, P, P, P]),
+    "nerfb200_gen_rays_posed": (I32, [P, I32, P, I32, I32, F32, P, I64, I32, F32, F32, I32, I32, P, P]),
+    "nerfb200_gather_rows": (I32, [P, I64, P, P, I64, P, P]),
+    "nerfb200_mse_loss": (I32, [P, P, P, I64, P, P, P, P]),
+    "nerfb200_lr_schedule": (I32, [P, I64, F64, F64, F64, P, P]),
+    "nerfb200_adam_step_dev": (I32, [P, P, P, P, I64, P, F64, F64, F64, F32, F32, F32, F32, P]),
+    "nerfb200_step_advance": (I32, [P, P]),
 }
 
 _lib = None

@@ -87,6 +87,13 @@ struct Plan {
 //                            evaluated in fp64 and rounded once to fp32.
 // So every random number is a pure function of (seed, step, stream, global ray, sample): a ray gets the same numbers
 // whatever the chunking of the batch or its sharding across GPUs.  step < 2^30 keeps stream + 4 * step in 32 bits.
+//
+// The pixel draw of a training step (step.cu, nerfb200_draw_pixels) uses the same key and reserves a counter word:
+//   counter = (q, step & 0xffffffff, purpose, 0x80000000)
+// purpose 0: the 64-bit keys of pixels 2q (words 0, 1) and 2q + 1 (words 2, 3); purpose 1, q = 0: the image (words 0, 1).
+// The render streams' last word is the high half of a global ray index >= 0 and < 2^63, so its top bit is never set:
+// the draw's counters cannot coincide with any render stream's, for any step.  (A fifth render stream id instead would
+// be stream + 4 * step = 4 + 4 * step, which is stream 0 of the next step.)
 // ---------------------------------------------------------------------------------------------
 enum RandStream { kRandTRand = 0, kRandNoiseC = 1, kRandU = 2, kRandNoiseF = 3 };
 
@@ -157,6 +164,20 @@ int launch_sample_pdf_merge(const float* z_coarse, const float* weights_coarse, 
                             float* z_samples, int32_t* inds, float* cdf_out, cudaStream_t s);
 int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2,
                 float eps, float grad_scale, cudaStream_t s);
+
+// ---- a training step whose step count lives in device memory (step.cu; nerfb200.h "a training step ...") ----
+// the learning-rate schedule of parallel.FusedAdam: lr0 * factor ** (max(done - 1, 0) / (decay * 1000)); decay <= 0: lr0
+struct LrSchedule {
+  double lr0, decay, factor;
+};
+int launch_random_fill_dev(const RandSrc& src, const int64_t* step, int stream_id, int64_t n_rays, int per_ray,
+                           float* out, cudaStream_t s);
+int launch_gen_rays_posed(const float* poses, int pose_rows, const int64_t* image, int height, int width, float focal,
+                          const int64_t* pix, int64_t n, int ndc, float near, float far, int use_viewdirs, int out_stride,
+                          float* out, cudaStream_t s);
+int launch_lr_schedule(const int64_t* done, int64_t n, const LrSchedule& sch, float* out, cudaStream_t s);
+int launch_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* done, const LrSchedule& sch,
+                    float b1, float b2, float eps, float grad_scale, cudaStream_t s);
 
 // The MLP kernel families.  Each file's predicate says whether its kernels take a plan (NERFB200_OK, else the reason
 // in the last error, prefixed with `what`); api.cu's check_impl maps an impl code to them, and its mlp_forward /

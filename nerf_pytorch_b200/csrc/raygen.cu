@@ -56,21 +56,36 @@ __device__ __forceinline__ void finish_ray(const RayGenArgs& a, float ox, float 
   if (a.out_stride >= 11) { row[8] = vx; row[9] = vy; row[10] = vz; }
 }
 
+// the ray of pixel id = j * W + i of the camera with 3 x 4 camera-to-world rows c2w
+__device__ __forceinline__ void pixel_ray(const RayGenArgs& a, const float* c2w, int64_t id, float* __restrict__ row) {
+  const int j = (int)(id / a.width), i = (int)(id - (int64_t)j * a.width);
+  const float c0 = __fdiv_rn(__fadd_rn((float)i, -a.half_w), a.focal);
+  const float c1 = __fdiv_rn(-__fadd_rn((float)j, -a.half_h), a.focal);
+  const float c2 = -1.0f;
+  float d[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)  // sum(directions[..., None, :] * c2w[:3, :3], dim=-1)
+    d[r] = __fadd_rn(__fadd_rn(__fmul_rn(c0, c2w[4 * r]), __fmul_rn(c1, c2w[4 * r + 1])), __fmul_rn(c2, c2w[4 * r + 2]));
+  finish_ray(a, c2w[3], c2w[7], c2w[11], d[0], d[1], d[2], row);
+}
+
 // rays from (pose, pixel ids): pix[k] = j * W + i (row-major over the image), or all H*W pixels when pix == nullptr
 __global__ void gen_rays_kernel(const __grid_constant__ RayGenArgs a, const int64_t* __restrict__ pix, int64_t n,
                                 float* __restrict__ out) {
-  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t id = pix ? pix[k] : k;
-    const int j = (int)(id / a.width), i = (int)(id - (int64_t)j * a.width);
-    const float c0 = __fdiv_rn(__fadd_rn((float)i, -a.half_w), a.focal);
-    const float c1 = __fdiv_rn(-__fadd_rn((float)j, -a.half_h), a.focal);
-    const float c2 = -1.0f;
-    float d[3];
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
+    pixel_ray(a, a.c2w, pix ? pix[k] : k, out + k * a.out_stride);
+}
+
+// the same rays with the pose read on the device: entry *image of a [n_images][pose_rows][4] table (pose_rows 3 or 4)
+__global__ void gen_rays_posed_kernel(const __grid_constant__ RayGenArgs a, const float* __restrict__ poses, int pose_rows,
+                                      const int64_t* __restrict__ image, const int64_t* __restrict__ pix, int64_t n,
+                                      float* __restrict__ out) {
+  const float* pose = poses + *image * pose_rows * 4;
+  float c2w[12];
 #pragma unroll
-    for (int r = 0; r < 3; ++r)  // sum(directions[..., None, :] * c2w[:3, :3], dim=-1)
-      d[r] = __fadd_rn(__fadd_rn(__fmul_rn(c0, a.c2w[4 * r]), __fmul_rn(c1, a.c2w[4 * r + 1])), __fmul_rn(c2, a.c2w[4 * r + 2]));
-    finish_ray(a, a.c2w[3], a.c2w[7], a.c2w[11], d[0], d[1], d[2], out + k * a.out_stride);
-  }
+  for (int e = 0; e < 12; ++e) c2w[e] = pose[e];
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
+    pixel_ray(a, c2w, pix[k], out + k * a.out_stride);
 }
 
 // packing of caller-supplied origins / directions (the reference API: run_one_iter_of_nerf takes the two tensors)
@@ -104,6 +119,19 @@ int launch_gen_rays(const float* c2w12_host, int height, int width, float focal,
   gen_rays_kernel<<<(unsigned)blocks, 256, 0, s>>>(a, pix, n, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "gen_rays launch");
+}
+
+int launch_gen_rays_posed(const float* poses, int pose_rows, const int64_t* image, int height, int width, float focal,
+                          const int64_t* pix, int64_t n, int ndc, float near, float far, int use_viewdirs, int out_stride,
+                          float* out, cudaStream_t s) {
+  RayGenArgs a;
+  int rc = fill_args(&a, nullptr, height, width, focal, ndc, near, far, use_viewdirs, out_stride);
+  if (rc) return rc;
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  gen_rays_posed_kernel<<<(unsigned)blocks, 256, 0, s>>>(a, poses, pose_rows, image, pix, n, out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "gen_rays_posed launch");
 }
 
 int launch_pack_rays(const float* ro, const float* rd, int64_t n, int height, int width, float focal, int ndc, float near,

@@ -74,6 +74,34 @@ int launch_random_fill(const RandSrc& src, int stream_id, int64_t n_rays, int pe
   return check_cuda(cudaGetLastError(), "random_fill launch");
 }
 
+// the same with the step read from the device (src.ctr1 holds the stream id): a step >= 2^30, whose counter word would
+// alias another step's, writes NaN instead
+__global__ void random_fill_dev_kernel(RandSrc src, const int64_t* __restrict__ step, int normal, int64_t n_rays,
+                                       int per_ray, float* __restrict__ out) {
+  const int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (idx >= n_rays * per_ray) return;
+  const int64_t st = *step;
+  if (st < 0 || st >= (int64_t(1) << 30)) {
+    out[idx] = __int_as_float(0x7fc00000);
+    return;
+  }
+  src.ctr1 += 4u * (uint32_t)st;
+  const int64_t r = idx / per_ray;
+  const int j = (int)(idx - r * per_ray);
+  out[idx] = normal ? src.normal(r, j) : src.uniform(r, j);
+}
+
+int launch_random_fill_dev(const RandSrc& src, const int64_t* step, int stream_id, int64_t n_rays, int per_ray,
+                           float* out, cudaStream_t s) {
+  const int64_t total = n_rays * per_ray;
+  const int threads = 256;
+  const int64_t blocks = (total + threads - 1) / threads;
+  const int normal = stream_id == kRandNoiseC || stream_id == kRandNoiseF;
+  random_fill_dev_kernel<<<(unsigned)blocks, threads, 0, s>>>(src, step, normal, n_rays, per_ray, out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "random_fill_dev launch");
+}
+
 // ---------------------------------------------------------------------------------------------
 // stand-alone positional encoding (test hook; the MLP kernels encode in their prologue)
 // ---------------------------------------------------------------------------------------------
@@ -305,9 +333,9 @@ int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------
 // fused Adam over a flat vector (torch.optim.Adam, amsgrad off, weight_decay 0)
 // ---------------------------------------------------------------------------------------------
-__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                            float* __restrict__ v, int64_t n, float lr_over_bc1, float inv_sqrt_bc2, float b1,
-                            float b2, float eps, float grad_scale) {
+__device__ __forceinline__ void adam_update(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                            float* __restrict__ v, int64_t n, float lr_over_bc1, float inv_sqrt_bc2,
+                                            float b1, float b2, float eps, float grad_scale) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float gi = g[i] * grad_scale;
     const float mi = m[i] + (gi - m[i]) * (1.f - b1);         // exp_avg.lerp_(grad, 1 - beta1)
@@ -317,6 +345,12 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
     const float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;       // sqrt(v) / sqrt(bc2) + eps
     p[i] = p[i] - lr_over_bc1 * (mi / denom);                 // addcdiv_(m, denom, value=-lr/bc1)
   }
+}
+
+__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                            float* __restrict__ v, int64_t n, float lr_over_bc1, float inv_sqrt_bc2, float b1,
+                            float b2, float eps, float grad_scale) {
+  adam_update(p, g, m, v, n, lr_over_bc1, inv_sqrt_bc2, b1, b2, eps, grad_scale);
 }
 
 int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int step, float lr, float b1, float b2,
@@ -330,6 +364,54 @@ int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, int ste
                                                    eps, grad_scale);
   count_launch();
   return check_cuda(cudaGetLastError(), "adam launch");
+}
+
+// parallel.FusedAdam.current_lr after `done` steps, in fp64 and rounded once to fp32 as the float argument of adam_step
+// is: lr0 * factor ** (max(done - 1, 0) / (decay * 1000)), or lr0 without a schedule (decay <= 0)
+__device__ __forceinline__ float scheduled_lr(int64_t done, const LrSchedule& sch) {
+  if (!(sch.decay > 0.0)) return (float)sch.lr0;
+  const double e = (double)(done > 1 ? done - 1 : 0) / (sch.decay * 1000.0);
+  return (float)(sch.lr0 * pow(sch.factor, e));
+}
+
+__global__ void lr_schedule_kernel(const int64_t* __restrict__ done, int64_t n, LrSchedule sch, float* __restrict__ out) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = scheduled_lr(done[i], sch);
+}
+
+int launch_lr_schedule(const int64_t* done, int64_t n, const LrSchedule& sch, float* out, cudaStream_t s) {
+  lr_schedule_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(done, n, sch, out);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "lr_schedule launch");
+}
+
+// adam_kernel with the step count read from the device: *done steps before this one, so this is step *done + 1 at the
+// rate of scheduled_lr(*done); the scalars are formed in fp64 as launch_adam forms them on the host
+__global__ void adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                float* __restrict__ v, int64_t n, const int64_t* __restrict__ done, LrSchedule sch,
+                                float b1, float b2, float eps, float grad_scale) {
+  __shared__ float scal[2];
+  if (threadIdx.x == 0) {
+    const int64_t d = *done;
+    const float lr = scheduled_lr(d, sch);
+    const double step = (double)(d + 1);
+    const double bc1 = 1.0 - pow((double)b1, step);
+    const double bc2 = 1.0 - pow((double)b2, step);
+    scal[0] = (float)(lr / bc1);
+    scal[1] = (float)(1.0 / sqrt(bc2));
+  }
+  __syncthreads();
+  adam_update(p, g, m, v, n, scal[0], scal[1], b1, b2, eps, grad_scale);
+}
+
+int launch_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* done, const LrSchedule& sch,
+                    float b1, float b2, float eps, float grad_scale, cudaStream_t s) {
+  const int threads = 256;
+  int64_t blocks = (n + threads - 1) / threads;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  adam_dev_kernel<<<(unsigned)blocks, threads, 0, s>>>(p, g, m, v, n, done, sch, b1, b2, eps, grad_scale);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "adam_dev launch");
 }
 
 }  // namespace nerfb200

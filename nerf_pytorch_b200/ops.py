@@ -432,6 +432,106 @@ def adam_step(p, g, m, v, step, lr, beta1=0.9, beta2=0.999, eps=1e-8, grad_scale
 
 
 # ------------------------------------------------------------------------------------------------
+# a training step whose step count lives on the device (include/nerfb200.h: every value that changes from one step to
+# the next is read from ``step_dev``, an int64 CUDA tensor of one element holding the steps done before this one)
+# ------------------------------------------------------------------------------------------------
+def random_fill_dev(seed: int, step_dev, stream, n_rays: int, per_ray: int, ray_offset: int = 0, out=None):
+    """``random_fill(SeededRandoms(seed, step, ray_offset), ...)`` with step = ``step_dev`` read when the kernel runs."""
+    sid = RAND_STREAMS[stream] if isinstance(stream, str) else int(stream)
+    if out is None:
+        out = torch.empty(int(n_rays), int(per_ray), dtype=torch.float32, device=step_dev.device)
+    _lib.check(_lib.load().nerfb200_random_fill_dev(C.byref(SeededRandoms(seed, 0, ray_offset).c_struct()),
+                                                    _ptr(step_dev), sid, int(n_rays), int(per_ray), _ptr(out),
+                                                    _stream()), "random_fill_dev")
+    return out
+
+
+def draw_workspace_bytes(n_pixels: int) -> int:
+    n = _lib.load().nerfb200_draw_workspace_bytes(int(n_pixels))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, f"draw_workspace_bytes (n_pixels {n_pixels})")
+    return n
+
+
+def draw_pixels(seed: int, step_dev, n_images: int, n_pixels: int, n: int, image=None, ids=None, workspace=None):
+    """One image index out of ``n_images`` and ``n`` distinct pixel ids out of ``n_pixels`` from (seed, step): returns
+    (image int64[1], ids int64[n]), both on the device."""
+    dev = step_dev.device
+    if image is None:
+        image = torch.empty(1, dtype=torch.int64, device=dev)
+    if ids is None:
+        ids = torch.empty(int(n), dtype=torch.int64, device=dev)
+    if workspace is None:
+        workspace = torch.empty(draw_workspace_bytes(n_pixels), dtype=torch.uint8, device=dev)
+    _lib.check(_lib.load().nerfb200_draw_pixels(int(seed), _ptr(step_dev), int(n_images), int(n_pixels), int(n),
+                                                _ptr(image), _ptr(ids), _ptr(workspace), _stream()), "draw_pixels")
+    return image, ids
+
+
+def gen_rays_posed(poses, image, height, width, focal, pixel_ids, ndc=False, near=0.0, far=1.0, use_viewdirs=True,
+                   out=None):
+    """``gen_rays`` of the pose ``poses[image]`` of a device table (n_images, 3 | 4, 4), ``image`` an int64[1] tensor."""
+    stride = 11 if use_viewdirs else 8
+    if out is None:
+        out = torch.empty(pixel_ids.numel(), stride, dtype=torch.float32, device=pixel_ids.device)
+    _lib.check(_lib.load().nerfb200_gen_rays_posed(_ptr(poses), int(poses.shape[1]), _ptr(image), int(height),
+                                                   int(width), float(focal), _ptr(pixel_ids), pixel_ids.numel(),
+                                                   int(bool(ndc)), float(near), float(far), int(bool(use_viewdirs)),
+                                                   stride, _ptr(out), _stream()), "gen_rays_posed")
+    return out
+
+
+def gather_rows(src, rows_per_image: int, image, ids, out=None):
+    """Rows ``image * rows_per_image + ids`` of ``src`` (rows of 3 floats): (n, 3)."""
+    if out is None:
+        out = torch.empty(ids.numel(), 3, dtype=torch.float32, device=ids.device)
+    _lib.check(_lib.load().nerfb200_gather_rows(_ptr(src), int(rows_per_image), _ptr(image), _ptr(ids), ids.numel(),
+                                                _ptr(out), _stream()), "gather_rows")
+    return out
+
+
+def mse_loss(out_c, out_f, target, loss=None, g_c=None, g_f=None):
+    """mse(out_c[:, :3], target) (+ the same of out_f) into a 0-dim tensor, and the (n, 8) upstream gradients of
+    ``render_bwd``.  Returns (loss, g_c, g_f)."""
+    n = out_c.shape[0]
+    dev = out_c.device
+    if loss is None:
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+    if g_c is None:
+        g_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    if out_f is not None and g_f is None:
+        g_f = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().nerfb200_mse_loss(_ptr(out_c), _ptr(out_f), _ptr(target), n, _ptr(loss), _ptr(g_c),
+                                             _ptr(g_f), _stream()), "mse_loss")
+    return loss, g_c, g_f
+
+
+def _schedule(lr0, lr_decay, lr_decay_factor):
+    return float(lr0), (0.0 if lr_decay is None else float(lr_decay)), float(lr_decay_factor)
+
+
+def lr_schedule(done, lr0, lr_decay=None, lr_decay_factor=0.1):
+    """The fp32 rate ``parallel.FusedAdam`` uses after ``done`` (int64 CUDA tensor) steps, computed on the device."""
+    out = torch.empty(done.numel(), dtype=torch.float32, device=done.device)
+    _lib.check(_lib.load().nerfb200_lr_schedule(_ptr(done), done.numel(), *_schedule(lr0, lr_decay, lr_decay_factor),
+                                                _ptr(out), _stream()), "lr_schedule")
+    return out
+
+
+def adam_step_dev(p, g, m, v, step_dev, lr0, lr_decay=None, lr_decay_factor=0.1, beta1=0.9, beta2=0.999, eps=1e-8,
+                  grad_scale=1.0):
+    """``adam_step`` of step ``step_dev + 1`` at the scheduled rate, both read on the device."""
+    _lib.check(_lib.load().nerfb200_adam_step_dev(_ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), _ptr(step_dev),
+                                                  *_schedule(lr0, lr_decay, lr_decay_factor), float(beta1),
+                                                  float(beta2), float(eps), float(grad_scale), _stream()),
+               "adam_step_dev")
+
+
+def step_advance(step_dev):
+    _lib.check(_lib.load().nerfb200_step_advance(_ptr(step_dev), _stream()), "step_advance")
+
+
+# ------------------------------------------------------------------------------------------------
 # whole path
 # ------------------------------------------------------------------------------------------------
 WS_SECTIONS = ("z_coarse", "raw_coarse", "weights_coarse", "z_fine", "raw_fine", "stash_coarse", "stash_fine",
