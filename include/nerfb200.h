@@ -276,6 +276,62 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
                             void* stream);
 
+/* ---- occupancy grid: inference renders that skip the MLP in empty space ---------------------------------------
+ * A bitfield over the axis-aligned box [lo, hi) in the coordinates the MLP encodes (world space, or NDC for forward-facing
+ * scenes), res[0] x res[1] x res[2] cells.  The cell of a point x, per axis c, all in fp32 with round-to-nearest:
+ *     scale_c = (float)res[c] / (hi[c] - lo[c]);   t_c = (x_c - lo[c]) * scale_c
+ * x is inside the box iff 0 <= t_c < res[c] on every axis (a NaN coordinate is outside); then i_c = (int)t_c and the
+ * cell's index is  idx = (i_2 * res[1] + i_1) * res[0] + i_0  (x fastest).  The bitfield is uint32
+ * words[nerfb200_grid_words(grid)], cell idx at bit (idx & 31) of word idx >> 5 (least significant bit first); a set bit
+ * is an occupied cell.  A sample inside the box whose cell bit is clear is skipped; a sample outside the box is always
+ * evaluated. */
+typedef struct nerfb200_grid {
+  float lo[3];
+  float hi[3];
+  int32_t res[3]; /* cells per axis, 1 .. 4096 */
+} nerfb200_grid_t;
+#define NERFB200_GRID_MAX_RES 4096
+
+/* uint32 words of the grid's bitfield; -1 for an invalid descriptor (res outside 1 .. 4096, hi <= lo, non-finite). */
+int64_t nerfb200_grid_words(const nerfb200_grid_t* grid);
+/* Host restatement of the cell rule above (test hook): cell_out[i] = the cell index of point xyz_host[i][3], or -1 when
+ * the point lies outside the box.  Host memory only. */
+int32_t nerfb200_grid_locate(const nerfb200_grid_t* grid, const float* xyz_host, int64_t n, int64_t* cell_out);
+
+/* Sample compaction of one pass (stage entry point and test hook).  For every sample s of ray r, the point
+ * o + d z[r][s] is formed as the MLP forward forms it and looked up in the grid:
+ *   - a skipped sample gets raw[r][s] = [0 0 0 -inf]: the compositing then gives it alpha = 0 and weight 0 exactly, with
+ *     or without noise (-inf + noise * std = -inf, ReLU -> sigma 0, exp(-0 * delta) = 1);
+ *   - the evaluated samples, in (ray, sample) order, become the rows of map[]: rays are taken in groups of 10
+ *     consecutive rays (the most one 64-row MLP block may touch), each group's evaluated samples fill whole 64-row
+ *     blocks, and the rows after a group's last sample up to its block's end hold -1 (padding).  map[row] = r * n_samples
+ *     + s.  blocks[2 b], blocks[2 b + 1] = the first and last ray block b touches.
+ * *n_blocks (device int32) = the number of blocks written, *n_evaluated (device int64, may be NULL) = evaluated samples.
+ * Sizes: map int32[64 * nerfb200_grid_max_blocks(n_rays, n_samples)], blocks int32[2 * that];
+ * scratch int32[nerfb200_grid_scratch_ints(n_rays, n_samples)].  Prefix sums throughout: the same inputs give the
+ * same map.  No host synchronisation: the counts stay in device memory. */
+int64_t nerfb200_grid_max_blocks(int64_t n_rays, int32_t n_samples);
+int64_t nerfb200_grid_scratch_ints(int64_t n_rays, int32_t n_samples);
+int32_t nerfb200_grid_compact(const nerfb200_grid_t* grid, const uint32_t* bits, const float* rays, int32_t ray_stride,
+                              const float* z, int64_t n_rays, int32_t n_samples, float* raw, int32_t* map,
+                              int32_t* blocks, int32_t* n_blocks, int64_t* n_evaluated, int32_t* scratch, void* stream);
+
+/* nerfb200_render_fwd for inference (training = 0) with an occupancy grid: after each pass's depths, the compaction above
+ * decides which samples run the MLP; the wgmma forward runs over the map only (impl 1 or 3; impl 0 is refused with
+ * NERFB200_ERR_UNSUPPORTED) and writes raw[point] of each evaluated point, bit for bit what render_fwd computes for it.
+ * The random inputs are those of render_fwd.  With every cell occupied the six outputs equal render_fwd's bit for bit.
+ * workspace: nerfb200_render_grid_workspace_bytes(...) bytes; its first sections are those of render_fwd's inference
+ * workspace (nerfb200_render_workspace_layout with training = 0).  n_evaluated: device int64[2] receiving the evaluated
+ * samples of the coarse and the fine pass, or NULL. */
+int64_t nerfb200_render_grid_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                             const nerfb200_render_opts_t* opts, int64_t n_rays);
+int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                 const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                 const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                 const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                 const nerfb200_grid_t* grid, const uint32_t* bits, float* out_coarse, float* out_fine,
+                                 void* workspace, int32_t impl, int64_t* n_evaluated, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

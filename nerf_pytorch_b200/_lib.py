@@ -56,9 +56,19 @@ class Rng(C.Structure):
     ]
 
 
+class Grid(C.Structure):
+    """nerfb200_grid_t: the box [lo, hi) and its cells per axis (the bit order is in include/nerfb200.h)"""
+
+    _fields_ = [
+        ("lo", C.c_float * 3),
+        ("hi", C.c_float * 3),
+        ("res", C.c_int32 * 3),
+    ]
+
+
 P = C.c_void_p
 I32, I64, F32, F64, U64 = C.c_int32, C.c_int64, C.c_float, C.c_double, C.c_uint64
-AP, OP, RP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng)
+AP, OP, RP, GP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng), C.POINTER(Grid)
 
 # name -> (restype, argtypes); mirrors include/nerfb200.h one-to-one
 SIGNATURES = {
@@ -104,6 +114,13 @@ SIGNATURES = {
     "nerfb200_lr_schedule": (I32, [P, I64, F64, F64, F64, P, P]),
     "nerfb200_adam_step_dev": (I32, [P, P, P, P, I64, P, F64, F64, F64, F32, F32, F32, F32, P]),
     "nerfb200_step_advance": (I32, [P, P]),
+    "nerfb200_grid_words": (I64, [GP]),
+    "nerfb200_grid_locate": (I32, [GP, C.POINTER(F32), I64, C.POINTER(I64)]),
+    "nerfb200_grid_max_blocks": (I64, [I64, I32]),
+    "nerfb200_grid_scratch_ints": (I64, [I64, I32]),
+    "nerfb200_grid_compact": (I32, [GP, P, P, I32, P, I64, I32, P, P, P, P, P, P, P]),
+    "nerfb200_render_grid_workspace_bytes": (I64, [AP, AP, OP, I64]),
+    "nerfb200_render_fwd_grid": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, P, P, P, I32, P, P]),
 }
 
 _lib = None

@@ -717,33 +717,71 @@ static int render_randoms(const char* what, const nerfb200_render_opts_t& o, con
 
 extern "C" {
 
-int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                            const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
-                            float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
-                            void* stream) {
+}  // extern "C"
+
+namespace nerfb200 {
+
+// The sections an occupancy-grid render adds after render_fwd's inference workspace, sized for the larger (fine) pass
+// and reused by both passes: the compaction scratch, the row map, its blocks and the live block count.
+struct GridWorkspace {
+  int64_t scratch, map, blocks, n_blocks, total;
+};
+static GridWorkspace carve_grid(int64_t base, int64_t n_rays, int n_samples) {
+  GridWorkspace g;
+  const int64_t mb = grid_max_blocks(n_rays, n_samples);
+  g.scratch = base;
+  g.map = g.scratch + align256(grid_scratch_ints(n_rays, n_samples) * 4);
+  g.blocks = g.map + align256(mb * 64 * 4);
+  g.n_blocks = g.blocks + align256(mb * 8);
+  g.total = g.n_blocks + 256;
+  return g;
+}
+
+// render_fwd, and with a grid (grid != NULL, inference only) the same passes with the MLP run over each pass's compacted
+// samples.  Without a grid the launches are exactly render_fwd's.
+static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                          const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                          const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                          const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                          const nerfb200_grid_t* grid, const uint32_t* bits, int64_t* n_evaluated, float* out_coarse,
+                          float* out_fine, void* workspace, int32_t training, int32_t impl, void* stream) {
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
   const float* const tensor[4] = {t_rand, noise_c, u, noise_f};
   RandSrc rnd[4];
-  NB_TRY(render_randoms("render_fwd", *opts, rng, tensor, rnd));
+  NB_TRY(render_randoms(what, *opts, rng, tensor, rnd));
   const bool fine = opts->n_fine > 0;
   if (fine) {
     if (!arch_f || !blob_f || !out_fine) {
-      set_error("render_fwd: fine pass requested but fine model / output missing");
+      set_error("%s: fine pass requested but fine model / output missing", what);
       return NERFB200_ERR_INVALID;
     }
     NB_TRY(build_plan(arch_f, &pf));
   }
   if (!rays || !out_coarse || !workspace || !blob_c || n_rays <= 0) {
-    set_error("render_fwd: null pointer or empty batch");
+    set_error("%s: null pointer or empty batch", what);
     return NERFB200_ERR_INVALID;
   }
   if (opts->perturb && (!rnd[kRandTRand].present() || (fine && !rnd[kRandU].present()))) {
-    set_error("render_fwd: perturb set but t_rand or u missing");
+    set_error("%s: perturb set but t_rand or u missing", what);
     return NERFB200_ERR_INVALID;
+  }
+  if (grid) {
+    NB_TRY(check_grid(grid, what));
+    if (!bits) {
+      set_error("%s: null grid bitfield", what);
+      return NERFB200_ERR_INVALID;
+    }
+    if (training || impl == 0) {
+      set_error("%s: the occupancy grid renders only (training = 0), on the wgmma inference forward: impl 1 or 3, not "
+                "impl=%d", what, impl);
+      return NERFB200_ERR_UNSUPPORTED;
+    }
+    if (grid_max_blocks(n_rays, opts->n_coarse + opts->n_fine) * 64 >= (int64_t(1) << 31)) {
+      set_error("%s: more than 2^31 map rows in one call; chunk the rays", what);
+      return NERFB200_ERR_UNSUPPORTED;
+    }
   }
   Workspace w;
   carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
@@ -753,11 +791,24 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const Need need = training ? kStash : kInference;
   NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
-  NB_TRY(check_impl(pc, impl, nc, need, "render_fwd"));
+  NB_TRY(check_impl(pc, impl, nc, need, what));
   if (fine) {
     NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
-    NB_TRY(check_impl(pf, impl, ns, need, "render_fwd"));
+    NB_TRY(check_impl(pf, impl, ns, need, what));
   }
+  const GridWorkspace gw = carve_grid(w.total, n_rays, fine ? ns : nc);
+  // the MLP of one pass: every sample, or with a grid the compacted samples (skipped ones get raw = [0 0 0 -inf])
+  auto mlp = [&](bool is_fine, const Plan& p, const float* blob, int n, const float* z, float* raw, float* stash) {
+    if (!grid)
+      return mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, training ? stash : nullptr, s);
+    int* nb = reinterpret_cast<int*>(base + gw.n_blocks);
+    NB_TRY(launch_grid_compact(*grid, bits, rays, ray_stride, z, n_rays, n, raw, reinterpret_cast<int*>(base + gw.map),
+                               reinterpret_cast<int*>(base + gw.blocks), nb, n_evaluated ? n_evaluated + is_fine : nullptr,
+                               reinterpret_cast<int*>(base + gw.scratch), s));
+    const RowMap m{reinterpret_cast<const int*>(base + gw.map), reinterpret_cast<const int2*>(base + gw.blocks), nb};
+    return launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, grid_max_blocks(n_rays, n), raw, impl == 3,
+                                 s);
+  };
 
   // one pass: depths -> MLP -> compositing.  The coarse pass (train_utils.py:45-94) takes stratified depths, the fine
   // pass (:96-125) resamples the coarse weights' pdf and merges the two sets.
@@ -768,13 +819,55 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                                      nullptr, nullptr, s));
     else
       NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, z, s));
-    NB_TRY(mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, training ? stash : nullptr, s));
+    NB_TRY(mlp(is_fine, p, blob, n, z, raw, stash));
     return launch_composite_fwd(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
                                 opts->noise_std, opts->white_bkgd, out, weights, s);
   };
   NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse, F(w.w_c)));
   if (!fine) return NERFB200_OK;
   return pass(true, pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), out_fine, nullptr);
+}
+
+}  // namespace nerfb200
+
+extern "C" {
+
+int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                            const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                            const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                            const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                            float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
+                            void* stream) {
+  return render_forward("render_fwd", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand,
+                        noise_c, u, noise_f, nullptr, nullptr, nullptr, out_coarse, out_fine, workspace, training, impl,
+                        stream);
+}
+
+int64_t nerfb200_render_grid_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                             const nerfb200_render_opts_t* opts, int64_t n_rays) {
+  Plan pc, pf;
+  if (build_plan(coarse, &pc) != NERFB200_OK) return -1;
+  if (fine && build_plan(fine, &pf) != NERFB200_OK) return -1;
+  if (check_opts(opts) != NERFB200_OK || n_rays <= 0) return -1;
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
+  const bool has_fine = fine && opts->n_fine > 0;
+  return carve_grid(w.total, n_rays, has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse).total;
+}
+
+int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                 const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                 const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                 const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                 const nerfb200_grid_t* grid, const uint32_t* bits, float* out_coarse, float* out_fine,
+                                 void* workspace, int32_t impl, int64_t* n_evaluated, void* stream) {
+  if (!grid) {
+    set_error("render_fwd_grid: null grid descriptor");
+    return NERFB200_ERR_INVALID;
+  }
+  return render_forward("render_fwd_grid", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand,
+                        noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace, /*training=*/0,
+                        impl, stream);
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,

@@ -205,6 +205,27 @@ int launch_mlp_bwd_tc(const Plan& p, const float* blob, const float* dirs, int d
                       const float* d_raw, const float* stash, float* scratch, float* flat_grad, cudaStream_t s);
 int64_t bwd_tc_scratch_floats(const Plan& p);
 
+// ---- occupancy grid (occupancy.cu; nerfb200.h "occupancy grid") ----
+// The rows the wgmma forward runs when a grid decides which samples are evaluated: map[row] = point (-1: padding), in
+// 64-row blocks; blocks[b] = (first ray, last ray) of block b; *n_blocks blocks, read by the kernel from device memory.
+constexpr int kGridGroupRays = 10;  // rays per compaction group: at most this many per 64-row block (tc kMaxRaysPerTile)
+struct RowMap {
+  const int* map;
+  const int2* blocks;
+  const int* n_blocks;
+};
+int64_t grid_max_blocks(int64_t n_rays, int n_samples);
+int64_t grid_scratch_ints(int64_t n_rays, int n_samples);
+int check_grid(const nerfb200_grid_t* g, const char* what);
+int launch_grid_compact(const nerfb200_grid_t& g, const uint32_t* bits, const float* rays, int ray_stride, const float* z,
+                        int64_t n_rays, int n_samples, float* raw, int* map, int* blocks, int* n_blocks,
+                        int64_t* n_evaluated, int* scratch, cudaStream_t s);
+// the wgmma inference forward (impl 1, or fast: impl 3) over a RowMap of the points o + d z of the ray rows; max_blocks
+// bounds *n_blocks (the grid size is chosen on the host)
+int launch_mlp_fwd_tc_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                          int64_t n_rays, int n_samples, const RowMap& m, int64_t max_blocks, float* raw, bool fast,
+                          cudaStream_t s);
+
 // ---------------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------------

@@ -245,13 +245,18 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
 // kFast: the single-pass fp16 products (inference only, see the file header)
 // kPts: the points come from pts[P][3] and the view directions from (dirs, dir_stride) instead of o + d z and the ray
 // rows' columns 8..10 (a template parameter, so that the render path's instances compile as they did without it)
-template <bool kTrain, int kH, bool kFast, bool kPts>
+// kMap: inference over an occupancy grid's row map (occupancy.cu): tile rows are map rows, row -> point through map[],
+// each 64-row block's rays from blocks[], and the tile count from *n_blocks in device memory.  Every row is computed as
+// the default instance computes its point, so an evaluated point's raw has the same bits.
+template <bool kTrain, int kH, bool kFast, bool kPts, bool kMap>
 __global__ void __launch_bounds__(128 * (kH == 128 ? 2 : 1) + 32, 1)
 mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ z, int64_t P, int S, int64_t n_tiles,
                   float* __restrict__ raw,          // out [P][4]
                   float* __restrict__ stash,        // out (kTrain)
-                  const float* __restrict__ pts, const float* __restrict__ dirs, int dir_stride) {  // kPts
+                  const float* __restrict__ pts, const float* __restrict__ dirs, int dir_stride,  // kPts
+                  const int* __restrict__ map, const int2* __restrict__ blocks, const int* __restrict__ n_blocks) {  // kMap
+  static_assert(!(kMap && (kTrain || kPts)), "the row map is an inference path of the render points");
   constexpr int kWG = kH == 128 ? 2 : 1, kRows = 64 * kWG, kThreads = 128 * kWG + 32;
   uint8_t* sm = smem_base();
   const SmemMap mp = smem_map(p);
@@ -289,6 +294,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   }
   __syncthreads();
 
+  if constexpr (kMap) n_tiles = ((int64_t)*n_blocks + kWG - 1) / kWG;
   const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
 
   if (warp == 4 * kWG) {
@@ -321,18 +327,35 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll 1
     for (int j = 0; j < my_tiles; ++j) {
       const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
-      const int64_t p0 = tile * kRows + 64 * wg;   // first point of this warpgroup
-      const TileRays tr = tile_rays(p0, 64, P, S);
+      const int64_t p0 = tile * kRows + 64 * wg;   // first point (kMap: first map row) of this warpgroup
+      TileRays tr;
+      RowState rs;
+      bool block_live = true;                      // kMap: this warpgroup's 64-row block exists
+      if constexpr (kMap) {
+        block_live = (p0 >> 6) < *n_blocks;        // an odd block count leaves the last tile's second half empty
+        const int2 b = block_live ? blocks[p0 >> 6] : make_int2(0, 0);
+        tr.first = b.x;
+        tr.n = b.y - b.x + 1;
+        rs = map_row_state(map, p0, 16 * (wt >> 5) + ((tid & 31) >> 2), block_live, S, tr.first);
+      } else {
+        tr = tile_rays(p0, 64, P, S);
+        rs = row_state(p0, 16 * (wt >> 5) + ((tid & 31) >> 2), P, S, tr.first);
+      }
       const int64_t first_ray = tr.first;
       const int n_rays_wg = tr.n;
-      const RowState rs = row_state(p0, 16 * (wt >> 5) + ((tid & 31) >> 2), P, S, first_ray);
       // ================= encodings of this row -> operand tile (value / 16), the two halves split the frequencies
       if (kTrain) {  // the previous tile's encoding store must have finished reading the tile
         if (wt == 0) bulk_wait_read();
         wg_bar();
       }
       {
-        const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
+        int64_t pt;
+        if constexpr (kMap) {  // a padding row encodes the block's first ray's first point; its raw is never written
+          const int m = block_live ? map[p0 + row] : -1;
+          pt = m >= 0 ? m : first_ray * S;
+        } else {
+          pt = (p0 + row < P) ? p0 + row : P - 1;
+        }
         const int64_t ray = (int64_t)((uint32_t)pt / (uint32_t)S);
         const float* rr = rays + ray * ray_stride;
         const float zz = kPts ? 0.f : z[pt];
@@ -432,9 +455,35 @@ static int launch_fwd(const Plan& p, const float* blob, const PointSrc& src, int
   constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
   const int64_t tiles = (P + kRows - 1) / kRows;
   const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // = tiles whenever the stash is written (hidden 128)
-  auto kern = src.pts ? mlp_fwd_tc_kernel<kTrain, kH, kFast, true> : mlp_fwd_tc_kernel<kTrain, kH, kFast, false>;
+  auto kern = src.pts ? mlp_fwd_tc_kernel<kTrain, kH, kFast, true, false>
+                      : mlp_fwd_tc_kernel<kTrain, kH, kFast, false, false>;
   return launch_persistent(kern, tiles, kThreads, smem_map(p).total, s, what, p, blob, src.rays, src.ray_stride, src.z, P,
-                           n_samples, kTrain ? stash_tiles : tiles, raw, stash, src.pts, src.dirs, src.dir_stride);
+                           n_samples, kTrain ? stash_tiles : tiles, raw, stash, src.pts, src.dirs, src.dir_stride,
+                           (const int*)nullptr, (const int2*)nullptr, (const int*)nullptr);
+}
+
+// over a row map: the grid covers max_blocks blocks; the kernel reads the live count from m.n_blocks
+template <int kH, bool kFast>
+static int launch_fwd_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                          int64_t P, int n_samples, const RowMap& m, int64_t max_blocks, float* raw, cudaStream_t s,
+                          const char* what) {
+  constexpr int kWG = kH == 128 ? 2 : 1, kThreads = 128 * kWG + 32;
+  const int64_t tiles = (max_blocks + kWG - 1) / kWG;
+  return launch_persistent(mlp_fwd_tc_kernel<false, kH, kFast, false, true>, tiles, kThreads, smem_map(p).total, s, what,
+                           p, blob, rays, ray_stride, z, P, n_samples, tiles, raw, (float*)nullptr,
+                           (const float*)nullptr, rays + 8, ray_stride, m.map, m.blocks, m.n_blocks);
+}
+
+int launch_mlp_fwd_tc_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
+                          int64_t n_rays, int n_samples, const RowMap& m, int64_t max_blocks, float* raw, bool fast,
+                          cudaStream_t s) {
+  const int64_t P = n_rays * n_samples;
+  auto go = [&](auto launch, const char* what) {
+    return launch(p, blob, rays, ray_stride, z, P, n_samples, m, max_blocks, raw, s, what);
+  };
+  if (fast)
+    return go(p.hidden == 256 ? launch_fwd_map<256, true> : launch_fwd_map<128, true>, "mlp_fwd_tc_fast grid launch");
+  return go(p.hidden == 256 ? launch_fwd_map<256, false> : launch_fwd_map<128, false>, "mlp_fwd_tc grid launch");
 }
 
 // stash non-null: the training forward; fast: the single-pass forward (never with a stash)

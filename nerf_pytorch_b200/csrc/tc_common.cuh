@@ -206,6 +206,20 @@ __device__ __forceinline__ RowState row_state(int64_t p0, int r0, int64_t P, int
   }
   return rs;
 }
+// the same over an occupancy grid's row map (occupancy.cu): rows p0 + r0 (+ 8) of the map; a padding row, or any row of a
+// block past the last (live = false), is invalid and stands in for the block's first ray's first point
+__device__ __forceinline__ RowState map_row_state(const int* __restrict__ map, int64_t p0, int r0, bool live, int S,
+                                                  int64_t first_ray) {
+  RowState rs;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int m = live ? map[p0 + r0 + 8 * i] : -1;
+    rs.valid[i] = m >= 0;
+    rs.pt[i] = m >= 0 ? m : (int)(first_ray * S);
+    rs.ray_slot[i] = (int)((uint32_t)rs.pt[i] / (uint32_t)S - first_ray);
+  }
+  return rs;
+}
 
 // Weight ring: n_stages stages of kStage bytes from `base`, filled by one producer thread with bulk copies from the
 // L2-resident blob and read by the consumer warpgroups' MMAs.  full[i] (bars + 8 i, one producer arrival + the bytes):

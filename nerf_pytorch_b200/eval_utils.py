@@ -17,7 +17,7 @@ from .ops import SeededRandoms
 
 def render_image(height, width, focal_length, tform_cam2world, model_coarse, model_fine, options, mode="validation",
                  encode_position_fn=None, encode_direction_fn=None, *, rays_per_chunk: Optional[int] = None,
-                 device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None):
+                 device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None, grid=None):
     """One pose -> (rgb_coarse (H,W,3), disp_coarse (H,W), acc_coarse (H,W), rgb_fine, disp_fine, acc_fine).
 
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
@@ -29,12 +29,19 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
     ray ``ray_offset + j * width + i`` of the seeded stream whatever the chunk size.  Default: torch draws per chunk.
 
     ``impl=ops.IMPL_TC_FAST`` renders with the single-pass fp16 wgmma forward (INTEGRATION.md, "Optional fast paths"):
-    fewer MMAs, fp16 operands, judged by PSNR against the default path rather than by parity with it."""
+    fewer MMAs, fp16 operands, judged by PSNR against the default path rather than by parity with it.
+
+    ``grid``: an ``OccupancyGrid`` (INTEGRATION.md, "Optional fast paths"): samples in its empty cells skip the MLP and
+    get zero density; impl 1 or 3 only.  Every other sample, and so every ray none of whose skipped samples had density,
+    is computed bit for bit as without the grid."""
     if randoms is not None and not isinstance(randoms, SeededRandoms):
         raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:
         device = next(model_coarse.parameters()).device
     use_viewdirs = bool(options.nerf.use_viewdirs)
+    if grid is not None:
+        with torch.no_grad():
+            train_utils.check_grid_call(grid, device, model_coarse, model_fine)
     with torch.no_grad():
         rays = ops.gen_rays(tform_cam2world, height, width, focal_length, None, device,
                             ndc=options.dataset.no_ndc is False, near=options.dataset.near, far=options.dataset.far,
@@ -45,7 +52,7 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
         parts = [train_utils.predict_and_render_radiance(
             rays[i:i + chunk], model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
-            encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl,
+            encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl, grid=grid,
             randoms=randoms.shifted(i) if randoms is not None else None)
             for i in range(0, n, chunk)]
     cols = [torch.cat(c, 0) if c[0] is not None else None for c in zip(*parts)]

@@ -12,7 +12,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import Arch, RenderOpts, Rng
+from ._lib import Arch, Grid, RenderOpts, Rng
 
 IMPL_SIMT = 0  # fp32 CUDA cores
 IMPL_TC = 1    # wgmma tensor cores (fp16x2 three-term splits, fp32 accumulation)
@@ -273,6 +273,14 @@ def mlp_fwd(arch: ArchSpec, blob, rays, z, impl=IMPL_SIMT, want_stash=False):
 def impl_supported(arch: ArchSpec, n_samples: int, impl: int) -> bool:
     """Can `impl` run this architecture forward and backward (the library decides, not Python)?"""
     return _lib.load().nerfb200_impl_supported(C.byref(arch.c_struct()), int(n_samples), int(impl)) == _lib.OK
+
+
+def impl_refusal(arch: ArchSpec, n_samples: int, impl: int) -> Optional[str]:
+    """None when ``impl_supported(arch, n_samples, impl)``, else the library's reason."""
+    lib = _lib.load()
+    if lib.nerfb200_impl_supported(C.byref(arch.c_struct()), int(n_samples), int(impl)) == _lib.OK:
+        return None
+    return lib.nerfb200_last_error().decode(errors="replace")
 
 
 def mlp_bwd(arch: ArchSpec, blob, rays, z, d_raw, stash, impl=IMPL_SIMT, flat_grad=None):
@@ -602,3 +610,105 @@ def render_bwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, 
                                        rays.shape[0], rng, noise_c, noise_f, _ptr(g_c), _ptr(g_f) if fine else None,
                                        _ptr(workspace), _ptr(flat_grad_c), _ptr(flat_grad_f) if fine else None, impl,
                                        int(parts), _stream()), "render_bwd")
+
+
+# ------------------------------------------------------------------------------------------------
+# occupancy grid (include/nerfb200.h "occupancy grid"; nerf_pytorch_b200/occupancy.py builds the grids)
+# ------------------------------------------------------------------------------------------------
+def grid_struct(bounds, resolution) -> Grid:
+    """nerfb200_grid_t of ``bounds`` ((lo_x, lo_y, lo_z), (hi_x, hi_y, hi_z)) and ``resolution`` (three ints)."""
+    g = Grid()
+    (lo, hi), res = bounds, resolution
+    for c in range(3):
+        g.lo[c], g.hi[c], g.res[c] = float(lo[c]), float(hi[c]), int(res[c])
+    return g
+
+
+def grid_words(g: Grid) -> int:
+    n = _lib.load().nerfb200_grid_words(C.byref(g))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, "grid_words")
+    return int(n)
+
+
+def grid_locate(g: Grid, xyz: torch.Tensor) -> torch.Tensor:
+    """The library's host restatement of the cell rule: int64 cell index of each (n, 3) CPU point, -1 outside."""
+    x = xyz.detach().to(device="cpu", dtype=torch.float32).contiguous()
+    out = torch.empty(x.shape[0], dtype=torch.int64)
+    _lib.check(_lib.load().nerfb200_grid_locate(C.byref(g), C.cast(x.data_ptr(), C.POINTER(C.c_float)), x.shape[0],
+                                                C.cast(out.data_ptr(), C.POINTER(C.c_int64))), "grid_locate")
+    return out
+
+
+def _grid_args(grid):
+    """(descriptor, bits) of an OccupancyGrid-like object: ``.c_struct()`` and ``.bits`` (int32 words on the device)."""
+    bits = grid.bits
+    if not bits.is_cuda or bits.dtype != torch.int32 or bits.dim() != 1 or not bits.is_contiguous():
+        raise RuntimeError("nerfb200: the grid's bits must be a contiguous 1-d int32 CUDA tensor")
+    g = grid.c_struct()
+    if bits.numel() != grid_words(g):
+        raise RuntimeError(f"nerfb200: the grid's bits hold {bits.numel()} words, its resolution needs {grid_words(g)}")
+    return g, bits
+
+
+def grid_compact(grid, rays, z, raw=None):
+    """Sample compaction of one pass (nerfb200_grid_compact): writes [0 0 0 -inf] into ``raw`` (n, s, 4) at every
+    skipped sample and returns (raw, map int32[rows], blocks int32[max_blocks, 2], n_blocks int32[1],
+    n_evaluated int64[1]); rows past 64 * n_blocks are not written."""
+    lib = _lib.load()
+    g, bits = _grid_args(grid)
+    n, s = z.shape
+    dev = z.device
+    if raw is None:
+        raw = torch.zeros(n, s, 4, dtype=torch.float32, device=dev)
+    mb = lib.nerfb200_grid_max_blocks(n, s)
+    if mb < 0:
+        _lib.check(_lib.ERR_INVALID, "grid_max_blocks")
+    m = torch.full((mb * 64,), -2, dtype=torch.int32, device=dev)
+    blocks = torch.full((mb, 2), -2, dtype=torch.int32, device=dev)
+    nb = torch.empty(1, dtype=torch.int32, device=dev)
+    ne = torch.empty(1, dtype=torch.int64, device=dev)
+    scratch = torch.empty(lib.nerfb200_grid_scratch_ints(n, s), dtype=torch.int32, device=dev)
+    _lib.check(lib.nerfb200_grid_compact(C.byref(g), _ptr(bits), _ptr(rays), rays.shape[1], _ptr(z), n, s, _ptr(raw),
+                                         _ptr(m), _ptr(blocks), _ptr(nb), _ptr(ne), _ptr(scratch), _stream()),
+               "grid_compact")
+    return raw, m, blocks, nb, ne
+
+
+def render_grid_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int) -> int:
+    lib = _lib.load()
+    af = arch_f.c_struct() if arch_f is not None else None
+    n = lib.nerfb200_render_grid_workspace_bytes(C.byref(arch_c.c_struct()), C.byref(af) if af is not None else None,
+                                                 C.byref(opts), n_rays)
+    if n < 0:
+        _lib.check(_lib.ERR_UNSUPPORTED, "render_grid_workspace_bytes")
+    return n
+
+
+def render_fwd_grid(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid, impl: int = IMPL_TC,
+                    workspace: Optional[torch.Tensor] = None, n_evaluated: Optional[torch.Tensor] = None):
+    """``render_fwd`` for inference with an occupancy grid (impl 1 or 3).  ``n_evaluated``: an int64 CUDA tensor of 2
+    receiving the evaluated samples of the coarse and fine pass, or None.  Returns (out_coarse, out_fine | None,
+    workspace); the workspace's first sections are laid out as ``render_workspace_layout(..., training=False)``."""
+    lib = _lib.load()
+    n = rays.shape[0]
+    dev = rays.device
+    fine = opts.n_fine > 0
+    g, bits = _grid_args(grid)
+    if bits.device != dev:
+        raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
+    if n_evaluated is not None and (n_evaluated.dtype != torch.int64 or n_evaluated.numel() < 2):
+        raise RuntimeError("nerfb200: n_evaluated must be an int64 tensor of 2 elements")
+    need = render_grid_workspace_bytes(arch_c, arch_f if fine else None, opts, n)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
+    ac = arch_c.c_struct()
+    af = arch_f.c_struct() if fine else None
+    _lib.check(lib.nerfb200_render_fwd_grid(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
+                                            _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
+                                            *_random_args(randoms), C.byref(g), _ptr(bits), _ptr(out_c), _ptr(out_f),
+                                            _ptr(workspace), int(impl), _ptr(n_evaluated), _stream()),
+               "render_fwd_grid")
+    return out_c, out_f, workspace

@@ -376,6 +376,44 @@ def run_network(network_fn, pts, ray_batch, chunksize, embed_fn, embeddirs_fn, *
 
 
 
+def check_grid_call(grid, device, *models):
+    """The refusals of an occupancy-grid render that precede any launch: not an OccupancyGrid, a call that would train,
+    a grid on another device than ``device`` (None: not known yet) or whose bits are not the int32 words its resolution
+    needs."""
+    from .occupancy import OccupancyGrid
+
+    if not isinstance(grid, OccupancyGrid):
+        raise TypeError(f"nerfb200: grid must be an OccupancyGrid, got {type(grid).__name__}")
+    if _trains(p for m in models if m is not None for p in m.parameters()):
+        raise NotImplementedError("nerfb200: an occupancy grid renders only (inference); render under torch.no_grad() "
+                                  "or with parameters that do not require grad")
+    bits = grid.bits
+    if device is not None and bits.device != torch.device(device):
+        raise RuntimeError(f"nerfb200: the occupancy grid is on {bits.device}, the rays on {device}")
+    want = ops.grid_words(grid.c_struct())
+    if bits.dtype != torch.int32 or bits.dim() != 1 or bits.numel() != want or not bits.is_contiguous():
+        raise RuntimeError(f"nerfb200: the occupancy grid's bits must be contiguous int32[{want}], got {bits.dtype}"
+                           f"{list(bits.shape)}")
+
+
+def _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine):
+    """The impl an occupancy-grid render runs on, after every refusal that precedes a launch: those of check_grid_call,
+    impl 0, and an architecture the wgmma inference forward refuses (the library's reason)."""
+    check_grid_call(grid, rays.device, model_coarse, model_fine)
+    if impl is None:
+        impl = _auto_impl(arch_c, arch_f, nc, nf, training=False)
+    if impl == ops.IMPL_SIMT:
+        raise NotImplementedError("nerfb200: an occupancy grid runs on the wgmma inference forward (impl 1 or 3), not "
+                                  "impl 0 (fp32 CUDA cores)" + "".join(
+                                      f"; {why}" for a, n in ((arch_c, nc), (arch_f, nc + nf)) if a is not None
+                                      for why in [ops.impl_refusal(a, n, ops.IMPL_TC_FWD)] if why))
+    for a, n in ((arch_c, nc), (arch_f, nc + nf)):
+        why = ops.impl_refusal(a, n, ops.IMPL_TC_FWD if impl == ops.IMPL_TC else impl) if a is not None else None
+        if why:
+            raise NotImplementedError(f"nerfb200 grid render: {why}")
+    return impl
+
+
 def predict_and_render_radiance(
     ray_batch,
     model_coarse,
@@ -387,6 +425,7 @@ def predict_and_render_radiance(
     *,
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
+    grid=None,
     _n_chunks: int = 1,
 ):
     """nerf/train_utils.py:28-127 for one chunk of packed rays ``[o d near far (viewdir)]``.
@@ -397,8 +436,13 @@ def predict_and_render_radiance(
     ``ray_offset`` (the global index of ``ray_batch[0]``): no torch random number is drawn.
 
     ``impl``: None picks the kernels (``DEFAULT_IMPL``, else the automatic choice); ``ops.IMPL_TC_FAST`` renders with
-    the single-pass fp16 forward and raises ``NotImplementedError`` if the call would train."""
+    the single-pass fp16 forward and raises ``NotImplementedError`` if the call would train.
+
+    ``grid``: an ``OccupancyGrid`` on the rays' device (inference only, impl 1 or 3): samples in its empty cells skip
+    the MLP and get zero density.  None is the path without a grid."""
     impl = _requested_impl(impl, model_coarse, model_fine)
+    if grid is not None:
+        check_grid_call(grid, None, model_coarse, model_fine)
     o = getattr(options.nerf, mode)
     if not ray_batch.is_cuda:
         raise NotImplementedError("nerfb200: rays must be on a CUDA device (there is no CPU path)")
@@ -414,6 +458,8 @@ def predict_and_render_radiance(
     if fine and not model_fine:
         raise RuntimeError("nerfb200: num_fine > 0 but model_fine is None (the reference fails here as well)")
     arch_f = _arch_of(model_fine, enc_xyz, enc_dir) if fine else None
+    if grid is not None:
+        impl = _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine)
     params_c, blob_c = _packed(model_coarse, arch_c)
     params_f, blob_f = _packed(model_fine, arch_f) if fine else ([], None)
     noise_std = float(o.radiance_field_noise_std)
@@ -446,8 +492,11 @@ def predict_and_render_radiance(
     training = _trains(all_params)
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, impl, int(_n_chunks))
-    out_c, out_f = _RenderChunk.apply(cfg, rays, rnd, *all_params)
+    if grid is not None:
+        out_c, out_f, _ = ops.render_fwd_grid(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid, impl=impl)
+    else:
+        cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, impl, int(_n_chunks))
+        out_c, out_f = _RenderChunk.apply(cfg, rays, rnd, *all_params)
     rgb_c, disp_c, acc_c = out_c[:, :3], out_c[:, 3], out_c[:, 4]
     if out_f is None:
         return rgb_c, disp_c, acc_c, None, None, None
@@ -469,11 +518,14 @@ def run_one_iter_of_nerf(
     *,
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
+    grid=None,
 ):
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
     the reshape back to image shape."""
     impl = _requested_impl(impl, model_coarse, model_fine)
+    if grid is not None:
+        check_grid_call(grid, ray_directions.device, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     restore_shapes = [ray_directions.shape, ray_directions.shape[:-1], ray_directions.shape[:-1]]
     if model_fine:
@@ -487,7 +539,7 @@ def run_one_iter_of_nerf(
                          options.dataset.far, use_viewdirs)
 
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl)
+                          encode_direction_fn, randoms, impl, grid)
 
 
 def run_one_iter_of_nerf_from_pose(
@@ -505,6 +557,7 @@ def run_one_iter_of_nerf_from_pose(
     *,
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
+    grid=None,
 ):
     """``run_one_iter_of_nerf`` for callers that hold a pose and pixel ids instead of ray tensors (SURVEY.md section 8f-2):
     the reference's training loop builds ALL H*W rays of the image with get_ray_bundle and then indexes the few
@@ -513,17 +566,19 @@ def run_one_iter_of_nerf_from_pose(
     target device (None = the whole image, returned image-shaped in "validation" mode)."""
     impl = _requested_impl(impl, model_coarse, model_fine)
     dev = pixel_ids.device if pixel_ids is not None else next(model_coarse.parameters()).device
+    if grid is not None:
+        check_grid_call(grid, dev, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     rays = ops.gen_rays(tform_cam2world, height, width, focal_length, pixel_ids, dev, ndc=options.dataset.no_ndc is False,
                         near=options.dataset.near, far=options.dataset.far, use_viewdirs=use_viewdirs)
     lead = (height, width) if pixel_ids is None else tuple(pixel_ids.shape)
     restore_shapes = [lead + (3,), lead, lead] * (2 if model_fine else 1)
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl)
+                          encode_direction_fn, randoms, impl, grid)
 
 
 def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn, encode_direction_fn,
-                   randoms, impl):
+                   randoms, impl, grid=None):
     """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202.
     Seeded randoms follow each ray: chunk i starts at ``ray_offset`` + the index of its first ray."""
     chunksize = getattr(options.nerf, mode).chunksize
@@ -537,7 +592,8 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             batch, model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if options.nerf.use_viewdirs else None,
-            randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, _n_chunks=len(batches),
+            randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, grid=grid,
+            _n_chunks=len(batches),
         )
         for i, batch in enumerate(batches)
     ]
