@@ -8,8 +8,11 @@
 // fp32 accumulator.  The A operand holds activation / 16 (fp16 range 65504 -> 1.05e6: the shipped lego checkpoints
 // reach 6e4); conversions do not saturate, an out-of-range value turns the output into inf / NaN instead of clamping.
 //
-// Persistent kernel, one CTA per SM.  A tile is 64 points per consumer warpgroup: two warpgroups (128 points) for
+// Persistent kernel, one CTA per SM.  A tile is 64 points per consumer warpgroup: three warpgroups (192 points) for
 // hidden 128, one (64 points) for hidden 256, whose 64 x 256 fp32 accumulator takes half of a thread's registers.
+// Three warpgroups and the producer warp put four warps on one of the SM's schedulers, whose quarter of the register
+// file then allows 128 registers per thread.  The stash keeps 128-point tiles (the fused backward's operand tiles): the
+// 64-row block b of a batch is half b & 1 of stash tile b >> 1, whichever CTA tile b / 3 computes it.
 //   consumer warpgroups  per tile: positional encodings of its 64 rows -> fp16 operand tile (shared memory); per layer:
 //              wgmma over the ring's weight stages (A = the warpgroup's rows of the activation or encoding tile, B =
 //              the weight copies), then the epilogue on the accumulator registers: bias at the accumulator's 2^11
@@ -17,10 +20,12 @@
 //              into fp16 hi + lo (mixed-precision FMA, tc_common.cuh split_f16x2_y) -> the activation tile in shared
 //              memory, the next layer's A operand.  Training: the same hi / lo registers also go to the activation
 //              stash as an operand tile (tc_common.cuh "Operand tiles"), plus one ReLU bit per activation.
-//              The two warpgroups run independently; each one's epilogue overlaps the other's MMAs.
-//   last warp  weight producer: fills the weight ring (tc_common.cuh WeightRing) with one cp.async.bulk per 24 KB
-//              stage from the L2-resident blob, mbarrier complete_tx; a stage is free again once every consumer warp
-//              has seen its MMAs complete.
+//              The warpgroups run independently on the same weight stages; each one's epilogue overlaps the others'
+//              MMAs.
+//   last warp  weight producer: fills the weight ring (tc_common.cuh WeightRing) with one cp.async.bulk per stage
+//              (12 KB, one N = 128 k-step, at hidden 128: the 192-row tiles leave the ring 48 KB, four stages; 24 KB
+//              at hidden 256) from the L2-resident blob, mbarrier complete_tx; a stage is free again once every
+//              consumer warp has seen its MMAs complete.
 // The direction encoding enters layers_dir[0] through a per-ray fp32 bias computed on the CUDA cores (it is constant
 // along a ray: SURVEY.md section 7.3 item 5), so that layer contracts over K = H only.
 //
@@ -28,7 +33,7 @@
 // copy the blob already holds, so the accumulator sits at the same 2^11 scale and bias, ReLU, heads and the per-ray
 // view bias are unchanged.  Products are fp16(activation / 16) * fp16(w) with fp32 accumulation (~11 significant bits
 // per operand instead of 22); the heads and the direction term stay fp32.  The producer streams only the hs part of
-// each k-step (32 n bytes, contiguous in the blob) and packs kStageBytes / (32 n) k-steps into a ring stage; the
+// each k-step (32 n bytes, contiguous in the blob) and packs stage bytes / (32 n) k-steps into a ring stage; the
 // prologue and the epilogue write only the hi half of the operand tiles.
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -36,10 +41,20 @@
 namespace nerfb200 {
 
 namespace tc {
-constexpr int kStepsPerStage = 2;                       // k-steps per ring stage at N <= 128
+// consumer warpgroups at hidden 128 (-DNERFB200_FWD_WG=2 builds the two-warpgroup shape, for timing one against the other)
+#ifndef NERFB200_FWD_WG
+#define NERFB200_FWD_WG 3
+#endif
+constexpr int kFwdWG128 = NERFB200_FWD_WG;
+static_assert(kFwdWG128 == 2 || kFwdWG128 == 3, "hidden 128 runs two or three consumer warpgroups");
+
+constexpr int kStepsPerStage = 2;                       // k-steps per ring stage at most (split products)
 constexpr int kStageBytes = kStepsPerStage * 96 * 128;  // 24 KB: 3 copies x 2 slabs x 128 rows x 16 B per k-step
 
-__host__ __device__ inline int n_wg(int hidden) { return hidden == 128 ? 2 : 1; }  // consumer warpgroups = tile / 64
+__host__ __device__ constexpr int n_wg(int hidden) { return hidden == 128 ? kFwdWG128 : 1; }  // consumer warpgroups = tile / 64
+// bytes of a ring stage: 24 KB, or 12 KB (one N = 128 k-step) beside the 192-row tiles of three warpgroups, which leave
+// the ring 48 KB: four shallow stages keep more copies in flight than two deep ones
+__host__ __device__ constexpr int stage_bytes(int hidden) { return n_wg(hidden) == 3 ? kStageBytes / 2 : kStageBytes; }
 
 // Shared memory map (bytes from the 1 KB-aligned base), computed identically on host and device.
 struct SmemMap {
@@ -58,8 +73,8 @@ __host__ __device__ inline SmemMap smem_map(const Plan& p) {
   m.wv = off;        off += 32 * (p.hidden / 2) * 4;  // direction-encoding rows of layers_dir[0]'s weight: Wt[k_h + k][n]
   m.bars = off;      off += 256;
   m.ring = (off + 1023) & ~1023;
-  m.n_stages = ring_depth(m.ring, kStageBytes);
-  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * kStageBytes;
+  m.n_stages = ring_depth(m.ring, stage_bytes(p.hidden));
+  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * stage_bytes(p.hidden);
   return m;
 }
 
@@ -68,40 +83,44 @@ struct MmaInfo {
   const uint8_t* src;   // blob copy of the layer's weights (three fp16 copies, k-step major)
   uint32_t kbytes;      // bytes of one k-step
   int ksteps, ksteps_h; // k-steps, of which the first ksteps_h read the activation tile (the rest: encodings)
-  int sps;              // k-steps per ring stage (a stage holds 24 KB: two k-steps at N <= 128, one at N = 256;
-                        // single-pass: fast_sps(n) hs parts)
+  int sps;              // k-steps per ring stage (split_sps, single pass: fast_sps)
 };
-// single pass: k-steps per ring stage, each the 32 n bytes of its hs copy (12 at N = 64, 6 at 128, 3 at 256)
-__host__ __device__ constexpr int fast_sps(int n) { return kStageBytes / (32 * n); }
-__device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, int e, bool fast) {
+// split products: k-steps of 96 n bytes per ring stage, two if they fit and one otherwise (24 KB: two at N <= 128, one
+// at N = 256; 12 KB: two at N = 64, one at N = 128)
+__host__ __device__ constexpr int split_sps(int stage, int n) { return n > stage / (96 * kStepsPerStage) ? 1 : kStepsPerStage; }
+// single pass: k-steps per ring stage, each the 32 n bytes of its hs copy (24 KB: 12 at N = 64, 6 at 128, 3 at 256)
+__host__ __device__ constexpr int fast_sps(int stage, int n) { return stage / (32 * n); }
+__device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, int e, bool fast, int stage) {
   MmaInfo mi;
   const GemmLayer& g = p.g[e];
   mi.src = reinterpret_cast<const uint8_t*>(blob + g.tc_off);
   mi.ksteps = (g.k_tc + 15) >> 4;
   mi.ksteps_h = g.k_h >> 4;
   mi.kbytes = 96u * (uint32_t)g.n;
-  mi.sps = fast ? fast_sps(g.n) : g.n > 128 ? 1 : kStepsPerStage;
+  mi.sps = fast ? fast_sps(stage, g.n) : split_sps(stage, g.n);
   return mi;
 }
 
 }  // namespace tc
 
 using namespace tc;
-using Ring = WeightRing<kStageBytes>;
 
 // One layer of one warpgroup: MMAs over the ring, then the epilogue on the accumulator fragment.
 // Fragment of wgmma m64nN (per warp 16 rows): thread (warp wi, lane) holds rows r = 16 wi + lane / 4 (+ 8) and columns
 // 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row r + 8 i, column 8 j + 2 (lane % 4) + c).
-template <bool kTrain, bool kFast, int N>
+// kStage: bytes of a ring stage.  blk (kTrain): the warpgroup's 64-row block of the batch, whose rows are half blk & 1 of
+// stash tile blk >> 1.
+template <bool kTrain, bool kFast, int N, int kStage>
 __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, float* __restrict__ raw, float* __restrict__ stash,
-                                          uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t tile,
-                                          int64_t P_pad, const RowState& rs, Ring& ring, const float* s_bias,
+                                          uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t blk,
+                                          int64_t P_pad, const RowState& rs, WeightRing<kStage>& ring, const float* s_bias,
                                           const float* s_headw, const float* s_headb, const float* viewb, int hw1) {
   static_assert(!(kTrain && kFast), "the single-pass forward is inference only");
-  constexpr int kSps = kFast ? fast_sps(N) : kStepsPerStage;  // k-steps a ring stage can hold
+  // k-steps a ring stage can hold (the unrolled bound; 24 KB stages keep two for every width, mi.sps decides at run time)
+  constexpr int kSps = kFast ? fast_sps(kStage, N) : kStage == kStageBytes ? kStepsPerStage : split_sps(kStage, N);
   const int wt = threadIdx.x & 127, wi = wt >> 5, lane = wt & 31, q = lane & 3;
   const GemmLayer& g = p.g[e];
-  const MmaInfo mi = mma_info(p, blob, e, kFast);
+  const MmaInfo mi = mma_info(p, blob, e, kFast, kStage);
   const int enc_w = p.enc_tile_w;
   const uint32_t act_a = smem_u32(sm + mp.act), enc_a = smem_u32(sm + mp.enc);
   const int fin = g.k_h > 0 ? g.k_h : 16;
@@ -119,7 +138,7 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
   wgmma_fence();
   for (int ks0 = 0; ks0 < mi.ksteps; ks0 += mi.sps) {
     const uint32_t st = ring.acquire();
-    const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStageBytes);
+    const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStage);
 #pragma unroll
     for (int hh = 0; hh < kSps; ++hh) {
       const int ks = ks0 + hh;
@@ -168,8 +187,12 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
     for (int m = 0; m < N / 32; ++m) mbits[i][m] = 0u;
   uint8_t* act = sm + mp.act;
   const int act_lo = rows * N * 2;
+  // the stash tile's hi block, moved so that the shared-memory tile's offsets (rows 64 wg ...) land on rows 64 (blk & 1) ...:
+  // 64 rows of a hi block are 128 N bytes
   uint8_t* st_hi = nullptr;
-  if (kTrain) st_hi = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * g.cum_n) + (size_t)tile * tile_bytes(N);
+  if (kTrain)
+    st_hi = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * g.cum_n) + (size_t)(blk >> 1) * tile_bytes(N) +
+            ((int)(blk & 1) - wg) * (128 * N);
   const int r0 = 64 * wg + 16 * wi + (lane >> 2);  // tile row of acc row 0 (row 1: + 8)
 
 #pragma unroll
@@ -249,15 +272,17 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
 // each 64-row block's rays from blocks[], and the tile count from *n_blocks in device memory.  Every row is computed as
 // the default instance computes its point, so an evaluated point's raw has the same bits.
 template <bool kTrain, int kH, bool kFast, bool kPts, bool kMap>
-__global__ void __launch_bounds__(128 * (kH == 128 ? 2 : 1) + 32, 1)
+__global__ void __launch_bounds__(128 * n_wg(kH) + 32, 1)
 mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ rays,
                   int ray_stride, const float* __restrict__ z, int64_t P, int S, int64_t n_tiles,
                   float* __restrict__ raw,          // out [P][4]
                   float* __restrict__ stash,        // out (kTrain)
                   const float* __restrict__ pts, const float* __restrict__ dirs, int dir_stride,  // kPts
-                  const int* __restrict__ map, const int2* __restrict__ blocks, const int* __restrict__ n_blocks) {  // kMap
+                  const int* __restrict__ map, const int2* __restrict__ blocks, const int* __restrict__ n_blocks,  // kMap
+                  int64_t stash_tiles) {  // kTrain: 128-point tiles of the stash, ceil(P / 128)
   static_assert(!(kMap && (kTrain || kPts)), "the row map is an inference path of the render points");
-  constexpr int kWG = kH == 128 ? 2 : 1, kRows = 64 * kWG, kThreads = 128 * kWG + 32;
+  constexpr int kWG = n_wg(kH), kRows = 64 * kWG, kThreads = 128 * kWG + 32, kStage = stage_bytes(kH);
+  using Ring = WeightRing<kStage>;
   uint8_t* sm = smem_base();
   const SmemMap mp = smem_map(p);
   float* s_bias = reinterpret_cast<float*>(sm + mp.bias);
@@ -269,7 +294,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
-  const int64_t P_pad = n_tiles * kTileRows;       // the stash sections are sized in 128-point tiles
+  const int64_t P_pad = stash_tiles * kTileRows;   // the stash sections are sized in 128-point tiles
   const int enc_w = p.enc_tile_w;                  // encoding operand tile width (dim_xyz padded to 16)
 
   if (tid == 0) {
@@ -303,7 +328,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       const uint64_t pol = l2_policy_evict_last();
       for (int j = 0; j < my_tiles; ++j)
         for (int e = 0; e < p.n_gemm; ++e) {
-          const MmaInfo mi = mma_info(p, blob, e, kFast);
+          const MmaInfo mi = mma_info(p, blob, e, kFast, kStage);
           for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
             const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
             const uint8_t* src = mi.src + (size_t)ks * mi.kbytes;
@@ -327,7 +352,13 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
 #pragma unroll 1
     for (int j = 0; j < my_tiles; ++j) {
       const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
-      const int64_t p0 = tile * kRows + 64 * wg;   // first point (kMap: first map row) of this warpgroup
+      const int64_t p0 = tile * kRows + 64 * wg;   // first point (kMap: first map row) of this warpgroup's 64-row block
+      // kTrain: the block is one half of a 128-point stash tile.  A block past P inside the last stash tile fills its
+      // half from the last point, so the backward reads whole tiles.  A block past the last stash tile (the end of the
+      // last CTA tile) has nowhere to write: its warpgroup runs the layers as the inference forward does, which keeps it
+      // walking the weight ring with the others, and every row of it is invalid.
+      const int64_t blk = p0 >> 6;
+      const bool stashes = kTrain && (blk >> 1) < stash_tiles;
       TileRays tr;
       RowState rs;
       bool block_live = true;                      // kMap: this warpgroup's 64-row block exists
@@ -405,20 +436,28 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       }
       fence_proxy_async();  // the tile was written through the generic proxy; wgmma / the bulk store read it via the async proxy
       wg_bar();             // also publishes viewb
-      if (kTrain && wt == 0) {  // this warpgroup's half of the encoding tile goes to the stash as it is: two bulk stores
-        uint8_t* dst = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * p.enc_cum[0]) + (size_t)tile * tile_bytes(enc_w);
-        const int part = enc_hb / kWG;
-        bulk_s2g(dst + wg * part, enc + wg * part, (uint32_t)part);
-        bulk_s2g(dst + tile_half_bytes(enc_w) + wg * part, enc + enc_hb + wg * part, (uint32_t)part);
+      if (stashes && wt == 0) {  // this warpgroup's rows of the encoding tile go to the stash as they are:
+        // two bulk stores into half blk & 1 of stash tile blk >> 1 (64 rows of a hi or lo block are contiguous)
+        uint8_t* dst = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * p.enc_cum[0]) + (size_t)(blk >> 1) * tile_bytes(enc_w);
+        const int part = enc_hb / kWG, dpart = (int)(blk & 1) * part;
+        bulk_s2g(dst + dpart, enc + wg * part, (uint32_t)part);
+        bulk_s2g(dst + tile_half_bytes(enc_w) + dpart, enc + enc_hb + wg * part, (uint32_t)part);
       }
 #pragma unroll 1
       for (int e = 0; e < p.n_gemm; ++e) {
-        if (p.g[e].n == kH)
-          fwd_layer<kTrain, kFast, kH>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, ring, s_bias,
-                                    s_headw, s_headb, viewb, hw1);
-        else
-          fwd_layer<kTrain, kFast, kH / 2>(p, blob, raw, stash, sm, mp, e, wg, kRows, tile, P_pad, rs, ring, s_bias,
-                                        s_headw, s_headb, viewb, hw1);
+        auto layer = [&](auto train, auto width) {
+          fwd_layer<decltype(train)::value, kFast, decltype(width)::value, kStage>(
+              p, blob, raw, stash, sm, mp, e, wg, kRows, blk, P_pad, rs, ring, s_bias, s_headw, s_headb, viewb, hw1);
+        };
+        using std::bool_constant;
+        using std::integral_constant;
+        if (p.g[e].n == kH) {
+          if (stashes || !kTrain) layer(bool_constant<kTrain>{}, integral_constant<int, kH>{});
+          else layer(bool_constant<false>{}, integral_constant<int, kH>{});
+        } else {
+          if (stashes || !kTrain) layer(bool_constant<kTrain>{}, integral_constant<int, kH / 2>{});
+          else layer(bool_constant<false>{}, integral_constant<int, kH / 2>{});
+        }
       }
     }
     if (kTrain && wt == 0) bulk_wait_all();  // this warpgroup's encoding-tile stores
@@ -452,14 +491,15 @@ int tc_supported(const Plan& p, int n_samples, bool training, const char* what) 
 template <bool kTrain, int kH, bool kFast>
 static int launch_fwd(const Plan& p, const float* blob, const PointSrc& src, int64_t P, int n_samples, float* raw,
                       float* stash, cudaStream_t s, const char* what) {
-  constexpr int kRows = 64 * (kH == 128 ? 2 : 1), kThreads = 2 * kRows + 32;
-  const int64_t tiles = (P + kRows - 1) / kRows;
-  const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // = tiles whenever the stash is written (hidden 128)
+  constexpr int kRows = 64 * n_wg(kH), kThreads = 2 * kRows + 32;
+  const int64_t stash_tiles = (P + kTileRows - 1) / kTileRows;  // the stash keeps 128-point tiles whatever the CTA tile
+  // training covers both halves of every stash tile, the last one's second half too when it lies past P
+  const int64_t tiles = ((kTrain ? stash_tiles * kTileRows : P) + kRows - 1) / kRows;
   auto kern = src.pts ? mlp_fwd_tc_kernel<kTrain, kH, kFast, true, false>
                       : mlp_fwd_tc_kernel<kTrain, kH, kFast, false, false>;
   return launch_persistent(kern, tiles, kThreads, smem_map(p).total, s, what, p, blob, src.rays, src.ray_stride, src.z, P,
-                           n_samples, kTrain ? stash_tiles : tiles, raw, stash, src.pts, src.dirs, src.dir_stride,
-                           (const int*)nullptr, (const int2*)nullptr, (const int*)nullptr);
+                           n_samples, tiles, raw, stash, src.pts, src.dirs, src.dir_stride, (const int*)nullptr,
+                           (const int2*)nullptr, (const int*)nullptr, stash_tiles);
 }
 
 // over a row map: the grid covers max_blocks blocks; the kernel reads the live count from m.n_blocks
@@ -467,11 +507,11 @@ template <int kH, bool kFast>
 static int launch_fwd_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
                           int64_t P, int n_samples, const RowMap& m, int64_t max_blocks, float* raw, cudaStream_t s,
                           const char* what) {
-  constexpr int kWG = kH == 128 ? 2 : 1, kThreads = 128 * kWG + 32;
+  constexpr int kWG = n_wg(kH), kThreads = 128 * kWG + 32;
   const int64_t tiles = (max_blocks + kWG - 1) / kWG;
   return launch_persistent(mlp_fwd_tc_kernel<false, kH, kFast, false, true>, tiles, kThreads, smem_map(p).total, s, what,
                            p, blob, rays, ray_stride, z, P, n_samples, tiles, raw, (float*)nullptr,
-                           (const float*)nullptr, rays + 8, ray_stride, m.map, m.blocks, m.n_blocks);
+                           (const float*)nullptr, rays + 8, ray_stride, m.map, m.blocks, m.n_blocks, (int64_t)0);
 }
 
 int launch_mlp_fwd_tc_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,
