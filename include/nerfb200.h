@@ -332,6 +332,45 @@ int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_a
                                  const nerfb200_grid_t* grid, const uint32_t* bits, float* out_coarse, float* out_fine,
                                  void* workspace, int32_t impl, int64_t* n_evaluated, void* stream);
 
+/* ---- meshes: marching cubes over a lattice of values -------------------------------------------------------------
+ * The box is a nerfb200_grid_t read as res[c] cubes per axis; its lattice is the (res[0] + 1) x (res[1] + 1) x
+ * (res[2] + 1) cube corners, point (i_0, i_1, i_2) at linear index (i_2 * n_1 + i_1) * n_0 + i_0 with n_c = res[c] + 1
+ * (x fastest), at coordinates, per axis c, in fp32 with round-to-nearest and no contraction:
+ *     p_c(i) = lo[c] + ((hi[c] - lo[c]) * (float)i) / (float)res[c]
+ * volume[n_2][n_1][n_0] holds one fp32 value per lattice point.  A point is inside when its value exceeds `level` (NaN is
+ * outside).  The lattice edge (q, a) runs from point q to its +1 neighbour along axis a; it crosses when exactly one of
+ * its ends is inside, and then carries one vertex, at t = (level - v0) / (v1 - v0) from q:
+ *     coordinate a = p_a(q_a) + t * (p_a(q_a + 1) - p_a(q_a)),  the other two = those of q   (fp32, each op rounded)
+ * Vertex ids follow lattice-edge order: the crossing edges sorted by (linear index of q, a).  Each cube (named by its low
+ * corner) takes its triangles from the face-consistent case table csrc/mc_table.cuh (generated by tools/gen_mc_table.py,
+ * which states the corner and edge numbering): every face of a cube carries segments chosen by that face's four corner
+ * signs alone (on a face with two diagonal inside corners the inside corners stay apart), so two cubes sharing a face
+ * agree on it and the mesh is closed wherever the surface stays inside the lattice.  Faces are int32 vertex-id triples,
+ * counter-clockwise seen from outside (the normal by the right-hand rule points from inside to outside), cube by cube in
+ * linear order and, within a cube, in table order.  Prefix sums throughout, no atomics: the mesh is a function of the
+ * volume and the level.
+ *
+ * mesh_lattice_points: pts[nz][n_1][n_0][3] = the lattice points of planes i_2 = z0 .. z0 + nz - 1 (the points a caller
+ *   evaluates its field at; they depend on the lattice index alone, not on how the planes are split into calls).
+ * mesh_workspace_bytes: device bytes of the workspace mesh_count fills and mesh_emit reads; -1 for an invalid box or
+ *   more than 2^31 lattice points.
+ * mesh_count: classify every lattice point (its crossing edges, and its cube's case) and scan: totals[0] = vertices,
+ *   totals[1] = faces (device int64[2]).  The counts stay in device memory; a caller sizing the outputs reads them once.
+ * mesh_emit: with the workspace of mesh_count on the same volume and level, writes vertices[V][3] and faces[F][3]
+ *   (V, F = the totals; max_vertices, max_faces bound every write).  view_dirs[V][3] (may be NULL) receives, per vertex,
+ *   the direction of a ray reaching it head-on from outside: the normalised density gradient, i.e. -n for the outward
+ *   normal n.  The gradient at lattice point i is, per axis c, (v[i_hi] - v[i_lo]) / (h_c * (float)(i_hi - i_lo)) with
+ *   i_lo = max(i_c - 1, 0), i_hi = min(i_c + 1, res[c]) (central differences, one-sided at the lattice's faces) and
+ *   h_c = (hi[c] - lo[c]) / (float)res[c]; along the edge g = g0 + t * (g1 - g0) per component;
+ *   s = (gx * gx + gy * gy) + gz * gz; dir = g / sqrt(s) when 0 < s < inf, else (0, 0, 1).  All fp32, each op rounded. */
+int64_t nerfb200_mesh_workspace_bytes(const nerfb200_grid_t* box);
+int32_t nerfb200_mesh_lattice_points(const nerfb200_grid_t* box, int32_t z0, int32_t nz, float* pts, void* stream);
+int32_t nerfb200_mesh_count(const nerfb200_grid_t* box, const float* volume, float level, void* workspace,
+                            int64_t* totals, void* stream);
+int32_t nerfb200_mesh_emit(const nerfb200_grid_t* box, const float* volume, float level, const void* workspace,
+                           int64_t max_vertices, int64_t max_faces, float* vertices, int32_t* faces, float* view_dirs,
+                           void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

@@ -15,12 +15,14 @@ from .cache_pool import CachedRayPool, CachedValidationSet
 from .ops import SeededRandoms
 from .graph_step import CapturedTrainStep
 from .occupancy import OccupancyGrid
+from .mesh import Mesh, density_volume, extract_mesh, extract_mesh_from_volume
 from . import ops, parallel
 
 __all__ = [
     "FlexibleNeRFModel", "Embedder", "get_embedding_function", "get_minibatches", "get_ray_bundle", "img2mse",
     "meshgrid_xy", "mse2psnr", "ndc_rays", "positional_encoding", "sample_pdf", "predict_and_render_radiance",
     "run_network", "volume_render_radiance_field",
-    "run_one_iter_of_nerf", "run_one_iter_of_nerf_from_pose", "set_default_impl", "invalidate", "render_image", "cast_to_image", "cast_to_disparity_image", "CachedRayPool", "CachedValidationSet", "SeededRandoms", "CapturedTrainStep", "OccupancyGrid", "ops",
+    "run_one_iter_of_nerf", "run_one_iter_of_nerf_from_pose", "set_default_impl", "invalidate", "render_image", "cast_to_image", "cast_to_disparity_image", "CachedRayPool", "CachedValidationSet", "SeededRandoms", "CapturedTrainStep", "OccupancyGrid", "Mesh",
+    "density_volume", "extract_mesh", "extract_mesh_from_volume", "ops",
     "parallel",
 ]

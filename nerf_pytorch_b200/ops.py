@@ -712,3 +712,48 @@ def render_fwd_grid(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, rand
                                             _ptr(workspace), int(impl), _ptr(n_evaluated), _stream()),
                "render_fwd_grid")
     return out_c, out_f, workspace
+
+
+# ------------------------------------------------------------------------------------------------
+# meshes (include/nerfb200.h "meshes"; nerf_pytorch_b200/mesh.py is the public interface).  The box is a Grid read as
+# res cubes per axis, its lattice the (res + 1) points per axis at the cube corners.
+# ------------------------------------------------------------------------------------------------
+def mesh_workspace_bytes(box: Grid) -> int:
+    n = _lib.load().nerfb200_mesh_workspace_bytes(C.byref(box))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, "mesh_workspace_bytes")
+    return int(n)
+
+
+def mesh_lattice_points(box: Grid, z0: int, nz: int, out: torch.Tensor) -> torch.Tensor:
+    """The lattice points of planes z0 .. z0 + nz - 1 into the first nz * (res_y + 1) * (res_x + 1) rows of ``out``
+    (fp32 CUDA, (rows, 3) or anything of that many floats)."""
+    _lib.check(_lib.load().nerfb200_mesh_lattice_points(C.byref(box), int(z0), int(nz), _ptr(out), _stream()),
+               "mesh_lattice_points")
+    return out
+
+
+def mesh_count(box: Grid, volume: torch.Tensor, level: float, workspace: Optional[torch.Tensor] = None):
+    """Classify and scan: returns (totals int64[2] = [vertices, faces] on the device, workspace)."""
+    need = mesh_workspace_bytes(box)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=volume.device)
+    totals = torch.empty(2, dtype=torch.int64, device=volume.device)
+    _lib.check(_lib.load().nerfb200_mesh_count(C.byref(box), _ptr(volume), float(level), _ptr(workspace), _ptr(totals),
+                                               _stream()), "mesh_count")
+    return totals, workspace
+
+
+def mesh_emit(box: Grid, volume: torch.Tensor, level: float, workspace: torch.Tensor, n_vertices: int, n_faces: int,
+              want_dirs: bool = False):
+    """Vertices (V, 3) fp32, faces (F, 3) int32 and, with ``want_dirs``, each vertex's view direction (V, 3)."""
+    dev = volume.device
+    verts = torch.empty(n_vertices, 3, dtype=torch.float32, device=dev)
+    faces = torch.empty(n_faces, 3, dtype=torch.int32, device=dev)
+    dirs = torch.empty(n_vertices, 3, dtype=torch.float32, device=dev) if want_dirs else None
+    _lib.check(_lib.load().nerfb200_mesh_emit(C.byref(box), _ptr(volume), float(level), _ptr(workspace),
+                                              int(n_vertices), int(n_faces), _ptr(verts) if n_vertices else None,
+                                              _ptr(faces) if n_faces else None,
+                                              _ptr(dirs) if want_dirs and n_vertices else None, _stream()),
+               "mesh_emit")
+    return verts, faces, dirs
