@@ -332,6 +332,45 @@ int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_a
                                  const nerfb200_grid_t* grid, const uint32_t* bits, float* out_coarse, float* out_fine,
                                  void* workspace, int32_t impl, int64_t* n_evaluated, void* stream);
 
+/* ---- early ray termination: inference renders that stop a ray's last pass once it is opaque ----------------------
+ * nerfb200_render_fwd_early_stop is render_fwd for inference (impl 1 or 3), with or without an occupancy grid (grid and
+ * bits both NULL: no grid), and a threshold t = stop_transmittance, 0 <= t < 1.
+ *   - Only the last pass terminates: the fine pass when n_fine > 0, else the coarse pass.  The coarse pass of a two-pass
+ *     render runs as render_fwd / render_fwd_grid run it, so its outputs, weights and the fine depths are bit-identical.
+ *   - Rounds.  In the last pass a ray's evaluated samples are those the grid keeps (all of them without a grid).  They
+ *     run the MLP in rounds, in sample order: round k takes evaluated samples k K .. k K + K - 1 (K = NERFB200_STOP_ROUND)
+ *     of every ray still live, compacted as nerfb200_grid_compact compacts (groups of 10 rays, 64-row blocks).
+ *   - Termination.  After each round in which a ray evaluated samples, its transmittance T is the fp32 product, in sample
+ *     order, of the compositing's q = (1 - alpha) + 1e-10 over its samples evaluated so far, alpha from the same sigma
+ *     gate, noise, delta and |d| as the compositing.  The ray stops when T < t (strict) and it has samples left to
+ *     evaluate; each of those gets raw = [0 0 0 -inf].  With t = 0 no ray stops.
+ *   - Outputs.  The last pass is composited as render_fwd composites it, over the full raw.  An evaluated sample's raw is
+ *     bit for bit render_fwd's (a row's MLP result does not depend on its block).
+ *   - Guarantee.  A ray that never stops gets render_fwd's outputs (render_fwd_grid's with a grid) bit for bit.  For a
+ *     ray that stops, the weights left out sum to at most its T at the stop, which is below t: without a white
+ *     background rgb and acc can only drop, by at most t, and depth by at most t * max z; with a white background rgb
+ *     can only rise, by at most t.
+ * stop_sample (device int32[n_rays], may be NULL): one past the last sample the ray evaluated when it stopped, so every
+ * sample from there on that it would have evaluated was skipped by termination; n_samples of the pass if it never
+ * stopped.  n_evaluated (device int64[2], may be NULL): the MLP rows each pass ran (the coarse pass of a two-pass render
+ * without a grid runs all n_rays * n_coarse).  No host synchronisation: rounds after every ray has finished run empty.
+ * Refused before any launch: impl 0 (NERFB200_ERR_UNSUPPORTED); t outside [0, 1) or NaN, an invalid grid, a grid without
+ * bits or bits without a grid (NERFB200_ERR_INVALID); an architecture the wgmma inference forward refuses (its reason).
+ * workspace: nerfb200_render_early_stop_workspace_bytes(...) bytes; its first sections are those of render_fwd's
+ * inference workspace. */
+#define NERFB200_STOP_ROUND 32
+/* NERFB200_STOP_ROUND, for bindings that do not read this header */
+int32_t nerfb200_render_early_stop_round(void);
+int64_t nerfb200_render_early_stop_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                                   const nerfb200_render_opts_t* opts, int64_t n_rays);
+int32_t nerfb200_render_fwd_early_stop(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                       const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                       const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                       const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                       const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                                       float* out_coarse, float* out_fine, void* workspace, int32_t impl,
+                                       int64_t* n_evaluated, int32_t* stop_sample, void* stream);
+
 /* ---- meshes: marching cubes over a lattice of values -------------------------------------------------------------
  * The box is a nerfb200_grid_t read as res[c] cubes per axis; its lattice is the (res[0] + 1) x (res[1] + 1) x
  * (res[2] + 1) cube corners, point (i_0, i_1, i_2) at linear index (i_2 * n_1 + i_1) * n_0 + i_0 with n_c = res[c] + 1

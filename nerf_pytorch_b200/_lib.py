@@ -121,6 +121,10 @@ SIGNATURES = {
     "nerfb200_grid_compact": (I32, [GP, P, P, I32, P, I64, I32, P, P, P, P, P, P, P]),
     "nerfb200_render_grid_workspace_bytes": (I64, [AP, AP, OP, I64]),
     "nerfb200_render_fwd_grid": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, P, P, P, I32, P, P]),
+    "nerfb200_render_early_stop_round": (I32, []),
+    "nerfb200_render_early_stop_workspace_bytes": (I64, [AP, AP, OP, I64]),
+    "nerfb200_render_fwd_early_stop": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, F32, P, P, P, I32, P,
+                                             P, P]),
     "nerfb200_mesh_workspace_bytes": (I64, [GP]),
     "nerfb200_mesh_lattice_points": (I32, [GP, I32, I32, P, P]),
     "nerfb200_mesh_count": (I32, [GP, P, F32, P, P, P]),

@@ -737,6 +737,35 @@ static GridWorkspace carve_grid(int64_t base, int64_t n_rays, int n_samples) {
   return g;
 }
 
+// The sections an early-stopping render adds after the grid sections (sized for the coarse pass, which the grid may
+// compact): the per-ray state of the last pass (StopState), the groups' first blocks, one round's row map, its blocks,
+// block count and row total.
+struct StopWorkspace {
+  int64_t order, n_eval, T, counts, first_block, map, blocks, n_blocks, rows, total;
+};
+static StopWorkspace carve_stop(int64_t base, int64_t n_rays, int n_samples) {
+  StopWorkspace sw;
+  const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
+  const int64_t mb = stop_round_max_blocks(n_rays, n_samples);
+  sw.order = base;
+  sw.n_eval = sw.order + align256(n_rays * n_samples * 4);
+  sw.T = sw.n_eval + align256(n_rays * 4);
+  sw.counts = sw.T + align256(n_rays * 4);
+  sw.first_block = sw.counts + align256(groups * 4);
+  sw.map = sw.first_block + align256(groups * 4);
+  sw.blocks = sw.map + align256(mb * 64 * 4);
+  sw.n_blocks = sw.blocks + align256(mb * 8);
+  sw.rows = sw.n_blocks + 256;
+  sw.total = sw.rows + 256;
+  return sw;
+}
+
+// early ray termination of the last pass: the threshold and the optional stop_sample output
+struct StopArgs {
+  float t;
+  int32_t* stop_sample;
+};
+
 // render_fwd, and with a grid (grid != NULL, inference only) the same passes with the MLP run over each pass's compacted
 // samples.  Without a grid the launches are exactly render_fwd's.
 static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
@@ -744,7 +773,8 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
                           const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
                           const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
                           const nerfb200_grid_t* grid, const uint32_t* bits, int64_t* n_evaluated, float* out_coarse,
-                          float* out_fine, void* workspace, int32_t training, int32_t impl, void* stream) {
+                          float* out_fine, void* workspace, int32_t training, int32_t impl, void* stream,
+                          const StopArgs* stop = nullptr) {
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
@@ -783,10 +813,22 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
       return NERFB200_ERR_UNSUPPORTED;
     }
   }
+  if (stop) {
+    if (training || impl == 0) {
+      set_error("%s: early ray termination renders only (training = 0), on the wgmma inference forward: impl 1 or 3, "
+                "not impl=%d", what, impl);
+      return NERFB200_ERR_UNSUPPORTED;
+    }
+    if (!(stop->t >= 0.f && stop->t < 1.f)) {
+      set_error("%s: stop_transmittance %g must be in [0, 1)", what, stop->t);
+      return NERFB200_ERR_INVALID;
+    }
+  }
   Workspace w;
   carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
   char* base = static_cast<char*>(workspace);
   auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
+  auto I = [&](int64_t off) { return reinterpret_cast<int*>(base + off); };
   const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const Need need = training ? kStash : kInference;
@@ -796,9 +838,34 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
     NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
     NB_TRY(check_impl(pf, impl, ns, need, what));
   }
-  const GridWorkspace gw = carve_grid(w.total, n_rays, fine ? ns : nc);
-  // the MLP of one pass: every sample, or with a grid the compacted samples (skipped ones get raw = [0 0 0 -inf])
+  const GridWorkspace gw = carve_grid(w.total, n_rays, fine && !stop ? ns : nc);
+  const StopWorkspace sw = carve_stop(gw.total, n_rays, fine ? ns : nc);
+  // the last pass with early ray termination: one marking launch, then rounds of compaction, MLP and the per-ray
+  // transmittance update.  Rounds after every ray has finished have no blocks.
+  auto stop_rounds = [&](bool is_fine, const Plan& p, const float* blob, int n, const float* z, float* raw) {
+    const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
+    const StopState st{I(sw.order), I(sw.n_eval), F(sw.T), stop->stop_sample, I(sw.counts)};
+    int* nb = I(sw.n_blocks);
+    int64_t* rows = reinterpret_cast<int64_t*>(base + sw.rows);
+    // the coarse pass of a two-pass render without a grid ran every sample
+    int64_t* coarse_rows = (is_fine && !grid && n_evaluated) ? n_evaluated : nullptr;
+    NB_TRY(launch_stop_mark(grid ? *grid : nerfb200_grid_t{}, bits, rays, ray_stride, z, n_rays, n, raw, st, coarse_rows,
+                            n_rays * nc, s));
+    const RowMap m{I(sw.map), reinterpret_cast<const int2*>(base + sw.blocks), nb};
+    const int64_t mb = stop_round_max_blocks(n_rays, n);
+    for (int k = 0; k * kStopRound < n; ++k) {
+      NB_TRY(launch_grid_scan(I(sw.counts), groups, I(sw.first_block), nb, rows, s));
+      NB_TRY(launch_stop_scatter(st, I(sw.first_block), n_rays, n, k, I(sw.map), I(sw.blocks), s));
+      NB_TRY(launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, mb, raw, impl == 3, s));
+      NB_TRY(launch_stop_update(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], opts->noise_std,
+                                n_rays, n, k, stop->t, st, rows, n_evaluated ? n_evaluated + is_fine : nullptr, s));
+    }
+    return NERFB200_OK;
+  };
+  // the MLP of one pass: every sample, or with a grid the compacted samples (skipped ones get raw = [0 0 0 -inf]), or
+  // in the last pass of an early-stopping render the rounds above
   auto mlp = [&](bool is_fine, const Plan& p, const float* blob, int n, const float* z, float* raw, float* stash) {
+    if (stop && is_fine == fine) return stop_rounds(is_fine, p, blob, n, z, raw);
     if (!grid)
       return mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, training ? stash : nullptr, s);
     int* nb = reinterpret_cast<int*>(base + gw.n_blocks);
@@ -868,6 +935,39 @@ int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_a
   return render_forward("render_fwd_grid", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand,
                         noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace, /*training=*/0,
                         impl, stream);
+}
+
+int32_t nerfb200_render_early_stop_round(void) { return kStopRound; }
+
+int64_t nerfb200_render_early_stop_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                                   const nerfb200_render_opts_t* opts, int64_t n_rays) {
+  Plan pc, pf;
+  if (build_plan(coarse, &pc) != NERFB200_OK) return -1;
+  if (fine && build_plan(fine, &pf) != NERFB200_OK) return -1;
+  if (check_opts(opts) != NERFB200_OK || n_rays <= 0) return -1;
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
+  const bool has_fine = fine && opts->n_fine > 0;
+  const GridWorkspace gw = carve_grid(w.total, n_rays, opts->n_coarse);
+  return carve_stop(gw.total, n_rays, has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse).total;
+}
+
+int32_t nerfb200_render_fwd_early_stop(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                       const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                       const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                       const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                       const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                                       float* out_coarse, float* out_fine, void* workspace, int32_t impl,
+                                       int64_t* n_evaluated, int32_t* stop_sample, void* stream) {
+  if ((grid == nullptr) != (bits == nullptr)) {
+    set_error("render_fwd_early_stop: a grid descriptor and its bits come together (descriptor %s, bits %s)",
+              grid ? "given" : "NULL", bits ? "given" : "NULL");
+    return NERFB200_ERR_INVALID;
+  }
+  const StopArgs stop{stop_transmittance, stop_sample};
+  return render_forward("render_fwd_early_stop", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                        t_rand, noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace,
+                        /*training=*/0, impl, stream, &stop);
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,

@@ -220,6 +220,35 @@ int check_grid(const nerfb200_grid_t* g, const char* what);
 int launch_grid_compact(const nerfb200_grid_t& g, const uint32_t* bits, const float* rays, int ray_stride, const float* z,
                         int64_t n_rays, int n_samples, float* raw, int* map, int* blocks, int* n_blocks,
                         int64_t* n_evaluated, int* scratch, cudaStream_t s);
+// ---- early ray termination of an inference render's last pass (nerfb200.h "early ray termination") ----
+// Per-ray state in device memory: order[r][i] = the sample of the ray's i-th evaluated sample, n_eval[r] = its evaluated
+// count (cut to what it ran when it stops), T[r] = its transmittance; counts[g] = the rows of group g in the next round.
+constexpr int kStopRound = NERFB200_STOP_ROUND;
+struct StopState {
+  int* order;
+  int* n_eval;
+  float* T;
+  int* stop;  // stop_sample, or null
+  int* counts;
+};
+// the 64-row blocks one round can fill
+int64_t stop_round_max_blocks(int64_t n_rays, int n_samples);
+// marks the pass's samples (grid lookup when bits is non-null, skipped ones get raw = [0 0 0 -inf]), fills order /
+// n_eval / T / stop and round 0's counts; *other_rows = other_value when other_rows is non-null
+int launch_stop_mark(const nerfb200_grid_t& g, const uint32_t* bits, const float* rays, int ray_stride, const float* z,
+                     int64_t n_rays, int n_samples, float* raw, const StopState& st, int64_t* other_rows,
+                     int64_t other_value, cudaStream_t s);
+// round k's row map from the counts and the first blocks grid_scan_kernel made of them (RowMap format)
+int launch_stop_scatter(const StopState& st, const int* first_block, int64_t n_rays, int n_samples, int round, int* map,
+                        int* blocks, cudaStream_t s);
+// after round k's MLP: T of every ray that ran rows, the stop test, raw = [0 0 0 -inf] for a stopped ray's remaining
+// samples, round k + 1's counts; *n_evaluated (if non-null) gets round k's rows added (round 0: set)
+int launch_stop_update(float* raw, const float* z, const float* dirs, int dir_stride,
+                       const RandSrc& noise, float noise_std, int64_t n_rays, int n_samples, int round, float threshold,
+                       const StopState& st, const int64_t* round_rows, int64_t* n_evaluated, cudaStream_t s);
+// grid_scan_kernel (occupancy.cu) alone: first blocks, block count and row total of per-group row counts
+int launch_grid_scan(const int* counts, int64_t n_groups, int* first_block, int* n_blocks, int64_t* n_rows,
+                     cudaStream_t s);
 // the wgmma inference forward (impl 1, or fast: impl 3) over a RowMap of the points o + d z of the ray rows; max_blocks
 // bounds *n_blocks (the grid size is chosen on the host)
 int launch_mlp_fwd_tc_map(const Plan& p, const float* blob, const float* rays, int ray_stride, const float* z,

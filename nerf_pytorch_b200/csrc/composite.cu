@@ -212,6 +212,78 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
   }
 }
 
+// Early ray termination (nerfb200.h): after round `round` of a pass's MLP, one warp per ray multiplies the q of the
+// ray's rows of that round into its T, in sample order, with the terms composite_fwd_kernel uses.  A ray with samples
+// left stops when T < threshold: the rest of its evaluated samples get raw = [0 0 0 -inf] and its count is cut to what
+// it ran.  One CTA per compaction group writes the group's rows of the next round.
+constexpr int kStopGroupRays = kGridGroupRays;
+
+__global__ void __launch_bounds__(kStopGroupRays * 32)
+stop_update_kernel(float* __restrict__ raw, const float* __restrict__ z, const float* __restrict__ dirs, int dir_stride,
+                   const RandSrc noise, float noise_std, int64_t n_rays, int S, int round, float threshold, StopState st,
+                   const int64_t* __restrict__ round_rows, int64_t* __restrict__ n_evaluated) {
+  __shared__ int rows[kStopGroupRays];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t r = (int64_t)blockIdx.x * kStopGroupRays + w;
+  const int k0 = round * kStopRound;
+  int next = 0;
+  if (r < n_rays) {
+    int n = st.n_eval[r];
+    const int end = min(n, k0 + kStopRound);
+    if (end > k0) {
+      const float* rd = dirs + r * dir_stride;
+      const float dx = rd[0], dy = rd[1], dz = rd[2];
+      const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)));
+      const bool has_noise = noise.present() && noise_std > 0.f;
+      const int* ord = st.order + r * S;
+      const float4* raw4 = reinterpret_cast<const float4*>(raw) + r * S;
+      const float* zr = z + r * S;
+      float T = st.T[r];
+      for (int b = k0; b < end; b += 32) {
+        float q = 1.f;
+        if (b + lane < end) {
+          const int j = ord[b + lane];
+          const bool last = j == S - 1;
+          q = sample_terms(raw4[j].w, has_noise ? noise.normal(r, j) : 0.f, noise_std, has_noise, zr[j],
+                           last ? 0.f : zr[j + 1], last, dnorm).q;
+        }
+        const int m = min(32, end - b);
+        for (int i = 0; i < m; ++i) T = __fmul_rn(T, __shfl_sync(0xffffffffu, q, i));
+      }
+      if (T < threshold && end < n) {
+        float4* out4 = reinterpret_cast<float4*>(raw) + r * S;
+        for (int i = end + lane; i < n; i += 32) out4[ord[i]] = make_float4(0.f, 0.f, 0.f, -INFINITY);
+        n = end;
+        if (lane == 0) {
+          st.n_eval[r] = n;
+          if (st.stop) st.stop[r] = ord[end - 1] + 1;
+        }
+      }
+      if (lane == 0) st.T[r] = T;
+    }
+    next = min(max(n - (k0 + kStopRound), 0), kStopRound);
+  }
+  if (lane == 0) rows[w] = next;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int i = 0; i < kStopGroupRays; ++i) total += rows[i];
+    st.counts[blockIdx.x] = total;
+    if (n_evaluated && blockIdx.x == 0) *n_evaluated = (round ? *n_evaluated : 0) + *round_rows;
+  }
+}
+
+int launch_stop_update(float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
+                       float noise_std, int64_t n_rays, int n_samples, int round, float threshold, const StopState& st,
+                       const int64_t* round_rows, int64_t* n_evaluated, cudaStream_t s) {
+  const int64_t groups = (n_rays + kStopGroupRays - 1) / kStopGroupRays;
+  stop_update_kernel<<<(unsigned)groups, kStopGroupRays * 32, 0, s>>>(raw, z, dirs, dir_stride, noise, noise_std, n_rays,
+                                                                      n_samples, round, threshold, st, round_rows,
+                                                                      n_evaluated);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "stop_update launch");
+}
+
 int launch_composite_fwd(const float* raw, const float* z, const float* dirs, int dir_stride, const RandSrc& noise,
                          int64_t n_rays, int n_samples, float noise_std, int white_bkgd, float* out,
                          float* weights, cudaStream_t s) {

@@ -146,7 +146,125 @@ grid_scatter_kernel(const int* __restrict__ rank, const int* __restrict__ counts
   for (int r = cnt + (int)threadIdx.x; r < padded; r += kMarkThreads) map[row0 + r] = -1;
 }
 
+// ---- early ray termination (nerfb200.h "early ray termination"): one CTA per compaction group, one warp per ray ----
+constexpr int kStopThreads = 32 * kGridGroupRays;
+
+__device__ __forceinline__ int round_rows(int n_eval, int round) {
+  const int left = n_eval - round * kStopRound;
+  return left <= 0 ? 0 : left < kStopRound ? left : kStopRound;
+}
+
+// Each evaluated sample's place in its ray's order (ballots in sample order), the ray's count, T = 1, stop = S, and
+// the group's rows in round 0.
+__global__ void __launch_bounds__(kStopThreads)
+stop_mark_kernel(const nerfb200_grid_t g, const uint32_t* __restrict__ bits, const float* __restrict__ rays,
+                 int ray_stride, const float* __restrict__ z, int64_t n_rays, int S, float4* __restrict__ raw,
+                 StopState st, int64_t* __restrict__ other_rows, int64_t other_value) {
+  __shared__ int rows[kGridGroupRays];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t r = (int64_t)blockIdx.x * kGridGroupRays + w;
+  int n = 0;
+  if (r < n_rays) {
+    const float* rr = rays + r * ray_stride;
+    for (int j0 = 0; j0 < S; j0 += 32) {
+      const int j = j0 + lane;
+      bool keep = j < S;
+      if (keep && bits) {
+        const int64_t pt = r * S + j;
+        const float zz = z[pt];
+        float x[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) x[c] = __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));  // as the MLP prologue forms it
+        const int64_t cell = grid_cell(g, x);
+        keep = cell < 0 || ((bits[cell >> 5] >> (cell & 31)) & 1u);
+        if (!keep) raw[pt] = make_float4(0.f, 0.f, 0.f, -INFINITY);
+      }
+      const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+      if (keep) st.order[r * S + n + __popc(ballot & ((1u << lane) - 1u))] = j;
+      n += __popc(ballot);
+    }
+    if (lane == 0) {
+      st.n_eval[r] = n;
+      st.T[r] = 1.f;
+      if (st.stop) st.stop[r] = S;
+    }
+  }
+  if (lane == 0) rows[w] = round_rows(n, 0);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int i = 0; i < kGridGroupRays; ++i) total += rows[i];
+    st.counts[blockIdx.x] = total;
+    if (other_rows && blockIdx.x == 0) *other_rows = other_value;
+  }
+}
+
+// Round k's rows of each live ray, in (ray, sample) order from the group's first block; padding rows -1, each block's
+// first and last ray: the RowMap grid_scatter_kernel writes.
+__global__ void __launch_bounds__(kStopThreads)
+stop_scatter_kernel(StopState st, const int* __restrict__ first_block, int64_t n_rays, int S, int round,
+                    int* __restrict__ map, int2* __restrict__ blocks) {
+  __shared__ int rows[kGridGroupRays];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t r = (int64_t)blockIdx.x * kGridGroupRays + w;
+  const int c = r < n_rays ? round_rows(st.n_eval[r], round) : 0;
+  if (lane == 0) rows[w] = c;
+  __syncthreads();
+  int off = 0, cnt = 0;
+#pragma unroll
+  for (int i = 0; i < kGridGroupRays; ++i) {
+    if (i < w) off += rows[i];
+    cnt += rows[i];
+  }
+  const int fb = first_block[blockIdx.x];
+  const int64_t row0 = (int64_t)fb * 64;
+  int* bx = reinterpret_cast<int*>(blocks);
+  const int* ord = st.order + r * S + round * kStopRound;
+  for (int i = lane; i < c; i += 32) {
+    const int rk = off + i;
+    map[row0 + rk] = (int)(r * S + ord[i]);
+    const int64_t b = fb + (rk >> 6);
+    if ((rk & 63) == 0) bx[2 * b] = (int)r;
+    if ((rk & 63) == 63 || rk == cnt - 1) bx[2 * b + 1] = (int)r;
+  }
+  const int padded = (cnt + 63) & ~63;
+  for (int i = cnt + (int)threadIdx.x; i < padded; i += kStopThreads) map[row0 + i] = -1;
+}
+
 }  // namespace
+
+int64_t stop_round_max_blocks(int64_t n_rays, int n_samples) {
+  const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
+  const int per_ray = n_samples < kStopRound ? n_samples : kStopRound;
+  return groups * (((int64_t)kGridGroupRays * per_ray + 63) / 64);
+}
+
+int launch_stop_mark(const nerfb200_grid_t& g, const uint32_t* bits, const float* rays, int ray_stride, const float* z,
+                     int64_t n_rays, int n_samples, float* raw, const StopState& st, int64_t* other_rows,
+                     int64_t other_value, cudaStream_t s) {
+  const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
+  stop_mark_kernel<<<(unsigned)groups, kStopThreads, 0, s>>>(g, bits, rays, ray_stride, z, n_rays, n_samples,
+                                                             reinterpret_cast<float4*>(raw), st, other_rows,
+                                                             other_value);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "stop_mark launch");
+}
+
+int launch_stop_scatter(const StopState& st, const int* first_block, int64_t n_rays, int n_samples, int round, int* map,
+                        int* blocks, cudaStream_t s) {
+  const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
+  stop_scatter_kernel<<<(unsigned)groups, kStopThreads, 0, s>>>(st, first_block, n_rays, n_samples, round, map,
+                                                                reinterpret_cast<int2*>(blocks));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "stop_scatter launch");
+}
+
+int launch_grid_scan(const int* counts, int64_t n_groups, int* first_block, int* n_blocks, int64_t* n_rows,
+                     cudaStream_t s) {
+  grid_scan_kernel<<<1, kScanThreads, 0, s>>>(counts, n_groups, first_block, n_blocks, n_rows);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "grid_scan launch");
+}
 
 int64_t grid_max_blocks(int64_t n_rays, int n_samples) {
   const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;

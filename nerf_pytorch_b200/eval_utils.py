@@ -17,7 +17,8 @@ from .ops import SeededRandoms
 
 def render_image(height, width, focal_length, tform_cam2world, model_coarse, model_fine, options, mode="validation",
                  encode_position_fn=None, encode_direction_fn=None, *, rays_per_chunk: Optional[int] = None,
-                 device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None, grid=None):
+                 device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None, grid=None,
+                 early_stop: Optional[float] = None):
     """One pose -> (rgb_coarse (H,W,3), disp_coarse (H,W), acc_coarse (H,W), rgb_fine, disp_fine, acc_fine).
 
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
@@ -33,7 +34,11 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
 
     ``grid``: an ``OccupancyGrid`` (INTEGRATION.md, "Optional fast paths"): samples in its empty cells skip the MLP and
     get zero density; impl 1 or 3 only.  Every other sample, and so every ray none of whose skipped samples had density,
-    is computed bit for bit as without the grid."""
+    is computed bit for bit as without the grid.
+
+    ``early_stop``: a transmittance threshold t in [0, 1) (INTEGRATION.md, "Optional fast paths"; combines with
+    ``grid``): the fine pass stops a ray once its transmittance falls below t.  A ray that never stops is bit for bit
+    the render without it; one that stops moves its rgb and acc by at most t."""
     if randoms is not None and not isinstance(randoms, SeededRandoms):
         raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:
@@ -42,6 +47,9 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
     if grid is not None:
         with torch.no_grad():
             train_utils.check_grid_call(grid, device, model_coarse, model_fine)
+    if early_stop is not None:
+        with torch.no_grad():
+            train_utils.check_early_stop_call(early_stop, model_coarse, model_fine)
     with torch.no_grad():
         rays = ops.gen_rays(tform_cam2world, height, width, focal_length, None, device,
                             ndc=options.dataset.no_ndc is False, near=options.dataset.near, far=options.dataset.far,
@@ -53,7 +61,7 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
             rays[i:i + chunk], model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl, grid=grid,
-            randoms=randoms.shifted(i) if randoms is not None else None)
+            early_stop=early_stop, randoms=randoms.shifted(i) if randoms is not None else None)
             for i in range(0, n, chunk)]
     cols = [torch.cat(c, 0) if c[0] is not None else None for c in zip(*parts)]
     shapes = [(height, width, 3), (height, width), (height, width)] * 2

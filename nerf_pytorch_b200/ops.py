@@ -715,6 +715,61 @@ def render_fwd_grid(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, rand
 
 
 # ------------------------------------------------------------------------------------------------
+# early ray termination (include/nerfb200.h "early ray termination")
+# ------------------------------------------------------------------------------------------------
+def stop_round() -> int:
+    """K: the evaluated samples per ray each round of an early-stopping pass runs (NERFB200_STOP_ROUND)."""
+    return int(_lib.load().nerfb200_render_early_stop_round())
+
+
+def render_early_stop_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int) -> int:
+    lib = _lib.load()
+    af = arch_f.c_struct() if arch_f is not None else None
+    n = lib.nerfb200_render_early_stop_workspace_bytes(C.byref(arch_c.c_struct()),
+                                                       C.byref(af) if af is not None else None, C.byref(opts), n_rays)
+    if n < 0:
+        _lib.check(_lib.ERR_UNSUPPORTED, "render_early_stop_workspace_bytes")
+    return n
+
+
+def render_fwd_early_stop(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid, stop,
+                          impl: int = IMPL_TC, want_stop: bool = False, workspace: Optional[torch.Tensor] = None):
+    """``render_fwd`` for inference (impl 1 or 3) whose last pass stops each ray once its transmittance falls below
+    ``stop`` (0 <= stop < 1), with an occupancy ``grid`` or None.  Returns (out_coarse, out_fine | None, n_evaluated
+    int64[2]) and, with ``want_stop``, the int32 ``stop_sample`` of every ray (the header's definition).  A given
+    ``workspace`` large enough is used; its first sections are laid out as ``render_workspace_layout(...,
+    training=False)``."""
+    lib = _lib.load()
+    n = rays.shape[0]
+    dev = rays.device
+    fine = opts.n_fine > 0
+    g, bits = (None, None)
+    if grid is not None:
+        g, bits = _grid_args(grid)
+        if bits.device != dev:
+            raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
+    need = render_early_stop_workspace_bytes(arch_c, arch_f if fine else None, opts, n)
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
+    n_evaluated = torch.zeros(2, dtype=torch.int64, device=dev)
+    stop_sample = torch.empty(n, dtype=torch.int32, device=dev) if want_stop else None
+    ac = arch_c.c_struct()
+    af = arch_f.c_struct() if fine else None
+    _lib.check(lib.nerfb200_render_fwd_early_stop(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
+                                                  _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays),
+                                                  rays.shape[1], n, *_random_args(randoms),
+                                                  C.byref(g) if g is not None else None, _ptr(bits), float(stop),
+                                                  _ptr(out_c), _ptr(out_f), _ptr(workspace), int(impl),
+                                                  _ptr(n_evaluated), _ptr(stop_sample), _stream()),
+               "render_fwd_early_stop")
+    if want_stop:
+        return out_c, out_f, n_evaluated, stop_sample
+    return out_c, out_f, n_evaluated
+
+
+# ------------------------------------------------------------------------------------------------
 # meshes (include/nerfb200.h "meshes"; nerf_pytorch_b200/mesh.py is the public interface).  The box is a Grid read as
 # res cubes per axis, its lattice the (res + 1) points per axis at the cube corners.
 # ------------------------------------------------------------------------------------------------

@@ -16,6 +16,7 @@ There is no PyTorch fallback: an unsupported model / device / dtype raises.
 from __future__ import annotations
 
 import math
+import numbers
 import weakref
 from typing import Optional, Union
 
@@ -414,6 +415,33 @@ def _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fin
     return impl
 
 
+def check_early_stop_call(early_stop, *models):
+    """The refusals of an early-stopping render that precede any launch: a threshold that is not a number in [0, 1), a
+    call that would train."""
+    if isinstance(early_stop, bool) or not isinstance(early_stop, numbers.Real) or not 0.0 <= float(early_stop) < 1.0:
+        raise ValueError(f"nerfb200: early_stop must be a transmittance threshold in [0, 1), got {early_stop!r}")
+    if _trains(p for m in models if m is not None for p in m.parameters()):
+        raise NotImplementedError("nerfb200: early ray termination renders only (inference); render under "
+                                  "torch.no_grad() or with parameters that do not require grad")
+
+
+def _early_stop_impl(impl, arch_c, arch_f, nc, nf):
+    """The impl an early-stopping render without a grid runs on, after the refusals that precede a launch: impl 0 and an
+    architecture the wgmma inference forward refuses (the library's reason).  With a grid, _grid_impl decides."""
+    if impl is None:
+        impl = _auto_impl(arch_c, arch_f, nc, nf, training=False)
+    if impl == ops.IMPL_SIMT:
+        raise NotImplementedError("nerfb200: early ray termination runs on the wgmma inference forward (impl 1 or 3), "
+                                  "not impl 0 (fp32 CUDA cores)" + "".join(
+                                      f"; {why}" for a, n in ((arch_c, nc), (arch_f, nc + nf)) if a is not None
+                                      for why in [ops.impl_refusal(a, n, ops.IMPL_TC_FWD)] if why))
+    for a, n in ((arch_c, nc), (arch_f, nc + nf)):
+        why = ops.impl_refusal(a, n, ops.IMPL_TC_FWD if impl == ops.IMPL_TC else impl) if a is not None else None
+        if why:
+            raise NotImplementedError(f"nerfb200 early-stopping render: {why}")
+    return impl
+
+
 def predict_and_render_radiance(
     ray_batch,
     model_coarse,
@@ -426,6 +454,7 @@ def predict_and_render_radiance(
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
     grid=None,
+    early_stop: Optional[float] = None,
     _n_chunks: int = 1,
 ):
     """nerf/train_utils.py:28-127 for one chunk of packed rays ``[o d near far (viewdir)]``.
@@ -439,10 +468,16 @@ def predict_and_render_radiance(
     the single-pass fp16 forward and raises ``NotImplementedError`` if the call would train.
 
     ``grid``: an ``OccupancyGrid`` on the rays' device (inference only, impl 1 or 3): samples in its empty cells skip
-    the MLP and get zero density.  None is the path without a grid."""
+    the MLP and get zero density.  None is the path without a grid.
+
+    ``early_stop``: a transmittance threshold t in [0, 1) (inference only, impl 1 or 3, with or without ``grid``): the
+    last pass stops a ray once its transmittance falls below t, so its rgb and acc move by at most t
+    (include/nerfb200.h "early ray termination").  None is the path without it."""
     impl = _requested_impl(impl, model_coarse, model_fine)
     if grid is not None:
         check_grid_call(grid, None, model_coarse, model_fine)
+    if early_stop is not None:
+        check_early_stop_call(early_stop, model_coarse, model_fine)
     o = getattr(options.nerf, mode)
     if not ray_batch.is_cuda:
         raise NotImplementedError("nerfb200: rays must be on a CUDA device (there is no CPU path)")
@@ -460,6 +495,8 @@ def predict_and_render_radiance(
     arch_f = _arch_of(model_fine, enc_xyz, enc_dir) if fine else None
     if grid is not None:
         impl = _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine)
+    elif early_stop is not None:
+        impl = _early_stop_impl(impl, arch_c, arch_f, nc, nf)
     params_c, blob_c = _packed(model_coarse, arch_c)
     params_f, blob_f = _packed(model_fine, arch_f) if fine else ([], None)
     noise_std = float(o.radiance_field_noise_std)
@@ -492,7 +529,10 @@ def predict_and_render_radiance(
     training = _trains(all_params)
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    if grid is not None:
+    if early_stop is not None:
+        out_c, out_f, _ = ops.render_fwd_early_stop(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid,
+                                                    float(early_stop), impl=impl)
+    elif grid is not None:
         out_c, out_f, _ = ops.render_fwd_grid(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid, impl=impl)
     else:
         cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, impl, int(_n_chunks))
@@ -519,6 +559,7 @@ def run_one_iter_of_nerf(
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
     grid=None,
+    early_stop: Optional[float] = None,
 ):
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
@@ -526,6 +567,8 @@ def run_one_iter_of_nerf(
     impl = _requested_impl(impl, model_coarse, model_fine)
     if grid is not None:
         check_grid_call(grid, ray_directions.device, model_coarse, model_fine)
+    if early_stop is not None:
+        check_early_stop_call(early_stop, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     restore_shapes = [ray_directions.shape, ray_directions.shape[:-1], ray_directions.shape[:-1]]
     if model_fine:
@@ -539,7 +582,7 @@ def run_one_iter_of_nerf(
                          options.dataset.far, use_viewdirs)
 
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl, grid)
+                          encode_direction_fn, randoms, impl, grid, early_stop)
 
 
 def run_one_iter_of_nerf_from_pose(
@@ -558,6 +601,7 @@ def run_one_iter_of_nerf_from_pose(
     randoms: Union[dict, SeededRandoms, None] = None,
     impl: Optional[int] = None,
     grid=None,
+    early_stop: Optional[float] = None,
 ):
     """``run_one_iter_of_nerf`` for callers that hold a pose and pixel ids instead of ray tensors (SURVEY.md section 8f-2):
     the reference's training loop builds ALL H*W rays of the image with get_ray_bundle and then indexes the few
@@ -568,17 +612,19 @@ def run_one_iter_of_nerf_from_pose(
     dev = pixel_ids.device if pixel_ids is not None else next(model_coarse.parameters()).device
     if grid is not None:
         check_grid_call(grid, dev, model_coarse, model_fine)
+    if early_stop is not None:
+        check_early_stop_call(early_stop, model_coarse, model_fine)
     use_viewdirs = bool(options.nerf.use_viewdirs)
     rays = ops.gen_rays(tform_cam2world, height, width, focal_length, pixel_ids, dev, ndc=options.dataset.no_ndc is False,
                         near=options.dataset.near, far=options.dataset.far, use_viewdirs=use_viewdirs)
     lead = (height, width) if pixel_ids is None else tuple(pixel_ids.shape)
     restore_shapes = [lead + (3,), lead, lead] * (2 if model_fine else 1)
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl, grid)
+                          encode_direction_fn, randoms, impl, grid, early_stop)
 
 
 def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn, encode_direction_fn,
-                   randoms, impl, grid=None):
+                   randoms, impl, grid=None, early_stop=None):
     """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202.
     Seeded randoms follow each ray: chunk i starts at ``ray_offset`` + the index of its first ray."""
     chunksize = getattr(options.nerf, mode).chunksize
@@ -593,7 +639,7 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if options.nerf.use_viewdirs else None,
             randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, grid=grid,
-            _n_chunks=len(batches),
+            early_stop=early_stop, _n_chunks=len(batches),
         )
         for i, batch in enumerate(batches)
     ]
