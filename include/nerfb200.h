@@ -410,6 +410,47 @@ int32_t nerfb200_mesh_emit(const nerfb200_grid_t* box, const float* volume, floa
                            int64_t max_vertices, int64_t max_faces, float* vertices, int32_t* faces, float* view_dirs,
                            void* stream);
 
+/* ---- density gradient: sigma and its gradient w.r.t. the points (normals, field probes) -------------------------
+ * density_grad: out[P][4] = (sigma_raw, d sigma_raw / dx, d / dy, d / dz) at pts[P][3], P >= 1 and < 2^31.  sigma_raw is
+ *   the network's sigma output before the ReLU (fc_alpha, or column 3 of fc_out without view directions), bit for bit
+ *   what nerfb200_mlp_fwd_pts with impl 1 writes to raw[p][3] at the same point; sigma reads no view direction, so none
+ *   is taken.  The gradient is w.r.t. the coordinates the MLP encodes (world space for Blender scenes, NDC for LLFF):
+ *   the exact chain rule of the trunk (layer1 without, the other trunk layers with their ReLU; a ReLU's derivative is
+ *   1 where its output is nonzero) and of the positional encoding (d sin(f x) = f cos(f x), d cos(f x) = -f sin(f x), the
+ *   argument f x rounded to fp32 as the forward rounds it), each product in the forward's three-term fp16 split with
+ *   fp32 accumulation.  Inference only (no backward); impl 1 alone: impl 0 and 3 are refused.  An operand out of the
+ *   fp16 range gives inf / NaN, not a clamped value.
+ * density_grad_supported: NERFB200_OK if density_grad runs this architecture with `impl`, else the reason (the last
+ *   error), without touching a device.
+ * The surface normal of a level set of sigma is -grad / |grad| (outward: toward lower density). */
+int32_t nerfb200_density_grad_supported(const nerfb200_arch_t* arch, int32_t impl);
+
+/* ---- normal maps: the composited surface normal of an inference render's last pass ------------------------------
+ * render_fwd_normals: render_fwd for inference (training = 0) -- with an occupancy grid when grid / bits are given, and
+ *   with early ray termination of the last pass when stop_transmittance >= 0 (negative: none; NaN is refused) -- whose
+ *   out_coarse / out_fine are bit for bit those of nerfb200_render_fwd, _fwd_grid or _fwd_early_stop on the same
+ *   inputs, plus normals[n_rays][3] of the last pass (the fine pass, or the coarse pass of a coarse-only network):
+ *     n_i = -g_i / |g_i| at the last pass's sample i, g_i = density_grad's gradient at the point o + d z_i formed as the
+ *         MLP forms it; |g| = sqrt((gx * gx + gy * gy) + gz * gz), n_i = 0 where that is 0 (fp32, each op rounded);
+ *     N = sum over the samples with w_i != 0, in sample order, of w_i * n_i (fp32, each op rounded), w_i the weights the
+ *         render's own compositing of that pass computed (with its noise, when noise_std > 0).
+ *   N is not renormalised: |N| <= acc up to rounding, and N = 0 for a ray whose weights are all 0.  The gradient is
+ *   evaluated at the samples with a nonzero weight alone, compacted on the device (no host read); with a grid or early
+ *   stopping every such sample ran the MLP.  impl 1 alone (density_grad's refusal for impl 0 and 3), before any launch.
+ * render_normals_workspace_bytes: bytes of the workspace render_fwd_normals takes (-1 on invalid arguments); its first
+ *   sections are laid out as nerfb200_render_workspace_layout(..., training = 0). */
+int64_t nerfb200_render_normals_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                                const nerfb200_render_opts_t* opts, int64_t n_rays);
+int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                    const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                    const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                    const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                    const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                                    float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
+                                    void* stream);
+int32_t nerfb200_density_grad(const nerfb200_arch_t* arch, const float* blob, const float* pts, int64_t n_points,
+                              float* out, int32_t impl, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

@@ -129,6 +129,10 @@ SIGNATURES = {
     "nerfb200_mesh_lattice_points": (I32, [GP, I32, I32, P, P]),
     "nerfb200_mesh_count": (I32, [GP, P, F32, P, P, P]),
     "nerfb200_mesh_emit": (I32, [GP, P, F32, P, I64, I64, P, P, P, P]),
+    "nerfb200_density_grad_supported": (I32, [AP, I32]),
+    "nerfb200_density_grad": (I32, [AP, P, P, I64, P, I32, P]),
+    "nerfb200_render_normals_workspace_bytes": (I64, [AP, AP, OP, I64]),
+    "nerfb200_render_fwd_normals": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, F32, P, P, P, P, I32, P]),
 }
 
 _lib = None

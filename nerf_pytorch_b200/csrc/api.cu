@@ -244,6 +244,7 @@ enum Need {
   kStash,      // the forward that writes the activation stash a backward reads
   kBackward,   // the backward (its forward has run)
   kHalves,     // the backward as two calls, mlp_dgrad and mlp_wgrad: the fp32 kernels only
+  kGradient,   // the density gradient at points (density_grad): the wgmma kernels only
 };
 
 // The one place that maps an impl code to the kernel families' predicates: 0 the fp32 CUDA cores, 1 wgmma, 3 the
@@ -251,6 +252,11 @@ enum Need {
 // not a family).  A refusal reads "<what> impl=N (<label>): <reason>".
 static int check_impl(const Plan& p, int impl, int n_samples, Need need, const char* what) {
   char who[96];
+  if (need == kGradient && (impl == 0 || impl == 3)) {
+    set_error("%s impl=%d: the density gradient runs on the split-precision wgmma kernels only (impl=1); the %s is not "
+              "differentiated", what, impl, impl == 0 ? "fp32 CUDA-core forward" : "single-pass fp16 forward");
+    return NERFB200_ERR_UNSUPPORTED;
+  }
   switch (impl) {
     case 0:
       snprintf(who, sizeof(who), "%s impl=0 (fp32 CUDA cores)", what);
@@ -261,7 +267,8 @@ static int check_impl(const Plan& p, int impl, int n_samples, Need need, const c
         return NERFB200_ERR_UNSUPPORTED;
       }
       snprintf(who, sizeof(who), "%s impl=1 (wgmma)", what);
-      NB_TRY(tc_supported(p, n_samples, /*training=*/need != kInference, who));
+      NB_TRY(tc_supported(p, n_samples, /*training=*/need != kInference && need != kGradient, who));
+      if (need == kGradient) return grad_tc_supported(p, who);
       return need == kBackward ? bwd_tc_supported(p, who) : NERFB200_OK;
     case 3:
       if (need != kInference) {
@@ -582,6 +589,28 @@ int32_t nerfb200_mlp_fwd_pts(const nerfb200_arch_t* arch, const float* blob, con
                      stash, static_cast<cudaStream_t>(stream));
 }
 
+int32_t nerfb200_density_grad_supported(const nerfb200_arch_t* arch, int32_t impl) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  return check_impl(p, impl, 0, kGradient, "density_grad");
+}
+
+int32_t nerfb200_density_grad(const nerfb200_arch_t* arch, const float* blob, const float* pts, int64_t n_points,
+                              float* out, int32_t impl, void* stream) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  if (!blob || !pts || !out || n_points <= 0) {
+    set_error("density_grad: null pointer or empty input");
+    return NERFB200_ERR_INVALID;
+  }
+  if (n_points >= (int64_t(1) << 31)) {
+    set_error("density_grad: more than 2^31 points in one call; chunk the points");
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  NB_TRY(check_impl(p, impl, 0, kGradient, "density_grad"));
+  return launch_density_grad_tc(p, blob, pts, n_points, out, nullptr, static_cast<cudaStream_t>(stream));
+}
+
 int32_t nerfb200_mlp_bwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* dirs, int32_t dir_stride,
                              int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash, float* gstash,
                              float* flat_grad, int32_t impl, void* stream) {
@@ -774,7 +803,7 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
                           const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
                           const nerfb200_grid_t* grid, const uint32_t* bits, int64_t* n_evaluated, float* out_coarse,
                           float* out_fine, void* workspace, int32_t training, int32_t impl, void* stream,
-                          const StopArgs* stop = nullptr) {
+                          const StopArgs* stop = nullptr, float* last_weights = nullptr) {
   Plan pc, pf;
   NB_TRY(build_plan(arch_c, &pc));
   NB_TRY(check_opts(opts));
@@ -890,9 +919,11 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
     return launch_composite_fwd(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
                                 opts->noise_std, opts->white_bkgd, out, weights, s);
   };
-  NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse, F(w.w_c)));
+  // last_weights (normal maps): the last pass's compositing also writes its weights there
+  NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse,
+              fine || !last_weights ? F(w.w_c) : last_weights));
   if (!fine) return NERFB200_OK;
-  return pass(true, pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), out_fine, nullptr);
+  return pass(true, pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), out_fine, last_weights);
 }
 
 }  // namespace nerfb200
@@ -968,6 +999,105 @@ int32_t nerfb200_render_fwd_early_stop(const nerfb200_arch_t* arch_c, const nerf
   return render_forward("render_fwd_early_stop", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
                         t_rand, noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace,
                         /*training=*/0, impl, stream, &stop);
+}
+
+}  // extern "C"
+
+namespace nerfb200 {
+
+// The sections a normal-map render adds after everything render_forward may use (the grid and early-stopping sections
+// of either layout): the last pass's weights, the compaction's count / first / total, the compacted points and their
+// density_grad output.
+struct NormalWorkspace {
+  int64_t weights, count, first, total, pts, grad, end;
+};
+static int normal_workspace(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                            const nerfb200_render_opts_t* opts, int64_t n_rays, NormalWorkspace* nw) {
+  Plan pc, pf;
+  NB_TRY(build_plan(coarse, &pc));
+  if (fine) NB_TRY(build_plan(fine, &pf));
+  NB_TRY(check_opts(opts));
+  if (n_rays <= 0) {
+    set_error("render_fwd_normals: empty batch");
+    return NERFB200_ERR_INVALID;
+  }
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
+  const bool has_fine = fine && opts->n_fine > 0;
+  const int n_last = has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse;
+  const int64_t a = carve_stop(carve_grid(w.total, n_rays, opts->n_coarse).total, n_rays, n_last).total;
+  const int64_t b = carve_stop(carve_grid(w.total, n_rays, n_last).total, n_rays, n_last).total;
+  const int64_t P = n_rays * n_last;
+  nw->weights = a > b ? a : b;
+  nw->count = nw->weights + align256(P * 4);
+  nw->first = nw->count + align256(n_rays * 4);
+  nw->total = nw->first + align256(n_rays * 4);
+  nw->pts = nw->total + 256;
+  nw->grad = nw->pts + align256(P * 12);
+  nw->end = nw->grad + align256(P * 16);
+  return NERFB200_OK;
+}
+
+}  // namespace nerfb200
+
+extern "C" {
+
+int64_t nerfb200_render_normals_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                                const nerfb200_render_opts_t* opts, int64_t n_rays) {
+  NormalWorkspace nw;
+  if (normal_workspace(coarse, fine, opts, n_rays, &nw) != NERFB200_OK) return -1;
+  return nw.end;
+}
+
+int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                    const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                    const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                    const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                    const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                                    float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
+                                    void* stream) {
+  const char* what = "render_fwd_normals";
+  if ((grid == nullptr) != (bits == nullptr)) {
+    set_error("%s: a grid descriptor and its bits come together", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (stop_transmittance != stop_transmittance) {
+    set_error("%s: stop_transmittance is NaN (negative: no early stopping)", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (!normals || !workspace) {
+    set_error("%s: null normals or workspace", what);
+    return NERFB200_ERR_INVALID;
+  }
+  NB_TRY(check_opts(opts));
+  const bool fine = opts->n_fine > 0;
+  const nerfb200_arch_t* arch_last = fine ? arch_f : arch_c;
+  const float* blob_last = fine ? blob_f : blob_c;
+  Plan pl;
+  NB_TRY(build_plan(arch_last, &pl));
+  NB_TRY(check_impl(pl, impl, 0, kGradient, what));  // impl 1 alone, before any launch
+  NormalWorkspace nw;
+  NB_TRY(normal_workspace(arch_c, fine ? arch_f : nullptr, opts, n_rays, &nw));
+  char* base = static_cast<char*>(workspace);
+  float* W = reinterpret_cast<float*>(base + nw.weights);
+  const StopArgs stop{stop_transmittance, nullptr};
+  NB_TRY(render_forward(what, arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand, noise_c, u,
+                        noise_f, grid, bits, nullptr, out_coarse, out_fine, workspace, /*training=*/0, impl, stream,
+                        stop_transmittance >= 0.f ? &stop : nullptr, W));
+  Plan pc, pf;
+  NB_TRY(build_plan(arch_c, &pc));
+  if (fine) NB_TRY(build_plan(arch_f, &pf));
+  Workspace w;
+  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
+  const int n_last = fine ? opts->n_coarse + opts->n_fine : opts->n_coarse;
+  const float* z_last = reinterpret_cast<const float*>(base + (fine ? w.z_f : w.z_c));
+  const NormalState st{reinterpret_cast<int*>(base + nw.count), reinterpret_cast<int*>(base + nw.first),
+                       reinterpret_cast<int*>(base + nw.total), reinterpret_cast<float*>(base + nw.pts),
+                       reinterpret_cast<float*>(base + nw.grad)};
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  NB_TRY(launch_normal_compact(rays, ray_stride, z_last, W, n_rays, n_last, st, s));
+  NB_TRY(launch_density_grad_tc(pl, blob_last, st.pts, n_rays * n_last, st.grad, st.total, s));
+  return launch_normal_sum(W, n_rays, n_last, st, normals, s);
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,

@@ -197,6 +197,25 @@ int launch_wgrad_simt(const Plan& p, const float* rays, int ray_stride, const fl
 int tc_supported(const Plan& p, int n_samples, bool training, const char* what);
 int launch_mlp_fwd_tc(const Plan& p, const float* blob, const PointSrc& src, int64_t n_rays, int n_samples, float* raw,
                       float* stash, bool fast, cudaStream_t s);
+// density gradient (mlp_tc.cu, nerfb200.h "density gradient"), impl 1 only: sigma_raw and its gradient w.r.t. the points;
+// grad_tc_supported checks what it needs beyond tc_supported(training = false)
+int grad_tc_supported(const Plan& p, const char* what);
+int launch_density_grad_tc(const Plan& p, const float* blob, const float* pts, int64_t n_points, float* out,
+                           const int* n_dev, cudaStream_t s);
+// ---- normal maps of a render's last pass (normals.cu; nerfb200.h "normal maps") ----
+// The samples with nonzero compositing weight, compacted: count[r], first[r] (their first slot), *total; pts[slot][3] =
+// o + d z as the MLP forms it
+struct NormalState {
+  int* count;
+  int* first;
+  int* total;
+  float* pts;
+  float* grad;  // [slot][4], density_grad's output
+};
+int launch_normal_compact(const float* rays, int ray_stride, const float* z, const float* weights, int64_t n_rays,
+                          int n_samples, const NormalState& ns, cudaStream_t s);
+int launch_normal_sum(const float* weights, int64_t n_rays, int n_samples, const NormalState& ns, float* normals,
+                      cudaStream_t s);
 // wgmma backward (mlp_tc_bwd.cu), impl 1: data-gradient chain + every weight gradient in one kernel; `scratch` holds
 // the L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into.
 // bwd_tc_supported checks what it needs beyond tc_supported(training = true).

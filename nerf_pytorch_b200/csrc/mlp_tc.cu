@@ -110,12 +110,17 @@ using namespace tc;
 // 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row r + 8 i, column 8 j + 2 (lane % 4) + c).
 // kStage: bytes of a ring stage.  blk (kTrain): the warpgroup's 64-row block of the batch, whose rows are half blk & 1 of
 // stash tile blk >> 1.
-template <bool kTrain, bool kFast, int N, int kStage>
+// kGrad (the density-gradient kernel's trunk, below): the ReLU bits go to the warpgroup's shared-memory masks s_mask
+// ([64 rows][mask_words], layer e at word g.mask_cum) instead of a stash, and the head writes raw sigma alone, to
+// column 0 of raw.  Every other instance compiles without these paths.
+template <bool kTrain, bool kFast, int N, int kStage, bool kGrad = false>
 __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, float* __restrict__ raw, float* __restrict__ stash,
                                           uint8_t* sm, const SmemMap& mp, int e, int wg, int rows, int64_t blk,
                                           int64_t P_pad, const RowState& rs, WeightRing<kStage>& ring, const float* s_bias,
-                                          const float* s_headw, const float* s_headb, const float* viewb, int hw1) {
+                                          const float* s_headw, const float* s_headb, const float* viewb, int hw1,
+                                          uint32_t* s_mask = nullptr, int mask_words = 0) {
   static_assert(!(kTrain && kFast), "the single-pass forward is inference only");
+  static_assert(!(kGrad && (kTrain || kFast)), "the density gradient runs the split-precision inference trunk");
   // k-steps a ring stage can hold (the unrolled bound; 24 KB stages keep two for every width, mi.sps decides at run time)
   constexpr int kSps = kFast ? fast_sps(kStage, N) : kStage == kStageBytes ? kStepsPerStage : split_sps(kStage, N);
   const int wt = threadIdx.x & 127, wi = wt >> 5, lane = wt & 31, q = lane & 3;
@@ -211,7 +216,7 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
             hacc[i][c] = fmaf(x0, w.x, fmaf(x1, w.y, hacc[i][c]));
           }
       }
-      if (kTrain)  // ReLU bits (Y >= 0 here: Y > 0 <=> a nonzero bit pattern)
+      if (kTrain || kGrad)  // ReLU bits (Y >= 0 here: Y > 0 <=> a nonzero bit pattern)
         mbits[i][j >> 2] |= (min(__float_as_uint(Y0), 1u) | (min(__float_as_uint(Y1), 1u) << 1)) << (8 * (j & 3) + 2 * q);
       if (kFast) {
         if (has_next)
@@ -248,6 +253,18 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
       }
     }
   }
+  if (kGrad) {  // the same bits into this warpgroup's shared-memory masks (row-local; read back by the reverse chain)
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int m = 0; m < N / 32; ++m) {
+        uint32_t w = mbits[i][m];
+        w |= __shfl_xor_sync(0xffffffffu, w, 1);
+        w |= __shfl_xor_sync(0xffffffffu, w, 2);
+        if ((m & 3) == q) s_mask[(16 * wi + (lane >> 2) + 8 * i) * mask_words + g.mask_cum + m] = w;
+      }
+    }
+  }
   if (hsel >= 0) {
     const int hcol = p.h[hsel].out_col;
 #pragma unroll
@@ -257,7 +274,12 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
         hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 1);
         hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 2);
       }
-      if (q == 0 && rs.valid[i])
+      if (kGrad) {  // raw sigma: output column 3 of the trunk's head (fc_alpha, or fc_out without view directions)
+        if (q == 0 && rs.valid[i])
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            if (c < hn && hcol + c == 3) raw[(int64_t)rs.pt[i] * 4] = hacc[i][c] + s_headb[hsel * 4 + c];
+      } else if (q == 0 && rs.valid[i])
         for (int c = 0; c < hn; ++c) raw[(int64_t)rs.pt[i] * 4 + hcol + c] = hacc[i][c] + s_headb[hsel * 4 + c];
     }
   }
@@ -536,6 +558,371 @@ int launch_mlp_fwd_tc(const Plan& p, const float* blob, const PointSrc& src, int
   if (fast)
     return go(p.hidden == 256 ? launch_fwd<false, 256, true> : launch_fwd<false, 128, true>, "mlp_fwd_tc_fast launch");
   return go(p.hidden == 256 ? launch_fwd<false, 256, false> : launch_fwd<false, 128, false>, "mlp_fwd_tc launch");
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------
+// Density gradient (nerfb200.h "density gradient"): sigma_raw and d sigma_raw / d x at a flat list of points, x in the
+// coordinates the MLP encodes.  A kernel of its own beside mlp_fwd_tc_kernel, so that the forward's instances stay as
+// they are: its trunk is fwd_layer<..., kGrad> (the forward's encoding, operand split, MMAs and epilogue, so sigma has
+// the forward's bits), which keeps each layer's ReLU bits in shared memory.  Then, per 64-row block, the reverse chain
+//     G_{L-1} = w_sigma (.) mask_{L-1},    G_{t-1} = (G_t W_t[:, :H]) (.) mask_{t-1}     (layer1 has no ReLU: no mask)
+// on wgmma with the three-term split -- A = G_t / 16, split hi / lo into the activation tile's place; B = the blob's
+// transposed dgrad copies (tcd_off), as the fused backward's chain_mma reads them -- and the encoding gradient
+//     d_enc = sum over the layers that read the xyz encoding (layer1, the skip layers) of G_t W_t[:, enc]
+// against the forward's own weight copies read MN-major: one 16-column k-step of the encoding per ring stage, N = 16
+// MMAs into register accumulators that live through the chain.  The epilogue takes d_enc through the positional
+// encoding to x.  No view direction, fc_feat, layers_dir or fc_rgb runs; HBM traffic is the points in and 16 B out.
+// ---------------------------------------------------------------------------------------------------------------
+namespace tc {
+// consumer warpgroups: two at hidden 128 (the chain accumulator and the encoding-gradient accumulators are live
+// together, which the 128 registers per thread of three warpgroups do not hold), one at 256
+__host__ __device__ constexpr int grad_wg(int hidden) { return hidden == 128 ? 2 : 1; }
+constexpr int kMaxEncSteps = 4;  // 16-column k-steps of the xyz encoding (tc_supported: at most 64 wide)
+
+struct GradSmemMap {
+  SmemMap m;       // act (the G tile once the trunk has run), enc, bias, headw, bars and ring, as fwd_layer reads them
+  int mask;        // the trunk's ReLU bits: [warpgroup][64 rows][mask_words]
+  int mask_words;  // per row: the sum over the trunk of n / 32
+};
+__host__ __device__ inline GradSmemMap grad_smem_map(const Plan& p) {
+  GradSmemMap gm;
+  SmemMap& m = gm.m;
+  const int rows = 64 * grad_wg(p.hidden);
+  gm.mask_words = 0;
+  for (int t = 0; t < p.n_trunk; ++t) gm.mask_words += p.g[t].n / 32;
+  m.act = 0;
+  int off = rows * p.hidden * 4;
+  m.enc = off;    off += rows * 64 * 4;
+  m.bias = off;   off += p.enc_cum[0] * 4;
+  m.headw = off;  off += (4 * p.hidden + 3 * (p.hidden / 2) + 16) * 4;
+  gm.mask = off;  off += rows * gm.mask_words * 4;
+  m.viewb = m.encd = m.wv = 0;  // no view directions
+  m.bars = off;   off += 256;
+  m.ring = (off + 1023) & ~1023;
+  m.n_stages = ring_depth(m.ring, kStageBytes);
+  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * kStageBytes;
+  return gm;
+}
+}  // namespace tc
+
+// G_t of this thread's fragment (y at the accumulator's 2^11 scale, G / 16) (.) the ReLU bits of layer t (none without
+// a ReLU) -> hi / lo -> the warpgroup's rows of the activation tile, the K-major A operand of the next MMAs.
+// mrow[i]: the mask row of accumulator row i; r0: tile row of accumulator row 0.
+template <int N>
+__device__ __forceinline__ void grad_g_store(const Plan& p, const float (&y)[N / 2], int t, uint8_t* act, int rows,
+                                             const uint32_t* const (&mrow)[2], int r0) {
+  const int q = threadIdx.x & 3;
+  const GemmLayer& g = p.g[t];
+  const int act_lo = rows * N * 2;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const uint32_t word = g.relu ? mrow[i][g.mask_cum + (j >> 2)] : 0xFFFFFFFFu;
+      const int bit = 8 * (j & 3) + 2 * q;
+      const float Y0 = (word & (1u << bit)) ? y[4 * j + 2 * i] : 0.f;
+      const float Y1 = (word & (2u << bit)) ? y[4 * j + 2 * i + 1] : 0.f;
+      uint32_t hi, lo;
+      split_f16x2_y(Y0, Y1, Y0 * kLoInv, Y1 * kLoInv, hi, lo);
+      const int off = tile_piece(r0 + 8 * i, j, N) + q * 4;
+      *reinterpret_cast<uint32_t*>(act + off) = hi;
+      *reinterpret_cast<uint32_t*>(act + act_lo + off) = lo;
+    }
+  }
+}
+
+// acc = 2^11 G_t W_t[:, :N] of this warpgroup's rows: A = the G tile (a_hi, lo block a_lo_off on), B = layer t's tcd
+// copy, one k-step (16 n x all N columns: [hs | h | l][slab 0 | 1][k][8 n]) per ring stage
+template <int N, int kStage>
+__device__ __forceinline__ void grad_chain_mma(float (&acc)[N / 2], WeightRing<kStage>& ring, uint64_t a_hi,
+                                               uint32_t a_lo_off) {
+  const uint32_t slab = 16u * N;
+  const uint64_t b_ring = make_desc(ring.base, slab, 128);
+  wgmma_fence();
+#pragma unroll 1
+  for (int ks = 0; ks < N / 16; ++ks) {
+    const uint32_t st = ring.acquire();
+    const uint64_t b = desc_adv(b_ring, st * (uint32_t)kStage);
+    const uint64_t ah = desc_adv(a_hi, (uint32_t)ks * 256u);
+    wgmma_f16<N>(acc, ah, b, ks > 0 ? 1 : 0);
+    wgmma_f16<N>(acc, desc_adv(ah, a_lo_off), desc_adv(b, 2 * slab), 1);
+    wgmma_f16<N>(acc, ah, desc_adv(b, 4 * slab), 1);
+    wgmma_commit();
+    ring.release_behind(acc);
+  }
+  ring.release_last(acc);
+}
+
+// acc_e[c] += 2^11 G_t W_t[:, k_h + 16 c .. + 16] for the nch encoding k-steps of layer t: B = the forward copy's k-step
+// k_h / 16 + c ([hs | h | l][slab 0 | 1][n][8 k]) read MN-major -- the n rows are K (8-deep groups 128 B apart), the
+// two slabs the two 8-wide column groups (16 N bytes apart)
+template <int N, int kStage>
+__device__ __forceinline__ void grad_enc_mma(float (&acc_e)[kMaxEncSteps][8], WeightRing<kStage>& ring, uint64_t a_hi,
+                                             uint32_t a_lo_off, int nch) {
+  const uint32_t slab = 16u * N;
+  const uint64_t b_ring = make_desc(ring.base, 128, slab);
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < kMaxEncSteps; ++c) {
+    if (c < nch) {
+      const uint32_t st = ring.acquire();
+      const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStage);
+#pragma unroll 4
+      for (int ks = 0; ks < N / 16; ++ks) {
+        const uint64_t ah = desc_adv(a_hi, (uint32_t)ks * 256u), b = desc_adv(b_st, (uint32_t)ks * 256u);
+        wgmma_f16<16, 0, 1>(acc_e[c], ah, b, 1);
+        wgmma_f16<16, 0, 1>(acc_e[c], desc_adv(ah, a_lo_off), desc_adv(b, 2 * slab), 1);
+        wgmma_f16<16, 0, 1>(acc_e[c], ah, desc_adv(b, 4 * slab), 1);
+      }
+      wgmma_commit();
+      ring.release_behind(acc_e[c]);
+    }
+  }
+  ring.release_last(acc_e[0]);  // waits for every group; the other chunks are fenced before they are read
+}
+
+// d_enc (acc_e: 2^11 / 16 times its value) -> d sigma / d x of this thread's two rows through the positional encoding
+// (x itself, then f cos(f x) and -f sin(f x) per band, the bands' arguments rounded as the forward rounds them),
+// summed over the quad and written beside sigma
+__device__ __forceinline__ void grad_x_store(const Plan& p, const float (&acc_e)[kMaxEncSteps][8], int nch,
+                                             const float* __restrict__ pts, float* __restrict__ out, const RowState& rs) {
+  const int q = threadIdx.x & 3;
+  const int base = p.inc_xyz ? 3 : 0;
+  float x[2][3], gx[2][3];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      x[i][c] = pts[(int64_t)rs.pt[i] * 3 + c];
+      gx[i][c] = 0.f;
+    }
+#pragma unroll
+  for (int ch = 0; ch < kMaxEncSteps; ++ch) {
+    if (ch < nch) {
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+          const int k = 16 * ch + 8 * j + 2 * q + cc;
+          if (k < p.dim_xyz) {
+            const int kk = k - base, f = kk >= 0 ? kk / 6 : 0, r = kk - 6 * f;
+            const int co = k < base ? k : (r >= 3 ? r - 3 : r);
+            const float fr = p.freq_xyz[f];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const float d = acc_e[ch][4 * j + 2 * i + cc] * (kActInv * kLoInv);
+              const float xc = co == 0 ? x[i][0] : co == 1 ? x[i][1] : x[i][2];
+              float v = d;
+              if (k >= base) {
+                float sn, cs;
+                sincosf(__fmul_rn(xc, fr), &sn, &cs);
+                v = r < 3 ? d * fr * cs : -(d * fr * sn);
+              }
+              gx[i][0] += co == 0 ? v : 0.f;
+              gx[i][1] += co == 1 ? v : 0.f;
+              gx[i][2] += co == 2 ? v : 0.f;
+            }
+          }
+        }
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      gx[i][c] += __shfl_xor_sync(0xffffffffu, gx[i][c], 1);
+      gx[i][c] += __shfl_xor_sync(0xffffffffu, gx[i][c], 2);
+    }
+    if (q == 0 && rs.valid[i])
+#pragma unroll
+      for (int c = 0; c < 3; ++c) out[(int64_t)rs.pt[i] * 4 + 1 + c] = gx[i][c];
+  }
+}
+
+template <int kH>
+__global__ void __launch_bounds__(128 * grad_wg(kH) + 32, 1)
+density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob, const float* __restrict__ pts,
+                       int64_t P, int64_t n_tiles, float* __restrict__ out,  // out [P][4] = sigma_raw, d/dx, d/dy, d/dz
+                       const int* __restrict__ n_dev) {  // non-null: the point count in device memory (at most P)
+  constexpr int kWG = grad_wg(kH), kRows = 64 * kWG, kThreads = 128 * kWG + 32, kStage = kStageBytes;
+  using Ring = WeightRing<kStage>;
+  uint8_t* sm = smem_base();
+  const GradSmemMap gm = grad_smem_map(p);
+  const SmemMap& mp = gm.m;
+  float* s_bias = reinterpret_cast<float*>(sm + mp.bias);
+  float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
+  Ring ring{smem_u32(sm + mp.ring), smem_u32(sm + mp.bars), (uint32_t)mp.n_stages};
+
+  const int tid = threadIdx.x;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
+  const int enc_w = p.enc_tile_w;
+  const int L = p.n_trunk;
+
+  if (tid == 0) {
+    ring.init(4 * kWG);
+    fence_barrier_init();
+  }
+  // the trunk's biases and the sigma head, scaled as mlp_fwd_tc_kernel scales them
+  for (int gi = 0; gi < L; ++gi)
+    for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
+  const int hw1 = p.h[0].n_out * p.h[0].k;
+  for (int i = tid; i < hw1; i += kThreads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
+  float* s_headb = s_headw + ((hw1 + 3) & ~3);
+  if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
+  __syncthreads();
+
+  if (n_dev) {
+    P = *n_dev;
+    n_tiles = (P + kRows - 1) / kRows;
+  }
+  const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
+
+  if (warp == 4 * kWG) {
+    // ===================== weight producer: the trunk forward's copies, then per layer from the last: the encoding
+    // k-steps of its forward copy (layers that read the encoding), its tcd copy (layers after layer1) =============
+    if ((tid & 31) == 0) {
+      const uint64_t pol = l2_policy_evict_last();
+      for (int j = 0; j < my_tiles; ++j) {
+        for (int e = 0; e < L; ++e) {
+          const MmaInfo mi = mma_info(p, blob, e, false, kStage);
+          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
+            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
+            ring.fill(mi.src + (size_t)ks * mi.kbytes, 1, nk * mi.kbytes, 0, pol);
+          }
+        }
+        for (int t = L - 1; t >= 0; --t) {
+          const GemmLayer& g = p.g[t];
+          if (g.k_enc > 0 && g.enc_sel == 0) {
+            const MmaInfo mi = mma_info(p, blob, t, false, kStage);
+            for (int ks = mi.ksteps_h; ks < mi.ksteps; ++ks) ring.fill(mi.src + (size_t)ks * mi.kbytes, 1, mi.kbytes, 0, pol);
+          }
+          if (t > 0) {
+            const uint8_t* src = reinterpret_cast<const uint8_t*>(blob + g.tcd_off);
+            const uint32_t kbytes = 96u * (uint32_t)g.k_h;
+            for (int ks = 0; ks < (g.n >> 4); ++ks) ring.fill(src + (size_t)ks * kbytes, 1, kbytes, 0, pol);
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
+    const int wg = warp >> 2, wt = tid & 127, lane = tid & 31;
+    const int row = wt & 63, half = wt >> 6;  // prologue: two threads per row split the frequencies
+    uint8_t* act = sm + mp.act;
+    uint8_t* enc = sm + mp.enc;
+    const int enc_hb = kRows * enc_w * 2;
+    uint32_t* s_mask = reinterpret_cast<uint32_t*>(sm + gm.mask) + wg * 64 * gm.mask_words;
+    const int lr0 = 16 * (wt >> 5) + (lane >> 2);  // warpgroup row of accumulator row 0 (row 1: + 8)
+    const uint32_t* const mrow[2] = {s_mask + lr0 * gm.mask_words, s_mask + (lr0 + 8) * gm.mask_words};
+    const uint64_t g_hi = make_desc(smem_u32(act) + (uint32_t)(wg * 64 * kH * 2), 128, kH * 16);
+    const uint32_t g_lo_off = (uint32_t)(kRows * kH * 2);
+    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
+#pragma unroll 1
+    for (int j = 0; j < my_tiles; ++j) {
+      const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
+      const int64_t p0 = tile * kRows + 64 * wg;
+      const RowState rs = row_state(p0, lr0, P, 1, 0);
+      // ---- encodings of this row -> operand tile (value / 16), as mlp_fwd_tc_kernel's prologue writes them for pts
+      {
+        const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
+        const int nf = p.n_freq_xyz, mid = nf >> 1;
+        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
+        const int base = p.inc_xyz ? 3 : 0;
+        const int trow = 64 * wg + row;
+        auto put = [&](int k, float v) {
+          uint32_t hi, lo;
+          split_f16x2(v * kActScale, 0.f, hi, lo);
+          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
+          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
+          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
+        };
+        for (int c = 0; c < 3; ++c) {
+          const float x = pts[pt * 3 + c];
+          if (p.inc_xyz && half == 0) put(c, x);
+          for (int f = f0; f < f1; ++f) {
+            float sn, cs;
+            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
+            put(base + 6 * f + c, sn);
+            put(base + 6 * f + 3 + c, cs);
+          }
+        }
+        if (half == 1)
+          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+      }
+      fence_proxy_async();
+      wg_bar();
+      // ---- the trunk: sigma_raw -> out[pt][0], the ReLU bits -> s_mask
+#pragma unroll 1
+      for (int e = 0; e < L; ++e)
+        fwd_layer<false, false, kH, kStage, true>(p, blob, out, nullptr, sm, mp, e, wg, kRows, 0, 0, rs, ring, s_bias,
+                                                  s_headw, s_headb, nullptr, hw1, s_mask, gm.mask_words);
+      wg_bar();  // the last layer's bits are in place
+      // ---- the reverse chain from G_{L-1} = w_sigma (.) mask_{L-1}, stored / 16 (s_headw holds 16 w: Y = 8 s_headw)
+      float chain[kH / 2];
+      {
+        const float* wsig = s_headw + (3 - p.h[0].out_col) * p.h[0].k;
+        const int q = tid & 3;
+#pragma unroll
+        for (int jj = 0; jj < kH / 8; ++jj)
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            chain[4 * jj + 2 * i] = wsig[8 * jj + 2 * q] * 8.f;
+            chain[4 * jj + 2 * i + 1] = wsig[8 * jj + 2 * q + 1] * 8.f;
+          }
+      }
+      grad_g_store<kH>(p, chain, L - 1, act, kRows, mrow, 64 * wg + lr0);
+      float acc_e[kMaxEncSteps][8];
+#pragma unroll
+      for (int c = 0; c < kMaxEncSteps; ++c)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc_e[c][i] = 0.f;
+      int nch = 0;
+#pragma unroll 1
+      for (int t = L - 1; t >= 0; --t) {
+        fence_proxy_async();  // generic-proxy stores of G_t -> the MMAs read them through the async proxy
+        wg_bar();
+        const GemmLayer& g = p.g[t];
+        if (g.k_enc > 0 && g.enc_sel == 0) {
+          nch = ((g.k_tc + 15) >> 4) - (g.k_h >> 4);
+          grad_enc_mma<kH, kStage>(acc_e, ring, g_hi, g_lo_off, nch);
+        }
+        if (t > 0) {
+          grad_chain_mma<kH, kStage>(chain, ring, g_hi, g_lo_off);
+          wg_bar();  // every warp's MMAs have read G_t
+          grad_g_store<kH>(p, chain, t - 1, act, kRows, mrow, 64 * wg + lr0);
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < kMaxEncSteps; ++c) reg_fence(acc_e[c]);
+      grad_x_store(p, acc_e, nch, pts, out, rs);
+    }
+  }
+}
+
+// what the density gradient needs beyond the wgmma inference forward (tc_supported); `what` names the call and the impl
+int grad_tc_supported(const Plan& p, const char* what) {
+  if (grad_smem_map(p).m.n_stages < 2) {
+    set_error("%s: network too deep for the density gradient's shared-memory budget (%d trunk layers)", what, p.n_trunk);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  return NERFB200_OK;
+}
+
+template <int kH>
+static int launch_grad(const Plan& p, const float* blob, const float* pts, int64_t P, float* out, const int* n_dev,
+                       cudaStream_t s) {
+  constexpr int kRows = 64 * grad_wg(kH), kThreads = 2 * kRows + 32;
+  const int64_t tiles = (P + kRows - 1) / kRows;
+  return launch_persistent(density_grad_tc_kernel<kH>, tiles, kThreads, grad_smem_map(p).m.total, s, "density_grad launch",
+                           p, blob, pts, P, tiles, out, n_dev);
+}
+
+// n_dev non-null: the kernel reads the point count there (at most n_points, which sizes the grid)
+int launch_density_grad_tc(const Plan& p, const float* blob, const float* pts, int64_t n_points, float* out,
+                           const int* n_dev, cudaStream_t s) {
+  return p.hidden == 256 ? launch_grad<256>(p, blob, pts, n_points, out, n_dev, s)
+                         : launch_grad<128>(p, blob, pts, n_points, out, n_dev, s);
 }
 
 }  // namespace nerfb200

@@ -19,6 +19,7 @@ __device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t a, uint64_
                : NB_F8(0) : "l"(a), "l"(b), "r"(scale_d))
 template <> __device__ __forceinline__ void wgmma_f16<16, 0, 0>(float (&d)[8], uint64_t a, uint64_t b, int scale_d) { NB_WGMMA_16(0, 0); }
 template <> __device__ __forceinline__ void wgmma_f16<16, 1, 1>(float (&d)[8], uint64_t a, uint64_t b, int scale_d) { NB_WGMMA_16(1, 1); }
+template <> __device__ __forceinline__ void wgmma_f16<16, 0, 1>(float (&d)[8], uint64_t a, uint64_t b, int scale_d) { NB_WGMMA_16(0, 1); }
 #undef NB_WGMMA_16
 #define NB_WGMMA_32(TA, TB)                                                                         \
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\nwgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "    \

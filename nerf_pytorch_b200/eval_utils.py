@@ -18,7 +18,7 @@ from .ops import SeededRandoms
 def render_image(height, width, focal_length, tform_cam2world, model_coarse, model_fine, options, mode="validation",
                  encode_position_fn=None, encode_direction_fn=None, *, rays_per_chunk: Optional[int] = None,
                  device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None, grid=None,
-                 early_stop: Optional[float] = None):
+                 early_stop: Optional[float] = None, normals: bool = False):
     """One pose -> (rgb_coarse (H,W,3), disp_coarse (H,W), acc_coarse (H,W), rgb_fine, disp_fine, acc_fine).
 
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
@@ -38,7 +38,12 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
 
     ``early_stop``: a transmittance threshold t in [0, 1) (INTEGRATION.md, "Optional fast paths"; combines with
     ``grid``): the fine pass stops a ray once its transmittance falls below t.  A ray that never stops is bit for bit
-    the render without it; one that stops moves its rgb and acc by at most t."""
+    the render without it; one that stops moves its rgb and acc by at most t.
+
+    ``normals=True`` (impl 1, inference; combines with ``grid`` and ``early_stop``) returns a seventh output, the normal
+    map (H, W, 3) of the last pass: the compositing weights times the outward unit normals -grad sigma / |grad sigma| at
+    its samples, summed per ray and not renormalised (include/nerfb200.h "normal maps"); ``cast_to_normal_image``
+    turns it into uint8.  The six other outputs are exactly those of the call without it."""
     if randoms is not None and not isinstance(randoms, SeededRandoms):
         raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:
@@ -61,16 +66,23 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
             rays[i:i + chunk], model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl, grid=grid,
-            early_stop=early_stop, randoms=randoms.shifted(i) if randoms is not None else None)
+            early_stop=early_stop, normals=normals, randoms=randoms.shifted(i) if randoms is not None else None)
             for i in range(0, n, chunk)]
     cols = [torch.cat(c, 0) if c[0] is not None else None for c in zip(*parts)]
-    shapes = [(height, width, 3), (height, width), (height, width)] * 2
+    shapes = [(height, width, 3), (height, width), (height, width)] * 2 + [(height, width, 3)]
     return tuple(c.view(s) if c is not None else None for c, s in zip(cols, shapes))
 
 
 def cast_to_image(rgb: torch.Tensor) -> torch.Tensor:
     """eval_nerf.py:23-30: (H, W, 3) floats in [0, 1] -> uint8 (H, W, 3) the way ToPILImage does it (x * 255, truncated)."""
     return rgb[..., :3].mul(255).clamp(0, 255).to(torch.uint8)
+
+
+def cast_to_normal_image(normals: torch.Tensor) -> torch.Tensor:
+    """A normal map (..., 3) with components in [-1, 1] -> uint8 (..., 3): (N * 0.5 + 0.5) * 255, converted as
+    ``cast_to_image`` converts."""
+    img = (normals.detach() * 0.5 + 0.5) * 255
+    return img.clamp(0, 255).to(torch.uint8)
 
 
 def cast_to_disparity_image(disp: torch.Tensor) -> torch.Tensor:

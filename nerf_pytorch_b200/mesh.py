@@ -48,27 +48,35 @@ def _level(level):
 
 class Mesh:
     """A triangle mesh on the device: ``vertices`` (V, 3) fp32, ``faces`` (F, 3) int32 vertex ids, counter-clockwise
-    seen from outside (where density <= level), and ``colors`` (V, 3) fp32 in [0, 1] or None."""
+    seen from outside (where density <= level), ``colors`` (V, 3) fp32 in [0, 1] or None, and ``normals`` (V, 3) fp32
+    outward unit normals or None."""
 
-    def __init__(self, vertices: torch.Tensor, faces: torch.Tensor, colors: Optional[torch.Tensor] = None):
+    def __init__(self, vertices: torch.Tensor, faces: torch.Tensor, colors: Optional[torch.Tensor] = None,
+                 normals: Optional[torch.Tensor] = None):
         self.vertices = vertices
         self.faces = faces
         self.colors = colors
+        self.normals = normals
 
     def __repr__(self):
         return (f"Mesh({self.vertices.shape[0]} vertices, {self.faces.shape[0]} faces"
-                f"{', colors' if self.colors is not None else ''})")
+                f"{', colors' if self.colors is not None else ''}{', normals' if self.normals is not None else ''})")
 
     def save_ply(self, path) -> None:
-        """Binary little-endian PLY: float x y z (and uchar red green blue when colored), faces as uchar-counted int
-        lists.  Written on the host with numpy."""
+        """Binary little-endian PLY: float x y z (then float nx ny nz with normals, and uchar red green blue when
+        colored), faces as uchar-counted int lists.  Written on the host with numpy."""
         v = self.vertices.detach().cpu().numpy().astype("<f4")
         f = self.faces.detach().cpu().numpy().astype("<i4")
         fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+        if self.normals is not None:
+            fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
         if self.colors is not None:
             fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
         vrec = np.empty(v.shape[0], dtype=fields)
         vrec["x"], vrec["y"], vrec["z"] = v[:, 0], v[:, 1], v[:, 2]
+        if self.normals is not None:
+            n = self.normals.detach().cpu().numpy().astype("<f4")
+            vrec["nx"], vrec["ny"], vrec["nz"] = n[:, 0], n[:, 1], n[:, 2]
         if self.colors is not None:
             c = np.clip(np.rint(self.colors.detach().cpu().numpy() * 255.0), 0, 255).astype("u1")
             vrec["red"], vrec["green"], vrec["blue"] = c[:, 0], c[:, 1], c[:, 2]
@@ -77,6 +85,8 @@ class Mesh:
         frec["v"] = f
         head = ["ply", "format binary_little_endian 1.0", f"element vertex {v.shape[0]}",
                 "property float x", "property float y", "property float z"]
+        if self.normals is not None:
+            head += ["property float nx", "property float ny", "property float nz"]
         if self.colors is not None:
             head += ["property uchar red", "property uchar green", "property uchar blue"]
         head += [f"element face {f.shape[0]}", "property list uchar int vertex_indices", "end_header"]
@@ -177,7 +187,7 @@ def density_volume(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), 
 
 def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), resolution=256, level: float = 50.0,
                  encode_direction_fn=None, colors: bool = False, impl: Optional[int] = None, *,
-                 planes_per_slab: Optional[int] = None) -> Mesh:
+                 planes_per_slab: Optional[int] = None, normals: bool = False) -> Mesh:
     """The level set sigma = ``level`` of a trained FlexibleNeRFModel over ``bounds``, by marching cubes on the GPU.
 
     The density is ``density_volume(model, ...)`` (the fused MLP at the (R + 1)^3 lattice points); inside is
@@ -186,13 +196,17 @@ def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), re
     direction of a ray reaching it head-on from outside: the normalised density gradient (-n for the outward normal n;
     +z where the gradient vanishes), from central differences of the volume at the edge's two lattice points,
     interpolated along the edge.  That query has one sample per vertex, below the wgmma forward's minimum, so it runs on
-    the fp32 kernels.  Argument errors raise ValueError, an unsupported model or device NotImplementedError, before any
-    launch."""
+    the fp32 kernels.  ``normals=True`` sets ``Mesh.normals``: the outward unit normal -grad / |grad| of the density at
+    each vertex, from the analytic gradient of ``density_gradient`` (impl 1 whatever ``impl`` the lattice query ran
+    on; (0, 0, 0) where the gradient vanishes).  Argument errors raise ValueError, an unsupported model or device
+    NotImplementedError, before any launch."""
     from . import train_utils
+    from . import density
 
     lo, hi, res = _box(bounds, resolution)
     level = _level(level)
     arch = _network(model, encode_position_fn, encode_direction_fn)
+    grad_impl = density.refusal(arch, None) if normals else None
     vol = density_volume(model, encode_position_fn, (lo, hi), res, encode_direction_fn=encode_direction_fn, impl=impl,
                          planes_per_slab=planes_per_slab)
     box = ops.grid_struct((lo, hi), res)
@@ -207,4 +221,10 @@ def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), re
             with torch.no_grad():
                 raw = ops.mlp_fwd_pts(arch, blob, verts.view(-1, 1, 3), dirs, impl=use)
             rgb = torch.sigmoid(raw.view(-1, 4)[:, :3])
-    return Mesh(verts, faces, rgb)
+    nrm = None
+    if normals:
+        _, blob = train_utils._packed(model, arch)
+        _, g = density.density_grad_points(arch, blob, verts, grad_impl)
+        norm = torch.linalg.vector_norm(g, dim=-1, keepdim=True)
+        nrm = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
+    return Mesh(verts, faces, rgb, nrm)

@@ -347,6 +347,26 @@ def mlp_fwd_pts(arch: ArchSpec, blob, pts, dirs, impl=IMPL_SIMT, want_stash=Fals
     return (raw, stash) if want_stash else raw
 
 
+def density_grad_refusal(arch: ArchSpec, impl: int = IMPL_TC) -> Optional[str]:
+    """None when ``density_grad`` runs ``arch`` with ``impl``, else the library's reason (no device is touched)."""
+    lib = _lib.load()
+    if lib.nerfb200_density_grad_supported(C.byref(arch.c_struct()), int(impl)) == _lib.OK:
+        return None
+    return lib.nerfb200_last_error().decode(errors="replace")
+
+
+def density_grad(arch: ArchSpec, blob, pts, impl=IMPL_TC):
+    """(P, 4) = (sigma_raw, d sigma_raw / dx, dy, dz) at ``pts`` (P, 3), P >= 1 (include/nerfb200.h, "density
+    gradient")."""
+    lib = _lib.load()
+    if pts.dim() != 2 or pts.shape[1] != 3:
+        raise RuntimeError(f"nerfb200: density_grad takes points (P, 3), got {tuple(pts.shape)}")
+    out = torch.empty(pts.shape[0], 4, dtype=torch.float32, device=pts.device)
+    _lib.check(lib.nerfb200_density_grad(C.byref(arch.c_struct()), _ptr(blob), _ptr(pts), pts.shape[0], _ptr(out),
+                                         int(impl), _stream()), "density_grad")
+    return out
+
+
 def mlp_bwd_pts(arch: ArchSpec, blob, dirs, d_raw, stash, impl=IMPL_SIMT, flat_grad=None):
     """Backward of ``mlp_fwd_pts`` w.r.t. the parameters, accumulated into ``flat_grad`` (a fresh zero vector when
     None); ``d_raw`` (n_rays, n_samples, 4).  Returns flat_grad."""
@@ -730,6 +750,40 @@ def render_early_stop_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: 
     if n < 0:
         _lib.check(_lib.ERR_UNSUPPORTED, "render_early_stop_workspace_bytes")
     return n
+
+
+def render_fwd_normals(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid=None,
+                       stop: Optional[float] = None, impl: int = IMPL_TC):
+    """Inference ``render_fwd`` (with an occupancy ``grid`` and / or early stopping at ``stop`` when given) that also
+    returns the normal map of the last pass (include/nerfb200.h, "normal maps").  Returns (out_coarse, out_fine | None,
+    normals[N, 3], workspace); the workspace's first sections are laid out as ``render_workspace_layout(...,
+    training=False)``."""
+    lib = _lib.load()
+    n = rays.shape[0]
+    dev = rays.device
+    fine = opts.n_fine > 0
+    g, bits = (None, None)
+    if grid is not None:
+        g, bits = _grid_args(grid)
+        if bits.device != dev:
+            raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
+    ac = arch_c.c_struct()
+    af = arch_f.c_struct() if fine else None
+    need = lib.nerfb200_render_normals_workspace_bytes(C.byref(ac), C.byref(af) if af is not None else None,
+                                                       C.byref(opts), n)
+    if need < 0:
+        _lib.check(_lib.ERR_UNSUPPORTED, "render_normals_workspace_bytes")
+    workspace = torch.empty(need, dtype=torch.uint8, device=dev)
+    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
+    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
+    normals = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    _lib.check(lib.nerfb200_render_fwd_normals(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
+                                               _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
+                                               n, *_random_args(randoms), C.byref(g) if g is not None else None,
+                                               _ptr(bits), -1.0 if stop is None else float(stop), _ptr(out_c),
+                                               _ptr(out_f), _ptr(normals), _ptr(workspace), int(impl), _stream()),
+               "render_fwd_normals")
+    return out_c, out_f, normals, workspace
 
 
 def render_fwd_early_stop(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid, stop,

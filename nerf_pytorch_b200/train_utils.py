@@ -442,6 +442,27 @@ def _early_stop_impl(impl, arch_c, arch_f, nc, nf):
     return impl
 
 
+def check_normals_call(impl, *models):
+    """The refusals of a normal-map render that need no architecture: a call that would train, impl 0 or 3."""
+    if _trains(p for m in models if m is not None for p in m.parameters()):
+        raise NotImplementedError("nerfb200: normal maps render only (inference); render under torch.no_grad() or with "
+                                  "parameters that do not require grad")
+    if impl is not None and int(impl) != ops.IMPL_TC:
+        raise NotImplementedError(f"nerfb200: normal maps run on the wgmma kernels (impl 1), not impl={int(impl)}: the "
+                                  "density gradient is built for impl 1 alone")
+
+
+def _normals_impl(impl, arch_c, arch_f, nc, nf):
+    """impl 1, after the library's refusal of the last pass's density gradient (the render's own come from the library
+    before its first launch)."""
+    impl = ops.IMPL_TC if impl is None else int(impl)
+    last = arch_f if nf > 0 else arch_c
+    why = ops.density_grad_refusal(last, impl)
+    if why:
+        raise NotImplementedError(f"nerfb200 normal-map render: {why}")
+    return impl
+
+
 def predict_and_render_radiance(
     ray_batch,
     model_coarse,
@@ -455,6 +476,7 @@ def predict_and_render_radiance(
     impl: Optional[int] = None,
     grid=None,
     early_stop: Optional[float] = None,
+    normals: bool = False,
     _n_chunks: int = 1,
 ):
     """nerf/train_utils.py:28-127 for one chunk of packed rays ``[o d near far (viewdir)]``.
@@ -472,8 +494,15 @@ def predict_and_render_radiance(
 
     ``early_stop``: a transmittance threshold t in [0, 1) (inference only, impl 1 or 3, with or without ``grid``): the
     last pass stops a ray once its transmittance falls below t, so its rgb and acc move by at most t
-    (include/nerfb200.h "early ray termination").  None is the path without it."""
+    (include/nerfb200.h "early ray termination").  None is the path without it.
+
+    ``normals``: also return the last pass's normal map N (n_rays, 3) as a seventh output (inference only, impl 1,
+    with or without ``grid`` / ``early_stop``): the sum of the compositing weights times the outward unit normals
+    -grad sigma / |grad sigma| at the pass's samples (include/nerfb200.h "normal maps"); not renormalised, so |N| <=
+    acc.  False returns exactly the six outputs."""
     impl = _requested_impl(impl, model_coarse, model_fine)
+    if normals:
+        check_normals_call(impl, model_coarse, model_fine)
     if grid is not None:
         check_grid_call(grid, None, model_coarse, model_fine)
     if early_stop is not None:
@@ -497,6 +526,8 @@ def predict_and_render_radiance(
         impl = _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine)
     elif early_stop is not None:
         impl = _early_stop_impl(impl, arch_c, arch_f, nc, nf)
+    if normals:
+        impl = _normals_impl(impl, arch_c, arch_f, nc, nf)
     params_c, blob_c = _packed(model_coarse, arch_c)
     params_f, blob_f = _packed(model_fine, arch_f) if fine else ([], None)
     noise_std = float(o.radiance_field_noise_std)
@@ -529,7 +560,11 @@ def predict_and_render_radiance(
     training = _trains(all_params)
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training)
-    if early_stop is not None:
+    nrm = None
+    if normals:
+        out_c, out_f, nrm, _ = ops.render_fwd_normals(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid,
+                                                   None if early_stop is None else float(early_stop), impl=impl)
+    elif early_stop is not None:
         out_c, out_f, _ = ops.render_fwd_early_stop(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid,
                                                     float(early_stop), impl=impl)
     elif grid is not None:
@@ -538,9 +573,8 @@ def predict_and_render_radiance(
         cfg = (arch_c, arch_f, opts, blob_c, blob_f, training, impl, int(_n_chunks))
         out_c, out_f = _RenderChunk.apply(cfg, rays, rnd, *all_params)
     rgb_c, disp_c, acc_c = out_c[:, :3], out_c[:, 3], out_c[:, 4]
-    if out_f is None:
-        return rgb_c, disp_c, acc_c, None, None, None
-    return rgb_c, disp_c, acc_c, out_f[:, :3], out_f[:, 3], out_f[:, 4]
+    six = (rgb_c, disp_c, acc_c) + ((None, None, None) if out_f is None else (out_f[:, :3], out_f[:, 3], out_f[:, 4]))
+    return six + (nrm,) if normals else six
 
 
 def run_one_iter_of_nerf(
@@ -560,11 +594,15 @@ def run_one_iter_of_nerf(
     impl: Optional[int] = None,
     grid=None,
     early_stop: Optional[float] = None,
+    normals: bool = False,
 ):
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
-    the reshape back to image shape."""
+    the reshape back to image shape.  ``normals=True`` appends the normal map of the last pass (see
+    ``predict_and_render_radiance``) as a seventh output."""
     impl = _requested_impl(impl, model_coarse, model_fine)
+    if normals:
+        check_normals_call(impl, model_coarse, model_fine)
     if grid is not None:
         check_grid_call(grid, ray_directions.device, model_coarse, model_fine)
     if early_stop is not None:
@@ -582,7 +620,7 @@ def run_one_iter_of_nerf(
                          options.dataset.far, use_viewdirs)
 
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl, grid, early_stop)
+                          encode_direction_fn, randoms, impl, grid, early_stop, normals)
 
 
 def run_one_iter_of_nerf_from_pose(
@@ -624,7 +662,7 @@ def run_one_iter_of_nerf_from_pose(
 
 
 def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn, encode_direction_fn,
-                   randoms, impl, grid=None, early_stop=None):
+                   randoms, impl, grid=None, early_stop=None, normals=False):
     """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202.
     Seeded randoms follow each ray: chunk i starts at ``ray_offset`` + the index of its first ray."""
     chunksize = getattr(options.nerf, mode).chunksize
@@ -639,10 +677,16 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if options.nerf.use_viewdirs else None,
             randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, grid=grid,
-            early_stop=early_stop, _n_chunks=len(batches),
+            early_stop=early_stop, normals=normals, _n_chunks=len(batches),
         )
         for i, batch in enumerate(batches)
     ]
+    nrm = None
+    if normals:
+        nrm = torch.cat([p[6] for p in pred], dim=0)
+        if mode == "validation":
+            nrm = nrm.view(restore_shapes[0])
+        pred = [p[:6] for p in pred]
     synthesized_images = list(zip(*pred))
     synthesized_images = [
         torch.cat(image, dim=0) if image[0] is not None else None for image in synthesized_images
@@ -652,7 +696,6 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             image.view(shape) if image is not None else None
             for (image, shape) in zip(synthesized_images, restore_shapes)
         ]
-        if model_fine:
-            return tuple(synthesized_images)
-        return tuple(synthesized_images + [None, None, None])
-    return tuple(synthesized_images)
+        if not model_fine:
+            synthesized_images = synthesized_images + [None, None, None]
+    return tuple(synthesized_images) + ((nrm,) if normals else ())
