@@ -410,6 +410,64 @@ int32_t nerfb200_mesh_emit(const nerfb200_grid_t* box, const float* volume, floa
                            int64_t max_vertices, int64_t max_faces, float* vertices, int32_t* faces, float* view_dirs,
                            void* stream);
 
+/* ---- sparse meshes: marching cubes over the bricks an occupancy grid calls occupied ------------------------------
+ * The lattice, its values, the vertex rule, the case table and the winding are those of "meshes" above; only the cubes
+ * that are marched, and so the numbering, differ.  A lattice point depends on its index alone, so the sparse path
+ * evaluates exactly the points (and gets exactly the values) the dense path would at the same indices.
+ *   - Bricks.  Brick (b_0, b_1, b_2), b_c = 0 .. ceil(res[c] / B) - 1 with B = NERFB200_MESH_BRICK, holds the cubes
+ *     whose low corner q has floor(q_c / B) = b_c; its corner points are the lattice points i with b_c B <= i_c <=
+ *     min(b_c B + B, res[c]) (bricks on the box's upper faces are partial).  Brick index (b_2 * nb_1 + b_1) * nb_0 + b_0,
+ *     x fastest.  Brick indices are int32 (at most 512^3 bricks).
+ *   - Activity.  A brick is active when one of its corner points, at the fp32 coordinates p_c(i) of "meshes", lies
+ *     outside the grid's box or in an occupied cell under the cell rule of "occupancy grid" (a point outside the box is
+ *     always evaluated by renders too).  The cell rule is separable per axis, so the library tests each distinct cell
+ *     the corners' axis cells combine to; the result is exactly that of the point rule.
+ *   - Output.  The faces are those of the dense mesh over the same values and level restricted to the cubes of active
+ *     bricks; the vertices are the crossing edges those cubes use, with bit-identical coordinates (and view
+ *     directions).  Each crossing edge carries one vertex, owned by the lowest-index active brick with a cube using the
+ *     edge.  Vertex ids run by owning brick, then by (linear lattice index of q, a) within it; faces by brick, then by
+ *     cube linear index, then in table order.  Prefix sums throughout, no atomics: the mesh is a function of the values,
+ *     the level and the grid.  If no face of the dense mesh lies in a cube of an inactive brick, the sparse mesh is the
+ *     dense mesh up to this renumbering.
+ *   - Values are brick-major over the active bricks in slot order: slot s holds P = p1^3 values, p1 = B + 1 + 2 halo,
+ *     corner point l (0 .. B per axis, lattice index b B + l) at s * P + ((l_2 + halo) * p1 + l_1 + halo) * p1 + l_0 + halo.
+ *     halo = 1 adds the points one outside the brick, which the view directions' central differences read; there a
+ *     lattice index outside 0 .. res[c] is clamped onto the lattice (those values are never read).
+ *   - Memory.  brick_map and the brick list are int32 per brick of the box; the scratch of mesh_sparse_bricks is
+ *     three axis tables of 4097 int32 and 20 bytes per 256 bricks; everything else is per active brick: P values and
+ *     mesh_sparse_workspace_bytes (392 bytes per brick).
+ *
+ * mesh_brick: B.  mesh_sparse_brick_count: bricks of the box (-1 for an invalid box).
+ * mesh_sparse_bricks: the activity test and its compaction.  brick_map[brick] = the brick's slot (its rank among the
+ *   active bricks, in brick order) or -1; bricks[slot] = brick (int32[mesh_sparse_brick_count], the first *n_active
+ *   written); *n_active (device int64) = the count.  scratch: mesh_sparse_scratch_bytes(box) device bytes.
+ * mesh_sparse_bricks_host: the activity test on the host (test hook): active[brick] = 0 / 1, host memory only.
+ * mesh_sparse_points: pts[count * P][3] = the lattice points of slots first .. first + count - 1 in value order.
+ * mesh_sparse_count / _emit: mesh_count / mesh_emit over the active bricks' values.  totals[0] = vertices, totals[1] =
+ *   faces (device int64[2]).  view_dirs (may be NULL; needs halo = 1) as in mesh_emit; edge_keys (int64[V], may be
+ *   NULL) = q * 3 + a of each vertex's lattice edge, q its low end's linear lattice index.
+ * Refused before any launch: an invalid box or grid, a null pointer, halo other than 0 / 1, a non-finite level, an
+ * active count outside 0 .. the box's bricks. */
+#define NERFB200_MESH_BRICK 8
+int32_t nerfb200_mesh_brick(void);
+int64_t nerfb200_mesh_sparse_brick_count(const nerfb200_grid_t* box);
+int64_t nerfb200_mesh_sparse_scratch_bytes(const nerfb200_grid_t* box);
+int64_t nerfb200_mesh_sparse_workspace_bytes(const nerfb200_grid_t* box, int64_t n_active);
+int32_t nerfb200_mesh_sparse_bricks(const nerfb200_grid_t* box, const nerfb200_grid_t* grid, const uint32_t* bits,
+                                    int32_t* brick_map, int32_t* bricks, int64_t* n_active, void* scratch,
+                                    void* stream);
+int32_t nerfb200_mesh_sparse_bricks_host(const nerfb200_grid_t* box, const nerfb200_grid_t* grid,
+                                         const uint32_t* bits_host, uint8_t* active_host);
+int32_t nerfb200_mesh_sparse_points(const nerfb200_grid_t* box, const int32_t* bricks, int64_t first, int64_t count,
+                                    int32_t halo, float* pts, void* stream);
+int32_t nerfb200_mesh_sparse_count(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                   int64_t n_active, const float* values, int32_t halo, float level, void* workspace,
+                                   int64_t* totals, void* stream);
+int32_t nerfb200_mesh_sparse_emit(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                  int64_t n_active, const float* values, int32_t halo, float level,
+                                  const void* workspace, int64_t max_vertices, int64_t max_faces, float* vertices,
+                                  int32_t* faces, float* view_dirs, int64_t* edge_keys, void* stream);
+
 /* ---- density gradient: sigma and its gradient w.r.t. the points (normals, field probes) -------------------------
  * density_grad: out[P][4] = (sigma_raw, d sigma_raw / dx, d / dy, d / dz) at pts[P][3], P >= 1 and < 2^31.  sigma_raw is
  *   the network's sigma output before the ReLU (fc_alpha, or column 3 of fc_out without view directions), bit for bit

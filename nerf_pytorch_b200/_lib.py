@@ -129,6 +129,15 @@ SIGNATURES = {
     "nerfb200_mesh_lattice_points": (I32, [GP, I32, I32, P, P]),
     "nerfb200_mesh_count": (I32, [GP, P, F32, P, P, P]),
     "nerfb200_mesh_emit": (I32, [GP, P, F32, P, I64, I64, P, P, P, P]),
+    "nerfb200_mesh_brick": (I32, []),
+    "nerfb200_mesh_sparse_brick_count": (I64, [GP]),
+    "nerfb200_mesh_sparse_scratch_bytes": (I64, [GP]),
+    "nerfb200_mesh_sparse_workspace_bytes": (I64, [GP, I64]),
+    "nerfb200_mesh_sparse_bricks": (I32, [GP, GP, P, P, P, P, P, P]),
+    "nerfb200_mesh_sparse_bricks_host": (I32, [GP, GP, P, P]),
+    "nerfb200_mesh_sparse_points": (I32, [GP, P, I64, I64, I32, P, P]),
+    "nerfb200_mesh_sparse_count": (I32, [GP, P, P, I64, P, I32, F32, P, P, P]),
+    "nerfb200_mesh_sparse_emit": (I32, [GP, P, P, I64, P, I32, F32, P, I64, I64, P, P, P, P, P]),
     "nerfb200_density_grad_supported": (I32, [AP, I32]),
     "nerfb200_density_grad": (I32, [AP, P, P, I64, P, I32, P]),
     "nerfb200_render_normals_workspace_bytes": (I64, [AP, AP, OP, I64]),

@@ -11,8 +11,8 @@
 // No atomics: the mesh is a function of the volume and the level.
 #include <cmath>
 
-#include "common.cuh"
 #include "mc_table.cuh"
+#include "mesh_common.cuh"
 
 namespace nerfb200 {
 
@@ -20,29 +20,6 @@ namespace {
 
 constexpr int kMeshThreads = 256;  // lattice points per tile, one CTA's threads: 8 warps
 constexpr int kWarps = kMeshThreads / 32;
-constexpr int kMeshScanThreads = 1024;
-constexpr int kCtasPerSm = 8;
-
-struct Lattice {
-  int n[3];        // points per axis = res + 1
-  int res[3];
-  float lo[3], hi[3];
-  int64_t n01;     // points per z plane
-  int64_t total;   // lattice points
-};
-
-Lattice make_lattice(const nerfb200_grid_t& g) {
-  Lattice L;
-  for (int c = 0; c < 3; ++c) {
-    L.res[c] = g.res[c];
-    L.n[c] = g.res[c] + 1;
-    L.lo[c] = g.lo[c];
-    L.hi[c] = g.hi[c];
-  }
-  L.n01 = (int64_t)L.n[0] * L.n[1];
-  L.total = L.n01 * L.n[2];
-  return L;
-}
 
 struct Workspace {
   uint4* warp;       // per warp: +x, +y, +z crossing ballots, first vertex relative to the tile
@@ -72,11 +49,6 @@ Workspace workspace_layout(const Lattice& L, void* base) {
   off += align16(tiles * 8);
   w.bytes = off;
   return w;
-}
-
-// p_c(i) of the header: lo + ((hi - lo) * i) / res, each op rounded
-__device__ __forceinline__ float lattice_coord(const Lattice& L, int c, int i) {
-  return __fadd_rn(L.lo[c], __fdiv_rn(__fmul_rn(__fsub_rn(L.hi[c], L.lo[c]), (float)i), (float)L.res[c]));
 }
 
 __device__ __forceinline__ int64_t axis_stride(const Lattice& L, int a) {
@@ -113,8 +85,7 @@ __device__ __forceinline__ void lattice_grad(const Lattice& L, const float* __re
   for (int c = 0; c < 3; ++c) {
     const int lo = i[c] > 0 ? i[c] - 1 : 0, hi = i[c] + 1 < L.n[c] ? i[c] + 1 : L.n[c] - 1;
     const int64_t s = axis_stride(L, c);
-    const float h = __fdiv_rn(__fsub_rn(L.hi[c], L.lo[c]), (float)L.res[c]);
-    g[c] = __fdiv_rn(__fsub_rn(vol[q + (hi - i[c]) * s], vol[q + (lo - i[c]) * s]), __fmul_rn(h, (float)(hi - lo)));
+    g[c] = grad_component(L, c, vol[q + (hi - i[c]) * s], vol[q + (lo - i[c]) * s], hi, lo);
   }
 }
 
@@ -165,43 +136,6 @@ mesh_classify_kernel(const Lattice L, const float* __restrict__ vol, float level
   }
 }
 
-// exclusive prefix sums of the tile totals, one CTA: each thread sums a contiguous run of tiles, the runs are scanned in
-// shared memory, then each thread writes its run's offsets
-__global__ void __launch_bounds__(kMeshScanThreads)
-mesh_scan_kernel(const int* __restrict__ tile_v, const int* __restrict__ tile_f, int64_t n_tiles,
-                 long long* __restrict__ voff, long long* __restrict__ foff, long long* __restrict__ totals) {
-  __shared__ long long sv[kMeshScanThreads], sf[kMeshScanThreads];
-  const int tid = threadIdx.x;
-  const int64_t run = (n_tiles + kMeshScanThreads - 1) / kMeshScanThreads;
-  const int64_t b0 = min(n_tiles, tid * run), b1 = min(n_tiles, b0 + run);
-  long long v = 0, f = 0;
-  for (int64_t b = b0; b < b1; ++b) {
-    v += tile_v[b];
-    f += tile_f[b];
-  }
-  sv[tid] = v;
-  sf[tid] = f;
-  __syncthreads();
-  for (int o = 1; o < kMeshScanThreads; o <<= 1) {
-    const long long av = tid >= o ? sv[tid - o] : 0, af = tid >= o ? sf[tid - o] : 0;
-    __syncthreads();
-    sv[tid] += av;
-    sf[tid] += af;
-    __syncthreads();
-  }
-  long long rv = sv[tid] - v, rf = sf[tid] - f;
-  for (int64_t b = b0; b < b1; ++b) {
-    voff[b] = rv;
-    foff[b] = rf;
-    rv += tile_v[b];
-    rf += tile_f[b];
-  }
-  if (tid == kMeshScanThreads - 1) {
-    totals[0] = sv[tid];
-    totals[1] = sf[tid];
-  }
-}
-
 __global__ void __launch_bounds__(kMeshThreads)
 mesh_emit_kernel(const Lattice L, const float* __restrict__ vol, float level, int64_t n_tiles,
                  const uint4* __restrict__ warp_info, const long long* __restrict__ voff,
@@ -236,26 +170,18 @@ mesh_emit_kernel(const Lattice L, const float* __restrict__ vol, float level, in
         if (id >= max_v) continue;
         const int64_t q1 = p + axis_stride(L, a);
         const float v0 = vol[p], v1 = vol[q1];
-        const float t = __fdiv_rn(__fsub_rn(level, v0), __fsub_rn(v1, v0));
+        const float t = edge_t(level, v0, v1);
         float x[3] = {p0[0], p0[1], p0[2]};
-        x[a] = __fadd_rn(p0[a], __fmul_rn(t, __fsub_rn(lattice_coord(L, a, i[a] + 1), p0[a])));
+        x[a] = edge_coord(L, a, i[a], p0[a], t);
 #pragma unroll
         for (int c = 0; c < 3; ++c) verts[3 * id + c] = x[c];
         if (dirs) {
           int j[3] = {i[0], i[1], i[2]};
           j[a] += 1;
-          float g0[3], g1[3], g[3];
+          float g0[3], g1[3], d[3];
           lattice_grad(L, vol, p, i, g0);
           lattice_grad(L, vol, q1, j, g1);
-#pragma unroll
-          for (int c = 0; c < 3; ++c) g[c] = __fadd_rn(g0[c], __fmul_rn(t, __fsub_rn(g1[c], g0[c])));
-          const float s = __fadd_rn(__fadd_rn(__fmul_rn(g[0], g[0]), __fmul_rn(g[1], g[1])), __fmul_rn(g[2], g[2]));
-          float d[3] = {0.f, 0.f, 1.f};
-          if (s > 0.f && s < INFINITY) {
-            const float r = __fsqrt_rn(s);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) d[c] = __fdiv_rn(g[c], r);
-          }
+          edge_dir(g0, g1, t, d);
 #pragma unroll
           for (int c = 0; c < 3; ++c) dirs[3 * id + c] = d[c];
         }
@@ -301,13 +227,6 @@ __global__ void mesh_lattice_points_kernel(const Lattice L, int z0, int64_t n, f
   pts[3 * k + 0] = lattice_coord(L, 0, x);
   pts[3 * k + 1] = lattice_coord(L, 1, y);
   pts[3 * k + 2] = lattice_coord(L, 2, z);
-}
-
-// CTAs of the two tile loops: enough to fill every SM several times over, few enough that each loads the case table
-// into shared memory once for many tiles
-unsigned grid_for(int64_t tiles) {
-  const int64_t cap = (int64_t)device_sms() * kCtasPerSm;
-  return (unsigned)(tiles < cap ? tiles : cap);
 }
 
 int check_box(const nerfb200_grid_t* box, const char* what) {

@@ -1,9 +1,10 @@
 """Meshes from trained networks: the density of a FlexibleNeRFModel on a lattice over a box, queried through the fused
 MLP forward (``ops.mlp_fwd_pts``), and marching cubes over it on the GPU (csrc/mesh.cu).
 
-The lattice, the vertex rule, the case table and the face order are defined once, in include/nerfb200.h ("meshes");
-this file validates arguments, sizes buffers and moves pointers.  The surface step reads its two totals back once to
-allocate the outputs: that is its only host synchronisation."""
+The lattice, the vertex rule, the case table and the face order are defined once, in include/nerfb200.h ("meshes"; the
+sparse path over an occupancy grid's bricks in "sparse meshes", csrc/mesh_sparse.cu); this file validates arguments,
+sizes buffers and moves pointers.  The surface step reads its two totals back once to allocate the outputs: that is its
+only host synchronisation, besides the sparse path's read of its active brick count."""
 from __future__ import annotations
 
 import math
@@ -18,8 +19,9 @@ from . import ops
 _SLAB_POINTS = 1 << 22
 
 
-def _box(bounds, resolution):
-    """(lo, hi, res) after the refusals that need no device: ValueError for a malformed box or lattice."""
+def _box(bounds, resolution, dense=True):
+    """(lo, hi, res) after the refusals that need no device: ValueError for a malformed box or lattice (and, for the
+    dense path, one past 2^31 points)."""
     try:
         lo, hi = bounds
         lo, hi = tuple(float(v) for v in lo), tuple(float(v) for v in hi)
@@ -34,7 +36,7 @@ def _box(bounds, resolution):
         raise ValueError(f"mesh: resolution must be an int or three ints, got {resolution!r}")
     if not all(2 <= r <= 4096 for r in res):
         raise ValueError(f"mesh: resolution must be 2 .. 4096 cubes per axis, got {resolution!r}")
-    if math.prod(r + 1 for r in res) > 2 ** 31:
+    if dense and math.prod(r + 1 for r in res) > 2 ** 31:
         raise ValueError(f"mesh: a lattice of {' x '.join(str(r + 1) for r in res)} points is past 2^31")
     return lo, hi, res
 
@@ -139,6 +141,20 @@ def _network(model, encode_position_fn, encode_direction_fn):
     return arch
 
 
+def _query_impl(arch, impl):
+    """The MLP kernels of the lattice query: None picks the wgmma inference forward where the architecture allows it,
+    else the fp32 kernels; an explicit impl the architecture refuses raises NotImplementedError."""
+    from . import train_utils
+
+    if impl is None:
+        return train_utils._auto_impl(arch, None, 64, 0, training=False)
+    use = int(impl)
+    why = ops.impl_refusal(arch, 64, ops.IMPL_TC_FWD if use == ops.IMPL_TC else use)
+    if why is not None:
+        raise NotImplementedError(f"nerfb200 mesh: impl {use}: {why}")
+    return use
+
+
 def density_volume(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), resolution=256, *,
                    encode_direction_fn=None, impl: Optional[int] = None,
                    planes_per_slab: Optional[int] = None) -> torch.Tensor:
@@ -153,13 +169,7 @@ def density_volume(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), 
 
     lo, hi, res = _box(bounds, resolution)
     arch = _network(model, encode_position_fn, encode_direction_fn)
-    if impl is None:
-        use = train_utils._auto_impl(arch, None, 64, 0, training=False)
-    else:
-        use = int(impl)
-        why = ops.impl_refusal(arch, 64, ops.IMPL_TC_FWD if use == ops.IMPL_TC else use)
-        if why is not None:
-            raise NotImplementedError(f"nerfb200 mesh: impl {use}: {why}")
+    use = _query_impl(arch, impl)
     n0, n1, n2 = (r + 1 for r in res)
     plane = n0 * n1
     slab = int(planes_per_slab) if planes_per_slab is not None else max(1, _SLAB_POINTS // plane)
@@ -185,9 +195,57 @@ def density_volume(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), 
     return vol.view(n2, n1, n0)
 
 
+def _check_grid(grid, device):
+    """The refusals of a sparse extraction's grid: ValueError for anything but an OccupancyGrid with well-formed bits
+    on ``device``, NotImplementedError for bits on the CPU."""
+    from .occupancy import OccupancyGrid
+
+    if not isinstance(grid, OccupancyGrid):
+        raise ValueError(f"mesh: grid must be an nb.OccupancyGrid, got {type(grid).__name__}")
+    bits = grid.bits
+    if not isinstance(bits, torch.Tensor) or not bits.is_cuda:
+        raise NotImplementedError("nerfb200: the grid's bits must be a CUDA tensor (there is no CPU path)")
+    if bits.device != device:
+        raise ValueError(f"mesh: the grid is on {bits.device}, the model on {device}")
+    if bits.dtype != torch.int32 or bits.dim() != 1 or not bits.is_contiguous() or \
+            bits.numel() != ops.grid_words(grid.c_struct()):
+        raise ValueError(f"mesh: the grid's bits must be contiguous int32[{ops.grid_words(grid.c_struct())}], got "
+                         f"{bits.dtype}{list(bits.shape)}")
+
+
+def _sparse_surface(arch, blob, use, box, grid, level: float, want_dirs: bool, bricks_per_call, want_keys=False):
+    """The sparse path (include/nerfb200.h "sparse meshes"): the grid's active bricks, the MLP at their lattice points
+    (with the one-point halo when view directions are wanted), then classify, scan and emit over them.  Two host reads:
+    the active brick count, which sizes the query, and the mesh's two totals."""
+    halo = bool(want_dirs)
+    brick_map, bricks, n_dev = ops.mesh_sparse_bricks(box, grid)
+    n_active = int(n_dev.item())
+    per_brick = (ops.mesh_brick() + 1 + 2 * halo) ** 3
+    chunk = max(1, min(n_active, int(bricks_per_call) if bricks_per_call is not None else _SLAB_POINTS // per_brick))
+    dev = blob.device
+    values = torch.empty(n_active * per_brick, dtype=torch.float32, device=dev)
+    if n_active:
+        rows_max = -(-chunk * per_brick // 64)
+        pts = torch.zeros(rows_max * 64, 3, dtype=torch.float32, device=dev)
+        direction = torch.tensor([[0.0, 0.0, 1.0]], dtype=torch.float32, device=dev)
+        with torch.no_grad():
+            for first in range(0, n_active, chunk):
+                n = min(chunk, n_active - first) * per_brick
+                rows = -(-n // 64)  # the tail past n holds earlier points and is discarded
+                ops.mesh_sparse_points(box, bricks, first, min(chunk, n_active - first), halo, pts)
+                dirs = direction.expand(rows, 3) if arch.use_viewdirs else None
+                raw = ops.mlp_fwd_pts(arch, blob, pts[:rows * 64].view(rows, 64, 3), dirs, impl=use)
+                values[first * per_brick:first * per_brick + n].copy_(torch.relu(raw.view(-1, 4)[:n, 3]))
+    totals, ws = ops.mesh_sparse_count(box, brick_map, bricks, n_active, values, halo, level)
+    n_v, n_f = (int(t) for t in totals.tolist())
+    return ops.mesh_sparse_emit(box, brick_map, bricks, n_active, values, halo, level, ws, n_v, n_f,
+                                want_dirs=want_dirs, want_keys=want_keys)
+
+
 def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), resolution=256, level: float = 50.0,
                  encode_direction_fn=None, colors: bool = False, impl: Optional[int] = None, *,
-                 planes_per_slab: Optional[int] = None, normals: bool = False) -> Mesh:
+                 planes_per_slab: Optional[int] = None, normals: bool = False, grid=None,
+                 bricks_per_call: Optional[int] = None) -> Mesh:
     """The level set sigma = ``level`` of a trained FlexibleNeRFModel over ``bounds``, by marching cubes on the GPU.
 
     The density is ``density_volume(model, ...)`` (the fused MLP at the (R + 1)^3 lattice points); inside is
@@ -199,18 +257,50 @@ def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), re
     the fp32 kernels.  ``normals=True`` sets ``Mesh.normals``: the outward unit normal -grad / |grad| of the density at
     each vertex, from the analytic gradient of ``density_gradient`` (impl 1 whatever ``impl`` the lattice query ran
     on; (0, 0, 0) where the gradient vanishes).  Argument errors raise ValueError, an unsupported model or device
-    NotImplementedError, before any launch."""
+    NotImplementedError, before any launch.
+
+    ``grid`` (an ``nb.OccupancyGrid`` on the model's device) makes the extraction sparse: the lattice is cut into bricks
+    of ``ops.mesh_brick()``^3 cubes, and only the bricks with a corner point in an occupied cell or outside the grid's
+    box have their points queried and their cubes marched, ``bricks_per_call`` bricks per MLP call (default: about 4 M
+    points).  Each lattice point gets the same value as in the dense path, so the faces are those of the dense mesh in
+    the active bricks and the vertices (colors and normals too) are bit-identical, numbered brick by brick
+    (include/nerfb200.h "sparse meshes").  Nothing is allocated at (R + 1)^3, so the lattice may pass 2^31 points (up to
+    4096 cubes per axis).  Build the grid with ``OccupancyGrid.from_models(..., threshold=t)`` for some t below
+    ``level`` (the default t = 0 is conservative): a surface in a brick the grid calls empty is missing from the mesh.
+    ``planes_per_slab`` belongs to the dense path and is refused with a grid."""
+    return _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_direction_fn, colors, impl,
+                         planes_per_slab, normals, grid, bricks_per_call)[0]
+
+
+def _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_direction_fn, colors, impl,
+                  planes_per_slab, normals, grid, bricks_per_call, edge_keys=False):
+    """extract_mesh, and with ``edge_keys`` on the sparse path also each vertex's lattice edge q * 3 + a (a test
+    hook: the dense mesh numbers its vertices in that key's order)."""
     from . import train_utils
     from . import density
 
-    lo, hi, res = _box(bounds, resolution)
+    lo, hi, res = _box(bounds, resolution, dense=grid is None)
     level = _level(level)
+    if grid is not None:
+        if planes_per_slab is not None:
+            raise ValueError("mesh: planes_per_slab applies to the dense path; it cannot be given with grid=")
+        if bricks_per_call is not None and int(bricks_per_call) < 1:
+            raise ValueError(f"mesh: bricks_per_call must be >= 1, got {bricks_per_call}")
     arch = _network(model, encode_position_fn, encode_direction_fn)
     grad_impl = density.refusal(arch, None) if normals else None
-    vol = density_volume(model, encode_position_fn, (lo, hi), res, encode_direction_fn=encode_direction_fn, impl=impl,
-                         planes_per_slab=planes_per_slab)
     box = ops.grid_struct((lo, hi), res)
-    verts, faces, dirs = _surface(vol, box, level, want_dirs=colors and arch.use_viewdirs)
+    want_dirs = colors and arch.use_viewdirs
+    keys = None
+    if grid is None:
+        vol = density_volume(model, encode_position_fn, (lo, hi), res, encode_direction_fn=encode_direction_fn,
+                             impl=impl, planes_per_slab=planes_per_slab)
+        verts, faces, dirs = _surface(vol, box, level, want_dirs=want_dirs)
+    else:
+        _check_grid(grid, next(model.parameters()).device)
+        use = _query_impl(arch, impl)
+        _, blob = train_utils._packed(model, arch)
+        verts, faces, dirs, keys = _sparse_surface(arch, blob, use, box, grid, level, want_dirs, bricks_per_call,
+                                                   want_keys=edge_keys)
     rgb = None
     if colors:
         if verts.shape[0] == 0:
@@ -227,4 +317,4 @@ def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), re
         _, g = density.density_grad_points(arch, blob, verts, grad_impl)
         norm = torch.linalg.vector_norm(g, dim=-1, keepdim=True)
         nrm = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
-    return Mesh(verts, faces, rgb, nrm)
+    return Mesh(verts, faces, rgb, nrm), keys

@@ -866,3 +866,98 @@ def mesh_emit(box: Grid, volume: torch.Tensor, level: float, workspace: torch.Te
                                               _ptr(dirs) if want_dirs and n_vertices else None, _stream()),
                "mesh_emit")
     return verts, faces, dirs
+
+
+# ------------------------------------------------------------------------------------------------
+# sparse meshes (include/nerfb200.h "sparse meshes"): marching cubes over the bricks an occupancy grid calls occupied
+# ------------------------------------------------------------------------------------------------
+def mesh_brick() -> int:
+    """Cubes per brick axis (NERFB200_MESH_BRICK)."""
+    return int(_lib.load().nerfb200_mesh_brick())
+
+
+def mesh_sparse_brick_count(box: Grid) -> int:
+    n = _lib.load().nerfb200_mesh_sparse_brick_count(C.byref(box))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, "mesh_sparse_brick_count")
+    return int(n)
+
+
+def mesh_sparse_workspace_bytes(box: Grid, n_active: int) -> int:
+    n = _lib.load().nerfb200_mesh_sparse_workspace_bytes(C.byref(box), int(n_active))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, "mesh_sparse_workspace_bytes")
+    return int(n)
+
+
+def mesh_sparse_scratch_bytes(box: Grid) -> int:
+    n = _lib.load().nerfb200_mesh_sparse_scratch_bytes(C.byref(box))
+    if n < 0:
+        _lib.check(_lib.ERR_INVALID, "mesh_sparse_scratch_bytes")
+    return int(n)
+
+
+def mesh_sparse_bricks(box: Grid, grid):
+    """The activity test of an OccupancyGrid-like ``grid`` over the box's bricks: (brick_map int32[bricks] = slot or
+    -1, bricks int32[bricks] whose first n_active entries are the active bricks in order, n_active int64[1] on the
+    device)."""
+    lib = _lib.load()
+    g, bits = _grid_args(grid)
+    n = mesh_sparse_brick_count(box)
+    dev = bits.device
+    brick_map = torch.empty(n, dtype=torch.int32, device=dev)
+    bricks = torch.empty(n, dtype=torch.int32, device=dev)
+    n_active = torch.empty(1, dtype=torch.int64, device=dev)
+    scratch = torch.empty(mesh_sparse_scratch_bytes(box), dtype=torch.uint8, device=dev)
+    _lib.check(lib.nerfb200_mesh_sparse_bricks(C.byref(box), C.byref(g), _ptr(bits), _ptr(brick_map), _ptr(bricks),
+                                               _ptr(n_active), _ptr(scratch), _stream()), "mesh_sparse_bricks")
+    return brick_map, bricks, n_active
+
+
+def mesh_sparse_bricks_host(box: Grid, grid: Grid, bits: torch.Tensor) -> torch.Tensor:
+    """The library's host statement of the activity test: bool[bricks] from int32 grid words on the CPU."""
+    b = bits.detach().to(device="cpu", dtype=torch.int32).contiguous()
+    out = torch.empty(mesh_sparse_brick_count(box), dtype=torch.uint8)
+    _lib.check(_lib.load().nerfb200_mesh_sparse_bricks_host(C.byref(box), C.byref(grid), C.c_void_p(b.data_ptr()),
+                                                            C.c_void_p(out.data_ptr())), "mesh_sparse_bricks_host")
+    return out.bool()
+
+
+def mesh_sparse_points(box: Grid, bricks: torch.Tensor, first: int, count: int, halo: bool, out: torch.Tensor):
+    """The lattice points of active slots first .. first + count - 1, brick-major (with the one-point halo when
+    ``halo``), into the first count * P rows of ``out`` (fp32 CUDA, P = (B + 1 + 2 halo)^3)."""
+    _lib.check(_lib.load().nerfb200_mesh_sparse_points(C.byref(box), _ptr(bricks), int(first), int(count), int(halo),
+                                                       _ptr(out), _stream()), "mesh_sparse_points")
+    return out
+
+
+def mesh_sparse_count(box: Grid, brick_map, bricks, n_active: int, values, halo: bool, level: float,
+                      workspace: Optional[torch.Tensor] = None):
+    """Classify and scan over the active bricks' values: (totals int64[2] on the device, workspace)."""
+    need = mesh_sparse_workspace_bytes(box, n_active)
+    dev = brick_map.device
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(max(need, 1), dtype=torch.uint8, device=dev)
+    totals = torch.empty(2, dtype=torch.int64, device=dev)
+    _lib.check(_lib.load().nerfb200_mesh_sparse_count(C.byref(box), _ptr(brick_map), _ptr(bricks), int(n_active),
+                                                      _ptr(values), int(halo), float(level), _ptr(workspace),
+                                                      _ptr(totals), _stream()), "mesh_sparse_count")
+    return totals, workspace
+
+
+def mesh_sparse_emit(box: Grid, brick_map, bricks, n_active: int, values, halo: bool, level: float, workspace,
+                     n_vertices: int, n_faces: int, want_dirs: bool = False, want_keys: bool = False):
+    """Vertices (V, 3) fp32, faces (F, 3) int32, view directions (V, 3) with ``want_dirs`` (needs the halo) and the
+    lattice edge key q * 3 + a of each vertex, int64 (V,), with ``want_keys``."""
+    dev = brick_map.device
+    verts = torch.empty(n_vertices, 3, dtype=torch.float32, device=dev)
+    faces = torch.empty(n_faces, 3, dtype=torch.int32, device=dev)
+    dirs = torch.empty(n_vertices, 3, dtype=torch.float32, device=dev) if want_dirs else None
+    keys = torch.empty(n_vertices, dtype=torch.int64, device=dev) if want_keys else None
+    nv = n_vertices > 0
+    _lib.check(_lib.load().nerfb200_mesh_sparse_emit(
+        C.byref(box), _ptr(brick_map), _ptr(bricks), int(n_active), _ptr(values), int(halo), float(level),
+        _ptr(workspace), int(n_vertices), int(n_faces), _ptr(verts) if nv else None, _ptr(faces) if n_faces else None,
+        _ptr(dirs) if want_dirs and nv else None, _ptr(keys) if want_keys and nv else None, _stream()),
+        "mesh_sparse_emit")
+    return verts, faces, dirs, keys
