@@ -480,7 +480,8 @@ int32_t nerfb200_mesh_sparse_emit(const nerfb200_grid_t* box, const int32_t* bri
  *   fp16 range gives inf / NaN, not a clamped value.
  * density_grad_supported: NERFB200_OK if density_grad runs this architecture with `impl`, else the reason (the last
  *   error), without touching a device.
- * The surface normal of a level set of sigma is -grad / |grad| (outward: toward lower density). */
+ * The surface normal of a level set of sigma is -grad / |grad| (outward: toward lower density).  "NDC scenes" below maps
+ * an NDC gradient to world space. */
 int32_t nerfb200_density_grad_supported(const nerfb200_arch_t* arch, int32_t impl);
 
 /* ---- normal maps: the composited surface normal of an inference render's last pass ------------------------------
@@ -508,6 +509,58 @@ int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb20
                                     void* stream);
 int32_t nerfb200_density_grad(const nerfb200_arch_t* arch, const float* blob, const float* pts, int64_t n_points,
                               float* out, int32_t impl, void* stream);
+
+/* ---- NDC scenes: world-space geometry of forward-facing scenes --------------------------------------------------
+ * A forward-facing (LLFF) scene's MLP encodes NDC points: ray generation with ndc != 0 applies ndc_rays(H, W, focal,
+ * 1.0, ...) (nerf_helpers.py:170-197), which maps a world point p with p_z < 0 to the point q the MLP encodes,
+ *     N(p):  q_x = (sw * p_x) / p_z,   q_y = (sh * p_y) / p_z,   q_z = 1 + 2 / p_z,
+ * with sw = fp32(-1 / (W / (2 focal))) and sh = fp32(-1 / (H / (2 focal))) evaluated in double and rounded once,
+ * exactly as nerfb200_gen_rays / pack_rays compute them (W, H the image's width and height as integers, focal the fp32
+ * focal length).  Every formula below is fp32 with round-to-nearest, each op rounded, in the order written (no
+ * contraction):
+ *   - inverse (defined for q_z < 1; q_z = 1 is the far plane at infinity):
+ *         p_z = 2 / (q_z - 1),   p_x = (q_x * p_z) / sw,   p_y = (q_y * p_z) / sh;
+ *   - gradient: the world gradient of a field sigma(N(p)) is J^T(q) g for its NDC gradient g,
+ *         s = (q_z - 1) * 0.5,   G_x = s * (sw * g_x),   G_y = s * (sh * g_y),
+ *         G_z = s * (-((q_x * g_x) + (q_y * g_y)) - ((q_z - 1) * g_z));
+ *     s = 1 / p_z is negative inside the frustum, so it flips the direction as well as scaling it;
+ *   - orientation: det J = -2 sw sh / p_z^4 < 0, so N reverses orientation.  N is projective, so a straight edge stays
+ *     straight and a triangle mesh extracted in NDC is exactly a triangle mesh in world space once each face's second
+ *     and third vertex ids are swapped (faces stay counter-clockwise seen from outside).
+ * The unit world direction of a vector v is the rule of mesh_emit's view directions: l = (v_x * v_x + v_y * v_y) +
+ * v_z * v_z; v / sqrt(l) when 0 < l < inf, else (0, 0, 1).
+ *
+ * ndc_mesh_to_world: one pass over a mesh extracted in NDC (mesh_emit / mesh_sparse_emit): world_vertices[i] =
+ *   N^-1(vertices[i]); world_faces[f] = (faces[f][0], faces[f][2], faces[f][1]); world_dirs[i] = the unit world direction
+ *   of J^T(vertices[i]) view_dirs[i] (view_dirs / world_dirs both NULL, or both given).  Each output may be its input.
+ * ndc_from_world: q[i] = N(p[i]) for p[n][3] (p_z < 0 for a meaningful result; not checked on the device).
+ * ndc_grad_to_world: rows[n][4] = (sigma, g_x, g_y, g_z) as density_grad writes them at the NDC points q[n][3];
+ *   out[n][4] = (sigma, J^T(q) g), sigma copied.  out may be rows.
+ * render_fwd_normals_ndc: render_fwd_normals of an NDC render (rays from gen_rays / pack_rays with ndc != 0 and this
+ *   H, W, focal) with the normal map in world space: each sample's gradient g_i is replaced by J^T(q_i) g_i at the
+ *   sample's NDC point q_i = o + d z_i BEFORE it is normalised and weighted; the sums, outputs, refusals and workspace are
+ *   render_fwd_normals'.
+ * Refused before any launch: a null ndc, height or width <= 0, focal not finite and > 0, a null pointer where one is
+ * needed, a negative count (NERFB200_ERR_INVALID).  No atomics, no host synchronisation. */
+typedef struct nerfb200_ndc {
+  int32_t height;
+  int32_t width;
+  float focal;
+} nerfb200_ndc_t;
+int32_t nerfb200_ndc_mesh_to_world(const nerfb200_ndc_t* ndc, const float* vertices, const int32_t* faces,
+                                   const float* view_dirs, int64_t n_vertices, int64_t n_faces, float* world_vertices,
+                                   int32_t* world_faces, float* world_dirs, void* stream);
+int32_t nerfb200_ndc_from_world(const nerfb200_ndc_t* ndc, const float* p, int64_t n, float* q, void* stream);
+int32_t nerfb200_ndc_grad_to_world(const nerfb200_ndc_t* ndc, const float* q, const float* rows, int64_t n, float* out,
+                                   void* stream);
+int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                        const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                        const float* rays, int32_t ray_stride, int64_t n_rays,
+                                        const nerfb200_rng_t* rng, const float* t_rand, const float* noise_c,
+                                        const float* u, const float* noise_f, const nerfb200_grid_t* grid,
+                                        const uint32_t* bits, float stop_transmittance, const nerfb200_ndc_t* ndc,
+                                        float* out_coarse, float* out_fine, float* normals, void* workspace,
+                                        int32_t impl, void* stream);
 
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale

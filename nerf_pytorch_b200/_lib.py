@@ -56,6 +56,16 @@ class Rng(C.Structure):
     ]
 
 
+class Ndc(C.Structure):
+    """nerfb200_ndc_t: the camera of a forward-facing scene's NDC map (include/nerfb200.h "NDC scenes")"""
+
+    _fields_ = [
+        ("height", C.c_int32),
+        ("width", C.c_int32),
+        ("focal", C.c_float),
+    ]
+
+
 class Grid(C.Structure):
     """nerfb200_grid_t: the box [lo, hi) and its cells per axis (the bit order is in include/nerfb200.h)"""
 
@@ -68,7 +78,7 @@ class Grid(C.Structure):
 
 P = C.c_void_p
 I32, I64, F32, F64, U64 = C.c_int32, C.c_int64, C.c_float, C.c_double, C.c_uint64
-AP, OP, RP, GP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng), C.POINTER(Grid)
+AP, OP, RP, GP, NP = C.POINTER(Arch), C.POINTER(RenderOpts), C.POINTER(Rng), C.POINTER(Grid), C.POINTER(Ndc)
 
 # name -> (restype, argtypes); mirrors include/nerfb200.h one-to-one
 SIGNATURES = {
@@ -142,6 +152,11 @@ SIGNATURES = {
     "nerfb200_density_grad": (I32, [AP, P, P, I64, P, I32, P]),
     "nerfb200_render_normals_workspace_bytes": (I64, [AP, AP, OP, I64]),
     "nerfb200_render_fwd_normals": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, F32, P, P, P, P, I32, P]),
+    "nerfb200_ndc_mesh_to_world": (I32, [NP, P, P, P, I64, I64, P, P, P, P]),
+    "nerfb200_ndc_from_world": (I32, [NP, P, I64, P, P]),
+    "nerfb200_ndc_grad_to_world": (I32, [NP, P, P, I64, P, P]),
+    "nerfb200_render_fwd_normals_ndc": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, F32, NP, P, P, P, P,
+                                              I32, P]),
 }
 
 _lib = None

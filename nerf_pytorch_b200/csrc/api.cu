@@ -1049,14 +1049,18 @@ int64_t nerfb200_render_normals_workspace_bytes(const nerfb200_arch_t* coarse, c
   return nw.end;
 }
 
-int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                                    const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                                    const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                                    const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
-                                    const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
-                                    float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
-                                    void* stream) {
-  const char* what = "render_fwd_normals";
+}  // extern "C"
+
+namespace nerfb200 {
+
+// render_fwd_normals, and with `world` its NDC render's world-space normal map (nerfb200.h "NDC scenes")
+static int render_normals(const char* what, const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                          const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                          const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                          const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                          const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                          float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
+                          void* stream, const NdcMap* world) {
   if ((grid == nullptr) != (bits == nullptr)) {
     set_error("%s: a grid descriptor and its bits come together", what);
     return NERFB200_ERR_INVALID;
@@ -1097,7 +1101,73 @@ int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb20
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   NB_TRY(launch_normal_compact(rays, ray_stride, z_last, W, n_rays, n_last, st, s));
   NB_TRY(launch_density_grad_tc(pl, blob_last, st.pts, n_rays * n_last, st.grad, st.total, s));
-  return launch_normal_sum(W, n_rays, n_last, st, normals, s);
+  return launch_normal_sum(W, n_rays, n_last, st, normals, s, world);
+}
+
+}  // namespace nerfb200
+
+extern "C" {
+
+int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                    const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                    const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
+                                    const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
+                                    const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
+                                    float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
+                                    void* stream) {
+  return render_normals("render_fwd_normals", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                        t_rand, noise_c, u, noise_f, grid, bits, stop_transmittance, out_coarse, out_fine, normals,
+                        workspace, impl, stream, nullptr);
+}
+
+int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
+                                        const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
+                                        const float* rays, int32_t ray_stride, int64_t n_rays,
+                                        const nerfb200_rng_t* rng, const float* t_rand, const float* noise_c,
+                                        const float* u, const float* noise_f, const nerfb200_grid_t* grid,
+                                        const uint32_t* bits, float stop_transmittance, const nerfb200_ndc_t* ndc,
+                                        float* out_coarse, float* out_fine, float* normals, void* workspace,
+                                        int32_t impl, void* stream) {
+  NdcMap m;
+  NB_TRY(make_ndc_map(ndc, &m, "render_fwd_normals_ndc"));
+  return render_normals("render_fwd_normals_ndc", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                        t_rand, noise_c, u, noise_f, grid, bits, stop_transmittance, out_coarse, out_fine, normals,
+                        workspace, impl, stream, &m);
+}
+
+int32_t nerfb200_ndc_mesh_to_world(const nerfb200_ndc_t* ndc, const float* vertices, const int32_t* faces,
+                                   const float* view_dirs, int64_t n_vertices, int64_t n_faces, float* world_vertices,
+                                   int32_t* world_faces, float* world_dirs, void* stream) {
+  NdcMap m;
+  NB_TRY(make_ndc_map(ndc, &m, "ndc_mesh_to_world"));
+  if (n_vertices < 0 || n_faces < 0 || (n_vertices > 0 && (!vertices || !world_vertices)) ||
+      (n_faces > 0 && (!faces || !world_faces)) || ((view_dirs == nullptr) != (world_dirs == nullptr))) {
+    set_error("ndc_mesh_to_world: a negative count, a null pointer, or view_dirs without world_dirs (or the reverse)");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_ndc_mesh_to_world(m, vertices, faces, view_dirs, n_vertices, n_faces, world_vertices, world_faces,
+                                  n_vertices > 0 ? world_dirs : nullptr, static_cast<cudaStream_t>(stream));
+}
+
+int32_t nerfb200_ndc_from_world(const nerfb200_ndc_t* ndc, const float* p, int64_t n, float* q, void* stream) {
+  NdcMap m;
+  NB_TRY(make_ndc_map(ndc, &m, "ndc_from_world"));
+  if (n < 0 || (n > 0 && (!p || !q))) {
+    set_error("ndc_from_world: a negative count or a null pointer");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_ndc_from_world(m, p, n, q, static_cast<cudaStream_t>(stream));
+}
+
+int32_t nerfb200_ndc_grad_to_world(const nerfb200_ndc_t* ndc, const float* q, const float* rows, int64_t n, float* out,
+                                   void* stream) {
+  NdcMap m;
+  NB_TRY(make_ndc_map(ndc, &m, "ndc_grad_to_world"));
+  if (n < 0 || (n > 0 && (!q || !rows || !out))) {
+    set_error("ndc_grad_to_world: a negative count or a null pointer");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_ndc_grad_to_world(m, q, rows, n, out, static_cast<cudaStream_t>(stream));
 }
 
 int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,

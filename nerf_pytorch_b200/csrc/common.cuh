@@ -214,8 +214,42 @@ struct NormalState {
 };
 int launch_normal_compact(const float* rays, int ray_stride, const float* z, const float* weights, int64_t n_rays,
                           int n_samples, const NormalState& ns, cudaStream_t s);
+// ---- NDC scenes (ndc.cu; nerfb200.h "NDC scenes"): the map N of ndc_rays and its Jacobian ----
+// sw, sh of the header, as raygen.cu's finish_ray computes them
+struct NdcMap {
+  float sw, sh;
+};
+// NERFB200_ERR_INVALID (reason prefixed with `what`) for a null or malformed camera
+int make_ndc_map(const nerfb200_ndc_t* ndc, NdcMap* m, const char* what);
+// q = N(p)
+__device__ __forceinline__ void ndc_forward(const NdcMap& m, const float p[3], float q[3]) {
+  q[0] = __fdiv_rn(__fmul_rn(m.sw, p[0]), p[2]);
+  q[1] = __fdiv_rn(__fmul_rn(m.sh, p[1]), p[2]);
+  q[2] = __fadd_rn(1.0f, __fdiv_rn(2.0f, p[2]));
+}
+// p = N^-1(q)
+__device__ __forceinline__ void ndc_inverse(const NdcMap& m, const float q[3], float p[3]) {
+  p[2] = __fdiv_rn(2.0f, __fsub_rn(q[2], 1.0f));
+  p[0] = __fdiv_rn(__fmul_rn(q[0], p[2]), m.sw);
+  p[1] = __fdiv_rn(__fmul_rn(q[1], p[2]), m.sh);
+}
+// G = J^T(q) g: the world gradient of a field whose NDC gradient at q is g
+__device__ __forceinline__ void ndc_grad_to_world(const NdcMap& m, const float q[3], const float g[3], float G[3]) {
+  const float qz1 = __fsub_rn(q[2], 1.0f);
+  const float s = __fmul_rn(qz1, 0.5f);
+  const float t = __fadd_rn(__fmul_rn(q[0], g[0]), __fmul_rn(q[1], g[1]));
+  G[0] = __fmul_rn(s, __fmul_rn(m.sw, g[0]));
+  G[1] = __fmul_rn(s, __fmul_rn(m.sh, g[1]));
+  G[2] = __fmul_rn(s, __fsub_rn(-t, __fmul_rn(qz1, g[2])));
+}
+int launch_ndc_mesh_to_world(const NdcMap& m, const float* vertices, const int32_t* faces, const float* view_dirs,
+                             int64_t n_vertices, int64_t n_faces, float* world_vertices, int32_t* world_faces,
+                             float* world_dirs, cudaStream_t s);
+int launch_ndc_from_world(const NdcMap& m, const float* p, int64_t n, float* q, cudaStream_t s);
+int launch_ndc_grad_to_world(const NdcMap& m, const float* q, const float* rows, int64_t n, float* out, cudaStream_t s);
+// world: each gradient is mapped by J^T at its point ns.pts[slot] before it is normalised (nerfb200.h "NDC scenes")
 int launch_normal_sum(const float* weights, int64_t n_rays, int n_samples, const NormalState& ns, float* normals,
-                      cudaStream_t s);
+                      cudaStream_t s, const NdcMap* world = nullptr);
 // wgmma backward (mlp_tc_bwd.cu), impl 1: data-gradient chain + every weight gradient in one kernel; `scratch` holds
 // the L2-resident fixed-point gradient blob (bwd_tc_scratch_floats) the weight-gradient tiles are reduced into.
 // bwd_tc_supported checks what it needs beyond tc_supported(training = true).

@@ -74,10 +74,12 @@ normal_scatter_kernel(const float* __restrict__ rays, int ray_stride, const floa
   }
 }
 
-// normals[r] = sum over the samples with a nonzero weight, in sample order, of w (-g / |g|) (0 where g = 0)
+// normals[r] = sum over the samples with a nonzero weight, in sample order, of w (-g / |g|) (0 where g = 0); kWorld maps
+// each g by J^T at its NDC point pts[slot] first (nerfb200.h "NDC scenes")
+template <bool kWorld>
 __global__ void __launch_bounds__(kNrmWarps * 32)
 normal_sum_kernel(const float* __restrict__ weights, int64_t n_rays, int S, const int* __restrict__ first,
-                  const float* __restrict__ grad, float* __restrict__ normals) {
+                  const float* __restrict__ grad, float* __restrict__ normals, NdcMap m, const float* __restrict__ pts) {
   const int lane = threadIdx.x & 31;
   const int64_t r = blockIdx.x * (int64_t)kNrmWarps + (threadIdx.x >> 5);
   if (r >= n_rays) return;
@@ -90,7 +92,17 @@ normal_sum_kernel(const float* __restrict__ weights, int64_t n_rays, int S, cons
     const uint32_t b = __ballot_sync(0xffffffffu, on);
     float t[3] = {0.f, 0.f, 0.f};  // w n of this lane's sample
     if (on) {
-      const float4 g = reinterpret_cast<const float4*>(grad)[slot + __popc(b & ((1u << lane) - 1u))];
+      const int k = slot + __popc(b & ((1u << lane) - 1u));
+      float4 g = reinterpret_cast<const float4*>(grad)[k];
+      if constexpr (kWorld) {
+        const float q[3] = {pts[(int64_t)k * 3], pts[(int64_t)k * 3 + 1], pts[(int64_t)k * 3 + 2]};
+        const float gn[3] = {g.y, g.z, g.w};
+        float gw[3];
+        ndc_grad_to_world(m, q, gn, gw);
+        g.y = gw[0];
+        g.z = gw[1];
+        g.w = gw[2];
+      }
       const float ss = __fadd_rn(__fadd_rn(__fmul_rn(g.y, g.y), __fmul_rn(g.z, g.z)), __fmul_rn(g.w, g.w));
       if (ss != 0.f) {
         const float len = __fsqrt_rn(ss);
@@ -130,9 +142,14 @@ int launch_normal_compact(const float* rays, int ray_stride, const float* z, con
 }
 
 int launch_normal_sum(const float* weights, int64_t n_rays, int n_samples, const NormalState& ns, float* normals,
-                      cudaStream_t s) {
+                      cudaStream_t s, const NdcMap* world) {
   const unsigned blocks = (unsigned)((n_rays + kNrmWarps - 1) / kNrmWarps);
-  normal_sum_kernel<<<blocks, kNrmWarps * 32, 0, s>>>(weights, n_rays, n_samples, ns.first, ns.grad, normals);
+  if (world)
+    normal_sum_kernel<true><<<blocks, kNrmWarps * 32, 0, s>>>(weights, n_rays, n_samples, ns.first, ns.grad, normals,
+                                                              *world, ns.pts);
+  else
+    normal_sum_kernel<false><<<blocks, kNrmWarps * 32, 0, s>>>(weights, n_rays, n_samples, ns.first, ns.grad, normals,
+                                                               NdcMap{0.f, 0.f}, nullptr);
   count_launch();
   return check_cuda(cudaGetLastError(), "normal_sum launch");
 }

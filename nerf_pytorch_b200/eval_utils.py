@@ -18,7 +18,7 @@ from .ops import SeededRandoms
 def render_image(height, width, focal_length, tform_cam2world, model_coarse, model_fine, options, mode="validation",
                  encode_position_fn=None, encode_direction_fn=None, *, rays_per_chunk: Optional[int] = None,
                  device=None, impl: Optional[int] = None, randoms: Optional[SeededRandoms] = None, grid=None,
-                 early_stop: Optional[float] = None, normals: bool = False):
+                 early_stop: Optional[float] = None, normals=False):
     """One pose -> (rgb_coarse (H,W,3), disp_coarse (H,W), acc_coarse (H,W), rgb_fine, disp_fine, acc_fine).
 
     Like the reference, the per-chunk sampler options come from ``options.nerf.train`` unless
@@ -43,7 +43,14 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
     ``normals=True`` (impl 1, inference; combines with ``grid`` and ``early_stop``) returns a seventh output, the normal
     map (H, W, 3) of the last pass: the compositing weights times the outward unit normals -grad sigma / |grad sigma| at
     its samples, summed per ray and not renormalised (include/nerfb200.h "normal maps"); ``cast_to_normal_image``
-    turns it into uint8.  The six other outputs are exactly those of the call without it."""
+    turns it into uint8.  The six other outputs are exactly those of the call without it.  ``normals="world"`` gives
+    the normal map in world space: for an NDC scene (``options.dataset.no_ndc`` false) the gradient at each sample is
+    mapped by the Jacobian of this call's NDC map (``height``, ``width``, ``focal_length``) before it is normalised
+    and weighted (include/nerfb200.h "NDC scenes"); for a Blender scene it is exactly ``normals=True``."""
+    normals = train_utils.normals_mode(normals)
+    ndc = (height, width, focal_length) if normals == "world" else None
+    if ndc is not None:
+        train_utils._world_ndc(normals, options, ndc)  # a malformed camera is refused before any launch
     if randoms is not None and not isinstance(randoms, SeededRandoms):
         raise TypeError("render_image: randoms must be a SeededRandoms (tensors cannot span several chunks)")
     if device is None:
@@ -66,7 +73,8 @@ def render_image(height, width, focal_length, tform_cam2world, model_coarse, mod
             rays[i:i + chunk], model_coarse, model_fine, options, mode=inner_mode,
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if use_viewdirs else None, impl=impl, grid=grid,
-            early_stop=early_stop, normals=normals, randoms=randoms.shifted(i) if randoms is not None else None)
+            early_stop=early_stop, normals=normals, randoms=randoms.shifted(i) if randoms is not None else None,
+            _ndc=ndc)
             for i in range(0, n, chunk)]
     cols = [torch.cat(c, 0) if c[0] is not None else None for c in zip(*parts)]
     shapes = [(height, width, 3), (height, width), (height, width)] * 2 + [(height, width, 3)]

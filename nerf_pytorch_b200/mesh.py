@@ -245,7 +245,7 @@ def _sparse_surface(arch, blob, use, box, grid, level: float, want_dirs: bool, b
 def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), resolution=256, level: float = 50.0,
                  encode_direction_fn=None, colors: bool = False, impl: Optional[int] = None, *,
                  planes_per_slab: Optional[int] = None, normals: bool = False, grid=None,
-                 bricks_per_call: Optional[int] = None) -> Mesh:
+                 bricks_per_call: Optional[int] = None, ndc=None) -> Mesh:
     """The level set sigma = ``level`` of a trained FlexibleNeRFModel over ``bounds``, by marching cubes on the GPU.
 
     The density is ``density_volume(model, ...)`` (the fused MLP at the (R + 1)^3 lattice points); inside is
@@ -267,19 +267,33 @@ def extract_mesh(model, encode_position_fn, bounds=((-1.5,) * 3, (1.5,) * 3), re
     (include/nerfb200.h "sparse meshes").  Nothing is allocated at (R + 1)^3, so the lattice may pass 2^31 points (up to
     4096 cubes per axis).  Build the grid with ``OccupancyGrid.from_models(..., threshold=t)`` for some t below
     ``level`` (the default t = 0 is conservative): a surface in a brick the grid calls empty is missing from the mesh.
-    ``planes_per_slab`` belongs to the dense path and is refused with a grid."""
+    ``planes_per_slab`` belongs to the dense path and is refused with a grid.
+
+    ``ndc=(H, W, focal)`` is for a forward-facing (LLFF) scene, whose network encodes NDC points: ``bounds`` (and
+    ``grid``, e.g. ``OccupancyGrid.from_models`` of that scene) stay in NDC, where the lattice is uniform in
+    disparity as the render's samples are, with hi_z < 1 (z = 1 is the far plane at infinity), and the mesh is
+    extracted there as above, then mapped to world space by the inverse of ndc_rays (include/nerfb200.h "NDC
+    scenes"): the vertices are N^-1 of the NDC vertices, each face has its last two ids swapped so that it stays
+    counter-clockwise seen from outside (the map reverses orientation), colors are the network's at the NDC vertex
+    seen along the world direction of the density gradient (the frame the network's view directions were trained
+    in), and normals are the world normals -J^T g / |J^T g| of the NDC gradient g.  A malformed ``ndc`` or a box
+    reaching z = 1 raises ValueError before any launch."""
     return _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_direction_fn, colors, impl,
-                         planes_per_slab, normals, grid, bricks_per_call)[0]
+                         planes_per_slab, normals, grid, bricks_per_call, ndc=ndc)[0]
 
 
 def _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_direction_fn, colors, impl,
-                  planes_per_slab, normals, grid, bricks_per_call, edge_keys=False):
+                  planes_per_slab, normals, grid, bricks_per_call, edge_keys=False, ndc=None):
     """extract_mesh, and with ``edge_keys`` on the sparse path also each vertex's lattice edge q * 3 + a (a test
     hook: the dense mesh numbers its vertices in that key's order)."""
     from . import train_utils
     from . import density
 
+    cam = density.ndc_camera(ndc) if ndc is not None else None
     lo, hi, res = _box(bounds, resolution, dense=grid is None)
+    if cam is not None and not hi[2] < 1.0:
+        raise ValueError(f"mesh: with ndc=, the NDC bounds need hi_z < 1 (z = 1 is the far plane at infinity), got "
+                         f"{bounds!r}")
     level = _level(level)
     if grid is not None:
         if planes_per_slab is not None:
@@ -301,6 +315,9 @@ def _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_d
         _, blob = train_utils._packed(model, arch)
         verts, faces, dirs, keys = _sparse_surface(arch, blob, use, box, grid, level, want_dirs, bricks_per_call,
                                                    want_keys=edge_keys)
+    out_verts, out_faces = verts, faces
+    if cam is not None:  # the MLP queries below stay at the NDC vertices; what they return is in world space
+        out_verts, out_faces, dirs = ops.ndc_mesh_to_world(cam, verts, faces, dirs)
     rgb = None
     if colors:
         if verts.shape[0] == 0:
@@ -314,7 +331,10 @@ def _extract_mesh(model, encode_position_fn, bounds, resolution, level, encode_d
     nrm = None
     if normals:
         _, blob = train_utils._packed(model, arch)
-        _, g = density.density_grad_points(arch, blob, verts, grad_impl)
+        if cam is None:
+            _, g = density.density_grad_points(arch, blob, verts, grad_impl)
+        else:
+            _, g = density.ndc_density_grad_points(arch, blob, verts, grad_impl, cam)
         norm = torch.linalg.vector_norm(g, dim=-1, keepdim=True)
         nrm = torch.where(norm > 0, -g / norm, torch.zeros_like(g))
-    return Mesh(verts, faces, rgb, nrm), keys
+    return Mesh(out_verts, out_faces, rgb, nrm), keys

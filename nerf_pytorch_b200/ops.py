@@ -12,7 +12,7 @@ from typing import Optional, Sequence, Tuple
 import torch
 
 from . import _lib
-from ._lib import Arch, Grid, RenderOpts, Rng
+from ._lib import Arch, Grid, Ndc, RenderOpts, Rng
 
 IMPL_SIMT = 0  # fp32 CUDA cores
 IMPL_TC = 1    # wgmma tensor cores (fp16x2 three-term splits, fp32 accumulation)
@@ -753,9 +753,10 @@ def render_early_stop_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: 
 
 
 def render_fwd_normals(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid=None,
-                       stop: Optional[float] = None, impl: int = IMPL_TC):
+                       stop: Optional[float] = None, impl: int = IMPL_TC, ndc: Optional[Ndc] = None):
     """Inference ``render_fwd`` (with an occupancy ``grid`` and / or early stopping at ``stop`` when given) that also
-    returns the normal map of the last pass (include/nerfb200.h, "normal maps").  Returns (out_coarse, out_fine | None,
+    returns the normal map of the last pass (include/nerfb200.h, "normal maps").  ``ndc`` (an ``ndc_struct``) makes it
+    the world-space normal map of an NDC render of that camera ("NDC scenes").  Returns (out_coarse, out_fine | None,
     normals[N, 3], workspace); the workspace's first sections are laid out as ``render_workspace_layout(...,
     training=False)``."""
     lib = _lib.load()
@@ -777,12 +778,14 @@ def render_fwd_normals(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, r
     out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
     out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
     normals = torch.empty(n, 3, dtype=torch.float32, device=dev)
-    _lib.check(lib.nerfb200_render_fwd_normals(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                               _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
-                                               n, *_random_args(randoms), C.byref(g) if g is not None else None,
-                                               _ptr(bits), -1.0 if stop is None else float(stop), _ptr(out_c),
-                                               _ptr(out_f), _ptr(normals), _ptr(workspace), int(impl), _stream()),
-               "render_fwd_normals")
+    head = (C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts), _ptr(blob_c),
+            _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n, *_random_args(randoms),
+            C.byref(g) if g is not None else None, _ptr(bits), -1.0 if stop is None else float(stop))
+    tail = (_ptr(out_c), _ptr(out_f), _ptr(normals), _ptr(workspace), int(impl), _stream())
+    if ndc is None:
+        _lib.check(lib.nerfb200_render_fwd_normals(*head, *tail), "render_fwd_normals")
+    else:
+        _lib.check(lib.nerfb200_render_fwd_normals_ndc(*head, C.byref(ndc), *tail), "render_fwd_normals_ndc")
     return out_c, out_f, normals, workspace
 
 
@@ -961,3 +964,45 @@ def mesh_sparse_emit(box: Grid, brick_map, bricks, n_active: int, values, halo: 
         _ptr(dirs) if want_dirs and nv else None, _ptr(keys) if want_keys and nv else None, _stream()),
         "mesh_sparse_emit")
     return verts, faces, dirs, keys
+
+
+# ------------------------------------------------------------------------------------------------
+# NDC scenes (include/nerfb200.h "NDC scenes"): the map N of ndc_rays between world space and the NDC points a
+# forward-facing scene's MLP encodes, and its Jacobian
+# ------------------------------------------------------------------------------------------------
+def ndc_struct(height: int, width: int, focal: float) -> Ndc:
+    """The nerfb200_ndc_t of an image of ``height`` x ``width`` pixels and focal length ``focal`` (the call's H, W,
+    focal: the NDC map of its rays)."""
+    return Ndc(int(height), int(width), float(focal))
+
+
+def ndc_mesh_to_world(ndc: Ndc, vertices, faces, view_dirs=None):
+    """A mesh extracted in NDC, in world space: (N^-1 of each vertex (V, 3), faces (F, 3) with their last two ids
+    swapped, and with ``view_dirs`` each one's unit world direction J^T d, else None).  New tensors; the inputs are
+    kept."""
+    nv, nf = vertices.shape[0], faces.shape[0]
+    wv, wf = torch.empty_like(vertices), torch.empty_like(faces)
+    wd = torch.empty_like(view_dirs) if view_dirs is not None else None
+    _lib.check(_lib.load().nerfb200_ndc_mesh_to_world(
+        C.byref(ndc), _ptr(vertices) if nv else None, _ptr(faces) if nf else None,
+        _ptr(view_dirs) if view_dirs is not None and nv else None, nv, nf, _ptr(wv) if nv else None,
+        _ptr(wf) if nf else None, _ptr(wd) if wd is not None and nv else None, _stream()), "ndc_mesh_to_world")
+    return wv, wf, wd
+
+
+def ndc_from_world(ndc: Ndc, pts) -> torch.Tensor:
+    """q = N(p) for world points ``pts`` (P, 3)."""
+    q = torch.empty_like(pts)
+    _lib.check(_lib.load().nerfb200_ndc_from_world(C.byref(ndc), _ptr(pts) if pts.shape[0] else None, pts.shape[0],
+                                                   _ptr(q) if pts.shape[0] else None, _stream()), "ndc_from_world")
+    return q
+
+
+def ndc_grad_to_world(ndc: Ndc, q, rows, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(sigma, J^T(q) g) of ``density_grad`` rows (P, 4) = (sigma, g) at NDC points ``q`` (P, 3); ``out`` may be
+    ``rows``."""
+    out = torch.empty_like(rows) if out is None else out
+    n = q.shape[0]
+    _lib.check(_lib.load().nerfb200_ndc_grad_to_world(C.byref(ndc), _ptr(q) if n else None, _ptr(rows) if n else None,
+                                                      n, _ptr(out) if n else None, _stream()), "ndc_grad_to_world")
+    return out

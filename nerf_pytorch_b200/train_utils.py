@@ -452,6 +452,29 @@ def check_normals_call(impl, *models):
                                   "density gradient is built for impl 1 alone")
 
 
+def normals_mode(normals):
+    """The ``normals=`` of the render entry points: "world", or its truth value (ValueError for any other string)."""
+    if isinstance(normals, str):
+        if normals != "world":
+            raise ValueError(f"nerfb200: normals must be False, True or \"world\", got {normals!r}")
+        return normals
+    return bool(normals)
+
+
+def _world_ndc(normals, options, ndc):
+    """The NDC camera of a ``normals="world"`` render of NDC ``options`` (None otherwise: the MLP's frame is world
+    space already); ValueError when such a render has no (H, W, focal) to map with."""
+    if normals != "world" or getattr(getattr(options, "dataset", None), "no_ndc", True) is not False:
+        return None
+    if ndc is None:
+        raise ValueError("nerfb200: normals=\"world\" on an NDC scene needs the image's H, W and focal, which "
+                         "predict_and_render_radiance's packed rays do not carry; call run_one_iter_of_nerf or "
+                         "render_image")
+    from .density import ndc_camera
+
+    return ndc_camera(ndc)
+
+
 def _normals_impl(impl, arch_c, arch_f, nc, nf):
     """impl 1, after the library's refusal of the last pass's density gradient (the render's own come from the library
     before its first launch)."""
@@ -476,8 +499,9 @@ def predict_and_render_radiance(
     impl: Optional[int] = None,
     grid=None,
     early_stop: Optional[float] = None,
-    normals: bool = False,
+    normals: Union[bool, str] = False,
     _n_chunks: int = 1,
+    _ndc=None,
 ):
     """nerf/train_utils.py:28-127 for one chunk of packed rays ``[o d near far (viewdir)]``.
 
@@ -499,7 +523,12 @@ def predict_and_render_radiance(
     ``normals``: also return the last pass's normal map N (n_rays, 3) as a seventh output (inference only, impl 1,
     with or without ``grid`` / ``early_stop``): the sum of the compositing weights times the outward unit normals
     -grad sigma / |grad sigma| at the pass's samples (include/nerfb200.h "normal maps"); not renormalised, so |N| <=
-    acc.  False returns exactly the six outputs."""
+    acc.  False returns exactly the six outputs.  ``normals="world"`` is the normal map in world space: for a Blender
+    scene the same as True; for an NDC scene (``options.dataset.no_ndc`` false) it needs the image's H, W and focal,
+    which packed rays do not carry, so it is refused here (ValueError): ``run_one_iter_of_nerf`` and ``render_image``
+    provide it."""
+    normals = normals_mode(normals)
+    cam = _world_ndc(normals, options, _ndc)
     impl = _requested_impl(impl, model_coarse, model_fine)
     if normals:
         check_normals_call(impl, model_coarse, model_fine)
@@ -563,7 +592,8 @@ def predict_and_render_radiance(
     nrm = None
     if normals:
         out_c, out_f, nrm, _ = ops.render_fwd_normals(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid,
-                                                   None if early_stop is None else float(early_stop), impl=impl)
+                                                   None if early_stop is None else float(early_stop), impl=impl,
+                                                   ndc=cam)
     elif early_stop is not None:
         out_c, out_f, _ = ops.render_fwd_early_stop(arch_c, arch_f, opts, blob_c, blob_f, rays, rnd, grid,
                                                     float(early_stop), impl=impl)
@@ -594,12 +624,17 @@ def run_one_iter_of_nerf(
     impl: Optional[int] = None,
     grid=None,
     early_stop: Optional[float] = None,
-    normals: bool = False,
+    normals: Union[bool, str] = False,
 ):
     """nerf/train_utils.py:130-202: ray packing (viewdirs, optional NDC, near/far), chunking by
     ``options.nerf.<mode>.chunksize``, per-chunk render, concatenation and -- in "validation" mode --
     the reshape back to image shape.  ``normals=True`` appends the normal map of the last pass (see
-    ``predict_and_render_radiance``) as a seventh output."""
+    ``predict_and_render_radiance``) as a seventh output; ``normals="world"`` gives it in world space, for an NDC
+    scene through the NDC map of ``height``, ``width`` and ``focal_length`` (include/nerfb200.h "NDC scenes")."""
+    normals = normals_mode(normals)
+    ndc = (height, width, focal_length) if normals == "world" else None
+    if ndc is not None:
+        _world_ndc(normals, options, ndc)  # a malformed camera is refused before any launch
     impl = _requested_impl(impl, model_coarse, model_fine)
     if normals:
         check_normals_call(impl, model_coarse, model_fine)
@@ -620,7 +655,7 @@ def run_one_iter_of_nerf(
                          options.dataset.far, use_viewdirs)
 
     return _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn,
-                          encode_direction_fn, randoms, impl, grid, early_stop, normals)
+                          encode_direction_fn, randoms, impl, grid, early_stop, normals, ndc)
 
 
 def run_one_iter_of_nerf_from_pose(
@@ -662,7 +697,7 @@ def run_one_iter_of_nerf_from_pose(
 
 
 def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode, encode_position_fn, encode_direction_fn,
-                   randoms, impl, grid=None, early_stop=None, normals=False):
+                   randoms, impl, grid=None, early_stop=None, normals=False, ndc=None):
     """Chunking, per-chunk render, concatenation and the validation reshape of train_utils.py:170-202.
     Seeded randoms follow each ray: chunk i starts at ``ray_offset`` + the index of its first ray."""
     chunksize = getattr(options.nerf, mode).chunksize
@@ -677,7 +712,7 @@ def _render_packed(rays, restore_shapes, model_coarse, model_fine, options, mode
             encode_position_fn=encode_position_fn,
             encode_direction_fn=encode_direction_fn if options.nerf.use_viewdirs else None,
             randoms=randoms.shifted(i * chunksize) if seeded else randoms, impl=impl, grid=grid,
-            early_stop=early_stop, normals=normals, _n_chunks=len(batches),
+            early_stop=early_stop, normals=normals, _n_chunks=len(batches), _ndc=ndc,
         )
         for i, batch in enumerate(batches)
     ]
