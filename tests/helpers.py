@@ -176,6 +176,48 @@ def composite64(raw, z, dirs, noise_std=0.0, white_background=False, noise=None,
     return rgb, disp, acc, weights, depth
 
 
+def transmittance64(raw, z, rays, noise, std):
+    """fp64 exclusive transmittance [n, S + 1] of fp32 raw [n, S, 4] at depths z [n, S] along rays [n, >= 6]:
+    T[:, p] = prod over samples < p of 1 - alpha + 1e-10, with the sigma gate and the last sample's sigma taken from the
+    fp32 pre-activation as the compositing rounds them (noise [n, S] times std, or std 0 and noise None)."""
+    pre32, pre64 = raw[..., 3], raw[..., 3].double()
+    if std > 0:
+        std32 = torch.tensor(std, dtype=torch.float32, device=raw.device)
+        pre32 = pre32 + noise * std32
+        pre64 = pre64 + noise.double() * float(std32)
+    sigma = torch.where(pre32 > 0, torch.cat((pre64[:, :-1], pre32[:, -1:].double()), 1), 0.0)
+    z64 = z.double()
+    dists = torch.cat((z64[:, 1:] - z64[:, :-1], torch.full_like(z64[:, :1], 1e10)), 1)
+    dists = dists * rays[:, 3:6].double().norm(dim=1, keepdim=True)
+    q = torch.exp(-sigma * dists) + 1e-10
+    return torch.cat((torch.ones_like(q[:, :1]), torch.cumprod(q, 1)), 1)
+
+
+def skipped_samples(grid, rays, z):
+    """bool [n, S]: the samples at depths z [n, S] of rays [n, >= 6] that an occupancy grid skips, the fp32 points
+    o + d z inside its box in a clear cell (OccupancyGrid.cell_of); points outside the box are always evaluated."""
+    pts = rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]
+    cell = grid.cell_of(pts)
+    occ = grid.occupancy().reshape(-1)
+    return (cell >= 0) & ~occ[cell.clamp_min(0)]
+
+
+def compaction_reference(grid, rays, z):
+    """Torch restatement of one pass's sample compaction (nerfb200_grid_compact): (keep [n, S], map rows, blocks).  The
+    kept points of each group of 10 rays, in (ray, sample) order, fill 64-row blocks from the group's first block; a
+    group's last block is padded with -1; each block is (first ray, last ray) of its rows."""
+    n, s = z.shape
+    keep = ~skipped_samples(grid, rays, z)
+    rows, blocks = [], []
+    for g0 in range(0, n, 10):
+        pts = (torch.nonzero(keep[g0:g0 + 10].reshape(-1)).reshape(-1) + g0 * s).tolist()
+        for b0 in range(0, len(pts), 64):
+            chunk = pts[b0:b0 + 64]
+            blocks.append((chunk[0] // s, chunk[-1] // s))
+            rows += chunk + [-1] * (64 - len(chunk))
+    return keep, rows, blocks
+
+
 def bits_equal(a, b):
     """Same shape and the same bits (4-byte elements); two Nones are equal."""
     if a is None or b is None:

@@ -60,6 +60,59 @@ FP32_TIE_TOL = 1e-5
 # (test_stage_parity_gpu.py).
 COMP_TOL = 1e-4
 COMP_GRAD_TOL = 2e-4
+# Early ray termination (helpers.transmittance64): how far the fp64 transmittance of the default raw may sit on the wrong
+# side of the threshold t, relative to t.  Measured on an H100 80GB HBM3 over test_early_stop_gpu.py's cases: at most
+# 0.99934 t at a stop and at least 1.00004 t at every earlier boundary.
+T_REL = 2e-3
+# Normal maps against normals64: |N - N64| per ray against the conditioning of its samples.  A gradient error of G_ERR
+# times the pass's largest |grad| (test_density_grad_gpu bounds it by 2e-5 off ReLU ties) turns a sample's unit normal by
+# at most 2 G_ERR max|g| / |g_i| (and never by more than 2), times its weight.  Samples where |grad| nearly vanishes are
+# where N is ill-conditioned; a sample with a ReLU tie may turn its normal by up to 2 (times its weight).  Measured on an
+# H100 80GB HBM3 at 700 W, the unconditioned worst is 1.1e-6 (lego), 6.8e-3 (fern, lego with noise).  ACC_EPS: |N| <= acc
+# + ACC_EPS.
+G_ERR = 1e-4
+N_FLOOR = 1e-5
+ACC_EPS = 1e-5
+
+
+# Scenes of the render tests (test_occupancy_gpu, test_early_stop_gpu, test_normals_render_gpu): (shipped weights or
+# None, H, W, focal, pose, no_ndc, near, far, L_xyz, (coarse, fine) networks, bounds of a grid).  A network is (layers,
+# hidden, skip, weights): "shipped" (the scene's coarse / fine pair), "init" (torch's init under seed 7, in order) or
+# ("scaled", seed) (arch_weights: max |raw| ~ 3e3, so rays turn opaque and early stopping fires).  These run the
+# pretrained architecture, 8 x 256 skip 4 (A2), in the last pass, the first or both, on the lego camera; their grid box
+# leaves the image's outer rays outside it.
+_BOX = ((-0.7,) * 3, (0.7,) * 3)
+H256_SCENES = {
+    "a2": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10, ((8, 256, 4, ("scaled", 1)), (8, 256, 4, ("scaled", 2))),
+           _BOX),
+    "mixed": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10,
+              ((8, 128, 3, ("scaled", 3)), (8, 256, 4, ("scaled", 2))), _BOX),
+    "mixed_rev": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10,
+                  ((8, 256, 4, ("scaled", 1)), (8, 128, 3, ("scaled", 5))), _BOX),
+}
+
+
+def scene_models(scene):
+    """The (coarse, fine) FlexibleNeRFModels of a scene row (H256_SCENES' format) on the GPU."""
+    import nerf_pytorch_b200 as nb
+    from helpers import load_weights
+    from nerf_pytorch_b200 import ops
+
+    weights, *_, l_xyz, nets, _ = scene
+    shipped = load_weights(weights) if weights else None
+    if any(state == "init" for *_, state in nets):
+        torch.manual_seed(7)
+    out = []
+    for i, (layers, hidden, skip, state) in enumerate(nets):
+        m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=hidden, skip_connect_every=skip,
+                                 num_encoding_fn_xyz=l_xyz, num_encoding_fn_dir=4)
+        if state == "shipped":
+            m.load_state_dict(shipped[i])
+        elif state != "init":
+            arch = ops.ArchSpec(num_layers=layers, hidden=hidden, skip_every=skip, n_freq_xyz=l_xyz, n_freq_dir=4)
+            m.load_state_dict(arch_weights(arch, *state))
+        out.append(m.cuda())
+    return out
 
 
 def spec(name):
@@ -69,6 +122,11 @@ def spec(name):
     if name in H256_ARCHS:
         return ops.ArchSpec(hidden=256, skip_every=4, **H256_ARCHS[name])
     return ops.ArchSpec(hidden=128, **ALL_ARCHS[name])
+
+
+def arch_name(arch):
+    """The table name of an ops.ArchSpec (its repr if it is in neither table)."""
+    return next((k for k in [*H256_ARCHS, *ALL_ARCHS] if spec(k) == arch), repr(arch))
 
 
 def sms():
@@ -144,12 +202,12 @@ def _scaled(sd, c):
 
 
 @functools.lru_cache(maxsize=None)
-def arch_weights(arch, state):
-    """Seeded reference init of `arch` (an ops.ArchSpec); "scaled": every gemm layer's weight and bias times one factor
-    c, found by bisection so that max |raw| over a probe batch is ~3e3."""
+def arch_weights(arch, state, seed=2024):
+    """Reference init of `arch` (an ops.ArchSpec) seeded with `seed`; "scaled": every gemm layer's weight and bias times
+    one factor c, found by bisection so that max |raw| over a probe batch is ~3e3."""
     sd = O.init_flexible_nerf(arch.num_layers, arch.hidden, arch.skip_every, arch.n_freq_xyz, arch.n_freq_dir,
                               include_input_xyz=arch.include_input_xyz, include_input_dir=arch.include_input_dir,
-                              use_viewdirs=arch.use_viewdirs, generator=torch.Generator().manual_seed(2024))
+                              use_viewdirs=arch.use_viewdirs, generator=torch.Generator().manual_seed(seed))
     if state == "init":
         return sd
     rays, z = points(arch, 16, 64, seed=99)
@@ -505,6 +563,86 @@ def oracle_tiles(arch, sd, rays, z, G=None, tiles=None, chunk_tiles=128, visit=N
             visit(p0, p1, rays_c, z_c, acts)
         del raw, acts, dpre, grads
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# density gradients and normal maps
+# ------------------------------------------------------------------------------------------------------------------------
+def relu_tie_points(sd64, xyz, hidden):
+    """Points with a ReLU tie: a layers_xyz unit within STASH_TOL of its layer's largest activation (over this batch)
+    from zero in fp64, where the kernel's decision may be the other one.  xyz: the fp64 xyz encoding [P][dim_xyz]."""
+    h = torch.nn.functional.linear(xyz, sd64["layer1.weight"], sd64["layer1.bias"])
+    tie = torch.zeros(xyz.shape[0], dtype=torch.bool, device=xyz.device)
+    i = 0
+    while f"layers_xyz.{i}.weight" in sd64:
+        w = sd64[f"layers_xyz.{i}.weight"]
+        if w.shape[1] != hidden:
+            h = torch.cat((h, xyz), -1)
+        pre = torch.nn.functional.linear(h, w, sd64[f"layers_xyz.{i}.bias"])
+        tie |= (pre.abs() <= STASH_TOL * pre.max().clamp_min(0.0)).any(-1)
+        h = torch.relu(pre)
+        i += 1
+    return tie
+
+
+def sigma_grad64(arch, sd, pts):
+    """fp64 autograd of sigma (raw column 3, the fc_alpha output or fc_out's fourth) with respect to the fp32 points
+    pts [P][3], and the points with a ReLU tie (relu_tie_points).  The bands' arguments are the fp32 products x * f as
+    values (as embed forms them) with the derivative f, for log-sampled and linear bands, with or without the raw input;
+    sigma does not depend on the view direction, which is +z."""
+    from nerf_pytorch_b200 import ops
+
+    sd64 = {k: v.double().to(pts.device) for k, v in sd.items()}
+    bands = ops.frequency_bands(arch.n_freq_xyz, arch.log_sampling_xyz).tolist()
+    d = torch.tensor([0.0, 0.0, 1.0], device=pts.device)
+    out, ties = [], []
+    for p0 in range(0, pts.shape[0], 1 << 17):
+        x32 = pts[p0:p0 + (1 << 17)]
+        x64 = x32.double().requires_grad_()
+        parts = [x64] if arch.include_input_xyz else []
+        for f in bands:
+            a = x64 * f + ((x32 * f).double() - x64.detach() * f)
+            parts += [torch.sin(a), torch.cos(a)]
+        xyz = torch.cat(parts, -1)
+        emb = xyz
+        if arch.use_viewdirs:
+            view = embed(d.expand(x32.shape[0], 3), arch.n_freq_dir, arch.include_input_dir, arch.log_sampling_dir)
+            emb = torch.cat((xyz, view), -1)
+        raw = O.flexible_nerf_forward(sd64, emb, arch.dim_xyz)
+        g, = torch.autograd.grad(raw[:, 3].sum(), x64)
+        out.append(g)
+        with torch.no_grad():
+            ties.append(relu_tie_points(sd64, xyz.detach(), arch.hidden))
+    return torch.cat(out), torch.cat(ties)
+
+
+def normals64(arch, sd, rays, z, raw, noise_std=0.0, noise=None):
+    """fp64 restatement of a render's normal map from its last pass: depths z [n][S] and raw [n][S][4] read from the
+    render's workspace, the fp64 compositing weights of that raw (helpers.composite64, with the noise the render used),
+    and the outward unit normal -grad sigma / |grad sigma| by sigma_grad64 at o + d z, summed in sample order.
+    Returns (N64 [n][3], bound [n], live samples, tie samples): bound is the allowance on |N - N64| per ray, the sum of
+    its samples' weights times how far each may turn (G_ERR relative to the pass's largest |grad|, 2 at a ReLU tie),
+    plus N_FLOOR."""
+    from helpers import composite64
+
+    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).reshape(-1, 3)
+    _, _, _, w64, _ = composite64(raw, z, rays[:, 3:6], noise_std=noise_std, noise=noise)
+    w64 = w64.reshape(-1)
+    live = w64 != 0
+    g = torch.zeros(pts.shape[0], 3, dtype=torch.float64, device=pts.device)
+    tie = torch.zeros(pts.shape[0], dtype=torch.bool, device=pts.device)
+    if live.any():
+        g[live], tie[live] = sigma_grad64(arch, sd, pts[live].contiguous())
+    mag = g.norm(dim=-1, keepdim=True)
+    nrm64 = torch.where(mag > 0, -g / mag, torch.zeros_like(g))
+    terms = (w64[:, None] * nrm64).view(rays.shape[0], -1, 3)
+    N64 = torch.zeros(rays.shape[0], 3, dtype=torch.float64, device=pts.device)
+    for j in range(terms.shape[1]):  # in sample order
+        N64 += terms[:, j]
+    turn = torch.clamp(2 * G_ERR * mag.max() / mag.squeeze(-1).clamp_min(1e-300), max=2.0)
+    turn[tie] = 2.0  # a ReLU tie may turn its sample's normal anywhere
+    bound = (w64 * turn).view(rays.shape[0], -1).sum(-1) + N_FLOOR
+    return N64, bound, int(live.sum()), int(tie.sum())
 
 
 # ------------------------------------------------------------------------------------------------------------------------

@@ -13,16 +13,23 @@ import math
 import pytest
 import torch
 
-from helpers import OUT_NAMES, bits_equal, load_weights
+import mlp_checks as M
+from helpers import OUT_NAMES, bits_equal, transmittance64
+from mlp_checks import T_REL
 
 pytestmark = pytest.mark.gpu
 
-# (weights or None for A1 at init, H, W, focal, pose, no_ndc, near, far, L_xyz, layers, skip, bounds of a grid)
+# (shipped weights or None, H, W, focal, pose, no_ndc, near, far, L_xyz, (coarse, fine) networks, bounds of a grid):
+# mlp_checks.H256_SCENES' format
+A0, A1 = (4, 128, 4, "shipped"), (8, 128, 3, "init")
 SCENES = {
-    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, 4, 4, ((-1.5,) * 3, (1.5,) * 3)),
-    "a1": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10, 8, 3, ((-1.5,) * 3, (1.5,) * 3)),
-    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, 4, 4, ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, (A0, A0), ((-1.5,) * 3, (1.5,) * 3)),
+    "a1": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10, (A1, A1), ((-1.5,) * 3, (1.5,) * 3)),
+    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, (A0, A0), ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    **M.H256_SCENES,
 }
+# the scenes whose networks run hidden 256 in some pass
+H256 = list(M.H256_SCENES)
 VARIANTS = {  # (perturb, noise_std, white_bkgd)
     "det": (False, 0.0, False),
     "perturb_noise": (True, 1.0, False),
@@ -30,10 +37,8 @@ VARIANTS = {  # (perturb, noise_std, white_bkgd)
 }
 IMPLS = {"impl1": 1, "impl3": 3}
 SKIP = torch.tensor([0.0, 0.0, 0.0, -math.inf])
-# fp32 rounding allowances (figures printed under -s).  Measured on an H100 80GB HBM3 over every case below: the fp64
-# transmittance of the default raw is at most 0.99934 t at a stop and at least 1.00004 t at every earlier boundary, and
-# no output moved against the guarantee's sign by more than 1.2e-7
-T_REL = 2e-3
+# fp32 rounding allowance of the outputs (figures printed under -s; T_REL, the transmittance's, is mlp_checks').
+# Measured on an H100 80GB HBM3 over every case below, no output moved against the guarantee's sign by more than 1.2e-7
 OUT_ABS = 2e-6
 
 
@@ -42,20 +47,7 @@ def report(what, ctx, value):
 
 
 def _models(scene):
-    import nerf_pytorch_b200 as nb
-
-    weights, *_, l_xyz, layers, skip, _ = SCENES[scene]
-    if weights is None:
-        torch.manual_seed(7)
-        return [nb.FlexibleNeRFModel(num_layers=layers, hidden_size=128, skip_connect_every=skip,
-                                     num_encoding_fn_xyz=l_xyz, num_encoding_fn_dir=4).cuda() for _ in range(2)]
-    out = []
-    for sd in load_weights(weights):
-        m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=128, skip_connect_every=skip, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out
+    return M.scene_models(SCENES[scene])
 
 
 def _pose(kind):
@@ -71,12 +63,13 @@ def _setup(scene, variant="det", n_fine=128):
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
     mc, mf = _models(scene)
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
-    arch = train_utils._arch_of(mc, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
-    blobs = [train_utils._packed(m, arch)[1] for m in (mc, mf)]
+    archs = tuple(train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
+                  for m in (mc, mf))
+    blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
     opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
     rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
-    return arch, blobs, opts, rays, (mc, mf), (epf, edf)
+    return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
 
 def _grid(scene, kind, models=None, encoders=None):
@@ -118,17 +111,29 @@ def _reference(arch, arch_f, blobs, opts, rays, rng, grid, impl):
 @pytest.mark.parametrize("variant", list(VARIANTS))
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_zero_threshold_is_the_default_render_bit_for_bit(impl, variant, grid_kind):
+    _zero_threshold_is_the_default_render_bit_for_bit(impl, "lego", variant, grid_kind)
+
+
+@pytest.mark.parametrize("grid_kind", [None, "rand50", "full"])
+@pytest.mark.parametrize("variant", list(VARIANTS))
+@pytest.mark.parametrize("scene", H256)
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_zero_threshold_is_the_default_render_bit_for_bit_at_hidden_256(impl, scene, variant, grid_kind):
+    _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid_kind)
+
+
+def _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid_kind):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    arch, blobs, opts, rays, _, _ = _setup("lego", variant)
-    grid = _grid("lego", grid_kind)
+    (arch, arch_f), blobs, opts, rays, _, _ = _setup(scene, variant)
+    grid = _grid(scene, grid_kind)
     rng = nb.SeededRandoms(5, 2)
     n = rays.shape[0]
-    oc, of, _, ne_ref = _reference(arch, arch, blobs, opts, rays, rng, grid, IMPLS[impl])
-    ec, ef, ne, stop = ops.render_fwd_early_stop(arch, arch, opts, blobs[0], blobs[1], rays, rng, grid, 0.0,
+    oc, of, _, ne_ref = _reference(arch, arch_f, blobs, opts, rays, rng, grid, IMPLS[impl])
+    ec, ef, ne, stop = ops.render_fwd_early_stop(arch, arch_f, opts, blobs[0], blobs[1], rays, rng, grid, 0.0,
                                                  impl=IMPLS[impl], want_stop=True)
-    assert bits_equal(ec, oc) and bits_equal(ef, of), (impl, variant, grid_kind)
+    assert bits_equal(ec, oc) and bits_equal(ef, of), (impl, scene, variant, grid_kind)
     assert (stop == 192).all()
     assert ne.tolist() == ([n * 64, n * 192] if grid is None else ne_ref.tolist())
 
@@ -144,22 +149,6 @@ def test_zero_threshold_is_the_default_render_bit_for_bit(impl, variant, grid_ki
 # ------------------------------------------------------------------------------------------------------------------------
 # 2, 3. per ray, and the output bounds
 # ------------------------------------------------------------------------------------------------------------------------
-def _transmittance64(raw, z, rays, noise, std):
-    """fp64 exclusive transmittance [n, S + 1] of fp32 raw: T[:, p] = prod over samples < p of 1 - alpha + 1e-10, with
-    the sigma gate and the last sample's sigma taken from the fp32 pre-activation as the compositing rounds them."""
-    pre32, pre64 = raw[..., 3], raw[..., 3].double()
-    if std > 0:
-        std32 = torch.tensor(std, dtype=torch.float32, device=raw.device)
-        pre32 = pre32 + noise * std32
-        pre64 = pre64 + noise.double() * float(std32)
-    sigma = torch.where(pre32 > 0, torch.cat((pre64[:, :-1], pre32[:, -1:].double()), 1), 0.0)
-    z64 = z.double()
-    dists = torch.cat((z64[:, 1:] - z64[:, :-1], torch.full_like(z64[:, :1], 1e10)), 1)
-    dists = dists * rays[:, 3:6].double().norm(dim=1, keepdim=True)
-    q = torch.exp(-sigma * dists) + 1e-10
-    return torch.cat((torch.ones_like(q[:, :1]), torch.cumprod(q, 1)), 1)
-
-
 _CACHE = {}
 
 
@@ -171,16 +160,16 @@ def _stopped_render(impl, scene, variant, grid_kind, t):
     if key in _CACHE:
         return _CACHE[key]
     _CACHE.clear()
-    arch, blobs, opts, rays, models, enc = _setup(scene, variant)
+    archs, blobs, opts, rays, models, enc = _setup(scene, variant)
     grid = _grid(scene, grid_kind, models, enc)
     rng = nb.SeededRandoms(9, 4)
-    oc, of, ws, _ = _reference(arch, arch, blobs, opts, rays, rng, grid, IMPLS[impl])
-    ec, ef, ne, stop = ops.render_fwd_early_stop(arch, arch, opts, blobs[0], blobs[1], rays, rng, grid, t,
+    oc, of, ws, _ = _reference(*archs, blobs, opts, rays, rng, grid, IMPLS[impl])
+    ec, ef, ne, stop = ops.render_fwd_early_stop(*archs, opts, blobs[0], blobs[1], rays, rng, grid, t,
                                                  impl=IMPLS[impl], want_stop=True)
     n = rays.shape[0]
-    lay = ops.render_workspace_layout(arch, arch, opts, n, False)
-    es_ws = torch.empty(ops.render_early_stop_workspace_bytes(arch, arch, opts, n), dtype=torch.uint8, device="cuda")
-    ops.render_fwd_early_stop(arch, arch, opts, blobs[0], blobs[1], rays, rng, grid, t, impl=IMPLS[impl],
+    lay = ops.render_workspace_layout(*archs, opts, n, False)
+    es_ws = torch.empty(ops.render_early_stop_workspace_bytes(*archs, opts, n), dtype=torch.uint8, device="cuda")
+    ops.render_fwd_early_stop(*archs, opts, blobs[0], blobs[1], rays, rng, grid, t, impl=IMPLS[impl],
                               workspace=es_ws)
     torch.cuda.synchronize()
     out = dict(opts=opts, rays=rays, rng=rng, ref=(oc, of), es=(ec, ef), ne=ne, stop=stop.long(),
@@ -193,7 +182,10 @@ def _stopped_render(impl, scene, variant, grid_kind, t):
 PER_RAY = [(impl, scene, variant, grid_kind, t)
            for impl in IMPLS for t in (1e-4, 1e-2, 0.1)
            for scene, variant, grid_kind in (("lego", "det", None), ("lego", "perturb_noise", "rand50"),
-                                             ("lego", "white_perturb", None), ("fern", "det", "model"))]
+                                             ("lego", "white_perturb", None), ("fern", "det", "model"),
+                                             ("a2", "det", None), ("a2", "perturb_noise", "rand50"),
+                                             ("a2", "white_perturb", "model"), ("mixed", "det", "rand50"),
+                                             ("mixed_rev", "perturb_noise", None))]
 
 
 @pytest.mark.parametrize("impl,scene,variant,grid_kind,t", PER_RAY)
@@ -214,6 +206,8 @@ def test_per_ray_contract(impl, scene, variant, grid_kind, t):
     assert bits_equal(es_raw, want), ctx
     stopped = stop < S
     report("stopped rays / all", ctx, f"{int(stopped.sum())} / {n}")
+    if scene == "a2" and t >= 1e-2:
+        assert stopped.any(), ctx  # the scaled weights turn rays opaque: the contract is not vacuous
     assert (r["ne"][1] == (keep & before).sum()).item(), ctx
     assert bits_equal(r["es"][1][~stopped], r["ref"][1][~stopped]), ctx
 
@@ -226,7 +220,7 @@ def test_per_ray_contract(impl, scene, variant, grid_kind, t):
     assert (stop[stopped] == last_ran[stopped] + 1).all(), ctx
 
     noise = ops.random_fill(r["rng"], "noise_f", n, S) if r["opts"].noise_std > 0 else None
-    T = _transmittance64(raw, z, r["rays"], noise, r["opts"].noise_std)
+    T = transmittance64(raw, z, r["rays"], noise, r["opts"].noise_std)
     # at the stop T < t; at every earlier boundary with samples left (and every boundary of an unstopped ray) T >= t
     if stopped.any():
         at_stop = T[stopped, stop[stopped]]
@@ -285,17 +279,29 @@ def _image(scene, impl, chunk, grid=None, randoms=None, early_stop=None, perturb
 @pytest.mark.parametrize("grid_kind", [None, "rand50"])
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_render_image_is_deterministic_and_chunking_invariant(impl, grid_kind):
+    _render_image_is_deterministic_and_chunking_invariant(impl, "lego", grid_kind)
+
+
+@pytest.mark.parametrize("grid_kind", [None, "rand50"])
+@pytest.mark.parametrize("scene", H256)
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_render_image_is_deterministic_and_chunking_invariant_at_hidden_256(impl, scene, grid_kind):
+    _render_image_is_deterministic_and_chunking_invariant(impl, scene, grid_kind)
+
+
+def _render_image_is_deterministic_and_chunking_invariant(impl, scene, grid_kind):
     import nerf_pytorch_b200 as nb
 
-    grid = _grid("lego", grid_kind)
+    grid = _grid(scene, grid_kind)
     rng = nb.SeededRandoms(21, 1)
-    whole = _image("lego", IMPLS[impl], 48 * 48, grid, rng, 1e-2)
-    again = _image("lego", IMPLS[impl], 48 * 48, grid, rng, 1e-2)
+    n = SCENES[scene][1] * SCENES[scene][2]
+    whole = _image(scene, IMPLS[impl], n, grid, rng, 1e-2)
+    again = _image(scene, IMPLS[impl], n, grid, rng, 1e-2)
     assert all(bits_equal(a, b) for a, b in zip(whole, again))
     for chunk in (1000, 333):
-        part = _image("lego", IMPLS[impl], chunk, grid, rng, 1e-2)
-        assert all(bits_equal(a, b) for a, b in zip(whole, part)), chunk
-    default = _image("lego", IMPLS[impl], 48 * 48, grid, rng)
+        part = _image(scene, IMPLS[impl], chunk, grid, rng, 1e-2)
+        assert all(bits_equal(a, b) for a, b in zip(whole, part)), (scene, chunk)
+    default = _image(scene, IMPLS[impl], n, grid, rng)
     assert not all(bits_equal(a, b) for a, b in zip(whole, default))  # some ray did stop
     assert bits_equal(whole[0], default[0])  # the coarse pass never stops
 
@@ -315,7 +321,7 @@ def test_shipped_weights(impl, scene, grid_kind):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    arch, blobs, opts, rays, models, enc = _setup(scene)
+    (arch, _), blobs, opts, rays, models, enc = _setup(scene)
     grid = _grid(scene, grid_kind, models, enc)
     rng = nb.SeededRandoms(3, 0)
     full = _grid(scene, "full")
@@ -344,7 +350,7 @@ def test_early_stop_refusals_fire_before_any_launch():
     from nerf_pytorch_b200 import ops
     from oracle import nerf_oracle as O
 
-    arch, blobs, opts, rays, (mc, mf), (epf, edf) = _setup("lego")
+    (arch, _), blobs, opts, rays, (mc, mf), (epf, edf) = _setup("lego")
     kw = dict(encode_position_fn=epf, encode_direction_fn=edf)
     o = O.make_options(num_coarse=64, num_fine=64)
     with torch.no_grad():  # pack both models once, so that nothing below is a first use
@@ -377,4 +383,19 @@ def test_early_stop_refusals_fire_before_any_launch():
                 ops.render_fwd_early_stop(arch, arch, opts, blobs[0], blobs[1], rays, {}, None, t)
         with pytest.raises(NotImplementedError, match="impl=0"):
             ops.render_fwd_early_stop(arch, arch, opts, blobs[0], blobs[1], rays, {}, grid, 0.1, impl=ops.IMPL_SIMT)
+        # 8x256 with L_dir 6: 39 direction channels, wider than the wgmma forward's 32
+        ldir6 = [nb.FlexibleNeRFModel(num_layers=8, hidden_size=256, num_encoding_fn_xyz=10, num_encoding_fn_dir=6).cuda()
+                 for _ in range(2)]
+        kw6 = dict(encode_position_fn=epf, encode_direction_fn=nb.get_embedding_function(6))
+        for g in (None, grid):
+            for impl in (None, ops.IMPL_TC, ops.IMPL_TC_FAST):
+                with pytest.raises(NotImplementedError, match="32"):
+                    nb.predict_and_render_radiance(rays, *ldir6, o, grid=g, early_stop=0.1, impl=impl, **kw6)
+        a6 = ops.ArchSpec(num_layers=8, hidden=256, n_freq_xyz=10, n_freq_dir=6)
+        blob6 = torch.zeros(a6.blob_floats(), device="cuda")
+        for impl in (ops.IMPL_TC, ops.IMPL_TC_FAST):
+            with pytest.raises(NotImplementedError, match="32"):
+                ops.render_fwd_early_stop(a6, a6, opts, blob6, blob6, rays, {}, None, 0.1, impl=impl)
     assert ops.launch_count() == before
+    with torch.no_grad(), pytest.raises(NotImplementedError, match="32"):  # after generating the image's rays
+        nb.render_image(16, 16, 20.0, torch.eye(4), *ldir6, o, early_stop=0.1, **kw6)

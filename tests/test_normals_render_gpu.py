@@ -1,33 +1,32 @@
 """Normal maps of renders (include/nerfb200.h, "normal maps"; csrc/normals.cu and density_grad_tc_kernel) on the GPU:
   * with normals=True the six render outputs are bit for bit those of the same call without it: the default render,
     with an occupancy grid, with early stopping, and with both;
-  * N against an fp64 restatement from the render's own workspace: the last pass's depths and raw outputs, the fp64
-    compositing weights of that raw (with the seeded noise the render used), and grad sigma by fp64 autograd at o + d z,
-    summed in sample order -- lego A0 (Blender), fern A0 (NDC), a coarse-only network, a seeded perturb + noise render;
+  * N against an fp64 restatement from the render's own workspace (mlp_checks.normals64): the last pass's depths and
+    raw outputs, the fp64 compositing weights of that raw (with the seeded noise the render used), and grad sigma by fp64
+    autograd at o + d z, summed in sample order -- lego A0 (Blender), fern A0 (NDC), a coarse-only network, a seeded
+    perturb + noise render, 8 x 256 networks (A2) and A1 / A2 mixed across the two passes, with and without a grid and
+    early stopping;
   * |N| <= acc + eps, N = 0 exactly where acc = 0;
   * cast_to_normal_image, and the refusals (a call that would train, impl 0, impl 3) before any launch."""
 import pytest
 import torch
 
 import mlp_checks as M
-from helpers import bits_equal, composite64, load_weights
+from helpers import bits_equal
+from mlp_checks import ACC_EPS, G_ERR, N_FLOOR
 from oracle import nerf_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-# (weights, H, W, focal, pose, no_ndc, near, far, L_xyz, bounds of a grid)
+# (shipped weights or None, H, W, focal, pose, no_ndc, near, far, L_xyz, (coarse, fine) networks, bounds of a grid):
+# mlp_checks.H256_SCENES' format.  The bars on N (G_ERR, N_FLOOR, ACC_EPS) are mlp_checks'.
+A0 = (4, 128, 4, "shipped")
 SCENES = {
-    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, ((-1.5,) * 3, (1.5,) * 3)),
-    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, (A0, A0), ((-1.5,) * 3, (1.5,) * 3)),
+    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, (A0, A0), ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    **M.H256_SCENES,
 }
-# |N - N64| per ray against the conditioning of its samples: a gradient error of G_ERR times the pass's largest |grad|
-# (test_density_grad_gpu bounds it by 2e-5 off ReLU ties) turns a sample's unit normal by at most 2 G_ERR max|g| / |g_i|
-# (and never by more than 2), times its weight.  Samples where |grad| nearly vanishes are where N is ill-conditioned:
-# A sample with a ReLU tie may turn its normal by up to 2 (times its weight).  Measured on an H100 80GB HBM3 at 700 W,
-# the unconditioned worst is 1.1e-6 (lego), 6.8e-3 (fern, lego with noise).
-G_ERR = 1e-4
-N_FLOOR = 1e-5
-ACC_EPS = 1e-5
+H256 = list(M.H256_SCENES)
 
 
 def report(what, ctx, value):
@@ -35,16 +34,7 @@ def report(what, ctx, value):
 
 
 def _models(scene):
-    import nerf_pytorch_b200 as nb
-
-    weights, *_, l_xyz, _ = SCENES[scene]
-    out = []
-    for sd in load_weights(weights):
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out
+    return M.scene_models(SCENES[scene])
 
 
 def _pose(kind):
@@ -66,7 +56,7 @@ def _grid(scene, models, encoders):
 def _image(scene, normals, grid=None, early_stop=None, randoms=None, perturb=False, noise=0.0):
     import nerf_pytorch_b200 as nb
 
-    _, H, W, focal, pose, _, _, _, l_xyz, _ = SCENES[scene]
+    _, H, W, focal, pose, _, _, _, l_xyz, *_ = SCENES[scene]
     mc, mf = _models(scene)
     return nb.render_image(H, W, focal, _pose(pose), mc, mf, _options(scene, perturb, noise), mode="validation",
                            encode_position_fn=nb.get_embedding_function(l_xyz),
@@ -74,50 +64,66 @@ def _image(scene, normals, grid=None, early_stop=None, randoms=None, perturb=Fal
                            early_stop=early_stop, randoms=randoms, normals=normals)
 
 
-@pytest.mark.parametrize("variant", ["default", "grid", "early_stop", "grid+early_stop"])
+VARIANTS = ["default", "grid", "early_stop", "grid+early_stop"]
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
 def test_six_outputs_are_those_of_the_render_without_normals(variant):
+    _six_outputs_are_those_of_the_render_without_normals("lego", variant)
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("scene", H256)
+def test_six_outputs_are_those_of_the_render_without_normals_at_hidden_256(scene, variant):
+    _six_outputs_are_those_of_the_render_without_normals(scene, variant)
+
+
+def _six_outputs_are_those_of_the_render_without_normals(scene, variant):
     import nerf_pytorch_b200 as nb
 
     grid = None
     if "grid" in variant:
-        mc, mf = _models("lego")
-        grid = _grid("lego", [mc, mf], (nb.get_embedding_function(10), nb.get_embedding_function(4)))
+        mc, mf = _models(scene)
+        grid = _grid(scene, [mc, mf], (nb.get_embedding_function(SCENES[scene][8]), nb.get_embedding_function(4)))
     stop = 1e-3 if "early_stop" in variant else None
     rng = nb.SeededRandoms(5, 2)
-    plain = _image("lego", False, grid, stop, rng, perturb=True, noise=0.2)
-    with_n = _image("lego", True, grid, stop, rng, perturb=True, noise=0.2)
+    plain = _image(scene, False, grid, stop, rng, perturb=True, noise=0.2)
+    with_n = _image(scene, True, grid, stop, rng, perturb=True, noise=0.2)
     assert len(plain) == 6 and len(with_n) == 7
-    assert all(bits_equal(a, b) for a, b in zip(plain, with_n[:6])), variant
+    assert all(bits_equal(a, b) for a, b in zip(plain, with_n[:6])), (scene, variant)
     n, acc = with_n[6], with_n[5]
-    assert n.shape == (48, 48, 3) and torch.isfinite(n).all()
+    assert n.shape == (*SCENES[scene][1:3], 3) and torch.isfinite(n).all()
     norm = n.norm(dim=-1)
-    report("max |N| - acc", variant, f"{(norm - acc).max().item():.3e}")
+    report("max |N| - acc", (scene, variant), f"{(norm - acc).max().item():.3e}")
     assert (norm <= acc + ACC_EPS).all()
     assert (n[acc == 0] == 0).all()
     img = nb.cast_to_normal_image(n)
     assert img.dtype == torch.uint8 and img.shape == n.shape
 
 
-def _render(scene, perturb, noise, coarse_only, seed):
+def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None):
     """(arch of the last pass, its state dict, rays, z, raw, noise of the last pass or None, noise_std, normals, acc)
-    of one render_fwd_normals call, read back from its workspace."""
+    of one render_fwd_normals call (with a grid of the networks' density for grid_kind "model", early stopping at
+    `stop`), read back from its workspace."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
-    _, H, W, focal, pose, no_ndc, near, far, l_xyz, _ = SCENES[scene]
+    _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
     mc, mf = _models(scene)
-    sd_last = load_weights(SCENES[scene][0])[0 if coarse_only else 1]
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
-    arch = train_utils._arch_of(mc, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
-    blobs = [train_utils._packed(m, arch)[1] for m in (mc, mf)]
+    archs = [train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
+             for m in (mc, mf)]
+    blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
+    sd_last = {k: v.detach().cpu() for k, v in (mc if coarse_only else mf).state_dict().items()}
+    grid = _grid(scene, [mc, mf], (epf, edf)) if grid_kind == "model" else None
     nf = 0 if coarse_only else 128
     opts = ops.make_opts(64, nf, perturb, False, False, noise)
     rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     rng = nb.SeededRandoms(seed, 0)
-    arch_f = None if coarse_only else arch
+    arch, arch_f = archs[0], None if coarse_only else archs[1]
     with torch.no_grad():
         out_c, out_f, normals, ws = ops.render_fwd_normals(arch, arch_f, opts, blobs[0], blobs[1] if nf else None, rays,
-                                                           rng, None, None, impl=1)
+                                                           rng, grid, stop, impl=1)
     n, s = rays.shape[0], 64 + nf
     lay = ops.render_workspace_layout(arch, arch_f, opts, n, False)
     zname, rname = ("z_coarse", "raw_coarse") if coarse_only else ("z_fine", "raw_fine")
@@ -126,75 +132,32 @@ def _render(scene, perturb, noise, coarse_only, seed):
     raw = f[lay[rname] // 4: lay[rname] // 4 + n * s * 4].view(n, s, 4)
     nz = ops.random_fill(rng, "noise_c" if coarse_only else "noise_f", n, s) if noise > 0 else None
     acc = (out_c if coarse_only else out_f)[:, 4]
-    return arch, sd_last, rays, z.clone(), raw.clone(), nz, noise, normals, acc
-
-
-def _ties(sd64, xyz, hidden):
-    """Points with a ReLU tie: a layers_xyz unit within mlp_checks.STASH_TOL of its layer's largest activation (over
-    this batch) from zero in fp64, where the kernel's decision may be the other one."""
-    h = torch.nn.functional.linear(xyz, sd64["layer1.weight"], sd64["layer1.bias"])
-    tie = torch.zeros(xyz.shape[0], dtype=torch.bool, device=xyz.device)
-    i = 0
-    while f"layers_xyz.{i}.weight" in sd64:
-        w = sd64[f"layers_xyz.{i}.weight"]
-        if w.shape[1] != hidden:
-            h = torch.cat((h, xyz), -1)
-        pre = torch.nn.functional.linear(h, w, sd64[f"layers_xyz.{i}.bias"])
-        tie |= (pre.abs() <= M.STASH_TOL * pre.max().clamp_min(0.0)).any(-1)
-        h = torch.relu(pre)
-        i += 1
-    return tie
-
-
-def _grad64(arch, sd, pts):
-    """fp64 autograd of sigma w.r.t. the points, the bands' fp32 arguments as values (test_density_grad_gpu), and
-    the points with a ReLU tie."""
-    sd64 = {k: v.double().cuda() for k, v in sd.items()}
-    out, ties = [], []
-    d = torch.tensor([0.0, 0.0, 1.0], device="cuda")
-    for p0 in range(0, pts.shape[0], 1 << 17):
-        x32 = pts[p0:p0 + (1 << 17)]
-        x64 = x32.double().requires_grad_()
-        parts = [x64]
-        for k in range(arch.n_freq_xyz):
-            f = 2.0 ** k  # log-sampled bands: 2^k, exact in fp32
-            a = x64 * f + ((x32 * f).double() - x64.detach() * f)
-            parts += [torch.sin(a), torch.cos(a)]
-        emb = torch.cat(parts + [M.embed(d.expand(x32.shape[0], 3), arch.n_freq_dir, True, True)], -1)
-        raw = O.flexible_nerf_forward(sd64, emb, arch.dim_xyz)
-        g, = torch.autograd.grad(raw[:, 3].sum(), x64)
-        out.append(g)
-        with torch.no_grad():
-            ties.append(_ties(sd64, torch.cat(parts, -1).detach(), arch.hidden))
-    return torch.cat(out), torch.cat(ties)
+    return arch_f or arch, sd_last, rays, z.clone(), raw.clone(), nz, noise, normals, acc
 
 
 @pytest.mark.parametrize("scene,perturb,noise,coarse_only", [
-    ("lego", False, 0.0, False), ("fern", False, 0.0, False), ("lego", False, 0.0, True), ("lego", True, 0.2, False)])
+    ("lego", False, 0.0, False), ("fern", False, 0.0, False), ("lego", False, 0.0, True), ("lego", True, 0.2, False),
+    ("a2", False, 0.0, False), ("mixed", False, 0.0, False), ("mixed_rev", True, 0.2, False)])
 def test_normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only):
-    ctx = (scene, perturb, noise, coarse_only)
-    arch, sd, rays, z, raw, nz, std, normals, acc = _render(scene, perturb, noise, coarse_only, seed=3)
-    assert arch.log_sampling_xyz and arch.include_input_xyz
-    pts = (rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]).reshape(-1, 3)
-    _, _, _, w64, _ = composite64(raw, z, rays[:, 3:6], noise_std=std, noise=nz)
-    w64 = w64.reshape(-1)
-    live = w64 != 0
-    g = torch.zeros(pts.shape[0], 3, dtype=torch.float64, device="cuda")
-    tie = torch.zeros(pts.shape[0], dtype=torch.bool, device="cuda")
-    g[live], tie[live] = _grad64(arch, sd, pts[live].contiguous())
-    mag = g.norm(dim=-1, keepdim=True)
-    nrm64 = torch.where(mag > 0, -g / mag, torch.zeros_like(g))
-    terms = (w64[:, None] * nrm64).view(rays.shape[0], -1, 3)
-    N64 = torch.zeros(rays.shape[0], 3, dtype=torch.float64, device="cuda")
-    for j in range(terms.shape[1]):  # in sample order
-        N64 += terms[:, j]
+    _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, None, None)
+
+
+@pytest.mark.parametrize("scene,perturb,noise,coarse_only,grid_kind,stop", [
+    ("lego", True, 0.2, False, "model", 1e-2), ("a2", True, 0.2, False, "model", 1e-2),
+    ("a2", False, 0.0, True, None, 1e-2), ("mixed", False, 0.0, False, "model", None),
+    ("mixed_rev", True, 0.2, False, None, 1e-2)])
+def test_normals_with_a_grid_or_early_stopping_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind,
+                                                                          stop):
+    _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind, stop)
+
+
+def _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind, stop):
+    ctx = (scene, perturb, noise, coarse_only, grid_kind, stop)
+    arch, sd, rays, z, raw, nz, std, normals, acc = _render(scene, perturb, noise, coarse_only, 3, grid_kind, stop)
+    N64, bound, n_live, n_tie = M.normals64(arch, sd, rays, z, raw, std, nz)
     err = (normals.double() - N64).abs().max(-1).values
-    gmax = mag.max()
-    turn = torch.clamp(2 * G_ERR * gmax / mag.squeeze(-1).clamp_min(1e-300), max=2.0)
-    turn[tie] = 2.0  # a ReLU tie may turn its sample's normal anywhere
-    bound = (w64 * turn).view(rays.shape[0], -1).sum(-1) + N_FLOOR
     report("max |N - N64|", ctx, f"{err.max().item():.3e}, max err / bound {(err / bound).max().item():.3f} (rays "
-                                 f"{rays.shape[0]}, live samples {int(live.sum())}, tie samples {int(tie.sum())})")
+                                 f"{rays.shape[0]}, live samples {n_live}, tie samples {n_tie})")
     assert (err <= bound).all(), ctx
     assert (normals.norm(dim=-1) <= acc + ACC_EPS).all(), ctx
     assert (normals[acc == 0] == 0).all(), ctx
@@ -203,6 +166,7 @@ def test_normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only):
 def test_normals_refusals_fire_before_any_launch():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
 
     mc, mf = _models("lego")
     kw = dict(encode_position_fn=nb.get_embedding_function(10), encode_direction_fn=nb.get_embedding_function(4))
@@ -224,4 +188,20 @@ def test_normals_refusals_fire_before_any_launch():
                 ops.render_fwd_normals(ops.ArchSpec(num_layers=4, hidden=128, skip_every=4, n_freq_xyz=10,
                                                     n_freq_dir=4), None, ops.make_opts(64, 0, False, False, False, 0.0),
                                        torch.zeros(1, device="cuda"), None, rays, {}, impl=bad)
+        # 8x256 with L_dir 6: 39 direction channels, wider than the wgmma forward's 32
+        ldir6 = [nb.FlexibleNeRFModel(num_layers=8, hidden_size=256, num_encoding_fn_xyz=10, num_encoding_fn_dir=6).cuda()
+                 for _ in range(2)]
+        kw6 = dict(encode_position_fn=kw["encode_position_fn"], encode_direction_fn=nb.get_embedding_function(6))
+        grid = OccupancyGrid.full(SCENES["lego"][-1], 16)
+        for g, stop in ((None, None), (grid, None), (None, 1e-2), (grid, 1e-2)):
+            with pytest.raises(NotImplementedError, match="32"):
+                nb.predict_and_render_radiance(rays, *ldir6, o, normals=True, grid=g, early_stop=stop, **kw6)
+        a6 = ops.ArchSpec(num_layers=8, hidden=256, n_freq_xyz=10, n_freq_dir=6)
+        assert "32" in ops.density_grad_refusal(a6)
+        with pytest.raises(NotImplementedError, match="32"):
+            ops.render_fwd_normals(a6, a6, ops.make_opts(64, 64, False, False, False, 0.0),
+                                   torch.zeros(a6.blob_floats(), device="cuda"), torch.zeros(a6.blob_floats(), device="cuda"),
+                                   rays, {}, impl=ops.IMPL_TC)
     assert ops.launch_count() == before
+    with torch.no_grad(), pytest.raises(NotImplementedError, match="32"):  # after generating the image's rays
+        nb.render_image(8, 8, 10.0, torch.eye(4), *ldir6, o, normals=True, **kw6)

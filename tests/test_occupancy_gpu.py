@@ -13,16 +13,22 @@ import math
 import pytest
 import torch
 
-from helpers import OUT_NAMES, bits_equal, load_weights
+import mlp_checks as M
+from helpers import OUT_NAMES, bits_equal, compaction_reference, skipped_samples
 
 pytestmark = pytest.mark.gpu
 
-# (weights or None for A1 at init, H, W, focal, pose, no_ndc, near, far, L_xyz, layers, skip, bounds of the grid)
+# (shipped weights or None, H, W, focal, pose, no_ndc, near, far, L_xyz, (coarse, fine) networks, bounds of the grid):
+# mlp_checks.H256_SCENES' format
+A0, A1 = (4, 128, 4, "shipped"), (8, 128, 3, "init")
 SCENES = {
-    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, 4, 4, ((-1.5,) * 3, (1.5,) * 3)),
-    "a1": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10, 8, 3, ((-1.5,) * 3, (1.5,) * 3)),
-    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, 4, 4, ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    "lego": ("lego_lowres", 48, 48, 66.7, "spherical", True, 2.0, 6.0, 10, (A0, A0), ((-1.5,) * 3, (1.5,) * 3)),
+    "a1": (None, 40, 40, 55.0, "spherical", True, 2.0, 6.0, 10, (A1, A1), ((-1.5,) * 3, (1.5,) * 3)),
+    "fern": ("fern_lowres", 42, 56, 45.3, "eye", False, 0.0, 1.0, 6, (A0, A0), ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
+    **M.H256_SCENES,
 }
+# the scenes whose networks run hidden 256 in some pass
+H256 = list(M.H256_SCENES)
 VARIANTS = {  # (perturb, noise_std, white_bkgd)
     "det": (False, 0.0, False),
     "perturb_noise": (True, 1.0, False),
@@ -36,20 +42,7 @@ def report(what, ctx, value):
 
 
 def _models(scene):
-    import nerf_pytorch_b200 as nb
-
-    weights, *_, l_xyz, layers, skip, _ = SCENES[scene]
-    if weights is None:
-        torch.manual_seed(7)
-        return [nb.FlexibleNeRFModel(num_layers=layers, hidden_size=128, skip_connect_every=skip,
-                                     num_encoding_fn_xyz=l_xyz, num_encoding_fn_dir=4).cuda() for _ in range(2)]
-    out = []
-    for sd in load_weights(weights):
-        m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=128, skip_connect_every=skip, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out
+    return M.scene_models(SCENES[scene])
 
 
 def _pose(kind):
@@ -59,19 +52,20 @@ def _pose(kind):
 
 
 def _setup(scene, variant="det", n_fine=128):
-    """(arch, blobs, opts, rays, models, encoders) of a scene at the ops level."""
+    """((arch_c, arch_f), blobs, opts, rays, models, encoders) of a scene at the ops level."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
     mc, mf = _models(scene)
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
-    arch = train_utils._arch_of(mc, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
-    blobs = [train_utils._packed(m, arch)[1] for m in (mc, mf)]
+    archs = tuple(train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
+                  for m in (mc, mf))
+    blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
     opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
     rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
-    return arch, blobs, opts, rays, (mc, mf), (epf, edf)
+    return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
 
 def _grid_random(scene, frac, seed, res=32):
@@ -98,12 +92,12 @@ def _ws(ws, layout, name, n, s, cols):
     return t.view(n, s, cols) if cols > 1 else t.view(n, s)
 
 
-def _render_both(arch, blobs, opts, rays, grid, impl, rng):
+def _render_both(archs, blobs, opts, rays, grid, impl, rng):
     from nerf_pytorch_b200 import ops
 
-    oc, of, ws = ops.render_fwd(arch, arch, opts, blobs[0], blobs[1], rays, rng, training=False, impl=impl)
+    oc, of, ws = ops.render_fwd(*archs, opts, blobs[0], blobs[1], rays, rng, training=False, impl=impl)
     ne = torch.zeros(2, dtype=torch.int64, device="cuda")
-    gc, gf, gws = ops.render_fwd_grid(arch, arch, opts, blobs[0], blobs[1], rays, rng, grid, impl=impl, n_evaluated=ne)
+    gc, gf, gws = ops.render_fwd_grid(*archs, opts, blobs[0], blobs[1], rays, rng, grid, impl=impl, n_evaluated=ne)
     torch.cuda.synchronize()
     return (oc, of, ws), (gc, gf, gws), ne
 
@@ -118,9 +112,9 @@ def test_full_grid_is_the_default_render_bit_for_bit(impl, scene, variant):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200.occupancy import OccupancyGrid
 
-    arch, blobs, opts, rays, _, _ = _setup(scene, variant)
+    archs, blobs, opts, rays, _, _ = _setup(scene, variant)
     grid = OccupancyGrid.full(SCENES[scene][-1], 32)
-    (oc, of, _), (gc, gf, _), ne = _render_both(arch, blobs, opts, rays, grid, IMPLS[impl], nb.SeededRandoms(5, 2))
+    (oc, of, _), (gc, gf, _), ne = _render_both(archs, blobs, opts, rays, grid, IMPLS[impl], nb.SeededRandoms(5, 2))
     n = rays.shape[0]
     assert bits_equal(gc, oc) and bits_equal(gf, of), (impl, scene, variant)
     assert ne.tolist() == [n * 64, n * 192]
@@ -132,15 +126,26 @@ def test_full_grid_is_the_default_render_bit_for_bit(impl, scene, variant):
 @pytest.mark.parametrize("variant", list(VARIANTS))
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_empty_grid_composites_zero_density(impl, variant):
+    _empty_grid_composites_zero_density(impl, "lego", variant)
+
+
+@pytest.mark.parametrize("variant", list(VARIANTS))
+@pytest.mark.parametrize("scene", H256)
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_empty_grid_composites_zero_density_at_hidden_256(impl, scene, variant):
+    _empty_grid_composites_zero_density(impl, scene, variant)
+
+
+def _empty_grid_composites_zero_density(impl, scene, variant):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
     from nerf_pytorch_b200.occupancy import OccupancyGrid
 
-    arch, blobs, opts, rays, _, _ = _setup("lego", variant)
+    archs, blobs, opts, rays, _, _ = _setup(scene, variant)
     grid = OccupancyGrid.empty(((-100.0,) * 3, (100.0,) * 3), 16)
     before = ops.launch_count()
     ne = torch.full((2,), -1, dtype=torch.int64, device="cuda")
-    oc, of, _ = ops.render_fwd_grid(arch, arch, opts, blobs[0], blobs[1], rays, nb.SeededRandoms(1), grid,
+    oc, of, _ = ops.render_fwd_grid(*archs, opts, blobs[0], blobs[1], rays, nb.SeededRandoms(1), grid,
                                     impl=IMPLS[impl], n_evaluated=ne)
     torch.cuda.synchronize()
     assert ne.tolist() == [0, 0]
@@ -156,13 +161,6 @@ def test_empty_grid_composites_zero_density(impl, variant):
 # ------------------------------------------------------------------------------------------------------------------------
 # 3. the exact per-ray statement and the evaluated raw
 # ------------------------------------------------------------------------------------------------------------------------
-def _skipped(grid, rays, z):
-    pts = rays[:, None, :3] + rays[:, None, 3:6] * z[..., None]
-    cell = grid.cell_of(pts)
-    occ = grid.occupancy().reshape(-1)
-    return (cell >= 0) & ~occ[cell.clamp_min(0)]
-
-
 def _dense(raw, noise, std):
     pre = raw[..., 3]
     if std > 0:
@@ -181,21 +179,21 @@ def test_rays_without_skipped_density_are_bit_identical(impl, scene, variant, gr
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    arch, blobs, opts, rays, models, enc = _setup(scene, variant)
+    archs, blobs, opts, rays, models, enc = _setup(scene, variant)
     if grid_kind == "model":
         grid = _grid_model(scene, models, enc)
     else:
         grid = _grid_random(scene, int(grid_kind[4:]) / 100, seed=len(scene) + int(grid_kind[4:]))
     rng = nb.SeededRandoms(9, 4)
-    (oc, of, ws), (gc, gf, gws), ne = _render_both(arch, blobs, opts, rays, grid, IMPLS[impl], rng)
+    (oc, of, ws), (gc, gf, gws), ne = _render_both(archs, blobs, opts, rays, grid, IMPLS[impl], rng)
     n, nc, ns = rays.shape[0], 64, 192
-    lay = ops.render_workspace_layout(arch, arch, opts, n, False)
+    lay = ops.render_workspace_layout(*archs, opts, n, False)
     z_c, z_f = _ws(ws, lay, "z_coarse", n, nc, 1), _ws(ws, lay, "z_fine", n, ns, 1)
     raw_c, raw_f = _ws(ws, lay, "raw_coarse", n, nc, 4), _ws(ws, lay, "raw_fine", n, ns, 4)
     std = opts.noise_std
     noise_c = ops.random_fill(rng, "noise_c", n, nc) if std > 0 else None
     noise_f = ops.random_fill(rng, "noise_f", n, ns) if std > 0 else None
-    sk_c, sk_f = _skipped(grid, rays, z_c), _skipped(grid, rays, z_f)
+    sk_c, sk_f = skipped_samples(grid, rays, z_c), skipped_samples(grid, rays, z_f)
     bad = (sk_c & _dense(raw_c, noise_c, std)).any(1) | (sk_f & _dense(raw_f, noise_f, std)).any(1)
     clean = ~bad
     ctx = (impl, scene, variant, grid_kind)
@@ -213,7 +211,7 @@ def test_rays_without_skipped_density_are_bit_identical(impl, scene, variant, gr
     assert bits_equal(g_rc[~sk_c], raw_c[~sk_c])
     skip_raw = torch.tensor([0.0, 0.0, 0.0, -math.inf], device="cuda")
     assert torch.equal(g_rc[sk_c], skip_raw.expand(int(sk_c.sum()), 4))
-    g_sk_f = _skipped(grid, rays, g_zf)
+    g_sk_f = skipped_samples(grid, rays, g_zf)
     same_z = g_zf.view(torch.int32) == z_f.view(torch.int32)
     ev = ~g_sk_f & same_z
     assert bits_equal(g_rf[ev], raw_f[ev])
@@ -221,26 +219,13 @@ def test_rays_without_skipped_density_are_bit_identical(impl, scene, variant, gr
     # points whose depth moved: compare with the default kernel at the grid render's own depths
     moved = ~g_sk_f & ~same_z
     if moved.any():
-        raw_at = ops.mlp_fwd(arch, blobs[1], rays, g_zf.contiguous(), impl=IMPLS[impl])
+        raw_at = ops.mlp_fwd(archs[1], blobs[1], rays, g_zf.contiguous(), impl=IMPLS[impl])
         assert bits_equal(g_rf[moved], raw_at[moved])
 
 
 # ------------------------------------------------------------------------------------------------------------------------
 # 4. compaction against a torch restatement
 # ------------------------------------------------------------------------------------------------------------------------
-def _compaction_reference(grid, rays, z):
-    n, s = z.shape
-    keep = ~_skipped(grid, rays, z)
-    rows, blocks = [], []
-    for g0 in range(0, n, 10):
-        pts = (torch.nonzero(keep[g0:g0 + 10].reshape(-1)).reshape(-1) + g0 * s).tolist()
-        for b0 in range(0, len(pts), 64):
-            chunk = pts[b0:b0 + 64]
-            blocks.append((chunk[0] // s, chunk[-1] // s))
-            rows += chunk + [-1] * (64 - len(chunk))
-    return keep, rows, blocks
-
-
 @pytest.mark.parametrize("shape", [(1237, 64), (403, 192), (7, 15)])
 def test_compaction_matches_torch_restatement_and_repeats(shape):
     from nerf_pytorch_b200 import ops
@@ -255,7 +240,7 @@ def test_compaction_matches_torch_restatement_and_repeats(shape):
     raw, m, blocks, nb_, ne = ops.grid_compact(grid, rays, z, raw0.clone())
     raw2, m2, blocks2, nb2, ne2 = ops.grid_compact(grid, rays, z, raw0.clone())
     torch.cuda.synchronize()
-    keep, rows, want_blocks = _compaction_reference(grid, rays, z)
+    keep, rows, want_blocks = compaction_reference(grid, rays, z)
     nb = nb_.item()
     assert nb == len(want_blocks) and ne.item() == int(keep.sum())
     assert m[:64 * nb].tolist() == rows
@@ -287,16 +272,27 @@ def _image(scene, impl, chunk, grid=None, randoms=None, perturb=True, noise=0.5)
 
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_grid_render_image_is_chunking_invariant(impl):
+    _grid_render_image_is_chunking_invariant(impl, "lego")
+
+
+@pytest.mark.parametrize("scene", H256)
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_grid_render_image_is_chunking_invariant_at_hidden_256(impl, scene):
+    _grid_render_image_is_chunking_invariant(impl, scene)
+
+
+def _grid_render_image_is_chunking_invariant(impl, scene):
     import nerf_pytorch_b200 as nb
 
-    grid = _grid_random("lego", 0.5, seed=3)
+    grid = _grid_random(scene, 0.5, seed=3)
     rng = nb.SeededRandoms(21, 1)
-    whole = _image("lego", IMPLS[impl], 48 * 48, grid, rng)
+    n = SCENES[scene][1] * SCENES[scene][2]
+    whole = _image(scene, IMPLS[impl], n, grid, rng)
     for chunk in (1000, 333):
-        part = _image("lego", IMPLS[impl], chunk, grid, rng)
-        assert all(bits_equal(a, b) for a, b in zip(whole, part)), chunk
-    default = _image("lego", IMPLS[impl], 48 * 48, None, rng)
-    assert not all(bits_equal(a, b) for a, b in zip(whole, default))  # the grid did skip density
+        part = _image(scene, IMPLS[impl], chunk, grid, rng)
+        assert all(bits_equal(a, b) for a, b in zip(whole, part)), (scene, chunk)
+    default = _image(scene, IMPLS[impl], n, None, rng)
+    assert not all(bits_equal(a, b) for a, b in zip(whole, default)), scene  # the grid did skip density
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -347,7 +343,16 @@ def test_grid_refusals_fire_before_any_launch():
         bad.bits = torch.zeros(7, dtype=torch.int32, device="cuda")
         with pytest.raises(RuntimeError, match="int32"):
             nb.render_image(16, 16, 20.0, torch.eye(4), mc, mf, opts, grid=bad, **kw)
+        # 8x256 with L_dir 6: 39 direction channels, wider than the wgmma forward's 32
+        ldir6 = [nb.FlexibleNeRFModel(num_layers=8, hidden_size=256, num_encoding_fn_xyz=10, num_encoding_fn_dir=6).cuda()
+                 for _ in range(2)]
+        kw6 = dict(encode_position_fn=epf, encode_direction_fn=nb.get_embedding_function(6))
+        for impl in (None, ops.IMPL_TC, ops.IMPL_TC_FAST):
+            with pytest.raises(NotImplementedError, match="32"):
+                nb.predict_and_render_radiance(rays, *ldir6, opts, grid=grid, impl=impl, **kw6)
     assert ops.launch_count() == before
+    with torch.no_grad(), pytest.raises(NotImplementedError, match="32"):  # after generating the image's rays
+        nb.render_image(16, 16, 20.0, torch.eye(4), *ldir6, opts, grid=grid, **kw6)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
