@@ -562,6 +562,74 @@ int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const ner
                                         float* out_coarse, float* out_fine, float* normals, void* workspace,
                                         int32_t impl, void* stream);
 
+/* ---- baked fields: a trained network sampled once on the bricks of a lattice, rendered without the MLP ------------
+ * The box and its lattice are those of "meshes"; the bricks, their activity under an occupancy grid, their slots and the
+ * point order inside a brick are those of "sparse meshes" with halo = 0 (P = 9^3 = 729 points per brick, corner point l
+ * of slot s at row s * 729 + (l_2 * 9 + l_1) * 9 + l_0, lattice index b B + l clamped onto 0 .. res).  The field lives in
+ * the coordinates the MLP encodes (world space for Blender scenes, NDC for LLFF scenes).
+ *   - Directions.  D = NERFB200_BAKE_DIRS = 64 on a spherical Fibonacci lattice: for i = 0 .. 63, z = 1 - (2 i + 1) / 64,
+ *     r = sqrt(1 - z^2), phi = i pi (3 - sqrt 5), d_i = (r cos phi, r sin phi, z), in fp64, rounded once to fp32.
+ *   - Basis.  Real spherical harmonics of degree <= 2, 9 functions of a unit vector (x, y, z):
+ *       Y_0 = 0.28209479177387814,
+ *       Y_1 = -0.4886025119029199 y,  Y_2 = 0.4886025119029199 z,  Y_3 = -0.4886025119029199 x,
+ *       Y_4 = 1.0925484305920792 x y,  Y_5 = -1.0925484305920792 y z,  Y_6 = 0.31539156525252005 (2 z^2 - x^2 - y^2),
+ *       Y_7 = -1.0925484305920792 x z,  Y_8 = 0.5462742152960396 (x^2 - y^2).
+ *     (Y_1..Y_3 carry the Condon-Shortley sign of the complex harmonics they are made from.)  The projection
+ *     M = (Y^T Y)^-1 Y^T (9 x 64), Y[i][j] = Y_j(d_i) in fp64 at the fp32 directions, is computed in fp64 by the
+ *     library and rounded once to fp32.  bake_basis returns the directions and M.
+ *   - Values.  values[slot][729][32] fp32 (128 B per lattice point, NERFB200_BAKE_CHANNELS):
+ *       [0]          sigma_raw: the bits nerfb200_mlp_fwd_pts with impl 1 writes to raw[p][3] at that point;
+ *       [1 + 9 c + j] the coefficient of Y_j of colour channel c's PRE-sigmoid logit: acc = 0, then for d = 0 .. 63 in
+ *                    order acc = fmaf(M[j][d], logit_c(d), acc), logit_c(d) the bits mlp_fwd_pts with impl 1 writes to
+ *                    raw[p][c] at the point with view direction d_d.  Without view directions coefficient 0 is
+ *                    logit_c / Y_0 (fp32) and the others are 0;
+ *       [28 .. 31]   0.
+ *   - Rendering (baked_render).  Rays are rows [o(3) d(3) near far (viewdir(3))] as gen_rays / pack_rays write them.
+ *     All fp32 with round-to-nearest, each op rounded, no contraction unless fmaf is named.
+ *       interval  [t_a, t_b] = [near, far] intersected with the box's slab interval (per axis (lo - o) / d and
+ *                 (hi - o) / d); h = min over c of (hi_c - lo_c) / res_c, |d| = sqrt((dx dx + dy dy) + dz dz),
+ *                 dt = (0.5 h) / |d|; sample k is t_k = t_a + (k + 0.5) dt for every k with t_k < t_b.
+ *       lookup    x = o + d t_k, per axis as the MLP forms its points; its cube i is the cell of x under the cell rule of
+ *                 "occupancy grid" applied to the box (t_c = (x_c - lo_c) scale_c, i_c = (int) t_c), f_c = t_c - i_c; the
+ *                 brick floor(i / 8) and brick_map give the slot.  A sample outside the box, or in a brick whose slot is
+ *                 -1, has sigma_raw = 0 and colour 0.
+ *       interp    channels 0 .. 27 trilinear over the cube's 8 corners k = 0 .. 7 (corner offset (k & 1, k >> 1 & 1,
+ *                 k >> 2), point l + offset of the brick), weight w_k = (w_x w_y) w_z with w_c = f_c for offset 1 and
+ *                 1 - f_c for 0; v = 0, then v = fmaf(w_k, value_k, v) for k = 0 .. 7.
+ *       colour    with view directions s_c = sum over j = 0 .. 8 of Y_j(viewdir) coef_cj (acc = 0, acc = fmaf(Y_j, coef_cj,
+ *                 acc), Y_j in fp32 from the constants above as written, x x etc. rounded), without them s_c = Y_0 coef_c0;
+ *                 rgb_c = 1 / (1 + exp(-s_c)).
+ *       composite alpha and q = (1 - alpha) + 1e-10 as the library's compositing (volume_render_radiance_field) forms
+ *                 them with noise 0 and z_next = t_k + dt for every sample (no 1e10 last interval).  Samples go in rounds
+ *                 of 32; in a round, lane L's transmittance is T_round times the exclusive product scan of q over the
+ *                 round's lanes (Hillis-Steele order), w = alpha T, and T_next = (T_lane 31) q_31.  rgb, acc = sum w and
+ *                 depth = sum w t are summed in sample order; disp = 1 / max(1e-10, depth / acc) (NaN when acc = 0, as
+ *                 composite_fwd); a white background adds 1 - acc to rgb.  out[n_rays][8] = [r g b disp acc depth 0 0].
+ *       stopping  stop_transmittance t in [0, 1): after each round the ray stops once T < t.  t = 0 never stops, and a ray
+ *                 that does not stop gets the t = 0 outputs bit for bit; for a ray that stops the weights left out sum
+ *                 to less than t.
+ *
+ * bake_basis: dirs_host[64][3], proj_host[9][64] (host memory).
+ * bake_supported: NERFB200_OK if bake runs this architecture, else the reason (the last error), without a device.  The
+ *   wgmma inference forward's refusals apply (NERFB200_ERR_UNSUPPORTED); hidden 128 or 256, with or without view
+ *   directions.
+ * bake: the values of slots first .. first + count - 1 (bricks from mesh_sparse_bricks) into values + slot * 729 * 32.
+ *   logits (test hook, may be NULL): logits[(slot - first) * 729 + l][64][3] = logit_c(d).  count * 729 < 2^31.
+ * baked_render: the rendering above; brick_map from mesh_sparse_bricks over the same box, values from bake.
+ *   ray_stride >= 11 with view directions, >= 8 without.
+ * Refused before any launch: an invalid box, a null pointer, a count or range outside the box's bricks, an architecture
+ * bake_supported refuses, t outside [0, 1) or NaN.  No atomics, no host synchronisation. */
+#define NERFB200_BAKE_DIRS 64
+#define NERFB200_BAKE_SH 9
+#define NERFB200_BAKE_CHANNELS 32
+int32_t nerfb200_bake_basis(float* dirs_host, float* proj_host);
+int32_t nerfb200_bake_supported(const nerfb200_arch_t* arch);
+int32_t nerfb200_bake(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box, const int32_t* bricks,
+                      int64_t first, int64_t count, float* values, float* logits, void* stream);
+int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                              int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                              int32_t white_background, float stop_transmittance, float* out, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

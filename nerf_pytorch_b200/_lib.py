@@ -157,6 +157,10 @@ SIGNATURES = {
     "nerfb200_ndc_grad_to_world": (I32, [NP, P, P, I64, P, P]),
     "nerfb200_render_fwd_normals_ndc": (I32, [AP, AP, OP, P, P, P, I32, I64, RP, P, P, P, P, GP, P, F32, NP, P, P, P, P,
                                               I32, P]),
+    "nerfb200_bake_basis": (I32, [C.POINTER(F32), C.POINTER(F32)]),
+    "nerfb200_bake_supported": (I32, [AP]),
+    "nerfb200_bake": (I32, [AP, P, GP, P, I64, I64, P, P, P]),
+    "nerfb200_baked_render": (I32, [GP, P, P, I32, P, I32, I64, I32, F32, P, P]),
 }
 
 _lib = None

@@ -611,6 +611,39 @@ int32_t nerfb200_density_grad(const nerfb200_arch_t* arch, const float* blob, co
   return launch_density_grad_tc(p, blob, pts, n_points, out, nullptr, static_cast<cudaStream_t>(stream));
 }
 
+// the bake runs the wgmma inference forward's trunk (impl 1) and its own direction loop
+static int bake_check(const Plan& p) {
+  NB_TRY(check_impl(p, 1, 0, kInference, "bake"));
+  return bake_tc_supported(p, "bake impl=1 (wgmma)");
+}
+
+int32_t nerfb200_bake_supported(const nerfb200_arch_t* arch) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  return bake_check(p);
+}
+
+int32_t nerfb200_bake(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box, const int32_t* bricks,
+                      int64_t first, int64_t count, float* values, float* logits, void* stream) {
+  Plan p;
+  NB_TRY(build_plan(arch, &p));
+  NB_TRY(check_grid(box, "bake"));
+  const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
+  if (!blob || !bricks || !values || first < 0 || count <= 0 || first + count > n_bricks) {
+    set_error("bake: null pointer, or slots %lld .. %lld outside the box's %lld bricks", (long long)first,
+              (long long)(first + count - 1), (long long)n_bricks);
+    return NERFB200_ERR_INVALID;
+  }
+  if (count * kBakePts >= (int64_t(1) << 31)) {
+    set_error("bake: %lld bricks are 2^31 lattice points or more in one call; split the slots", (long long)count);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  NB_TRY(bake_check(p));
+  BakeBasis basis;
+  bake_basis(&basis);
+  return launch_bake_tc(p, blob, *box, bricks, first, count, values, logits, basis, static_cast<cudaStream_t>(stream));
+}
+
 int32_t nerfb200_mlp_bwd_pts(const nerfb200_arch_t* arch, const float* blob, const float* dirs, int32_t dir_stride,
                              int64_t n_rays, int32_t n_samples, const float* d_raw, const float* stash, float* gstash,
                              float* flat_grad, int32_t impl, void* stream) {

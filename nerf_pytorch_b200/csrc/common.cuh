@@ -202,6 +202,21 @@ int launch_mlp_fwd_tc(const Plan& p, const float* blob, const PointSrc& src, int
 int grad_tc_supported(const Plan& p, const char* what);
 int launch_density_grad_tc(const Plan& p, const float* blob, const float* pts, int64_t n_points, float* out,
                            const int* n_dev, cudaStream_t s);
+// ---- baked fields (nerfb200.h "baked fields"): the directions, the SH projection and the value layout ----
+constexpr int kBakeDirs = NERFB200_BAKE_DIRS;
+constexpr int kBakeSh = NERFB200_BAKE_SH;
+constexpr int kBakeCh = NERFB200_BAKE_CHANNELS;  // floats per lattice point
+constexpr int kBakeBrick = 8;                    // NERFB200_MESH_BRICK: cubes per brick axis
+constexpr int kBakePts = (kBakeBrick + 1) * (kBakeBrick + 1) * (kBakeBrick + 1);  // lattice points per brick
+struct BakeBasis {
+  float dir[kBakeDirs][3];
+  float proj[kBakeSh][kBakeDirs];  // M = (Y^T Y)^-1 Y^T
+};
+void bake_basis(BakeBasis* b);  // host, fp64 rounded once (baked.cu)
+// the bake kernel (mlp_tc.cu), impl 1 only; bake_tc_supported checks what it needs beyond tc_supported(training = false)
+int bake_tc_supported(const Plan& p, const char* what);
+int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
+                   int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s);
 // ---- normal maps of a render's last pass (normals.cu; nerfb200.h "normal maps") ----
 // The samples with nonzero compositing weight, compacted: count[r], first[r] (their first slot), *total; pts[slot][3] =
 // o + d z as the MLP forms it

@@ -6,52 +6,16 @@
 // Algorithmic HBM bytes per ray (fp32): forward reads raw (16 S) + z (4 S) + noise (4 S; none when the noise is
 // generated in-kernel from the seeded stream) + ray (12), writes weights (4 S, coarse only) + 32 B of outputs;
 // SURVEY.md section 8(d).
-#include "common.cuh"
+#include "composite.cuh"
 
 namespace nerfb200 {
 
 constexpr int kCompWarps = 4;
 
-struct SampleTerms {
-  float alpha, q, sigma_delta_exp, delta;  // alpha, 1 - alpha + 1e-10, exp(-sigma*delta), delta
-  bool gate;                               // raw_sigma + noise > 0 (ReLU open)
-};
-
-__device__ __forceinline__ SampleTerms sample_terms(float raw_sigma, float noise, float noise_std, bool has_noise,
-                                                    float z_i, float z_next, bool last, float dnorm) {
-  SampleTerms t;
-  float delta = last ? 1e10f : __fsub_rn(z_next, z_i);   // volume_rendering_utils.py:14-23
-  delta = __fmul_rn(delta, dnorm);                       // :24
-  float pre = raw_sigma;
-  if (has_noise) pre = __fadd_rn(raw_sigma, __fmul_rn(noise, noise_std));  // :27-38
-  t.gate = pre > 0.f;
-  const float sigma = fmaxf(pre, 0.f);
-  const float e = expf(-__fmul_rn(sigma, delta));        // :39
-  t.alpha = __fsub_rn(1.0f, e);
-  t.q = __fadd_rn(__fsub_rn(1.0f, t.alpha), 1e-10f);     // :40
-  t.sigma_delta_exp = e;
-  t.delta = delta;
-  return t;
-}
-
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-
-// exclusive multiplicative scan across lanes
-__device__ __forceinline__ float warp_excl_prod(float v, int lane) {
-  float inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float n = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc *= n;
-  }
-  const float ex = __shfl_up_sync(0xffffffffu, inc, 1);
-  return lane == 0 ? 1.0f : ex;
 }
 
 // exclusive additive SUFFIX scan across lanes: sum of v over lanes > lane

@@ -925,4 +925,352 @@ int launch_density_grad_tc(const Plan& p, const float* blob, const float* pts, i
                          : launch_grad<128>(p, blob, pts, n_points, out, n_dev, s);
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Bake (nerfb200.h "baked fields"): sigma_raw and the degree-2 SH coefficients of the rgb logits over 64 directions at
+// the lattice points of active bricks.  A kernel of its own beside mlp_fwd_tc_kernel, whose rows are the flattened
+// (slot, lattice point) pairs; each row's point is formed in the kernel from the lattice rule.  The trunk and fc_feat run
+// through fwd_layer as the pts forward runs them, with the heads written to a 64 x 4 shared-memory block per warpgroup
+// (RowState rows are block rows), so sigma_raw (and, without view directions, the logits) have the forward's bits.
+// The view direction enters layers_dir[0] only through its per-ray bias (viewb), so one set of that layer's MMAs serves
+// all 64 directions: the CTA computes the 64 biases once with viewb's encoding and fmaf loop, and the epilogue loops
+// over the directions with the forward's bias, NaN-propagating ReLU and fc_rgb dot product, then folds each logit into
+// the SH accumulators.  A quad's four lanes share a row's logits and split its 27 coefficients: lane q owns value
+// columns q, q + 4, ..., q + 28, i.e. coefficients k = q + 4 m - 1.
+// ---------------------------------------------------------------------------------------------------------------
+namespace tc {
+// consumer warpgroups: three at hidden 128 as the forward (ptxas fits the direction loop in its 128 registers), one at 256
+__host__ __device__ constexpr int bake_wg(int hidden) { return hidden == 128 ? 3 : 1; }
+__host__ __device__ constexpr int bake_stage(int hidden) { return bake_wg(hidden) == 3 ? kStageBytes / 2 : kStageBytes; }
+
+struct BakeSmemMap {
+  SmemMap m;  // act, enc, bias, headw, bars and ring, as fwd_layer reads them
+  int head;   // per warpgroup [64 rows][4]: the heads' outputs
+  int dirb;   // [64 directions][hidden / 2]: layers_dir[0]'s bias per direction (x 2048 / 16)
+  int basis;  // BakeBasis
+};
+__host__ __device__ inline BakeSmemMap bake_smem_map(const Plan& p) {
+  BakeSmemMap bm;
+  SmemMap& m = bm.m;
+  const int rows = 64 * bake_wg(p.hidden);
+  m.act = 0;
+  int off = rows * p.hidden * 4;
+  m.enc = off;     off += rows * 64 * 4;
+  m.bias = off;    off += p.enc_cum[0] * 4;
+  m.headw = off;   off += (4 * p.hidden + 3 * (p.hidden / 2) + 16) * 4;
+  bm.head = off;   off += rows * 4 * 4;
+  bm.dirb = off;   off += kBakeDirs * (p.hidden / 2) * 4;
+  bm.basis = off;  off += (int)sizeof(BakeBasis);
+  m.viewb = m.encd = m.wv = 0;
+  m.bars = off;    off += 256;
+  m.ring = (off + 1023) & ~1023;
+  m.n_stages = ring_depth(m.ring, bake_stage(p.hidden));
+  m.total = m.ring + (m.n_stages > 0 ? m.n_stages : 0) * bake_stage(p.hidden);
+  return bm;
+}
+}  // namespace tc
+
+// layers_dir[0]'s MMAs (K = hidden, the activation tile alone), exactly as fwd_layer issues them for that layer
+template <int N, int kStage>
+__device__ __forceinline__ void bake_dir_mma(const Plan& p, const float* blob, float (&acc)[N / 2], uint8_t* sm,
+                                             const SmemMap& mp, int wg, int rows, WeightRing<kStage>& ring) {
+  constexpr int kSps = kStage == kStageBytes ? kStepsPerStage : split_sps(kStage, N);
+  const int e = p.n_gemm - 1;
+  const int fin = p.g[e].k_h;
+  const MmaInfo mi = mma_info(p, blob, e, false, kStage);
+  const uint64_t a_hi0 = make_desc(smem_u32(sm + mp.act) + (uint32_t)(wg * 64 * fin * 2), 128, (uint32_t)fin * 16);
+  const uint32_t a_lo_off = (uint32_t)(rows * fin * 2);
+  const uint32_t slab_b = 16u * (uint32_t)N;
+  const uint64_t b_ring = make_desc(ring.base, slab_b, 128);
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
+  wgmma_fence();
+  for (int ks0 = 0; ks0 < mi.ksteps; ks0 += mi.sps) {
+    const uint32_t st = ring.acquire();
+    const uint64_t b_st = desc_adv(b_ring, st * (uint32_t)kStage);
+#pragma unroll
+    for (int hh = 0; hh < kSps; ++hh) {
+      const int ks = ks0 + hh;
+      if (hh < mi.sps && ks < mi.ksteps) {
+        const uint64_t b_hs = desc_adv(b_st, hh * 6 * slab_b);
+        const uint64_t ah = desc_adv(a_hi0, (uint32_t)ks * 256u), al = desc_adv(ah, a_lo_off);
+        wgmma_f16<N>(acc, ah, b_hs, ks > 0 ? 1 : 0);
+        wgmma_f16<N>(acc, al, desc_adv(b_hs, 2 * slab_b), 1);
+        wgmma_f16<N>(acc, ah, desc_adv(b_hs, 4 * slab_b), 1);
+      }
+    }
+    wgmma_commit();
+    ring.release_behind(acc);
+  }
+  ring.release_last(acc);
+}
+
+// p_c(i) of "meshes" (mesh_common.cuh lattice_coord): lo + ((hi - lo) * i) / res, each op rounded
+__device__ __forceinline__ float bake_coord(const nerfb200_grid_t& b, int c, int i) {
+  return __fadd_rn(b.lo[c], __fdiv_rn(__fmul_rn(__fsub_rn(b.hi[c], b.lo[c]), (float)i), (float)b.res[c]));
+}
+
+template <int kH>
+__global__ void __launch_bounds__(128 * bake_wg(kH) + 32, 1)
+bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis basis, const float* __restrict__ blob,
+               const nerfb200_grid_t box, const int* __restrict__ bricks, int64_t first, int64_t R, int64_t n_tiles,
+               float* __restrict__ values,   // out [slot][729][32]
+               float* __restrict__ logits) { // out [R][64][3] or null
+  constexpr int kWG = bake_wg(kH), kRows = 64 * kWG, kThreads = 128 * kWG + 32, kStage = bake_stage(kH);
+  constexpr int kN = kH / 2;  // layers_dir[0]'s width
+  using Ring = WeightRing<kStage>;
+  uint8_t* sm = smem_base();
+  const BakeSmemMap bm = bake_smem_map(p);
+  const SmemMap& mp = bm.m;
+  float* s_bias = reinterpret_cast<float*>(sm + mp.bias);
+  float* s_headw = reinterpret_cast<float*>(sm + mp.headw);
+  float* s_dirb = reinterpret_cast<float*>(sm + bm.dirb);
+  BakeBasis* s_basis = reinterpret_cast<BakeBasis*>(sm + bm.basis);
+  Ring ring{smem_u32(sm + mp.ring), smem_u32(sm + mp.bars), (uint32_t)mp.n_stages};
+
+  const int tid = threadIdx.x;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
+  const int enc_w = p.enc_tile_w;
+  const int n_body = p.use_viewdirs ? p.n_gemm - 1 : p.n_gemm;  // the layers fwd_layer runs
+
+  if (tid == 0) {
+    ring.init(4 * kWG);
+    fence_barrier_init();
+  }
+  // biases and heads as mlp_fwd_tc_kernel scales them; the basis; the directions' encodings (in the activation tile)
+  for (int gi = 0; gi < p.n_gemm; ++gi)
+    for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
+  const int hw1 = p.h[0].n_out * p.h[0].k;
+  const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
+  for (int i = tid; i < hw1; i += kThreads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
+  for (int i = tid; i < hw2; i += kThreads) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
+  float* s_headb = s_headw + ((hw1 + hw2 + 3) & ~3);
+  if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
+  if (tid >= 4 && tid < 8) s_headb[tid] = p.n_head > 1 ? blob[p.h[1].b_off + tid - 4] : 0.f;
+  for (int i = tid; i < (int)(sizeof(BakeBasis) / 4); i += kThreads)
+    reinterpret_cast<float*>(s_basis)[i] = reinterpret_cast<const float*>(&basis)[i];
+  float* encd = reinterpret_cast<float*>(sm + mp.act);  // [64][32], free until the first tile
+  if (p.use_viewdirs) {
+    for (int i = tid; i < kBakeDirs * 32; i += kThreads) encd[i] = 0.f;
+    __syncthreads();
+    for (int i = tid; i < kBakeDirs * 3; i += kThreads) {  // 160 threads at hidden 256
+      const int d = i / 3, c = i - 3 * d;
+      encode_coord(basis.dir[d][c], c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + d * 32);
+    }
+  }
+  __syncthreads();
+  if (p.use_viewdirs) {  // viewb of the forward, per direction
+    const GemmLayer& gd = p.g[p.n_gemm - 1];
+    const float* wv_g = blob + gd.wt_off + (size_t)gd.k_h * gd.n;  // rows k_h.. of Wt[k][n]
+    for (int i = tid; i < kBakeDirs * gd.n; i += kThreads) {
+      const int d = i / gd.n, n = i - d * gd.n;
+      float a = 0.f;
+      for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[d * 32 + k], wv_g[k * gd.n + n], a);
+      s_dirb[d * kN + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);
+    }
+  }
+  __syncthreads();
+
+  const int my_tiles = (n_tiles > blockIdx.x) ? (int)((n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x) : 0;
+
+  if (warp == 4 * kWG) {
+    // ===================== weight producer: every layer's forward copy, per tile, as the forward streams them =========
+    if ((tid & 31) == 0) {
+      const uint64_t pol = l2_policy_evict_last();
+      for (int j = 0; j < my_tiles; ++j)
+        for (int e = 0; e < p.n_gemm; ++e) {
+          const MmaInfo mi = mma_info(p, blob, e, false, kStage);
+          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
+            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
+            ring.fill(mi.src + (size_t)ks * mi.kbytes, 1, nk * mi.kbytes, 0, pol);
+          }
+        }
+    }
+  } else {
+    // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
+    const int wg = warp >> 2, wt = tid & 127, lane = tid & 31, q = lane & 3;
+    const int row = wt & 63, half = wt >> 6;  // prologue: two threads per row split the frequencies
+    uint8_t* enc = sm + mp.enc;
+    const int enc_hb = kRows * enc_w * 2;
+    float* s_head = reinterpret_cast<float*>(sm + bm.head) + wg * 64 * 4;
+    const int lr0 = 16 * (wt >> 5) + (lane >> 2);  // block row of accumulator row 0 (row 1: + 8)
+    int nb[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) nb[c] = (box.res[c] + kBakeBrick - 1) / kBakeBrick;
+    RowState rs;  // rows of the 64 x 4 head block
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      rs.pt[i] = lr0 + 8 * i;
+      rs.valid[i] = true;
+      rs.ray_slot[i] = 0;
+    }
+    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
+    // this lane's coefficients k = q + 4 m - 1 (m = 0 .. 6; k = -1 is sigma's column): channel and basis row
+    int kc[7], kj[7];
+#pragma unroll
+    for (int m = 0; m < 7; ++m) {
+      const int k = q + 4 * m - 1;
+      kc[m] = k < 0 ? 0 : k / kBakeSh;
+      kj[m] = k < 0 ? 0 : k - kBakeSh * (k / kBakeSh);
+    }
+#pragma unroll 1
+    for (int j = 0; j < my_tiles; ++j) {
+      const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
+      const int64_t p0 = tile * kRows + 64 * wg;  // first row of this warpgroup's block
+      // ---- the row's lattice point (mesh_sparse_points, halo 0) -> encodings -> operand tile, as the pts forward
+      {
+        const int64_t r = (p0 + row < R) ? p0 + row : R - 1;
+        const int64_t slot = first + r / kBakePts;
+        const int lp = (int)(r % kBakePts);
+        const int l[3] = {lp % 9, (lp / 9) % 9, lp / 81};
+        const int b = bricks[slot];
+        const int bc[3] = {b % nb[0], (b / nb[0]) % nb[1], b / (nb[0] * nb[1])};
+        const int nf = p.n_freq_xyz, mid = nf >> 1;
+        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
+        const int base = p.inc_xyz ? 3 : 0;
+        const int trow = 64 * wg + row;
+        auto put = [&](int k, float v) {
+          uint32_t hi, lo;
+          split_f16x2(v * kActScale, 0.f, hi, lo);
+          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
+          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
+          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
+        };
+        for (int c = 0; c < 3; ++c) {
+          const int li = min(bc[c] * kBakeBrick + l[c], box.res[c]);
+          const float x = bake_coord(box, c, li);
+          if (p.inc_xyz && half == 0) put(c, x);
+          for (int f = f0; f < f1; ++f) {
+            float sn, cs;
+            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
+            put(base + 6 * f + c, sn);
+            put(base + 6 * f + 3 + c, cs);
+          }
+        }
+        if (half == 1)
+          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+      }
+      fence_proxy_async();
+      wg_bar();
+      // ---- trunk (+ fc_feat): the heads' outputs -> s_head
+#pragma unroll 1
+      for (int e = 0; e < n_body; ++e) {
+        if (p.g[e].n == kH)
+          fwd_layer<false, false, kH, kStage>(p, blob, s_head, nullptr, sm, mp, e, wg, kRows, 0, 0, rs, ring, s_bias,
+                                              s_headw, s_headb, nullptr, hw1);
+        else
+          fwd_layer<false, false, kH / 2, kStage>(p, blob, s_head, nullptr, sm, mp, e, wg, kRows, 0, 0, rs, ring, s_bias,
+                                                  s_headw, s_headb, nullptr, hw1);
+      }
+      __syncwarp();  // a quad's head row was written by its lane 0
+      float sh[2][7];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int m = 0; m < 7; ++m) sh[i][m] = 0.f;
+      if (p.use_viewdirs) {
+        // ---- layers_dir[0] once, then per direction: bias, ReLU, fc_rgb, SH accumulation
+        float acc[kN / 2];
+        bake_dir_mma<kN, kStage>(p, blob, acc, sm, mp, wg, kRows, ring);
+        const GemmLayer& gd = p.g[p.n_gemm - 1];
+        const float lb = gd.relu ? 0.f : -3.4e38f;
+        const float* hw = s_headw + hw1;
+        const int hk = p.h[1].k;
+#pragma unroll 1
+        for (int d = 0; d < kBakeDirs; ++d) {
+          const float* vb = s_dirb + d * kN;
+          float hacc[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+          for (int jj = 0; jj < kN / 8; ++jj) {
+            const int col = 8 * jj + 2 * q;
+            const float2 bb = *reinterpret_cast<const float2*>(vb + col);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const float Y0 = fmax_nan(acc[4 * jj + 2 * i] + bb.x, lb), Y1 = fmax_nan(acc[4 * jj + 2 * i + 1] + bb.y, lb);
+              const float x0 = Y0 * kLoInv, x1 = Y1 * kLoInv;
+#pragma unroll
+              for (int c = 0; c < 3; ++c) {
+                const float2 w = *reinterpret_cast<const float2*>(hw + c * hk + col);
+                hacc[i][c] = fmaf(x0, w.x, fmaf(x1, w.y, hacc[i][c]));
+              }
+            }
+          }
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float lg[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+              hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 1);
+              hacc[i][c] += __shfl_xor_sync(0xffffffffu, hacc[i][c], 2);
+              lg[c] = hacc[i][c] + s_headb[4 + c];
+            }
+            const int64_t r = p0 + lr0 + 8 * i;
+            if (logits && q < 3 && r < R) logits[(r * kBakeDirs + d) * 3 + q] = lg[q == 0 ? 0 : q == 1 ? 1 : 2];
+#pragma unroll
+            for (int m = 0; m < 7; ++m) {
+              const float v = kc[m] == 0 ? lg[0] : kc[m] == 1 ? lg[1] : lg[2];
+              sh[i][m] = fmaf(s_basis->proj[kj[m]][d], v, sh[i][m]);
+            }
+          }
+        }
+      } else {
+        // ---- no view directions: fc_out's logits; coefficient 0 = logit / Y_0
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float* hr = s_head + (lr0 + 8 * i) * 4;
+          const int64_t r = p0 + lr0 + 8 * i;
+          if (logits && q < 3 && r < R)
+            for (int d = 0; d < kBakeDirs; ++d) logits[(r * kBakeDirs + d) * 3 + q] = hr[q];
+#pragma unroll
+          for (int m = 0; m < 7; ++m)
+            if (q + 4 * m - 1 >= 0 && kj[m] == 0) sh[i][m] = __fdiv_rn(hr[kc[m]], 0.28209479177387814f);
+        }
+      }
+      // ---- values: lane q writes columns q, q + 4, ..., q + 28 of its two rows
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int64_t r = p0 + lr0 + 8 * i;
+        if (r < R) {
+          float* out = values + (first * kBakePts + r) * kBakeCh;
+          const float sigma = s_head[(lr0 + 8 * i) * 4 + 3];
+#pragma unroll
+          for (int m = 0; m < 8; ++m) {
+            const int k = q + 4 * m - 1;
+            out[q + 4 * m] = k < 0 ? sigma : (m < 7 && k < kBakeSh * 3) ? sh[i][m < 7 ? m : 0] : 0.f;
+          }
+        }
+      }
+      wg_bar();  // s_head is read before the next tile's heads overwrite it
+    }
+  }
+}
+
+// what the bake needs beyond the wgmma inference forward (tc_supported)
+int bake_tc_supported(const Plan& p, const char* what) {
+  if (bake_smem_map(p).m.n_stages < 2) {
+    set_error("%s: network too deep for the bake's shared-memory budget (%d layers)", what, p.n_gemm);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  if (p.use_viewdirs && (p.h[1].n_out != 3 || p.h[1].out_col != 0)) {
+    set_error("%s: the colour head must be fc_rgb with 3 outputs", what);
+    return NERFB200_ERR_UNSUPPORTED;
+  }
+  return NERFB200_OK;
+}
+
+template <int kH>
+static int launch_bake(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
+                       int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
+  constexpr int kRows = 64 * bake_wg(kH), kThreads = 2 * kRows + 32;
+  const int64_t R = count * kBakePts;
+  const int64_t tiles = (R + kRows - 1) / kRows;
+  return launch_persistent(bake_tc_kernel<kH>, tiles, kThreads, bake_smem_map(p).m.total, s, "bake launch", p, basis,
+                           blob, box, (const int*)bricks, first, R, tiles, values, logits);
+}
+
+int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
+                   int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
+  return p.hidden == 256 ? launch_bake<256>(p, blob, box, bricks, first, count, values, logits, basis, s)
+                         : launch_bake<128>(p, blob, box, bricks, first, count, values, logits, basis, s);
+}
+
 }  // namespace nerfb200

@@ -1006,3 +1006,47 @@ def ndc_grad_to_world(ndc: Ndc, q, rows, out: Optional[torch.Tensor] = None) -> 
     _lib.check(_lib.load().nerfb200_ndc_grad_to_world(C.byref(ndc), _ptr(q) if n else None, _ptr(rows) if n else None,
                                                       n, _ptr(out) if n else None, _stream()), "ndc_grad_to_world")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# baked fields (include/nerfb200.h "baked fields"): density and SH colour coefficients on the bricks of a lattice
+# ------------------------------------------------------------------------------------------------
+def bake_dirs() -> int:
+    """Directions a bake evaluates the colour at (NERFB200_BAKE_DIRS)."""
+    return 64
+
+
+def bake_basis() -> Tuple[torch.Tensor, torch.Tensor]:
+    """The library's bake directions (64, 3) and SH projection M (9, 64), fp32 CPU tensors."""
+    dirs = torch.empty(bake_dirs(), 3, dtype=torch.float32)
+    proj = torch.empty(9, bake_dirs(), dtype=torch.float32)
+    f = C.POINTER(C.c_float)
+    _lib.check(_lib.load().nerfb200_bake_basis(C.cast(dirs.data_ptr(), f), C.cast(proj.data_ptr(), f)), "bake_basis")
+    return dirs, proj
+
+
+def bake_refusal(arch: ArchSpec) -> Optional[str]:
+    """None when ``bake`` runs ``arch``, else the library's reason (no device is touched)."""
+    lib = _lib.load()
+    if lib.nerfb200_bake_supported(C.byref(arch.c_struct())) == _lib.OK:
+        return None
+    return lib.nerfb200_last_error().decode(errors="replace")
+
+
+def bake(arch: ArchSpec, blob, box: Grid, bricks, first: int, count: int, values, logits=None):
+    """The values of slots first .. first + count - 1 into ``values`` (n_active, 729, 32); ``logits`` (count * 729, 64,
+    3) or None receives the network's rgb logits at the 64 directions (a test hook)."""
+    _lib.check(_lib.load().nerfb200_bake(C.byref(arch.c_struct()), _ptr(blob), C.byref(box), _ptr(bricks), int(first),
+                                         int(count), _ptr(values), _ptr(logits), _stream()), "bake")
+    return values
+
+
+def baked_render(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool,
+                 stop_transmittance: float = 0.0, out=None) -> torch.Tensor:
+    """Rows (n, 8) = [r g b disp acc depth 0 0] of the packed ``rays`` through a baked field."""
+    n = rays.shape[0]
+    out = torch.empty(n, 8, dtype=torch.float32, device=rays.device) if out is None else out
+    _lib.check(_lib.load().nerfb200_baked_render(C.byref(box), _ptr(brick_map), _ptr(values), int(bool(use_viewdirs)),
+                                                 _ptr(rays), rays.shape[1], n, int(bool(white_background)),
+                                                 float(stop_transmittance), _ptr(out), _stream()), "baked_render")
+    return out

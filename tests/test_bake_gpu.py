@@ -1,0 +1,329 @@
+"""GPU: baked fields (nb.bake / nb.render_baked; csrc/mlp_tc.cu bake_tc_kernel, csrc/baked.cu; include/nerfb200.h
+"baked fields").
+
+  1. the bake against the network: sigma_raw and the logits hook at all 64 directions bit-equal mlp_fwd_pts(impl=1) at
+     the same points; the SH coefficients match an fp64 projection of those logits.  Lego A0 (shipped), A1 and A2 at
+     init, a coarse-only network without view directions, fern A0 in NDC; 1 brick and a count that ends mid-tile;
+  2. the bricks are mesh_sparse_bricks'; an empty grid renders acc = 0 and the background;
+  3. the renderer against an fp64 restatement that gathers from the kernel's own values: Blender and NDC rays, with and
+     without view directions and a white background, rays that miss the box; early stopping;
+  4. reproducibility, save / load;
+  5. quality: PSNR of render_baked against render_image's fine output on lego (256^3, 512^3) and fern."""
+import math
+
+import numpy as np
+import pytest
+import torch
+
+from helpers import bits_equal, load_weights
+
+pytestmark = pytest.mark.gpu
+
+LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
+FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
+# coefficients against the fp64 projection of the kernel's own logits: |c - c64| <= COEF_REL * max |logit| of the point.
+# The fp32 fmaf chain over 64 terms; measured on an H100 80GB HBM3 at 700 W: at most 1.5e-6 (lego, fern).
+COEF_REL = 4e-6
+# the renderer against its fp64 restatement (absolute on rgb / acc, relative to far on depth); measured on an H100 80GB
+# HBM3 at 700 W: rgb 1.1e-6, acc 1.6e-6, depth 1.1e-6 far
+OUT_ABS = 1e-5
+
+
+def report(what, ctx, value):
+    print(f"[bake] {what} {ctx}: {value}")
+
+
+def _pose(kind):
+    from oracle import nerf_oracle as O
+
+    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
+
+
+def _model(kind, coarse=False):
+    """(model, encode_position_fn, encode_direction_fn, camera (H, W, focal, pose, no_ndc, near, far), box); with
+    ``coarse`` the shipped scenes' coarse network instead of the fine one."""
+    import nerf_pytorch_b200 as nb
+
+    lego_cam = (48, 48, 66.7, "spherical", True, 2.0, 6.0)
+    if kind in ("lego", "fern"):
+        w = load_weights(f"{kind}_lowres")
+        l_xyz = 10 if kind == "lego" else 6
+        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
+                                 num_encoding_fn_dir=4)
+        m.load_state_dict(w[0 if coarse else 1])
+        cam = lego_cam if kind == "lego" else (42, 56, 45.3, "eye", False, 0.0, 1.0)
+        return m.cuda(), nb.get_embedding_function(l_xyz), nb.get_embedding_function(4), cam, \
+            LEGO_BOX if kind == "lego" else FERN_BOX
+    torch.manual_seed(7)
+    if kind == "a1":
+        m = nb.FlexibleNeRFModel(num_layers=8, hidden_size=128, skip_connect_every=3, num_encoding_fn_xyz=10)
+    elif kind == "a2":
+        m = nb.FlexibleNeRFModel(num_layers=8, hidden_size=256, skip_connect_every=4, num_encoding_fn_xyz=10)
+    else:  # "noview": coarse-only, no view directions
+        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
+                                 use_viewdirs=False)
+    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4), lego_cam, ((-1.0,) * 3, (1.0,) * 3)
+
+
+def _arch_blob(m, epf, edf):
+    from nerf_pytorch_b200 import mesh, train_utils
+
+    arch = mesh._network(m, epf, edf)
+    return arch, train_utils._packed(m, arch)[1]
+
+
+def _field(kind, res=16, grid=None):
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
+
+    m, epf, edf, cam, box = _model(kind)
+    grid = OccupancyGrid.full(box, 8) if grid is None else grid
+    return nb.bake(m, epf, edf if m.use_viewdirs else None, bounds=box, resolution=res, grid=grid), m, epf, edf, cam
+
+
+def _net_at(arch, blob, pts, direction):
+    """raw (P, 4) of mlp_fwd_pts(impl=1) at pts (P, 3), every point with `direction` (None without view directions)."""
+    from nerf_pytorch_b200 import ops
+
+    P = pts.shape[0]
+    rows = -(-P // 64)
+    pad = torch.cat([pts, pts[-1:].expand(rows * 64 - P, 3)]).contiguous()
+    dirs = None if direction is None else direction.view(1, 3).expand(rows, 3).contiguous()
+    return ops.mlp_fwd_pts(arch, blob, pad.view(rows, 64, 3), dirs, impl=1).view(-1, 4)[:P]
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 1. the bake against the network
+# ------------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("count", [1, 3])
+@pytest.mark.parametrize("kind", ["lego", "a1", "a2", "noview", "fern"])
+def test_bake_matches_the_network(kind, count):
+    from nerf_pytorch_b200 import ops
+
+    m, epf, edf, _, box = _model(kind)
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
+
+    arch, blob = _arch_blob(m, epf, edf if m.use_viewdirs else None)
+    g = ops.grid_struct(box, (24, 24, 24))
+    brick_map, bricks, n = ops.mesh_sparse_bricks(g, OccupancyGrid.full(box, 8))
+    first = 5
+    P = count * 729
+    values = torch.full((int(n.item()), 729, 32), float("nan"), device="cuda")
+    logits = torch.empty(P, 64, 3, device="cuda")
+    ops.bake(arch, blob, g, bricks, first, count, values, logits)
+    pts = torch.empty(P, 3, device="cuda")
+    ops.mesh_sparse_points(g, bricks, first, count, False, pts)
+    dirs, proj = ops.bake_basis()
+    got = values[first:first + count].reshape(P, 32)
+    want_sigma = _net_at(arch, blob, pts, None if not arch.use_viewdirs else dirs[0].cuda())[:, 3]
+    assert bits_equal(got[:, 0], want_sigma), kind
+    if arch.use_viewdirs:
+        for d in range(64):
+            raw = _net_at(arch, blob, pts, dirs[d].cuda())
+            assert bits_equal(logits[:, d], raw[:, :3]), (kind, d)
+        coef64 = torch.einsum("jd,pdc->pcj", proj.double().cuda(), logits.double())
+    else:
+        raw = _net_at(arch, blob, pts, None)
+        assert bits_equal(logits, raw[:, None, :3].expand(P, 64, 3)), kind
+        coef64 = torch.zeros(P, 3, 9, dtype=torch.float64, device="cuda")
+        coef64[:, :, 0] = raw[:, :3].double() / np.float32(0.28209479177387814)
+    scale = logits.abs().amax(dim=(1, 2)).double()[:, None]
+    err = ((got[:, 1:28].double().view(P, 3, 9) - coef64).abs().view(P, 27) / scale.clamp_min(1e-30)).max().item()
+    report("coefficient error / max |logit|", (kind, count), err)
+    assert err <= COEF_REL, (kind, err)
+    assert (got[:, 28:] == 0).all()
+    untouched = torch.ones(values.shape[0], dtype=torch.bool)
+    untouched[first:first + count] = False
+    assert torch.isnan(values[untouched.cuda()]).all()
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 2. bricks; an empty grid
+# ------------------------------------------------------------------------------------------------------------------------
+def test_bricks_are_the_sparse_meshes_and_an_empty_grid_renders_the_background():
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200 import ops
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
+    from oracle import nerf_oracle as O
+
+    m, epf, edf, cam, box = _model("lego")
+    grid = OccupancyGrid.from_models([m], epf, box, 32, encode_direction_fn=edf)
+    f = nb.bake(m, epf, edf, bounds=box, resolution=40, grid=grid)
+    bm, br, n = ops.mesh_sparse_bricks(ops.grid_struct(box, (40,) * 3), grid)
+    assert bits_equal(f.brick_map, bm) and bits_equal(f.bricks, br[:int(n.item())])
+    assert 0 < f.n_active < bm.numel()
+    H, W, focal, pose, no_ndc, near, far = cam
+    # a lattice point outside the grid's box makes its brick active: the empty grid covers the whole lattice
+    empty = OccupancyGrid.empty(((-2.0,) * 3, (2.0,) * 3), 32)
+    for white in (False, True):
+        e = nb.bake(m, epf, edf, bounds=box, resolution=40, grid=empty)
+        assert e.n_active == 0
+        opts = O.make_options(no_ndc=no_ndc, near=near, far=far, white_background=white)
+        rgb, disp, acc = nb.render_baked(e, H, W, focal, _pose(pose), opts)
+        assert (acc == 0).all() and (rgb == (1.0 if white else 0.0)).all() and torch.isnan(disp).all()
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 3. the renderer against fp64
+# ------------------------------------------------------------------------------------------------------------------------
+def _render64(field, rays, white):
+    """fp64 restatement of the header's rendering, gathering from the kernel's values; the sample depths, points and
+    cells are formed in fp32 as the header states.  (rgb, acc, depth, disp) per ray."""
+    f32 = torch.float32
+    lo = torch.tensor(field.bounds[0], dtype=f32, device="cuda")
+    hi = torch.tensor(field.bounds[1], dtype=f32, device="cuda")
+    res = torch.tensor(field.resolution, device="cuda")
+    o, d = rays[:, :3], rays[:, 3:6]
+    t0, t1 = (lo - o) / d, (hi - o) / d
+    ta = torch.fmax(rays[:, 6], torch.fmin(t0, t1).nan_to_num(nan=-math.inf).amax(-1))
+    tb = torch.fmin(rays[:, 7], torch.fmax(t0, t1).nan_to_num(nan=math.inf).amin(-1))
+    h = ((hi - lo) / res.to(f32)).min()
+    dn = torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
+    dt = (torch.tensor(0.5, dtype=f32, device="cuda") * h) / dn
+    K = int(((tb - ta) / dt).clamp(0, 1 << 16).nan_to_num(0).max().item()) + 2
+    k = torch.arange(K, device="cuda", dtype=f32) + 0.5
+    t = ta[:, None] + k[None] * dt[:, None]
+    valid = t < tb[:, None]
+    x = o[:, None] + d[:, None] * t[..., None]
+    scale = res.to(f32) / (hi - lo)
+    tc = (x - lo) * scale
+    inside = ((tc >= 0) & (tc < res.to(f32))).all(-1) & valid
+    i = torch.where(inside[..., None], tc, torch.zeros_like(tc)).to(torch.int64).clamp_max(res - 1)
+    fr = (tc - i.to(f32)).double()
+    nb_ = (res + 7) // 8
+    b = i // 8
+    slot = field.brick_map.long()[((b[..., 2] * nb_[1] + b[..., 1]) * nb_[0] + b[..., 0]).clamp(0, field.brick_map.numel() - 1)]
+    hit = inside & (slot >= 0)
+    l = i % 8
+    vals = field.values.double() if field.n_active else torch.zeros(1, 729, 32, dtype=torch.float64, device="cuda")
+    v = torch.zeros(*t.shape, 28, dtype=torch.float64, device="cuda")
+    for c in range(8):
+        off = torch.tensor([c & 1, c >> 1 & 1, c >> 2], device="cuda")
+        lc = l + off
+        w = torch.where(off.bool(), fr, 1 - fr).prod(-1)
+        idx = (lc[..., 2] * 9 + lc[..., 1]) * 9 + lc[..., 0]
+        v += w[..., None] * vals[slot.clamp_min(0), idx][..., :28]
+    sigma = torch.where(hit, v[..., 0], torch.zeros_like(v[..., 0]))
+    coef = v[..., 1:].view(*t.shape, 3, 9)
+    if field.use_viewdirs:
+        vd = rays[:, 8:11].double()
+        X, Y, Z = vd[:, 0], vd[:, 1], vd[:, 2]
+        Ysh = torch.stack([torch.full_like(X, 0.28209479177387814), -0.4886025119029199 * Y, 0.4886025119029199 * Z,
+                           -0.4886025119029199 * X, 1.0925484305920792 * X * Y, -1.0925484305920792 * Y * Z,
+                           0.31539156525252005 * (2 * Z * Z - X * X - Y * Y), -1.0925484305920792 * X * Z,
+                           0.5462742152960396 * (X * X - Y * Y)], -1)
+        s = (coef * Ysh[:, None, None, :]).sum(-1)
+    else:
+        s = coef[..., 0] * 0.28209479177387814
+    rgb = torch.where(hit[..., None], torch.sigmoid(s), torch.zeros_like(s))
+    alpha = 1 - torch.exp(-torch.relu(sigma) * (dt.double() * dn.double())[:, None])
+    alpha = torch.where(valid, alpha, torch.zeros_like(alpha))
+    q = 1 - alpha + 1e-10
+    T = torch.cat([torch.ones_like(q[:, :1]), torch.cumprod(q, -1)[:, :-1]], -1)
+    w = alpha * T
+    acc = w.sum(-1)
+    depth = (w * t.double()).sum(-1)
+    out_rgb = (w[..., None] * rgb).sum(1) + ((1 - acc)[:, None] if white else 0)
+    return out_rgb, acc, depth, 1 / torch.clamp(depth / acc, min=1e-10)
+
+
+def _rays(cam, use_viewdirs):
+    from nerf_pytorch_b200 import ops
+
+    H, W, focal, pose, no_ndc, near, far = cam
+    return ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far,
+                        use_viewdirs=use_viewdirs)
+
+
+@pytest.mark.parametrize("white", [False, True])
+@pytest.mark.parametrize("kind", ["lego", "noview", "fern"])
+def test_renderer_matches_fp64(kind, white):
+    from nerf_pytorch_b200 import ops
+
+    field, m, *_, cam = _field(kind, res=(24, 20, 28))
+    rays = _rays(cam, field.use_viewdirs)
+    if kind == "lego":  # rays that miss the box: turned away from it
+        rays[::7, 3:6] = -rays[::7, 3:6]
+    out = ops.baked_render(field.box(), field.brick_map, field.values, field.use_viewdirs, rays, white)
+    rgb, acc, depth, disp = _render64(field, rays, white)
+    far = float(rays[:, 7].max())
+    e_rgb = (out[:, :3].double() - rgb).abs().max().item()
+    e_acc = (out[:, 4].double() - acc).abs().max().item()
+    e_depth = (out[:, 5].double() - depth).abs().max().item() / far
+    report("rgb / acc / depth error", (kind, white), (e_rgb, e_acc, e_depth))
+    assert e_rgb <= OUT_ABS and e_acc <= OUT_ABS and e_depth <= OUT_ABS
+    empty = acc == 0
+    assert torch.isnan(out[empty, 3]).all()
+    ok = acc > 1e-3
+    assert torch.allclose(out[ok, 3].double(), disp[ok], rtol=1e-3)
+    if kind == "lego":
+        assert bool(empty.any()) and bool((acc > 0.5).any())
+
+
+def test_early_stop_guarantee():
+    from nerf_pytorch_b200 import ops
+
+    field, *_, cam = _field("lego", res=32)
+    rays = _rays(cam, True)
+    base = ops.baked_render(field.box(), field.brick_map, field.values, True, rays, False)
+    for t in (1e-3, 0.1, 0.5):
+        e = ops.baked_render(field.box(), field.brick_map, field.values, True, rays, False, t)
+        same = (e == base).all(-1) | ((e[:, 3] != e[:, 3]) & (base[:, 3] != base[:, 3]))
+        stopped = ~same
+        report("rays stopped", t, int(stopped.sum()))
+        assert bool(stopped.any()) and bool(same.any())
+        d = e[stopped] - base[stopped]
+        assert ((d[:, :3] <= 1e-6) & (d[:, :3] >= -t - 1e-6)).all() and ((d[:, 4] <= 1e-6) & (d[:, 4] >= -t - 1e-6)).all()
+        assert (base[stopped, 4] >= 1 - t - 1e-5).all()  # a ray stops only once it is nearly opaque
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 4. reproducibility
+# ------------------------------------------------------------------------------------------------------------------------
+def test_bake_and_render_are_reproducible_and_survive_save_load(tmp_path):
+    import nerf_pytorch_b200 as nb
+    from oracle import nerf_oracle as O
+
+    f1, m, epf, edf, cam = _field("a2", res=24)
+    f2, *_ = _field("a2", res=24)
+    assert bits_equal(f1.values, f2.values)
+    H, W, focal, pose, no_ndc, near, far = cam
+    opts = O.make_options(no_ndc=no_ndc, near=near, far=far)
+    a = nb.render_baked(f1, H, W, focal, _pose(pose), opts)
+    b = nb.render_baked(f1, H, W, focal, _pose(pose), opts)
+    f1.save(tmp_path / "field.pt")
+    g = nb.BakedField.load(tmp_path / "field.pt")
+    c = nb.render_baked(g, H, W, focal, _pose(pose), opts)
+    for x, y, z in zip(a, b, c):
+        assert bits_equal(x, y) and bits_equal(x, z)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 5. quality against the network's render
+# ------------------------------------------------------------------------------------------------------------------------
+# PSNR (dB) of render_baked against render_image's fine output, measured on an H100 80GB HBM3 at 700 W; the test allows
+# PSNR_MARGIN below each
+PSNR_MEASURED = {("lego", 256): 29.38, ("lego", 512): 35.39, ("fern", 256): 27.53}
+PSNR_MARGIN = 1.0
+
+
+@pytest.mark.parametrize("kind,res", list(PSNR_MEASURED))
+def test_quality_against_the_network(kind, res):
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
+    from oracle import nerf_oracle as O
+
+    m, epf, edf, cam, box = _model(kind)
+    H, W, focal, pose, no_ndc, near, far = cam
+    grid = OccupancyGrid.from_models([m], epf, box, 128, encode_direction_fn=edf)
+    field = nb.bake(m, epf, edf, bounds=box, resolution=res, grid=grid)
+    opts = O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=128, perturb=False,
+                          radiance_field_noise_std=0.0)
+    mc = _model(kind, coarse=True)[0]
+    ref = nb.render_image(H, W, focal, _pose(pose), mc, m, opts, encode_position_fn=epf, encode_direction_fn=edf,
+                          impl=1)[3]
+    rgb, _, _ = nb.render_baked(field, H, W, focal, _pose(pose), opts)
+    mse = torch.mean((rgb - ref) ** 2).item()
+    psnr = -10 * math.log10(max(mse, 1e-12))
+    report("PSNR vs render_image", (kind, res, field.n_active), psnr)
+    assert psnr >= PSNR_MEASURED[(kind, res)] - PSNR_MARGIN
