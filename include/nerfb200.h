@@ -587,7 +587,9 @@ int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const ner
  *   - Rendering (baked_render).  Rays are rows [o(3) d(3) near far (viewdir(3))] as gen_rays / pack_rays write them.
  *     All fp32 with round-to-nearest, each op rounded, no contraction unless fmaf is named.
  *       interval  [t_a, t_b] = [near, far] intersected with the box's slab interval (per axis (lo - o) / d and
- *                 (hi - o) / d); h = min over c of (hi_c - lo_c) / res_c, |d| = sqrt((dx dx + dy dy) + dz dz),
+ *                 (hi - o) / d, fminf / fmaxf order).  An axis with d_c = +-0 has x_c = o_c at every sample: it leaves
+ *                 the interval as it is when lo_c <= o_c < hi_c and makes the ray empty otherwise (o_c NaN included);
+ *                 h = min over c of (hi_c - lo_c) / res_c, |d| = sqrt((dx dx + dy dy) + dz dz),
  *                 dt = (0.5 h) / |d|; sample k is t_k = t_a + (k + 0.5) dt for every k with t_k < t_b.
  *       lookup    x = o + d t_k, per axis as the MLP forms its points; its cube i is the cell of x under the cell rule of
  *                 "occupancy grid" applied to the box (t_c = (x_c - lo_c) scale_c, i_c = (int) t_c), f_c = t_c - i_c; the

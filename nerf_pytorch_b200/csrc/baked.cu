@@ -99,10 +99,15 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const f
     o[c] = rr[c];
     d[c] = rr[3 + c];
   }
-  // the interval: [near, far] and the box's slabs
+  // the interval: [near, far] and the box's slabs.  An axis with d_c = +-0 keeps x_c = o_c at every sample: it does not
+  // restrict the interval when lo_c <= o_c < hi_c and empties the ray otherwise (its slab terms would be 0/0 or inf)
   float ta = rr[6], tb = rr[7];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
+    if (d[c] == 0.f) {
+      if (!(o[c] >= B.g.lo[c] && o[c] < B.g.hi[c])) tb = -INFINITY;
+      continue;
+    }
     const float t0 = __fdiv_rn(__fsub_rn(B.g.lo[c], o[c]), d[c]), t1 = __fdiv_rn(__fsub_rn(B.g.hi[c], o[c]), d[c]);
     ta = fmaxf(ta, fminf(t0, t1));
     tb = fminf(tb, fmaxf(t0, t1));

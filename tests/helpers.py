@@ -218,6 +218,104 @@ def compaction_reference(grid, rays, z):
     return keep, rows, blocks
 
 
+# ------------------------------------------------------------------------------------------------------------------------
+# baked fields (include/nerfb200.h "baked fields")
+# ------------------------------------------------------------------------------------------------------------------------
+# coefficients against the fp64 projection of the kernel's own logits: |c - c64| <= COEF_REL * max |logit| of the point.
+# The fp32 fmaf chain over 64 terms; measured on an H100 80GB HBM3 at 700 W: at most 1.5e-6 (lego, fern), 2.0e-6 over the
+# architecture table (test_bake_sweep_gpu, 8x256 "scaled").
+COEF_REL = 4e-6
+# the renderer against its fp64 restatement (absolute on rgb / acc, relative to far on depth); measured on an H100 80GB
+# HBM3 at 700 W: rgb 1.1e-6, acc 1.6e-6, depth 1.1e-6 far on camera rays (test_bake_gpu); rgb 4.8e-6, acc 5.4e-6,
+# depth 1.0e-6 far on the edge rays of test_bake_sweep_gpu (rays through two box corners, ~440 samples)
+OUT_ABS = 1e-5
+
+
+def net_at(arch, blob, pts, direction):
+    """raw (P, 4) of mlp_fwd_pts(impl=1) at pts (P, 3), every point with `direction` (None without view directions)."""
+    from nerf_pytorch_b200 import ops
+
+    P = pts.shape[0]
+    rows = -(-P // 64)
+    pad = torch.cat([pts, pts[-1:].expand(rows * 64 - P, 3)]).contiguous()
+    dirs = None if direction is None else direction.view(1, 3).expand(rows, 3).contiguous()
+    return ops.mlp_fwd_pts(arch, blob, pad.view(rows, 64, 3), dirs, impl=1).view(-1, 4)[:P]
+
+
+def baked_render64(field, rays, white):
+    """fp64 restatement of the header's rendering of a baked field (nb.BakedField), gathering from its values; the
+    interval, sample depths, points and cells are formed in fp32 as the header states.  (rgb, acc, depth, disp) per ray.
+    The slab terms go through fmin / fmax as the kernel's fminf / fmaxf (a NaN term drops out); an axis with d = +-0
+    leaves the interval as it is when lo <= o < hi and empties the ray otherwise.  A ray is live when t_a < t_b and dt is
+    positive, finite and (t_b - t_a) / dt < 2^24."""
+    import math
+
+    f32 = torch.float32
+    dev = rays.device
+    lo = torch.tensor(field.bounds[0], dtype=f32, device=dev)
+    hi = torch.tensor(field.bounds[1], dtype=f32, device=dev)
+    res = torch.tensor(field.resolution, device=dev)
+    o, d = rays[:, :3], rays[:, 3:6]
+    t0, t1 = (lo - o) / d, (hi - o) / d
+    flat = d == 0
+    tmin = torch.where(flat, -math.inf, torch.fmin(t0, t1).nan_to_num(nan=-math.inf))
+    tmax = torch.where(flat, math.inf, torch.fmax(t0, t1).nan_to_num(nan=math.inf))
+    outside = (flat & ~((o >= lo) & (o < hi))).any(-1)
+    ta = torch.fmax(rays[:, 6], tmin.amax(-1))
+    tb = torch.where(outside, -math.inf, torch.fmin(rays[:, 7], tmax.amin(-1)))
+    h = ((hi - lo) / res.to(f32)).min()
+    dn = torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
+    dt = (torch.tensor(0.5, dtype=f32, device=dev) * h) / dn
+    live = (ta < tb) & (dt > 0) & (dt < math.inf) & ((tb - ta) / dt < 16777216.0)
+    K = int(torch.where(live, (tb - ta) / dt, 0.0).max().item()) + 2
+    k = torch.arange(K, device=dev, dtype=f32) + 0.5
+    t = ta[:, None] + k[None] * dt[:, None]
+    valid = (t < tb[:, None]) & live[:, None]
+    t = torch.where(valid, t, 0.0)
+    x = o[:, None] + d[:, None] * t[..., None]
+    scale = res.to(f32) / (hi - lo)
+    tc = (x - lo) * scale
+    inside = ((tc >= 0) & (tc < res.to(f32))).all(-1) & valid
+    i = torch.where(inside[..., None], tc, torch.zeros_like(tc)).to(torch.int64).clamp_max(res - 1)
+    fr = (tc - i.to(f32)).double()
+    nb_ = (res + 7) // 8
+    b = i // 8
+    slot = field.brick_map.long()[((b[..., 2] * nb_[1] + b[..., 1]) * nb_[0] + b[..., 0]).clamp(0, field.brick_map.numel() - 1)]
+    hit = inside & (slot >= 0)
+    l = i % 8
+    vals = field.values.double() if field.n_active else torch.zeros(1, 729, 32, dtype=torch.float64, device=dev)
+    v = torch.zeros(*t.shape, 28, dtype=torch.float64, device=dev)
+    for c in range(8):
+        off = torch.tensor([c & 1, c >> 1 & 1, c >> 2], device=dev)
+        lc = l + off
+        w = torch.where(off.bool(), fr, 1 - fr).prod(-1)
+        idx = (lc[..., 2] * 9 + lc[..., 1]) * 9 + lc[..., 0]
+        w = torch.where(hit, w, 0.0)  # a miss's fractions may be NaN (a NaN origin)
+        v += w[..., None] * vals[slot.clamp_min(0), idx][..., :28]
+    sigma = torch.where(hit, v[..., 0], torch.zeros_like(v[..., 0]))
+    coef = v[..., 1:].view(*t.shape, 3, 9)
+    if field.use_viewdirs:
+        vd = rays[:, 8:11].double()
+        X, Y, Z = vd[:, 0], vd[:, 1], vd[:, 2]
+        Ysh = torch.stack([torch.full_like(X, 0.28209479177387814), -0.4886025119029199 * Y, 0.4886025119029199 * Z,
+                           -0.4886025119029199 * X, 1.0925484305920792 * X * Y, -1.0925484305920792 * Y * Z,
+                           0.31539156525252005 * (2 * Z * Z - X * X - Y * Y), -1.0925484305920792 * X * Z,
+                           0.5462742152960396 * (X * X - Y * Y)], -1)
+        s = (coef * Ysh[:, None, None, :]).sum(-1)
+    else:
+        s = coef[..., 0] * 0.28209479177387814
+    rgb = torch.where(hit[..., None], torch.sigmoid(s), torch.zeros_like(s))
+    alpha = 1 - torch.exp(-torch.relu(sigma) * (dt.double() * dn.double())[:, None])
+    alpha = torch.where(valid, alpha, torch.zeros_like(alpha))
+    q = 1 - alpha + 1e-10
+    T = torch.cat([torch.ones_like(q[:, :1]), torch.cumprod(q, -1)[:, :-1]], -1)
+    w = alpha * T
+    acc = w.sum(-1)
+    depth = (w * t.double()).sum(-1)
+    out_rgb = (w[..., None] * rgb).sum(1) + ((1 - acc)[:, None] if white else 0)
+    return out_rgb, acc, depth, 1 / torch.clamp(depth / acc, min=1e-10)
+
+
 def bits_equal(a, b):
     """Same shape and the same bits (4-byte elements); two Nones are equal."""
     if a is None or b is None:

@@ -15,18 +15,12 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import bits_equal, load_weights
+from helpers import COEF_REL, OUT_ABS, baked_render64, bits_equal, load_weights, net_at
 
 pytestmark = pytest.mark.gpu
 
 LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
 FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
-# coefficients against the fp64 projection of the kernel's own logits: |c - c64| <= COEF_REL * max |logit| of the point.
-# The fp32 fmaf chain over 64 terms; measured on an H100 80GB HBM3 at 700 W: at most 1.5e-6 (lego, fern).
-COEF_REL = 4e-6
-# the renderer against its fp64 restatement (absolute on rgb / acc, relative to far on depth); measured on an H100 80GB
-# HBM3 at 700 W: rgb 1.1e-6, acc 1.6e-6, depth 1.1e-6 far
-OUT_ABS = 1e-5
 
 
 def report(what, ctx, value):
@@ -81,17 +75,6 @@ def _field(kind, res=16, grid=None):
     return nb.bake(m, epf, edf if m.use_viewdirs else None, bounds=box, resolution=res, grid=grid), m, epf, edf, cam
 
 
-def _net_at(arch, blob, pts, direction):
-    """raw (P, 4) of mlp_fwd_pts(impl=1) at pts (P, 3), every point with `direction` (None without view directions)."""
-    from nerf_pytorch_b200 import ops
-
-    P = pts.shape[0]
-    rows = -(-P // 64)
-    pad = torch.cat([pts, pts[-1:].expand(rows * 64 - P, 3)]).contiguous()
-    dirs = None if direction is None else direction.view(1, 3).expand(rows, 3).contiguous()
-    return ops.mlp_fwd_pts(arch, blob, pad.view(rows, 64, 3), dirs, impl=1).view(-1, 4)[:P]
-
-
 # ------------------------------------------------------------------------------------------------------------------------
 # 1. the bake against the network
 # ------------------------------------------------------------------------------------------------------------------------
@@ -115,15 +98,15 @@ def test_bake_matches_the_network(kind, count):
     ops.mesh_sparse_points(g, bricks, first, count, False, pts)
     dirs, proj = ops.bake_basis()
     got = values[first:first + count].reshape(P, 32)
-    want_sigma = _net_at(arch, blob, pts, None if not arch.use_viewdirs else dirs[0].cuda())[:, 3]
+    want_sigma = net_at(arch, blob, pts, None if not arch.use_viewdirs else dirs[0].cuda())[:, 3]
     assert bits_equal(got[:, 0], want_sigma), kind
     if arch.use_viewdirs:
         for d in range(64):
-            raw = _net_at(arch, blob, pts, dirs[d].cuda())
+            raw = net_at(arch, blob, pts, dirs[d].cuda())
             assert bits_equal(logits[:, d], raw[:, :3]), (kind, d)
         coef64 = torch.einsum("jd,pdc->pcj", proj.double().cuda(), logits.double())
     else:
-        raw = _net_at(arch, blob, pts, None)
+        raw = net_at(arch, blob, pts, None)
         assert bits_equal(logits, raw[:, None, :3].expand(P, 64, 3)), kind
         coef64 = torch.zeros(P, 3, 9, dtype=torch.float64, device="cuda")
         coef64[:, :, 0] = raw[:, :3].double() / np.float32(0.28209479177387814)
@@ -166,67 +149,6 @@ def test_bricks_are_the_sparse_meshes_and_an_empty_grid_renders_the_background()
 # ------------------------------------------------------------------------------------------------------------------------
 # 3. the renderer against fp64
 # ------------------------------------------------------------------------------------------------------------------------
-def _render64(field, rays, white):
-    """fp64 restatement of the header's rendering, gathering from the kernel's values; the sample depths, points and
-    cells are formed in fp32 as the header states.  (rgb, acc, depth, disp) per ray."""
-    f32 = torch.float32
-    lo = torch.tensor(field.bounds[0], dtype=f32, device="cuda")
-    hi = torch.tensor(field.bounds[1], dtype=f32, device="cuda")
-    res = torch.tensor(field.resolution, device="cuda")
-    o, d = rays[:, :3], rays[:, 3:6]
-    t0, t1 = (lo - o) / d, (hi - o) / d
-    ta = torch.fmax(rays[:, 6], torch.fmin(t0, t1).nan_to_num(nan=-math.inf).amax(-1))
-    tb = torch.fmin(rays[:, 7], torch.fmax(t0, t1).nan_to_num(nan=math.inf).amin(-1))
-    h = ((hi - lo) / res.to(f32)).min()
-    dn = torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
-    dt = (torch.tensor(0.5, dtype=f32, device="cuda") * h) / dn
-    K = int(((tb - ta) / dt).clamp(0, 1 << 16).nan_to_num(0).max().item()) + 2
-    k = torch.arange(K, device="cuda", dtype=f32) + 0.5
-    t = ta[:, None] + k[None] * dt[:, None]
-    valid = t < tb[:, None]
-    x = o[:, None] + d[:, None] * t[..., None]
-    scale = res.to(f32) / (hi - lo)
-    tc = (x - lo) * scale
-    inside = ((tc >= 0) & (tc < res.to(f32))).all(-1) & valid
-    i = torch.where(inside[..., None], tc, torch.zeros_like(tc)).to(torch.int64).clamp_max(res - 1)
-    fr = (tc - i.to(f32)).double()
-    nb_ = (res + 7) // 8
-    b = i // 8
-    slot = field.brick_map.long()[((b[..., 2] * nb_[1] + b[..., 1]) * nb_[0] + b[..., 0]).clamp(0, field.brick_map.numel() - 1)]
-    hit = inside & (slot >= 0)
-    l = i % 8
-    vals = field.values.double() if field.n_active else torch.zeros(1, 729, 32, dtype=torch.float64, device="cuda")
-    v = torch.zeros(*t.shape, 28, dtype=torch.float64, device="cuda")
-    for c in range(8):
-        off = torch.tensor([c & 1, c >> 1 & 1, c >> 2], device="cuda")
-        lc = l + off
-        w = torch.where(off.bool(), fr, 1 - fr).prod(-1)
-        idx = (lc[..., 2] * 9 + lc[..., 1]) * 9 + lc[..., 0]
-        v += w[..., None] * vals[slot.clamp_min(0), idx][..., :28]
-    sigma = torch.where(hit, v[..., 0], torch.zeros_like(v[..., 0]))
-    coef = v[..., 1:].view(*t.shape, 3, 9)
-    if field.use_viewdirs:
-        vd = rays[:, 8:11].double()
-        X, Y, Z = vd[:, 0], vd[:, 1], vd[:, 2]
-        Ysh = torch.stack([torch.full_like(X, 0.28209479177387814), -0.4886025119029199 * Y, 0.4886025119029199 * Z,
-                           -0.4886025119029199 * X, 1.0925484305920792 * X * Y, -1.0925484305920792 * Y * Z,
-                           0.31539156525252005 * (2 * Z * Z - X * X - Y * Y), -1.0925484305920792 * X * Z,
-                           0.5462742152960396 * (X * X - Y * Y)], -1)
-        s = (coef * Ysh[:, None, None, :]).sum(-1)
-    else:
-        s = coef[..., 0] * 0.28209479177387814
-    rgb = torch.where(hit[..., None], torch.sigmoid(s), torch.zeros_like(s))
-    alpha = 1 - torch.exp(-torch.relu(sigma) * (dt.double() * dn.double())[:, None])
-    alpha = torch.where(valid, alpha, torch.zeros_like(alpha))
-    q = 1 - alpha + 1e-10
-    T = torch.cat([torch.ones_like(q[:, :1]), torch.cumprod(q, -1)[:, :-1]], -1)
-    w = alpha * T
-    acc = w.sum(-1)
-    depth = (w * t.double()).sum(-1)
-    out_rgb = (w[..., None] * rgb).sum(1) + ((1 - acc)[:, None] if white else 0)
-    return out_rgb, acc, depth, 1 / torch.clamp(depth / acc, min=1e-10)
-
-
 def _rays(cam, use_viewdirs):
     from nerf_pytorch_b200 import ops
 
@@ -245,7 +167,7 @@ def test_renderer_matches_fp64(kind, white):
     if kind == "lego":  # rays that miss the box: turned away from it
         rays[::7, 3:6] = -rays[::7, 3:6]
     out = ops.baked_render(field.box(), field.brick_map, field.values, field.use_viewdirs, rays, white)
-    rgb, acc, depth, disp = _render64(field, rays, white)
+    rgb, acc, depth, disp = baked_render64(field, rays, white)
     far = float(rays[:, 7].max())
     e_rgb = (out[:, :3].double() - rgb).abs().max().item()
     e_acc = (out[:, 4].double() - acc).abs().max().item()

@@ -136,3 +136,33 @@ def test_python_refusals_precede_any_launch():
     with pytest.raises(NotImplementedError):
         nb.render_baked(f, 8, 8, 10.0, torch.eye(4), opts)
     assert ops.launch_count() == before
+
+
+# encodings of the support sweep: (n_freq_xyz, n_freq_dir) 10/4 as shipped, 10/5 without the raw direction input (30
+# channels), none, and no view directions
+SUPPORT_ENCODINGS = {
+    "10/4": dict(n_freq_xyz=10, n_freq_dir=4),
+    "10/5_noinput_dir": dict(n_freq_xyz=10, n_freq_dir=5, include_input_dir=False),
+    "0/0": dict(n_freq_xyz=0, n_freq_dir=0),
+    "noview": dict(n_freq_xyz=10, use_viewdirs=False),
+}
+
+
+@pytest.mark.parametrize("hidden", [128, 256])
+def test_bake_takes_exactly_what_the_wgmma_forward_takes(hidden):
+    """Over 1 .. 16 layers, skip 1 .. 5 and SUPPORT_ENCODINGS, bake_refusal is None exactly when the wgmma inference
+    forward takes the architecture.  The bake's own "too deep for its shared-memory budget" refusal is unreachable
+    there: a layout change that makes it reachable shows up here first."""
+    from nerf_pytorch_b200 import ops
+
+    taken = 0
+    for layers in range(1, 17):
+        for skip in range(1, 6):
+            for enc, kw in SUPPORT_ENCODINGS.items():
+                arch = ops.ArchSpec(num_layers=layers, hidden=hidden, skip_every=skip, **kw)
+                why = ops.bake_refusal(arch)
+                fwd = ops.impl_supported(arch, 64, ops.IMPL_TC_FWD)
+                assert (why is None) == fwd, (layers, skip, enc, why)
+                assert why is None or "too deep" not in why, (layers, skip, enc, why)
+                taken += why is None
+    assert taken > 0
