@@ -632,6 +632,59 @@ int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_m
                               int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                               int32_t white_background, float stop_transmittance, float* out, void* stream);
 
+/* ---- baked fields: gradients and fine-tuning -------------------------------------------------------------------------
+ * The gradient of baked_render (stop_transmittance 0) with respect to the values, the tie that keeps every stored copy
+ * of a lattice point equal, and an Adam step over the values, so a baked field can be fine-tuned on images through its
+ * own renderer (as PlenOctrees / SNeRG fine-tune theirs).  All fp32, each op rounded, no contraction.
+ *   - Backward (baked_render_bwd).  One warp per ray re-marches the ray exactly as baked_render does (interval, t_k,
+ *     lookup, interp, colour, alpha, q, T in rounds of 32).  out is the forward's [n][8] rows, g_out the upstream
+ *     gradient rows in the same layout [g_r g_g g_b g_disp g_acc g_depth - -].  Per ray:
+ *       G_acc = g_acc, G_depth = g_depth; a white background adds -(g_r + g_g + g_b) to G_acc; when g_disp != 0 and
+ *       ratio = depth / acc is > 1e-10 or NaN, disp = 1 / ratio, G_depth += g_disp (-disp disp) / acc and G_acc +=
+ *       g_disp (disp disp) depth / (acc acc) (the compositing backward's rule, one shared device function);
+ *       E = (((g_r r' + g_g g') + g_b b') + G_acc acc) + G_depth depth from the forward's totals, r' = r - (1 - acc) etc.
+ *       with a white background.
+ *     Per sample (c its rgb, w = alpha T): v = (((g_r c_r + g_g c_g) + g_b c_b) + G_acc) + G_depth t;
+ *       P = the running sum of w v in sample order, this sample included (one fp32 add per sample, lane order);
+ *       dL/dalpha = T v - (E - P) / q;  dsigma_raw = gate ? (dL/dalpha delta) exp(-sigma delta) : 0;
+ *       d s_c = ((w g_c) c_c) (1 - c_c);  d coef_cj = d s_c Y_j with view directions; without them d coef_c0 = d s_c Y_0
+ *       and the other coefficients receive 0.
+ *     S = E - P stands for the suffix sum over later samples that composite_bwd forms by a reverse pass (the baked
+ *     renderer stores no samples).  It carries the rounding of E and of the prefix's adds, a few ulps of E, where the true
+ *     suffix of a saturated ray is ~0; dsigma sees that error times delta exp(-sigma delta) / q <= delta.  Corner k of
+ *     the sample's cube receives fp32(w_k x) of each of the 28 channel gradients x, added into d_values (layout of
+ *     values; channels 28 .. 31 receive nothing) with vector fp32 reductions, seven float4 per corner, which flush
+ *     subnormal sums to zero as every fp32 atomic add on sm_90 does.  A sample outside the box, in an inactive brick, or
+ *     with a closed gate and w = 0 adds nothing.  The order of the reductions is the order the hardware runs them in:
+ *     the raw gradients may differ in the last bits between runs (bit-reproducible baked gradients are not offered); the
+ *     tie below keeps the field's copies equal whatever those bits are.  d_values is added into, so chunks of rays
+ *     accumulate; zero it first.
+ *   - Tie (baked_tie).  A lattice point on a brick face is stored once per active brick holding it, and on the box's upper
+ *     faces the clamp of b B + l onto 0 .. res stores it again under several l of one brick.  Along one axis the copies
+ *     of lattice index q are, in ascending brick order: for q < res, (q / 8 - 1, l = 8) when q is a positive multiple of
+ *     8, then (q / 8, q mod 8); for q = res, (nb - 1, l) for l = res - 8 (nb - 1) .. 8.  A point's stored copies are the
+ *     products of its three axes' lists (z outer, then y, then x) whose brick is active.  d_tied[copy] = 0, then += each
+ *     copy's d_values in that order; channels 28 .. 31 are written 0.  Every copy of a point sums the same terms in the
+ *     same order, so every copy gets the same bits; an elementwise optimiser (baked_adam_step_dev, torch.optim.Adam) then
+ *     keeps copies that start bit-equal (as the bake writes them) bit-equal.  Out of place: d_values must not overlap
+ *     d_tied.
+ *   - Adam (baked_adam_step_dev).  adam_step_dev's update of step *step_dev + 1 with grad_scale 1 over values[n_active]
+ *     [729][32]: channel 0 (sigma_raw) at rate lr_schedule(lr_sigma), channels 1 .. 27 at rate lr_schedule(lr_sh), the
+ *     same lr_decay / lr_decay_factor: on each channel group the bits adam_step_dev gives at that rate.  Channels 28 .. 31
+ *     of values, m and v are not touched.  The step counter is not advanced (step_advance does that).
+ * Refused before any launch: an invalid box, a null pointer, n_rays <= 0, ray_stride < 11 with view directions (< 8
+ * without), n_active outside 1 .. the box's bricks (tie; <= 0 for Adam), d_values overlapping d_tied, rates or a
+ * schedule adam_step_dev refuses.  No host synchronisation. */
+int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                  int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                  int32_t white_background, const float* out, const float* g_out, float* d_values,
+                                  void* stream);
+int32_t nerfb200_baked_tie(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks, int64_t n_active,
+                           const float* d_values, float* d_tied, void* stream);
+int32_t nerfb200_baked_adam_step_dev(float* values, const float* g, float* m, float* v, int64_t n_active,
+                                     const int64_t* step_dev, double lr_sigma, double lr_sh, double lr_decay,
+                                     double lr_decay_factor, float beta1, float beta2, float eps, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

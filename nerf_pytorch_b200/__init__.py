@@ -17,7 +17,7 @@ from .graph_step import CapturedTrainStep
 from .occupancy import OccupancyGrid
 from .mesh import Mesh, density_volume, extract_mesh, extract_mesh_from_volume
 from .density import density_gradient
-from .bake import BakedField, bake, render_baked
+from .bake import BakedField, BakedFieldTrainer, bake, render_baked, render_baked_rays
 from . import ops, parallel
 
 __all__ = [
@@ -26,6 +26,7 @@ __all__ = [
     "run_network", "volume_render_radiance_field",
     "run_one_iter_of_nerf", "run_one_iter_of_nerf_from_pose", "set_default_impl", "invalidate", "render_image", "cast_to_image", "cast_to_disparity_image", "cast_to_normal_image", "CachedRayPool", "CachedValidationSet", "SeededRandoms", "CapturedTrainStep", "OccupancyGrid", "Mesh",
     "density_volume", "extract_mesh", "extract_mesh_from_volume", "density_gradient", "BakedField", "bake", "render_baked",
+    "render_baked_rays", "BakedFieldTrainer",
     "ops",
     "parallel",
 ]

@@ -4,8 +4,10 @@ rendered by trilinear interpolation of those values, without the MLP (PlenOctree
 
 The bricks are the sparse meshes' (include/nerfb200.h "sparse meshes"), the values and the renderer are defined in
 include/nerfb200.h "baked fields"; the bake is one fused wgmma kernel (csrc/mlp_tc.cu, bake_tc_kernel) and the renderer
-one warp per ray (csrc/baked.cu).  This file validates arguments, sizes buffers and moves pointers; the bake reads the
-active brick count back once to size its values."""
+one warp per ray (csrc/baked.cu).  A baked field can be fine-tuned against images through that renderer
+(render_baked_rays, BakedFieldTrainer; include/nerfb200.h "baked fields: gradients and fine-tuning").  This file
+validates arguments, sizes buffers and moves pointers; the bake reads the active brick count back once to size its
+values."""
 from __future__ import annotations
 
 import torch
@@ -106,3 +108,149 @@ def render_baked(field: BakedField, height, width, focal_length, tform_cam2world
     values = field.values if field.n_active else field.values.new_zeros(1, 729, 32)
     out = ops.baked_render(field.box(), field.brick_map, values, use_viewdirs, rays, bool(white), stop)
     return out[:, :3].view(height, width, 3), out[:, 3].view(height, width), out[:, 4].view(height, width)
+
+
+def _check_values(field, what):
+    if not isinstance(field, BakedField):
+        raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
+    if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda and field.values.dtype == torch.float32):
+        raise ValueError(f"{what}: field.values must be an fp32 CUDA tensor (there is no CPU or fp16 path)")
+
+
+class _BakedRender(torch.autograd.Function):
+    """Rows (n, 8) of ``ops.baked_render`` (stop 0); the backward is ``baked_render_bwd`` then ``baked_tie``."""
+
+    @staticmethod
+    def forward(ctx, values, field, rays, white):
+        vals = values if values.shape[0] else values.new_zeros(1, 729, 32)
+        out = ops.baked_render(field.box(), field.brick_map, vals.detach(), field.use_viewdirs, rays, white, 0.0)
+        ctx.save_for_backward(values, rays, out)
+        ctx.field, ctx.white = field, white
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        values, rays, out = ctx.saved_tensors
+        if values.shape[0] == 0:
+            return torch.zeros_like(values), None, None, None
+        f = ctx.field
+        box = f.box()
+        d = torch.zeros_like(values)
+        ops.baked_render_bwd(box, f.brick_map, values.detach(), f.use_viewdirs, rays, ctx.white, out, g.contiguous(), d)
+        return ops.baked_tie(box, f.brick_map, f.bricks, d), None, None, None
+
+
+def render_baked_rays(field: BakedField, rays, *, white_background=False, early_stop=None):
+    """(rgb (N, 3), disp (N,), acc (N,), depth (N,)) of the packed ``rays`` (N, 11) with view directions or (N, 8)
+    without (``ops.gen_rays`` / ``ops.gen_rays_posed``) through ``field``.  Differentiable with respect to
+    ``field.values`` when it requires grad: the gradient is the baked renderer's backward summed over every stored copy
+    of each lattice point (include/nerfb200.h "baked fields: gradients and fine-tuning"), so copies that start equal stay
+    equal under any elementwise optimiser.  ``early_stop`` as in ``render_baked``, for renders without a gradient."""
+    _check_values(field, "render_baked_rays")
+    stride = 11 if field.use_viewdirs else 8
+    if not (isinstance(rays, torch.Tensor) and rays.dim() == 2 and rays.shape[1] == stride):
+        raise ValueError(f"render_baked_rays: rays must be (N, {stride}) for a field "
+                         f"{'with' if field.use_viewdirs else 'without'} view directions")
+    grad = field.values.requires_grad and torch.is_grad_enabled()
+    stop = 0.0
+    if early_stop is not None:
+        if grad:
+            raise ValueError("render_baked_rays: early_stop has no gradient; render under torch.no_grad()")
+        stop = float(early_stop)
+        if not 0.0 <= stop < 1.0:
+            raise ValueError(f"render_baked_rays: early_stop must lie in [0, 1), got {early_stop!r}")
+    white = bool(white_background)
+    if grad:
+        out = _BakedRender.apply(field.values, field, rays, white)
+    else:
+        values = field.values.detach() if field.n_active else field.values.new_zeros(1, 729, 32)
+        out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, white, stop)
+    return out[:, :3], out[:, 3], out[:, 4], out[:, 5]
+
+
+# default rates of BakedFieldTrainer: the best held-out PSNR of a sweep on lego A0 at 256^3 (DESIGN §4)
+DEFAULT_LR_SIGMA = 1.0
+DEFAULT_LR_SH = 1e-2
+
+
+class BakedFieldTrainer:
+    """Fine-tunes ``field.values`` in place through the baked renderer against images.  Each ``step()``, with no host
+    synchronisation: draw one image and ``rays_per_step`` distinct pixels from (``seed``, step) (``ops.draw_pixels``),
+    their rays (``gen_rays_posed``: NDC, near / far from ``options.dataset``, view directions as the field) and targets,
+    ``baked_render`` (stop 0, the white background of ``options.nerf.train``), ``mse(rgb, target)``, the backward and the
+    tie into a gradient buffer, and one Adam step (``ops.baked_adam_step_dev``: sigma_raw at ``lr_sigma``, the SH
+    coefficients at ``lr_sh``, both times ``0.1 ** (step / (lr_decay * 1000))`` when ``lr_decay`` is given).
+
+    ``images`` (n, H, W, 3) and ``poses`` (n, 3 | 4, 4) are fp32 on the field's device.  The trainer owns the Adam
+    moments and the step counter (``step_dev``); ``loss`` is the last step's loss, a device tensor.  Memory: four
+    buffers the size of ``field.values`` (gradient, tied gradient, m, v): 3.9 GiB for lego at 256^3 and 22.5 GiB at
+    512^3 over the grid of both lego networks, 2.1 and 11.0 GiB over the fine network's grid (DESIGN §4).
+    ``rays_per_step`` pixels are drawn from one image per step, so it cannot exceed H * W.  The backward's vector reductions run in hardware order, so two runs agree to fp32 rounding, not bitwise;
+    every stored copy of a lattice point stays bit-equal to the others."""
+
+    def __init__(self, field, images, poses, focal, options, *, lr_sigma=DEFAULT_LR_SIGMA, lr_sh=DEFAULT_LR_SH,
+                 lr_decay=None, rays_per_step=4096, seed=0):
+        _check_values(field, "BakedFieldTrainer")
+        if field.n_active == 0:
+            raise ValueError("BakedFieldTrainer: the field has no active brick")
+        dev = field.values.device
+        for name, t in (("images", images), ("poses", poses)):
+            if not (isinstance(t, torch.Tensor) and t.device == dev and t.dtype == torch.float32):
+                raise ValueError(f"BakedFieldTrainer: {name} must be fp32 on the field's device {dev}")
+        if images.dim() != 4 or images.shape[3] != 3 or poses.dim() != 3 or poses.shape[1] not in (3, 4) \
+                or poses.shape[2] != 4 or poses.shape[0] != images.shape[0]:
+            raise ValueError("BakedFieldTrainer: need images (n, H, W, 3) and poses (n, 3 | 4, 4)")
+        use_viewdirs = bool(options.nerf.use_viewdirs)
+        if use_viewdirs != field.use_viewdirs:
+            raise ValueError(f"BakedFieldTrainer: options.nerf.use_viewdirs is {use_viewdirs}, the baked network "
+                             f"{'had' if field.use_viewdirs else 'had no'} view directions")
+        n_img, H, W = images.shape[:3]
+        n = int(rays_per_step)
+        if not 0 < n <= H * W:
+            raise ValueError(f"BakedFieldTrainer: rays_per_step must lie in 1 .. {H * W}, got {rays_per_step}")
+        if not (float(lr_sigma) >= 0 and float(lr_sh) >= 0) or (lr_decay is not None and not float(lr_decay) > 0):
+            raise ValueError("BakedFieldTrainer: need lr_sigma, lr_sh >= 0 and lr_decay None or > 0")
+        if not 0 <= int(seed) < 2 ** 64:
+            raise ValueError("BakedFieldTrainer: seed must be in [0, 2^64)")
+        self.field, self.seed = field, int(seed)
+        self.images, self.poses = images.contiguous(), poses.contiguous()
+        self.focal, self.H, self.W, self.n_images, self.n = float(focal), int(H), int(W), int(n_img), n
+        self.lr_sigma, self.lr_sh, self.lr_decay = float(lr_sigma), float(lr_sh), lr_decay
+        self.ndc = options.dataset.no_ndc is False
+        self.near, self.far = float(options.dataset.near), float(options.dataset.far)
+        self.white = bool(options.nerf.train.white_background)
+        self._box = field.box()
+        v = field.values
+        self.d_values, self.d_tied = torch.zeros_like(v), torch.zeros_like(v)
+        self.m, self.v = torch.zeros_like(v), torch.zeros_like(v)
+        self.step_dev = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._image = torch.empty(1, dtype=torch.int64, device=dev)
+        self._ids = torch.empty(n, dtype=torch.int64, device=dev)
+        self._ws = torch.empty(ops.draw_workspace_bytes(H * W), dtype=torch.uint8, device=dev)
+        self._rays = torch.empty(n, 11 if use_viewdirs else 8, dtype=torch.float32, device=dev)
+        self._target = torch.empty(n, 3, dtype=torch.float32, device=dev)
+        self._out = torch.empty(n, 8, dtype=torch.float32, device=dev)
+        self._g = torch.empty(n, 8, dtype=torch.float32, device=dev)
+        self.loss = torch.zeros((), dtype=torch.float32, device=dev)
+
+    def step(self, n: int = 1):
+        """Runs ``n`` steps; returns the last step's loss (a device tensor)."""
+        f = self.field
+        with torch.no_grad():
+            for _ in range(int(n)):
+                ops.draw_pixels(self.seed, self.step_dev, self.n_images, self.H * self.W, self.n, self._image,
+                                self._ids, self._ws)
+                ops.gen_rays_posed(self.poses, self._image, self.H, self.W, self.focal, self._ids, self.ndc, self.near,
+                                   self.far, f.use_viewdirs, out=self._rays)
+                ops.gather_rows(self.images.view(-1, 3), self.H * self.W, self._image, self._ids, out=self._target)
+                ops.baked_render(self._box, f.brick_map, f.values, f.use_viewdirs, self._rays, self.white, 0.0,
+                                 out=self._out)
+                ops.mse_loss(self._out, None, self._target, self.loss, self._g)
+                self.d_values.zero_()
+                ops.baked_render_bwd(self._box, f.brick_map, f.values, f.use_viewdirs, self._rays, self.white,
+                                     self._out, self._g, self.d_values)
+                ops.baked_tie(self._box, f.brick_map, f.bricks, self.d_values, self.d_tied)
+                ops.baked_adam_step_dev(f.values, self.d_tied, self.m, self.v, self.step_dev, self.lr_sigma,
+                                        self.lr_sh, self.lr_decay)
+                ops.step_advance(self.step_dev)
+        return self.loss

@@ -6,6 +6,11 @@
 //             compositing forms them.  T is the warp's exclusive product scan of q; rgb, acc and depth are summed in
 //             sample order by broadcasting each lane's terms.  A round whose lanes all miss (ballot) adds nothing and
 //             skips its gathers.  No atomics, no shared memory.
+//   backward  the renderer's warp re-marches the ray through the same helpers and scatters each sample's 28 channel
+//             gradients to its cube's 8 corners with vector fp32 reductions (include/nerfb200.h "baked fields: gradients
+//             and fine-tuning"); their order is the hardware's, so raw gradients may differ in the last bits between runs.
+//   tie       one thread per float4: the sum over every stored copy of the value's lattice point, gathered in one fixed
+//             order, so all copies get the same bits.
 #include <cmath>
 
 #include "composite.cuh"
@@ -85,23 +90,18 @@ __device__ __forceinline__ void sh_basis(float x, float y, float z, float Y[kBak
   Y[8] = __fmul_rn(0.5462742152960396f, __fsub_rn(xx, yy));
 }
 
-__global__ void __launch_bounds__(kBakedWarps * 32)
-baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
-                    int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
-                    float stop_t, float* __restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
-  if (r >= n_rays) return;
-  const float* rr = rays + r * ray_stride;
-  float o[3], d[3];
+// a ray's origin, direction and interval: [near, far] and the box's slabs.  An axis with d_c = +-0 keeps x_c = o_c at
+// every sample: it does not restrict the interval when lo_c <= o_c < hi_c and empties the ray otherwise (its slab terms
+// would be 0/0 or inf)
+__device__ __forceinline__ void baked_ray(const BakedBox& B, const float* rr, float o[3], float d[3], float& ta,
+                                          float& tb, float& dnorm, float& dt) {
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     o[c] = rr[c];
     d[c] = rr[3 + c];
   }
-  // the interval: [near, far] and the box's slabs.  An axis with d_c = +-0 keeps x_c = o_c at every sample: it does not
-  // restrict the interval when lo_c <= o_c < hi_c and empties the ray otherwise (its slab terms would be 0/0 or inf)
-  float ta = rr[6], tb = rr[7];
+  ta = rr[6];
+  tb = rr[7];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     if (d[c] == 0.f) {
@@ -112,74 +112,118 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const f
     ta = fmaxf(ta, fminf(t0, t1));
     tb = fminf(tb, fmaxf(t0, t1));
   }
-  const float dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
-  const float dt = __fdiv_rn(__fmul_rn(0.5f, B.h), dnorm);
+  dnorm = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2])));
+  dt = __fdiv_rn(__fmul_rn(0.5f, B.h), dnorm);
+}
+
+// dt > 0 and finite, and sample indices exact in fp32: anything else is an empty ray
+__device__ __forceinline__ bool baked_live(float ta, float tb, float dt) {
+  return ta < tb && dt > 0.f && dt < INFINITY && __fdiv_rn(__fsub_rn(tb, ta), dt) < 16777216.f;
+}
+
+// the sample at depth t (in_ray: t < t_b): its cube's fractions f, its point l inside the brick and the brick's slot,
+// or -1 outside the box, in an inactive brick or past t_b
+__device__ __forceinline__ int baked_lookup(const BakedBox& B, const int* __restrict__ brick_map, const float o[3],
+                                            const float d[3], float t, bool in_ray, float f[3], int l[3]) {
+  int slot = -1;
+  if (in_ray) {
+    bool inside = true;
+    int bi[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float x = __fadd_rn(o[c], __fmul_rn(d[c], t));
+      const float tc = __fmul_rn(__fsub_rn(x, B.g.lo[c]), B.scale[c]);
+      inside = inside && tc >= 0.f && tc < (float)B.g.res[c];
+      const int i = inside ? (int)tc : 0;
+      f[c] = __fsub_rn(tc, (float)i);
+      bi[c] = i >> 3;
+      l[c] = i & 7;
+    }
+    if (inside) slot = brick_map[((int64_t)bi[2] * B.nb[1] + bi[1]) * B.nb[0] + bi[0]];
+  }
+  return slot;
+}
+
+// trilinear weight of corner k = 0 .. 7 of a cube with fractions f
+__device__ __forceinline__ float corner_weight(const float f[3], int k) {
+  const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
+  const float wx = dx ? f[0] : __fsub_rn(1.0f, f[0]), wy = dy ? f[1] : __fsub_rn(1.0f, f[1]);
+  const float wz = dz ? f[2] : __fsub_rn(1.0f, f[2]);
+  return __fmul_rn(__fmul_rn(wx, wy), wz);
+}
+
+// float4 offset of corner k of the cube at brick point l, from the slot's first value
+__device__ __forceinline__ int corner_offset(const int l[3], int k) {
+  const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
+  return (((l[2] + dz) * 9 + l[1] + dy) * 9 + l[0] + dx) * (kBakeCh / 4);
+}
+
+// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0)
+__device__ __forceinline__ void baked_interp(const float* __restrict__ values, int slot, const float f[3],
+                                             const int l[3], float v[kBakedVals]) {
+#pragma unroll
+  for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = 0.f;
+  if (slot >= 0) {
+    const float4* base = reinterpret_cast<const float4*>(values + (int64_t)slot * kBakePts * kBakeCh);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float w = corner_weight(f, k);
+      const float4* pv = base + corner_offset(l, k);
+#pragma unroll
+      for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+        const float4 a = __ldg(pv + c4);
+        v[4 * c4] = fmaf(w, a.x, v[4 * c4]);
+        v[4 * c4 + 1] = fmaf(w, a.y, v[4 * c4 + 1]);
+        v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
+        v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
+      }
+    }
+  }
+}
+
+// rgb = sigmoid(s_c) of the interpolated coefficients v[1 ..]
+__device__ __forceinline__ void baked_colour(int use_viewdirs, const float Y[kBakeSh], const float v[kBakedVals],
+                                             float rgb[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float s = 0.f;
+    if (use_viewdirs) {
+#pragma unroll
+      for (int j = 0; j < kBakeSh; ++j) s = fmaf(Y[j], v[1 + kBakeSh * c + j], s);
+    } else {
+      s = __fmul_rn(Y[0], v[1 + kBakeSh * c]);
+    }
+    rgb[c] = sigmoidf_(s);
+  }
+}
+
+__global__ void __launch_bounds__(kBakedWarps * 32)
+baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
+                    int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
+                    float stop_t, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
+  if (r >= n_rays) return;
+  const float* rr = rays + r * ray_stride;
+  float o[3], d[3], ta, tb, dnorm, dt;
+  baked_ray(B, rr, o, d, ta, tb, dnorm, dt);
   float Y[kBakeSh];
   if (use_viewdirs) sh_basis(rr[8], rr[9], rr[10], Y);
   else Y[0] = 0.28209479177387814f;
 
   float T = 1.0f, ar = 0.f, ag = 0.f, ab = 0.f, aacc = 0.f, adepth = 0.f;
-  // dt > 0 and finite, and sample indices exact in fp32: anything else is an empty ray
-  const bool live = ta < tb && dt > 0.f && dt < INFINITY && __fdiv_rn(__fsub_rn(tb, ta), dt) < 16777216.f;
+  const bool live = baked_live(ta, tb, dt);
   for (int k0 = 0; live; k0 += 32) {
     const float t = __fadd_rn(ta, __fmul_rn(__fadd_rn((float)(k0 + lane), 0.5f), dt));
     if (!(__shfl_sync(0xffffffffu, t, 0) < tb)) break;  // t grows with k: no sample left
-    const bool in_ray = t < tb;
-    int slot = -1;
     float f[3];
     int l[3];
-    if (in_ray) {
-      bool inside = true;
-      int bi[3];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const float x = __fadd_rn(o[c], __fmul_rn(d[c], t));
-        const float tc = __fmul_rn(__fsub_rn(x, B.g.lo[c]), B.scale[c]);
-        inside = inside && tc >= 0.f && tc < (float)B.g.res[c];
-        const int i = inside ? (int)tc : 0;
-        f[c] = __fsub_rn(tc, (float)i);
-        bi[c] = i >> 3;
-        l[c] = i & 7;
-      }
-      if (inside) slot = brick_map[((int64_t)bi[2] * B.nb[1] + bi[1]) * B.nb[0] + bi[0]];
-    }
+    const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
     if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // q = 1 and w = 0 everywhere: T and the sums stay
     float v[kBakedVals];
-#pragma unroll
-    for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = 0.f;
-    if (slot >= 0) {
-      const float4* base = reinterpret_cast<const float4*>(values + (int64_t)slot * kBakePts * kBakeCh);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
-        const float wx = dx ? f[0] : __fsub_rn(1.0f, f[0]), wy = dy ? f[1] : __fsub_rn(1.0f, f[1]);
-        const float wz = dz ? f[2] : __fsub_rn(1.0f, f[2]);
-        const float w = __fmul_rn(__fmul_rn(wx, wy), wz);
-        const float4* pv = base + (((l[2] + dz) * 9 + l[1] + dy) * 9 + l[0] + dx) * (kBakeCh / 4);
-#pragma unroll
-        for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
-          const float4 a = __ldg(pv + c4);
-          v[4 * c4] = fmaf(w, a.x, v[4 * c4]);
-          v[4 * c4 + 1] = fmaf(w, a.y, v[4 * c4 + 1]);
-          v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
-          v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
-        }
-      }
-    }
+    baked_interp(values, slot, f, l, v);
     float rgb[3] = {0.f, 0.f, 0.f};
-    if (slot >= 0) {
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float s = 0.f;
-        if (use_viewdirs) {
-#pragma unroll
-          for (int j = 0; j < kBakeSh; ++j) s = fmaf(Y[j], v[1 + kBakeSh * c + j], s);
-        } else {
-          s = __fmul_rn(Y[0], v[1 + kBakeSh * c]);
-        }
-        rgb[c] = sigmoidf_(s);
-      }
-    }
+    if (slot >= 0) baked_colour(use_viewdirs, Y, v, rgb);
     const SampleTerms st = sample_terms(slot >= 0 ? v[0] : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
     const float Tl = __fmul_rn(T, warp_excl_prod(st.q, lane));
     const float w = __fmul_rn(st.alpha, Tl);
@@ -210,6 +254,169 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const f
     o4[0] = make_float4(ar, ag, ab, disp_out);
     o4[1] = make_float4(aacc, adepth, 0.f, 0.f);
   }
+}
+
+// The gradient of baked_render_kernel (stop_transmittance 0) with respect to the values, added into d_values.  The warp
+// re-marches the ray as the forward does; per sample v = g_rgb . c + G_acc + G_depth t, dL/dalpha = T v - S / q with
+// S = E - (inclusive prefix of w v in sample order) and E = sum w v formed from the forward's totals; the 28 channel
+// gradients go to the cube's 8 corners with vector reductions (seven float4 per corner).
+__global__ void __launch_bounds__(kBakedWarps * 32)
+baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
+                        int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
+                        const float* __restrict__ out, const float* __restrict__ g_out, float* __restrict__ d_values) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
+  if (r >= n_rays) return;
+  const float* rr = rays + r * ray_stride;
+  float o[3], d[3], ta, tb, dnorm, dt;
+  baked_ray(B, rr, o, d, ta, tb, dnorm, dt);
+  if (!baked_live(ta, tb, dt)) return;  // no sample: nothing to add
+  float Y[kBakeSh];
+#pragma unroll
+  for (int j = 0; j < kBakeSh; ++j) Y[j] = 0.f;  // without view directions only coefficient 0 is read
+  if (use_viewdirs) sh_basis(rr[8], rr[9], rr[10], Y);
+  else Y[0] = 0.28209479177387814f;
+
+  const float4 o0 = reinterpret_cast<const float4*>(out + r * 8)[0], o1 = reinterpret_cast<const float4*>(out + r * 8)[1];
+  const float4 g0 = reinterpret_cast<const float4*>(g_out + r * 8)[0];
+  const float4 g1 = reinterpret_cast<const float4*>(g_out + r * 8)[1];
+  const float aacc = o1.x, adepth = o1.y;
+  float G_acc = g1.x, G_depth = g1.y;
+  composite_upstream(g0, white_bkgd, adepth, aacc, G_acc, G_depth);
+  // E = sum_i w_i v_i = g_rgb . rgb + G_acc acc + G_depth depth, rgb without the white background
+  float er = o0.x, eg = o0.y, eb = o0.z;
+  if (white_bkgd) {
+    const float bg = __fsub_rn(1.0f, aacc);
+    er = __fsub_rn(er, bg);
+    eg = __fsub_rn(eg, bg);
+    eb = __fsub_rn(eb, bg);
+  }
+  const float E = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(g0.x, er), __fmul_rn(g0.y, eg)), __fmul_rn(g0.z, eb)),
+                                      __fmul_rn(G_acc, aacc)), __fmul_rn(G_depth, adepth));
+
+  float T = 1.0f, prefix = 0.f;
+  for (int k0 = 0;; k0 += 32) {
+    const float t = __fadd_rn(ta, __fmul_rn(__fadd_rn((float)(k0 + lane), 0.5f), dt));
+    if (!(__shfl_sync(0xffffffffu, t, 0) < tb)) break;
+    float f[3];
+    int l[3];
+    const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
+    if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // as the forward: T and the prefix stay
+    float v[kBakedVals];
+    baked_interp(values, slot, f, l, v);
+    float rgb[3] = {0.f, 0.f, 0.f};
+    if (slot >= 0) baked_colour(use_viewdirs, Y, v, rgb);
+    const SampleTerms st = sample_terms(slot >= 0 ? v[0] : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
+    const float Tl = __fmul_rn(T, warp_excl_prod(st.q, lane));
+    const float w = __fmul_rn(st.alpha, Tl);
+    const float vi = __fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(g0.x, rgb[0]), __fmul_rn(g0.y, rgb[1])),
+                                                   __fmul_rn(g0.z, rgb[2])), G_acc), __fmul_rn(G_depth, t));
+    const float wv = __fmul_rn(w, vi);
+    float incl = 0.f;
+#pragma unroll 4
+    for (int i = 0; i < 32; ++i) {  // in sample order
+      prefix = __fadd_rn(prefix, __shfl_sync(0xffffffffu, wv, i));
+      if (i == lane) incl = prefix;
+    }
+    T = __shfl_sync(0xffffffffu, __fmul_rn(Tl, st.q), 31);
+    if (slot < 0 || (!st.gate && w == 0.f)) continue;  // adds nothing
+    const float dalpha = __fsub_rn(__fmul_rn(Tl, vi), __fdiv_rn(__fsub_rn(E, incl), st.q));
+    const float dsigma = st.gate ? __fmul_rn(__fmul_rn(dalpha, st.delta), st.sigma_delta_exp) : 0.f;
+    float ds[3];
+    const float gc[3] = {g0.x, g0.y, g0.z};
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      ds[c] = __fmul_rn(__fmul_rn(__fmul_rn(w, gc[c]), rgb[c]), __fsub_rn(1.0f, rgb[c]));
+    float4* base = reinterpret_cast<float4*>(d_values + (int64_t)slot * kBakePts * kBakeCh);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float wk = corner_weight(f, k);
+      float4* pv = base + corner_offset(l, k);
+      float gk[kBakedVals];
+      gk[0] = __fmul_rn(wk, dsigma);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+#pragma unroll
+        for (int j = 0; j < kBakeSh; ++j) gk[1 + kBakeSh * c + j] = __fmul_rn(wk, __fmul_rn(ds[c], Y[j]));
+#pragma unroll
+      for (int c4 = 0; c4 < kBakedVals / 4; ++c4)
+        atomicAdd(pv + c4, make_float4(gk[4 * c4], gk[4 * c4 + 1], gk[4 * c4 + 2], gk[4 * c4 + 3]));
+    }
+  }
+}
+
+// the copies of lattice index q along one axis (res cubes, nb bricks): (brick, point) pairs in ascending brick order.
+// q < res: (q / 8 - 1, 8) when q is a positive multiple of 8, then (q / 8, q % 8); q = res: (nb - 1, l) for l =
+// res - 8 (nb - 1) .. 8 (the upper face's point and its clamped repeats)
+struct AxisCopies {
+  int n, b0, l0;  // n copies; entry e is (b0, l0 + e) on the upper face, else (b0 + e, l0 - 8 e)
+  bool face;
+};
+
+__device__ __forceinline__ AxisCopies axis_copies(int q, int res, int nb) {
+  if (q == res) return AxisCopies{8 - (res - kBakeBrick * (nb - 1)) + 1, nb - 1, res - kBakeBrick * (nb - 1), true};
+  if (q > 0 && (q & 7) == 0) return AxisCopies{2, (q >> 3) - 1, kBakeBrick, false};
+  return AxisCopies{1, q >> 3, q & 7, false};
+}
+
+__device__ __forceinline__ void axis_entry(const AxisCopies& a, int e, int& b, int& l) {
+  b = a.face ? a.b0 : a.b0 + e;
+  l = a.face ? a.l0 + e : a.l0 - kBakeBrick * e;
+}
+
+// d_tied[copy] = the sum over every stored copy of the copy's lattice point of d_values, in one fixed order (z copies
+// outer, then y, then x, each ascending), so every copy of a point gets the same bits.  One thread per float4.
+__global__ void baked_tie_kernel(const BakedBox B, const int* __restrict__ brick_map, const int* __restrict__ bricks,
+                                 int64_t n_active, const float4* __restrict__ d_values, float4* __restrict__ d_tied) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= n_active * kBakePts * (kBakeCh / 4)) return;
+  const int c4 = (int)(e & 7);
+  if (c4 >= kBakedVals / 4) {  // channels 28 .. 31
+    d_tied[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const int64_t sp = e >> 3;
+  const int64_t slot = sp / kBakePts;
+  const int p = (int)(sp - slot * kBakePts);
+  const int brick = bricks[slot];
+  const int bc[3] = {brick % B.nb[0], (brick / B.nb[0]) % B.nb[1], brick / (B.nb[0] * B.nb[1])};
+  const int lc[3] = {p % 9, (p / 9) % 9, p / 81};
+  AxisCopies a[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) a[c] = axis_copies(min(bc[c] * kBakeBrick + lc[c], B.g.res[c]), B.g.res[c], B.nb[c]);
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int ez = 0; ez < a[2].n; ++ez) {
+    int bz, lz;
+    axis_entry(a[2], ez, bz, lz);
+    for (int ey = 0; ey < a[1].n; ++ey) {
+      int by, ly;
+      axis_entry(a[1], ey, by, ly);
+      for (int ex = 0; ex < a[0].n; ++ex) {
+        int bx, lx;
+        axis_entry(a[0], ex, bx, lx);
+        const int cs = brick_map[((int64_t)bz * B.nb[1] + by) * B.nb[0] + bx];
+        if (cs < 0) continue;
+        const float4 g = d_values[((int64_t)cs * kBakePts + (lz * 9 + ly) * 9 + lx) * (kBakeCh / 4) + c4];
+        s.x = __fadd_rn(s.x, g.x);
+        s.y = __fadd_rn(s.y, g.y);
+        s.z = __fadd_rn(s.z, g.z);
+        s.w = __fadd_rn(s.w, g.w);
+      }
+    }
+  }
+  d_tied[e] = s;
+}
+
+BakedBox baked_box(const nerfb200_grid_t* box) {
+  BakedBox B;
+  B.g = *box;
+  B.h = INFINITY;
+  for (int c = 0; c < 3; ++c) {
+    B.nb[c] = (box->res[c] + kBakeBrick - 1) / kBakeBrick;
+    B.scale[c] = (float)box->res[c] / (box->hi[c] - box->lo[c]);
+    B.h = std::fmin(B.h, (box->hi[c] - box->lo[c]) / (float)box->res[c]);
+  }
+  return B;
 }
 
 }  // namespace
@@ -245,20 +452,54 @@ int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_m
     set_error("baked_render: stop_transmittance must lie in [0, 1), got %g", (double)stop_transmittance);
     return NERFB200_ERR_INVALID;
   }
-  BakedBox B;
-  B.g = *box;
-  B.h = INFINITY;
-  for (int c = 0; c < 3; ++c) {
-    B.nb[c] = (box->res[c] + kBakeBrick - 1) / kBakeBrick;
-    B.scale[c] = (float)box->res[c] / (box->hi[c] - box->lo[c]);
-    B.h = std::fmin(B.h, (box->hi[c] - box->lo[c]) / (float)box->res[c]);
-  }
+  const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_render_kernel<<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0,
       stop_transmittance, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "baked_render launch");
+}
+
+int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                  int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                  int32_t white_background, const float* out, const float* g_out, float* d_values,
+                                  void* stream) {
+  if (int rc = check_grid(box, "baked_render_bwd")) return rc;
+  if (!brick_map || !values || !rays || !out || !g_out || !d_values || n_rays <= 0 ||
+      ray_stride < (use_viewdirs ? 11 : 8)) {
+    set_error("baked_render_bwd: null pointer, n_rays <= 0 or ray_stride %d too short", ray_stride);
+    return NERFB200_ERR_INVALID;
+  }
+  const BakedBox B = baked_box(box);
+  const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
+  baked_render_bwd_kernel<<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0, out, g_out,
+      d_values);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_render_bwd launch");
+}
+
+int32_t nerfb200_baked_tie(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks, int64_t n_active,
+                           const float* d_values, float* d_tied, void* stream) {
+  if (int rc = check_grid(box, "baked_tie")) return rc;
+  const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
+  if (!brick_map || !bricks || !d_values || !d_tied || n_active <= 0 || n_active > n_bricks) {
+    set_error("baked_tie: null pointer or n_active %lld outside 1 .. %lld", (long long)n_active, (long long)n_bricks);
+    return NERFB200_ERR_INVALID;
+  }
+  const int64_t n4 = n_active * kBakePts * (kBakeCh / 4);
+  const float* a_end = d_values + 4 * n4;
+  const float* b_end = d_tied + 4 * n4;
+  if (d_values < b_end && d_tied < a_end) {
+    set_error("baked_tie: d_values and d_tied overlap (the tie is out of place)");
+    return NERFB200_ERR_INVALID;
+  }
+  const BakedBox B = baked_box(box);
+  baked_tie_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      B, brick_map, bricks, n_active, reinterpret_cast<const float4*>(d_values), reinterpret_cast<float4*>(d_tied));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_tie launch");
 }
 
 }  // extern "C"

@@ -178,6 +178,9 @@ int launch_gen_rays_posed(const float* poses, int pose_rows, const int64_t* imag
 int launch_lr_schedule(const int64_t* done, int64_t n, const LrSchedule& sch, float* out, cudaStream_t s);
 int launch_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* done, const LrSchedule& sch,
                     float b1, float b2, float eps, float grad_scale, cudaStream_t s);
+// adam_dev over baked values[n / 32][32]: channel 0 at the rate of `sigma`, 1 .. 27 at `sh`, 28 .. 31 untouched
+int launch_baked_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* done,
+                          const LrSchedule& sigma, const LrSchedule& sh, float b1, float b2, float eps, cudaStream_t s);
 
 // The MLP kernel families.  Each file's predicate says whether its kernels take a plan (NERFB200_OK, else the reason
 // in the last error, prefixed with `what`); api.cu's check_impl maps an impl code to them, and its mlp_forward /

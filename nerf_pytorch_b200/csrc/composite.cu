@@ -137,15 +137,7 @@ composite_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ z,
 
   // upstream coefficients: L = sum_i w_i * v_i,  v_i = g_rgb . c_i + G_acc + G_depth * z_i (+ g_w_i)
   float G_acc = g_acc_in, G_depth = kSampleGrads ? g_out[r * 8 + 5] : 0.f;
-  if (white_bkgd) G_acc -= (g0.x + g0.y + g0.z);  // rgb_map += 1 - acc  (:50-51)
-  if (g0.w != 0.f) {                              // disp = 1 / max(1e-10, depth / acc)  (:48)
-    const float ratio = adepth / aacc;
-    if (ratio > 1e-10f || ratio != ratio) {
-      const float disp = 1.0f / ratio;
-      G_depth += g0.w * (-disp * disp) / aacc;
-      G_acc += g0.w * (disp * disp) * adepth / (aacc * aacc);
-    }
-  }
+  composite_upstream(g0, white_bkgd, adepth, aacc, G_acc, G_depth);
 
   // pass 2: v_i and the suffix sums S_i = sum_{j>i} v_j w_j
   float local = 0.f;

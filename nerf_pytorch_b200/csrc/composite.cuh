@@ -31,6 +31,22 @@ __device__ __forceinline__ SampleTerms sample_terms(float raw_sigma, float noise
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// the upstream coefficients of a ray's samples, L = sum_i w_i v_i with v_i = g_rgb . c_i + G_acc + G_depth z_i: adds to
+// G_acc and G_depth the terms of the white background (rgb_map += 1 - acc, :50-51) and of disp = 1 / max(1e-10,
+// depth / acc) (:48), given the ray's upstream rgb / disp gradient g0 and its totals depth and acc
+__device__ __forceinline__ void composite_upstream(const float4& g0, int white_bkgd, float adepth, float aacc,
+                                                   float& G_acc, float& G_depth) {
+  if (white_bkgd) G_acc -= (g0.x + g0.y + g0.z);
+  if (g0.w != 0.f) {
+    const float ratio = adepth / aacc;
+    if (ratio > 1e-10f || ratio != ratio) {
+      const float disp = 1.0f / ratio;
+      G_depth += g0.w * (-disp * disp) / aacc;
+      G_acc += g0.w * (disp * disp) * adepth / (aacc * aacc);
+    }
+  }
+}
+
 // exclusive multiplicative scan across lanes
 __device__ __forceinline__ float warp_excl_prod(float v, int lane) {
   float inc = v;

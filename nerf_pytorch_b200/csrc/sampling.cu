@@ -333,18 +333,23 @@ int launch_pack(const Plan& p, const float* flat, float* blob, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------
 // fused Adam over a flat vector (torch.optim.Adam, amsgrad off, weight_decay 0)
 // ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ void adam_element(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                             float* __restrict__ v, int64_t i, float lr_over_bc1, float inv_sqrt_bc2,
+                                             float b1, float b2, float eps, float grad_scale) {
+  const float gi = g[i] * grad_scale;
+  const float mi = m[i] + (gi - m[i]) * (1.f - b1);         // exp_avg.lerp_(grad, 1 - beta1)
+  const float vi = v[i] * b2 + (1.f - b2) * gi * gi;        // exp_avg_sq.mul_(b2).addcmul_(g, g, 1 - b2)
+  m[i] = mi;
+  v[i] = vi;
+  const float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;       // sqrt(v) / sqrt(bc2) + eps
+  p[i] = p[i] - lr_over_bc1 * (mi / denom);                 // addcdiv_(m, denom, value=-lr/bc1)
+}
+
 __device__ __forceinline__ void adam_update(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
                                             float* __restrict__ v, int64_t n, float lr_over_bc1, float inv_sqrt_bc2,
                                             float b1, float b2, float eps, float grad_scale) {
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const float gi = g[i] * grad_scale;
-    const float mi = m[i] + (gi - m[i]) * (1.f - b1);         // exp_avg.lerp_(grad, 1 - beta1)
-    const float vi = v[i] * b2 + (1.f - b2) * gi * gi;        // exp_avg_sq.mul_(b2).addcmul_(g, g, 1 - b2)
-    m[i] = mi;
-    v[i] = vi;
-    const float denom = sqrtf(vi) * inv_sqrt_bc2 + eps;       // sqrt(v) / sqrt(bc2) + eps
-    p[i] = p[i] - lr_over_bc1 * (mi / denom);                 // addcdiv_(m, denom, value=-lr/bc1)
-  }
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    adam_element(p, g, m, v, i, lr_over_bc1, inv_sqrt_bc2, b1, b2, eps, grad_scale);
 }
 
 __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
@@ -412,6 +417,40 @@ int launch_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, con
   adam_dev_kernel<<<(unsigned)blocks, threads, 0, s>>>(p, g, m, v, n, done, sch, b1, b2, eps, grad_scale);
   count_launch();
   return check_cuda(cudaGetLastError(), "adam_dev launch");
+}
+
+// adam_dev_kernel over baked values (rows of kBakeCh floats): channel 0 (sigma_raw) at the rate of `sigma`, channels
+// 1 .. 27 (SH coefficients) at the rate of `sh`, channels 28 .. 31 untouched.  grad_scale is a kernel argument (1) as
+// in adam_dev_kernel, so the compiler forms the update from the same operations and the bits match adam_step_dev's.
+__global__ void baked_adam_dev_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
+                                      float* __restrict__ v, int64_t n, const int64_t* __restrict__ done,
+                                      LrSchedule sigma, LrSchedule sh, float b1, float b2, float eps, float grad_scale) {
+  __shared__ float scal[3];
+  if (threadIdx.x == 0) {
+    const int64_t d = *done;
+    const double step = (double)(d + 1);
+    const double bc1 = 1.0 - pow((double)b1, step);
+    const double bc2 = 1.0 - pow((double)b2, step);
+    scal[0] = (float)(scheduled_lr(d, sigma) / bc1);
+    scal[1] = (float)(scheduled_lr(d, sh) / bc1);
+    scal[2] = (float)(1.0 / sqrt(bc2));
+  }
+  __syncthreads();
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int ch = (int)(i & (kBakeCh - 1));
+    if (ch >= 1 + 3 * kBakeSh) continue;
+    adam_element(p, g, m, v, i, ch == 0 ? scal[0] : scal[1], scal[2], b1, b2, eps, grad_scale);
+  }
+}
+
+int launch_baked_adam_dev(float* p, const float* g, float* m, float* v, int64_t n, const int64_t* done,
+                          const LrSchedule& sigma, const LrSchedule& sh, float b1, float b2, float eps, cudaStream_t s) {
+  const int threads = 256;
+  int64_t blocks = (n + threads - 1) / threads;
+  if (blocks > device_sms() * 8) blocks = device_sms() * 8;
+  baked_adam_dev_kernel<<<(unsigned)blocks, threads, 0, s>>>(p, g, m, v, n, done, sigma, sh, b1, b2, eps, 1.f);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_adam_dev launch");
 }
 
 }  // namespace nerfb200

@@ -366,6 +366,22 @@ int32_t nerfb200_adam_step_dev(float* p, const float* g, float* m, float* v, int
                          grad_scale, static_cast<cudaStream_t>(stream));
 }
 
+int32_t nerfb200_baked_adam_step_dev(float* values, const float* g, float* m, float* v, int64_t n_active,
+                                     const int64_t* step_dev, double lr_sigma, double lr_sh, double lr_decay,
+                                     double lr_decay_factor, float beta1, float beta2, float eps, void* stream) {
+  if (check_schedule(lr_sigma, lr_decay, lr_decay_factor, "baked_adam_step_dev") ||
+      check_schedule(lr_sh, lr_decay, lr_decay_factor, "baked_adam_step_dev"))
+    return NERFB200_ERR_INVALID;
+  if (!values || !g || !m || !v || !step_dev || n_active <= 0) {
+    set_error("baked_adam_step_dev: null pointer or n_active <= 0");
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_baked_adam_dev(values, g, m, v, n_active * kBakePts * kBakeCh, step_dev,
+                               LrSchedule{lr_sigma, lr_decay, lr_decay_factor},
+                               LrSchedule{lr_sh, lr_decay, lr_decay_factor}, beta1, beta2, eps,
+                               static_cast<cudaStream_t>(stream));
+}
+
 int32_t nerfb200_step_advance(int64_t* step_dev, void* stream) {
   if (!step_dev) {
     set_error("step_advance: null pointer");

@@ -1050,3 +1050,33 @@ def baked_render(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_b
                                                  _ptr(rays), rays.shape[1], n, int(bool(white_background)),
                                                  float(stop_transmittance), _ptr(out), _stream()), "baked_render")
     return out
+
+
+def baked_render_bwd(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool, out, g_out,
+                     d_values):
+    """Adds into ``d_values`` (the layout of ``values``) the gradient of ``baked_render`` (stop 0) whose rows were
+    ``out``, given upstream gradient rows ``g_out`` (n, 8).  Untied: see ``baked_tie``."""
+    _lib.check(_lib.load().nerfb200_baked_render_bwd(C.byref(box), _ptr(brick_map), _ptr(values),
+                                                     int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], rays.shape[0],
+                                                     int(bool(white_background)), _ptr(out), _ptr(g_out),
+                                                     _ptr(d_values), _stream()), "baked_render_bwd")
+    return d_values
+
+
+def baked_tie(box: Grid, brick_map, bricks, d_values, d_tied=None):
+    """Every stored copy of a lattice point receives the sum over all its copies of ``d_values``: (n_active, 729, 32)."""
+    if d_tied is None:
+        d_tied = torch.empty_like(d_values)
+    _lib.check(_lib.load().nerfb200_baked_tie(C.byref(box), _ptr(brick_map), _ptr(bricks), d_values.shape[0],
+                                              _ptr(d_values), _ptr(d_tied), _stream()), "baked_tie")
+    return d_tied
+
+
+def baked_adam_step_dev(values, g, m, v, step_dev, lr_sigma, lr_sh, lr_decay=None, lr_decay_factor=0.1, beta1=0.9,
+                        beta2=0.999, eps=1e-8):
+    """``adam_step_dev`` over baked values: sigma_raw at ``lr_sigma``, the SH coefficients at ``lr_sh``."""
+    _, decay, factor = _schedule(0.0, lr_decay, lr_decay_factor)
+    _lib.check(_lib.load().nerfb200_baked_adam_step_dev(_ptr(values), _ptr(g), _ptr(m), _ptr(v), values.shape[0],
+                                                        _ptr(step_dev), float(lr_sigma), float(lr_sh), decay, factor,
+                                                        float(beta1), float(beta2), float(eps), _stream()),
+               "baked_adam_step_dev")
