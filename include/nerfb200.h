@@ -685,6 +685,45 @@ int32_t nerfb200_baked_adam_step_dev(float* values, const float* g, float* m, fl
                                      const int64_t* step_dev, double lr_sigma, double lr_sh, double lr_decay,
                                      double lr_decay_factor, float beta1, float beta2, float eps, void* stream);
 
+/* ---- baked fields: pruning ------------------------------------------------------------------------------------------
+ * Which active bricks a baked field's renders use, so that the others can be dropped (as PlenOctrees prunes voxels
+ * whose largest rendering weight over the training rays is small).  Dropping bricks is host-side compaction of the
+ * field (brick_map, bricks, values); the library supplies each brick's peak weight over a set of rays.
+ *   - Peak weights (baked_max_weights).  One warp per ray re-marches the ray exactly as baked_render does with
+ *     stop_transmittance 0: the same interval, t_k, lookup, alpha, q and T in rounds of 32 with the same Hillis-Steele
+ *     scan.  For every sample whose slot is >= 0, max_w[slot] = max(max_w[slot], w), w = alpha T the bits the renderer
+ *     forms for that sample; a NaN w is recorded as +inf, so that brick survives any finite threshold.  w depends on
+ *     sigma_raw alone, so only channel 0 is interpolated: the 8 corners in the same order through the same fmaf chain as
+ *     the renderer's interp, which gives the renderer's sigma_raw bits while reading 4 B of each 128-B point; no colour
+ *     or SH is formed.  A ray is marched to t_b (no stop at T = 0: a NaN later in the ray must still be seen).
+ *     max_w is fp32[n_active] and max-accumulated: zero it once and pass it to every chunk of rays.  A max is exact, so
+ *     the result is the same bits for every chunking, ray order and run.
+ *   - Transparent bricks.  A brick every stored sigma_raw of which is <= 0 (-0 included) and whose channels 0 .. 27 are
+ *     all finite can be dropped (its brick_map entry set to -1) leaving every render bit for bit the same, from any ray,
+ *     with or without a white background or early stopping.  Every sample in such a brick interpolates sigma_raw <= 0
+ *     (non-negative weights times non-positive values), so sigma = 0, alpha = +0 and q = (1 - 0) + 1e-10 = 1 exactly
+ *     (1e-10 is below half an ulp of 1): T passes unchanged, w = +0, and w rgb and w t are +-0, which leave every sum
+ *     (each starts at +0) unchanged.  A dropped sample is a miss, which has the same alpha, q and w, and a round whose
+ *     lanes all miss (skipped by the renderer) is equivalent to one in which they hit such a brick.
+ *   - Unseen bricks.  A brick with max_w == 0 over a set of rays can be dropped leaving the renders of those rays bit
+ *     for bit the same (with or without early stopping: the march agrees at every round).  A dropped sample had w = +0,
+ *     so either alpha = 0 (q = 1 as for a miss) or T = 0 before it; T is a product of factors q in [1e-10, 1], so once
+ *     it is 0 it stays 0 when the dropped q becomes 1, and every later sample keeps w = +0.  The one exception is a
+ *     product that rounds to 0 exactly at the fp32 underflow boundary: alpha > 0 and T > 0 with alpha T (or a partial
+ *     product of the scan) below 2^-150, so 0 under one association and not under the other.  T is then subnormal and
+ *     the later weights that can differ are below 2^-126.
+ *   - Non-finite fields.  Both statements hold for finite fields only.  A NaN or infinite coefficient in a brick whose
+ *     samples have w = 0 still makes the render NaN (0 NaN and 0 inf are NaN), and dropping that brick changes it; the
+ *     transparency rule therefore asks that channels 0 .. 27 be finite, and a NaN w keeps its brick through +inf.
+ * baked_max_weights: box, brick_map, values, rays and ray_stride as baked_render; max_w[n_active] fp32.
+ * Refused before any launch: an invalid box, a null pointer, n_rays <= 0, ray_stride < 11 with view directions (< 8
+ * without).  No host synchronisation; the only atomics are integer atomicMax on the bits of non-negative floats (which
+ * order as unsigned integers): per round the lanes are grouped by slot (__match_any_sync), each group's largest weight
+ * found by __reduce_max_sync, and one lane per group issues the atomic; w = 0 is skipped, as max_w starts at 0. */
+int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                   int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                   float* max_w, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

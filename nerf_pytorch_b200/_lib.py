@@ -164,6 +164,7 @@ SIGNATURES = {
     "nerfb200_baked_render_bwd": (I32, [GP, P, P, I32, P, I32, I64, I32, P, P, P, P]),
     "nerfb200_baked_tie": (I32, [GP, P, P, I64, P, P, P]),
     "nerfb200_baked_adam_step_dev": (I32, [P, P, P, P, I64, P, F64, F64, F64, F64, F32, F32, F32, P]),
+    "nerfb200_baked_max_weights": (I32, [GP, P, P, I32, P, I32, I64, P, P]),
 }
 
 _lib = None

@@ -5,9 +5,10 @@ rendered by trilinear interpolation of those values, without the MLP (PlenOctree
 The bricks are the sparse meshes' (include/nerfb200.h "sparse meshes"), the values and the renderer are defined in
 include/nerfb200.h "baked fields"; the bake is one fused wgmma kernel (csrc/mlp_tc.cu, bake_tc_kernel) and the renderer
 one warp per ray (csrc/baked.cu).  A baked field can be fine-tuned against images through that renderer
-(render_baked_rays, BakedFieldTrainer; include/nerfb200.h "baked fields: gradients and fine-tuning").  This file
-validates arguments, sizes buffers and moves pointers; the bake reads the active brick count back once to size its
-values."""
+(render_baked_rays, BakedFieldTrainer; include/nerfb200.h "baked fields: gradients and fine-tuning"), and pruned to the
+bricks its renders use (baked_transparent_bricks, baked_brick_weights, prune_baked, BakedFieldTrainer.prune;
+include/nerfb200.h "baked fields: pruning").  This file validates arguments, sizes buffers and moves pointers; the bake
+reads the active brick count back once to size its values."""
 from __future__ import annotations
 
 import torch
@@ -92,22 +93,31 @@ def render_baked(field: BakedField, height, width, focal_length, tform_cam2world
         raise ValueError(f"render_baked: field must be an nb.BakedField, got {type(field).__name__}")
     if not field.values.is_cuda:
         raise NotImplementedError("nerfb200: the baked field must be on a CUDA device (there is no CPU path)")
-    use_viewdirs = bool(options.nerf.use_viewdirs)
-    if use_viewdirs != field.use_viewdirs:
-        raise ValueError(f"render_baked: options.nerf.use_viewdirs is {use_viewdirs}, the baked network "
-                         f"{'had' if field.use_viewdirs else 'had no'} view directions")
+    _check_viewdirs(field, options, "render_baked")
     stop = 0.0
     if early_stop is not None:
         stop = float(early_stop)
         if not 0.0 <= stop < 1.0:
             raise ValueError(f"render_baked: early_stop must lie in [0, 1), got {early_stop!r}")
     white = getattr(options.nerf, "train" if train_utils.COMPAT_MODE_QUIRK else mode).white_background
-    dev = field.values.device
-    rays = ops.gen_rays(tform_cam2world, height, width, focal_length, None, dev, ndc=options.dataset.no_ndc is False,
-                        near=options.dataset.near, far=options.dataset.far, use_viewdirs=use_viewdirs)
+    rays = _pose_rays(field, height, width, focal_length, tform_cam2world, options)
     values = field.values if field.n_active else field.values.new_zeros(1, 729, 32)
-    out = ops.baked_render(field.box(), field.brick_map, values, use_viewdirs, rays, bool(white), stop)
+    out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white), stop)
     return out[:, :3].view(height, width, 3), out[:, 3].view(height, width), out[:, 4].view(height, width)
+
+
+def _check_viewdirs(field, options, what):
+    use_viewdirs = bool(options.nerf.use_viewdirs)
+    if use_viewdirs != field.use_viewdirs:
+        raise ValueError(f"{what}: options.nerf.use_viewdirs is {use_viewdirs}, the baked network "
+                         f"{'had' if field.use_viewdirs else 'had no'} view directions")
+
+
+def _pose_rays(field, height, width, focal_length, tform_cam2world, options):
+    """``render_image``'s rays of every pixel of one pose on the field's device (``_check_viewdirs`` first)."""
+    return ops.gen_rays(tform_cam2world, height, width, focal_length, None, field.values.device,
+                        ndc=options.dataset.no_ndc is False, near=options.dataset.near, far=options.dataset.far,
+                        use_viewdirs=field.use_viewdirs)
 
 
 def _check_values(field, what):
@@ -254,3 +264,124 @@ class BakedFieldTrainer:
                                         self.lr_sh, self.lr_decay)
                 ops.step_advance(self.step_dev)
         return self.loss
+
+    def prune(self, keep) -> None:
+        """Compacts the trainer's field in place to the bricks where ``keep`` (bool[n_active] on the field's device) is
+        true, as ``prune_baked`` does: the ``BakedField`` passed to the constructor then holds the pruned ``brick_map``,
+        ``bricks`` and ``values``, the Adam moments ``m`` and ``v`` go through the same row gather, and the gradient
+        buffers are reallocated at the new size (the old ones are freed first).  ``step_dev``, the seed, the rates and
+        the schedule carry on.  A pruned brick never comes back: its samples become misses, and the tie no longer carries
+        gradient into it.  Keeping no brick raises ValueError, as the constructor does.  Reads the kept count back once."""
+        f = self.field
+        _check_keep(f, keep, "BakedFieldTrainer.prune")
+        idx = torch.nonzero(keep).reshape(-1)
+        if idx.numel() == 0:
+            raise ValueError("BakedFieldTrainer.prune: keep selects no brick (the field would have no active brick)")
+        self.d_values = self.d_tied = None
+        with torch.no_grad():
+            f.brick_map, f.bricks, f.values = _pruned(f, idx)
+            self.m, self.v = self.m.index_select(0, idx), self.v.index_select(0, idx)
+        self.d_values, self.d_tied = torch.zeros_like(f.values), torch.zeros_like(f.values)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# pruning (include/nerfb200.h "baked fields: pruning")
+# ------------------------------------------------------------------------------------------------------------------------
+def _check_keep(field, keep, what):
+    if not isinstance(field, BakedField):
+        raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
+    if not (isinstance(keep, torch.Tensor) and keep.dtype == torch.bool and keep.shape == (field.n_active,)
+            and keep.device == field.values.device):
+        raise ValueError(f"{what}: keep must be a bool tensor of shape ({field.n_active},) on {field.values.device}")
+
+
+def _pruned(field, idx):
+    """(brick_map, bricks, values) of ``field`` restricted to the slots ``idx`` (ascending int64)."""
+    bricks = field.bricks.index_select(0, idx)
+    brick_map = torch.full_like(field.brick_map, -1)
+    brick_map[bricks.long()] = torch.arange(idx.numel(), dtype=brick_map.dtype, device=brick_map.device)
+    return brick_map, bricks, field.values.detach().index_select(0, idx)
+
+
+def prune_baked(field: BakedField, keep) -> BakedField:
+    """A new ``BakedField`` holding the bricks of ``field`` where ``keep`` (bool[n_active] on the field's device) is
+    true.  Slots stay in ascending order (so ``bricks`` stays sorted), ``brick_map`` is rebuilt with -1 for the dropped
+    bricks, and the kept rows of ``values`` are copied unchanged; ``field`` is not touched.  The copy needs the kept
+    values' size again while both fields are alive.  Plain torch indexing: it works on a CPU field too.  Keeping no brick
+    gives a field with ``n_active == 0``, which ``render_baked`` renders as empty.
+
+    Lossless criteria (include/nerfb200.h "baked fields: pruning"): ``~baked_transparent_bricks(field)`` leaves every
+    render the same bits; ``baked_brick_weights(...) > 0`` leaves the renders of the rays it was measured over the same
+    bits."""
+    _check_keep(field, keep, "prune_baked")
+    with torch.no_grad():
+        brick_map, bricks, values = _pruned(field, torch.nonzero(keep).reshape(-1))
+    return BakedField(field.bounds, field.resolution, brick_map, bricks, values, field.use_viewdirs)
+
+
+def baked_transparent_bricks(field: BakedField, chunk: int = 1024) -> torch.Tensor:
+    """bool[n_active]: the bricks every stored sigma_raw of which is <= 0 and whose channels 0 .. 27 are all finite.
+    Dropping them leaves every render of the field the same bits (include/nerfb200.h "baked fields: pruning").  Torch
+    over ``chunk`` slots at a time; works on a CPU field too."""
+    if not isinstance(field, BakedField):
+        raise ValueError(f"baked_transparent_bricks: field must be an nb.BakedField, got {type(field).__name__}")
+    v = field.values.detach()
+    out = torch.empty(field.n_active, dtype=torch.bool, device=v.device)
+    for s in range(0, field.n_active, chunk):
+        c = v[s:s + chunk, :, :28]
+        out[s:s + chunk] = (c[..., 0] <= 0).all(1) & torch.isfinite(c).flatten(1).all(1)
+    return out
+
+
+def baked_brick_weights_rays(field: BakedField, rays, out=None) -> torch.Tensor:
+    """fp32[n_active]: each brick slot's peak rendering weight w = alpha T over the packed ``rays`` (N, 11) with view
+    directions or (N, 8) without, laid out as ``render_baked_rays`` takes them: ``baked_render``'s weights at stop 0, a
+    NaN weight as +inf (include/nerfb200.h "baked fields: pruning").  With ``out`` (fp32[n_active] on the field's
+    device) the peaks are max-accumulated into it, so chunks of rays give the bits of one call.  A field without active
+    bricks returns an empty tensor without a launch."""
+    if not isinstance(field, BakedField):
+        raise ValueError(f"baked_brick_weights_rays: field must be an nb.BakedField, got {type(field).__name__}")
+    stride = 11 if field.use_viewdirs else 8
+    if not (isinstance(rays, torch.Tensor) and rays.dim() == 2 and rays.shape[1] == stride
+            and rays.dtype == torch.float32):
+        raise ValueError(f"baked_brick_weights_rays: rays must be fp32 (N, {stride}) for a field "
+                         f"{'with' if field.use_viewdirs else 'without'} view directions")
+    if out is not None and not (isinstance(out, torch.Tensor) and out.dtype == torch.float32
+                                and out.shape == (field.n_active,) and out.is_contiguous()):
+        raise ValueError(f"baked_brick_weights_rays: out must be a contiguous fp32 tensor of shape ({field.n_active},)")
+    _check_values(field, "baked_brick_weights_rays")
+    dev = field.values.device
+    if rays.device != dev or (out is not None and out.device != dev):
+        raise ValueError(f"baked_brick_weights_rays: rays and out must be on the field's device {dev}")
+    if out is None:
+        out = torch.zeros(field.n_active, dtype=torch.float32, device=dev)
+    if field.n_active and rays.shape[0]:
+        ops.baked_max_weights(field.box(), field.brick_map, field.values.detach(), field.use_viewdirs,
+                              rays.contiguous(), out)
+    return out
+
+
+def baked_brick_weights(field: BakedField, poses, height, width, focal_length, options) -> torch.Tensor:
+    """fp32[n_active]: each brick slot's peak rendering weight over every pixel of every pose in ``poses`` (n, 3 | 4,
+    4), the rays formed as ``render_baked`` forms them (``options.dataset`` near / far / no_ndc, view directions as the
+    field, which must match ``options.nerf.use_viewdirs``).  One launch per view, with no host synchronisation between
+    them (the poses are copied to the host once).  ``weights > tau`` is the PlenOctrees pruning mask; ``weights > 0``
+    prunes without changing those views' renders."""
+    if not isinstance(field, BakedField):
+        raise ValueError(f"baked_brick_weights: field must be an nb.BakedField, got {type(field).__name__}")
+    if not (isinstance(poses, torch.Tensor) and poses.dim() == 3 and poses.shape[0] > 0 and poses.shape[1] in (3, 4)
+            and poses.shape[2] == 4 and poses.is_floating_point()):
+        raise ValueError("baked_brick_weights: poses must be a float tensor (n, 3 | 4, 4) with n >= 1")
+    if not (int(height) > 0 and int(width) > 0):
+        raise ValueError(f"baked_brick_weights: need height, width > 0, got {height}, {width}")
+    _check_values(field, "baked_brick_weights")
+    _check_viewdirs(field, options, "baked_brick_weights")
+    out = torch.zeros(field.n_active, dtype=torch.float32, device=field.values.device)
+    if field.n_active == 0:
+        return out
+    host = poses.detach().to("cpu", torch.float32)
+    values, box = field.values.detach(), field.box()
+    for p in host:
+        rays = _pose_rays(field, height, width, focal_length, p, options)
+        ops.baked_max_weights(box, field.brick_map, values, field.use_viewdirs, rays, out)
+    return out

@@ -11,6 +11,9 @@
 //             and fine-tuning"); their order is the hardware's, so raw gradients may differ in the last bits between runs.
 //   tie       one thread per float4: the sum over every stored copy of the value's lattice point, gathered in one fixed
 //             order, so all copies get the same bits.
+//   peak      the renderer's warp re-marches the ray interpolating sigma_raw alone and max-accumulates each sample's
+//             weight into its brick slot (include/nerfb200.h "baked fields: pruning"): one integer atomicMax per slot
+//             per round, so the result is the same bits for every chunking and order.
 #include <cmath>
 
 #include "composite.cuh"
@@ -181,6 +184,19 @@ __device__ __forceinline__ void baked_interp(const float* __restrict__ values, i
   }
 }
 
+// channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B load
+// per corner
+__device__ __forceinline__ float baked_interp_sigma(const float* __restrict__ values, int slot, const float f[3],
+                                                    const int l[3]) {
+  float v = 0.f;
+  if (slot >= 0) {
+    const float* base = values + (int64_t)slot * kBakePts * kBakeCh;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) v = fmaf(corner_weight(f, k), __ldg(base + 4 * corner_offset(l, k)), v);
+  }
+  return v;
+}
+
 // rgb = sigmoid(s_c) of the interpolated coefficients v[1 ..]
 __device__ __forceinline__ void baked_colour(int use_viewdirs, const float Y[kBakeSh], const float v[kBakedVals],
                                              float rgb[3]) {
@@ -345,6 +361,41 @@ baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, con
   }
 }
 
+// max_w[slot] = max over the ray's samples in the slot of w = alpha T, the renderer's bits (stop_transmittance 0), a NaN
+// w as +inf.  The warp re-marches the ray as baked_render_kernel does, interpolating sigma_raw alone; per round the lanes
+// with w > 0 are grouped by slot and one lane per group issues an integer atomicMax of the group's largest bits
+// (non-negative floats order as unsigned integers).  No stop at T = 0: a NaN later in the ray must still be recorded.
+__global__ void __launch_bounds__(kBakedWarps * 32)
+baked_max_weight_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
+                        const float* __restrict__ rays, int ray_stride, int64_t n_rays, unsigned* __restrict__ max_w) {
+  const int lane = threadIdx.x & 31;
+  const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
+  if (r >= n_rays) return;
+  const float* rr = rays + r * ray_stride;
+  float o[3], d[3], ta, tb, dnorm, dt;
+  baked_ray(B, rr, o, d, ta, tb, dnorm, dt);
+  if (!baked_live(ta, tb, dt)) return;  // no sample
+  float T = 1.0f;
+  for (int k0 = 0;; k0 += 32) {
+    const float t = __fadd_rn(ta, __fmul_rn(__fadd_rn((float)(k0 + lane), 0.5f), dt));
+    if (!(__shfl_sync(0xffffffffu, t, 0) < tb)) break;
+    float f[3];
+    int l[3];
+    const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
+    if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // as the renderer: T stays
+    const float s = baked_interp_sigma(values, slot, f, l);
+    const SampleTerms st = sample_terms(slot >= 0 ? s : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
+    const float Tl = __fmul_rn(T, warp_excl_prod(st.q, lane));
+    const float w = __fmul_rn(st.alpha, Tl);
+    T = __shfl_sync(0xffffffffu, __fmul_rn(Tl, st.q), 31);
+    const bool rec = slot >= 0 && w != 0.f;  // w is >= 0 or NaN; max_w starts at 0
+    const unsigned bits = w != w ? __float_as_uint(INFINITY) : __float_as_uint(w);
+    const unsigned group = __match_any_sync(0xffffffffu, rec ? slot : -1);
+    const unsigned top = __reduce_max_sync(group, rec ? bits : 0u);
+    if (rec && lane == __ffs(group) - 1) atomicMax(max_w + slot, top);
+  }
+}
+
 // the copies of lattice index q along one axis (res cubes, nb bricks): (brick, point) pairs in ascending brick order.
 // q < res: (q / 8 - 1, 8) when q is a positive multiple of 8, then (q / 8, q % 8); q = res: (nb - 1, l) for l =
 // res - 8 (nb - 1) .. 8 (the upper face's point and its clamped repeats)
@@ -459,6 +510,22 @@ int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_m
       stop_transmittance, out);
   count_launch();
   return check_cuda(cudaGetLastError(), "baked_render launch");
+}
+
+int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                   int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                   float* max_w, void* stream) {
+  if (int rc = check_grid(box, "baked_max_weights")) return rc;
+  if (!brick_map || !values || !rays || !max_w || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
+    set_error("baked_max_weights: null pointer, n_rays <= 0 or ray_stride %d too short", ray_stride);
+    return NERFB200_ERR_INVALID;
+  }
+  const BakedBox B = baked_box(box);
+  const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
+  baked_max_weight_kernel<<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_max_weights launch");
 }
 
 int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,

@@ -1072,6 +1072,16 @@ def baked_tie(box: Grid, brick_map, bricks, d_values, d_tied=None):
     return d_tied
 
 
+def baked_max_weights(box: Grid, brick_map, values, use_viewdirs: bool, rays, max_w):
+    """Max-accumulates into ``max_w`` fp32[n_active] each brick slot's largest rendering weight over the packed
+    ``rays`` (``baked_render``'s weights at stop 0; a NaN weight as +inf).  Zero ``max_w`` once before the first
+    chunk."""
+    _lib.check(_lib.load().nerfb200_baked_max_weights(C.byref(box), _ptr(brick_map), _ptr(values),
+                                                      int(bool(use_viewdirs)), _ptr(rays), rays.shape[1],
+                                                      rays.shape[0], _ptr(max_w), _stream()), "baked_max_weights")
+    return max_w
+
+
 def baked_adam_step_dev(values, g, m, v, step_dev, lr_sigma, lr_sh, lr_decay=None, lr_decay_factor=0.1, beta1=0.9,
                         beta2=0.999, eps=1e-8):
     """``adam_step_dev`` over baked values: sigma_raw at ``lr_sigma``, the SH coefficients at ``lr_sh``."""
