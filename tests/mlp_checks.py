@@ -40,6 +40,26 @@ FWD_ONLY_ARCHS = {
     "4x128_noview": dict(num_layers=4, skip_every=4, n_freq_xyz=5, log_sampling_xyz=False, use_viewdirs=False),
 }
 ALL_ARCHS = {**TC_ARCHS, **FWD_ONLY_ARCHS}
+# hidden 128 that the wgmma training path refuses (encodings wider than 64 xyz / 32 direction channels, or a direction
+# encoding wider than 28 in the fused backward): all of them train, and all but the last also render, on the fp32
+# kernels.  The comments give xyz / direction channels and the wgrad_block<RN, RK> instances their encoding items reach.
+SIMT128_ARCHS = {
+    # the widest encodings (NERFB200_MAX_FREQS bands each) and the largest fp32 forward smem, 213 568 B: (8, 7), (4, 7)
+    "8x128_lxyz16_ldir16": dict(num_layers=8, skip_every=4, n_freq_xyz=16, n_freq_dir=16),
+    "6x128_lxyz13_ldir5_skip2": dict(num_layers=6, skip_every=2, n_freq_xyz=13, n_freq_dir=5),  # 81 / 33: (8, 6), (4, 3)
+    "4x128_lxyz11_noinput_ldir8": dict(num_layers=4, skip_every=4, n_freq_xyz=11, n_freq_dir=8,
+                                       include_input_xyz=False),                                # 66 / 51: (8, 5), (4, 4)
+    # linear bands, not powers of two, so the fp32 product x * f rounds: 75 / 81, (8, 5), (4, 6)
+    "10x128_lin12_ldir13": dict(num_layers=10, skip_every=4, n_freq_xyz=12, n_freq_dir=13, log_sampling_xyz=False,
+                                log_sampling_dir=False),
+    "3x128_ldir11_skip1": dict(num_layers=3, skip_every=1, n_freq_xyz=6, n_freq_dir=11),       # 39 / 69: (8, 3), (4, 5)
+    # fc_out reads layer1's output, which has no ReLU; layer1 has no hidden columns: 99 / -, (8, 7)
+    "1x128_lxyz16_noview": dict(num_layers=1, skip_every=4, n_freq_xyz=16, use_viewdirs=False),
+    # the wgmma forward takes it, the fused backward does not: 63 / 30, (8, 4), (4, 2)
+    "8x128_ldir5_noinput": FWD_ONLY_ARCHS["8x128_ldir5_noinput"],
+}
+# every architecture the fp32-kernel checks run (test_simt_mlp_gpu.py)
+SIMT_NAMES = [*H256_ARCHS, *SIMT128_ARCHS]
 STATES = ["init", "scaled"]
 # one ray at the smallest sample count the wgmma kernels accept; tiles spanning 10 rays; ragged tiles
 SHAPES = [(1, 15), (37, 15), (33, 17)]
@@ -47,7 +67,7 @@ SHAPES = [(1, 15), (37, 15), (33, 17)]
 # Worst raw element per output column as a fraction of the column's scale, wgmma forward (stash-writing and inference)
 # against fp64.  Measured on an H100 80GB HBM3, worst over all parameter sets and both weight states [1.1e-5].
 TC_FWD_TOL = 3e-5
-# The fp32 kernels' raw outputs per column (test_simt_hidden256_gpu.py FWD_TOL) [7.8e-7, test_tc_full_size_gpu.py].
+# The fp32 kernels' raw outputs per column (test_simt_mlp_gpu.py FWD_TOL) [7.8e-7, test_tc_full_size_gpu.py].
 SIMT_FWD_TOL = 3e-5
 # Parameter gradients per block, relative to the block's scale (test_tc_arch_sweep_gpu.py BLOCK_TOL): at training size
 # wgmma [6.3e-6, a probe], fp32 kernels [4.1e-6, A2] (test_tc_full_size_gpu.py, H100 80GB HBM3, 700 W, 1980 MHz).
@@ -116,17 +136,18 @@ def scene_models(scene):
 
 
 def spec(name):
-    """The ops.ArchSpec of a table entry: H256_ARCHS at hidden 256 / skip 4, ALL_ARCHS at hidden 128."""
+    """The ops.ArchSpec of a table entry: H256_ARCHS at hidden 256 / skip 4, ALL_ARCHS and SIMT128_ARCHS at hidden
+    128."""
     from nerf_pytorch_b200 import ops
 
     if name in H256_ARCHS:
         return ops.ArchSpec(hidden=256, skip_every=4, **H256_ARCHS[name])
-    return ops.ArchSpec(hidden=128, **ALL_ARCHS[name])
+    return ops.ArchSpec(hidden=128, **(ALL_ARCHS[name] if name in ALL_ARCHS else SIMT128_ARCHS[name]))
 
 
 def arch_name(arch):
-    """The table name of an ops.ArchSpec (its repr if it is in neither table)."""
-    return next((k for k in [*H256_ARCHS, *ALL_ARCHS] if spec(k) == arch), repr(arch))
+    """The table name of an ops.ArchSpec (its repr if it is in no table)."""
+    return next((k for k in [*H256_ARCHS, *ALL_ARCHS, *SIMT128_ARCHS] if spec(k) == arch), repr(arch))
 
 
 def sms():

@@ -19,6 +19,20 @@ def test_fp32_support_query_refuses_a_forward_that_exceeds_shared_memory():
     assert "impl=0" in why and "shared memory" in why, why
 
 
+def test_hidden128_widest_encodings_run_on_the_fp32_kernels_only():
+    """8 x 128 with 16 xyz and 16 direction bands (NERFB200_MAX_FREQS, 99 channels each): the fp32 forward fits it
+    (213 568 B of shared memory), and every wgmma code refuses encodings wider than 64 xyz / 32 direction channels."""
+    from nerf_pytorch_b200 import _lib, ops
+
+    lib = _lib.load()
+    arch = ops.ArchSpec(num_layers=8, hidden=128, n_freq_xyz=16, n_freq_dir=16)
+    assert lib.nerfb200_impl_supported(C.byref(arch.c_struct()), 64, ops.IMPL_SIMT) == _lib.OK
+    for impl in (1, 2, 3):
+        assert lib.nerfb200_impl_supported(C.byref(arch.c_struct()), 64, impl) == _lib.ERR_UNSUPPORTED, impl
+        why = lib.nerfb200_last_error().decode()
+        assert f"impl={1 if impl == 2 else impl}" in why and "encodings wider than 64" in why, (impl, why)
+
+
 @pytest.mark.parametrize("impl", [2, 4, -1])
 def test_backward_scratch_query_refuses_codes_that_have_no_backward(impl):
     from nerf_pytorch_b200 import _lib, ops

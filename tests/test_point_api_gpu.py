@@ -13,8 +13,8 @@ import pytest
 import torch
 
 from helpers import Case, bits_equal, build_models, composite64
-from mlp_checks import (ALL_ARCHS, BLOCK_TOL, COMP_GRAD_TOL, COMP_TOL, H256_ARCHS, SHAPES, SIMT_FWD_TOL, TC_ARCHS,
-                        TC_FWD_TOL, _floors, _split_floors, arch_weights, check_blocks, oracle, report, spec,
+from mlp_checks import (ALL_ARCHS, BLOCK_TOL, COMP_GRAD_TOL, COMP_TOL, H256_ARCHS, SHAPES, SIMT128_ARCHS, SIMT_FWD_TOL,
+                        TC_ARCHS, TC_FWD_TOL, _floors, _split_floors, arch_weights, check_blocks, oracle, report, spec,
                         tc_blocks, upstream)
 
 pytestmark = pytest.mark.gpu
@@ -120,7 +120,9 @@ def _box_points(arch, lead, s, seed):
 
 
 FWD_SHAPES = [((n,), s) for n, s in SHAPES] + [((1,), 100000), ((2, 3, 4), 16)]
-NAMES = [f"h128_{k}" for k in ALL_ARCHS] + [f"h256_{k}" for k in H256_ARCHS]
+# hidden 128 on both kernel families, hidden-128 encodings that only the fp32 kernels take, hidden 256
+NAMES = ([f"h128_{k}" for k in ALL_ARCHS] + [f"h128_{k}" for k in SIMT128_ARCHS if k not in ALL_ARCHS]
+         + [f"h256_{k}" for k in H256_ARCHS])
 
 
 @pytest.mark.parametrize("shape", FWD_SHAPES, ids=lambda s: "x".join(map(str, s[0] + (s[1],))))
@@ -148,7 +150,9 @@ def test_run_network_forward_matches_fp64_at_points_off_any_ray(name, shape):
             assert e <= tol, (name, shape, impl, e)
 
 
-GRAD_CASES = [(f"h128_{k}", 1) for k in TC_ARCHS] + [(f"h256_{k}", 0) for k in H256_ARCHS]
+# each architecture on the kernels that train it
+GRAD_CASES = ([(f"h128_{k}", 1) for k in TC_ARCHS] + [(f"h128_{k}", 0) for k in SIMT128_ARCHS]
+              + [(f"h256_{k}", 0) for k in H256_ARCHS])
 
 
 @pytest.mark.parametrize("shape", SHAPES, ids=lambda s: f"{s[0]}x{s[1]}")

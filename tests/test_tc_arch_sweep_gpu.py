@@ -21,8 +21,8 @@ Checks, each printed with -s:
   4. the sample-count and encoding-width limits of the wgmma path;
   5. one training step through run_one_iter_of_nerf that picks the wgmma kernels, against fp64 autograd.
 Two more architectures get the forward checks: L_dir 5 without input (30 direction channels: the wgmma forward takes it,
-the fused backward does not) and a model without view directions, whose training backward runs on the fp32 kernels and
-is checked here with those.
+the fused backward does not, and test_simt_mlp_gpu.py checks its training backward on the fp32 kernels) and a model
+without view directions, whose training backward runs on the fp32 kernels and is checked here with those.
 
 The oracle and its inputs are those of mlp_checks.py (fp32 points and band products, fp64 from there on);
 weights are the seeded reference init ("init") and the same with every gemm layer scaled until max |raw| ~ 3e3
@@ -48,7 +48,7 @@ pytestmark = pytest.mark.gpu
 STASH_TOL = 2e-5     # stashed activation and encoding tiles, per layer; also how far from zero a ReLU tie may sit [9.8e-6]
 BLOCK_TOL = 3e-5     # parameter gradients, per block: wgmma [1.3e-5], fp32 kernels [5.2e-6]
 ACCUM_TOL = 2e-6     # accumulated minus previous contents vs the gradient, per block [2.5e-7]
-FP32_TIE_TOL = 1e-5  # how far from zero an fp32 ReLU tie may sit: test_simt_hidden256_gpu.py's STASH_TOL [1.4e-6]
+FP32_TIE_TOL = 1e-5  # how far from zero an fp32 ReLU tie may sit: test_simt_mlp_gpu.py's STASH_TOL [1.4e-6]
 
 # tiles inside one ray; one CTA with two tiles; ~four tiles per CTA ("sms": the device's multiprocessor count)
 MULTI_ARCHS = ["6x128_skip1", "16x128_skip5"]
@@ -221,7 +221,7 @@ def test_tc_sample_count_and_encoding_width_limits():
 # ------------------------------------------------------------------------------------------------------------------------
 # 5. one training step end to end on the wgmma kernels
 # ------------------------------------------------------------------------------------------------------------------------
-# As in test_simt_hidden256_gpu: the step forms depths and points in fp32, so the coarse network's worst element is
+# As in test_simt_mlp_gpu: the step forms depths and points in fp32, so the coarse network's worst element is
 # bounded in units of the fp32 reference's own distance from fp64, per tensor, and the fine network (whose samples the
 # resampler places from the coarse weights) by relative L2.  At loss scale the fixed-point floor is not negligible, so it
 # is added to both bars.  Measured on an H100 80GB HBM3 in brackets.
