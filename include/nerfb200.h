@@ -724,6 +724,48 @@ int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* br
                                    int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                    float* max_w, void* stream);
 
+/* ---- baked fields: regularisers -------------------------------------------------------------------------------------
+ * Squared total variation of the density and of the SH coefficients over the lattice, and a Cauchy sparsity term on the
+ * density (as Plenoxels regularises its voxels), with their gradient in the tie's convention, so that fine-tuning can
+ * trade fitting the training views for a smoother, emptier field.
+ *   - Lattice points.  The points q of 0 .. res (per axis) with at least one stored copy in an active brick, the copies
+ *     enumerated as the tie enumerates them ("baked fields: gradients and fine-tuning").  P is their number.
+ *   - Canonical copy.  A point's first copy in the tie's order (z outer, then y, then x, bricks ascending) whose brick is
+ *     active.  Every value read below is read at the canonical copy of its point, so the result does not depend on which
+ *     copy a thread holds, even if copies differ.
+ *   - Edges.  The pairs (q, q + e_c) with q_c + 1 <= res_c such that an active brick holds both points: brick q_c / 8
+ *     along c (the only brick whose points 8 b .. min(8 b + 8, res) hold q_c and q_c + 1) and, along each other axis a,
+ *     any brick of q_a's copy list (at most two distinct bricks, so at most 4 candidates in brick_map).  The clamped
+ *     repeats on the upper faces are one point and never form an edge.
+ *   - Loss.  With v_ch channel ch of a point, sigma = v_0 and sigma+ = max(sigma, 0):
+ *       L = (1 / P) [ l_sigma sum_edges (d sigma)^2 + l_sh sum_edges sum_{ch = 1 .. 27} (d v_ch)^2
+ *                     + l_s sum_points log(1 + 2 sigma+^2) ],
+ *     squared TV on sigma_raw, squared TV on the 27 coefficients and a Cauchy sparsity term on the density at the
+ *     lattice points.  Dividing by P keeps a weight meaningful across resolutions and prunes.
+ *   - Gradient.  Written for every stored copy as dL / d(the copy's lattice point), the convention of the tied gradient
+ *     of baked_render_bwd + baked_tie.  fp32, each op rounded, no contraction:
+ *       S_ch = 0, then S_ch += (v_p - v_n) over the point's edges in the order -x, +x, -y, +y, -z, +z;
+ *       g_ch = a_ch S_ch with a_0 = fp32(2 l_sigma / P) and a_1..27 = fp32(2 l_sh / P), each formed in fp64 and rounded
+ *       once; channel 0 then adds (b sigma+) / (1 + 2 (sigma+ sigma+)) with b = fp32(4 l_s / P) formed the same way;
+ *       d[copy][ch] += g_ch for ch = 0 .. 27 (added into the caller's buffer); channels 28 .. 31 are not touched.
+ *     Every copy of a point computes the same terms in the same order, so every copy gets the same bits, and a d whose
+ *     copies were bit-equal (the tie's output) stays so.
+ *   - Value.  partials[slot] = (sum over the slot's stored points that are canonical copies of l_sigma (sum of the
+ *     point's +x / +y / +z edges' (d sigma)^2) + l_sh (the same over channels 1 .. 27) + l_s log1p(2 sigma+^2)) / P, in
+ *     fp64 (differences of the fp32 values, exact in fp64), each point's edges and sparsity term counted once; the
+ *     per-point sums are reduced over the slot in a fixed order, so the partials are the same bits every run.  L is
+ *     their sum.
+ * baked_lattice_count: *count = P (int64, device memory; one memset and one launch, integer atomics).
+ * baked_regularizer: reads P from *count when it runs (no host synchronisation), adds the gradient into d (layout of
+ *   values; may be NULL) and writes partials fp64[n_active] (may be NULL, not both).  One CTA per slot.
+ * Refused before any launch: an invalid box, a null pointer where one is needed (d and partials both NULL included),
+ * n_active outside 1 .. the box's bricks, a weight that is negative, NaN or infinite, d overlapping values. */
+int32_t nerfb200_baked_lattice_count(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                     int64_t n_active, int64_t* count, void* stream);
+int32_t nerfb200_baked_regularizer(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                   int64_t n_active, const float* values, const int64_t* count, double tv_sigma,
+                                   double tv_sh, double sparsity, float* d, double* partials, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

@@ -165,6 +165,8 @@ SIGNATURES = {
     "nerfb200_baked_tie": (I32, [GP, P, P, I64, P, P, P]),
     "nerfb200_baked_adam_step_dev": (I32, [P, P, P, P, I64, P, F64, F64, F64, F64, F32, F32, F32, P]),
     "nerfb200_baked_max_weights": (I32, [GP, P, P, I32, P, I32, I64, P, P]),
+    "nerfb200_baked_lattice_count": (I32, [GP, P, P, I64, P, P]),
+    "nerfb200_baked_regularizer": (I32, [GP, P, P, I64, P, P, F64, F64, F64, P, P, P]),
 }
 
 _lib = None

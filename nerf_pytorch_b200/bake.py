@@ -7,8 +7,9 @@ include/nerfb200.h "baked fields"; the bake is one fused wgmma kernel (csrc/mlp_
 one warp per ray (csrc/baked.cu).  A baked field can be fine-tuned against images through that renderer
 (render_baked_rays, BakedFieldTrainer; include/nerfb200.h "baked fields: gradients and fine-tuning"), and pruned to the
 bricks its renders use (baked_transparent_bricks, baked_brick_weights, prune_baked, BakedFieldTrainer.prune;
-include/nerfb200.h "baked fields: pruning").  This file validates arguments, sizes buffers and moves pointers; the bake
-reads the active brick count back once to size its values."""
+include/nerfb200.h "baked fields: pruning"), with total-variation and sparsity regularisers over the lattice
+(baked_regularizer, BakedFieldTrainer's tv_sigma / tv_sh / sparsity; include/nerfb200.h "baked fields: regularisers").  This file validates arguments, sizes buffers and moves
+pointers; the bake reads the active brick count back once to size its values."""
 from __future__ import annotations
 
 import torch
@@ -178,6 +179,59 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
     return out[:, :3], out[:, 3], out[:, 4], out[:, 5]
 
 
+def _check_weights(what, tv_sigma, tv_sh, sparsity):
+    """The three regulariser weights as floats, each finite and >= 0 (ValueError otherwise)."""
+    lam = (float(tv_sigma), float(tv_sh), float(sparsity))
+    if not all(0.0 <= x < float("inf") for x in lam):
+        raise ValueError(f"{what}: tv_sigma, tv_sh and sparsity must be finite and >= 0, got {lam}")
+    return lam
+
+
+class _BakedRegularizer(torch.autograd.Function):
+    """The 0-dim fp32 loss of ``baked_regularizer``; the backward is the kernel's gradient times the upstream scalar."""
+
+    @staticmethod
+    def forward(ctx, values, field, lam):
+        loss, count = _regularizer_value(field, values.detach(), lam)
+        ctx.save_for_backward(values, count)
+        ctx.field, ctx.lam = field, lam
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        values, count = ctx.saved_tensors
+        f = ctx.field
+        d = torch.zeros_like(values)
+        ops.baked_regularizer(f.box(), f.brick_map, f.bricks, values.detach(), count, *ctx.lam, d=d)
+        return d * g, None, None
+
+
+def baked_regularizer(field: BakedField, *, tv_sigma=0.0, tv_sh=0.0, sparsity=0.0) -> torch.Tensor:
+    """The 0-dim fp32 loss L = (1 / P) [tv_sigma sum_edges (d sigma_raw)^2 + tv_sh sum_edges sum over the 27 SH
+    coefficients of (d coef)^2 + sparsity sum_points log(1 + 2 max(sigma_raw, 0)^2)] over the field's lattice points
+    (P of them) and lattice edges (include/nerfb200.h "baked fields: regularisers"): the fp64 sum of the kernel's
+    per-slot partials, rounded once.  Differentiable with respect to ``field.values``: the gradient is written at every
+    stored copy of each lattice point and is the same bits at all of them, so ``mse + baked_regularizer(...)`` under
+    ``torch.optim.Adam`` keeps the copies bit-equal, as ``render_baked_rays`` does.  Each call counts P (one memset and
+    one launch) and forms the value (one launch); the backward is one more launch."""
+    _check_values(field, "baked_regularizer")
+    lam = _check_weights("baked_regularizer", tv_sigma, tv_sh, sparsity)
+    if field.n_active == 0:
+        raise ValueError("baked_regularizer: the field has no active brick")
+    if field.values.requires_grad and torch.is_grad_enabled():
+        return _BakedRegularizer.apply(field.values, field, lam)
+    return _regularizer_value(field, field.values.detach(), lam)[0]
+
+
+def _regularizer_value(field, values, lam):
+    """(the fp32 loss, the device count P) of ``field``'s lattice at ``values``."""
+    box = field.box()
+    count = ops.baked_lattice_count(box, field.brick_map, field.bricks)
+    partials = torch.empty(field.n_active, dtype=torch.float64, device=values.device)
+    ops.baked_regularizer(box, field.brick_map, field.bricks, values, count, *lam, partials=partials)
+    return partials.sum().float(), count
+
+
 # default rates of BakedFieldTrainer: the best held-out PSNR of a sweep on lego A0 at 256^3 (DESIGN §4)
 DEFAULT_LR_SIGMA = 1.0
 DEFAULT_LR_SH = 1e-2
@@ -196,10 +250,16 @@ class BakedFieldTrainer:
     buffers the size of ``field.values`` (gradient, tied gradient, m, v): 3.9 GiB for lego at 256^3 and 22.5 GiB at
     512^3 over the grid of both lego networks, 2.1 and 11.0 GiB over the fine network's grid (DESIGN §4).
     ``rays_per_step`` pixels are drawn from one image per step, so it cannot exceed H * W.  The backward's vector reductions run in hardware order, so two runs agree to fp32 rounding, not bitwise;
-    every stored copy of a lattice point stays bit-equal to the others."""
+    every stored copy of a lattice point stays bit-equal to the others.
+
+    ``tv_sigma``, ``tv_sh`` and ``sparsity`` (finite, >= 0; all 0 by default) add ``baked_regularizer``'s gradient at
+    those weights into the tied gradient before the Adam step: one more launch per step when any is nonzero, none when
+    all are 0, which leaves the step exactly the unregularised one.  P is counted on the device at construction and
+    again by ``prune``.  ``loss`` stays the MSE alone (the regulariser's value would cost a reduction per step; call
+    ``baked_regularizer`` for it)."""
 
     def __init__(self, field, images, poses, focal, options, *, lr_sigma=DEFAULT_LR_SIGMA, lr_sh=DEFAULT_LR_SH,
-                 lr_decay=None, rays_per_step=4096, seed=0):
+                 lr_decay=None, rays_per_step=4096, seed=0, tv_sigma=0.0, tv_sh=0.0, sparsity=0.0):
         _check_values(field, "BakedFieldTrainer")
         if field.n_active == 0:
             raise ValueError("BakedFieldTrainer: the field has no active brick")
@@ -222,6 +282,7 @@ class BakedFieldTrainer:
             raise ValueError("BakedFieldTrainer: need lr_sigma, lr_sh >= 0 and lr_decay None or > 0")
         if not 0 <= int(seed) < 2 ** 64:
             raise ValueError("BakedFieldTrainer: seed must be in [0, 2^64)")
+        self.reg = _check_weights("BakedFieldTrainer", tv_sigma, tv_sh, sparsity)
         self.field, self.seed = field, int(seed)
         self.images, self.poses = images.contiguous(), poses.contiguous()
         self.focal, self.H, self.W, self.n_images, self.n = float(focal), int(H), int(W), int(n_img), n
@@ -242,6 +303,7 @@ class BakedFieldTrainer:
         self._out = torch.empty(n, 8, dtype=torch.float32, device=dev)
         self._g = torch.empty(n, 8, dtype=torch.float32, device=dev)
         self.loss = torch.zeros((), dtype=torch.float32, device=dev)
+        self._count = ops.baked_lattice_count(self._box, field.brick_map, field.bricks)
 
     def step(self, n: int = 1):
         """Runs ``n`` steps; returns the last step's loss (a device tensor)."""
@@ -260,6 +322,9 @@ class BakedFieldTrainer:
                 ops.baked_render_bwd(self._box, f.brick_map, f.values, f.use_viewdirs, self._rays, self.white,
                                      self._out, self._g, self.d_values)
                 ops.baked_tie(self._box, f.brick_map, f.bricks, self.d_values, self.d_tied)
+                if any(self.reg):
+                    ops.baked_regularizer(self._box, f.brick_map, f.bricks, f.values, self._count, *self.reg,
+                                          d=self.d_tied)
                 ops.baked_adam_step_dev(f.values, self.d_tied, self.m, self.v, self.step_dev, self.lr_sigma,
                                         self.lr_sh, self.lr_decay)
                 ops.step_advance(self.step_dev)
@@ -270,8 +335,9 @@ class BakedFieldTrainer:
         true, as ``prune_baked`` does: the ``BakedField`` passed to the constructor then holds the pruned ``brick_map``,
         ``bricks`` and ``values``, the Adam moments ``m`` and ``v`` go through the same row gather, and the gradient
         buffers are reallocated at the new size (the old ones are freed first).  ``step_dev``, the seed, the rates and
-        the schedule carry on.  A pruned brick never comes back: its samples become misses, and the tie no longer carries
-        gradient into it.  Keeping no brick raises ValueError, as the constructor does.  Reads the kept count back once."""
+        the schedule carry on, and the regularisers' P is counted again over the kept bricks.  A pruned brick never comes
+        back: its samples become misses, and the tie no longer carries gradient into it.  Keeping no brick raises
+        ValueError, as the constructor does.  Reads the kept count back once."""
         f = self.field
         _check_keep(f, keep, "BakedFieldTrainer.prune")
         idx = torch.nonzero(keep).reshape(-1)
@@ -282,6 +348,7 @@ class BakedFieldTrainer:
             f.brick_map, f.bricks, f.values = _pruned(f, idx)
             self.m, self.v = self.m.index_select(0, idx), self.v.index_select(0, idx)
         self.d_values, self.d_tied = torch.zeros_like(f.values), torch.zeros_like(f.values)
+        ops.baked_lattice_count(self._box, f.brick_map, f.bricks, self._count)
 
 
 # ------------------------------------------------------------------------------------------------------------------------

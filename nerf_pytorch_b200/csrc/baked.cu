@@ -14,6 +14,9 @@
 //   peak      the renderer's warp re-marches the ray interpolating sigma_raw alone and max-accumulates each sample's
 //             weight into its brick slot (include/nerfb200.h "baked fields: pruning"): one integer atomicMax per slot
 //             per round, so the result is the same bits for every chunking and order.
+//   regularisers  one CTA per slot, one thread per stored point (include/nerfb200.h "baked fields: regularisers"):
+//             the TV and sparsity gradient from canonical-copy reads, the same bits at every copy, and the slot's fp64
+//             value partial reduced in a fixed order.
 #include <cmath>
 
 #include "composite.cuh"
@@ -458,6 +461,181 @@ __global__ void baked_tie_kernel(const BakedBox B, const int* __restrict__ brick
   d_tied[e] = s;
 }
 
+// the canonical copy of lattice point q (include/nerfb200.h "baked fields: regularisers"): the float offset of its first
+// stored copy in the tie's order whose brick is active, or -1 when no active brick holds q
+__device__ __forceinline__ int64_t canonical_copy(const BakedBox& B, const int* __restrict__ brick_map, const int q[3]) {
+  AxisCopies a[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) a[c] = axis_copies(q[c], B.g.res[c], B.nb[c]);
+  for (int ez = 0; ez < a[2].n; ++ez) {
+    int bz, lz;
+    axis_entry(a[2], ez, bz, lz);
+    for (int ey = 0; ey < a[1].n; ++ey) {
+      int by, ly;
+      axis_entry(a[1], ey, by, ly);
+      for (int ex = 0; ex < a[0].n; ++ex) {
+        int bx, lx;
+        axis_entry(a[0], ex, bx, lx);
+        const int cs = brick_map[((int64_t)bz * B.nb[1] + by) * B.nb[0] + bx];
+        if (cs >= 0) return ((int64_t)cs * kBakePts + (lz * 9 + ly) * 9 + lx) * kBakeCh;
+      }
+    }
+  }
+  return -1;
+}
+
+// whether (q, q + e_c) is an edge: q_c < res_c and an active brick holds both points, brick q_c / 8 along c and any
+// brick of q's copy list along the other two axes (at most two distinct bricks each)
+__device__ __forceinline__ bool lattice_edge(const BakedBox& B, const int* __restrict__ brick_map, const int q[3], int c) {
+  int lo[3], hi[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {  // a == c compared, not q[c] indexed: the arrays stay in registers
+    if (a == c) {
+      if (q[a] >= B.g.res[a]) return false;
+      lo[a] = hi[a] = q[a] >> 3;
+    } else {
+      const AxisCopies ac = axis_copies(q[a], B.g.res[a], B.nb[a]);
+      lo[a] = ac.b0;
+      hi[a] = ac.face ? ac.b0 : ac.b0 + ac.n - 1;
+    }
+  }
+  for (int bz = lo[2]; bz <= hi[2]; ++bz)
+    for (int by = lo[1]; by <= hi[1]; ++by)
+      for (int bx = lo[0]; bx <= hi[0]; ++bx)
+        if (brick_map[((int64_t)bz * B.nb[1] + by) * B.nb[0] + bx] >= 0) return true;
+  return false;
+}
+
+// the lattice point a stored point holds: b B + l clamped onto 0 .. res
+__device__ __forceinline__ void stored_point(const BakedBox& B, int brick, int p, int q[3]) {
+  const int bc[3] = {brick % B.nb[0], (brick / B.nb[0]) % B.nb[1], brick / (B.nb[0] * B.nb[1])};
+  const int lc[3] = {p % 9, (p / 9) % 9, p / 81};
+#pragma unroll
+  for (int c = 0; c < 3; ++c) q[c] = min(bc[c] * kBakeBrick + lc[c], B.g.res[c]);
+}
+
+constexpr int kRegThreads = 256;
+
+// *count = P, the lattice points with a copy in an active brick: the stored points that are their point's canonical
+// copy, one warp ballot and one integer atomic per warp (*count zeroed first).  One thread per stored point.
+__global__ void __launch_bounds__(kRegThreads)
+baked_count_kernel(const BakedBox B, const int* __restrict__ brick_map, const int* __restrict__ bricks,
+                   int64_t n_active, unsigned long long* __restrict__ count) {
+  const int64_t sp = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  bool canon = false;
+  if (sp < n_active * kBakePts) {
+    const int64_t slot = sp / kBakePts;
+    const int p = (int)(sp - slot * kBakePts);
+    int q[3];
+    stored_point(B, bricks[slot], p, q);
+    canon = canonical_copy(B, brick_map, q) == sp * kBakeCh;
+  }
+  const unsigned votes = __ballot_sync(0xffffffffu, canon);
+  if ((threadIdx.x & 31) == 0 && votes) atomicAdd(count, (unsigned long long)__popc(votes));
+}
+
+// The regularisers' gradient and value (include/nerfb200.h "baked fields: regularisers").  One CTA per slot, one thread
+// per stored point (the CTA strides over the slot's 729): every value is read at its point's canonical copy; S_ch sums
+// v_p - v_n over the point's edges in the order -x, +x, -y, +y, -z, +z, g_ch = a_ch S_ch (plus the Cauchy term on
+// channel 0) is added into d at the thread's own copy.  A thread whose copy is canonical adds its +x / +y / +z edges'
+// squares and its sparsity term to an fp64 sum, reduced over the CTA in a fixed order into partials[slot].
+__global__ void __launch_bounds__(kRegThreads)
+baked_reg_kernel(const BakedBox B, const int* __restrict__ brick_map, const int* __restrict__ bricks,
+                 const float* __restrict__ values, const long long* __restrict__ count, double tv_sigma, double tv_sh,
+                 double sparsity, float* __restrict__ d, double* __restrict__ partials) {
+  const int64_t slot = blockIdx.x;
+  const double P = (double)*count;
+  const float a_sigma = (float)(2.0 * tv_sigma / P), a_sh = (float)(2.0 * tv_sh / P);
+  const float a_sparse = (float)(4.0 * sparsity / P);
+  const int brick = bricks[slot];
+  double acc = 0.0;
+  for (int p = threadIdx.x; p < kBakePts; p += kRegThreads) {
+    const int64_t own = (slot * kBakePts + p) * kBakeCh;
+    int q[3];
+    stored_point(B, brick, p, q);
+    const int64_t cp = canonical_copy(B, brick_map, q);  // >= 0: the thread's own brick is active
+    const bool canon = cp == own;
+    const float4* vp4 = reinterpret_cast<const float4*>(values + cp);
+    float vp[kBakedVals], S[kBakedVals];
+#pragma unroll
+    for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+      const float4 a = __ldg(vp4 + c4);
+      vp[4 * c4] = a.x;
+      vp[4 * c4 + 1] = a.y;
+      vp[4 * c4 + 2] = a.z;
+      vp[4 * c4 + 3] = a.w;
+    }
+#pragma unroll
+    for (int ch = 0; ch < kBakedVals; ++ch) S[ch] = 0.f;
+    double tvs = 0.0, tvh = 0.0;
+#pragma unroll 1
+    for (int k = 0; k < 6; ++k) {  // -x, +x, -y, +y, -z, +z
+      const int c = k >> 1;
+      const bool up = k & 1;
+      int lo[3], qn[3];  // the edge's lower point and the neighbour
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        lo[a] = a == c && !up ? q[a] - 1 : q[a];
+        qn[a] = a == c ? (up ? q[a] + 1 : q[a] - 1) : q[a];
+      }
+      if ((lo[0] | lo[1] | lo[2]) < 0 || !lattice_edge(B, brick_map, lo, c)) continue;
+      const float4* vn4 = reinterpret_cast<const float4*>(values + canonical_copy(B, brick_map, qn));
+#pragma unroll
+      for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+        const float4 a = __ldg(vn4 + c4);
+        const float n[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int ch = 4 * c4 + j;
+          S[ch] = __fadd_rn(S[ch], __fsub_rn(vp[ch], n[j]));
+          if (up && canon) {
+            const double e = (double)vp[ch] - (double)n[j];
+            if (ch == 0) tvs += e * e;
+            else tvh += e * e;
+          }
+        }
+      }
+    }
+    const float sp = fmaxf(vp[0], 0.f);
+    if (canon) {
+      const double s = sp;
+      acc += tv_sigma * tvs + tv_sh * tvh + sparsity * log1p(2.0 * s * s);
+    }
+    if (d) {
+      float4* d4 = reinterpret_cast<float4*>(d + own);
+#pragma unroll
+      for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+        float g[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int ch = 4 * c4 + j;
+          g[j] = __fmul_rn(ch == 0 ? a_sigma : a_sh, S[ch]);
+        }
+        if (c4 == 0)
+          g[0] = __fadd_rn(g[0], __fdiv_rn(__fmul_rn(a_sparse, sp), __fadd_rn(1.0f, __fmul_rn(2.0f, __fmul_rn(sp, sp)))));
+        float4 o = d4[c4];
+        o.x = __fadd_rn(o.x, g[0]);
+        o.y = __fadd_rn(o.y, g[1]);
+        o.z = __fadd_rn(o.z, g[2]);
+        o.w = __fadd_rn(o.w, g[3]);
+        d4[c4] = o;
+      }
+    }
+  }
+  if (!partials) return;
+  // the CTA's sum in a fixed order: each warp by a shuffle tree, then warp 0 over the warps' sums
+  __shared__ double warp_sum[kRegThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < kRegThreads / 32; ++w) s += warp_sum[w];
+    partials[slot] = s / P;
+  }
+}
+
 BakedBox baked_box(const nerfb200_grid_t* box) {
   BakedBox B;
   B.g = *box;
@@ -567,6 +745,53 @@ int32_t nerfb200_baked_tie(const nerfb200_grid_t* box, const int32_t* brick_map,
       B, brick_map, bricks, n_active, reinterpret_cast<const float4*>(d_values), reinterpret_cast<float4*>(d_tied));
   count_launch();
   return check_cuda(cudaGetLastError(), "baked_tie launch");
+}
+
+int32_t nerfb200_baked_lattice_count(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                     int64_t n_active, int64_t* count, void* stream) {
+  if (int rc = check_grid(box, "baked_lattice_count")) return rc;
+  const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
+  if (!brick_map || !bricks || !count || n_active <= 0 || n_active > n_bricks) {
+    set_error("baked_lattice_count: null pointer or n_active %lld outside 1 .. %lld", (long long)n_active,
+              (long long)n_bricks);
+    return NERFB200_ERR_INVALID;
+  }
+  const BakedBox B = baked_box(box);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (int rc = check_cuda(cudaMemsetAsync(count, 0, sizeof(int64_t), s), "baked_lattice_count memset")) return rc;
+  const int64_t n = n_active * kBakePts;
+  baked_count_kernel<<<(unsigned)((n + kRegThreads - 1) / kRegThreads), kRegThreads, 0, s>>>(
+      B, brick_map, bricks, n_active, reinterpret_cast<unsigned long long*>(count));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_lattice_count launch");
+}
+
+int32_t nerfb200_baked_regularizer(const nerfb200_grid_t* box, const int32_t* brick_map, const int32_t* bricks,
+                                   int64_t n_active, const float* values, const int64_t* count, double tv_sigma,
+                                   double tv_sh, double sparsity, float* d, double* partials, void* stream) {
+  if (int rc = check_grid(box, "baked_regularizer")) return rc;
+  const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
+  if (!brick_map || !bricks || !values || !count || (!d && !partials) || n_active <= 0 || n_active > n_bricks) {
+    set_error("baked_regularizer: null pointer, d and partials both null, or n_active %lld outside 1 .. %lld",
+              (long long)n_active, (long long)n_bricks);
+    return NERFB200_ERR_INVALID;
+  }
+  const double lam[3] = {tv_sigma, tv_sh, sparsity};
+  for (double l : lam)
+    if (!(l >= 0.0 && l < INFINITY)) {
+      set_error("baked_regularizer: the weights must be finite and >= 0, got %g %g %g", tv_sigma, tv_sh, sparsity);
+      return NERFB200_ERR_INVALID;
+    }
+  const int64_t n = n_active * kBakePts * kBakeCh;
+  if (d && d < values + n && values < d + n) {
+    set_error("baked_regularizer: d overlaps values");
+    return NERFB200_ERR_INVALID;
+  }
+  const BakedBox B = baked_box(box);
+  baked_reg_kernel<<<(unsigned)n_active, kRegThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      B, brick_map, bricks, values, reinterpret_cast<const long long*>(count), tv_sigma, tv_sh, sparsity, d, partials);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_regularizer launch");
 }
 
 }  // extern "C"

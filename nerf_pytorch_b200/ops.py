@@ -1082,6 +1082,29 @@ def baked_max_weights(box: Grid, brick_map, values, use_viewdirs: bool, rays, ma
     return max_w
 
 
+def baked_lattice_count(box: Grid, brick_map, bricks, count=None):
+    """int64[1] on the device: P, the lattice points with a copy in an active brick (include/nerfb200.h "baked fields:
+    regularisers").  ``bricks`` is int32[n_active]."""
+    if count is None:
+        count = torch.empty(1, dtype=torch.int64, device=bricks.device)
+    _lib.check(_lib.load().nerfb200_baked_lattice_count(C.byref(box), _ptr(brick_map), _ptr(bricks), bricks.shape[0],
+                                                        _ptr(count), _stream()), "baked_lattice_count")
+    return count
+
+
+def baked_regularizer(box: Grid, brick_map, bricks, values, count, tv_sigma, tv_sh, sparsity, d=None, partials=None):
+    """Adds the regularisers' gradient into ``d`` (the layout of ``values``; None: not formed) and writes their fp64
+    per-slot value partials into ``partials`` (fp64[n_active]; None: not formed), P read from ``count``
+    (``baked_lattice_count``) on the device."""
+    if partials is not None and partials.dtype != torch.float64:
+        raise RuntimeError("nerfb200: baked_regularizer partials must be fp64")
+    pp = None if partials is None else _ptr(partials.view(torch.int64))  # _ptr takes no fp64; the bits are the same
+    _lib.check(_lib.load().nerfb200_baked_regularizer(C.byref(box), _ptr(brick_map), _ptr(bricks), values.shape[0],
+                                                      _ptr(values), _ptr(count), float(tv_sigma), float(tv_sh),
+                                                      float(sparsity), _ptr(d), pp, _stream()), "baked_regularizer")
+    return d, partials
+
+
 def baked_adam_step_dev(values, g, m, v, step_dev, lr_sigma, lr_sh, lr_decay=None, lr_decay_factor=0.1, beta1=0.9,
                         beta2=0.999, eps=1e-8):
     """``adam_step_dev`` over baked values: sigma_raw at ``lr_sigma``, the SH coefficients at ``lr_sh``."""

@@ -1,0 +1,457 @@
+"""GPU: the baked-field regularisers (csrc/baked.cu baked_count_kernel / baked_reg_kernel; nb.baked_regularizer,
+BakedFieldTrainer's tv_sigma / tv_sh / sparsity; include/nerfb200.h "baked fields: regularisers").
+
+  1. value and gradient against fp64: an fp64 dense (res + 1)^3 lattice read at each point's canonical copy, the edge
+     and point masks of a numpy restatement of the header's rules, L by torch autograd and dL/dpoint gathered at every stored copy; synthetic
+     fields at res 16, (24, 20, 28), 13 and 13 with half the bricks inactive, with and without view directions, each
+     weight alone and all three together, and a lego bake;
+  2. copies and channels: the kernel's gradient is bit-equal across copies, also on a field whose copies differ; after
+     regularised trainer steps and after torch.optim.Adam steps on mse + baked_regularizer every lattice point's copies
+     are bit-equal and channels 28 .. 31 are untouched;
+  3. no change when off: with every weight 0 a trainer step issues the unregularised step's launches, one more with a
+     weight set;
+  4. prune: BakedFieldTrainer.prune recounts P, checked against the restatement;
+  5. effect on lego A0 at 256^3 over a 128^3 grid of the fine network, 40 + 4 poses, 2048 rays per step: sparsity leaves
+     more transparent bricks, TV lowers the field's TV, and held-out PSNR with the chosen sparsity weight costs at most
+     0.1 dB against plain fine-tuning (REG_* below).
+
+Measured on an H100 80GB HBM3 at 700 W: the value's relative error (the fp64 sum of the partials against the oracle's
+fp64 L) is at most 3.7e-16, and the gradient's error per channel group (max |d - d64| over the group's max |d64|,
+channel 0 and channels 1 .. 27) at most 2.0e-7 (synthetic fields; 8.5e-8 on the lego bake), against bars of 1e-12 and
+1e-6.  The file runs in about 25 s."""
+import math
+
+import numpy as np
+import pytest
+import torch
+
+from helpers import bits_equal, load_weights
+
+pytestmark = pytest.mark.gpu
+
+LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
+LEGO_CAM = (48, 48, 66.7)
+
+VALUE_BAR = 1e-12
+GRAD_BAR = 1e-6
+
+
+def report(what, ctx, value):
+    print(f"[baked-reg] {what} {ctx}: {value}")
+
+
+def _model(coarse=False):
+    import nerf_pytorch_b200 as nb
+
+    w = load_weights("lego_lowres")
+    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
+                             num_encoding_fn_dir=4)
+    m.load_state_dict(w[0 if coarse else 1])
+    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4)
+
+
+def _bake(res, grid_res=None):
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200.occupancy import OccupancyGrid
+
+    m, epf, edf = _model()
+    grid = OccupancyGrid.full(LEGO_BOX, 8) if grid_res is None else \
+        OccupancyGrid.from_models([m], epf, LEGO_BOX, grid_res, encode_direction_fn=edf)
+    return nb.bake(m, epf, edf, bounds=LEGO_BOX, resolution=res, grid=grid)
+
+
+def _lattice_index(field):
+    """int64 [n_active, 729]: the linear lattice index (x fastest over res + 1 points per axis) each stored value holds."""
+    res = torch.tensor(field.resolution, device="cuda")
+    nb_ = (res + 7) // 8
+    br = field.bricks.long()
+    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)  # [n, 3]
+    p = torch.arange(729, device="cuda")
+    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)  # [729, 3]
+    q = torch.minimum(b[:, None] * 8 + l[None], res)
+    return (q[..., 2] * (res[1] + 1) + q[..., 1]) * (res[0] + 1) + q[..., 0]
+
+
+def _canonical_rows(field, idx):
+    """int64 [(res + 1)^3]: the stored row (slot * 729 + point) of each lattice point's canonical copy, its first copy in
+    the tie's order (z outer, then y, then x; per axis the lower brick's l = 8 before the upper brick's l = 0, and on the
+    upper face l ascending), -1 where no active brick holds the point."""
+    res = torch.tensor(field.resolution, device="cuda")
+    nb_ = (res + 7) // 8
+    br = field.bricks.long()
+    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)
+    p = torch.arange(729, device="cuda")
+    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)[None].expand(b.shape[0], 729, 3)
+    q = torch.minimum(b[:, None] * 8 + l, res)
+    e = torch.where(q == res, l - (res - 8 * (nb_ - 1)), torch.where((q > 0) & (q % 8 == 0) & (l == 0), 1, 0))
+    key = (e[..., 2] * 9 + e[..., 1]) * 9 + e[..., 0]
+    n = key.numel()
+    comb = key.reshape(-1) * n + torch.arange(n, device="cuda")
+    pts = int((res + 1).prod())
+    best = torch.full((pts,), -1, dtype=torch.int64, device="cuda")
+    best.scatter_reduce_(0, idx.reshape(-1), comb, reduce="amin", include_self=False)
+    return torch.where(best >= 0, best % n, -1)
+
+
+def _copies_bit_equal(x, idx):
+    """Every copy of every lattice point holds the same bits in all 32 channels."""
+    flat = idx.reshape(-1)
+    bits = x.reshape(-1, 32).contiguous().view(torch.int32)
+    first = torch.full((int(flat.max()) + 1,), -1, dtype=torch.int64, device=x.device)
+    first.scatter_reduce_(0, flat, torch.arange(flat.numel(), device=x.device), reduce="amin", include_self=False)
+    return bool((bits == bits[first[flat]]).all())
+
+
+def _synthetic(res, *, viewdirs=True, active=1.0, sigma=(-4.0, 8.0), seed=0, box=((-1.0,) * 3, (1.0,) * 3)):
+    """A field with random values per lattice point (every copy of a point the same bits), on a random subset of
+    bricks: sigma_raw uniform in ``sigma``, coefficients normal with std 0.7 (coefficients 1 .. 8 zero without view
+    directions, as a bake writes them)."""
+    import nerf_pytorch_b200 as nb
+
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    nb_ = [-(-r // 8) for r in res]
+    n_bricks = nb_[0] * nb_[1] * nb_[2]
+    keep = torch.rand(n_bricks, generator=g, device="cuda") < active
+    keep[0] = True
+    brick_map = torch.where(keep, torch.cumsum(keep.int(), 0) - 1, -1).int()
+    bricks = torch.nonzero(keep).reshape(-1).int()
+    pts = (res[0] + 1) * (res[1] + 1) * (res[2] + 1)
+    dense = torch.zeros(pts, 32, device="cuda")
+    dense[:, 0] = sigma[0] + (sigma[1] - sigma[0]) * torch.rand(pts, generator=g, device="cuda")
+    dense[:, 1:28] = 0.7 * torch.randn(pts, 27, generator=g, device="cuda")
+    if not viewdirs:
+        coef = dense[:, 1:28].reshape(pts, 3, 9).clone()
+        coef[:, :, 1:] = 0
+        dense[:, 1:28] = coef.reshape(pts, 27)
+    f = nb.BakedField(box, res, brick_map, bricks, torch.empty(bricks.numel(), 729, 32, device="cuda"), viewdirs)
+    f.values = dense[_lattice_index(f)].contiguous()
+    return f
+
+
+def _axis_bricks(res, nb, c=None):
+    """bool [res + 1, nb]: the bricks of lattice index q's copy list along one axis (include/nerfb200.h "baked fields:
+    gradients and fine-tuning", Tie): {nb - 1} at q = res, {q / 8 - 1, q / 8} at a positive multiple of 8 below res, {q
+    // 8} otherwise.  With ``c`` set (the edge axis) instead the one brick q // 8 for q < res and none at q = res."""
+    q = np.arange(res + 1)
+    m = np.zeros((res + 1, nb), dtype=bool)
+    if c is not None:
+        m[q[:-1], q[:-1] // 8] = True
+        return m
+    inner = q < res
+    m[q[inner], q[inner] // 8] = True
+    face = inner & (q > 0) & (q % 8 == 0)
+    m[q[face], q[face] // 8 - 1] = True
+    m[res, nb - 1] = True
+    return m
+
+
+def _baked_lattice(res, active):
+    """The regularisers' lattice (include/nerfb200.h "baked fields: regularisers") restated in numpy: (points, edges)
+    with points bool [res_2 + 1, res_1 + 1, res_0 + 1] (the lattice points with a copy in an active brick) and edges a
+    list over the axes c = 0, 1, 2 (x, y, z) of bool arrays of that shape, edges[c][q] for the edge (q, q + e_c): brick q_c
+    // 8 along c and any brick of q's copy list along the other axes.  ``active`` is bool [nb_2, nb_1, nb_0]."""
+    res = tuple(int(r) for r in res)
+    nb = [-(-r // 8) for r in res]
+    a = np.asarray(active).astype(np.int64)
+
+    def spread(mx, my, mz):  # [qz, qy, qx] = any over bricks of mz[qz, bz] my[qy, by] mx[qx, bx] active[bz, by, bx]
+        t = np.tensordot(a, mx.astype(np.int64), axes=([2], [1]))       # [bz, by, qx]
+        t = np.tensordot(t, my.astype(np.int64), axes=([1], [1]))       # [bz, qx, qy]
+        t = np.tensordot(t, mz.astype(np.int64), axes=([0], [1]))       # [qx, qy, qz]
+        return t.transpose(2, 1, 0) > 0
+
+    copies = [_axis_bricks(res[c], nb[c]) for c in range(3)]
+    points = spread(*copies)
+    edges = []
+    for c in range(3):
+        m = list(copies)
+        m[c] = _axis_bricks(res[c], nb[c], c)
+        edges.append(spread(*m))
+    return points, edges
+
+def _restated(field):
+    """(points, edges) of _baked_lattice for the field's active bricks, as torch bool tensors on the device."""
+    res = field.resolution
+    nb_ = [-(-r // 8) for r in res]
+    active = (field.brick_map >= 0).view(nb_[2], nb_[1], nb_[0]).cpu().numpy()
+    points, edges = _baked_lattice(res, active)
+    return torch.from_numpy(points).cuda(), [torch.from_numpy(e).cuda() for e in edges]
+
+
+def _oracle(field, lam):
+    """(L in fp64, dL/dpoint fp64 [n_active, 729, 28] at every stored copy, P) by autograd over the dense lattice."""
+    res = field.resolution
+    idx = _lattice_index(field)
+    rows = _canonical_rows(field, idx)
+    points, edges = _restated(field)
+    present = rows >= 0
+    assert bool((present.view(points.shape) == points).all())  # the restated points are the stored ones
+    X = torch.zeros(rows.numel(), 28, dtype=torch.float64, device="cuda")
+    X[present] = field.values.detach().reshape(-1, 32)[rows[present], :28].double()
+    X.requires_grad_()
+    X3 = X.view(res[2] + 1, res[1] + 1, res[0] + 1, 28)
+    P = int(points.sum())
+    ts, th = X.new_zeros(()), X.new_zeros(())
+    for c in range(3):
+        ax, n = 2 - c, res[c] + 1
+        diff = X3.narrow(ax, 1, n - 1) - X3.narrow(ax, 0, n - 1)
+        m = edges[c].narrow(ax, 0, n - 1)
+        ts = ts + (diff[..., 0] ** 2)[m].sum()
+        th = th + (diff[..., 1:] ** 2)[m].sum()
+    s = torch.clamp(X[:, 0], min=0.0)
+    sp = torch.log1p(2.0 * s * s)[points.reshape(-1)].sum()
+    L = (lam[0] * ts + lam[1] * th + lam[2] * sp) / P
+    L.backward()
+    return L.detach(), X.grad[idx], P
+
+
+def _kernel(field, lam, d=None):
+    """(the fp64 sum of the kernel's partials, the fp32 loss, its gradient added into zeros, P) for ``lam``."""
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200 import ops
+
+    box = field.box()
+    count = ops.baked_lattice_count(box, field.brick_map, field.bricks)
+    partials = torch.empty(field.n_active, dtype=torch.float64, device="cuda")
+    ops.baked_regularizer(box, field.brick_map, field.bricks, field.values.detach(), count, *lam, partials=partials)
+    d = torch.zeros_like(field.values) if d is None else d
+    ops.baked_regularizer(box, field.brick_map, field.bricks, field.values.detach(), count, *lam, d=d)
+    loss = nb.baked_regularizer(field, tv_sigma=lam[0], tv_sh=lam[1], sparsity=lam[2])
+    return partials.sum(), loss, d, int(count)
+
+
+def _check(field, lam, ctx):
+    """Asserts value and gradient against the oracle and the copies' bits; returns (value error, gradient error)."""
+    L64, g64, P = _oracle(field, lam)
+    v, loss, d, Pk = _kernel(field, lam)
+    assert Pk == P, (ctx, Pk, P)
+    assert bits_equal(loss, v.float()), ctx  # the fp64 sum rounded once
+    ev = abs(v.item() - L64.item()) / max(abs(L64.item()), 1e-300)
+    assert L64.item() > 0 and ev <= VALUE_BAR, (ctx, ev)
+    assert (d[..., 28:] == 0).all() and torch.isfinite(d).all()
+    idx = _lattice_index(field)
+    assert _copies_bit_equal(d, idx), ctx
+    eg = 0.0
+    for sl in (slice(0, 1), slice(1, 28)):
+        want, got = g64[..., sl], d[..., sl].double()
+        top = want.abs().max().item()
+        if top == 0.0:
+            assert (got == 0).all(), ctx
+            continue
+        eg = max(eg, (got - want).abs().max().item() / top)
+    report("value / gradient error", ctx, (ev, eg))
+    assert eg <= GRAD_BAR, (ctx, eg)
+    return ev, eg
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 1. value and gradient against fp64
+# ------------------------------------------------------------------------------------------------------------------------
+LAMS = {"tv_sigma": (1.0, 0.0, 0.0), "tv_sh": (0.0, 1.0, 0.0), "sparsity": (0.0, 0.0, 1.0), "all": (0.3, 2.0, 0.7)}
+FIELDS = {"res16": dict(res=(16, 16, 16), seed=1), "res24_20_28": dict(res=(24, 20, 28), seed=2),
+          "res13": dict(res=(13, 13, 13), seed=3), "res13_half": dict(res=(13, 13, 13), active=0.5, seed=4),
+          "res24_20_28_half": dict(res=(24, 20, 28), active=0.5, seed=5)}
+
+
+@pytest.mark.parametrize("viewdirs", [True, False])
+@pytest.mark.parametrize("fkind", list(FIELDS))
+def test_value_and_gradient_match_fp64_on_synthetic_fields(fkind, viewdirs):
+    kw = dict(FIELDS[fkind])
+    f = _synthetic(kw.pop("res"), viewdirs=viewdirs, **kw)
+    if "half" in fkind:
+        assert 0 < f.n_active < f.brick_map.numel()
+    for name, lam in LAMS.items():
+        _check(f, lam, (fkind, viewdirs, name))
+
+
+def test_value_and_gradient_match_fp64_on_a_lego_bake():
+    f = _bake((24, 20, 28), grid_res=32)
+    assert 0 < f.n_active < f.brick_map.numel()
+    for name, lam in LAMS.items():
+        _check(f, lam, ("lego", name))
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 2. copies and channels
+# ------------------------------------------------------------------------------------------------------------------------
+def test_gradient_reads_canonical_copies_when_copies_differ():
+    """On a field whose non-canonical copies hold other values, the kernel's gradient and value are those of the
+    canonical copies (the oracle reads nothing else), and every copy gets the same bits."""
+    f = _synthetic((20, 17, 12), active=0.6, seed=9)
+    idx = _lattice_index(f)
+    rows = _canonical_rows(f, idx)
+    canon = torch.zeros(f.values.shape[:2], dtype=torch.bool, device="cuda").view(-1)
+    canon[rows[rows >= 0]] = True
+    noise = torch.randn(f.values.shape, generator=torch.Generator(device="cuda").manual_seed(3), device="cuda")
+    f.values = torch.where(canon.view(-1, 729, 1), f.values, f.values + noise).contiguous()
+    assert not _copies_bit_equal(f.values, idx)
+    _check(f, LAMS["all"], "copies differ")
+
+
+def _sphere_poses(n, radius=4.0, phis=(-30.0, -45.0, -15.0)):
+    from oracle import nerf_oracle as O
+
+    return torch.stack([O.pose_spherical(360.0 * i / n + 7.0 * (i % len(phis)), phis[i % len(phis)], radius)
+                        for i in range(n)])
+
+
+def _targets(poses):
+    import nerf_pytorch_b200 as nb
+    from oracle import nerf_oracle as O
+
+    m, epf, edf = _model()
+    mc = _model(coarse=True)[0]
+    H, W, focal = LEGO_CAM
+    opts = O.make_options(no_ndc=True, near=2.0, far=6.0, num_coarse=64, num_fine=128, perturb=False,
+                          radiance_field_noise_std=0.0)
+    with torch.no_grad():
+        imgs = torch.stack([nb.render_image(H, W, focal, p, mc, m, opts, encode_position_fn=epf,
+                                            encode_direction_fn=edf, impl=1)[3] for p in poses])
+    return imgs.contiguous(), opts
+
+
+def _camera_rays(pose):
+    from nerf_pytorch_b200 import ops
+
+    H, W, focal = LEGO_CAM
+    return ops.gen_rays(pose, H, W, focal, None, "cuda", ndc=False, near=2.0, far=6.0, use_viewdirs=True)
+
+
+def test_copies_stay_bit_equal_under_regularised_trainer_and_torch_adam():
+    import nerf_pytorch_b200 as nb
+
+    f = _bake((24, 20, 28), grid_res=32)
+    idx = _lattice_index(f)
+    poses = _sphere_poses(6)
+    imgs, opts = _targets(poses)
+    t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=2048, seed=3, tv_sigma=1e-3,
+                             tv_sh=1e-2, sparsity=1e-3)
+    before = f.values.clone()
+    t.step(20)
+    assert not bits_equal(before, f.values) and _copies_bit_equal(f.values, idx)
+    assert bits_equal(before[..., 28:], f.values[..., 28:])
+    g = _bake((24, 20, 28), grid_res=32)
+    g.values.requires_grad_()
+    before = g.values.detach().clone()
+    opt = torch.optim.Adam([g.values], lr=1e-2)
+    for i in range(20):
+        rgb, *_ = nb.render_baked_rays(g, _camera_rays(poses[i % 6]))
+        loss = ((rgb - imgs[i % 6].reshape(-1, 3)) ** 2).mean() + nb.baked_regularizer(g, tv_sigma=1e-3, tv_sh=1e-2,
+                                                                                          sparsity=1e-3)
+        opt.zero_grad()
+        loss.backward()
+        assert _copies_bit_equal(g.values.grad, idx)
+        opt.step()
+    assert _copies_bit_equal(g.values.detach(), idx)
+    assert bits_equal(before[..., 28:], g.values.detach()[..., 28:])
+
+
+def test_autograd_gradient_is_the_kernel_gradient_times_the_upstream_scalar():
+    import nerf_pytorch_b200 as nb
+
+    f = _synthetic((16, 12, 20), active=0.6, seed=6)
+    lam = LAMS["all"]
+    _, _, d, _ = _kernel(f, lam)
+    f.values.requires_grad_()
+    loss = nb.baked_regularizer(f, tv_sigma=lam[0], tv_sh=lam[1], sparsity=lam[2])
+    (2.5 * loss).backward()
+    assert bits_equal(f.values.grad, d * 2.5)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 3. no change when off
+# ------------------------------------------------------------------------------------------------------------------------
+def test_launch_count_unchanged_when_off_and_one_more_when_on():
+    import nerf_pytorch_b200 as nb
+    from nerf_pytorch_b200 import ops
+
+    poses = _sphere_poses(4)
+    imgs, opts = _targets(poses)
+    counts, fields = {}, {}
+    for name, kw in (("plain", {}), ("zero", dict(tv_sigma=0.0, tv_sh=0.0, sparsity=0.0)), ("tv", dict(tv_sigma=1e-3)),
+                     ("all", dict(tv_sigma=1e-3, tv_sh=1e-3, sparsity=1e-3))):
+        f = _bake((24, 20, 28), grid_res=32)
+        t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=1024, seed=4, **kw)
+        t.step(1)
+        n0 = ops.launch_count()
+        t.step(1)
+        counts[name] = ops.launch_count() - n0
+        fields[name] = (f.values.clone(), t.loss.clone())
+    report("launches per step", "", counts)
+    assert counts["zero"] == counts["plain"] and counts["tv"] == counts["plain"] + 1
+    assert counts["all"] == counts["plain"] + 1
+    assert bits_equal(fields["zero"][1], fields["plain"][1])  # the same loss bits after two steps
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 4. prune
+# ------------------------------------------------------------------------------------------------------------------------
+def test_prune_recounts_lattice_points():
+    import nerf_pytorch_b200 as nb
+
+    f = _bake((40, 40, 40))  # every brick active: the box's corners are transparent
+    poses = _sphere_poses(4)
+    imgs, opts = _targets(poses)
+    t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=1024, seed=5, tv_sigma=1e-3,
+                             sparsity=1e-3)
+    assert int(t._count) == int(_restated(f)[0].sum()) == 41 ** 3
+    t.step(3)
+    keep = ~nb.baked_transparent_bricks(f)
+    assert 0 < int(keep.sum()) < f.n_active
+    t.prune(keep)
+    P = int(_restated(f)[0].sum())
+    assert int(t._count) == P < 41 ** 3
+    t.step(5)  # regularised steps at the recounted P
+    assert _copies_bit_equal(f.values, _lattice_index(f))
+    _check(f, t.reg, "pruned")
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 5. effect on lego A0 at 256^3
+# ------------------------------------------------------------------------------------------------------------------------
+# held-out PSNR (dB) against render_image of lego A0 baked at 256^3 over a 128^3 grid of the fine network after
+# FT_STEPS trainer steps, 2048 rays per step, 40 training and 4 held-out poses.  REG_SPARSITY is the best weight of the
+# sweep in tools/baked_reg_time.py (DESIGN §4), measured on an H100 80GB HBM3 at 700 W: 30.895 dB against 30.856 dB
+# unregularised after 300 steps, with 4 057 transparent bricks of 6 067 against 3 919.  That gain is within the
+# run-to-run spread of plain fine-tuning (0.01 dB), and no TV weight of the sweep beat plain fine-tuning, so the test
+# asks that the chosen weight cost at most 0.1 dB.  REG_TV_SIGMA is the sweep's middle TV weight, which lowers the
+# field's TV by 29 % (and costs 1 dB).
+FT_STEPS = 300
+REG_SPARSITY = 1e-3
+REG_TV_SIGMA = 1e-5
+REG_GAIN_MEASURED = 0.04
+REG_GAIN_BAR = -0.1  # regularised minus plain held-out PSNR: at most a 0.1 dB loss
+
+
+def _psnr(a, b):
+    return -10.0 * math.log10(max(torch.mean((a - b) ** 2).item(), 1e-12))
+
+
+def _heldout_psnr(field, poses, imgs):
+    import nerf_pytorch_b200 as nb
+
+    with torch.no_grad():
+        return sum(_psnr(nb.render_baked_rays(field, _camera_rays(p))[0], im.reshape(-1, 3))
+                   for p, im in zip(poses, imgs)) / len(poses)
+
+
+def test_regularisers_on_lego_256():
+    import nerf_pytorch_b200 as nb
+
+    poses = _sphere_poses(44)
+    imgs, opts = _targets(poses)
+    held = [5, 16, 27, 38]
+    train = [i for i in range(44) if i not in held]
+    res = {}
+    for name, kw in (("plain", {}), ("sparsity", dict(sparsity=REG_SPARSITY)), ("tv", dict(tv_sigma=REG_TV_SIGMA))):
+        f = _bake(256, grid_res=128)
+        t = nb.BakedFieldTrainer(f, imgs[train].contiguous(), poses[train].cuda(), LEGO_CAM[2], opts,
+                                 rays_per_step=2048, seed=1, **kw)
+        t.step(FT_STEPS)
+        tv = nb.baked_regularizer(f, tv_sigma=1.0, tv_sh=1.0).item()
+        res[name] = (_heldout_psnr(f, poses[held], imgs[held]), int(nb.baked_transparent_bricks(f).sum()), tv)
+        del t, f
+    report("held-out PSNR, transparent bricks, TV", FT_STEPS, res)
+    assert res["sparsity"][1] > res["plain"][1]
+    assert res["tv"][2] < res["plain"][2]
+    assert res["sparsity"][0] - res["plain"][0] >= REG_GAIN_BAR, res
