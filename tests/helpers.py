@@ -1,6 +1,7 @@
 """Shared test plumbing: golden-case loading, oracle drivers, error metrics.  (tests/ may use oracle/.)"""
 from __future__ import annotations
 
+import math
 import os
 import sys
 
@@ -140,6 +141,96 @@ def build_models(c: Case):
     return mc, mf, epf, edf
 
 
+# ------------------------------------------------------------------------------------------------------------------------
+# the shipped low-res networks and their scenes
+# ------------------------------------------------------------------------------------------------------------------------
+LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
+FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
+# (H, W, focal): lego at pose_spherical(30, -30, 4), near 2, far 6; fern forward-facing at the identity in NDC, near 0,
+# far 1
+LEGO_CAM = (48, 48, 66.7)
+FERN_CAM = (42, 56, 45.3)
+
+
+def shipped_models(kind):
+    """(coarse, fine, encode_position_fn, encode_direction_fn) of the shipped low-res "lego" or "fern" networks
+    (golden/weights_<kind>_lowres.npz): A0, 4 x 128 skip 4, 10 (lego) or 6 (fern) position bands and 4 direction bands,
+    the models on the GPU."""
+    import nerf_pytorch_b200 as nb
+
+    l_xyz = 10 if kind == "lego" else 6
+    out = []
+    for sd in load_weights(f"{kind}_lowres"):
+        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
+                                 num_encoding_fn_dir=4)
+        m.load_state_dict(sd)
+        out.append(m.cuda())
+    return out[0], out[1], nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
+
+
+def scene_pose(kind):
+    """A scene's camera pose: "spherical" is pose_spherical(30, -30, 4), "eye" the identity."""
+    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
+
+
+def scene_options(kind):
+    """Reference options of a deterministic render_image of the shipped scene: 64 coarse and 128 fine samples."""
+    ndc = kind == "fern"
+    return O.make_options(no_ndc=not ndc, near=0.0 if ndc else 2.0, far=1.0 if ndc else 6.0, num_coarse=64,
+                          num_fine=128, perturb=False, radiance_field_noise_std=0.0)
+
+
+def camera_rays(kind, pose=None, viewdirs=True):
+    """The ray rows of the scene's camera (LEGO_CAM, FERN_CAM) at ``pose``, by default the scene's own."""
+    from nerf_pytorch_b200 import ops
+
+    if kind == "fern":
+        H, W, focal = FERN_CAM
+        return ops.gen_rays(torch.eye(4) if pose is None else pose, H, W, focal, None, "cuda", ndc=True, near=0.0,
+                            far=1.0, use_viewdirs=viewdirs)
+    H, W, focal = LEGO_CAM
+    pose = O.pose_spherical(30.0, -30.0, 4.0) if pose is None else pose
+    return ops.gen_rays(pose, H, W, focal, None, "cuda", ndc=False, near=2.0, far=6.0, use_viewdirs=viewdirs)
+
+
+def sphere_poses(n, radius=4.0, phis=(-30.0, -45.0, -15.0), offset=7.0):
+    """n poses around the lego scene: azimuth 360 i / n + offset (i mod len(phis)), elevation phis[i mod len(phis)]."""
+    return torch.stack([O.pose_spherical(360.0 * i / n + offset * (i % len(phis)), phis[i % len(phis)], radius)
+                        for i in range(n)])
+
+
+def targets(kind, poses):
+    """(fine rgb images [n, H, W, 3] of render_image of the shipped networks at ``poses``, scene_options(kind))."""
+    import nerf_pytorch_b200 as nb
+
+    mc, mf, epf, edf = shipped_models(kind)
+    H, W, focal = FERN_CAM if kind == "fern" else LEGO_CAM
+    opts = scene_options(kind)
+    with torch.no_grad():
+        imgs = torch.stack([nb.render_image(H, W, focal, p, mc, mf, opts, encode_position_fn=epf,
+                                            encode_direction_fn=edf, impl=1)[3] for p in poses])
+    return imgs.contiguous(), opts
+
+
+def psnr32(a, b):
+    """PSNR (dB) from the fp32 mean squared error, at most 120 dB (the error clamped at 1e-12)."""
+    return -10.0 * math.log10(max(torch.mean((a - b) ** 2).item(), 1e-12))
+
+
+def psnr64(a, b):
+    """PSNR (dB) from the fp64 mean squared error; inf when a and b are equal."""
+    mse = (a.double() - b.double()).pow(2).mean().item()
+    return math.inf if mse == 0 else -10.0 * math.log10(mse)
+
+
+def ws_view(ws, layout, name, n, s, cols):
+    """The fp32 section ``name`` of a render workspace (ops.render_workspace_layout) as [n, s, cols], or [n, s] for one
+    column."""
+    off = layout[name] // 4
+    t = ws.view(torch.float32)[off: off + n * s * cols]
+    return t.view(n, s, cols) if cols > 1 else t.view(n, s)
+
+
 def composite64(raw, z, dirs, noise_std=0.0, white_background=False, noise=None, raw64=None):
     """fp64 O.volume_render_radiance_field of the fp32 samples raw [.., S, 4], z [.., S], dirs [.., 3] with unit normals
     noise [.., S]: (rgb, disp, acc, weights, depth), differentiable with respect to raw64 (default raw.double()).
@@ -248,8 +339,6 @@ def baked_render64(field, rays, white):
     The slab terms go through fmin / fmax as the kernel's fminf / fmaxf (a NaN term drops out); an axis with d = +-0
     leaves the interval as it is when lo <= o < hi and empties the ray otherwise.  A ray is live when t_a < t_b and dt is
     positive, finite and (t_b - t_a) / dt < 2^24."""
-    import math
-
     f32 = torch.float32
     dev = rays.device
     lo = torch.tensor(field.bounds[0], dtype=f32, device=dev)
@@ -314,6 +403,175 @@ def baked_render64(field, rays, white):
     depth = (w * t.double()).sum(-1)
     out_rgb = (w[..., None] * rgb).sum(1) + ((1 - acc)[:, None] if white else 0)
     return out_rgb, acc, depth, 1 / torch.clamp(depth / acc, min=1e-10)
+
+
+def bake_scene(kind, res, grid_res=None, grid_from="fine"):
+    """nb.bake of a scene's network over its box at ``res``.  "lego" and "fern" bake the shipped fine network (LEGO_BOX,
+    FERN_BOX); "noview" a coarse-only network without view directions at torch's init under seed 7, over [-1, 1]^3.
+    Bricks: every one with grid_res None, else those of OccupancyGrid.from_models at grid_res over the fine network
+    (grid_from "fine") or over the coarse and fine networks ("both")."""
+    import nerf_pytorch_b200 as nb
+
+    if kind == "noview":
+        torch.manual_seed(7)
+        mc, mf = None, nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
+                                            use_viewdirs=False).cuda()
+        epf, edf, box = nb.get_embedding_function(10), None, ((-1.0,) * 3, (1.0,) * 3)
+    else:
+        mc, mf, epf, edf = shipped_models(kind)
+        box = FERN_BOX if kind == "fern" else LEGO_BOX
+    nets = {"fine": [mf], "both": [mc, mf]}[grid_from]
+    grid = nb.OccupancyGrid.full(box, 8) if grid_res is None else \
+        nb.OccupancyGrid.from_models(nets, epf, box, grid_res, encode_direction_fn=edf)
+    return nb.bake(mf, epf, edf, bounds=box, resolution=res, grid=grid)
+
+
+def lattice_index(field):
+    """int64 [n_active, 729]: the linear lattice index (x fastest over res + 1 points per axis) each stored value holds."""
+    res = torch.tensor(field.resolution, device="cuda")
+    nb_ = (res + 7) // 8
+    br = field.bricks.long()
+    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)  # [n, 3]
+    p = torch.arange(729, device="cuda")
+    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)  # [729, 3]
+    q = torch.minimum(b[:, None] * 8 + l[None], res)
+    return (q[..., 2] * (res[1] + 1) + q[..., 1]) * (res[0] + 1) + q[..., 0]
+
+
+def copies_bit_equal(x, idx):
+    """Every copy of every lattice point (idx: lattice_index) holds the same bits in all 32 channels."""
+    flat = idx.reshape(-1)
+    bits = x.reshape(-1, 32).contiguous().view(torch.int32)
+    first = torch.full((int(flat.max()) + 1,), -1, dtype=torch.int64, device=x.device)
+    first.scatter_reduce_(0, flat, torch.arange(flat.numel(), device=x.device), reduce="amin", include_self=False)
+    return bool((bits == bits[first[flat]]).all())
+
+
+def synthetic_field(res, *, viewdirs=True, active=1.0, sigma=(-4.0, 8.0), seed=0, box=((-1.0,) * 3, (1.0,) * 3)):
+    """A field with random values per lattice point (every copy of a point the same bits), on a random subset of
+    bricks: sigma_raw uniform in ``sigma``, coefficients normal with std 0.7 (coefficients 1 .. 8 zero without view
+    directions, as a bake writes them)."""
+    import nerf_pytorch_b200 as nb
+
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    nb_ = [-(-r // 8) for r in res]
+    keep = torch.rand(nb_[0] * nb_[1] * nb_[2], generator=g, device="cuda") < active
+    keep[0] = True
+    brick_map = torch.where(keep, torch.cumsum(keep.int(), 0) - 1, -1).int()
+    bricks = torch.nonzero(keep).reshape(-1).int()
+    pts = (res[0] + 1) * (res[1] + 1) * (res[2] + 1)
+    dense = torch.zeros(pts, 32, device="cuda")
+    dense[:, 0] = sigma[0] + (sigma[1] - sigma[0]) * torch.rand(pts, generator=g, device="cuda")
+    dense[:, 1:28] = 0.7 * torch.randn(pts, 27, generator=g, device="cuda")
+    if not viewdirs:
+        coef = dense[:, 1:28].reshape(pts, 3, 9).clone()
+        coef[:, :, 1:] = 0
+        dense[:, 1:28] = coef.reshape(pts, 27)
+    f = nb.BakedField(box, res, brick_map, bricks, torch.empty(bricks.numel(), 729, 32, device="cuda"), viewdirs)
+    f.values = dense[lattice_index(f)].contiguous()
+    return f
+
+
+def ray_rows(o, d, viewdirs=True, near=0.0, far=6.0):
+    """Ray rows (o, d, near, far[, unit d]) on the GPU; near and far are numbers or per-ray tensors."""
+    n = o.shape[0]
+    near = torch.full((n, 1), near, device="cuda") if not torch.is_tensor(near) else near.view(n, 1)
+    far = torch.full((n, 1), far, device="cuda") if not torch.is_tensor(far) else far.view(n, 1)
+    cols = [o, d, near, far]
+    if viewdirs:
+        cols.append(d / d.norm(dim=1, keepdim=True))
+    return torch.cat(cols, 1).contiguous()
+
+
+def random_rays(n, seed, viewdirs=True, lo=-1.0, hi=1.0, misses=False):
+    """Rays from a sphere of radius 3 towards random points of the box [lo, hi]^3, near 0, far 6; with ``misses`` every
+    7th turned away from the box."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    o = torch.randn(n, 3, generator=g, device="cuda")
+    o = 3.0 * o / o.norm(dim=1, keepdim=True)
+    d = lo + (hi - lo) * torch.rand(n, 3, generator=g, device="cuda") - o
+    if misses:
+        d[::7] = -d[::7]
+    return ray_rows(o, d, viewdirs)
+
+
+def edge_rays(field, viewdirs=True):
+    """Axis-parallel rays in brick-face planes (and on brick edges), and diagonals through brick corners."""
+    lo = torch.tensor(field.bounds[0], device="cuda")
+    hi = torch.tensor(field.bounds[1], device="cuda")
+    res = torch.tensor(field.resolution, device="cuda", dtype=torch.float32)
+    h = (hi - lo) / res
+    o, d = [], []
+    for a in range(3):  # along axis a, in the plane of the first brick face of axis b, at several offsets on axis c
+        b, c = (a + 1) % 3, (a + 2) % 3
+        for k in range(6):
+            p = lo + (hi - lo) * 0.37
+            p[b] = lo[b] + 8 * h[b] if res[b] > 8 else lo[b] + h[b]
+            p[c] = lo[c] + (k / 5.0) * (hi[c] - lo[c]) * 0.99
+            if k == 5:
+                p[c] = lo[c] + 8 * h[c] if res[c] > 8 else lo[c]  # a brick edge
+            p[a] = lo[a] - 1.0
+            dd = torch.zeros(3, device="cuda")
+            dd[a] = 1.0
+            o.append(p.clone())
+            d.append(dd)
+    corner = lo + 8 * h * (res > 8)  # a brick corner point (or the box's lower corner)
+    for s in ([1, 1, 1], [1, -1, 1], [-1, 1, 1], [1, 1, -1]):
+        dd = torch.tensor(s, device="cuda", dtype=torch.float32)
+        o.append(corner - 2.0 * dd)
+        d.append(dd)
+    return ray_rows(torch.stack(o), torch.stack(d), viewdirs)
+
+
+def heldout_psnr(field, poses, imgs):
+    """Mean psnr32 of the baked field's renders at lego-camera ``poses`` against ``imgs``."""
+    import nerf_pytorch_b200 as nb
+
+    with torch.no_grad():
+        return sum(psnr32(nb.render_baked_rays(field, camera_rays("lego", p))[0], im.reshape(-1, 3))
+                   for p, im in zip(poses, imgs)) / len(poses)
+
+
+def axis_bricks(res, nb, c=None):
+    """bool [res + 1, nb]: the bricks of lattice index q's copy list along one axis (include/nerfb200.h "baked fields:
+    gradients and fine-tuning", Tie): {nb - 1} at q = res, {q / 8 - 1, q / 8} at a positive multiple of 8 below res, {q
+    // 8} otherwise.  With ``c`` set (the edge axis) instead the one brick q // 8 for q < res and none at q = res."""
+    q = np.arange(res + 1)
+    m = np.zeros((res + 1, nb), dtype=bool)
+    if c is not None:
+        m[q[:-1], q[:-1] // 8] = True
+        return m
+    inner = q < res
+    m[q[inner], q[inner] // 8] = True
+    face = inner & (q > 0) & (q % 8 == 0)
+    m[q[face], q[face] // 8 - 1] = True
+    m[res, nb - 1] = True
+    return m
+
+
+def baked_lattice(res, active):
+    """The regularisers' lattice (include/nerfb200.h "baked fields: regularisers") restated in numpy: (points, edges)
+    with points bool [res_2 + 1, res_1 + 1, res_0 + 1] (the lattice points with a copy in an active brick) and edges a
+    list over the axes c = 0, 1, 2 (x, y, z) of bool arrays of that shape, edges[c][q] for the edge (q, q + e_c): brick q_c
+    // 8 along c and any brick of q's copy list along the other axes.  ``active`` is bool [nb_2, nb_1, nb_0]."""
+    res = tuple(int(r) for r in res)
+    nb = [-(-r // 8) for r in res]
+    a = np.asarray(active).astype(np.int64)
+
+    def spread(mx, my, mz):  # [qz, qy, qx] = any over bricks of mz[qz, bz] my[qy, by] mx[qx, bx] active[bz, by, bx]
+        t = np.tensordot(a, mx.astype(np.int64), axes=([2], [1]))       # [bz, by, qx]
+        t = np.tensordot(t, my.astype(np.int64), axes=([1], [1]))       # [bz, qx, qy]
+        t = np.tensordot(t, mz.astype(np.int64), axes=([0], [1]))       # [qx, qy, qz]
+        return t.transpose(2, 1, 0) > 0
+
+    copies = [axis_bricks(res[c], nb[c]) for c in range(3)]
+    points = spread(*copies)
+    edges = []
+    for c in range(3):
+        m = list(copies)
+        m[c] = axis_bricks(res[c], nb[c], c)
+        edges.append(spread(*m))
+    return points, edges
 
 
 def bits_equal(a, b):

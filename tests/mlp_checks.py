@@ -113,22 +113,24 @@ H256_SCENES = {
 
 
 def scene_models(scene):
-    """The (coarse, fine) FlexibleNeRFModels of a scene row (H256_SCENES' format) on the GPU."""
+    """The (coarse, fine) FlexibleNeRFModels of a scene row (H256_SCENES' format) on the GPU; "shipped" networks are
+    helpers.shipped_models'."""
     import nerf_pytorch_b200 as nb
-    from helpers import load_weights
+    from helpers import shipped_models
     from nerf_pytorch_b200 import ops
 
     weights, *_, l_xyz, nets, _ = scene
-    shipped = load_weights(weights) if weights else None
+    shipped = shipped_models(weights.removesuffix("_lowres")) if weights else None
     if any(state == "init" for *_, state in nets):
         torch.manual_seed(7)
     out = []
     for i, (layers, hidden, skip, state) in enumerate(nets):
+        if state == "shipped":
+            out.append(shipped[i])
+            continue
         m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=hidden, skip_connect_every=skip,
                                  num_encoding_fn_xyz=l_xyz, num_encoding_fn_dir=4)
-        if state == "shipped":
-            m.load_state_dict(shipped[i])
-        elif state != "init":
+        if state != "init":
             arch = ops.ArchSpec(num_layers=layers, hidden=hidden, skip_every=skip, n_freq_xyz=l_xyz, n_freq_dir=4)
             m.load_state_dict(arch_weights(arch, *state))
         out.append(m.cuda())

@@ -9,45 +9,31 @@
      without view directions and a white background, rays that miss the box; early stopping;
   4. reproducibility, save / load;
   5. quality: PSNR of render_baked against render_image's fine output on lego (256^3, 512^3) and fern."""
-import math
-
 import numpy as np
 import pytest
 import torch
 
-from helpers import COEF_REL, OUT_ABS, baked_render64, bits_equal, load_weights, net_at
+from helpers import (COEF_REL, FERN_BOX, FERN_CAM, LEGO_BOX, LEGO_CAM, OUT_ABS, baked_render64, bits_equal, net_at,
+                     psnr32, scene_pose, shipped_models)
 
 pytestmark = pytest.mark.gpu
-
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
-FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
 
 
 def report(what, ctx, value):
     print(f"[bake] {what} {ctx}: {value}")
 
 
-def _pose(kind):
-    from oracle import nerf_oracle as O
-
-    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
-
-
-def _model(kind, coarse=False):
-    """(model, encode_position_fn, encode_direction_fn, camera (H, W, focal, pose, no_ndc, near, far), box); with
-    ``coarse`` the shipped scenes' coarse network instead of the fine one."""
+def _model(kind):
+    """(model, encode_position_fn, encode_direction_fn, camera (H, W, focal, pose, no_ndc, near, far), box): the shipped
+    scenes' fine network (helpers.shipped_models), or "a1", "a2" and "noview" (coarse-only, no view directions) at
+    torch's init under seed 7 on the lego camera."""
     import nerf_pytorch_b200 as nb
 
-    lego_cam = (48, 48, 66.7, "spherical", True, 2.0, 6.0)
+    lego_cam = (*LEGO_CAM, "spherical", True, 2.0, 6.0)
     if kind in ("lego", "fern"):
-        w = load_weights(f"{kind}_lowres")
-        l_xyz = 10 if kind == "lego" else 6
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(w[0 if coarse else 1])
-        cam = lego_cam if kind == "lego" else (42, 56, 45.3, "eye", False, 0.0, 1.0)
-        return m.cuda(), nb.get_embedding_function(l_xyz), nb.get_embedding_function(4), cam, \
-            LEGO_BOX if kind == "lego" else FERN_BOX
+        _, m, epf, edf = shipped_models(kind)
+        cam = lego_cam if kind == "lego" else (*FERN_CAM, "eye", False, 0.0, 1.0)
+        return m, epf, edf, cam, LEGO_BOX if kind == "lego" else FERN_BOX
     torch.manual_seed(7)
     if kind == "a1":
         m = nb.FlexibleNeRFModel(num_layers=8, hidden_size=128, skip_connect_every=3, num_encoding_fn_xyz=10)
@@ -142,7 +128,7 @@ def test_bricks_are_the_sparse_meshes_and_an_empty_grid_renders_the_background()
         e = nb.bake(m, epf, edf, bounds=box, resolution=40, grid=empty)
         assert e.n_active == 0
         opts = O.make_options(no_ndc=no_ndc, near=near, far=far, white_background=white)
-        rgb, disp, acc = nb.render_baked(e, H, W, focal, _pose(pose), opts)
+        rgb, disp, acc = nb.render_baked(e, H, W, focal, scene_pose(pose), opts)
         assert (acc == 0).all() and (rgb == (1.0 if white else 0.0)).all() and torch.isnan(disp).all()
 
 
@@ -153,7 +139,7 @@ def _rays(cam, use_viewdirs):
     from nerf_pytorch_b200 import ops
 
     H, W, focal, pose, no_ndc, near, far = cam
-    return ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far,
+    return ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far,
                         use_viewdirs=use_viewdirs)
 
 
@@ -211,11 +197,11 @@ def test_bake_and_render_are_reproducible_and_survive_save_load(tmp_path):
     assert bits_equal(f1.values, f2.values)
     H, W, focal, pose, no_ndc, near, far = cam
     opts = O.make_options(no_ndc=no_ndc, near=near, far=far)
-    a = nb.render_baked(f1, H, W, focal, _pose(pose), opts)
-    b = nb.render_baked(f1, H, W, focal, _pose(pose), opts)
+    a = nb.render_baked(f1, H, W, focal, scene_pose(pose), opts)
+    b = nb.render_baked(f1, H, W, focal, scene_pose(pose), opts)
     f1.save(tmp_path / "field.pt")
     g = nb.BakedField.load(tmp_path / "field.pt")
-    c = nb.render_baked(g, H, W, focal, _pose(pose), opts)
+    c = nb.render_baked(g, H, W, focal, scene_pose(pose), opts)
     for x, y, z in zip(a, b, c):
         assert bits_equal(x, y) and bits_equal(x, z)
 
@@ -241,11 +227,10 @@ def test_quality_against_the_network(kind, res):
     field = nb.bake(m, epf, edf, bounds=box, resolution=res, grid=grid)
     opts = O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=128, perturb=False,
                           radiance_field_noise_std=0.0)
-    mc = _model(kind, coarse=True)[0]
-    ref = nb.render_image(H, W, focal, _pose(pose), mc, m, opts, encode_position_fn=epf, encode_direction_fn=edf,
+    mc = shipped_models(kind)[0]
+    ref = nb.render_image(H, W, focal, scene_pose(pose), mc, m, opts, encode_position_fn=epf, encode_direction_fn=edf,
                           impl=1)[3]
-    rgb, _, _ = nb.render_baked(field, H, W, focal, _pose(pose), opts)
-    mse = torch.mean((rgb - ref) ** 2).item()
-    psnr = -10 * math.log10(max(mse, 1e-12))
+    rgb, _, _ = nb.render_baked(field, H, W, focal, scene_pose(pose), opts)
+    psnr = psnr32(rgb, ref)
     report("PSNR vs render_image", (kind, res, field.n_active), psnr)
     assert psnr >= PSNR_MEASURED[(kind, res)] - PSNR_MARGIN

@@ -22,14 +22,10 @@ import math
 import pytest
 import torch
 
-from helpers import baked_render64, bits_equal, load_weights
+from helpers import (FERN_CAM, LEGO_CAM, baked_render64, bake_scene, bits_equal, camera_rays, copies_bit_equal,
+                     edge_rays, heldout_psnr, lattice_index, random_rays, sphere_poses, synthetic_field, targets)
 
 pytestmark = pytest.mark.gpu
-
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
-FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
-LEGO_CAM = (48, 48, 66.7)
-FERN_CAM = (42, 56, 45.3)
 
 # the kernel's gradient against the fp64 oracle: max |d - d64| over a channel group divided by the group's max |d64|
 # (sigma_raw: channel 0; coefficients: channels 1 .. 27), and the tied gradient against the fp64 sum over copies, the
@@ -50,45 +46,6 @@ def report(what, ctx, value):
     print(f"[baked-grad] {what} {ctx}: {value}")
 
 
-def _model(kind, coarse=False):
-    import nerf_pytorch_b200 as nb
-
-    if kind in ("lego", "fern"):
-        w = load_weights(f"{kind}_lowres")
-        l_xyz = 10 if kind == "lego" else 6
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(w[0 if coarse else 1])
-        return m.cuda(), nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
-    torch.manual_seed(7)  # "noview": coarse-only, no view directions
-    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                             use_viewdirs=False)
-    return m.cuda(), nb.get_embedding_function(10), None
-
-
-def _bake(kind, res, grid_res=None):
-    import nerf_pytorch_b200 as nb
-    from nerf_pytorch_b200.occupancy import OccupancyGrid
-
-    m, epf, edf = _model(kind)
-    box = FERN_BOX if kind == "fern" else (LEGO_BOX if kind == "lego" else ((-1.0,) * 3, (1.0,) * 3))
-    grid = OccupancyGrid.full(box, 8) if grid_res is None else \
-        OccupancyGrid.from_models([m], epf, box, grid_res, encode_direction_fn=edf)
-    return nb.bake(m, epf, edf, bounds=box, resolution=res, grid=grid)
-
-
-def _lattice_index(field):
-    """int64 [n_active, 729]: the linear lattice index (x fastest over res + 1 points per axis) each stored value holds."""
-    res = torch.tensor(field.resolution, device="cuda")
-    nb_ = (res + 7) // 8
-    br = field.bricks.long()
-    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)  # [n, 3]
-    p = torch.arange(729, device="cuda")
-    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)  # [729, 3]
-    q = torch.minimum(b[:, None] * 8 + l[None], res)
-    return (q[..., 2] * (res[1] + 1) + q[..., 1]) * (res[0] + 1) + q[..., 0]
-
-
 def _sum_over_copies(x, idx):
     """x [n, 729, C] summed over every stored copy of each lattice point (fp64), returned at every copy."""
     C = x.shape[-1]
@@ -96,100 +53,6 @@ def _sum_over_copies(x, idx):
     acc = torch.zeros(int(flat.max()) + 1, C, dtype=torch.float64, device=x.device)
     acc.index_add_(0, flat, x.reshape(-1, C).double())
     return acc[flat].view(x.shape)
-
-
-def _copies_bit_equal(x, idx):
-    """Every copy of every lattice point holds the same bits in all 32 channels."""
-    flat = idx.reshape(-1)
-    bits = x.reshape(-1, 32).contiguous().view(torch.int32)
-    first = torch.full((int(flat.max()) + 1,), -1, dtype=torch.int64, device=x.device)
-    first.scatter_reduce_(0, flat, torch.arange(flat.numel(), device=x.device), reduce="amin", include_self=False)
-    return bool((bits == bits[first[flat]]).all())
-
-
-def _synthetic(res, *, viewdirs=True, active=1.0, sigma=(-4.0, 8.0), seed=0, box=((-1.0,) * 3, (1.0,) * 3)):
-    """A field with random values per lattice point (every copy of a point the same bits), on a random subset of
-    bricks: sigma_raw uniform in ``sigma``, coefficients normal with std 0.7 (coefficients 1 .. 8 zero without view
-    directions, as a bake writes them)."""
-    import nerf_pytorch_b200 as nb
-
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    nb_ = [-(-r // 8) for r in res]
-    n_bricks = nb_[0] * nb_[1] * nb_[2]
-    keep = torch.rand(n_bricks, generator=g, device="cuda") < active
-    keep[0] = True
-    brick_map = torch.where(keep, torch.cumsum(keep.int(), 0) - 1, -1).int()
-    bricks = torch.nonzero(keep).reshape(-1).int()
-    pts = (res[0] + 1) * (res[1] + 1) * (res[2] + 1)
-    dense = torch.zeros(pts, 32, device="cuda")
-    dense[:, 0] = sigma[0] + (sigma[1] - sigma[0]) * torch.rand(pts, generator=g, device="cuda")
-    dense[:, 1:28] = 0.7 * torch.randn(pts, 27, generator=g, device="cuda")
-    if not viewdirs:
-        coef = dense[:, 1:28].reshape(pts, 3, 9).clone()
-        coef[:, :, 1:] = 0
-        dense[:, 1:28] = coef.reshape(pts, 27)
-    f = nb.BakedField(box, res, brick_map, bricks, torch.empty(bricks.numel(), 729, 32, device="cuda"), viewdirs)
-    f.values = dense[_lattice_index(f)].contiguous()
-    return f
-
-
-def _camera_rays(kind, pose=None, viewdirs=True):
-    from nerf_pytorch_b200 import ops
-    from oracle import nerf_oracle as O
-
-    if kind == "fern":
-        H, W, focal = FERN_CAM
-        return ops.gen_rays(torch.eye(4) if pose is None else pose, H, W, focal, None, "cuda", ndc=True, near=0.0,
-                            far=1.0, use_viewdirs=viewdirs)
-    H, W, focal = LEGO_CAM
-    pose = O.pose_spherical(30.0, -30.0, 4.0) if pose is None else pose
-    return ops.gen_rays(pose, H, W, focal, None, "cuda", ndc=False, near=2.0, far=6.0, use_viewdirs=viewdirs)
-
-
-def _random_rays(n, seed, viewdirs=True, lo=-1.0, hi=1.0):
-    """Rays from a sphere of radius 3 towards random points of the box, near 0, far 6."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    o = torch.randn(n, 3, generator=g, device="cuda")
-    o = 3.0 * o / o.norm(dim=1, keepdim=True)
-    tgt = lo + (hi - lo) * torch.rand(n, 3, generator=g, device="cuda")
-    d = tgt - o
-    return _pack(o, d, viewdirs)
-
-
-def _pack(o, d, viewdirs=True, near=0.0, far=6.0):
-    n = o.shape[0]
-    cols = [o, d, torch.full((n, 1), near, device="cuda"), torch.full((n, 1), far, device="cuda")]
-    if viewdirs:
-        cols.append(d / d.norm(dim=1, keepdim=True))
-    return torch.cat(cols, 1).contiguous()
-
-
-def _edge_rays(field, viewdirs=True):
-    """Axis-parallel rays in brick-face planes (and on brick edges), and diagonals through brick corners."""
-    lo = torch.tensor(field.bounds[0], device="cuda")
-    hi = torch.tensor(field.bounds[1], device="cuda")
-    res = torch.tensor(field.resolution, device="cuda", dtype=torch.float32)
-    h = (hi - lo) / res
-    o, d = [], []
-    for a in range(3):  # along axis a, in the plane of the first brick face of axis b, at several offsets on axis c
-        b, c = (a + 1) % 3, (a + 2) % 3
-        for k in range(6):
-            p = lo + (hi - lo) * 0.37
-            p[b] = lo[b] + 8 * h[b] if res[b] > 8 else lo[b] + h[b]
-            p[c] = lo[c] + (k / 5.0) * (hi[c] - lo[c]) * 0.99
-            if k == 5:
-                p[c] = lo[c] + 8 * h[c] if res[c] > 8 else lo[c]  # a brick edge
-            p[a] = lo[a] - 1.0
-            dd = torch.zeros(3, device="cuda")
-            dd[a] = 1.0
-            o.append(p.clone())
-            d.append(dd)
-    corner = lo + 8 * h * (res > 8)  # a brick corner point (or the box's lower corner)
-    for s in ([1, 1, 1], [1, -1, 1], [-1, 1, 1], [1, 1, -1]):
-        dd = torch.tensor(s, device="cuda", dtype=torch.float32)
-        o.append(corner - 2.0 * dd)
-        d.append(dd)
-    return _pack(torch.stack(o), torch.stack(d), viewdirs)
 
 
 def _gate_flips(field, rays):
@@ -283,8 +146,8 @@ def _grad_check(field, rays, white, loss, ctx, bar, seed=0):
 @pytest.mark.parametrize("loss", ["dot", "mse"])
 @pytest.mark.parametrize("kind,white", [("lego", False), ("lego", True), ("noview", False), ("fern", False)])
 def test_gradient_matches_fp64_on_baked_networks(kind, white, loss):
-    field = _bake(kind, (24, 20, 28))
-    rays = _camera_rays(kind, viewdirs=field.use_viewdirs)
+    field = bake_scene(kind, (24, 20, 28))
+    rays = camera_rays(kind, viewdirs=field.use_viewdirs)
     if kind == "lego":  # rays that miss the box: turned away from it
         rays[::7, 3:6] = -rays[::7, 3:6]
     _grad_check(field, rays, white, loss, (kind, white, loss), SAT_REL)
@@ -293,16 +156,16 @@ def test_gradient_matches_fp64_on_baked_networks(kind, white, loss):
 @pytest.mark.parametrize("case", ["opaque", "edges", "res13", "inactive", "noview_inactive"])
 def test_gradient_matches_fp64_on_synthetic_fields(case):
     if case == "opaque":  # sigma delta in 0.5 .. 3: rays saturate within a few cubes, E - prefix cancels to the tail
-        f = _synthetic((16, 16, 16), sigma=(8.0, 48.0), seed=1)
+        f = synthetic_field((16, 16, 16), sigma=(8.0, 48.0), seed=1)
     elif case == "edges":
-        f = _synthetic((24, 24, 24), seed=2)
+        f = synthetic_field((24, 24, 24), seed=2)
     elif case == "res13":
-        f = _synthetic((13, 9, 17), seed=3)
+        f = synthetic_field((13, 9, 17), seed=3)
     elif case == "inactive":
-        f = _synthetic((20, 17, 33), active=0.5, seed=4)
+        f = synthetic_field((20, 17, 33), active=0.5, seed=4)
     else:
-        f = _synthetic((20, 17, 12), viewdirs=False, active=0.5, seed=5)
-    rays = torch.cat([_random_rays(1024, 10, f.use_viewdirs), _edge_rays(f, f.use_viewdirs)])
+        f = synthetic_field((20, 17, 12), viewdirs=False, active=0.5, seed=5)
+    rays = torch.cat([random_rays(1024, 10, f.use_viewdirs), edge_rays(f, f.use_viewdirs)])
     for white in (False, True):
         for loss in ("dot", "mse"):
             _grad_check(f, rays, white, loss, (case, white, loss), SAT_REL if case == "opaque" else SYN_REL)
@@ -313,8 +176,8 @@ def test_autograd_path_is_the_tied_kernel_gradient():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    f = _synthetic((16, 12, 20), active=0.6, seed=6)
-    rays = _random_rays(512, 11)
+    f = synthetic_field((16, 12, 20), active=0.6, seed=6)
+    rays = random_rays(512, 11)
     f.values.requires_grad_()
     rgb, disp, acc, depth = nb.render_baked_rays(f, rays, white_background=True)
     out = ops.baked_render(f.box(), f.brick_map, f.values.detach(), True, rays, True)
@@ -325,8 +188,8 @@ def test_autograd_path_is_the_tied_kernel_gradient():
     gout[:, :3] = g
     d = torch.zeros_like(f.values)
     ops.baked_render_bwd(f.box(), f.brick_map, f.values.detach(), True, rays, True, out, gout, d)
-    idx = _lattice_index(f)
-    assert _copies_bit_equal(f.values.grad, idx)
+    idx = lattice_index(f)
+    assert copies_bit_equal(f.values.grad, idx)
     want = _sum_over_copies(d, idx)
     err = ((f.values.grad.double() - want).abs().max() / want.abs().max()).item()
     assert err <= SYN_REL, err
@@ -347,22 +210,23 @@ def test_tie_gives_every_copy_the_fp64_sum_over_copies(kind):
 
     bar = SAT_REL if kind == "lego" else SYN_REL
     if kind == "lego":
-        f = _bake("lego", (24, 20, 28), grid_res=32)
-        rays = _camera_rays("lego")
+        f = bake_scene("lego", (24, 20, 28), grid_res=32)
+        rays = camera_rays("lego")
         assert 0 < f.n_active < f.brick_map.numel()
     else:
-        f = _synthetic((13, 9, 17), seed=3) if kind == "res13" else _synthetic((20, 17, 33), active=0.5, seed=4)
-        rays = torch.cat([_random_rays(1024, 12), _edge_rays(f)])
-    idx = _lattice_index(f)
-    assert _copies_bit_equal(f.values, idx)  # the bake (and _synthetic) write every copy the same bits
+        f = synthetic_field((13, 9, 17), seed=3) if kind == "res13" else \
+            synthetic_field((20, 17, 33), active=0.5, seed=4)
+        rays = torch.cat([random_rays(1024, 12), edge_rays(f)])
+    idx = lattice_index(f)
+    assert copies_bit_equal(f.values, idx)  # the bake (and synthetic_field) write every copy the same bits
     d, d64 = _grad_check(f, rays, False, "dot", ("tie", kind), bar)
     tied = ops.baked_tie(f.box(), f.brick_map, f.bricks, d)
-    assert _copies_bit_equal(tied, idx) and (tied[..., 28:] == 0).all()
+    assert copies_bit_equal(tied, idx) and (tied[..., 28:] == 0).all()
     want = _sum_over_copies(d64, idx)
     err = ((tied.double() - want).abs().max() / want.abs().max()).item()
     report("tied gradient error", kind, err)
     assert err <= bar, err
-    assert not _copies_bit_equal(d, idx)  # the untied gradient differs between copies: the tie did something
+    assert not copies_bit_equal(d, idx)  # the untied gradient differs between copies: the tie did something
 
 
 def test_baked_adam_is_adam_step_dev_per_channel_group():
@@ -387,53 +251,30 @@ def test_baked_adam_is_adam_step_dev_per_channel_group():
     assert int(step) == 1500  # the counter is step_advance's to move
 
 
-def _sphere_poses(n, radius=4.0, phis=(-30.0, -45.0, -15.0)):
-    from oracle import nerf_oracle as O
-
-    return torch.stack([O.pose_spherical(360.0 * i / n + 7.0 * (i % len(phis)), phis[i % len(phis)], radius)
-                        for i in range(n)])
-
-
-def _targets(kind, poses):
-    import nerf_pytorch_b200 as nb
-    from oracle import nerf_oracle as O
-
-    m, epf, edf = _model(kind)
-    mc = _model(kind, coarse=True)[0]
-    H, W, focal = FERN_CAM if kind == "fern" else LEGO_CAM
-    ndc = kind == "fern"
-    opts = O.make_options(no_ndc=not ndc, near=0.0 if ndc else 2.0, far=1.0 if ndc else 6.0, num_coarse=64,
-                          num_fine=128, perturb=False, radiance_field_noise_std=0.0)
-    with torch.no_grad():
-        imgs = torch.stack([nb.render_image(H, W, focal, p, mc, m, opts, encode_position_fn=epf,
-                                            encode_direction_fn=edf, impl=1)[3] for p in poses])
-    return imgs.contiguous(), opts
-
-
 def test_copies_stay_bit_equal_under_the_trainer_and_torch_adam():
     import nerf_pytorch_b200 as nb
 
-    f = _bake("lego", (24, 20, 28), grid_res=32)
-    idx = _lattice_index(f)
-    poses = _sphere_poses(6)
-    imgs, opts = _targets("lego", poses)
+    f = bake_scene("lego", (24, 20, 28), grid_res=32)
+    idx = lattice_index(f)
+    poses = sphere_poses(6)
+    imgs, opts = targets("lego", poses)
     t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=2048, seed=3)
     before = f.values.clone()
     t.step(20)
-    assert not bits_equal(before, f.values) and _copies_bit_equal(f.values, idx)
+    assert not bits_equal(before, f.values) and copies_bit_equal(f.values, idx)
     assert bits_equal(before[..., 28:], f.values[..., 28:])
     # torch.optim.Adam on render_baked_rays
-    g = _bake("lego", (24, 20, 28), grid_res=32)
+    g = bake_scene("lego", (24, 20, 28), grid_res=32)
     g.values.requires_grad_()
     opt = torch.optim.Adam([g.values], lr=1e-2)
     for i in range(20):
-        rays = _camera_rays("lego", poses[i % 6])
+        rays = camera_rays("lego", poses[i % 6])
         rgb, *_ = nb.render_baked_rays(g, rays)
         loss = ((rgb - imgs[i % 6].reshape(-1, 3)) ** 2).mean()
         opt.zero_grad()
         loss.backward()
         opt.step()
-    assert _copies_bit_equal(g.values.detach(), idx)
+    assert copies_bit_equal(g.values.detach(), idx)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -447,33 +288,21 @@ FT_GAIN_MEASURED = 1.13
 FT_GAIN_BAR = 0.6
 
 
-def _psnr(a, b):
-    return -10.0 * math.log10(max(torch.mean((a - b) ** 2).item(), 1e-12))
-
-
-def _heldout_psnr(field, poses, imgs):
-    import nerf_pytorch_b200 as nb
-
-    with torch.no_grad():
-        return sum(_psnr(nb.render_baked_rays(field, _camera_rays("lego", p))[0], im.reshape(-1, 3))
-                   for p, im in zip(poses, imgs)) / len(poses)
-
-
 def test_fine_tuning_raises_heldout_psnr_on_lego():
     import nerf_pytorch_b200 as nb
 
-    f = _bake("lego", 256, grid_res=128)
-    poses = _sphere_poses(44)
-    imgs, opts = _targets("lego", poses)
+    f = bake_scene("lego", 256, grid_res=128)
+    poses = sphere_poses(44)
+    imgs, opts = targets("lego", poses)
     train, held = list(range(0, 44)), [5, 16, 27, 38]
     train = [i for i in train if i not in held]
-    p0 = _heldout_psnr(f, poses[held], imgs[held])
+    p0 = heldout_psnr(f, poses[held], imgs[held])
     t = nb.BakedFieldTrainer(f, imgs[train].contiguous(), poses[train].cuda(), LEGO_CAM[2], opts, rays_per_step=2048, seed=1)
     first = t.step(1).item()
     losses = [t.step(1).item() for _ in range(9)]
     t.step(FT_STEPS - 20)
     last = [t.step(1).item() for _ in range(10)]
-    p1 = _heldout_psnr(f, poses[held], imgs[held])
+    p1 = heldout_psnr(f, poses[held], imgs[held])
     report("lego 256^3 held-out PSNR before / after, loss first / last, peak GiB", FT_STEPS,
            (p0, p1, first, sum(losses) / 9, sum(last) / 10, torch.cuda.max_memory_allocated() / 2 ** 30))
     assert sum(last) / 10 < 0.8 * (first + sum(losses)) / 10
@@ -483,14 +312,14 @@ def test_fine_tuning_raises_heldout_psnr_on_lego():
 def test_fine_tuning_lowers_the_loss_on_fern():
     import nerf_pytorch_b200 as nb
 
-    f = _bake("fern", 256, grid_res=128)
+    f = bake_scene("fern", 256, grid_res=128)
     poses = []
     for i in range(8):
         p = torch.eye(4)
         p[0, 3], p[1, 3] = 0.03 * math.cos(i), 0.03 * math.sin(i)
         poses.append(p)
     poses = torch.stack(poses)
-    imgs, opts = _targets("fern", poses)
+    imgs, opts = targets("fern", poses)
     t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), FERN_CAM[2], opts, rays_per_step=2048, seed=2)
     first = sum(t.step(1).item() for _ in range(10)) / 10
     t.step(80)
@@ -505,11 +334,11 @@ def test_fine_tuning_lowers_the_loss_on_fern():
 def test_same_seed_same_pixels_and_runs_agree_to_rounding():
     import nerf_pytorch_b200 as nb
 
-    poses = _sphere_poses(6)
-    imgs, opts = _targets("lego", poses)
+    poses = sphere_poses(6)
+    imgs, opts = targets("lego", poses)
     runs = []
     for _ in range(2):
-        f = _bake("lego", (24, 20, 28), grid_res=32)
+        f = bake_scene("lego", (24, 20, 28), grid_res=32)
         t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=1024, seed=5)
         loss = t.step(10).item()
         runs.append((f.values.clone(), t._ids.clone(), t._image.clone(), t._target.clone(), t._rays.clone(), loss))

@@ -23,14 +23,11 @@ import math
 import pytest
 import torch
 
-from helpers import baked_render64, bits_equal, load_weights
+from helpers import (LEGO_CAM, baked_render64, bake_scene, bits_equal, camera_rays, copies_bit_equal,
+                     edge_rays, heldout_psnr, lattice_index, random_rays, ray_rows, scene_options, sphere_poses,
+                     synthetic_field, targets)
 
 pytestmark = pytest.mark.gpu
-
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
-FERN_BOX = ((-1.2, -1.2, -1.0), (1.2, 1.2, 0.98))
-LEGO_CAM = (48, 48, 66.7)
-FERN_CAM = (42, 56, 45.3)
 
 # peak weights against the fp64 oracle, absolute (weights lie in [0, 1]).  A weight is alpha times T, T a product of the
 # ray's earlier q (fp32, up to ~900 factors for lego at 256^3), so its error grows with the samples before it: up to about
@@ -50,137 +47,16 @@ def report(what, ctx, value):
 _CACHE = {}
 
 
-def _models(kind):
+def _bake(kind, res, grid_res=None):
+    """A fresh copy of helpers.bake_scene over the grid of both networks, each bake made once per file."""
     import nerf_pytorch_b200 as nb
 
-    w = load_weights(f"{kind}_lowres")
-    l_xyz = 10 if kind == "lego" else 6
-    out = []
-    for sd in w[:2]:
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out[0], out[1], nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
-
-
-def _bake(kind, res, grid_res=None, both=True):
-    """The fine network baked over the grid of both networks (or the fine network's alone); grid_res None: all bricks."""
-    import nerf_pytorch_b200 as nb
-
-    key = (kind, res, grid_res, both)
+    key = (kind, res, grid_res)
     if key not in _CACHE:
-        mc, mf, epf, edf = _models(kind)
-        box = FERN_BOX if kind == "fern" else LEGO_BOX
-        grid = nb.OccupancyGrid.full(box, 8) if grid_res is None else \
-            nb.OccupancyGrid.from_models([mc, mf] if both else [mf], epf, box, grid_res, encode_direction_fn=edf)
-        _CACHE[key] = nb.bake(mf, epf, edf, bounds=box, resolution=res, grid=grid)
+        _CACHE[key] = bake_scene(kind, res, grid_res, grid_from="both")
     f = _CACHE[key]
     return nb.BakedField(f.bounds, f.resolution, f.brick_map.clone(), f.bricks.clone(), f.values.clone(),
                          f.use_viewdirs)
-
-
-def _lattice_index(field):
-    res = torch.tensor(field.resolution, device="cuda")
-    nb_ = (res + 7) // 8
-    br = field.bricks.long()
-    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)
-    p = torch.arange(729, device="cuda")
-    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)
-    q = torch.minimum(b[:, None] * 8 + l[None], res)
-    return (q[..., 2] * (res[1] + 1) + q[..., 1]) * (res[0] + 1) + q[..., 0]
-
-
-def _copies_bit_equal(x, idx):
-    flat = idx.reshape(-1)
-    bits = x.reshape(-1, 32).contiguous().view(torch.int32)
-    first = torch.full((int(flat.max()) + 1,), -1, dtype=torch.int64, device=x.device)
-    first.scatter_reduce_(0, flat, torch.arange(flat.numel(), device=x.device), reduce="amin", include_self=False)
-    return bool((bits == bits[first[flat]]).all())
-
-
-def _synthetic(res, *, viewdirs=True, active=1.0, sigma=(-4.0, 8.0), seed=0, box=((-1.0,) * 3, (1.0,) * 3)):
-    """Random values per lattice point (every copy of a point the same bits) on a random subset of bricks."""
-    import nerf_pytorch_b200 as nb
-
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    nb_ = [-(-r // 8) for r in res]
-    keep = torch.rand(nb_[0] * nb_[1] * nb_[2], generator=g, device="cuda") < active
-    keep[0] = True
-    brick_map = torch.where(keep, torch.cumsum(keep.int(), 0) - 1, -1).int()
-    bricks = torch.nonzero(keep).reshape(-1).int()
-    pts = (res[0] + 1) * (res[1] + 1) * (res[2] + 1)
-    dense = torch.zeros(pts, 32, device="cuda")
-    dense[:, 0] = sigma[0] + (sigma[1] - sigma[0]) * torch.rand(pts, generator=g, device="cuda")
-    dense[:, 1:28] = 0.7 * torch.randn(pts, 27, generator=g, device="cuda")
-    if not viewdirs:
-        coef = dense[:, 1:28].reshape(pts, 3, 9).clone()
-        coef[:, :, 1:] = 0
-        dense[:, 1:28] = coef.reshape(pts, 27)
-    f = nb.BakedField(box, res, brick_map, bricks, torch.empty(bricks.numel(), 729, 32, device="cuda"), viewdirs)
-    f.values = dense[_lattice_index(f)].contiguous()
-    return f
-
-
-def _pack(o, d, viewdirs=True, near=0.0, far=6.0):
-    n = o.shape[0]
-    near = torch.full((n, 1), near, device="cuda") if not torch.is_tensor(near) else near.view(n, 1)
-    far = torch.full((n, 1), far, device="cuda") if not torch.is_tensor(far) else far.view(n, 1)
-    cols = [o, d, near, far]
-    if viewdirs:
-        cols.append(d / d.norm(dim=1, keepdim=True))
-    return torch.cat(cols, 1).contiguous()
-
-
-def _random_rays(n, seed, viewdirs=True, lo=-1.0, hi=1.0):
-    """Rays from a sphere of radius 3 towards random points of the box, near 0, far 6; every 7th turned away (a miss)."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    o = torch.randn(n, 3, generator=g, device="cuda")
-    o = 3.0 * o / o.norm(dim=1, keepdim=True)
-    d = lo + (hi - lo) * torch.rand(n, 3, generator=g, device="cuda") - o
-    d[::7] = -d[::7]
-    return _pack(o, d, viewdirs)
-
-
-def _edge_rays(field, viewdirs=True):
-    """Axis-parallel rays in brick-face planes (and on brick edges), and diagonals through brick corners."""
-    lo = torch.tensor(field.bounds[0], device="cuda")
-    hi = torch.tensor(field.bounds[1], device="cuda")
-    res = torch.tensor(field.resolution, device="cuda", dtype=torch.float32)
-    h = (hi - lo) / res
-    o, d = [], []
-    for a in range(3):
-        b, c = (a + 1) % 3, (a + 2) % 3
-        for k in range(6):
-            p = lo + (hi - lo) * 0.37
-            p[b] = lo[b] + 8 * h[b] if res[b] > 8 else lo[b] + h[b]
-            p[c] = lo[c] + (k / 5.0) * (hi[c] - lo[c]) * 0.99
-            if k == 5:
-                p[c] = lo[c] + 8 * h[c] if res[c] > 8 else lo[c]
-            p[a] = lo[a] - 1.0
-            dd = torch.zeros(3, device="cuda")
-            dd[a] = 1.0
-            o.append(p.clone())
-            d.append(dd)
-    corner = lo + 8 * h * (res > 8)
-    for s in ([1, 1, 1], [1, -1, 1], [-1, 1, 1], [1, 1, -1]):
-        dd = torch.tensor(s, device="cuda", dtype=torch.float32)
-        o.append(corner - 2.0 * dd)
-        d.append(dd)
-    return _pack(torch.stack(o), torch.stack(d), viewdirs)
-
-
-def _camera_rays(kind, pose=None, viewdirs=True):
-    from nerf_pytorch_b200 import ops
-    from oracle import nerf_oracle as O
-
-    if kind == "fern":
-        H, W, focal = FERN_CAM
-        return ops.gen_rays(torch.eye(4) if pose is None else pose, H, W, focal, None, "cuda", ndc=True, near=0.0,
-                            far=1.0, use_viewdirs=viewdirs)
-    H, W, focal = LEGO_CAM
-    pose = O.pose_spherical(30.0, -30.0, 4.0) if pose is None else pose
-    return ops.gen_rays(pose, H, W, focal, None, "cuda", ndc=False, near=2.0, far=6.0, use_viewdirs=viewdirs)
 
 
 Y0 = 0.28209479177387814
@@ -294,49 +170,34 @@ def _render_rows(field, rays, white, stop):
     return ops.baked_render(field.box(), field.brick_map, vals, field.use_viewdirs, rays, white, stop)
 
 
-def _sphere_poses(n, radius=4.0, phis=(-30.0, -45.0, -15.0), offset=7.0):
-    from oracle import nerf_oracle as O
-
-    return torch.stack([O.pose_spherical(360.0 * i / n + offset * (i % len(phis)), phis[i % len(phis)], radius)
-                        for i in range(n)])
-
-
-def _opts(kind="lego"):
-    from oracle import nerf_oracle as O
-
-    ndc = kind == "fern"
-    return O.make_options(no_ndc=not ndc, near=0.0 if ndc else 2.0, far=1.0 if ndc else 6.0, num_coarse=64,
-                          num_fine=128, perturb=False, radiance_field_noise_std=0.0)
-
-
 # ------------------------------------------------------------------------------------------------------------------------
 # 1. peak weights against fp64
 # ------------------------------------------------------------------------------------------------------------------------
 def test_peak_weights_match_fp64_on_lego_both_network_grid():
     f = _bake("lego", 256, grid_res=128)
-    rays = _camera_rays("lego")[::23].contiguous()  # 101 rays of up to ~900 samples each
+    rays = camera_rays("lego")[::23].contiguous()  # 101 rays of up to ~900 samples each
     rays[::11, 3:6] = -rays[::11, 3:6]  # rays that miss the box
     _peak_check(f, rays, "lego 256^3 both grids")
 
 
 def test_peak_weights_match_fp64_on_fern_ndc():
     f = _bake("fern", (40, 36, 44), grid_res=32)
-    _peak_check(f, _camera_rays("fern")[::3].contiguous(), "fern ndc")
+    _peak_check(f, camera_rays("fern")[::3].contiguous(), "fern ndc")
 
 
 @pytest.mark.parametrize("case", ["edges", "res13", "inactive", "noview_inactive", "opaque"])
 def test_peak_weights_match_fp64_on_synthetic_fields(case):
     if case == "edges":
-        f = _synthetic((24, 24, 24), seed=2)
+        f = synthetic_field((24, 24, 24), seed=2)
     elif case == "res13":
-        f = _synthetic((13, 9, 17), seed=3)
+        f = synthetic_field((13, 9, 17), seed=3)
     elif case == "inactive":
-        f = _synthetic((20, 17, 33), active=0.5, seed=4)
+        f = synthetic_field((20, 17, 33), active=0.5, seed=4)
     elif case == "noview_inactive":
-        f = _synthetic((20, 17, 12), viewdirs=False, active=0.5, seed=5)
+        f = synthetic_field((20, 17, 12), viewdirs=False, active=0.5, seed=5)
     else:
-        f = _synthetic((16, 16, 16), sigma=(8.0, 48.0), seed=1)
-    rays = torch.cat([_random_rays(1024, 10, f.use_viewdirs), _edge_rays(f, f.use_viewdirs)])
+        f = synthetic_field((16, 16, 16), sigma=(8.0, 48.0), seed=1)
+    rays = torch.cat([random_rays(1024, 10, f.use_viewdirs, misses=True), edge_rays(f, f.use_viewdirs)])
     _peak_check(f, rays, case)
 
 
@@ -358,14 +219,14 @@ def _one_sample_rays(field, n, seed):
     dn = torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])
     dt = (0.5 * h) / dn
     near = 1.0 - 0.5 * dt
-    return _pack(o, d, field.use_viewdirs, near, near + dt)
+    return ray_rows(o, d, field.use_viewdirs, near, near + dt)
 
 
 @pytest.mark.parametrize("kind", ["synthetic", "lego"])
 def test_peak_is_the_largest_single_sample_acc_bit_for_bit(kind):
     import nerf_pytorch_b200 as nb
 
-    f = _synthetic((24, 24, 24), active=0.7, sigma=(-2.0, 6.0), seed=21) if kind == "synthetic" \
+    f = synthetic_field((24, 24, 24), active=0.7, sigma=(-2.0, 6.0), seed=21) if kind == "synthetic" \
         else _bake("lego", (24, 20, 28), grid_res=32)
     rays = _one_sample_rays(f, 200_000, 22)
     rgb, pacc, *_ = baked_render64(_probe(f), rays, False)  # one sample: its colour names its slot
@@ -384,7 +245,7 @@ def test_peaks_are_the_same_bits_for_every_chunking_order_and_run():
     import nerf_pytorch_b200 as nb
 
     f = _bake("lego", (40, 36, 44), grid_res=32)
-    rays = torch.cat([_camera_rays("lego", p) for p in _sphere_poses(6, offset=3.0)])
+    rays = torch.cat([camera_rays("lego", p) for p in sphere_poses(6, offset=3.0)])
     one = nb.baked_brick_weights_rays(f, rays)
     assert int((one > 0).sum()) > 0
     for chunk in (997, 4096, 5000, rays.shape[0] - 1):
@@ -396,10 +257,10 @@ def test_peaks_are_the_same_bits_for_every_chunking_order_and_run():
     assert bits_equal(nb.baked_brick_weights_rays(f, rays[perm].contiguous()), one)
     assert bits_equal(nb.baked_brick_weights_rays(f, rays), one)
     # baked_brick_weights over poses: the same as the rays of those poses, packed
-    poses = _sphere_poses(6, offset=3.0)
+    poses = sphere_poses(6, offset=3.0)
     H, W, focal = LEGO_CAM
-    assert bits_equal(nb.baked_brick_weights(f, poses, H, W, focal, _opts()), one)
-    assert bits_equal(nb.baked_brick_weights(f, poses.cuda(), H, W, focal, _opts()), one)
+    assert bits_equal(nb.baked_brick_weights(f, poses, H, W, focal, scene_options("lego")), one)
+    assert bits_equal(nb.baked_brick_weights(f, poses.cuda(), H, W, focal, scene_options("lego")), one)
 
 
 def test_nan_weight_is_recorded_as_inf_and_empty_field_launches_nothing():
@@ -409,9 +270,9 @@ def test_nan_weight_is_recorded_as_inf_and_empty_field_launches_nothing():
     # sigma_raw = +inf everywhere and a ray from x = -1e6 whose steps dt (1 / 64) are below half an ulp of t (1 / 16):
     # delta = (t + dt) - t = 0, so alpha = 1 - exp(-(inf 0)) is NaN, w is NaN and T stays NaN after it.  The box is
     # offset so that no corner weight is 0 (0 inf would make the interpolated sigma_raw NaN, which sigma's fmaxf drops)
-    f = _synthetic((64, 16, 16), seed=9, box=((-1.01, -1.0, -1.0), (0.99, 1.0, 1.0)))
+    f = synthetic_field((64, 16, 16), seed=9, box=((-1.01, -1.0, -1.0), (0.99, 1.0, 1.0)))
     f.values[..., 0] = float("inf")
-    ray = _pack(torch.tensor([[-1.0e6, 0.1, 0.1]], device="cuda"), torch.tensor([[1.0, 0.0, 0.0]], device="cuda"),
+    ray = ray_rows(torch.tensor([[-1.0e6, 0.1, 0.1]], device="cuda"), torch.tensor([[1.0, 0.0, 0.0]], device="cuda"),
                 far=1.0e7)
     got = nb.baked_brick_weights_rays(f, ray)
     assert not torch.isnan(got).any()
@@ -421,8 +282,8 @@ def test_nan_weight_is_recorded_as_inf_and_empty_field_launches_nothing():
     # a field without active bricks returns an empty tensor without a launch
     empty = nb.prune_baked(f, torch.zeros(f.n_active, dtype=torch.bool, device="cuda"))
     before = ops.launch_count()
-    assert nb.baked_brick_weights_rays(empty, _random_rays(64, 9)).shape == (0,)
-    assert nb.baked_brick_weights(empty, _sphere_poses(2), 8, 8, 10.0, _opts()).shape == (0,)
+    assert nb.baked_brick_weights_rays(empty, random_rays(64, 9, misses=True)).shape == (0,)
+    assert nb.baked_brick_weights(empty, sphere_poses(2), 8, 8, 10.0, scene_options("lego")).shape == (0,)
     assert ops.launch_count() == before
 
 
@@ -445,12 +306,12 @@ def test_dropping_transparent_bricks_keeps_every_render_bit_for_bit():
     p = nb.prune_baked(f, ~tr)
     report("lego 256^3 both grids: transparent bricks dropped / active", "", (int(tr.sum()), f.n_active))
     assert 0 < p.n_active < f.n_active
-    poses = _sphere_poses(3, radius=3.3, phis=(-60.0, 10.0, -5.0), offset=41.0)
+    poses = sphere_poses(3, radius=3.3, phis=(-60.0, 10.0, -5.0), offset=41.0)
     for i, pose in enumerate(poses):
-        rays = _camera_rays("lego", pose)
+        rays = camera_rays("lego", pose)
         _renders_bit_equal(f, p, rays, ("lego", i))
     # a synthetic field with planted transparent bricks (some of them -0, one with NaN in channels 28 .. 31)
-    s = _synthetic((24, 24, 16), active=0.8, sigma=(-3.0, 5.0), seed=31)
+    s = synthetic_field((24, 24, 16), active=0.8, sigma=(-3.0, 5.0), seed=31)
     planted = torch.arange(s.n_active, device="cuda") % 3 == 1
     s.values[planted, :, 0] = -s.values[planted, :, 0].abs()
     s.values[planted.nonzero()[0], :, 0] = -0.0
@@ -459,7 +320,7 @@ def test_dropping_transparent_bricks_keeps_every_render_bit_for_bit():
     assert bool(tr[planted].all())
     q = nb.prune_baked(s, ~tr)
     assert q.n_active <= s.n_active - int(planted.sum())
-    rays = torch.cat([_random_rays(4096, 32), _edge_rays(s)])
+    rays = torch.cat([random_rays(4096, 32, misses=True), edge_rays(s)])
     _renders_bit_equal(s, q, rays, "synthetic")
 
 
@@ -468,8 +329,8 @@ def test_dropping_unseen_bricks_keeps_the_measuring_renders_and_tau_keeps_psnr()
 
     f = _bake("lego", 256, grid_res=128)
     H, W, focal = LEGO_CAM
-    opts = _opts()
-    poses = _sphere_poses(8, offset=13.0)
+    opts = scene_options("lego")
+    poses = sphere_poses(8, offset=13.0)
     w = nb.baked_brick_weights(f, poses, H, W, focal, opts)
     tr = nb.baked_transparent_bricks(f)
     p0 = nb.prune_baked(f, w > 0)
@@ -478,17 +339,17 @@ def test_dropping_unseen_bricks_keeps_the_measuring_renders_and_tau_keeps_psnr()
            (f.n_active, int(tr.sum()), int((w == 0).sum()), unseen_opaque))
     assert unseen_opaque > 0  # interior bricks with density: never seen by these views
     for i, pose in enumerate(poses):
-        rays = _camera_rays("lego", pose)
+        rays = camera_rays("lego", pose)
         for stop in (0.0, 1e-3):
             assert _out_bits_equal(_render_rows(f, rays, False, stop), _render_rows(p0, rays, False, stop)), (i, stop)
     # tau = 1e-2 over 40 poses, held-out PSNR against the unpruned field
-    train = _sphere_poses(40, offset=7.0)
-    held = _sphere_poses(4, phis=(-20.0, -40.0), offset=29.0)
+    train = sphere_poses(40, offset=7.0)
+    held = sphere_poses(4, phis=(-20.0, -40.0), offset=29.0)
     w = nb.baked_brick_weights(f, train, H, W, focal, opts)
     p2 = nb.prune_baked(f, w > 1e-2)
     vals = []
     for pose in held:
-        rays = _camera_rays("lego", pose)
+        rays = camera_rays("lego", pose)
         a, b = _render_rows(f, rays, False, 0.0)[:, :3], _render_rows(p2, rays, False, 0.0)[:, :3]
         vals.append(-10.0 * math.log10(max(((a - b) ** 2).mean().item(), 1e-20)))
     psnr = sum(vals) / len(vals)
@@ -508,7 +369,7 @@ TAU_PSNR_BAR = 70.0
 def test_pruned_field_saves_loads_and_differentiates(tmp_path):
     import nerf_pytorch_b200 as nb
 
-    f = _synthetic((20, 17, 33), active=0.5, seed=4)
+    f = synthetic_field((20, 17, 33), active=0.5, seed=4)
     keep = torch.arange(f.n_active, device="cuda") % 2 == 0
     p = nb.prune_baked(f, keep)
     path = tmp_path / "pruned.pt"
@@ -518,9 +379,9 @@ def test_pruned_field_saves_loads_and_differentiates(tmp_path):
         assert bits_equal(x, y)
     assert (q.bounds, q.resolution, q.use_viewdirs, q.n_active) == (p.bounds, p.resolution, p.use_viewdirs, p.n_active)
     # the tied gradient of render_baked_rays against the fp64 sum over copies of fp64 autograd
-    idx = _lattice_index(p)
-    assert _copies_bit_equal(p.values, idx)
-    rays = torch.cat([_random_rays(1024, 12), _edge_rays(p)])
+    idx = lattice_index(p)
+    assert copies_bit_equal(p.values, idx)
+    rays = torch.cat([random_rays(1024, 12, misses=True), edge_rays(p)])
     v64 = p.values.detach().double().requires_grad_()
     rgb64, *_ = baked_render64(nb.BakedField(p.bounds, p.resolution, p.brick_map, p.bricks, v64, True), rays, False)
     g = torch.randn(rays.shape[0], 3, generator=torch.Generator(device="cuda").manual_seed(3), device="cuda")
@@ -534,31 +395,8 @@ def test_pruned_field_saves_loads_and_differentiates(tmp_path):
     (rgb * g).sum().backward()
     err = ((p.values.grad.double() - want).abs().max() / want.abs().max()).item()
     report("pruned field: tied gradient error", "", err)
-    assert _copies_bit_equal(p.values.grad, idx)
+    assert copies_bit_equal(p.values.grad, idx)
     assert err <= SYN_REL, err
-
-
-def _targets(poses):
-    import nerf_pytorch_b200 as nb
-
-    mc, mf, epf, edf = _models("lego")
-    H, W, focal = LEGO_CAM
-    opts = _opts()
-    with torch.no_grad():
-        imgs = torch.stack([nb.render_image(H, W, focal, p, mc, mf, opts, encode_position_fn=epf,
-                                            encode_direction_fn=edf, impl=1)[3] for p in poses])
-    return imgs.contiguous(), opts
-
-
-def _heldout_psnr(field, poses, imgs):
-    import nerf_pytorch_b200 as nb
-
-    vals = []
-    with torch.no_grad():
-        for p, im in zip(poses, imgs):
-            rgb = nb.render_baked_rays(field, _camera_rays("lego", p))[0]
-            vals.append(-10.0 * math.log10(max(((rgb - im.reshape(-1, 3)) ** 2).mean().item(), 1e-12)))
-    return sum(vals) / len(vals)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -568,12 +406,12 @@ def test_trainer_prune_keeps_rows_and_state_and_trains_on():
     import nerf_pytorch_b200 as nb
 
     f = _bake("lego", (40, 36, 44), grid_res=32)
-    idx = _lattice_index(f)
-    poses = _sphere_poses(6)
-    imgs, opts = _targets(poses)
+    idx = lattice_index(f)
+    poses = sphere_poses(6)
+    imgs, opts = targets("lego", poses)
     t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=2048, seed=3)
     t.step(20)
-    assert _copies_bit_equal(f.values, idx)
+    assert copies_bit_equal(f.values, idx)
     H, W, focal = LEGO_CAM
     keep = nb.baked_brick_weights(f, poses, H, W, focal, opts) > 0
     assert 0 < int(keep.sum()) < f.n_active
@@ -590,13 +428,13 @@ def test_trainer_prune_keeps_rows_and_state_and_trains_on():
         assert x.shape == (kept.numel(), 729, 32)
     assert bool((f.brick_map[f.bricks.long()] == torch.arange(f.n_active, device="cuda", dtype=torch.int32)).all())
     assert int((f.brick_map >= 0).sum()) == f.n_active and int((old_map >= 0).sum()) > f.n_active
-    idx = _lattice_index(f)
-    assert _copies_bit_equal(f.values, idx)
+    idx = lattice_index(f)
+    assert copies_bit_equal(f.values, idx)
     for _ in range(10):
         loss = t.step(10)
         assert math.isfinite(loss.item())
     assert int(t.step_dev) == 120
-    assert _copies_bit_equal(f.values, idx)
+    assert copies_bit_equal(f.values, idx)
     with pytest.raises(ValueError):
         t.prune(torch.zeros(f.n_active, dtype=torch.bool, device="cuda"))
     with pytest.raises(ValueError):
@@ -614,8 +452,8 @@ PRUNE_PSNR_MARGIN = 0.1
 def test_prune_transparent_then_train_matches_train_unpruned():
     import nerf_pytorch_b200 as nb
 
-    poses = _sphere_poses(44)
-    imgs, opts = _targets(poses)
+    poses = sphere_poses(44)
+    imgs, opts = targets("lego", poses)
     held = [5, 16, 27, 38]
     train = [i for i in range(44) if i not in held]
     psnr = {}
@@ -626,7 +464,7 @@ def test_prune_transparent_then_train_matches_train_unpruned():
         if arm == "transparent":
             t.prune(~nb.baked_transparent_bricks(f))
         t.step(FT_STEPS)
-        psnr[arm] = (_heldout_psnr(f, poses[held], imgs[held]), f.n_active)
+        psnr[arm] = (heldout_psnr(f, poses[held], imgs[held]), f.n_active)
         del t, f
         torch.cuda.empty_cache()
     report("held-out PSNR, n_active after 300 steps", "", psnr)

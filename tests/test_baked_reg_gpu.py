@@ -19,18 +19,13 @@ Measured on an H100 80GB HBM3 at 700 W: the value's relative error (the fp64 sum
 fp64 L) is at most 3.7e-16, and the gradient's error per channel group (max |d - d64| over the group's max |d64|,
 channel 0 and channels 1 .. 27) at most 2.0e-7 (synthetic fields; 8.5e-8 on the lego bake), against bars of 1e-12 and
 1e-6.  The file runs in about 25 s."""
-import math
-
-import numpy as np
 import pytest
 import torch
 
-from helpers import bits_equal, load_weights
+from helpers import (LEGO_CAM, baked_lattice, bake_scene, bits_equal, camera_rays, copies_bit_equal, heldout_psnr,
+                     lattice_index, sphere_poses, synthetic_field, targets)
 
 pytestmark = pytest.mark.gpu
-
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
-LEGO_CAM = (48, 48, 66.7)
 
 VALUE_BAR = 1e-12
 GRAD_BAR = 1e-6
@@ -38,38 +33,6 @@ GRAD_BAR = 1e-6
 
 def report(what, ctx, value):
     print(f"[baked-reg] {what} {ctx}: {value}")
-
-
-def _model(coarse=False):
-    import nerf_pytorch_b200 as nb
-
-    w = load_weights("lego_lowres")
-    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                             num_encoding_fn_dir=4)
-    m.load_state_dict(w[0 if coarse else 1])
-    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4)
-
-
-def _bake(res, grid_res=None):
-    import nerf_pytorch_b200 as nb
-    from nerf_pytorch_b200.occupancy import OccupancyGrid
-
-    m, epf, edf = _model()
-    grid = OccupancyGrid.full(LEGO_BOX, 8) if grid_res is None else \
-        OccupancyGrid.from_models([m], epf, LEGO_BOX, grid_res, encode_direction_fn=edf)
-    return nb.bake(m, epf, edf, bounds=LEGO_BOX, resolution=res, grid=grid)
-
-
-def _lattice_index(field):
-    """int64 [n_active, 729]: the linear lattice index (x fastest over res + 1 points per axis) each stored value holds."""
-    res = torch.tensor(field.resolution, device="cuda")
-    nb_ = (res + 7) // 8
-    br = field.bricks.long()
-    b = torch.stack([br % nb_[0], br // nb_[0] % nb_[1], br // (nb_[0] * nb_[1])], -1)  # [n, 3]
-    p = torch.arange(729, device="cuda")
-    l = torch.stack([p % 9, p // 9 % 9, p // 81], -1)  # [729, 3]
-    q = torch.minimum(b[:, None] * 8 + l[None], res)
-    return (q[..., 2] * (res[1] + 1) + q[..., 1]) * (res[0] + 1) + q[..., 0]
 
 
 def _canonical_rows(field, idx):
@@ -93,95 +56,19 @@ def _canonical_rows(field, idx):
     return torch.where(best >= 0, best % n, -1)
 
 
-def _copies_bit_equal(x, idx):
-    """Every copy of every lattice point holds the same bits in all 32 channels."""
-    flat = idx.reshape(-1)
-    bits = x.reshape(-1, 32).contiguous().view(torch.int32)
-    first = torch.full((int(flat.max()) + 1,), -1, dtype=torch.int64, device=x.device)
-    first.scatter_reduce_(0, flat, torch.arange(flat.numel(), device=x.device), reduce="amin", include_self=False)
-    return bool((bits == bits[first[flat]]).all())
-
-
-def _synthetic(res, *, viewdirs=True, active=1.0, sigma=(-4.0, 8.0), seed=0, box=((-1.0,) * 3, (1.0,) * 3)):
-    """A field with random values per lattice point (every copy of a point the same bits), on a random subset of
-    bricks: sigma_raw uniform in ``sigma``, coefficients normal with std 0.7 (coefficients 1 .. 8 zero without view
-    directions, as a bake writes them)."""
-    import nerf_pytorch_b200 as nb
-
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    nb_ = [-(-r // 8) for r in res]
-    n_bricks = nb_[0] * nb_[1] * nb_[2]
-    keep = torch.rand(n_bricks, generator=g, device="cuda") < active
-    keep[0] = True
-    brick_map = torch.where(keep, torch.cumsum(keep.int(), 0) - 1, -1).int()
-    bricks = torch.nonzero(keep).reshape(-1).int()
-    pts = (res[0] + 1) * (res[1] + 1) * (res[2] + 1)
-    dense = torch.zeros(pts, 32, device="cuda")
-    dense[:, 0] = sigma[0] + (sigma[1] - sigma[0]) * torch.rand(pts, generator=g, device="cuda")
-    dense[:, 1:28] = 0.7 * torch.randn(pts, 27, generator=g, device="cuda")
-    if not viewdirs:
-        coef = dense[:, 1:28].reshape(pts, 3, 9).clone()
-        coef[:, :, 1:] = 0
-        dense[:, 1:28] = coef.reshape(pts, 27)
-    f = nb.BakedField(box, res, brick_map, bricks, torch.empty(bricks.numel(), 729, 32, device="cuda"), viewdirs)
-    f.values = dense[_lattice_index(f)].contiguous()
-    return f
-
-
-def _axis_bricks(res, nb, c=None):
-    """bool [res + 1, nb]: the bricks of lattice index q's copy list along one axis (include/nerfb200.h "baked fields:
-    gradients and fine-tuning", Tie): {nb - 1} at q = res, {q / 8 - 1, q / 8} at a positive multiple of 8 below res, {q
-    // 8} otherwise.  With ``c`` set (the edge axis) instead the one brick q // 8 for q < res and none at q = res."""
-    q = np.arange(res + 1)
-    m = np.zeros((res + 1, nb), dtype=bool)
-    if c is not None:
-        m[q[:-1], q[:-1] // 8] = True
-        return m
-    inner = q < res
-    m[q[inner], q[inner] // 8] = True
-    face = inner & (q > 0) & (q % 8 == 0)
-    m[q[face], q[face] // 8 - 1] = True
-    m[res, nb - 1] = True
-    return m
-
-
-def _baked_lattice(res, active):
-    """The regularisers' lattice (include/nerfb200.h "baked fields: regularisers") restated in numpy: (points, edges)
-    with points bool [res_2 + 1, res_1 + 1, res_0 + 1] (the lattice points with a copy in an active brick) and edges a
-    list over the axes c = 0, 1, 2 (x, y, z) of bool arrays of that shape, edges[c][q] for the edge (q, q + e_c): brick q_c
-    // 8 along c and any brick of q's copy list along the other axes.  ``active`` is bool [nb_2, nb_1, nb_0]."""
-    res = tuple(int(r) for r in res)
-    nb = [-(-r // 8) for r in res]
-    a = np.asarray(active).astype(np.int64)
-
-    def spread(mx, my, mz):  # [qz, qy, qx] = any over bricks of mz[qz, bz] my[qy, by] mx[qx, bx] active[bz, by, bx]
-        t = np.tensordot(a, mx.astype(np.int64), axes=([2], [1]))       # [bz, by, qx]
-        t = np.tensordot(t, my.astype(np.int64), axes=([1], [1]))       # [bz, qx, qy]
-        t = np.tensordot(t, mz.astype(np.int64), axes=([0], [1]))       # [qx, qy, qz]
-        return t.transpose(2, 1, 0) > 0
-
-    copies = [_axis_bricks(res[c], nb[c]) for c in range(3)]
-    points = spread(*copies)
-    edges = []
-    for c in range(3):
-        m = list(copies)
-        m[c] = _axis_bricks(res[c], nb[c], c)
-        edges.append(spread(*m))
-    return points, edges
-
 def _restated(field):
-    """(points, edges) of _baked_lattice for the field's active bricks, as torch bool tensors on the device."""
+    """(points, edges) of baked_lattice for the field's active bricks, as torch bool tensors on the device."""
     res = field.resolution
     nb_ = [-(-r // 8) for r in res]
     active = (field.brick_map >= 0).view(nb_[2], nb_[1], nb_[0]).cpu().numpy()
-    points, edges = _baked_lattice(res, active)
+    points, edges = baked_lattice(res, active)
     return torch.from_numpy(points).cuda(), [torch.from_numpy(e).cuda() for e in edges]
 
 
 def _oracle(field, lam):
     """(L in fp64, dL/dpoint fp64 [n_active, 729, 28] at every stored copy, P) by autograd over the dense lattice."""
     res = field.resolution
-    idx = _lattice_index(field)
+    idx = lattice_index(field)
     rows = _canonical_rows(field, idx)
     points, edges = _restated(field)
     present = rows >= 0
@@ -229,8 +116,8 @@ def _check(field, lam, ctx):
     ev = abs(v.item() - L64.item()) / max(abs(L64.item()), 1e-300)
     assert L64.item() > 0 and ev <= VALUE_BAR, (ctx, ev)
     assert (d[..., 28:] == 0).all() and torch.isfinite(d).all()
-    idx = _lattice_index(field)
-    assert _copies_bit_equal(d, idx), ctx
+    idx = lattice_index(field)
+    assert copies_bit_equal(d, idx), ctx
     eg = 0.0
     for sl in (slice(0, 1), slice(1, 28)):
         want, got = g64[..., sl], d[..., sl].double()
@@ -257,7 +144,7 @@ FIELDS = {"res16": dict(res=(16, 16, 16), seed=1), "res24_20_28": dict(res=(24, 
 @pytest.mark.parametrize("fkind", list(FIELDS))
 def test_value_and_gradient_match_fp64_on_synthetic_fields(fkind, viewdirs):
     kw = dict(FIELDS[fkind])
-    f = _synthetic(kw.pop("res"), viewdirs=viewdirs, **kw)
+    f = synthetic_field(kw.pop("res"), viewdirs=viewdirs, **kw)
     if "half" in fkind:
         assert 0 < f.n_active < f.brick_map.numel()
     for name, lam in LAMS.items():
@@ -265,7 +152,7 @@ def test_value_and_gradient_match_fp64_on_synthetic_fields(fkind, viewdirs):
 
 
 def test_value_and_gradient_match_fp64_on_a_lego_bake():
-    f = _bake((24, 20, 28), grid_res=32)
+    f = bake_scene("lego", (24, 20, 28), grid_res=32)
     assert 0 < f.n_active < f.brick_map.numel()
     for name, lam in LAMS.items():
         _check(f, lam, ("lego", name))
@@ -277,79 +164,50 @@ def test_value_and_gradient_match_fp64_on_a_lego_bake():
 def test_gradient_reads_canonical_copies_when_copies_differ():
     """On a field whose non-canonical copies hold other values, the kernel's gradient and value are those of the
     canonical copies (the oracle reads nothing else), and every copy gets the same bits."""
-    f = _synthetic((20, 17, 12), active=0.6, seed=9)
-    idx = _lattice_index(f)
+    f = synthetic_field((20, 17, 12), active=0.6, seed=9)
+    idx = lattice_index(f)
     rows = _canonical_rows(f, idx)
     canon = torch.zeros(f.values.shape[:2], dtype=torch.bool, device="cuda").view(-1)
     canon[rows[rows >= 0]] = True
     noise = torch.randn(f.values.shape, generator=torch.Generator(device="cuda").manual_seed(3), device="cuda")
     f.values = torch.where(canon.view(-1, 729, 1), f.values, f.values + noise).contiguous()
-    assert not _copies_bit_equal(f.values, idx)
+    assert not copies_bit_equal(f.values, idx)
     _check(f, LAMS["all"], "copies differ")
-
-
-def _sphere_poses(n, radius=4.0, phis=(-30.0, -45.0, -15.0)):
-    from oracle import nerf_oracle as O
-
-    return torch.stack([O.pose_spherical(360.0 * i / n + 7.0 * (i % len(phis)), phis[i % len(phis)], radius)
-                        for i in range(n)])
-
-
-def _targets(poses):
-    import nerf_pytorch_b200 as nb
-    from oracle import nerf_oracle as O
-
-    m, epf, edf = _model()
-    mc = _model(coarse=True)[0]
-    H, W, focal = LEGO_CAM
-    opts = O.make_options(no_ndc=True, near=2.0, far=6.0, num_coarse=64, num_fine=128, perturb=False,
-                          radiance_field_noise_std=0.0)
-    with torch.no_grad():
-        imgs = torch.stack([nb.render_image(H, W, focal, p, mc, m, opts, encode_position_fn=epf,
-                                            encode_direction_fn=edf, impl=1)[3] for p in poses])
-    return imgs.contiguous(), opts
-
-
-def _camera_rays(pose):
-    from nerf_pytorch_b200 import ops
-
-    H, W, focal = LEGO_CAM
-    return ops.gen_rays(pose, H, W, focal, None, "cuda", ndc=False, near=2.0, far=6.0, use_viewdirs=True)
 
 
 def test_copies_stay_bit_equal_under_regularised_trainer_and_torch_adam():
     import nerf_pytorch_b200 as nb
 
-    f = _bake((24, 20, 28), grid_res=32)
-    idx = _lattice_index(f)
-    poses = _sphere_poses(6)
-    imgs, opts = _targets(poses)
+    f = bake_scene("lego", (24, 20, 28), grid_res=32)
+    idx = lattice_index(f)
+    poses = sphere_poses(6)
+    imgs, opts = targets("lego", poses)
     t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=2048, seed=3, tv_sigma=1e-3,
                              tv_sh=1e-2, sparsity=1e-3)
     before = f.values.clone()
     t.step(20)
-    assert not bits_equal(before, f.values) and _copies_bit_equal(f.values, idx)
+    assert not bits_equal(before, f.values) and copies_bit_equal(f.values, idx)
     assert bits_equal(before[..., 28:], f.values[..., 28:])
-    g = _bake((24, 20, 28), grid_res=32)
+    g = bake_scene("lego", (24, 20, 28), grid_res=32)
     g.values.requires_grad_()
     before = g.values.detach().clone()
     opt = torch.optim.Adam([g.values], lr=1e-2)
     for i in range(20):
-        rgb, *_ = nb.render_baked_rays(g, _camera_rays(poses[i % 6]))
+        rgb, *_ = nb.render_baked_rays(g, camera_rays("lego", poses[i % 6]))
         loss = ((rgb - imgs[i % 6].reshape(-1, 3)) ** 2).mean() + nb.baked_regularizer(g, tv_sigma=1e-3, tv_sh=1e-2,
                                                                                           sparsity=1e-3)
         opt.zero_grad()
         loss.backward()
-        assert _copies_bit_equal(g.values.grad, idx)
+        assert copies_bit_equal(g.values.grad, idx)
         opt.step()
-    assert _copies_bit_equal(g.values.detach(), idx)
+    assert copies_bit_equal(g.values.detach(), idx)
     assert bits_equal(before[..., 28:], g.values.detach()[..., 28:])
 
 
 def test_autograd_gradient_is_the_kernel_gradient_times_the_upstream_scalar():
     import nerf_pytorch_b200 as nb
 
-    f = _synthetic((16, 12, 20), active=0.6, seed=6)
+    f = synthetic_field((16, 12, 20), active=0.6, seed=6)
     lam = LAMS["all"]
     _, _, d, _ = _kernel(f, lam)
     f.values.requires_grad_()
@@ -365,12 +223,12 @@ def test_launch_count_unchanged_when_off_and_one_more_when_on():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    poses = _sphere_poses(4)
-    imgs, opts = _targets(poses)
+    poses = sphere_poses(4)
+    imgs, opts = targets("lego", poses)
     counts, fields = {}, {}
     for name, kw in (("plain", {}), ("zero", dict(tv_sigma=0.0, tv_sh=0.0, sparsity=0.0)), ("tv", dict(tv_sigma=1e-3)),
                      ("all", dict(tv_sigma=1e-3, tv_sh=1e-3, sparsity=1e-3))):
-        f = _bake((24, 20, 28), grid_res=32)
+        f = bake_scene("lego", (24, 20, 28), grid_res=32)
         t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=1024, seed=4, **kw)
         t.step(1)
         n0 = ops.launch_count()
@@ -389,9 +247,9 @@ def test_launch_count_unchanged_when_off_and_one_more_when_on():
 def test_prune_recounts_lattice_points():
     import nerf_pytorch_b200 as nb
 
-    f = _bake((40, 40, 40))  # every brick active: the box's corners are transparent
-    poses = _sphere_poses(4)
-    imgs, opts = _targets(poses)
+    f = bake_scene("lego", (40, 40, 40))  # every brick active: the box's corners are transparent
+    poses = sphere_poses(4)
+    imgs, opts = targets("lego", poses)
     t = nb.BakedFieldTrainer(f, imgs, poses.cuda(), LEGO_CAM[2], opts, rays_per_step=1024, seed=5, tv_sigma=1e-3,
                              sparsity=1e-3)
     assert int(t._count) == int(_restated(f)[0].sum()) == 41 ** 3
@@ -402,7 +260,7 @@ def test_prune_recounts_lattice_points():
     P = int(_restated(f)[0].sum())
     assert int(t._count) == P < 41 ** 3
     t.step(5)  # regularised steps at the recounted P
-    assert _copies_bit_equal(f.values, _lattice_index(f))
+    assert copies_bit_equal(f.values, lattice_index(f))
     _check(f, t.reg, "pruned")
 
 
@@ -423,33 +281,21 @@ REG_GAIN_MEASURED = 0.04
 REG_GAIN_BAR = -0.1  # regularised minus plain held-out PSNR: at most a 0.1 dB loss
 
 
-def _psnr(a, b):
-    return -10.0 * math.log10(max(torch.mean((a - b) ** 2).item(), 1e-12))
-
-
-def _heldout_psnr(field, poses, imgs):
-    import nerf_pytorch_b200 as nb
-
-    with torch.no_grad():
-        return sum(_psnr(nb.render_baked_rays(field, _camera_rays(p))[0], im.reshape(-1, 3))
-                   for p, im in zip(poses, imgs)) / len(poses)
-
-
 def test_regularisers_on_lego_256():
     import nerf_pytorch_b200 as nb
 
-    poses = _sphere_poses(44)
-    imgs, opts = _targets(poses)
+    poses = sphere_poses(44)
+    imgs, opts = targets("lego", poses)
     held = [5, 16, 27, 38]
     train = [i for i in range(44) if i not in held]
     res = {}
     for name, kw in (("plain", {}), ("sparsity", dict(sparsity=REG_SPARSITY)), ("tv", dict(tv_sigma=REG_TV_SIGMA))):
-        f = _bake(256, grid_res=128)
+        f = bake_scene("lego", 256, grid_res=128)
         t = nb.BakedFieldTrainer(f, imgs[train].contiguous(), poses[train].cuda(), LEGO_CAM[2], opts,
                                  rays_per_step=2048, seed=1, **kw)
         t.step(FT_STEPS)
         tv = nb.baked_regularizer(f, tv_sigma=1.0, tv_sh=1.0).item()
-        res[name] = (_heldout_psnr(f, poses[held], imgs[held]), int(nb.baked_transparent_bricks(f).sum()), tv)
+        res[name] = (heldout_psnr(f, poses[held], imgs[held]), int(nb.baked_transparent_bricks(f).sum()), tv)
         del t, f
     report("held-out PSNR, transparent bricks, TV", FT_STEPS, res)
     assert res["sparsity"][1] > res["plain"][1]

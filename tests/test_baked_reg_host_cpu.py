@@ -9,6 +9,8 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import baked_lattice
+
 NAMES = ("nerfb200_baked_lattice_count", "nerfb200_baked_regularizer")
 
 
@@ -119,46 +121,6 @@ def test_trainer_weights_are_checked_before_any_launch():
 # ------------------------------------------------------------------------------------------------------------------------
 # the lattice's points and edges (header, "Lattice points", "Edges"): the restatement against a brute force
 # ------------------------------------------------------------------------------------------------------------------------
-def _axis_bricks(res, nb, c=None):
-    """bool [res + 1, nb]: the bricks of lattice index q's copy list along one axis (include/nerfb200.h "baked fields:
-    gradients and fine-tuning", Tie): {nb - 1} at q = res, {q / 8 - 1, q / 8} at a positive multiple of 8 below res, {q
-    // 8} otherwise.  With ``c`` set (the edge axis) instead the one brick q // 8 for q < res and none at q = res."""
-    q = np.arange(res + 1)
-    m = np.zeros((res + 1, nb), dtype=bool)
-    if c is not None:
-        m[q[:-1], q[:-1] // 8] = True
-        return m
-    inner = q < res
-    m[q[inner], q[inner] // 8] = True
-    face = inner & (q > 0) & (q % 8 == 0)
-    m[q[face], q[face] // 8 - 1] = True
-    m[res, nb - 1] = True
-    return m
-
-
-def _baked_lattice(res, active):
-    """The regularisers' lattice (include/nerfb200.h "baked fields: regularisers") restated in numpy: (points, edges)
-    with points bool [res_2 + 1, res_1 + 1, res_0 + 1] (the lattice points with a copy in an active brick) and edges a
-    list over the axes c = 0, 1, 2 (x, y, z) of bool arrays of that shape, edges[c][q] for the edge (q, q + e_c): brick q_c
-    // 8 along c and any brick of q's copy list along the other axes.  ``active`` is bool [nb_2, nb_1, nb_0]."""
-    res = tuple(int(r) for r in res)
-    nb = [-(-r // 8) for r in res]
-    a = np.asarray(active).astype(np.int64)
-
-    def spread(mx, my, mz):  # [qz, qy, qx] = any over bricks of mz[qz, bz] my[qy, by] mx[qx, bx] active[bz, by, bx]
-        t = np.tensordot(a, mx.astype(np.int64), axes=([2], [1]))       # [bz, by, qx]
-        t = np.tensordot(t, my.astype(np.int64), axes=([1], [1]))       # [bz, qx, qy]
-        t = np.tensordot(t, mz.astype(np.int64), axes=([0], [1]))       # [qx, qy, qz]
-        return t.transpose(2, 1, 0) > 0
-
-    copies = [_axis_bricks(res[c], nb[c]) for c in range(3)]
-    points = spread(*copies)
-    edges = []
-    for c in range(3):
-        m = list(copies)
-        m[c] = _axis_bricks(res[c], nb[c], c)
-        edges.append(spread(*m))
-    return points, edges
 
 
 def _brute_force(res, active):
@@ -207,7 +169,7 @@ CASES = [((16, 16, 16), "full"), ((13, 9, 17), "full"), ((13, 9, 17), "random"),
 @pytest.mark.parametrize("res,kind", CASES)
 def test_restated_lattice_matches_brute_force(res, kind):
     active = _active(res, kind, seed=sum(res))
-    points, edges = _baked_lattice(res, active)
+    points, edges = baked_lattice(res, active)
     want_points, want_edges = _brute_force(res, active)
     assert np.array_equal(points, want_points)
     for c in range(3):
@@ -228,7 +190,7 @@ def test_lattice_point_count_is_the_canonical_copies(res, kind):
     """P from the restatement equals the number of stored copies that are their point's first copy in the tie's order
     (the counting kernel's rule), enumerated from the stored copies directly."""
     active = _active(res, kind, seed=sum(res))
-    points, _ = _baked_lattice(res, active)
+    points, _ = baked_lattice(res, active)
     nb = [-(-r // 8) for r in res]
     first = {}
     for bz, by, bx in zip(*np.nonzero(active)):  # bricks in ascending order give the stored copies' points

@@ -15,7 +15,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import bits_equal, load_weights
+from helpers import LEGO_BOX, bits_equal, load_weights, shipped_models
 from oracle import nerf_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -217,22 +217,14 @@ def test_out_of_range_operands_are_not_clamped():
 
 
 # ---- the public API and mesh normals ---------------------------------------------------------------------------------
-def _lego():
-    import nerf_pytorch_b200 as nb
-
-    _, sd_f = load_weights("lego_lowres")
-    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                             num_encoding_fn_dir=4)
-    m.load_state_dict(sd_f)
-    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4), sd_f
 
 
 def test_density_gradient_api_is_the_kernel_and_keeps_shapes():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    model, epf, _, sd = _lego()
-    arch, _ = _shipped("lego_lowres")
+    _, model, epf, _ = shipped_models("lego")
+    arch, sd = _shipped("lego_lowres")
     pts = uniform_points(2 * 3 * 50, seed=17).view(2, 3, 50, 3)
     with torch.no_grad():
         sigma, grad = nb.density_gradient(model, epf, pts)
@@ -253,9 +245,9 @@ def test_density_gradient_api_is_the_kernel_and_keeps_shapes():
 def test_mesh_vertex_normals():
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf, sd = _lego()
-    arch, _ = _shipped("lego_lowres")
-    box = ((-1.5,) * 3, (1.5,) * 3)
+    _, model, epf, edf = shipped_models("lego")
+    arch, sd = _shipped("lego_lowres")
+    box = LEGO_BOX
     with torch.no_grad():
         plain = nb.extract_mesh(model, epf, box, 128, 50.0, encode_direction_fn=edf)
         m = nb.extract_mesh(model, epf, box, 128, 50.0, encode_direction_fn=edf, normals=True)
@@ -285,9 +277,9 @@ def test_mesh_vertex_normals():
 def test_ply_with_normals(tmp_path):
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf, _ = _lego()
+    _, model, epf, edf = shipped_models("lego")
     with torch.no_grad():
-        m = nb.extract_mesh(model, epf, ((-1.5,) * 3, (1.5,) * 3), 64, 50.0, encode_direction_fn=edf, normals=True)
+        m = nb.extract_mesh(model, epf, LEGO_BOX, 64, 50.0, encode_direction_fn=edf, normals=True)
     path = tmp_path / "lego_n.ply"
     m.save_ply(path)
     data = path.read_bytes()

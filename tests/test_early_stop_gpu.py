@@ -14,7 +14,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import OUT_NAMES, bits_equal, transmittance64
+from helpers import OUT_NAMES, bits_equal, psnr64, scene_pose, transmittance64, ws_view
 from mlp_checks import T_REL
 
 pytestmark = pytest.mark.gpu
@@ -46,29 +46,19 @@ def report(what, ctx, value):
     print(f"[early_stop] {what} {ctx}: {value}")
 
 
-def _models(scene):
-    return M.scene_models(SCENES[scene])
-
-
-def _pose(kind):
-    from oracle import nerf_oracle as O
-
-    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
-
-
 def _setup(scene, variant="det", n_fine=128):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
+    mc, mf = M.scene_models(SCENES[scene])
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
     archs = tuple(train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
                   for m in (mc, mf))
     blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
     opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
-    rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
+    rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
 
@@ -84,12 +74,6 @@ def _grid(scene, kind, models=None, encoders=None):
         return OccupancyGrid.from_models(models, encoders[0], bounds, 128, encode_direction_fn=encoders[1])
     g = torch.Generator(device="cuda").manual_seed(11)
     return OccupancyGrid.from_occupancy(bounds, torch.rand(32, 32, 32, generator=g, device="cuda") < 0.5)
-
-
-def _ws(ws, layout, name, n, s, cols):
-    off = layout[name] // 4
-    t = ws.view(torch.float32)[off: off + n * s * cols]
-    return t.view(n, s, cols) if cols > 1 else t.view(n, s)
 
 
 def _reference(arch, arch_f, blobs, opts, rays, rng, grid, impl):
@@ -173,8 +157,8 @@ def _stopped_render(impl, scene, variant, grid_kind, t):
                               workspace=es_ws)
     torch.cuda.synchronize()
     out = dict(opts=opts, rays=rays, rng=rng, ref=(oc, of), es=(ec, ef), ne=ne, stop=stop.long(),
-               raw=_ws(ws, lay, "raw_fine", n, 192, 4), z=_ws(ws, lay, "z_fine", n, 192, 1),
-               es_raw=_ws(es_ws, lay, "raw_fine", n, 192, 4), es_z=_ws(es_ws, lay, "z_fine", n, 192, 1))
+               raw=ws_view(ws, lay, "raw_fine", n, 192, 4), z=ws_view(ws, lay, "z_fine", n, 192, 1),
+               es_raw=ws_view(es_ws, lay, "raw_fine", n, 192, 4), es_z=ws_view(es_ws, lay, "z_fine", n, 192, 1))
     _CACHE[key] = out
     return out
 
@@ -267,10 +251,10 @@ def _image(scene, impl, chunk, grid=None, randoms=None, early_stop=None, perturb
     from oracle import nerf_oracle as O
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
+    mc, mf = M.scene_models(SCENES[scene])
     opts = O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=128, perturb=perturb,
                           radiance_field_noise_std=noise)
-    return nb.render_image(H, W, focal, _pose(pose), mc, mf, opts, mode="validation",
+    return nb.render_image(H, W, focal, scene_pose(pose), mc, mf, opts, mode="validation",
                            encode_position_fn=nb.get_embedding_function(l_xyz),
                            encode_direction_fn=nb.get_embedding_function(4), rays_per_chunk=chunk, impl=impl,
                            randoms=randoms, grid=grid, early_stop=early_stop)
@@ -309,11 +293,6 @@ def _render_image_is_deterministic_and_chunking_invariant(impl, scene, grid_kind
 # ------------------------------------------------------------------------------------------------------------------------
 # 5. shipped weights
 # ------------------------------------------------------------------------------------------------------------------------
-def _psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
-
-
 @pytest.mark.parametrize("grid_kind", [None, "model"])
 @pytest.mark.parametrize("scene", ["lego", "fern"])
 @pytest.mark.parametrize("impl", list(IMPLS))
@@ -333,7 +312,7 @@ def test_shipped_weights(impl, scene, grid_kind):
     ctx = (impl, scene, grid_kind)
     n = rays.shape[0]
     stopped = int((stop < 192).sum())
-    p = _psnr(ef[:, :3], of[:, :3])
+    p = psnr64(ef[:, :3], of[:, :3])
     report("stopped rays, fine rows early_stop / grid-only, PSNR dB", ctx,
            (f"{stopped} / {n}", f"{ne[1].item()} / {ne_ref[1].item()}", p))
     assert stopped > 0, ctx

@@ -19,7 +19,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import bits_equal, load_weights
+from helpers import LEGO_BOX, bits_equal, shipped_models
 
 pytestmark = pytest.mark.gpu
 
@@ -255,19 +255,6 @@ def test_mesh_repeats_bit_for_bit():
 
 
 # ---- networks --------------------------------------------------------------------------------------------------------
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
-
-
-def _lego():
-    import nerf_pytorch_b200 as nb
-
-    sd_c, sd_f = load_weights("lego_lowres")
-    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                             num_encoding_fn_dir=4)
-    m.load_state_dict(sd_f)
-    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4)
-
-
 def _init_net(hidden, layers, skip, res):
     """A network at init, its sigma bias shifted so that raw sigma changes sign inside the box (at init it may be
     negative everywhere, which leaves no surface)."""
@@ -317,7 +304,7 @@ def _open_edges_on_box_faces(v, f, bounds, res):
 def test_lego_volume_is_run_networks_sigma_and_the_mesh_is_open_only_on_the_box():
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     res = 128
     vol = nb.density_volume(model, epf, LEGO_BOX, res, encode_direction_fn=edf)
     want = _run_network_sigma(model, epf, edf, LEGO_BOX, res)
@@ -335,7 +322,7 @@ def test_lego_volume_is_run_networks_sigma_and_the_mesh_is_open_only_on_the_box(
 def test_lego_colors_are_run_networks_at_the_vertices():
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     res, level = 64, 50.0
     m = nb.extract_mesh(model, epf, LEGO_BOX, res, level, encode_direction_fn=edf, colors=True)
     vol = nb.density_volume(model, epf, LEGO_BOX, res, encode_direction_fn=edf)
@@ -368,7 +355,7 @@ def test_other_networks_run_through_the_same_path(net):
 def test_volume_and_mesh_do_not_depend_on_the_slab_size():
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     res = 40
     vols = [nb.density_volume(model, epf, LEGO_BOX, res, encode_direction_fn=edf, planes_per_slab=s)
             for s in (None, 1, 7, 41)]
@@ -381,7 +368,7 @@ def test_volume_and_mesh_do_not_depend_on_the_slab_size():
 def test_save_ply_round_trips(tmp_path):
     import nerf_pytorch_b200 as nb
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     m = nb.extract_mesh(model, epf, LEGO_BOX, 32, 50.0, encode_direction_fn=edf, colors=True)
     path = tmp_path / "lego.ply"
     m.save_ply(path)
@@ -399,7 +386,7 @@ def test_refusals_launch_nothing():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     before = ops.launch_count()
     cases = [
         (lambda: nb.extract_mesh(model, epf, LEGO_BOX, 1), ValueError),

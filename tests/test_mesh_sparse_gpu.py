@@ -17,12 +17,11 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import bits_equal, load_weights
+from helpers import LEGO_BOX, bits_equal, shipped_models
 
 pytestmark = pytest.mark.gpu
 
 BOX = ((-1.0,) * 3, (1.0,) * 3)
-LEGO_BOX = ((-1.5,) * 3, (1.5,) * 3)
 
 
 def report(what, ctx, value):
@@ -100,16 +99,6 @@ def _assert_same(dense, sparse, skeys, dvol, level, brick_map=None, extras=()):
 
 
 # ---- networks ---------------------------------------------------------------------------------------------------------
-def _lego():
-    import nerf_pytorch_b200 as nb
-
-    _, sd_f = load_weights("lego_lowres")
-    m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                             num_encoding_fn_dir=4)
-    m.load_state_dict(sd_f)
-    return m.cuda(), nb.get_embedding_function(10), nb.get_embedding_function(4)
-
-
 def _init_net(hidden, layers, skip):
     """A network at init, its sigma bias shifted so that raw sigma changes sign inside the box."""
     import nerf_pytorch_b200 as nb
@@ -127,7 +116,7 @@ def _init_net(hidden, layers, skip):
 
 def _net(name):
     if name == "lego_a0":
-        return _lego()
+        return shipped_models("lego")[1:]
     if name == "a1_init":
         return _init_net(128, 8, 3)
     return _init_net(256, 4, 4)
@@ -312,7 +301,7 @@ def test_repeatable_and_independent_of_bricks_per_call():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import mesh
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     grid = nb.OccupancyGrid.from_models([model], epf, LEGO_BOX, 64, encode_direction_fn=edf)
     outs = [mesh._extract_mesh(model, epf, LEGO_BOX, 96, 50.0, edf, True, None, None, False, grid, bpc,
                                edge_keys=True) for bpc in (None, None, 1, 7)]
@@ -328,7 +317,7 @@ def test_model_grid(res):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import mesh, ops
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     level = 50.0
     grid = nb.OccupancyGrid.from_models([model], epf, LEGO_BOX, 128, threshold=0.0, encode_direction_fn=edf)
     box = ops.grid_struct(LEGO_BOX, (res,) * 3)
@@ -351,7 +340,7 @@ def test_past_the_dense_limit():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import mesh, ops
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     res, level = 2048, 50.0
     grid = nb.OccupancyGrid.from_models([model], epf, LEGO_BOX, 128, threshold=0.0, encode_direction_fn=edf)
     box = ops.grid_struct(LEGO_BOX, (res,) * 3)
@@ -445,7 +434,7 @@ def test_refusals_launch_nothing():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    model, epf, edf = _lego()
+    model, epf, edf = shipped_models("lego")[1:]
     full = nb.OccupancyGrid.full(LEGO_BOX, 8)
     bad_bits = nb.OccupancyGrid.full(LEGO_BOX, 8)
     bad_bits.bits = bad_bits.bits[:-1]

@@ -17,7 +17,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import bits_equal, load_weights
+from helpers import bits_equal, shipped_models
 from oracle import nerf_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -103,24 +103,20 @@ def _net(name):
     from nerf_pytorch_b200 import ops
 
     if name == "fern":
-        _, sd = load_weights("fern_lowres")
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=6,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        m = m.cuda()
+        _, m, epf, edf = shipped_models("fern")
         arch = ops.ArchSpec(num_layers=4, hidden=128, skip_every=4, n_freq_xyz=6, n_freq_dir=4)
-        return m, nb.get_embedding_function(6), nb.get_embedding_function(4), sd, arch
-    torch.manual_seed(11)  # A1 at init, its sigma bias shifted so that raw sigma changes sign inside the box
-    m = nb.FlexibleNeRFModel(num_layers=8, hidden_size=128, skip_connect_every=3, num_encoding_fn_xyz=10,
-                             num_encoding_fn_dir=4).cuda()
-    epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
-    lo, hi = torch.tensor(BOX[0]), torch.tensor(BOX[1])
-    pts = (torch.rand(1 << 14, 3, generator=torch.Generator().manual_seed(3)) * (hi - lo) + lo).cuda()
-    with torch.no_grad():
-        sigma, _ = nb.density_gradient(m, epf, pts)
-        m.fc_alpha.bias -= sigma.median()
+    else:
+        torch.manual_seed(11)  # A1 at init, its sigma bias shifted so that raw sigma changes sign inside the box
+        m = nb.FlexibleNeRFModel(num_layers=8, hidden_size=128, skip_connect_every=3, num_encoding_fn_xyz=10,
+                                 num_encoding_fn_dir=4).cuda()
+        epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
+        lo, hi = torch.tensor(BOX[0]), torch.tensor(BOX[1])
+        pts = (torch.rand(1 << 14, 3, generator=torch.Generator().manual_seed(3)) * (hi - lo) + lo).cuda()
+        with torch.no_grad():
+            sigma, _ = nb.density_gradient(m, epf, pts)
+            m.fc_alpha.bias -= sigma.median()
+        arch = ops.ArchSpec(num_layers=8, hidden=128, skip_every=3, n_freq_xyz=10, n_freq_dir=4)
     sd = {k: v.detach().cpu() for k, v in m.state_dict().items()}
-    arch = ops.ArchSpec(num_layers=8, hidden=128, skip_every=3, n_freq_xyz=10, n_freq_dir=4)
     return m, epf, edf, sd, arch
 
 
@@ -414,24 +410,11 @@ def test_sparse_world_mesh_is_the_dense_one_on_active_bricks():
 
 
 # ---- normal maps ------------------------------------------------------------------------------------------------------
-def _models(weights, l_xyz):
-    import nerf_pytorch_b200 as nb
-
-    out = []
-    for sd in load_weights(weights):
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out
-
-
 def test_world_normal_map_of_a_fern_render():
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
-    mc, mf = _models("fern_lowres", 6)
-    epf, edf = nb.get_embedding_function(6), nb.get_embedding_function(4)
+    mc, mf, epf, edf = shipped_models("fern")
     opts_o = O.make_options(no_ndc=False, near=0.0, far=1.0, num_coarse=64, num_fine=128, perturb=False,
                             radiance_field_noise_std=0.0)
     kw = dict(mode="validation", encode_position_fn=epf, encode_direction_fn=edf, impl=1)
@@ -482,11 +465,11 @@ def test_world_normal_map_of_a_fern_render():
 def test_world_normal_map_of_a_blender_render_is_normals_true():
     import nerf_pytorch_b200 as nb
 
-    mc, mf = _models("lego_lowres", 10)
+    mc, mf, epf, edf = shipped_models("lego")
     opts = O.make_options(no_ndc=True, near=2.0, far=6.0, num_coarse=64, num_fine=128, perturb=True,
                           radiance_field_noise_std=0.2)
-    kw = dict(mode="validation", encode_position_fn=nb.get_embedding_function(10),
-              encode_direction_fn=nb.get_embedding_function(4), impl=1, randoms=nb.SeededRandoms(5, 2))
+    kw = dict(mode="validation", encode_position_fn=epf, encode_direction_fn=edf, impl=1,
+              randoms=nb.SeededRandoms(5, 2))
     pose = O.pose_spherical(30.0, -30.0, 4.0)
     with torch.no_grad():
         a = nb.render_image(48, 48, 66.7, pose, mc, mf, opts, normals=True, **kw)

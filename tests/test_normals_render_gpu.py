@@ -12,7 +12,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import bits_equal
+from helpers import bits_equal, scene_pose
 from mlp_checks import ACC_EPS, G_ERR, N_FLOOR
 from oracle import nerf_oracle as O
 
@@ -33,14 +33,6 @@ def report(what, ctx, value):
     print(f"measured {what} {ctx}: {value}")
 
 
-def _models(scene):
-    return M.scene_models(SCENES[scene])
-
-
-def _pose(kind):
-    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
-
-
 def _options(scene, perturb=False, noise=0.0, num_fine=128):
     _, H, W, focal, pose, no_ndc, near, far, *_ = SCENES[scene]
     return O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=num_fine, perturb=perturb,
@@ -57,8 +49,8 @@ def _image(scene, normals, grid=None, early_stop=None, randoms=None, perturb=Fal
     import nerf_pytorch_b200 as nb
 
     _, H, W, focal, pose, _, _, _, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
-    return nb.render_image(H, W, focal, _pose(pose), mc, mf, _options(scene, perturb, noise), mode="validation",
+    mc, mf = M.scene_models(SCENES[scene])
+    return nb.render_image(H, W, focal, scene_pose(pose), mc, mf, _options(scene, perturb, noise), mode="validation",
                            encode_position_fn=nb.get_embedding_function(l_xyz),
                            encode_direction_fn=nb.get_embedding_function(4), impl=1, grid=grid,
                            early_stop=early_stop, randoms=randoms, normals=normals)
@@ -83,7 +75,7 @@ def _six_outputs_are_those_of_the_render_without_normals(scene, variant):
 
     grid = None
     if "grid" in variant:
-        mc, mf = _models(scene)
+        mc, mf = M.scene_models(SCENES[scene])
         grid = _grid(scene, [mc, mf], (nb.get_embedding_function(SCENES[scene][8]), nb.get_embedding_function(4)))
     stop = 1e-3 if "early_stop" in variant else None
     rng = nb.SeededRandoms(5, 2)
@@ -109,7 +101,7 @@ def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None)
     from nerf_pytorch_b200 import ops, train_utils
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
+    mc, mf = M.scene_models(SCENES[scene])
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
     archs = [train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
              for m in (mc, mf)]
@@ -118,7 +110,7 @@ def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None)
     grid = _grid(scene, [mc, mf], (epf, edf)) if grid_kind == "model" else None
     nf = 0 if coarse_only else 128
     opts = ops.make_opts(64, nf, perturb, False, False, noise)
-    rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
+    rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     rng = nb.SeededRandoms(seed, 0)
     arch, arch_f = archs[0], None if coarse_only else archs[1]
     with torch.no_grad():
@@ -168,7 +160,7 @@ def test_normals_refusals_fire_before_any_launch():
     from nerf_pytorch_b200 import ops
     from nerf_pytorch_b200.occupancy import OccupancyGrid
 
-    mc, mf = _models("lego")
+    mc, mf = M.scene_models(SCENES["lego"])
     kw = dict(encode_position_fn=nb.get_embedding_function(10), encode_direction_fn=nb.get_embedding_function(4))
     o = _options("lego", num_fine=64)
     rays = ops.gen_rays(torch.eye(4), 8, 8, 10.0, None, "cuda", ndc=False, near=2.0, far=6.0)

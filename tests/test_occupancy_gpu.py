@@ -14,7 +14,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import OUT_NAMES, bits_equal, compaction_reference, skipped_samples
+from helpers import OUT_NAMES, bits_equal, compaction_reference, psnr64, scene_pose, skipped_samples, ws_view
 
 pytestmark = pytest.mark.gpu
 
@@ -41,30 +41,20 @@ def report(what, ctx, value):
     print(f"[occupancy] {what} {ctx}: {value}")
 
 
-def _models(scene):
-    return M.scene_models(SCENES[scene])
-
-
-def _pose(kind):
-    from oracle import nerf_oracle as O
-
-    return O.pose_spherical(30.0, -30.0, 4.0) if kind == "spherical" else torch.eye(4)
-
-
 def _setup(scene, variant="det", n_fine=128):
     """((arch_c, arch_f), blobs, opts, rays, models, encoders) of a scene at the ops level."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
+    mc, mf = M.scene_models(SCENES[scene])
     epf, edf = nb.get_embedding_function(l_xyz), nb.get_embedding_function(4)
     archs = tuple(train_utils._arch_of(m, train_utils._probe_encoder(epf, None), train_utils._probe_encoder(edf, None))
                   for m in (mc, mf))
     blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
     opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
-    rays = ops.gen_rays(_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
+    rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
 
@@ -84,12 +74,6 @@ def _grid_model(scene, models, encoders, res=64):
     from nerf_pytorch_b200.occupancy import OccupancyGrid
 
     return OccupancyGrid.from_models(models, encoders[0], SCENES[scene][-1], res, encode_direction_fn=encoders[1])
-
-
-def _ws(ws, layout, name, n, s, cols):
-    off = layout[name] // 4
-    t = ws.view(torch.float32)[off: off + n * s * cols]
-    return t.view(n, s, cols) if cols > 1 else t.view(n, s)
 
 
 def _render_both(archs, blobs, opts, rays, grid, impl, rng):
@@ -188,8 +172,8 @@ def test_rays_without_skipped_density_are_bit_identical(impl, scene, variant, gr
     (oc, of, ws), (gc, gf, gws), ne = _render_both(archs, blobs, opts, rays, grid, IMPLS[impl], rng)
     n, nc, ns = rays.shape[0], 64, 192
     lay = ops.render_workspace_layout(*archs, opts, n, False)
-    z_c, z_f = _ws(ws, lay, "z_coarse", n, nc, 1), _ws(ws, lay, "z_fine", n, ns, 1)
-    raw_c, raw_f = _ws(ws, lay, "raw_coarse", n, nc, 4), _ws(ws, lay, "raw_fine", n, ns, 4)
+    z_c, z_f = ws_view(ws, lay, "z_coarse", n, nc, 1), ws_view(ws, lay, "z_fine", n, ns, 1)
+    raw_c, raw_f = ws_view(ws, lay, "raw_coarse", n, nc, 4), ws_view(ws, lay, "raw_fine", n, ns, 4)
     std = opts.noise_std
     noise_c = ops.random_fill(rng, "noise_c", n, nc) if std > 0 else None
     noise_f = ops.random_fill(rng, "noise_f", n, ns) if std > 0 else None
@@ -205,8 +189,8 @@ def test_rays_without_skipped_density_are_bit_identical(impl, scene, variant, gr
     assert ne[0].item() == int((~sk_c).sum())
 
     # every evaluated point's raw is the default raw at that point; skipped samples hold [0 0 0 -inf]
-    g_zc, g_zf = _ws(gws, lay, "z_coarse", n, nc, 1), _ws(gws, lay, "z_fine", n, ns, 1)
-    g_rc, g_rf = _ws(gws, lay, "raw_coarse", n, nc, 4), _ws(gws, lay, "raw_fine", n, ns, 4)
+    g_zc, g_zf = ws_view(gws, lay, "z_coarse", n, nc, 1), ws_view(gws, lay, "z_fine", n, ns, 1)
+    g_rc, g_rf = ws_view(gws, lay, "raw_coarse", n, nc, 4), ws_view(gws, lay, "raw_fine", n, ns, 4)
     assert bits_equal(g_zc, z_c)
     assert bits_equal(g_rc[~sk_c], raw_c[~sk_c])
     skip_raw = torch.tensor([0.0, 0.0, 0.0, -math.inf], device="cuda")
@@ -261,10 +245,10 @@ def _image(scene, impl, chunk, grid=None, randoms=None, perturb=True, noise=0.5)
     from oracle import nerf_oracle as O
 
     _, H, W, focal, pose, no_ndc, near, far, l_xyz, *_ = SCENES[scene]
-    mc, mf = _models(scene)
+    mc, mf = M.scene_models(SCENES[scene])
     opts = O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=128, perturb=perturb,
                           radiance_field_noise_std=noise)
-    return nb.render_image(H, W, focal, _pose(pose), mc, mf, opts, mode="validation",
+    return nb.render_image(H, W, focal, scene_pose(pose), mc, mf, opts, mode="validation",
                            encode_position_fn=nb.get_embedding_function(l_xyz),
                            encode_direction_fn=nb.get_embedding_function(4), rays_per_chunk=chunk, impl=impl,
                            randoms=randoms, grid=grid)
@@ -304,12 +288,12 @@ def test_grid_refusals_fire_before_any_launch():
     from nerf_pytorch_b200.occupancy import OccupancyGrid
     from oracle import nerf_oracle as O
 
-    mc, mf = _models("lego")
+    mc, mf = M.scene_models(SCENES["lego"])
     epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
     kw = dict(encode_position_fn=epf, encode_direction_fn=edf)
     opts = O.make_options(num_coarse=64, num_fine=64)
     grid = OccupancyGrid.full(SCENES["lego"][-1], 16)
-    rays = ops.gen_rays(_pose("spherical"), 16, 16, 20.0, None, "cuda")
+    rays = ops.gen_rays(scene_pose("spherical"), 16, 16, 20.0, None, "cuda")
     with torch.no_grad():  # pack both models once, so that nothing below is a first use
         nb.predict_and_render_radiance(rays, mc, mf, opts, grid=grid, **kw)
     torch.cuda.synchronize()
@@ -369,11 +353,6 @@ PSNR_BARS = {
 }
 
 
-def _psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
-
-
 @pytest.mark.parametrize("scene", ["lego", "fern"])
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_model_grid_render_psnr_against_default(impl, scene):
@@ -386,6 +365,6 @@ def test_model_grid_render_psnr_against_default(impl, scene):
     got = _image(scene, IMPLS[impl], 4096, grid, perturb=False, noise=0.0)
     for out in ("rgb_fine", "rgb_coarse"):
         i = OUT_NAMES.index(out)
-        p = _psnr(got[i], ref[i])
+        p = psnr64(got[i], ref[i])
         report(f"PSNR dB grid vs default {out}", (impl, scene), p)
         assert p >= PSNR_BARS[(scene, out)], (impl, scene, out, p)

@@ -31,7 +31,7 @@ import pytest
 import torch
 
 import mlp_checks as M
-from helpers import bits_equal, compaction_reference, transmittance64
+from helpers import bits_equal, compaction_reference, transmittance64, ws_view
 from mlp_checks import ACC_EPS, ALL_ARCHS, H256_ARCHS, STATES, T_REL, TC_FWD_TOL
 
 pytestmark = pytest.mark.gpu
@@ -77,12 +77,6 @@ def _grid(kind):
     if kind == "box":
         return OccupancyGrid.from_occupancy(BOX, torch.rand(16, 16, 16, generator=g, device="cuda") < 0.3)
     return OccupancyGrid.from_occupancy(BOUNDS, torch.rand(32, 32, 32, generator=g, device="cuda") < int(kind[4:]) / 100)
-
-
-def _ws(ws, layout, name, n, s, cols):
-    off = layout[name] // 4
-    t = ws.view(torch.float32)[off: off + n * s * cols]
-    return t.view(n, s, cols) if cols > 1 else t.view(n, s)
 
 
 def _setup(name, state):
@@ -149,8 +143,8 @@ def _grid_case(arch, sd, blob, shape, kind, impl, edges, worst, stop_check):
     lay = ops.render_workspace_layout(arch, arch_f, opts, n, False)
     keeps, zs, raws = [], [], []
     for i, (pname, s) in enumerate(passes):
-        z = _ws(gws, lay, f"z_{pname}", n, s, 1).clone()
-        raw = _ws(gws, lay, f"raw_{pname}", n, s, 4).clone()
+        z = ws_view(gws, lay, f"z_{pname}", n, s, 1).clone()
+        raw = ws_view(gws, lay, f"raw_{pname}", n, s, 4).clone()
         keep, _, blocks = compaction_reference(grid, rays, z)
         edges.blocks(arch, blocks, n)
         skip = ~keep
@@ -186,7 +180,7 @@ def _grid_case(arch, sd, blob, shape, kind, impl, edges, worst, stop_check):
                                                    impl=impl, want_stop=True, workspace=es_ws)
     torch.cuda.synchronize()
     last, lname = (ef, gf) if arch_f is not None else (ec, gc), passes[-1][0]
-    es_z, es_raw = _ws(es_ws, lay, f"z_{lname}", n, S, 1), _ws(es_ws, lay, f"raw_{lname}", n, S, 4)
+    es_z, es_raw = ws_view(es_ws, lay, f"z_{lname}", n, S, 1), ws_view(es_ws, lay, f"raw_{lname}", n, S, 4)
     keep, z, raw = keeps[-1], zs[-1], raws[-1]
     stop = stop.long()
     assert bits_equal(es_z, z), ctx
@@ -298,7 +292,7 @@ def test_normal_maps_over_the_row_map(name, state):
             torch.cuda.synchronize()
             assert bits_equal(oc[:, :6], pc[:, :6]) and bits_equal(of[:, :6], pf[:, :6]), ctx
             lay = ops.render_workspace_layout(arch, arch_f, opts, n, False)
-            z, raw = _ws(ws, lay, f"z_{lname}", n, S, 1), _ws(ws, lay, f"raw_{lname}", n, S, 4)
+            z, raw = ws_view(ws, lay, f"z_{lname}", n, S, 1), ws_view(ws, lay, f"raw_{lname}", n, S, 4)
             N64, bound, _, _ = M.normals64(arch, sd, rays, z, raw)
             err = (N.double() - N64).abs().max(-1).values
             worst = max(worst, (err / bound).max().item())

@@ -9,12 +9,10 @@ fp16(w) x fp16(activation / 16) product per k-step with fp32 accumulation instea
 
 Bars: each is below 10x the worst figure measured on an H100 over every parameter set (figures beside the constants);
 the PSNR bars are 3 dB under the H100 figure.  Run with -s to print the measured figures."""
-import math
-
 import pytest
 import torch
 
-from helpers import OUT_NAMES, bits_equal, load_weights
+from helpers import OUT_NAMES, bits_equal, psnr64, scene_pose, shipped_models
 from mlp_checks import (ALL_ARCHS, H256_ARCHS, SHAPES, STATES, TC_FWD_TOL, arch_weights, encodings, oracle, points,
                         report, sms_shape, spec)
 
@@ -129,24 +127,12 @@ PSNR_BARS = {
     ("fern", "rgb_fine"): 62.4,    # [65.48; max abs 0.020, 0.34 %]
     ("fern", "rgb_coarse"): 71.2,  # [74.20; max abs 0.0037, 0 %]
 }
-# (weights, H, W, focal, pose, no_ndc, near, far, L_xyz): lego at pose_spherical(30, -30, 4); fern forward-facing in NDC
+# (H, W, focal, pose, no_ndc, near, far) of the shipped scenes: lego at pose_spherical(30, -30, 4); fern forward-facing
+# in NDC
 VIEWS = {
-    "lego": ("lego_lowres", 100, 100, 138.89, "spherical", True, 2.0, 6.0, 10),
-    "fern": ("fern_lowres", 63, 84, 67.9, "eye", False, 0.0, 1.0, 6),
+    "lego": (100, 100, 138.89, "spherical", True, 2.0, 6.0),
+    "fern": (63, 84, 67.9, "eye", False, 0.0, 1.0),
 }
-
-
-def _models(weights, l_xyz):
-    import nerf_pytorch_b200 as nb
-
-    sd_c, sd_f = load_weights(weights)
-    out = []
-    for sd in (sd_c, sd_f):
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict(sd)
-        out.append(m.cuda())
-    return out
 
 
 def _render(view, impl, perturb=False, noise=0.0, chunk=None, randoms=None):
@@ -155,20 +141,12 @@ def _render(view, impl, perturb=False, noise=0.0, chunk=None, randoms=None):
     import nerf_pytorch_b200 as nb
     from oracle import nerf_oracle as O
 
-    weights, H, W, focal, pose, no_ndc, near, far, l_xyz = VIEWS[view]
-    mc, mf = _models(weights, l_xyz)
-    pose = O.pose_spherical(30.0, -30.0, 4.0) if pose == "spherical" else torch.eye(4)
+    H, W, focal, pose, no_ndc, near, far = VIEWS[view]
+    mc, mf, epf, edf = shipped_models(view)
     opts = O.make_options(no_ndc=no_ndc, near=near, far=far, num_coarse=64, num_fine=128, perturb=perturb,
                           radiance_field_noise_std=noise)
-    return nb.render_image(H, W, focal, pose, mc, mf, opts, mode="validation",
-                           encode_position_fn=nb.get_embedding_function(l_xyz),
-                           encode_direction_fn=nb.get_embedding_function(4), rays_per_chunk=chunk or H * W,
-                           impl=impl, randoms=randoms)
-
-
-def _psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
+    return nb.render_image(H, W, focal, scene_pose(pose), mc, mf, opts, mode="validation", encode_position_fn=epf,
+                           encode_direction_fn=edf, rays_per_chunk=chunk or H * W, impl=impl, randoms=randoms)
 
 
 @pytest.mark.parametrize("view", list(VIEWS))
@@ -182,7 +160,7 @@ def test_fast_render_psnr_against_impl1(view):
         i = OUT_NAMES.index(out)
         a, b = fast[i], ref[i]
         assert torch.isfinite(a).all(), (view, out)
-        p = _psnr(a, b)
+        p = psnr64(a, b)
         d = (a - b).abs()
         report(f"PSNR dB fast vs impl 1 {out}", (view,), p)
         report(f"max abs fast vs impl 1 {out}", (view,), d.max().item())
@@ -226,12 +204,12 @@ def test_training_with_the_fast_forward_raises_before_any_launch():
     from nerf_pytorch_b200 import ops
     from oracle import nerf_oracle as O
 
-    mc, mf = _models("lego_lowres", 10)
+    mc, mf, epf, edf = shipped_models("lego")
     opts = O.make_options(num_coarse=64, num_fine=64)
     g = torch.Generator().manual_seed(3)
     ro = torch.nn.functional.normalize(torch.randn(256, 3, generator=g), dim=-1).cuda() * 4.0
     rd = -ro / 4.0
-    kw = dict(encode_position_fn=nb.get_embedding_function(10), encode_direction_fn=nb.get_embedding_function(4))
+    kw = dict(encode_position_fn=epf, encode_direction_fn=edf)
     torch.cuda.synchronize()
     before = ops.launch_count()
     with pytest.raises(NotImplementedError, match="inference"):

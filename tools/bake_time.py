@@ -13,63 +13,21 @@ and their range.  The card's name, power limit and SM clock are read in the same
     python tools/bake_time.py [--rounds 3] [--json OUT]"""
 import argparse
 import json
-import math
 import os
-import statistics
-import subprocess
 import sys
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, median, psnr, timed_once  # noqa: E402
+from helpers import shipped_models  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import mesh, ops, train_utils  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
 
 BOX = ((-1.5,) * 3, (1.5,) * 3)
 ARCHS = {"A0": (4, 128, 4), "A1": (8, 128, 3), "A2": (8, 256, 4)}  # layers, hidden, skip
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def lego_pair():
-    z = np.load(os.path.join(ROOT, "tests", "golden", "weights_lego_lowres.npz"))
-    out = []
-    for pre in ("c.", "f."):
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict({k[2:]: torch.from_numpy(z[k]) for k in z.files if k.startswith(pre)})
-        out.append(m.cuda())
-    return out
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1), out
-
-
-def psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
-
-
-def median(ms):
-    return dict(ms=statistics.median(ms), range=(min(ms), max(ms)))
 
 
 def bake_table(grid, rounds):
@@ -79,7 +37,7 @@ def bake_table(grid, rounds):
     rows = []
     for name, (layers, hidden, skip) in ARCHS.items():
         if name == "A0":
-            m = lego_pair()[1]
+            m = shipped_models("lego")[1]
         else:
             torch.manual_seed(0)
             m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=hidden, skip_connect_every=skip,
@@ -112,8 +70,8 @@ def bake_table(grid, rounds):
                 fused(), unfused()
             t_f, t_u = [], []
             for _ in range(rounds):
-                t_f.append(timed(fused)[0])
-                t_u.append(timed(unfused)[0])
+                t_f.append(timed_once(fused)[0])
+                t_u.append(timed_once(unfused)[0])
             # the two agree up to the projection's summation order
             diff = (values.view(P, 32)[:, 1:28] - coef).abs().max().item()
             r = dict(arch=name, res=res, n_active=n, bricks=ops.mesh_sparse_brick_count(box), bytes=values.numel() * 4,
@@ -160,7 +118,7 @@ def render_table(mc, mf, grid, rounds):
         imgs = {}
         for _ in range(rounds):
             for k, f in configs.items():
-                dt, imgs[k] = timed(f)
+                dt, imgs[k] = timed_once(f)
                 ms[k].append(dt)
         for k in configs:
             r = dict(size=H, config=k, psnr=psnr(imgs[k], imgs["default_impl1"]), **median(ms[k]))
@@ -176,7 +134,7 @@ def main():
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     print("card:", card(), flush=True)
-    mc, mf = lego_pair()
+    mc, mf = shipped_models("lego")[:2]
     grid = nb.OccupancyGrid.from_models([mc, mf], nb.get_embedding_function(10), BOX, 128,
                                         encode_direction_fn=nb.get_embedding_function(4))
     out = dict(card=card(), occupied_fraction=grid.occupied_fraction, bake=bake_table(grid, a.rounds),

@@ -14,17 +14,15 @@ the mean of REPS launches) and their range.  The card's name, power limit and SM
     python tools/baked_finetune_time.py [--rounds 3] [--sweep] [--json OUT]"""
 import argparse
 import json
-import math
 import os
-import statistics
-import subprocess
 import sys
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, median, psnr, timed_mean  # noqa: E402
+from helpers import shipped_models  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
@@ -33,47 +31,6 @@ BOX = ((-1.5,) * 3, (1.5,) * 3)
 H, FOCAL = 48, 66.7
 REPS = 10
 HELD = (5, 16, 27, 38)
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def lego_pair():
-    z = np.load(os.path.join(ROOT, "tests", "golden", "weights_lego_lowres.npz"))
-    out = []
-    for pre in ("c.", "f."):
-        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4, num_encoding_fn_xyz=10,
-                                 num_encoding_fn_dir=4)
-        m.load_state_dict({k[2:]: torch.from_numpy(z[k]) for k in z.files if k.startswith(pre)})
-        out.append(m.cuda())
-    return out
-
-
-def timed(fn, reps=REPS):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def median(ms):
-    return dict(ms=statistics.median(ms), range=(min(ms), max(ms)))
-
-
-def psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
 
 
 def poses_and_targets(mc, mf):
@@ -131,7 +88,7 @@ def kernel_table(field, poses, imgs, opts, rounds, res):
     ms = {k: [] for k in arms}
     for _ in range(rounds):
         for k, f in arms.items():
-            ms[k].append(timed(f))
+            ms[k].append(timed_mean(f, REPS))
     rows = []
     for k in arms:
         r = dict(res=res, arm=k, **median(ms[k]))
@@ -182,7 +139,7 @@ def main():
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     print("card:", card(), flush=True)
-    mc, mf = lego_pair()
+    mc, mf = shipped_models("lego")[:2]
     epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
     grid = nb.OccupancyGrid.from_models([mf], epf, BOX, 128, encode_direction_fn=edf)
     poses, imgs, opts = poses_and_targets(mc, mf)

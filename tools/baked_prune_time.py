@@ -31,8 +31,9 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import nerf_pytorch_b200 as nb  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
-from baked_finetune_time import BOX, FOCAL, H, HELD, card, heldout_psnr, lego_pair, median, poses_and_targets, timed, \
-    trainer  # noqa: E402
+from baked_finetune_time import BOX, FOCAL, H, HELD, heldout_psnr, poses_and_targets, trainer  # noqa: E402
+from common import card, median, timed_mean  # noqa: E402
+from helpers import shipped_models  # noqa: E402
 
 BIG, BIG_FOCAL = 800, 1111.1
 TAUS = (0.0, 1e-3, 1e-2)
@@ -72,7 +73,7 @@ def one_grid(mf, grid, grid_name, res, poses, imgs, opts, rounds):
     ms = {k: [] for k in arms}
     for _ in range(rounds):
         for k, (fn, per) in arms.items():
-            ms[k].append(timed(fn, reps=3 if "48x48" in k[1] else 10) / per)
+            ms[k].append(timed_mean(fn, 3 if "48x48" in k[1] else 10) / per)
     rows = []
     for k, f in fields.items():
         r = dict(res=res, grid=grid_name, criterion=k, n_active=f.n_active, values_gib=gib(f),
@@ -92,7 +93,7 @@ def one_grid(mf, grid, grid_name, res, poses, imgs, opts, rounds):
         torch.cuda.reset_peak_memory_stats()
         t = trainer(tuned, poses, imgs, opts, seed=1)
         t.step(5)
-        step_ms = [timed(lambda: t.step(1), reps=20) for _ in range(rounds)]
+        step_ms = [timed_mean(lambda: t.step(1), 20) for _ in range(rounds)]
         t.step(max(0, STEPS - 5 - 20 * rounds))
         torch.cuda.synchronize()
         r["trainer step 2048"] = median(step_ms)
@@ -117,7 +118,7 @@ def main():
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     print("card:", card(), flush=True)
-    mc, mf = lego_pair()
+    mc, mf = shipped_models("lego")[:2]
     epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
     grids = {"both": nb.OccupancyGrid.from_models([mc, mf], epf, BOX, 128, encode_direction_fn=edf),
              "fine": nb.OccupancyGrid.from_models([mf], epf, BOX, 128, encode_direction_fn=edf)}

@@ -20,8 +20,9 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from baked_finetune_time import (BOX, HELD, card, heldout_psnr, lego_pair, median, poses_and_targets,  # noqa: E402
-                                 timed, trainer)
+from baked_finetune_time import BOX, HELD, REPS, heldout_psnr, poses_and_targets, trainer  # noqa: E402
+from common import card, median, timed_mean  # noqa: E402
+from helpers import shipped_models  # noqa: E402
 
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
@@ -55,7 +56,7 @@ def kernel_table(field, poses, opts, rounds, label):
     ms = {k: [] for k in arms}
     for _ in range(rounds):
         for k, f in arms.items():
-            ms[k].append(timed(f))
+            ms[k].append(timed_mean(f, REPS))
     rows = []
     for k in arms:
         r = dict(field=label, n_active=field.n_active, P=int(count), arm=k, **median(ms[k]))
@@ -112,7 +113,7 @@ def main():
     ap.add_argument("--json", default=None)
     a = ap.parse_args()
     print("card:", card(), flush=True)
-    mc, mf = lego_pair()
+    mc, mf = shipped_models("lego")[:2]
     epf, edf = nb.get_embedding_function(10), nb.get_embedding_function(4)
     grid = nb.OccupancyGrid.from_models([mf], epf, BOX, 128, encode_direction_fn=edf)
     poses, imgs, opts = poses_and_targets(mc, mf)

@@ -11,13 +11,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, timed_mean  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
@@ -30,27 +30,6 @@ ARCHS = {  # bench.py's architectures
 IMPLS = {"impl1": ops.IMPL_TC, "impl3": ops.IMPL_TC_FAST}
 
 
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def timed(fn, iters):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
 def compare(name, fns, rounds, iters, warmup=3):
     """fns: {impl label: callable}; alternates them, returns a result dict and prints one line."""
     for _ in range(warmup):
@@ -59,7 +38,7 @@ def compare(name, fns, rounds, iters, warmup=3):
     ms = {k: [] for k in fns}
     for _ in range(rounds):
         for k, f in fns.items():
-            ms[k].append(timed(f, iters))
+            ms[k].append(timed_mean(f, iters))
     speed = [a / b for a, b in zip(ms["impl1"], ms["impl3"])]
     res = {k: {"median_ms": statistics.median(v), "all_ms": v} for k, v in ms.items()}
     res["speedup"] = {"median": statistics.median(speed), "min": min(speed), "max": max(speed)}

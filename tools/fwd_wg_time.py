@@ -13,13 +13,13 @@ import ctypes
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, timed_mean  # noqa: E402
 from nerf_pytorch_b200 import _lib, ops  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
 
@@ -36,27 +36,6 @@ def open_build(path):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = res, args
     return lib
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def timed(fn, iters):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
 
 
 def compare(name, builds, fn, rounds, iters, warmup=3, reset=None):
@@ -81,7 +60,7 @@ def compare(name, builds, fn, rounds, iters, warmup=3, reset=None):
     for _ in range(rounds):
         for k, lib in builds.items():
             _lib._lib = lib
-            ms[k].append(timed(fn, iters))
+            ms[k].append(timed_mean(fn, iters))
     res = {k: {"median_ms": statistics.median(v), "min_ms": min(v), "max_ms": max(v)} for k, v in ms.items()}
     print(f"{name:42s} " + "   ".join(f"{k} {r['median_ms']:7.3f} ms ({r['min_ms']:.3f} - {r['max_ms']:.3f})"
                                       for k, r in res.items()), flush=True)

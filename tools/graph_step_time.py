@@ -15,7 +15,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
@@ -24,6 +23,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import parallel, train_utils  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
@@ -33,16 +33,6 @@ ARCHS = {"A0": dict(num_layers=4, hidden_size=128, skip_connect_every=4),
 H = W = 400
 FOCAL = 555.5555155968841
 N_IMAGES = 20
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
 
 
 def poses(n):

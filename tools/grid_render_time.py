@@ -8,18 +8,16 @@ and the PSNR of the grid render against the default one.  The card's name, power
     python tools/grid_render_time.py [--rounds 5] [--json OUT]"""
 import argparse
 import json
-import math
 import os
 import statistics
-import subprocess
 import sys
 import time
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, models, psnr, timed_once  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops, train_utils  # noqa: E402
 from oracle import nerf_oracle as O  # noqa: E402
@@ -32,45 +30,6 @@ CASES = {
     "fern_A0_ndc": ("fern", 4, 4, 6, 378, 504, 407.6, True, 0.0, 1.0, ((-1.2, -1.2, -1.0), (1.2, 1.2, 1.0))),
 }
 IMPLS = {"impl1": ops.IMPL_TC, "impl3": ops.IMPL_TC_FAST}
-
-
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def models(weights, layers, skip, l_xyz):
-    out = []
-    torch.manual_seed(0)
-    for i in range(2):
-        m = nb.FlexibleNeRFModel(num_layers=layers, hidden_size=128, skip_connect_every=skip, num_encoding_fn_xyz=l_xyz,
-                                 num_encoding_fn_dir=4)
-        if weights:
-            z = np.load(os.path.join(ROOT, "tests", "golden", f"weights_{weights}_lowres.npz"))
-            pre = "cf"[i] + "."
-            m.load_state_dict({k[2:]: torch.from_numpy(z[k]) for k in z.files if k.startswith(pre)})
-        out.append(m.cuda())
-    return out
-
-
-def timed(fn):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    out = fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1), out
-
-
-def psnr(a, b):
-    mse = (a.double() - b.double()).pow(2).mean().item()
-    return math.inf if mse == 0 else -10.0 * math.log10(mse)
 
 
 def run_case(name, rounds):
@@ -109,7 +68,7 @@ def run_case(name, rounds):
         outs = {}
         for _ in range(rounds):
             for path, g in (("default", None), ("grid", grid)):
-                t, outs[path] = timed(lambda: render(impl, g))
+                t, outs[path] = timed_once(lambda: render(impl, g))
                 ms[path].append(t)
         speed = [d / g for d, g in zip(ms["default"], ms["grid"])]
         res[label] = dict(

@@ -25,7 +25,8 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import mesh, ops, train_utils  # noqa: E402
 from mesh_time import BOX, LEVEL, lego_fine  # noqa: E402
-from run_network_time import card, compare  # noqa: E402
+from common import card  # noqa: E402
+from run_network_time import compare  # noqa: E402
 
 
 def peak_bytes(fn):

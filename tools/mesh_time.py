@@ -23,7 +23,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import mesh, ops, train_utils  # noqa: E402
-from run_network_time import EAGER_CHUNK, card, compare, eager_run_network  # noqa: E402
+from common import card  # noqa: E402
+from run_network_time import EAGER_CHUNK, compare, eager_run_network  # noqa: E402
 
 BOX = ((-1.5,) * 3, (1.5,) * 3)
 LEVEL = 50.0

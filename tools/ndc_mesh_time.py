@@ -22,7 +22,8 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
-from run_network_time import card, compare  # noqa: E402
+from common import card  # noqa: E402
+from run_network_time import compare  # noqa: E402
 
 BOX = ((-1.0, -1.0, -1.0), (1.0, 1.0, 0.95))
 HWF = (42, 56, 45.3)

@@ -13,13 +13,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from common import card, timed_mean  # noqa: E402
 import nerf_pytorch_b200 as nb  # noqa: E402
 from nerf_pytorch_b200 import ops  # noqa: E402
 
@@ -31,27 +31,6 @@ GRID = 256
 EAGER_CHUNK = 1 << 20
 
 
-def card():
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader",
-                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True,
-                           timeout=30).stdout.strip()
-    except Exception as e:  # pragma: no cover - depends on the host
-        q = f"nvidia-smi unavailable ({e})"
-    return q or torch.cuda.get_device_name()
-
-
-def timed(fn, iters):
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
 def compare(name, fns, rounds, iters, points, warmup=2):
     """fns: {label: callable}, alternated; prints and returns median ms, points/s and the range over the rounds."""
     for _ in range(warmup):
@@ -60,7 +39,7 @@ def compare(name, fns, rounds, iters, points, warmup=2):
     ms = {k: [] for k in fns}
     for _ in range(rounds):
         for k, f in fns.items():
-            ms[k].append(timed(f, iters))
+            ms[k].append(timed_mean(f, iters))
     res = {}
     for k, v in ms.items():
         med = statistics.median(v)
