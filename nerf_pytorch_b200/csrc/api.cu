@@ -204,40 +204,6 @@ struct Workspace {
   int64_t z_c, raw_c, w_c, z_f, raw_f, stash_c, stash_f, gstash, d_raw, total;
 };
 
-static void carve(const Plan& pc, const Plan* pf, const nerfb200_render_opts_t& o, int64_t n, int training,
-                  Workspace* w) {
-  const int64_t nc = o.n_coarse, ns = o.n_coarse + o.n_fine;
-  int64_t off = 0;
-  auto take = [&](int64_t floats) {
-    int64_t r = off;
-    off += align256(floats * 4);
-    return r;
-  };
-  w->z_c = take(n * nc);
-  w->raw_c = take(n * nc * 4);
-  w->w_c = take(n * nc);
-  const bool fine = o.n_fine > 0 && pf != nullptr;
-  w->z_f = take(fine ? n * ns : 0);
-  w->raw_f = take(fine ? n * ns * 4 : 0);
-  if (training) {
-    const int64_t sc = stash_floats(pc, n * nc);
-    const int64_t sf = fine ? stash_floats(*pf, n * ns) : 0;
-    w->stash_c = take(sc);
-    w->stash_f = take(sf);
-    // backward scratch: the gradient stash of the CUDA-core path / the gradient blob of the wgmma path
-    int64_t gs = sc > sf ? sc : sf;
-    const int64_t bc = pc.hidden == 128 ? bwd_tc_scratch_floats(pc) : 0;
-    const int64_t bf = (fine && pf->hidden == 128) ? bwd_tc_scratch_floats(*pf) : 0;
-    if (bc > gs) gs = bc;
-    if (bf > gs) gs = bf;
-    w->gstash = take(gs);
-    w->d_raw = take(n * (fine ? ns : nc) * 4);
-  } else {
-    w->stash_c = w->stash_f = w->gstash = w->d_raw = off;
-  }
-  w->total = off;
-}
-
 // What a call needs of the MLP kernels it selects with `impl`.
 enum Need {
   kInference,  // the forward alone: render_fwd(training = 0), mlp_fwd without a stash
@@ -320,6 +286,61 @@ static int check_opts(const nerfb200_render_opts_t* o) {
     set_error("hierarchical sampling needs n_coarse >= 4");
     return NERFB200_ERR_UNSUPPORTED;
   }
+  return NERFB200_OK;
+}
+
+// What every render-family call starts from: the plans, the sample counts and the base workspace.
+struct RenderSetup {
+  Plan pc, pf;
+  bool fine;  // a fine pass: n_fine > 0 and a fine arch
+  int nc, ns;
+  Workspace w;
+};
+
+// Builds the coarse plan, the fine plan when arch_f is given, checks the options and n_rays > 0 (refused with the
+// text `empty`, or with none when it is NULL) and carves the base workspace.  The workspace queries pass arch_f as
+// given, so that they refuse an invalid one even with n_fine = 0; the renders pass it only for a fine pass.
+static int render_setup(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f, const nerfb200_render_opts_t* opts,
+                        int64_t n, int training, const char* empty, RenderSetup* r) {
+  NB_TRY(build_plan(arch_c, &r->pc));
+  if (arch_f) NB_TRY(build_plan(arch_f, &r->pf));
+  NB_TRY(check_opts(opts));
+  if (n <= 0) {
+    if (empty) set_error("%s", empty);
+    return NERFB200_ERR_INVALID;
+  }
+  const Plan &pc = r->pc, &pf = r->pf;
+  const bool fine = r->fine = arch_f && opts->n_fine > 0;
+  const int64_t nc = r->nc = opts->n_coarse, ns = r->ns = opts->n_coarse + opts->n_fine;
+  Workspace* w = &r->w;
+  int64_t off = 0;
+  auto take = [&](int64_t floats) {
+    int64_t at = off;
+    off += align256(floats * 4);
+    return at;
+  };
+  w->z_c = take(n * nc);
+  w->raw_c = take(n * nc * 4);
+  w->w_c = take(n * nc);
+  w->z_f = take(fine ? n * ns : 0);
+  w->raw_f = take(fine ? n * ns * 4 : 0);
+  if (training) {
+    const int64_t sc = stash_floats(pc, n * nc);
+    const int64_t sf = fine ? stash_floats(pf, n * ns) : 0;
+    w->stash_c = take(sc);
+    w->stash_f = take(sf);
+    // backward scratch: the gradient stash of the CUDA-core path / the gradient blob of the wgmma path
+    int64_t gs = sc > sf ? sc : sf;
+    const int64_t bc = pc.hidden == 128 ? bwd_tc_scratch_floats(pc) : 0;
+    const int64_t bf = (fine && pf.hidden == 128) ? bwd_tc_scratch_floats(pf) : 0;
+    if (bc > gs) gs = bc;
+    if (bf > gs) gs = bf;
+    w->gstash = take(gs);
+    w->d_raw = take(n * (fine ? ns : nc) * 4);
+  } else {
+    w->stash_c = w->stash_f = w->gstash = w->d_raw = off;
+  }
+  w->total = off;
   return NERFB200_OK;
 }
 
@@ -706,37 +727,6 @@ int32_t nerfb200_sample_pdf_merge(const float* z_coarse, const float* weights_co
                                  z_fine, z_samples, inds, cdf_out, static_cast<cudaStream_t>(stream));
 }
 
-int64_t nerfb200_render_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
-                                        const nerfb200_render_opts_t* opts, int64_t n_rays, int32_t training) {
-  Plan pc, pf;
-  if (build_plan(coarse, &pc) != NERFB200_OK) return -1;
-  if (fine && build_plan(fine, &pf) != NERFB200_OK) return -1;
-  if (check_opts(opts) != NERFB200_OK || n_rays <= 0) return -1;
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
-  return w.total;
-}
-
-/* Byte offsets of the named sections of the render workspace (test hook): order
- * z_coarse, raw_coarse, weights_coarse, z_fine, raw_fine, stash_coarse, stash_fine, gstash, d_raw. */
-int32_t nerfb200_render_workspace_layout(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
-                                         const nerfb200_render_opts_t* opts, int64_t n_rays, int32_t training,
-                                         int64_t* offsets9) {
-  Plan pc, pf;
-  NB_TRY(build_plan(coarse, &pc));
-  if (fine) NB_TRY(build_plan(fine, &pf));
-  NB_TRY(check_opts(opts));
-  if (n_rays <= 0 || !offsets9) {
-    set_error("workspace_layout: invalid argument");
-    return NERFB200_ERR_INVALID;
-  }
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
-  const int64_t v[9] = {w.z_c, w.raw_c, w.w_c, w.z_f, w.raw_f, w.stash_c, w.stash_f, w.gstash, w.d_raw};
-  for (int i = 0; i < 9; ++i) offsets9[i] = v[i];
-  return NERFB200_OK;
-}
-
 }  // extern "C"
 
 namespace nerfb200 {
@@ -775,16 +765,8 @@ static int render_randoms(const char* what, const nerfb200_render_opts_t& o, con
   return NERFB200_OK;
 }
 
-}  // namespace nerfb200
-
-extern "C" {
-
-}  // extern "C"
-
-namespace nerfb200 {
-
-// The sections an occupancy-grid render adds after render_fwd's inference workspace, sized for the larger (fine) pass
-// and reused by both passes: the compaction scratch, the row map, its blocks and the live block count.
+// An occupancy grid's sections, reused by both passes: the compaction scratch, the row map, its blocks and the live
+// block count.
 struct GridWorkspace {
   int64_t scratch, map, blocks, n_blocks, total;
 };
@@ -799,9 +781,8 @@ static GridWorkspace carve_grid(int64_t base, int64_t n_rays, int n_samples) {
   return g;
 }
 
-// The sections an early-stopping render adds after the grid sections (sized for the coarse pass, which the grid may
-// compact): the per-ray state of the last pass (StopState), the groups' first blocks, one round's row map, its blocks,
-// block count and row total.
+// The sections of an early-stopping last pass: its per-ray state (StopState), the groups' first blocks, one round's row
+// map, its blocks, block count and row total.
 struct StopWorkspace {
   int64_t order, n_eval, T, counts, first_block, map, blocks, n_blocks, rows, total;
 };
@@ -822,121 +803,176 @@ static StopWorkspace carve_stop(int64_t base, int64_t n_rays, int n_samples) {
   return sw;
 }
 
-// early ray termination of the last pass: the threshold and the optional stop_sample output
-struct StopArgs {
-  float t;
+// A normal map's sections: the last pass's weights, the compaction's count / first / total, the compacted points and
+// their density_grad output.
+struct NormalWorkspace {
+  int64_t weights, count, first, total, pts, grad, end;
+};
+static NormalWorkspace carve_normal(int64_t base, int64_t n_rays, int n_samples) {
+  NormalWorkspace nw;
+  const int64_t P = n_rays * n_samples;
+  nw.weights = base;
+  nw.count = nw.weights + align256(P * 4);
+  nw.first = nw.count + align256(n_rays * 4);
+  nw.total = nw.first + align256(n_rays * 4);
+  nw.pts = nw.total + 256;
+  nw.grad = nw.pts + align256(P * 12);
+  nw.end = nw.grad + align256(P * 16);
+  return nw;
+}
+
+// The sections the inference variants add after the base workspace, in this order.  The grid's are sized for the
+// larger pass it compacts: the fine pass, unless that pass stops early (then the stop rounds compact it).  The stop
+// sections are sized for the last pass.  The normal map's follow the layout without early stopping, the larger of the
+// two, so that their offsets do not depend on it.
+struct ExtraWorkspace {
+  GridWorkspace grid;
+  StopWorkspace stop;
+  NormalWorkspace normal;
+};
+static ExtraWorkspace carve_extras(const RenderSetup& r, int64_t n_rays, bool stop) {
+  const int n_last = r.fine ? r.ns : r.nc;
+  const GridWorkspace g = carve_grid(r.w.total, n_rays, stop ? r.nc : n_last);
+  const StopWorkspace widest = carve_stop(carve_grid(r.w.total, n_rays, n_last).total, n_rays, n_last);
+  return {g, carve_stop(g.total, n_rays, n_last), carve_normal(widest.total, n_rays, n_last)};
+}
+
+// A render_fwd-family call: render_fwd's arguments, then what the inference variants add to them.  Those are an
+// occupancy grid (grid != NULL), early ray termination of the last pass below transmittance stop_t with its optional
+// stop_sample output, the last pass's weights written to last_weights (normal maps), and the evaluated samples of each
+// pass counted into n_evaluated.
+struct RenderCall {
+  const nerfb200_arch_t *arch_c, *arch_f;
+  const nerfb200_render_opts_t* opts;
+  const float *blob_c, *blob_f, *rays;
+  int32_t ray_stride;
+  int64_t n_rays;
+  const nerfb200_rng_t* rng;
+  const float* tensor[4];  // t_rand, noise_c, u, noise_f
+  float *out_coarse, *out_fine;
+  void* workspace;
+  int32_t training, impl;
+  void* stream;
+  const nerfb200_grid_t* grid;
+  const uint32_t* bits;
+  bool stop;
+  float stop_t;
   int32_t* stop_sample;
+  float* last_weights;
+  int64_t* n_evaluated;
 };
 
-// render_fwd, and with a grid (grid != NULL, inference only) the same passes with the MLP run over each pass's compacted
-// samples.  Without a grid the launches are exactly render_fwd's.
-static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                          const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                          const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                          const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
-                          const nerfb200_grid_t* grid, const uint32_t* bits, int64_t* n_evaluated, float* out_coarse,
-                          float* out_fine, void* workspace, int32_t training, int32_t impl, void* stream,
-                          const StopArgs* stop = nullptr, float* last_weights = nullptr) {
-  Plan pc, pf;
-  NB_TRY(build_plan(arch_c, &pc));
-  NB_TRY(check_opts(opts));
-  const float* const tensor[4] = {t_rand, noise_c, u, noise_f};
-  RandSrc rnd[4];
-  NB_TRY(render_randoms(what, *opts, rng, tensor, rnd));
-  const bool fine = opts->n_fine > 0;
-  if (fine) {
-    if (!arch_f || !blob_f || !out_fine) {
-      set_error("%s: fine pass requested but fine model / output missing", what);
-      return NERFB200_ERR_INVALID;
-    }
-    NB_TRY(build_plan(arch_f, &pf));
+static int check_grid_bits(const char* what, const nerfb200_grid_t* grid, const uint32_t* bits) {
+  if ((grid == nullptr) == (bits == nullptr)) return NERFB200_OK;
+  set_error("%s: a grid descriptor and its bits come together (descriptor %s, bits %s)", what, grid ? "given" : "NULL",
+            bits ? "given" : "NULL");
+  return NERFB200_ERR_INVALID;
+}
+
+// The refusals of a render_fwd-family call after its setup, in order and before any launch; rnd receives the call's
+// random sources.
+static int check_forward(const char* what, const RenderCall& a, const RenderSetup& r, RandSrc rnd[4]) {
+  const nerfb200_render_opts_t& o = *a.opts;
+  NB_TRY(render_randoms(what, o, a.rng, a.tensor, rnd));
+  if (o.n_fine > 0 && (!a.arch_f || !a.blob_f || !a.out_fine)) {
+    set_error("%s: fine pass requested but fine model / output missing", what);
+    return NERFB200_ERR_INVALID;
   }
-  if (!rays || !out_coarse || !workspace || !blob_c || n_rays <= 0) {
+  if (!a.rays || !a.out_coarse || !a.workspace || !a.blob_c) {
     set_error("%s: null pointer or empty batch", what);
     return NERFB200_ERR_INVALID;
   }
-  if (opts->perturb && (!rnd[kRandTRand].present() || (fine && !rnd[kRandU].present()))) {
+  if (o.perturb && (!rnd[kRandTRand].present() || (r.fine && !rnd[kRandU].present()))) {
     set_error("%s: perturb set but t_rand or u missing", what);
     return NERFB200_ERR_INVALID;
   }
-  if (grid) {
-    NB_TRY(check_grid(grid, what));
-    if (!bits) {
+  if (a.grid) {
+    NB_TRY(check_grid(a.grid, what));
+    if (!a.bits) {
       set_error("%s: null grid bitfield", what);
       return NERFB200_ERR_INVALID;
     }
-    if (training || impl == 0) {
+    if (a.training || a.impl == 0) {
       set_error("%s: the occupancy grid renders only (training = 0), on the wgmma inference forward: impl 1 or 3, not "
-                "impl=%d", what, impl);
+                "impl=%d", what, a.impl);
       return NERFB200_ERR_UNSUPPORTED;
     }
-    if (grid_max_blocks(n_rays, opts->n_coarse + opts->n_fine) * 64 >= (int64_t(1) << 31)) {
+    if (grid_max_blocks(a.n_rays, r.ns) * 64 >= (int64_t(1) << 31)) {
       set_error("%s: more than 2^31 map rows in one call; chunk the rays", what);
       return NERFB200_ERR_UNSUPPORTED;
     }
   }
-  if (stop) {
-    if (training || impl == 0) {
+  if (a.stop) {
+    if (a.training || a.impl == 0) {
       set_error("%s: early ray termination renders only (training = 0), on the wgmma inference forward: impl 1 or 3, "
-                "not impl=%d", what, impl);
+                "not impl=%d", what, a.impl);
       return NERFB200_ERR_UNSUPPORTED;
     }
-    if (!(stop->t >= 0.f && stop->t < 1.f)) {
-      set_error("%s: stop_transmittance %g must be in [0, 1)", what, stop->t);
+    if (!(a.stop_t >= 0.f && a.stop_t < 1.f)) {
+      set_error("%s: stop_transmittance %g must be in [0, 1)", what, a.stop_t);
       return NERFB200_ERR_INVALID;
     }
   }
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, training, &w);
-  char* base = static_cast<char*>(workspace);
+  const char* base = static_cast<const char*>(a.workspace);
+  const Need need = a.training ? kStash : kInference;
+  NB_TRY(check_mlp_args(r.pc, a.blob_c, a.rays, a.ray_stride, reinterpret_cast<const float*>(base + r.w.z_c), a.n_rays,
+                        r.nc));
+  NB_TRY(check_impl(r.pc, a.impl, r.nc, need, what));
+  if (!r.fine) return NERFB200_OK;
+  NB_TRY(check_mlp_args(r.pf, a.blob_f, a.rays, a.ray_stride, reinterpret_cast<const float*>(base + r.w.z_f), a.n_rays,
+                        r.ns));
+  return check_impl(r.pf, a.impl, r.ns, need, what);
+}
+
+// The passes of a checked render_fwd-family call.  Without extras the launches are exactly render_fwd's; with a grid
+// (inference only) the MLP runs over each pass's compacted samples.
+static int render_forward(const RenderCall& a, const RenderSetup& r, const RandSrc rnd[4]) {
+  const nerfb200_render_opts_t& o = *a.opts;
+  const int64_t n_rays = a.n_rays;
+  const float* rays = a.rays;
+  const int ray_stride = a.ray_stride, nc = r.nc;
+  char* base = static_cast<char*>(a.workspace);
   auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
   auto I = [&](int64_t off) { return reinterpret_cast<int*>(base + off); };
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const Need need = training ? kStash : kInference;
-  NB_TRY(check_mlp_args(pc, blob_c, rays, ray_stride, F(w.z_c), n_rays, nc));
-  NB_TRY(check_impl(pc, impl, nc, need, what));
-  if (fine) {
-    NB_TRY(check_mlp_args(pf, blob_f, rays, ray_stride, F(w.z_f), n_rays, ns));
-    NB_TRY(check_impl(pf, impl, ns, need, what));
-  }
-  const GridWorkspace gw = carve_grid(w.total, n_rays, fine && !stop ? ns : nc);
-  const StopWorkspace sw = carve_stop(gw.total, n_rays, fine ? ns : nc);
+  cudaStream_t s = static_cast<cudaStream_t>(a.stream);
+  const ExtraWorkspace e = carve_extras(r, n_rays, a.stop);
   // the last pass with early ray termination: one marking launch, then rounds of compaction, MLP and the per-ray
   // transmittance update.  Rounds after every ray has finished have no blocks.
   auto stop_rounds = [&](bool is_fine, const Plan& p, const float* blob, int n, const float* z, float* raw) {
+    const StopWorkspace& sw = e.stop;
     const int64_t groups = (n_rays + kGridGroupRays - 1) / kGridGroupRays;
-    const StopState st{I(sw.order), I(sw.n_eval), F(sw.T), stop->stop_sample, I(sw.counts)};
+    const StopState st{I(sw.order), I(sw.n_eval), F(sw.T), a.stop_sample, I(sw.counts)};
     int* nb = I(sw.n_blocks);
     int64_t* rows = reinterpret_cast<int64_t*>(base + sw.rows);
     // the coarse pass of a two-pass render without a grid ran every sample
-    int64_t* coarse_rows = (is_fine && !grid && n_evaluated) ? n_evaluated : nullptr;
-    NB_TRY(launch_stop_mark(grid ? *grid : nerfb200_grid_t{}, bits, rays, ray_stride, z, n_rays, n, raw, st, coarse_rows,
-                            n_rays * nc, s));
+    int64_t* coarse_rows = (is_fine && !a.grid && a.n_evaluated) ? a.n_evaluated : nullptr;
+    NB_TRY(launch_stop_mark(a.grid ? *a.grid : nerfb200_grid_t{}, a.bits, rays, ray_stride, z, n_rays, n, raw, st,
+                            coarse_rows, n_rays * nc, s));
     const RowMap m{I(sw.map), reinterpret_cast<const int2*>(base + sw.blocks), nb};
     const int64_t mb = stop_round_max_blocks(n_rays, n);
     for (int k = 0; k * kStopRound < n; ++k) {
       NB_TRY(launch_grid_scan(I(sw.counts), groups, I(sw.first_block), nb, rows, s));
       NB_TRY(launch_stop_scatter(st, I(sw.first_block), n_rays, n, k, I(sw.map), I(sw.blocks), s));
-      NB_TRY(launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, mb, raw, impl == 3, s));
-      NB_TRY(launch_stop_update(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], opts->noise_std,
-                                n_rays, n, k, stop->t, st, rows, n_evaluated ? n_evaluated + is_fine : nullptr, s));
+      NB_TRY(launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, mb, raw, a.impl == 3, s));
+      NB_TRY(launch_stop_update(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], o.noise_std,
+                                n_rays, n, k, a.stop_t, st, rows, a.n_evaluated ? a.n_evaluated + is_fine : nullptr, s));
     }
     return NERFB200_OK;
   };
   // the MLP of one pass: every sample, or with a grid the compacted samples (skipped ones get raw = [0 0 0 -inf]), or
   // in the last pass of an early-stopping render the rounds above
   auto mlp = [&](bool is_fine, const Plan& p, const float* blob, int n, const float* z, float* raw, float* stash) {
-    if (stop && is_fine == fine) return stop_rounds(is_fine, p, blob, n, z, raw);
-    if (!grid)
-      return mlp_forward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, training ? stash : nullptr, s);
-    int* nb = reinterpret_cast<int*>(base + gw.n_blocks);
-    NB_TRY(launch_grid_compact(*grid, bits, rays, ray_stride, z, n_rays, n, raw, reinterpret_cast<int*>(base + gw.map),
-                               reinterpret_cast<int*>(base + gw.blocks), nb, n_evaluated ? n_evaluated + is_fine : nullptr,
-                               reinterpret_cast<int*>(base + gw.scratch), s));
-    const RowMap m{reinterpret_cast<const int*>(base + gw.map), reinterpret_cast<const int2*>(base + gw.blocks), nb};
-    return launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, grid_max_blocks(n_rays, n), raw, impl == 3,
-                                 s);
+    if (a.stop && is_fine == r.fine) return stop_rounds(is_fine, p, blob, n, z, raw);
+    if (!a.grid)
+      return mlp_forward(p, a.impl, blob, ray_points(rays, ray_stride, z), n_rays, n, raw, a.training ? stash : nullptr,
+                         s);
+    const GridWorkspace& gw = e.grid;
+    int* nb = I(gw.n_blocks);
+    NB_TRY(launch_grid_compact(*a.grid, a.bits, rays, ray_stride, z, n_rays, n, raw, I(gw.map), I(gw.blocks), nb,
+                               a.n_evaluated ? a.n_evaluated + is_fine : nullptr, I(gw.scratch), s));
+    const RowMap m{I(gw.map), reinterpret_cast<const int2*>(base + gw.blocks), nb};
+    return launch_mlp_fwd_tc_map(p, blob, rays, ray_stride, z, n_rays, n, m, grid_max_blocks(n_rays, n), raw,
+                                 a.impl == 3, s);
   };
 
   // one pass: depths -> MLP -> compositing.  The coarse pass (train_utils.py:45-94) takes stratified depths, the fine
@@ -944,24 +980,98 @@ static int render_forward(const char* what, const nerfb200_arch_t* arch_c, const
   auto pass = [&](bool is_fine, const Plan& p, const float* blob, int n, float* z, float* raw, float* stash,
                   float* out, float* weights) {
     if (is_fine)
-      NB_TRY(launch_sample_pdf_merge(F(w.z_c), F(w.w_c), rnd[kRandU], nullptr, n_rays, nc, opts->n_fine, z, nullptr,
+      NB_TRY(launch_sample_pdf_merge(F(r.w.z_c), F(r.w.w_c), rnd[kRandU], nullptr, n_rays, nc, o.n_fine, z, nullptr,
                                      nullptr, nullptr, s));
     else
-      NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, opts->perturb, opts->lindisp, z, s));
+      NB_TRY(launch_sample_coarse(rays, ray_stride, n_rays, rnd[kRandTRand], nc, o.perturb, o.lindisp, z, s));
     NB_TRY(mlp(is_fine, p, blob, n, z, raw, stash));
     return launch_composite_fwd(raw, z, rays + 3, ray_stride, rnd[is_fine ? kRandNoiseF : kRandNoiseC], n_rays, n,
-                                opts->noise_std, opts->white_bkgd, out, weights, s);
+                                o.noise_std, o.white_bkgd, out, weights, s);
   };
   // last_weights (normal maps): the last pass's compositing also writes its weights there
-  NB_TRY(pass(false, pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), out_coarse,
-              fine || !last_weights ? F(w.w_c) : last_weights));
-  if (!fine) return NERFB200_OK;
-  return pass(true, pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), out_fine, last_weights);
+  NB_TRY(pass(false, r.pc, a.blob_c, nc, F(r.w.z_c), F(r.w.raw_c), F(r.w.stash_c), a.out_coarse,
+              r.fine || !a.last_weights ? F(r.w.w_c) : a.last_weights));
+  if (!r.fine) return NERFB200_OK;
+  return pass(true, r.pf, a.blob_f, r.ns, F(r.w.z_f), F(r.w.raw_f), F(r.w.stash_f), a.out_fine, a.last_weights);
+}
+
+// render_fwd, render_fwd_grid and render_fwd_early_stop: the setup, the checks, then the passes
+static int render_forward_call(const char* what, const RenderCall& a) {
+  char empty[96];
+  snprintf(empty, sizeof(empty), "%s: null pointer or empty batch", what);
+  RenderSetup r;
+  NB_TRY(render_setup(a.arch_c, a.opts && a.opts->n_fine > 0 ? a.arch_f : nullptr, a.opts, a.n_rays, a.training, empty,
+                      &r));
+  RandSrc rnd[4];
+  NB_TRY(check_forward(what, a, r, rnd));
+  return render_forward(a, r, rnd);
+}
+
+// render_fwd_normals, and with `world` its NDC render's world-space normal map (nerfb200.h "NDC scenes")
+static int render_normals(const char* what, RenderCall a, float* normals, const NdcMap* world) {
+  NB_TRY(check_grid_bits(what, a.grid, a.bits));
+  if (a.stop_t != a.stop_t) {
+    set_error("%s: stop_transmittance is NaN (negative: no early stopping)", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (!normals || !a.workspace) {
+    set_error("%s: null normals or workspace", what);
+    return NERFB200_ERR_INVALID;
+  }
+  NB_TRY(check_opts(a.opts));
+  const bool fine = a.opts->n_fine > 0;
+  Plan pl;
+  NB_TRY(build_plan(fine ? a.arch_f : a.arch_c, &pl));
+  NB_TRY(check_impl(pl, a.impl, 0, kGradient, what));  // impl 1 alone, before any launch
+  RenderSetup r;
+  NB_TRY(render_setup(a.arch_c, fine ? a.arch_f : nullptr, a.opts, a.n_rays, /*training=*/0,
+                      "render_fwd_normals: empty batch", &r));
+  a.stop = a.stop_t >= 0.f;
+  const NormalWorkspace nw = carve_extras(r, a.n_rays, a.stop).normal;
+  char* base = static_cast<char*>(a.workspace);
+  a.last_weights = reinterpret_cast<float*>(base + nw.weights);
+  RandSrc rnd[4];
+  NB_TRY(check_forward(what, a, r, rnd));
+  NB_TRY(render_forward(a, r, rnd));
+  const int64_t n_rays = a.n_rays;
+  const int n_last = fine ? r.ns : r.nc;
+  const float* z_last = reinterpret_cast<const float*>(base + (fine ? r.w.z_f : r.w.z_c));
+  const NormalState st{reinterpret_cast<int*>(base + nw.count), reinterpret_cast<int*>(base + nw.first),
+                       reinterpret_cast<int*>(base + nw.total), reinterpret_cast<float*>(base + nw.pts),
+                       reinterpret_cast<float*>(base + nw.grad)};
+  cudaStream_t s = static_cast<cudaStream_t>(a.stream);
+  NB_TRY(launch_normal_compact(a.rays, a.ray_stride, z_last, a.last_weights, n_rays, n_last, st, s));
+  NB_TRY(launch_density_grad_tc(pl, fine ? a.blob_f : a.blob_c, st.pts, n_rays * n_last, st.grad, st.total, s));
+  return launch_normal_sum(a.last_weights, n_rays, n_last, st, normals, s, world);
 }
 
 }  // namespace nerfb200
 
 extern "C" {
+
+int64_t nerfb200_render_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                        const nerfb200_render_opts_t* opts, int64_t n_rays, int32_t training) {
+  RenderSetup r;
+  if (render_setup(coarse, fine, opts, n_rays, training, nullptr, &r) != NERFB200_OK) return -1;
+  return r.w.total;
+}
+
+/* Byte offsets of the named sections of the render workspace (test hook): order
+ * z_coarse, raw_coarse, weights_coarse, z_fine, raw_fine, stash_coarse, stash_fine, gstash, d_raw. */
+int32_t nerfb200_render_workspace_layout(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
+                                         const nerfb200_render_opts_t* opts, int64_t n_rays, int32_t training,
+                                         int64_t* offsets9) {
+  RenderSetup r;
+  NB_TRY(render_setup(coarse, fine, opts, n_rays, training, "workspace_layout: invalid argument", &r));
+  if (!offsets9) {
+    set_error("workspace_layout: invalid argument");
+    return NERFB200_ERR_INVALID;
+  }
+  const Workspace& w = r.w;
+  const int64_t v[9] = {w.z_c, w.raw_c, w.w_c, w.z_f, w.raw_f, w.stash_c, w.stash_f, w.gstash, w.d_raw};
+  for (int i = 0; i < 9; ++i) offsets9[i] = v[i];
+  return NERFB200_OK;
+}
 
 int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
                             const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
@@ -969,21 +1079,16 @@ int32_t nerfb200_render_fwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
                             float* out_coarse, float* out_fine, void* workspace, int32_t training, int32_t impl,
                             void* stream) {
-  return render_forward("render_fwd", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand,
-                        noise_c, u, noise_f, nullptr, nullptr, nullptr, out_coarse, out_fine, workspace, training, impl,
-                        stream);
+  return render_forward_call("render_fwd", {arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                                            {t_rand, noise_c, u, noise_f}, out_coarse, out_fine, workspace, training,
+                                            impl, stream});
 }
 
 int64_t nerfb200_render_grid_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
                                              const nerfb200_render_opts_t* opts, int64_t n_rays) {
-  Plan pc, pf;
-  if (build_plan(coarse, &pc) != NERFB200_OK) return -1;
-  if (fine && build_plan(fine, &pf) != NERFB200_OK) return -1;
-  if (check_opts(opts) != NERFB200_OK || n_rays <= 0) return -1;
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
-  const bool has_fine = fine && opts->n_fine > 0;
-  return carve_grid(w.total, n_rays, has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse).total;
+  RenderSetup r;
+  if (render_setup(coarse, fine, opts, n_rays, /*training=*/0, nullptr, &r) != NERFB200_OK) return -1;
+  return carve_extras(r, n_rays, /*stop=*/false).grid.total;
 }
 
 int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
@@ -996,24 +1101,19 @@ int32_t nerfb200_render_fwd_grid(const nerfb200_arch_t* arch_c, const nerfb200_a
     set_error("render_fwd_grid: null grid descriptor");
     return NERFB200_ERR_INVALID;
   }
-  return render_forward("render_fwd_grid", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand,
-                        noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace, /*training=*/0,
-                        impl, stream);
+  return render_forward_call("render_fwd_grid", {arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                                                 {t_rand, noise_c, u, noise_f}, out_coarse, out_fine, workspace,
+                                                 /*training=*/0, impl, stream, grid, bits, false, 0.f, nullptr,
+                                                 nullptr, n_evaluated});
 }
 
 int32_t nerfb200_render_early_stop_round(void) { return kStopRound; }
 
 int64_t nerfb200_render_early_stop_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
                                                    const nerfb200_render_opts_t* opts, int64_t n_rays) {
-  Plan pc, pf;
-  if (build_plan(coarse, &pc) != NERFB200_OK) return -1;
-  if (fine && build_plan(fine, &pf) != NERFB200_OK) return -1;
-  if (check_opts(opts) != NERFB200_OK || n_rays <= 0) return -1;
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
-  const bool has_fine = fine && opts->n_fine > 0;
-  const GridWorkspace gw = carve_grid(w.total, n_rays, opts->n_coarse);
-  return carve_stop(gw.total, n_rays, has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse).total;
+  RenderSetup r;
+  if (render_setup(coarse, fine, opts, n_rays, /*training=*/0, nullptr, &r) != NERFB200_OK) return -1;
+  return carve_extras(r, n_rays, /*stop=*/true).stop.total;
 }
 
 int32_t nerfb200_render_fwd_early_stop(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
@@ -1023,123 +1123,20 @@ int32_t nerfb200_render_fwd_early_stop(const nerfb200_arch_t* arch_c, const nerf
                                        const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
                                        float* out_coarse, float* out_fine, void* workspace, int32_t impl,
                                        int64_t* n_evaluated, int32_t* stop_sample, void* stream) {
-  if ((grid == nullptr) != (bits == nullptr)) {
-    set_error("render_fwd_early_stop: a grid descriptor and its bits come together (descriptor %s, bits %s)",
-              grid ? "given" : "NULL", bits ? "given" : "NULL");
-    return NERFB200_ERR_INVALID;
-  }
-  const StopArgs stop{stop_transmittance, stop_sample};
-  return render_forward("render_fwd_early_stop", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
-                        t_rand, noise_c, u, noise_f, grid, bits, n_evaluated, out_coarse, out_fine, workspace,
-                        /*training=*/0, impl, stream, &stop);
+  NB_TRY(check_grid_bits("render_fwd_early_stop", grid, bits));
+  return render_forward_call("render_fwd_early_stop", {arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays,
+                                                       rng, {t_rand, noise_c, u, noise_f}, out_coarse, out_fine,
+                                                       workspace, /*training=*/0, impl, stream, grid, bits, true,
+                                                       stop_transmittance, stop_sample, nullptr, n_evaluated});
 }
-
-}  // extern "C"
-
-namespace nerfb200 {
-
-// The sections a normal-map render adds after everything render_forward may use (the grid and early-stopping sections
-// of either layout): the last pass's weights, the compaction's count / first / total, the compacted points and their
-// density_grad output.
-struct NormalWorkspace {
-  int64_t weights, count, first, total, pts, grad, end;
-};
-static int normal_workspace(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
-                            const nerfb200_render_opts_t* opts, int64_t n_rays, NormalWorkspace* nw) {
-  Plan pc, pf;
-  NB_TRY(build_plan(coarse, &pc));
-  if (fine) NB_TRY(build_plan(fine, &pf));
-  NB_TRY(check_opts(opts));
-  if (n_rays <= 0) {
-    set_error("render_fwd_normals: empty batch");
-    return NERFB200_ERR_INVALID;
-  }
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
-  const bool has_fine = fine && opts->n_fine > 0;
-  const int n_last = has_fine ? opts->n_coarse + opts->n_fine : opts->n_coarse;
-  const int64_t a = carve_stop(carve_grid(w.total, n_rays, opts->n_coarse).total, n_rays, n_last).total;
-  const int64_t b = carve_stop(carve_grid(w.total, n_rays, n_last).total, n_rays, n_last).total;
-  const int64_t P = n_rays * n_last;
-  nw->weights = a > b ? a : b;
-  nw->count = nw->weights + align256(P * 4);
-  nw->first = nw->count + align256(n_rays * 4);
-  nw->total = nw->first + align256(n_rays * 4);
-  nw->pts = nw->total + 256;
-  nw->grad = nw->pts + align256(P * 12);
-  nw->end = nw->grad + align256(P * 16);
-  return NERFB200_OK;
-}
-
-}  // namespace nerfb200
-
-extern "C" {
 
 int64_t nerfb200_render_normals_workspace_bytes(const nerfb200_arch_t* coarse, const nerfb200_arch_t* fine,
                                                 const nerfb200_render_opts_t* opts, int64_t n_rays) {
-  NormalWorkspace nw;
-  if (normal_workspace(coarse, fine, opts, n_rays, &nw) != NERFB200_OK) return -1;
-  return nw.end;
+  RenderSetup r;
+  if (render_setup(coarse, fine, opts, n_rays, /*training=*/0, "render_fwd_normals: empty batch", &r) != NERFB200_OK)
+    return -1;
+  return carve_extras(r, n_rays, /*stop=*/false).normal.end;
 }
-
-}  // extern "C"
-
-namespace nerfb200 {
-
-// render_fwd_normals, and with `world` its NDC render's world-space normal map (nerfb200.h "NDC scenes")
-static int render_normals(const char* what, const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
-                          const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
-                          const float* rays, int32_t ray_stride, int64_t n_rays, const nerfb200_rng_t* rng,
-                          const float* t_rand, const float* noise_c, const float* u, const float* noise_f,
-                          const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
-                          float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
-                          void* stream, const NdcMap* world) {
-  if ((grid == nullptr) != (bits == nullptr)) {
-    set_error("%s: a grid descriptor and its bits come together", what);
-    return NERFB200_ERR_INVALID;
-  }
-  if (stop_transmittance != stop_transmittance) {
-    set_error("%s: stop_transmittance is NaN (negative: no early stopping)", what);
-    return NERFB200_ERR_INVALID;
-  }
-  if (!normals || !workspace) {
-    set_error("%s: null normals or workspace", what);
-    return NERFB200_ERR_INVALID;
-  }
-  NB_TRY(check_opts(opts));
-  const bool fine = opts->n_fine > 0;
-  const nerfb200_arch_t* arch_last = fine ? arch_f : arch_c;
-  const float* blob_last = fine ? blob_f : blob_c;
-  Plan pl;
-  NB_TRY(build_plan(arch_last, &pl));
-  NB_TRY(check_impl(pl, impl, 0, kGradient, what));  // impl 1 alone, before any launch
-  NormalWorkspace nw;
-  NB_TRY(normal_workspace(arch_c, fine ? arch_f : nullptr, opts, n_rays, &nw));
-  char* base = static_cast<char*>(workspace);
-  float* W = reinterpret_cast<float*>(base + nw.weights);
-  const StopArgs stop{stop_transmittance, nullptr};
-  NB_TRY(render_forward(what, arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng, t_rand, noise_c, u,
-                        noise_f, grid, bits, nullptr, out_coarse, out_fine, workspace, /*training=*/0, impl, stream,
-                        stop_transmittance >= 0.f ? &stop : nullptr, W));
-  Plan pc, pf;
-  NB_TRY(build_plan(arch_c, &pc));
-  if (fine) NB_TRY(build_plan(arch_f, &pf));
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/0, &w);
-  const int n_last = fine ? opts->n_coarse + opts->n_fine : opts->n_coarse;
-  const float* z_last = reinterpret_cast<const float*>(base + (fine ? w.z_f : w.z_c));
-  const NormalState st{reinterpret_cast<int*>(base + nw.count), reinterpret_cast<int*>(base + nw.first),
-                       reinterpret_cast<int*>(base + nw.total), reinterpret_cast<float*>(base + nw.pts),
-                       reinterpret_cast<float*>(base + nw.grad)};
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  NB_TRY(launch_normal_compact(rays, ray_stride, z_last, W, n_rays, n_last, st, s));
-  NB_TRY(launch_density_grad_tc(pl, blob_last, st.pts, n_rays * n_last, st.grad, st.total, s));
-  return launch_normal_sum(W, n_rays, n_last, st, normals, s, world);
-}
-
-}  // namespace nerfb200
-
-extern "C" {
 
 int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
                                     const nerfb200_render_opts_t* opts, const float* blob_c, const float* blob_f,
@@ -1148,9 +1145,10 @@ int32_t nerfb200_render_fwd_normals(const nerfb200_arch_t* arch_c, const nerfb20
                                     const nerfb200_grid_t* grid, const uint32_t* bits, float stop_transmittance,
                                     float* out_coarse, float* out_fine, float* normals, void* workspace, int32_t impl,
                                     void* stream) {
-  return render_normals("render_fwd_normals", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
-                        t_rand, noise_c, u, noise_f, grid, bits, stop_transmittance, out_coarse, out_fine, normals,
-                        workspace, impl, stream, nullptr);
+  return render_normals("render_fwd_normals", {arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                                               {t_rand, noise_c, u, noise_f}, out_coarse, out_fine, workspace,
+                                               /*training=*/0, impl, stream, grid, bits, false, stop_transmittance},
+                        normals, nullptr);
 }
 
 int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const nerfb200_arch_t* arch_f,
@@ -1163,9 +1161,11 @@ int32_t nerfb200_render_fwd_normals_ndc(const nerfb200_arch_t* arch_c, const ner
                                         int32_t impl, void* stream) {
   NdcMap m;
   NB_TRY(make_ndc_map(ndc, &m, "render_fwd_normals_ndc"));
-  return render_normals("render_fwd_normals_ndc", arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
-                        t_rand, noise_c, u, noise_f, grid, bits, stop_transmittance, out_coarse, out_fine, normals,
-                        workspace, impl, stream, &m);
+  return render_normals("render_fwd_normals_ndc", {arch_c, arch_f, opts, blob_c, blob_f, rays, ray_stride, n_rays, rng,
+                                                   {t_rand, noise_c, u, noise_f}, out_coarse, out_fine, workspace,
+                                                   /*training=*/0, impl, stream, grid, bits, false,
+                                                   stop_transmittance},
+                        normals, &m);
 }
 
 int32_t nerfb200_ndc_mesh_to_world(const nerfb200_ndc_t* ndc, const float* vertices, const int32_t* faces,
@@ -1209,21 +1209,18 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
                             const float* noise_c, const float* noise_f, const float* g_coarse, const float* g_fine,
                             void* workspace, float* flat_grad_c, float* flat_grad_f, int32_t impl, int32_t parts,
                             void* stream) {
-  Plan pc, pf;
-  NB_TRY(build_plan(arch_c, &pc));
-  NB_TRY(check_opts(opts));
+  RenderSetup r;
+  NB_TRY(render_setup(arch_c, opts && opts->n_fine > 0 ? arch_f : nullptr, opts, n_rays, /*training=*/1,
+                      "render_bwd: null pointer or empty batch", &r));
   const float* const tensor[4] = {nullptr, noise_c, nullptr, noise_f};
   RandSrc rnd[4];
   NB_TRY(render_randoms("render_bwd", *opts, rng, tensor, rnd));
   const bool fine = opts->n_fine > 0;
-  if (fine) {
-    if (!arch_f || !blob_f || !g_fine || !flat_grad_f) {
-      set_error("render_bwd: fine pass present but fine model / grads missing");
-      return NERFB200_ERR_INVALID;
-    }
-    NB_TRY(build_plan(arch_f, &pf));
+  if (fine && (!arch_f || !blob_f || !g_fine || !flat_grad_f)) {
+    set_error("render_bwd: fine pass present but fine model / grads missing");
+    return NERFB200_ERR_INVALID;
   }
-  if (!rays || !g_coarse || !workspace || !blob_c || !flat_grad_c || n_rays <= 0) {
+  if (!rays || !g_coarse || !workspace || !blob_c || !flat_grad_c) {
     set_error("render_bwd: null pointer or empty batch");
     return NERFB200_ERR_INVALID;
   }
@@ -1232,11 +1229,8 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
     return NERFB200_ERR_INVALID;
   }
   const bool run_fine = fine && (parts & 1), run_coarse = parts & 2;
-  const int nc = opts->n_coarse, ns = opts->n_coarse + opts->n_fine;
-  if (run_fine) NB_TRY(check_impl(pf, impl, ns, kBackward, "render_bwd"));
-  if (run_coarse) NB_TRY(check_impl(pc, impl, nc, kBackward, "render_bwd"));
-  Workspace w;
-  carve(pc, fine ? &pf : nullptr, *opts, n_rays, /*training=*/1, &w);
+  if (run_fine) NB_TRY(check_impl(r.pf, impl, r.ns, kBackward, "render_bwd"));
+  if (run_coarse) NB_TRY(check_impl(r.pc, impl, r.nc, kBackward, "render_bwd"));
   char* base = static_cast<char*>(workspace);
   auto F = [&](int64_t off) { return reinterpret_cast<float*>(base + off); };
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1245,16 +1239,16 @@ int32_t nerfb200_render_bwd(const nerfb200_arch_t* arch_c, const nerfb200_arch_t
   auto part = [&](const Plan& p, const float* blob, int n, const float* z, const float* raw, const float* stash,
                   const RandSrc& noise, const float* g, float* flat_grad) {
     NB_TRY(launch_composite_bwd(raw, z, rays + 3, ray_stride, noise, g, nullptr, /*sample_grads=*/false, n_rays, n,
-                                opts->noise_std, opts->white_bkgd, F(w.d_raw), s));
-    return mlp_backward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, F(w.d_raw), stash, F(w.gstash),
+                                opts->noise_std, opts->white_bkgd, F(r.w.d_raw), s));
+    return mlp_backward(p, impl, blob, ray_points(rays, ray_stride, z), n_rays, n, F(r.w.d_raw), stash, F(r.w.gstash),
                         flat_grad, s);
   };
   if (run_fine)
-    NB_TRY(part(pf, blob_f, ns, F(w.z_f), F(w.raw_f), F(w.stash_f), rnd[kRandNoiseF], g_fine, flat_grad_f));
+    NB_TRY(part(r.pf, blob_f, r.ns, F(r.w.z_f), F(r.w.raw_f), F(r.w.stash_f), rnd[kRandNoiseF], g_fine, flat_grad_f));
   if (!run_coarse) return NERFB200_OK;
   // the coarse weights feed the resampler only through a detach (train_utils.py:103), so the
   // coarse net's gradient comes from rgb/disp/acc_coarse alone.
-  return part(pc, blob_c, nc, F(w.z_c), F(w.raw_c), F(w.stash_c), rnd[kRandNoiseC], g_coarse, flat_grad_c);
+  return part(r.pc, blob_c, r.nc, F(r.w.z_c), F(r.w.raw_c), F(r.w.stash_c), rnd[kRandNoiseC], g_coarse, flat_grad_c);
 }
 
 int32_t nerfb200_random_fill(const nerfb200_rng_t* rng, int32_t stream_id, int64_t n_rays, int32_t per_ray, float* out,

@@ -566,24 +566,27 @@ WS_SECTIONS = ("z_coarse", "raw_coarse", "weights_coarse", "z_fine", "raw_fine",
                "gstash", "d_raw")
 
 
-def render_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int, training: bool) -> int:
-    lib = _lib.load()
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if arch_f is not None else None
-    n = lib.nerfb200_render_workspace_bytes(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                            n_rays, int(training))
+def _archs(arch_c, arch_f):
+    """The C arguments of a coarse and an optional fine ArchSpec."""
+    return C.byref(arch_c.c_struct()), (C.byref(arch_f.c_struct()) if arch_f is not None else None)
+
+
+def _render_bytes(query, arch_c, arch_f, opts: RenderOpts, n_rays: int, *rest) -> int:
+    """The workspace bytes nerfb200_<query> returns; its -1 raises NotImplementedError."""
+    n = getattr(_lib.load(), "nerfb200_" + query)(*_archs(arch_c, arch_f), C.byref(opts), n_rays, *rest)
     if n < 0:
-        _lib.check(_lib.ERR_UNSUPPORTED, "render_workspace_bytes")
+        _lib.check(_lib.ERR_UNSUPPORTED, query)
     return n
 
 
+def render_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int, training: bool) -> int:
+    return _render_bytes("render_workspace_bytes", arch_c, arch_f, opts, n_rays, int(training))
+
+
 def render_workspace_layout(arch_c, arch_f, opts: RenderOpts, n_rays: int, training: bool) -> dict:
-    lib = _lib.load()
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if arch_f is not None else None
     offs = (C.c_int64 * 9)()
-    _lib.check(lib.nerfb200_render_workspace_layout(C.byref(ac), C.byref(af) if af is not None else None,
-                                                    C.byref(opts), n_rays, int(training), offs), "workspace_layout")
+    _lib.check(_lib.load().nerfb200_render_workspace_layout(*_archs(arch_c, arch_f), C.byref(opts), n_rays,
+                                                            int(training), offs), "workspace_layout")
     return dict(zip(WS_SECTIONS, list(offs)))
 
 
@@ -595,24 +598,36 @@ def _random_args(randoms):
     return (None,) + tuple(_ptr(randoms.get(k)) for k in RAND_STREAMS)
 
 
-def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, training: bool, impl: int = IMPL_SIMT,
-               workspace: Optional[torch.Tensor] = None):
-    """One ray chunk through the whole path.  Returns (out_coarse[N,8], out_fine[N,8] | None, workspace)."""
-    lib = _lib.load()
-    n = rays.shape[0]
-    dev = rays.device
+def _render_call(query, arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid, workspace, *rest):
+    """What the forward render calls share.  Returns (args, grid_args, out_c, out_f, workspace): the leading C
+    arguments (the arch pair, options, blobs, rays and random inputs), the optional grid's (descriptor, bits) checked
+    to be on the rays' device, the outputs, and ``workspace`` when it holds nerfb200_<query>'s bytes, else a new one."""
+    n, dev = rays.shape[0], rays.device
     fine = opts.n_fine > 0
-    need = render_workspace_bytes(arch_c, arch_f if fine else None, opts, n, training)
+    af = arch_f if fine else None
+    grid_args = (None, None)
+    if grid is not None:
+        g, bits = _grid_args(grid)
+        if bits.device != dev:
+            raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
+        grid_args = (C.byref(g), _ptr(bits))
+    need = _render_bytes(query, arch_c, af, opts, n, *rest)
     if workspace is None or workspace.numel() < need:
         workspace = torch.empty(need, dtype=torch.uint8, device=dev)
     out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
     out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
-    _lib.check(lib.nerfb200_render_fwd(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                       _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
-                                       *_random_args(randoms), _ptr(out_c), _ptr(out_f), _ptr(workspace),
-                                       int(training), impl, _stream()), "render_fwd")
+    args = (*_archs(arch_c, af), C.byref(opts), _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays),
+            rays.shape[1], n, *_random_args(randoms))
+    return args, grid_args, out_c, out_f, workspace
+
+
+def render_fwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, training: bool, impl: int = IMPL_SIMT,
+               workspace: Optional[torch.Tensor] = None):
+    """One ray chunk through the whole path.  Returns (out_coarse[N,8], out_fine[N,8] | None, workspace)."""
+    args, _, out_c, out_f, workspace = _render_call("render_workspace_bytes", arch_c, arch_f, opts, blob_c, blob_f,
+                                                    rays, randoms, None, workspace, int(training))
+    _lib.check(_lib.load().nerfb200_render_fwd(*args, _ptr(out_c), _ptr(out_f), _ptr(workspace), int(training), impl,
+                                               _stream()), "render_fwd")
     return out_c, out_f, workspace
 
 
@@ -620,16 +635,14 @@ def render_bwd(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, 
                flat_grad_f, impl: int = IMPL_SIMT, parts: int = 3):
     """Backward of a ``render_fwd`` workspace, given the same ``randoms`` (only the noise is needed again: a
     ``SeededRandoms`` regenerates it in-kernel, a dict supplies the tensors)."""
-    lib = _lib.load()
     fine = opts.n_fine > 0
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
     rng, _, noise_c, _, noise_f = _random_args(randoms)
-    _lib.check(lib.nerfb200_render_bwd(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                       _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
-                                       rays.shape[0], rng, noise_c, noise_f, _ptr(g_c), _ptr(g_f) if fine else None,
-                                       _ptr(workspace), _ptr(flat_grad_c), _ptr(flat_grad_f) if fine else None, impl,
-                                       int(parts), _stream()), "render_bwd")
+    _lib.check(_lib.load().nerfb200_render_bwd(*_archs(arch_c, arch_f if fine else None), C.byref(opts), _ptr(blob_c),
+                                               _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1],
+                                               rays.shape[0], rng, noise_c, noise_f, _ptr(g_c),
+                                               _ptr(g_f) if fine else None, _ptr(workspace), _ptr(flat_grad_c),
+                                               _ptr(flat_grad_f) if fine else None, impl, int(parts), _stream()),
+               "render_bwd")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -696,13 +709,7 @@ def grid_compact(grid, rays, z, raw=None):
 
 
 def render_grid_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int) -> int:
-    lib = _lib.load()
-    af = arch_f.c_struct() if arch_f is not None else None
-    n = lib.nerfb200_render_grid_workspace_bytes(C.byref(arch_c.c_struct()), C.byref(af) if af is not None else None,
-                                                 C.byref(opts), n_rays)
-    if n < 0:
-        _lib.check(_lib.ERR_UNSUPPORTED, "render_grid_workspace_bytes")
-    return n
+    return _render_bytes("render_grid_workspace_bytes", arch_c, arch_f, opts, n_rays)
 
 
 def render_fwd_grid(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid, impl: int = IMPL_TC,
@@ -710,27 +717,12 @@ def render_fwd_grid(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, rand
     """``render_fwd`` for inference with an occupancy grid (impl 1 or 3).  ``n_evaluated``: an int64 CUDA tensor of 2
     receiving the evaluated samples of the coarse and fine pass, or None.  Returns (out_coarse, out_fine | None,
     workspace); the workspace's first sections are laid out as ``render_workspace_layout(..., training=False)``."""
-    lib = _lib.load()
-    n = rays.shape[0]
-    dev = rays.device
-    fine = opts.n_fine > 0
-    g, bits = _grid_args(grid)
-    if bits.device != dev:
-        raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
+    args, grid_args, out_c, out_f, workspace = _render_call("render_grid_workspace_bytes", arch_c, arch_f, opts,
+                                                            blob_c, blob_f, rays, randoms, grid, workspace)
     if n_evaluated is not None and (n_evaluated.dtype != torch.int64 or n_evaluated.numel() < 2):
         raise RuntimeError("nerfb200: n_evaluated must be an int64 tensor of 2 elements")
-    need = render_grid_workspace_bytes(arch_c, arch_f if fine else None, opts, n)
-    if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
-    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
-    _lib.check(lib.nerfb200_render_fwd_grid(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                            _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n,
-                                            *_random_args(randoms), C.byref(g), _ptr(bits), _ptr(out_c), _ptr(out_f),
-                                            _ptr(workspace), int(impl), _ptr(n_evaluated), _stream()),
-               "render_fwd_grid")
+    _lib.check(_lib.load().nerfb200_render_fwd_grid(*args, *grid_args, _ptr(out_c), _ptr(out_f), _ptr(workspace),
+                                                    int(impl), _ptr(n_evaluated), _stream()), "render_fwd_grid")
     return out_c, out_f, workspace
 
 
@@ -743,13 +735,7 @@ def stop_round() -> int:
 
 
 def render_early_stop_workspace_bytes(arch_c, arch_f, opts: RenderOpts, n_rays: int) -> int:
-    lib = _lib.load()
-    af = arch_f.c_struct() if arch_f is not None else None
-    n = lib.nerfb200_render_early_stop_workspace_bytes(C.byref(arch_c.c_struct()),
-                                                       C.byref(af) if af is not None else None, C.byref(opts), n_rays)
-    if n < 0:
-        _lib.check(_lib.ERR_UNSUPPORTED, "render_early_stop_workspace_bytes")
-    return n
+    return _render_bytes("render_early_stop_workspace_bytes", arch_c, arch_f, opts, n_rays)
 
 
 def render_fwd_normals(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, randoms, grid=None,
@@ -759,28 +745,11 @@ def render_fwd_normals(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays, r
     the world-space normal map of an NDC render of that camera ("NDC scenes").  Returns (out_coarse, out_fine | None,
     normals[N, 3], workspace); the workspace's first sections are laid out as ``render_workspace_layout(...,
     training=False)``."""
+    args, grid_args, out_c, out_f, workspace = _render_call("render_normals_workspace_bytes", arch_c, arch_f, opts,
+                                                            blob_c, blob_f, rays, randoms, grid, None)
+    normals = torch.empty(rays.shape[0], 3, dtype=torch.float32, device=rays.device)
     lib = _lib.load()
-    n = rays.shape[0]
-    dev = rays.device
-    fine = opts.n_fine > 0
-    g, bits = (None, None)
-    if grid is not None:
-        g, bits = _grid_args(grid)
-        if bits.device != dev:
-            raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
-    need = lib.nerfb200_render_normals_workspace_bytes(C.byref(ac), C.byref(af) if af is not None else None,
-                                                       C.byref(opts), n)
-    if need < 0:
-        _lib.check(_lib.ERR_UNSUPPORTED, "render_normals_workspace_bytes")
-    workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
-    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
-    normals = torch.empty(n, 3, dtype=torch.float32, device=dev)
-    head = (C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts), _ptr(blob_c),
-            _ptr(blob_f) if fine else None, _ptr(rays), rays.shape[1], n, *_random_args(randoms),
-            C.byref(g) if g is not None else None, _ptr(bits), -1.0 if stop is None else float(stop))
+    head = (*args, *grid_args, -1.0 if stop is None else float(stop))
     tail = (_ptr(out_c), _ptr(out_f), _ptr(normals), _ptr(workspace), int(impl), _stream())
     if ndc is None:
         _lib.check(lib.nerfb200_render_fwd_normals(*head, *tail), "render_fwd_normals")
@@ -796,31 +765,14 @@ def render_fwd_early_stop(arch_c, arch_f, opts: RenderOpts, blob_c, blob_f, rays
     int64[2]) and, with ``want_stop``, the int32 ``stop_sample`` of every ray (the header's definition).  A given
     ``workspace`` large enough is used; its first sections are laid out as ``render_workspace_layout(...,
     training=False)``."""
-    lib = _lib.load()
-    n = rays.shape[0]
-    dev = rays.device
-    fine = opts.n_fine > 0
-    g, bits = (None, None)
-    if grid is not None:
-        g, bits = _grid_args(grid)
-        if bits.device != dev:
-            raise RuntimeError(f"nerfb200: the grid is on {bits.device}, the rays on {dev}")
-    need = render_early_stop_workspace_bytes(arch_c, arch_f if fine else None, opts, n)
-    if workspace is None or workspace.numel() < need:
-        workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-    out_c = torch.empty(n, 8, dtype=torch.float32, device=dev)
-    out_f = torch.empty(n, 8, dtype=torch.float32, device=dev) if fine else None
+    args, grid_args, out_c, out_f, workspace = _render_call("render_early_stop_workspace_bytes", arch_c, arch_f,
+                                                            opts, blob_c, blob_f, rays, randoms, grid, workspace)
+    n, dev = rays.shape[0], rays.device
     n_evaluated = torch.zeros(2, dtype=torch.int64, device=dev)
     stop_sample = torch.empty(n, dtype=torch.int32, device=dev) if want_stop else None
-    ac = arch_c.c_struct()
-    af = arch_f.c_struct() if fine else None
-    _lib.check(lib.nerfb200_render_fwd_early_stop(C.byref(ac), C.byref(af) if af is not None else None, C.byref(opts),
-                                                  _ptr(blob_c), _ptr(blob_f) if fine else None, _ptr(rays),
-                                                  rays.shape[1], n, *_random_args(randoms),
-                                                  C.byref(g) if g is not None else None, _ptr(bits), float(stop),
-                                                  _ptr(out_c), _ptr(out_f), _ptr(workspace), int(impl),
-                                                  _ptr(n_evaluated), _ptr(stop_sample), _stream()),
-               "render_fwd_early_stop")
+    _lib.check(_lib.load().nerfb200_render_fwd_early_stop(*args, *grid_args, float(stop), _ptr(out_c), _ptr(out_f),
+                                                          _ptr(workspace), int(impl), _ptr(n_evaluated),
+                                                          _ptr(stop_sample), _stream()), "render_fwd_early_stop")
     if want_stop:
         return out_c, out_f, n_evaluated, stop_sample
     return out_c, out_f, n_evaluated

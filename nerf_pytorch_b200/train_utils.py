@@ -397,21 +397,21 @@ def check_grid_call(grid, device, *models):
                            f"{list(bits.shape)}")
 
 
-def _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine):
-    """The impl an occupancy-grid render runs on, after every refusal that precedes a launch: those of check_grid_call,
-    impl 0, and an architecture the wgmma inference forward refuses (the library's reason)."""
-    check_grid_call(grid, rays.device, model_coarse, model_fine)
+def _inference_impl(feature, render, impl, arch_c, arch_f, nc, nf):
+    """The impl a grid or early-stopping render runs on, after the refusals that precede a launch: impl 0 and an
+    architecture the wgmma inference forward refuses (the library's reason).  ``feature`` names the option in the impl 0
+    refusal ("an occupancy grid"), ``render`` the render in the library's ("grid render")."""
     if impl is None:
         impl = _auto_impl(arch_c, arch_f, nc, nf, training=False)
     if impl == ops.IMPL_SIMT:
-        raise NotImplementedError("nerfb200: an occupancy grid runs on the wgmma inference forward (impl 1 or 3), not "
+        raise NotImplementedError(f"nerfb200: {feature} runs on the wgmma inference forward (impl 1 or 3), not "
                                   "impl 0 (fp32 CUDA cores)" + "".join(
                                       f"; {why}" for a, n in ((arch_c, nc), (arch_f, nc + nf)) if a is not None
                                       for why in [ops.impl_refusal(a, n, ops.IMPL_TC_FWD)] if why))
     for a, n in ((arch_c, nc), (arch_f, nc + nf)):
         why = ops.impl_refusal(a, n, ops.IMPL_TC_FWD if impl == ops.IMPL_TC else impl) if a is not None else None
         if why:
-            raise NotImplementedError(f"nerfb200 grid render: {why}")
+            raise NotImplementedError(f"nerfb200 {render}: {why}")
     return impl
 
 
@@ -423,23 +423,6 @@ def check_early_stop_call(early_stop, *models):
     if _trains(p for m in models if m is not None for p in m.parameters()):
         raise NotImplementedError("nerfb200: early ray termination renders only (inference); render under "
                                   "torch.no_grad() or with parameters that do not require grad")
-
-
-def _early_stop_impl(impl, arch_c, arch_f, nc, nf):
-    """The impl an early-stopping render without a grid runs on, after the refusals that precede a launch: impl 0 and an
-    architecture the wgmma inference forward refuses (the library's reason).  With a grid, _grid_impl decides."""
-    if impl is None:
-        impl = _auto_impl(arch_c, arch_f, nc, nf, training=False)
-    if impl == ops.IMPL_SIMT:
-        raise NotImplementedError("nerfb200: early ray termination runs on the wgmma inference forward (impl 1 or 3), "
-                                  "not impl 0 (fp32 CUDA cores)" + "".join(
-                                      f"; {why}" for a, n in ((arch_c, nc), (arch_f, nc + nf)) if a is not None
-                                      for why in [ops.impl_refusal(a, n, ops.IMPL_TC_FWD)] if why))
-    for a, n in ((arch_c, nc), (arch_f, nc + nf)):
-        why = ops.impl_refusal(a, n, ops.IMPL_TC_FWD if impl == ops.IMPL_TC else impl) if a is not None else None
-        if why:
-            raise NotImplementedError(f"nerfb200 early-stopping render: {why}")
-    return impl
 
 
 def check_normals_call(impl, *models):
@@ -533,7 +516,7 @@ def predict_and_render_radiance(
     if normals:
         check_normals_call(impl, model_coarse, model_fine)
     if grid is not None:
-        check_grid_call(grid, None, model_coarse, model_fine)
+        check_grid_call(grid, ray_batch.device, model_coarse, model_fine)
     if early_stop is not None:
         check_early_stop_call(early_stop, model_coarse, model_fine)
     o = getattr(options.nerf, mode)
@@ -552,9 +535,9 @@ def predict_and_render_radiance(
         raise RuntimeError("nerfb200: num_fine > 0 but model_fine is None (the reference fails here as well)")
     arch_f = _arch_of(model_fine, enc_xyz, enc_dir) if fine else None
     if grid is not None:
-        impl = _grid_impl(grid, rays, impl, arch_c, arch_f, nc, nf, model_coarse, model_fine)
+        impl = _inference_impl("an occupancy grid", "grid render", impl, arch_c, arch_f, nc, nf)
     elif early_stop is not None:
-        impl = _early_stop_impl(impl, arch_c, arch_f, nc, nf)
+        impl = _inference_impl("early ray termination", "early-stopping render", impl, arch_c, arch_f, nc, nf)
     if normals:
         impl = _normals_impl(impl, arch_c, arch_f, nc, nf)
     params_c, blob_c = _packed(model_coarse, arch_c)
