@@ -267,6 +267,19 @@ def composite64(raw, z, dirs, noise_std=0.0, white_background=False, noise=None,
     return rgb, disp, acc, weights, depth
 
 
+def composite_grad64(raw, z, dirs, g, noise_std=0.0, white_background=False, noise=None):
+    """fp64 d(sum(outputs * g)) / d(raw) of composite64: g [n][8] weighs rgb, disp (rays where g is 0 excluded) and acc,
+    the render entry points' upstream layout.  raw: fp32 [n][S][4], or (fp32, fp64) to differentiate the fp64 values
+    with the fp32 ones' gates."""
+    r32, r64 = raw if isinstance(raw, tuple) else (raw, raw.double())
+    r64 = r64.detach().clone().requires_grad_(True)
+    rgb, disp, acc, _, _ = composite64(r32, z, dirs, noise_std, white_background, noise, raw64=r64)
+    g = g.double()
+    disp = torch.where(g[:, 3] != 0, disp, 0.0)
+    loss = (rgb * g[:, :3]).sum() + (disp * g[:, 3]).sum() + (acc * g[:, 4]).sum()
+    return torch.autograd.grad(loss, r64)[0]
+
+
 def transmittance64(raw, z, rays, noise, std):
     """fp64 exclusive transmittance [n, S + 1] of fp32 raw [n, S, 4] at depths z [n, S] along rays [n, >= 6]:
     T[:, p] = prod over samples < p of 1 - alpha + 1e-10, with the sigma gate and the last sample's sigma taken from the

@@ -3,6 +3,7 @@
   2. per ray at t in {1e-4, 1e-2, 0.1}: evaluated raw is the default raw, the rest of the grid's samples from stop_sample
      on are [0 0 0 -inf], stop_sample is on a round boundary, the fp64 transmittance of the default raw is below t at the
      stop and not below it at every earlier boundary, unstopped rays and the coarse pass are bit-identical;
+     1 and 2 also at the sample counts where the rounds change shape (COUNTS);
   3. the guarantee's output bounds, with their signs;
   4. determinism and chunking invariance;
   5. the shipped lego and fern weights at t = 1e-3, with and without a model-built grid;
@@ -46,7 +47,7 @@ def report(what, ctx, value):
     print(f"[early_stop] {what} {ctx}: {value}")
 
 
-def _setup(scene, variant="det", n_fine=128):
+def _setup(scene, variant="det", n_fine=128, n_coarse=64):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
@@ -57,7 +58,7 @@ def _setup(scene, variant="det", n_fine=128):
                   for m in (mc, mf))
     blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
-    opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
+    opts = ops.make_opts(n_coarse, n_fine, perturb, False, white, noise)
     rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
@@ -106,28 +107,32 @@ def test_zero_threshold_is_the_default_render_bit_for_bit_at_hidden_256(impl, sc
     _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid_kind)
 
 
-def _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid_kind):
+def _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid_kind, nc=64, nf=128):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    (arch, arch_f), blobs, opts, rays, _, _ = _setup(scene, variant)
+    ctx = (impl, scene, variant, grid_kind, nc, nf)
+    (arch, arch_f), blobs, opts, rays, _, _ = _setup(scene, variant, nf, nc)
     grid = _grid(scene, grid_kind)
     rng = nb.SeededRandoms(5, 2)
     n = rays.shape[0]
-    oc, of, _, ne_ref = _reference(arch, arch_f, blobs, opts, rays, rng, grid, IMPLS[impl])
-    ec, ef, ne, stop = ops.render_fwd_early_stop(arch, arch_f, opts, blobs[0], blobs[1], rays, rng, grid, 0.0,
-                                                 impl=IMPLS[impl], want_stop=True)
-    assert bits_equal(ec, oc) and bits_equal(ef, of), (impl, scene, variant, grid_kind)
-    assert (stop == 192).all()
-    assert ne.tolist() == ([n * 64, n * 192] if grid is None else ne_ref.tolist())
+    if nf:
+        oc, of, _, ne_ref = _reference(arch, arch_f, blobs, opts, rays, rng, grid, IMPLS[impl])
+        ec, ef, ne, stop = ops.render_fwd_early_stop(arch, arch_f, opts, blobs[0], blobs[1], rays, rng, grid, 0.0,
+                                                     impl=IMPLS[impl], want_stop=True)
+        assert bits_equal(ec, oc) and bits_equal(ef, of), ctx
+        assert (stop == nc + nf).all(), ctx
+        assert ne.tolist() == ([n * nc, n * (nc + nf)] if grid is None else ne_ref.tolist()), ctx
 
     # a coarse-only network: its one pass is the last
     perturb, noise, white = VARIANTS[variant]
-    opts0 = ops.make_opts(64, 0, perturb, False, white, noise)
+    opts0 = ops.make_opts(nc, 0, perturb, False, white, noise)
     oc, _, _, ne_ref = _reference(arch, None, blobs, opts0, rays, rng, grid, IMPLS[impl])
-    ec, ef, ne = ops.render_fwd_early_stop(arch, None, opts0, blobs[0], None, rays, rng, grid, 0.0, impl=IMPLS[impl])
-    assert ef is None and bits_equal(ec, oc)
-    assert ne.tolist() == ([n * 64, 0] if grid is None else ne_ref.tolist())
+    ec, ef, ne, stop = ops.render_fwd_early_stop(arch, None, opts0, blobs[0], None, rays, rng, grid, 0.0,
+                                                 impl=IMPLS[impl], want_stop=True)
+    assert ef is None and bits_equal(ec, oc), ctx
+    assert (stop == nc).all(), ctx
+    assert ne.tolist() == ([n * nc, 0] if grid is None else ne_ref.tolist()), ctx
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -136,29 +141,34 @@ def _zero_threshold_is_the_default_render_bit_for_bit(impl, scene, variant, grid
 _CACHE = {}
 
 
-def _stopped_render(impl, scene, variant, grid_kind, t):
+def _stopped_render(impl, scene, variant, grid_kind, t, nc=64, nf=128):
+    """The default render and the early-stopping one; raw and z of the last pass (the fine pass, or the coarse pass
+    when nf is 0) read from both workspaces."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops
 
-    key = (impl, scene, variant, grid_kind, t)
+    key = (impl, scene, variant, grid_kind, t, nc, nf)
     if key in _CACHE:
         return _CACHE[key]
     _CACHE.clear()
-    archs, blobs, opts, rays, models, enc = _setup(scene, variant)
+    archs, blobs, opts, rays, models, enc = _setup(scene, variant, nf, nc)
+    if not nf:
+        archs = (archs[0], None)
+        blobs = [blobs[0], None]
     grid = _grid(scene, grid_kind, models, enc)
     rng = nb.SeededRandoms(9, 4)
     oc, of, ws, _ = _reference(*archs, blobs, opts, rays, rng, grid, IMPLS[impl])
     ec, ef, ne, stop = ops.render_fwd_early_stop(*archs, opts, blobs[0], blobs[1], rays, rng, grid, t,
                                                  impl=IMPLS[impl], want_stop=True)
-    n = rays.shape[0]
+    n, S, last = rays.shape[0], nc + nf, "fine" if nf else "coarse"
     lay = ops.render_workspace_layout(*archs, opts, n, False)
     es_ws = torch.empty(ops.render_early_stop_workspace_bytes(*archs, opts, n), dtype=torch.uint8, device="cuda")
     ops.render_fwd_early_stop(*archs, opts, blobs[0], blobs[1], rays, rng, grid, t, impl=IMPLS[impl],
                               workspace=es_ws)
     torch.cuda.synchronize()
-    out = dict(opts=opts, rays=rays, rng=rng, ref=(oc, of), es=(ec, ef), ne=ne, stop=stop.long(),
-               raw=ws_view(ws, lay, "raw_fine", n, 192, 4), z=ws_view(ws, lay, "z_fine", n, 192, 1),
-               es_raw=ws_view(es_ws, lay, "raw_fine", n, 192, 4), es_z=ws_view(es_ws, lay, "z_fine", n, 192, 1))
+    out = dict(opts=opts, rays=rays, rng=rng, ref=(oc, of), es=(ec, ef), ne=ne, stop=stop.long(), last=last,
+               raw=ws_view(ws, lay, f"raw_{last}", n, S, 4), z=ws_view(ws, lay, f"z_{last}", n, S, 1),
+               es_raw=ws_view(es_ws, lay, f"raw_{last}", n, S, 4), es_z=ws_view(es_ws, lay, f"z_{last}", n, S, 1))
     _CACHE[key] = out
     return out
 
@@ -174,14 +184,20 @@ PER_RAY = [(impl, scene, variant, grid_kind, t)
 
 @pytest.mark.parametrize("impl,scene,variant,grid_kind,t", PER_RAY)
 def test_per_ray_contract(impl, scene, variant, grid_kind, t):
+    _per_ray_contract(impl, scene, variant, grid_kind, t)
+
+
+def _per_ray_contract(impl, scene, variant, grid_kind, t, nc=64, nf=128):
     from nerf_pytorch_b200 import ops
 
-    r = _stopped_render(impl, scene, variant, grid_kind, t)
-    ctx = (impl, scene, variant, grid_kind, t)
+    r = _stopped_render(impl, scene, variant, grid_kind, t, nc, nf)
+    ctx = (impl, scene, variant, grid_kind, t, nc, nf)
     K = ops.stop_round()
     raw, z, es_raw, stop = r["raw"], r["z"], r["es_raw"], r["stop"]
     n, S = z.shape
-    assert bits_equal(r["es"][0], r["ref"][0]), ctx  # the coarse pass and so the fine depths are untouched
+    i_last = 1 if nf else 0
+    if nf:
+        assert bits_equal(r["es"][0], r["ref"][0]), ctx  # the coarse pass and so the fine depths are untouched
     assert bits_equal(r["es_z"], z), ctx
     keep = raw[..., 3] != -math.inf  # the samples the grid keeps (all of them without a grid)
     j = torch.arange(S, device="cuda")[None, :]
@@ -190,10 +206,12 @@ def test_per_ray_contract(impl, scene, variant, grid_kind, t):
     assert bits_equal(es_raw, want), ctx
     stopped = stop < S
     report("stopped rays / all", ctx, f"{int(stopped.sum())} / {n}")
-    if scene == "a2" and t >= 1e-2:
+    if scene == "a2" and t >= 1e-2 and S > K:
         assert stopped.any(), ctx  # the scaled weights turn rays opaque: the contract is not vacuous
-    assert (r["ne"][1] == (keep & before).sum()).item(), ctx
-    assert bits_equal(r["es"][1][~stopped], r["ref"][1][~stopped]), ctx
+    if S <= K:
+        assert not stopped.any(), ctx  # one round: no ray has samples left after it
+    assert (r["ne"][i_last] == (keep & before).sum()).item(), ctx
+    assert bits_equal(r["es"][i_last][~stopped], r["ref"][i_last][~stopped]), ctx
 
     # round boundaries: the rank (1-based) of each kept sample among its ray's kept samples
     rank = torch.cumsum(keep.long(), 1)
@@ -203,7 +221,7 @@ def test_per_ray_contract(impl, scene, variant, grid_kind, t):
     last_ran = torch.where(keep & before, j, -1).max(1).values
     assert (stop[stopped] == last_ran[stopped] + 1).all(), ctx
 
-    noise = ops.random_fill(r["rng"], "noise_f", n, S) if r["opts"].noise_std > 0 else None
+    noise = ops.random_fill(r["rng"], f"noise_{r['last'][0]}", n, S) if r["opts"].noise_std > 0 else None
     T = transmittance64(raw, z, r["rays"], noise, r["opts"].noise_std)
     # at the stop T < t; at every earlier boundary with samples left (and every boundary of an unstopped ray) T >= t
     if stopped.any():
@@ -241,6 +259,27 @@ def test_output_bounds(impl, scene, variant, grid_kind, t):
         ro, re = 1.0 / o[clear, 3], 1.0 / e[clear, 3]
         bound = 2 * t * zmax / (o[clear, 4] - t) + OUT_ABS * zmax
         assert ((ro - re).abs() <= bound).all(), ctx
+
+
+# (n_coarse, n_fine) where the last pass's rounds of K = 32 change shape: one partial round (15 samples), a last round of
+# one sample (33), exactly one round (15 + 17) and 32 rounds (15 + 1009).  With a grid, each compaction group of 10 rays
+# holds 10 S rows, which no count here makes a multiple of the 64-row blocks.
+COUNTS = [(15, 0), (33, 0), (15, 17), (15, 1009)]
+COUNT_IDS = [f"{nc}+{nf}" for nc, nf in COUNTS]
+
+
+@pytest.mark.parametrize("counts", COUNTS, ids=COUNT_IDS)
+@pytest.mark.parametrize("grid_kind", [None, "rand50"])
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_zero_threshold_is_the_default_render_bit_for_bit_at_boundary_counts(impl, grid_kind, counts):
+    _zero_threshold_is_the_default_render_bit_for_bit(impl, "lego", "perturb_noise", grid_kind, *counts)
+
+
+@pytest.mark.parametrize("counts", COUNTS, ids=COUNT_IDS)
+@pytest.mark.parametrize("scene,variant,grid_kind", [("a2", "perturb_noise", "rand50"), ("lego", "det", None)])
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_per_ray_contract_at_boundary_counts(impl, scene, variant, grid_kind, counts):
+    _per_ray_contract(impl, scene, variant, grid_kind, 1e-2, *counts)
 
 
 # ------------------------------------------------------------------------------------------------------------------------

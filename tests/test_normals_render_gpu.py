@@ -5,7 +5,7 @@
     raw outputs, the fp64 compositing weights of that raw (with the seeded noise the render used), and grad sigma by fp64
     autograd at o + d z, summed in sample order -- lego A0 (Blender), fern A0 (NDC), a coarse-only network, a seeded
     perturb + noise render, 8 x 256 networks (A2) and A1 / A2 mixed across the two passes, with and without a grid and
-    early stopping;
+    early stopping, and a last pass of 1024 samples;
   * |N| <= acc + eps, N = 0 exactly where acc = 0;
   * cast_to_normal_image, and the refusals (a call that would train, impl 0, impl 3) before any launch."""
 import pytest
@@ -93,10 +93,10 @@ def _six_outputs_are_those_of_the_render_without_normals(scene, variant):
     assert img.dtype == torch.uint8 and img.shape == n.shape
 
 
-def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None):
+def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None, counts=(64, 128)):
     """(arch of the last pass, its state dict, rays, z, raw, noise of the last pass or None, noise_std, normals, acc)
-    of one render_fwd_normals call (with a grid of the networks' density for grid_kind "model", early stopping at
-    `stop`), read back from its workspace."""
+    of one render_fwd_normals call at (n_coarse, n_fine) `counts` (with a grid of the networks' density for grid_kind
+    "model", early stopping at `stop`), read back from its workspace."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
 
@@ -108,15 +108,15 @@ def _render(scene, perturb, noise, coarse_only, seed, grid_kind=None, stop=None)
     blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     sd_last = {k: v.detach().cpu() for k, v in (mc if coarse_only else mf).state_dict().items()}
     grid = _grid(scene, [mc, mf], (epf, edf)) if grid_kind == "model" else None
-    nf = 0 if coarse_only else 128
-    opts = ops.make_opts(64, nf, perturb, False, False, noise)
+    nc, nf = counts[0], 0 if coarse_only else counts[1]
+    opts = ops.make_opts(nc, nf, perturb, False, False, noise)
     rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     rng = nb.SeededRandoms(seed, 0)
     arch, arch_f = archs[0], None if coarse_only else archs[1]
     with torch.no_grad():
         out_c, out_f, normals, ws = ops.render_fwd_normals(arch, arch_f, opts, blobs[0], blobs[1] if nf else None, rays,
                                                            rng, grid, stop, impl=1)
-    n, s = rays.shape[0], 64 + nf
+    n, s = rays.shape[0], nc + nf
     lay = ops.render_workspace_layout(arch, arch_f, opts, n, False)
     zname, rname = ("z_coarse", "raw_coarse") if coarse_only else ("z_fine", "raw_fine")
     f = ws.view(torch.float32)
@@ -143,9 +143,15 @@ def test_normals_with_a_grid_or_early_stopping_match_an_fp64_restatement(scene, 
     _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind, stop)
 
 
-def _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind, stop):
-    ctx = (scene, perturb, noise, coarse_only, grid_kind, stop)
-    arch, sd, rays, z, raw, nz, std, normals, acc = _render(scene, perturb, noise, coarse_only, 3, grid_kind, stop)
+def test_normals_at_1024_samples_match_an_fp64_restatement():
+    """The largest pass the library takes: the density gradient runs over n_rays x 1024 compacted points."""
+    _normals_match_an_fp64_restatement("lego", True, 0.2, False, None, None, (64, 960))
+
+
+def _normals_match_an_fp64_restatement(scene, perturb, noise, coarse_only, grid_kind, stop, counts=(64, 128)):
+    ctx = (scene, perturb, noise, coarse_only, grid_kind, stop, counts)
+    arch, sd, rays, z, raw, nz, std, normals, acc = _render(scene, perturb, noise, coarse_only, 3, grid_kind, stop,
+                                                            counts)
     N64, bound, n_live, n_tie = M.normals64(arch, sd, rays, z, raw, std, nz)
     err = (normals.double() - N64).abs().max(-1).values
     report("max |N - N64|", ctx, f"{err.max().item():.3e}, max err / bound {(err / bound).max().item():.3f} (rays "

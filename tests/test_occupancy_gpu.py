@@ -1,5 +1,6 @@
 """GPU: occupancy-grid inference renders (nb.OccupancyGrid, ops.render_fwd_grid, render_image(grid=...)).
-  1. a full grid gives render_fwd's six outputs bit for bit, every sample evaluated;
+  1. a full grid gives render_fwd's six outputs bit for bit, every sample evaluated, also at the sample counts where
+     compaction and the wgmma tiles change shape (COUNTS);
   2. an empty grid evaluates nothing: every ray composites zero density;
   3. per ray: a ray none of whose skipped samples (either pass) has positive density in the default render's raw is
      bit-identical to the default render; every evaluated point's raw equals the default raw at that point;
@@ -41,7 +42,7 @@ def report(what, ctx, value):
     print(f"[occupancy] {what} {ctx}: {value}")
 
 
-def _setup(scene, variant="det", n_fine=128):
+def _setup(scene, variant="det", n_fine=128, n_coarse=64):
     """((arch_c, arch_f), blobs, opts, rays, models, encoders) of a scene at the ops level."""
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200 import ops, train_utils
@@ -53,7 +54,7 @@ def _setup(scene, variant="det", n_fine=128):
                   for m in (mc, mf))
     blobs = [train_utils._packed(m, a)[1] for m, a in zip((mc, mf), archs)]
     perturb, noise, white = VARIANTS[variant]
-    opts = ops.make_opts(64, n_fine, perturb, False, white, noise)
+    opts = ops.make_opts(n_coarse, n_fine, perturb, False, white, noise)
     rays = ops.gen_rays(scene_pose(pose), H, W, focal, None, "cuda", ndc=not no_ndc, near=near, far=far)
     return archs, blobs, opts, rays, (mc, mf), (epf, edf)
 
@@ -93,15 +94,34 @@ def _render_both(archs, blobs, opts, rays, grid, impl, rng):
 @pytest.mark.parametrize("scene", list(SCENES))
 @pytest.mark.parametrize("impl", list(IMPLS))
 def test_full_grid_is_the_default_render_bit_for_bit(impl, scene, variant):
+    _full_grid_is_the_default_render_bit_for_bit(impl, scene, variant)
+
+
+# (n_coarse, n_fine) where compaction changes shape: each group of 10 rays holds 10 S rows, no multiple of the 64-row
+# blocks here; the wgmma kernels' smallest pass (15 samples, 10 rays per tile); the early-stopping counts of
+# test_early_stop_gpu.py (one partial round of 32, a last round of one, exactly one round, 32 rounds)
+COUNTS = [(15, 0), (33, 0), (15, 17), (15, 1009)]
+
+
+@pytest.mark.parametrize("counts", COUNTS, ids=[f"{nc}+{nf}" for nc, nf in COUNTS])
+@pytest.mark.parametrize("scene", ["lego", "a2"])
+@pytest.mark.parametrize("impl", list(IMPLS))
+def test_full_grid_is_the_default_render_bit_for_bit_at_boundary_counts(impl, scene, counts):
+    _full_grid_is_the_default_render_bit_for_bit(impl, scene, "perturb_noise", *counts)
+
+
+def _full_grid_is_the_default_render_bit_for_bit(impl, scene, variant, nc=64, nf=128):
     import nerf_pytorch_b200 as nb
     from nerf_pytorch_b200.occupancy import OccupancyGrid
 
-    archs, blobs, opts, rays, _, _ = _setup(scene, variant)
+    archs, blobs, opts, rays, _, _ = _setup(scene, variant, nf, nc)
+    if not nf:
+        archs, blobs = (archs[0], None), [blobs[0], None]
     grid = OccupancyGrid.full(SCENES[scene][-1], 32)
     (oc, of, _), (gc, gf, _), ne = _render_both(archs, blobs, opts, rays, grid, IMPLS[impl], nb.SeededRandoms(5, 2))
     n = rays.shape[0]
-    assert bits_equal(gc, oc) and bits_equal(gf, of), (impl, scene, variant)
-    assert ne.tolist() == [n * 64, n * 192]
+    assert bits_equal(gc, oc) and bits_equal(gf, of), (impl, scene, variant, nc, nf)
+    assert ne.tolist() == [n * nc, n * (nc + nf) if nf else 0], (impl, scene, variant, nc, nf)
 
 
 # ------------------------------------------------------------------------------------------------------------------------

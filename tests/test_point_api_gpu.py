@@ -248,8 +248,11 @@ def _trained_inputs(n, s, seed):
 
 
 # "random": raw ~ 2 N(0, 1); "trained": the saturated regime of _trained_inputs, also at 199 samples (not a multiple of
-# the warp's 32 lanes).  The random regime keeps its original test ids.
-COMP_REGIMES = [("random", s) for s in (2, 64, 192, 1024)] + [("trained", s) for s in (2, 64, 192, 199, 1024)]
+# the warp's 32 lanes).  The random regime keeps its original test ids.  The kernels' lane L owns samples [L C, (L + 1) C)
+# with C = ceil(S / 32): 1 and 31 samples leave lanes idle, 33 gives lane 16 a single sample and 1023 leaves lane 31 one
+# short of 32.
+COMP_REGIMES = ([("random", s) for s in (2, 64, 192, 1024, 1, 31, 33, 1023)] +
+                [("trained", s) for s in (2, 64, 192, 199, 1024, 31, 33, 1023)])
 COMP_IDS = [str(s) if r == "random" else f"{r}-{s}" for r, s in COMP_REGIMES]
 
 

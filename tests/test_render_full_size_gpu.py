@@ -1,6 +1,6 @@
 """GPU: the whole render step at training size against fp64, stage by stage, from the render workspace.
 
-Each case runs ops.render_fwd(training=True) once on 4096 rays and reads the workspace's sections through
+Each case runs ops.render_fwd(training=True) once on 4096 rays (or its own count) and reads the workspace's sections through
 ops.render_workspace_layout.  Every stage is checked on this library's own previous stage, so that one stage's rounding
 never shows as another's error:
   z_coarse     O.stratified_z in fp32 on the CPU with the same t_rand: bit for bit;
@@ -23,14 +23,15 @@ Bars: the figures in brackets are the worst over this file's cases, measured on 
 limit and 1980 MHz SM clock.  There the whole file runs in 20 s (4.4 s for the longest case) and holds at most 19.5 GiB
 of device memory: the impl-1 bench step, whose seeded run takes a second 9.3 GiB workspace while the first is alive
 (the impl-0 bench step holds 10.2 GiB).  The 8 x 128 network with 16 xyz bands, which only the fp32 kernels take, adds
-3.3 s and holds 10.6 GiB."""
+3.3 s and holds 10.6 GiB.  The cases at the sample counts where the kernels change shape ("nc2" .. "nc1024") add 9.3 s
+together (1.6 s for the longest, nc1023_nf1) and hold at most 4.8 GiB (nc683_nf1)."""
 import math
 import time
 
 import pytest
 import torch
 
-from helpers import bits_equal, composite64, load_weights
+from helpers import bits_equal, composite64, composite_grad64, load_weights
 from mlp_checks import (BLOCK_TOL, COMP_GRAD_TOL, COMP_TOL, FP32_TIE_TOL, SIMT_FWD_TOL, STASH_TOL, TC_FWD_TOL,
                         as_state_dict, blob_range_factor, check_blocks, oracle_tiles, relu_ties, report, sms,
                         tc_blocks, _floors)
@@ -42,7 +43,8 @@ pytestmark = pytest.mark.gpu
 # raw per column [2.1e-5, fern]; compositing outputs [2.8e-6, deterministic lego, fine]; disp [7.9e-3 of its bar];
 # d_raw [1.5e-6; 1.0e-5 with the disp and acc terms]; parameter gradient blocks, figure / (scale + floor / bar) [5.4e-6
 # at the loss's scale, fern; 3.1e-6 at max |d_raw| in [4, 8)].  At the loss's own scale the fixed-point floor is up to
-# 99.98 % of a block's bar (every case's smallest block: 93 % to 99.98 %).
+# 99.98 % of a block's bar (every case's smallest block: 93 % to 99.98 %).  At the boundary sample counts: compositing
+# outputs [9.5e-6, 1024 samples]; d_raw [9.1e-6, 1024 samples]; disp [1.9e-2 of its bar, 4 + 1]; raw [2.0e-6].
 CDF_ULPS = 3         # in-kernel cdf against the fp64 cdf of the same weights, in units of 2^-24 [2.02]
 DISP_K = 4.0         # disp's bar on rays with small acc, a derived bound (see _check_compositing)
 # Parameter gradients against the oracle at fp64 d_raw (the compositing of the oracle's raw), per block, relative to its
@@ -73,10 +75,39 @@ CASES = {
     # no view directions: the fused backward needs the fc_rgb / fc_alpha heads, so this network trains on impl 0
     "coarse_only": dict(net="A0_noview", weights="init", config=2, nc=64, nf=0, perturb=True, noise=0.2),
     "wide_encodings": dict(net="wide_enc", weights="init", config=2, nc=64, nf=128, perturb=True, noise=0.2),
+    # The sample counts where the per-ray kernels and the wgmma tiling change shape (test_sample_counts_gpu.py lists the
+    # kernels' boundaries).  Each ray count is a multiple of neither 4 (the per-ray kernels' warps per CTA) nor 10 (rays
+    # per compaction group), and each pass's points end partway through a 128-point tile (no S = 1024 count can) and
+    # partway through the last wave of CTAs on 132 SMs.
+    "nc2": dict(net="A1", weights="init", config=2, nc=2, nf=0, perturb=True, noise=0.2, rays=4095),
+    # the smallest hierarchical step: four coarse samples, two interior weights, one fine sample
+    "nc4_nf1": dict(net="A1", weights="init", config=2, nc=4, nf=1, perturb=True, noise=0.2, white=True, rays=4095),
+    # 14 samples: the wgmma kernels refuse it (test_wgmma_refuses_fewer_than_15_samples_before_any_launch)
+    "nc14": dict(net="A1", weights="init", config=2, nc=14, nf=0, perturb=True, noise=0.2, rays=4095),
+    # the smallest pass the wgmma kernels take: 10 rays per 128-point tile
+    "nc15_nf1": dict(net="A1", weights="init", config=2, nc=15, nf=1, perturb=True, noise=0.2, rays=4095),
+    # 31 interior weights; a fine pass of 64 samples, so the composite kernels' lanes hold two samples each
+    "nc33_nf31": dict(net="A1", weights="init", config=2, nc=33, nf=31, perturb=True, noise=0.2, lindisp=True,
+                      rays=4097),
+    # 129 fine samples: the resampling sort pads to 256
+    "nc64_nf65": dict(net="A1", weights="init", config=2, nc=64, nf=65, perturb=False, noise=0.0, white=True,
+                      rays=2047),
+    # resampling's shared memory passes 48 KiB and takes the opt-in
+    "nc683_nf1": dict(net="A1", weights="init", config=2, nc=683, nf=1, perturb=True, noise=0.2, rays=399),
+    # the largest coarse pass with a fine pass, whose 1024 samples fill every lane's 32
+    "nc1023_nf1": dict(net="A0", weights="init", config=2, nc=1023, nf=1, perturb=True, noise=0.2, rays=399),
+    # 1024 samples in one pass: the composite backward's shared memory is exactly 48 KiB
+    "nc1024": dict(net="A0", weights="init", config=2, nc=1024, nf=0, perturb=True, noise=0.2, white=True, rays=399),
 }
 RUNS = [("bench_step", 1), ("bench_step", 0), ("lego", 1), ("fern_ndc", 1), ("odd_counts", 1), ("deterministic", 1),
-        ("coarse_only", 0), ("wide_encodings", 0)]
-N_RAYS = 4096
+        ("coarse_only", 0), ("wide_encodings", 0),
+        ("nc2", 0), ("nc4_nf1", 0), ("nc14", 0), ("nc15_nf1", 1), ("nc15_nf1", 0), ("nc33_nf31", 1), ("nc64_nf65", 1),
+        ("nc683_nf1", 1), ("nc1023_nf1", 1), ("nc1024", 1), ("nc1024", 0)]
+N_RAYS = 4096  # a case's rays unless it sets "rays"
+
+
+def _n_rays(cfg):
+    return cfg.get("rays", N_RAYS)
 
 
 @pytest.fixture(autouse=True)
@@ -116,15 +147,16 @@ def _camera(cfg):
     """Pose, pixel ids (a randperm pick, as bench.py) and the seeded targets of the batch."""
     cam = CONFIGS[cfg["config"]]
     g = torch.Generator().manual_seed(17)
-    pix = torch.randperm(cam["H"] * cam["W"], generator=g)[:N_RAYS].contiguous()
-    target = torch.rand(N_RAYS, 3, generator=g)
+    n = _n_rays(cfg)
+    pix = torch.randperm(cam["H"] * cam["W"], generator=g)[:n].contiguous()
+    target = torch.rand(n, 3, generator=g)
     pose = torch.eye(4) if cam["ndc"] else O.pose_spherical(30.0, -30.0, 4.0)
     return cam, pose, pix, target
 
 
 def _randoms(cfg, seed):
     """The random tensors the options use, torch-drawn (CPU generator) and moved to the device."""
-    n, nc, nf = N_RAYS, cfg["nc"], cfg["nf"]
+    n, nc, nf = _n_rays(cfg), cfg["nc"], cfg["nf"]
     g = torch.Generator().manual_seed(seed)
     rnd = {}
     if cfg["perturb"]:
@@ -146,7 +178,7 @@ def _seeded_tensors(cfg, rng):
     per_ray = {"t_rand": nc, "noise_c": nc, "u": nf, "noise_f": nc + nf}
     used = {"t_rand": cfg["perturb"], "noise_c": cfg["noise"] > 0, "u": nf and cfg["perturb"],
             "noise_f": nf and cfg["noise"] > 0}
-    return {k: ops.random_fill(rng, k, N_RAYS, per_ray[k]) for k in per_ray if used[k]}
+    return {k: ops.random_fill(rng, k, _n_rays(cfg), per_ray[k]) for k in per_ray if used[k]}
 
 
 class Workspace:
@@ -253,7 +285,7 @@ def _check_resampling(ws, rnd, cfg, ctx):
     _, zs_in, inds_in, _ = ops.sample_pdf_merge(ws.z_c, ws.w_c, u, nf, cdf_in=cdf, want_aux=True)
     z_c = ws.z_c.cpu()
     bins = 0.5 * (z_c[:, 1:] + z_c[:, :-1])
-    u_cpu = u.cpu() if u is not None else torch.linspace(0.0, 1.0, nf).expand(N_RAYS, nf).contiguous()
+    u_cpu = u.cpu() if u is not None else torch.linspace(0.0, 1.0, nf).expand(_n_rays(cfg), nf).contiguous()
     want_zs, want_inds = O.sample_from_cdf(bins, cdf.cpu(), u_cpu)
     assert torch.equal(inds_in.cpu().long(), want_inds), ctx + ("indices given the cdf",)
     assert bits_equal(zs_in.cpu(), want_zs) and bits_equal(zs_in, zs), ctx + ("samples given the cdf",)
@@ -261,15 +293,8 @@ def _check_resampling(ws, rnd, cfg, ctx):
 
 
 def _composite_grad64(raw, z, rays, noise, g, cfg):
-    """fp64 d(sum(outputs * g)) / d(raw) of composite64: g [n][8] weighs rgb, disp (rays where g is 0 excluded) and
-    acc.  raw: fp32 [n][S][4], or (fp32, fp64) to differentiate the fp64 values with the fp32 ones' gates."""
-    r32, r64 = raw if isinstance(raw, tuple) else (raw, raw.double())
-    r64 = r64.detach().clone().requires_grad_(True)
-    rgb, disp, acc, _, _ = composite64(r32, z, rays[:, 3:6], cfg["noise"], cfg.get("white", False), noise, raw64=r64)
-    g = g.double()
-    disp = torch.where(g[:, 3] != 0, disp, 0.0)
-    loss = (rgb * g[:, :3]).sum() + (disp * g[:, 3]).sum() + (acc * g[:, 4]).sum()
-    return torch.autograd.grad(loss, r64)[0]
+    """helpers.composite_grad64 with the case's noise and background."""
+    return composite_grad64(raw, z, rays[:, 3:6], g, cfg["noise"], cfg.get("white", False), noise)
 
 
 def _floor_share(arch, want, floors, tol):
@@ -301,7 +326,7 @@ class Step:
         cam = self.cam
         self.rays = ops.gen_rays(self.pose, cam["H"], cam["W"], cam["focal"], self.pix.cuda(), "cuda", ndc=cam["ndc"],
                                  near=cam["near"], far=cam["far"], use_viewdirs=self.arch_c.use_viewdirs)
-        self.nc, self.nf = cfg["nc"], cfg["nf"]
+        self.nc, self.nf, self.n = cfg["nc"], cfg["nf"], _n_rays(cfg)
         self.ns = self.nc + self.nf if self.nf else 0
         self.opts = ops.make_opts(self.nc, self.nf, cfg["perturb"], cfg.get("lindisp", False), cfg.get("white", False),
                                   cfg["noise"])
@@ -316,12 +341,12 @@ class Step:
         arch_f = self.arch_f if self.nf else None
         ws = None
         if zeroed:
-            need = self.ops.render_workspace_bytes(self.arch_c, arch_f, self.opts, N_RAYS, training)
+            need = self.ops.render_workspace_bytes(self.arch_c, arch_f, self.opts, self.n, training)
             ws = torch.zeros(need, dtype=torch.uint8, device="cuda")
         out_c, out_f, ws = self.ops.render_fwd(self.arch_c, self.arch_f, self.opts, self.blob_c, self.blob_f, self.rays,
                                                randoms, training=training, impl=self.impl, workspace=ws)
-        lay = self.ops.render_workspace_layout(self.arch_c, arch_f, self.opts, N_RAYS, training)
-        return out_c, out_f, Workspace(ws, lay, N_RAYS, self.nc, self.ns)
+        lay = self.ops.render_workspace_layout(self.arch_c, arch_f, self.opts, self.n, training)
+        return out_c, out_f, Workspace(ws, lay, self.n, self.nc, self.ns)
 
     def backward(self, randoms, ws, g_c, g_f, parts):
         """render_bwd into zeroed flat gradients; returns (flat_c, flat_f)."""
@@ -352,7 +377,7 @@ def _check_part(step, tag, arch, sd, ws, z, raw, stash, noise, out_g, rnd, ctx):
     parts, which = (1, 1) if tag == "fine" else (2, 0)
     impl = step.impl
     S = z.shape[1]
-    P = N_RAYS * S
+    P = step.n * S
     ctx = ctx + (tag,)
     family = "wgmma" if impl == 1 else "fp32"
 
@@ -399,7 +424,7 @@ def _check_part(step, tag, arch, sd, ws, z, raw, stash, noise, out_g, rnd, ctx):
                  _floors(arch, P, {k: v * c for k, v in split.items()} if split else None))
 
     # the whole chain: compositing of the oracle's raw in fp64 -> the oracle MLP, against training's gradient
-    raw_o = ref.raw.view(N_RAYS, S, 4)
+    raw_o = ref.raw.view(step.n, S, 4)
     d64 = _composite_grad64((raw_o.float(), raw_o), z, step.rays, noise, g_loss[which], step.cfg)
     chain = oracle_tiles(arch, sd, step.rays, z, d64)
     check_blocks(arch, flat_train, chain.grads, tc_blocks(arch), CHAIN_TOL, ctx + ("whole chain",),
@@ -441,12 +466,14 @@ def _check_against_training(step, rnd, g_c, g_f, fc, ff, ctx):
         return
     nb, ops = step.nb, step.ops
     cam, arch = step.cam, step.arch_c
-    models = []
-    for sd in (step.sd_c, step.sd_f):
+    models = [None, None]
+    for i, sd in enumerate((step.sd_c, step.sd_f)):
+        if sd is None:
+            continue
         m = nb.FlexibleNeRFModel(num_layers=arch.num_layers, hidden_size=arch.hidden, skip_connect_every=arch.skip_every,
                                  num_encoding_fn_xyz=arch.n_freq_xyz, num_encoding_fn_dir=arch.n_freq_dir)
         m.load_state_dict(sd)
-        models.append(m.cuda())
+        models[i] = m.cuda()
     cfg = step.cfg
     options = O.make_options(no_ndc=not cam["ndc"], near=cam["near"], far=cam["far"], num_coarse=step.nc,
                              num_fine=step.nf, perturb=cfg["perturb"], lindisp=cfg.get("lindisp", False),
@@ -456,9 +483,13 @@ def _check_against_training(step, rnd, g_c, g_f, fc, ff, ctx):
                                             encode_position_fn=nb.get_embedding_function(arch.n_freq_xyz),
                                             encode_direction_fn=nb.get_embedding_function(arch.n_freq_dir),
                                             randoms=rnd, impl=1)
-    loss = torch.nn.functional.mse_loss(out[0], step.target) + torch.nn.functional.mse_loss(out[3], step.target)
+    loss = torch.nn.functional.mse_loss(out[0], step.target)
+    if step.nf:
+        loss = loss + torch.nn.functional.mse_loss(out[3], step.target)
     loss.backward()
     for m, flat in zip(models, (fc, ff)):
+        if m is None:
+            continue
         got = ops.flatten_state_dict(arch, {k: p.grad for k, p in m.named_parameters()}, "cuda")
         assert torch.equal(got.view(torch.int32), flat.view(torch.int32)), ctx + ("run_one_iter_of_nerf_from_pose",)
 
@@ -472,7 +503,7 @@ def test_render_step_matches_fp64_stage_by_stage(name, impl):
     ctx = (name, f"impl {impl}")
     if cfg.get("variants") and impl == 1:
         # seeded randoms, the 4096 rays' global indices straddling 2^32, against ops.random_fill's tensors
-        rng = ops.SeededRandoms(seed=0x5EED, step=3, ray_offset=2 ** 32 - N_RAYS // 2)
+        rng = ops.SeededRandoms(seed=0x5EED, step=3, ray_offset=2 ** 32 - step.n // 2)
         rnd = _seeded_tensors(cfg, rng)
     else:
         rnd = _randoms(cfg, seed=5)
@@ -515,8 +546,8 @@ def test_render_step_matches_fp64_stage_by_stage(name, impl):
         for g, out in ((g_c, out_c), (g_f, out_f)):
             g = g.clone()
             scale = g[:, :3].abs().max().item()
-            g[:, 3] = torch.where(torch.isnan(out[:, 3]), 0.0, torch.randn(N_RAYS, generator=gen).cuda() * scale)
-            g[:, 4] = torch.randn(N_RAYS, generator=gen).cuda() * scale
+            g[:, 3] = torch.where(torch.isnan(out[:, 3]), 0.0, torch.randn(step.n, generator=gen).cuda() * scale)
+            g[:, 4] = torch.randn(step.n, generator=gen).cuda() * scale
             extra.append(g.contiguous())
         out_g["extra"] = tuple(extra)
 
@@ -534,3 +565,26 @@ def test_render_step_matches_fp64_stage_by_stage(name, impl):
         for a, b in zip(seeded, (fc, ff)):
             assert torch.equal(a.view(torch.int32), b.view(torch.int32)), ctx + ("seeded gradients",)
     _check_against_training(step, rnd, g_c, g_f, fc, ff, ctx)
+
+
+def test_wgmma_refuses_fewer_than_15_samples_before_any_launch():
+    """A 14-sample pass needs 11 rays in a 128-point tile, one more than the wgmma kernels hold: render_fwd (training or
+    not) and render_bwd on impl 1 refuse it before launching anything; impl 0 runs the same step (RUNS "nc14")."""
+    from nerf_pytorch_b200 import ops
+
+    step = Step("nc14", 1)
+    rnd = _randoms(step.cfg, seed=5)
+    n = step.n
+    ws = torch.zeros(ops.render_workspace_bytes(step.arch_c, None, step.opts, n, True), dtype=torch.uint8,
+                     device="cuda")
+    g = torch.zeros(n, 8, device="cuda")
+    flat = torch.zeros(step.arch_c.flat_param_count(), device="cuda")
+    torch.cuda.synchronize()
+    before = ops.launch_count()
+    for training in (True, False):
+        with pytest.raises(NotImplementedError, match="fewer than 15 samples"):
+            step.forward(rnd, training=training)
+    with pytest.raises(NotImplementedError, match="fewer than 15 samples"):
+        ops.render_bwd(step.arch_c, None, step.opts, step.blob_c, None, step.rays, rnd, g, None, ws, flat, None,
+                       impl=1, parts=3)
+    assert ops.launch_count() == before
