@@ -724,6 +724,36 @@ int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* br
                                    int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                    float* max_w, void* stream);
 
+/* ---- baked fields: half precision ----------------------------------------------------------------------------------
+ * A baked field whose values are stored in IEEE binary16, at half the bytes of the fp32 field, for fields that are kept,
+ * saved, rendered and pruned (PlenOctrees and SNeRG ship their fields in half precision).  Fine-tuning stays fp32: the
+ * fp16 entry points have no gradient, tie, Adam or regulariser twins; fine-tune the widened field and convert it back.
+ *   - Layout.  values[slot][729][32] binary16 (64 B per lattice point), the bits as uint16_t; the channels mean what they
+ *     mean in the fp32 field ("baked fields"), channels 28 .. 31 are 0.
+ *   - Conversion rule, fp32 -> fp16 channel by channel: a finite x with |x| > 65504 saturates to +-65504, then every
+ *     finite value is rounded to nearest even; +-inf and NaN stay +-inf and NaN (the NaN payload is not specified).  No
+ *     finite value becomes an infinity the fp32 field did not have (a -inf corner would make the trilinear sum -inf or
+ *     NaN).  In torch: torch.where(x.isfinite(), x.clamp(-65504, 65504), x).half(), the same bits.
+ *   - Rendering and peak weights (baked_render_f16, baked_max_weights_f16).  Each value is widened exactly to fp32 as it
+ *     is gathered; every other op is the fp32 rule of "baked fields" and "baked fields: pruning": the same corners in the
+ *     same order through the same fmaf chain.  An fp16 field therefore renders, and gives peak weights, bit for bit like
+ *     the fp32 field holding its widened values.  A corner's channels 0 .. 27 are three 16-B loads and one 8-B load (56
+ *     of its 64 B); the peak weights read sigma_raw alone, 2 B per corner.
+ *   - Bake (bake_f16).  The fp32 bake's values with the conversion rule applied at the store: bit-equal to converting
+ *     bake's output (NaN compared as a class).  The logits test hook stays fp32.
+ * bake_f16, baked_render_f16, baked_max_weights_f16: the arguments of bake, baked_render and baked_max_weights, values
+ *   binary16.  Refused before any launch: whatever their fp32 twins refuse (the same checks), and a values pointer that
+ *   is not 16-B aligned. */
+int32_t nerfb200_bake_f16(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box,
+                          const int32_t* bricks, int64_t first, int64_t count, uint16_t* values, float* logits,
+                          void* stream);
+int32_t nerfb200_baked_render_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                  int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                  int32_t white_background, float stop_transmittance, float* out, void* stream);
+int32_t nerfb200_baked_max_weights_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                       int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                       float* max_w, void* stream);
+
 /* ---- baked fields: regularisers -------------------------------------------------------------------------------------
  * Squared total variation of the density and of the SH coefficients over the lattice, and a Cauchy sparsity term on the
  * density (as Plenoxels regularises its voxels), with their gradient in the tie's convention, so that fine-tuning can

@@ -9,7 +9,9 @@ one warp per ray (csrc/baked.cu).  A baked field can be fine-tuned against image
 bricks its renders use (baked_transparent_bricks, baked_brick_weights, prune_baked, BakedFieldTrainer.prune;
 include/nerfb200.h "baked fields: pruning"), with total-variation and sparsity regularisers over the lattice
 (baked_regularizer, BakedFieldTrainer's tv_sigma / tv_sh / sparsity; include/nerfb200.h "baked fields: regularisers").  This file validates arguments, sizes buffers and moves
-pointers; the bake reads the active brick count back once to size its values."""
+pointers; the bake reads the active brick count back once to size its values.  A field kept, saved, rendered or pruned
+may store its values in fp16 (``bake(dtype=torch.float16)``, ``BakedField.half``; include/nerfb200.h "baked fields: half
+precision"); fine-tuning and the regularisers take fp32 fields only (``BakedField.float``)."""
 from __future__ import annotations
 
 import torch
@@ -20,7 +22,8 @@ from . import ops
 class BakedField:
     """A baked field on the device: ``bounds`` ((lo), (hi)) and ``resolution`` (three ints) of the lattice box,
     ``brick_map`` int32[bricks] (slot or -1), ``bricks`` int32[n_active] (slot -> brick), ``values``
-    fp32[n_active, 729, 32] and ``use_viewdirs`` (whether the network had view directions)."""
+    fp32[n_active, 729, 32] or fp16 of that shape (include/nerfb200.h "baked fields: half precision") and
+    ``use_viewdirs`` (whether the network had view directions)."""
 
     def __init__(self, bounds, resolution, brick_map, bricks, values, use_viewdirs: bool):
         self.bounds = (tuple(float(v) for v in bounds[0]), tuple(float(v) for v in bounds[1]))
@@ -34,15 +37,43 @@ class BakedField:
     def n_active(self) -> int:
         return int(self.values.shape[0])
 
+    @property
+    def dtype(self) -> torch.dtype:
+        """The values' dtype: torch.float32 or torch.float16."""
+        return self.values.dtype
+
     def box(self):
         return ops.grid_struct(self.bounds, self.resolution)
 
+    def half(self, chunk: int = 1024) -> "BakedField":
+        """A new field with fp16 values under the conversion rule (include/nerfb200.h "baked fields: half precision"): a
+        finite value saturates to +-65504 and rounds to nearest even, +-inf and NaN stay.  Converted ``chunk`` slots at a
+        time, so the peak is both fields plus one chunk's temporaries; ``brick_map`` and ``bricks`` are shared.  Renders
+        and peak weights of the result are bit for bit those of ``result.float()``.  Works on a CPU field too."""
+        chunk = int(chunk)
+        if chunk < 1:
+            raise ValueError(f"BakedField.half: chunk must be >= 1, got {chunk}")
+        v = self.values.detach()
+        out = torch.empty(v.shape, dtype=torch.float16, device=v.device)
+        for s in range(0, self.n_active, chunk):
+            c = v[s:s + chunk]
+            out[s:s + chunk] = torch.where(c.isfinite(), c.clamp(-65504.0, 65504.0), c)  # the copy rounds to nearest even
+        return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, out, self.use_viewdirs)
+
+    def float(self) -> "BakedField":
+        """A field with fp32 values: an fp16 field widened exactly (a new tensor), an fp32 field's own values tensor.
+        ``brick_map`` and ``bricks`` are shared.  Fine-tune ``field.float()``, then convert back with ``half()``."""
+        v = self.values if self.values.dtype == torch.float32 else self.values.detach().float()
+        return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, v, self.use_viewdirs)
+
     def __repr__(self):
         return (f"BakedField({self.n_active} bricks of {ops.mesh_sparse_brick_count(self.box())}, "
-                f"{self.values.numel() * 4 / 2 ** 20:.1f} MiB, resolution {self.resolution}"
+                f"{self.values.numel() * self.values.element_size() / 2 ** 20:.1f} MiB"
+                f"{' fp16' if self.dtype == torch.float16 else ''}, resolution {self.resolution}"
                 f"{', view directions' if self.use_viewdirs else ''})")
 
     def save(self, path) -> None:
+        """Writes the field with torch.save; the values keep their dtype."""
         torch.save({"bounds": self.bounds, "resolution": self.resolution, "brick_map": self.brick_map.cpu(),
                     "bricks": self.bricks.cpu(), "values": self.values.cpu(), "use_viewdirs": self.use_viewdirs}, path)
 
@@ -53,15 +84,20 @@ class BakedField:
                    d["values"].to(device), d["use_viewdirs"])
 
 
-def bake(model, encode_position_fn, encode_direction_fn=None, *, bounds, resolution, grid) -> BakedField:
+def bake(model, encode_position_fn, encode_direction_fn=None, *, bounds, resolution, grid,
+         dtype=torch.float32) -> BakedField:
     """Bake ``model`` (the network that renders the final image: pass ``model_fine``) over the lattice box ``bounds``
     / ``resolution`` (as ``extract_mesh``; up to 4096 cubes per axis) on the bricks ``grid`` (an ``nb.OccupancyGrid`` on
     the model's device) calls occupied, under the sparse meshes' activity rule.  The field lives in the coordinates the
-    MLP encodes: world space for Blender scenes, NDC for LLFF scenes.  Argument errors raise ValueError, an
+    MLP encodes: world space for Blender scenes, NDC for LLFF scenes.  ``dtype`` torch.float16 stores the values in
+    half precision straight from the kernel (the conversion rule of ``BakedField.half`` at the store: the bits of
+    ``bake(...).half()``, at half the memory and without an fp32 copy).  Argument errors raise ValueError, an
     architecture the wgmma inference forward refuses NotImplementedError, before any launch."""
     from . import train_utils
     from .mesh import _box, _check_grid, _network
 
+    if dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"bake: dtype must be torch.float32 or torch.float16, got {dtype!r}")
     lo, hi, res = _box(bounds, resolution, dense=False)
     arch = _network(model, encode_position_fn, encode_direction_fn)
     dev = next(model.parameters()).device
@@ -73,7 +109,7 @@ def bake(model, encode_position_fn, encode_direction_fn=None, *, bounds, resolut
     box = ops.grid_struct((lo, hi), res)
     brick_map, bricks, n_dev = ops.mesh_sparse_bricks(box, grid)
     n_active = int(n_dev.item())
-    values = torch.empty(n_active, 729, 32, dtype=torch.float32, device=dev)
+    values = torch.empty(n_active, 729, 32, dtype=dtype, device=dev)
     if n_active:
         with torch.no_grad():
             ops.bake(arch, blob, box, bricks, 0, n_active, values)
@@ -121,11 +157,16 @@ def _pose_rays(field, height, width, focal_length, tform_cam2world, options):
                         use_viewdirs=field.use_viewdirs)
 
 
-def _check_values(field, what):
+def _check_values(field, what, half=False):
+    """A CUDA field with fp32 values, or fp16 ones where ``half`` (renders and peak weights; fine-tuning is fp32 only)."""
     if not isinstance(field, BakedField):
         raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
-    if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda and field.values.dtype == torch.float32):
-        raise ValueError(f"{what}: field.values must be an fp32 CUDA tensor (there is no CPU or fp16 path)")
+    if isinstance(field.values, torch.Tensor) and field.values.dtype == torch.float16 and not half:
+        raise ValueError(f"{what}: an fp16 field has no gradient or fine-tuning path; fine-tune field.float() and "
+                         f"convert it back with .half()")
+    if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda
+            and field.values.dtype in (torch.float32, torch.float16)):
+        raise ValueError(f"{what}: field.values must be an fp32 or fp16 CUDA tensor (there is no CPU path)")
 
 
 class _BakedRender(torch.autograd.Function):
@@ -156,8 +197,17 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
     without (``ops.gen_rays`` / ``ops.gen_rays_posed``) through ``field``.  Differentiable with respect to
     ``field.values`` when it requires grad: the gradient is the baked renderer's backward summed over every stored copy
     of each lattice point (include/nerfb200.h "baked fields: gradients and fine-tuning"), so copies that start equal stay
-    equal under any elementwise optimiser.  ``early_stop`` as in ``render_baked``, for renders without a gradient."""
-    _check_values(field, "render_baked_rays")
+    equal under any elementwise optimiser.  ``early_stop`` as in ``render_baked``, for renders without a gradient.
+
+    An fp16 field renders bit for bit like ``field.float()`` and has no gradient.  This is the differentiable render,
+    which refuses an fp16 field in grad mode as it did before fp16 fields could be rendered at all; under
+    ``torch.no_grad()`` (or inference mode) it renders one whose values do not require grad.  Anything else raises
+    ValueError (fine-tune ``field.float()``).  ``render_baked`` renders an fp16 field in any grad mode."""
+    _check_values(field, "render_baked_rays", half=True)
+    # grad mode alone keeps the refusal every fp16 field met here before half precision (pinned by the fine-tuning tests)
+    if field.values.dtype == torch.float16 and (field.values.requires_grad or torch.is_grad_enabled()):
+        raise ValueError("render_baked_rays: an fp16 field has no gradient; render it under torch.no_grad(), or "
+                         "fine-tune field.float() and convert it back with .half()")
     stride = 11 if field.use_viewdirs else 8
     if not (isinstance(rays, torch.Tensor) and rays.dim() == 2 and rays.shape[1] == stride):
         raise ValueError(f"render_baked_rays: rays must be (N, {stride}) for a field "
@@ -416,7 +466,7 @@ def baked_brick_weights_rays(field: BakedField, rays, out=None) -> torch.Tensor:
     if out is not None and not (isinstance(out, torch.Tensor) and out.dtype == torch.float32
                                 and out.shape == (field.n_active,) and out.is_contiguous()):
         raise ValueError(f"baked_brick_weights_rays: out must be a contiguous fp32 tensor of shape ({field.n_active},)")
-    _check_values(field, "baked_brick_weights_rays")
+    _check_values(field, "baked_brick_weights_rays", half=True)
     dev = field.values.device
     if rays.device != dev or (out is not None and out.device != dev):
         raise ValueError(f"baked_brick_weights_rays: rays and out must be on the field's device {dev}")
@@ -441,7 +491,7 @@ def baked_brick_weights(field: BakedField, poses, height, width, focal_length, o
         raise ValueError("baked_brick_weights: poses must be a float tensor (n, 3 | 4, 4) with n >= 1")
     if not (int(height) > 0 and int(width) > 0):
         raise ValueError(f"baked_brick_weights: need height, width > 0, got {height}, {width}")
-    _check_values(field, "baked_brick_weights")
+    _check_values(field, "baked_brick_weights", half=True)
     _check_viewdirs(field, options, "baked_brick_weights")
     out = torch.zeros(field.n_active, dtype=torch.float32, device=field.values.device)
     if field.n_active == 0:

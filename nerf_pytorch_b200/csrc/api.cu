@@ -644,22 +644,40 @@ int32_t nerfb200_bake_supported(const nerfb200_arch_t* arch) {
   return bake_check(p);
 }
 
-int32_t nerfb200_bake(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box, const int32_t* bricks,
-                      int64_t first, int64_t count, float* values, float* logits, void* stream) {
-  Plan p;
-  NB_TRY(build_plan(arch, &p));
-  NB_TRY(check_grid(box, "bake"));
+// the checks bake and bake_f16 share: the plan into *p, then the box, the pointers, the slot range, the architecture
+static int check_bake(const char* what, const nerfb200_arch_t* arch, Plan* p, const float* blob,
+                      const nerfb200_grid_t* box, const int32_t* bricks, int64_t first, int64_t count,
+                      const void* values) {
+  NB_TRY(build_plan(arch, p));
+  NB_TRY(check_grid(box, what));
   const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
   if (!blob || !bricks || !values || first < 0 || count <= 0 || first + count > n_bricks) {
-    set_error("bake: null pointer, or slots %lld .. %lld outside the box's %lld bricks", (long long)first,
+    set_error("%s: null pointer, or slots %lld .. %lld outside the box's %lld bricks", what, (long long)first,
               (long long)(first + count - 1), (long long)n_bricks);
     return NERFB200_ERR_INVALID;
   }
   if (count * kBakePts >= (int64_t(1) << 31)) {
-    set_error("bake: %lld bricks are 2^31 lattice points or more in one call; split the slots", (long long)count);
+    set_error("%s: %lld bricks are 2^31 lattice points or more in one call; split the slots", what, (long long)count);
     return NERFB200_ERR_UNSUPPORTED;
   }
-  NB_TRY(bake_check(p));
+  return bake_check(*p);
+}
+
+int32_t nerfb200_bake(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box, const int32_t* bricks,
+                      int64_t first, int64_t count, float* values, float* logits, void* stream) {
+  Plan p;
+  NB_TRY(check_bake("bake", arch, &p, blob, box, bricks, first, count, values));
+  BakeBasis basis;
+  bake_basis(&basis);
+  return launch_bake_tc(p, blob, *box, bricks, first, count, values, logits, basis, static_cast<cudaStream_t>(stream));
+}
+
+int32_t nerfb200_bake_f16(const nerfb200_arch_t* arch, const float* blob, const nerfb200_grid_t* box,
+                          const int32_t* bricks, int64_t first, int64_t count, uint16_t* values, float* logits,
+                          void* stream) {
+  Plan p;
+  NB_TRY(check_bake("bake_f16", arch, &p, blob, box, bricks, first, count, values));
+  NB_TRY(check_f16_values("bake_f16", values));
   BakeBasis basis;
   bake_basis(&basis);
   return launch_bake_tc(p, blob, *box, bricks, first, count, values, logits, basis, static_cast<cudaStream_t>(stream));

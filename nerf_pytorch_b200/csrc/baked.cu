@@ -19,6 +19,8 @@
 //             value partial reduced in a fixed order.
 #include <cmath>
 
+#include <cuda_fp16.h>
+
 #include "composite.cuh"
 
 namespace nerfb200 {
@@ -67,6 +69,14 @@ void bake_basis(BakeBasis* b) {
   }
   for (int j = 0; j < kBakeSh; ++j)
     for (int i = 0; i < kBakeDirs; ++i) b->proj[j][i] = (float)A[j][kBakeSh + i];
+}
+
+int check_f16_values(const char* what, const void* values) {
+  if (reinterpret_cast<uintptr_t>(values) % 16 != 0) {
+    set_error("%s: values must be 16-B aligned", what);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
 }
 
 namespace {
@@ -158,44 +168,79 @@ __device__ __forceinline__ float corner_weight(const float f[3], int k) {
   return __fmul_rn(__fmul_rn(wx, wy), wz);
 }
 
-// float4 offset of corner k of the cube at brick point l, from the slot's first value
+// 16-B offset of corner k of the cube at brick point l, from the slot's first value: a point is kBakeCh values of type V
+// (8 vectors of fp32, 4 of fp16)
+template <typename V>
 __device__ __forceinline__ int corner_offset(const int l[3], int k) {
   const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
-  return (((l[2] + dz) * 9 + l[1] + dy) * 9 + l[0] + dx) * (kBakeCh / 4);
+  return (((l[2] + dz) * 9 + l[1] + dy) * 9 + l[0] + dx) * (kBakeCh * (int)sizeof(V) / 16);
 }
 
-// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0)
-__device__ __forceinline__ void baked_interp(const float* __restrict__ values, int slot, const float f[3],
-                                             const int l[3], float v[kBakedVals]) {
+// four fp16 values (the bits of two 32-bit words) widened exactly to fp32
+__device__ __forceinline__ void widen4(unsigned a, unsigned b, float out[4]) {
+  out[0] = __half2float(__ushort_as_half((unsigned short)(a & 0xffffu)));
+  out[1] = __half2float(__ushort_as_half((unsigned short)(a >> 16)));
+  out[2] = __half2float(__ushort_as_half((unsigned short)(b & 0xffffu)));
+  out[3] = __half2float(__ushort_as_half((unsigned short)(b >> 16)));
+}
+
+// one stored value, widened to fp32
+__device__ __forceinline__ float baked_ld(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float baked_ld(const __half* p) {
+  return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(p))));
+}
+
+// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0).  fp32: seven 16-B loads per corner; fp16:
+// three 16-B loads and one 8-B load (56 of the point's 64 B), each value widened exactly, then the same fmaf chain
+template <typename V>
+__device__ __forceinline__ void baked_interp(const V* __restrict__ values, int slot, const float f[3], const int l[3],
+                                             float v[kBakedVals]) {
 #pragma unroll
   for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = 0.f;
   if (slot >= 0) {
-    const float4* base = reinterpret_cast<const float4*>(values + (int64_t)slot * kBakePts * kBakeCh);
+    const V* sv = values + (int64_t)slot * kBakePts * kBakeCh;
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const float w = corner_weight(f, k);
-      const float4* pv = base + corner_offset(l, k);
+      if constexpr (sizeof(V) == 4) {
+        const float4* pv = reinterpret_cast<const float4*>(sv) + corner_offset<V>(l, k);
 #pragma unroll
-      for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
-        const float4 a = __ldg(pv + c4);
-        v[4 * c4] = fmaf(w, a.x, v[4 * c4]);
-        v[4 * c4 + 1] = fmaf(w, a.y, v[4 * c4 + 1]);
-        v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
-        v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
+        for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+          const float4 a = __ldg(pv + c4);
+          v[4 * c4] = fmaf(w, a.x, v[4 * c4]);
+          v[4 * c4 + 1] = fmaf(w, a.y, v[4 * c4 + 1]);
+          v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
+          v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
+        }
+      } else {
+        const uint4* pv = reinterpret_cast<const uint4*>(sv) + corner_offset<V>(l, k);
+        float a[kBakedVals];
+#pragma unroll
+        for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {  // channels 0 .. 23
+          const uint4 u = __ldg(pv + c8);
+          widen4(u.x, u.y, a + 8 * c8);
+          widen4(u.z, u.w, a + 8 * c8 + 4);
+        }
+        const uint2 u = __ldg(reinterpret_cast<const uint2*>(pv + kBakedVals / 8));  // channels 24 .. 27
+        widen4(u.x, u.y, a + 24);
+#pragma unroll
+        for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(w, a[ch], v[ch]);
       }
     }
   }
 }
 
-// channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B load
-// per corner
-__device__ __forceinline__ float baked_interp_sigma(const float* __restrict__ values, int slot, const float f[3],
+// channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B (fp32)
+// or 2-B (fp16) load per corner
+template <typename V>
+__device__ __forceinline__ float baked_interp_sigma(const V* __restrict__ values, int slot, const float f[3],
                                                     const int l[3]) {
   float v = 0.f;
   if (slot >= 0) {
-    const float* base = values + (int64_t)slot * kBakePts * kBakeCh;
+    const V* base = values + (int64_t)slot * kBakePts * kBakeCh;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) v = fmaf(corner_weight(f, k), __ldg(base + 4 * corner_offset(l, k)), v);
+    for (int k = 0; k < 8; ++k)
+      v = fmaf(corner_weight(f, k), baked_ld(base + (16 / (int)sizeof(V)) * corner_offset<V>(l, k)), v);
   }
   return v;
 }
@@ -216,8 +261,9 @@ __device__ __forceinline__ void baked_colour(int use_viewdirs, const float Y[kBa
   }
 }
 
+template <typename V>
 __global__ void __launch_bounds__(kBakedWarps * 32)
-baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
+baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values,
                     int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
                     float stop_t, float* __restrict__ out) {
   const int lane = threadIdx.x & 31;
@@ -350,7 +396,7 @@ baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, con
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const float wk = corner_weight(f, k);
-      float4* pv = base + corner_offset(l, k);
+      float4* pv = base + corner_offset<float>(l, k);
       float gk[kBakedVals];
       gk[0] = __fmul_rn(wk, dsigma);
 #pragma unroll
@@ -368,8 +414,9 @@ baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, con
 // w as +inf.  The warp re-marches the ray as baked_render_kernel does, interpolating sigma_raw alone; per round the lanes
 // with w > 0 are grouped by slot and one lane per group issues an integer atomicMax of the group's largest bits
 // (non-negative floats order as unsigned integers).  No stop at T = 0: a NaN later in the ray must still be recorded.
+template <typename V>
 __global__ void __launch_bounds__(kBakedWarps * 32)
-baked_max_weight_kernel(const BakedBox B, const int* __restrict__ brick_map, const float* __restrict__ values,
+baked_max_weight_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values,
                         const float* __restrict__ rays, int ray_stride, int64_t n_rays, unsigned* __restrict__ max_w) {
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
@@ -669,41 +716,107 @@ int32_t nerfb200_bake_basis(float* dirs_host, float* proj_host) {
   return NERFB200_OK;
 }
 
-int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
-                              int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
-                              int32_t white_background, float stop_transmittance, float* out, void* stream) {
-  if (int rc = check_grid(box, "baked_render")) return rc;
+}  // extern "C"
+
+namespace {
+
+// the checks baked_render and baked_render_f16 share (what: the entry point's name in the error)
+int check_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
+                       int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                       float stop_transmittance, const float* out) {
+  if (int rc = check_grid(box, what)) return rc;
   if (!brick_map || !values || !rays || !out || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
-    set_error("baked_render: null pointer, n_rays <= 0 or ray_stride %d too short", ray_stride);
+    set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
     return NERFB200_ERR_INVALID;
   }
   if (!(stop_transmittance >= 0.f && stop_transmittance < 1.f)) {
-    set_error("baked_render: stop_transmittance must lie in [0, 1), got %g", (double)stop_transmittance);
+    set_error("%s: stop_transmittance must lie in [0, 1), got %g", what, (double)stop_transmittance);
     return NERFB200_ERR_INVALID;
   }
+  return NERFB200_OK;
+}
+
+// the checks baked_max_weights and baked_max_weights_f16 share
+int check_baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
+                            int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                            const float* max_w) {
+  if (int rc = check_grid(box, what)) return rc;
+  if (!brick_map || !values || !rays || !max_w || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
+    set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
+}
+
+template <typename V>
+int launch_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                        int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                        int32_t white_background, float stop_transmittance, float* out, void* stream) {
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
-  baked_render_kernel<<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+  baked_render_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0,
       stop_transmittance, out);
   count_launch();
-  return check_cuda(cudaGetLastError(), "baked_render launch");
+  return check_cuda(cudaGetLastError(), what);
+}
+
+template <typename V>
+int launch_baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                             const float* rays, int32_t ray_stride, int64_t n_rays, float* max_w, void* stream) {
+  const BakedBox B = baked_box(box);
+  const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
+  baked_max_weight_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+      B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w));
+  count_launch();
+  return check_cuda(cudaGetLastError(), what);
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                              int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                              int32_t white_background, float stop_transmittance, float* out, void* stream) {
+  const char *what = "baked_render", *launch = "baked_render launch";
+  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                                  stop_transmittance, out))
+    return rc;
+  return launch_baked_render(launch, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, white_background,
+                             stop_transmittance, out, stream);
+}
+
+int32_t nerfb200_baked_render_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                  int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                  int32_t white_background, float stop_transmittance, float* out, void* stream) {
+  const char *what = "baked_render_f16", *launch = "baked_render_f16 launch";
+  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                                  stop_transmittance, out))
+    return rc;
+  if (int rc = check_f16_values(what, values)) return rc;
+  return launch_baked_render(launch, box, brick_map, reinterpret_cast<const __half*>(values), use_viewdirs, rays,
+                             ray_stride, n_rays, white_background, stop_transmittance, out, stream);
 }
 
 int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                                    int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                    float* max_w, void* stream) {
-  if (int rc = check_grid(box, "baked_max_weights")) return rc;
-  if (!brick_map || !values || !rays || !max_w || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
-    set_error("baked_max_weights: null pointer, n_rays <= 0 or ray_stride %d too short", ray_stride);
-    return NERFB200_ERR_INVALID;
-  }
-  const BakedBox B = baked_box(box);
-  const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
-  baked_max_weight_kernel<<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
-      B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w));
-  count_launch();
-  return check_cuda(cudaGetLastError(), "baked_max_weights launch");
+  const char *what = "baked_max_weights", *launch = "baked_max_weights launch";
+  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
+    return rc;
+  return launch_baked_max_weights(launch, box, brick_map, values, rays, ray_stride, n_rays, max_w, stream);
+}
+
+int32_t nerfb200_baked_max_weights_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                       int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                       float* max_w, void* stream) {
+  const char *what = "baked_max_weights_f16", *launch = "baked_max_weights_f16 launch";
+  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
+    return rc;
+  if (int rc = check_f16_values(what, values)) return rc;
+  return launch_baked_max_weights(launch, box, brick_map, reinterpret_cast<const __half*>(values), rays, ray_stride,
+                                  n_rays, max_w, stream);
 }
 
 int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,

@@ -220,6 +220,12 @@ void bake_basis(BakeBasis* b);  // host, fp64 rounded once (baked.cu)
 int bake_tc_supported(const Plan& p, const char* what);
 int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
                    int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s);
+// the check every fp16 baked-field entry point adds to its fp32 twin's: values 16-B aligned, as the renderer's vector
+// gathers need (baked.cu)
+int check_f16_values(const char* what, const void* values);
+// the same bake storing fp16 values (the conversion rule of nerfb200.h "baked fields: half precision" at the store)
+int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
+                   int64_t count, uint16_t* values, float* logits, const BakeBasis& basis, cudaStream_t s);
 // ---- normal maps of a render's last pass (normals.cu; nerfb200.h "normal maps") ----
 // The samples with nonzero compositing weight, compacted: count[r], first[r] (their first slot), *total; pts[slot][3] =
 // o + d z as the MLP forms it

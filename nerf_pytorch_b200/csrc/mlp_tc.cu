@@ -35,6 +35,8 @@
 // per operand instead of 22); the heads and the direction term stay fp32.  The producer streams only the hs part of
 // each k-step (32 n bytes, contiguous in the blob) and packs stage bytes / (32 n) k-steps into a ring stage; the
 // prologue and the epilogue write only the hi half of the operand tiles.
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -1009,11 +1011,18 @@ __device__ __forceinline__ float bake_coord(const nerfb200_grid_t& b, int c, int
   return __fadd_rn(b.lo[c], __fdiv_rn(__fmul_rn(__fsub_rn(b.hi[c], b.lo[c]), (float)i), (float)b.res[c]));
 }
 
-template <int kH>
+// fp32 -> fp16 under the half-precision fields' conversion rule (nerfb200.h "baked fields: half precision"): a finite x
+// saturates to +-65504, then rounds to nearest even; +-inf and NaN stay what they are
+__device__ __forceinline__ __half half_saturated(float x) {
+  return __float2half_rn(fabsf(x) < INFINITY ? fminf(fmaxf(x, -65504.f), 65504.f) : x);
+}
+
+// V: the stored value type, float or __half (the conversion rule applied at the store; everything else is shared)
+template <int kH, typename V>
 __global__ void __launch_bounds__(128 * bake_wg(kH) + 32, 1)
 bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis basis, const float* __restrict__ blob,
                const nerfb200_grid_t box, const int* __restrict__ bricks, int64_t first, int64_t R, int64_t n_tiles,
-               float* __restrict__ values,   // out [slot][729][32]
+               V* __restrict__ values,       // out [slot][729][32]
                float* __restrict__ logits) { // out [R][64][3] or null
   constexpr int kWG = bake_wg(kH), kRows = 64 * kWG, kThreads = 128 * kWG + 32, kStage = bake_stage(kH);
   constexpr int kN = kH / 2;  // layers_dir[0]'s width
@@ -1230,12 +1239,14 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
       for (int i = 0; i < 2; ++i) {
         const int64_t r = p0 + lr0 + 8 * i;
         if (r < R) {
-          float* out = values + (first * kBakePts + r) * kBakeCh;
+          V* out = values + (first * kBakePts + r) * kBakeCh;
           const float sigma = s_head[(lr0 + 8 * i) * 4 + 3];
 #pragma unroll
           for (int m = 0; m < 8; ++m) {
             const int k = q + 4 * m - 1;
-            out[q + 4 * m] = k < 0 ? sigma : (m < 7 && k < kBakeSh * 3) ? sh[i][m < 7 ? m : 0] : 0.f;
+            const float x = k < 0 ? sigma : (m < 7 && k < kBakeSh * 3) ? sh[i][m < 7 ? m : 0] : 0.f;
+            if constexpr (sizeof(V) == 4) out[q + 4 * m] = x;
+            else out[q + 4 * m] = half_saturated(x);
           }
         }
       }
@@ -1257,13 +1268,13 @@ int bake_tc_supported(const Plan& p, const char* what) {
   return NERFB200_OK;
 }
 
-template <int kH>
+template <int kH, typename V>
 static int launch_bake(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
-                       int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
+                       int64_t count, V* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
   constexpr int kRows = 64 * bake_wg(kH), kThreads = 2 * kRows + 32;
   const int64_t R = count * kBakePts;
   const int64_t tiles = (R + kRows - 1) / kRows;
-  return launch_persistent(bake_tc_kernel<kH>, tiles, kThreads, bake_smem_map(p).m.total, s, "bake launch", p, basis,
+  return launch_persistent(bake_tc_kernel<kH, V>, tiles, kThreads, bake_smem_map(p).m.total, s, "bake launch", p, basis,
                            blob, box, (const int*)bricks, first, R, tiles, values, logits);
 }
 
@@ -1271,6 +1282,13 @@ int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box,
                    int64_t count, float* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
   return p.hidden == 256 ? launch_bake<256>(p, blob, box, bricks, first, count, values, logits, basis, s)
                          : launch_bake<128>(p, blob, box, bricks, first, count, values, logits, basis, s);
+}
+
+int launch_bake_tc(const Plan& p, const float* blob, const nerfb200_grid_t& box, const int32_t* bricks, int64_t first,
+                   int64_t count, uint16_t* values, float* logits, const BakeBasis& basis, cudaStream_t s) {
+  __half* h = reinterpret_cast<__half*>(values);
+  return p.hidden == 256 ? launch_bake<256>(p, blob, box, bricks, first, count, h, logits, basis, s)
+                         : launch_bake<128>(p, blob, box, bricks, first, count, h, logits, basis, s);
 }
 
 }  // namespace nerfb200

@@ -985,22 +985,37 @@ def bake_refusal(arch: ArchSpec) -> Optional[str]:
     return lib.nerfb200_last_error().decode(errors="replace")
 
 
+def _baked_values(values, what):
+    """(entry point suffix, pointer) of baked ``values``: "" for fp32, "_f16" for fp16 (include/nerfb200.h "baked
+    fields: half precision"); any other dtype is refused."""
+    if values.dtype == torch.float32:
+        return "", _ptr(values)
+    if values.dtype == torch.float16:
+        return "_f16", _ptr(values.view(torch.uint8))  # _ptr takes no fp16; the pointer is the same
+    raise ValueError(f"nerfb200 {what}: baked values must be fp32 or fp16, got {values.dtype}")
+
+
 def bake(arch: ArchSpec, blob, box: Grid, bricks, first: int, count: int, values, logits=None):
-    """The values of slots first .. first + count - 1 into ``values`` (n_active, 729, 32); ``logits`` (count * 729, 64,
-    3) or None receives the network's rgb logits at the 64 directions (a test hook)."""
-    _lib.check(_lib.load().nerfb200_bake(C.byref(arch.c_struct()), _ptr(blob), C.byref(box), _ptr(bricks), int(first),
-                                         int(count), _ptr(values), _ptr(logits), _stream()), "bake")
+    """The values of slots first .. first + count - 1 into ``values`` (n_active, 729, 32), fp32 or fp16 (the conversion
+    rule at the store); ``logits`` (count * 729, 64, 3) fp32 or None receives the network's rgb logits at the 64
+    directions (a test hook)."""
+    sfx, pv = _baked_values(values, "bake")
+    _lib.check(getattr(_lib.load(), "nerfb200_bake" + sfx)(C.byref(arch.c_struct()), _ptr(blob), C.byref(box),
+                                                           _ptr(bricks), int(first), int(count), pv, _ptr(logits),
+                                                           _stream()), "bake" + sfx)
     return values
 
 
 def baked_render(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool,
                  stop_transmittance: float = 0.0, out=None) -> torch.Tensor:
-    """Rows (n, 8) = [r g b disp acc depth 0 0] of the packed ``rays`` through a baked field."""
+    """Rows (n, 8) = [r g b disp acc depth 0 0] of the packed ``rays`` through a baked field whose ``values`` are fp32
+    or fp16."""
+    sfx, pv = _baked_values(values, "baked_render")
     n = rays.shape[0]
     out = torch.empty(n, 8, dtype=torch.float32, device=rays.device) if out is None else out
-    _lib.check(_lib.load().nerfb200_baked_render(C.byref(box), _ptr(brick_map), _ptr(values), int(bool(use_viewdirs)),
-                                                 _ptr(rays), rays.shape[1], n, int(bool(white_background)),
-                                                 float(stop_transmittance), _ptr(out), _stream()), "baked_render")
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_render" + sfx)(
+        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], n,
+        int(bool(white_background)), float(stop_transmittance), _ptr(out), _stream()), "baked_render" + sfx)
     return out
 
 
@@ -1027,10 +1042,11 @@ def baked_tie(box: Grid, brick_map, bricks, d_values, d_tied=None):
 def baked_max_weights(box: Grid, brick_map, values, use_viewdirs: bool, rays, max_w):
     """Max-accumulates into ``max_w`` fp32[n_active] each brick slot's largest rendering weight over the packed
     ``rays`` (``baked_render``'s weights at stop 0; a NaN weight as +inf).  Zero ``max_w`` once before the first
-    chunk."""
-    _lib.check(_lib.load().nerfb200_baked_max_weights(C.byref(box), _ptr(brick_map), _ptr(values),
-                                                      int(bool(use_viewdirs)), _ptr(rays), rays.shape[1],
-                                                      rays.shape[0], _ptr(max_w), _stream()), "baked_max_weights")
+    chunk.  ``values`` fp32 or fp16."""
+    sfx, pv = _baked_values(values, "baked_max_weights")
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_max_weights" + sfx)(
+        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], rays.shape[0],
+        _ptr(max_w), _stream()), "baked_max_weights" + sfx)
     return max_w
 
 
