@@ -796,6 +796,42 @@ int32_t nerfb200_baked_regularizer(const nerfb200_grid_t* box, const int32_t* br
                                    int64_t n_active, const float* values, const int64_t* count, double tv_sigma,
                                    double tv_sh, double sparsity, float* d, double* partials, void* stream);
 
+/* ---- baked fields: subdivision --------------------------------------------------------------------------------------
+ * The field on the box (lo, hi, 2 res) that holds the same trilinear function as a field on (lo, hi, res), so that a
+ * field can be trained coarse to fine (as Plenoxels upsamples its grid): train, prune, subdivide, train again.
+ *   - Child bricks.  Per axis, parent brick pb has the children 2 pb + delta, delta in {0, 1}, that exist in the child
+ *     box (8 (2 pb + delta) < 2 res, i.e. 2 pb + delta < the child box's bricks along that axis); a partial parent brick
+ *     on an upper face can have only delta = 0 along that axis.  The child field's active bricks are the children of
+ *     every active parent brick, in ascending child-brick order (so its bricks are sorted and its brick_map is their
+ *     rank, as mesh_sparse_bricks produces them).  The caller forms this list; the library fills its values.
+ *   - Values.  Child corner point l of child brick b' holds the child lattice index q' = min(8 b' + l, 2 res) per axis,
+ *     which lies at the parent half-index q' / 2.  Along an axis where q' is even it uses the parent point q' / 2 with
+ *     weight 1; where q' is odd it uses (q' - 1) / 2 and (q' + 1) / 2 with weight 1/2 each.  With m the number of odd
+ *     axes, the value is over the 2^m parent points:
+ *       m = 0: the parent point's bits (a copy: -0, inf and NaN payloads included);
+ *       m >= 1: the points visited in the renderer's corner order (k = 0 .. 7, offset (k & 1, k >> 1 & 1, k >> 2))
+ *               skipping those with offset 1 along an even axis; each term is w v with w = 2^-m, acc = the first term,
+ *               then acc = acc + term.  fp32, each op rounded, no contraction, no flush to zero (w v is exact unless it
+ *               is subnormal).
+ *     Every parent point is read from its copy in parent brick floor(b' / 2) (local points 4 delta .. 4 delta + 4 per
+ *     axis), so child copies are bit-equal wherever the parent's copies are, as they are after a bake and after every
+ *     tied update.  All 28 channels go through the rule; channels 28 .. 31 are written 0.  A child whose parent brick's
+ *     brick_map entry is -1 (or not below n_active) is written as all zeros.
+ *   - Why the function is preserved.  The cell rule's scale = (float) res / (hi - lo) doubles exactly, so the child
+ *     cell coordinate is exactly twice the parent's, and a trilinear function restricted to a sub-cube is its
+ *     interpolation of the sub-cube's corner values.  The child field therefore renders the parent's continuous
+ *     sigma_raw and SH field up to the fp32 rounding of the new lattice values; only the renderer's sample spacing,
+ *     half the smallest cube side, halves.
+ * baked_subdivide: box, brick_map and values[n_active][729][32] the parent field (fp32); child_bricks[n_child] the child
+ *   box's active bricks as above; child_values[n_child][729][32] fp32 receives the child field.  One CTA per child slot
+ *   staging the 5 x 5 x 5 parent points it reads in shared memory; offsets in 64 bits.  n_child 0 launches nothing.
+ * Refused before any launch: an invalid box or 2 res > 4096 on any axis, a null pointer, n_active outside 0 .. the
+ * parent box's bricks, n_child outside 0 .. the child box's bricks, child_values overlapping values.  No atomics, no host
+ * synchronisation.  fp16 fields have no subdivision: subdivide the widened field. */
+int32_t nerfb200_baked_subdivide(const nerfb200_grid_t* box, const int32_t* brick_map, int64_t n_active,
+                                 const float* values, const int32_t* child_bricks, int64_t n_child,
+                                 float* child_values, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

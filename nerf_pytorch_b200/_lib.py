@@ -170,6 +170,7 @@ SIGNATURES = {
     "nerfb200_bake_f16": (I32, [AP, P, GP, P, I64, I64, P, P, P]),
     "nerfb200_baked_render_f16": (I32, [GP, P, P, I32, P, I32, I64, I32, F32, P, P]),
     "nerfb200_baked_max_weights_f16": (I32, [GP, P, P, I32, P, I32, I64, P, P]),
+    "nerfb200_baked_subdivide": (I32, [GP, P, I64, P, P, I64, P, P]),
 }
 
 _lib = None

@@ -9,10 +9,15 @@ one warp per ray (csrc/baked.cu).  A baked field can be fine-tuned against image
 bricks its renders use (baked_transparent_bricks, baked_brick_weights, prune_baked, BakedFieldTrainer.prune;
 include/nerfb200.h "baked fields: pruning"), with total-variation and sparsity regularisers over the lattice
 (baked_regularizer, BakedFieldTrainer's tv_sigma / tv_sh / sparsity; include/nerfb200.h "baked fields: regularisers").  This file validates arguments, sizes buffers and moves
-pointers; the bake reads the active brick count back once to size its values.  A field kept, saved, rendered or pruned
+pointers; the bake reads the active brick count back once to size its values.  A field can also start without a network
+(``BakedField.full``) and be trained coarse to fine: train, prune, then subdivide to twice the resolution holding the
+same trilinear function (subdivide_baked, BakedFieldTrainer.subdivide; include/nerfb200.h "baked fields:
+subdivision").  A field kept, saved, rendered or pruned
 may store its values in fp16 (``bake(dtype=torch.float16)``, ``BakedField.half``; include/nerfb200.h "baked fields: half
 precision"); fine-tuning and the regularisers take fp32 fields only (``BakedField.float``)."""
 from __future__ import annotations
+
+import math
 
 import torch
 
@@ -32,6 +37,25 @@ class BakedField:
         self.bricks = bricks
         self.values = values
         self.use_viewdirs = bool(use_viewdirs)
+
+    @classmethod
+    def full(cls, bounds, resolution, *, sigma_raw=0.1, use_viewdirs=True, device="cuda") -> "BakedField":
+        """A field on every brick of the lattice box ``bounds`` / ``resolution`` (checked as ``bake`` checks them),
+        ``brick_map`` and ``bricks`` the identity, ``sigma_raw`` at every lattice point and every SH coefficient 0 (grey:
+        sigmoid(0) = 0.5).  fp32.  The networkless starting point of a coarse-to-fine fit, as ``OccupancyGrid.full`` is
+        of a grid.  The renderer's density is relu(sigma_raw), whose gradient is 0 at sigma_raw <= 0, so a start that can
+        learn density is positive.  A non-finite ``sigma_raw`` raises ValueError."""
+        from .mesh import _box
+
+        lo, hi, res = _box(bounds, resolution, dense=False)
+        sigma = float(sigma_raw)
+        if not math.isfinite(sigma):
+            raise ValueError(f"BakedField.full: sigma_raw must be finite, got {sigma_raw!r}")
+        n = math.prod(-(-r // 8) for r in res)
+        ids = torch.arange(n, dtype=torch.int32, device=device)
+        values = torch.zeros(n, 729, 32, dtype=torch.float32, device=device)
+        values[..., 0] = sigma
+        return cls((lo, hi), res, ids, ids.clone(), values, use_viewdirs)
 
     @property
     def n_active(self) -> int:
@@ -400,6 +424,27 @@ class BakedFieldTrainer:
         self.d_values, self.d_tied = torch.zeros_like(f.values), torch.zeros_like(f.values)
         ops.baked_lattice_count(self._box, f.brick_map, f.bricks, self._count)
 
+    def subdivide(self) -> None:
+        """Replaces the trainer's field in place by ``subdivide_baked`` of it: the ``BakedField`` passed to the
+        constructor then holds twice the ``resolution`` and the child ``brick_map``, ``bricks`` and ``values``, and the
+        Adam moments ``m`` and ``v`` go through the same kernel.  The gradient buffers are freed first and reallocated at
+        the new size; while the child's values, m and v are formed the parent's are still held, so the peak is those
+        six arrays, below the trainer's five buffers at the new size.  ``step_dev``, the seed, the rates and the schedule carry on, and the
+        regularisers' P is counted again.  The refusals are ``subdivide_baked``'s, checked before anything changes.
+        Reads the child brick count back once."""
+        f = self.field
+        res = _check_subdivide(f, "BakedFieldTrainer.subdivide")
+        self.d_values = self.d_tied = None
+        with torch.no_grad():
+            brick_map, bricks = _child_bricks(f, res)
+            box = f.box()
+            values, m, v = (_subdivided(box, f.brick_map, x, bricks) for x in (f.values, self.m, self.v))
+        f.resolution, f.brick_map, f.bricks, f.values = res, brick_map, bricks, values
+        self.m, self.v = m, v
+        self._box = f.box()
+        self.d_values, self.d_tied = torch.zeros_like(f.values), torch.zeros_like(f.values)
+        ops.baked_lattice_count(self._box, f.brick_map, f.bricks, self._count)
+
 
 # ------------------------------------------------------------------------------------------------------------------------
 # pruning (include/nerfb200.h "baked fields: pruning")
@@ -502,3 +547,63 @@ def baked_brick_weights(field: BakedField, poses, height, width, focal_length, o
         rays = _pose_rays(field, height, width, focal_length, p, options)
         ops.baked_max_weights(box, field.brick_map, values, field.use_viewdirs, rays, out)
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# subdivision (include/nerfb200.h "baked fields: subdivision")
+# ------------------------------------------------------------------------------------------------------------------------
+def _check_subdivide(field, what):
+    """The child resolution of a CUDA fp32 ``field`` whose resolution is at most 2048 per axis (ValueError
+    otherwise)."""
+    if not isinstance(field, BakedField):
+        raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
+    if field.values.dtype == torch.float16:
+        raise ValueError(f"{what}: an fp16 field has no subdivision; subdivide field.float() and convert it back "
+                         f"with .half()")
+    if not all(r <= 2048 for r in field.resolution):
+        raise ValueError(f"{what}: resolution {field.resolution} is past 2048 on an axis (the child would pass 4096)")
+    if not (field.values.is_cuda and field.values.dtype == torch.float32):
+        raise ValueError(f"{what}: field.values must be an fp32 CUDA tensor (there is no CPU path)")
+    return tuple(2 * r for r in field.resolution)
+
+
+def _child_bricks(field, res):
+    """(brick_map, bricks) int32 of the child box at ``res`` (twice the field's resolution): the children 2 pb + delta
+    of every active parent brick pb that exist in the child box, ascending, and their rank.  Plain torch on the field's
+    device; reads the child count back once."""
+    dev = field.bricks.device
+    nbp = [-(-r // 8) for r in field.resolution]
+    nbc = [-(-r // 8) for r in res]
+    br = field.bricks.long()
+    b = torch.stack([br % nbp[0], br // nbp[0] % nbp[1], br // (nbp[0] * nbp[1])], -1)  # [n, 3]
+    k = torch.arange(8, device=dev)
+    c = 2 * b[:, None] + torch.stack([k & 1, k >> 1 & 1, k >> 2], -1)[None]  # [n, 8, 3]
+    exists = (c < torch.tensor(nbc, device=dev)).all(-1)
+    bricks = torch.sort(((c[..., 2] * nbc[1] + c[..., 1]) * nbc[0] + c[..., 0])[exists]).values.int()
+    brick_map = torch.full((nbc[0] * nbc[1] * nbc[2],), -1, dtype=torch.int32, device=dev)
+    brick_map[bricks.long()] = torch.arange(bricks.numel(), dtype=torch.int32, device=dev)
+    return brick_map, bricks
+
+
+def _subdivided(box, brick_map, values, child_bricks):
+    """fp32 (n_child, 729, 32): ``values`` (of the parent ``box`` / ``brick_map``) subdivided onto ``child_bricks``."""
+    out = torch.empty(child_bricks.numel(), 729, 32, dtype=torch.float32, device=values.device)
+    if child_bricks.numel():
+        ops.baked_subdivide(box, brick_map, values.detach(), child_bricks, out)
+    return out
+
+
+def subdivide_baked(field: BakedField) -> BakedField:
+    """A new ``BakedField`` at twice ``field``'s resolution over the same bounds, holding the same trilinear function
+    (include/nerfb200.h "baked fields: subdivision"): its active bricks are the children of ``field``'s, in ascending
+    order, and every child lattice point is the parent's value there (a copy where it coincides with a parent point,
+    the mean of 2, 4 or 8 parent points otherwise, each op rounded in fp32).  It renders the parent's continuous field
+    with samples half as far apart.  ``field`` is not touched; the child needs up to 8 times the parent's values.  Prune
+    first (``prune_baked``) to subdivide only the bricks worth keeping.  A field without active bricks gives an empty
+    child without a launch.  ValueError for an fp16 field (subdivide ``field.float()``), a CPU field, or a resolution
+    past 2048 on an axis.  Reads the child brick count back once."""
+    res = _check_subdivide(field, "subdivide_baked")
+    with torch.no_grad():
+        brick_map, bricks = _child_bricks(field, res)
+        values = _subdivided(field.box(), field.brick_map, field.values, bricks)
+    return BakedField(field.bounds, res, brick_map, bricks, values, field.use_viewdirs)

@@ -908,3 +908,118 @@ int32_t nerfb200_baked_regularizer(const nerfb200_grid_t* box, const int32_t* br
 }
 
 }  // extern "C"
+
+// ---- subdivision (include/nerfb200.h "baked fields: subdivision") ----
+namespace nerfb200 {
+namespace {
+
+constexpr int kSubThreads = 256;
+constexpr int kSubStage = 5;  // parent points per axis a child brick reads: 4 delta .. 4 delta + 4 of its parent brick
+constexpr int kSubStaged = kSubStage * kSubStage * kSubStage;
+
+// One CTA per child slot.  The 5 x 5 x 5 parent points the child brick reads (channels 0 .. 27, seven float4 each) are
+// staged in shared memory from the parent brick's slot; the child slot's 729 x 8 float4 are then written point-major,
+// one thread per float4, each channel group summed over the point's 2^m parent points in corner order.
+__global__ void __launch_bounds__(kSubThreads)
+baked_subdivide_kernel(const BakedBox C, const int* __restrict__ brick_map, int nb0, int nb1, int64_t n_active,
+                       const float4* __restrict__ values, const int* __restrict__ child_bricks,
+                       float4* __restrict__ child_values) {
+  __shared__ float4 stage[kSubStaged][kBakedVals / 4];
+  const int64_t slot = blockIdx.x;
+  const int cb = child_bricks[slot];
+  const int bc[3] = {cb % C.nb[0], (cb / C.nb[0]) % C.nb[1], cb / (C.nb[0] * C.nb[1])};
+  const int64_t ps = brick_map[((int64_t)(bc[2] >> 1) * nb1 + (bc[1] >> 1)) * nb0 + (bc[0] >> 1)];
+  const bool have = ps >= 0 && ps < n_active;  // a CTA-uniform branch
+  float4* out = child_values + slot * (kBakePts * (kBakeCh / 4));
+  if (!have) {
+    for (int e = threadIdx.x; e < kBakePts * (kBakeCh / 4); e += kSubThreads) out[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+    return;
+  }
+  const float4* src = values + ps * (kBakePts * (kBakeCh / 4));
+  for (int e = threadIdx.x; e < kSubStaged * (kBakedVals / 4); e += kSubThreads) {
+    const int sp = e / (kBakedVals / 4), c4 = e - sp * (kBakedVals / 4);
+    const int sx = sp % kSubStage, sy = (sp / kSubStage) % kSubStage, sz = sp / (kSubStage * kSubStage);
+    const int lx = 4 * (bc[0] & 1) + sx, ly = 4 * (bc[1] & 1) + sy, lz = 4 * (bc[2] & 1) + sz;
+    stage[sp][c4] = __ldg(src + ((lz * 9 + ly) * 9 + lx) * (kBakeCh / 4) + c4);
+  }
+  __syncthreads();
+  for (int e = threadIdx.x; e < kBakePts * (kBakeCh / 4); e += kSubThreads) {
+    const int p = e >> 3, c4 = e & 7;
+    if (c4 >= kBakedVals / 4) {  // channels 28 .. 31
+      out[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+      continue;
+    }
+    const int l[3] = {p % 9, (p / 9) % 9, p / 81};
+    int s0[3], odd[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const int q = min(kBakeBrick * bc[c] + l[c], C.g.res[c]);  // the child lattice index
+      s0[c] = (q >> 1) - 4 * bc[c];
+      odd[c] = q & 1;
+    }
+    const int m = odd[0] + odd[1] + odd[2];
+    if (m == 0) {  // a parent point: its bits
+      out[e] = stage[(s0[2] * kSubStage + s0[1]) * kSubStage + s0[0]][c4];
+      continue;
+    }
+    const float w = m == 1 ? 0.5f : (m == 2 ? 0.25f : 0.125f);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool first = true;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
+      if ((dx && !odd[0]) || (dy && !odd[1]) || (dz && !odd[2])) continue;  // absent along an even axis
+      const float4 v = stage[((s0[2] + dz) * kSubStage + s0[1] + dy) * kSubStage + s0[0] + dx][c4];
+      const float4 t = make_float4(__fmul_rn(w, v.x), __fmul_rn(w, v.y), __fmul_rn(w, v.z), __fmul_rn(w, v.w));
+      if (first) {
+        acc = t;
+        first = false;
+      } else {
+        acc = make_float4(__fadd_rn(acc.x, t.x), __fadd_rn(acc.y, t.y), __fadd_rn(acc.z, t.z), __fadd_rn(acc.w, t.w));
+      }
+    }
+    out[e] = acc;
+  }
+}
+
+}  // namespace
+}  // namespace nerfb200
+
+extern "C" {
+
+int32_t nerfb200_baked_subdivide(const nerfb200_grid_t* box, const int32_t* brick_map, int64_t n_active,
+                                 const float* values, const int32_t* child_bricks, int64_t n_child,
+                                 float* child_values, void* stream) {
+  if (int rc = check_grid(box, "baked_subdivide")) return rc;
+  nerfb200_grid_t child = *box;
+  for (int c = 0; c < 3; ++c) {
+    if (box->res[c] > NERFB200_GRID_MAX_RES / 2) {
+      set_error("baked_subdivide: the child resolution 2 x %d on axis %d is past %d", box->res[c], c,
+                NERFB200_GRID_MAX_RES);
+      return NERFB200_ERR_INVALID;
+    }
+    child.res[c] = 2 * box->res[c];
+  }
+  const int64_t n_bricks = nerfb200_mesh_sparse_brick_count(box);
+  const int64_t n_child_bricks = nerfb200_mesh_sparse_brick_count(&child);
+  if (!brick_map || !values || !child_bricks || !child_values || n_active < 0 || n_active > n_bricks ||
+      n_child < 0 || n_child > n_child_bricks) {
+    set_error("baked_subdivide: null pointer, n_active %lld outside 0 .. %lld or n_child %lld outside 0 .. %lld",
+              (long long)n_active, (long long)n_bricks, (long long)n_child, (long long)n_child_bricks);
+    return NERFB200_ERR_INVALID;
+  }
+  const int64_t per = (int64_t)kBakePts * kBakeCh;
+  if (child_values < values + n_active * per && values < child_values + n_child * per) {
+    set_error("baked_subdivide: child_values overlaps values");
+    return NERFB200_ERR_INVALID;
+  }
+  if (n_child == 0) return NERFB200_OK;
+  const BakedBox B = baked_box(box), Cb = baked_box(&child);
+  baked_subdivide_kernel<<<(unsigned)n_child, kSubThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      Cb, brick_map, B.nb[0], B.nb[1], n_active, reinterpret_cast<const float4*>(values), child_bricks,
+      reinterpret_cast<float4*>(child_values));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "baked_subdivide launch");
+}
+
+}  // extern "C"

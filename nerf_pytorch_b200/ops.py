@@ -1081,3 +1081,13 @@ def baked_adam_step_dev(values, g, m, v, step_dev, lr_sigma, lr_sh, lr_decay=Non
                                                         _ptr(step_dev), float(lr_sigma), float(lr_sh), decay, factor,
                                                         float(beta1), float(beta2), float(eps), _stream()),
                "baked_adam_step_dev")
+
+
+def baked_subdivide(box: Grid, brick_map, values, child_bricks, child_values):
+    """Writes into ``child_values`` (n_child, 729, 32) fp32 the field on the box at twice ``box``'s resolution whose
+    active bricks are ``child_bricks`` int32[n_child] (the children of the parent's active bricks, ascending), from the
+    parent's fp32 ``values`` (include/nerfb200.h "baked fields: subdivision")."""
+    _lib.check(_lib.load().nerfb200_baked_subdivide(C.byref(box), _ptr(brick_map), values.shape[0], _ptr(values),
+                                                    _ptr(child_bricks), child_bricks.shape[0], _ptr(child_values),
+                                                    _stream()), "baked_subdivide")
+    return child_values
