@@ -832,6 +832,64 @@ int32_t nerfb200_baked_subdivide(const nerfb200_grid_t* box, const int32_t* bric
                                  const float* values, const int32_t* child_bricks, int64_t n_child,
                                  float* child_values, void* stream);
 
+/* ---- baked fields: meshes -------------------------------------------------------------------------------------------
+ * The level set of a baked field's own density as a triangle mesh, with the normals and colours the field itself gives
+ * (as Plenoxels / PlenOctrees export meshes of their fitted grids), without a network.  All fp32 with round-to-nearest,
+ * each op rounded, no contraction unless fmaf is named.
+ *   - Values.  Marching cubes runs over sigma_raw itself (channel 0, widened exactly to fp32 from an fp16 field), not
+ *     over relu(sigma_raw): mesh_sparse_count / mesh_sparse_emit with halo = 0 on the field's box, brick_map and bricks,
+ *     the field's layout being that of "sparse meshes" with halo = 0.  Along a lattice edge the renderer's density is
+ *     relu of a linear function, so for level >= 0 its crossing is the crossing of sigma_raw itself; relu'd values would
+ *     move the vertex wherever an endpoint is negative (endpoints -100 and 100 at level 50: t = 0.75 on sigma_raw, 0.5 on
+ *     relu values, a quarter of a cube off the renderer's surface).  For level >= 0 the inside / outside classification
+ *     is relu's, so the faces and the vertex numbering are those of the sparse mesh of relu(sigma_raw) (extract_mesh of
+ *     the baked network over the same grid); vertices differ only on edges with a negative endpoint.  A negative level
+ *     is refused by the library's Python interface: the density is never negative.
+ *   - Direction and normal (baked_mesh_dirs).  Vertex i's lattice edge (q, a) is edge_keys[i] = q * 3 + a (mesh_sparse_
+ *     emit's keys); t = (level - v0) / (v1 - v0) on the endpoints' sigma_raw.  The gradient at each endpoint is
+ *     mesh_emit's (central differences, one-sided at the lattice's faces) over sigma_raw read at each point's canonical
+ *     copy ("baked fields: regularisers"); a lattice point no active brick holds reads 0, the renderer's miss.  dir is
+ *     mesh_emit's view-direction rule on those gradients: -n, or (0, 0, 1) where the interpolated gradient vanishes or is
+ *     not finite; normal = -dir, or (0, 0, 0) where the rule fell back.  On a field whose every brick is active, dir is
+ *     bit for bit mesh_sparse_emit's view_dirs with halo = 1 over the same sigma_raw.
+ *   - Colour (baked_mesh_colors).  Channels 0 .. 27 at the vertex from the edge's two endpoints' canonical copies by the
+ *     renderer's fmaf chain restricted to those two corners: v = 0, v = fmaf(1 - t, v0, v), v = fmaf(t, v1, v); then the
+ *     renderer's colour with Y_j(dirs[i]) (Y_0 alone without view directions): the colour the renderer gives that point
+ *     seen head-on from outside, as extract_mesh(colors=True) gives for a network.
+ *   - NDC.  A field baked from a forward-facing scene lives in NDC: the NDC vertices, faces and dirs go through
+ *     ndc_mesh_to_world; the colours are formed with the WORLD direction (the baked SH were fitted to world view
+ *     directions); the normals are -(world dir), or 0 where the NDC rule fell back.
+ *   - Copies.  Every lookup reads canonical copies, so the attributes do not depend on which copy a thread holds.  The
+ *     vertex positions come from the copy the marching brick holds, and agree with t whenever the field's copies are
+ *     bit-equal, which holds for every field the library produces (bake, tie, subdivide, prune, half).
+ *   - Transparent prune.  Dropping transparent bricks ("baked fields: pruning") leaves the faces and the vertices (ids
+ *     included) the same bits at level >= 0: such a brick holds no endpoint of a crossing edge (sigma_raw <= 0 <= level at
+ *     all its points), so it owns no vertex.  Normals and colours are the same bits at every vertex whose gradient
+ *     stencil keeps a copy of every point; a stencil point stored only in a dropped brick then reads 0 instead of its
+ *     sigma_raw <= 0.  This is the one place where pruning a transparent brick changes what is read, while renders stay
+ *     the same bits.
+ *   - Robustness.  A key off the lattice's edges, or an endpoint no active brick holds, reads nothing out of bounds and
+ *     writes NaN for that vertex.  Keys are meant to come from mesh_sparse_emit over the same field and level; the device
+ *     does not check that.
+ * baked_mesh_dirs: dirs[n_vertices][3], normals[n_vertices][3] (may be NULL).
+ * baked_mesh_colors: colors[n_vertices][3]; dirs[n_vertices][3] is read with view directions (may be NULL without).
+ * _f16: values binary16 ("baked fields: half precision"), each value widened exactly as it is read.
+ * One thread per vertex, offsets in 64 bits, no atomics, no host synchronisation; n_vertices 0 launches nothing.
+ * Refused before any launch: an invalid box, a null pointer where one is needed, n_vertices < 0, a non-finite level,
+ * an fp16 values pointer that is not 16-B aligned. */
+int32_t nerfb200_baked_mesh_dirs(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                 float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
+                                 float* normals, void* stream);
+int32_t nerfb200_baked_mesh_dirs_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                     float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
+                                     float* normals, void* stream);
+int32_t nerfb200_baked_mesh_colors(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                   int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                                   int64_t n_vertices, float* colors, void* stream);
+int32_t nerfb200_baked_mesh_colors_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                       int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                                       int64_t n_vertices, float* colors, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

@@ -14,7 +14,8 @@ pointers; the bake reads the active brick count back once to size its values.  A
 same trilinear function (subdivide_baked, BakedFieldTrainer.subdivide; include/nerfb200.h "baked fields:
 subdivision").  A field kept, saved, rendered or pruned
 may store its values in fp16 (``bake(dtype=torch.float16)``, ``BakedField.half``; include/nerfb200.h "baked fields: half
-precision"); fine-tuning and the regularisers take fp32 fields only (``BakedField.float``)."""
+precision"); fine-tuning and the regularisers take fp32 fields only (``BakedField.float``).  Any field, fp32 or fp16, can
+be meshed without a network (extract_baked_mesh; include/nerfb200.h "baked fields: meshes")."""
 from __future__ import annotations
 
 import math
@@ -607,3 +608,76 @@ def subdivide_baked(field: BakedField) -> BakedField:
         brick_map, bricks = _child_bricks(field, res)
         values = _subdivided(field.box(), field.brick_map, field.values, bricks)
     return BakedField(field.bounds, res, brick_map, bricks, values, field.use_viewdirs)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# meshes (include/nerfb200.h "baked fields: meshes")
+# ------------------------------------------------------------------------------------------------------------------------
+def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool = False, normals: bool = False,
+                       ndc=None):
+    """The level set sigma = ``level`` of a baked field's own density as an ``nb.Mesh``, by sparse marching cubes over
+    the field's active bricks on the GPU (include/nerfb200.h "baked fields: meshes").  No network is needed, so this
+    meshes a fine-tuned, pruned, subdivided or from-scratch field as it renders.
+
+    Marching cubes runs over sigma_raw (channel 0, an fp16 field's widened exactly): for ``level`` >= 0 the crossing of
+    the renderer's density relu(sigma_raw) along a lattice edge is the crossing of sigma_raw, so the faces and vertex
+    numbering are those of ``extract_mesh`` on the baked network over the same grid, and the vertices lie on the
+    renderer's surface.  ``normals=True`` sets ``Mesh.normals``: the outward unit normal from central differences of
+    sigma_raw (a lattice point no active brick holds reads 0), (0, 0, 0) where the gradient vanishes.  ``colors=True``
+    gives each vertex the renderer's colour of that point seen head-on from outside.
+
+    ``ndc=(H, W, focal)`` is for a field baked from a forward-facing scene, which lives in NDC: the mesh is extracted in
+    NDC and returned in world space, as ``extract_mesh(ndc=)`` does; the colours are seen along world directions.  A
+    field that is not a ``BakedField``, a non-finite or negative ``level``, a malformed ``ndc`` or one whose box reaches
+    z = 1 raises ValueError, a CPU field NotImplementedError, before any launch.  A field without active bricks or a
+    level with no crossing gives an empty mesh.  Reads the mesh's two totals back once."""
+    from . import density
+    from .mesh import Mesh, _level
+
+    if not isinstance(field, BakedField):
+        raise ValueError(f"extract_baked_mesh: field must be an nb.BakedField, got {type(field).__name__}")
+    level = _level(level)
+    if level < 0.0:
+        raise ValueError(f"extract_baked_mesh: level must be >= 0 (the density relu(sigma_raw) is never negative), got "
+                         f"{level}")
+    cam = density.ndc_camera(ndc) if ndc is not None else None
+    if cam is not None and not field.bounds[1][2] < 1.0:
+        raise ValueError(f"extract_baked_mesh: with ndc=, the field's NDC box needs hi_z < 1 (z = 1 is the far plane at "
+                         f"infinity), got {field.bounds!r}")
+    values = field.values
+    if not (isinstance(values, torch.Tensor) and values.is_cuda):
+        raise NotImplementedError("nerfb200: the baked field must be on a CUDA device (there is no CPU path)")
+    if values.dtype not in (torch.float32, torch.float16):
+        raise ValueError(f"extract_baked_mesh: field.values must be fp32 or fp16, got {values.dtype}")
+    dev = values.device
+
+    def empty():
+        z = torch.zeros(0, 3, dtype=torch.float32, device=dev)
+        return Mesh(z, torch.zeros(0, 3, dtype=torch.int32, device=dev), z.clone() if colors else None,
+                    z.clone() if normals else None)
+
+    if field.n_active == 0:
+        return empty()
+    box = field.box()
+    values = values.detach()
+    with torch.no_grad():
+        sigma = values[..., 0].float().contiguous()  # (n_active, 729): the halo-0 sparse layout
+        totals, ws = ops.mesh_sparse_count(box, field.brick_map, field.bricks, field.n_active, sigma, False, level)
+        n_v, n_f = (int(t) for t in totals.tolist())  # the one host sync: the outputs' sizes
+        if n_v == 0:
+            return empty()
+        want_dirs = normals or (colors and field.use_viewdirs)
+        verts, faces, _, keys = ops.mesh_sparse_emit(box, field.brick_map, field.bricks, field.n_active, sigma, False,
+                                                     level, ws, n_v, n_f, want_keys=colors or normals)
+        dirs = nrm = None
+        if want_dirs:
+            dirs, nrm = ops.baked_mesh_dirs(box, field.brick_map, values, level, keys, want_normals=normals)
+        if cam is not None:
+            verts, faces, dirs = ops.ndc_mesh_to_world(cam, verts, faces, dirs)
+            if normals:  # -(world dir), 0 where the NDC direction fell back (its normal is 0 there)
+                nrm = torch.where((nrm == 0).all(-1, keepdim=True), torch.zeros_like(dirs), -dirs)
+        rgb = None
+        if colors:
+            rgb = ops.baked_mesh_colors(box, field.brick_map, values, field.use_viewdirs, level, keys,
+                                        dirs if field.use_viewdirs else None)
+    return Mesh(verts, faces, rgb, nrm)

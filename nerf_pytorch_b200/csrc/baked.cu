@@ -22,6 +22,7 @@
 #include <cuda_fp16.h>
 
 #include "composite.cuh"
+#include "mesh_rules.cuh"
 
 namespace nerfb200 {
 
@@ -1020,6 +1021,231 @@ int32_t nerfb200_baked_subdivide(const nerfb200_grid_t* box, const int32_t* bric
       reinterpret_cast<float4*>(child_values));
   count_launch();
   return check_cuda(cudaGetLastError(), "baked_subdivide launch");
+}
+
+}  // extern "C"
+
+// ---- meshes (include/nerfb200.h "baked fields: meshes") ----
+namespace nerfb200 {
+namespace {
+
+constexpr int kMeshAttrThreads = 256;
+
+// the lattice edge (q, a) of an edge key q * 3 + a, or false for a key outside the lattice's edges
+__device__ __forceinline__ bool edge_of_key(const Lattice& L, int64_t key, int q[3], int& a) {
+  if (key < 0 || key >= 3 * L.total) return false;
+  const int64_t p = key / 3;
+  a = (int)(key - 3 * p);
+  q[0] = (int)(p % L.n[0]);
+  q[1] = (int)((p / L.n[0]) % L.n[1]);
+  q[2] = (int)(p / L.n01);
+  return (a == 0 ? q[0] : (a == 1 ? q[1] : q[2])) < (a == 0 ? L.res[0] : (a == 1 ? L.res[1] : L.res[2]));
+}
+
+// sigma_raw at lattice point q, read at its canonical copy; 0 (the renderer's miss) when no active brick holds q
+template <typename V>
+__device__ __forceinline__ float lattice_sigma(const BakedBox& B, const int* __restrict__ brick_map,
+                                               const V* __restrict__ values, const int q[3]) {
+  const int64_t cp = canonical_copy(B, brick_map, q);
+  return cp < 0 ? 0.f : baked_ld(values + cp);
+}
+
+// mesh_emit's gradient at lattice point q over sigma_raw at canonical copies (central differences, one-sided at the
+// lattice's faces)
+template <typename V>
+__device__ __forceinline__ void lattice_grad(const BakedBox& B, const Lattice& L, const int* __restrict__ brick_map,
+                                             const V* __restrict__ values, const int q[3], float g[3]) {
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int lo = q[c] > 0 ? q[c] - 1 : 0, hi = q[c] < L.res[c] ? q[c] + 1 : L.res[c];
+    int ph[3] = {q[0], q[1], q[2]}, pl[3] = {q[0], q[1], q[2]};
+    ph[c] = hi;
+    pl[c] = lo;
+    g[c] = grad_component(L, c, lattice_sigma(B, brick_map, values, ph), lattice_sigma(B, brick_map, values, pl), hi,
+                          lo);
+  }
+}
+
+// channels 0 .. 27 of one stored point, widened exactly to fp32
+__device__ __forceinline__ void baked_point(const float* __restrict__ p, float a[kBakedVals]) {
+  const float4* p4 = reinterpret_cast<const float4*>(p);
+#pragma unroll
+  for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+    const float4 u = __ldg(p4 + c4);
+    a[4 * c4] = u.x;
+    a[4 * c4 + 1] = u.y;
+    a[4 * c4 + 2] = u.z;
+    a[4 * c4 + 3] = u.w;
+  }
+}
+__device__ __forceinline__ void baked_point(const __half* __restrict__ p, float a[kBakedVals]) {
+  const uint4* p4 = reinterpret_cast<const uint4*>(p);
+#pragma unroll
+  for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {
+    const uint4 u = __ldg(p4 + c8);
+    widen4(u.x, u.y, a + 8 * c8);
+    widen4(u.z, u.w, a + 8 * c8 + 4);
+  }
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p4 + kBakedVals / 8));
+  widen4(u.x, u.y, a + 24);
+}
+
+// One thread per vertex: t on the edge's sigma_raw, the endpoints' gradients, the view direction and (normals may be
+// NULL) the outward normal, -dir or 0 where the direction fell back.  NaN for a key off the lattice or an endpoint no
+// active brick holds.
+template <typename V>
+__global__ void __launch_bounds__(kMeshAttrThreads)
+baked_mesh_dirs_kernel(const BakedBox B, const Lattice L, const int* __restrict__ brick_map,
+                       const V* __restrict__ values, float level, const int64_t* __restrict__ keys, int64_t n,
+                       float* __restrict__ dirs, float* __restrict__ normals) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float d[3] = {NAN, NAN, NAN}, nrm[3] = {NAN, NAN, NAN};
+  int q[3], a;
+  if (edge_of_key(L, keys[i], q, a)) {
+    const int q1[3] = {q[0] + (a == 0), q[1] + (a == 1), q[2] + (a == 2)};  // a compared, not indexed: registers
+    const int64_t c0 = canonical_copy(B, brick_map, q), c1 = canonical_copy(B, brick_map, q1);
+    if (c0 >= 0 && c1 >= 0) {
+      const float t = edge_t(level, baked_ld(values + c0), baked_ld(values + c1));
+      float g0[3], g1[3];
+      lattice_grad(B, L, brick_map, values, q, g0);
+      lattice_grad(B, L, brick_map, values, q1, g1);
+      const bool ok = edge_dir(g0, g1, t, d);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) nrm[c] = ok ? -d[c] : 0.f;
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) dirs[3 * i + c] = d[c];
+  if (normals) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) normals[3 * i + c] = nrm[c];
+  }
+}
+
+// One thread per vertex: channels 0 .. 27 at the vertex by the renderer's fmaf chain over the edge's two endpoints
+// (weights 1 - t and t), then the renderer's colour seen along dirs[i] (Y_0 alone without view directions).  NaN where
+// baked_mesh_dirs_kernel writes NaN.
+template <typename V>
+__global__ void __launch_bounds__(kMeshAttrThreads)
+baked_mesh_colors_kernel(const BakedBox B, const Lattice L, const int* __restrict__ brick_map,
+                         const V* __restrict__ values, int use_viewdirs, float level,
+                         const int64_t* __restrict__ keys, const float* __restrict__ dirs, int64_t n,
+                         float* __restrict__ colors) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float rgb[3] = {NAN, NAN, NAN};
+  int q[3], a;
+  if (edge_of_key(L, keys[i], q, a)) {
+    const int q1[3] = {q[0] + (a == 0), q[1] + (a == 1), q[2] + (a == 2)};  // a compared, not indexed: registers
+    const int64_t c0 = canonical_copy(B, brick_map, q), c1 = canonical_copy(B, brick_map, q1);
+    if (c0 >= 0 && c1 >= 0) {
+      float v0[kBakedVals], v1[kBakedVals], v[kBakedVals];
+      baked_point(values + c0, v0);
+      baked_point(values + c1, v1);
+      const float t = edge_t(level, v0[0], v1[0]), u = __fsub_rn(1.0f, t);
+#pragma unroll
+      for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(t, v1[ch], fmaf(u, v0[ch], 0.f));
+      float Y[kBakeSh];
+      if (use_viewdirs) sh_basis(dirs[3 * i], dirs[3 * i + 1], dirs[3 * i + 2], Y);
+      else Y[0] = 0.28209479177387814f;
+      baked_colour(use_viewdirs, Y, v, rgb);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) colors[3 * i + c] = rgb[c];
+}
+
+int check_baked_mesh(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
+                     float level, const int64_t* edge_keys, int64_t n_vertices, const void* out) {
+  if (int rc = check_grid(box, what)) return rc;
+  if (!brick_map || !values || !edge_keys || !out || n_vertices < 0) {
+    set_error("%s: null pointer or n_vertices %lld < 0", what, (long long)n_vertices);
+    return NERFB200_ERR_INVALID;
+  }
+  if (!std::isfinite(level)) {
+    set_error("%s: level must be finite, got %g", what, (double)level);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
+}
+
+template <typename V>
+int launch_baked_mesh_dirs(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                           float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs, float* normals,
+                           void* stream) {
+  if (n_vertices == 0) return NERFB200_OK;
+  baked_mesh_dirs_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads, 0,
+                              static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
+                                                                   values, level, edge_keys, n_vertices, dirs,
+                                                                   normals);
+  count_launch();
+  return check_cuda(cudaGetLastError(), what);
+}
+
+template <typename V>
+int launch_baked_mesh_colors(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                             int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                             int64_t n_vertices, float* colors, void* stream) {
+  if (n_vertices == 0) return NERFB200_OK;
+  baked_mesh_colors_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads,
+                                0, static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
+                                                                        values, use_viewdirs ? 1 : 0, level, edge_keys,
+                                                                        dirs, n_vertices, colors);
+  count_launch();
+  return check_cuda(cudaGetLastError(), what);
+}
+
+}  // namespace
+}  // namespace nerfb200
+
+extern "C" {
+
+int32_t nerfb200_baked_mesh_dirs(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                 float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
+                                 float* normals, void* stream) {
+  if (int rc = check_baked_mesh("baked_mesh_dirs", box, brick_map, values, level, edge_keys, n_vertices, dirs))
+    return rc;
+  return launch_baked_mesh_dirs("baked_mesh_dirs launch", box, brick_map, values, level, edge_keys, n_vertices, dirs,
+                                normals, stream);
+}
+
+int32_t nerfb200_baked_mesh_dirs_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                     float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
+                                     float* normals, void* stream) {
+  const char* what = "baked_mesh_dirs_f16";
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, dirs)) return rc;
+  if (int rc = check_f16_values(what, values)) return rc;
+  return launch_baked_mesh_dirs("baked_mesh_dirs_f16 launch", box, brick_map, reinterpret_cast<const __half*>(values),
+                                level, edge_keys, n_vertices, dirs, normals, stream);
+}
+
+int32_t nerfb200_baked_mesh_colors(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                   int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                                   int64_t n_vertices, float* colors, void* stream) {
+  const char* what = "baked_mesh_colors";
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
+  if (use_viewdirs && !dirs) {
+    set_error("%s: view directions need dirs", what);
+    return NERFB200_ERR_INVALID;
+  }
+  return launch_baked_mesh_colors("baked_mesh_colors launch", box, brick_map, values, use_viewdirs, level, edge_keys,
+                                  dirs, n_vertices, colors, stream);
+}
+
+int32_t nerfb200_baked_mesh_colors_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                       int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                                       int64_t n_vertices, float* colors, void* stream) {
+  const char* what = "baked_mesh_colors_f16";
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
+  if (use_viewdirs && !dirs) {
+    set_error("%s: view directions need dirs", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (int rc = check_f16_values(what, values)) return rc;
+  return launch_baked_mesh_colors("baked_mesh_colors_f16 launch", box, brick_map,
+                                  reinterpret_cast<const __half*>(values), use_viewdirs, level, edge_keys, dirs,
+                                  n_vertices, colors, stream);
 }
 
 }  // extern "C"

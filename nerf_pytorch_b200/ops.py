@@ -1091,3 +1091,29 @@ def baked_subdivide(box: Grid, brick_map, values, child_bricks, child_values):
                                                     _ptr(child_bricks), child_bricks.shape[0], _ptr(child_values),
                                                     _stream()), "baked_subdivide")
     return child_values
+
+
+def baked_mesh_dirs(box: Grid, brick_map, values, level: float, edge_keys, want_normals: bool = False):
+    """(dirs (V, 3), normals (V, 3) or None) of the vertices whose lattice edges are ``edge_keys`` int64 (V,) on a baked
+    field's fp32 or fp16 ``values`` (include/nerfb200.h "baked fields: meshes"): the view direction -n and the outward
+    normal n (0 where the direction fell back)."""
+    sfx, pv = _baked_values(values, "baked_mesh_dirs")
+    n = edge_keys.shape[0]
+    dirs = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device)
+    normals = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device) if want_normals else None
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_mesh_dirs" + sfx)(
+        C.byref(box), _ptr(brick_map), pv, float(level), _ptr(edge_keys), n, _ptr(dirs), _ptr(normals), _stream()),
+        "baked_mesh_dirs" + sfx)
+    return dirs, normals
+
+
+def baked_mesh_colors(box: Grid, brick_map, values, use_viewdirs: bool, level: float, edge_keys, dirs=None):
+    """colors (V, 3) of the vertices whose lattice edges are ``edge_keys`` int64 (V,) on a baked field's fp32 or fp16
+    ``values``, seen along ``dirs`` (V, 3) with view directions (include/nerfb200.h "baked fields: meshes")."""
+    sfx, pv = _baked_values(values, "baked_mesh_colors")
+    n = edge_keys.shape[0]
+    colors = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device)
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_mesh_colors" + sfx)(
+        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), float(level), _ptr(edge_keys), _ptr(dirs), n,
+        _ptr(colors), _stream()), "baked_mesh_colors" + sfx)
+    return colors
