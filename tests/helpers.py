@@ -212,6 +212,55 @@ def targets(kind, poses):
     return imgs.contiguous(), opts
 
 
+# The seven pretrained low-res scenes (golden/weights_<scene>_lowres.npz: oracle/make_golden.py writes lego and fern,
+# oracle/make_pretrained.py the other five).  Every network is A0 by its tensors' shapes, whatever the scene's config
+# says: 4 layers, hidden 128, skip 4, 4 direction bands, 10 position bands (fern 6).  Per scene: position bands, the
+# config's fine samples per ray (64 coarse everywhere), NDC, near, far, white background, noise std of training and the
+# camera (H, W, focal): the Blender scenes' half-resolution 400 x 400 camera, fern's 378 x 504 forward-facing one.
+PRETRAINED_SCENES = {
+    "chair": (10, 64, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+    "drums": (10, 64, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+    "fern": (6, 64, True, 0.0, 1.0, False, 1.0, (378, 504, 407.5658)),
+    "hotdog": (10, 128, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+    "lego": (10, 64, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+    "materials": (10, 64, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+    "ship": (10, 128, False, 2.0, 6.0, True, 0.2, (400, 400, 555.5555155968841)),
+}
+# The boxes the scenes' geometry lies in: the Blender scenes' objects inside [-1.5, 1.5]^3, fern's NDC box (FERN_BOX).
+PRETRAINED_BOX = {s: (FERN_BOX if s == "fern" else LEGO_BOX) for s in PRETRAINED_SCENES}
+
+
+def pretrained_arch(scene):
+    """The ops.ArchSpec of a pretrained scene's networks."""
+    from nerf_pytorch_b200 import ops
+
+    return ops.ArchSpec(num_layers=4, hidden=128, skip_every=4, n_freq_xyz=PRETRAINED_SCENES[scene][0], n_freq_dir=4)
+
+
+def pretrained_poses(scene, n):
+    """n camera poses of a pretrained scene: for the Blender scenes a ring of pose_spherical at radius 4.03 (the
+    datasets' camera distance), azimuth 360 i / n + 7 (i mod 3), elevation -30, -45, -15 in turn; for fern the identity
+    and n - 1 translations in the image plane by up to 0.1 (forward-facing captures move little)."""
+    if scene != "fern":
+        return sphere_poses(n, radius=4.03)
+    out = []
+    for i in range(n):
+        p = torch.eye(4)
+        if i:
+            a = 2 * math.pi * (i - 1) / max(n - 1, 1)
+            p[0, 3], p[1, 3] = 0.1 * math.cos(a), 0.1 * math.sin(a)
+        out.append(p)
+    return torch.stack(out)
+
+
+def pretrained_options(scene, perturb=True):
+    """Reference options of a pretrained scene's training step (perturbed, with its noise) or, perturb False, of its
+    deterministic render."""
+    _, nf, ndc, near, far, white, noise, _ = PRETRAINED_SCENES[scene]
+    return O.make_options(no_ndc=not ndc, near=near, far=far, num_coarse=64, num_fine=nf, perturb=perturb,
+                          radiance_field_noise_std=noise if perturb else 0.0, white_background=white)
+
+
 def psnr32(a, b):
     """PSNR (dB) from the fp32 mean squared error, at most 120 dB (the error clamped at 1e-12)."""
     return -10.0 * math.log10(max(torch.mean((a - b) ** 2).item(), 1e-12))

@@ -79,3 +79,24 @@ def test_tiny_nerf_oracle_matches_reference_outputs_and_gradients():
     # the jittered grid: depth = linspace + U[0,1) * (far - near) / S, NOT clamped to its cell (tiny_nerf.py:47-56)
     _, depth = T.compute_query_points_from_rays(torch.zeros(4, 3), torch.ones(4, 3), 2.0, 6.0, 64, rand=torch.ones(4, 64) * 0.999)
     assert depth.shape == (4, 64) and float(depth[0, 0]) > 2.0 and float(depth[0, -1]) > 6.0
+
+
+@pytest.mark.parametrize("scene", ["chair", "drums", "fern", "hotdog", "lego", "materials", "ship"])
+def test_pretrained_fixtures_load_with_a0_shapes(scene):
+    """Every pretrained scene's coarse and fine state dicts load with the shapes of A0 (4 x 128, skip 4, 4 direction
+    bands, 10 position bands or fern's 6), finite, into the oracle's functional forward and into FlexibleNeRFModel."""
+    from helpers import PRETRAINED_SCENES, load_weights, pretrained_arch
+    from oracle import nerf_oracle as O
+    import nerf_pytorch_b200 as nb
+
+    assert sorted(PRETRAINED_SCENES) == ["chair", "drums", "fern", "hotdog", "lego", "materials", "ship"]
+    arch = pretrained_arch(scene)
+    for sd in load_weights(f"{scene}_lowres"):
+        want = O.init_flexible_nerf(4, 128, 4, arch.n_freq_xyz, 4)
+        assert {k: tuple(v.shape) for k, v in sd.items()} == {k: tuple(v.shape) for k, v in want.items()}
+        assert all(v.dtype == torch.float32 and bool(torch.isfinite(v).all()) for v in sd.values())
+        assert O.arch_from_state_dict(sd, arch.dim_xyz, arch.dim_dir) == dict(num_layers=4, hidden=128, wide=[],
+                                                                               use_viewdirs=True)
+        m = nb.FlexibleNeRFModel(num_layers=4, hidden_size=128, skip_connect_every=4,
+                                 num_encoding_fn_xyz=arch.n_freq_xyz, num_encoding_fn_dir=4)
+        m.load_state_dict(sd)
