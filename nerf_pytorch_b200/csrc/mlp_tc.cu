@@ -103,6 +103,98 @@ __device__ __forceinline__ MmaInfo mma_info(const Plan& p, const float* blob, in
   return mi;
 }
 
+// Pieces of the CTA the forward, density-gradient and bake kernels share, so that the rows they have in common get the
+// same bits from one copy of the code: the constants, the weight stream, the encoding prologue, the direction bias.
+
+// named barrier of consumer warpgroup wg's 128 threads
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+// Once per CTA, by its `threads` threads: the ring's mbarriers; the biases of the gemm layers (x 2048 / 16) and the head
+// weights (x 16, they multiply activation / 16) to shared memory, then the head biases (4 per head) past the weights.
+// Returns the head biases; hw1 = where h[1]'s weights start.
+template <int kStage>
+__device__ __forceinline__ float* cta_constants(const Plan& p, const float* blob, WeightRing<kStage>& ring,
+                                                int consumer_warps, int threads, float* s_bias, float* s_headw, int& hw1) {
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    ring.init(consumer_warps);
+    fence_barrier_init();
+  }
+  for (int gi = 0; gi < p.n_gemm; ++gi)
+    for (int i = tid; i < p.g[gi].n; i += threads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
+  hw1 = p.h[0].n_out * p.h[0].k;
+  const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
+  for (int i = tid; i < hw1; i += threads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
+  for (int i = tid; i < hw2; i += threads) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
+  float* s_headb = s_headw + ((hw1 + hw2 + 3) & ~3);
+  if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
+  if (tid >= 4 && tid < 8) s_headb[tid] = p.n_head > 1 ? blob[p.h[1].b_off + tid - 4] : 0.f;
+  return s_headb;
+}
+
+// Producer, per tile: the forward copies of layers [0, n_layers), in the stages fwd_layer's MMAs read them
+template <bool kFast, int kStage>
+__device__ __forceinline__ void fill_layers(const Plan& p, const float* blob, WeightRing<kStage>& ring, int n_layers,
+                                            uint64_t pol) {
+  for (int e = 0; e < n_layers; ++e) {
+    const MmaInfo mi = mma_info(p, blob, e, kFast, kStage);
+    for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
+      const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
+      const uint8_t* src = mi.src + (size_t)ks * mi.kbytes;
+      if (kFast)  // the hs part of each k-step: one bulk copy each
+        ring.fill(src, nk, mi.kbytes / 3, mi.kbytes, pol);
+      else        // the k-steps' three copies are contiguous in the blob: one bulk copy
+        ring.fill(src, 1, nk * mi.kbytes, 0, pol);
+    }
+  }
+}
+
+// Prologue of tile row trow: the xyz positional encoding of its point x(c), c = 0, 1, 2 -> the encoding operand tile
+// enc (value / 16, hi block | lo block enc_hb bytes on; the single pass writes the hi block alone).  The row's two
+// threads (half 0, 1) split the frequency bands; half 1 zeroes the padding up to the operand width.
+template <bool kFast, typename X>
+__device__ __forceinline__ void encode_row(const Plan& p, uint8_t* enc, int enc_w, int enc_hb, int trow, int half, X x) {
+  const int nf = p.n_freq_xyz, mid = nf >> 1;
+  const int f0 = half ? mid : 0, f1 = half ? nf : mid;
+  const int base = p.inc_xyz ? 3 : 0;
+  auto put = [&](int k, float v) {
+    uint32_t hi, lo = 0;
+    if (kFast)
+      hi = f16x2_hi(v * kActScale, 0.f);
+    else
+      split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
+    const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
+    *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
+    if (!kFast) *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
+  };
+  for (int c = 0; c < 3; ++c) {
+    const float xc = x(c);
+    if (p.inc_xyz && half == 0) put(c, xc);
+    for (int f = f0; f < f1; ++f) {
+      float sn, cs;
+      sincosf(__fmul_rn(xc, p.freq_xyz[f]), &sn, &cs);
+      put(base + 6 * f + c, sn);
+      put(base + 6 * f + 3 + c, cs);
+    }
+  }
+  if (half == 1)  // zero padding up to the operand width (one fp16 k-step = 16 granular)
+    for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+}
+
+// The direction term of layers_dir[0] as a bias, for n_dirs view directions, by threads t, t + threads, ...:
+// vb[d][n] = (sum_k encd[d][k] W[n][H + k] + b[n]) / 16, at the accumulator's 2^11 scale.  encd: [d][32] direction
+// encodings; wv: the weight's direction rows Wt[k_h + k][n]; vb rows vb_stride apart.
+__device__ __forceinline__ void dir_bias(const Plan& p, const float* encd, const float* wv, const float* s_bias,
+                                         float* vb, int vb_stride, int n_dirs, int t, int threads) {
+  const GemmLayer& gd = p.g[p.n_gemm - 1];
+  for (int i = t; i < n_dirs * gd.n; i += threads) {
+    const int d = i / gd.n, n = i - d * gd.n;
+    float a = 0.f;
+    for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[d * 32 + k], wv[k * gd.n + n], a);
+    vb[d * vb_stride + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);
+  }
+}
+
 }  // namespace tc
 
 using namespace tc;
@@ -174,8 +266,7 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
   ring.release_last(acc);
 
   // ---------------- epilogue ----------------
-  const int wg_bar_id = 1 + wg;
-  asm volatile("bar.sync %0, 128;" ::"r"(wg_bar_id) : "memory");  // every warp's MMAs have read the activation tile
+  wg_bar(wg);  // every warp's MMAs have read the activation tile
   const bool has_next = e + 1 < p.n_gemm;
   const int hsel = head_of(p, e);
   const float* hw = hsel == 1 ? s_headw + hw1 : s_headw;
@@ -240,7 +331,7 @@ __device__ __forceinline__ void fwd_layer(const Plan& p, const float* blob, floa
   }
   if (has_next) {
     fence_proxy_async();  // generic-proxy stores -> the next layer's wgmma reads them through the async proxy
-    asm volatile("bar.sync %0, 128;" ::"r"(wg_bar_id) : "memory");
+    wg_bar(wg);
   }
   if (kTrain) {
 #pragma unroll
@@ -321,20 +412,8 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   const int64_t P_pad = stash_tiles * kTileRows;   // the stash sections are sized in 128-point tiles
   const int enc_w = p.enc_tile_w;                  // encoding operand tile width (dim_xyz padded to 16)
 
-  if (tid == 0) {
-    ring.init(4 * kWG);
-    fence_barrier_init();
-  }
-  // biases (/16) + head weights (x16, they multiply activation / 16): once per CTA
-  for (int gi = 0; gi < p.n_gemm; ++gi)
-    for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
-  const int hw1 = p.h[0].n_out * p.h[0].k;
-  const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
-  for (int i = tid; i < hw1; i += kThreads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
-  for (int i = tid; i < hw2; i += kThreads) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
-  float* s_headb = s_headw + ((hw1 + hw2 + 3) & ~3);
-  if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
-  if (tid >= 4 && tid < 8) s_headb[tid] = p.n_head > 1 ? blob[p.h[1].b_off + tid - 4] : 0.f;
+  int hw1;
+  const float* s_headb = cta_constants(p, blob, ring, 4 * kWG, kThreads, s_bias, s_headw, hw1);
   for (int i = tid; i < kWG * kMaxRaysPerTile * 32; i += kThreads) s_encd[i] = 0.f;  // padding channels stay zero
   if (p.use_viewdirs) {
     const GemmLayer& gd = p.g[p.n_gemm - 1];
@@ -350,18 +429,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     // ===================== weight producer =====================
     if ((tid & 31) == 0) {
       const uint64_t pol = l2_policy_evict_last();
-      for (int j = 0; j < my_tiles; ++j)
-        for (int e = 0; e < p.n_gemm; ++e) {
-          const MmaInfo mi = mma_info(p, blob, e, kFast, kStage);
-          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
-            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
-            const uint8_t* src = mi.src + (size_t)ks * mi.kbytes;
-            if (kFast)  // the hs part of each k-step: one bulk copy each
-              ring.fill(src, nk, mi.kbytes / 3, mi.kbytes, pol);
-            else        // the k-steps' three copies are contiguous in the blob: one bulk copy
-              ring.fill(src, 1, nk * mi.kbytes, 0, pol);
-          }
-        }
+      for (int j = 0; j < my_tiles; ++j) fill_layers<kFast>(p, blob, ring, p.n_gemm, pol);
     }
   } else {
     // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
@@ -372,7 +440,6 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     float* encd = s_encd + wg * kMaxRaysPerTile * 32;
     uint8_t* enc = sm + mp.enc;
     const int enc_hb = kRows * enc_w * 2;          // bytes of the hi (or lo) block of the encoding tile
-    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
 #pragma unroll 1
     for (int j = 0; j < my_tiles; ++j) {
       const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
@@ -401,7 +468,7 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
       // ================= encodings of this row -> operand tile (value / 16), the two halves split the frequencies
       if (kTrain) {  // the previous tile's encoding store must have finished reading the tile
         if (wt == 0) bulk_wait_read();
-        wg_bar();
+        wg_bar(wg);
       }
       {
         int64_t pt;
@@ -414,33 +481,10 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
         const int64_t ray = (int64_t)((uint32_t)pt / (uint32_t)S);
         const float* rr = rays + ray * ray_stride;
         const float zz = kPts ? 0.f : z[pt];
-        const int nf = p.n_freq_xyz, mid = nf >> 1;
-        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
-        const int base = p.inc_xyz ? 3 : 0;
-        const int trow = 64 * wg + row;
-        auto put = [&](int k, float v) {
-          uint32_t hi, lo = 0;
-          if (kFast)
-            hi = f16x2_hi(v * kActScale, 0.f);
-          else
-            split_f16x2(v * kActScale, 0.f, hi, lo);  // this element in the low halves
-          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
-          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
-          if (!kFast) *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
-        };
-        for (int c = 0; c < 3; ++c) {
-          // pts = ro + rd * z (train_utils.py:67), or the caller's point
-          const float x = kPts ? pts[pt * 3 + c] : __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));
-          if (p.inc_xyz && half == 0) put(c, x);
-          for (int f = f0; f < f1; ++f) {
-            float sn, cs;
-            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
-            put(base + 6 * f + c, sn);
-            put(base + 6 * f + 3 + c, cs);
-          }
-        }
-        if (half == 1)  // zero padding up to the operand width (one fp16 k-step = 16 granular)
-          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+        // pts = ro + rd * z (train_utils.py:67), or the caller's point
+        encode_row<kFast>(p, enc, enc_w, enc_hb, 64 * wg + row, half, [&](int c) {
+          return kPts ? pts[pt * 3 + c] : __fadd_rn(rr[c], __fmul_rn(rr[3 + c], zz));
+        });
       }
       // ---- per-ray direction term of layers_dir[0]: vb[ray][n] = (sum_k enc_dir(ray)[k] * W[n][H + k] + b[n]) / 16
       if (p.use_viewdirs) {
@@ -449,17 +493,11 @@ mlp_fwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
           const float v = kPts ? dirs[(first_ray + jr) * dir_stride + c] : rays[(first_ray + jr) * ray_stride + 8 + c];
           encode_coord(v, c, p.inc_dir, 0, p.n_freq_dir, p.freq_dir, encd + jr * 32);
         }
-        wg_bar();
-        const GemmLayer& gd = p.g[p.n_gemm - 1];
-        for (int i = wt; i < n_rays_wg * gd.n; i += 128) {
-          const int jr = i / gd.n, n = i - jr * gd.n;
-          float a = 0.f;
-          for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[jr * 32 + k], s_wv[k * gd.n + n], a);
-          viewb[jr * vbs + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);  // per-ray bias of layers_dir[0] (x 2048 / 16)
-        }
+        wg_bar(wg);
+        dir_bias(p, encd, s_wv, s_bias, viewb, vbs, n_rays_wg, wt, 128);
       }
       fence_proxy_async();  // the tile was written through the generic proxy; wgmma / the bulk store read it via the async proxy
-      wg_bar();             // also publishes viewb
+      wg_bar(wg);  // also publishes viewb
       if (stashes && wt == 0) {  // this warpgroup's rows of the encoding tile go to the stash as they are:
         // two bulk stores into half blk & 1 of stash tile blk >> 1 (64 rows of a hi or lo block are contiguous)
         uint8_t* dst = reinterpret_cast<uint8_t*>(stash + (size_t)P_pad * p.enc_cum[0]) + (size_t)(blk >> 1) * tile_bytes(enc_w);
@@ -765,7 +803,7 @@ density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__
     ring.init(4 * kWG);
     fence_barrier_init();
   }
-  // the trunk's biases and the sigma head, scaled as mlp_fwd_tc_kernel scales them
+  // the trunk's biases and the sigma head, scaled as cta_constants scales them
   for (int gi = 0; gi < L; ++gi)
     for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
   const int hw1 = p.h[0].n_out * p.h[0].k;
@@ -786,13 +824,7 @@ density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__
     if ((tid & 31) == 0) {
       const uint64_t pol = l2_policy_evict_last();
       for (int j = 0; j < my_tiles; ++j) {
-        for (int e = 0; e < L; ++e) {
-          const MmaInfo mi = mma_info(p, blob, e, false, kStage);
-          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
-            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
-            ring.fill(mi.src + (size_t)ks * mi.kbytes, 1, nk * mi.kbytes, 0, pol);
-          }
-        }
+        fill_layers<false>(p, blob, ring, L, pol);
         for (int t = L - 1; t >= 0; --t) {
           const GemmLayer& g = p.g[t];
           if (g.k_enc > 0 && g.enc_sel == 0) {
@@ -819,47 +851,22 @@ density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__
     const uint32_t* const mrow[2] = {s_mask + lr0 * gm.mask_words, s_mask + (lr0 + 8) * gm.mask_words};
     const uint64_t g_hi = make_desc(smem_u32(act) + (uint32_t)(wg * 64 * kH * 2), 128, kH * 16);
     const uint32_t g_lo_off = (uint32_t)(kRows * kH * 2);
-    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
 #pragma unroll 1
     for (int j = 0; j < my_tiles; ++j) {
       const int64_t tile = blockIdx.x + (int64_t)j * gridDim.x;
       const int64_t p0 = tile * kRows + 64 * wg;
       const RowState rs = row_state(p0, lr0, P, 1, 0);
-      // ---- encodings of this row -> operand tile (value / 16), as mlp_fwd_tc_kernel's prologue writes them for pts
-      {
-        const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
-        const int nf = p.n_freq_xyz, mid = nf >> 1;
-        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
-        const int base = p.inc_xyz ? 3 : 0;
-        const int trow = 64 * wg + row;
-        auto put = [&](int k, float v) {
-          uint32_t hi, lo;
-          split_f16x2(v * kActScale, 0.f, hi, lo);
-          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
-          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
-          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
-        };
-        for (int c = 0; c < 3; ++c) {
-          const float x = pts[pt * 3 + c];
-          if (p.inc_xyz && half == 0) put(c, x);
-          for (int f = f0; f < f1; ++f) {
-            float sn, cs;
-            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
-            put(base + 6 * f + c, sn);
-            put(base + 6 * f + 3 + c, cs);
-          }
-        }
-        if (half == 1)
-          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
-      }
+      // ---- encodings of this row -> operand tile, as the pts forward writes them
+      const int64_t pt = (p0 + row < P) ? p0 + row : P - 1;
+      encode_row<false>(p, enc, enc_w, enc_hb, 64 * wg + row, half, [&](int c) { return pts[pt * 3 + c]; });
       fence_proxy_async();
-      wg_bar();
+      wg_bar(wg);
       // ---- the trunk: sigma_raw -> out[pt][0], the ReLU bits -> s_mask
 #pragma unroll 1
       for (int e = 0; e < L; ++e)
         fwd_layer<false, false, kH, kStage, true>(p, blob, out, nullptr, sm, mp, e, wg, kRows, 0, 0, rs, ring, s_bias,
                                                   s_headw, s_headb, nullptr, hw1, s_mask, gm.mask_words);
-      wg_bar();  // the last layer's bits are in place
+      wg_bar(wg);  // the last layer's bits are in place
       // ---- the reverse chain from G_{L-1} = w_sigma (.) mask_{L-1}, stored / 16 (s_headw holds 16 w: Y = 8 s_headw)
       float chain[kH / 2];
       {
@@ -883,7 +890,7 @@ density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__
 #pragma unroll 1
       for (int t = L - 1; t >= 0; --t) {
         fence_proxy_async();  // generic-proxy stores of G_t -> the MMAs read them through the async proxy
-        wg_bar();
+        wg_bar(wg);
         const GemmLayer& g = p.g[t];
         if (g.k_enc > 0 && g.enc_sel == 0) {
           nch = ((g.k_tc + 15) >> 4) - (g.k_h >> 4);
@@ -891,7 +898,7 @@ density_grad_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__
         }
         if (t > 0) {
           grad_chain_mma<kH, kStage>(chain, ring, g_hi, g_lo_off);
-          wg_bar();  // every warp's MMAs have read G_t
+          wg_bar(wg);  // every warp's MMAs have read G_t
           grad_g_store<kH>(p, chain, t - 1, act, kRows, mrow, 64 * wg + lr0);
         }
       }
@@ -1041,20 +1048,8 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
   const int enc_w = p.enc_tile_w;
   const int n_body = p.use_viewdirs ? p.n_gemm - 1 : p.n_gemm;  // the layers fwd_layer runs
 
-  if (tid == 0) {
-    ring.init(4 * kWG);
-    fence_barrier_init();
-  }
-  // biases and heads as mlp_fwd_tc_kernel scales them; the basis; the directions' encodings (in the activation tile)
-  for (int gi = 0; gi < p.n_gemm; ++gi)
-    for (int i = tid; i < p.g[gi].n; i += kThreads) s_bias[p.g[gi].cum_n + i] = blob[p.g[gi].b_off + i] * (kActScale * kLoScale);
-  const int hw1 = p.h[0].n_out * p.h[0].k;
-  const int hw2 = p.n_head > 1 ? p.h[1].n_out * p.h[1].k : 0;
-  for (int i = tid; i < hw1; i += kThreads) s_headw[i] = blob[p.h[0].w_off + i] * kActInv;
-  for (int i = tid; i < hw2; i += kThreads) s_headw[hw1 + i] = blob[p.h[1].w_off + i] * kActInv;
-  float* s_headb = s_headw + ((hw1 + hw2 + 3) & ~3);
-  if (tid < 4) s_headb[tid] = blob[p.h[0].b_off + tid];
-  if (tid >= 4 && tid < 8) s_headb[tid] = p.n_head > 1 ? blob[p.h[1].b_off + tid - 4] : 0.f;
+  int hw1;
+  const float* s_headb = cta_constants(p, blob, ring, 4 * kWG, kThreads, s_bias, s_headw, hw1);
   for (int i = tid; i < (int)(sizeof(BakeBasis) / 4); i += kThreads)
     reinterpret_cast<float*>(s_basis)[i] = reinterpret_cast<const float*>(&basis)[i];
   float* encd = reinterpret_cast<float*>(sm + mp.act);  // [64][32], free until the first tile
@@ -1069,13 +1064,7 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
   __syncthreads();
   if (p.use_viewdirs) {  // viewb of the forward, per direction
     const GemmLayer& gd = p.g[p.n_gemm - 1];
-    const float* wv_g = blob + gd.wt_off + (size_t)gd.k_h * gd.n;  // rows k_h.. of Wt[k][n]
-    for (int i = tid; i < kBakeDirs * gd.n; i += kThreads) {
-      const int d = i / gd.n, n = i - d * gd.n;
-      float a = 0.f;
-      for (int k = 0; k < p.dim_dir; ++k) a = fmaf(encd[d * 32 + k], wv_g[k * gd.n + n], a);
-      s_dirb[d * kN + n] = fmaf(a, kActScale * kLoScale, s_bias[gd.cum_n + n]);
-    }
+    dir_bias(p, encd, blob + gd.wt_off + (size_t)gd.k_h * gd.n, s_bias, s_dirb, kN, kBakeDirs, tid, kThreads);
   }
   __syncthreads();
 
@@ -1085,14 +1074,7 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
     // ===================== weight producer: every layer's forward copy, per tile, as the forward streams them =========
     if ((tid & 31) == 0) {
       const uint64_t pol = l2_policy_evict_last();
-      for (int j = 0; j < my_tiles; ++j)
-        for (int e = 0; e < p.n_gemm; ++e) {
-          const MmaInfo mi = mma_info(p, blob, e, false, kStage);
-          for (int ks = 0; ks < mi.ksteps; ks += mi.sps) {
-            const uint32_t nk = (uint32_t)min(mi.sps, mi.ksteps - ks);
-            ring.fill(mi.src + (size_t)ks * mi.kbytes, 1, nk * mi.kbytes, 0, pol);
-          }
-        }
+      for (int j = 0; j < my_tiles; ++j) fill_layers<false>(p, blob, ring, p.n_gemm, pol);
     }
   } else {
     // ===================== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of every tile =====================
@@ -1112,7 +1094,6 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
       rs.valid[i] = true;
       rs.ray_slot[i] = 0;
     }
-    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); };
     // this lane's coefficients k = q + 4 m - 1 (m = 0 .. 6; k = -1 is sigma's column): channel and basis row
     int kc[7], kj[7];
 #pragma unroll
@@ -1133,33 +1114,11 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
         const int l[3] = {lp % 9, (lp / 9) % 9, lp / 81};
         const int b = bricks[slot];
         const int bc[3] = {b % nb[0], (b / nb[0]) % nb[1], b / (nb[0] * nb[1])};
-        const int nf = p.n_freq_xyz, mid = nf >> 1;
-        const int f0 = half ? mid : 0, f1 = half ? nf : mid;
-        const int base = p.inc_xyz ? 3 : 0;
-        const int trow = 64 * wg + row;
-        auto put = [&](int k, float v) {
-          uint32_t hi, lo;
-          split_f16x2(v * kActScale, 0.f, hi, lo);
-          const int off = tile_piece(trow, k >> 3, enc_w) + (k & 7) * 2;
-          *reinterpret_cast<uint16_t*>(enc + off) = (uint16_t)hi;
-          *reinterpret_cast<uint16_t*>(enc + enc_hb + off) = (uint16_t)lo;
-        };
-        for (int c = 0; c < 3; ++c) {
-          const int li = min(bc[c] * kBakeBrick + l[c], box.res[c]);
-          const float x = bake_coord(box, c, li);
-          if (p.inc_xyz && half == 0) put(c, x);
-          for (int f = f0; f < f1; ++f) {
-            float sn, cs;
-            sincosf(__fmul_rn(x, p.freq_xyz[f]), &sn, &cs);
-            put(base + 6 * f + c, sn);
-            put(base + 6 * f + 3 + c, cs);
-          }
-        }
-        if (half == 1)
-          for (int k = p.dim_xyz; k < enc_w; ++k) put(k, 0.f);
+        encode_row<false>(p, enc, enc_w, enc_hb, 64 * wg + row, half,
+                          [&](int c) { return bake_coord(box, c, min(bc[c] * kBakeBrick + l[c], box.res[c])); });
       }
       fence_proxy_async();
-      wg_bar();
+      wg_bar(wg);
       // ---- trunk (+ fc_feat): the heads' outputs -> s_head
 #pragma unroll 1
       for (int e = 0; e < n_body; ++e) {
@@ -1250,7 +1209,7 @@ bake_tc_kernel(const __grid_constant__ Plan p, const __grid_constant__ BakeBasis
           }
         }
       }
-      wg_bar();  // s_head is read before the next tile's heads overwrite it
+      wg_bar(wg);  // s_head is read before the next tile's heads overwrite it
     }
   }
 }
