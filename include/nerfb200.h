@@ -890,6 +890,49 @@ int32_t nerfb200_baked_mesh_colors_f16(const nerfb200_grid_t* box, const int32_t
                                        int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
                                        int64_t n_vertices, float* colors, void* stream);
 
+/* ---- baked fields: 8-bit values -------------------------------------------------------------------------------------
+ * A baked field whose values are stored as one byte per channel with a per-channel scale and offset, at a quarter of
+ * the bytes of the fp32 field and half of the fp16 one, for fields that are kept, saved, rendered, pruned and meshed
+ * (SNeRG ships its baked grids as 8-bit values).  Fine-tuning, the regularisers and subdivision stay fp32: dequantise
+ * the field, work on it, and quantise it again.
+ *   - Layout.  values[slot][729][32] uint8 codes (32 B per lattice point, one 32-B sector); channels 28 .. 31 hold 0
+ *     and are never read.  dequant[2][28] fp32 in device memory: row 0 the scale s_c of channel c, row 1 its offset o_c.
+ *   - Quantisation (done by the library's Python interface, BakedField.quantize), for c = 0 .. 27, every op rounded to
+ *     fp32: lo_c = min(0, min v) and hi_c = max(0, max v) over every stored value of channel c (every slot and lattice
+ *     point), so the range holds 0; s_c = (hi_c - lo_c) / 255, or 1 where that is 0; z_c = clamp(rint(-lo_c / s_c), 0,
+ *     255), an integer held as +0 when it is 0 (never -0), so o_c = -(z_c s_c) is -0 for z_c = 0; q = clamp(rint((v -
+ *     o_c) / s_c), 0, 255), rint rounding half to even.  Every division is correctly rounded (not a multiplication by
+ *     a rounded reciprocal), so the codes and the table are the same bits on every device.  A field with a non-finite
+ *     value in channels 0 .. 27, or whose range hi_c - lo_c overflows fp32, is refused.
+ *   - Dequantisation.  v' = fl(fl(q s_c) + o_c): two rounded ops, no contraction (in torch q.float() * s + o).  Zero is
+ *     exact: v'(z_c) = fl(z_c s_c) - fl(z_c s_c) = +0, so a sigma_raw <= 0 gets a code <= z_0 and dequantises to <= 0,
+ *     and a transparent brick ("baked fields: pruning") stays transparent.  Equal values get equal codes, so the stored
+ *     copies of a lattice point stay bit-equal and the mesh rule of "baked fields: meshes" ("Copies") still holds.  The
+ *     scales are per channel, not per brick, for that reason.
+ *   - Rendering, peak weights and meshes (baked_render_u8, baked_max_weights_u8, baked_mesh_dirs_u8,
+ *     baked_mesh_colors_u8).  Each code is dequantised as it is gathered; every other op is the fp32 rule of "baked
+ *     fields", "baked fields: pruning" and "baked fields: meshes": the same corners in the same order through the same
+ *     fmaf chain.  A uint8 field therefore renders, gives peak weights and meshes bit for bit like the fp32 field holding
+ *     its dequantised values.  A corner's channels 0 .. 27 are two 16-B loads; the peak weights and the mesh's sigma_raw
+ *     reads are one byte per point.  The 56 table entries are copied into each CTA's shared memory once.
+ * baked_render_u8, baked_max_weights_u8, baked_mesh_dirs_u8, baked_mesh_colors_u8: the arguments of baked_render,
+ *   baked_max_weights, baked_mesh_dirs and baked_mesh_colors, values uint8 codes followed by dequant.  Refused before any
+ *   launch: whatever their fp32 twins refuse (the same checks), a values pointer that is not 16-B aligned, and a null
+ *   dequant. */
+int32_t nerfb200_baked_render_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                 const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
+                                 int64_t n_rays, int32_t white_background, float stop_transmittance, float* out,
+                                 void* stream);
+int32_t nerfb200_baked_max_weights_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                      const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
+                                      int64_t n_rays, float* max_w, void* stream);
+int32_t nerfb200_baked_mesh_dirs_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                    const float* dequant, float level, const int64_t* edge_keys, int64_t n_vertices,
+                                    float* dirs, float* normals, void* stream);
+int32_t nerfb200_baked_mesh_colors_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                      const float* dequant, int32_t use_viewdirs, float level, const int64_t* edge_keys,
+                                      const float* dirs, int64_t n_vertices, float* colors, void* stream);
+
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale
  * multiplies g first (1/world_size after a summed all-reduce). */

@@ -175,6 +175,10 @@ SIGNATURES = {
     "nerfb200_baked_mesh_dirs_f16": (I32, [GP, P, P, F32, P, I64, P, P, P]),
     "nerfb200_baked_mesh_colors": (I32, [GP, P, P, I32, F32, P, P, I64, P, P]),
     "nerfb200_baked_mesh_colors_f16": (I32, [GP, P, P, I32, F32, P, P, I64, P, P]),
+    "nerfb200_baked_render_u8": (I32, [GP, P, P, P, I32, P, I32, I64, I32, F32, P, P]),
+    "nerfb200_baked_max_weights_u8": (I32, [GP, P, P, P, I32, P, I32, I64, P, P]),
+    "nerfb200_baked_mesh_dirs_u8": (I32, [GP, P, P, P, F32, P, I64, P, P, P]),
+    "nerfb200_baked_mesh_colors_u8": (I32, [GP, P, P, P, I32, F32, P, P, I64, P, P]),
 }
 
 _lib = None

@@ -14,8 +14,10 @@ pointers; the bake reads the active brick count back once to size its values.  A
 same trilinear function (subdivide_baked, BakedFieldTrainer.subdivide; include/nerfb200.h "baked fields:
 subdivision").  A field kept, saved, rendered or pruned
 may store its values in fp16 (``bake(dtype=torch.float16)``, ``BakedField.half``; include/nerfb200.h "baked fields: half
-precision"); fine-tuning and the regularisers take fp32 fields only (``BakedField.float``).  Any field, fp32 or fp16, can
-be meshed without a network (extract_baked_mesh; include/nerfb200.h "baked fields: meshes")."""
+precision") or as 8-bit codes with a per-channel scale and offset (``BakedField.quantize``; include/nerfb200.h "baked
+fields: 8-bit values"); fine-tuning, the regularisers and subdivision take fp32 fields only (``BakedField.float``).  Any
+field, fp32, fp16 or 8-bit, can be meshed without a network (extract_baked_mesh; include/nerfb200.h "baked fields:
+meshes")."""
 from __future__ import annotations
 
 import math
@@ -28,16 +30,19 @@ from . import ops
 class BakedField:
     """A baked field on the device: ``bounds`` ((lo), (hi)) and ``resolution`` (three ints) of the lattice box,
     ``brick_map`` int32[bricks] (slot or -1), ``bricks`` int32[n_active] (slot -> brick), ``values``
-    fp32[n_active, 729, 32] or fp16 of that shape (include/nerfb200.h "baked fields: half precision") and
-    ``use_viewdirs`` (whether the network had view directions)."""
+    fp32[n_active, 729, 32], fp16 of that shape (include/nerfb200.h "baked fields: half precision") or uint8 codes of
+    that shape, ``use_viewdirs`` (whether the network had view directions) and ``dequant``: for uint8 codes the fp32
+    (2, 28) table of per-channel scales and offsets on the values' device (include/nerfb200.h "baked fields: 8-bit
+    values"), None otherwise."""
 
-    def __init__(self, bounds, resolution, brick_map, bricks, values, use_viewdirs: bool):
+    def __init__(self, bounds, resolution, brick_map, bricks, values, use_viewdirs: bool, *, dequant=None):
         self.bounds = (tuple(float(v) for v in bounds[0]), tuple(float(v) for v in bounds[1]))
         self.resolution = tuple(int(r) for r in resolution)
         self.brick_map = brick_map
         self.bricks = bricks
         self.values = values
         self.use_viewdirs = bool(use_viewdirs)
+        self.dequant = dequant
 
     @classmethod
     def full(cls, bounds, resolution, *, sigma_raw=0.1, use_viewdirs=True, device="cuda") -> "BakedField":
@@ -64,7 +69,7 @@ class BakedField:
 
     @property
     def dtype(self) -> torch.dtype:
-        """The values' dtype: torch.float32 or torch.float16."""
+        """The values' dtype: torch.float32, torch.float16 or torch.uint8."""
         return self.values.dtype
 
     def box(self):
@@ -78,6 +83,8 @@ class BakedField:
         chunk = int(chunk)
         if chunk < 1:
             raise ValueError(f"BakedField.half: chunk must be >= 1, got {chunk}")
+        if self.dtype == torch.uint8:
+            raise ValueError("BakedField.half: the field is 8-bit; dequantise it with .float() first")
         v = self.values.detach()
         out = torch.empty(v.shape, dtype=torch.float16, device=v.device)
         for s in range(0, self.n_active, chunk):
@@ -85,28 +92,81 @@ class BakedField:
             out[s:s + chunk] = torch.where(c.isfinite(), c.clamp(-65504.0, 65504.0), c)  # the copy rounds to nearest even
         return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, out, self.use_viewdirs)
 
-    def float(self) -> "BakedField":
-        """A field with fp32 values: an fp16 field widened exactly (a new tensor), an fp32 field's own values tensor.
-        ``brick_map`` and ``bricks`` are shared.  Fine-tune ``field.float()``, then convert back with ``half()``."""
-        v = self.values if self.values.dtype == torch.float32 else self.values.detach().float()
+    def quantize(self, chunk: int = 1024) -> "BakedField":
+        """A new 8-bit field under the quantisation rule (include/nerfb200.h "baked fields: 8-bit values"): per channel
+        c = 0 .. 27 the range [min(0, min v), max(0, max v)] over every stored value, scale s_c = range / 255 (1 for an
+        empty range), zero point z_c = clamp(rint(-lo_c / s_c), 0, 255) (an integer: 0 is +0), offset o_c = -(z_c s_c)
+        and codes clamp(rint((v - o_c) / s_c), 0, 255), each op rounded to fp32; channels 28 .. 31 hold 0.  A CUDA field
+        and its CPU copy give the same codes and dequant bits.  An fp16 field is widened exactly first, so its codes are
+        those of ``field.float().quantize()``.  Two passes of ``chunk`` slots (the range, then
+        the codes), so the peak is both fields plus one chunk's temporaries; ``brick_map`` and ``bricks`` are shared.
+        Renders, peak weights and meshes of the result are bit for bit those of ``result.float()``.  Reads the range
+        back once.  ValueError for a non-finite value in channels 0 .. 27, a range that overflows fp32, or an 8-bit
+        field.  Works on a CPU field too."""
+        chunk = int(chunk)
+        if chunk < 1:
+            raise ValueError(f"BakedField.quantize: chunk must be >= 1, got {chunk}")
+        if self.dtype == torch.uint8:
+            raise ValueError("BakedField.quantize: the field is already 8-bit; dequantise it with .float() first")
+        v = self.values.detach()
+        lo = torch.zeros(28, dtype=torch.float32, device=v.device)
+        hi = torch.zeros(28, dtype=torch.float32, device=v.device)
+        for s in range(0, self.n_active, chunk):
+            c = v[s:s + chunk, :, :28].float().reshape(-1, 28)
+            lo = torch.minimum(lo, c.amin(0))  # NaN propagates, so the finiteness check below sees it
+            hi = torch.maximum(hi, c.amax(0))
+        # a tensor divisor: torch's CUDA division by a Python scalar multiplies by its rounded reciprocal, which is not
+        # the rule's correctly rounded (hi - lo) / 255
+        scale = (hi - lo) / torch.full_like(hi, 255.0)
+        if not bool(torch.isfinite(torch.cat([lo, hi, scale])).all()):
+            raise ValueError("BakedField.quantize: channels 0 .. 27 must be finite and their range must fit in fp32")
+        scale = torch.where(scale == 0, torch.ones_like(scale), scale)
+        zero = torch.round(-lo / scale).clamp(0, 255)
+        zero = torch.where(zero == 0, torch.zeros_like(zero), zero)  # the integer 0 as +0 (clamp may keep a -0)
+        offset = -(zero * scale)
+        out = torch.zeros(v.shape, dtype=torch.uint8, device=v.device)
+        for s in range(0, self.n_active, chunk):
+            c = v[s:s + chunk, :, :28].float()
+            out[s:s + chunk, :, :28] = torch.round((c - offset) / scale).clamp(0, 255).to(torch.uint8)
+        return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, out, self.use_viewdirs,
+                          dequant=torch.stack([scale, offset]))
+
+    def float(self, chunk: int = 1024) -> "BakedField":
+        """A field with fp32 values: an fp16 field widened exactly (a new tensor), an 8-bit field dequantised exactly
+        under its rule, q.float() * s + o, ``chunk`` slots at a time (a new tensor, channels 28 .. 31 zero), an fp32
+        field's own values tensor.  ``brick_map`` and ``bricks`` are shared.  Fine-tune ``field.float()``, then convert
+        back with ``half()`` or ``quantize()``."""
+        if self.values.dtype == torch.uint8:
+            q, chunk = self.values.detach(), int(chunk)
+            if chunk < 1:
+                raise ValueError(f"BakedField.float: chunk must be >= 1, got {chunk}")
+            v = torch.zeros(q.shape, dtype=torch.float32, device=q.device)
+            for s in range(0, self.n_active, chunk):
+                v[s:s + chunk, :, :28] = q[s:s + chunk, :, :28].float() * self.dequant[0] + self.dequant[1]
+        else:
+            v = self.values if self.values.dtype == torch.float32 else self.values.detach().float()
         return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, v, self.use_viewdirs)
 
     def __repr__(self):
         return (f"BakedField({self.n_active} bricks of {ops.mesh_sparse_brick_count(self.box())}, "
                 f"{self.values.numel() * self.values.element_size() / 2 ** 20:.1f} MiB"
-                f"{' fp16' if self.dtype == torch.float16 else ''}, resolution {self.resolution}"
+                f"{' fp16' if self.dtype == torch.float16 else ' 8-bit' if self.dtype == torch.uint8 else ''}, "
+                f"resolution {self.resolution}"
                 f"{', view directions' if self.use_viewdirs else ''})")
 
     def save(self, path) -> None:
-        """Writes the field with torch.save; the values keep their dtype."""
+        """Writes the field with torch.save; the values keep their dtype, an 8-bit field its ``dequant``."""
         torch.save({"bounds": self.bounds, "resolution": self.resolution, "brick_map": self.brick_map.cpu(),
-                    "bricks": self.bricks.cpu(), "values": self.values.cpu(), "use_viewdirs": self.use_viewdirs}, path)
+                    "bricks": self.bricks.cpu(), "values": self.values.cpu(), "use_viewdirs": self.use_viewdirs,
+                    "dequant": None if self.dequant is None else self.dequant.cpu()}, path)
 
     @classmethod
     def load(cls, path, device="cuda") -> "BakedField":
+        """A field written by ``save``; a file without ``dequant`` (written before 8-bit fields) loads with None."""
         d = torch.load(path, map_location="cpu", weights_only=True)
+        dq = d.get("dequant")
         return cls(d["bounds"], d["resolution"], d["brick_map"].to(device), d["bricks"].to(device),
-                   d["values"].to(device), d["use_viewdirs"])
+                   d["values"].to(device), d["use_viewdirs"], dequant=None if dq is None else dq.to(device))
 
 
 def bake(model, encode_position_fn, encode_direction_fn=None, *, bounds, resolution, grid,
@@ -164,7 +224,8 @@ def render_baked(field: BakedField, height, width, focal_length, tform_cam2world
     white = getattr(options.nerf, "train" if train_utils.COMPAT_MODE_QUIRK else mode).white_background
     rays = _pose_rays(field, height, width, focal_length, tform_cam2world, options)
     values = field.values if field.n_active else field.values.new_zeros(1, 729, 32)
-    out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white), stop)
+    out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white), stop,
+                           dequant=field.dequant)
     return out[:, :3].view(height, width, 3), out[:, 3].view(height, width), out[:, 4].view(height, width)
 
 
@@ -183,15 +244,19 @@ def _pose_rays(field, height, width, focal_length, tform_cam2world, options):
 
 
 def _check_values(field, what, half=False):
-    """A CUDA field with fp32 values, or fp16 ones where ``half`` (renders and peak weights; fine-tuning is fp32 only)."""
+    """A CUDA field with fp32 values, or fp16 or 8-bit ones where ``half`` (renders and peak weights; fine-tuning is
+    fp32 only)."""
     if not isinstance(field, BakedField):
         raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
     if isinstance(field.values, torch.Tensor) and field.values.dtype == torch.float16 and not half:
         raise ValueError(f"{what}: an fp16 field has no gradient or fine-tuning path; fine-tune field.float() and "
                          f"convert it back with .half()")
+    if isinstance(field.values, torch.Tensor) and field.values.dtype == torch.uint8 and not half:
+        raise ValueError(f"{what}: an 8-bit field has no gradient or fine-tuning path; fine-tune field.float() and "
+                         f"quantise it again with .quantize()")
     if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda
-            and field.values.dtype in (torch.float32, torch.float16)):
-        raise ValueError(f"{what}: field.values must be an fp32 or fp16 CUDA tensor (there is no CPU path)")
+            and field.values.dtype in (torch.float32, torch.float16, torch.uint8)):
+        raise ValueError(f"{what}: field.values must be an fp32, fp16 or uint8 CUDA tensor (there is no CPU path)")
 
 
 class _BakedRender(torch.autograd.Function):
@@ -224,15 +289,18 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
     of each lattice point (include/nerfb200.h "baked fields: gradients and fine-tuning"), so copies that start equal stay
     equal under any elementwise optimiser.  ``early_stop`` as in ``render_baked``, for renders without a gradient.
 
-    An fp16 field renders bit for bit like ``field.float()`` and has no gradient.  This is the differentiable render,
-    which refuses an fp16 field in grad mode as it did before fp16 fields could be rendered at all; under
+    An fp16 or 8-bit field renders bit for bit like ``field.float()`` and has no gradient.  This is the differentiable
+    render, which refuses such a field in grad mode as it did before fp16 fields could be rendered at all; under
     ``torch.no_grad()`` (or inference mode) it renders one whose values do not require grad.  Anything else raises
-    ValueError (fine-tune ``field.float()``).  ``render_baked`` renders an fp16 field in any grad mode."""
+    ValueError (fine-tune ``field.float()``).  ``render_baked`` renders fp16 and 8-bit fields in any grad mode."""
     _check_values(field, "render_baked_rays", half=True)
     # grad mode alone keeps the refusal every fp16 field met here before half precision (pinned by the fine-tuning tests)
     if field.values.dtype == torch.float16 and (field.values.requires_grad or torch.is_grad_enabled()):
         raise ValueError("render_baked_rays: an fp16 field has no gradient; render it under torch.no_grad(), or "
                          "fine-tune field.float() and convert it back with .half()")
+    if field.values.dtype == torch.uint8 and torch.is_grad_enabled():
+        raise ValueError("render_baked_rays: an 8-bit field has no gradient; render it under torch.no_grad(), or "
+                         "fine-tune field.float() and quantise it again with .quantize()")
     stride = 11 if field.use_viewdirs else 8
     if not (isinstance(rays, torch.Tensor) and rays.dim() == 2 and rays.shape[1] == stride):
         raise ValueError(f"render_baked_rays: rays must be (N, {stride}) for a field "
@@ -250,7 +318,8 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
         out = _BakedRender.apply(field.values, field, rays, white)
     else:
         values = field.values.detach() if field.n_active else field.values.new_zeros(1, 729, 32)
-        out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, white, stop)
+        out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, white, stop,
+                               dequant=field.dequant)
     return out[:, :3], out[:, 3], out[:, 4], out[:, 5]
 
 
@@ -475,22 +544,28 @@ def prune_baked(field: BakedField, keep) -> BakedField:
 
     Lossless criteria (include/nerfb200.h "baked fields: pruning"): ``~baked_transparent_bricks(field)`` leaves every
     render the same bits; ``baked_brick_weights(...) > 0`` leaves the renders of the rays it was measured over the same
-    bits."""
+    bits.  An 8-bit field's codes are copied and its ``dequant`` shared, not formed again."""
     _check_keep(field, keep, "prune_baked")
     with torch.no_grad():
         brick_map, bricks, values = _pruned(field, torch.nonzero(keep).reshape(-1))
-    return BakedField(field.bounds, field.resolution, brick_map, bricks, values, field.use_viewdirs)
+    return BakedField(field.bounds, field.resolution, brick_map, bricks, values, field.use_viewdirs,
+                      dequant=field.dequant)
 
 
 def baked_transparent_bricks(field: BakedField, chunk: int = 1024) -> torch.Tensor:
-    """bool[n_active]: the bricks every stored sigma_raw of which is <= 0 and whose channels 0 .. 27 are all finite.
-    Dropping them leaves every render of the field the same bits (include/nerfb200.h "baked fields: pruning").  Torch
-    over ``chunk`` slots at a time; works on a CPU field too."""
+    """bool[n_active]: the bricks every stored sigma_raw of which is <= 0 and whose channels 0 .. 27 are all finite
+    (an 8-bit field's dequantised sigma_raw; its values are always finite).  Dropping them leaves every render of the
+    field the same bits (include/nerfb200.h "baked fields: pruning").  Torch over ``chunk`` slots at a time; works on a
+    CPU field too."""
     if not isinstance(field, BakedField):
         raise ValueError(f"baked_transparent_bricks: field must be an nb.BakedField, got {type(field).__name__}")
     v = field.values.detach()
     out = torch.empty(field.n_active, dtype=torch.bool, device=v.device)
     for s in range(0, field.n_active, chunk):
+        if v.dtype == torch.uint8:
+            sigma = v[s:s + chunk, :, 0].float() * field.dequant[0, 0] + field.dequant[1, 0]
+            out[s:s + chunk] = (sigma <= 0).all(1)
+            continue
         c = v[s:s + chunk, :, :28]
         out[s:s + chunk] = (c[..., 0] <= 0).all(1) & torch.isfinite(c).flatten(1).all(1)
     return out
@@ -520,7 +595,7 @@ def baked_brick_weights_rays(field: BakedField, rays, out=None) -> torch.Tensor:
         out = torch.zeros(field.n_active, dtype=torch.float32, device=dev)
     if field.n_active and rays.shape[0]:
         ops.baked_max_weights(field.box(), field.brick_map, field.values.detach(), field.use_viewdirs,
-                              rays.contiguous(), out)
+                              rays.contiguous(), out, dequant=field.dequant)
     return out
 
 
@@ -546,7 +621,7 @@ def baked_brick_weights(field: BakedField, poses, height, width, focal_length, o
     values, box = field.values.detach(), field.box()
     for p in host:
         rays = _pose_rays(field, height, width, focal_length, p, options)
-        ops.baked_max_weights(box, field.brick_map, values, field.use_viewdirs, rays, out)
+        ops.baked_max_weights(box, field.brick_map, values, field.use_viewdirs, rays, out, dequant=field.dequant)
     return out
 
 
@@ -561,6 +636,9 @@ def _check_subdivide(field, what):
     if field.values.dtype == torch.float16:
         raise ValueError(f"{what}: an fp16 field has no subdivision; subdivide field.float() and convert it back "
                          f"with .half()")
+    if field.values.dtype == torch.uint8:
+        raise ValueError(f"{what}: an 8-bit field has no subdivision; subdivide field.float() and quantise it again "
+                         f"with .quantize()")
     if not all(r <= 2048 for r in field.resolution):
         raise ValueError(f"{what}: resolution {field.resolution} is past 2048 on an axis (the child would pass 4096)")
     if not (field.values.is_cuda and field.values.dtype == torch.float32):
@@ -602,7 +680,7 @@ def subdivide_baked(field: BakedField) -> BakedField:
     with samples half as far apart.  ``field`` is not touched; the child needs up to 8 times the parent's values.  Prune
     first (``prune_baked``) to subdivide only the bricks worth keeping.  A field without active bricks gives an empty
     child without a launch.  ValueError for an fp16 field (subdivide ``field.float()``), a CPU field, or a resolution
-    past 2048 on an axis.  Reads the child brick count back once."""
+    past 2048 on an axis, and for an 8-bit field.  Reads the child brick count back once."""
     res = _check_subdivide(field, "subdivide_baked")
     with torch.no_grad():
         brick_map, bricks = _child_bricks(field, res)
@@ -619,7 +697,7 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
     the field's active bricks on the GPU (include/nerfb200.h "baked fields: meshes").  No network is needed, so this
     meshes a fine-tuned, pruned, subdivided or from-scratch field as it renders.
 
-    Marching cubes runs over sigma_raw (channel 0, an fp16 field's widened exactly): for ``level`` >= 0 the crossing of
+    Marching cubes runs over sigma_raw (channel 0, an fp16 field's widened exactly, an 8-bit field's dequantised): for ``level`` >= 0 the crossing of
     the renderer's density relu(sigma_raw) along a lattice edge is the crossing of sigma_raw, so the faces and vertex
     numbering are those of ``extract_mesh`` on the baked network over the same grid, and the vertices lie on the
     renderer's surface.  ``normals=True`` sets ``Mesh.normals``: the outward unit normal from central differences of
@@ -647,8 +725,8 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
     values = field.values
     if not (isinstance(values, torch.Tensor) and values.is_cuda):
         raise NotImplementedError("nerfb200: the baked field must be on a CUDA device (there is no CPU path)")
-    if values.dtype not in (torch.float32, torch.float16):
-        raise ValueError(f"extract_baked_mesh: field.values must be fp32 or fp16, got {values.dtype}")
+    if values.dtype not in (torch.float32, torch.float16, torch.uint8):
+        raise ValueError(f"extract_baked_mesh: field.values must be fp32, fp16 or uint8, got {values.dtype}")
     dev = values.device
 
     def empty():
@@ -662,6 +740,8 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
     values = values.detach()
     with torch.no_grad():
         sigma = values[..., 0].float().contiguous()  # (n_active, 729): the halo-0 sparse layout
+        if values.dtype == torch.uint8:
+            sigma = sigma * field.dequant[0, 0] + field.dequant[1, 0]
         totals, ws = ops.mesh_sparse_count(box, field.brick_map, field.bricks, field.n_active, sigma, False, level)
         n_v, n_f = (int(t) for t in totals.tolist())  # the one host sync: the outputs' sizes
         if n_v == 0:
@@ -671,7 +751,8 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
                                                      level, ws, n_v, n_f, want_keys=colors or normals)
         dirs = nrm = None
         if want_dirs:
-            dirs, nrm = ops.baked_mesh_dirs(box, field.brick_map, values, level, keys, want_normals=normals)
+            dirs, nrm = ops.baked_mesh_dirs(box, field.brick_map, values, level, keys, want_normals=normals,
+                                            dequant=field.dequant)
         if cam is not None:
             verts, faces, dirs = ops.ndc_mesh_to_world(cam, verts, faces, dirs)
             if normals:  # -(world dir), 0 where the NDC direction fell back (its normal is 0 there)
@@ -679,5 +760,5 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
         rgb = None
         if colors:
             rgb = ops.baked_mesh_colors(box, field.brick_map, values, field.use_viewdirs, level, keys,
-                                        dirs if field.use_viewdirs else None)
+                                        dirs if field.use_viewdirs else None, dequant=field.dequant)
     return Mesh(verts, faces, rgb, nrm)

@@ -170,7 +170,7 @@ __device__ __forceinline__ float corner_weight(const float f[3], int k) {
 }
 
 // 16-B offset of corner k of the cube at brick point l, from the slot's first value: a point is kBakeCh values of type V
-// (8 vectors of fp32, 4 of fp16)
+// (8 vectors of fp32, 4 of fp16, 2 of uint8 codes)
 template <typename V>
 __device__ __forceinline__ int corner_offset(const int l[3], int k) {
   const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
@@ -185,17 +185,41 @@ __device__ __forceinline__ void widen4(unsigned a, unsigned b, float out[4]) {
   out[3] = __half2float(__ushort_as_half((unsigned short)(b >> 16)));
 }
 
-// one stored value, widened to fp32
-__device__ __forceinline__ float baked_ld(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float baked_ld(const __half* p) {
-  return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(p))));
+// code q of channel ch dequantised (include/nerfb200.h "baked fields: 8-bit values"): fl(fl(q s_ch) + o_ch), dq the
+// [2][28] scales and offsets
+__device__ __forceinline__ float dequant(unsigned q, const float* dq, int ch) {
+  return __fadd_rn(__fmul_rn((float)q, dq[ch]), dq[kBakedVals + ch]);
 }
 
-// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0).  fp32: seven 16-B loads per corner; fp16:
-// three 16-B loads and one 8-B load (56 of the point's 64 B), each value widened exactly, then the same fmaf chain
+// channels 0 .. 27 of the 28 code bytes in w[0 .. 6], dequantised
+__device__ __forceinline__ void dequant28(const unsigned w[kBakedVals / 4], const float* dq, float a[kBakedVals]) {
+#pragma unroll
+  for (int ch = 0; ch < kBakedVals; ++ch) a[ch] = dequant((w[ch >> 2] >> (8 * (ch & 3))) & 0xffu, dq, ch);
+}
+
+// a uint8 field's dequant table copied into the CTA's shared memory dq_s; every thread of the CTA must call it before
+// any returns.  Nothing for fp32 and fp16 fields
 template <typename V>
-__device__ __forceinline__ void baked_interp(const V* __restrict__ values, int slot, const float f[3], const int l[3],
-                                             float v[kBakedVals]) {
+__device__ __forceinline__ void stage_dequant(const float* __restrict__ dequant_tab, float* dq_s) {
+  if constexpr (sizeof(V) == 1) {
+    if (threadIdx.x < 2 * kBakedVals) dq_s[threadIdx.x] = __ldg(dequant_tab + threadIdx.x);
+    __syncthreads();
+  }
+}
+
+// one stored value, widened to fp32 (channel 0 dequantised for uint8; dq is read for uint8 only)
+__device__ __forceinline__ float baked_ld(const float* p, const float*) { return __ldg(p); }
+__device__ __forceinline__ float baked_ld(const __half* p, const float*) {
+  return __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short*>(p))));
+}
+__device__ __forceinline__ float baked_ld(const uint8_t* p, const float* dq) { return dequant(__ldg(p), dq, 0); }
+
+// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0).  fp32: seven 16-B loads per corner; fp16:
+// three 16-B loads and one 8-B load (56 of the point's 64 B), each value widened exactly; uint8: two 16-B loads (the
+// point's one 32-B sector), each code dequantised with dq; then the same fmaf chain
+template <typename V>
+__device__ __forceinline__ void baked_interp(const V* __restrict__ values, const float* dq, int slot, const float f[3],
+                                             const int l[3], float v[kBakedVals]) {
 #pragma unroll
   for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = 0.f;
   if (slot >= 0) {
@@ -213,6 +237,14 @@ __device__ __forceinline__ void baked_interp(const V* __restrict__ values, int s
           v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
           v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
         }
+      } else if constexpr (sizeof(V) == 1) {
+        const uint4* pv = reinterpret_cast<const uint4*>(sv) + corner_offset<V>(l, k);
+        const uint4 u0 = __ldg(pv), u1 = __ldg(pv + 1);  // channels 28 .. 31 (u1.w) are not read
+        const unsigned wd[kBakedVals / 4] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z};
+        float a[kBakedVals];
+        dequant28(wd, dq, a);
+#pragma unroll
+        for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(w, a[ch], v[ch]);
       } else {
         const uint4* pv = reinterpret_cast<const uint4*>(sv) + corner_offset<V>(l, k);
         float a[kBakedVals];
@@ -231,17 +263,17 @@ __device__ __forceinline__ void baked_interp(const V* __restrict__ values, int s
   }
 }
 
-// channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B (fp32)
-// or 2-B (fp16) load per corner
+// channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B (fp32),
+// 2-B (fp16) or 1-B (uint8) load per corner
 template <typename V>
-__device__ __forceinline__ float baked_interp_sigma(const V* __restrict__ values, int slot, const float f[3],
-                                                    const int l[3]) {
+__device__ __forceinline__ float baked_interp_sigma(const V* __restrict__ values, const float* dq, int slot,
+                                                    const float f[3], const int l[3]) {
   float v = 0.f;
   if (slot >= 0) {
     const V* base = values + (int64_t)slot * kBakePts * kBakeCh;
 #pragma unroll
     for (int k = 0; k < 8; ++k)
-      v = fmaf(corner_weight(f, k), baked_ld(base + (16 / (int)sizeof(V)) * corner_offset<V>(l, k)), v);
+      v = fmaf(corner_weight(f, k), baked_ld(base + (16 / (int)sizeof(V)) * corner_offset<V>(l, k), dq), v);
   }
   return v;
 }
@@ -266,7 +298,9 @@ template <typename V>
 __global__ void __launch_bounds__(kBakedWarps * 32)
 baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values,
                     int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
-                    float stop_t, float* __restrict__ out) {
+                    float stop_t, float* __restrict__ out, const float* __restrict__ dequant_tab) {
+  __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
+  stage_dequant<V>(dequant_tab, dq);
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
   if (r >= n_rays) return;
@@ -287,7 +321,7 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
     const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
     if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // q = 1 and w = 0 everywhere: T and the sums stay
     float v[kBakedVals];
-    baked_interp(values, slot, f, l, v);
+    baked_interp(values, dq, slot, f, l, v);
     float rgb[3] = {0.f, 0.f, 0.f};
     if (slot >= 0) baked_colour(use_viewdirs, Y, v, rgb);
     const SampleTerms st = sample_terms(slot >= 0 ? v[0] : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
@@ -369,7 +403,7 @@ baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, con
     const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
     if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // as the forward: T and the prefix stay
     float v[kBakedVals];
-    baked_interp(values, slot, f, l, v);
+    baked_interp(values, nullptr, slot, f, l, v);
     float rgb[3] = {0.f, 0.f, 0.f};
     if (slot >= 0) baked_colour(use_viewdirs, Y, v, rgb);
     const SampleTerms st = sample_terms(slot >= 0 ? v[0] : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
@@ -418,7 +452,10 @@ baked_render_bwd_kernel(const BakedBox B, const int* __restrict__ brick_map, con
 template <typename V>
 __global__ void __launch_bounds__(kBakedWarps * 32)
 baked_max_weight_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values,
-                        const float* __restrict__ rays, int ray_stride, int64_t n_rays, unsigned* __restrict__ max_w) {
+                        const float* __restrict__ rays, int ray_stride, int64_t n_rays, unsigned* __restrict__ max_w,
+                        const float* __restrict__ dequant_tab) {
+  __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
+  stage_dequant<V>(dequant_tab, dq);
   const int lane = threadIdx.x & 31;
   const int64_t r = (int64_t)blockIdx.x * kBakedWarps + (threadIdx.x >> 5);
   if (r >= n_rays) return;
@@ -434,7 +471,7 @@ baked_max_weight_kernel(const BakedBox B, const int* __restrict__ brick_map, con
     int l[3];
     const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
     if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // as the renderer: T stays
-    const float s = baked_interp_sigma(values, slot, f, l);
+    const float s = baked_interp_sigma(values, dq, slot, f, l);
     const SampleTerms st = sample_terms(slot >= 0 ? s : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
     const float Tl = __fmul_rn(T, warp_excl_prod(st.q, lane));
     const float w = __fmul_rn(st.alpha, Tl);
@@ -749,26 +786,39 @@ int check_baked_max_weights(const char* what, const nerfb200_grid_t* box, const 
   return NERFB200_OK;
 }
 
+// the checks every uint8 entry point adds to its fp32 twin's: codes 16-B aligned (a point is two 16-B loads) and a
+// dequant table
+int check_u8_values(const char* what, const void* values, const float* dequant) {
+  if (int rc = check_f16_values(what, values)) return rc;
+  if (!dequant) {
+    set_error("%s: null dequant (a uint8 field needs its [2][28] scales and offsets)", what);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
+}
+
 template <typename V>
 int launch_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
                         int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
-                        int32_t white_background, float stop_transmittance, float* out, void* stream) {
+                        int32_t white_background, float stop_transmittance, float* out, void* stream,
+                        const float* dequant = nullptr) {
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_render_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0,
-      stop_transmittance, out);
+      stop_transmittance, out, dequant);
   count_launch();
   return check_cuda(cudaGetLastError(), what);
 }
 
 template <typename V>
 int launch_baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                             const float* rays, int32_t ray_stride, int64_t n_rays, float* max_w, void* stream) {
+                             const float* rays, int32_t ray_stride, int64_t n_rays, float* max_w, void* stream,
+                             const float* dequant = nullptr) {
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_max_weight_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
-      B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w));
+      B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w), dequant);
   count_launch();
   return check_cuda(cudaGetLastError(), what);
 }
@@ -800,6 +850,19 @@ int32_t nerfb200_baked_render_f16(const nerfb200_grid_t* box, const int32_t* bri
                              ray_stride, n_rays, white_background, stop_transmittance, out, stream);
 }
 
+int32_t nerfb200_baked_render_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                 const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
+                                 int64_t n_rays, int32_t white_background, float stop_transmittance, float* out,
+                                 void* stream) {
+  const char *what = "baked_render_u8", *launch = "baked_render_u8 launch";
+  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                                  stop_transmittance, out))
+    return rc;
+  if (int rc = check_u8_values(what, values, dequant)) return rc;
+  return launch_baked_render(launch, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, white_background,
+                             stop_transmittance, out, stream, dequant);
+}
+
 int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                                    int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                    float* max_w, void* stream) {
@@ -818,6 +881,16 @@ int32_t nerfb200_baked_max_weights_f16(const nerfb200_grid_t* box, const int32_t
   if (int rc = check_f16_values(what, values)) return rc;
   return launch_baked_max_weights(launch, box, brick_map, reinterpret_cast<const __half*>(values), rays, ray_stride,
                                   n_rays, max_w, stream);
+}
+
+int32_t nerfb200_baked_max_weights_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                      const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
+                                      int64_t n_rays, float* max_w, void* stream) {
+  const char *what = "baked_max_weights_u8", *launch = "baked_max_weights_u8 launch";
+  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
+    return rc;
+  if (int rc = check_u8_values(what, values, dequant)) return rc;
+  return launch_baked_max_weights(launch, box, brick_map, values, rays, ray_stride, n_rays, max_w, stream, dequant);
 }
 
 int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
@@ -1045,29 +1118,30 @@ __device__ __forceinline__ bool edge_of_key(const Lattice& L, int64_t key, int q
 // sigma_raw at lattice point q, read at its canonical copy; 0 (the renderer's miss) when no active brick holds q
 template <typename V>
 __device__ __forceinline__ float lattice_sigma(const BakedBox& B, const int* __restrict__ brick_map,
-                                               const V* __restrict__ values, const int q[3]) {
+                                               const V* __restrict__ values, const float* dq, const int q[3]) {
   const int64_t cp = canonical_copy(B, brick_map, q);
-  return cp < 0 ? 0.f : baked_ld(values + cp);
+  return cp < 0 ? 0.f : baked_ld(values + cp, dq);
 }
 
 // mesh_emit's gradient at lattice point q over sigma_raw at canonical copies (central differences, one-sided at the
 // lattice's faces)
 template <typename V>
 __device__ __forceinline__ void lattice_grad(const BakedBox& B, const Lattice& L, const int* __restrict__ brick_map,
-                                             const V* __restrict__ values, const int q[3], float g[3]) {
+                                             const V* __restrict__ values, const float* dq, const int q[3],
+                                             float g[3]) {
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const int lo = q[c] > 0 ? q[c] - 1 : 0, hi = q[c] < L.res[c] ? q[c] + 1 : L.res[c];
     int ph[3] = {q[0], q[1], q[2]}, pl[3] = {q[0], q[1], q[2]};
     ph[c] = hi;
     pl[c] = lo;
-    g[c] = grad_component(L, c, lattice_sigma(B, brick_map, values, ph), lattice_sigma(B, brick_map, values, pl), hi,
-                          lo);
+    g[c] = grad_component(L, c, lattice_sigma(B, brick_map, values, dq, ph),
+                          lattice_sigma(B, brick_map, values, dq, pl), hi, lo);
   }
 }
 
-// channels 0 .. 27 of one stored point, widened exactly to fp32
-__device__ __forceinline__ void baked_point(const float* __restrict__ p, float a[kBakedVals]) {
+// channels 0 .. 27 of one stored point, widened exactly to fp32 (dequantised with dq for uint8)
+__device__ __forceinline__ void baked_point(const float* __restrict__ p, const float*, float a[kBakedVals]) {
   const float4* p4 = reinterpret_cast<const float4*>(p);
 #pragma unroll
   for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
@@ -1078,7 +1152,7 @@ __device__ __forceinline__ void baked_point(const float* __restrict__ p, float a
     a[4 * c4 + 3] = u.w;
   }
 }
-__device__ __forceinline__ void baked_point(const __half* __restrict__ p, float a[kBakedVals]) {
+__device__ __forceinline__ void baked_point(const __half* __restrict__ p, const float*, float a[kBakedVals]) {
   const uint4* p4 = reinterpret_cast<const uint4*>(p);
 #pragma unroll
   for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {
@@ -1089,6 +1163,12 @@ __device__ __forceinline__ void baked_point(const __half* __restrict__ p, float 
   const uint2 u = __ldg(reinterpret_cast<const uint2*>(p4 + kBakedVals / 8));
   widen4(u.x, u.y, a + 24);
 }
+__device__ __forceinline__ void baked_point(const uint8_t* __restrict__ p, const float* dq, float a[kBakedVals]) {
+  const uint4* p4 = reinterpret_cast<const uint4*>(p);
+  const uint4 u0 = __ldg(p4), u1 = __ldg(p4 + 1);
+  const unsigned wd[kBakedVals / 4] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z};
+  dequant28(wd, dq, a);
+}
 
 // One thread per vertex: t on the edge's sigma_raw, the endpoints' gradients, the view direction and (normals may be
 // NULL) the outward normal, -dir or 0 where the direction fell back.  NaN for a key off the lattice or an endpoint no
@@ -1097,7 +1177,9 @@ template <typename V>
 __global__ void __launch_bounds__(kMeshAttrThreads)
 baked_mesh_dirs_kernel(const BakedBox B, const Lattice L, const int* __restrict__ brick_map,
                        const V* __restrict__ values, float level, const int64_t* __restrict__ keys, int64_t n,
-                       float* __restrict__ dirs, float* __restrict__ normals) {
+                       float* __restrict__ dirs, float* __restrict__ normals, const float* __restrict__ dequant_tab) {
+  __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
+  stage_dequant<V>(dequant_tab, dq);
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   float d[3] = {NAN, NAN, NAN}, nrm[3] = {NAN, NAN, NAN};
@@ -1106,10 +1188,10 @@ baked_mesh_dirs_kernel(const BakedBox B, const Lattice L, const int* __restrict_
     const int q1[3] = {q[0] + (a == 0), q[1] + (a == 1), q[2] + (a == 2)};  // a compared, not indexed: registers
     const int64_t c0 = canonical_copy(B, brick_map, q), c1 = canonical_copy(B, brick_map, q1);
     if (c0 >= 0 && c1 >= 0) {
-      const float t = edge_t(level, baked_ld(values + c0), baked_ld(values + c1));
+      const float t = edge_t(level, baked_ld(values + c0, dq), baked_ld(values + c1, dq));
       float g0[3], g1[3];
-      lattice_grad(B, L, brick_map, values, q, g0);
-      lattice_grad(B, L, brick_map, values, q1, g1);
+      lattice_grad(B, L, brick_map, values, dq, q, g0);
+      lattice_grad(B, L, brick_map, values, dq, q1, g1);
       const bool ok = edge_dir(g0, g1, t, d);
 #pragma unroll
       for (int c = 0; c < 3; ++c) nrm[c] = ok ? -d[c] : 0.f;
@@ -1131,7 +1213,9 @@ __global__ void __launch_bounds__(kMeshAttrThreads)
 baked_mesh_colors_kernel(const BakedBox B, const Lattice L, const int* __restrict__ brick_map,
                          const V* __restrict__ values, int use_viewdirs, float level,
                          const int64_t* __restrict__ keys, const float* __restrict__ dirs, int64_t n,
-                         float* __restrict__ colors) {
+                         float* __restrict__ colors, const float* __restrict__ dequant_tab) {
+  __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
+  stage_dequant<V>(dequant_tab, dq);
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
   float rgb[3] = {NAN, NAN, NAN};
@@ -1141,8 +1225,8 @@ baked_mesh_colors_kernel(const BakedBox B, const Lattice L, const int* __restric
     const int64_t c0 = canonical_copy(B, brick_map, q), c1 = canonical_copy(B, brick_map, q1);
     if (c0 >= 0 && c1 >= 0) {
       float v0[kBakedVals], v1[kBakedVals], v[kBakedVals];
-      baked_point(values + c0, v0);
-      baked_point(values + c1, v1);
+      baked_point(values + c0, dq, v0);
+      baked_point(values + c1, dq, v1);
       const float t = edge_t(level, v0[0], v1[0]), u = __fsub_rn(1.0f, t);
 #pragma unroll
       for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(t, v1[ch], fmaf(u, v0[ch], 0.f));
@@ -1173,12 +1257,12 @@ int check_baked_mesh(const char* what, const nerfb200_grid_t* box, const int32_t
 template <typename V>
 int launch_baked_mesh_dirs(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
                            float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs, float* normals,
-                           void* stream) {
+                           void* stream, const float* dequant = nullptr) {
   if (n_vertices == 0) return NERFB200_OK;
   baked_mesh_dirs_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads, 0,
                               static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
                                                                    values, level, edge_keys, n_vertices, dirs,
-                                                                   normals);
+                                                                   normals, dequant);
   count_launch();
   return check_cuda(cudaGetLastError(), what);
 }
@@ -1186,12 +1270,12 @@ int launch_baked_mesh_dirs(const char* what, const nerfb200_grid_t* box, const i
 template <typename V>
 int launch_baked_mesh_colors(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
                              int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
-                             int64_t n_vertices, float* colors, void* stream) {
+                             int64_t n_vertices, float* colors, void* stream, const float* dequant = nullptr) {
   if (n_vertices == 0) return NERFB200_OK;
   baked_mesh_colors_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads,
                                 0, static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
                                                                         values, use_viewdirs ? 1 : 0, level, edge_keys,
-                                                                        dirs, n_vertices, colors);
+                                                                        dirs, n_vertices, colors, dequant);
   count_launch();
   return check_cuda(cudaGetLastError(), what);
 }
@@ -1246,6 +1330,30 @@ int32_t nerfb200_baked_mesh_colors_f16(const nerfb200_grid_t* box, const int32_t
   return launch_baked_mesh_colors("baked_mesh_colors_f16 launch", box, brick_map,
                                   reinterpret_cast<const __half*>(values), use_viewdirs, level, edge_keys, dirs,
                                   n_vertices, colors, stream);
+}
+
+int32_t nerfb200_baked_mesh_dirs_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                    const float* dequant, float level, const int64_t* edge_keys, int64_t n_vertices,
+                                    float* dirs, float* normals, void* stream) {
+  const char* what = "baked_mesh_dirs_u8";
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, dirs)) return rc;
+  if (int rc = check_u8_values(what, values, dequant)) return rc;
+  return launch_baked_mesh_dirs("baked_mesh_dirs_u8 launch", box, brick_map, values, level, edge_keys, n_vertices,
+                                dirs, normals, stream, dequant);
+}
+
+int32_t nerfb200_baked_mesh_colors_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                      const float* dequant, int32_t use_viewdirs, float level, const int64_t* edge_keys,
+                                      const float* dirs, int64_t n_vertices, float* colors, void* stream) {
+  const char* what = "baked_mesh_colors_u8";
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
+  if (use_viewdirs && !dirs) {
+    set_error("%s: view directions need dirs", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (int rc = check_u8_values(what, values, dequant)) return rc;
+  return launch_baked_mesh_colors("baked_mesh_colors_u8 launch", box, brick_map, values, use_viewdirs, level,
+                                  edge_keys, dirs, n_vertices, colors, stream, dequant);
 }
 
 }  // extern "C"

@@ -985,21 +985,32 @@ def bake_refusal(arch: ArchSpec) -> Optional[str]:
     return lib.nerfb200_last_error().decode(errors="replace")
 
 
-def _baked_values(values, what):
-    """(entry point suffix, pointer) of baked ``values``: "" for fp32, "_f16" for fp16 (include/nerfb200.h "baked
-    fields: half precision"); any other dtype is refused."""
+def _baked_values(values, what, dequant=None):
+    """(entry point suffix, the values' leading arguments) of baked ``values``: "" and (pointer,) for fp32, "_f16" and
+    (pointer,) for fp16 (include/nerfb200.h "baked fields: half precision"), "_u8" and (codes, ``dequant``) for uint8
+    codes, whose ``dequant`` must be their fp32 (2, 28) table on the same device (include/nerfb200.h "baked fields:
+    8-bit values"); any other dtype is refused."""
     if values.dtype == torch.float32:
-        return "", _ptr(values)
+        return "", (_ptr(values),)
     if values.dtype == torch.float16:
-        return "_f16", _ptr(values.view(torch.uint8))  # _ptr takes no fp16; the pointer is the same
-    raise ValueError(f"nerfb200 {what}: baked values must be fp32 or fp16, got {values.dtype}")
+        return "_f16", (_ptr(values.view(torch.uint8)),)  # _ptr takes no fp16; the pointer is the same
+    if values.dtype == torch.uint8:
+        if not (isinstance(dequant, torch.Tensor) and dequant.dtype == torch.float32 and dequant.shape == (2, 28)
+                and dequant.device == values.device):
+            raise ValueError(f"nerfb200 {what}: uint8 baked values need their dequant, an fp32 (2, 28) tensor on "
+                             f"{values.device}")
+        return "_u8", (_ptr(values), _ptr(dequant))
+    raise ValueError(f"nerfb200 {what}: baked values must be fp32 or fp16, or uint8 with their dequant, got "
+                     f"{values.dtype}")
 
 
 def bake(arch: ArchSpec, blob, box: Grid, bricks, first: int, count: int, values, logits=None):
     """The values of slots first .. first + count - 1 into ``values`` (n_active, 729, 32), fp32 or fp16 (the conversion
     rule at the store); ``logits`` (count * 729, 64, 3) fp32 or None receives the network's rgb logits at the 64
     directions (a test hook)."""
-    sfx, pv = _baked_values(values, "bake")
+    if values.dtype == torch.uint8:
+        raise ValueError("nerfb200 bake: a bake writes fp32 or fp16 values; quantise the baked field afterwards")
+    sfx, (pv,) = _baked_values(values, "bake")
     _lib.check(getattr(_lib.load(), "nerfb200_bake" + sfx)(C.byref(arch.c_struct()), _ptr(blob), C.byref(box),
                                                            _ptr(bricks), int(first), int(count), pv, _ptr(logits),
                                                            _stream()), "bake" + sfx)
@@ -1007,14 +1018,14 @@ def bake(arch: ArchSpec, blob, box: Grid, bricks, first: int, count: int, values
 
 
 def baked_render(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool,
-                 stop_transmittance: float = 0.0, out=None) -> torch.Tensor:
+                 stop_transmittance: float = 0.0, out=None, dequant=None) -> torch.Tensor:
     """Rows (n, 8) = [r g b disp acc depth 0 0] of the packed ``rays`` through a baked field whose ``values`` are fp32
-    or fp16."""
-    sfx, pv = _baked_values(values, "baked_render")
+    or fp16, or uint8 codes with their ``dequant`` table."""
+    sfx, pv = _baked_values(values, "baked_render", dequant)
     n = rays.shape[0]
     out = torch.empty(n, 8, dtype=torch.float32, device=rays.device) if out is None else out
     _lib.check(getattr(_lib.load(), "nerfb200_baked_render" + sfx)(
-        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], n,
+        C.byref(box), _ptr(brick_map), *pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], n,
         int(bool(white_background)), float(stop_transmittance), _ptr(out), _stream()), "baked_render" + sfx)
     return out
 
@@ -1039,13 +1050,13 @@ def baked_tie(box: Grid, brick_map, bricks, d_values, d_tied=None):
     return d_tied
 
 
-def baked_max_weights(box: Grid, brick_map, values, use_viewdirs: bool, rays, max_w):
+def baked_max_weights(box: Grid, brick_map, values, use_viewdirs: bool, rays, max_w, dequant=None):
     """Max-accumulates into ``max_w`` fp32[n_active] each brick slot's largest rendering weight over the packed
     ``rays`` (``baked_render``'s weights at stop 0; a NaN weight as +inf).  Zero ``max_w`` once before the first
-    chunk.  ``values`` fp32 or fp16."""
-    sfx, pv = _baked_values(values, "baked_max_weights")
+    chunk.  ``values`` fp32 or fp16, or uint8 codes with their ``dequant`` table."""
+    sfx, pv = _baked_values(values, "baked_max_weights", dequant)
     _lib.check(getattr(_lib.load(), "nerfb200_baked_max_weights" + sfx)(
-        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], rays.shape[0],
+        C.byref(box), _ptr(brick_map), *pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], rays.shape[0],
         _ptr(max_w), _stream()), "baked_max_weights" + sfx)
     return max_w
 
@@ -1093,27 +1104,29 @@ def baked_subdivide(box: Grid, brick_map, values, child_bricks, child_values):
     return child_values
 
 
-def baked_mesh_dirs(box: Grid, brick_map, values, level: float, edge_keys, want_normals: bool = False):
+def baked_mesh_dirs(box: Grid, brick_map, values, level: float, edge_keys, want_normals: bool = False, dequant=None):
     """(dirs (V, 3), normals (V, 3) or None) of the vertices whose lattice edges are ``edge_keys`` int64 (V,) on a baked
-    field's fp32 or fp16 ``values`` (include/nerfb200.h "baked fields: meshes"): the view direction -n and the outward
-    normal n (0 where the direction fell back)."""
-    sfx, pv = _baked_values(values, "baked_mesh_dirs")
+    field's fp32 or fp16 ``values``, or uint8 codes with their ``dequant`` table (include/nerfb200.h "baked fields:
+    meshes"): the view direction -n and the outward normal n (0 where the direction fell back)."""
+    sfx, pv = _baked_values(values, "baked_mesh_dirs", dequant)
     n = edge_keys.shape[0]
     dirs = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device)
     normals = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device) if want_normals else None
     _lib.check(getattr(_lib.load(), "nerfb200_baked_mesh_dirs" + sfx)(
-        C.byref(box), _ptr(brick_map), pv, float(level), _ptr(edge_keys), n, _ptr(dirs), _ptr(normals), _stream()),
+        C.byref(box), _ptr(brick_map), *pv, float(level), _ptr(edge_keys), n, _ptr(dirs), _ptr(normals), _stream()),
         "baked_mesh_dirs" + sfx)
     return dirs, normals
 
 
-def baked_mesh_colors(box: Grid, brick_map, values, use_viewdirs: bool, level: float, edge_keys, dirs=None):
+def baked_mesh_colors(box: Grid, brick_map, values, use_viewdirs: bool, level: float, edge_keys, dirs=None,
+                      dequant=None):
     """colors (V, 3) of the vertices whose lattice edges are ``edge_keys`` int64 (V,) on a baked field's fp32 or fp16
-    ``values``, seen along ``dirs`` (V, 3) with view directions (include/nerfb200.h "baked fields: meshes")."""
-    sfx, pv = _baked_values(values, "baked_mesh_colors")
+    ``values``, or uint8 codes with their ``dequant`` table, seen along ``dirs`` (V, 3) with view directions
+    (include/nerfb200.h "baked fields: meshes")."""
+    sfx, pv = _baked_values(values, "baked_mesh_colors", dequant)
     n = edge_keys.shape[0]
     colors = torch.empty(n, 3, dtype=torch.float32, device=edge_keys.device)
     _lib.check(getattr(_lib.load(), "nerfb200_baked_mesh_colors" + sfx)(
-        C.byref(box), _ptr(brick_map), pv, int(bool(use_viewdirs)), float(level), _ptr(edge_keys), _ptr(dirs), n,
+        C.byref(box), _ptr(brick_map), *pv, int(bool(use_viewdirs)), float(level), _ptr(edge_keys), _ptr(dirs), n,
         _ptr(colors), _stream()), "baked_mesh_colors" + sfx)
     return colors
