@@ -26,6 +26,21 @@ import torch
 
 from . import ops
 
+_LOSSY = {torch.float16: ("an fp16 field", "convert it back with .half()"),
+          torch.uint8: ("an 8-bit field", "quantise it again with .quantize()")}
+
+
+def _lossy_refusal(what, dtype, lacks, fix="fine-tune field.float() and {back}"):
+    """The ValueError of ``what`` for a ``dtype`` field, which has no ``lacks``; ``fix`` may name its way ``{back}``."""
+    name, back = _LOSSY[dtype]
+    return ValueError(f"{what}: {name} has no {lacks}; {fix.format(back=back)}")
+
+
+def _widened(field, rows, ch):
+    """fp32 channels ``ch`` of slots ``rows``, 8-bit codes dequantised as the kernels read them: q.float() * s + o."""
+    v = field.values.detach()[rows, :, ch].float()
+    return v * field.dequant[0, ch] + field.dequant[1, ch] if field.dtype == torch.uint8 else v
+
 
 class BakedField:
     """A baked field on the device: ``bounds`` ((lo), (hi)) and ``resolution`` (three ints) of the lattice box,
@@ -84,7 +99,7 @@ class BakedField:
         if chunk < 1:
             raise ValueError(f"BakedField.half: chunk must be >= 1, got {chunk}")
         if self.dtype == torch.uint8:
-            raise ValueError("BakedField.half: the field is 8-bit; dequantise it with .float() first")
+            raise _lossy_refusal("BakedField.half", self.dtype, "fp16 conversion", "dequantise it with .float() first")
         v = self.values.detach()
         out = torch.empty(v.shape, dtype=torch.float16, device=v.device)
         for s in range(0, self.n_active, chunk):
@@ -107,7 +122,8 @@ class BakedField:
         if chunk < 1:
             raise ValueError(f"BakedField.quantize: chunk must be >= 1, got {chunk}")
         if self.dtype == torch.uint8:
-            raise ValueError("BakedField.quantize: the field is already 8-bit; dequantise it with .float() first")
+            raise _lossy_refusal("BakedField.quantize", self.dtype, "requantisation",
+                                 "dequantise it with .float() first")
         v = self.values.detach()
         lo = torch.zeros(28, dtype=torch.float32, device=v.device)
         hi = torch.zeros(28, dtype=torch.float32, device=v.device)
@@ -137,12 +153,12 @@ class BakedField:
         field's own values tensor.  ``brick_map`` and ``bricks`` are shared.  Fine-tune ``field.float()``, then convert
         back with ``half()`` or ``quantize()``."""
         if self.values.dtype == torch.uint8:
-            q, chunk = self.values.detach(), int(chunk)
+            chunk = int(chunk)
             if chunk < 1:
                 raise ValueError(f"BakedField.float: chunk must be >= 1, got {chunk}")
-            v = torch.zeros(q.shape, dtype=torch.float32, device=q.device)
+            v = torch.zeros(self.values.shape, dtype=torch.float32, device=self.values.device)
             for s in range(0, self.n_active, chunk):
-                v[s:s + chunk, :, :28] = q[s:s + chunk, :, :28].float() * self.dequant[0] + self.dequant[1]
+                v[s:s + chunk, :, :28] = _widened(self, slice(s, s + chunk), slice(0, 28))
         else:
             v = self.values if self.values.dtype == torch.float32 else self.values.detach().float()
         return BakedField(self.bounds, self.resolution, self.brick_map, self.bricks, v, self.use_viewdirs)
@@ -243,17 +259,12 @@ def _pose_rays(field, height, width, focal_length, tform_cam2world, options):
                         use_viewdirs=field.use_viewdirs)
 
 
-def _check_values(field, what, half=False):
-    """A CUDA field with fp32 values, or fp16 or 8-bit ones where ``half`` (renders and peak weights; fine-tuning is
-    fp32 only)."""
+def _check_values(field, what, stored=False):
+    """A CUDA fp32 field, or one in any storage format where ``stored`` (renders, peak weights); fine-tuning is fp32."""
     if not isinstance(field, BakedField):
         raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
-    if isinstance(field.values, torch.Tensor) and field.values.dtype == torch.float16 and not half:
-        raise ValueError(f"{what}: an fp16 field has no gradient or fine-tuning path; fine-tune field.float() and "
-                         f"convert it back with .half()")
-    if isinstance(field.values, torch.Tensor) and field.values.dtype == torch.uint8 and not half:
-        raise ValueError(f"{what}: an 8-bit field has no gradient or fine-tuning path; fine-tune field.float() and "
-                         f"quantise it again with .quantize()")
+    if not stored and getattr(field.values, "dtype", None) in _LOSSY:
+        raise _lossy_refusal(what, field.values.dtype, "gradient or fine-tuning path")
     if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda
             and field.values.dtype in (torch.float32, torch.float16, torch.uint8)):
         raise ValueError(f"{what}: field.values must be an fp32, fp16 or uint8 CUDA tensor (there is no CPU path)")
@@ -293,14 +304,11 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
     render, which refuses such a field in grad mode as it did before fp16 fields could be rendered at all; under
     ``torch.no_grad()`` (or inference mode) it renders one whose values do not require grad.  Anything else raises
     ValueError (fine-tune ``field.float()``).  ``render_baked`` renders fp16 and 8-bit fields in any grad mode."""
-    _check_values(field, "render_baked_rays", half=True)
+    _check_values(field, "render_baked_rays", stored=True)
     # grad mode alone keeps the refusal every fp16 field met here before half precision (pinned by the fine-tuning tests)
-    if field.values.dtype == torch.float16 and (field.values.requires_grad or torch.is_grad_enabled()):
-        raise ValueError("render_baked_rays: an fp16 field has no gradient; render it under torch.no_grad(), or "
-                         "fine-tune field.float() and convert it back with .half()")
-    if field.values.dtype == torch.uint8 and torch.is_grad_enabled():
-        raise ValueError("render_baked_rays: an 8-bit field has no gradient; render it under torch.no_grad(), or "
-                         "fine-tune field.float() and quantise it again with .quantize()")
+    if field.dtype in _LOSSY and (field.values.requires_grad or torch.is_grad_enabled()):
+        raise _lossy_refusal("render_baked_rays", field.dtype, "gradient",
+                             "render it under torch.no_grad(), or fine-tune field.float() and {back}")
     stride = 11 if field.use_viewdirs else 8
     if not (isinstance(rays, torch.Tensor) and rays.dim() == 2 and rays.shape[1] == stride):
         raise ValueError(f"render_baked_rays: rays must be (N, {stride}) for a field "
@@ -562,12 +570,9 @@ def baked_transparent_bricks(field: BakedField, chunk: int = 1024) -> torch.Tens
     v = field.values.detach()
     out = torch.empty(field.n_active, dtype=torch.bool, device=v.device)
     for s in range(0, field.n_active, chunk):
-        if v.dtype == torch.uint8:
-            sigma = v[s:s + chunk, :, 0].float() * field.dequant[0, 0] + field.dequant[1, 0]
-            out[s:s + chunk] = (sigma <= 0).all(1)
-            continue
-        c = v[s:s + chunk, :, :28]
-        out[s:s + chunk] = (c[..., 0] <= 0).all(1) & torch.isfinite(c).flatten(1).all(1)
+        out[s:s + chunk] = (_widened(field, slice(s, s + chunk), 0) <= 0).all(1)
+        if v.dtype != torch.uint8:  # codes dequantise to finite values
+            out[s:s + chunk] &= torch.isfinite(v[s:s + chunk, :, :28]).flatten(1).all(1)
     return out
 
 
@@ -587,7 +592,7 @@ def baked_brick_weights_rays(field: BakedField, rays, out=None) -> torch.Tensor:
     if out is not None and not (isinstance(out, torch.Tensor) and out.dtype == torch.float32
                                 and out.shape == (field.n_active,) and out.is_contiguous()):
         raise ValueError(f"baked_brick_weights_rays: out must be a contiguous fp32 tensor of shape ({field.n_active},)")
-    _check_values(field, "baked_brick_weights_rays", half=True)
+    _check_values(field, "baked_brick_weights_rays", stored=True)
     dev = field.values.device
     if rays.device != dev or (out is not None and out.device != dev):
         raise ValueError(f"baked_brick_weights_rays: rays and out must be on the field's device {dev}")
@@ -612,7 +617,7 @@ def baked_brick_weights(field: BakedField, poses, height, width, focal_length, o
         raise ValueError("baked_brick_weights: poses must be a float tensor (n, 3 | 4, 4) with n >= 1")
     if not (int(height) > 0 and int(width) > 0):
         raise ValueError(f"baked_brick_weights: need height, width > 0, got {height}, {width}")
-    _check_values(field, "baked_brick_weights", half=True)
+    _check_values(field, "baked_brick_weights", stored=True)
     _check_viewdirs(field, options, "baked_brick_weights")
     out = torch.zeros(field.n_active, dtype=torch.float32, device=field.values.device)
     if field.n_active == 0:
@@ -633,12 +638,8 @@ def _check_subdivide(field, what):
     otherwise)."""
     if not isinstance(field, BakedField):
         raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
-    if field.values.dtype == torch.float16:
-        raise ValueError(f"{what}: an fp16 field has no subdivision; subdivide field.float() and convert it back "
-                         f"with .half()")
-    if field.values.dtype == torch.uint8:
-        raise ValueError(f"{what}: an 8-bit field has no subdivision; subdivide field.float() and quantise it again "
-                         f"with .quantize()")
+    if field.dtype in _LOSSY:
+        raise _lossy_refusal(what, field.dtype, "subdivision", "subdivide field.float() and {back}")
     if not all(r <= 2048 for r in field.resolution):
         raise ValueError(f"{what}: resolution {field.resolution} is past 2048 on an axis (the child would pass 4096)")
     if not (field.values.is_cuda and field.values.dtype == torch.float32):
@@ -739,9 +740,7 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
     box = field.box()
     values = values.detach()
     with torch.no_grad():
-        sigma = values[..., 0].float().contiguous()  # (n_active, 729): the halo-0 sparse layout
-        if values.dtype == torch.uint8:
-            sigma = sigma * field.dequant[0, 0] + field.dequant[1, 0]
+        sigma = _widened(field, slice(None), 0).contiguous()  # (n_active, 729): the halo-0 sparse layout
         totals, ws = ops.mesh_sparse_count(box, field.brick_map, field.bricks, field.n_active, sigma, False, level)
         n_v, n_f = (int(t) for t in totals.tolist())  # the one host sync: the outputs' sizes
         if n_v == 0:

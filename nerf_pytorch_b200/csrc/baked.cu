@@ -82,6 +82,28 @@ int check_f16_values(const char* what, const void* values) {
 
 namespace {
 
+// the check a field's storage format adds to an entry point's own (what: the entry point's name in the error): none
+// for fp32; fp16 values and uint8 codes 16-B aligned, as the vector gathers need; and a dequant table for uint8
+template <typename V>
+int check_values(const char* what, const V* values, const float* dequant) {
+  if (sizeof(V) == 4) return NERFB200_OK;
+  if (int rc = check_f16_values(what, values)) return rc;
+  if (sizeof(V) == 1 && !dequant) {
+    set_error("%s: null dequant (a uint8 field needs its [2][28] scales and offsets)", what);
+    return NERFB200_ERR_INVALID;
+  }
+  return NERFB200_OK;
+}
+
+// counts the launch entry point what just made and checks it; a failure reads "<what> launch: <CUDA error>"
+int check_launch(const char* what) {
+  count_launch();
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) return NERFB200_OK;
+  set_error("%s launch: %s", what, cudaGetErrorString(e));
+  return NERFB200_ERR_CUDA;
+}
+
 constexpr int kBakedWarps = 4;
 constexpr int kBakedVals = 1 + 3 * kBakeSh;  // interpolated channels: sigma_raw and the 27 coefficients
 static_assert(kBakedVals == 28, "seven float4 per corner point");
@@ -191,12 +213,6 @@ __device__ __forceinline__ float dequant(unsigned q, const float* dq, int ch) {
   return __fadd_rn(__fmul_rn((float)q, dq[ch]), dq[kBakedVals + ch]);
 }
 
-// channels 0 .. 27 of the 28 code bytes in w[0 .. 6], dequantised
-__device__ __forceinline__ void dequant28(const unsigned w[kBakedVals / 4], const float* dq, float a[kBakedVals]) {
-#pragma unroll
-  for (int ch = 0; ch < kBakedVals; ++ch) a[ch] = dequant((w[ch >> 2] >> (8 * (ch & 3))) & 0xffu, dq, ch);
-}
-
 // a uint8 field's dequant table copied into the CTA's shared memory dq_s; every thread of the CTA must call it before
 // any returns.  Nothing for fp32 and fp16 fields
 template <typename V>
@@ -214,9 +230,52 @@ __device__ __forceinline__ float baked_ld(const __half* p, const float*) {
 }
 __device__ __forceinline__ float baked_ld(const uint8_t* p, const float* dq) { return dequant(__ldg(p), dq, 0); }
 
-// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0).  fp32: seven 16-B loads per corner; fp16:
-// three 16-B loads and one 8-B load (56 of the point's 64 B), each value widened exactly; uint8: two 16-B loads (the
-// point's one 32-B sector), each code dequantised with dq; then the same fmaf chain
+// channels 0 .. 27 of the stored point off16 16-B vectors past base, widened exactly to fp32 and handed to put(ch, x):
+// the one reader of a format's layout.  fp32: seven 16-B loads, each vector put before the next load (loading all seven
+// first reschedules the fp32 renderer and its backward); fp16: three 16-B loads and one 8-B load (56 of the point's
+// 64 B), each value widened exactly; uint8: two 16-B loads (the point's one 32-B sector), each code dequantised with dq
+// (read for uint8 only)
+template <typename Put>
+__device__ __forceinline__ void baked_point(const float* base, int off16, const float*, Put&& put) {
+  const float4* p4 = reinterpret_cast<const float4*>(base) + off16;
+#pragma unroll
+  for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
+    const float4 u = __ldg(p4 + c4);
+    put(4 * c4, u.x);
+    put(4 * c4 + 1, u.y);
+    put(4 * c4 + 2, u.z);
+    put(4 * c4 + 3, u.w);
+  }
+}
+template <typename Put>
+__device__ __forceinline__ void baked_point(const __half* base, int off16, const float*, Put&& put) {
+  const uint4* p4 = reinterpret_cast<const uint4*>(base) + off16;
+  float a[kBakedVals];
+#pragma unroll
+  for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {  // channels 0 .. 23
+    const uint4 u = __ldg(p4 + c8);
+    widen4(u.x, u.y, a + 8 * c8);
+    widen4(u.z, u.w, a + 8 * c8 + 4);
+  }
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p4 + kBakedVals / 8));  // channels 24 .. 27
+  widen4(u.x, u.y, a + 24);
+#pragma unroll
+  for (int ch = 0; ch < kBakedVals; ++ch) put(ch, a[ch]);
+}
+template <typename Put>
+__device__ __forceinline__ void baked_point(const uint8_t* base, int off16, const float* dq, Put&& put) {
+  const uint4* p4 = reinterpret_cast<const uint4*>(base) + off16;
+  const uint4 u0 = __ldg(p4), u1 = __ldg(p4 + 1);  // channels 28 .. 31 (u1.w) are not read
+  const unsigned w[kBakedVals / 4] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z};
+  float a[kBakedVals];
+#pragma unroll
+  for (int ch = 0; ch < kBakedVals; ++ch) a[ch] = dequant((w[ch >> 2] >> (8 * (ch & 3))) & 0xffu, dq, ch);
+#pragma unroll
+  for (int ch = 0; ch < kBakedVals; ++ch) put(ch, a[ch]);
+}
+
+// channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0): each corner's point from baked_point into
+// the same fmaf chain for every format
 template <typename V>
 __device__ __forceinline__ void baked_interp(const V* __restrict__ values, const float* dq, int slot, const float f[3],
                                              const int l[3], float v[kBakedVals]) {
@@ -227,38 +286,7 @@ __device__ __forceinline__ void baked_interp(const V* __restrict__ values, const
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const float w = corner_weight(f, k);
-      if constexpr (sizeof(V) == 4) {
-        const float4* pv = reinterpret_cast<const float4*>(sv) + corner_offset<V>(l, k);
-#pragma unroll
-        for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
-          const float4 a = __ldg(pv + c4);
-          v[4 * c4] = fmaf(w, a.x, v[4 * c4]);
-          v[4 * c4 + 1] = fmaf(w, a.y, v[4 * c4 + 1]);
-          v[4 * c4 + 2] = fmaf(w, a.z, v[4 * c4 + 2]);
-          v[4 * c4 + 3] = fmaf(w, a.w, v[4 * c4 + 3]);
-        }
-      } else if constexpr (sizeof(V) == 1) {
-        const uint4* pv = reinterpret_cast<const uint4*>(sv) + corner_offset<V>(l, k);
-        const uint4 u0 = __ldg(pv), u1 = __ldg(pv + 1);  // channels 28 .. 31 (u1.w) are not read
-        const unsigned wd[kBakedVals / 4] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z};
-        float a[kBakedVals];
-        dequant28(wd, dq, a);
-#pragma unroll
-        for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(w, a[ch], v[ch]);
-      } else {
-        const uint4* pv = reinterpret_cast<const uint4*>(sv) + corner_offset<V>(l, k);
-        float a[kBakedVals];
-#pragma unroll
-        for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {  // channels 0 .. 23
-          const uint4 u = __ldg(pv + c8);
-          widen4(u.x, u.y, a + 8 * c8);
-          widen4(u.z, u.w, a + 8 * c8 + 4);
-        }
-        const uint2 u = __ldg(reinterpret_cast<const uint2*>(pv + kBakedVals / 8));  // channels 24 .. 27
-        widen4(u.x, u.y, a + 24);
-#pragma unroll
-        for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(w, a[ch], v[ch]);
-      }
+      baked_point(sv, corner_offset<V>(l, k), dq, [&](int ch, float x) { v[ch] = fmaf(w, x, v[ch]); });
     }
   }
 }
@@ -758,10 +786,11 @@ int32_t nerfb200_bake_basis(float* dirs_host, float* proj_host) {
 
 namespace {
 
-// the checks baked_render and baked_render_f16 share (what: the entry point's name in the error)
-int check_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
-                       int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
-                       float stop_transmittance, const float* out) {
+// the renderer's entry points (what: the entry point's name in the errors): its checks, the format's, then the launch
+template <typename V>
+int baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                 int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays, int32_t white_background,
+                 float stop_transmittance, float* out, void* stream, const float* dequant) {
   if (int rc = check_grid(box, what)) return rc;
   if (!brick_map || !values || !rays || !out || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
     set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
@@ -771,56 +800,31 @@ int check_baked_render(const char* what, const nerfb200_grid_t* box, const int32
     set_error("%s: stop_transmittance must lie in [0, 1), got %g", what, (double)stop_transmittance);
     return NERFB200_ERR_INVALID;
   }
-  return NERFB200_OK;
-}
-
-// the checks baked_max_weights and baked_max_weights_f16 share
-int check_baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
-                            int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
-                            const float* max_w) {
-  if (int rc = check_grid(box, what)) return rc;
-  if (!brick_map || !values || !rays || !max_w || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
-    set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
-    return NERFB200_ERR_INVALID;
-  }
-  return NERFB200_OK;
-}
-
-// the checks every uint8 entry point adds to its fp32 twin's: codes 16-B aligned (a point is two 16-B loads) and a
-// dequant table
-int check_u8_values(const char* what, const void* values, const float* dequant) {
-  if (int rc = check_f16_values(what, values)) return rc;
-  if (!dequant) {
-    set_error("%s: null dequant (a uint8 field needs its [2][28] scales and offsets)", what);
-    return NERFB200_ERR_INVALID;
-  }
-  return NERFB200_OK;
-}
-
-template <typename V>
-int launch_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                        int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
-                        int32_t white_background, float stop_transmittance, float* out, void* stream,
-                        const float* dequant = nullptr) {
+  if (int rc = check_values(what, values, dequant)) return rc;
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_render_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0,
       stop_transmittance, out, dequant);
-  count_launch();
-  return check_cuda(cudaGetLastError(), what);
+  return check_launch(what);
 }
 
+// the peak weights' entry points, as baked_render
 template <typename V>
-int launch_baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                             const float* rays, int32_t ray_stride, int64_t n_rays, float* max_w, void* stream,
-                             const float* dequant = nullptr) {
+int baked_max_weights(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                      int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays, float* max_w,
+                      void* stream, const float* dequant) {
+  if (int rc = check_grid(box, what)) return rc;
+  if (!brick_map || !values || !rays || !max_w || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
+    set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
+    return NERFB200_ERR_INVALID;
+  }
+  if (int rc = check_values(what, values, dequant)) return rc;
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_max_weight_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, rays, ray_stride, n_rays, reinterpret_cast<unsigned*>(max_w), dequant);
-  count_launch();
-  return check_cuda(cudaGetLastError(), what);
+  return check_launch(what);
 }
 
 }  // namespace
@@ -830,67 +834,44 @@ extern "C" {
 int32_t nerfb200_baked_render(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                               int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                               int32_t white_background, float stop_transmittance, float* out, void* stream) {
-  const char *what = "baked_render", *launch = "baked_render launch";
-  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
-                                  stop_transmittance, out))
-    return rc;
-  return launch_baked_render(launch, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, white_background,
-                             stop_transmittance, out, stream);
+  return baked_render("baked_render", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, white_background,
+                      stop_transmittance, out, stream, nullptr);
 }
 
 int32_t nerfb200_baked_render_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
                                   int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                   int32_t white_background, float stop_transmittance, float* out, void* stream) {
-  const char *what = "baked_render_f16", *launch = "baked_render_f16 launch";
-  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
-                                  stop_transmittance, out))
-    return rc;
-  if (int rc = check_f16_values(what, values)) return rc;
-  return launch_baked_render(launch, box, brick_map, reinterpret_cast<const __half*>(values), use_viewdirs, rays,
-                             ray_stride, n_rays, white_background, stop_transmittance, out, stream);
+  return baked_render("baked_render_f16", box, brick_map, reinterpret_cast<const __half*>(values), use_viewdirs, rays,
+                      ray_stride, n_rays, white_background, stop_transmittance, out, stream, nullptr);
 }
 
 int32_t nerfb200_baked_render_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
                                  const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
                                  int64_t n_rays, int32_t white_background, float stop_transmittance, float* out,
                                  void* stream) {
-  const char *what = "baked_render_u8", *launch = "baked_render_u8 launch";
-  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
-                                  stop_transmittance, out))
-    return rc;
-  if (int rc = check_u8_values(what, values, dequant)) return rc;
-  return launch_baked_render(launch, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, white_background,
-                             stop_transmittance, out, stream, dequant);
+  return baked_render("baked_render_u8", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                      white_background, stop_transmittance, out, stream, dequant);
 }
 
 int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                                    int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                    float* max_w, void* stream) {
-  const char *what = "baked_max_weights", *launch = "baked_max_weights launch";
-  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
-    return rc;
-  return launch_baked_max_weights(launch, box, brick_map, values, rays, ray_stride, n_rays, max_w, stream);
+  return baked_max_weights("baked_max_weights", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w,
+                           stream, nullptr);
 }
 
 int32_t nerfb200_baked_max_weights_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
                                        int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
                                        float* max_w, void* stream) {
-  const char *what = "baked_max_weights_f16", *launch = "baked_max_weights_f16 launch";
-  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
-    return rc;
-  if (int rc = check_f16_values(what, values)) return rc;
-  return launch_baked_max_weights(launch, box, brick_map, reinterpret_cast<const __half*>(values), rays, ray_stride,
-                                  n_rays, max_w, stream);
+  return baked_max_weights("baked_max_weights_f16", box, brick_map, reinterpret_cast<const __half*>(values),
+                           use_viewdirs, rays, ray_stride, n_rays, max_w, stream, nullptr);
 }
 
 int32_t nerfb200_baked_max_weights_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
                                       const float* dequant, int32_t use_viewdirs, const float* rays, int32_t ray_stride,
                                       int64_t n_rays, float* max_w, void* stream) {
-  const char *what = "baked_max_weights_u8", *launch = "baked_max_weights_u8 launch";
-  if (int rc = check_baked_max_weights(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays, max_w))
-    return rc;
-  if (int rc = check_u8_values(what, values, dequant)) return rc;
-  return launch_baked_max_weights(launch, box, brick_map, values, rays, ray_stride, n_rays, max_w, stream, dequant);
+  return baked_max_weights("baked_max_weights_u8", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                           max_w, stream, dequant);
 }
 
 int32_t nerfb200_baked_render_bwd(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
@@ -1140,36 +1121,6 @@ __device__ __forceinline__ void lattice_grad(const BakedBox& B, const Lattice& L
   }
 }
 
-// channels 0 .. 27 of one stored point, widened exactly to fp32 (dequantised with dq for uint8)
-__device__ __forceinline__ void baked_point(const float* __restrict__ p, const float*, float a[kBakedVals]) {
-  const float4* p4 = reinterpret_cast<const float4*>(p);
-#pragma unroll
-  for (int c4 = 0; c4 < kBakedVals / 4; ++c4) {
-    const float4 u = __ldg(p4 + c4);
-    a[4 * c4] = u.x;
-    a[4 * c4 + 1] = u.y;
-    a[4 * c4 + 2] = u.z;
-    a[4 * c4 + 3] = u.w;
-  }
-}
-__device__ __forceinline__ void baked_point(const __half* __restrict__ p, const float*, float a[kBakedVals]) {
-  const uint4* p4 = reinterpret_cast<const uint4*>(p);
-#pragma unroll
-  for (int c8 = 0; c8 < kBakedVals / 8; ++c8) {
-    const uint4 u = __ldg(p4 + c8);
-    widen4(u.x, u.y, a + 8 * c8);
-    widen4(u.z, u.w, a + 8 * c8 + 4);
-  }
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p4 + kBakedVals / 8));
-  widen4(u.x, u.y, a + 24);
-}
-__device__ __forceinline__ void baked_point(const uint8_t* __restrict__ p, const float* dq, float a[kBakedVals]) {
-  const uint4* p4 = reinterpret_cast<const uint4*>(p);
-  const uint4 u0 = __ldg(p4), u1 = __ldg(p4 + 1);
-  const unsigned wd[kBakedVals / 4] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z};
-  dequant28(wd, dq, a);
-}
-
 // One thread per vertex: t on the edge's sigma_raw, the endpoints' gradients, the view direction and (normals may be
 // NULL) the outward normal, -dir or 0 where the direction fell back.  NaN for a key off the lattice or an endpoint no
 // active brick holds.
@@ -1225,8 +1176,8 @@ baked_mesh_colors_kernel(const BakedBox B, const Lattice L, const int* __restric
     const int64_t c0 = canonical_copy(B, brick_map, q), c1 = canonical_copy(B, brick_map, q1);
     if (c0 >= 0 && c1 >= 0) {
       float v0[kBakedVals], v1[kBakedVals], v[kBakedVals];
-      baked_point(values + c0, dq, v0);
-      baked_point(values + c1, dq, v1);
+      baked_point(values + c0, 0, dq, [&](int ch, float x) { v0[ch] = x; });
+      baked_point(values + c1, 0, dq, [&](int ch, float x) { v1[ch] = x; });
       const float t = edge_t(level, v0[0], v1[0]), u = __fsub_rn(1.0f, t);
 #pragma unroll
       for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = fmaf(t, v1[ch], fmaf(u, v0[ch], 0.f));
@@ -1240,6 +1191,7 @@ baked_mesh_colors_kernel(const BakedBox B, const Lattice L, const int* __restric
   for (int c = 0; c < 3; ++c) colors[3 * i + c] = rgb[c];
 }
 
+// the checks baked_mesh_dirs and baked_mesh_colors share
 int check_baked_mesh(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const void* values,
                      float level, const int64_t* edge_keys, int64_t n_vertices, const void* out) {
   if (int rc = check_grid(box, what)) return rc;
@@ -1254,30 +1206,39 @@ int check_baked_mesh(const char* what, const nerfb200_grid_t* box, const int32_t
   return NERFB200_OK;
 }
 
+// the mesh directions' entry points (what: the entry point's name in the errors): the mesh checks, the format's, then
+// the launch (none for no vertex)
 template <typename V>
-int launch_baked_mesh_dirs(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                           float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs, float* normals,
-                           void* stream, const float* dequant = nullptr) {
+int baked_mesh_dirs(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                    float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs, float* normals,
+                    void* stream, const float* dequant) {
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, dirs)) return rc;
+  if (int rc = check_values(what, values, dequant)) return rc;
   if (n_vertices == 0) return NERFB200_OK;
   baked_mesh_dirs_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads, 0,
                               static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
                                                                    values, level, edge_keys, n_vertices, dirs,
                                                                    normals, dequant);
-  count_launch();
-  return check_cuda(cudaGetLastError(), what);
+  return check_launch(what);
 }
 
+// the mesh colours' entry points, as baked_mesh_dirs
 template <typename V>
-int launch_baked_mesh_colors(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                             int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
-                             int64_t n_vertices, float* colors, void* stream, const float* dequant = nullptr) {
+int baked_mesh_colors(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                      int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
+                      int64_t n_vertices, float* colors, void* stream, const float* dequant) {
+  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
+  if (use_viewdirs && !dirs) {
+    set_error("%s: view directions need dirs", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (int rc = check_values(what, values, dequant)) return rc;
   if (n_vertices == 0) return NERFB200_OK;
   baked_mesh_colors_kernel<V><<<(unsigned)((n_vertices + kMeshAttrThreads - 1) / kMeshAttrThreads), kMeshAttrThreads,
                                 0, static_cast<cudaStream_t>(stream)>>>(baked_box(box), make_lattice(*box), brick_map,
                                                                         values, use_viewdirs ? 1 : 0, level, edge_keys,
                                                                         dirs, n_vertices, colors, dequant);
-  count_launch();
-  return check_cuda(cudaGetLastError(), what);
+  return check_launch(what);
 }
 
 }  // namespace
@@ -1288,72 +1249,43 @@ extern "C" {
 int32_t nerfb200_baked_mesh_dirs(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                                  float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
                                  float* normals, void* stream) {
-  if (int rc = check_baked_mesh("baked_mesh_dirs", box, brick_map, values, level, edge_keys, n_vertices, dirs))
-    return rc;
-  return launch_baked_mesh_dirs("baked_mesh_dirs launch", box, brick_map, values, level, edge_keys, n_vertices, dirs,
-                                normals, stream);
+  return baked_mesh_dirs("baked_mesh_dirs", box, brick_map, values, level, edge_keys, n_vertices, dirs, normals, stream,
+                         nullptr);
 }
 
 int32_t nerfb200_baked_mesh_dirs_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
                                      float level, const int64_t* edge_keys, int64_t n_vertices, float* dirs,
                                      float* normals, void* stream) {
-  const char* what = "baked_mesh_dirs_f16";
-  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, dirs)) return rc;
-  if (int rc = check_f16_values(what, values)) return rc;
-  return launch_baked_mesh_dirs("baked_mesh_dirs_f16 launch", box, brick_map, reinterpret_cast<const __half*>(values),
-                                level, edge_keys, n_vertices, dirs, normals, stream);
+  return baked_mesh_dirs("baked_mesh_dirs_f16", box, brick_map, reinterpret_cast<const __half*>(values), level,
+                         edge_keys, n_vertices, dirs, normals, stream, nullptr);
 }
 
 int32_t nerfb200_baked_mesh_colors(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
                                    int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
                                    int64_t n_vertices, float* colors, void* stream) {
-  const char* what = "baked_mesh_colors";
-  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
-  if (use_viewdirs && !dirs) {
-    set_error("%s: view directions need dirs", what);
-    return NERFB200_ERR_INVALID;
-  }
-  return launch_baked_mesh_colors("baked_mesh_colors launch", box, brick_map, values, use_viewdirs, level, edge_keys,
-                                  dirs, n_vertices, colors, stream);
+  return baked_mesh_colors("baked_mesh_colors", box, brick_map, values, use_viewdirs, level, edge_keys, dirs,
+                           n_vertices, colors, stream, nullptr);
 }
 
 int32_t nerfb200_baked_mesh_colors_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
                                        int32_t use_viewdirs, float level, const int64_t* edge_keys, const float* dirs,
                                        int64_t n_vertices, float* colors, void* stream) {
-  const char* what = "baked_mesh_colors_f16";
-  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
-  if (use_viewdirs && !dirs) {
-    set_error("%s: view directions need dirs", what);
-    return NERFB200_ERR_INVALID;
-  }
-  if (int rc = check_f16_values(what, values)) return rc;
-  return launch_baked_mesh_colors("baked_mesh_colors_f16 launch", box, brick_map,
-                                  reinterpret_cast<const __half*>(values), use_viewdirs, level, edge_keys, dirs,
-                                  n_vertices, colors, stream);
+  return baked_mesh_colors("baked_mesh_colors_f16", box, brick_map, reinterpret_cast<const __half*>(values),
+                           use_viewdirs, level, edge_keys, dirs, n_vertices, colors, stream, nullptr);
 }
 
 int32_t nerfb200_baked_mesh_dirs_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
                                     const float* dequant, float level, const int64_t* edge_keys, int64_t n_vertices,
                                     float* dirs, float* normals, void* stream) {
-  const char* what = "baked_mesh_dirs_u8";
-  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, dirs)) return rc;
-  if (int rc = check_u8_values(what, values, dequant)) return rc;
-  return launch_baked_mesh_dirs("baked_mesh_dirs_u8 launch", box, brick_map, values, level, edge_keys, n_vertices,
-                                dirs, normals, stream, dequant);
+  return baked_mesh_dirs("baked_mesh_dirs_u8", box, brick_map, values, level, edge_keys, n_vertices, dirs, normals,
+                         stream, dequant);
 }
 
 int32_t nerfb200_baked_mesh_colors_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
                                       const float* dequant, int32_t use_viewdirs, float level, const int64_t* edge_keys,
                                       const float* dirs, int64_t n_vertices, float* colors, void* stream) {
-  const char* what = "baked_mesh_colors_u8";
-  if (int rc = check_baked_mesh(what, box, brick_map, values, level, edge_keys, n_vertices, colors)) return rc;
-  if (use_viewdirs && !dirs) {
-    set_error("%s: view directions need dirs", what);
-    return NERFB200_ERR_INVALID;
-  }
-  if (int rc = check_u8_values(what, values, dequant)) return rc;
-  return launch_baked_mesh_colors("baked_mesh_colors_u8 launch", box, brick_map, values, use_viewdirs, level,
-                                  edge_keys, dirs, n_vertices, colors, stream, dequant);
+  return baked_mesh_colors("baked_mesh_colors_u8", box, brick_map, values, use_viewdirs, level, edge_keys, dirs,
+                           n_vertices, colors, stream, dequant);
 }
 
 }  // extern "C"
