@@ -704,7 +704,9 @@ int32_t nerfb200_baked_adam_step_dev(float* values, const float* g, float* m, fl
  *     (non-negative weights times non-positive values), so sigma = 0, alpha = +0 and q = (1 - 0) + 1e-10 = 1 exactly
  *     (1e-10 is below half an ulp of 1): T passes unchanged, w = +0, and w rgb and w t are +-0, which leave every sum
  *     (each starts at +0) unchanged.  A dropped sample is a miss, which has the same alpha, q and w, and a round whose
- *     lanes all miss (skipped by the renderer) is equivalent to one in which they hit such a brick.
+ *     lanes all miss (skipped by the renderer) is equivalent to one in which they hit such a brick.  Normal maps
+ *     (baked_render_normals) stay the same bits too: such samples have w = +0 and are skipped by the normal sum, as
+ *     they add nothing to the colour sums ("baked fields: normal maps and point queries").
  *   - Unseen bricks.  A brick with max_w == 0 over a set of rays can be dropped leaving the renders of those rays bit
  *     for bit the same (with or without early stopping: the march agrees at every round).  A dropped sample had w = +0,
  *     so either alpha = 0 (q = 1 as for a miss) or T = 0 before it; T is a product of factors q in [1e-10, 1], so once
@@ -932,6 +934,69 @@ int32_t nerfb200_baked_mesh_dirs_u8(const nerfb200_grid_t* box, const int32_t* b
 int32_t nerfb200_baked_mesh_colors_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
                                       const float* dequant, int32_t use_viewdirs, float level, const int64_t* edge_keys,
                                       const float* dirs, int64_t n_vertices, float* colors, void* stream);
+
+/* ---- baked fields: normal maps and point queries ---------------------------------------------------------------------
+ * The geometry probes a trained network has (normal maps of a render, raw outputs and the density gradient at caller-
+ * given points), for a baked field without its network.  All fp32 with round-to-nearest, each op rounded, no
+ * contraction unless fmaf is named, as in every baked section.
+ *   - Gradient at a point x.  The renderer's lookup of x ("baked fields": the cell rule, the cube, the fractions f, the
+ *     brick slot).  For each axis c: g_c = 0, then for the corners k = 0 .. 7 in the renderer's order g_c =
+ *     fmaf(s_kc * p_kc, v_k, g_c), then g_c = g_c * scale_c.  v_k is corner k's sigma_raw (channel 0, read as the
+ *     renderer reads it); s_kc is +1 where the corner's offset on axis c is 1 and -1 where it is 0 (exact); p_kc is the
+ *     product of the other two axes' trilinear weights in axis order (w_y w_z, w_x w_z, w_x w_y); scale_c = res_c / (hi_c -
+ *     lo_c) of the cell rule.  This is the exact gradient of the trilinear sigma_raw inside the cube; on a cube face it
+ *     is one-sided, the gradient of the cube the lookup picked.  A point outside the box or in an inactive brick has
+ *     sigma_raw = 0 and gradient 0.  It is the gradient of sigma_raw, not of relu(sigma_raw); wherever a sample has a
+ *     nonzero weight sigma_raw > 0 and the two agree.
+ *   - Normal map (baked_render_normals).  The march of baked_render (interval, t_k, rounds of 32, scan, early stopping,
+ *     outputs): out[n][8] is bit for bit what baked_render writes for the same inputs.  normals[n][3] = N: per sample,
+ *     the gradient above at the sample's point x = o + d t_k formed as the lookup forms it; with a camera ndc, g is
+ *     first replaced by J^T(x) g ("NDC scenes", ndc_grad_to_world); n = -g / |g| with |g| = sqrt((g_x g_x + g_y g_y) +
+ *     g_z g_z), n = 0 where |g| = 0 (render_fwd_normals' rule).  N = 0, then N += w n in sample order over the samples
+ *     with w != 0, broadcast across the round's lanes as the colour sums are; skipping w == 0 keeps a NaN gradient out
+ *     of rays that never reach it.  A stopped ray sums the samples before its stop.  N is not renormalised: |N| <= acc
+ *     up to rounding.  The gradient reads the sigma_raw corners the interp already loads.
+ *   - Point query (baked_query).  At pts[P][3], in the field's own frame: raw[P][4] = (s_r, s_g, s_b, sigma_raw),
+ *     run_network's raw layout (pre-sigmoid logits, then sigma_raw), each channel the renderer's interp at the point
+ *     and s_c the renderer's logit with Y_j(dirs[p]) (dirs taken as given, not normalised) or Y_0 alone without view
+ *     directions; (0, 0, 0, 0) outside the box or in an inactive brick.  grad[P][3] = the gradient above.  At a point
+ *     whose fractions are exactly 0 the channels are the stored values bit for bit (the lattice points of a box whose
+ *     cell rule puts them at f = 0, e.g. a power-of-two box).
+ *   - Formats.  fp16 values and uint8 codes go through the one per-format point reader of "baked fields: half
+ *     precision" / "baked fields: 8-bit values": such a field gives normals, raw values and gradients bit for bit like
+ *     its widened fp32 field.
+ *   - Transparent prune.  Dropping transparent bricks ("baked fields: pruning") leaves normal maps the same bits: their
+ *     samples have w = +0 and are skipped, exactly as for the colour sums.
+ * baked_render_normals: the arguments of baked_render plus ndc (NULL: normals in the field's frame; else the NDC camera
+ *   the rays were generated with, for world-space normals) and normals[n_rays][3].
+ * baked_query: dirs[P][3] is read with view directions when raw is given (may be NULL otherwise); raw and grad may each
+ *   be NULL, not both.  One thread per point; n_points 0 launches nothing.
+ * _f16 / _u8: values binary16, or uint8 codes followed by dequant, as baked_render_f16 / baked_render_u8.
+ * Refused before any launch: whatever baked_render refuses (the same checks), a null normals, an ndc make_ndc_map
+ * refuses ("NDC scenes"), n_points < 0, raw and grad both NULL, view directions with raw and no dirs.  No atomics, no
+ * host synchronisation. */
+int32_t nerfb200_baked_render_normals(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                      int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                      int32_t white_background, float stop_transmittance, const nerfb200_ndc_t* ndc,
+                                      float* out, float* normals, void* stream);
+int32_t nerfb200_baked_render_normals_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                          int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                          int32_t white_background, float stop_transmittance,
+                                          const nerfb200_ndc_t* ndc, float* out, float* normals, void* stream);
+int32_t nerfb200_baked_render_normals_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                         const float* dequant, int32_t use_viewdirs, const float* rays,
+                                         int32_t ray_stride, int64_t n_rays, int32_t white_background,
+                                         float stop_transmittance, const nerfb200_ndc_t* ndc, float* out,
+                                         float* normals, void* stream);
+int32_t nerfb200_baked_query(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                             int32_t use_viewdirs, const float* pts, const float* dirs, int64_t n_points, float* raw,
+                             float* grad, void* stream);
+int32_t nerfb200_baked_query_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                 int32_t use_viewdirs, const float* pts, const float* dirs, int64_t n_points,
+                                 float* raw, float* grad, void* stream);
+int32_t nerfb200_baked_query_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                const float* dequant, int32_t use_viewdirs, const float* pts, const float* dirs,
+                                int64_t n_points, float* raw, float* grad, void* stream);
 
 /* Fused Adam over a flat vector (torch.optim.Adam semantics, train_nerf.py:136-141,261-270):
  * p, m, v updated in place from g; step is the 1-based step count AFTER this update; grad_scale

@@ -18,8 +18,8 @@ from .occupancy import OccupancyGrid
 from .mesh import Mesh, density_volume, extract_mesh, extract_mesh_from_volume
 from .density import density_gradient
 from .bake import (BakedField, BakedFieldTrainer, bake, baked_brick_weights, baked_brick_weights_rays,
-                   baked_regularizer, baked_transparent_bricks, extract_baked_mesh, prune_baked, render_baked,
-                   render_baked_rays, subdivide_baked)
+                   baked_density_gradient, baked_raw, baked_regularizer, baked_transparent_bricks, extract_baked_mesh,
+                   prune_baked, render_baked, render_baked_rays, subdivide_baked)
 from . import ops, parallel
 
 __all__ = [
@@ -30,6 +30,7 @@ __all__ = [
     "density_volume", "extract_mesh", "extract_mesh_from_volume", "density_gradient", "BakedField", "bake", "render_baked",
     "render_baked_rays", "BakedFieldTrainer", "baked_brick_weights", "baked_brick_weights_rays",
     "baked_transparent_bricks", "prune_baked", "baked_regularizer", "subdivide_baked", "extract_baked_mesh",
+    "baked_density_gradient", "baked_raw",
     "ops",
     "parallel",
 ]

@@ -179,6 +179,12 @@ SIGNATURES = {
     "nerfb200_baked_max_weights_u8": (I32, [GP, P, P, P, I32, P, I32, I64, P, P]),
     "nerfb200_baked_mesh_dirs_u8": (I32, [GP, P, P, P, F32, P, I64, P, P, P]),
     "nerfb200_baked_mesh_colors_u8": (I32, [GP, P, P, P, I32, F32, P, P, I64, P, P]),
+    "nerfb200_baked_render_normals": (I32, [GP, P, P, I32, P, I32, I64, I32, F32, NP, P, P, P]),
+    "nerfb200_baked_render_normals_f16": (I32, [GP, P, P, I32, P, I32, I64, I32, F32, NP, P, P, P]),
+    "nerfb200_baked_render_normals_u8": (I32, [GP, P, P, P, I32, P, I32, I64, I32, F32, NP, P, P, P]),
+    "nerfb200_baked_query": (I32, [GP, P, P, I32, P, P, I64, P, P, P]),
+    "nerfb200_baked_query_f16": (I32, [GP, P, P, I32, P, P, I64, P, P, P]),
+    "nerfb200_baked_query_u8": (I32, [GP, P, P, P, I32, P, P, I64, P, P, P]),
 }
 
 _lib = None

@@ -17,7 +17,8 @@ may store its values in fp16 (``bake(dtype=torch.float16)``, ``BakedField.half``
 precision") or as 8-bit codes with a per-channel scale and offset (``BakedField.quantize``; include/nerfb200.h "baked
 fields: 8-bit values"); fine-tuning, the regularisers and subdivision take fp32 fields only (``BakedField.float``).  Any
 field, fp32, fp16 or 8-bit, can be meshed without a network (extract_baked_mesh; include/nerfb200.h "baked fields:
-meshes")."""
+meshes"), rendered as a normal map (render_baked(normals=), render_baked_rays(normals=)) and probed point by point
+(baked_raw, baked_density_gradient; include/nerfb200.h "baked fields: normal maps and point queries")."""
 from __future__ import annotations
 
 import math
@@ -218,17 +219,25 @@ def bake(model, encode_position_fn, encode_direction_fn=None, *, bounds, resolut
 
 
 def render_baked(field: BakedField, height, width, focal_length, tform_cam2world, options, mode="validation", *,
-                 early_stop=None):
+                 early_stop=None, normals=False):
     """(rgb (H, W, 3), disp (H, W), acc (H, W)) of ``field`` seen from the pose ``tform_cam2world``.  The rays are
     ``render_image``'s: ``ops.gen_rays`` with ``options.dataset`` near / far / no_ndc and ``options.nerf.use_viewdirs``
     (which must match the baked network), and the white background of ``options.nerf.<mode>`` (``options.nerf.train``
     while ``train_utils.COMPAT_MODE_QUIRK`` holds, as ``render_image``).  Samples are spaced half the smallest cube side
     apart along each ray inside the box.  ``early_stop`` t in [0, 1) stops a ray once its transmittance falls below t
-    (checked every 32 samples); a ray that never stops is bit for bit the render without it."""
+    (checked every 32 samples); a ray that never stops is bit for bit the render without it.
+
+    ``normals=True`` appends the normal map (H, W, 3) in the field's frame: per pixel the sum over its samples of
+    w (-g / |g|), g the gradient of the trilinear sigma_raw (include/nerfb200.h "baked fields: normal maps and point
+    queries"); the first three outputs stay bit for bit those without it.  ``normals="world"`` gives it in world space:
+    for an NDC field (``options.dataset.no_ndc`` false) through the NDC map of this call's ``height``, ``width`` and
+    ``focal_length``, for a Blender field the same as True.  ``cast_to_normal_image`` turns it into an image."""
     from . import train_utils
 
     if not isinstance(field, BakedField):
         raise ValueError(f"render_baked: field must be an nb.BakedField, got {type(field).__name__}")
+    normals = train_utils.normals_mode(normals)
+    cam = train_utils._world_ndc(normals, options, (height, width, focal_length))
     if not field.values.is_cuda:
         raise NotImplementedError("nerfb200: the baked field must be on a CUDA device (there is no CPU path)")
     _check_viewdirs(field, options, "render_baked")
@@ -240,9 +249,14 @@ def render_baked(field: BakedField, height, width, focal_length, tform_cam2world
     white = getattr(options.nerf, "train" if train_utils.COMPAT_MODE_QUIRK else mode).white_background
     rays = _pose_rays(field, height, width, focal_length, tform_cam2world, options)
     values = field.values if field.n_active else field.values.new_zeros(1, 729, 32)
-    out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white), stop,
-                           dequant=field.dequant)
-    return out[:, :3].view(height, width, 3), out[:, 3].view(height, width), out[:, 4].view(height, width)
+    if normals:
+        out, nrm = ops.baked_render_normals(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white),
+                                            stop, cam, dequant=field.dequant)
+    else:
+        out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, bool(white), stop,
+                               dequant=field.dequant)
+    img = out[:, :3].view(height, width, 3), out[:, 3].view(height, width), out[:, 4].view(height, width)
+    return img + (nrm.view(height, width, 3),) if normals else img
 
 
 def _check_viewdirs(field, options, what):
@@ -293,7 +307,7 @@ class _BakedRender(torch.autograd.Function):
         return ops.baked_tie(box, f.brick_map, f.bricks, d), None, None, None
 
 
-def render_baked_rays(field: BakedField, rays, *, white_background=False, early_stop=None):
+def render_baked_rays(field: BakedField, rays, *, white_background=False, early_stop=None, normals=False, ndc=None):
     """(rgb (N, 3), disp (N,), acc (N,), depth (N,)) of the packed ``rays`` (N, 11) with view directions or (N, 8)
     without (``ops.gen_rays`` / ``ops.gen_rays_posed``) through ``field``.  Differentiable with respect to
     ``field.values`` when it requires grad: the gradient is the baked renderer's backward summed over every stored copy
@@ -303,7 +317,22 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
     An fp16 or 8-bit field renders bit for bit like ``field.float()`` and has no gradient.  This is the differentiable
     render, which refuses such a field in grad mode as it did before fp16 fields could be rendered at all; under
     ``torch.no_grad()`` (or inference mode) it renders one whose values do not require grad.  Anything else raises
-    ValueError (fine-tune ``field.float()``).  ``render_baked`` renders fp16 and 8-bit fields in any grad mode."""
+    ValueError (fine-tune ``field.float()``).  ``render_baked`` renders fp16 and 8-bit fields in any grad mode.
+
+    ``normals=True`` (or "world") appends the normal map (N, 3) of ``render_baked(normals=)``, in the field's frame, or
+    with ``ndc=(H, W, focal)`` (the camera NDC ``rays`` were generated with) in world space, as
+    ``extract_baked_mesh(ndc=)`` maps its meshes.  Packed rays do not say whether the field lives in NDC, so "world"
+    alone is the field's frame: pass ``ndc`` for an NDC field.  Normals are inference only: with a gradient (values that
+    require grad, in grad mode) they raise ValueError, as ``early_stop`` does."""
+    from . import density, train_utils
+
+    normals = train_utils.normals_mode(normals)
+    cam = density.ndc_camera(ndc) if ndc is not None else None
+    if cam is not None and not normals:
+        raise ValueError("render_baked_rays: ndc= maps the normal map to world space; pass normals=True with it")
+    if normals and isinstance(field, BakedField) and isinstance(field.values, torch.Tensor) \
+            and field.values.requires_grad and torch.is_grad_enabled():
+        raise ValueError("render_baked_rays: normals have no gradient; render under torch.no_grad()")
     _check_values(field, "render_baked_rays", stored=True)
     # grad mode alone keeps the refusal every fp16 field met here before half precision (pinned by the fine-tuning tests)
     if field.dtype in _LOSSY and (field.values.requires_grad or torch.is_grad_enabled()):
@@ -326,6 +355,10 @@ def render_baked_rays(field: BakedField, rays, *, white_background=False, early_
         out = _BakedRender.apply(field.values, field, rays, white)
     else:
         values = field.values.detach() if field.n_active else field.values.new_zeros(1, 729, 32)
+        if normals:
+            out, nrm = ops.baked_render_normals(field.box(), field.brick_map, values, field.use_viewdirs, rays, white,
+                                                stop, cam, dequant=field.dequant)
+            return out[:, :3], out[:, 3], out[:, 4], out[:, 5], nrm
         out = ops.baked_render(field.box(), field.brick_map, values, field.use_viewdirs, rays, white, stop,
                                dequant=field.dequant)
     return out[:, :3], out[:, 3], out[:, 4], out[:, 5]
@@ -761,3 +794,90 @@ def extract_baked_mesh(field: BakedField, level: float = 50.0, *, colors: bool =
             rgb = ops.baked_mesh_colors(box, field.brick_map, values, field.use_viewdirs, level, keys,
                                         dirs if field.use_viewdirs else None, dequant=field.dequant)
     return Mesh(verts, faces, rgb, nrm)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# point queries (include/nerfb200.h "baked fields: normal maps and point queries")
+# ------------------------------------------------------------------------------------------------------------------------
+def _query_field(field, what):
+    """The refusals every point query shares: not a ``BakedField`` or values that require grad in grad mode
+    (ValueError), a CPU field (NotImplementedError)."""
+    if not isinstance(field, BakedField):
+        raise ValueError(f"{what}: field must be an nb.BakedField, got {type(field).__name__}")
+    if isinstance(field.values, torch.Tensor) and field.values.requires_grad and torch.is_grad_enabled():
+        raise ValueError(f"{what}: point queries are inference only (no gradient with respect to the values); call it "
+                         "under torch.no_grad() or on values that do not require grad")
+    if not (isinstance(field.values, torch.Tensor) and field.values.is_cuda):
+        raise NotImplementedError("nerfb200: the baked field must be on a CUDA device (there is no CPU path)")
+    if field.values.dtype not in (torch.float32, torch.float16, torch.uint8):
+        raise ValueError(f"{what}: field.values must be fp32, fp16 or uint8, got {field.values.dtype}")
+
+
+def _query(field, pts, dirs, want_raw, want_grad, use_viewdirs):
+    """``ops.baked_query`` at flat points (P, 3) on the field's device; P may be 0."""
+    if pts.device != field.values.device:
+        raise ValueError(f"nerfb200: the points are on {pts.device}, the baked field on {field.values.device}")
+    n = pts.shape[0]
+    if n == 0 or field.n_active == 0:  # nothing to read: every point misses
+        return (pts.new_zeros(n, 4) if want_raw else None), (pts.new_zeros(n, 3) if want_grad else None)
+    return ops.baked_query(field.box(), field.brick_map, field.values.detach(), use_viewdirs, pts.contiguous(), dirs,
+                           want_raw, want_grad, dequant=field.dequant)
+
+
+def baked_density_gradient(field: BakedField, pts: torch.Tensor, *, ndc=None):
+    """``(sigma_raw (...), grad (..., 3))`` of a baked field at ``pts`` (..., 3) fp32 CUDA on the field's device, as
+    ``nb.density_gradient`` gives them for a network: sigma_raw is the renderer's trilinear interp at the point and grad
+    its exact gradient inside the cube the renderer's lookup picks (one-sided on a cube face; include/nerfb200.h "baked
+    fields: normal maps and point queries").  A point outside the box or in an inactive brick gives 0 and 0.  Any
+    storage format; an fp16 or 8-bit field gives the bits of ``field.float()``.
+
+    ``ndc=(H, W, focal)`` takes an NDC field's ``pts`` in world space (every z < 0, in front of the camera; ValueError
+    otherwise): sigma_raw is read at the NDC point N(p) and grad is the world gradient J^T grad_q (include/nerfb200.h
+    "NDC scenes"), exactly as ``density_gradient(ndc=)`` maps a network's.  Inference only: values that require grad in
+    grad mode are refused (ValueError), as is a CPU field (NotImplementedError), before any launch."""
+    from . import density
+
+    cam = density.ndc_camera(ndc) if ndc is not None else None
+    _query_field(field, "baked_density_gradient")
+    pts = density._checked_points(pts, world_ndc=cam is not None)
+    flat = pts.reshape(-1, 3)
+    with torch.no_grad():
+        if cam is not None:
+            if flat.device != field.values.device:
+                raise ValueError(f"nerfb200: the points are on {flat.device}, the baked field on "
+                                 f"{field.values.device}")
+            flat = ops.ndc_from_world(cam, flat.contiguous())
+        raw, grad = _query(field, flat, None, True, True, False)  # sigma reads no view direction
+        if cam is not None and flat.shape[0]:
+            rows = torch.cat([raw[:, 3:], grad], 1)
+            ops.ndc_grad_to_world(cam, flat, rows, out=rows)
+            grad = rows[:, 1:]
+        sigma = raw[:, 3]
+    return sigma.reshape(pts.shape[:-1]), grad.reshape(pts.shape)
+
+
+def baked_raw(field: BakedField, pts: torch.Tensor, viewdirs=None) -> torch.Tensor:
+    """raw (..., 4) = (s_r, s_g, s_b, sigma_raw) of a baked field at ``pts`` (..., 3) in the field's own frame (world
+    space for Blender scenes, NDC for LLFF scenes, as ``run_network`` takes its points): ``run_network``'s raw layout,
+    the pre-sigmoid colour logits and the raw density, each the renderer's trilinear interp at the point, the logits seen
+    along ``viewdirs`` (..., 3) as given (not normalised).  ``viewdirs`` is required for a field with view directions and
+    refused for one without (the logits are then Y_0 coef_c0).  A point outside the box or in an inactive brick reads 0
+    in every channel; at a lattice point the cell rule puts at fractions 0 the channels are the stored values bit for
+    bit.  Any storage format, CUDA tensors on the field's device; inference only, as ``baked_density_gradient``."""
+    from . import density
+
+    _query_field(field, "baked_raw")
+    if field.use_viewdirs != (viewdirs is not None):
+        raise ValueError(f"baked_raw: the field {'has' if field.use_viewdirs else 'has no'} view directions; "
+                         f"{'pass' if field.use_viewdirs else 'do not pass'} viewdirs")
+    pts = density._checked_points(pts)
+    dirs = None
+    if viewdirs is not None:
+        if not (isinstance(viewdirs, torch.Tensor) and viewdirs.dtype == torch.float32
+                and viewdirs.shape == pts.shape and viewdirs.device == pts.device):
+            raise ValueError(f"baked_raw: viewdirs must be an fp32 tensor of the points' shape {list(pts.shape)} on "
+                             f"{pts.device}")
+        dirs = viewdirs.reshape(-1, 3).contiguous()
+    with torch.no_grad():
+        raw, _ = _query(field, pts.reshape(-1, 3), dirs, True, False, field.use_viewdirs)
+    return raw.reshape(*pts.shape[:-1], 4)

@@ -160,17 +160,23 @@ __device__ __forceinline__ bool baked_live(float ta, float tb, float dt) {
   return ta < tb && dt > 0.f && dt < INFINITY && __fdiv_rn(__fsub_rn(tb, ta), dt) < 16777216.f;
 }
 
-// the sample at depth t (in_ray: t < t_b): its cube's fractions f, its point l inside the brick and the brick's slot,
-// or -1 outside the box, in an inactive brick or past t_b
-__device__ __forceinline__ int baked_lookup(const BakedBox& B, const int* __restrict__ brick_map, const float o[3],
-                                            const float d[3], float t, bool in_ray, float f[3], int l[3]) {
+// the sample's point x = o + d t, per axis as the MLP forms its points
+__device__ __forceinline__ float baked_x(const float o[3], const float d[3], float t, int c) {
+  return __fadd_rn(o[c], __fmul_rn(d[c], t));
+}
+
+// the point x (in_ray: whether to look it up at all): its cube's fractions f, its point l inside the brick and the
+// brick's slot, or -1 outside the box, in an inactive brick or when !in_ray.  point(c) gives x_c
+template <typename Point>
+__device__ __forceinline__ int baked_locate(const BakedBox& B, const int* __restrict__ brick_map, Point&& point,
+                                            bool in_ray, float f[3], int l[3]) {
   int slot = -1;
   if (in_ray) {
     bool inside = true;
     int bi[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float x = __fadd_rn(o[c], __fmul_rn(d[c], t));
+      const float x = point(c);
       const float tc = __fmul_rn(__fsub_rn(x, B.g.lo[c]), B.scale[c]);
       inside = inside && tc >= 0.f && tc < (float)B.g.res[c];
       const int i = inside ? (int)tc : 0;
@@ -183,12 +189,30 @@ __device__ __forceinline__ int baked_lookup(const BakedBox& B, const int* __rest
   return slot;
 }
 
+// the sample at depth t (in_ray: t < t_b): baked_locate of its point, -1 past t_b
+__device__ __forceinline__ int baked_lookup(const BakedBox& B, const int* __restrict__ brick_map, const float o[3],
+                                            const float d[3], float t, bool in_ray, float f[3], int l[3]) {
+  return baked_locate(B, brick_map, [&](int c) { return baked_x(o, d, t, c); }, in_ray, f, l);
+}
+
 // trilinear weight of corner k = 0 .. 7 of a cube with fractions f
 __device__ __forceinline__ float corner_weight(const float f[3], int k) {
   const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
   const float wx = dx ? f[0] : __fsub_rn(1.0f, f[0]), wy = dy ? f[1] : __fsub_rn(1.0f, f[1]);
   const float wz = dz ? f[2] : __fsub_rn(1.0f, f[2]);
   return __fmul_rn(__fmul_rn(wx, wy), wz);
+}
+
+// corner k's factor in each axis' derivative of the trilinear interp (include/nerfb200.h "baked fields: normal maps and
+// point queries"): +-(the product of the other two axes' weights, in axis order), + where the corner's offset is 1
+__device__ __forceinline__ void corner_slopes(const float f[3], int k, float s[3]) {
+  const int dx = k & 1, dy = (k >> 1) & 1, dz = k >> 2;
+  const float wx = dx ? f[0] : __fsub_rn(1.0f, f[0]), wy = dy ? f[1] : __fsub_rn(1.0f, f[1]);
+  const float wz = dz ? f[2] : __fsub_rn(1.0f, f[2]);
+  const float px = __fmul_rn(wy, wz), py = __fmul_rn(wx, wz), pz = __fmul_rn(wx, wy);
+  s[0] = dx ? px : -px;
+  s[1] = dy ? py : -py;
+  s[2] = dz ? pz : -pz;
 }
 
 // 16-B offset of corner k of the cube at brick point l, from the slot's first value: a point is kBakeCh values of type V
@@ -275,10 +299,10 @@ __device__ __forceinline__ void baked_point(const uint8_t* base, int off16, cons
 }
 
 // channels 0 .. 27 interpolated over the cube's corners (0 when slot < 0): each corner's point from baked_point into
-// the same fmaf chain for every format
-template <typename V>
+// the same fmaf chain for every format.  sigma(k, x) also receives corner k's sigma_raw as it is fed to channel 0
+template <typename V, typename Sigma>
 __device__ __forceinline__ void baked_interp(const V* __restrict__ values, const float* dq, int slot, const float f[3],
-                                             const int l[3], float v[kBakedVals]) {
+                                             const int l[3], float v[kBakedVals], Sigma&& sigma) {
 #pragma unroll
   for (int ch = 0; ch < kBakedVals; ++ch) v[ch] = 0.f;
   if (slot >= 0) {
@@ -286,10 +310,35 @@ __device__ __forceinline__ void baked_interp(const V* __restrict__ values, const
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const float w = corner_weight(f, k);
-      baked_point(sv, corner_offset<V>(l, k), dq, [&](int ch, float x) { v[ch] = fmaf(w, x, v[ch]); });
+      baked_point(sv, corner_offset<V>(l, k), dq, [&](int ch, float x) {
+        v[ch] = fmaf(w, x, v[ch]);
+        if (ch == 0) sigma(k, x);
+      });
     }
   }
 }
+template <typename V>
+__device__ __forceinline__ void baked_interp(const V* __restrict__ values, const float* dq, int slot, const float f[3],
+                                             const int l[3], float v[kBakedVals]) {
+  baked_interp(values, dq, slot, f, l, v, [](int, float) {});
+}
+
+// the gradient of the trilinear sigma_raw inside a cube with fractions f (include/nerfb200.h "baked fields: normal maps
+// and point queries"): add(f, k, v_k) takes the corners in the renderer's order, then scale(B) multiplies each axis'
+// sum by the cell rule's scale
+struct SigmaGrad {
+  float g[3] = {0.f, 0.f, 0.f};
+  __device__ __forceinline__ void add(const float f[3], int k, float vk) {
+    float s[3];
+    corner_slopes(f, k, s);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = fmaf(s[c], vk, g[c]);
+  }
+  __device__ __forceinline__ void scale(const BakedBox& B) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = __fmul_rn(g[c], B.scale[c]);
+  }
+};
 
 // channel 0 (sigma_raw) of baked_interp: the same corners in the same order through the same fmaf chain, one 4-B (fp32),
 // 2-B (fp16) or 1-B (uint8) load per corner
@@ -306,27 +355,46 @@ __device__ __forceinline__ float baked_interp_sigma(const V* __restrict__ values
   return v;
 }
 
+// the pre-sigmoid logit s_c of colour channel c from the interpolated coefficients v[1 ..]
+__device__ __forceinline__ float baked_logit(int use_viewdirs, const float Y[kBakeSh], const float v[kBakedVals], int c) {
+  float s = 0.f;
+  if (use_viewdirs) {
+#pragma unroll
+    for (int j = 0; j < kBakeSh; ++j) s = fmaf(Y[j], v[1 + kBakeSh * c + j], s);
+  } else {
+    s = __fmul_rn(Y[0], v[1 + kBakeSh * c]);
+  }
+  return s;
+}
+
 // rgb = sigmoid(s_c) of the interpolated coefficients v[1 ..]
 __device__ __forceinline__ void baked_colour(int use_viewdirs, const float Y[kBakeSh], const float v[kBakedVals],
                                              float rgb[3]) {
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    float s = 0.f;
-    if (use_viewdirs) {
+  for (int c = 0; c < 3; ++c) rgb[c] = sigmoidf_(baked_logit(use_viewdirs, Y, v, c));
+}
+
+// w n of a sample (include/nerfb200.h "baked fields: normal maps and point queries"): n = -g / |g|, 0 where |g| is 0,
+// and 0 for w == 0 (a NaN gradient stays out of rays that never reach it)
+__device__ __forceinline__ void weighted_normal(float w, const float g[3], float out[3]) {
+  out[0] = out[1] = out[2] = 0.f;
+  const float ss = __fadd_rn(__fadd_rn(__fmul_rn(g[0], g[0]), __fmul_rn(g[1], g[1])), __fmul_rn(g[2], g[2]));
+  if (w != 0.f && ss != 0.f) {
+    const float len = __fsqrt_rn(ss);
 #pragma unroll
-      for (int j = 0; j < kBakeSh; ++j) s = fmaf(Y[j], v[1 + kBakeSh * c + j], s);
-    } else {
-      s = __fmul_rn(Y[0], v[1 + kBakeSh * c]);
-    }
-    rgb[c] = sigmoidf_(s);
+    for (int c = 0; c < 3; ++c) out[c] = __fmul_rn(w, -__fdiv_rn(g[c], len));
   }
 }
 
-template <typename V>
+// kNormals also sums each sample's w n into normals[r][3] (include/nerfb200.h "baked fields: normal maps and point
+// queries"), the gradient taken from the sigma_raw corners the interp already reads; kNdc maps each gradient by J^T of
+// ndc at the sample's point first.  The instances without normals never read normals or ndc.
+template <typename V, bool kNormals = false, bool kNdc = false>
 __global__ void __launch_bounds__(kBakedWarps * 32)
 baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values,
                     int use_viewdirs, const float* __restrict__ rays, int ray_stride, int64_t n_rays, int white_bkgd,
-                    float stop_t, float* __restrict__ out, const float* __restrict__ dequant_tab) {
+                    float stop_t, float* __restrict__ out, const float* __restrict__ dequant_tab,
+                    float* __restrict__ normals, const NdcMap ndc) {
   __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
   stage_dequant<V>(dequant_tab, dq);
   const int lane = threadIdx.x & 31;
@@ -340,6 +408,7 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
   else Y[0] = 0.28209479177387814f;
 
   float T = 1.0f, ar = 0.f, ag = 0.f, ab = 0.f, aacc = 0.f, adepth = 0.f;
+  float N[3] = {0.f, 0.f, 0.f};  // kNormals
   const bool live = baked_live(ta, tb, dt);
   for (int k0 = 0; live; k0 += 32) {
     const float t = __fadd_rn(ta, __fmul_rn(__fadd_rn((float)(k0 + lane), 0.5f), dt));
@@ -349,7 +418,9 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
     const int slot = baked_lookup(B, brick_map, o, d, t, t < tb, f, l);
     if (__ballot_sync(0xffffffffu, slot >= 0) == 0u) continue;  // q = 1 and w = 0 everywhere: T and the sums stay
     float v[kBakedVals];
-    baked_interp(values, dq, slot, f, l, v);
+    SigmaGrad sg;
+    if constexpr (kNormals) baked_interp(values, dq, slot, f, l, v, [&](int k, float x) { sg.add(f, k, x); });
+    else baked_interp(values, dq, slot, f, l, v);
     float rgb[3] = {0.f, 0.f, 0.f};
     if (slot >= 0) baked_colour(use_viewdirs, Y, v, rgb);
     const SampleTerms st = sample_terms(slot >= 0 ? v[0] : 0.f, 0.f, 0.f, false, t, __fadd_rn(t, dt), false, dnorm);
@@ -357,6 +428,16 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
     const float w = __fmul_rn(st.alpha, Tl);
     const float cr = __fmul_rn(w, rgb[0]), cg = __fmul_rn(w, rgb[1]), cb = __fmul_rn(w, rgb[2]);
     const float cd = __fmul_rn(w, t);
+    float cn[3];  // kNormals: w n
+    if constexpr (kNormals) {
+      sg.scale(B);
+      if constexpr (kNdc) {
+        const float x[3] = {baked_x(o, d, t, 0), baked_x(o, d, t, 1), baked_x(o, d, t, 2)};
+        const float gn[3] = {sg.g[0], sg.g[1], sg.g[2]};
+        ndc_grad_to_world(ndc, x, gn, sg.g);
+      }
+      weighted_normal(w, sg.g, cn);
+    }
 #pragma unroll 4
     for (int i = 0; i < 32; ++i) {  // in sample order
       ar = __fadd_rn(ar, __shfl_sync(0xffffffffu, cr, i));
@@ -364,6 +445,10 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
       ab = __fadd_rn(ab, __shfl_sync(0xffffffffu, cb, i));
       aacc = __fadd_rn(aacc, __shfl_sync(0xffffffffu, w, i));
       adepth = __fadd_rn(adepth, __shfl_sync(0xffffffffu, cd, i));
+      if constexpr (kNormals) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) N[c] = __fadd_rn(N[c], __shfl_sync(0xffffffffu, cn[c], i));
+      }
     }
     T = __shfl_sync(0xffffffffu, __fmul_rn(Tl, st.q), 31);
     if (T < stop_t) break;
@@ -381,6 +466,51 @@ baked_render_kernel(const BakedBox B, const int* __restrict__ brick_map, const V
     float4* o4 = reinterpret_cast<float4*>(out + r * 8);
     o4[0] = make_float4(ar, ag, ab, disp_out);
     o4[1] = make_float4(aacc, adepth, 0.f, 0.f);
+    if constexpr (kNormals) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) normals[r * 3 + c] = N[c];
+    }
+  }
+}
+
+constexpr int kQueryThreads = 256;
+
+// One thread per point (include/nerfb200.h "baked fields: normal maps and point queries"): the renderer's lookup, interp
+// and logits at pts[i], raw[i] = (s_r, s_g, s_b, sigma_raw) (0 outside the box or in an inactive brick) and grad[i] the
+// gradient of sigma_raw; either output may be null.  dirs[i] is read with view directions only, as given.
+template <typename V>
+__global__ void __launch_bounds__(kQueryThreads)
+baked_query_kernel(const BakedBox B, const int* __restrict__ brick_map, const V* __restrict__ values, int use_viewdirs,
+                   const float* __restrict__ pts, const float* __restrict__ dirs, int64_t n, float* __restrict__ raw,
+                   float* __restrict__ grad, const float* __restrict__ dequant_tab) {
+  __shared__ float dq[sizeof(V) == 1 ? 2 * kBakedVals : 1];  // uint8 fields only
+  stage_dequant<V>(dequant_tab, dq);
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float x[3] = {pts[3 * i], pts[3 * i + 1], pts[3 * i + 2]};
+  float f[3];
+  int l[3];
+  const int slot = baked_locate(B, brick_map, [&](int c) { return x[c]; }, true, f, l);
+  float v[kBakedVals];
+  SigmaGrad sg;
+  baked_interp(values, dq, slot, f, l, v, [&](int k, float s) { sg.add(f, k, s); });
+  sg.scale(B);
+  if (raw) {
+    float s[3] = {0.f, 0.f, 0.f};
+    if (slot >= 0) {
+      float Y[kBakeSh];
+      if (use_viewdirs) sh_basis(dirs[3 * i], dirs[3 * i + 1], dirs[3 * i + 2], Y);
+      else Y[0] = 0.28209479177387814f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s[c] = baked_logit(use_viewdirs, Y, v, c);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) raw[4 * i + c] = s[c];
+    raw[4 * i + 3] = v[0];
+  }
+  if (grad) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) grad[3 * i + c] = sg.g[c];
   }
 }
 
@@ -786,11 +916,11 @@ int32_t nerfb200_bake_basis(float* dirs_host, float* proj_host) {
 
 namespace {
 
-// the renderer's entry points (what: the entry point's name in the errors): its checks, the format's, then the launch
+// the renderer's checks (what: the entry point's name in the errors), then the format's
 template <typename V>
-int baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
-                 int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays, int32_t white_background,
-                 float stop_transmittance, float* out, void* stream, const float* dequant) {
+int check_baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                       int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                       float stop_transmittance, const float* out, const float* dequant) {
   if (int rc = check_grid(box, what)) return rc;
   if (!brick_map || !values || !rays || !out || n_rays <= 0 || ray_stride < (use_viewdirs ? 11 : 8)) {
     set_error("%s: null pointer, n_rays <= 0 or ray_stride %d too short", what, ray_stride);
@@ -800,12 +930,75 @@ int baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* br
     set_error("%s: stop_transmittance must lie in [0, 1), got %g", what, (double)stop_transmittance);
     return NERFB200_ERR_INVALID;
   }
-  if (int rc = check_values(what, values, dequant)) return rc;
+  return check_values(what, values, dequant);
+}
+
+// the renderer's entry points: its checks, then the launch
+template <typename V>
+int baked_render(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                 int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays, int32_t white_background,
+                 float stop_transmittance, float* out, void* stream, const float* dequant) {
+  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                                  stop_transmittance, out, dequant))
+    return rc;
   const BakedBox B = baked_box(box);
   const int64_t blocks = (n_rays + kBakedWarps - 1) / kBakedWarps;
   baked_render_kernel<V><<<(unsigned)blocks, kBakedWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       B, brick_map, values, use_viewdirs ? 1 : 0, rays, ray_stride, n_rays, white_background ? 1 : 0,
-      stop_transmittance, out, dequant);
+      stop_transmittance, out, dequant, nullptr, NdcMap{0.f, 0.f});
+  return check_launch(what);
+}
+
+// the normal-map renderer's entry points: the renderer's checks, a null normals, a camera make_ndc_map refuses (ndc
+// NULL: the field's frame), then the launch
+template <typename V>
+int baked_render_normals(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                         int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                         int32_t white_background, float stop_transmittance, const nerfb200_ndc_t* ndc, float* out,
+                         float* normals, void* stream, const float* dequant) {
+  if (int rc = check_baked_render(what, box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                                  stop_transmittance, out, dequant))
+    return rc;
+  if (!normals) {
+    set_error("%s: null normals", what);
+    return NERFB200_ERR_INVALID;
+  }
+  NdcMap m{0.f, 0.f};
+  if (ndc)
+    if (int rc = make_ndc_map(ndc, &m, what)) return rc;
+  const BakedBox B = baked_box(box);
+  const unsigned blocks = (unsigned)((n_rays + kBakedWarps - 1) / kBakedWarps);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int vd = use_viewdirs ? 1 : 0, white = white_background ? 1 : 0;
+  if (ndc)
+    baked_render_kernel<V, true, true><<<blocks, kBakedWarps * 32, 0, s>>>(
+        B, brick_map, values, vd, rays, ray_stride, n_rays, white, stop_transmittance, out, dequant, normals, m);
+  else
+    baked_render_kernel<V, true, false><<<blocks, kBakedWarps * 32, 0, s>>>(
+        B, brick_map, values, vd, rays, ray_stride, n_rays, white, stop_transmittance, out, dequant, normals, m);
+  return check_launch(what);
+}
+
+// the point queries' entry points: the box, null pointers, n_points < 0, raw and grad both null, view directions
+// without dirs, the format's checks; n_points 0 launches nothing
+template <typename V>
+int baked_query(const char* what, const nerfb200_grid_t* box, const int32_t* brick_map, const V* values,
+                int32_t use_viewdirs, const float* pts, const float* dirs, int64_t n_points, float* raw, float* grad,
+                void* stream, const float* dequant) {
+  if (int rc = check_grid(box, what)) return rc;
+  if (!brick_map || !values || !pts || n_points < 0 || (!raw && !grad)) {
+    set_error("%s: null pointer, raw and grad both null, or n_points %lld < 0", what, (long long)n_points);
+    return NERFB200_ERR_INVALID;
+  }
+  if (use_viewdirs && raw && !dirs) {
+    set_error("%s: view directions need dirs", what);
+    return NERFB200_ERR_INVALID;
+  }
+  if (int rc = check_values(what, values, dequant)) return rc;
+  if (n_points == 0) return NERFB200_OK;
+  baked_query_kernel<V><<<(unsigned)((n_points + kQueryThreads - 1) / kQueryThreads), kQueryThreads, 0,
+                          static_cast<cudaStream_t>(stream)>>>(baked_box(box), brick_map, values, use_viewdirs ? 1 : 0,
+                                                               pts, dirs, n_points, raw, grad, dequant);
   return check_launch(what);
 }
 
@@ -851,6 +1044,53 @@ int32_t nerfb200_baked_render_u8(const nerfb200_grid_t* box, const int32_t* bric
                                  void* stream) {
   return baked_render("baked_render_u8", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
                       white_background, stop_transmittance, out, stream, dequant);
+}
+
+int32_t nerfb200_baked_render_normals(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                                      int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                      int32_t white_background, float stop_transmittance, const nerfb200_ndc_t* ndc,
+                                      float* out, float* normals, void* stream) {
+  return baked_render_normals("baked_render_normals", box, brick_map, values, use_viewdirs, rays, ray_stride, n_rays,
+                              white_background, stop_transmittance, ndc, out, normals, stream, nullptr);
+}
+
+int32_t nerfb200_baked_render_normals_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                          int32_t use_viewdirs, const float* rays, int32_t ray_stride, int64_t n_rays,
+                                          int32_t white_background, float stop_transmittance,
+                                          const nerfb200_ndc_t* ndc, float* out, float* normals, void* stream) {
+  return baked_render_normals("baked_render_normals_f16", box, brick_map, reinterpret_cast<const __half*>(values),
+                              use_viewdirs, rays, ray_stride, n_rays, white_background, stop_transmittance, ndc, out,
+                              normals, stream, nullptr);
+}
+
+int32_t nerfb200_baked_render_normals_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                         const float* dequant, int32_t use_viewdirs, const float* rays,
+                                         int32_t ray_stride, int64_t n_rays, int32_t white_background,
+                                         float stop_transmittance, const nerfb200_ndc_t* ndc, float* out,
+                                         float* normals, void* stream) {
+  return baked_render_normals("baked_render_normals_u8", box, brick_map, values, use_viewdirs, rays, ray_stride,
+                              n_rays, white_background, stop_transmittance, ndc, out, normals, stream, dequant);
+}
+
+int32_t nerfb200_baked_query(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,
+                             int32_t use_viewdirs, const float* pts, const float* dirs, int64_t n_points, float* raw,
+                             float* grad, void* stream) {
+  return baked_query("baked_query", box, brick_map, values, use_viewdirs, pts, dirs, n_points, raw, grad, stream,
+                     nullptr);
+}
+
+int32_t nerfb200_baked_query_f16(const nerfb200_grid_t* box, const int32_t* brick_map, const uint16_t* values,
+                                 int32_t use_viewdirs, const float* pts, const float* dirs, int64_t n_points,
+                                 float* raw, float* grad, void* stream) {
+  return baked_query("baked_query_f16", box, brick_map, reinterpret_cast<const __half*>(values), use_viewdirs, pts,
+                     dirs, n_points, raw, grad, stream, nullptr);
+}
+
+int32_t nerfb200_baked_query_u8(const nerfb200_grid_t* box, const int32_t* brick_map, const uint8_t* values,
+                                const float* dequant, int32_t use_viewdirs, const float* pts, const float* dirs,
+                                int64_t n_points, float* raw, float* grad, void* stream) {
+  return baked_query("baked_query_u8", box, brick_map, values, use_viewdirs, pts, dirs, n_points, raw, grad, stream,
+                     dequant);
 }
 
 int32_t nerfb200_baked_max_weights(const nerfb200_grid_t* box, const int32_t* brick_map, const float* values,

@@ -1030,6 +1030,39 @@ def baked_render(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_b
     return out
 
 
+def baked_render_normals(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool,
+                         stop_transmittance: float = 0.0, ndc: Optional[Ndc] = None, dequant=None):
+    """(rows (n, 8) bit for bit ``baked_render``'s, normal map (n, 3)) of the packed ``rays`` through a baked field
+    (include/nerfb200.h "baked fields: normal maps and point queries"): the sum of w (-g / |g|) in sample order, g the
+    gradient of the trilinear sigma_raw, in the field's frame, or with ``ndc`` (``ndc_struct`` of the rays' camera)
+    mapped to world space by J^T first."""
+    sfx, pv = _baked_values(values, "baked_render_normals", dequant)
+    n = rays.shape[0]
+    out = torch.empty(n, 8, dtype=torch.float32, device=rays.device)
+    normals = torch.empty(n, 3, dtype=torch.float32, device=rays.device)
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_render_normals" + sfx)(
+        C.byref(box), _ptr(brick_map), *pv, int(bool(use_viewdirs)), _ptr(rays), rays.shape[1], n,
+        int(bool(white_background)), float(stop_transmittance), None if ndc is None else C.byref(ndc), _ptr(out),
+        _ptr(normals), _stream()), "baked_render_normals" + sfx)
+    return out, normals
+
+
+def baked_query(box: Grid, brick_map, values, use_viewdirs: bool, pts, dirs=None, want_raw: bool = True,
+                want_grad: bool = True, dequant=None):
+    """(raw (P, 4) or None, grad (P, 3) or None) of a baked field at the field-frame points ``pts`` (P, 3)
+    (include/nerfb200.h "baked fields: normal maps and point queries"): raw = (s_r, s_g, s_b, sigma_raw) with the
+    logits seen along ``dirs`` (P, 3, read with view directions only) and grad the gradient of the trilinear
+    sigma_raw."""
+    sfx, pv = _baked_values(values, "baked_query", dequant)
+    n = pts.shape[0]
+    raw = torch.empty(n, 4, dtype=torch.float32, device=pts.device) if want_raw else None
+    grad = torch.empty(n, 3, dtype=torch.float32, device=pts.device) if want_grad else None
+    _lib.check(getattr(_lib.load(), "nerfb200_baked_query" + sfx)(
+        C.byref(box), _ptr(brick_map), *pv, int(bool(use_viewdirs)), _ptr(pts), _ptr(dirs), n, _ptr(raw), _ptr(grad),
+        _stream()), "baked_query" + sfx)
+    return raw, grad
+
+
 def baked_render_bwd(box: Grid, brick_map, values, use_viewdirs: bool, rays, white_background: bool, out, g_out,
                      d_values):
     """Adds into ``d_values`` (the layout of ``values``) the gradient of ``baked_render`` (stop 0) whose rows were
