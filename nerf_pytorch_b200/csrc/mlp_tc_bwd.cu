@@ -18,10 +18,11 @@
 //
 // Persistent kernel, one CTA per SM, two consumer warpgroups (warpgroup w owns points [64 w, 64 w + 64) of the chain
 // and features [64 w, 64 w + 64) of every weight gradient) and one producer warpgroup, of which one thread streams the
-// chain's weight copies through the weight ring (tc_common.cuh WeightRing); the producer gives its registers to the
-// consumers (setmaxnreg), which hold the chain accumulator and a job accumulator at once.  Every wgmma is issued in
-// warpgroup-uniform control flow (the warp index is broadcast from lane 0), so ptxas keeps the MMAs of a k-loop
-// asynchronous.  The consumers' phases, per tile: tile_scale; per event e (layer t = n_gemm - 1 - e): g_epilogue (chain +
+// chain's weight copies through the weight ring (tc_common.cuh WeightRing) and another bulk-copies each event's ReLU
+// masks and each tile's d_raw into shared memory one event ahead, so that no epilogue waits on HBM; the producer gives
+// its registers to the consumers (setmaxnreg), which hold the chain accumulator and a job accumulator at once.  Every
+// wgmma is issued in warpgroup-uniform control flow (the warp index is broadcast from lane 0), so ptxas keeps the MMAs
+// of a k-loop asynchronous.  The consumers' phases, per tile: tile_scale; per event e (layer t = n_gemm - 1 - e): g_epilogue (chain +
 // head term, ReLU mask, hi / lo split -> G tile), chain_mma, then one job loop whose wgrad_job waits for the job's
 // activation tile (bulk-copied from the stash one job ahead), runs its MMAs, hands the tile back (thread 0 requests the
 // next job's once both warpgroups have) and drains the accumulator into the L2-resident gradient blob as 64-bit fixed
@@ -44,8 +45,11 @@ constexpr int kGBytes = 65536;                    // G tile: hi block 32 KB, lo 
 constexpr int kXBytes = 65536;                    // activation tile of the running job
 constexpr int kIndBytes = 4096;                   // ray-indicator tile: 128 points x 16 "features" (hi only)
 
+constexpr int kDrBytes = kTileRows * 16;          // d_raw of a tile (float4 per point)
+constexpr int kMaskBytes = kTileRows * 16;        // ReLU masks of one layer of a tile: 128 points x up to 4 words
+
 struct SmemMapB {
-  int g, x, ind, headw, bgrad, encd, sums, dacc, misc, bars, ring, total, n_stages;
+  int g, x, ind, headw, bgrad, encd, sums, dacc, dr, mask, misc, bars, ring, total, n_stages;
 };
 __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   SmemMapB m;
@@ -54,6 +58,8 @@ __host__ __device__ inline SmemMapB smem_map_b(const Plan& p) {
   m.x = off;      off += kXBytes;
   m.ind = off;    off += kIndBytes;
   m.headw = off;  off += (4 * 128 + 3 * 64 + 16) * 4;
+  m.dr = off;     off += 2 * kDrBytes;            // d_raw of the tile (alternating tiles)
+  m.mask = off;   off += 2 * kMaskBytes;          // ReLU masks of the event (alternating events)
   m.bgrad = off;  off += (p.enc_cum[0] + 8) * 4;   // bias gradients of every gemm layer + the heads' (8)
   m.encd = off;   off += kMaxRaysPerTile * 32 * 4;
   m.sums = off;   off += 64 * 16 * 4;             // per-ray sums of layers_dir[0]'s G (one tile)
@@ -151,6 +157,8 @@ __device__ __forceinline__ void cta_bar() { asm volatile("bar.sync 1, 256;" ::: 
 struct BwdSmem {
   uint8_t *g, *x, *ind;  // G tile, activation tile of the running job, ray-indicator tile
   float *headw, *bgrad, *encd, *sums, *dacc;
+  const float4* dr;      // [2][128]: d_raw of the tile (alternating tiles)
+  const uint32_t* mask;  // [2][128 x n / 32]: ReLU masks of the event's layer (alternating events)
   uint32_t* max;         // [2]: tile max of |d_raw| (alternating tiles)
 };
 
@@ -164,11 +172,9 @@ struct BwdTile {
 // Tile scale: max |d_raw| of the tile's points (warpgroup 0, one point per thread) -> a power of two that puts it in
 // [4, 8).  The maxima alternate between two slots, so the one barrier both publishes this tile's and orders the reset
 // of the next tile's slot after every read of the previous one.
-__device__ __forceinline__ void tile_scale(const float* __restrict__ d_raw, int64_t p0, int64_t P, uint32_t* s_max, int it,
-                                           BwdTile& tl) {
+__device__ __forceinline__ void tile_scale(const float4* dr, int64_t p0, int64_t P, uint32_t* s_max, int it, BwdTile& tl) {
   const int tid = threadIdx.x, rowm = tid & 127;
-  const float4 d4 = (p0 + rowm < P && tid < 128) ? reinterpret_cast<const float4*>(d_raw)[p0 + rowm]
-                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4 d4 = (p0 + rowm < P && tid < 128) ? dr[rowm] : make_float4(0.f, 0.f, 0.f, 0.f);
   const float m = fmaxf(fmaxf(fabsf(d4.x), fabsf(d4.y)), fmaxf(fabsf(d4.z), fabsf(d4.w)));
   uint32_t mb = __float_as_uint(m);
   mb = __reduce_max_sync(0xffffffffu, mb);
@@ -184,10 +190,10 @@ __device__ __forceinline__ void tile_scale(const float* __restrict__ d_raw, int6
 // G-tile epilogue of event e (layer t): G_t of this thread's elements = (chain + d_raw W_head) (.) relu'(layer t) -> hi /
 // lo -> the G tile (r0: warpgroup-local row of accumulator row 0).  The 64-wide layers_dir[0] also puts d_raw into feature
 // rows 64..67 (zeros up to 79) for the heads' jobs; event 0 writes the ray-indicator tile and the direction encodings.
+// d_raw and the layer's ReLU masks come from the tile's and the event's shared-memory copies (s_dr, s_mask).
 __device__ __forceinline__ void g_epilogue(const Plan& p, int e, const float (&chain)[64], const BwdTile& tl,
-                                           const float* __restrict__ d_raw, const float* __restrict__ stash, int64_t P_pad,
-                                           const float* __restrict__ dirs, int dir_stride, const BwdSmem& s, int hw1, int wg,
-                                           int r0) {
+                                           const float4* s_dr, const uint32_t* s_mask, const float* __restrict__ dirs,
+                                           int dir_stride, const BwdSmem& s, int hw1, int wg, int r0) {
   const int tid = threadIdx.x, q = tid & 3;
   const int t = p.n_gemm - 1 - e;
   const GemmLayer& g = p.g[t];
@@ -202,18 +208,14 @@ __device__ __forceinline__ void g_epilogue(const Plan& p, int e, const float (&c
 #pragma unroll
     for (int m = 0; m < 4; ++m) {
       mw[i][m] = 0xFFFFFFFFu;
-      if (g.relu && m < (g.n >> 5)) {
-        const uint32_t* mask_row = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * (p.mask_base + g.mask_cum) +
-                                   (size_t)tl.rs.pt[i] * (g.n >> 5);
-        mw[i][m] = tl.rs.valid[i] ? __ldg(mask_row + m) : 0u;
-      }
+      if (g.relu && m < (g.n >> 5)) mw[i][m] = tl.rs.valid[i] ? s_mask[(64 * wg + r0 + 8 * i) * (g.n >> 5) + m] : 0u;
     }
   // d_raw of this thread's rows at the tile scale (re-read per event rather than kept live through the MMAs), and
   // the head outputs' entries of it selected once (a runtime index into dr would put it in local memory)
   float dr[2][4], hd[2][4];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    const float4 d4 = tl.rs.valid[i] ? reinterpret_cast<const float4*>(d_raw)[tl.rs.pt[i]] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float4 d4 = tl.rs.valid[i] ? s_dr[64 * wg + r0 + 8 * i] : make_float4(0.f, 0.f, 0.f, 0.f);
     dr[i][0] = d4.x * tl.sc; dr[i][1] = d4.y * tl.sc; dr[i][2] = d4.z * tl.sc; dr[i][3] = d4.w * tl.sc;
   }
 #pragma unroll
@@ -480,9 +482,16 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   s.encd = reinterpret_cast<float*>(sm + mp.encd);
   s.sums = reinterpret_cast<float*>(sm + mp.sums);
   s.dacc = reinterpret_cast<float*>(sm + mp.dacc);
+  s.dr = reinterpret_cast<const float4*>(sm + mp.dr);
+  s.mask = reinterpret_cast<const uint32_t*>(sm + mp.mask);
   s.max = reinterpret_cast<uint32_t*>(sm + mp.misc);
   RingB ring{smem_u32(sm + mp.ring), smem_u32(sm + mp.bars), (uint32_t)mp.n_stages};
   const uint32_t x_full = ring.bars + 16 * kMaxStages;  // the running job's activation tile landed (after the ring's)
+  // Event k's copies (its layer's masks into slot k & 1, and at the first event of tile it, the tile's d_raw into
+  // dr[it & 1]): ev_full(k & 1) -- they landed; ev_empty(k & 1) -- both warpgroups' epilogue of event k is through.
+  // A d_raw buffer is rewritten two tiles on, after an event of the tile in between has been released.
+  auto ev_full = [&](uint32_t k) { return x_full + 8 + 8 * (k & 1); };
+  auto ev_empty = [&](uint32_t k) { return x_full + 24 + 8 * (k & 1); };
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);  // warp-uniform for ptxas: the role branches hold the wgmma
@@ -496,6 +505,10 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
   if (tid == 0) {
     ring.init(4 * kWG);
     mbar_init(x_full, 1);
+    for (uint32_t k = 0; k < 2; ++k) {
+      mbar_init(ev_full(k), 1);
+      mbar_init(ev_empty(k), 1);
+    }
     fence_barrier_init();
     s.max[0] = s.max[1] = 0u;
   }
@@ -523,6 +536,23 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
           const uint32_t kbytes = 96u * (uint32_t)g.k_h;
           for (int ks = 0; ks < (g.n >> 4); ++ks) ring.fill(src + (size_t)ks * kbytes, 1, kbytes, 0, pol);
         }
+    } else if (warp == 4 * kWG + 1 && lane == 0) {
+      // ---- the epilogues' operands, one event ahead: each layer's masks (the tile's 128 points, contiguous in the
+      // stash) and each tile's d_raw (its valid points only: rows past P are never read)
+      const uint32_t* masks = reinterpret_cast<const uint32_t*>(stash) + (size_t)P_pad * p.mask_base;
+      uint32_t k = 0;
+      for (int64_t p0 = (int64_t)blockIdx.x * kTileRows; p0 < P; p0 += (int64_t)gridDim.x * kTileRows) {
+        const uint32_t db = 16u * (uint32_t)(P - p0 < kTileRows ? P - p0 : kTileRows);
+        for (int e = 0; e < E; ++e, ++k) {
+          const GemmLayer& g = p.g[E - 1 - e];
+          const uint32_t mb = g.relu ? 16u * (uint32_t)g.n : 0u;  // 128 points x n / 32 words
+          mbar_wait(ev_empty(k), ((k >> 1) & 1) ^ 1);
+          mbar_arrive_expect_tx(ev_full(k), (e == 0 ? db : 0u) + mb);
+          if (e == 0) bulk_g2s(smem_u32(s.dr + ((k / E) & 1) * kTileRows), d_raw + 4 * p0, db, ev_full(k));
+          if (mb) bulk_g2s(smem_u32(s.mask) + (k & 1) * kMaskBytes,
+                           masks + (size_t)P_pad * g.mask_cum + (size_t)p0 * (g.n >> 5), mb, ev_full(k));
+        }
+      }
     }
   } else {
     // ===================== consumer warpgroups =====================
@@ -543,21 +573,26 @@ mlp_bwd_tc_kernel(const __grid_constant__ Plan p, const float* __restrict__ blob
     };
     if (tid == 0 && my_tiles > 0) issue_x(0, 0, 0);
 
+    uint32_t k = 0;  // running event index of the epilogues' copies
     for (int it = 0; it < my_tiles; ++it) {
       const int64_t tile = blockIdx.x + (int64_t)it * gridDim.x;
       const int64_t p0 = tile * kTileRows;
+      const float4* s_dr = s.dr + (it & 1) * kTileRows;
       BwdTile tl;
       tl.tr = tile_rays(p0, kTileRows, P, S);
       tl.rs = row_state(p0 + 64 * wg, r0, P, S, tl.tr.first);
-      tile_scale(d_raw, p0, P, s.max, it, tl);
+      mbar_wait(ev_full(k), (k >> 1) & 1);  // the tile's d_raw (with the first event's masks)
+      tile_scale(s_dr, p0, P, s.max, it, tl);
 
       float chain[64];  // G_{t+1} W_{t+1}[:, :128] of this warpgroup's rows (the previous event's chain MMA)
 #pragma unroll
       for (int i = 0; i < 64; ++i) chain[i] = 0.f;
-      for (int e = 0; e < E; ++e) {
-        g_epilogue(p, e, chain, tl, d_raw, stash, P_pad, dirs, dir_stride, s, hw1, wg, r0);
+      for (int e = 0; e < E; ++e, ++k) {
+        if (e > 0) mbar_wait(ev_full(k), (k >> 1) & 1);
+        g_epilogue(p, e, chain, tl, s_dr, s.mask + (k & 1) * (kMaskBytes / 4), dirs, dir_stride, s, hw1, wg, r0);
         fence_proxy_async();
         cta_bar();  // the G tile (and the indicator tile) complete
+        if (tid == 0) mbar_arrive(ev_empty(k));  // and nothing reads event k's copies any more
         if (e + 1 < E) chain_mma(chain, ring, s.g, p.g[E - 1 - e].n, wg);
 
         // ---- the job loop: every consumer thread waits for each job's activation tile once and hands it back once
